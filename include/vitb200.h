@@ -1,4 +1,4 @@
-/* libvitb200 -- C-ABI of the B200-native ViT-family forward engine.
+/* libvitb200 -- C-ABI of the H100-native ViT-family forward engine.
  *
  * The reference (taki0112/vit-tensorflow) has NO plugin / FFI interface: its hot path sits behind plain
  * Python classes (SURVEY.md section 8b).  The boundary preserved is the constructor + call surface
@@ -48,7 +48,7 @@ enum { VB_MEM_HOST = 0, VB_MEM_DEVICE = 1 };
 typedef struct vb_config {
   int32_t struct_size;            /* sizeof(vb_config), ABI guard */
   int32_t kind;                   /* VB_KIND_* */
-  int32_t precision;              /* VB_PRECISION_*: FP32 = exact-fp32 SIMT path (numerics gate); BF16 = tcgen05 path */
+  int32_t precision;              /* VB_PRECISION_*: FP32 = exact-fp32 SIMT path (numerics gate); BF16 = tensor-core path */
   int32_t image_h, image_w;       /* vit.py:133 pair(image_size) */
   int32_t patch_h, patch_w;       /* vit.py:134 pair(patch_size) */
   int32_t channels;               /* 3 */
@@ -161,9 +161,9 @@ VB_API int vb_forward_allgather(vb_handle* h, const float* img, int32_t img_mem,
 VB_API int64_t vb_last_launch_count(vb_handle* h);
 
 /* Per-kernel-class device timing (CUDA events recorded on the launch stream around every launch of the class)
- * for the roofline report.  Classes: 0 tcgen05 GEMM (plain / LayerNorm-folded epilogue: to_qkv, to_q, to_kv), 1 attention,
- * 2 LayerNorm / row statistics, 3 im2col, 4 other (SIMT fallbacks), 5 tcgen05 GEMM with GELU epilogue (fc1),
- * 6 tcgen05 GEMM with residual epilogue (patch embed, to_out, fc2).
+ * for the roofline report.  Classes: 0 wgmma GEMM (plain / LayerNorm-folded epilogue: to_qkv, to_q, to_kv), 1 attention,
+ * 2 LayerNorm / row statistics, 3 im2col, 4 other (SIMT fallbacks), 5 wgmma GEMM with GELU epilogue (fc1),
+ * 6 wgmma GEMM with residual epilogue (patch embed, to_out, fc2).
  * vb_profile_read synchronises the device and returns accumulated milliseconds, algorithmic FLOPs, algorithmic
  * bytes and launch counts per class (arrays of VB_PROF_NUM); reset != 0 clears the accumulators. */
 #define VB_PROF_NUM 7
@@ -178,7 +178,7 @@ VB_API void vb_destroy(vb_handle* h);
  * *elapsed_ms (may be NULL) receives the average device time per launch over `iters` launches (CUDA events). */
 
 /* out[M,N] = epi(a[M,K] x w[K,N]): epi = (+bias[N]) -> exact-erf GELU (gelu!=0) -> (*scale[N]) -> (+res[M,N]).
- * Any of bias/scale/res may be NULL.  precision BF16 runs the tcgen05 kernel, FP32 the SIMT kernel. */
+ * Any of bias/scale/res may be NULL.  precision BF16 runs the wgmma kernel, FP32 the SIMT kernel. */
 VB_API int vb_op_linear(int32_t precision, const float* a, const float* w, const float* bias, const float* scale,
                  const float* res, int32_t gelu, float* out, int32_t M, int32_t N, int32_t K, int32_t iters,
                  float* elapsed_ms);

@@ -15,7 +15,7 @@ variables by attribute path, and their logits equal ``spec_numpy``'s to 2e-15 in
 (tests/test_reference_shim.py; committed as tests/golden/*__refshim.npz by tests/golden/make_ref_golden.py so that the
 GPU box, which has no /root/reference, can compare the CUDA engine with them).  What stays assumed is the semantics
 of those primitives (Dense, LayerNormalization epsilon 1e-3, extract_patches 'SAME', ...: listed in ``tf_shim``'s
-docstring and DESIGN.md section 2) -- checked against PyTorch's operators, confirmable only by TensorFlow itself
+docstring and SURVEY.md Appendix A) -- checked against PyTorch's operators, confirmable only by TensorFlow itself
 (``tools/ref_tf_dump.py`` is the hook).  Further anchors: (1) two independent restatements -- a numpy-float64 "spec"
 (``spec_numpy``) and a torch-CPU-float32 one (``ref_torch``) -- that must agree, (2) einops itself (installed here) used
 as the ground truth for the patch ``Rearrange``, (3) ``tests/test_oracle_vs_hf_vit.py``: the ViT restatement reproduces

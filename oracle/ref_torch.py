@@ -1,7 +1,7 @@
 """torch-CPU float32 restatement of the reference forward pass.
 
 TEST INFRASTRUCTURE (see oracle/__init__.py); doubles as the timed CPU baseline
-("restated reference (torch CPU); TF unavailable", BASELINE.md section 3).
+("restated reference (torch CPU); TF unavailable").
 PARITY UNPINNED at the TensorFlow boundary.
 
 Written independently of oracle/spec_numpy.py (explicit reshape/permute instead of einops,

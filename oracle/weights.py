@@ -272,7 +272,7 @@ def stress_weights(cfg: dict, seed: int = 1) -> "collections.OrderedDict[str, np
 
 
 def make_image(cfg: dict, batch: int, seed: int = 0, h: int | None = None, w: int | None = None) -> np.ndarray:
-    """Synthetic NHWC float32 image batch (BASELINE.md section 2)."""
+    """Synthetic NHWC float32 image batch."""
     rng = np.random.default_rng(seed)
     h = cfg["image_h"] if h is None else h
     w = cfg["image_w"] if w is None else w

@@ -11,7 +11,7 @@ SMALL = {
     "vit_small": dict(kind="vit", image_size=64, patch_size=16, num_classes=10, dim=64, depth=2, heads=4, mlp_dim=128, dim_head=16),
     "vit_mean_rect": dict(kind="vit", image_size=(48, 64), patch_size=(8, 16), num_classes=7, dim=64, depth=1, heads=2,
                           mlp_dim=96, dim_head=32, pool="mean"),
-    # widths that are multiples of neither 64 nor 8: every general (non-tcgen05, unaligned) kernel path of the bf16 engine
+    # widths that are multiples of neither 64 nor 8: every general (non-wgmma, unaligned) kernel path of the bf16 engine
     "vit_odd_dims": dict(kind="vit", image_size=(40, 56), patch_size=8, num_classes=11, dim=50, depth=2, heads=3, mlp_dim=70,
                          dim_head=14, pool="mean"),
     "vit_noproj": dict(kind="vit", image_size=32, patch_size=8, num_classes=5, dim=64, depth=2, heads=1, mlp_dim=64, dim_head=64),
@@ -40,7 +40,7 @@ SMALL = {
                              cross_attn_depth=1, cross_attn_heads=2, cross_attn_dim_head=32, depth=1),
 }
 
-# Mid-size bf16 cases exercising the tcgen05 kernels at the real head / sequence geometry (n = 197, dh = 64).
+# Mid-size bf16 cases exercising the tensor-core kernels at the real head / sequence geometry (n = 197, dh = 64).
 MID = {
     "vit_mid": dict(kind="vit", image_size=224, patch_size=16, num_classes=1000, dim=256, depth=2, heads=4, mlp_dim=512),
     "parallel_mid": dict(kind="parallel_vit", image_size=224, patch_size=16, num_classes=100, dim=256, depth=2, heads=4, mlp_dim=512),

@@ -1,6 +1,6 @@
 """CPU double of libvitb200's C-ABI, for tests of the HOST logic only.
 
-Constructing a `vit_tensorflow_b200.ViT` needs a B200 (`vb_create` refuses without one, and there is no CPU fallback in the
+Constructing a `vit_tensorflow_b200.ViT` needs an H100 (`vb_create` refuses without one, and there is no CPU fallback in the
 product).  What sits between the user and the C-ABI -- kwargs, ctypes marshalling, the attribute surface the reference's wrappers
 poke at (`patch_embedding.layers[:2]`, `.weights`, `pos_embedding[:, 1:n]`, `transformer(tokens)`, `.numpy()` on results) -- is
 plain Python, though, and can be exercised on a CPU box by handing the host classes an object that answers the same `vb_*`

@@ -1,4 +1,4 @@
-"""CPU tests of the boundary: the C-ABI library builds for sm_100a, loads, exports every symbol
+"""CPU tests of the boundary: the C-ABI library builds for sm_90a, loads, exports every symbol
 include/vitb200.h declares, refuses to compute without a GPU, and the Python host classes validate kwargs with
 the reference's assertion messages (vit.py:136,139; deepvit.py:117; cait.py:160; cross_vit.py:207)."""
 import ctypes
@@ -138,8 +138,8 @@ def test_drop_in_import_names():
                                                                    vb.PatchMerger, vb.EfficientViT)
 
 
-def test_built_for_sm100a_with_tcgen05(lib):
-    """The shipped library contains sm_100a SASS with tcgen05 (UTCHMMA), TMA (UTMALDG/UTMASTG) and TMEM loads."""
+def test_built_for_sm90a_with_wgmma(lib):
+    """The shipped library contains sm_90a SASS with wgmma (HGMMA), TMA loads (UTMALDG) and tensor-core MMA (HMMA)."""
     import shutil
     import subprocess
     from vit_tensorflow_b200 import _lib
@@ -147,15 +147,15 @@ def test_built_for_sm100a_with_tcgen05(lib):
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", _lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
-    for mnemonic in ("UTCHMMA", "UTMALDG", "UTMASTG", "LDTM"):
+    assert "sm_90a" in sass
+    for mnemonic in ("HGMMA", "UTMALDG", "HMMA"):
         assert mnemonic in sass, mnemonic
 
 
 def test_attribute_surface_supports_the_wrapper_expressions():
     """`model.pos_embedding` / `model.cls_token` as mae.py:54, simmim.py:95, mpp.py:204-208 use them (slicing, einops repeat,
     arithmetic).  They are properties over the model's weight dict, so a stub holding `_specs` / `_weights` is enough on a CPU
-    box (constructing a real model needs a B200)."""
+    box (constructing a real model needs an H100)."""
     import numpy as np
     from einops import repeat
     from vit_tensorflow_b200.models import _EngineModel

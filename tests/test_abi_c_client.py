@@ -1,7 +1,7 @@
 """The boundary is a C ABI: tests/abi_client.c is compiled by gcc as strict C99 against include/vitb200.h (no C++, no
 Python host code), linked to libvitb200.so, and
   * without a GPU it must stop at vb_create with the no-CPU-fallback error (CPU test),
-  * on a B200 its logits (weights and image generated inside the C program) must match the oracle (GPU test)."""
+  * on an H100 its logits (weights and image generated inside the C program) must match the oracle (GPU test)."""
 import os
 import subprocess
 import zlib

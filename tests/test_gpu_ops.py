@@ -149,7 +149,7 @@ def test_attention(lib, precision, variant, B, nq, nk, heads, dh):
 @pytest.mark.parametrize("B,nq,nk,heads,dh", [(2, 130, 130, 8, 64), (1, 64, 256, 16, 32), (3, 65, 65, 8, 16), (2, 5, 37, 16, 48),
                                                (1, 256, 256, 8, 48), (5, 197, 197, 16, 64), (2, 16, 16, 8, 64), (150, 70, 70, 8, 32)])
 def test_attention_mix_shapes(lib, variant, B, nq, nk, heads, dh):
-    """Fused tcgen05 head-mixing attention (attn_mix_tcgen05.cu; deepvit.py:79-87, cait.py:121-127) at the edges of its tiling:
+    """Head-mixing attention (attn_generic_mma.cu; deepvit.py:79-87, cait.py:121-127) at the edges of its tiling:
     partial 64-row query tiles (nq = 130, 65, 5), a single key block, the 256-key limit, key counts that leave the second
     block of a super-block empty (nk = 16, 37, 70), dim_head 16 / 32 / 48 / 64, more items than CTAs (B = 150 x 2 tiles)."""
     from vit_tensorflow_b200 import _lib
@@ -167,7 +167,7 @@ def test_attention_mix_shapes(lib, variant, B, nq, nk, heads, dh):
     _assert_close_sigma(out, ref, ATTN_BF16_SIGMA[variant], ATTN_BF16_REL)
 
 
-# bf16 attention bound: |err| <= SIGMA * std(ref) + REL * |ref|  (measured maxima: DESIGN.md section 6)
+# bf16 attention bound: |err| <= SIGMA * std(ref) + REL * |ref|  (bf16 operands and probabilities, fp32 accumulation)
 ATTN_BF16_SIGMA = {0: 1.5e-2, 1: 1.5e-2, 2: 1.5e-2}
 ATTN_BF16_REL = 1.0e-2
 
@@ -185,8 +185,8 @@ def _assert_close_sigma(out, ref, sigma_frac, rel):
 @pytest.mark.parametrize("ramp", ["up", "down", "zigzag"])
 @pytest.mark.parametrize("B,n,heads", [(2, 577, 2), (3, 197, 3), (1, 300, 1)])
 def test_attention_lazy_rescale(lib, B, n, heads, ramp):
-    """The tcgen05 kernel keeps its softmax reference point until a 128-key block's row max exceeds it by more than 2^8 and
-    only then rescales O in tensor memory (attn_tcgen05.cu, `need`).  N(0,1) scores never do that, so this case scales the
+    """The fused attention kernel rescales its running output whenever a key block raises a row max;
+    N(0,1) scores barely move it (attn_flash.cu, `alpha`), so this case scales the
     keys of block j by a ramp: with 'up' every later block beats the running reference by ~15 in log2 units (the rescale and
     the l correction run for every j > 0), 'down' keeps the first block's reference throughout (later exponents underflow
     towards 0), 'zigzag' alternates."""

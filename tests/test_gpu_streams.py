@@ -6,7 +6,7 @@ SAME bits as the single-stream forward.
   * ViT: the batch as two half-batches on two streams (VB_FWD_STREAMS=2; off by default, kept as a measured experiment)
 
 The switches are read once per process, so every setting runs in its own subprocess; each prints the sha256 of the logits of
-three consecutive calls (eager, graph capture, graph replay -- DESIGN.md section 1) on seeded weights and images."""
+three consecutive calls (eager, graph capture, graph replay) on seeded weights and images."""
 import hashlib
 import os
 import subprocess

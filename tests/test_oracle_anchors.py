@@ -1,6 +1,6 @@
 """Second, independent anchors for the oracle's building blocks (VERDICT r1 item 9): the numpy-float64 spec against PyTorch's own
 implementations of the same published operators, on random inputs.  None of this is TensorFlow (absent from this image: the reference's own
-code is pinned by tests/test_reference_shim.py, the TensorFlow primitives under it stay assumed, DESIGN.md section 2), but it is
+code is pinned by tests/test_reference_shim.py, the TensorFlow primitives under it stay assumed, SURVEY.md Appendix A), but it is
 third-party code the spec did not come from:
 
   attention core (vit.py:77-82)            F.scaled_dot_product_attention

@@ -1,4 +1,4 @@
-"""Error of the erf approximations used by the fc1 GELU epilogue (csrc/gemm_tcgen05.cu), against scipy's erf,
+"""Error of the erf approximations used by the fc1 GELU epilogue (csrc/gemm_wgmma.cu), against scipy's erf,
 in absolute terms and in bf16 ulps of the GELU output.  Runs on CPU."""
 import numpy as np
 from scipy.special import erf
@@ -32,7 +32,7 @@ def fit_tail(deg=5, amax=6.0):
 
 
 c = fit_tail()
-print("tail polynomial q(a), a = |x| (gemm_tcgen05.cu uses -a, odd terms negated):", [f"{float(v):.9e}" for v in c])
+print("tail polynomial q(a), a = |x| (gemm_wgmma.cu uses -a, odd terms negated):", [f"{float(v):.9e}" for v in c])
 xa = np.minimum(np.abs(x), 6.0).astype(np.float32)
 q = np.full_like(xa, c[-1])
 for k in range(len(c) - 2, -1, -1):

@@ -1,6 +1,6 @@
 """ctypes binding of libvitb200.so (include/vitb200.h).  No torch, no numpy-side compute: this module only
 marshals pointers and sizes across the C-ABI.  There is NO CPU fallback: if the library is missing it is an
-ImportError-style failure, and every entry point fails loudly when no B200 is visible."""
+ImportError-style failure, and every entry point fails loudly when no H100 is visible."""
 from __future__ import annotations
 
 import ctypes as C
@@ -137,7 +137,7 @@ def op_layernorm(x, gamma, beta, precision="bf16", iters=0):
 
 
 def op_ln_linear(x, gamma, beta, w, bias=None, gelu=False, iters=0):
-    """out = act(LayerNorm(x) @ w + bias) through the LayerNorm-folded tcgen05 GEMM (bf16 engine); returns (out, ms)."""
+    """out = act(LayerNorm(x) @ w + bias) through the LayerNorm-folded wgmma GEMM (bf16 engine); returns (out, ms)."""
     x, gamma, beta, w, bias = map(_f32, (x, gamma, beta, w, bias))
     M, K = x.shape
     N = w.shape[1]

@@ -1,5 +1,5 @@
 // Generic attention through materialised fp32 scores (the reference's own dataflow, vit.py:77-82): used by the
-// exact-fp32 gate path and as the fallback of the bf16 path for shapes the tcgen05 kernel does not cover.
+// exact-fp32 gate path and as the fallback of the bf16 path for shapes the fused kernels do not cover.
 #include "attention.cuh"
 #include "kernels.cuh"
 #include <cmath>

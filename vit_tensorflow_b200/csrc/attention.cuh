@@ -1,5 +1,5 @@
 // Attention entry points: the generic materialised-scores path (any shape / variant, both precisions) and the
-// tcgen05 fast path (bf16; returns false when the shape is not covered so the caller falls back to generic).
+// fused fast path (bf16; returns false when the shape is not covered so the caller falls back to generic).
 #pragma once
 #include "common.h"
 
@@ -39,17 +39,10 @@ struct MixParams {
 bool attention_mix_params(const float* mix_a, const float* mix_b, const float* ln_gamma, const float* ln_beta, int heads,
                           cudaStream_t s, MixParams* out);
 
-// Fused tcgen05 head-mixing attention (attn_mix_tcgen05.cu): variants 1 / 2, heads 8 / 16, dim_head <= 64, nk <= 256.
-bool attention_mix(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, int ldk, const __nv_bfloat16* v, int ldv,
-                   __nv_bfloat16* out, int ldo, int B, int nq, int nk, int heads, int dh, int variant, const float* mix_a,
-                   const float* mix_b, const float* ln_gamma, const float* ln_beta, cudaStream_t s, float scale = 0.f);
-
 // One-kernel attention for a single query row per image (CaiT class attention, CrossViT cross attention; any variant):
 // attn_cls.cu.  false if the shape is not covered.
 bool attention_cls(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, int ldk, const __nv_bfloat16* v, int ldv,
                    __nv_bfloat16* out, int ldo, int B, int nk, int heads, int dh, int variant, const float* mix_a,
                    const float* mix_b, const float* ln_gamma, const float* ln_beta, cudaStream_t s, float scale = 0.f);
-
-long long*& attn_trace_buffer();   // debugging aid: device trace buffer of the tcgen05 attention kernel (null = off)
 
 }  // namespace vb

@@ -47,8 +47,8 @@ attn_cls_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloat1
   __syncthreads();
   // ---- 1. scores (in log2 units: scale * log2(e) folded in; the pre-softmax mix is linear, so it commutes with the factor)
   // thread = (key j, head h), adjacent threads = adjacent heads of one key: a warp's eight 16-byte loads per thread sweep four
-  // whole K rows (4 KB, L1-resident), all issued before the arithmetic.  (The first form -- thread = key, 64 dependent loads
-  // along a 1 KB row, 32 KB of rows per warp -- ran CrossViT's 257-key cross-attention at ~220 us per launch.)
+  // whole K rows (4 KB, L1-resident), all issued before the arithmetic, instead of 64 dependent loads along one 1 KB row per
+  // thread.
   const int chunks = dh >> 3;
   for (int idx = tid; idx < nk * heads; idx += CLS_THREADS) {
     const int j = idx / heads, h = idx - j * heads;

@@ -1,0 +1,210 @@
+// Tensor-core multi-head attention for the bf16 engine (bf16 operands, fp32 accumulation, dim_head = 64).
+//
+//   out[b, i, h, :] = softmax_j( scale * q[b,i,h,:] . k[b,j,h,:] ) @ v[b,j,h,:]        (vit.py:77-82)
+//
+// The [b,h,n,n] score tensor the reference materialises twice in memory (dots, attn) lives only in registers.
+// One CTA per (64 query rows, b, h) on a flat grid index (no 65535 limit on B*h), 4 warps of 16 query rows each.  Q, K and
+// V are read straight out of the row-major projection output ([B, n, 3*h*dh] for the fused to_qkv), so the head split 'b n (h d) -> b h n d' (vit.py:74) costs
+// nothing; 64-key blocks of K and V stream through a two-stage cp.async ring.  Per block and warp:
+//   S = Q K^T       mma.sync m16n8k16 (Q fragments loaded once, K fragments from the row-major K tile),
+//   online softmax  row max / exp2 / row sum on the S fragments (a row lives in the 4 lanes of a quad),
+//   O += P V        the S fragments, rounded to bf16, ARE the A fragments of the next product; V fragments by
+//                   ldmatrix.trans from the row-major V tile.
+// Final 1/l normalisation and bf16 stores in 'b n (h d)' order (the merge-heads rearrange, vit.py:82).
+#include "attention.cuh"
+#include "kernels.cuh"
+#include "ptx.cuh"
+
+#include <cmath>
+
+namespace vb {
+namespace {
+
+constexpr int DH = 64;
+constexpr int FQ = 64;             // query rows per CTA
+constexpr int FK = 64;             // keys per block
+constexpr int FP = DH + 8;         // smem row pitch (bf16): +16 bytes keeps the fragment loads bank-conflict free
+
+__device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+}
+
+__global__ void __launch_bounds__(128)
+attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloat16* __restrict__ k, int ldk,
+                  const __nv_bfloat16* __restrict__ v, int ldv, __nv_bfloat16* __restrict__ out, int ldo, int heads, int nq, int nk,
+                  float scale_log2) {
+  __shared__ __align__(16) __nv_bfloat16 Qs[FQ][FP];
+  __shared__ __align__(16) __nv_bfloat16 Ks[2][FK][FP];
+  __shared__ __align__(16) __nv_bfloat16 Vs[2][FK][FP];
+  const int qtiles = (nq + FQ - 1) / FQ;
+  const int bh = blockIdx.x / qtiles, b = bh / heads, h = bh % heads;
+  const int i0 = (blockIdx.x % qtiles) * FQ;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nblk = (nk + FK - 1) / FK;
+
+  pdl_wait();                 // Q/K/V come from the previous kernel of the stream
+  pdl_launch_dependents();
+
+  // rows past n are zero-filled (never read from the next image); 8 16-byte vectors per 64-column row
+  for (int e = threadIdx.x; e < FQ * 8; e += 128) {
+    const int r = e >> 3, c = (e & 7) * 8;
+    if (i0 + r < nq) cp_async16(smem_u32(&Qs[r][c]), q + (static_cast<size_t>(b) * nq + i0 + r) * ldq + h * DH + c);
+    else *reinterpret_cast<uint4*>(&Qs[r][c]) = make_uint4(0, 0, 0, 0);
+  }
+  auto stage = [&](int j) {
+    if (j < nblk) {
+      const int s = j & 1, j0 = j * FK;
+      for (int e = threadIdx.x; e < FK * 8; e += 128) {
+        const int r = e >> 3, c = (e & 7) * 8;
+        if (j0 + r < nk) {
+          const size_t row = static_cast<size_t>(b) * nk + j0 + r;
+          cp_async16(smem_u32(&Ks[s][r][c]), k + row * ldk + h * DH + c);
+          cp_async16(smem_u32(&Vs[s][r][c]), v + row * ldv + h * DH + c);
+        } else {                                                     // zero V rows: 0 * garbage could be NaN
+          *reinterpret_cast<uint4*>(&Ks[s][r][c]) = make_uint4(0, 0, 0, 0);
+          *reinterpret_cast<uint4*>(&Vs[s][r][c]) = make_uint4(0, 0, 0, 0);
+        }
+      }
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+  stage(0);
+
+  const int qr = lane >> 2, qc = 2 * (lane & 3);                     // fragment row (and row + 8) / column pair of this lane
+  uint32_t qf[DH / 16][4];
+  float o[DH / 8][4];
+#pragma unroll
+  for (int n = 0; n < DH / 8; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};    // running max (log2 units) / partial row sums
+
+  for (int j = 0; j < nblk; ++j) {
+    stage(j + 1);
+    asm volatile("cp.async.wait_group 1;" ::: "memory");
+    __syncthreads();
+    if (j == 0) {
+      const uint32_t qa = smem_u32(&Qs[warp * 16 + (lane & 15)][8 * (lane >> 4)]);
+#pragma unroll
+      for (int kk = 0; kk < DH / 16; ++kk)
+        asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                     : "=r"(qf[kk][0]), "=r"(qf[kk][1]), "=r"(qf[kk][2]), "=r"(qf[kk][3]) : "r"(qa + kk * 32));
+    }
+    const int s = j & 1;
+    // ---- S = Q K^T for this warp's 16 rows x 64 keys
+    float sc[FK / 8][4];
+#pragma unroll
+    for (int n = 0; n < FK / 8; ++n) {
+      sc[n][0] = sc[n][1] = sc[n][2] = sc[n][3] = 0.f;
+#pragma unroll
+      for (int kk = 0; kk < DH / 16; ++kk) {
+        const uint32_t b0 = *reinterpret_cast<const uint32_t*>(&Ks[s][n * 8 + qr][kk * 16 + qc]);
+        const uint32_t b1 = *reinterpret_cast<const uint32_t*>(&Ks[s][n * 8 + qr][kk * 16 + qc + 8]);
+        mma_bf16_16816(sc[n], qf[kk], b0, b1);
+      }
+    }
+    // ---- online softmax (rows qr and qr + 8 of the warp's tile)
+    const int valid = nk - j * FK;
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int n = 0; n < FK / 8; ++n) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        if (n * 8 + qc + (e & 1) >= valid) sc[n][e] = -INFINITY;
+        mx[e >> 1] = fmaxf(mx[e >> 1], sc[n][e]);
+      }
+    }
+    float alpha[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      const float m_new = fmaxf(m_run[r], mx[r] * scale_log2);       // every block holds at least one valid key: finite
+      alpha[r] = ex2_approx(m_run[r] - m_new);                       // first block: 2^-inf = 0
+      m_run[r] = m_new;
+      l_run[r] *= alpha[r];
+    }
+#pragma unroll
+    for (int n = 0; n < DH / 8; ++n) {
+      o[n][0] *= alpha[0]; o[n][1] *= alpha[0];
+      o[n][2] *= alpha[1]; o[n][3] *= alpha[1];
+    }
+    uint32_t pf[FK / 16][4];                                         // P as the A fragments of the PV product
+#pragma unroll
+    for (int n = 0; n < FK / 8; ++n) {
+      const float p0 = ex2_approx(fmaf(sc[n][0], scale_log2, -m_run[0]));
+      const float p1 = ex2_approx(fmaf(sc[n][1], scale_log2, -m_run[0]));
+      const float p2 = ex2_approx(fmaf(sc[n][2], scale_log2, -m_run[1]));
+      const float p3 = ex2_approx(fmaf(sc[n][3], scale_log2, -m_run[1]));
+      l_run[0] += p0 + p1;
+      l_run[1] += p2 + p3;
+      pf[n >> 1][(n & 1) * 2 + 0] = pack_bf16x2(p0, p1);
+      pf[n >> 1][(n & 1) * 2 + 1] = pack_bf16x2(p2, p3);
+    }
+    // ---- O += P V
+    const uint32_t va = smem_u32(&Vs[s][lane & 15][0]);
+#pragma unroll
+    for (int kk = 0; kk < FK / 16; ++kk) {
+#pragma unroll
+      for (int n = 0; n < DH / 8; ++n) {
+        uint32_t b0, b1;
+        asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0, %1}, [%2];"
+                     : "=r"(b0), "=r"(b1) : "r"(va + (kk * 16 * FP + n * 8) * 2));
+        mma_bf16_16816(o[n], pf[kk], b0, b1);
+      }
+    }
+    __syncthreads();                       // the next iteration's prefetch overwrites this stage only after every warp is done
+  }
+
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
+    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
+    l_run[r] = 1.0f / l_run[r];
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = i0 + warp * 16 + qr + 8 * r;
+    if (row >= nq) continue;
+    __nv_bfloat16* orow = out + (static_cast<size_t>(b) * nq + row) * ldo + h * DH + qc;
+#pragma unroll
+    for (int n = 0; n < DH / 8; ++n)
+      *reinterpret_cast<uint32_t*>(orow + n * 8) = pack_bf16x2(o[n][2 * r] * l_run[r], o[n][2 * r + 1] * l_run[r]);
+  }
+}
+
+}  // namespace
+
+template <>
+bool attention_fast<__nv_bfloat16>(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, int ldk, const __nv_bfloat16* v, int ldv,
+                                   __nv_bfloat16* out, int ldo, int B, int nq, int nk, int heads, int dh, int variant,
+                                   const float* mix_a, const float* mix_b, const float* ln_g, const float* ln_b, cudaStream_t s,
+                                   float scale) {
+  if (nq == 1 && attention_cls(q, ldq, k, ldk, v, ldv, out, ldo, B, nk, heads, dh, variant, mix_a, mix_b, ln_g, ln_b, s, scale)) return true;
+  // DeepViT re-attention / CaiT talking heads: the materialised-scores path (attn_generic_mma.cu) -- a fused form with all heads'
+  // scores of a 16-row tile in shared memory measured 9-11 % slower on the H100 (one CTA per SM at 16 heads)
+  if (variant != 0 || dh != DH || nq < 2) return false;
+  if ((ldq % 8) || (ldk % 8) || (ldv % 8) || (ldo % 2)) return false;
+  if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
+       reinterpret_cast<uintptr_t>(out)) % 16) return false;
+  const float scale_log2 = (scale > 0.f ? scale : 1.0f / sqrtf(static_cast<float>(dh))) * 1.4426950408889634f;
+  cudaLaunchConfig_t cfg = {};
+  const long long blocks = static_cast<long long>(B) * heads * ((nq + FQ - 1) / FQ);
+  if (blocks > 0x7fffffffLL) return false;
+  cfg.gridDim = dim3(static_cast<unsigned>(blocks));
+  cfg.blockDim = dim3(128);
+  cfg.stream = s;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2));
+  count_launch();
+  return true;
+}
+
+}  // namespace vb

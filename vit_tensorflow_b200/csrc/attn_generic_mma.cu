@@ -1,10 +1,10 @@
-// Second-tier attention path for the bf16 engine: shapes / variants the tcgen05 kernel does not cover yet
+// Second-tier attention path for the bf16 engine: shapes / variants the fused kernel (attn_flash.cu) does not cover
 // (DeepViT re-attention deepvit.py:83-84, CaiT talking heads cait.py:121-127, dim_head != 64, 1-row class-attention
 // queries).  The score tensor is still materialised (fp32, like the reference does), but
 //   * QK^T and PV run on the tensor cores through mma.sync.m16n8k16 (legacy HMMA path: simple, any dh % 16 == 0),
 //   * pre-mix -> softmax -> post-mix / LayerNorm-over-heads is ONE kernel (one read + one write of the scores
 //     instead of three full passes).
-// Fusing these variants into the tcgen05 kernel (head mixing as in-kernel epilogues) is the next step (DESIGN.md).
+// (DeepViT re-attention and CaiT talking heads are served here: the head mix couples every head of a query row.)
 #include "attention.cuh"
 #include "kernels.cuh"
 #include "ptx.cuh"

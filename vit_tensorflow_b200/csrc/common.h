@@ -50,29 +50,25 @@ inline bool first_use_on_this_device(unsigned long long (&seen)[4]) {
   return true;
 }
 
-// 2-D / 3-D bf16 tensor maps (innermost dimension first), 128-byte swizzle unless swizzle == false.
+// 2-D bf16 (or fp32) tensor map (innermost dimension first), 128-byte swizzle unless swizzle128 == false.
 CUtensorMap make_tmap_2d(const void* base, uint64_t inner, uint64_t outer, uint64_t outer_stride_bytes,
                          uint32_t box_inner, uint32_t box_outer, bool swizzle128 = true, bool f32 = false);
-CUtensorMap make_tmap_3d(const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1_bytes,
-                         uint64_t stride2_bytes, uint32_t box0, uint32_t box1, uint32_t box2, bool swizzle128 = true);
 
-// ------------------------------------------------------------------------------------------ tcgen05 GEMM
-// out[M,N] = epilogue(A[M,K] * Wt[N,K]^T): bf16 operands (K-major), fp32 accumulation in TMEM.
+// ------------------------------------------------------------------------------------------ wgmma GEMM
+// out[M,N] = epilogue(A[M,K] * Wt[N,K]^T): bf16 operands (K-major), fp32 accumulation in registers.
 // epilogue: (+bias[n]) -> (exact-erf GELU) -> (*scale[n]) -> (+res[m,n]); out bf16.
 struct GemmBf16 {
-  CUtensorMap tmap_a, tmap_b, tmap_c, tmap_r;   // A, B (weights), output, residual
+  CUtensorMap tmap_a, tmap_b;           // A, B (weights)
   int M = 0, N = 0, K = 0;
   __nv_bfloat16* out = nullptr;         // [M, ldc] (the epilogue stores rows straight from registers)
   int ldc = 0;
   bool out_f32 = false;                 // `out` is float* (ldc in floats): plain / bias epilogue only
   int block_n = 256;
-  int cta_group = 2;                    // 2: CTA pairs (cta_group::2) on 256-row tiles; 1: single-CTA 128-row tiles
   const float* bias = nullptr;          // [N] or null
   const float* scale = nullptr;         // [N] or null (LayerScale)
   const __nv_bfloat16* res = nullptr;   // [M, ldr] or null (may alias out)
   int ldr = 0;
   bool gelu = false;
-  int grid = 0;
   // Folded LayerNorm of the A operand (Wt must hold gamma-scaled weights, bias the beta.W + b term):
   //   out = rstd[m] * (acc - mu[m] * ln_c1[n]) + bias[n], with (mu, rstd) of row m reduced in the epilogue from the
   //   ln_parts (sum, sumsq) partials of that row (the stats_out format below) over 1 / ln_inv_d elements.
@@ -82,7 +78,6 @@ struct GemmBf16 {
   float ln_inv_d = 0.f;
   // Emit (sum, sumsq) of every 64-column chunk of the stored bf16 output rows: [N/64, M, 2]
   float* stats_out = nullptr;
-  int stats_parts = 0;
 };
 // lda/ldw/ldc/ldr in elements; all must be multiples of 8 (16-byte TMA strides); N % 64 == 0.
 GemmBf16 gemm_bf16_plan(const __nv_bfloat16* A, int lda, const __nv_bfloat16* Wt, int ldw, __nv_bfloat16* out, int ldc,
@@ -90,6 +85,5 @@ GemmBf16 gemm_bf16_plan(const __nv_bfloat16* A, int lda, const __nv_bfloat16* Wt
                         bool gelu, bool out_f32 = false, int b_rows = 0);
 void gemm_bf16_run(const GemmBf16& g, cudaStream_t stream);
 bool gemm_bf16_supported(int M, int N, int K, int lda, int ldw, int ldc);
-long long*& gemm_trace_buffer();
 
 }  // namespace vb

@@ -4,7 +4,7 @@
 // The op sequences restate the reference's call graphs (SURVEY.md section 3):
 //   ViT / DeepViT  vit.py:159-177, deepvit.py:139-157      CaiT  cait.py:180-194      CrossViT  cross_vit.py:290-303
 // with inference semantics (dropout = identity).  T = float runs the exact-fp32 SIMT kernels (numerics gate),
-// T = __nv_bfloat16 runs the tcgen05 GEMM / attention kernels with fp32 accumulation and statistics.
+// T = __nv_bfloat16 runs the wgmma GEMM / tensor-core attention kernels with fp32 accumulation and statistics.
 #include "../../include/vitb200.h"
 #include "attention.cuh"
 #include "common.h"
@@ -274,7 +274,7 @@ struct vb_handle {
   struct ResKey { const void* e; int B, rows; bool operator<(const ResKey& o) const { return std::tie(e, B, rows) < std::tie(o.e, o.B, o.rows); } };
   std::map<ResKey, std::unique_ptr<DevMem>> embed_res;
 
-  // cached tcgen05 GEMM plans (TMA descriptors)
+  // cached wgmma GEMM plans (TMA descriptors)
   using PlanKey = std::array<uintptr_t, 16>;
   std::map<PlanKey, GemmBf16> plans;
 
@@ -451,7 +451,7 @@ struct vb_handle {
     }
     return L;
   }
-  // Two bias-free Dense layers applied to the same input (CaiT to_q / to_kv on x, cait.py:114-119) as ONE tcgen05 GEMM:
+  // Two bias-free Dense layers applied to the same input (CaiT to_q / to_kv on x, cait.py:114-119) as ONE wgmma GEMM:
   // the packed K-major weights and the LayerNorm-fold constants of `a` and `b` are laid out back to back, so the output
   // columns are [a | b] = [q | k | v], the layout the fused to_qkv of vit.py produces.  bf16 engine only.
   Linear make_linear_pair(const std::string& na, int NA, const std::string& nb, int NB, int K, const Norm* fold) {
@@ -485,7 +485,7 @@ struct vb_handle {
   LayerW make_layer(const std::string& pre, int dim, int heads, int dh, int mlp, int kind, bool fold_ok = true) {
     LayerW l;
     l.dh_model = dh;
-    // Plain softmax attention with dim_head < 64 (bf16 engine): widen every head to the tcgen05 attention kernel's 64 columns
+    // Plain softmax attention with dim_head < 64 (bf16 engine): widen every head to the fused attention kernel's 64 columns
     // with zero weights -- extra to_qkv / to_q / to_kv output columns (q, k, v pad columns are exactly 0, so QK^T and the
     // real PV columns are unchanged) and zero to_out input rows.  Costs (64 / dh - 1) more flops in those two GEMMs and buys
     // the tensor-core attention path for e.g. dim_head 48 / 32 (the head-mixing variants have their own kernel, attn_mix).
@@ -509,7 +509,7 @@ struct vb_handle {
     l.heads = heads; l.dim_head = dh;
     l.attn_norm = make_norm(pre + "attn_norm", dim);
     l.ff_norm = make_norm(pre + "ff_norm", dim);
-    // LayerNorm folding needs every GEMM of the layer on the tcgen05 path (all widths multiples of 64)
+    // LayerNorm folding needs every GEMM of the layer on the wgmma path (all widths multiples of 64)
     l.folded = bf16() && fold_ok && dim % 64 == 0 && inner % 64 == 0 && mlp % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr;
     const Norm* fa = l.folded ? &l.attn_norm : nullptr;
     const Norm* ff = l.folded ? &l.ff_norm : nullptr;
@@ -532,7 +532,7 @@ struct vb_handle {
   // One-layer transformer between two T2T soft splits (t2t.py:35,45-46: heads = 1, dim_head = mlp_dim = dim = D = channels * prod(k^2),
   // 147 and 1323 at the default t2t_layers; no out-projection, vit.py:53) on the tensor cores: every width is zero-padded to
   // Dp = round_up(D, 64) -- token rows [n, Dp] with zero pad columns, to_qkv columns [q | k | v] each Dp wide, fc1 / fc2 Dp x Dp --
-  // so that all four GEMMs and the per-image QK^T / PV products run on the tcgen05 GEMM kernel; LayerNorm and the softmax scale keep
+  // so that all four GEMMs and the per-image QK^T / PV products run on the wgmma GEMM kernel; LayerNorm and the softmax scale keep
   // the true D.  Zero weights and biases keep the pad columns exactly zero through the layer (GELU(0) = 0).
   static bool t2t_tensor_path_enabled() { static const bool off = getenv("VB_NO_T2T_TC") != nullptr; return !off; }
   LayerW make_t2t_layer(const std::string& pre, int D) {
@@ -787,7 +787,7 @@ struct vb_handle {
     return O;
   }
 
-  // tcgen05 GEMM on raw operands through the plan cache (the T2T soft-split attention products)
+  // wgmma GEMM on raw operands through the plan cache (the T2T soft-split attention products)
   void gemm_cached(const __nv_bfloat16* A, int lda, const __nv_bfloat16* Wt, int ldw, int b_rows, void* out, int ldc, int M, int N, int K,
                    const __nv_bfloat16* res, int ldr, bool out_f32, int cls, cudaStream_t s) {
     ProfScope ps(this, cls, 2.0 * M * N * K, 2.0 * (static_cast<double>(M) * K + static_cast<double>(N) * K) + (out_f32 ? 4.0 : 2.0) * M * N, s);
@@ -809,9 +809,9 @@ struct vb_handle {
 
   // One T2T soft-split transformer layer on the tensor cores (see make_t2t_layer).  X [B*n, Dp] bf16, zero pad columns, updated
   // in place.  Attention with ONE head of width D = 147 / 1323 over n = 3136 / 784 tokens (t2t.py:35) does not fit the fused
-  // attention kernels' head widths: per image, S = Q K^T (tcgen05 GEMM, fp32 out), softmax rows -> bf16 P, O = P V (tcgen05 GEMM
+  // attention kernels' head widths: per image, S = Q K^T (wgmma GEMM, fp32 out), softmax rows -> bf16 P, O = P V (wgmma GEMM
   // against V^T, residual X added in its epilogue).  The score / probability buffers of ONE image (39 + 20 MB at n = 3136) are
-  // reused for every image, so they stay in the 126 MB L2 instead of streaming B x n x n floats through HBM.
+  // reused for every image, so at n = 784 (4 MB) they stay in the 50 MB L2 instead of streaming B x n x n floats through HBM.
   template <typename T>
   void layer_t2t(T* X, int B, int n, const LayerW& l, cudaStream_t s);
 
@@ -985,12 +985,10 @@ struct vb_handle {
   // forked / joined with timing-less events and therefore part of a captured graph): while one half's kernel drains -- last
   // epilogues, CTAs finishing at different times, the dependent launch waiting for the whole grid -- the other half's next
   // kernel already has CTAs on the freed SMs.  Results are bit-identical to the unsplit forward (every kernel's tile
-  // arithmetic is independent of the batch, tests: test_batch_independence_and_determinism).  ViT, DeepViT and CaiT only (the
-  // head-mixing attention kernel's scratch is per stream; T2T and CrossViT fork streams of their own).
-  // MEASURED (profiles/r02_ab_fwd_streams.txt): correct (253 GPU tests, identical logits) but no faster -- ViT-B/16 B = 256
-  // 9.02 / 9.14 ms unsplit vs 9.42 / 9.11 ms split, ViT-L/16-384 47.06 vs 47.30 ms: every kernel here is a persistent grid of
-  // one CTA per SM, so the second stream's CTAs only get SMs as the first kernel's CTAs exit, and what the overlap of the tails
-  // gains the doubled per-launch cost (half the tiles per kernel) loses.  Off by default (VB_FWD_STREAMS=2 enables it).
+  // arithmetic is independent of the batch, tests: test_batch_independence_and_determinism).  ViT, DeepViT and CaiT only (T2T
+  // and CrossViT fork streams of their own).
+  // The split doubles the number of launches (half the tiles per kernel); its speed on the H100 is not measured.  Off by
+  // default (VB_FWD_STREAMS=2 enables it).
   template <typename T>
   void forward_impl(const float* img, int B, int H, int Wd, float* logits, cudaStream_t s) {
     arena.reset();
@@ -1206,8 +1204,8 @@ void vb_handle::linear<__nv_bfloat16>(const __nv_bfloat16* A, int lda, int M, co
   const __nv_bfloat16* res = static_cast<const __nv_bfloat16*>(e.res);
   const bool fast = gemm_bf16_supported(M, L.N, K, lda, L.ldw, ldc) && (res == nullptr || e.ldr % 8 == 0);
   const bool folded = L.ln_c1 != nullptr;
-  VB_CHECK(!folded || (fast && e.ln_stats != nullptr && K % 64 == 0), "internal: LayerNorm-folded Dense needs the tcgen05 path and row statistics");
-  VB_CHECK(e.stats_out == nullptr || fast, "internal: row statistics requested from a non-tcgen05 GEMM");
+  VB_CHECK(!folded || (fast && e.ln_stats != nullptr && K % 64 == 0), "internal: LayerNorm-folded Dense needs the wgmma path and row statistics");
+  VB_CHECK(e.stats_out == nullptr || fast, "internal: row statistics requested from a non-wgmma GEMM");
   ProfScope ps(this, !fast ? PROF_OTHER : e.gelu ? PROF_GEMM_GELU : res ? PROF_GEMM_RES : PROF_GEMM, 2.0 * M * L.N * K,
                2.0 * (static_cast<double>(M) * K + static_cast<double>(L.N) * K + static_cast<double>(M) * L.N * (res ? 2 : 1)), s);
   if (fast) {
@@ -1225,7 +1223,7 @@ void vb_handle::linear<__nv_bfloat16>(const __nv_bfloat16* A, int lda, int M, co
       if (plans.size() > 8192) plans.clear();      // shape sweeps: bounded host memory (a plan is four 128-byte tensor maps)
       GemmBf16 g = gemm_bf16_plan(A, lda, L.Wt, L.ldw, out, ldc, M, L.N, K, e.bias, e.scale, res, e.ldr, e.gelu);
       if (folded) { g.ln_c1 = L.ln_c1; g.ln_stats = e.ln_stats; g.ln_parts = K / 64; g.ln_inv_d = 1.0f / static_cast<float>(K); }
-      if (e.stats_out) { g.stats_out = e.stats_out; g.stats_parts = L.N / 64; }
+      if (e.stats_out) { g.stats_out = e.stats_out; }
       it = plans.emplace(key, g).first;
     }
     gemm_bf16_run(it->second, s);
@@ -1254,8 +1252,8 @@ void vb_handle::layer_t2t<__nv_bfloat16>(__nv_bfloat16* X, int B, int n, const L
   bf* Vt = arena.get<bf>(static_cast<size_t>(B) * Dp * npad);
   // Images are independent: ns of them are in flight on ns streams (the forward's own + side streams), each with its own score /
   // probability buffers.  The per-image kernels are small (16 pair tiles for Q K^T at n = 784) and strictly dependent, so one
-  // stream leaves most SMs idle and pays every launch gap (389 launches, 6.1 of the 6.9 ms T2T step at batch 64).  Two streams
-  // when one image's buffers are large (n = 3136: 59 MB, two of them still fit the 126 MB L2), four otherwise.
+  // stream leaves most SMs idle and pays every launch gap (389 launches per T2T step at batch 64).  Two streams
+  // when one image's buffers are large (n = 3136: 59 MB each, more than the 50 MB L2 already), four otherwise.
   const size_t s_elems = static_cast<size_t>(n) * npad;
   static const char* ns_env = getenv("VB_T2T_STREAMS");
   int ns = ns_env != nullptr ? atoi(ns_env) : (s_elems * 6 > (48u << 20) ? 2 : 4);
@@ -1308,7 +1306,7 @@ void vb_handle::attention_dispatch(const T* q, int ldq, const T* k, int ldk, con
   ProfScope ps(this, PROF_ATTN, 4.0 * B * heads * nq * nk * dh + (variant == 1 ? 2.0 : variant == 2 ? 4.0 : 0.0) * B * nq * nk * heads * heads,
                static_cast<double>(sizeof(T)) * B * heads * dh * (2.0 * nq + 2.0 * nk), s);
   if (attention_fast<T>(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, heads, dh, variant, mix_a, mix_b, g, b, s, scale)) return;
-  VB_CHECK(scale <= 0.f, "internal: a head-padded layer must run on the tcgen05 attention kernel");
+  VB_CHECK(scale <= 0.f, "internal: a head-padded layer must run on the fused attention kernel");
   float* S = arena.get<float>(static_cast<size_t>(B) * heads * nq * ((nk + 15) & ~15));   // row pitch padded for the bf16-P path
   attention_generic<T>(q, ldq, k, ldk, v, ldv, out, ldo, S, B, nq, nk, heads, dh, variant, mix_a, mix_b, g, b, s);
 }
@@ -1479,7 +1477,7 @@ int vb_create(const vb_config* cfg, int device, vb_handle** out) {
     VB_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     VB_CUDA(cudaGetDeviceProperties(&prop, device));
-    VB_CHECK(prop.major == 10, "vb_create: libvitb200 is built for sm_100a (Blackwell B200) only");
+    VB_CHECK(prop.major == 9 && prop.minor == 0, "vb_create: libvitb200 is built for sm_90a (Hopper H100) only");
     std::unique_ptr<vb_handle> h(new vb_handle());
     h->cfg = *cfg;
     h->device = device;
@@ -1848,22 +1846,6 @@ int vb_op_linear(int32_t precision, const float* a, const float* w, const float*
       dO.ensure(static_cast<size_t>(M) * N * 2);
       __nv_bfloat16* dout = static_cast<__nv_bfloat16*>(dO.p);
       GemmBf16 g = gemm_bf16_plan(da, K, static_cast<const __nv_bfloat16*>(dWt.p), K, dout, N, M, N, K, db, ds, dr, N, gelu != 0);
-      if (const char* trace_path = getenv("VB_GEMM_TRACE")) {   // one traced launch, dumped as text: role tag clock
-        DevMem dTrace;
-        dTrace.ensure(4 * 512 * 8);
-        VB_CUDA(cudaMemset(dTrace.p, 0, 4 * 512 * 8));
-        gemm_trace_buffer() = static_cast<long long*>(dTrace.p);
-        gemm_bf16_run(g, 0);
-        VB_CUDA(cudaDeviceSynchronize());
-        gemm_trace_buffer() = nullptr;
-        std::vector<long long> h(4 * 512);
-        VB_CUDA(cudaMemcpy(h.data(), dTrace.p, h.size() * 8, cudaMemcpyDeviceToHost));
-        if (FILE* f = fopen(trace_path, "w")) {
-          for (int r = 0; r < 4; ++r)
-            for (int i = 0; i < 250 && h[r * 512 + 2 * i + 1] != 0; ++i) fprintf(f, "%d %lld %lld\n", r, h[r * 512 + 2 * i], h[r * 512 + 2 * i + 1]);
-          fclose(f);
-        }
-      }
       timed(iters, elapsed_ms, [&] { gemm_bf16_run(g, 0); });
       download<__nv_bfloat16>(dout, out, static_cast<size_t>(M) * N);
     }
@@ -1893,22 +1875,6 @@ int vb_op_attention(int32_t precision, int32_t variant, const float* q, const fl
       dO.ensure(cq * sizeof(T));
       T* o_d = static_cast<T*>(dO.p);
       dS.ensure(static_cast<size_t>(B) * heads * nq * ((nk + 15) & ~15) * 4);
-      DevMem dTrace;
-      const char* trace_path = getenv("VB_ATTN_TRACE");
-      if (trace_path) { dTrace.ensure(4 * 512 * 8); VB_CUDA(cudaMemset(dTrace.p, 0, 4 * 512 * 8)); attn_trace_buffer() = static_cast<long long*>(dTrace.p); }
-      struct TraceOff { ~TraceOff() { attn_trace_buffer() = nullptr; } } trace_off;
-      if (trace_path) {   // one traced launch, dumped as text: role tag clock
-        attention_fast<T>(q_d, inner, k_d, inner, v_d, inner, o_d, inner, B, nq, nk, heads, dim_head, variant, ma, mb, g, bt, 0);
-        VB_CUDA(cudaDeviceSynchronize());
-        std::vector<long long> h(4 * 512);
-        VB_CUDA(cudaMemcpy(h.data(), dTrace.p, h.size() * 8, cudaMemcpyDeviceToHost));
-        attn_trace_buffer() = nullptr;
-        if (FILE* f = fopen(trace_path, "w")) {
-          for (int r = 0; r < 4; ++r)
-            for (int i = 0; i < 250 && h[r * 512 + 2 * i + 1] != 0; ++i) fprintf(f, "%d %lld %lld\n", r, h[r * 512 + 2 * i], h[r * 512 + 2 * i + 1]);
-          fclose(f);
-        }
-      }
       timed(iters, elapsed_ms, [&] {
         if (!attention_fast<T>(q_d, inner, k_d, inner, v_d, inner, o_d, inner, B, nq, nk, heads, dim_head, variant, ma, mb, g, bt, 0))
           attention_generic<T>(q_d, inner, k_d, inner, v_d, inner, o_d, inner, static_cast<float*>(dS.p), B, nq, nk, heads,

@@ -558,8 +558,8 @@ __global__ void broadcast_rows_kernel(const float* __restrict__ vec, T* __restri
 
 // Soft split of T2T: tf.image.extract_patches(sizes k x k, strides s, rates 1, padding SAME) (t2t.py:43) followed by
 // 'b h w c -> b (h w) c' (:44).  Taps outside the image read 0; the patch vector is (k_row, k_col, channel) with the channel
-// fastest.  One CTA per output row (b, t): no 64-bit index arithmetic and no division per element (the first form -- one
-// thread per output element, six divisions each, two of them 64-bit -- ran at 0.4 TB/s: 1.8 of the 8.2 ms T2T step at batch 64).
+// fastest.  One CTA per output row (b, t): no 64-bit index arithmetic and no division per element (one thread per output
+// element would cost six divisions each, two of them 64-bit).
 // C >= 32 (the 147-channel layers): the threads walk the k*k taps and copy each tap's C contiguous channels;
 // small C (the image, C = 3): one thread per column with 32-bit divisions.
 template <typename TI, typename TO>

@@ -1,5 +1,5 @@
 // Launch interfaces of the non-tensor-core kernels (kernels.cu).  T is float (exact-fp32 gate path) or
-// __nv_bfloat16 (activations of the tcgen05 path); all reductions / statistics are fp32.
+// __nv_bfloat16 (activations of the tensor-core path); all reductions / statistics are fp32.
 #pragma once
 #include "common.h"
 
@@ -85,7 +85,7 @@ void pack_weight_bf16(const float* W, __nv_bfloat16* Wt, int K, int N, int ldw, 
 // groups*heads*dhp columns, column (g, h, d >= dh) = 0 (to_qkv: groups 3, to_q: 1, to_kv: 2).  pad_rows == 1: the
 // K = heads*dh input rows become heads*dhp rows, row (h, d >= dh) = 0 (to_out).  `other` is the untouched dimension.
 void pad_heads_f32(const float* W, float* Wp, int other, int groups, int heads, int dh, int dhp, int pad_rows, cudaStream_t s);
-// Constants of a LayerNorm folded into the following Dense (see gemm_tcgen05.cu):
+// Constants of a LayerNorm folded into the following Dense (see gemm_wgmma.cu):
 //   c1[n] = sum_k float(Wt[n,k])   (the gamma-scaled, bf16-rounded weights the tensor core really multiplies)
 //   c2[n] = sum_k beta[k] * W[k,n] + (bias ? bias[n] : 0)
 void ln_fold_consts(const float* W, const __nv_bfloat16* Wt, int ldw, const float* beta, const float* bias, float* c1, float* c2,

@@ -8,9 +8,9 @@
 
 Same constructor kwargs, defaults and assertion messages; `model(img, training=True, **kwargs) -> logits`
 with `img` NHWC float32 `[b, H, W, 3]` and logits float32 `[b, num_classes]`.  Everything below the call is
-hand-written sm_100a CUDA behind `include/vitb200.h`; this file only validates arguments, owns the weight dict
+hand-written sm_90a CUDA behind `include/vitb200.h`; this file only validates arguments, owns the weight dict
 (Keras layouts, SURVEY.md App. B) and marshals pointers.  Two extra keyword-only constructor arguments that the
-reference does not have: `precision` ("bf16" tcgen05 path, default; "fp32" exact gate path) and `device`.
+reference does not have: `precision` ("bf16" tensor-core path, default; "fp32" exact gate path) and `device`.
 
 Semantics notes (SURVEY.md App. D): inference only -- dropout is the identity, so a non-zero
 dropout / emb_dropout / layer_dropout with `training=True` (the reference's default!) cannot be reproduced and
@@ -331,7 +331,7 @@ class _EngineModel:
         self.dropout = _Layer(lambda x: x)               # inference semantics: identity (vit.py:148,166)
         self.mlp_head = _Layer(self.forward_head)
 
-    PROFILE_CLASSES = ("gemm_tcgen05", "attention", "layernorm", "im2col", "other", "gemm_tcgen05_gelu", "gemm_tcgen05_residual")
+    PROFILE_CLASSES = ("gemm_wgmma", "attention", "layernorm", "im2col", "other", "gemm_wgmma_gelu", "gemm_wgmma_residual")
 
     def profile(self, on=True):
         """Record CUDA events around every kernel class on the launch stream (for the roofline report)."""
