@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 4
+#define VB_ABI_VERSION 5
 #if defined(__GNUC__)
 #define VB_API __attribute__((visibility("default")))
 #else
@@ -206,6 +206,42 @@ VB_API int vb_op_patch_merger(int32_t precision, const float* x, const float* ga
  * out [M,N] = act(LN(x) w + bias), act = exact-erf GELU when gelu != 0.  bf16 engine only; N % 64 == 0, K % 64 == 0. */
 VB_API int vb_op_ln_linear(const float* x, const float* gamma, const float* beta, const float* w, const float* bias,
                     int32_t gelu, float* out, int32_t M, int32_t N, int32_t K, int32_t iters, float* elapsed_ms);
+
+/* ---- the kernels in the operand layouts the engine itself uses (strided rows, in-place residuals, row statistics,
+ * fused q|k|v rows, head-padded attention).  Same conventions as above; a result is that of the FIRST launch (later timed
+ * launches may update an in-place residual again). ------------------------------------------------------------------------ */
+
+/* bf16 wgmma GEMM: out[m, out_off + n] = epi(sum_k a[m, k] wt[n, k]), m < M, n < N, k < K.
+ *   a       [M, lda], lda >= K: only columns < K are read.
+ *   wt      the weight in its K-major packed form [b_rows, ldw] (b_rows = 0: N); rows [b_rows, N) read as zero.
+ *   out     [M, ldc]: the whole buffer is uploaded (rounded to bf16 unless out_f32) and downloaded again, so columns the
+ *           GEMM does not write come back unchanged.  out_f32 != 0: fp32 output, plain or bias epilogue only.
+ *   epi     (+bias[N]) -> exact-erf GELU (gelu != 0) -> (*scale[N]) -> (+res[m, n]).  res == out: the residual is the
+ *           output region itself (in place, ldr must equal ldc); otherwise res is a separate [M, ldr] buffer at column 0.
+ *   ln_stats, ln_c1: folded LayerNorm of the A rows (as vb_op_ln_linear runs it): wt must hold gamma-scaled weights, bias the
+ *           c2 = beta.W + bias term, ln_c1[N] the row sums of wt, ln_stats [K/64][M] (sum, sumsq) float pairs of the rows.
+ *   stats_out (may be NULL): receives [N/64][M] (sum, sumsq) float pairs of each 64-column chunk of the stored bf16 rows.
+ * Every leading dimension and out_off must be a multiple of 8; N % 64 == 0, K % 8 == 0. */
+VB_API int vb_op_gemm(const float* a, int32_t lda, const float* wt, int32_t ldw, int32_t b_rows, const float* bias,
+                      const float* scale, int32_t gelu, const float* res, int32_t ldr, const float* ln_stats, const float* ln_c1,
+                      float* out, int32_t ldc, int32_t out_off, int32_t out_f32, float* stats_out, int32_t M, int32_t N, int32_t K,
+                      int32_t iters, float* elapsed_ms);
+
+/* Multi-head attention with explicit layouts, run exactly as the engine dispatches it (fused kernels first, the
+ * materialised-scores path otherwise).  q: [B*nq, ldq], head h of row i at columns [h*dh, (h+1)*dh).  kv == NULL: k and v
+ * are the columns [k_off, ..) and [v_off, ..) of the q buffer (the fused [q|k|v] rows, nk == nq, pitch ldq); otherwise of
+ * kv [B*nk, ldkv] (the [k|v] rows of class / cross attention).  out: [B*nq, ldo], uploaded and downloaded whole.
+ * dh: the activation head width; scale: softmax scale, <= 0 means dh^-0.5 (a head-padded layer passes its model
+ * dim_head^-0.5).  variant / mixes as vb_op_attention. */
+VB_API int vb_op_attention_ex(int32_t precision, int32_t variant, const float* q, int32_t ldq, const float* kv, int32_t ldkv,
+                              int32_t k_off, int32_t v_off, const float* mix_a, const float* mix_b, const float* ln_gamma,
+                              const float* ln_beta, float* out, int32_t ldo, int32_t B, int32_t nq, int32_t nk, int32_t heads,
+                              int32_t dh, float scale, int32_t iters, float* elapsed_ms);
+
+/* Row softmax of fp32 scores into bf16 probabilities (the T2T attention): p[r, j] = softmax_j(s[r, j] * scale) for j < n,
+ * p[r, n..npad) = 0.  s [rows, lds], p [rows, ldp] (uploaded and downloaded whole); n <= npad <= ldp. */
+VB_API int vb_op_softmax_rows(const float* s, int32_t lds, float* p, int32_t ldp, int32_t rows, int32_t n, int32_t npad, float scale,
+                              int32_t iters, float* elapsed_ms);
 
 #ifdef __cplusplus
 }

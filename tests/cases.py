@@ -48,6 +48,9 @@ MID = {
     "merger_mid": dict(kind="patch_merger_vit", image_size=224, patch_size=16, num_classes=100, dim=256, depth=4, heads=4, mlp_dim=512,
                        patch_merge_layer=2),
     "t2t_mid": dict(kind="t2t_vit", image_size=224, num_classes=100, dim=256, depth=2, heads=4, mlp_dim=512),
+    # t2t_small's widths at 288^2 with the default t2t_layers: the first soft-split layer attends over 72^2 = 5184 > 4096 tokens
+    # (the three-pass row softmax, kernels.cu softmax_rows_bf16_big_kernel)
+    "t2t_big_image": dict(kind="t2t_vit", image_size=288, num_classes=10, dim=64, depth=2, heads=4, mlp_dim=128, dim_head=16),
     "cait_mid": dict(kind="cait", image_size=224, patch_size=16, num_classes=100, dim=192, depth=2, cls_depth=2, heads=4,
                      mlp_dim=384, dim_head=48),
 }

@@ -23,7 +23,11 @@ def test_header_symbols_are_exported_and_bound(lib):
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in include/vitb200.h but not exported"
     assert sorted(_lib.SIGNATURES) == declared, "ctypes SIGNATURES must cover exactly the declared ABI"
-    assert lib.vb_abi_version() == 4
+    # ABI 5 added vb_op_gemm / vb_op_attention_ex / vb_op_softmax_rows: header, library and ctypes binding agree on it
+    header = int(re.search(r"#define VB_ABI_VERSION (\d+)", open(os.path.join(ROOT, "include", "vitb200.h")).read()).group(1))
+    assert lib.vb_abi_version() == header == _lib.ABI_VERSION == 5
+    for name in ("vb_op_gemm", "vb_op_attention_ex", "vb_op_softmax_rows"):
+        assert name in declared
 
 
 def test_config_struct_layout_matches_header():

@@ -244,6 +244,25 @@ def test_ragged_batches(lib, name, batch):
     assert (np.abs(got - ref) <= BF16_ATOL + BF16_RTOL * np.abs(ref)).all()
 
 
+@pytest.mark.parametrize("precision", ["fp32", "bf16"])
+def test_deepvit_batch_times_heads_beyond_65535(lib, precision):
+    """DeepViT with 16 heads at batch 4100 on a one-patch image (n = 2 tokens): the re-attention runs over 65 600 (image,
+    head) items, more than a grid's y / z dimension holds (attn_generic_mma.cu rows path in bf16, kernels.cu SIMT path in fp32)."""
+    cfg = oracle.make_config("deepvit", image_size=16, patch_size=16, num_classes=10, dim=64, depth=2, heads=16, mlp_dim=64,
+                             dim_head=16)
+    w = oracle.stress_weights(cfg, 41) if precision == "bf16" else oracle.init_weights(cfg, 41)
+    img = oracle.make_image(cfg, 4100, 42)
+    m = _model(cfg, precision)
+    m.set_weights_dict(w)
+    got = m(img, training=False)
+    ref = oracle.forward_numpy(img, w, cfg)
+    assert got.shape == (4100, 10)
+    if precision == "fp32":
+        np.testing.assert_allclose(got, ref, rtol=1e-3, atol=1e-4)
+    else:
+        assert (np.abs(got - ref) <= BF16_ATOL + BF16_RTOL * np.abs(ref)).all()
+
+
 def test_batch_independence_and_determinism(lib):
     """Images are independent (no cross-sample op): logits of a batch equal logits of its halves, bit for bit,
     and repeated calls are bit-identical (what the data-parallel sharding relies on)."""

@@ -40,15 +40,19 @@ def _linear_case(lib, M, N, K, bias, scale, res, gelu, precision, seed=0):
     return out, ref
 
 
+# M <= 64: the second consumer warpgroup of the 128-row tile has no rows (CaiT class layers, CrossViT cross attention: M = batch)
+SMALL_M = [(1, 256, 64), (2, 192, 128), (8, 768, 192), (63, 384, 64), (64, 256, 256), (65, 128, 64), (127, 512, 200)]
+
+
 @pytest.mark.parametrize("M,N,K", [(128, 256, 64), (128, 128, 64), (256, 512, 768), (394, 768, 768), (100, 64, 8),
-                                   (777, 3072, 768), (1000, 384, 384), (130, 1024, 200), (50432, 768, 768)])
+                                   (777, 3072, 768), (1000, 384, 384), (130, 1024, 200), (50432, 768, 768)] + SMALL_M)
 def test_gemm_bf16_plain(lib, M, N, K):
     out, ref = _linear_case(lib, M, N, K, False, False, False, False, "bf16")
     np.testing.assert_allclose(out, ref, rtol=BF16_RTOL, atol=BF16_ATOL)
 
 
 @pytest.mark.parametrize("bias,scale,res,gelu", [(1, 0, 0, 0), (1, 0, 0, 1), (1, 0, 1, 0), (1, 1, 1, 0), (0, 0, 1, 0), (1, 1, 1, 1)])
-@pytest.mark.parametrize("M,N,K", [(394, 768, 192), (5000, 384, 1536), (641, 2304, 768), (700, 1152, 384)])   # last: 192-wide tiles
+@pytest.mark.parametrize("M,N,K", [(394, 768, 192), (5000, 384, 1536), (641, 2304, 768), (700, 1152, 384)] + SMALL_M)   # 4th: 128-wide tiles
 def test_gemm_bf16_epilogues(lib, M, N, K, bias, scale, res, gelu):
     out, ref = _linear_case(lib, M, N, K, bias, scale, res, gelu, "bf16", seed=M + N)
     np.testing.assert_allclose(out, ref, rtol=BF16_RTOL, atol=BF16_ATOL)
@@ -172,49 +176,77 @@ ATTN_BF16_SIGMA = {0: 1.5e-2, 1: 1.5e-2, 2: 1.5e-2}
 ATTN_BF16_REL = 1.0e-2
 
 
-def _assert_close_sigma(out, ref, sigma_frac, rel):
+def _sigma_worst(out, ref, sigma_frac, rel):
+    """max over elements of |out - ref| / (sigma_frac * std(ref) + rel * |ref|), and the max error itself"""
     err = np.abs(out - ref)
+    bound = sigma_frac * float(ref.std()) + rel * np.abs(ref)
+    return float((err / bound).max()), float(err.max())
+
+
+def _assert_close_sigma(out, ref, sigma_frac, rel):
+    worst, emax = _sigma_worst(out, ref, sigma_frac, rel)
     sig = float(ref.std())
-    bound = sigma_frac * sig + rel * np.abs(ref)
-    worst = float((err / bound).max())
-    print(f"\n[attention bf16] max err {err.max():.3e}, sigma_out {sig:.3e}, max err / sigma_out {err.max() / sig:.3e}, "
+    print(f"\n[attention bf16] max err {emax:.3e}, sigma_out {sig:.3e}, max err / sigma_out {emax / sig:.3e}, "
           f"worst err / bound {worst:.3f}")
-    assert worst <= 1.0, f"max err {err.max():.4e} at sigma_out {sig:.4e}: {worst:.2f} x the bound"
+    assert worst <= 1.0, f"max err {emax:.4e} at sigma_out {sig:.4e}: {worst:.2f} x the bound"
 
 
-@pytest.mark.parametrize("ramp", ["up", "down", "zigzag"])
-@pytest.mark.parametrize("B,n,heads", [(2, 577, 2), (3, 197, 3), (1, 300, 1)])
-def test_attention_lazy_rescale(lib, B, n, heads, ramp):
-    """The fused attention kernel rescales its running output whenever a key block raises a row max;
-    N(0,1) scores barely move it (attn_flash.cu, `alpha`), so this case scales the
-    keys of block j by a ramp: with 'up' every later block beats the running reference by ~15 in log2 units (the rescale and
-    the l correction run for every j > 0), 'down' keeps the first block's reference throughout (later exponents underflow
-    towards 0), 'zigzag' alternates."""
-    from vit_tensorflow_b200 import _lib
-    dh = 64
+FLASH_FK = 64      # keys per block of attn_flash.cu (FK)
+
+
+def _rescale_case(B, n, heads, ramp, dh=64):
+    """q, k, v (bf16-rounded) for test_attention_lazy_rescale, and the fraction of rows the construction reaches: the scores
+    in the kernel's log2 units (dh^-0.5 * log2(e)) per 64-key block."""
     rng = np.random.default_rng(n + heads)
     inner = heads * dh
-    q = bf16_round(rng.standard_normal((B, n, inner), dtype=np.float32))
+    nblk = (n + FLASH_FK - 1) // FLASH_FK
+    blk = lambda j: slice(j * FLASH_FK, min((j + 1) * FLASH_FK, n))
+    q = rng.standard_normal((B, n, inner), dtype=np.float32)
     k = rng.standard_normal((B, n, inner), dtype=np.float32)
     v = bf16_round(rng.standard_normal((B, n, inner), dtype=np.float32))
-    nblk = (n + 127) // 128
-    f = {"up": [1 + 4 * j for j in range(nblk)], "down": [1 + 4 * (nblk - 1 - j) for j in range(nblk)],
-         "zigzag": [1 + 6 * (j % 2) + j for j in range(nblk)]}[ramp]
-    for j in range(nblk):
-        k[:, j * 128:(j + 1) * 128] *= f[j]
-    k = bf16_round(k)
-    out, _ = _lib.op_attention(q, k, v, heads, 0, precision="bf16")
-    ref = _attention_ref(q, k, v, heads, 0, None, None, None, None)
-    # the ramp must really cross the kernel's threshold (8 in log2 units after the dh^-0.5 * log2(e) scaling) ...
+    u = np.ones(inner, np.float32)
+    if ramp in ("up", "down", "zigzag"):          # geometric: a block's max beats the previous blocks' by ~1.6x
+        f = {"up": [1.6 ** j for j in range(nblk)], "down": [1.6 ** (nblk - 1 - j) for j in range(nblk)],
+             "zigzag": [(1 + 5 * (j % 2)) * 1.1 ** j for j in range(nblk)]}[ramp]
+        for j in range(nblk):
+            k[:, blk(j)] *= f[j]
+    elif ramp == "ragged_max":   # every query leans on u, the last block's keys on 2u: q.k dh^-0.5 ~ 16 there, ~N(0, 1) elsewhere
+        q = u + 0.5 * q
+        k[:, blk(nblk - 1)] = 2 * u + 0.5 * k[:, blk(nblk - 1)]
+    else:   # "underflow": every query leans on u, block 0 on +8u, block 1 on -8u: q.k dh^-0.5 = +-64 (+-2 of noise)
+        q = u + 0.25 * q
+        k[:, blk(0)] = 8 * u + 0.25 * k[:, blk(0)]
+        k[:, blk(1)] = -8 * u + 0.25 * k[:, blk(1)]
+    q, k = bf16_round(q), bf16_round(k)
     sp = lambda t: t.reshape(B, n, heads, dh).transpose(0, 2, 1, 3).astype(np.float64)
     s2 = np.einsum('bhid,bhjd->bhij', sp(q), sp(k)) * dh ** -0.5 * 1.4426950408889634
-    bm = np.stack([s2[..., j * 128:(j + 1) * 128].max(-1) for j in range(nblk)], -1)      # [B, h, n, nblk] block row maxima
+    bm = np.stack([s2[..., blk(j)].max(-1) for j in range(nblk)], -1)          # [B, h, n, nblk] block row maxima
     run = np.maximum.accumulate(bm, -1)
-    crossed = (bm[..., 1:] > run[..., :-1] + 8.0)
-    if ramp != "down":
-        assert crossed.any(-1).mean() > 0.9, "test construction: the ramp does not trigger the lazy rescale"
-    else:
-        assert crossed.any(-1).mean() < 0.2      # a few rows whose first block happens to score low still cross
+    full = n // FLASH_FK                                                      # blocks of 64 valid keys
+    raised = bm[..., 1:full] > run[..., :full - 1]                            # a full block j > 0 raises the running max: alpha < 1
+    arg = s2.argmax(-1)
+    reach = {"up": raised.mean(), "down": (arg < FLASH_FK).mean(), "zigzag": raised.any(-1).mean(),
+             "ragged_max": (arg >= (nblk - 1) * FLASH_FK).mean(),
+             # p of block 1 below 2^-149, the smallest fp32 subnormal: exactly 0 however exp2 is evaluated
+             "underflow": (s2[..., blk(1)].max(-1) - s2.max(-1) < -150).mean()}[ramp]
+    return q, k, v, float(reach)
+
+
+@pytest.mark.parametrize("ramp", ["up", "down", "zigzag", "ragged_max", "underflow"])
+@pytest.mark.parametrize("B,n,heads", [(2, 577, 2), (3, 197, 3), (1, 300, 1), (3, 191, 3), (2, 129, 2)])
+def test_attention_lazy_rescale(lib, B, n, heads, ramp):
+    """The flash kernel (attn_flash.cu) streams the keys in blocks of FK = 64 and on every block raises its running row max
+    and rescales the running output and row sum by alpha = 2^(m_old - m_new).  N(0,1) scores barely move the max after the
+    first block, so the keys are scaled per 64-key block: 'up' makes (almost) every later block raise the max, 'down' keeps
+    the first block's max throughout, 'zigzag' alternates.  'ragged_max' puts the row maxima into the last, partial block
+    (n % 64 = 1 at n = 577 / 129, 5 at n = 197, 63 at n = 191: valid keys next to masked ones).  'underflow' puts block 1's scores ~180
+    log2 units below block 0's, so its probabilities are exactly 0 and it must contribute nothing (and no NaN)."""
+    from vit_tensorflow_b200 import _lib
+    q, k, v, reach = _rescale_case(B, n, heads, ramp)
+    assert reach > (0.99 if ramp in ("ragged_max", "underflow") else 0.9), f"test construction reaches only {reach:.2f} of the rows"
+    out, _ = _lib.op_attention(q, k, v, heads, 0, precision="bf16")
+    ref = _attention_ref(q, k, v, heads, 0, None, None, None, None)
+    assert np.isfinite(out).all()
     _assert_close_sigma(out, ref, 1.5e-2, 1.0e-2)
 
 

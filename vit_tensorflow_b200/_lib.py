@@ -14,6 +14,7 @@ LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "libvitb200.so")
 KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6}
 PRECISION = {"fp32": 0, "float32": 0, "bf16": 1, "bfloat16": 1}
 MEM_HOST, MEM_DEVICE = 0, 1
+ABI_VERSION = 5                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
 
 
 class VbConfig(C.Structure):
@@ -65,6 +66,11 @@ SIGNATURES = {
     "vb_op_layernorm": (C.c_int, [C.c_int32] + [C.c_void_p] * 4 + [C.c_int32] * 3 + [_f32p]),
     "vb_op_patch_merger": (C.c_int, [C.c_int32] + [C.c_void_p] * 5 + [C.c_int32] * 5 + [_f32p]),
     "vb_op_ln_linear": (C.c_int, [C.c_void_p] * 5 + [C.c_int32, C.c_void_p] + [C.c_int32] * 4 + [_f32p]),
+    "vb_op_gemm": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                             C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] + [C.c_int32] * 4 + [_f32p]),
+    "vb_op_attention_ex": (C.c_int, [C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 5 +
+                           [C.c_int32] * 6 + [C.c_float, C.c_int32, _f32p]),
+    "vb_op_softmax_rows": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 4 + [C.c_float, C.c_int32, _f32p]),
 }
 
 _lib = None
@@ -82,7 +88,7 @@ def load() -> C.CDLL:
             fn = getattr(lib, name)
             fn.restype = res
             fn.argtypes = args
-        if lib.vb_abi_version() != 4:
+        if lib.vb_abi_version() != ABI_VERSION:
             raise VbError("libvitb200 ABI version mismatch")
         _lib = lib
     return _lib
@@ -146,6 +152,55 @@ def op_ln_linear(x, gamma, beta, w, bias=None, gelu=False, iters=0):
     check(load().vb_op_ln_linear(_ptr(x), _ptr(gamma), _ptr(beta), _ptr(w), _ptr(bias), int(bool(gelu)), _ptr(out), M, N, K, iters,
                                  C.byref(ms)))
     return out, (ms.value if iters > 0 else None)
+
+
+def op_gemm(a, wt, N, K, out, bias=None, scale=None, gelu=False, res=None, out_off=0, out_f32=False, ln_stats=None, ln_c1=None,
+            want_stats=False, iters=0):
+    """The bf16 wgmma GEMM in the engine's operand layouts (vb_op_gemm): a [M, lda], wt K-major [b_rows, ldw] (b_rows < N: the
+    missing rows read as zero), out [M, ldc] initial contents (columns [out_off, out_off + N) are written); res: None, a
+    separate [M, ldr] array, or the string "out" for the in-place residual.  Returns (out [M, ldc], stats [N/64, M, 2] or None,
+    ms per launch or None)."""
+    a, wt, bias, scale, ln_stats, ln_c1 = map(_f32, (a, wt, bias, scale, ln_stats, ln_c1))
+    out = np.array(out, dtype=np.float32, order="C", copy=True)
+    M, lda = a.shape
+    b_rows, ldw = wt.shape
+    ldc = out.shape[1]
+    if isinstance(res, str):
+        assert res == "out"
+        res_p, ldr = _ptr(out), ldc
+    else:
+        res = _f32(res)
+        res_p, ldr = _ptr(res), (0 if res is None else res.shape[1])
+    stats = np.empty((N // 64, M, 2), np.float32) if want_stats else None
+    ms = C.c_float(0)
+    check(load().vb_op_gemm(_ptr(a), lda, _ptr(wt), ldw, b_rows, _ptr(bias), _ptr(scale), int(bool(gelu)), res_p, ldr, _ptr(ln_stats),
+                            _ptr(ln_c1), _ptr(out), ldc, out_off, int(bool(out_f32)), _ptr(stats), M, N, K, iters, C.byref(ms)))
+    return out, stats, (ms.value if iters > 0 else None)
+
+
+def op_attention_ex(q, heads, dh, out, kv=None, k_off=0, v_off=0, variant=0, mix_a=None, mix_b=None, ln_gamma=None,
+                    ln_beta=None, scale=0.0, precision="bf16", iters=0):
+    """Attention in the engine's layouts (vb_op_attention_ex): q [B, nq, ldq]; kv None (k, v at columns k_off / v_off of the q rows)
+    or [B, nk, ldkv]; out [B, nq, ldo] initial contents, returned whole.  scale <= 0: dh^-0.5.  Returns (out, ms or None)."""
+    q, kv, mix_a, mix_b, ln_gamma, ln_beta = map(_f32, (q, kv, mix_a, mix_b, ln_gamma, ln_beta))
+    out = np.array(out, dtype=np.float32, order="C", copy=True)
+    B, nq, ldq = q.shape
+    nk = nq if kv is None else kv.shape[1]
+    ldkv = 0 if kv is None else kv.shape[2]
+    ms = C.c_float(0)
+    check(load().vb_op_attention_ex(PRECISION[precision], variant, _ptr(q), ldq, _ptr(kv), ldkv, k_off, v_off, _ptr(mix_a), _ptr(mix_b),
+                                    _ptr(ln_gamma), _ptr(ln_beta), _ptr(out), out.shape[2], B, nq, nk, heads, dh, float(scale), iters,
+                                    C.byref(ms)))
+    return out, (ms.value if iters > 0 else None)
+
+
+def op_softmax_rows(s, n, npad, scale, p, iters=0):
+    """softmax_rows_bf16 (vb_op_softmax_rows): s [rows, lds] fp32 scores, p [rows, ldp] initial contents; returns (p, ms or None)."""
+    s = _f32(s)
+    p = np.array(p, dtype=np.float32, order="C", copy=True)
+    ms = C.c_float(0)
+    check(load().vb_op_softmax_rows(_ptr(s), s.shape[1], _ptr(p), p.shape[1], s.shape[0], n, npad, float(scale), iters, C.byref(ms)))
+    return p, (ms.value if iters > 0 else None)
 
 
 def op_patch_merger(x, gamma, beta, queries, precision="bf16", iters=0):

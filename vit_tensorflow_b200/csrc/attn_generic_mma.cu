@@ -27,14 +27,23 @@ __device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a
 constexpr int MAXDH = 128;
 constexpr int PITCH = MAXDH + 8;   // bf16 elements; +8 keeps the fragment loads bank-conflict free
 
+// Every kernel of this file takes its (tile, b * heads + h) item from a flat blockIdx.x, tile index fastest, so B * heads is
+// not bounded by the 65 535 of gridDim.y / gridDim.z; flat_blocks() checks the product against gridDim.x's 2^31 - 1.
+unsigned flat_blocks(long long tiles, long long items) {
+  const long long n = tiles * items;
+  VB_CHECK(n > 0 && n <= 0x7fffffffLL, "attention: grid of " + std::to_string(n) + " blocks exceeds 2^31 - 1");
+  return static_cast<unsigned>(n);
+}
+
 // S[bh, i, j] = scale * sum_d q[b,i,h,d] k[b,j,h,d];  block: 64 x 64 tile, 4 warps x (16 rows x 64 cols)
 __global__ void __launch_bounds__(128)
 scores_mma_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloat16* __restrict__ k, int ldk, float* __restrict__ S,
                   int heads, int nq, int nk, int dh, float scale, int lds) {
   __shared__ __align__(16) __nv_bfloat16 Qs[64][PITCH];
   __shared__ __align__(16) __nv_bfloat16 Ks[64][PITCH];
-  const int bh = blockIdx.z, b = bh / heads, h = bh % heads;
-  const int i0 = blockIdx.y * 64, j0 = blockIdx.x * 64;
+  const int kt = (nk + 63) / 64, qt = (nq + 63) / 64;
+  const int bh = blockIdx.x / (kt * qt), b = bh / heads, h = bh % heads;
+  const int i0 = (blockIdx.x / kt % qt) * 64, j0 = (blockIdx.x % kt) * 64;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int vec = dh >> 3;                                        // 16-byte vectors per row
   for (int e = threadIdx.x; e < 64 * vec; e += 128) {
@@ -91,8 +100,9 @@ pv_mma_kernel(const float* __restrict__ P, const __nv_bfloat16* __restrict__ v, 
   __shared__ __align__(16) __nv_bfloat16 Ps[64][64 + 8];
   __shared__ __align__(16) __nv_bfloat16 Pl[SPLIT ? 64 : 1][64 + 8];
   __shared__ __align__(16) __nv_bfloat16 Vt[MAXDH][64 + 8];        // transposed: Vt[d][j]
-  const int bh = blockIdx.y, b = bh / heads, h = bh % heads;
-  const int i0 = blockIdx.x * 64;
+  const int qt = (nq + 63) / 64;
+  const int bh = blockIdx.x / qt, b = bh / heads, h = bh % heads;
+  const int i0 = (blockIdx.x % qt) * 64;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int ntiles = dh >> 3;
   float acc[MAXDH / 8][4];
@@ -168,7 +178,7 @@ mid_fused_kernel(float* __restrict__ S, const float* __restrict__ mix_a, const f
   extern __shared__ float buf[];                    // [heads][nk] then 2 x [heads*heads] mix matrices
   float* Wa = buf + heads * nk;
   float* Wb = Wa + heads * heads;
-  const int i = blockIdx.x, b = blockIdx.y;
+  const int i = blockIdx.x % nq, b = blockIdx.x / nq;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
   const size_t plane = static_cast<size_t>(nq) * nk;
   float* base = S + (static_cast<size_t>(b) * heads * nq + i) * nk;        // head h row at base + h * plane
@@ -233,8 +243,9 @@ scores_stripe_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bf
   const int pitch = dh + 8;                                         // bf16; rows stay 16-byte aligned and conflict free
   __nv_bfloat16* Qs = reinterpret_cast<__nv_bfloat16*>(sc_smem);    // [64][pitch]
   __nv_bfloat16* Ks = Qs + 64 * pitch;                              // [nk8][pitch]
-  const int bh = blockIdx.y, b = bh / heads, h = bh % heads;
-  const int i0 = blockIdx.x * 64;
+  const int qt = (nq + 63) / 64;
+  const int bh = blockIdx.x / qt, b = bh / heads, h = bh % heads;
+  const int i0 = (blockIdx.x % qt) * 64;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int vec = dh >> 3, nk8 = (nk + 7) & ~7;
   // (per-row 1-D bulk/TMA copies were tried here and in the PV kernel: 96-832 byte copies issued by one warp were
@@ -433,8 +444,9 @@ pv_rows_kernel(const float* __restrict__ S, int lds, int nkp, const __nv_bfloat1
   constexpr int P_ELEMS = 64 * PP, V_ELEMS = 64 * VP;
   constexpr int STAGE_ELEMS = (SPLIT ? 2 : 1) * P_ELEMS + V_ELEMS;
   __nv_bfloat16* sm = reinterpret_cast<__nv_bfloat16*>(pv_smem);
-  const int bh = blockIdx.y, b = bh / heads, h = bh % heads;
-  const int i0 = blockIdx.x * 64;
+  const int qt = (nq + 63) / 64;
+  const int bh = blockIdx.x / qt, b = bh / heads, h = bh % heads;
+  const int i0 = (blockIdx.x % qt) * 64;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int ntiles = dh >> 3, vec = dh >> 3;
   const int nchunks = (nk + 63) / 64;
@@ -557,7 +569,8 @@ bool attention_rows_path(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k
       VB_CUDA(cudaFuncSetAttribute(scores_stripe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sc_smem));
       configured[dev & 255] = sc_smem;
     }
-    scores_stripe_kernel<<<dim3((nq + 63) / 64, B * heads), 128, sc_smem, s>>>(q, ldq, k, ldk, S, heads, nq, nk, dh, scale, lds);
+    scores_stripe_kernel<<<flat_blocks((nq + 63) / 64, static_cast<long long>(B) * heads), 128, sc_smem, s>>>(q, ldq, k, ldk, S, heads, nq,
+                                                                                                             nk, dh, scale, lds);
   }
   VB_CUDA(cudaGetLastError());
   const long long rows = static_cast<long long>(B) * nq;
@@ -571,7 +584,7 @@ bool attention_rows_path(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k
     else launch_mid_rows<16, 4, 2>(S, mixp, nq, nk, lds, nkp, rows, variant, s);
   }
   VB_CUDA(cudaGetLastError());
-  const dim3 grid((nq + 63) / 64, B * heads);
+  const unsigned grid = flat_blocks((nq + 63) / 64, static_cast<long long>(B) * heads);
   if (variant == 1) {
     constexpr int smem = 2 * (2 * 64 * 72 + 64 * (MAXDH + 8)) * 2;
     static unsigned long long seen[4] = {0, 0, 0, 0};
@@ -633,12 +646,15 @@ bool attention_generic_mma(const __nv_bfloat16* q, int ldq, const __nv_bfloat16*
   static unsigned long long seen[4] = {0, 0, 0, 0};
   if (first_use_on_this_device(seen)) VB_CUDA(cudaFuncSetAttribute(mid_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   const float scale = 1.0f / sqrtf(static_cast<float>(dh));
-  scores_mma_kernel<<<dim3((nk + 63) / 64, (nq + 63) / 64, B * heads), 128, 0, s>>>(q, ldq, k, ldk, S, heads, nq, nk, dh, scale, nk);
+  const long long items = static_cast<long long>(B) * heads;
+  scores_mma_kernel<<<flat_blocks(static_cast<long long>((nk + 63) / 64) * ((nq + 63) / 64), items), 128, 0, s>>>(q, ldq, k, ldk, S, heads,
+                                                                                                                  nq, nk, dh, scale, nk);
   VB_CUDA(cudaGetLastError());
-  mid_fused_kernel<<<dim3(nq, B), 256, smem, s>>>(S, mix_a, mix_b, ln_gamma, ln_beta, heads, nq, nk, variant);
+  mid_fused_kernel<<<flat_blocks(nq, B), 256, smem, s>>>(S, mix_a, mix_b, ln_gamma, ln_beta, heads, nq, nk, variant);
   VB_CUDA(cudaGetLastError());
-  if (variant == 1) pv_mma_kernel<true><<<dim3((nq + 63) / 64, B * heads), 128, 0, s>>>(S, v, ldv, out, ldo, heads, nq, nk, dh);
-  else pv_mma_kernel<false><<<dim3((nq + 63) / 64, B * heads), 128, 0, s>>>(S, v, ldv, out, ldo, heads, nq, nk, dh);
+  const unsigned pv_grid = flat_blocks((nq + 63) / 64, items);
+  if (variant == 1) pv_mma_kernel<true><<<pv_grid, 128, 0, s>>>(S, v, ldv, out, ldo, heads, nq, nk, dh);
+  else pv_mma_kernel<false><<<pv_grid, 128, 0, s>>>(S, v, ldv, out, ldo, heads, nq, nk, dh);
   VB_CUDA(cudaGetLastError());
   count_launch(3);
   return true;

@@ -1970,4 +1970,101 @@ int vb_op_ln_linear(const float* x, const float* gamma, const float* beta, const
   });
 }
 
+int vb_op_gemm(const float* a, int32_t lda, const float* wt, int32_t ldw, int32_t b_rows, const float* bias, const float* scale,
+               int32_t gelu, const float* res, int32_t ldr, const float* ln_stats, const float* ln_c1, float* out, int32_t ldc,
+               int32_t out_off, int32_t out_f32, float* stats_out, int32_t M, int32_t N, int32_t K, int32_t iters, float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    VB_CHECK(a && wt && out && M > 0 && N > 0 && K > 0 && lda >= K && ldw >= K && b_rows >= 0 && b_rows <= N && out_off >= 0 &&
+             out_off + N <= ldc, "vb_op_gemm: bad arguments");
+    const bool in_place = res != nullptr && res == out;
+    VB_CHECK(!in_place || ldr == ldc, "vb_op_gemm: an in-place residual has the output's pitch (ldr == ldc)");
+    VB_CHECK(res == nullptr || in_place || ldr >= N, "vb_op_gemm: ldr < N");
+    VB_CHECK((ln_stats == nullptr) == (ln_c1 == nullptr), "vb_op_gemm: the folded LayerNorm needs both ln_stats and ln_c1");
+    VB_CHECK(ln_c1 == nullptr || (bias != nullptr && K % 64 == 0), "vb_op_gemm: the folded LayerNorm needs the c2 bias and K % 64 == 0");
+    DevMem dA, dW, dB, dS, dR, dO, dC1, dLs, dSo;
+    const __nv_bfloat16* da = upload<__nv_bfloat16>(dA, a, static_cast<size_t>(M) * lda);
+    const __nv_bfloat16* dw = upload<__nv_bfloat16>(dW, wt, static_cast<size_t>(b_rows > 0 ? b_rows : N) * ldw);
+    const float* db = bias ? upload<float>(dB, bias, N) : nullptr;
+    const float* ds = scale ? upload<float>(dS, scale, N) : nullptr;
+    const size_t co = static_cast<size_t>(M) * ldc;
+    void* dout = out_f32 ? static_cast<void*>(upload<float>(dO, out, co) + out_off)
+                         : static_cast<void*>(upload<__nv_bfloat16>(dO, out, co) + out_off);
+    const __nv_bfloat16* dr = in_place ? static_cast<const __nv_bfloat16*>(dout)
+                              : res ? upload<__nv_bfloat16>(dR, res, static_cast<size_t>(M) * ldr) : nullptr;
+    // the plan exactly as vb_handle::linear / gemm_cached build it
+    GemmBf16 g = gemm_bf16_plan(da, lda, dw, ldw, static_cast<__nv_bfloat16*>(dout), ldc, M, N, K, db, ds, dr, ldr, gelu != 0,
+                                out_f32 != 0, b_rows);
+    if (ln_c1) {
+      g.ln_c1 = upload<float>(dC1, ln_c1, N);
+      g.ln_stats = upload<float>(dLs, ln_stats, static_cast<size_t>(K / 64) * M * 2);
+      g.ln_parts = K / 64;
+      g.ln_inv_d = 1.0f / static_cast<float>(K);
+    }
+    const size_t cs = static_cast<size_t>(N / 64) * M * 2;
+    if (stats_out) { dSo.ensure(cs * sizeof(float)); g.stats_out = static_cast<float*>(dSo.p); }
+    auto launch = [&] { gemm_bf16_run(g, 0); };
+    timed(0, nullptr, launch);                 // the result is the first launch's: an in-place residual accumulates on every launch
+    if (out_f32) download<float>(static_cast<const float*>(dO.p), out, co);
+    else download<__nv_bfloat16>(static_cast<const __nv_bfloat16*>(dO.p), out, co);
+    if (stats_out) download<float>(g.stats_out, stats_out, cs);
+    if (iters > 0) timed(iters, elapsed_ms, launch);
+  });
+}
+
+int vb_op_attention_ex(int32_t precision, int32_t variant, const float* q, int32_t ldq, const float* kv, int32_t ldkv, int32_t k_off,
+                       int32_t v_off, const float* mix_a, const float* mix_b, const float* ln_gamma, const float* ln_beta, float* out,
+                       int32_t ldo, int32_t B, int32_t nq, int32_t nk, int32_t heads, int32_t dh, float scale, int32_t iters,
+                       float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    const bool fused = kv == nullptr;                  // k, v inside the q rows ([q|k|v]) or inside separate [k|v] rows
+    const int ldk = fused ? ldq : ldkv;
+    const long long inner = static_cast<long long>(heads) * dh;
+    VB_CHECK(q && out && B > 0 && nq > 0 && nk > 0 && heads > 0 && dh > 0 && ldq >= inner && ldo >= inner && k_off >= 0 &&
+             v_off >= 0 && k_off + inner <= ldk && v_off + inner <= ldk && (!fused || nk == nq), "vb_op_attention_ex: bad arguments");
+    VB_CHECK(variant >= 0 && variant <= 2, "vb_op_attention_ex: variant must be 0, 1 or 2");
+    attention_mix_cache_clear();
+    DevMem dQ, dKV, dO, dS, dMa, dMb, dG, dBt;
+    const float* ma = mix_a ? upload<float>(dMa, mix_a, heads * heads) : nullptr;
+    const float* mb = mix_b ? upload<float>(dMb, mix_b, heads * heads) : nullptr;
+    const float* g = ln_gamma ? upload<float>(dG, ln_gamma, heads) : nullptr;
+    const float* bt = ln_beta ? upload<float>(dBt, ln_beta, heads) : nullptr;
+    const size_t cq = static_cast<size_t>(B) * nq * ldq, ckv = static_cast<size_t>(B) * nk * ldk, co = static_cast<size_t>(B) * nq * ldo;
+    auto run = [&](auto tag) {
+      using T = decltype(tag);
+      const T* q_d = upload<T>(dQ, q, cq);
+      const T* kv_d = fused ? q_d : upload<T>(dKV, kv, ckv);
+      T* o_d = upload<T>(dO, out, co);
+      dS.ensure(static_cast<size_t>(B) * heads * nq * ((nk + 15) & ~15) * 4);
+      // vb_handle::attention_dispatch without the handle's arena and profiler
+      timed(iters, elapsed_ms, [&] {
+        if (attention_fast<T>(q_d, ldq, kv_d + k_off, ldk, kv_d + v_off, ldk, o_d, ldo, B, nq, nk, heads, dh, variant, ma, mb, g, bt, 0,
+                              scale))
+          return;
+        VB_CHECK(scale <= 0.f, "vb_op_attention_ex: an explicit softmax scale needs the fused attention kernels");
+        attention_generic<T>(q_d, ldq, kv_d + k_off, ldk, kv_d + v_off, ldk, o_d, ldo, static_cast<float*>(dS.p), B, nq, nk, heads, dh,
+                             variant, ma, mb, g, bt, 0);
+      });
+      download<T>(o_d, out, co);
+    };
+    if (precision == VB_PRECISION_FP32) run(float());
+    else run(__nv_bfloat16());
+  });
+}
+
+int vb_op_softmax_rows(const float* s, int32_t lds, float* p, int32_t ldp, int32_t rows, int32_t n, int32_t npad, float scale,
+                       int32_t iters, float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    VB_CHECK(s && p && rows > 0 && n > 0 && n <= lds && n <= npad && npad <= ldp, "vb_op_softmax_rows: bad arguments");
+    DevMem dS, dP;
+    const float* s_d = upload<float>(dS, s, static_cast<size_t>(rows) * lds);
+    __nv_bfloat16* p_d = upload<__nv_bfloat16>(dP, p, static_cast<size_t>(rows) * ldp);
+    const float scale_log2 = scale * 1.4426950408889634f;       // as vb_handle::layer_t2t passes it
+    timed(iters, elapsed_ms, [&] { softmax_rows_bf16(s_d, lds, p_d, ldp, rows, n, npad, scale_log2, 0); });
+    download<__nv_bfloat16>(p_d, p, static_cast<size_t>(rows) * ldp);
+  });
+}
+
 }  // extern "C"

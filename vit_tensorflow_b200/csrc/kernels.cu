@@ -364,8 +364,9 @@ attn_scores_kernel(const T* __restrict__ q, int ldq, const T* __restrict__ k, in
                    int nk, int dh, float scale) {
   __shared__ float Qs[32][33];
   __shared__ float Ks[32][33];
-  const int bh = blockIdx.z, b = bh / heads, h = bh % heads;
-  const int i0 = blockIdx.y * 32, j0 = blockIdx.x * 32;
+  const int kt = (nk + 31) / 32, qt = (nq + 31) / 32;              // flat grid, key tile fastest: no 65 535 limit on B * heads
+  const int bh = blockIdx.x / (kt * qt), b = bh / heads, h = bh % heads;
+  const int i0 = (blockIdx.x / kt % qt) * 32, j0 = (blockIdx.x % kt) * 32;
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   float acc[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
   for (int d0 = 0; d0 < dh; d0 += 32) {
@@ -448,8 +449,9 @@ attn_pv_kernel(const float* __restrict__ S, const T* __restrict__ v, int ldv, T*
                int dh) {
   __shared__ float Ps[32][33];
   __shared__ float Vs[32][33];
-  const int bh = blockIdx.z, b = bh / heads, h = bh % heads;
-  const int i0 = blockIdx.y * 32, d0 = blockIdx.x * 32;
+  const int dt = (dh + 31) / 32, qt = (nq + 31) / 32;              // flat grid, column tile fastest
+  const int bh = blockIdx.x / (dt * qt), b = bh / heads, h = bh % heads;
+  const int i0 = (blockIdx.x / dt % qt) * 32, d0 = (blockIdx.x % dt) * 32;
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   float acc[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
   for (int j0 = 0; j0 < nk; j0 += 32) {
@@ -791,8 +793,9 @@ void gemm_simt(const TA* A, int lda, const TW* W, int wsk, int wsn, TO* out, int
 template <typename T>
 void attn_scores(const T* q, int ldq, const T* k, int ldk, float* S, int B, int heads, int nq, int nk, int dh, float scale,
                  cudaStream_t s) {
-  dim3 grid((nk + 31) / 32, (nq + 31) / 32, B * heads);
-  attn_scores_kernel<T><<<grid, 256, 0, s>>>(q, ldq, k, ldk, S, heads, nq, nk, dh, scale);
+  const long long blocks = static_cast<long long>((nk + 31) / 32) * ((nq + 31) / 32) * B * heads;
+  VB_CHECK(blocks <= 0x7fffffffLL, "attention scores: grid of " + std::to_string(blocks) + " blocks exceeds 2^31 - 1");
+  attn_scores_kernel<T><<<static_cast<unsigned>(blocks), 256, 0, s>>>(q, ldq, k, ldk, S, heads, nq, nk, dh, scale);
   VB_LAUNCHED();
 }
 
@@ -812,8 +815,9 @@ void attn_softmax(float* S, long long rows, int nk, cudaStream_t s) {
 
 template <typename T>
 void attn_pv(const float* S, const T* v, int ldv, T* out, int ldo, int B, int heads, int nq, int nk, int dh, cudaStream_t s) {
-  dim3 grid((dh + 31) / 32, (nq + 31) / 32, B * heads);
-  attn_pv_kernel<T><<<grid, 256, 0, s>>>(S, v, ldv, out, ldo, heads, nq, nk, dh);
+  const long long blocks = static_cast<long long>((dh + 31) / 32) * ((nq + 31) / 32) * B * heads;
+  VB_CHECK(blocks <= 0x7fffffffLL, "attention PV: grid of " + std::to_string(blocks) + " blocks exceeds 2^31 - 1");
+  attn_pv_kernel<T><<<static_cast<unsigned>(blocks), 256, 0, s>>>(S, v, ldv, out, ldo, heads, nq, nk, dh);
   VB_LAUNCHED();
 }
 
