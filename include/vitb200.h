@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 5
+#define VB_ABI_VERSION 6
 #if defined(__GNUC__)
 #define VB_API __attribute__((visibility("default")))
 #else
@@ -93,7 +93,11 @@ VB_API int vb_finalize(vb_handle* h);
  * memory (img_mem); logits: float32 [batch,num_classes] written to host or device memory (logits_mem).
  * stream: a cudaStream_t (may be NULL = default stream).  With device buffers the call is asynchronous on
  * `stream`; with a host logits buffer it returns after the copy completes.
- * h, w may be smaller than the configured image (pos_embedding[:, :n+1] truncation, vit.py:165). */
+ * h, w may be smaller than the configured image (pos_embedding[:, :n+1] truncation, vit.py:165).
+ * On a stream other than NULL / cudaStreamLegacy the forward of one (image pointer, logits pointer, batch, h, w, stream)
+ * combination runs eagerly on its first call, is captured into a CUDA graph on its second and replayed from the third on
+ * (vb_graph_stats counts this).  Every call of a handle uses the same workspace, so calls on different streams must be
+ * ordered by the caller (an event or a synchronisation between them). */
 VB_API int vb_forward(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, int32_t img_h, int32_t img_w,
                float* logits, int32_t logits_mem, void* stream);
 
@@ -159,6 +163,12 @@ VB_API int vb_forward_allgather(vb_handle* h, const float* img, int32_t img_mem,
 
 /* Kernels launched by this handle's most recent forward call. */
 VB_API int64_t vb_last_launch_count(vb_handle* h);
+
+/* CUDA-graph activity of vb_forward on this handle, cumulative since vb_create: forwards captured into a graph (the second call
+ * of a key on a capturable stream), forwards served by replaying one, and captures that failed -- that key then runs eagerly
+ * until its graph is dropped.  *last_failure: the reason of the most recent failed capture ("" if none); valid until the
+ * handle's next vb_forward or vb_destroy.  Any pointer may be NULL. */
+VB_API int vb_graph_stats(vb_handle* h, int64_t* captures, int64_t* replays, int64_t* failures, const char** last_failure);
 
 /* Per-kernel-class device timing (CUDA events recorded on the launch stream around every launch of the class)
  * for the roofline report.  Classes: 0 wgmma GEMM (plain / LayerNorm-folded epilogue: to_qkv, to_q, to_kv), 1 attention,

@@ -16,18 +16,26 @@ def _declared_symbols():
     return sorted(set(re.findall(r"VB_API[^;(]*?\b(vb_\w+)\s*\(", src)))
 
 
-def test_header_symbols_are_exported_and_bound(lib):
+def test_header_symbols_are_exported_and_bound_at_abi_6(lib):
     from vit_tensorflow_b200 import _lib
     declared = _declared_symbols()
     assert len(declared) >= 14
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in include/vitb200.h but not exported"
     assert sorted(_lib.SIGNATURES) == declared, "ctypes SIGNATURES must cover exactly the declared ABI"
-    # ABI 5 added vb_op_gemm / vb_op_attention_ex / vb_op_softmax_rows: header, library and ctypes binding agree on it
+    # ABI 5 added vb_op_gemm / vb_op_attention_ex / vb_op_softmax_rows, ABI 6 vb_graph_stats: header, library and ctypes binding
+    # agree on the version
     header = int(re.search(r"#define VB_ABI_VERSION (\d+)", open(os.path.join(ROOT, "include", "vitb200.h")).read()).group(1))
-    assert lib.vb_abi_version() == header == _lib.ABI_VERSION == 5
-    for name in ("vb_op_gemm", "vb_op_attention_ex", "vb_op_softmax_rows"):
+    assert lib.vb_abi_version() == header == _lib.ABI_VERSION == 6
+    for name in ("vb_op_gemm", "vb_op_attention_ex", "vb_op_softmax_rows", "vb_graph_stats"):
         assert name in declared
+
+
+def test_graph_stats_refuses_a_null_handle(lib):
+    import ctypes as C
+    n = C.c_int64(-1)
+    assert lib.vb_graph_stats(None, C.byref(n), None, None, None) != 0 and n.value == -1
+    assert b"null handle" in lib.vb_last_error(None)
 
 
 def test_config_struct_layout_matches_header():

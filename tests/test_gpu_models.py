@@ -296,8 +296,9 @@ def test_full_size_batch_permutation_equivariance(lib):
 
 def test_native_dp_single_rank_allgather(lib, tmp_path):
     """vb_dp_init / vb_forward_allgather (SURVEY.md 8e through the C-ABI itself) with a world of one rank: the in-place
-    ncclAllGather must leave exactly vb_forward's logits in the gather buffer.  Runs in a child process (its own NCCL
-    communicator, with a time limit); any failure fails the test.  The 2-GPU form of the same check is
+    ncclAllGather must leave exactly vb_forward's logits in the gather buffer.  Three calls under a torch side stream: eager,
+    graph capture and graph replay of the forward in front of the collective (checked through graph_stats).  Runs in a child
+    process (its own NCCL communicator, with a time limit); any failure fails the test.  The 2-GPU form of the same check is
     tools/dp_check.py, run on two or more GPUs."""
     import subprocess
     import sys
@@ -312,9 +313,18 @@ m = from_config(cfg, precision="bf16", seed=3)
 img = oracle.make_image(cfg, 4, 5)
 ref = m(img, training=False)
 dp = NativeDataParallel(m, 4, (64, 64), rank=0, world=1, id_bytes=None)
-out = dp.forward_device(torch.from_numpy(img).cuda())
+x = torch.from_numpy(img).cuda()
+s = torch.cuda.Stream()
 torch.cuda.synchronize()
-np.testing.assert_array_equal(out.cpu().numpy(), ref)
+st0 = m.graph_stats()
+for _ in range(3):
+    with torch.cuda.stream(s):
+        out = dp.forward_device(x)
+    s.synchronize()
+    np.testing.assert_array_equal(out.cpu().numpy(), ref)
+st = m.graph_stats()
+delta = (st["captures"] - st0["captures"], st["replays"] - st0["replays"], st["failures"] - st0["failures"])
+assert delta == (1, 1, 0), (delta, st["last_failure"])
 print("native dp ok")
 """ % os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300)

@@ -3,8 +3,8 @@
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29511 tools/dp_check.py
 
 Every rank runs its shard through (a) `NativeDataParallel` (vb_dp_init + vb_forward_allgather: forward + in-place ncclAllGather
-inside the library) and (b) `DataParallel` (torch.distributed all_gather_into_tensor); rank 0 additionally runs the WHOLE batch on
-its own GPU.  All three gathered logit matrices must be bit-identical on every rank (images are independent and the kernels
+inside the library; three calls on a side stream, so that the second captures the forward into a CUDA graph and the third replays
+it) and (b) `DataParallel` (torch.distributed all_gather_into_tensor); rank 0 additionally runs the WHOLE batch on its own GPU.  All three gathered logit matrices must be bit-identical on every rank (images are independent and the kernels
 deterministic, tests/test_gpu_models.py::test_batch_independence_and_determinism)."""
 import json
 import os
@@ -35,17 +35,27 @@ def main():
         h, w = cfg["image_h"], cfg["image_w"]
         a = DataParallel(m, B, (h, w), rank, world).forward_device(shard).clone()
         ndp = NativeDataParallel(m, B, (h, w), rank, world)
-        b = ndp.forward_device(shard).clone()
-        b2 = ndp.forward_device(shard).clone()          # second / third call: the captured CUDA graph replays in front of the collective
-        b3 = ndp.forward_device(shard).clone()
+        # on a side stream (the default stream is never captured): eager, graph capture, then the captured CUDA graph replays in
+        # front of the collective
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        st0 = m.graph_stats()
+        with torch.cuda.stream(side):
+            b = ndp.forward_device(shard).clone()
+            b2 = ndp.forward_device(shard).clone()
+            b3 = ndp.forward_device(shard).clone()
         torch.cuda.synchronize()
-        same = bool(torch.equal(a, b) and torch.equal(b, b2) and torch.equal(b, b3))
+        st = m.graph_stats()
+        graphs = dict(captures=st["captures"] - st0["captures"], replays=st["replays"] - st0["replays"],
+                      failures=st["failures"] - st0["failures"])
+        same = bool(torch.equal(a, b) and torch.equal(b, b2) and torch.equal(b, b3)) and graphs == dict(captures=1, replays=1, failures=0)
         if rank == 0:
             whole = m(full, training=False)
             same = same and bool(np.array_equal(whole, b.cpu().numpy()))
         flag = torch.tensor([1 if same else 0], device=f"cuda:{local}")
         dist.all_reduce(flag, op=dist.ReduceOp.MIN)
-        out[name] = dict(bit_identical=bool(flag.item()), gathered_shape=list(b.shape), checksum=float(b.double().sum().item()))
+        out[name] = dict(bit_identical=bool(flag.item()), gathered_shape=list(b.shape), checksum=float(b.double().sum().item()),
+                         graphs_rank0=graphs)
     if rank == 0:
         print(json.dumps(dict(world=world, numa_node_rank0=node, results=out)), flush=True)
         assert all(v["bit_identical"] for v in out.values()), out

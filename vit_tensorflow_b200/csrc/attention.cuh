@@ -3,6 +3,8 @@
 #pragma once
 #include "common.h"
 
+#include <vector>
+
 namespace vb {
 
 // variant 0: softmax(QK^T*scale)V                    (vit.py:77-82, cross_vit.py:87-91)
@@ -20,9 +22,11 @@ bool attention_fast(const T* q, int ldq, const T* k, int ldk, const T* v, int ld
                     int heads, int dh, int variant, const float* mix_a, const float* mix_b, const float* ln_gamma,
                     const float* ln_beta, cudaStream_t s, float scale = 0.f);
 
-// The talking-heads / re-attention path keeps host copies of the head-mix weights keyed by their device pointers; whoever
-// frees or rewrites such weights (vb_finalize, vb_destroy, the op-level test entry) must drop them.
-void attention_mix_cache_clear();
+// The talking-heads / re-attention path keeps host copies of the head-mix weights keyed by their device pointers (one process-
+// wide cache for all handles); whoever frees or rewrites such weights (vb_finalize, vb_destroy, the op-level test entries) must
+// erase the entries that name any of those pointers -- and only those: another handle's entries must survive, because a miss
+// inside that handle's graph capture would make the capture fail.
+void attention_mix_cache_erase(const std::vector<const void*>& ptrs);
 
 // Tensor-core (mma.sync) + fused-middle version of attention_generic for the bf16 engine; false if the shape is not covered.
 bool attention_generic_mma(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, int ldk, const __nv_bfloat16* v, int ldv,

@@ -13,7 +13,9 @@
 #include <cmath>
 #include <cstdlib>
 #include <map>
+#include <set>
 #include <tuple>
+#include <vector>
 
 namespace vb {
 namespace {
@@ -603,24 +605,38 @@ bool attention_rows_path(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k
 
 }  // namespace
 
-void attention_mix_cache_clear() {
+void attention_mix_cache_erase(const std::vector<const void*>& ptrs) {
+  std::set<const void*> gone(ptrs.begin(), ptrs.end());
+  gone.erase(nullptr);                                            // an absent operand (DeepViT has no mix_b) names nothing
+  if (gone.empty()) return;
   std::lock_guard<std::mutex> lock(global_cache_mutex());
-  mix_cache().clear();
+  auto& cache = mix_cache();
+  for (auto it = cache.begin(); it != cache.end();) {
+    const MixKey& k = it->first;
+    if (gone.count(k.a) || gone.count(k.b) || gone.count(k.g) || gone.count(k.be)) it = cache.erase(it);
+    else ++it;
+  }
 }
 
 // The head-mix weights are tiny and constant per layer: they are read back from the device once per pointer set and then travel
-// as kernel parameters (constant-bank operands).  The value is copied out under the lock: handles on other threads may clear the
-// cache.  The first use of a pointer set synchronises the stream (never inside a stream capture: first calls are eager).
+// as kernel parameters (constant-bank operands).  The value is copied out under the lock: handles on other threads may erase
+// their own entries.  The first use of a pointer set synchronises the stream, which a stream capture does not allow: the first
+// call of a graph key is eager and fills the entry, and the entries of a handle are erased only by that handle (vb_finalize,
+// vb_destroy), which drops its graphs at the same time.
 bool attention_mix_params(const float* mix_a, const float* mix_b, const float* ln_gamma, const float* ln_beta, int heads,
                           cudaStream_t s, MixParams* out) {
   if (heads > 16 || heads < 1) return false;
   const MixKey key{mix_a, mix_b, ln_gamma, ln_beta};
   {
-    std::lock_guard<std::mutex> lock(global_cache_mutex());       // weights are immutable between attention_mix_cache_clear() calls
+    std::lock_guard<std::mutex> lock(global_cache_mutex());       // weights are immutable while their entries exist
     auto& cache = mix_cache();
     auto it = cache.find(key);
     if (it != cache.end()) { *out = it->second; return true; }
   }
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  VB_CUDA(cudaStreamIsCapturing(s, &cs));
+  VB_CHECK(cs == cudaStreamCaptureStatusNone, "attention_mix_params: head-mix weights first used inside a stream capture "
+                                              "(their host copies were erased after the eager call of this key)");
   MixParams P = {};
   const size_t hh = static_cast<size_t>(heads) * heads * sizeof(float);
   VB_CUDA(cudaStreamSynchronize(s));

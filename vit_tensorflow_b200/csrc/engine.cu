@@ -290,12 +290,21 @@ struct vb_handle {
   };
   struct GraphEntry { cudaGraphExec_t exec = nullptr; int calls = 0; long long launches = 0; bool failed = false; };
   std::map<GraphKey, GraphEntry> graphs;
+  // cumulative over the handle's life (vb_graph_stats): a key whose capture failed runs eagerly until its graph is dropped
+  long long graph_captures = 0, graph_replays = 0, graph_failures = 0;
+  std::string graph_last_failure;
   void drop_graphs() {
     for (auto& g : graphs) if (g.second.exec) cudaGraphExecDestroy(g.second.exec);
     graphs.clear();
   }
 
   bool bf16() const { return cfg.precision == VB_PRECISION_BF16; }
+  // the device copies of the registered weights: what this handle's head-mix cache entries are keyed by
+  std::vector<const void*> weight_pointers() const {
+    std::vector<const void*> p;
+    for (const auto& w : weights) p.push_back(w.dev);
+    return p;
+  }
 
   // ---------------------------------------------------------------- weight registry
   void expect(const std::string& name, std::vector<int64_t> shape) {
@@ -1421,6 +1430,12 @@ T* upload(DevMem& m, const float* host, size_t count) {
   }
   return static_cast<T*>(m.p);
 }
+// Erases the head-mix cache entries of an op entry's temporary weight copies when the entry returns: the copies are freed then,
+// and a later allocation at the same address must not find their values.  No other handle's entry is touched.
+struct MixCacheScope {
+  std::vector<const void*> p;
+  ~MixCacheScope() { attention_mix_cache_erase(p); }
+};
 template <typename T>
 void download(const T* dev, float* host, size_t count) {
   if (sizeof(T) == 4) {
@@ -1519,7 +1534,7 @@ int vb_set_weight(vb_handle* h, const char* name, const float* host_data, const 
 int vb_finalize(vb_handle* h) {
   return guarded(h, [&] {
     VB_CHECK(h != nullptr, "null handle");
-    attention_mix_cache_clear();
+    attention_mix_cache_erase(h->weight_pointers());        // new values behind the same pointers; other handles keep theirs
     h->finalize();
   });
 }
@@ -1560,27 +1575,36 @@ int vb_forward(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, i
       if (ge.exec != nullptr) {
         VB_CUDA(cudaGraphLaunch(ge.exec, s));
         count_launch(static_cast<int>(ge.launches));
+        ++h->graph_replays;
         done = true;
       } else if (ge.calls == 2 && !ge.failed) {
         cudaGraph_t graph = nullptr;
         const long long l0 = launch_counter();
-        if (cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
+        std::string why;
+        const cudaError_t eb = cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal);
+        if (eb == cudaSuccess) {
           bool ok = true;
-          std::string why;
           try { run_eager(); } catch (const std::exception& e) { ok = false; why = e.what(); }
           const cudaError_t ec = cudaStreamEndCapture(s, &graph);
-          if (ok && ec == cudaSuccess && graph != nullptr && cudaGraphInstantiate(&ge.exec, graph, 0) == cudaSuccess) {
+          cudaError_t ei = cudaSuccess;
+          if (ok && ec == cudaSuccess && graph != nullptr && (ei = cudaGraphInstantiate(&ge.exec, graph, 0)) == cudaSuccess) {
             ge.launches = launch_counter() - l0;
             VB_CUDA(cudaGraphLaunch(ge.exec, s));
+            ++h->graph_captures;
             done = true;
           } else {
-            ge.failed = true;                                               // stay eager for this key
+            if (ok) why = std::string(ec != cudaSuccess ? "cudaStreamEndCapture: " : "cudaGraphInstantiate: ") +
+                          cudaGetErrorString(ec != cudaSuccess ? ec : ei);
             ge.exec = nullptr;
-            cudaGetLastError();
           }
           if (graph != nullptr) cudaGraphDestroy(graph);
         } else {
+          why = std::string("cudaStreamBeginCapture: ") + cudaGetErrorString(eb);
+        }
+        if (!done) {                                                        // stay eager for this key
           ge.failed = true;
+          ++h->graph_failures;
+          h->graph_last_failure = why;
           cudaGetLastError();
         }
       }
@@ -1781,6 +1805,16 @@ int vb_forward_allgather(vb_handle* h, const float* img, int32_t img_mem, int32_
 
 int64_t vb_last_launch_count(vb_handle* h) { return h ? h->last_launches : -1; }
 
+int vb_graph_stats(vb_handle* h, int64_t* captures, int64_t* replays, int64_t* failures, const char** last_failure) {
+  return guarded(h, [&] {
+    VB_CHECK(h != nullptr, "null handle");
+    if (captures) *captures = h->graph_captures;
+    if (replays) *replays = h->graph_replays;
+    if (failures) *failures = h->graph_failures;
+    if (last_failure) *last_failure = h->graph_last_failure.c_str();
+  });
+}
+
 int vb_profile_enable(vb_handle* h, int32_t on) {
   return guarded(h, [&] {
     VB_CHECK(h != nullptr, "null handle");
@@ -1811,7 +1845,7 @@ void vb_destroy(vb_handle* h) {
   if (!h) return;
   cudaSetDevice(h->device);
   if (h->dp_comm != nullptr) { nccl().CommDestroy(h->dp_comm); h->dp_comm = nullptr; }
-  attention_mix_cache_clear();
+  attention_mix_cache_erase(h->weight_pointers());
   h->drop_graphs();
   for (auto& w : h->weights) if (w.dev) cudaFree(w.dev);
   h->prof_collect();
@@ -1859,13 +1893,13 @@ int vb_op_attention(int32_t precision, int32_t variant, const float* q, const fl
     require_gpu();
     VB_CHECK(q && k && v && out && B > 0 && nq > 0 && nk > 0 && heads > 0 && dim_head > 0, "vb_op_attention: bad arguments");
     VB_CHECK(variant >= 0 && variant <= 2, "vb_op_attention: variant must be 0, 1 or 2");
-    attention_mix_cache_clear();
     const int inner = heads * dim_head;
     DevMem dQ, dK, dV, dO, dS, dMa, dMb, dG, dBt;
     const float* ma = mix_a ? upload<float>(dMa, mix_a, heads * heads) : nullptr;
     const float* mb = mix_b ? upload<float>(dMb, mix_b, heads * heads) : nullptr;
     const float* g = ln_gamma ? upload<float>(dG, ln_gamma, heads) : nullptr;
     const float* bt = ln_beta ? upload<float>(dBt, ln_beta, heads) : nullptr;
+    const MixCacheScope mix_scope{{ma, mb, g, bt}};
     const size_t cq = static_cast<size_t>(B) * nq * inner, ck = static_cast<size_t>(B) * nk * inner;
     auto run = [&](auto tag) {
       using T = decltype(tag);
@@ -2024,12 +2058,12 @@ int vb_op_attention_ex(int32_t precision, int32_t variant, const float* q, int32
     VB_CHECK(q && out && B > 0 && nq > 0 && nk > 0 && heads > 0 && dh > 0 && ldq >= inner && ldo >= inner && k_off >= 0 &&
              v_off >= 0 && k_off + inner <= ldk && v_off + inner <= ldk && (!fused || nk == nq), "vb_op_attention_ex: bad arguments");
     VB_CHECK(variant >= 0 && variant <= 2, "vb_op_attention_ex: variant must be 0, 1 or 2");
-    attention_mix_cache_clear();
     DevMem dQ, dKV, dO, dS, dMa, dMb, dG, dBt;
     const float* ma = mix_a ? upload<float>(dMa, mix_a, heads * heads) : nullptr;
     const float* mb = mix_b ? upload<float>(dMb, mix_b, heads * heads) : nullptr;
     const float* g = ln_gamma ? upload<float>(dG, ln_gamma, heads) : nullptr;
     const float* bt = ln_beta ? upload<float>(dBt, ln_beta, heads) : nullptr;
+    const MixCacheScope mix_scope{{ma, mb, g, bt}};
     const size_t cq = static_cast<size_t>(B) * nq * ldq, ckv = static_cast<size_t>(B) * nk * ldk, co = static_cast<size_t>(B) * nq * ldo;
     auto run = [&](auto tag) {
       using T = decltype(tag);

@@ -347,6 +347,13 @@ class _EngineModel:
     def last_launch_count(self):
         return int(self._lib.vb_last_launch_count(self._h))
 
+    def graph_stats(self):
+        """CUDA-graph activity of `forward_raw` on a stream (vb_graph_stats), cumulative: captures, replays, failed captures and
+        the reason of the last failure ("" if none)."""
+        cap, rep, fail, why = C.c_int64(), C.c_int64(), C.c_int64(), C.c_char_p()
+        _lib.check(self._lib.vb_graph_stats(self._h, C.byref(cap), C.byref(rep), C.byref(fail), C.byref(why)), self._h)
+        return dict(captures=cap.value, replays=rep.value, failures=fail.value, last_failure=(why.value or b"").decode())
+
     def close(self):
         h, self._h = getattr(self, "_h", None), None
         if h:
