@@ -7,10 +7,10 @@
 // to_out + residual (vit.py:62-69,101), MLP fc1+GELU / fc2 + residual (vit.py:38-44,102), CaiT to_q/to_kv
 // (cait.py:94-95) with LayerScale folded in (cait.py:48).
 //
-// Structure: one CTA per 128 x BN output tile, 3 warpgroups.
-//   warpgroup 0     TMA producer: one thread streams A (128 x 64) and B (BN x 64) k-blocks into a STAGES-deep ring of
-//                   128B-swizzled tiles (mbarrier full / empty pairs); its registers are handed to the consumers.
-//   warpgroups 1-2  consumers, 64 rows each: wgmma m64 x BN x 16 from shared memory into register accumulators, one
+// Structure: one CTA per 128 x BN output tile; BN = 128 tiles run two CTAs per SM (see Cfg).
+//   producer        one thread streams A (128 x 64) and B (BN x 64) k-blocks into a STAGES-deep ring of 128B-swizzled
+//                   tiles (mbarrier full / empty pairs).
+//   2 consumer warpgroups, 64 rows each: wgmma m64 x BN x 16 from shared memory into register accumulators, one
 //                   k-block in flight while the previous one's stage is released; then the epilogue straight from the
 //                   accumulator registers (bias / folded LayerNorm / GELU / LayerScale / residual, bf16 or fp32 stores,
 //                   optional per-64-column row statistics of the stored values).
@@ -24,15 +24,23 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BK = 64;             // 64 bf16 = 128 bytes = one swizzle row
-constexpr int THREADS = 384;
 
+// BN = 128 runs two CTAs per SM, so that one CTA's epilogue and pipeline fill overlap the other's main loop; BN = 256
+// (128 fp32 accumulators per consumer thread) fills the register file with one CTA.
+//   one CTA per SM:  warpgroup 0 is the producer (its registers handed to the consumers by setmaxnreg), 1-2 the consumers;
+//   two CTAs per SM: warpgroups 0-1 are the consumers and a single warp 8 the producer, 288 threads at up to 96
+//                    registers (ptxas holds the whole kernel to the launch-bound cap, and 384 threads x 2 CTAs would
+//                    leave 80, too few for a 64-accumulator wgmma).
 template <int BN>
 struct Cfg {
+  static constexpr int CTAS_PER_SM = BN == 128 ? 2 : 1;
+  static constexpr int THREADS = CTAS_PER_SM == 1 ? 384 : 288;
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES_FIT = (227 * 1024 - 256 - 1024) / STAGE_BYTES;
-  static constexpr int STAGES = STAGES_FIT > 6 ? 6 : STAGES_FIT;   // 6 x 32 KB (BN = 128), 4 x 48 KB (BN = 256)
+  // 228 KB of shared memory per SM, 1 KB of it reserved per CTA
+  static constexpr int STAGES_FIT = ((228 * 1024) / CTAS_PER_SM - 1024 - 256 - 1024) / STAGE_BYTES;
+  static constexpr int STAGES = STAGES_FIT > 6 ? 6 : STAGES_FIT;   // 3 x 32 KB (BN = 128), 4 x 48 KB (BN = 256)
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 /*barriers*/ + 1024 /*align*/;
 };
 
@@ -61,7 +69,7 @@ __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t da, uint
 
 // EPI: 0 = no per-column addend, 1 = + bias[n], 2 = folded LayerNorm (c1 = ln_c1, c2 = bias)
 template <int BN, bool GELU, bool RES, int EPI, bool OF32>
-__global__ void __launch_bounds__(THREADS, 1)
+__global__ void __launch_bounds__(Cfg<BN>::THREADS, Cfg<BN>::CTAS_PER_SM)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, int M, int N, int K,
                  void* __restrict__ out, int ldc, const float* __restrict__ bias, const float* __restrict__ scale,
                  const __nv_bfloat16* res, int ldr, const float* __restrict__ ln_c1, const float2* ln_stats, int ln_parts,
@@ -94,9 +102,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   pdl_wait();
   pdl_launch_dependents();
 
-  if (wg == 0) {
+  if (wg == (C::CTAS_PER_SM == 1 ? 0 : 2)) {
     // ===================================================================== TMA producer
-    setmaxnreg_dec<40>();
+    if (C::CTAS_PER_SM == 1) setmaxnreg_dec<40>();
     if (tid == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -113,8 +121,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   }
 
   // ===================================================================== consumers
-  setmaxnreg_inc<232>();
-  const int cw = wg - 1;                                           // 64-row half of the tile
+  if (C::CTAS_PER_SM == 1) setmaxnreg_inc<232>();
+  const int cw = C::CTAS_PER_SM == 1 ? wg - 1 : wg;                // 64-row half of the tile
   const int warp = tid >> 5, lane = tid & 31;
   const int row_a = m0 + cw * 64 + warp * 16 + (lane >> 2);        // this thread's two accumulator rows: row_a, row_a + 8
   const int col_t = 2 * (lane & 3);
@@ -250,7 +258,7 @@ void launch(const GemmBf16& g, cudaStream_t stream) {
   if (first_use_on_this_device(seen)) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM_BYTES));
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((g.N + BN - 1) / BN, (g.M + BM - 1) / BM);
-  cfg.blockDim = dim3(THREADS);
+  cfg.blockDim = dim3(Cfg<BN>::THREADS);
   cfg.dynamicSmemBytes = Cfg<BN>::SMEM_BYTES;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
@@ -324,9 +332,11 @@ GemmBf16 gemm_bf16_plan(const __nv_bfloat16* A, int lda, const __nv_bfloat16* Wt
   g.M = M; g.N = N; g.K = K;
   g.bias = bias; g.scale = scale; g.res = res; g.ldr = ldr; g.gelu = gelu;
   g.out = out; g.ldc = ldc; g.out_f32 = out_f32;
-  // 256-wide tiles when they divide N (half the A re-reads and twice the math per operand byte); 128-wide ones otherwise,
-  // so that no tile column is more than half empty
-  g.block_n = (N % 256 == 0) ? 256 : 128;
+  // Each tile pays a fixed cost (pipeline fill, epilogue) of about as much as a 12-k-block main loop.  128-wide tiles run
+  // two CTAs per SM, so that cost overlaps the other CTA's main loop; 256-wide tiles (one CTA per SM, half the A re-reads)
+  // are faster only once the main loop is long.  On an H100 (400 W) at M = 50 432: K = 768 128-wide 0.24-0.77 ms against
+  // 0.28-0.90 ms 256-wide, K = 3072 (N = 768) 0.651 ms against 0.609 ms.
+  g.block_n = (N % 256 == 0 && K >= 2048) ? 256 : 128;
   g.tmap_a = make_tmap_2d(A, K, M, static_cast<uint64_t>(lda) * 2, BK, BM);
   // b_rows: rows of Wt that exist (< N when the output is column-padded: TMA zero-fills the rest instead of reading on)
   g.tmap_b = make_tmap_2d(Wt, K, b_rows > 0 ? b_rows : N, static_cast<uint64_t>(ldw) * 2, BK, g.block_n);
