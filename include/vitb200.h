@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 6
+#define VB_ABI_VERSION 7
 #if defined(__GNUC__)
 #define VB_API __attribute__((visibility("default")))
 #else
@@ -169,6 +169,19 @@ VB_API int64_t vb_last_launch_count(vb_handle* h);
  * until its graph is dropped.  *last_failure: the reason of the most recent failed capture ("" if none); valid until the
  * handle's next vb_forward or vb_destroy.  Any pointer may be NULL. */
 VB_API int vb_graph_stats(vb_handle* h, int64_t* captures, int64_t* replays, int64_t* failures, const char** last_failure);
+
+/* Which attention kernels served the most recent attention call made on the calling thread since the previous
+ * vb_last_attention_path call (which it resets): VB_ATTN_PATH_NONE if there was none.  FLASH: attn_flash_kernel; CLS:
+ * attn_cls_kernel (one query row); ROWS: scores_stripe / mid_rows / pv_rows (head mixing, 8 or 16 heads, <= 256 keys);
+ * MID_FUSED: scores_mma / mid_fused / pv_mma (bf16 tensor-core scores, every head's scores in shared memory); SIMT:
+ * attn_scores / attn_softmax / attn_pv (+ attn_head_mix), every fp32 call and the bf16 fallback. */
+#define VB_ATTN_PATH_NONE 0
+#define VB_ATTN_PATH_FLASH 1
+#define VB_ATTN_PATH_CLS 2
+#define VB_ATTN_PATH_ROWS 3
+#define VB_ATTN_PATH_MID_FUSED 4
+#define VB_ATTN_PATH_SIMT 5
+VB_API int32_t vb_last_attention_path(void);
 
 /* Per-kernel-class device timing (CUDA events recorded on the launch stream around every launch of the class)
  * for the roofline report.  Classes: 0 wgmma GEMM (plain / LayerNorm-folded epilogue: to_qkv, to_q, to_kv), 1 attention,

@@ -53,6 +53,23 @@ MID = {
     "t2t_big_image": dict(kind="t2t_vit", image_size=288, num_classes=10, dim=64, depth=2, heads=4, mlp_dim=128, dim_head=16),
     "cait_mid": dict(kind="cait", image_size=224, patch_size=16, num_classes=100, dim=192, depth=2, cls_depth=2, heads=4,
                      mlp_dim=384, dim_head=48),
+    # dim_head > 64 (ViT-H/14 has 80; 128 is a common setting): plain softmax through scores_mma / mid_fused / pv_mma
+    "vit_dh80_p14": dict(kind="vit", image_size=224, patch_size=14, num_classes=100, dim=192, depth=1, heads=4, mlp_dim=256,
+                         dim_head=80),
+    "vit_dh128": dict(kind="vit", image_size=224, patch_size=16, num_classes=100, dim=192, depth=2, heads=2, mlp_dim=256,
+                      dim_head=128),
+    # 384^2: 577 tokens, past the rows path's 256 keys, so 8 and 16 heads take mid_fused; CaiT's class layers attn_cls at 578 keys
+    "deepvit_384_h8": dict(kind="deepvit", image_size=384, patch_size=16, num_classes=100, dim=128, depth=1, heads=8, mlp_dim=256,
+                           dim_head=32),
+    "deepvit_384_h16": dict(kind="deepvit", image_size=384, patch_size=16, num_classes=100, dim=128, depth=1, heads=16, mlp_dim=256,
+                            dim_head=16),
+    "cait_384_h8": dict(kind="cait", image_size=384, patch_size=16, num_classes=100, dim=128, depth=1, cls_depth=1, heads=8,
+                        mlp_dim=256, dim_head=32),
+    "cait_384_h16": dict(kind="cait", image_size=384, patch_size=16, num_classes=100, dim=128, depth=1, cls_depth=1, heads=16,
+                         mlp_dim=256, dim_head=16),
+    # the class layers reach attn_cls at dim_head 128
+    "cait_dh128": dict(kind="cait", image_size=224, patch_size=16, num_classes=100, dim=192, depth=1, cls_depth=2, heads=2,
+                       mlp_dim=256, dim_head=128),
 }
 
 # BASELINE.json configs[1..4] (batch replaced by 2: the path has no cross-image op, see test_batch_independence)

@@ -16,19 +16,28 @@ def _declared_symbols():
     return sorted(set(re.findall(r"VB_API[^;(]*?\b(vb_\w+)\s*\(", src)))
 
 
-def test_header_symbols_are_exported_and_bound_at_abi_6(lib):
+def test_header_symbols_are_exported_and_bound_at_abi_7(lib):
     from vit_tensorflow_b200 import _lib
     declared = _declared_symbols()
     assert len(declared) >= 14
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in include/vitb200.h but not exported"
     assert sorted(_lib.SIGNATURES) == declared, "ctypes SIGNATURES must cover exactly the declared ABI"
-    # ABI 5 added vb_op_gemm / vb_op_attention_ex / vb_op_softmax_rows, ABI 6 vb_graph_stats: header, library and ctypes binding
-    # agree on the version
+    # ABI 5 added vb_op_gemm / vb_op_attention_ex / vb_op_softmax_rows, ABI 6 vb_graph_stats, ABI 7 vb_last_attention_path:
+    # header, library and ctypes binding agree on the version
     header = int(re.search(r"#define VB_ABI_VERSION (\d+)", open(os.path.join(ROOT, "include", "vitb200.h")).read()).group(1))
-    assert lib.vb_abi_version() == header == _lib.ABI_VERSION == 6
-    for name in ("vb_op_gemm", "vb_op_attention_ex", "vb_op_softmax_rows", "vb_graph_stats"):
+    assert lib.vb_abi_version() == header == _lib.ABI_VERSION == 7
+    for name in ("vb_op_gemm", "vb_op_attention_ex", "vb_op_softmax_rows", "vb_graph_stats", "vb_last_attention_path"):
         assert name in declared
+
+
+def test_attention_path_names_match_header_and_start_empty(lib):
+    """The VB_ATTN_PATH_* values of the header are the ones the binding names; a thread that ran no attention reads NONE."""
+    from vit_tensorflow_b200 import _lib
+    src = open(os.path.join(ROOT, "include", "vitb200.h")).read()
+    values = {int(v): k.lower() for k, v in re.findall(r"#define VB_ATTN_PATH_(\w+) (\d+)", src)}
+    assert values == {k: (v or "none") for k, v in _lib.ATTENTION_PATHS.items()}
+    assert _lib.last_attention_path() is None and lib.vb_last_attention_path() == 0
 
 
 def test_graph_stats_refuses_a_null_handle(lib):

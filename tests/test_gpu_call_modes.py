@@ -9,6 +9,7 @@ import pytest
 from cases import bf16_round
 from test_gpu_ops import (ATTN_BF16_REL, ATTN_BF16_SIGMA, BF16_ATOL, BF16_RTOL, _assert_close_sigma, _attention_ref, _gelu,
                           _ln_linear_ref, _sigma_worst)
+from test_gpu_attention_paths import served_by  # noqa: F401 (fixture)
 
 pytestmark = pytest.mark.gpu
 
@@ -278,21 +279,21 @@ def test_attention_head_padded_scale(lib, dh, nq):
 
 # B * heads > 65 535 (the gridDim.y / gridDim.z limit) at a few MB: nq = nk = 5
 GRID_PATHS = {
-    "fp32_generic": dict(precision="fp32", heads=16, dh=16, variants=(0, 1, 2)),
-    "bf16_simt_dh14": dict(precision="bf16", heads=16, dh=14, variants=(0,)),
-    "bf16_rows_h8": dict(precision="bf16", heads=8, dh=16, variants=(1, 2)),
-    "bf16_rows_h16": dict(precision="bf16", heads=16, dh=16, variants=(1, 2)),
-    "bf16_mid_fused_h4": dict(precision="bf16", heads=4, dh=16, variants=(1, 2)),
-    "bf16_mid_fused_h1": dict(precision="bf16", heads=1, dh=16, variants=(2,)),       # B alone > 65 535 (mid_fused_kernel)
-    "bf16_flash": dict(precision="bf16", heads=16, dh=64, variants=(0,)),             # controls: flat grids already
-    "bf16_cls": dict(precision="bf16", heads=16, dh=16, variants=(0,), nq=1),
+    "fp32_generic": dict(precision="fp32", heads=16, dh=16, variants=(0, 1, 2), path="simt"),
+    "bf16_simt_dh14": dict(precision="bf16", heads=16, dh=14, variants=(0,), path="simt"),
+    "bf16_rows_h8": dict(precision="bf16", heads=8, dh=16, variants=(1, 2), path="rows"),
+    "bf16_rows_h16": dict(precision="bf16", heads=16, dh=16, variants=(1, 2), path="rows"),
+    "bf16_mid_fused_h4": dict(precision="bf16", heads=4, dh=16, variants=(1, 2), path="mid_fused"),
+    "bf16_mid_fused_h1": dict(precision="bf16", heads=1, dh=16, variants=(2,), path="mid_fused"),   # B alone > 65 535 (mid_fused_kernel)
+    "bf16_flash": dict(precision="bf16", heads=16, dh=64, variants=(0,), path="flash"),             # controls: flat grids already
+    "bf16_cls": dict(precision="bf16", heads=16, dh=16, variants=(0,), nq=1, path="cls"),
 }
 
 
 @pytest.mark.parametrize("path", sorted(GRID_PATHS))
-def test_attention_batch_times_heads_beyond_65535(lib, path):
+def test_attention_batch_times_heads_beyond_65535(lib, served_by, path):
     """Every attention path at B * heads > 65 535 against the float64 reference, and the last images of the batch equal the
-    same images run alone (bit for bit)."""
+    same images run alone (bit for bit).  The named path must be the one that served the call."""
     from vit_tensorflow_b200 import _lib
     p = GRID_PATHS[path]
     heads, dh, precision = p["heads"], p["dh"], p["precision"]
@@ -307,7 +308,7 @@ def test_attention_batch_times_heads_beyond_65535(lib, path):
     for variant in p["variants"]:
         ma, mb, g, b = _mixes(rng, variant, heads)
         kw = dict(kv=kv, k_off=0, v_off=inner, variant=variant, mix_a=ma, mix_b=mb, ln_gamma=g, ln_beta=b, precision=precision)
-        out, _ = _lib.op_attention_ex(q, heads, dh, np.zeros((B, nq, inner), np.float32), **kw)
+        out, _ = served_by(lambda: _lib.op_attention_ex(q, heads, dh, np.zeros((B, nq, inner), np.float32), **kw), p["path"])
         _check_attention(out, _attention_ref(q, k, v, heads, variant, ma, mb, g, b), precision, variant)
         kw["kv"] = kv[-3:]
         tail, _ = _lib.op_attention_ex(q[-3:], heads, dh, np.zeros((3, nq, inner), np.float32), **kw)

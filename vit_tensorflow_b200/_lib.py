@@ -14,7 +14,7 @@ LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "libvitb200.so")
 KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6}
 PRECISION = {"fp32": 0, "float32": 0, "bf16": 1, "bfloat16": 1}
 MEM_HOST, MEM_DEVICE = 0, 1
-ABI_VERSION = 6                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
+ABI_VERSION = 7                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
 
 
 class VbConfig(C.Structure):
@@ -58,6 +58,7 @@ SIGNATURES = {
     "vb_forward_allgather": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "vb_last_launch_count": (C.c_int64, [C.c_void_p]),
     "vb_graph_stats": (C.c_int, [C.c_void_p, _i64p, _i64p, _i64p, C.POINTER(C.c_char_p)]),
+    "vb_last_attention_path": (C.c_int32, []),
     "vb_profile_enable": (C.c_int, [C.c_void_p, C.c_int32]),
     "vb_profile_read": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double), _i64p, C.c_int32]),
     "vb_last_error": (C.c_char_p, [C.c_void_p]),
@@ -93,6 +94,15 @@ def load() -> C.CDLL:
             raise VbError("libvitb200 ABI version mismatch")
         _lib = lib
     return _lib
+
+
+ATTENTION_PATHS = {0: None, 1: "flash", 2: "cls", 3: "rows", 4: "mid_fused", 5: "simt"}   # VB_ATTN_PATH_* of include/vitb200.h
+
+
+def last_attention_path():
+    """The attention branch ("flash", "cls", "rows", "mid_fused" or "simt") that served the most recent attention call of this
+    thread since the previous last_attention_path() call, or None (vb_last_attention_path; reading it resets it)."""
+    return ATTENTION_PATHS[load().vb_last_attention_path()]
 
 
 def check(rc: int, handle=None):

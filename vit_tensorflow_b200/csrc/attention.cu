@@ -6,10 +6,23 @@
 
 namespace vb {
 
+namespace {
+thread_local int t_last_attention_path = ATTN_PATH_NONE;
+}  // namespace
+
+void note_attention_path(AttentionPath p) { t_last_attention_path = p; }
+
+int take_last_attention_path() {
+  const int p = t_last_attention_path;
+  t_last_attention_path = ATTN_PATH_NONE;
+  return p;
+}
+
 template <typename T>
 void attention_generic(const T* q, int ldq, const T* k, int ldk, const T* v, int ldv, T* out, int ldo, float* S, int B, int nq,
                        int nk, int heads, int dh, int variant, const float* mix_a, const float* mix_b, const float* ln_gamma,
                        const float* ln_beta, cudaStream_t s) {
+  note_attention_path(ATTN_PATH_SIMT);
   const float scale = 1.0f / sqrtf(static_cast<float>(dh));
   attn_scores<T>(q, ldq, k, ldk, S, B, heads, nq, nk, dh, scale, s);
   if (variant == 2) attn_head_mix(S, mix_a, nullptr, nullptr, B, heads, nq, nk, s);            // cait.py:123
@@ -26,6 +39,7 @@ void attention_generic<__nv_bfloat16>(const __nv_bfloat16* q, int ldq, const __n
                                       cudaStream_t s) {
   if (attention_generic_mma(q, ldq, k, ldk, v, ldv, out, ldo, S, B, nq, nk, heads, dh, variant, mix_a, mix_b, ln_gamma, ln_beta, s))
     return;
+  note_attention_path(ATTN_PATH_SIMT);
   const float scale = 1.0f / sqrtf(static_cast<float>(dh));
   attn_scores<__nv_bfloat16>(q, ldq, k, ldk, S, B, heads, nq, nk, dh, scale, s);
   if (variant == 2) attn_head_mix(S, mix_a, nullptr, nullptr, B, heads, nq, nk, s);

@@ -7,7 +7,14 @@
 
 namespace vb {
 
-// variant 0: softmax(QK^T*scale)V                    (vit.py:77-82, cross_vit.py:87-91)
+// Which branch of the dispatch ran the most recent attention call of the calling thread (vb_last_attention_path): every
+// branch notes itself when it launches, so a test can tell which kernels served a shape.  Values as in include/vitb200.h.
+enum AttentionPath { ATTN_PATH_NONE = 0, ATTN_PATH_FLASH = 1, ATTN_PATH_CLS = 2, ATTN_PATH_ROWS = 3, ATTN_PATH_MID_FUSED = 4,
+                     ATTN_PATH_SIMT = 5 };
+void note_attention_path(AttentionPath p);
+int take_last_attention_path();                  // and reset it to ATTN_PATH_NONE
+
+// variant 0: softmax(QK^T*scale)V                   (vit.py:77-82, cross_vit.py:87-91)
 // variant 1: DeepViT re-attention: softmax -> head mix (mix_a [h,h]) -> LayerNorm over heads (deepvit.py:79-87)
 // variant 2: CaiT talking heads: mix_a before softmax, mix_b after (cait.py:121-127)
 template <typename T>

@@ -179,6 +179,7 @@ bool attention_cls(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, int 
   VB_CUDA(cudaLaunchKernelEx(&cfg, attn_cls_kernel, q, ldq, k, ldk, v, ldv, out, ldo, nk, heads, dh, variant, mix_a, mix_b, ln_g, ln_b,
                              scale_log2));
   count_launch();
+  note_attention_path(ATTN_PATH_CLS);
   return true;
 }
 

@@ -204,6 +204,7 @@ bool attention_fast<__nv_bfloat16>(const __nv_bfloat16* q, int ldq, const __nv_b
   cfg.numAttrs = 1;
   VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2));
   count_launch();
+  note_attention_path(ATTN_PATH_FLASH);
   return true;
 }
 

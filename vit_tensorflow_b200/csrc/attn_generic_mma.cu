@@ -30,12 +30,7 @@ constexpr int MAXDH = 128;
 constexpr int PITCH = MAXDH + 8;   // bf16 elements; +8 keeps the fragment loads bank-conflict free
 
 // Every kernel of this file takes its (tile, b * heads + h) item from a flat blockIdx.x, tile index fastest, so B * heads is
-// not bounded by the 65 535 of gridDim.y / gridDim.z; flat_blocks() checks the product against gridDim.x's 2^31 - 1.
-unsigned flat_blocks(long long tiles, long long items) {
-  const long long n = tiles * items;
-  VB_CHECK(n > 0 && n <= 0x7fffffffLL, "attention: grid of " + std::to_string(n) + " blocks exceeds 2^31 - 1");
-  return static_cast<unsigned>(n);
-}
+// not bounded by the 65 535 of gridDim.y / gridDim.z; flat_blocks() (common.h) checks the product against gridDim.x's 2^31 - 1.
 
 // S[bh, i, j] = scale * sum_d q[b,i,h,d] k[b,j,h,d];  block: 64 x 64 tile, 4 warps x (16 rows x 64 cols)
 __global__ void __launch_bounds__(128)
@@ -600,6 +595,7 @@ bool attention_rows_path(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k
   }
   VB_CUDA(cudaGetLastError());
   count_launch(3);
+  note_attention_path(ATTN_PATH_ROWS);
   return true;
 }
 
@@ -673,6 +669,7 @@ bool attention_generic_mma(const __nv_bfloat16* q, int ldq, const __nv_bfloat16*
   else pv_mma_kernel<false><<<pv_grid, 128, 0, s>>>(S, v, ldv, out, ldo, heads, nq, nk, dh);
   VB_CUDA(cudaGetLastError());
   count_launch(3);
+  note_attention_path(ATTN_PATH_MID_FUSED);
   return true;
 }
 

@@ -50,6 +50,14 @@ inline bool first_use_on_this_device(unsigned long long (&seen)[4]) {
   return true;
 }
 
+// Kernels whose grid counts images, rows or (image, head) items take their (tile, item) from a flat blockIdx.x, tile index
+// fastest: gridDim.y and gridDim.z stop at 65 535, gridDim.x at 2^31 - 1.  The block count of such a grid, checked.
+inline unsigned flat_blocks(long long tiles, long long items, const char* what = "attention") {
+  const long long n = tiles * items;
+  VB_CHECK(n > 0 && n <= 0x7fffffffLL, std::string(what) + ": grid of " + std::to_string(n) + " blocks exceeds 2^31 - 1");
+  return static_cast<unsigned>(n);
+}
+
 // 2-D bf16 (or fp32) tensor map (innermost dimension first), 128-byte swizzle unless swizzle128 == false.
 CUtensorMap make_tmap_2d(const void* base, uint64_t inner, uint64_t outer, uint64_t outer_stride_bytes,
                          uint32_t box_inner, uint32_t box_outer, bool swizzle128 = true, bool f32 = false);

@@ -1815,6 +1815,8 @@ int vb_graph_stats(vb_handle* h, int64_t* captures, int64_t* replays, int64_t* f
   });
 }
 
+int32_t vb_last_attention_path(void) { return take_last_attention_path(); }
+
 int vb_profile_enable(vb_handle* h, int32_t on) {
   return guarded(h, [&] {
     VB_CHECK(h != nullptr, "null handle");

@@ -7,7 +7,7 @@
 // to_out + residual (vit.py:62-69,101), MLP fc1+GELU / fc2 + residual (vit.py:38-44,102), CaiT to_q/to_kv
 // (cait.py:94-95) with LayerScale folded in (cait.py:48).
 //
-// Structure: one CTA per 128 x BN output tile; BN = 128 tiles run two CTAs per SM (see Cfg).
+// Structure: one CTA per 128 x BN output tile (flat grid, n fastest); BN = 128 tiles run two CTAs per SM (see Cfg).
 //   producer        one thread streams A (128 x 64) and B (BN x 64) k-blocks into a STAGES-deep ring of 128B-swizzled
 //                   tiles (mbarrier full / empty pairs).
 //   2 consumer warpgroups, 64 rows each: wgmma m64 x BN x 16 from shared memory into register accumulators, one
@@ -84,8 +84,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 
   const int wg = threadIdx.x >> 7;
   const int tid = threadIdx.x & 127;
-  const int n0 = blockIdx.x * BN;                                  // n fastest: the CTAs that share an A row block run together
-  const int m0 = blockIdx.y * BM;
+  // flat grid, n fastest: the CTAs that share an A row block run together, and M is not bounded by gridDim.y's 65 535 tiles
+  const int n_tiles = (N + BN - 1) / BN;
+  const int n0 = static_cast<int>(blockIdx.x % n_tiles) * BN;
+  const int m0 = static_cast<int>(blockIdx.x / n_tiles) * BM;
   const int num_kb = (K + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
@@ -257,7 +259,7 @@ void launch(const GemmBf16& g, cudaStream_t stream) {
   static unsigned long long seen[4] = {0, 0, 0, 0};
   if (first_use_on_this_device(seen)) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM_BYTES));
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((g.N + BN - 1) / BN, (g.M + BM - 1) / BM);
+  cfg.gridDim = dim3(flat_blocks((g.N + BN - 1) / BN, (g.M + BM - 1) / BM, "gemm_bf16"));
   cfg.blockDim = dim3(Cfg<BN>::THREADS);
   cfg.dynamicSmemBytes = Cfg<BN>::SMEM_BYTES;
   cfg.stream = stream;

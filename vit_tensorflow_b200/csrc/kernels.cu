@@ -274,7 +274,9 @@ softmax_rows_bf16_big_kernel(const float* __restrict__ S, int lds, __nv_bfloat16
 __global__ void transpose_rows_bf16_kernel(const __nv_bfloat16* __restrict__ in, int ldi, long long in_batch, __nv_bfloat16* __restrict__ out,
                                            int ldo, long long out_batch, int n, int npad, int cols) {
   __shared__ __nv_bfloat16 tile[32][33];
-  const int b = blockIdx.z, j0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
+  const int jt = (npad + 31) / 32, ct = (cols + 31) / 32;            // flat grid, j tile fastest: no 65 535 limit on B
+  const int tile_idx = static_cast<int>(blockIdx.x % (jt * ct)), b = static_cast<int>(blockIdx.x / (jt * ct));
+  const int j0 = (tile_idx % jt) * 32, c0 = (tile_idx / jt) * 32;
   const __nv_bfloat16* ib = in + b * in_batch;
   __nv_bfloat16* ob = out + b * out_batch;
   for (int r = threadIdx.y; r < 32; r += blockDim.y) {
@@ -301,7 +303,8 @@ gemm_simt_kernel(const TA* __restrict__ A, int lda, const TW* __restrict__ W, in
   __shared__ float As[16][BMT + 1];
   __shared__ __align__(16) float Ws[16][64 + 4];   // pitch 68 floats: 16-byte aligned rows, one LDS.128 per thread and k
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  const int m0 = blockIdx.y * BMT, n0 = blockIdx.x * 64;
+  const int n_tiles = (N + 63) / 64;                                // flat grid, n fastest: no 65 535 limit on the row tiles
+  const int m0 = static_cast<int>(blockIdx.x / n_tiles) * BMT, n0 = static_cast<int>(blockIdx.x % n_tiles) * 64;
   float acc[TM][4];
 #pragma unroll
   for (int i = 0; i < TM; ++i)
@@ -741,7 +744,7 @@ void softmax_rows_bf16(const float* S, int lds, __nv_bfloat16* P, int ldp, long 
 
 void transpose_rows_bf16(const __nv_bfloat16* in, int ldi, long long in_batch, __nv_bfloat16* out, int ldo, long long out_batch, int B,
                          int n, int npad, int cols, cudaStream_t s) {
-  dim3 grid((npad + 31) / 32, (cols + 31) / 32, B);
+  const unsigned grid = flat_blocks(static_cast<long long>((npad + 31) / 32) * ((cols + 31) / 32), B, "transpose_rows_bf16");
   transpose_rows_bf16_kernel<<<grid, dim3(32, 8), 0, s>>>(in, ldi, in_batch, out, ldo, out_batch, n, npad, cols);
   VB_LAUNCHED();
 }
@@ -781,10 +784,10 @@ template <typename TA, typename TW, typename TO>
 void gemm_simt(const TA* A, int lda, const TW* W, int wsk, int wsn, TO* out, int ldc, int M, int N, int K, const float* bias,
                const float* scale, const TO* res, int ldr, int gelu, cudaStream_t s) {
   if (static_cast<long long>((N + 63) / 64) * ((M + 63) / 64) >= 2 * sm_count()) {
-    dim3 grid((N + 63) / 64, (M + 63) / 64);
+    const unsigned grid = flat_blocks((N + 63) / 64, (M + 63) / 64, "gemm_simt");
     gemm_simt_kernel<TA, TW, TO, 4><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, gelu);
   } else {
-    dim3 grid((N + 63) / 64, (M + 15) / 16);
+    const unsigned grid = flat_blocks((N + 63) / 64, (M + 15) / 16, "gemm_simt");
     gemm_simt_kernel<TA, TW, TO, 1><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, gelu);
   }
   VB_LAUNCHED();
