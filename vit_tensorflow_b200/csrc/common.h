@@ -71,7 +71,6 @@ struct GemmBf16 {
   __nv_bfloat16* out = nullptr;         // [M, ldc] (the epilogue stores rows straight from registers)
   int ldc = 0;
   bool out_f32 = false;                 // `out` is float* (ldc in floats): plain / bias epilogue only
-  int block_n = 256;
   const float* bias = nullptr;          // [N] or null
   const float* scale = nullptr;         // [N] or null (LayerScale)
   const __nv_bfloat16* res = nullptr;   // [M, ldr] or null (may alias out)
