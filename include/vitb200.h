@@ -39,7 +39,8 @@ extern "C" {
 typedef struct vb_handle vb_handle;
 
 enum { VB_KIND_VIT = 0, VB_KIND_DEEPVIT = 1, VB_KIND_CAIT = 2, VB_KIND_CROSSVIT = 3, VB_KIND_PARALLEL_VIT = 4,
-       VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6 };
+       VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6, VB_KIND_CCT = 7 };
+enum { VB_CCT_POS_SINE = 0, VB_CCT_POS_LEARNABLE = 1, VB_CCT_POS_NONE = 2 };   /* cct.py:233-234,250-256 */
 enum { VB_PRECISION_FP32 = 0, VB_PRECISION_BF16 = 1 };
 enum { VB_POOL_CLS = 0, VB_POOL_MEAN = 1 };
 enum { VB_MEM_HOST = 0, VB_MEM_DEVICE = 1 };
@@ -70,7 +71,15 @@ typedef struct vb_config {
   /* T2TViT `t2t_layers` (t2t.py:54): up to 4 (kernel_size, stride) soft-split layers; image_h == image_w, patch_* unused */
   int32_t t2t_num_layers;
   int32_t t2t_k0, t2t_s0, t2t_k1, t2t_s1, t2t_k2, t2t_s2, t2t_k3, t2t_s3;
+  /* CCT (cct.py:307-339; appended within ABI 7): a Tokenizer of cct_conv_layers x [Conv2D(cct_kernel, cct_stride, SAME,
+   * no bias) -> ReLU -> MaxPool2D(cct_pool_kernel, cct_pool_stride, SAME)], 64 channels between layers and `dim` after the last;
+   * cct_pos_emb: VB_CCT_POS_*.  Uses dim, depth, heads, dim_head (= dim / heads), mlp_dim, num_classes, image_h / image_w. */
+  int32_t cct_conv_layers, cct_kernel, cct_stride, cct_pool_kernel, cct_pool_stride, cct_pos_emb;
 } vb_config;
+
+/* A client built against the ABI-7 struct before the CCT fields were appended passes struct_size = VB_CONFIG_SIZE_ABI7;
+ * vb_create reads only that prefix and treats the fields after it as zero. */
+#define VB_CONFIG_SIZE_ABI7 ((int32_t)(45 * sizeof(int32_t)))
 
 VB_API int vb_abi_version(void);
 

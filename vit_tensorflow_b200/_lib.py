@@ -11,7 +11,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "libvitb200.so")   # VB_LIB_PATH: developer A/B builds
 
-KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6}
+KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6, "cct": 7}
 PRECISION = {"fp32": 0, "float32": 0, "bf16": 1, "bfloat16": 1}
 MEM_HOST, MEM_DEVICE = 0, 1
 ABI_VERSION = 7                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
@@ -26,7 +26,12 @@ class VbConfig(C.Structure):
         "lg_patch_size", "lg_enc_depth", "lg_enc_heads", "lg_enc_mlp_dim", "lg_enc_dim_head",
         "cross_attn_depth", "cross_attn_heads", "cross_attn_dim_head", "cross_depth", "parallel_branches",
         "patch_merge_layer_index", "patch_merge_num_tokens",
-        "t2t_num_layers", "t2t_k0", "t2t_s0", "t2t_k1", "t2t_s1", "t2t_k2", "t2t_s2", "t2t_k3", "t2t_s3")]
+        "t2t_num_layers", "t2t_k0", "t2t_s0", "t2t_k1", "t2t_s1", "t2t_k2", "t2t_s2", "t2t_k3", "t2t_s3",
+        "cct_conv_layers", "cct_kernel", "cct_stride", "cct_pool_kernel", "cct_pool_stride", "cct_pos_emb")]
+
+
+CONFIG_SIZE_ABI7 = VbConfig.cct_conv_layers.offset   # VB_CONFIG_SIZE_ABI7: the struct before the CCT fields were appended
+CCT_POS = {"sine": 0, "learnable": 1, "none": 2}     # VB_CCT_POS_*
 
 
 class VbError(RuntimeError):

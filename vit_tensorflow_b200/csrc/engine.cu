@@ -14,6 +14,7 @@
 
 #include <array>
 #include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -132,6 +133,8 @@ inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 }  // namespace vb
 
 using namespace vb;
+
+static_assert(offsetof(vb_config, cct_conv_layers) == VB_CONFIG_SIZE_ABI7, "VB_CONFIG_SIZE_ABI7 is the struct before the CCT fields");
 
 // ------------------------------------------------------------------------------------------ NCCL (loaded on demand)
 // The five entry points of the NCCL 2.x C API the data-parallel path needs, declared here so that neither nccl.h nor a
@@ -265,6 +268,21 @@ struct vb_handle {
   static int conv_output_size(int size, int k, int stride) {   // t2t.py:14-15 with padding = stride // 2
     return static_cast<int>((static_cast<double>(size - k + 2 * (stride / 2)) / stride) + 1);
   }
+  // CCT tokenizer (cct.py:188-200): conv layer i maps cin -> cout channels, 64 (Tokenizer in_planes) between layers, dim after the last
+  std::vector<Linear> cct_convs;
+  Norm cct_norm;
+  const float* cct_pool_w = nullptr;                      // attention_pool Dense(1): kernel [dim, 1], bias [1]
+  const float* cct_pool_b = nullptr;
+  int cct_conv_cin(int i) const { return i == 0 ? cfg.channels : 64; }
+  int cct_conv_cout(int i) const { return i == cfg.cct_conv_layers - 1 ? cfg.dim : 64; }
+  // token grid of an h x w image after the tokenizer: SAME convolution and max-pool, ceil(size / stride) each
+  void cct_grid(int* h, int* w) const {
+    for (int i = 0; i < cfg.cct_conv_layers; ++i) {
+      *h = (*h + cfg.cct_stride - 1) / cfg.cct_stride; *w = (*w + cfg.cct_stride - 1) / cfg.cct_stride;
+      *h = (*h + cfg.cct_pool_stride - 1) / cfg.cct_pool_stride; *w = (*w + cfg.cct_pool_stride - 1) / cfg.cct_pool_stride;
+    }
+  }
+  int cct_sequence_length() const { int h = cfg.image_h, w = cfg.image_w; cct_grid(&h, &w); return h * w; }   // cct.py:331-333
   struct XBlock { std::vector<LayerW> sm_layers, lg_layers; Norm sm_final, lg_final; std::vector<CrossW> sm_attend_lg, lg_attend_sm; };
   std::vector<XBlock> xblocks;
   Norm head_norm, sm_head_norm, lg_head_norm;
@@ -375,6 +393,22 @@ struct vb_handle {
       for (int L = 0; L < c.depth; ++L) expect_layer("layers." + std::to_string(L) + ".", c.dim, c.heads, c.dim_head, c.mlp_dim, VB_KIND_VIT);
       expect_ln("head_norm", c.dim);
       expect_dense("head", c.dim, c.num_classes);
+    } else if (c.kind == VB_KIND_CCT) {
+      for (int i = 0; i < c.cct_conv_layers; ++i)                         // Conv2D(use_bias=False) kernel [k, k, cin, cout]
+        expect("tokenizer.conv." + std::to_string(i) + ".kernel", {c.cct_kernel, c.cct_kernel, cct_conv_cin(i), cct_conv_cout(i)});
+      if (c.cct_pos_emb != VB_CCT_POS_NONE) expect("positional_emb", {1, cct_sequence_length(), c.dim});   // cct.py:250-256
+      for (int L = 0; L < c.depth; ++L) {                                 // TransformerEncoderLayer cct.py:139-157
+        const std::string pre = "layers." + std::to_string(L) + ".";
+        expect_ln(pre + "attn_norm", c.dim);                              // pre_norm
+        expect_dense(pre + "to_qkv", c.dim, 3 * c.dim, false);
+        expect_dense(pre + "to_out", c.dim, c.dim);                       // self_attn.proj
+        expect_ln(pre + "norm1", c.dim);
+        expect_dense(pre + "fc1", c.dim, c.mlp_dim);                      // linear1
+        expect_dense(pre + "fc2", c.mlp_dim, c.dim);                      // linear2
+      }
+      expect_ln("norm", c.dim);                                           // cct.py:266
+      expect_dense("attention_pool", c.dim, 1);                           // :248
+      expect_dense("head", c.dim, c.num_classes);                         // fc :267
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       expect("pos_embedding", {1, np, c.dim});
@@ -571,6 +605,21 @@ struct vb_handle {
     l.to_qkv.K = Dp; l.fc1.K = Dp;                                                        // the A operands are Dp wide (zero pad columns)
     return l;
   }
+  // CCT TransformerEncoderLayer (cct.py:159-174): pre_norm folds into to_qkv as in make_layer; norm1 replaces the stream itself
+  // (the fc2 residual is the normalised row), so it runs as a LayerNorm in place and fc1 reads the normalised rows unfolded.
+  LayerW make_cct_layer(const std::string& pre, int dim, int heads, int mlp) {
+    LayerW l;
+    l.heads = heads; l.dim_head = dim / heads; l.dh_model = l.dim_head;
+    l.attn_norm = make_norm(pre + "attn_norm", dim);
+    l.ff_norm = make_norm(pre + "norm1", dim);
+    l.folded = bf16() && dim % 64 == 0 && mlp % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr;   // every GEMM on the wgmma path
+    l.fused_qkv = true;
+    l.to_qkv = make_linear(pre + "to_qkv", dim, 3 * dim, false, l.folded ? &l.attn_norm : nullptr);
+    l.to_out = make_linear(pre + "to_out", dim, dim);
+    l.fc1 = make_linear(pre + "fc1", dim, mlp);
+    l.fc2 = make_linear(pre + "fc2", mlp, dim);
+    return l;
+  }
   EmbedW make_embed(const std::string& pre, int p_h, int p_w, int dim, int n_pos, bool with_cls = true, int K = 0) {
     EmbedW e;
     e.patch = make_linear(pre + "patch", K > 0 ? K : p_h * p_w * cfg.channels, dim);
@@ -583,7 +632,7 @@ struct vb_handle {
   void finalize() {
     for (auto& w : weights) VB_CHECK(w.set, "vb_finalize: weight '" + w.name + "' was never set");
     VB_CUDA(cudaSetDevice(device));
-    owned.clear(); layers.clear(); cls_layers.clear(); t2t_layers.clear(); xblocks.clear(); plans.clear(); embed_res.clear();
+    owned.clear(); layers.clear(); cls_layers.clear(); t2t_layers.clear(); xblocks.clear(); plans.clear(); embed_res.clear(); cct_convs.clear();
     woverride.clear();
     drop_graphs();
     const vb_config& c = cfg;
@@ -622,6 +671,15 @@ struct vb_handle {
       embed = make_embed("", 0, 0, c.dim, out * out + 1, true, st.back().dim);
       for (int L = 0; L < c.depth; ++L) layers.push_back(make_layer("layers." + std::to_string(L) + ".", c.dim, c.heads, c.dim_head, c.mlp_dim, VB_KIND_VIT));
       head_norm = make_norm("head_norm", c.dim);
+      head = make_linear_f32("head", c.dim, c.num_classes);
+    } else if (c.kind == VB_KIND_CCT) {
+      // the 4-D kernel [k, k, cin, cout] is the Dense [k*k*cin, cout] over unfold_same's (row, column, channel) vectors
+      for (int i = 0; i < c.cct_conv_layers; ++i)
+        cct_convs.push_back(make_linear("tokenizer.conv." + std::to_string(i), c.cct_kernel * c.cct_kernel * cct_conv_cin(i), cct_conv_cout(i), false));
+      for (int L = 0; L < c.depth; ++L) layers.push_back(make_cct_layer("layers." + std::to_string(L) + ".", c.dim, c.heads, c.mlp_dim));
+      cct_norm = make_norm("norm", c.dim);
+      cct_pool_w = W("attention_pool.kernel");
+      cct_pool_b = W("attention_pool.bias");
       head = make_linear_f32("head", c.dim, c.num_classes);
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
@@ -775,6 +833,53 @@ struct vb_handle {
     return nullptr;
   }
 
+  // CCT Tokenizer + positional embedding (cct.py:211-215,278-286): per conv layer, unfold_same of the previous map (the fp32
+  // image first) into the Dense operand (zero-padded to the packed weight pitch), the GEMM, then ReLU + SAME max-pool.  The last
+  // pool adds the positions ('sine' / 'learnable') or writes zero rows up to sequence_length ('none').  -> X [B*rows, dim]
+  template <typename T>
+  T* tokenize_cct(const float* img, int B, int H, int Wd, int* rows_out, cudaStream_t s) {
+    const vb_config& c = cfg;
+    const T* map = nullptr;
+    T* out = nullptr;
+    int mh = H, mw = Wd, mc = c.channels;
+    for (int i = 0; i < c.cct_conv_layers; ++i) {
+      const Linear& conv = cct_convs[i];
+      const int oh = (mh + c.cct_stride - 1) / c.cct_stride, ow = (mw + c.cct_stride - 1) / c.cct_stride;
+      const int M = B * oh * ow, Kp = bf16() ? conv.ldw : conv.K;
+      T* col = arena.get<T>(static_cast<size_t>(M) * Kp);
+      {
+        ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(i == 0 ? 4 : sizeof(T)) * B * mh * mw * mc + static_cast<double>(sizeof(T)) * M * Kp, s);
+        if (i == 0) unfold_same<float, T>(img, col, B, mh, mw, mc, c.cct_kernel, c.cct_stride, 0, Kp, s);
+        else unfold_same<T, T>(map, col, B, mh, mw, mc, c.cct_kernel, c.cct_stride, 0, Kp, s);
+      }
+      T* conv_out = arena.get<T>(static_cast<size_t>(M) * conv.N);
+      Linear L = conv;
+      L.K = Kp;
+      linear<T>(col, Kp, M, L, conv_out, conv.N, Epi(), s);
+      const int ph = (oh + c.cct_pool_stride - 1) / c.cct_pool_stride, pw = (ow + c.cct_pool_stride - 1) / c.cct_pool_stride;
+      int rows = ph * pw;
+      const float* pos = nullptr;
+      if (i + 1 == c.cct_conv_layers) {
+        const int n_seq = cct_sequence_length();
+        if (c.cct_pos_emb != VB_CCT_POS_NONE) {                          // cct.py:286: x += positional_emb must broadcast
+          VB_CHECK(rows == n_seq, "CCT: the image gives " + std::to_string(rows) + " tokens but the positional embedding has " +
+                                  std::to_string(n_seq) + " rows (with 'sine' / 'learnable' the image must give img_size's token count)");
+          pos = W("positional_emb");
+        } else if (rows < n_seq) {
+          rows = n_seq;                                                  // cct.py:278-280: zero rows up to sequence_length
+        }
+      }
+      out = arena.get<T>(static_cast<size_t>(B) * rows * conv.N);
+      {
+        ProfScope ps(this, PROF_OTHER, 0.0, static_cast<double>(sizeof(T)) * (static_cast<double>(M) + static_cast<double>(B) * rows) * conv.N, s);
+        maxpool_relu_same<T>(conv_out, out, B, oh, ow, conv.N, c.cct_pool_kernel, c.cct_pool_stride, pos, rows, s);
+      }
+      map = out; mh = ph; mw = pw; mc = conv.N;
+      *rows_out = rows;
+    }
+    return out;
+  }
+
   // `call` up to the transformer for every kind with one token stream
   template <typename T>
   T* embed_any(const float* img, int B, int H, int Wd, int* rows_out, cudaStream_t s, float** stats_out) {
@@ -862,6 +967,38 @@ struct vb_handle {
       if (fold) ensure_stats(X, dim, stats, M, s);
     }
     feed_forward<T>(X, M, dim, l, Y, s, fold ? stats : nullptr);
+  }
+  // One CCT TransformerEncoderLayer (cct.py:159-174, dropout / drop-path the identity):
+  //   x = x + proj(MHA(pre_norm(x)));  x = norm1(x);  x = x + linear2(GELU(linear1(x)))
+  // pre_norm is folded into to_qkv through the row statistics (bf16 engine); norm1 rewrites the rows in place, and fc2, whose
+  // residual is those normalised rows, emits the statistics the next layer's fold reads.
+  template <typename T>
+  void layer_cct(T* X, int B, int rows, int dim, const LayerW& l, cudaStream_t s, float* stats, bool* stats_valid) {
+    const int M = B * rows, inner = l.heads * l.dim_head;
+    const bool fold = l.folded && stats != nullptr;
+    if (fold && !*stats_valid) { ensure_stats(X, dim, stats, M, s); *stats_valid = true; }
+    T* QKV = arena.get<T>(static_cast<size_t>(M) * 3 * inner);
+    T* O = arena.get<T>(static_cast<size_t>(M) * inner);
+    const T* A = X;
+    Epi eq;
+    if (fold) { eq.ln_stats = stats; eq.bias = l.to_qkv.ln_c2; }
+    else {
+      VB_CHECK(!l.folded, "internal: folded layer without statistics");
+      T* Y = arena.get<T>(static_cast<size_t>(M) * dim);
+      ln<T>(X, l.attn_norm, Y, M, dim, s);
+      A = Y;
+    }
+    linear<T>(A, dim, M, l.to_qkv, QKV, 3 * inner, eq, s);
+    attention<T>(QKV, 3 * inner, QKV + inner, 3 * inner, QKV + 2 * inner, 3 * inner, O, inner, B, rows, rows, l, s);
+    Epi e; e.bias = l.to_out.bias; e.res = X; e.ldr = dim;
+    linear<T>(O, inner, M, l.to_out, X, dim, e, s);
+    ln<T>(X, l.ff_norm, X, M, dim, s);                                  // cct.py:165: the stream is replaced by norm1(x)
+    T* Hb = arena.get<T>(static_cast<size_t>(M) * l.fc1.N);
+    Epi e1; e1.gelu = true; e1.bias = l.fc1.bias;
+    linear<T>(X, dim, M, l.fc1, Hb, l.fc1.N, e1, s);
+    Epi e2; e2.bias = l.fc2.bias; e2.res = X; e2.ldr = dim;
+    if (fold) e2.stats_out = stats;
+    linear<T>(Hb, l.fc1.N, M, l.fc2, X, dim, e2, s);
   }
   // One parallel_vit layer (parallel_vit.py:114-117): x = sum_i attn_i(LN_i(x)) + x ; x = sum_i ff_i(LN'_i(x)) + x.
   // Every branch reads the SAME x, so the sums accumulate in a second buffer through the residual epilogue of the
@@ -1061,6 +1198,20 @@ struct vb_handle {
       copy_tokens<T>(X, rows, 0, ctx, rows + 1, 1, rows, B, c.dim, s);
       for (const auto& l : cls_layers) layer_cls<T>(Cx, ctx, B, rows + 1, c.dim, l, s);
       classify<T>(Cx, 1, c.dim, head_norm, head, B, 0, logits, false, s);
+    } else if (c.kind == VB_KIND_CCT) {                   // CCT.call cct.py:342-345, TransformerClassifier.call :277-305
+      int rows = 0;
+      T* X = tokenize_cct<T>(img, B, H, Wd, &rows, s);
+      float* stats = (bf16() && c.dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr)
+                         ? arena.get<float>(static_cast<size_t>(B) * rows * (c.dim / 64) * 2) : nullptr;
+      bool sv = false;
+      for (const auto& l : layers) layer_cct<T>(X, B, rows, c.dim, l, s, stats, &sv);
+      float* z = arena.get<float>(static_cast<size_t>(B) * c.dim);
+      {
+        ProfScope ps(this, PROF_LN, 4.0 * B * rows * c.dim, static_cast<double>(sizeof(T)) * B * rows * c.dim, s);
+        seq_pool<T>(X, rows, c.dim, cct_norm.gamma, cct_norm.beta, cct_pool_w, cct_pool_b, z, B, s);   // :291-299
+      }
+      gemm_simt<float, float, float>(z, c.dim, head.W, head.N, 1, logits, head.N, B, head.N, c.dim, head.bias, nullptr, nullptr,
+                                     head.N, 0, s);                                                   // fc :303
     } else {
       int ns = 0, nl = 0;
       float *st_s = nullptr, *st_g = nullptr;
@@ -1151,8 +1302,10 @@ struct vb_handle {
   }
 
   // ---------------------------------------------------------------- stage entries (vb_forward_embed / _head / vb_patch_to_emb)
+  static constexpr const char* kCctNoStages = "CCT runs as a whole forward only: its tokenizer / classifier stages have no entry of their own";
   int embed_rows(int H, int Wd) const {
     VB_CHECK(cfg.kind != VB_KIND_CROSSVIT, "CrossViT has two token streams: no single embedding stage");
+    VB_CHECK(cfg.kind != VB_KIND_CCT, kCctNoStages);
     if (cfg.kind == VB_KIND_T2T_VIT) {
       int h = H, w = Wd;
       for (const auto& st : t2t_stages()) { h = (h + st.stride - 1) / st.stride; w = (w + st.stride - 1) / st.stride; }
@@ -1177,6 +1330,7 @@ struct vb_handle {
   template <typename T>
   void head_impl(const float* tok, int B, int n, float* logits, cudaStream_t s) {
     VB_CHECK(cfg.kind != VB_KIND_CROSSVIT, "CrossViT sums two heads: no single mlp_head stage");
+    VB_CHECK(cfg.kind != VB_KIND_CCT, kCctNoStages);
     arena.reset();
     const long long count = static_cast<long long>(B) * n * cfg.dim;
     T* X = arena.get<T>(count);
@@ -1187,6 +1341,7 @@ struct vb_handle {
   template <typename T>
   void patch_to_emb_impl(const float* patches, int rows, float* out, cudaStream_t s) {
     VB_CHECK(cfg.kind != VB_KIND_CROSSVIT, "CrossViT has two patch embeddings");
+    VB_CHECK(cfg.kind != VB_KIND_CCT, kCctNoStages);
     arena.reset();
     const int K = embed.patch.K, Kp = bf16() ? embed.patch.ldw : K;
     T* col = arena.get<T>(static_cast<size_t>(rows) * Kp);
@@ -1354,8 +1509,20 @@ int guarded(vb_handle* h, F&& f) {
 }
 
 void validate(const vb_config& c) {
-  VB_CHECK(c.struct_size == static_cast<int32_t>(sizeof(vb_config)), "vb_config.struct_size mismatch (ABI)");
-  VB_CHECK(c.kind >= VB_KIND_VIT && c.kind <= VB_KIND_T2T_VIT, "unknown model kind");
+  VB_CHECK(c.struct_size == static_cast<int32_t>(sizeof(vb_config)) || c.struct_size == VB_CONFIG_SIZE_ABI7,
+           "vb_config.struct_size mismatch (ABI)");
+  VB_CHECK(c.kind >= VB_KIND_VIT && c.kind <= VB_KIND_CCT, "unknown model kind");
+  if (c.kind == VB_KIND_CCT) {
+    VB_CHECK(c.channels == 3 && c.num_classes > 0 && c.image_h > 0 && c.image_w > 0, "bad image / class configuration");
+    VB_CHECK(c.cct_conv_layers >= 1 && c.cct_conv_layers <= 8, "CCT: n_conv_layers must be in [1, 8]");
+    VB_CHECK(c.cct_kernel > 0 && c.cct_stride > 0 && c.cct_pool_kernel > 0 && c.cct_pool_stride > 0,
+             "CCT: kernel / stride / pooling sizes must be positive");
+    VB_CHECK(c.cct_pos_emb >= VB_CCT_POS_SINE && c.cct_pos_emb <= VB_CCT_POS_NONE, "CCT: unknown positional embedding kind");
+    VB_CHECK(c.dim > 0 && c.dim <= 1024 && c.depth >= 0 && c.heads > 0 && c.heads <= 32 && c.mlp_dim > 0, "bad transformer dimensions");
+    VB_CHECK(c.dim % c.heads == 0 && c.dim_head == c.dim / c.heads, "CCT: embedding_dim must be divisible by num_heads");
+    VB_CHECK(c.precision == VB_PRECISION_FP32 || c.precision == VB_PRECISION_BF16, "unknown precision");
+    return;
+  }
   VB_CHECK(c.kind != VB_KIND_PARALLEL_VIT || (c.parallel_branches >= 1 && c.parallel_branches <= 8), "num_parallel_branches must be in [1, 8]");
   VB_CHECK(c.precision == VB_PRECISION_FP32 || c.precision == VB_PRECISION_BF16, "unknown precision");
   VB_CHECK(c.channels > 0 && c.num_classes > 0 && c.image_h > 0 && c.image_w > 0, "bad image / class configuration");
@@ -1484,7 +1651,13 @@ int vb_abi_version(void) { return VB_ABI_VERSION; }
 int vb_create(const vb_config* cfg, int device, vb_handle** out) {
   return guarded(nullptr, [&] {
     VB_CHECK(cfg != nullptr && out != nullptr, "vb_create: null argument");
-    validate(*cfg);
+    // a client of the ABI-7 struct without the CCT fields passes the shorter size: read only its bytes, zero the rest
+    const int32_t size = cfg->struct_size;
+    VB_CHECK(size == static_cast<int32_t>(sizeof(vb_config)) || size == VB_CONFIG_SIZE_ABI7, "vb_config.struct_size mismatch (ABI)");
+    vb_config c;
+    memset(&c, 0, sizeof c);
+    memcpy(&c, cfg, static_cast<size_t>(size));
+    validate(c);
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
     VB_CHECK(e == cudaSuccess && ndev > 0, "vb_create: no CUDA device available -- libvitb200 has no CPU fallback");
@@ -1494,7 +1667,7 @@ int vb_create(const vb_config* cfg, int device, vb_handle** out) {
     VB_CUDA(cudaGetDeviceProperties(&prop, device));
     VB_CHECK(prop.major == 9 && prop.minor == 0, "vb_create: libvitb200 is built for sm_90a (Hopper H100) only");
     std::unique_ptr<vb_handle> h(new vb_handle());
-    h->cfg = *cfg;
+    h->cfg = c;
     h->device = device;
     h->build_expected();
     *out = h.release();
@@ -1735,7 +1908,8 @@ int vb_to_patch(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, 
                 int32_t patches_mem, void* stream) {
   return guarded(h, [&] {
     VB_CHECK(h != nullptr && img != nullptr && patches != nullptr, "vb_to_patch: null argument");
-    VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT && h->cfg.kind != VB_KIND_T2T_VIT, "vb_to_patch: the model has no single Rearrange patch layer");
+    VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT && h->cfg.kind != VB_KIND_T2T_VIT && h->cfg.kind != VB_KIND_CCT,
+             "vb_to_patch: the model has no single Rearrange patch layer");
     VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_to_patch: bad batch / image size");
     const vb_config& c = h->cfg;
     VB_CHECK(img_h % c.patch_h == 0 && img_w % c.patch_w == 0, "Image dimensions must be divisible by the patch size.");
@@ -1754,6 +1928,7 @@ int vb_patch_to_emb(vb_handle* h, const float* patches, int32_t patches_mem, int
     VB_CHECK(h != nullptr && patches != nullptr && out != nullptr, "vb_patch_to_emb: null argument");
     VB_CHECK(h->finalized, "vb_patch_to_emb: call vb_finalize after setting the weights");
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT, "vb_patch_to_emb: CrossViT has two patch embeddings");
+    VB_CHECK(h->cfg.kind != VB_KIND_CCT, vb_handle::kCctNoStages);
     VB_CHECK(rows > 0, "vb_patch_to_emb: bad shape");
     const size_t in_bytes = static_cast<size_t>(rows) * h->embed.patch.K * sizeof(float);
     const size_t out_bytes = static_cast<size_t>(rows) * h->cfg.dim * sizeof(float);

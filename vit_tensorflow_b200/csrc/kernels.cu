@@ -606,6 +606,119 @@ __global__ void unfold_same_kernel(const TI* __restrict__ in, int ldi, TO* __res
   for (int col = K + threadIdx.x; col < ldo; col += blockDim.x) orow[col] = from_f<TO>(0.f);   // pitch padding
 }
 
+// One thread per output element (b, t, c), c fastest: the k*k taps of a thread are C apart, so a warp reads whole channel runs.
+template <typename T>
+__global__ void maxpool_relu_same_kernel(const T* __restrict__ in, T* __restrict__ out, int H, int W, int C, int k, int stride, int oh,
+                                         int ow, int pad_top, int pad_left, const float* __restrict__ pos, int rows, long long total) {
+  for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
+       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int c = static_cast<int>(idx % C);
+    const long long r = idx / C;
+    const int t = static_cast<int>(r % rows);
+    const long long b = r / rows;
+    float v = 0.f;
+    if (t < oh * ow) {
+      const int oy = t / ow, ox = t - oy * ow;
+      const int y0 = oy * stride - pad_top, x0 = ox * stride - pad_left;
+      const T* __restrict__ img = in + b * H * W * C + c;
+      float m = -INFINITY;
+      for (int ky = 0; ky < k; ++ky) {
+        const int y = y0 + ky;
+        if (y < 0 || y >= H) continue;
+        for (int kx = 0; kx < k; ++kx) {
+          const int x = x0 + kx;
+          if (x >= 0 && x < W) m = fmaxf(m, to_f(img[(static_cast<long long>(y) * W + x) * C]));
+        }
+      }
+      v = fmaxf(m, 0.f);
+      if (pos != nullptr) v += pos[static_cast<long long>(t) * C + c];
+    }
+    out[idx] = from_f<T>(v);
+  }
+}
+
+// One CTA per image, 8 warps; warp w takes rows w, w + 8, ...: LayerNorm of the row in registers (lane holds columns
+// lane + 32 j), score by a warp reduction, and a running (max, sum, weighted row sum) per warp; the warps' partial states are
+// merged through shared memory at the end.  The LayerNorm affine is taken out of the loop: with x^ the standardised row,
+// score = x^ . (gamma * pw) + (beta . pw + pb), and since the weights sum to one, z = gamma * sum_t w_t x^_t + beta.
+constexpr int SEQ_POOL_WARPS = 8;
+template <typename T, int J>
+__global__ void __launch_bounds__(SEQ_POOL_WARPS * 32)
+seq_pool_kernel(const T* __restrict__ X, int n, int D, const float* __restrict__ gamma, const float* __restrict__ beta,
+                const float* __restrict__ pw, const float* __restrict__ pb, float* __restrict__ z) {
+  extern __shared__ float sp[];                  // [SEQ_POOL_WARPS][D] partial sums, then [2][SEQ_POOL_WARPS] (max, sum)
+  float* acc_s = sp;
+  float* ml = sp + SEQ_POOL_WARPS * D;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const T* __restrict__ xb = X + static_cast<long long>(blockIdx.x) * n * D;
+  float gw[J], acc[J], cb = 0.f;
+#pragma unroll
+  for (int j = 0; j < J; ++j) {
+    const int d = lane + 32 * j;
+    const bool in = d < D;
+    gw[j] = in ? gamma[d] * pw[d] : 0.f;
+    if (in) cb = fmaf(beta[d], pw[d], cb);
+    acc[j] = 0.f;
+  }
+  const float bias = warp_sum(cb) + pb[0], inv_d = 1.0f / static_cast<float>(D);
+  float m = -INFINITY, l = 0.f;
+  for (int t = warp; t < n; t += SEQ_POOL_WARPS) {
+    const T* __restrict__ row = xb + static_cast<long long>(t) * D;
+    float v[J];
+    float s = 0.f;
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+      const int d = lane + 32 * j;
+      v[j] = d < D ? to_f(row[d]) : 0.f;
+      s += v[j];
+    }
+    const float mean = warp_sum(s) * inv_d;
+    float q = 0.f;
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+      const float e = lane + 32 * j < D ? v[j] - mean : 0.f;
+      q += e * e;
+    }
+    const float rstd = rsqrtf(warp_sum(q) * inv_d + 1e-3f);
+    float sc = 0.f;
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+      v[j] = (v[j] - mean) * rstd;
+      sc = fmaf(v[j], gw[j], sc);                    // gw = 0 beyond D
+    }
+    sc = warp_sum(sc) + bias;
+    const float m_new = fmaxf(m, sc);
+    const float corr = expf(m - m_new), p = expf(sc - m_new);
+    l = l * corr + p;
+#pragma unroll
+    for (int j = 0; j < J; ++j) acc[j] = fmaf(acc[j], corr, p * v[j]);
+    m = m_new;
+  }
+#pragma unroll
+  for (int j = 0; j < J; ++j) {
+    const int d = lane + 32 * j;
+    if (d < D) acc_s[warp * D + d] = acc[j];
+  }
+  if (lane == 0) { ml[warp] = m; ml[SEQ_POOL_WARPS + warp] = l; }
+  __syncthreads();
+  float M = -INFINITY;
+#pragma unroll
+  for (int w = 0; w < SEQ_POOL_WARPS; ++w) M = fmaxf(M, ml[w]);
+  float f[SEQ_POOL_WARPS], L = 0.f;
+#pragma unroll
+  for (int w = 0; w < SEQ_POOL_WARPS; ++w) {
+    f[w] = ml[SEQ_POOL_WARPS + w] > 0.f ? expf(ml[w] - M) : 0.f;   // warps without rows hold (-inf, 0)
+    L = fmaf(ml[SEQ_POOL_WARPS + w], f[w], L);
+  }
+  const float inv_l = 1.0f / L;
+  for (int d = threadIdx.x; d < D; d += blockDim.x) {
+    float a = 0.f;
+#pragma unroll
+    for (int w = 0; w < SEQ_POOL_WARPS; ++w) a = fmaf(acc_s[w * D + d], f[w], a);
+    z[static_cast<long long>(blockIdx.x) * D + d] = fmaf(gamma[d], a * inv_l, beta[d]);
+  }
+}
+
 // out[r, c] = in[r, c] for c < cols, 0 for cols <= c < ldo (row-pitch change with conversion)
 template <typename TI, typename TO>
 __global__ void convert_rows_kernel(const TI* __restrict__ in, int ldi, TO* __restrict__ out, int ldo, long long rows, int cols) {
@@ -863,6 +976,29 @@ void unfold_same(const TI* in, TO* out, int B, int H, int W, int C, int k, int s
   VB_LAUNCHED();
 }
 
+template <typename T>
+void maxpool_relu_same(const T* in, T* out, int B, int H, int W, int C, int k, int stride, const float* pos, int rows, cudaStream_t s) {
+  const int oh = (H + stride - 1) / stride, ow = (W + stride - 1) / stride;
+  VB_CHECK(rows >= oh * ow, "maxpool_relu_same: fewer output rows than pooled positions");
+  const int ph = std::max((oh - 1) * stride + k - H, 0), pw = std::max((ow - 1) * stride + k - W, 0);
+  const long long total = static_cast<long long>(B) * rows * C;
+  maxpool_relu_same_kernel<T><<<grid_1d(total), 256, 0, s>>>(in, out, H, W, C, k, stride, oh, ow, ph / 2, pw / 2, pos, rows, total);
+  VB_LAUNCHED();
+}
+
+template <typename T>
+void seq_pool(const T* X, int n, int D, const float* gamma, const float* beta, const float* pw, const float* pb, float* z, int B,
+              cudaStream_t s) {
+  VB_CHECK(D > 0 && D <= 1024 && n > 0, "seq_pool: needs 0 < dim <= 1024 and at least one token");
+  const size_t smem = (static_cast<size_t>(SEQ_POOL_WARPS) * D + 2 * SEQ_POOL_WARPS) * sizeof(float);
+  const dim3 block(SEQ_POOL_WARPS * 32);
+  if (D <= 128) seq_pool_kernel<T, 4><<<B, block, smem, s>>>(X, n, D, gamma, beta, pw, pb, z);
+  else if (D <= 256) seq_pool_kernel<T, 8><<<B, block, smem, s>>>(X, n, D, gamma, beta, pw, pb, z);
+  else if (D <= 512) seq_pool_kernel<T, 16><<<B, block, smem, s>>>(X, n, D, gamma, beta, pw, pb, z);
+  else seq_pool_kernel<T, 32><<<B, block, smem, s>>>(X, n, D, gamma, beta, pw, pb, z);
+  VB_LAUNCHED();
+}
+
 template <typename TI, typename TO>
 void convert_rows(const TI* in, int ldi, TO* out, int ldo, long long rows, int cols, cudaStream_t s) {
   if (rows == 0) return;
@@ -914,7 +1050,9 @@ void row_stats_bf16(const __nv_bfloat16* X, int ldx, float* stats, int M, int D,
   template void broadcast_row<T>(const float*, T*, int, int, int, cudaStream_t);                                            \
   template void broadcast_rows<T>(const float*, T*, int, int, int, cudaStream_t);                                           \
   template void unfold_same<float, T>(const float*, T*, int, int, int, int, int, int, int, int, cudaStream_t, int);         \
-  template void convert_rows<float, T>(const float*, int, T*, int, long long, int, cudaStream_t);
+  template void convert_rows<float, T>(const float*, int, T*, int, long long, int, cudaStream_t);                           \
+  template void maxpool_relu_same<T>(const T*, T*, int, int, int, int, int, int, const float*, int, cudaStream_t);         \
+  template void seq_pool<T>(const T*, int, int, const float*, const float*, const float*, const float*, float*, int, cudaStream_t);
 VB_INST_T(float)
 VB_INST_T(__nv_bfloat16)
 

@@ -70,6 +70,19 @@ void broadcast_rows(const float* vec, T* dst, int B, int nt, int D, cudaStream_t
 template <typename TI, typename TO>
 void unfold_same(const TI* in, TO* out, int B, int H, int W, int C, int k, int stride, int cls_row, int ldo, cudaStream_t s, int ldi = 0);
 
+// CCT tokenizer tail (cct.py:196-200,213): ReLU -> MaxPool2D(k, stride, padding 'SAME') -> 'b h w c -> b (h w) c', NHWC.
+// in [B, H, W, C] -> out [B, rows, C], oh = ceil(H / stride), rows >= oh * ow; total padding max((oh-1)*stride + k - H, 0) with
+// the smaller half first, padded taps never win the max.  ReLU is applied after the max (both are monotone: the same value).
+// pos (fp32 [oh*ow, C], may be null) is added after the ReLU; rows [oh*ow, rows) are zero (the 'none' embedding's zero padding).
+template <typename T>
+void maxpool_relu_same(const T* in, T* out, int B, int H, int W, int C, int k, int stride, const float* pos, int rows, cudaStream_t s);
+
+// CCT sequence pooling (cct.py:291-299): per image b, y_t = LayerNorm(X[b, t]) (eps 1e-3), w_t = softmax_t(y_t . pw + pb),
+// z[b] = sum_t w_t y_t.  X [B, n, D] -> z fp32 [B, D]; D <= 1024.  One CTA per image, fp32 statistics, online softmax.
+template <typename T>
+void seq_pool(const T* X, int n, int D, const float* gamma, const float* beta, const float* pw, const float* pb, float* z, int B,
+              cudaStream_t s);
+
 // out[r, 0:cols] = in[r, 0:cols], out[r, cols:ldo] = 0 (type conversion with a row-pitch change).
 template <typename TI, typename TO>
 void convert_rows(const TI* in, int ldi, TO* out, int ldo, long long rows, int cols, cudaStream_t s);

@@ -154,7 +154,8 @@ class _EngineModel:
         for name, shape in self._specs.items():
             leaf = name.rsplit(".", 1)[-1]
             if leaf == "kernel":
-                lim = np.sqrt(6.0 / (shape[0] + shape[1]))
+                receptive = int(np.prod(shape[:-2]))          # Conv2D kernel [k, k, cin, cout]: fans count the window (1 for Dense)
+                lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
                 a = rng.uniform(-lim, lim, size=shape)
             elif leaf in ("bias", "beta"):
                 a = np.zeros(shape)
@@ -163,6 +164,9 @@ class _EngineModel:
             elif leaf in ("attn_scale", "ff_scale"):
                 layer = int(name.split(".layers.")[1].split(".")[0])
                 a = np.full(shape, _layerscale_eps(layer + 1))
+            elif leaf == "positional_emb":                   # CCT cct.py:251-254
+                a = (sinusoidal_embedding(shape[1], shape[2]) if self._positional_embedding == "sine"
+                     else _truncated_normal(rng, shape, 0.2))
             else:  # pos_embedding, cls_token, reattn_weights, mix_pre, mix_post
                 a = rng.standard_normal(shape)
             w[name] = a.astype(np.float32)
@@ -604,8 +608,139 @@ class EfficientViT(_EngineModel):
     call = __call__
 
 
+def sinusoidal_embedding(n_channels, dim):
+    """TransformerClassifier.sinusoidal_embedding (cct.py:269-275) as the code spells it: the angles as Python floats, cast to
+    float32, then sin / cos in float32 on the even / odd columns.  -> float32 [1, n_channels, dim]."""
+    pe = np.asarray([[p / (10000 ** (2 * (i // 2) / dim)) for i in range(dim)] for p in range(n_channels)]).astype(np.float32)
+    pe[:, 0::2] = np.sin(pe[:, 0::2])
+    pe[:, 1::2] = np.cos(pe[:, 1::2])
+    return pe[None]
+
+
+def _truncated_normal(rng, shape, stddev):
+    """tf.random.truncated_normal: N(0, stddev) with draws beyond two standard deviations redrawn."""
+    a = rng.standard_normal(shape)
+    bad = np.abs(a) > 2.0
+    while bad.any():
+        a[bad] = rng.standard_normal(int(bad.sum()))
+        bad = np.abs(a) > 2.0
+    return a * stddev
+
+
+def cct_token_grid(h, w, n_conv_layers, stride, pooling_stride):
+    """Token grid of the CCT Tokenizer (cct.py:188-215): every Conv2D and MaxPool2D uses SAME padding, ceil(size / stride)."""
+    for _ in range(n_conv_layers):
+        h, w = -(-h // stride), -(-w // stride)
+        h, w = -(-h // pooling_stride), -(-w // pooling_stride)
+    return h, w
+
+
+class TransformerClassifier:
+    """The constructor-argument handling of the reference's TransformerClassifier (cct.py:217-242), which CCT forwards its
+    *args / **kwargs to: same parameter list, so positional extras and the kwargs CCT sets itself raise the same TypeError
+    (multiple values), unknown kwargs are swallowed and an unknown positional_embedding falls back to 'sine'.  Holds the
+    resolved configuration; the layers are the engine's."""
+
+    def __init__(self, seq_pool=True, embedding_dim=768, num_layers=12, num_heads=12, mlp_ratio=4.0, num_classes=1000,
+                 dropout_rate=0.1, attention_dropout=0.1, stochastic_depth_rate=0.1, positional_embedding='sine',
+                 sequence_length=None, *args, **kwargs):
+        positional_embedding = positional_embedding if positional_embedding in ['sine', 'learnable', 'none'] else 'sine'
+        self.embedding_dim, self.num_layers, self.num_heads, self.num_classes = embedding_dim, num_layers, num_heads, num_classes
+        self.mlp_dim = int(embedding_dim * mlp_ratio)                                 # cct.py:235
+        self.positional_embedding, self.sequence_length, self.seq_pool = positional_embedding, sequence_length, seq_pool
+        self.dropout_rates = (dropout_rate, attention_dropout, stochastic_depth_rate)
+        assert sequence_length is not None or positional_embedding == 'none', \
+            f"Positional embedding is set to {positional_embedding} and" \
+            f" the sequence length was not specified."
+
+
+class CCT(_EngineModel):
+    """cct.py:307-345: convolutional tokenizer (n_conv_layers x Conv2D SAME -> ReLU -> MaxPool2D SAME), positional embedding,
+    post-attention-norm encoder layers (x = norm1(x + attn(pre_norm(x))); x = x + mlp(x)), sequence pooling, fc.
+
+    Inference only: the reference hard-codes attention_dropout = stochastic_depth_rate = 0.1 (cct.py:336-338) and its call
+    resolves `training=None` to the classifier's default True, so every call without `training=False` is stochastic there;
+    here such a call raises NotImplementedError.  Images are NHWC with 3 channels; with a 'sine' / 'learnable' embedding they
+    must give the token count of `img_size`, with 'none' fewer tokens are zero-padded to it (cct.py:278-280).
+    Weights (SURVEY.md App. B): tokenizer.conv.{i}.kernel [k, k, cin, cout], positional_emb [1, n, dim],
+    layers.L.{attn_norm, to_qkv, to_out, norm1, fc1, fc2}, norm, attention_pool [dim, 1] + [1], head."""
+    _kind = "cct"
+
+    def __init__(self, img_size=224, embedding_dim=768, n_input_channels=3, n_conv_layers=1, kernel_size=7, stride=2,
+                 pooling_kernel_size=3, pooling_stride=2, *args, precision="bf16", device=0, seed=None, **kwargs):
+        img_height, img_width = pair(img_size)
+        if n_input_channels != 3:
+            raise NotImplementedError("libvitb200 takes NHWC images with 3 channels")
+        seq_h, seq_w = cct_token_grid(img_height, img_width, n_conv_layers, stride, pooling_stride)
+        tc = TransformerClassifier(sequence_length=seq_h * seq_w, embedding_dim=embedding_dim, seq_pool=True, dropout_rate=0.,
+                                   attention_dropout=0.1, stochastic_depth_rate=0.1, *args, **kwargs)   # cct.py:330-339
+        if embedding_dim % tc.num_heads != 0:
+            raise ValueError(f"CCT: embedding_dim ({embedding_dim}) must be divisible by num_heads ({tc.num_heads})")
+        self.num_classes, self.dim = tc.num_classes, embedding_dim
+        self.sequence_length = tc.sequence_length
+        self._positional_embedding = tc.positional_embedding
+        self._dropout_rates = tc.dropout_rates
+        self._create(precision, device, image_h=img_height, image_w=img_width, num_classes=tc.num_classes, dim=embedding_dim,
+                     depth=tc.num_layers, heads=tc.num_heads, dim_head=embedding_dim // tc.num_heads, mlp_dim=tc.mlp_dim,
+                     cct_conv_layers=n_conv_layers, cct_kernel=kernel_size, cct_stride=stride, cct_pool_kernel=pooling_kernel_size,
+                     cct_pool_stride=pooling_stride, cct_pos_emb=_lib.CCT_POS[tc.positional_embedding])
+        self.init_weights(seed)
+
+    def _check_training(self, training):
+        if training is None or training:
+            raise NotImplementedError(
+                "CCT runs inference only: the reference's call resolves training=None to True and then applies its "
+                "hard-coded attention dropout and stochastic depth of 0.1 (cct.py:336-338); pass training=False")
+
+    def __call__(self, img, training=None, **kwargs):
+        """cct.py:342: NHWC float image batch -> float32 logits [b, num_classes]; training must be False."""
+        return super().__call__(img, training=training)
+
+    call = __call__
+
+
+def _cct(num_layers, num_heads, mlp_ratio, embedding_dim, kernel_size=3, stride=None, *args, **kwargs):   # cct.py:51-61
+    stride = stride if stride is not None else max(1, (kernel_size // 2) - 1)
+    return CCT(num_layers=num_layers, num_heads=num_heads, mlp_ratio=mlp_ratio, embedding_dim=embedding_dim,
+               kernel_size=kernel_size, stride=stride, *args, **kwargs)
+
+
+def cct_2(*args, **kwargs):   # cct.py:16-48
+    return _cct(num_layers=2, num_heads=2, mlp_ratio=1, embedding_dim=128, *args, **kwargs)
+
+
+def cct_4(*args, **kwargs):
+    return _cct(num_layers=4, num_heads=2, mlp_ratio=1, embedding_dim=128, *args, **kwargs)
+
+
+def cct_6(*args, **kwargs):
+    return _cct(num_layers=6, num_heads=4, mlp_ratio=2, embedding_dim=256, *args, **kwargs)
+
+
+def cct_7(*args, **kwargs):
+    return _cct(num_layers=7, num_heads=4, mlp_ratio=2, embedding_dim=256, *args, **kwargs)
+
+
+def cct_8(*args, **kwargs):
+    return _cct(num_layers=8, num_heads=4, mlp_ratio=2, embedding_dim=256, *args, **kwargs)
+
+
+def cct_14(*args, **kwargs):
+    return _cct(num_layers=14, num_heads=6, mlp_ratio=3, embedding_dim=384, *args, **kwargs)
+
+
+def cct_16(*args, **kwargs):
+    return _cct(num_layers=16, num_heads=6, mlp_ratio=3, embedding_dim=384, *args, **kwargs)
+
+
+CCT_CTOR_KEYS = ("img_size", "embedding_dim", "n_input_channels", "n_conv_layers", "kernel_size", "stride", "pooling_kernel_size",
+                 "pooling_stride", "num_layers", "num_heads", "mlp_ratio", "num_classes", "positional_embedding")
+
+
 def from_config(cfg: dict, precision="bf16", device=0, seed=None):
     """Build a model from an oracle-style config dict (kind + reference kwargs)."""
+    if cfg["kind"] == "cct":
+        return CCT(**{k: v for k, v in cfg.items() if k in CCT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     kw = {k: v for k, v in cfg.items() if k not in ("kind", "channels", "image_h", "image_w", "patch_h", "patch_w", "num_patches",
                                                     "patch_merge_layer_index", "t2t_dims")}
     if cfg["kind"] == "patch_merger_vit":
