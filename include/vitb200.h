@@ -10,6 +10,7 @@
  *     T2TViT(...)(img)               vit_tensorflow/t2t.py:50-54,96-116               (SURVEY.md 8f, f3)
  *     vit_with_patch_merger.ViT(...)(img)   vit_tensorflow/vit_with_patch_merger.py:134-146,174-185   (8f, f4)
  *     efficient.ViT(...)(img)        vit_tensorflow/efficient.py:13-14,39-55 = vb_forward_embed -> caller's transformer -> vb_forward_head
+ *     LeViT(...)(img)                vit_tensorflow/levit.py:164-226 (vb_create_levit; distillation head: vb_forward_distill)
  * and this header is what the Python host classes (vit_tensorflow_b200/models.py, _lib.py) bind with ctypes.
  * Plain pointers and sizes only; no torch / C++ types cross the boundary.
  *
@@ -39,7 +40,7 @@ extern "C" {
 typedef struct vb_handle vb_handle;
 
 enum { VB_KIND_VIT = 0, VB_KIND_DEEPVIT = 1, VB_KIND_CAIT = 2, VB_KIND_CROSSVIT = 3, VB_KIND_PARALLEL_VIT = 4,
-       VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6, VB_KIND_CCT = 7 };
+       VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6, VB_KIND_CCT = 7, VB_KIND_LEVIT = 8 };
 enum { VB_CCT_POS_SINE = 0, VB_CCT_POS_LEARNABLE = 1, VB_CCT_POS_NONE = 2 };   /* cct.py:233-234,250-256 */
 enum { VB_PRECISION_FP32 = 0, VB_PRECISION_BF16 = 1 };
 enum { VB_POOL_CLS = 0, VB_POOL_MEAN = 1 };
@@ -83,8 +84,33 @@ typedef struct vb_config {
 
 VB_API int vb_abi_version(void);
 
-/* Replaces <Model>.__init__ (vit.py:107-157 etc.): validates the config and allocates device state. */
+/* Replaces <Model>.__init__ (vit.py:107-157 etc.): validates the config and allocates device state.  VB_KIND_LEVIT is refused
+ * here: a LeViT handle comes from vb_create_levit. */
 VB_API int vb_create(const vb_config* cfg, int device, vb_handle** out);
+
+/* LeViT (levit.py:164-212), appended within ABI 7.  `dims`, `depths` and `heads` hold `stages` entries each (cast_tuple already
+ * applied, :180-182).  The stem is four Conv2D(3x3, stride 2, SAME, bias) going channels -> 32 -> 64 -> 128 -> dims[0]; stage s
+ * is depths[s] x (Attention(dims[s], heads[s], dim_key, dim_value) + MLP(mlp_mult)) on a fmap x fmap map (fmap = image_h / 16,
+ * halved with ceil after each shrink); between stages s and s+1 one shrink block: attention with 2 * heads[s] heads whose queries
+ * are the even pixels, to dims[s+1], then an MLP of multiplier 2 (:203).  Head: global average pool -> Dense(num_classes), plus
+ * Dense(num_distill_classes) when num_distill_classes > 0 (:210). */
+#define VB_LEVIT_MAX_STAGES 8
+typedef struct vb_levit_config {
+  int32_t struct_size;            /* sizeof(vb_levit_config) */
+  int32_t stages;                 /* 1 .. VB_LEVIT_MAX_STAGES */
+  int32_t dims[VB_LEVIT_MAX_STAGES], depths[VB_LEVIT_MAX_STAGES], heads[VB_LEVIT_MAX_STAGES];
+  int32_t dim_key, dim_value, mlp_mult;
+  int32_t num_distill_classes;    /* 0: no distillation head */
+} vb_levit_config;
+
+/* LeViT.__init__: `base` supplies precision, image_h == image_w (image_size, a multiple of 16), channels, num_classes and
+ * max_batch; its kind must be VB_KIND_LEVIT and its other fields are ignored.  Weights (SURVEY.md App. B) are named by the
+ * reference's attribute paths: conv_embedding.{i}.kernel [3, 3, cin, cout] / .bias, backbone.{t}.layers.{l}.0.{to_q,to_k,to_v}.0
+ * .kernel [1, 1, cin, cout] with the BatchNormalization .1.{gamma,beta,moving_mean,moving_variance}, .0.pos_bias.embeddings
+ * [fmap^2, heads], .0.to_out.1.kernel / .bias and .0.to_out.2.{BatchNormalization}, .1.net.0 / .1.net.3 .kernel / .bias (the
+ * MLP), mlp_head and distill_head .kernel / .bias.  vb_finalize folds every BatchNormalization (inference statistics, eps 1e-5)
+ * into its convolution. */
+VB_API int vb_create_levit(const vb_config* base, const vb_levit_config* lv, int device, vb_handle** out);
 
 /* Replaces Keras variable assignment: one call per weight, names/shapes/layouts per SURVEY.md App. B
  * (Dense kernel [in,out], float32).  shape/ndim are checked against the config. */
@@ -120,12 +146,14 @@ VB_API int vb_forward_tokens(vb_handle* h, const float* tokens, int32_t tokens_m
  * patch embedding + cls + positions, the token appended as the LAST row, the transformer over n + 2 rows, then
  * logits = mlp_head(pool(x[:, :-1])) and distill_out = x[:, -1].
  * distill_token: HOST float32 [dim] (the caller's trainable variable, distill.py:133).  logits [batch, num_classes] and
- * distill_out [batch, dim] live in `out_mem` memory.  img as in vb_forward. */
+ * distill_out [batch, dim] live in `out_mem` memory.  img as in vb_forward.
+ * LeViT with a distillation head (levit.py:210,220-224): distill_token must be NULL; logits [batch, num_classes] =
+ * mlp_head(pool(x)) and distill_out [batch, num_distill_classes] = distill_head(pool(x)). */
 VB_API int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, int32_t img_h, int32_t img_w,
                        const float* distill_token, float* logits, float* distill_out, int32_t out_mem, void* stream);
 
 /* ---- the stages of <Model>.call on their own (SURVEY.md 8f f1/f4): the attribute surface the reference's wrappers and the
- * injected-transformer shell use.  ViT / DeepViT / parallel ViT / CaiT / patch-merger ViT / T2TViT; not CrossViT. ----------- */
+ * injected-transformer shell use.  ViT / DeepViT / parallel ViT / CaiT / patch-merger ViT / T2TViT; not CrossViT, CCT or LeViT. */
 
 /* Number of token rows vb_forward_embed produces for an img_h x img_w image (patches + cls where the model has one);
  * negative on error. */
@@ -196,6 +224,8 @@ VB_API int32_t vb_last_attention_path(void);
  * for the roofline report.  Classes: 0 wgmma GEMM (plain / LayerNorm-folded epilogue: to_qkv, to_q, to_kv), 1 attention,
  * 2 LayerNorm / row statistics, 3 im2col, 4 other (SIMT fallbacks), 5 wgmma GEMM with GELU epilogue (fc1),
  * 6 wgmma GEMM with residual epilogue (patch embed, to_out, fc2).
+ * LeViT: the stem's unfold is 3 and its convolutions 0; the q / k|v projections and the shrink blocks' to_out are 0, the biased
+ * attention 1, the hard-swish fc1 5, the residual to_out / fc2 6; the even-pixel gather is 4 and the average pool 2.
  * vb_profile_read synchronises the device and returns accumulated milliseconds, algorithmic FLOPs, algorithmic
  * bytes and launch counts per class (arrays of VB_PROF_NUM); reset != 0 clears the accumulators. */
 #define VB_PROF_NUM 7
@@ -269,6 +299,16 @@ VB_API int vb_op_attention_ex(int32_t precision, int32_t variant, const float* q
                               int32_t k_off, int32_t v_off, const float* mix_a, const float* mix_b, const float* ln_gamma,
                               const float* ln_beta, float* out, int32_t ldo, int32_t B, int32_t nq, int32_t nk, int32_t heads,
                               int32_t dh, float scale, int32_t iters, float* elapsed_ms);
+
+/* LeViT attention (levit.py:119-139) as the engine runs it: softmax(q k^T * scale + bias) v, then GELU (gelu_out != 0).
+ * q [B*nq, ldq], k [B*nk, ldk], v [B*nk, ldv] (head h at columns [h*dh, (h+1)*dh)); out [B*nq, ldo], uploaded and downloaded
+ * whole.  nk = fmap^2 keys on a fmap x fmap grid; nq = ceil(fmap / q_step)^2 queries on its pixels (q_step*r, q_step*c).
+ * pos_bias: the Embedding table [fmap^2, heads] (levit.py:101); the bias of (i, j) is pos_bias[|dr| * fmap + |dc|, h] / scale
+ * (:117), packed as vb_finalize packs it.  scale > 0 (the model's dim_key^-0.5).  The flash kernel serves dh == 64 (bf16);
+ * other widths and every fp32 call take the materialised-scores path (vb_last_attention_path tells which). */
+VB_API int vb_op_attention_bias(int32_t precision, const float* q, int32_t ldq, const float* k, int32_t ldk, const float* v,
+                                int32_t ldv, const float* pos_bias, float* out, int32_t ldo, int32_t B, int32_t heads, int32_t dh,
+                                int32_t fmap, int32_t q_step, float scale, int32_t gelu_out, int32_t iters, float* elapsed_ms);
 
 /* Row softmax of fp32 scores into bf16 probabilities (the T2T attention): p[r, j] = softmax_j(s[r, j] * scale) for j < n,
  * p[r, n..npad) = 0.  s [rows, lds], p [rows, ldp] (uploaded and downloaded whole); n <= npad <= ldp. */

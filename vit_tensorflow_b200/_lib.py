@@ -11,7 +11,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "libvitb200.so")   # VB_LIB_PATH: developer A/B builds
 
-KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6, "cct": 7}
+KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6, "cct": 7, "levit": 8}
 PRECISION = {"fp32": 0, "float32": 0, "bf16": 1, "bfloat16": 1}
 MEM_HOST, MEM_DEVICE = 0, 1
 ABI_VERSION = 7                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
@@ -32,6 +32,13 @@ class VbConfig(C.Structure):
 
 CONFIG_SIZE_ABI7 = VbConfig.cct_conv_layers.offset   # VB_CONFIG_SIZE_ABI7: the struct before the CCT fields were appended
 CCT_POS = {"sine": 0, "learnable": 1, "none": 2}     # VB_CCT_POS_*
+LEVIT_MAX_STAGES = 8                                # VB_LEVIT_MAX_STAGES
+
+
+class VbLevitConfig(C.Structure):
+    _fields_ = [("struct_size", C.c_int32), ("stages", C.c_int32), ("dims", C.c_int32 * LEVIT_MAX_STAGES),
+                ("depths", C.c_int32 * LEVIT_MAX_STAGES), ("heads", C.c_int32 * LEVIT_MAX_STAGES), ("dim_key", C.c_int32),
+                ("dim_value", C.c_int32), ("mlp_mult", C.c_int32), ("num_distill_classes", C.c_int32)]
 
 
 class VbError(RuntimeError):
@@ -45,6 +52,7 @@ _i64p = C.POINTER(C.c_int64)
 SIGNATURES = {
     "vb_abi_version": (C.c_int, []),
     "vb_create": (C.c_int, [C.POINTER(VbConfig), C.c_int, C.POINTER(C.c_void_p)]),
+    "vb_create_levit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbLevitConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, _i64p, C.c_int32]),
     "vb_num_weights": (C.c_int, [C.c_void_p]),
     "vb_weight_info": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), _i64p, C.POINTER(C.c_int32)]),
@@ -77,6 +85,8 @@ SIGNATURES = {
                              C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] + [C.c_int32] * 4 + [_f32p]),
     "vb_op_attention_ex": (C.c_int, [C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 5 +
                            [C.c_int32] * 6 + [C.c_float, C.c_int32, _f32p]),
+    "vb_op_attention_bias": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
+                                       C.c_void_p] + [C.c_int32] * 6 + [C.c_float, C.c_int32, C.c_int32, _f32p]),
     "vb_op_softmax_rows": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 4 + [C.c_float, C.c_int32, _f32p]),
 }
 
@@ -207,6 +217,19 @@ def op_attention_ex(q, heads, dh, out, kv=None, k_off=0, v_off=0, variant=0, mix
     check(load().vb_op_attention_ex(PRECISION[precision], variant, _ptr(q), ldq, _ptr(kv), ldkv, k_off, v_off, _ptr(mix_a), _ptr(mix_b),
                                     _ptr(ln_gamma), _ptr(ln_beta), _ptr(out), out.shape[2], B, nq, nk, heads, dh, float(scale), iters,
                                     C.byref(ms)))
+    return out, (ms.value if iters > 0 else None)
+
+
+def op_attention_bias(q, k, v, pos_bias, heads, dh, fmap, q_step, scale, out, gelu_out=True, precision="bf16", iters=0):
+    """LeViT attention (vb_op_attention_bias): q [B, nq, ldq], k / v [B, fmap^2, ld], pos_bias the Embedding table [fmap^2, heads],
+    out [B, nq, ldo] initial contents, returned whole.  Returns (out, ms or None)."""
+    q, k, v, pos_bias = map(_f32, (q, k, v, pos_bias))
+    out = np.array(out, dtype=np.float32, order="C", copy=True)
+    B = q.shape[0]
+    ms = C.c_float(0)
+    check(load().vb_op_attention_bias(PRECISION[precision], _ptr(q), q.shape[2], _ptr(k), k.shape[2], _ptr(v), v.shape[2], _ptr(pos_bias),
+                                      _ptr(out), out.shape[2], B, heads, dh, fmap, q_step, float(scale), int(bool(gelu_out)), iters,
+                                      C.byref(ms)))
     return out, (ms.value if iters > 0 else None)
 
 

@@ -17,17 +17,18 @@ int take_last_attention_path();                  // and reset it to ATTN_PATH_NO
 // variant 0: softmax(QK^T*scale)V                   (vit.py:77-82, cross_vit.py:87-91)
 // variant 1: DeepViT re-attention: softmax -> head mix (mix_a [h,h]) -> LayerNorm over heads (deepvit.py:79-87)
 // variant 2: CaiT talking heads: mix_a before softmax, mix_b after (cait.py:121-127)
+// scale: softmax scale; <= 0 means dh^-0.5 (vit.py:57).  A layer whose heads were zero-padded to the kernels' head width
+// (engine.cu: dh 48 -> 64) passes its true dim_head^-0.5 here.  pb (variant 0 only, may be null): LeViT's relative-position
+// bias and output GELU (common.h).
 template <typename T>
 void attention_generic(const T* q, int ldq, const T* k, int ldk, const T* v, int ldv, T* out, int ldo, float* S, int B, int nq,
                        int nk, int heads, int dh, int variant, const float* mix_a, const float* mix_b, const float* ln_gamma,
-                       const float* ln_beta, cudaStream_t s);
+                       const float* ln_beta, cudaStream_t s, float scale = 0.f, const PosBias* pb = nullptr);
 
-// scale: softmax scale; <= 0 means dh^-0.5 (vit.py:57).  A layer whose heads were zero-padded to the kernels' head width
-// (engine.cu: dh 48 -> 64) passes its true dim_head^-0.5 here.
 template <typename T>
 bool attention_fast(const T* q, int ldq, const T* k, int ldk, const T* v, int ldv, T* out, int ldo, int B, int nq, int nk,
                     int heads, int dh, int variant, const float* mix_a, const float* mix_b, const float* ln_gamma,
-                    const float* ln_beta, cudaStream_t s, float scale = 0.f);
+                    const float* ln_beta, cudaStream_t s, float scale = 0.f, const PosBias* pb = nullptr);
 
 // The talking-heads / re-attention path keeps host copies of the head-mix weights keyed by their device pointers (one process-
 // wide cache for all handles); whoever frees or rewrites such weights (vb_finalize, vb_destroy, the op-level test entries) must
@@ -38,7 +39,8 @@ void attention_mix_cache_erase(const std::vector<const void*>& ptrs);
 // Tensor-core (mma.sync) + fused-middle version of attention_generic for the bf16 engine; false if the shape is not covered.
 bool attention_generic_mma(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, int ldk, const __nv_bfloat16* v, int ldv,
                            __nv_bfloat16* out, int ldo, float* S, int B, int nq, int nk, int heads, int dh, int variant,
-                           const float* mix_a, const float* mix_b, const float* ln_gamma, const float* ln_beta, cudaStream_t s);
+                           const float* mix_a, const float* mix_b, const float* ln_gamma, const float* ln_beta, cudaStream_t s,
+                           float scale = 0.f, const PosBias* pb = nullptr);
 
 // Head-mix weights as kernel parameters (heads <= 16): wa = pre-softmax mix (CaiT) / re-attention weights (DeepViT), wb = CaiT's
 // post-softmax mix, both [h][g] with row pitch `heads`; gamma / beta = DeepViT's LayerNorm over heads.

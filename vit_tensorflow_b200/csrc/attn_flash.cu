@@ -11,6 +11,10 @@
 //   O += P V        the S fragments, rounded to bf16, ARE the A fragments of the next product; V fragments by
 //                   ldmatrix.trans from the row-major V tile.
 // Final 1/l normalisation and bf16 stores in 'b n (h d)' order (the merge-heads rearrange, vit.py:82).
+//
+// BIAS (LeViT, levit.py:114-117,94): the head's [fmap^2] relative-position table sits in shared memory (in log2 units); every
+// score gets table[pos_bias_index(i, j)] added before the online softmax, and the stored rows optionally go through GELU.
+// With BIAS the scores are moved to log2 units as soon as they are computed, so the softmax below runs with a unit scale.
 #include "attention.cuh"
 #include "kernels.cuh"
 #include "ptx.cuh"
@@ -34,10 +38,14 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
 
+constexpr int FLASH_BIAS_MAX = 4096;   // fmap^2 of the largest relative-position table (16 KB of shared memory)
+
+template <bool BIAS>
 __global__ void __launch_bounds__(128)
 attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloat16* __restrict__ k, int ldk,
                   const __nv_bfloat16* __restrict__ v, int ldv, __nv_bfloat16* __restrict__ out, int ldo, int heads, int nq, int nk,
-                  float scale_log2) {
+                  float scale_log2, const float* __restrict__ pos_tab, int fmap, int step, int gelu_out) {
+  extern __shared__ float tab[];                                     // BIAS: [fmap^2] of this head, times log2(e)
   __shared__ __align__(16) __nv_bfloat16 Qs[FQ][FP];
   __shared__ __align__(16) __nv_bfloat16 Ks[2][FK][FP];
   __shared__ __align__(16) __nv_bfloat16 Vs[2][FK][FP];
@@ -74,6 +82,13 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
     asm volatile("cp.async.commit_group;" ::: "memory");
   };
   stage(0);
+  int nqs = 1, qrow[2] = {0, 0};
+  if (BIAS) {
+    const int f2 = fmap * fmap;
+    for (int e = threadIdx.x; e < f2; e += 128) tab[e] = pos_tab[static_cast<size_t>(h) * f2 + e] * 1.4426950408889634f;
+    nqs = (fmap + step - 1) / step;
+    for (int r = 0; r < 2; ++r) qrow[r] = min(i0 + warp * 16 + (lane >> 2) + 8 * r, nq - 1);   // rows past nq: any valid index
+  }
 
   const int qr = lane >> 2, qc = 2 * (lane & 3);                     // fragment row (and row + 8) / column pair of this lane
   uint32_t qf[DH / 16][4];
@@ -113,16 +128,19 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
     for (int n = 0; n < FK / 8; ++n) {
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
+        if (BIAS && n * 8 + qc + (e & 1) < valid)
+          sc[n][e] = fmaf(sc[n][e], scale_log2, tab[pos_bias_index(qrow[e >> 1], j * FK + n * 8 + qc + (e & 1), fmap, step, nqs)]);
         if (n * 8 + qc + (e & 1) >= valid) sc[n][e] = -INFINITY;
         mx[e >> 1] = fmaxf(mx[e >> 1], sc[n][e]);
       }
     }
+    const float sl = BIAS ? 1.0f : scale_log2;                      // BIAS: the scores are already in log2 units
     float alpha[2];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
       mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-      const float m_new = fmaxf(m_run[r], mx[r] * scale_log2);       // every block holds at least one valid key: finite
+      const float m_new = fmaxf(m_run[r], mx[r] * sl);       // every block holds at least one valid key: finite
       alpha[r] = ex2_approx(m_run[r] - m_new);                       // first block: 2^-inf = 0
       m_run[r] = m_new;
       l_run[r] *= alpha[r];
@@ -135,10 +153,10 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
     uint32_t pf[FK / 16][4];                                         // P as the A fragments of the PV product
 #pragma unroll
     for (int n = 0; n < FK / 8; ++n) {
-      const float p0 = ex2_approx(fmaf(sc[n][0], scale_log2, -m_run[0]));
-      const float p1 = ex2_approx(fmaf(sc[n][1], scale_log2, -m_run[0]));
-      const float p2 = ex2_approx(fmaf(sc[n][2], scale_log2, -m_run[1]));
-      const float p3 = ex2_approx(fmaf(sc[n][3], scale_log2, -m_run[1]));
+      const float p0 = ex2_approx(fmaf(sc[n][0], sl, -m_run[0]));
+      const float p1 = ex2_approx(fmaf(sc[n][1], sl, -m_run[0]));
+      const float p2 = ex2_approx(fmaf(sc[n][2], sl, -m_run[1]));
+      const float p3 = ex2_approx(fmaf(sc[n][3], sl, -m_run[1]));
       l_run[0] += p0 + p1;
       l_run[1] += p2 + p3;
       pf[n >> 1][(n & 1) * 2 + 0] = pack_bf16x2(p0, p1);
@@ -171,8 +189,11 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
     if (row >= nq) continue;
     __nv_bfloat16* orow = out + (static_cast<size_t>(b) * nq + row) * ldo + h * DH + qc;
 #pragma unroll
-    for (int n = 0; n < DH / 8; ++n)
-      *reinterpret_cast<uint32_t*>(orow + n * 8) = pack_bf16x2(o[n][2 * r] * l_run[r], o[n][2 * r + 1] * l_run[r]);
+    for (int n = 0; n < DH / 8; ++n) {
+      float a0 = o[n][2 * r] * l_run[r], a1 = o[n][2 * r + 1] * l_run[r];
+      if (BIAS && gelu_out) { a0 = gelu_exact(a0); a1 = gelu_exact(a1); }
+      *reinterpret_cast<uint32_t*>(orow + n * 8) = pack_bf16x2(a0, a1);
+    }
   }
 }
 
@@ -182,11 +203,12 @@ template <>
 bool attention_fast<__nv_bfloat16>(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, int ldk, const __nv_bfloat16* v, int ldv,
                                    __nv_bfloat16* out, int ldo, int B, int nq, int nk, int heads, int dh, int variant,
                                    const float* mix_a, const float* mix_b, const float* ln_g, const float* ln_b, cudaStream_t s,
-                                   float scale) {
-  if (nq == 1 && attention_cls(q, ldq, k, ldk, v, ldv, out, ldo, B, nk, heads, dh, variant, mix_a, mix_b, ln_g, ln_b, s, scale)) return true;
+                                   float scale, const PosBias* pb) {
+  if (nq == 1 && pb == nullptr && attention_cls(q, ldq, k, ldk, v, ldv, out, ldo, B, nk, heads, dh, variant, mix_a, mix_b, ln_g, ln_b, s, scale)) return true;
   // DeepViT re-attention / CaiT talking heads: the materialised-scores path (attn_generic_mma.cu) -- a fused form with all heads'
   // scores of a 16-row tile in shared memory measured 9-11 % slower on the H100 (one CTA per SM at 16 heads)
-  if (variant != 0 || dh != DH || nq < 2) return false;
+  if (variant != 0 || dh != DH || (nq < 2 && pb == nullptr)) return false;
+  if (pb != nullptr && (pb->fmap * pb->fmap > FLASH_BIAS_MAX || nk != pb->fmap * pb->fmap || nq != pb->q_side() * pb->q_side())) return false;
   if ((ldq % 8) || (ldk % 8) || (ldv % 8) || (ldo % 2)) return false;
   if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
        reinterpret_cast<uintptr_t>(out)) % 16) return false;
@@ -197,12 +219,23 @@ bool attention_fast<__nv_bfloat16>(const __nv_bfloat16* q, int ldq, const __nv_b
   cfg.gridDim = dim3(static_cast<unsigned>(blocks));
   cfg.blockDim = dim3(128);
   cfg.stream = s;
+  if (pb != nullptr) {
+    static unsigned long long seen[4] = {0, 0, 0, 0};
+    if (first_use_on_this_device(seen))
+      VB_CUDA(cudaFuncSetAttribute(attn_flash_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FLASH_BIAS_MAX * 4));
+    cfg.dynamicSmemBytes = static_cast<size_t>(pb->fmap) * pb->fmap * sizeof(float);
+  }
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2));
+  if (pb != nullptr)
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<true>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2, pb->table,
+                               pb->fmap, pb->step, static_cast<int>(pb->gelu_out)));
+  else
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<false>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
+                               static_cast<const float*>(nullptr), 0, 1, 0));
   count_launch();
   note_attention_path(ATTN_PATH_FLASH);
   return true;

@@ -93,7 +93,7 @@ scores_mma_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
 template <bool SPLIT>
 __global__ void __launch_bounds__(128)
 pv_mma_kernel(const float* __restrict__ P, const __nv_bfloat16* __restrict__ v, int ldv, __nv_bfloat16* __restrict__ out, int ldo,
-              int heads, int nq, int nk, int dh) {
+              int heads, int nq, int nk, int dh, int gelu_out) {
   __shared__ __align__(16) __nv_bfloat16 Ps[64][64 + 8];
   __shared__ __align__(16) __nv_bfloat16 Pl[SPLIT ? 64 : 1][64 + 8];
   __shared__ __align__(16) __nv_bfloat16 Vt[MAXDH][64 + 8];        // transposed: Vt[d][j]
@@ -156,7 +156,8 @@ pv_mma_kernel(const float* __restrict__ P, const __nv_bfloat16* __restrict__ v, 
       for (int half = 0; half < 2; ++half) {
         const int r = i0 + ar + half * 8;
         if (r < nq) {
-          __nv_bfloat162 o = __floats2bfloat162_rn(acc[n][2 * half], acc[n][2 * half + 1]);
+          const float o0 = acc[n][2 * half], o1 = acc[n][2 * half + 1];
+          __nv_bfloat162 o = gelu_out ? __floats2bfloat162_rn(gelu_exact(o0), gelu_exact(o1)) : __floats2bfloat162_rn(o0, o1);
           *reinterpret_cast<__nv_bfloat162*>(out + (static_cast<size_t>(b) * nq + r) * ldo + h * dh + n * 8 + ac) = o;
         }
       }
@@ -171,7 +172,8 @@ constexpr int MIX_MAX_HEADS = 32;
 //   variant 0: softmax
 __global__ void __launch_bounds__(256)
 mid_fused_kernel(float* __restrict__ S, const float* __restrict__ mix_a, const float* __restrict__ mix_b, const float* __restrict__ gamma,
-                 const float* __restrict__ beta, int heads, int nq, int nk, int variant) {
+                 const float* __restrict__ beta, int heads, int nq, int nk, int variant, const float* __restrict__ pos_tab, int fmap,
+                 int step) {
   extern __shared__ float buf[];                    // [heads][nk] then 2 x [heads*heads] mix matrices
   float* Wa = buf + heads * nk;
   float* Wb = Wa + heads * heads;
@@ -183,8 +185,10 @@ mid_fused_kernel(float* __restrict__ S, const float* __restrict__ mix_a, const f
     Wa[e] = mix_a ? mix_a[e] : 0.f;
     Wb[e] = mix_b ? mix_b[e] : 0.f;
   }
+  const int nqs = (fmap + step - 1) / step;
   for (int h = 0; h < heads; ++h)
-    for (int j = threadIdx.x; j < nk; j += blockDim.x) buf[h * nk + j] = base[h * plane + j];
+    for (int j = threadIdx.x; j < nk; j += blockDim.x)                 // + LeViT's relative-position bias (levit.py:131)
+      buf[h * nk + j] = base[h * plane + j] + (pos_tab != nullptr ? pos_tab[h * fmap * fmap + pos_bias_index(i, j, fmap, step, nqs)] : 0.f);
   __syncthreads();
   auto mix = [&](const float* W, bool ln) {
     for (int j = threadIdx.x; j < nk; j += blockDim.x) {
@@ -648,25 +652,29 @@ bool attention_mix_params(const float* mix_a, const float* mix_b, const float* l
 
 bool attention_generic_mma(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, int ldk, const __nv_bfloat16* v, int ldv,
                            __nv_bfloat16* out, int ldo, float* S, int B, int nq, int nk, int heads, int dh, int variant,
-                           const float* mix_a, const float* mix_b, const float* ln_gamma, const float* ln_beta, cudaStream_t s) {
+                           const float* mix_a, const float* mix_b, const float* ln_gamma, const float* ln_beta, cudaStream_t s,
+                           float scale, const PosBias* pb) {
   if (dh % 16 != 0 || dh > MAXDH || heads > MIX_MAX_HEADS) return false;
   if ((ldq % 8) || (ldk % 8) || (ldv % 8) || (ldo % 2)) return false;
   if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k)) % 16) return false;
-  if (attention_rows_path(q, ldq, k, ldk, v, ldv, out, ldo, S, B, nq, nk, heads, dh, variant, mix_a, mix_b, ln_gamma, ln_beta, s)) return true;
+  if (pb != nullptr && variant != 0) return false;
+  if (pb == nullptr && attention_rows_path(q, ldq, k, ldk, v, ldv, out, ldo, S, B, nq, nk, heads, dh, variant, mix_a, mix_b, ln_gamma, ln_beta, s)) return true;
   const size_t smem = (static_cast<size_t>(heads) * nk + 2 * heads * heads) * sizeof(float);
   if (smem > 200 * 1024) return false;
   static unsigned long long seen[4] = {0, 0, 0, 0};
   if (first_use_on_this_device(seen)) VB_CUDA(cudaFuncSetAttribute(mid_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  const float scale = 1.0f / sqrtf(static_cast<float>(dh));
+  if (scale <= 0.f) scale = 1.0f / sqrtf(static_cast<float>(dh));
   const long long items = static_cast<long long>(B) * heads;
   scores_mma_kernel<<<flat_blocks(static_cast<long long>((nk + 63) / 64) * ((nq + 63) / 64), items), 128, 0, s>>>(q, ldq, k, ldk, S, heads,
                                                                                                                   nq, nk, dh, scale, nk);
   VB_CUDA(cudaGetLastError());
-  mid_fused_kernel<<<flat_blocks(nq, B), 256, smem, s>>>(S, mix_a, mix_b, ln_gamma, ln_beta, heads, nq, nk, variant);
+  mid_fused_kernel<<<flat_blocks(nq, B), 256, smem, s>>>(S, mix_a, mix_b, ln_gamma, ln_beta, heads, nq, nk, variant,
+                                                         pb ? pb->table : nullptr, pb ? pb->fmap : 1, pb ? pb->step : 1);
   VB_CUDA(cudaGetLastError());
   const unsigned pv_grid = flat_blocks((nq + 63) / 64, items);
-  if (variant == 1) pv_mma_kernel<true><<<pv_grid, 128, 0, s>>>(S, v, ldv, out, ldo, heads, nq, nk, dh);
-  else pv_mma_kernel<false><<<pv_grid, 128, 0, s>>>(S, v, ldv, out, ldo, heads, nq, nk, dh);
+  const int gelu_out = pb != nullptr && pb->gelu_out;
+  if (variant == 1) pv_mma_kernel<true><<<pv_grid, 128, 0, s>>>(S, v, ldv, out, ldo, heads, nq, nk, dh, gelu_out);
+  else pv_mma_kernel<false><<<pv_grid, 128, 0, s>>>(S, v, ldv, out, ldo, heads, nq, nk, dh, gelu_out);
   VB_CUDA(cudaGetLastError());
   count_launch(3);
   note_attention_path(ATTN_PATH_MID_FUSED);

@@ -58,13 +58,34 @@ inline unsigned flat_blocks(long long tiles, long long items, const char* what =
   return static_cast<unsigned>(n);
 }
 
+// LeViT attention (levit.py:100-117,94): an additive relative-position bias on the scores and GELU on the output rows.
+//   score(b, h, i, j) += table[h * fmap^2 + |qr - kr| * fmap + |qc - kc|]
+// with key j at grid position (kr, kc) = (j / fmap, j % fmap) and query i at (qr, qc) = step * (i / nqs, i % nqs), nqs =
+// ceil(fmap / step): the queries of a stride-2 "shrink" attention sit on the even pixels of the key grid.  `table` is fp32
+// [heads][fmap^2] in the units of the scaled scores (the reference adds pos_bias / scale, levit.py:117).  nk == fmap^2, nq == nqs^2.
+struct PosBias {
+  const float* table = nullptr;
+  int fmap = 0, step = 1;
+  bool gelu_out = false;                  // levit.py:94: to_out starts with an exact-erf GELU of the attention output
+  __host__ __device__ int q_side() const { return (fmap + step - 1) / step; }
+};
+__device__ __forceinline__ int pos_bias_index(int i, int j, int fmap, int step, int nqs) {
+  const int qr = (i / nqs) * step, qc = (i % nqs) * step, kr = j / fmap, kc = j - kr * fmap;
+  return abs(qr - kr) * fmap + abs(qc - kc);
+}
+__device__ __forceinline__ float gelu_exact(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
+
 // 2-D bf16 (or fp32) tensor map (innermost dimension first), 128-byte swizzle unless swizzle128 == false.
 CUtensorMap make_tmap_2d(const void* base, uint64_t inner, uint64_t outer, uint64_t outer_stride_bytes,
                          uint32_t box_inner, uint32_t box_outer, bool swizzle128 = true, bool f32 = false);
 
+// Activation of a GEMM epilogue: exact-erf GELU (vit.py:34) or hard-swish x * relu6(x + 3) / 6 (levit.py:36-38).  ACT_GELU is 1,
+// so the `gelu` flags (bool / int 0-1) of the older entry points convert to it unchanged.
+enum Act { ACT_NONE = 0, ACT_GELU = 1, ACT_HSWISH = 2 };
+
 // ------------------------------------------------------------------------------------------ wgmma GEMM
 // out[M,N] = epilogue(A[M,K] * Wt[N,K]^T): bf16 operands (K-major), fp32 accumulation in registers.
-// epilogue: (+bias[n]) -> (exact-erf GELU) -> (*scale[n]) -> (+res[m,n]); out bf16.
+// epilogue: (+bias[n]) -> (activation) -> (*scale[n]) -> (+res[m,n]); out bf16.
 struct GemmBf16 {
   CUtensorMap tmap_a, tmap_b;           // A, B (weights)
   int M = 0, N = 0, K = 0;
@@ -75,7 +96,7 @@ struct GemmBf16 {
   const float* scale = nullptr;         // [N] or null (LayerScale)
   const __nv_bfloat16* res = nullptr;   // [M, ldr] or null (may alias out)
   int ldr = 0;
-  bool gelu = false;
+  int act = ACT_NONE;                   // Act
   // Folded LayerNorm of the A operand (Wt must hold gamma-scaled weights, bias the beta.W + b term):
   //   out = rstd[m] * (acc - mu[m] * ln_c1[n]) + bias[n], with (mu, rstd) of row m reduced in the epilogue from the
   //   ln_parts (sum, sumsq) partials of that row (the stats_out format below) over 1 / ln_inv_d elements.
@@ -89,7 +110,7 @@ struct GemmBf16 {
 // lda/ldw/ldc/ldr in elements; all must be multiples of 8 (16-byte TMA strides); N % 64 == 0.
 GemmBf16 gemm_bf16_plan(const __nv_bfloat16* A, int lda, const __nv_bfloat16* Wt, int ldw, __nv_bfloat16* out, int ldc,
                         int M, int N, int K, const float* bias, const float* scale, const __nv_bfloat16* res, int ldr,
-                        bool gelu, bool out_f32 = false, int b_rows = 0);
+                        int act, bool out_f32 = false, int b_rows = 0);
 void gemm_bf16_run(const GemmBf16& g, cudaStream_t stream);
 bool gemm_bf16_supported(int M, int N, int K, int lda, int ldw, int ldc);
 

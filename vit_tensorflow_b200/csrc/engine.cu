@@ -105,6 +105,8 @@ struct Epi {
   const void* res = nullptr;
   int ldr = 0;
   bool gelu = false;
+  bool hswish = false;               // hard-swish instead (LeViT MLP, levit.py:37)
+  int act() const { return gelu ? ACT_GELU : hswish ? ACT_HSWISH : ACT_NONE; }
   const float* ln_stats = nullptr;   // (sum, sumsq) partials per 64-column chunk of the A operand's rows for a LayerNorm-folded Dense, [M, K/64, 2]
   float* stats_out = nullptr;        // emit (sum, sumsq) partials of every 64-column chunk of the output rows, [M, N/64, 2]
 };
@@ -122,6 +124,19 @@ struct LayerW {                    // one pre-norm transformer layer in any of t
   int dh_model = 0;                  // the model's dim_head: softmax scale dh_model^-0.5 (vit.py:57)
   int t2t_D = 0, t2t_Dp = 0;         // tensor-core T2T soft-split layer: true width D (LayerNorm, softmax scale), padded width Dp
   bool folded = false;               // attn_norm / ff_norm folded into to_qkv (to_q, to_kv) / fc1
+};
+
+// One LeViT Transformer layer (levit.py:141-162): attention (queries on every step-th pixel of the fmap x fmap map) + MLP.
+// The BatchNormalizations are folded into the convolutions; q, k and v heads are zero-padded to the activation head width dh.
+struct LevitBlockW {
+  int dim = 0, dim_out = 0, heads = 0, fmap = 0, step = 1, dh = 0;
+  int dp = 0, dp_out = 0;            // row pitches of the input / output token rows: dim / dim_out (bf16: padded, zero columns)
+  bool residual = false;             // attn_residual (levit.py:146): not downsampling and dim == dim_out
+  Linear qkv;                        // [q | k | v] (step 1) or [k | v] (step 2), each heads * dh wide
+  Linear q;                          // step 2: the queries of the even pixels
+  Linear to_out, fc1, fc2;
+  const float* pos = nullptr;        // [heads][fmap^2] relative-position bias / scale
+  float scale = 0.f;                 // dim_key^-0.5
 };
 
 struct EmbedW { Linear patch; const float* pos = nullptr; const float* cls = nullptr; int dim = 0, n_pos = 0; };
@@ -283,6 +298,38 @@ struct vb_handle {
     }
   }
   int cct_sequence_length() const { int h = cfg.image_h, w = cfg.image_w; cct_grid(&h, &w); return h * w; }   // cct.py:331-333
+  // LeViT (levit.py:164-226): the stem convolutions, the blocks of every Transformer in backbone order, the heads
+  vb_levit_config lv{};
+  std::vector<Linear> lv_stem;
+  std::vector<LevitBlockW> lv_blocks;
+  Linear lv_distill;
+  struct LevitPlan { std::string pre; int dim, dim_out, heads, fmap, mult; bool down; };
+  // levit.py:194-204: stage s = depths[s] blocks on the fmap map; between stages one shrink block (2 * heads, mlp_mult 2, the
+  // queries on the even pixels) after which fmap = ceil(fmap / 2).  pre: the attribute path of the block's [attn, mlp] pair.
+  std::vector<LevitPlan> levit_plan() const {
+    std::vector<LevitPlan> v;
+    int fmap = cfg.image_h / 16, t = 0;
+    for (int st = 0; st < lv.stages; ++st, ++t) {
+      for (int L = 0; L < lv.depths[st]; ++L)
+        v.push_back({"backbone." + std::to_string(t) + ".layers." + std::to_string(L) + ".", lv.dims[st], lv.dims[st], lv.heads[st], fmap,
+                     lv.mlp_mult, false});
+      if (st + 1 < lv.stages) {
+        ++t;
+        v.push_back({"backbone." + std::to_string(t) + ".layers.0.", lv.dims[st], lv.dims[st + 1], 2 * lv.heads[st], fmap, 2, true});
+        fmap = (fmap + 1) / 2;
+      }
+    }
+    return v;
+  }
+  int levit_stem_cout(int i) const { return i == 0 ? 32 : i == 1 ? 64 : i == 2 ? 128 : lv.dims[0]; }   // levit.py:187-192
+  // activation head width of q, k and v: the bf16 engine pads to the flash kernel's 64 (wider heads: a multiple of 64)
+  int levit_dh() const {
+    const int m = lv.dim_key > lv.dim_value ? lv.dim_key : lv.dim_value;
+    return bf16() ? round_up(m, 64) : m;
+  }
+  // Width the bf16 engine carries a channel dimension at: a multiple of 64, so that every GEMM of a block (N = a channel width)
+  // runs on the wgmma kernel.  Pad columns are zero and stay zero: zero weights and biases, and hard-swish(0) = GELU(0) = 0.
+  int levit_width(int d) const { return bf16() ? round_up(d, 64) : d; }
   struct XBlock { std::vector<LayerW> sm_layers, lg_layers; Norm sm_final, lg_final; std::vector<CrossW> sm_attend_lg, lg_attend_sm; };
   std::vector<XBlock> xblocks;
   Norm head_norm, sm_head_norm, lg_head_norm;
@@ -409,6 +456,34 @@ struct vb_handle {
       expect_ln("norm", c.dim);                                           // cct.py:266
       expect_dense("attention_pool", c.dim, 1);                           // :248
       expect_dense("head", c.dim, c.num_classes);                         // fc :267
+    } else if (c.kind == VB_KIND_LEVIT) {
+      auto expect_bn = [&](const std::string& n, int d) {
+        for (const char* leaf : {"gamma", "beta", "moving_mean", "moving_variance"}) expect(n + "." + leaf, {d});
+      };
+      for (int i = 0; i < 4; ++i) {
+        expect("conv_embedding." + std::to_string(i) + ".kernel", {3, 3, i == 0 ? C : levit_stem_cout(i - 1), levit_stem_cout(i)});
+        expect("conv_embedding." + std::to_string(i) + ".bias", {levit_stem_cout(i)});
+      }
+      for (const auto& b : levit_plan()) {
+        const std::string a = b.pre + "0.";                              // Attention levit.py:64-117
+        const int hk = b.heads * lv.dim_key, hv = b.heads * lv.dim_value, hidden = b.dim_out * b.mult;
+        for (const char* n : {"to_q", "to_k", "to_v"}) {
+          const int w = n[3] == 'v' ? hv : hk;
+          expect(a + n + ".0.kernel", {1, 1, b.dim, w});
+          expect_bn(a + n + ".1", w);
+        }
+        expect(a + "pos_bias.embeddings", {b.fmap * b.fmap, b.heads});
+        expect(a + "to_out.1.kernel", {1, 1, hv, b.dim_out});
+        expect(a + "to_out.1.bias", {b.dim_out});
+        expect_bn(a + "to_out.2", b.dim_out);
+        expect(b.pre + "1.net.0.kernel", {1, 1, b.dim_out, hidden});      // MLP levit.py:48-62
+        expect(b.pre + "1.net.0.bias", {hidden});
+        expect(b.pre + "1.net.3.kernel", {1, 1, hidden, b.dim_out});
+        expect(b.pre + "1.net.3.bias", {b.dim_out});
+      }
+      const int dl = lv.dims[lv.stages - 1];
+      expect_dense("mlp_head", dl, c.num_classes);
+      if (lv.num_distill_classes > 0) expect_dense("distill_head", dl, lv.num_distill_classes);
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       expect("pos_embedding", {1, np, c.dim});
@@ -633,6 +708,7 @@ struct vb_handle {
     for (auto& w : weights) VB_CHECK(w.set, "vb_finalize: weight '" + w.name + "' was never set");
     VB_CUDA(cudaSetDevice(device));
     owned.clear(); layers.clear(); cls_layers.clear(); t2t_layers.clear(); xblocks.clear(); plans.clear(); embed_res.clear(); cct_convs.clear();
+    lv_stem.clear(); lv_blocks.clear();
     woverride.clear();
     drop_graphs();
     const vb_config& c = cfg;
@@ -681,6 +757,8 @@ struct vb_handle {
       cct_pool_w = W("attention_pool.kernel");
       cct_pool_b = W("attention_pool.bias");
       head = make_linear_f32("head", c.dim, c.num_classes);
+    } else if (c.kind == VB_KIND_LEVIT) {
+      finalize_levit();
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       embed = make_embed("", c.patch_h, c.patch_w, c.dim, np, false);
@@ -723,6 +801,121 @@ struct vb_handle {
     VB_CUDA(cudaDeviceSynchronize());
     finalized = true;
   }
+  // ---- LeViT weight packing: BatchNormalization folded into the convolutions on the host in double, heads zero-padded
+  std::vector<double> host_weight(const std::string& name) const {
+    const Weight& w = weights[windex.at(name)];
+    std::vector<float> f(w.count);
+    VB_CUDA(cudaMemcpy(f.data(), w.dev, w.count * sizeof(float), cudaMemcpyDeviceToHost));
+    return std::vector<double>(f.begin(), f.end());
+  }
+  // y = BN(x W + b) = x (W s) + ((b - mean) s + beta),  s = gamma / sqrt(var + 1e-5)  (levit.py:76, inference statistics)
+  void fold_bn(std::vector<double>& Wkn, std::vector<double>& bias, int K, int N, const std::string& bn) const {
+    const auto g = host_weight(bn + ".gamma"), be = host_weight(bn + ".beta"), mu = host_weight(bn + ".moving_mean"),
+               var = host_weight(bn + ".moving_variance");
+    for (int n = 0; n < N; ++n) {
+      const double sc = g[n] / std::sqrt(var[n] + 1e-5);
+      for (int k = 0; k < K; ++k) Wkn[static_cast<size_t>(k) * N + n] *= sc;
+      bias[n] = (bias[n] - mu[n]) * sc + be[n];
+    }
+  }
+  const float* upload_owned(const std::vector<double>& v) {
+    std::vector<float> f(v.begin(), v.end());
+    owned.emplace_back(new DevMem());
+    owned.back()->ensure(f.size() * sizeof(float));
+    VB_CUDA(cudaMemcpy(owned.back()->p, f.data(), f.size() * sizeof(float), cudaMemcpyHostToDevice));
+    return static_cast<const float*>(owned.back()->p);
+  }
+  // W [K, N] (Keras layout) as the top-left block of a zero [Kp, Np]
+  static std::vector<double> pad_kn(const std::vector<double>& W, int K, int N, int Kp, int Np) {
+    std::vector<double> out(static_cast<size_t>(Kp) * Np, 0.0);
+    for (int k = 0; k < K; ++k)
+      for (int n = 0; n < N; ++n) out[static_cast<size_t>(k) * Np + n] = W[static_cast<size_t>(k) * N + n];
+    return out;
+  }
+  static std::vector<double> pad_n(const std::vector<double>& b, int Np) {
+    std::vector<double> out(b);
+    out.resize(Np, 0.0);
+    return out;
+  }
+  // a Dense [K, N] + bias made on the host, packed like a registered one (under a name of its own in woverride)
+  Linear linear_from_host(const std::string& key, const std::vector<double>& Wkn, const std::vector<double>& bias, int K, int N) {
+    woverride[key + ".kernel"] = upload_owned(Wkn);
+    woverride[key + ".bias"] = upload_owned(bias);
+    return make_linear(key, K, N);
+  }
+  void finalize_levit() {
+    const int dh = levit_dh();
+    int cin = cfg.channels;
+    for (int i = 0; i < 4; ++i) {                                       // stem; the 32-channel map is written 64 wide (zero columns)
+      const std::string n = "conv_embedding." + std::to_string(i);
+      const int cout = levit_stem_cout(i), np = i == 0 ? 64 : levit_width(cout), K = 9 * cin;
+      lv_stem.push_back(linear_from_host("levit." + n, pad_kn(host_weight(n + ".kernel"), K, cout, K, np),
+                                         pad_n(host_weight(n + ".bias"), np), K, np));
+      cin = cout;
+    }
+    for (const auto& p : levit_plan()) {
+      LevitBlockW b;
+      b.dim = p.dim; b.dim_out = p.dim_out; b.heads = p.heads; b.fmap = p.fmap; b.step = p.down ? 2 : 1; b.dh = dh;
+      b.dp = levit_width(p.dim); b.dp_out = levit_width(p.dim_out);
+      b.residual = !p.down && p.dim == p.dim_out;
+      const std::string a = p.pre + "0.", key = "levit." + a;
+      const int H = p.heads, dk = lv.dim_key, dv = lv.dim_value, HD = H * dh, dp = b.dp, dpo = b.dp_out;
+      // one projection folded and head-padded: head h's real columns [h*dh, h*dh + w) of a [dp, H*dh] block (rows >= dim zero)
+      auto proj = [&](const char* n, int w, std::vector<double>& Wcat, std::vector<double>& bcat, int off, int ncat) {
+        auto Wn = host_weight(a + n + ".0.kernel");
+        std::vector<double> bn(H * w, 0.0);
+        fold_bn(Wn, bn, p.dim, H * w, a + n + ".1");
+        for (int h = 0; h < H; ++h)
+          for (int d = 0; d < w; ++d) {
+            const int src = h * w + d, dst = off + h * dh + d;
+            for (int k = 0; k < p.dim; ++k) Wcat[static_cast<size_t>(k) * ncat + dst] = Wn[static_cast<size_t>(k) * H * w + src];
+            bcat[dst] = bn[src];
+          }
+      };
+      const int nkv = p.down ? 2 * HD : 3 * HD, koff = p.down ? 0 : HD;
+      std::vector<double> Wkv(static_cast<size_t>(dp) * nkv, 0.0), bkv(nkv, 0.0);
+      if (!p.down) proj("to_q", dk, Wkv, bkv, 0, nkv);
+      proj("to_k", dk, Wkv, bkv, koff, nkv);
+      proj("to_v", dv, Wkv, bkv, koff + HD, nkv);
+      b.qkv = linear_from_host(key + "qkv", Wkv, bkv, dp, nkv);
+      if (p.down) {
+        std::vector<double> Wq(static_cast<size_t>(dp) * HD, 0.0), bq(HD, 0.0);
+        proj("to_q", dk, Wq, bq, 0, HD);
+        b.q = linear_from_host(key + "q", Wq, bq, dp, HD);
+      }
+      {                                                                 // to_out: GELU -> Conv2D(1x1, bias) -> BN (levit.py:93-98)
+        auto Wo = host_weight(a + "to_out.1.kernel"), bo = host_weight(a + "to_out.1.bias");
+        fold_bn(Wo, bo, H * dv, p.dim_out, a + "to_out.2");
+        std::vector<double> Wp(static_cast<size_t>(HD) * dpo, 0.0);
+        for (int h = 0; h < H; ++h)
+          for (int d = 0; d < dv; ++d)
+            for (int o = 0; o < p.dim_out; ++o)
+              Wp[(static_cast<size_t>(h) * dh + d) * dpo + o] = Wo[(static_cast<size_t>(h) * dv + d) * p.dim_out + o];
+        b.to_out = linear_from_host(key + "to_out", Wp, pad_n(bo, dpo), HD, dpo);
+      }
+      b.scale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(dk)));
+      b.pos = upload_owned(levit_pos_table(host_weight(a + "pos_bias.embeddings"), p.fmap * p.fmap, H, dk));
+      const int hidden = p.dim_out * p.mult, hp = levit_width(hidden);
+      const std::string m0 = p.pre + "1.net.0", m3 = p.pre + "1.net.3";
+      b.fc1 = linear_from_host(key + "fc1", pad_kn(host_weight(m0 + ".kernel"), p.dim_out, hidden, dpo, hp), pad_n(host_weight(m0 + ".bias"), hp),
+                               dpo, hp);
+      b.fc2 = linear_from_host(key + "fc2", pad_kn(host_weight(m3 + ".kernel"), hidden, p.dim_out, hp, dpo), pad_n(host_weight(m3 + ".bias"), dpo),
+                               hp, dpo);
+      lv_blocks.push_back(std::move(b));
+    }
+    const int dl = lv.dims[lv.stages - 1];
+    head = make_linear_f32("mlp_head", dl, cfg.num_classes);
+    if (lv.num_distill_classes > 0) lv_distill = make_linear_f32("distill_head", dl, lv.num_distill_classes);
+  }
+  // [heads][fmap^2] = embeddings[e, h] / scale with scale = dim_key^-0.5 (levit.py:117): the table the attention kernels add
+  static std::vector<double> levit_pos_table(const std::vector<double>& emb, int f2, int heads, int dim_key) {
+    std::vector<double> t(static_cast<size_t>(heads) * f2);
+    const double inv_scale = std::sqrt(static_cast<double>(dim_key));
+    for (int h = 0; h < heads; ++h)
+      for (int e = 0; e < f2; ++e) t[static_cast<size_t>(h) * f2 + e] = emb[static_cast<size_t>(e) * heads + h] * inv_scale;
+    return t;
+  }
+
   Linear make_linear_f32(const std::string& n, int K, int N) {  // classifier head always runs in fp32
     Linear L;
     L.W = W(n + ".kernel"); L.bias = W(n + ".bias"); L.K = K; L.N = N; L.ldw = K;
@@ -1198,6 +1391,8 @@ struct vb_handle {
       copy_tokens<T>(X, rows, 0, ctx, rows + 1, 1, rows, B, c.dim, s);
       for (const auto& l : cls_layers) layer_cls<T>(Cx, ctx, B, rows + 1, c.dim, l, s);
       classify<T>(Cx, 1, c.dim, head_norm, head, B, 0, logits, false, s);
+    } else if (c.kind == VB_KIND_LEVIT) {
+      levit_forward<T>(img, B, H, Wd, logits, nullptr, s);
     } else if (c.kind == VB_KIND_CCT) {                   // CCT.call cct.py:342-345, TransformerClassifier.call :277-305
       int rows = 0;
       T* X = tokenize_cct<T>(img, B, H, Wd, &rows, s);
@@ -1253,6 +1448,102 @@ struct vb_handle {
     }
   }
 
+  // LeViT.call (levit.py:214-226): stem -> backbone -> GlobalAvgPool2D -> mlp_head (and distill_head when distill != null).
+  // The token rows of every block are the NHWC map, pixel-major: row b * fmap^2 + r * fmap + c.
+  static constexpr const char* kLevitNoStages = "LeViT runs as a whole forward only: its stem / backbone / head stages have no entry of their own";
+  template <typename T>
+  void levit_forward(const float* img, int B, int H, int Wd, float* logits, float* distill, cudaStream_t s) {
+    const int fmap = cfg.image_h / 16;
+    int mh = H, mw = Wd, mc = cfg.channels, ld_in = 0;
+    for (int i = 0; i < 4; ++i) { mh = (mh + 1) / 2; mw = (mw + 1) / 2; }
+    VB_CHECK(mh == fmap && mw == fmap, "LeViT: an " + std::to_string(H) + " x " + std::to_string(Wd) + " image gives a " + std::to_string(mh) +
+                                       " x " + std::to_string(mw) + " feature map after the four stride-2 stem convolutions, but the "
+                                       "position biases are built for " + std::to_string(fmap) + " x " + std::to_string(fmap) +
+                                       " (image_size // 16, levit.py:194)");
+    mh = H; mw = Wd;
+    const T* map = nullptr;
+    T* X = nullptr;
+    for (int i = 0; i < 4; ++i) {                                       // conv_embedding levit.py:187-192
+      const Linear& conv = lv_stem[i];
+      const int oh = (mh + 1) / 2, ow = (mw + 1) / 2, M = B * oh * ow, Kp = bf16() ? conv.ldw : conv.K;
+      T* col = arena.get<T>(static_cast<size_t>(M) * Kp);
+      {
+        ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(i == 0 ? 4 : sizeof(T)) * B * mh * mw * mc + static_cast<double>(sizeof(T)) * M * Kp, s);
+        if (i == 0) unfold_same<float, T>(img, col, B, mh, mw, mc, 3, 2, 0, Kp, s);
+        else unfold_same<T, T>(map, col, B, mh, mw, mc, 3, 2, 0, Kp, s, ld_in);
+      }
+      X = arena.get<T>(static_cast<size_t>(M) * conv.N);
+      Linear L = conv;
+      L.K = Kp;
+      Epi e; e.bias = conv.bias;
+      linear<T>(col, Kp, M, L, X, conv.N, e, s);
+      map = X; mh = oh; mw = ow; mc = levit_stem_cout(i); ld_in = conv.N;
+    }
+    int f = fmap;
+    for (const auto& b : lv_blocks) {
+      X = levit_block<T>(X, B, b, s);
+      f = (b.fmap + b.step - 1) / b.step;
+    }
+    const int dl = lv.dims[lv.stages - 1], ldl = levit_width(dl);
+    float* z = arena.get<float>(static_cast<size_t>(B) * dl);
+    {
+      ProfScope ps(this, PROF_LN, 1.0 * B * f * f * dl, static_cast<double>(sizeof(T)) * B * f * f * dl, s);
+      pool_layernorm<T>(X, f * f, ldl, nullptr, nullptr, z, B, dl, 1, s);  // GlobalAvgPool2D (levit.py:206-208)
+    }
+    gemm_simt<float, float, float>(z, dl, head.W, head.N, 1, logits, head.N, B, head.N, dl, head.bias, nullptr, nullptr, head.N, 0, s);
+    if (distill != nullptr)
+      gemm_simt<float, float, float>(z, dl, lv_distill.W, lv_distill.N, 1, distill, lv_distill.N, B, lv_distill.N, dl, lv_distill.bias,
+                                     nullptr, nullptr, lv_distill.N, 0, s);
+  }
+  // One LeViT block (levit.py:156-162): x = attn(x) + (x if attn_residual else 0); x = mlp(x) + x.  X [B * fmap^2, dp] ->
+  // [B * nq, dp_out] (a new buffer when the block shrinks the map, X updated in place otherwise); pad columns stay zero.
+  template <typename T>
+  T* levit_block(T* X, int B, const LevitBlockW& b, cudaStream_t s) {
+    const int f2 = b.fmap * b.fmap, nqs = (b.fmap + b.step - 1) / b.step, nq = nqs * nqs, HD = b.heads * b.dh;
+    const int Mk = B * f2, Mq = B * nq;
+    T* O = arena.get<T>(static_cast<size_t>(Mq) * HD);
+    PosBias pb;
+    pb.table = b.pos; pb.fmap = b.fmap; pb.step = b.step; pb.gelu_out = true;
+    if (b.step == 1) {
+      T* QKV = arena.get<T>(static_cast<size_t>(Mk) * 3 * HD);
+      Epi e; e.bias = b.qkv.bias;
+      linear<T>(X, b.dp, Mk, b.qkv, QKV, 3 * HD, e, s);
+      attention_bias<T>(QKV, 3 * HD, QKV + HD, 3 * HD, QKV + 2 * HD, 3 * HD, O, HD, B, nq, f2, b, pb, s);
+    } else {                                                            // queries of the even pixels (1x1 conv, stride 2, VALID)
+      T* Xq = arena.get<T>(static_cast<size_t>(Mq) * b.dp);
+      {
+        ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * Mq * b.dp, s);
+        gather_grid<T>(X, b.dp, Xq, b.dp, B, b.fmap, b.fmap, b.dp, b.step, s);
+      }
+      T* Q = arena.get<T>(static_cast<size_t>(Mq) * HD);
+      T* KV = arena.get<T>(static_cast<size_t>(Mk) * 2 * HD);
+      Epi eq; eq.bias = b.q.bias;
+      linear<T>(Xq, b.dp, Mq, b.q, Q, HD, eq, s);
+      Epi ek; ek.bias = b.qkv.bias;
+      linear<T>(X, b.dp, Mk, b.qkv, KV, 2 * HD, ek, s);
+      attention_bias<T>(Q, HD, KV, 2 * HD, KV + HD, 2 * HD, O, HD, B, nq, f2, b, pb, s);
+    }
+    T* Y = b.residual ? X : arena.get<T>(static_cast<size_t>(Mq) * b.dp_out);
+    Epi eo; eo.bias = b.to_out.bias;
+    if (b.residual) { eo.res = X; eo.ldr = b.dp; }
+    linear<T>(O, HD, Mq, b.to_out, Y, b.dp_out, eo, s);
+    T* Hb = arena.get<T>(static_cast<size_t>(Mq) * b.fc1.N);
+    Epi e1; e1.hswish = true; e1.bias = b.fc1.bias;
+    linear<T>(Y, b.dp_out, Mq, b.fc1, Hb, b.fc1.N, e1, s);
+    Epi e2; e2.bias = b.fc2.bias; e2.res = Y; e2.ldr = b.dp_out;
+    linear<T>(Hb, b.fc1.N, Mq, b.fc2, Y, b.dp_out, e2, s);
+    return Y;
+  }
+  template <typename T>
+  void attention_bias(const T* q, int ldq, const T* k, int ldk, const T* v, int ldv, T* out, int ldo, int B, int nq, int nk,
+                      const LevitBlockW& b, const PosBias& pb, cudaStream_t s) {
+    ProfScope ps(this, PROF_ATTN, 4.0 * B * b.heads * nq * nk * b.dh, static_cast<double>(sizeof(T)) * B * b.heads * b.dh * (2.0 * nq + 2.0 * nk), s);
+    if (attention_fast<T>(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, b.heads, b.dh, 0, nullptr, nullptr, nullptr, nullptr, s, b.scale, &pb))
+      return;
+    float* S = arena.get<float>(static_cast<size_t>(B) * b.heads * nq * ((nk + 15) & ~15));
+    attention_generic<T>(q, ldq, k, ldk, v, ldv, out, ldo, S, B, nq, nk, b.heads, b.dh, 0, nullptr, nullptr, nullptr, nullptr, s, b.scale, &pb);
+  }
+
   // DistillMixin.call (distill.py:16-45) on top of a ViT: embed -> append the distillation token as the LAST row ->
   // transformer over n + 2 rows -> head on the first n + 1 rows, and the last row returned as is.
   template <typename T>
@@ -1306,6 +1597,7 @@ struct vb_handle {
   int embed_rows(int H, int Wd) const {
     VB_CHECK(cfg.kind != VB_KIND_CROSSVIT, "CrossViT has two token streams: no single embedding stage");
     VB_CHECK(cfg.kind != VB_KIND_CCT, kCctNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_LEVIT, kLevitNoStages);
     if (cfg.kind == VB_KIND_T2T_VIT) {
       int h = H, w = Wd;
       for (const auto& st : t2t_stages()) { h = (h + st.stride - 1) / st.stride; w = (w + st.stride - 1) / st.stride; }
@@ -1331,6 +1623,7 @@ struct vb_handle {
   void head_impl(const float* tok, int B, int n, float* logits, cudaStream_t s) {
     VB_CHECK(cfg.kind != VB_KIND_CROSSVIT, "CrossViT sums two heads: no single mlp_head stage");
     VB_CHECK(cfg.kind != VB_KIND_CCT, kCctNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_LEVIT, kLevitNoStages);
     arena.reset();
     const long long count = static_cast<long long>(B) * n * cfg.dim;
     T* X = arena.get<T>(count);
@@ -1342,6 +1635,7 @@ struct vb_handle {
   void patch_to_emb_impl(const float* patches, int rows, float* out, cudaStream_t s) {
     VB_CHECK(cfg.kind != VB_KIND_CROSSVIT, "CrossViT has two patch embeddings");
     VB_CHECK(cfg.kind != VB_KIND_CCT, kCctNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_LEVIT, kLevitNoStages);
     arena.reset();
     const int K = embed.patch.K, Kp = bf16() ? embed.patch.ldw : K;
     T* col = arena.get<T>(static_cast<size_t>(rows) * Kp);
@@ -1359,7 +1653,7 @@ struct vb_handle {
 template <>
 void vb_handle::linear<float>(const float* A, int lda, int M, const Linear& L, float* out, int ldc, const Epi& e, cudaStream_t s) {
   gemm_simt<float, float, float>(A, lda, L.W, L.N, 1, out, ldc, M, L.N, L.K, e.bias, e.scale,
-                                 static_cast<const float*>(e.res), e.ldr, e.gelu ? 1 : 0, s);
+                                 static_cast<const float*>(e.res), e.ldr, e.act(), s);
 }
 template <>
 void vb_handle::linear<__nv_bfloat16>(const __nv_bfloat16* A, int lda, int M, const Linear& L, __nv_bfloat16* out, int ldc,
@@ -1370,7 +1664,7 @@ void vb_handle::linear<__nv_bfloat16>(const __nv_bfloat16* A, int lda, int M, co
   const bool folded = L.ln_c1 != nullptr;
   VB_CHECK(!folded || (fast && e.ln_stats != nullptr && K % 64 == 0), "internal: LayerNorm-folded Dense needs the wgmma path and row statistics");
   VB_CHECK(e.stats_out == nullptr || fast, "internal: row statistics requested from a non-wgmma GEMM");
-  ProfScope ps(this, !fast ? PROF_OTHER : e.gelu ? PROF_GEMM_GELU : res ? PROF_GEMM_RES : PROF_GEMM, 2.0 * M * L.N * K,
+  ProfScope ps(this, !fast ? PROF_OTHER : e.act() != ACT_NONE ? PROF_GEMM_GELU : res ? PROF_GEMM_RES : PROF_GEMM, 2.0 * M * L.N * K,
                2.0 * (static_cast<double>(M) * K + static_cast<double>(L.N) * K + static_cast<double>(M) * L.N * (res ? 2 : 1)), s);
   if (fast) {
     PlanKey key{};
@@ -1378,14 +1672,14 @@ void vb_handle::linear<__nv_bfloat16>(const __nv_bfloat16* A, int lda, int M, co
                                  reinterpret_cast<uintptr_t>(out), static_cast<uintptr_t>(ldc), static_cast<uintptr_t>(M),
                                  static_cast<uintptr_t>(L.N), static_cast<uintptr_t>(K), reinterpret_cast<uintptr_t>(e.bias),
                                  reinterpret_cast<uintptr_t>(e.scale), reinterpret_cast<uintptr_t>(res),
-                                 static_cast<uintptr_t>(e.ldr), static_cast<uintptr_t>(e.gelu),
+                                 static_cast<uintptr_t>(e.ldr), static_cast<uintptr_t>(e.act()),
                                  reinterpret_cast<uintptr_t>(e.ln_stats), reinterpret_cast<uintptr_t>(L.ln_c1),
                                  reinterpret_cast<uintptr_t>(e.stats_out)};
     for (int i = 0; i < 16; ++i) key[i] = parts[i];
     auto it = plans.find(key);
     if (it == plans.end()) {
       if (plans.size() > 8192) plans.clear();      // shape sweeps: bounded host memory (a plan is four 128-byte tensor maps)
-      GemmBf16 g = gemm_bf16_plan(A, lda, L.Wt, L.ldw, out, ldc, M, L.N, K, e.bias, e.scale, res, e.ldr, e.gelu);
+      GemmBf16 g = gemm_bf16_plan(A, lda, L.Wt, L.ldw, out, ldc, M, L.N, K, e.bias, e.scale, res, e.ldr, e.act());
       if (folded) { g.ln_c1 = L.ln_c1; g.ln_stats = e.ln_stats; g.ln_parts = K / 64; g.ln_inv_d = 1.0f / static_cast<float>(K); }
       if (e.stats_out) { g.stats_out = e.stats_out; }
       it = plans.emplace(key, g).first;
@@ -1393,7 +1687,7 @@ void vb_handle::linear<__nv_bfloat16>(const __nv_bfloat16* A, int lda, int M, co
     gemm_bf16_run(it->second, s);
   } else {
     gemm_simt<__nv_bfloat16, __nv_bfloat16, __nv_bfloat16>(A, lda, L.Wt, 1, L.ldw, out, ldc, M, L.N, K, e.bias, e.scale, res,
-                                                           e.ldr, e.gelu ? 1 : 0, s);
+                                                           e.ldr, e.act(), s);
   }
 }
 
@@ -1511,6 +1805,7 @@ int guarded(vb_handle* h, F&& f) {
 void validate(const vb_config& c) {
   VB_CHECK(c.struct_size == static_cast<int32_t>(sizeof(vb_config)) || c.struct_size == VB_CONFIG_SIZE_ABI7,
            "vb_config.struct_size mismatch (ABI)");
+  VB_CHECK(c.kind != VB_KIND_LEVIT, "LeViT: create the handle with vb_create_levit (its stages are a vb_levit_config)");
   VB_CHECK(c.kind >= VB_KIND_VIT && c.kind <= VB_KIND_CCT, "unknown model kind");
   if (c.kind == VB_KIND_CCT) {
     VB_CHECK(c.channels == 3 && c.num_classes > 0 && c.image_h > 0 && c.image_w > 0, "bad image / class configuration");
@@ -1552,6 +1847,21 @@ void validate(const vb_config& c) {
     VB_CHECK(c.heads <= 32, "at most 32 heads");
     VB_CHECK(c.pool == VB_POOL_CLS || c.pool == VB_POOL_MEAN, "pool type must be either cls (cls token) or mean (mean pooling)");
   }
+}
+
+void validate_levit(const vb_config& c, const vb_levit_config& lv) {
+  VB_CHECK(c.precision == VB_PRECISION_FP32 || c.precision == VB_PRECISION_BF16, "unknown precision");
+  VB_CHECK(c.channels > 0 && c.num_classes > 0 && c.image_h > 0 && c.image_h == c.image_w, "LeViT: bad image / class configuration");
+  VB_CHECK(lv.stages >= 1 && lv.stages <= VB_LEVIT_MAX_STAGES, "LeViT: stages must be in [1, 8]");
+  VB_CHECK(lv.dim_key > 0 && lv.dim_value > 0 && lv.mlp_mult > 0 && lv.num_distill_classes >= 0, "LeViT: bad dim_key / dim_value / mlp_mult");
+  for (int s = 0; s < lv.stages; ++s)
+    VB_CHECK(lv.dims[s] > 0 && lv.depths[s] >= 0 && lv.heads[s] > 0, "LeViT: bad stage dimensions");
+  // levit.py:194 vs the stem: image_size // 16 must be the size four ceil-halvings give, or the bias cannot broadcast
+  int f = c.image_h;
+  for (int i = 0; i < 4; ++i) f = (f + 1) / 2;
+  VB_CHECK(c.image_h >= 16 && f == c.image_h / 16,
+           "LeViT: image_size " + std::to_string(c.image_h) + " gives a " + std::to_string(f) + " x " + std::to_string(f) +
+           " map after the stem but position biases for image_size // 16 = " + std::to_string(c.image_h / 16));
 }
 
 }  // namespace
@@ -1668,6 +1978,35 @@ int vb_create(const vb_config* cfg, int device, vb_handle** out) {
     VB_CHECK(prop.major == 9 && prop.minor == 0, "vb_create: libvitb200 is built for sm_90a (Hopper H100) only");
     std::unique_ptr<vb_handle> h(new vb_handle());
     h->cfg = c;
+    h->device = device;
+    h->build_expected();
+    *out = h.release();
+  });
+}
+
+int vb_create_levit(const vb_config* base, const vb_levit_config* lv, int device, vb_handle** out) {
+  return guarded(nullptr, [&] {
+    VB_CHECK(base != nullptr && lv != nullptr && out != nullptr, "vb_create_levit: null argument");
+    VB_CHECK(base->struct_size == static_cast<int32_t>(sizeof(vb_config)) || base->struct_size == VB_CONFIG_SIZE_ABI7,
+             "vb_config.struct_size mismatch (ABI)");
+    VB_CHECK(lv->struct_size == static_cast<int32_t>(sizeof(vb_levit_config)), "vb_levit_config.struct_size mismatch (ABI)");
+    vb_config c;
+    memset(&c, 0, sizeof c);
+    memcpy(&c, base, static_cast<size_t>(base->struct_size));
+    VB_CHECK(c.kind == VB_KIND_LEVIT, "vb_create_levit: base.kind must be VB_KIND_LEVIT");
+    validate_levit(c, *lv);
+    int ndev = 0;
+    cudaError_t e = cudaGetDeviceCount(&ndev);
+    VB_CHECK(e == cudaSuccess && ndev > 0, "vb_create_levit: no CUDA device available -- libvitb200 has no CPU fallback");
+    VB_CHECK(device >= 0 && device < ndev, "vb_create_levit: bad device index");
+    VB_CUDA(cudaSetDevice(device));
+    cudaDeviceProp prop;
+    VB_CUDA(cudaGetDeviceProperties(&prop, device));
+    VB_CHECK(prop.major == 9 && prop.minor == 0, "vb_create_levit: libvitb200 is built for sm_90a (Hopper H100) only");
+    std::unique_ptr<vb_handle> h(new vb_handle());
+    h->cfg = c;
+    h->cfg.dim = lv->dims[lv->stages - 1];
+    h->lv = *lv;
     h->device = device;
     h->build_expected();
     *out = h.release();
@@ -1794,14 +2133,17 @@ int vb_forward(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, i
 int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, int32_t img_h, int32_t img_w,
                        const float* distill_token, float* logits, float* distill_out, int32_t out_mem, void* stream) {
   return guarded(h, [&] {
-    VB_CHECK(h != nullptr && img != nullptr && distill_token != nullptr && logits != nullptr && distill_out != nullptr,
-             "vb_forward_distill: null argument");
+    VB_CHECK(h != nullptr && img != nullptr && logits != nullptr && distill_out != nullptr, "vb_forward_distill: null argument");
     VB_CHECK(h->finalized, "vb_forward_distill: call vb_finalize after setting the weights");
     VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_forward_distill: bad batch / image size");
+    const bool levit = h->cfg.kind == VB_KIND_LEVIT;
+    VB_CHECK(levit || distill_token != nullptr, "vb_forward_distill: null argument");
+    VB_CHECK(!levit || (distill_token == nullptr && h->lv.num_distill_classes > 0),
+             "vb_forward_distill: a LeViT takes no distillation token (pass NULL) and needs num_distill_classes > 0");
     VB_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const long long before = launch_counter();
-    const int dim = h->cfg.dim;
+    const int dim = levit ? h->lv.num_distill_classes : h->cfg.dim;
     const size_t img_bytes = static_cast<size_t>(batch) * img_h * img_w * h->cfg.channels * sizeof(float);
     const size_t log_bytes = static_cast<size_t>(batch) * h->cfg.num_classes * sizeof(float);
     const size_t dis_bytes = static_cast<size_t>(batch) * dim * sizeof(float);
@@ -1812,8 +2154,10 @@ int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, int32_t 
       img_d = static_cast<const float*>(h->img_dev.p);
     }
     // the distillation token is always a host vector of `dim` floats (a trainable variable of the caller, distill.py:133)
-    h->tokens_in.ensure(static_cast<size_t>(dim) * sizeof(float));
-    VB_CUDA(cudaMemcpyAsync(h->tokens_in.p, distill_token, static_cast<size_t>(dim) * sizeof(float), cudaMemcpyHostToDevice, s));
+    if (!levit) {
+      h->tokens_in.ensure(static_cast<size_t>(dim) * sizeof(float));
+      VB_CUDA(cudaMemcpyAsync(h->tokens_in.p, distill_token, static_cast<size_t>(dim) * sizeof(float), cudaMemcpyHostToDevice, s));
+    }
     float* log_d = logits;
     float* dis_d = distill_out;
     if (out_mem == VB_MEM_HOST) {
@@ -1823,8 +2167,15 @@ int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, int32_t 
       dis_d = static_cast<float*>(h->tokens_out.p);
     }
     const float* tok_d = static_cast<const float*>(h->tokens_in.p);
-    if (h->bf16()) h->distill_impl<__nv_bfloat16>(img_d, batch, img_h, img_w, tok_d, log_d, dis_d, s);
-    else h->distill_impl<float>(img_d, batch, img_h, img_w, tok_d, log_d, dis_d, s);
+    if (levit) {
+      h->arena.reset();
+      if (h->bf16()) h->levit_forward<__nv_bfloat16>(img_d, batch, img_h, img_w, log_d, dis_d, s);
+      else h->levit_forward<float>(img_d, batch, img_h, img_w, log_d, dis_d, s);
+    } else if (h->bf16()) {
+      h->distill_impl<__nv_bfloat16>(img_d, batch, img_h, img_w, tok_d, log_d, dis_d, s);
+    } else {
+      h->distill_impl<float>(img_d, batch, img_h, img_w, tok_d, log_d, dis_d, s);
+    }
     h->last_launches = launch_counter() - before;
     if (out_mem == VB_MEM_HOST) {
       VB_CUDA(cudaMemcpyAsync(logits, log_d, log_bytes, cudaMemcpyDeviceToHost, s));
@@ -1908,8 +2259,8 @@ int vb_to_patch(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, 
                 int32_t patches_mem, void* stream) {
   return guarded(h, [&] {
     VB_CHECK(h != nullptr && img != nullptr && patches != nullptr, "vb_to_patch: null argument");
-    VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT && h->cfg.kind != VB_KIND_T2T_VIT && h->cfg.kind != VB_KIND_CCT,
-             "vb_to_patch: the model has no single Rearrange patch layer");
+    VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT && h->cfg.kind != VB_KIND_T2T_VIT && h->cfg.kind != VB_KIND_CCT &&
+             h->cfg.kind != VB_KIND_LEVIT, "vb_to_patch: the model has no single Rearrange patch layer");
     VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_to_patch: bad batch / image size");
     const vb_config& c = h->cfg;
     VB_CHECK(img_h % c.patch_h == 0 && img_w % c.patch_w == 0, "Image dimensions must be divisible by the patch size.");
@@ -1929,6 +2280,7 @@ int vb_patch_to_emb(vb_handle* h, const float* patches, int32_t patches_mem, int
     VB_CHECK(h->finalized, "vb_patch_to_emb: call vb_finalize after setting the weights");
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT, "vb_patch_to_emb: CrossViT has two patch embeddings");
     VB_CHECK(h->cfg.kind != VB_KIND_CCT, vb_handle::kCctNoStages);
+    VB_CHECK(h->cfg.kind != VB_KIND_LEVIT, vb_handle::kLevitNoStages);
     VB_CHECK(rows > 0, "vb_patch_to_emb: bad shape");
     const size_t in_bytes = static_cast<size_t>(rows) * h->embed.patch.K * sizeof(float);
     const size_t out_bytes = static_cast<size_t>(rows) * h->cfg.dim * sizeof(float);
@@ -2256,6 +2608,46 @@ int vb_op_attention_ex(int32_t precision, int32_t variant, const float* q, int32
         VB_CHECK(scale <= 0.f, "vb_op_attention_ex: an explicit softmax scale needs the fused attention kernels");
         attention_generic<T>(q_d, ldq, kv_d + k_off, ldk, kv_d + v_off, ldk, o_d, ldo, static_cast<float*>(dS.p), B, nq, nk, heads, dh,
                              variant, ma, mb, g, bt, 0);
+      });
+      download<T>(o_d, out, co);
+    };
+    if (precision == VB_PRECISION_FP32) run(float());
+    else run(__nv_bfloat16());
+  });
+}
+
+int vb_op_attention_bias(int32_t precision, const float* q, int32_t ldq, const float* k, int32_t ldk, const float* v, int32_t ldv,
+                         const float* pos_bias, float* out, int32_t ldo, int32_t B, int32_t heads, int32_t dh, int32_t fmap,
+                         int32_t q_step, float scale, int32_t gelu_out, int32_t iters, float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    const long long inner = static_cast<long long>(heads) * dh;
+    VB_CHECK(q && k && v && pos_bias && out && B > 0 && heads > 0 && dh > 0 && fmap > 0 && (q_step == 1 || q_step == 2) && scale > 0.f &&
+             ldq >= inner && ldk >= inner && ldv >= inner && ldo >= inner, "vb_op_attention_bias: bad arguments");
+    const int f2 = fmap * fmap, nqs = (fmap + q_step - 1) / q_step, nq = nqs * nqs, nk = f2;
+    std::vector<float> tab(static_cast<size_t>(heads) * f2);        // [heads][fmap^2] / scale, as vb_finalize packs it
+    for (int h = 0; h < heads; ++h)
+      for (int e = 0; e < f2; ++e)
+        tab[static_cast<size_t>(h) * f2 + e] = static_cast<float>(static_cast<double>(pos_bias[static_cast<size_t>(e) * heads + h]) / scale);
+    DevMem dQ, dK, dV, dO, dS, dT;
+    dT.ensure(tab.size() * sizeof(float));
+    VB_CUDA(cudaMemcpy(dT.p, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice));
+    PosBias pb;
+    pb.table = static_cast<const float*>(dT.p); pb.fmap = fmap; pb.step = q_step; pb.gelu_out = gelu_out != 0;
+    const size_t cq = static_cast<size_t>(B) * nq * ldq, co = static_cast<size_t>(B) * nq * ldo;
+    auto run = [&](auto tag) {
+      using T = decltype(tag);
+      const T* q_d = upload<T>(dQ, q, cq);
+      const T* k_d = upload<T>(dK, k, static_cast<size_t>(B) * nk * ldk);
+      const T* v_d = upload<T>(dV, v, static_cast<size_t>(B) * nk * ldv);
+      T* o_d = upload<T>(dO, out, co);
+      dS.ensure(static_cast<size_t>(B) * heads * nq * ((nk + 15) & ~15) * 4);
+      // vb_handle::attention_bias without the handle's arena and profiler
+      timed(iters, elapsed_ms, [&] {
+        if (attention_fast<T>(q_d, ldq, k_d, ldk, v_d, ldv, o_d, ldo, B, nq, nk, heads, dh, 0, nullptr, nullptr, nullptr, nullptr, 0, scale, &pb))
+          return;
+        attention_generic<T>(q_d, ldq, k_d, ldk, v_d, ldv, o_d, ldo, static_cast<float*>(dS.p), B, nq, nk, heads, dh, 0, nullptr, nullptr,
+                             nullptr, nullptr, 0, scale, &pb);
       });
       download<T>(o_d, out, co);
     };

@@ -1,7 +1,7 @@
 // Warp-specialised wgmma GEMM for sm_90a with fused epilogues.
 //
 //   out[M,N] (bf16) = epi( A[M,K] (bf16, K-major) x Wt[N,K]^T (bf16, K-major) ),  fp32 accumulation in registers
-//   epi(v) = (+bias[n]) -> exact-erf GELU -> (*scale[n]) -> (+res[m,n])
+//   epi(v) = (+bias[n]) -> exact-erf GELU or hard-swish -> (*scale[n]) -> (+res[m,n])
 //
 // Replaces, on the reference's hot path, every nn.Dense: patch embedding (vit.py:143), to_qkv (vit.py:59,72),
 // to_out + residual (vit.py:62-69,101), MLP fc1+GELU / fc2 + residual (vit.py:38-44,102), CaiT to_q/to_kv
@@ -56,6 +56,9 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return fmaf(na, e + -0.5f, x * 0.5f);
 }
 
+// levit.py:37: x * relu6(x + 3) / 6, rounded in the reference's order
+__device__ __forceinline__ float hard_swish(float x) { return __fdiv_rn(x * fminf(fmaxf(x + 3.0f, 0.0f), 6.0f), 6.0f); }
+
 // Advance a ring position (stage, phase) by n k-blocks.
 __device__ __forceinline__ void ring_advance(int& stage, uint32_t& phase, int n) {
   stage += n % STAGES;
@@ -64,13 +67,13 @@ __device__ __forceinline__ void ring_advance(int& stage, uint32_t& phase, int n)
 }
 
 // EPI: 0 = no per-column addend, 1 = + bias[n], 2 = folded LayerNorm (c1 = ln_c1, c2 = bias)
-template <bool GELU, bool RES, int EPI, bool OF32>
+template <int ACT, bool RES, int EPI, bool OF32>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, int M, int N, int K,
                  void* __restrict__ out, int ldc, const float* __restrict__ bias, const float* __restrict__ scale,
                  const __nv_bfloat16* res, int ldr, const float* __restrict__ ln_c1, const float2* ln_stats, int ln_parts,
                  float ln_inv_d, float2* __restrict__ stats_out) {
-  static_assert(!OF32 || (!GELU && !RES && EPI != 2), "fp32 output: plain / bias epilogue only");
+  static_assert(!OF32 || (ACT == ACT_NONE && !RES && EPI != 2), "fp32 output: plain / bias epilogue only");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = smem_base + STAGES * STAGE_BYTES;
@@ -251,7 +254,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
             v0 += cb0;
             v1 += cb1;
           }
-          if (GELU) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+          if (ACT == ACT_GELU) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+          if (ACT == ACT_HSWISH) { v0 = hard_swish(v0); v1 = hard_swish(v1); }
           // rounded on its own, as the reference's LayerScale is, never fused with the residual add into one FMA
           if (scale != nullptr) { v0 = __fmul_rn(v0, sc0); v1 = __fmul_rn(v1, sc1); }
           if (r >= M) continue;
@@ -302,9 +306,9 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-template <bool GELU, bool RES, int EPI, bool OF32 = false>
+template <int ACT, bool RES, int EPI, bool OF32 = false>
 void launch(const GemmBf16& g, cudaStream_t stream) {
-  auto kern = gemm_bf16_kernel<GELU, RES, EPI, OF32>;
+  auto kern = gemm_bf16_kernel<ACT, RES, EPI, OF32>;
   static unsigned long long seen[4] = {0, 0, 0, 0};
   if (first_use_on_this_device(seen)) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
   const long long tiles = static_cast<long long>((g.N + BN - 1) / BN) * ((g.M + BM - 1) / BM);
@@ -356,7 +360,7 @@ bool gemm_bf16_supported(int M, int N, int K, int lda, int ldw, int ldc) {
 }
 
 GemmBf16 gemm_bf16_plan(const __nv_bfloat16* A, int lda, const __nv_bfloat16* Wt, int ldw, __nv_bfloat16* out, int ldc, int M,
-                        int N, int K, const float* bias, const float* scale, const __nv_bfloat16* res, int ldr, bool gelu,
+                        int N, int K, const float* bias, const float* scale, const __nv_bfloat16* res, int ldr, int act,
                         bool out_f32, int b_rows) {
   VB_CHECK(gemm_bf16_supported(M, N, K, lda, ldw, ldc), "gemm_bf16: unsupported shape (need N%64==0, K%8==0, ld%8==0)");
   VB_CHECK(res == nullptr || ldr % 8 == 0, "gemm_bf16: residual leading dimension must be a multiple of 8");
@@ -364,7 +368,7 @@ GemmBf16 gemm_bf16_plan(const __nv_bfloat16* A, int lda, const __nv_bfloat16* Wt
             reinterpret_cast<uintptr_t>(res)) % 16 == 0, "gemm_bf16: operands must be 16-byte aligned");
   GemmBf16 g;
   g.M = M; g.N = N; g.K = K;
-  g.bias = bias; g.scale = scale; g.res = res; g.ldr = ldr; g.gelu = gelu;
+  g.bias = bias; g.scale = scale; g.res = res; g.ldr = ldr; g.act = act;
   g.out = out; g.ldc = ldc; g.out_f32 = out_f32;
   g.tmap_a = make_tmap_2d(A, K, M, static_cast<uint64_t>(lda) * 2, BK, BM);
   // b_rows: rows of Wt that exist (< N when the output is column-padded: TMA zero-fills the rest instead of reading on)
@@ -377,16 +381,18 @@ void gemm_bf16_run(const GemmBf16& g, cudaStream_t stream) {
   const int epi = g.ln_c1 != nullptr ? 2 : g.bias != nullptr ? 1 : 0;
   VB_CHECK(epi != 2 || (g.bias != nullptr && g.ln_stats != nullptr && g.ln_parts > 0), "folded LayerNorm needs c1, c2 and the row statistics");
   if (g.out_f32) {
-    VB_CHECK(!g.gelu && !res && epi != 2 && g.scale == nullptr && g.stats_out == nullptr, "fp32-output GEMM: plain or bias epilogue only");
-    if (epi == 0) return launch<false, false, 0, true>(g, stream);
-    return launch<false, false, 1, true>(g, stream);
+    VB_CHECK(g.act == ACT_NONE && !res && epi != 2 && g.scale == nullptr && g.stats_out == nullptr, "fp32-output GEMM: plain or bias epilogue only");
+    if (epi == 0) return launch<ACT_NONE, false, 0, true>(g, stream);
+    return launch<ACT_NONE, false, 1, true>(g, stream);
   }
-#define VB_GEMM_CASE(G, R, E) if (g.gelu == G && res == R && epi == E) return launch<G, R, E>(g, stream)
-  VB_GEMM_CASE(false, false, 0); VB_GEMM_CASE(false, false, 1); VB_GEMM_CASE(false, false, 2);
-  VB_GEMM_CASE(true, false, 0);  VB_GEMM_CASE(true, false, 1);  VB_GEMM_CASE(true, false, 2);
-  VB_GEMM_CASE(false, true, 0);  VB_GEMM_CASE(false, true, 1);  VB_GEMM_CASE(false, true, 2);
-  VB_GEMM_CASE(true, true, 0);   VB_GEMM_CASE(true, true, 1);   VB_GEMM_CASE(true, true, 2);
+#define VB_GEMM_CASE(A, R, E) if (g.act == A && res == R && epi == E) return launch<A, R, E>(g, stream)
+  VB_GEMM_CASE(ACT_NONE, false, 0); VB_GEMM_CASE(ACT_NONE, false, 1); VB_GEMM_CASE(ACT_NONE, false, 2);
+  VB_GEMM_CASE(ACT_GELU, false, 0); VB_GEMM_CASE(ACT_GELU, false, 1); VB_GEMM_CASE(ACT_GELU, false, 2);
+  VB_GEMM_CASE(ACT_NONE, true, 0);  VB_GEMM_CASE(ACT_NONE, true, 1);  VB_GEMM_CASE(ACT_NONE, true, 2);
+  VB_GEMM_CASE(ACT_GELU, true, 0);  VB_GEMM_CASE(ACT_GELU, true, 1);  VB_GEMM_CASE(ACT_GELU, true, 2);
+  VB_GEMM_CASE(ACT_HSWISH, false, 1);                                  // LeViT MLP fc1 (levit.py:53-54)
 #undef VB_GEMM_CASE
+  VB_CHECK(false, "gemm_bf16: no kernel instance for this epilogue (activation " + std::to_string(g.act) + ")");
 }
 
 }  // namespace vb

@@ -298,7 +298,7 @@ __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.0f +
 template <typename TA, typename TW, typename TO, int TM>
 __global__ void __launch_bounds__(256)
 gemm_simt_kernel(const TA* __restrict__ A, int lda, const TW* __restrict__ W, int wsk, int wsn, TO* out, int ldc, int M, int N,
-                 int K, const float* __restrict__ bias, const float* __restrict__ scale, const TO* res, int ldr, int gelu) {
+                 int K, const float* __restrict__ bias, const float* __restrict__ scale, const TO* res, int ldr, int act) {
   constexpr int BMT = 16 * TM;
   __shared__ float As[16][BMT + 1];
   __shared__ __align__(16) float Ws[16][64 + 4];   // pitch 68 floats: 16-byte aligned rows, one LDS.128 per thread and k
@@ -351,7 +351,8 @@ gemm_simt_kernel(const TA* __restrict__ A, int lda, const TW* __restrict__ W, in
       if (n >= N) continue;
       float v = acc[i][j];
       if (bias) v += bias[n];
-      if (gelu) v = gelu_erf_f(v);
+      if (act == ACT_GELU) v = gelu_erf_f(v);
+      else if (act == ACT_HSWISH) v = v * fminf(fmaxf(v + 3.0f, 0.0f), 6.0f) / 6.0f;   // levit.py:37
       if (scale) v *= scale[n];
       if (res) v += to_f(res[static_cast<long long>(m) * ldr + n]);
       out[static_cast<long long>(m) * ldc + n] = from_f<TO>(v);
@@ -449,7 +450,7 @@ __global__ void attn_softmax_kernel(float* __restrict__ S, long long rows, int n
 template <typename T>
 __global__ void __launch_bounds__(256)
 attn_pv_kernel(const float* __restrict__ S, const T* __restrict__ v, int ldv, T* __restrict__ out, int ldo, int heads, int nq, int nk,
-               int dh) {
+               int dh, int gelu_out) {
   __shared__ float Ps[32][33];
   __shared__ float Vs[32][33];
   const int dt = (dh + 31) / 32, qt = (nq + 31) / 32;              // flat grid, column tile fastest
@@ -480,8 +481,39 @@ attn_pv_kernel(const float* __restrict__ S, const T* __restrict__ v, int ldv, T*
 #pragma unroll
     for (int c = 0; c < 2; ++c) {
       const int i = i0 + ty * 2 + a, d = d0 + tx * 2 + c;
-      if (i < nq && d < dh) out[(static_cast<long long>(b) * nq + i) * ldo + h * dh + d] = from_f<T>(acc[a][c]);
+      if (i < nq && d < dh) out[(static_cast<long long>(b) * nq + i) * ldo + h * dh + d] = from_f<T>(gelu_out ? gelu_exact(acc[a][c]) : acc[a][c]);
     }
+}
+
+// S[b,h,i,j] += table[h, pos_bias_index(i, j)]  (materialised scores, row pitch nk)
+__global__ void attn_pos_bias_kernel(float* __restrict__ S, const float* __restrict__ table, int heads, int nq, int nk, int fmap,
+                                     int step, long long total) {
+  const int nqs = (fmap + step - 1) / step;
+  for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
+       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int j = static_cast<int>(idx % nk);
+    const long long r = idx / nk;
+    const int i = static_cast<int>(r % nq), h = static_cast<int>((r / nq) % heads);
+    S[idx] += table[static_cast<long long>(h) * fmap * fmap + pos_bias_index(i, j, fmap, step, nqs)];
+  }
+}
+
+// out[b, r*ow + c, :] = in[b, (step*r)*W + step*c, :]  (16-byte vectors when C, ld are multiples of the vector width)
+template <typename T>
+__global__ void gather_grid_kernel(const T* __restrict__ in, int ldi, T* __restrict__ out, int ldo, int H, int W, int C, int step,
+                                   int oh, int ow, long long total_vec, int vec) {
+  for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total_vec;
+       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int cv = C / vec;
+    const int c = static_cast<int>(idx % cv) * vec;
+    const long long p = idx / cv;
+    const int pc = static_cast<int>(p % ow), pr = static_cast<int>((p / ow) % oh);
+    const long long b = p / (static_cast<long long>(ow) * oh);
+    const T* src = in + ((b * H + static_cast<long long>(pr) * step) * W + static_cast<long long>(pc) * step) * ldi + c;
+    T* dst = out + p * ldo + c;
+    if (vec * sizeof(T) == 16) *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(src);
+    else for (int e = 0; e < vec; ++e) dst[e] = src[e];
+  }
 }
 
 // ------------------------------------------------------------------------------------------ pooling + head LN
@@ -504,6 +536,10 @@ __global__ void pool_layernorm_kernel(const T* __restrict__ X, int n, int ldx, c
     z[d] = v;
   }
   __syncthreads();
+  if (gamma == nullptr) {                                           // GlobalAvgPool2D alone (levit.py:206-208)
+    for (int d = threadIdx.x; d < D; d += blockDim.x) out[static_cast<long long>(b) * D + d] = z[d];
+    return;
+  }
   auto block_sum = [&](float v) {
     v = warp_sum(v);
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
@@ -895,13 +931,13 @@ void layernorm(const T* x, int ldx, const float* gamma, const float* beta, T* ou
 
 template <typename TA, typename TW, typename TO>
 void gemm_simt(const TA* A, int lda, const TW* W, int wsk, int wsn, TO* out, int ldc, int M, int N, int K, const float* bias,
-               const float* scale, const TO* res, int ldr, int gelu, cudaStream_t s) {
+               const float* scale, const TO* res, int ldr, int act, cudaStream_t s) {
   if (static_cast<long long>((N + 63) / 64) * ((M + 63) / 64) >= 2 * sm_count()) {
     const unsigned grid = flat_blocks((N + 63) / 64, (M + 63) / 64, "gemm_simt");
-    gemm_simt_kernel<TA, TW, TO, 4><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, gelu);
+    gemm_simt_kernel<TA, TW, TO, 4><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act);
   } else {
     const unsigned grid = flat_blocks((N + 63) / 64, (M + 15) / 16, "gemm_simt");
-    gemm_simt_kernel<TA, TW, TO, 1><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, gelu);
+    gemm_simt_kernel<TA, TW, TO, 1><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act);
   }
   VB_LAUNCHED();
 }
@@ -930,10 +966,26 @@ void attn_softmax(float* S, long long rows, int nk, cudaStream_t s) {
 }
 
 template <typename T>
-void attn_pv(const float* S, const T* v, int ldv, T* out, int ldo, int B, int heads, int nq, int nk, int dh, cudaStream_t s) {
+void attn_pv(const float* S, const T* v, int ldv, T* out, int ldo, int B, int heads, int nq, int nk, int dh, cudaStream_t s, int gelu_out) {
   const long long blocks = static_cast<long long>((dh + 31) / 32) * ((nq + 31) / 32) * B * heads;
   VB_CHECK(blocks <= 0x7fffffffLL, "attention PV: grid of " + std::to_string(blocks) + " blocks exceeds 2^31 - 1");
-  attn_pv_kernel<T><<<static_cast<unsigned>(blocks), 256, 0, s>>>(S, v, ldv, out, ldo, heads, nq, nk, dh);
+  attn_pv_kernel<T><<<static_cast<unsigned>(blocks), 256, 0, s>>>(S, v, ldv, out, ldo, heads, nq, nk, dh, gelu_out);
+  VB_LAUNCHED();
+}
+
+void attn_pos_bias(float* S, const PosBias& pb, int B, int heads, int nq, int nk, cudaStream_t s) {
+  const long long total = static_cast<long long>(B) * heads * nq * nk;
+  attn_pos_bias_kernel<<<grid_1d(total, 256), 256, 0, s>>>(S, pb.table, heads, nq, nk, pb.fmap, pb.step, total);
+  VB_LAUNCHED();
+}
+
+template <typename T>
+void gather_grid(const T* in, int ldi, T* out, int ldo, int B, int H, int W, int C, int step, cudaStream_t s) {
+  const int oh = (H + step - 1) / step, ow = (W + step - 1) / step;
+  const int vec = (C % (16 / sizeof(T)) == 0 && ldi % (16 / sizeof(T)) == 0 && ldo % (16 / sizeof(T)) == 0 &&
+                   (reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) % 16 == 0) ? 16 / sizeof(T) : 1;
+  const long long total = static_cast<long long>(B) * oh * ow * (C / vec);
+  gather_grid_kernel<T><<<grid_1d(total, 256), 256, 0, s>>>(in, ldi, out, ldo, H, W, C, step, oh, ow, total, vec);
   VB_LAUNCHED();
 }
 
@@ -1044,7 +1096,8 @@ void row_stats_bf16(const __nv_bfloat16* X, int ldx, float* stats, int M, int D,
   template void build_embed_residual<T>(T*, const float*, const float*, const float*, int, int, int, int, cudaStream_t);    \
   template void layernorm<T>(const T*, int, const float*, const float*, T*, int, int, int, cudaStream_t, int);                   \
   template void attn_scores<T>(const T*, int, const T*, int, float*, int, int, int, int, int, float, cudaStream_t);         \
-  template void attn_pv<T>(const float*, const T*, int, T*, int, int, int, int, int, int, cudaStream_t);                    \
+  template void attn_pv<T>(const float*, const T*, int, T*, int, int, int, int, int, int, cudaStream_t, int);               \
+  template void gather_grid<T>(const T*, int, T*, int, int, int, int, int, int, cudaStream_t);                              \
   template void pool_layernorm<T>(const T*, int, int, const float*, const float*, float*, int, int, int, cudaStream_t);     \
   template void copy_tokens<T>(const T*, int, int, T*, int, int, int, int, int, cudaStream_t);                              \
   template void broadcast_row<T>(const float*, T*, int, int, int, cudaStream_t);                                            \

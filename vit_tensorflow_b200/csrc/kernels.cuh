@@ -30,10 +30,10 @@ void transpose_rows_bf16(const __nv_bfloat16* in, int ldi, long long in_batch, _
                          int n, int npad, int cols, cudaStream_t s);
 
 // out[M,N] (TO) = epi(A[M,K] (TA, lda) x W), W element (k,n) at W[k*wsk + n*wsn]; fp32 FMA accumulation.
-// epi = (+bias) -> GELU(erf) -> (*scale) -> (+res[m*ldr + n]).
+// epi = (+bias) -> act (Act: GELU(erf) / hard-swish) -> (*scale) -> (+res[m*ldr + n]).
 template <typename TA, typename TW, typename TO>
 void gemm_simt(const TA* A, int lda, const TW* W, int wsk, int wsn, TO* out, int ldc, int M, int N, int K,
-               const float* bias, const float* scale, const TO* res, int ldr, int gelu, cudaStream_t s);
+               const float* bias, const float* scale, const TO* res, int ldr, int act, cudaStream_t s);
 
 // Generic attention through materialised scores (any n, d, variant), S fp32 [B,h,nq,nk] workspace.
 // q: [B, nq, *] rows of pitch ldq with head hh at columns [hh*dh, (hh+1)*dh); k, v likewise (nk rows per batch).
@@ -44,10 +44,19 @@ void attn_scores(const T* q, int ldq, const T* k, int ldk, float* S, int B, int 
 void attn_head_mix(float* S, const float* Wmix, const float* gamma, const float* beta, int B, int heads, int nq, int nk,
                    cudaStream_t s);
 void attn_softmax(float* S, long long rows, int nk, cudaStream_t s);
+// gelu_out: exact-erf GELU of every output element (PosBias::gelu_out)
 template <typename T>
-void attn_pv(const float* S, const T* v, int ldv, T* out, int ldo, int B, int heads, int nq, int nk, int dh, cudaStream_t s);
+void attn_pv(const float* S, const T* v, int ldv, T* out, int ldo, int B, int heads, int nq, int nk, int dh, cudaStream_t s,
+             int gelu_out = 0);
+// S[b,h,i,j] += the relative-position bias of (i, j) (PosBias, common.h); S fp32 [B,h,nq,nk]
+void attn_pos_bias(float* S, const PosBias& pb, int B, int heads, int nq, int nk, cudaStream_t s);
 
-// z[b,:] = LN(pool(X[b]))  with pool = row 0 (cls) or mean over the n rows; fp32 out [B, D].
+// The strided pixels of a map (LeViT's stride-2 1x1 VALID query convolution, levit.py:75): in [B, H, W, C] rows of pitch ldi ->
+// out [B, ceil(H/step) * ceil(W/step), C] rows of pitch ldo, out pixel (r, c) = in pixel (step*r, step*c).
+template <typename T>
+void gather_grid(const T* in, int ldi, T* out, int ldo, int B, int H, int W, int C, int step, cudaStream_t s);
+
+// z[b,:] = LN(pool(X[b]))  with pool = row 0 (cls) or mean over the n rows; fp32 out [B, D].  gamma == null: no LayerNorm.
 template <typename T>
 void pool_layernorm(const T* X, int n, int ldx, const float* gamma, const float* beta, float* out, int B, int D, int mean_pool,
                     cudaStream_t s);

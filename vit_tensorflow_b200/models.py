@@ -737,8 +737,133 @@ CCT_CTOR_KEYS = ("img_size", "embedding_dim", "n_input_channels", "n_conv_layers
                  "pooling_stride", "num_layers", "num_heads", "mlp_ratio", "num_classes", "positional_embedding")
 
 
+def levit_cast_tuple(val, l=3):
+    """levit.py:18-20: an int is repeated, a short tuple padded with its last element, a long one kept (the assert catches it)."""
+    val = val if isinstance(val, tuple) else (val,)
+    return (*val, *((val[-1],) * max(l - len(val), 0)))
+
+
+class LeViT(_EngineModel):
+    """levit.py:164-226: a four-convolution stem, `stages` stacks of BatchNorm attention with a learned relative-position bias and
+    hard-swish MLPs, a stride-2 "shrink" attention between stages, global average pooling, mlp_head (and distill_head).
+
+    Inference only: the reference's call defaults to training=True, which makes every BatchNormalization use the batch's statistics
+    and the dropout layers draw masks; a call without training=False raises NotImplementedError here.  The feature map after the
+    stem must be image_size // 16 square (levit.py:194): such an image_size is refused at construction, and an image whose stem
+    output has another size is refused at call time.
+    Weights (SURVEY.md App. B) keep the reference's attribute paths: conv_embedding.{i}, backbone.{t}.layers.{l}.0 (attention:
+    to_q / to_k / to_v .0 conv + .1 BatchNormalization, pos_bias.embeddings, to_out.1 conv + .2 BatchNormalization),
+    backbone.{t}.layers.{l}.1.net.{0,3} (MLP), mlp_head, distill_head."""
+    _kind = "levit"
+
+    def __init__(self, image_size, num_classes, dim, depth, heads, mlp_mult, stages=3, dim_key=32, dim_value=64, dropout=0.0,
+                 num_distill_classes=None, *, precision="bf16", device=0, seed=None):
+        dims = levit_cast_tuple(dim, stages)
+        depths = levit_cast_tuple(depth, stages)
+        layer_heads = levit_cast_tuple(heads, stages)
+        assert all(map(lambda t: len(t) == stages, (dims, depths, layer_heads))), \
+            'dimensions, depths, and heads must be a tuple that is less than the designated number of stages'
+        f = image_size
+        for _ in range(4):
+            f = -(-f // 2)
+        if f != image_size // 16:
+            raise ValueError(f"LeViT: image_size {image_size} gives a {f} x {f} map after the four stride-2 stem convolutions, but "
+                             f"the position biases are built for image_size // 16 = {image_size // 16} (levit.py:194); the "
+                             "reference fails at its first call")
+        if stages > _lib.LEVIT_MAX_STAGES:
+            raise ValueError(f"LeViT: at most {_lib.LEVIT_MAX_STAGES} stages")
+        self.num_classes, self.num_distill_classes = num_classes, num_distill_classes
+        self.dims, self.depths, self.layer_heads = dims, depths, layer_heads
+        self.image_size, self.dim_key, self.dim_value, self.mlp_mult, self.stages = image_size, dim_key, dim_value, mlp_mult, stages
+        self._dropout_rates = (dropout,)
+        self.precision = precision
+        self.device = int(device)
+        cfg = _lib.VbConfig()
+        cfg.struct_size = C.sizeof(_lib.VbConfig)
+        cfg.kind = _lib.KIND["levit"]
+        if precision not in _lib.PRECISION:
+            raise ValueError(f"precision must be one of {sorted(_lib.PRECISION)}")
+        cfg.precision = _lib.PRECISION[precision]
+        cfg.channels, cfg.image_h, cfg.image_w, cfg.num_classes = 3, image_size, image_size, num_classes
+        cfg.dim = dims[-1]                               # the pooled width (what the engine's handle records as dim)
+        lv = _lib.VbLevitConfig()
+        lv.struct_size = C.sizeof(_lib.VbLevitConfig)
+        lv.stages = stages
+        for i in range(stages):
+            lv.dims[i], lv.depths[i], lv.heads[i] = dims[i], depths[i], layer_heads[i]
+        lv.dim_key, lv.dim_value, lv.mlp_mult = dim_key, dim_value, mlp_mult
+        lv.num_distill_classes = num_distill_classes or 0
+        self._cfg, self._lv = cfg, lv
+        self._lib = _lib.load()
+        h = C.c_void_p()
+        _lib.check(self._lib.vb_create_levit(C.byref(cfg), C.byref(lv), self.device, C.byref(h)))
+        self._h = h
+        self._finalized = False
+        self._specs = collections.OrderedDict()
+        name, shape, ndim = C.c_char_p(), (C.c_int64 * 4)(), C.c_int32()
+        for i in range(self._lib.vb_num_weights(h)):
+            _lib.check(self._lib.vb_weight_info(h, i, C.byref(name), shape, C.byref(ndim)), h)
+            self._specs[name.value.decode()] = tuple(int(shape[j]) for j in range(ndim.value))
+        self._weights = collections.OrderedDict()
+        self.init_weights(seed)
+
+    def init_weights(self, seed=None):
+        """The reference's initialisers: glorot-uniform over the receptive field and zero biases (Conv2D / Dense), BatchNormalization
+        gamma 1 / beta 0 / moving statistics 0 and 1 with the to_out gamma at 0 (levit.py:91), Embedding U(-0.05, 0.05)."""
+        rng = np.random.default_rng(seed)
+        w = collections.OrderedDict()
+        for name, shape in self._specs.items():
+            leaf = name.rsplit(".", 1)[-1]
+            if leaf == "kernel":
+                receptive = int(np.prod(shape[:-2]))
+                lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
+                a = rng.uniform(-lim, lim, size=shape)
+            elif leaf in ("bias", "beta", "moving_mean"):
+                a = np.zeros(shape)
+            elif leaf == "moving_variance":
+                a = np.ones(shape)
+            elif leaf == "gamma":
+                a = np.zeros(shape) if ".to_out." in name else np.ones(shape)
+            elif leaf == "embeddings":
+                a = rng.uniform(-0.05, 0.05, size=shape)
+            else:
+                raise AssertionError(name)
+            w[name] = a.astype(np.float32)
+        self.set_weights_dict(w)
+
+    def _check_training(self, training):
+        if training is None or training:
+            raise NotImplementedError(
+                "LeViT runs inference only: with training=True (the reference's default, levit.py:214) every BatchNormalization "
+                "normalises with the batch's own statistics and dropout draws masks; pass training=False")
+
+    def __call__(self, img, training=True, **kwargs):
+        """levit.py:214: NHWC float images -> logits [b, num_classes], or (logits, distill [b, num_distill_classes]) with a
+        distillation head.  training must be False."""
+        self._check_training(training)
+        if self.num_distill_classes is None:
+            return super().__call__(img, training=False)
+        self._finalize()
+        x = self._img(img)
+        b, h, w, _ = x.shape
+        logits = np.empty((b, self.num_classes), np.float32)
+        dist = np.empty((b, self.num_distill_classes), np.float32)
+        _lib.check(self._lib.vb_forward_distill(self._h, x.ctypes.data_as(C.c_void_p), _lib.MEM_HOST, b, h, w, None,
+                                                logits.ctypes.data_as(C.c_void_p), dist.ctypes.data_as(C.c_void_p), _lib.MEM_HOST,
+                                                None), self._h)
+        return _as_tensor(logits), _as_tensor(dist)
+
+    call = __call__
+
+
+LEVIT_CTOR_KEYS = ("image_size", "num_classes", "dim", "depth", "heads", "mlp_mult", "stages", "dim_key", "dim_value", "dropout",
+                   "num_distill_classes")
+
+
 def from_config(cfg: dict, precision="bf16", device=0, seed=None):
     """Build a model from an oracle-style config dict (kind + reference kwargs)."""
+    if cfg["kind"] == "levit":
+        return LeViT(**{k: v for k, v in cfg.items() if k in LEVIT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "cct":
         return CCT(**{k: v for k, v in cfg.items() if k in CCT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     kw = {k: v for k, v in cfg.items() if k not in ("kind", "channels", "image_h", "image_w", "patch_h", "patch_w", "num_patches",
