@@ -11,6 +11,7 @@
  *     vit_with_patch_merger.ViT(...)(img)   vit_tensorflow/vit_with_patch_merger.py:134-146,174-185   (8f, f4)
  *     efficient.ViT(...)(img)        vit_tensorflow/efficient.py:13-14,39-55 = vb_forward_embed -> caller's transformer -> vb_forward_head
  *     LeViT(...)(img)                vit_tensorflow/levit.py:164-226 (vb_create_levit; distillation head: vb_forward_distill)
+ *     CvT(...)(img)                  vit_tensorflow/cvt.py:149-202 (vb_create_cvt)
  * and this header is what the Python host classes (vit_tensorflow_b200/models.py, _lib.py) bind with ctypes.
  * Plain pointers and sizes only; no torch / C++ types cross the boundary.
  *
@@ -40,7 +41,8 @@ extern "C" {
 typedef struct vb_handle vb_handle;
 
 enum { VB_KIND_VIT = 0, VB_KIND_DEEPVIT = 1, VB_KIND_CAIT = 2, VB_KIND_CROSSVIT = 3, VB_KIND_PARALLEL_VIT = 4,
-       VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6, VB_KIND_CCT = 7, VB_KIND_LEVIT = 8 };
+       VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6, VB_KIND_CCT = 7, VB_KIND_LEVIT = 8,
+       VB_KIND_CVT = 9 };
 enum { VB_CCT_POS_SINE = 0, VB_CCT_POS_LEARNABLE = 1, VB_CCT_POS_NONE = 2 };   /* cct.py:233-234,250-256 */
 enum { VB_PRECISION_FP32 = 0, VB_PRECISION_BF16 = 1 };
 enum { VB_POOL_CLS = 0, VB_POOL_MEAN = 1 };
@@ -84,8 +86,8 @@ typedef struct vb_config {
 
 VB_API int vb_abi_version(void);
 
-/* Replaces <Model>.__init__ (vit.py:107-157 etc.): validates the config and allocates device state.  VB_KIND_LEVIT is refused
- * here: a LeViT handle comes from vb_create_levit. */
+/* Replaces <Model>.__init__ (vit.py:107-157 etc.): validates the config and allocates device state.  VB_KIND_LEVIT and
+ * VB_KIND_CVT are refused here: their handles come from vb_create_levit and vb_create_cvt. */
 VB_API int vb_create(const vb_config* cfg, int device, vb_handle** out);
 
 /* LeViT (levit.py:164-212), appended within ABI 7.  `dims`, `depths` and `heads` hold `stages` entries each (cast_tuple already
@@ -111,6 +113,31 @@ typedef struct vb_levit_config {
  * MLP), mlp_head and distill_head .kernel / .bias.  vb_finalize folds every BatchNormalization (inference statistics, eps 1e-5)
  * into its convolution. */
 VB_API int vb_create_levit(const vb_config* base, const vb_levit_config* lv, int device, vb_handle** out);
+
+/* CvT (cvt.py:149-202), appended within ABI 7: the reference's three stages s1, s2, s3 (index 0, 1, 2).  Stage s is a
+ * Conv2D(emb_dim, emb_kernel, emb_stride, SAME, bias) over the previous map, the channel LayerNorm (eps 1e-5, cvt.py:30-43), then
+ * depth x [x = attn(LN(x)) + x; x = mlp(LN(x)) + x] with heads of 64 (dim_head is fixed, cvt.py:130,189): q = pw_q(BN(dw_q(y))),
+ * kv = pw_kv(BN(dw_kv(y))) with depthwise proj_kernel x proj_kernel SAME convolutions of stride 1 and kv_proj_stride (no bias),
+ * softmax(q k^T / 8) v, to_out (1x1, bias); mlp = 1x1 (emb_dim * mlp_mult, bias) -> exact GELU -> 1x1 (emb_dim, bias).  Head:
+ * GlobalAvgPool2D -> Dense(num_classes).  No position embeddings: any image size. */
+#define VB_CVT_STAGES 3
+typedef struct vb_cvt_config {
+  int32_t struct_size;            /* sizeof(vb_cvt_config) */
+  int32_t emb_dim[VB_CVT_STAGES], emb_kernel[VB_CVT_STAGES], emb_stride[VB_CVT_STAGES];
+  int32_t proj_kernel[VB_CVT_STAGES];      /* 1 .. 7 */
+  int32_t kv_proj_stride[VB_CVT_STAGES];   /* 1 or 2 */
+  int32_t heads[VB_CVT_STAGES], depth[VB_CVT_STAGES], mlp_mult[VB_CVT_STAGES];
+} vb_cvt_config;
+
+/* CvT.__init__: `base` supplies precision, channels, num_classes and max_batch; its kind must be VB_KIND_CVT and its other
+ * fields (image size included: CvT takes any h x w at call time) are ignored.  Weights (SURVEY.md App. B) are named by the
+ * reference's attribute paths: cvt_layers.{s}.0.kernel [k, k, cin, emb_dim] / .bias, cvt_layers.{s}.1.g / .b [1, 1, 1, emb_dim],
+ * cvt_layers.{s}.2.layers.{l}.0.norm.g / .b, ....0.fn.to_q.net.0.kernel [k, k, 1, emb_dim] (depthwise), .net.1.{gamma, beta,
+ * moving_mean, moving_variance}, .net.2.kernel [1, 1, emb_dim, 64 * heads], the same for to_kv with 128 * heads,
+ * ....0.fn.to_out.0.kernel / .bias, ....1.norm.g / .b, ....1.fn.net.0 / .net.3 .kernel / .bias, cvt_layers.3.1.kernel / .bias
+ * (the Dense head).  vb_finalize folds every BatchNormalization (inference statistics, eps 1e-5) into the depthwise taps and a
+ * per-channel shift. */
+VB_API int vb_create_cvt(const vb_config* base, const vb_cvt_config* cvt, int device, vb_handle** out);
 
 /* Replaces Keras variable assignment: one call per weight, names/shapes/layouts per SURVEY.md App. B
  * (Dense kernel [in,out], float32).  shape/ndim are checked against the config. */
@@ -153,7 +180,8 @@ VB_API int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, i
                        const float* distill_token, float* logits, float* distill_out, int32_t out_mem, void* stream);
 
 /* ---- the stages of <Model>.call on their own (SURVEY.md 8f f1/f4): the attribute surface the reference's wrappers and the
- * injected-transformer shell use.  ViT / DeepViT / parallel ViT / CaiT / patch-merger ViT / T2TViT; not CrossViT, CCT or LeViT. */
+ * injected-transformer shell use.  ViT / DeepViT / parallel ViT / CaiT / patch-merger ViT / T2TViT; not CrossViT, CCT, LeViT or
+ * CvT. */
 
 /* Number of token rows vb_forward_embed produces for an img_h x img_w image (patches + cls where the model has one);
  * negative on error. */
@@ -226,6 +254,9 @@ VB_API int32_t vb_last_attention_path(void);
  * 6 wgmma GEMM with residual epilogue (patch embed, to_out, fc2).
  * LeViT: the stem's unfold is 3 and its convolutions 0; the q / k|v projections and the shrink blocks' to_out are 0, the biased
  * attention 1, the hard-swish fc1 5, the residual to_out / fc2 6; the even-pixel gather is 4 and the average pool 2.
+ * CvT: the stems' unfold is 3 and their convolutions 0, the stem LayerNorm (and its row statistics) and the average pool 2; the
+ * depthwise q / k|v convolutions (one launch per block) are 4, the pointwise projections 0, attention 1, the LayerNorm-folded GELU
+ * fc1 5, the residual to_out / fc2 6 (the fp32 engine adds its separate PreNorm LayerNorms to 2).
  * vb_profile_read synchronises the device and returns accumulated milliseconds, algorithmic FLOPs, algorithmic
  * bytes and launch counts per class (arrays of VB_PROF_NUM); reset != 0 clears the accumulators. */
 #define VB_PROF_NUM 7
@@ -309,6 +340,17 @@ VB_API int vb_op_attention_ex(int32_t precision, int32_t variant, const float* q
 VB_API int vb_op_attention_bias(int32_t precision, const float* q, int32_t ldq, const float* k, int32_t ldk, const float* v,
                                 int32_t ldv, const float* pos_bias, float* out, int32_t ldo, int32_t B, int32_t heads, int32_t dh,
                                 int32_t fmap, int32_t q_step, float scale, int32_t gelu_out, int32_t iters, float* elapsed_ms);
+
+/* CvT's depthwise projections (cvt.py:79-92,111-115) as the engine runs them, for one block: y = LN(x) over the C channels (eps
+ * 1e-5, ln_gamma / ln_beta [C]), q = BN_q(dw_q(y)) with stride 1 and kv = BN_kv(dw_kv(y)) with stride kv_stride (1 or 2), k x k
+ * (k <= 7) TF SAME depthwise convolutions whose padding is zeros of y.  x: [B, H, W, C] NHWC; wq / wkv: the depthwise kernels
+ * [k, k, 1, C]; bn_q / bn_kv: the BatchNormalization [4, C] = gamma, beta, moving_mean, moving_variance (folded on the host as
+ * vb_finalize does); q [B, H, W, C], kv [B, ceil(H/s), ceil(W/s), C].  bf16 (precision 1): x in bf16 with C zero-padded to a
+ * multiple of 64, the LayerNorm applied on load from the rows' (sum, sumsq) statistics; fp32: a separate LayerNorm, then the
+ * convolutions.  All buffers are host memory. */
+VB_API int vb_op_dwconv(int32_t precision, const float* x, int32_t B, int32_t H, int32_t W, int32_t C, const float* ln_gamma,
+                        const float* ln_beta, int32_t k, int32_t kv_stride, const float* wq, const float* bn_q, const float* wkv,
+                        const float* bn_kv, float* q, float* kv, int32_t iters, float* elapsed_ms);
 
 /* Row softmax of fp32 scores into bf16 probabilities (the T2T attention): p[r, j] = softmax_j(s[r, j] * scale) for j < n,
  * p[r, n..npad) = 0.  s [rows, lds], p [rows, ldp] (uploaded and downloaded whole); n <= npad <= ldp. */

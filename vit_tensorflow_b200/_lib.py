@@ -11,7 +11,8 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "libvitb200.so")   # VB_LIB_PATH: developer A/B builds
 
-KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6, "cct": 7, "levit": 8}
+KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6, "cct": 7, "levit": 8,
+        "cvt": 9}
 PRECISION = {"fp32": 0, "float32": 0, "bf16": 1, "bfloat16": 1}
 MEM_HOST, MEM_DEVICE = 0, 1
 ABI_VERSION = 7                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
@@ -41,6 +42,14 @@ class VbLevitConfig(C.Structure):
                 ("dim_value", C.c_int32), ("mlp_mult", C.c_int32), ("num_distill_classes", C.c_int32)]
 
 
+CVT_STAGES = 3                                      # VB_CVT_STAGES
+
+
+class VbCvtConfig(C.Structure):
+    _fields_ = [("struct_size", C.c_int32)] + [(n, C.c_int32 * CVT_STAGES) for n in (
+        "emb_dim", "emb_kernel", "emb_stride", "proj_kernel", "kv_proj_stride", "heads", "depth", "mlp_mult")]
+
+
 class VbError(RuntimeError):
     pass
 
@@ -53,6 +62,7 @@ SIGNATURES = {
     "vb_abi_version": (C.c_int, []),
     "vb_create": (C.c_int, [C.POINTER(VbConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_levit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbLevitConfig), C.c_int, C.POINTER(C.c_void_p)]),
+    "vb_create_cvt": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbCvtConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, _i64p, C.c_int32]),
     "vb_num_weights": (C.c_int, [C.c_void_p]),
     "vb_weight_info": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), _i64p, C.POINTER(C.c_int32)]),
@@ -87,6 +97,8 @@ SIGNATURES = {
                            [C.c_int32] * 6 + [C.c_float, C.c_int32, _f32p]),
     "vb_op_attention_bias": (C.c_int, [C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
                                        C.c_void_p] + [C.c_int32] * 6 + [C.c_float, C.c_int32, C.c_int32, _f32p]),
+    "vb_op_dwconv": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 2 + [C.c_int32] * 2 + [C.c_void_p] * 6 +
+                     [C.c_int32, _f32p]),
     "vb_op_softmax_rows": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 4 + [C.c_float, C.c_int32, _f32p]),
 }
 
@@ -231,6 +243,21 @@ def op_attention_bias(q, k, v, pos_bias, heads, dh, fmap, q_step, scale, out, ge
                                       _ptr(out), out.shape[2], B, heads, dh, fmap, q_step, float(scale), int(bool(gelu_out)), iters,
                                       C.byref(ms)))
     return out, (ms.value if iters > 0 else None)
+
+
+def op_dwconv(x, ln_gamma, ln_beta, wq, bn_q, wkv, bn_kv, kv_stride, precision="bf16", iters=0):
+    """CvT's depthwise q / k|v projections (vb_op_dwconv): x [B, H, W, C], the depthwise kernels [k, k, 1, C], the
+    BatchNormalizations [4, C] (gamma, beta, moving_mean, moving_variance).  Returns (q [B, H, W, C], kv [B, ceil(H/s),
+    ceil(W/s), C], ms or None)."""
+    x, ln_gamma, ln_beta, wq, bn_q, wkv, bn_kv = map(_f32, (x, ln_gamma, ln_beta, wq, bn_q, wkv, bn_kv))
+    B, H, W, Cc = x.shape
+    k = wq.shape[0]
+    q = np.empty((B, H, W, Cc), np.float32)
+    kv = np.empty((B, -(-H // kv_stride), -(-W // kv_stride), Cc), np.float32)
+    ms = C.c_float(0)
+    check(load().vb_op_dwconv(PRECISION[precision], _ptr(x), B, H, W, Cc, _ptr(ln_gamma), _ptr(ln_beta), k, kv_stride, _ptr(wq),
+                              _ptr(bn_q), _ptr(wkv), _ptr(bn_kv), _ptr(q), _ptr(kv), iters, C.byref(ms)))
+    return q, kv, (ms.value if iters > 0 else None)
 
 
 def op_softmax_rows(s, n, npad, scale, p, iters=0):

@@ -99,11 +99,13 @@ struct GemmBf16 {
   int act = ACT_NONE;                   // Act
   // Folded LayerNorm of the A operand (Wt must hold gamma-scaled weights, bias the beta.W + b term):
   //   out = rstd[m] * (acc - mu[m] * ln_c1[n]) + bias[n], with (mu, rstd) of row m reduced in the epilogue from the
-  //   ln_parts (sum, sumsq) partials of that row (the stats_out format below) over 1 / ln_inv_d elements.
+  //   ln_parts (sum, sumsq) partials of that row (the stats_out format below) over 1 / ln_inv_d elements, rstd =
+  //   1 / sqrt(var + ln_eps) (Keras LayerNormalization: 1e-3; CvT's own LayerNorm: 1e-5).
   const float* ln_c1 = nullptr;
   const float* ln_stats = nullptr;      // [ln_parts, M, 2]
   int ln_parts = 0;
   float ln_inv_d = 0.f;
+  float ln_eps = 1e-3f;
   // Emit (sum, sumsq) of every 64-column chunk of the stored bf16 output rows: [N/64, M, 2]
   float* stats_out = nullptr;
 };

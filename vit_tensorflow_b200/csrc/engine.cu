@@ -12,6 +12,7 @@
 
 #include <dlfcn.h>
 
+#include <algorithm>
 #include <array>
 #include <cmath>
 #include <cstddef>
@@ -22,6 +23,7 @@
 #include <memory>
 #include <string>
 #include <tuple>
+#include <type_traits>
 #include <vector>
 
 #ifndef VB_FWD_STREAMS
@@ -96,6 +98,8 @@ struct Linear {
   // LayerNorm folded into this Dense (bf16 engine): Wt holds gamma-scaled weights, ln_c2 replaces the bias
   const float* ln_c1 = nullptr;
   const float* ln_c2 = nullptr;
+  int ln_d = 0;                  // the LayerNorm's true width when K is zero-padded beyond it (0: K)
+  float ln_eps = 1e-3f;          // Keras LayerNormalization; CvT's own LayerNorm: 1e-5 (cvt.py:31)
 };
 struct Norm { const float* gamma = nullptr; const float* beta = nullptr; int D = 0; };
 
@@ -138,6 +142,37 @@ struct LevitBlockW {
   const float* pos = nullptr;        // [heads][fmap^2] relative-position bias / scale
   float scale = 0.f;                 // dim_key^-0.5
 };
+
+// One CvT Transformer layer (cvt.py:142-147) on channel rows zero-padded to dp (bf16) / dim (fp32).  The depthwise convolutions
+// carry their BatchNormalization folded (taps [k*k][dp] scaled, plus a per-channel shift); the MLP's PreNorm is folded into fc1
+// in the bf16 engine.
+struct CvtBlockW {
+  int dim = 0, dp = 0, heads = 0, k = 0, kv_stride = 1;
+  Norm attn_norm, ff_norm;           // gamma / beta [dp], zero on pad channels
+  const float *wq = nullptr, *bq = nullptr, *wkv = nullptr, *bkv = nullptr;
+  Linear pw_q, pw_kv, to_out, fc1, fc2;
+};
+struct CvtStageW {                   // cvt.py:186-192: Conv2D (SAME, bias) + LayerNorm + Transformer
+  int dim = 0, dp = 0, k = 0, stride = 1;
+  Linear conv;
+  Norm norm;
+  std::vector<CvtBlockW> blocks;
+};
+
+// CvT: BN(dw(y)) = dw_{s * taps}(y) + (beta - mean * s) with s = gamma / sqrt(var + 1e-5) (inference statistics, cvt.py:85).
+// Exact under SAME zero padding, which adds nothing to either form.  taps: the Keras depthwise kernel [k, k, 1, C]; w: taps
+// [k*k][Cp] and shift [Cp], zero on channels >= C.
+inline void cvt_fold_dw(const std::vector<double>& taps, const std::vector<double>& gamma, const std::vector<double>& beta,
+                        const std::vector<double>& mean, const std::vector<double>& var, int k, int C, int Cp, std::vector<double>& w,
+                        std::vector<double>& shift) {
+  w.assign(static_cast<size_t>(k) * k * Cp, 0.0);
+  shift.assign(Cp, 0.0);
+  for (int c = 0; c < C; ++c) {
+    const double sc = gamma[c] / std::sqrt(var[c] + 1e-5);
+    for (int t = 0; t < k * k; ++t) w[static_cast<size_t>(t) * Cp + c] = taps[static_cast<size_t>(t) * C + c] * sc;
+    shift[c] = beta[c] - mean[c] * sc;
+  }
+}
 
 struct EmbedW { Linear patch; const float* pos = nullptr; const float* cls = nullptr; int dim = 0, n_pos = 0; };
 struct CrossW { bool proj = false; Linear project_in, project_out, to_q, to_kv, to_out; Norm norm; };
@@ -327,9 +362,15 @@ struct vb_handle {
     const int m = lv.dim_key > lv.dim_value ? lv.dim_key : lv.dim_value;
     return bf16() ? round_up(m, 64) : m;
   }
-  // Width the bf16 engine carries a channel dimension at: a multiple of 64, so that every GEMM of a block (N = a channel width)
-  // runs on the wgmma kernel.  Pad columns are zero and stay zero: zero weights and biases, and hard-swish(0) = GELU(0) = 0.
-  int levit_width(int d) const { return bf16() ? round_up(d, 64) : d; }
+  // Width the bf16 engine carries a channel dimension of LeViT / CvT at: a multiple of 64, so that every GEMM of a block (N = a
+  // channel width) runs on the wgmma kernel.  Pad columns are zero and stay zero: zero weights and biases, hard-swish(0) = GELU(0) =
+  // 0, and LayerNorm gammas and betas padded with zeros.
+  int channel_width(int d) const { return bf16() ? round_up(d, 64) : d; }
+  // CvT (cvt.py:149-202): the three stages, then the average pool and the Dense head (`head`)
+  vb_cvt_config cv{};
+  std::vector<CvtStageW> cvt_stages;
+  static std::string cvt_pre(int st) { return "cvt_layers." + std::to_string(st) + "."; }
+  int cvt_cin(int st) const { return st == 0 ? cfg.channels : cv.emb_dim[st - 1]; }
   struct XBlock { std::vector<LayerW> sm_layers, lg_layers; Norm sm_final, lg_final; std::vector<CrossW> sm_attend_lg, lg_attend_sm; };
   std::vector<XBlock> xblocks;
   Norm head_norm, sm_head_norm, lg_head_norm;
@@ -484,6 +525,33 @@ struct vb_handle {
       const int dl = lv.dims[lv.stages - 1];
       expect_dense("mlp_head", dl, c.num_classes);
       if (lv.num_distill_classes > 0) expect_dense("distill_head", dl, lv.num_distill_classes);
+    } else if (c.kind == VB_KIND_CVT) {
+      auto expect_ln4 = [&](const std::string& n, int d) { expect(n + ".g", {1, 1, 1, d}); expect(n + ".b", {1, 1, 1, d}); };   // cvt.py:35-36
+      for (int st = 0; st < VB_CVT_STAGES; ++st) {
+        const std::string p = cvt_pre(st);
+        const int d = cv.emb_dim[st], k = cv.proj_kernel[st], inner = 64 * cv.heads[st], hidden = d * cv.mlp_mult[st];
+        expect(p + "0.kernel", {cv.emb_kernel[st], cv.emb_kernel[st], cvt_cin(st), d});          // cvt.py:187
+        expect(p + "0.bias", {d});
+        expect_ln4(p + "1", d);
+        for (int L = 0; L < cv.depth[st]; ++L) {
+          const std::string b = p + "2.layers." + std::to_string(L) + ".";
+          expect_ln4(b + "0.norm", d);
+          for (int kv = 0; kv < 2; ++kv) {                                // DepthWiseConv2d cvt.py:79-92, bias=False (:103-104)
+            const std::string n = b + (kv ? "0.fn.to_kv.net." : "0.fn.to_q.net.");
+            expect(n + "0.kernel", {k, k, 1, d});
+            for (const char* leaf : {"gamma", "beta", "moving_mean", "moving_variance"}) expect(n + "1." + leaf, {d});
+            expect(n + "2.kernel", {1, 1, d, (kv ? 2 : 1) * inner});
+          }
+          expect(b + "0.fn.to_out.0.kernel", {1, 1, inner, d});            // cvt.py:106-109
+          expect(b + "0.fn.to_out.0.bias", {d});
+          expect_ln4(b + "1.norm", d);
+          expect(b + "1.fn.net.0.kernel", {1, 1, d, hidden});              // MLP cvt.py:63-77
+          expect(b + "1.fn.net.0.bias", {hidden});
+          expect(b + "1.fn.net.3.kernel", {1, 1, hidden, d});
+          expect(b + "1.fn.net.3.bias", {d});
+        }
+      }
+      expect_dense("cvt_layers.3.1", cv.emb_dim[VB_CVT_STAGES - 1], c.num_classes);   // cvt.py:195-198
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       expect("pos_embedding", {1, np, c.dim});
@@ -708,7 +776,7 @@ struct vb_handle {
     for (auto& w : weights) VB_CHECK(w.set, "vb_finalize: weight '" + w.name + "' was never set");
     VB_CUDA(cudaSetDevice(device));
     owned.clear(); layers.clear(); cls_layers.clear(); t2t_layers.clear(); xblocks.clear(); plans.clear(); embed_res.clear(); cct_convs.clear();
-    lv_stem.clear(); lv_blocks.clear();
+    lv_stem.clear(); lv_blocks.clear(); cvt_stages.clear();
     woverride.clear();
     drop_graphs();
     const vb_config& c = cfg;
@@ -759,6 +827,8 @@ struct vb_handle {
       head = make_linear_f32("head", c.dim, c.num_classes);
     } else if (c.kind == VB_KIND_LEVIT) {
       finalize_levit();
+    } else if (c.kind == VB_KIND_CVT) {
+      finalize_cvt();
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       embed = make_embed("", c.patch_h, c.patch_w, c.dim, np, false);
@@ -837,18 +907,63 @@ struct vb_handle {
     out.resize(Np, 0.0);
     return out;
   }
-  // a Dense [K, N] + bias made on the host, packed like a registered one (under a name of its own in woverride)
-  Linear linear_from_host(const std::string& key, const std::vector<double>& Wkn, const std::vector<double>& bias, int K, int N) {
+  // a Dense [K, N] + bias (none when `bias` is empty) made on the host, packed like a registered one (under a name of its own in
+  // woverride), with the LayerNorm `fold` folded in when given
+  Linear linear_from_host(const std::string& key, const std::vector<double>& Wkn, const std::vector<double>& bias, int K, int N,
+                          const Norm* fold = nullptr) {
     woverride[key + ".kernel"] = upload_owned(Wkn);
-    woverride[key + ".bias"] = upload_owned(bias);
-    return make_linear(key, K, N);
+    if (!bias.empty()) woverride[key + ".bias"] = upload_owned(bias);
+    return make_linear(key, K, N, !bias.empty(), fold);
+  }
+  // ---- CvT weight packing: channel widths zero-padded (bf16), BatchNormalizations folded into the depthwise taps and a shift
+  Norm padded_norm(const std::string& n, int d, int dp) {        // CvT's LayerNorm g / b [1, 1, 1, d] -> [dp]
+    return Norm{upload_owned(pad_n(host_weight(n + ".g"), dp)), upload_owned(pad_n(host_weight(n + ".b"), dp)), d};
+  }
+  void finalize_cvt() {
+    for (int st = 0; st < VB_CVT_STAGES; ++st) {
+      CvtStageW S;
+      const std::string p = cvt_pre(st);
+      const int d = cv.emb_dim[st], dp = channel_width(d), ke = cv.emb_kernel[st], K = ke * ke * cvt_cin(st);
+      S.dim = d; S.dp = dp; S.k = ke; S.stride = cv.emb_stride[st];
+      S.conv = linear_from_host("cvt." + p + "0", pad_kn(host_weight(p + "0.kernel"), K, d, K, dp), pad_n(host_weight(p + "0.bias"), dp), K, dp);
+      S.norm = padded_norm(p + "1", d, dp);
+      const int inner = 64 * cv.heads[st], hidden = d * cv.mlp_mult[st], hp = channel_width(hidden), k = cv.proj_kernel[st];
+      for (int L = 0; L < cv.depth[st]; ++L) {
+        const std::string b = p + "2.layers." + std::to_string(L) + ".", key = "cvt." + b;
+        CvtBlockW w;
+        w.dim = d; w.dp = dp; w.heads = cv.heads[st]; w.k = k; w.kv_stride = cv.kv_proj_stride[st];
+        w.attn_norm = padded_norm(b + "0.norm", d, dp);
+        w.ff_norm = padded_norm(b + "1.norm", d, dp);
+        for (int kv = 0; kv < 2; ++kv) {
+          const std::string n = b + (kv ? "0.fn.to_kv.net." : "0.fn.to_q.net.");
+          std::vector<double> taps, shift;
+          cvt_fold_dw(host_weight(n + "0.kernel"), host_weight(n + "1.gamma"), host_weight(n + "1.beta"), host_weight(n + "1.moving_mean"),
+                      host_weight(n + "1.moving_variance"), k, d, dp, taps, shift);
+          const int N = (kv ? 2 : 1) * inner;
+          Linear pw = linear_from_host(key + (kv ? "pw_kv" : "pw_q"), pad_kn(host_weight(n + "2.kernel"), d, N, dp, N), {}, dp, N);
+          if (kv) { w.wkv = upload_owned(taps); w.bkv = upload_owned(shift); w.pw_kv = pw; }
+          else { w.wq = upload_owned(taps); w.bq = upload_owned(shift); w.pw_q = pw; }
+        }
+        const std::string o = b + "0.fn.to_out.0", m0 = b + "1.fn.net.0", m3 = b + "1.fn.net.3";
+        w.to_out = linear_from_host(key + "to_out", pad_kn(host_weight(o + ".kernel"), inner, d, inner, dp), pad_n(host_weight(o + ".bias"), dp),
+                                    inner, dp);
+        w.fc1 = linear_from_host(key + "fc1", pad_kn(host_weight(m0 + ".kernel"), d, hidden, dp, hp), pad_n(host_weight(m0 + ".bias"), hp), dp, hp,
+                                 bf16() ? &w.ff_norm : nullptr);
+        w.fc1.ln_d = d;
+        w.fc1.ln_eps = 1e-5f;
+        w.fc2 = linear_from_host(key + "fc2", pad_kn(host_weight(m3 + ".kernel"), hidden, d, hp, dp), pad_n(host_weight(m3 + ".bias"), dp), hp, dp);
+        S.blocks.push_back(std::move(w));
+      }
+      cvt_stages.push_back(std::move(S));
+    }
+    head = make_linear_f32("cvt_layers.3.1", cv.emb_dim[VB_CVT_STAGES - 1], cfg.num_classes);
   }
   void finalize_levit() {
     const int dh = levit_dh();
     int cin = cfg.channels;
     for (int i = 0; i < 4; ++i) {                                       // stem; the 32-channel map is written 64 wide (zero columns)
       const std::string n = "conv_embedding." + std::to_string(i);
-      const int cout = levit_stem_cout(i), np = i == 0 ? 64 : levit_width(cout), K = 9 * cin;
+      const int cout = levit_stem_cout(i), np = i == 0 ? 64 : channel_width(cout), K = 9 * cin;
       lv_stem.push_back(linear_from_host("levit." + n, pad_kn(host_weight(n + ".kernel"), K, cout, K, np),
                                          pad_n(host_weight(n + ".bias"), np), K, np));
       cin = cout;
@@ -856,7 +971,7 @@ struct vb_handle {
     for (const auto& p : levit_plan()) {
       LevitBlockW b;
       b.dim = p.dim; b.dim_out = p.dim_out; b.heads = p.heads; b.fmap = p.fmap; b.step = p.down ? 2 : 1; b.dh = dh;
-      b.dp = levit_width(p.dim); b.dp_out = levit_width(p.dim_out);
+      b.dp = channel_width(p.dim); b.dp_out = channel_width(p.dim_out);
       b.residual = !p.down && p.dim == p.dim_out;
       const std::string a = p.pre + "0.", key = "levit." + a;
       const int H = p.heads, dk = lv.dim_key, dv = lv.dim_value, HD = H * dh, dp = b.dp, dpo = b.dp_out;
@@ -895,7 +1010,7 @@ struct vb_handle {
       }
       b.scale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(dk)));
       b.pos = upload_owned(levit_pos_table(host_weight(a + "pos_bias.embeddings"), p.fmap * p.fmap, H, dk));
-      const int hidden = p.dim_out * p.mult, hp = levit_width(hidden);
+      const int hidden = p.dim_out * p.mult, hp = channel_width(hidden);
       const std::string m0 = p.pre + "1.net.0", m3 = p.pre + "1.net.3";
       b.fc1 = linear_from_host(key + "fc1", pad_kn(host_weight(m0 + ".kernel"), p.dim_out, hidden, dpo, hp), pad_n(host_weight(m0 + ".bias"), hp),
                                dpo, hp);
@@ -1393,6 +1508,8 @@ struct vb_handle {
       classify<T>(Cx, 1, c.dim, head_norm, head, B, 0, logits, false, s);
     } else if (c.kind == VB_KIND_LEVIT) {
       levit_forward<T>(img, B, H, Wd, logits, nullptr, s);
+    } else if (c.kind == VB_KIND_CVT) {
+      cvt_forward<T>(img, B, H, Wd, logits, s);
     } else if (c.kind == VB_KIND_CCT) {                   // CCT.call cct.py:342-345, TransformerClassifier.call :277-305
       int rows = 0;
       T* X = tokenize_cct<T>(img, B, H, Wd, &rows, s);
@@ -1484,7 +1601,7 @@ struct vb_handle {
       X = levit_block<T>(X, B, b, s);
       f = (b.fmap + b.step - 1) / b.step;
     }
-    const int dl = lv.dims[lv.stages - 1], ldl = levit_width(dl);
+    const int dl = lv.dims[lv.stages - 1], ldl = channel_width(dl);
     float* z = arena.get<float>(static_cast<size_t>(B) * dl);
     {
       ProfScope ps(this, PROF_LN, 1.0 * B * f * f * dl, static_cast<double>(sizeof(T)) * B * f * f * dl, s);
@@ -1544,6 +1661,89 @@ struct vb_handle {
     attention_generic<T>(q, ldq, k, ldk, v, ldv, out, ldo, S, B, nq, nk, b.heads, b.dh, 0, nullptr, nullptr, nullptr, nullptr, s, b.scale, &pb);
   }
 
+  // CvT.call (cvt.py:182-202): per stage, Conv2D (SAME, bias) -> LayerNorm -> blocks; then GlobalAvgPool2D -> Dense.  Token rows
+  // are the NHWC map, pixel-major, channel widths zero-padded to channel_width.  Any h x w: each SAME stride gives ceil.
+  static constexpr const char* kCvtNoStages = "CvT runs as a whole forward only: its stem / stage / head steps have no entry of their own";
+  template <typename T>
+  void cvt_forward(const float* img, int B, int H, int Wd, float* logits, cudaStream_t s) {
+    int mh = H, mw = Wd, mc = cfg.channels, ld_in = 0;
+    const T* map = nullptr;
+    T* X = nullptr;
+    for (const CvtStageW& S : cvt_stages) {
+      const int oh = (mh + S.stride - 1) / S.stride, ow = (mw + S.stride - 1) / S.stride, M = B * oh * ow;
+      const int Kp = bf16() ? S.conv.ldw : S.conv.K;
+      T* col = arena.get<T>(static_cast<size_t>(M) * Kp);
+      {
+        ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(map == nullptr ? 4 : sizeof(T)) * B * mh * mw * mc +
+                                                 static_cast<double>(sizeof(T)) * M * Kp, s);
+        if (map == nullptr) unfold_same<float, T>(img, col, B, mh, mw, mc, S.k, S.stride, 0, Kp, s);
+        else unfold_same<T, T>(map, col, B, mh, mw, mc, S.k, S.stride, 0, Kp, s, ld_in);
+      }
+      T* Y = arena.get<T>(static_cast<size_t>(M) * S.dp);
+      Linear L = S.conv;
+      L.K = Kp;
+      Epi e; e.bias = S.conv.bias;
+      linear<T>(col, Kp, M, L, Y, S.dp, e, s);
+      X = arena.get<T>(static_cast<size_t>(M) * S.dp);
+      float* stats = bf16() ? arena.get<float>(static_cast<size_t>(M) * (S.dp / 64) * 2) : nullptr;
+      {
+        ProfScope ps(this, PROF_LN, 8.0 * M * S.dim, 2.0 * sizeof(T) * M * S.dp, s);
+        layernorm<T>(Y, S.dp, S.norm.gamma, S.norm.beta, X, S.dp, M, S.dim, s, S.dp, 1e-5f);   // cvt.py:188
+      }
+      if (bf16()) ensure_stats<T>(X, S.dp, stats, M, s);               // the first block's PreNorm statistics
+      for (const CvtBlockW& b : S.blocks) cvt_block<T>(X, B, oh, ow, b, stats, s);
+      map = X; mh = oh; mw = ow; mc = S.dim; ld_in = S.dp;
+    }
+    const int dl = cv.emb_dim[VB_CVT_STAGES - 1];
+    float* z = arena.get<float>(static_cast<size_t>(B) * dl);
+    {
+      ProfScope ps(this, PROF_LN, 1.0 * B * mh * mw * dl, static_cast<double>(sizeof(T)) * B * mh * mw * dl, s);
+      pool_layernorm<T>(X, mh * mw, ld_in, nullptr, nullptr, z, B, dl, 1, s);   // GlobalAvgPool2D cvt.py:196
+    }
+    gemm_simt<float, float, float>(z, dl, head.W, head.N, 1, logits, head.N, B, head.N, dl, head.bias, nullptr, nullptr, head.N, 0, s);
+  }
+  // One CvT layer (cvt.py:144-145): x = attn(LN(x)) + x; x = mlp(LN(x)) + x, in place on X [B*H*W, dp].  bf16: `stats` holds the
+  // (sum, sumsq) partials of X's rows on entry and on exit (emitted by the residual epilogues), and the depthwise kernel and fc1
+  // apply the LayerNorms from them; fp32: separate LayerNorms.
+  template <typename T>
+  void cvt_block(T* X, int B, int H, int Wd, const CvtBlockW& b, float* stats, cudaStream_t s) {
+    const int dp = b.dp, HD = 64 * b.heads, st = b.kv_stride;
+    const int Ho = (H + st - 1) / st, Wo = (Wd + st - 1) / st, M = B * H * Wd, Mk = B * Ho * Wo;
+    T* Qd = arena.get<T>(static_cast<size_t>(M) * dp);
+    T* KVd = arena.get<T>(static_cast<size_t>(Mk) * dp);
+    T* Y = bf16() ? nullptr : arena.get<T>(static_cast<size_t>(M) * dp);
+    if (Y != nullptr) {                                                 // fp32: PreNorm LayerNorm of the attention (cvt.py:53)
+      ProfScope ps(this, PROF_LN, 8.0 * M * b.dim, 2.0 * sizeof(T) * M * dp, s);
+      layernorm<T>(X, dp, b.attn_norm.gamma, b.attn_norm.beta, Y, dp, M, b.dim, s, dp, 1e-5f);
+    }
+    {
+      ProfScope ps(this, PROF_OTHER, 2.0 * b.k * b.k * b.dim * (static_cast<double>(M) + Mk),
+                   static_cast<double>(sizeof(T)) * dp * (2.0 * M + Mk) + (stats ? 8.0 * M * (dp / 64) : 0.0), s);
+      dwconv_qkv<T>(Y ? Y : X, dp, Y ? nullptr : stats, b.attn_norm.gamma, b.attn_norm.beta, b.dim, 1e-5f, b.wq, b.bq, Qd, dp, b.wkv, b.bkv,
+                    KVd, dp, B, H, Wd, dp, b.k, st, s);
+    }
+    T* Q = arena.get<T>(static_cast<size_t>(M) * HD);
+    T* KV = arena.get<T>(static_cast<size_t>(Mk) * 2 * HD);
+    linear<T>(Qd, dp, M, b.pw_q, Q, HD, Epi(), s);                      // cvt.py:86 (no bias)
+    linear<T>(KVd, dp, Mk, b.pw_kv, KV, 2 * HD, Epi(), s);
+    T* O = arena.get<T>(static_cast<size_t>(M) * HD);
+    attention_dispatch<T>(Q, HD, KV, 2 * HD, KV + HD, 2 * HD, O, HD, B, H * Wd, Ho * Wo, b.heads, 64, 0, nullptr, nullptr, nullptr, nullptr, s);
+    Epi eo; eo.bias = b.to_out.bias; eo.res = X; eo.ldr = dp; eo.stats_out = stats;
+    linear<T>(O, HD, M, b.to_out, X, dp, eo, s);
+    const T* fin = X;
+    if (Y != nullptr) {
+      ProfScope ps(this, PROF_LN, 8.0 * M * b.dim, 2.0 * sizeof(T) * M * dp, s);
+      layernorm<T>(X, dp, b.ff_norm.gamma, b.ff_norm.beta, Y, dp, M, b.dim, s, dp, 1e-5f);
+      fin = Y;
+    }
+    T* Hb = arena.get<T>(static_cast<size_t>(M) * b.fc1.N);
+    Epi e1; e1.gelu = true;
+    if (Y == nullptr) { e1.bias = b.fc1.ln_c2; e1.ln_stats = stats; } else { e1.bias = b.fc1.bias; }
+    linear<T>(fin, dp, M, b.fc1, Hb, b.fc1.N, e1, s);
+    Epi e2; e2.bias = b.fc2.bias; e2.res = X; e2.ldr = dp; e2.stats_out = stats;
+    linear<T>(Hb, b.fc1.N, M, b.fc2, X, dp, e2, s);
+  }
+
   // DistillMixin.call (distill.py:16-45) on top of a ViT: embed -> append the distillation token as the LAST row ->
   // transformer over n + 2 rows -> head on the first n + 1 rows, and the last row returned as is.
   template <typename T>
@@ -1598,6 +1798,7 @@ struct vb_handle {
     VB_CHECK(cfg.kind != VB_KIND_CROSSVIT, "CrossViT has two token streams: no single embedding stage");
     VB_CHECK(cfg.kind != VB_KIND_CCT, kCctNoStages);
     VB_CHECK(cfg.kind != VB_KIND_LEVIT, kLevitNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_CVT, kCvtNoStages);
     if (cfg.kind == VB_KIND_T2T_VIT) {
       int h = H, w = Wd;
       for (const auto& st : t2t_stages()) { h = (h + st.stride - 1) / st.stride; w = (w + st.stride - 1) / st.stride; }
@@ -1624,6 +1825,7 @@ struct vb_handle {
     VB_CHECK(cfg.kind != VB_KIND_CROSSVIT, "CrossViT sums two heads: no single mlp_head stage");
     VB_CHECK(cfg.kind != VB_KIND_CCT, kCctNoStages);
     VB_CHECK(cfg.kind != VB_KIND_LEVIT, kLevitNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_CVT, kCvtNoStages);
     arena.reset();
     const long long count = static_cast<long long>(B) * n * cfg.dim;
     T* X = arena.get<T>(count);
@@ -1636,6 +1838,7 @@ struct vb_handle {
     VB_CHECK(cfg.kind != VB_KIND_CROSSVIT, "CrossViT has two patch embeddings");
     VB_CHECK(cfg.kind != VB_KIND_CCT, kCctNoStages);
     VB_CHECK(cfg.kind != VB_KIND_LEVIT, kLevitNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_CVT, kCvtNoStages);
     arena.reset();
     const int K = embed.patch.K, Kp = bf16() ? embed.patch.ldw : K;
     T* col = arena.get<T>(static_cast<size_t>(rows) * Kp);
@@ -1680,7 +1883,8 @@ void vb_handle::linear<__nv_bfloat16>(const __nv_bfloat16* A, int lda, int M, co
     if (it == plans.end()) {
       if (plans.size() > 8192) plans.clear();      // shape sweeps: bounded host memory (a plan is four 128-byte tensor maps)
       GemmBf16 g = gemm_bf16_plan(A, lda, L.Wt, L.ldw, out, ldc, M, L.N, K, e.bias, e.scale, res, e.ldr, e.act());
-      if (folded) { g.ln_c1 = L.ln_c1; g.ln_stats = e.ln_stats; g.ln_parts = K / 64; g.ln_inv_d = 1.0f / static_cast<float>(K); }
+      if (folded) { g.ln_c1 = L.ln_c1; g.ln_stats = e.ln_stats; g.ln_parts = K / 64; g.ln_inv_d = 1.0f / static_cast<float>(L.ln_d > 0 ? L.ln_d : K);
+                    g.ln_eps = L.ln_eps; }
       if (e.stats_out) { g.stats_out = e.stats_out; }
       it = plans.emplace(key, g).first;
     }
@@ -1806,6 +2010,7 @@ void validate(const vb_config& c) {
   VB_CHECK(c.struct_size == static_cast<int32_t>(sizeof(vb_config)) || c.struct_size == VB_CONFIG_SIZE_ABI7,
            "vb_config.struct_size mismatch (ABI)");
   VB_CHECK(c.kind != VB_KIND_LEVIT, "LeViT: create the handle with vb_create_levit (its stages are a vb_levit_config)");
+  VB_CHECK(c.kind != VB_KIND_CVT, "CvT: create the handle with vb_create_cvt (its stages are a vb_cvt_config)");
   VB_CHECK(c.kind >= VB_KIND_VIT && c.kind <= VB_KIND_CCT, "unknown model kind");
   if (c.kind == VB_KIND_CCT) {
     VB_CHECK(c.channels == 3 && c.num_classes > 0 && c.image_h > 0 && c.image_w > 0, "bad image / class configuration");
@@ -1862,6 +2067,17 @@ void validate_levit(const vb_config& c, const vb_levit_config& lv) {
   VB_CHECK(c.image_h >= 16 && f == c.image_h / 16,
            "LeViT: image_size " + std::to_string(c.image_h) + " gives a " + std::to_string(f) + " x " + std::to_string(f) +
            " map after the stem but position biases for image_size // 16 = " + std::to_string(c.image_h / 16));
+}
+
+void validate_cvt(const vb_config& c, const vb_cvt_config& cv) {
+  VB_CHECK(c.precision == VB_PRECISION_FP32 || c.precision == VB_PRECISION_BF16, "unknown precision");
+  VB_CHECK(c.channels > 0 && c.num_classes > 0, "CvT: bad channel / class configuration");
+  for (int st = 0; st < VB_CVT_STAGES; ++st) {
+    VB_CHECK(cv.emb_dim[st] > 0 && cv.emb_kernel[st] > 0 && cv.emb_stride[st] > 0 && cv.heads[st] > 0 && cv.depth[st] >= 0 &&
+             cv.mlp_mult[st] > 0, "CvT: bad stage configuration");
+    VB_CHECK(cv.proj_kernel[st] >= 1 && cv.proj_kernel[st] <= 7, "CvT: proj_kernel must be in [1, 7] (the depthwise kernel's halo tile)");
+    VB_CHECK(cv.kv_proj_stride[st] == 1 || cv.kv_proj_stride[st] == 2, "CvT: kv_proj_stride must be 1 or 2");
+  }
 }
 
 }  // namespace
@@ -2013,6 +2229,35 @@ int vb_create_levit(const vb_config* base, const vb_levit_config* lv, int device
   });
 }
 
+int vb_create_cvt(const vb_config* base, const vb_cvt_config* cvt, int device, vb_handle** out) {
+  return guarded(nullptr, [&] {
+    VB_CHECK(base != nullptr && cvt != nullptr && out != nullptr, "vb_create_cvt: null argument");
+    VB_CHECK(base->struct_size == static_cast<int32_t>(sizeof(vb_config)) || base->struct_size == VB_CONFIG_SIZE_ABI7,
+             "vb_config.struct_size mismatch (ABI)");
+    VB_CHECK(cvt->struct_size == static_cast<int32_t>(sizeof(vb_cvt_config)), "vb_cvt_config.struct_size mismatch (ABI)");
+    vb_config c;
+    memset(&c, 0, sizeof c);
+    memcpy(&c, base, static_cast<size_t>(base->struct_size));
+    VB_CHECK(c.kind == VB_KIND_CVT, "vb_create_cvt: base.kind must be VB_KIND_CVT");
+    validate_cvt(c, *cvt);
+    int ndev = 0;
+    cudaError_t e = cudaGetDeviceCount(&ndev);
+    VB_CHECK(e == cudaSuccess && ndev > 0, "vb_create_cvt: no CUDA device available -- libvitb200 has no CPU fallback");
+    VB_CHECK(device >= 0 && device < ndev, "vb_create_cvt: bad device index");
+    VB_CUDA(cudaSetDevice(device));
+    cudaDeviceProp prop;
+    VB_CUDA(cudaGetDeviceProperties(&prop, device));
+    VB_CHECK(prop.major == 9 && prop.minor == 0, "vb_create_cvt: libvitb200 is built for sm_90a (Hopper H100) only");
+    std::unique_ptr<vb_handle> h(new vb_handle());
+    h->cfg = c;
+    h->cfg.dim = cvt->emb_dim[VB_CVT_STAGES - 1];
+    h->cv = *cvt;
+    h->device = device;
+    h->build_expected();
+    *out = h.release();
+  });
+}
+
 int vb_num_weights(vb_handle* h) { return h ? static_cast<int>(h->weights.size()) : -1; }
 
 int vb_weight_info(vb_handle* h, int32_t index, const char** name, int64_t* shape4, int32_t* ndim) {
@@ -2136,6 +2381,7 @@ int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, int32_t 
     VB_CHECK(h != nullptr && img != nullptr && logits != nullptr && distill_out != nullptr, "vb_forward_distill: null argument");
     VB_CHECK(h->finalized, "vb_forward_distill: call vb_finalize after setting the weights");
     VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_forward_distill: bad batch / image size");
+    VB_CHECK(h->cfg.kind != VB_KIND_CVT, "vb_forward_distill: CvT has no distillation head");
     const bool levit = h->cfg.kind == VB_KIND_LEVIT;
     VB_CHECK(levit || distill_token != nullptr, "vb_forward_distill: null argument");
     VB_CHECK(!levit || (distill_token == nullptr && h->lv.num_distill_classes > 0),
@@ -2191,6 +2437,7 @@ int vb_forward_tokens(vb_handle* h, const float* tokens, int32_t tokens_mem, int
     VB_CHECK(h != nullptr && tokens != nullptr && out != nullptr, "vb_forward_tokens: null argument");
     VB_CHECK(h->finalized, "vb_forward_tokens: call vb_finalize after setting the weights");
     VB_CHECK(batch > 0 && n > 0, "vb_forward_tokens: bad shape");
+    VB_CHECK(h->cfg.kind != VB_KIND_CVT, vb_handle::kCvtNoStages);
     VB_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const long long before = launch_counter();
@@ -2260,7 +2507,7 @@ int vb_to_patch(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, 
   return guarded(h, [&] {
     VB_CHECK(h != nullptr && img != nullptr && patches != nullptr, "vb_to_patch: null argument");
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT && h->cfg.kind != VB_KIND_T2T_VIT && h->cfg.kind != VB_KIND_CCT &&
-             h->cfg.kind != VB_KIND_LEVIT, "vb_to_patch: the model has no single Rearrange patch layer");
+             h->cfg.kind != VB_KIND_LEVIT && h->cfg.kind != VB_KIND_CVT, "vb_to_patch: the model has no single Rearrange patch layer");
     VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_to_patch: bad batch / image size");
     const vb_config& c = h->cfg;
     VB_CHECK(img_h % c.patch_h == 0 && img_w % c.patch_w == 0, "Image dimensions must be divisible by the patch size.");
@@ -2281,6 +2528,7 @@ int vb_patch_to_emb(vb_handle* h, const float* patches, int32_t patches_mem, int
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT, "vb_patch_to_emb: CrossViT has two patch embeddings");
     VB_CHECK(h->cfg.kind != VB_KIND_CCT, vb_handle::kCctNoStages);
     VB_CHECK(h->cfg.kind != VB_KIND_LEVIT, vb_handle::kLevitNoStages);
+    VB_CHECK(h->cfg.kind != VB_KIND_CVT, vb_handle::kCvtNoStages);
     VB_CHECK(rows > 0, "vb_patch_to_emb: bad shape");
     const size_t in_bytes = static_cast<size_t>(rows) * h->embed.patch.K * sizeof(float);
     const size_t out_bytes = static_cast<size_t>(rows) * h->cfg.dim * sizeof(float);
@@ -2653,6 +2901,70 @@ int vb_op_attention_bias(int32_t precision, const float* q, int32_t ldq, const f
     };
     if (precision == VB_PRECISION_FP32) run(float());
     else run(__nv_bfloat16());
+  });
+}
+
+int vb_op_dwconv(int32_t precision, const float* x, int32_t B, int32_t H, int32_t W, int32_t C, const float* ln_gamma, const float* ln_beta,
+                 int32_t k, int32_t kv_stride, const float* wq, const float* bn_q, const float* wkv, const float* bn_kv, float* q, float* kv,
+                 int32_t iters, float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    VB_CHECK(x && ln_gamma && ln_beta && wq && bn_q && wkv && bn_kv && q && kv && B > 0 && H > 0 && W > 0 && C > 0 && k >= 1 && k <= 7 &&
+             (kv_stride == 1 || kv_stride == 2), "vb_op_dwconv: bad arguments");
+    const bool bf = precision == VB_PRECISION_BF16;
+    const int Cp = bf ? round_up(C, 64) : C, Ho = (H + kv_stride - 1) / kv_stride, Wo = (W + kv_stride - 1) / kv_stride;
+    const size_t M = static_cast<size_t>(B) * H * W, Mk = static_cast<size_t>(B) * Ho * Wo;
+    auto vec = [](const float* p, size_t n) { return std::vector<double>(p, p + n); };
+    auto fold = [&](const float* w, const float* bn, std::vector<float>& taps, std::vector<float>& shift) {   // as vb_finalize folds
+      std::vector<double> wd, sd;
+      cvt_fold_dw(vec(w, static_cast<size_t>(k) * k * C), vec(bn, C), vec(bn + C, C), vec(bn + 2 * C, C), vec(bn + 3 * C, C), k, C, Cp, wd, sd);
+      taps.assign(wd.begin(), wd.end());
+      shift.assign(sd.begin(), sd.end());
+    };
+    std::vector<float> tq, sq, tkv, skv, xp(M * Cp, 0.f), gp(Cp, 0.f), bp(Cp, 0.f);
+    fold(wq, bn_q, tq, sq);
+    fold(wkv, bn_kv, tkv, skv);
+    for (size_t r = 0; r < M; ++r) std::copy(x + r * C, x + (r + 1) * C, xp.begin() + r * Cp);
+    std::copy(ln_gamma, ln_gamma + C, gp.begin());
+    std::copy(ln_beta, ln_beta + C, bp.begin());
+    DevMem dX, dG, dB, dTq, dSq, dTkv, dSkv, dQ, dKV, dS, dY;
+    const float* g_d = upload<float>(dG, gp.data(), Cp);
+    const float* b_d = upload<float>(dB, bp.data(), Cp);
+    const float* tq_d = upload<float>(dTq, tq.data(), tq.size());
+    const float* sq_d = upload<float>(dSq, sq.data(), sq.size());
+    const float* tkv_d = upload<float>(dTkv, tkv.data(), tkv.size());
+    const float* skv_d = upload<float>(dSkv, skv.data(), skv.size());
+    std::vector<float> qh(M * Cp), kvh(Mk * Cp);
+    auto run = [&](auto tag) {
+      using T = decltype(tag);
+      const T* x_d = upload<T>(dX, xp.data(), M * Cp);
+      dQ.ensure(M * Cp * sizeof(T));
+      dKV.ensure(Mk * Cp * sizeof(T));
+      T* q_d = static_cast<T*>(dQ.p);
+      T* kv_d = static_cast<T*>(dKV.p);
+      // vb_handle::cvt_block's depthwise step, without the handle's arena and profiler
+      if constexpr (std::is_same<T, __nv_bfloat16>::value) {
+        dS.ensure(M * (Cp / 64) * 2 * sizeof(float));
+        float* st = static_cast<float*>(dS.p);
+        timed(iters, elapsed_ms, [&] {
+          row_stats_bf16(x_d, Cp, st, static_cast<int>(M), Cp, 0);
+          dwconv_qkv<T>(x_d, Cp, st, g_d, b_d, C, 1e-5f, tq_d, sq_d, q_d, Cp, tkv_d, skv_d, kv_d, Cp, B, H, W, Cp, k, kv_stride, 0);
+        });
+      } else {
+        dY.ensure(M * Cp * sizeof(T));
+        T* y = static_cast<T*>(dY.p);
+        timed(iters, elapsed_ms, [&] {
+          layernorm<T>(x_d, Cp, g_d, b_d, y, Cp, static_cast<int>(M), C, 0, Cp, 1e-5f);
+          dwconv_qkv<T>(y, Cp, nullptr, nullptr, nullptr, C, 1e-5f, tq_d, sq_d, q_d, Cp, tkv_d, skv_d, kv_d, Cp, B, H, W, Cp, k, kv_stride, 0);
+        });
+      }
+      download<T>(q_d, qh.data(), M * Cp);
+      download<T>(kv_d, kvh.data(), Mk * Cp);
+    };
+    if (bf) run(__nv_bfloat16());
+    else run(float());
+    for (size_t r = 0; r < M; ++r) std::copy(qh.begin() + r * Cp, qh.begin() + r * Cp + C, q + r * C);
+    for (size_t r = 0; r < Mk; ++r) std::copy(kvh.begin() + r * Cp, kvh.begin() + r * Cp + C, kv + r * C);
   });
 }
 

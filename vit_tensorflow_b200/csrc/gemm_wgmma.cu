@@ -72,7 +72,7 @@ __global__ void __launch_bounds__(THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, int M, int N, int K,
                  void* __restrict__ out, int ldc, const float* __restrict__ bias, const float* __restrict__ scale,
                  const __nv_bfloat16* res, int ldr, const float* __restrict__ ln_c1, const float2* ln_stats, int ln_parts,
-                 float ln_inv_d, float2* __restrict__ stats_out) {
+                 float ln_inv_d, float ln_eps, float2* __restrict__ stats_out) {
   static_assert(!OF32 || (ACT == ACT_NONE && !RES && EPI != 2), "fp32 output: plain / bias epilogue only");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -166,7 +166,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         const float mu = s1[q] * ln_inv_d;
-        const float rstd = rsqrtf(fmaxf(s2[q] * ln_inv_d - mu * mu, 0.f) + 1e-3f);
+        const float rstd = rsqrtf(fmaxf(s2[q] * ln_inv_d - mu * mu, 0.f) + ln_eps);
         ln_rstd[q] = rstd;
         ln_nmr[q] = -mu * rstd;
       }
@@ -324,7 +324,7 @@ void launch(const GemmBf16& g, cudaStream_t stream) {
   cfg.numAttrs = 1;
   VB_CUDA(cudaLaunchKernelEx(&cfg, kern, g.tmap_a, g.tmap_b, g.M, g.N, g.K, static_cast<void*>(g.out), g.ldc, g.bias, g.scale, g.res,
                              g.ldr, g.ln_c1, reinterpret_cast<const float2*>(g.ln_stats), g.ln_parts, g.ln_inv_d,
-                             reinterpret_cast<float2*>(g.stats_out)));
+                             g.ln_eps, reinterpret_cast<float2*>(g.stats_out)));
   count_launch();
 }
 

@@ -114,7 +114,7 @@ __global__ void embed_residual_kernel(T* __restrict__ R, const float* __restrict
 // One warp per row, row cached in registers (8-element chunks: 16-byte bf16 / 2x16-byte fp32 accesses).
 template <typename T, int MAXC>
 __global__ void layernorm_kernel(const T* __restrict__ x, int ldx, const float* __restrict__ gamma, const float* __restrict__ beta,
-                                 T* __restrict__ out, int ldo, int M, int D) {
+                                 T* __restrict__ out, int ldo, int M, int D, float eps) {
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= M) return;
   const int lane = threadIdx.x & 31;
@@ -153,7 +153,7 @@ __global__ void layernorm_kernel(const T* __restrict__ x, int ldx, const float* 
       for (int j = 0; j < 8; ++j) { const float d = v[i][j] - mean; sq += d * d; }
     }
   }
-  const float rstd = rsqrtf(warp_sum(sq) / D + 1e-3f);
+  const float rstd = rsqrtf(warp_sum(sq) / D + eps);
   T* orow = out + static_cast<long long>(row) * ldo;
 #pragma unroll
   for (int i = 0; i < MAXC; ++i) {
@@ -186,7 +186,8 @@ __global__ void layernorm_kernel(const T* __restrict__ x, int ldx, const float* 
 // Any D / alignment: one warp per row, three passes over the (L1-resident) row.
 template <typename T>
 __global__ void layernorm_generic_kernel(const T* __restrict__ x, int ldx, const float* __restrict__ gamma,
-                                         const float* __restrict__ beta, T* __restrict__ out, int ldo, int M, int D, int pad_to) {
+                                         const float* __restrict__ beta, T* __restrict__ out, int ldo, int M, int D, int pad_to,
+                                         float eps) {
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= M) return;
   const int lane = threadIdx.x & 31;
@@ -196,7 +197,7 @@ __global__ void layernorm_generic_kernel(const T* __restrict__ x, int ldx, const
   const float mean = warp_sum(sum) / D;
   float sq = 0.f;
   for (int d = lane; d < D; d += 32) { const float t = to_f(xr[d]) - mean; sq += t * t; }
-  const float rstd = rsqrtf(warp_sum(sq) / D + 1e-3f);
+  const float rstd = rsqrtf(warp_sum(sq) / D + eps);
   T* orow = out + static_cast<long long>(row) * ldo;
   for (int d = lane; d < D; d += 32) orow[d] = from_f<T>((to_f(xr[d]) - mean) * rstd * gamma[d] + beta[d]);
   for (int d = D + lane; d < pad_to; d += 32) orow[d] = from_f<T>(0.f);     // zero pad columns [D, pad_to) (pitch-padded token rows)
@@ -852,6 +853,123 @@ __global__ void pad_heads_kernel(const float* __restrict__ W, float* __restrict_
   }
 }
 
+// ------------------------------------------------------------------------------------------ CvT depthwise convolutions
+// One CTA: a DW_T x DW_T tile of the stride-1 (q) output map x DW_CG channels of one image.  The input tile with its halo
+// (DW_T + K - 1 square, zero outside the map) is read once into shared memory -- LayerNormed on load from the rows' (sum,
+// sumsq) partials when `stats` is given, so the halo holds zeros of the NORMALISED map, as the reference's SAME padding of
+// LN(x) does -- and both convolutions read it: warp w computes row w of the q tile (DW_T outputs per lane, one channel per
+// lane), and for the k|v map the outputs r whose 2r (stride 2) or r (stride 1) falls in the tile.  With TF SAME padding the
+// stride-2 map's top / left padding is the stride-1 one's or one less (kv_dy / kv_dx), so its windows lie inside the halo.
+constexpr int DW_T = 8, DW_CG = 32, DW_THREADS = DW_CG * DW_T, DW_MAXK = 7;
+// One row of DW_T stride-1 outputs of lane's channel: tile rows row .. row + K - 1; out points at the row's first output, n_valid
+// of them inside the map.
+template <typename T, int K>
+__device__ __forceinline__ void dw_conv_row(const float (*tile)[DW_CG], const float (*taps)[DW_CG], float shift, T* out, int ld, int row,
+                                            int lane, int n_valid) {
+  constexpr int TS = DW_T + K - 1;
+  float acc[DW_T];
+#pragma unroll
+  for (int xx = 0; xx < DW_T; ++xx) acc[xx] = 0.f;
+#pragma unroll
+  for (int i = 0; i < K; ++i) {
+    float xr[TS];
+#pragma unroll
+    for (int j = 0; j < TS; ++j) xr[j] = tile[(row + i) * TS + j][lane];
+#pragma unroll
+    for (int j = 0; j < K; ++j) {
+      const float w = taps[i * K + j][lane];
+#pragma unroll
+      for (int xx = 0; xx < DW_T; ++xx) acc[xx] = fmaf(xr[xx + j], w, acc[xx]);
+    }
+  }
+#pragma unroll
+  for (int xx = 0; xx < DW_T; ++xx)
+    if (xx < n_valid) out[static_cast<long long>(xx) * ld] = from_f<T>(acc[xx] + shift);
+}
+template <typename T, int K>
+__global__ void __launch_bounds__(DW_THREADS)
+dwconv_qkv_kernel(const T* __restrict__ x, int ldx, const float2* __restrict__ stats, int parts, const float* __restrict__ gamma,
+                  const float* __restrict__ beta, float inv_d, float eps, const float* __restrict__ wq, const float* __restrict__ bq,
+                  T* __restrict__ q, int ldq, const float* __restrict__ wkv, const float* __restrict__ bkv, T* __restrict__ kv, int ldkv,
+                  int H, int W, int C, int kv_stride, int Ho, int Wo, int kv_dy, int kv_dx, int tiles_x, int tiles_y, int groups,
+                  long long M) {
+  constexpr int TS = DW_T + K - 1, P = TS * TS, PAD = (K - 1) / 2;
+  __shared__ float tile[P][DW_CG];
+  __shared__ float mu_s[P], rs_s[P];
+  __shared__ float tq[K * K][DW_CG], tkv[K * K][DW_CG];
+  long long bid = blockIdx.x;
+  const int tx = static_cast<int>(bid % tiles_x); bid /= tiles_x;
+  const int ty = static_cast<int>(bid % tiles_y); bid /= tiles_y;
+  const int g = static_cast<int>(bid % groups);
+  const long long b = bid / groups;
+  const int y0 = ty * DW_T, x0 = tx * DW_T, c0 = g * DW_CG;
+  const int lane = threadIdx.x & 31, row = threadIdx.x >> 5;
+  const int c = c0 + lane;
+  const bool cok = c < C;
+  for (int i = threadIdx.x; i < K * K * DW_CG; i += DW_THREADS) {
+    const int t = i / DW_CG, cc = c0 + i % DW_CG;
+    tq[t][i % DW_CG] = cc < C ? __ldg(wq + static_cast<size_t>(t) * C + cc) : 0.f;
+    tkv[t][i % DW_CG] = cc < C ? __ldg(wkv + static_cast<size_t>(t) * C + cc) : 0.f;
+  }
+  if (stats != nullptr) {
+    for (int p = threadIdx.x; p < P; p += DW_THREADS) {
+      const int iy = y0 - PAD + p / TS, ix = x0 - PAD + p % TS;
+      float m = 0.f, r = 0.f;
+      if (iy >= 0 && iy < H && ix >= 0 && ix < W) {
+        const long long pix = (b * H + iy) * W + ix;
+        float s1 = 0.f, s2 = 0.f;
+        for (int j = 0; j < parts; ++j) {
+          const float2 v = __ldg(stats + j * M + pix);
+          s1 += v.x;
+          s2 += v.y;
+        }
+        m = s1 * inv_d;
+        r = rsqrtf(fmaxf(s2 * inv_d - m * m, 0.f) + eps);
+      }
+      mu_s[p] = m;
+      rs_s[p] = r;
+    }
+    __syncthreads();
+  }
+  const float ga = (stats != nullptr && cok) ? __ldg(gamma + c) : 1.f, be = (stats != nullptr && cok) ? __ldg(beta + c) : 0.f;
+  for (int p = row; p < P; p += DW_T) {
+    const int iy = y0 - PAD + p / TS, ix = x0 - PAD + p % TS;
+    float v = 0.f;
+    if (cok && iy >= 0 && iy < H && ix >= 0 && ix < W) {
+      v = to_f(x[((b * H + iy) * W + ix) * ldx + c]);
+      if (stats != nullptr) v = (v - mu_s[p]) * rs_s[p] * ga + be;
+    }
+    tile[p][lane] = v;
+  }
+  __syncthreads();
+  const int oy = y0 + row;
+  if (oy < H && cok) dw_conv_row<T, K>(tile, tq, bq[c], q + ((b * H + oy) * W + x0) * ldq + c, ldq, row, lane, W - x0);
+  if (kv_stride == 1) {
+    if (oy < H && cok) dw_conv_row<T, K>(tile, tkv, bkv[c], kv + ((b * H + oy) * W + x0) * ldkv + c, ldkv, row, lane, W - x0);
+  } else if (row < DW_T / 2 && cok) {                            // stride 2: outputs (y0/2 + row, x0/2 + xx), xx < DW_T/2
+    const int r = y0 / 2 + row;
+    if (r < Ho) {
+      float acc[DW_T / 2];
+#pragma unroll
+      for (int xx = 0; xx < DW_T / 2; ++xx) acc[xx] = 0.f;
+#pragma unroll
+      for (int i = 0; i < K; ++i) {
+        const int tr = (2 * row + kv_dy + i) * TS + kv_dx;
+#pragma unroll
+        for (int j = 0; j < K; ++j) {
+          const float w = tkv[i * K + j][lane];
+#pragma unroll
+          for (int xx = 0; xx < DW_T / 2; ++xx) acc[xx] = fmaf(tile[tr + 2 * xx + j][lane], w, acc[xx]);
+        }
+      }
+      const float sh = __ldg(bkv + c);
+#pragma unroll
+      for (int xx = 0; xx < DW_T / 2; ++xx)
+        if (x0 / 2 + xx < Wo) kv[((b * Ho + r) * Wo + x0 / 2 + xx) * ldkv + c] = from_f<T>(acc[xx] + sh);
+    }
+  }
+}
+
 inline int grid_1d(long long total, int block = 256) {
   long long g = (total + block - 1) / block;
   const long long cap = static_cast<long long>(sm_count()) * 16;
@@ -913,18 +1031,19 @@ void build_embed_residual(T* R, const float* pos, const float* cls, const float*
 }
 
 template <typename T>
-void layernorm(const T* x, int ldx, const float* gamma, const float* beta, T* out, int ldo, int M, int D, cudaStream_t s, int pad_to) {
+void layernorm(const T* x, int ldx, const float* gamma, const float* beta, T* out, int ldo, int M, int D, cudaStream_t s, int pad_to,
+               float eps) {
   const int warps = 8;
   const int blocks = (M + warps - 1) / warps;
   const bool aligned = (pad_to <= D) && (D % 8 == 0) && (ldx % 8 == 0) && (ldo % 8 == 0) &&
                        (reinterpret_cast<uintptr_t>(x) % 16 == 0) && (reinterpret_cast<uintptr_t>(out) % 16 == 0) &&
                        (reinterpret_cast<uintptr_t>(gamma) % 16 == 0) && (reinterpret_cast<uintptr_t>(beta) % 16 == 0);
   if (aligned && D <= 8 * 32 * 2) {
-    layernorm_kernel<T, 2><<<blocks, warps * 32, 0, s>>>(x, ldx, gamma, beta, out, ldo, M, D);
+    layernorm_kernel<T, 2><<<blocks, warps * 32, 0, s>>>(x, ldx, gamma, beta, out, ldo, M, D, eps);
   } else if (aligned && D <= 8 * 32 * 4) {
-    layernorm_kernel<T, 4><<<blocks, warps * 32, 0, s>>>(x, ldx, gamma, beta, out, ldo, M, D);
+    layernorm_kernel<T, 4><<<blocks, warps * 32, 0, s>>>(x, ldx, gamma, beta, out, ldo, M, D, eps);
   } else {
-    layernorm_generic_kernel<T><<<blocks, warps * 32, 0, s>>>(x, ldx, gamma, beta, out, ldo, M, D, pad_to);
+    layernorm_generic_kernel<T><<<blocks, warps * 32, 0, s>>>(x, ldx, gamma, beta, out, ldo, M, D, pad_to, eps);
   }
   VB_LAUNCHED();
 }
@@ -1090,11 +1209,36 @@ void row_stats_bf16(const __nv_bfloat16* X, int ldx, float* stats, int M, int D,
   VB_LAUNCHED();
 }
 
+template <typename T>
+void dwconv_qkv(const T* x, int ldx, const float* stats, const float* gamma, const float* beta, int D, float eps, const float* wq,
+                const float* bq, T* q, int ldq, const float* wkv, const float* bkv, T* kv, int ldkv, int B, int H, int W, int C, int k,
+                int kv_stride, cudaStream_t s) {
+  VB_CHECK(k >= 1 && k <= DW_MAXK && (kv_stride == 1 || kv_stride == 2), "dwconv_qkv: kernel size 1..7 and stride 1 or 2 only");
+  VB_CHECK(stats == nullptr || C % 64 == 0, "dwconv_qkv: LayerNorm statistics need a channel width that is a multiple of 64");
+  const int Ho = (H + kv_stride - 1) / kv_stride, Wo = (W + kv_stride - 1) / kv_stride;
+  const int pad = (k - 1) / 2;
+  const int kv_dy = pad - std::max((Ho - 1) * kv_stride + k - H, 0) / 2, kv_dx = pad - std::max((Wo - 1) * kv_stride + k - W, 0) / 2;
+  VB_CHECK(kv_dy >= 0 && kv_dy <= 1 && kv_dx >= 0 && kv_dx <= 1, "dwconv_qkv: internal: k|v window outside the tile halo");
+  const int tiles_x = (W + DW_T - 1) / DW_T, tiles_y = (H + DW_T - 1) / DW_T, groups = (C + DW_CG - 1) / DW_CG;
+  const unsigned grid = flat_blocks(static_cast<long long>(tiles_x) * tiles_y * groups, B, "dwconv_qkv");
+  const long long M = static_cast<long long>(B) * H * W;
+  const float2* st = reinterpret_cast<const float2*>(stats);
+#define VB_DW_CASE(KS)                                                                                                        \
+  case KS:                                                                                                                    \
+    dwconv_qkv_kernel<T, KS><<<grid, DW_THREADS, 0, s>>>(x, ldx, st, C / 64, gamma, beta, 1.0f / static_cast<float>(D), eps, wq, bq, \
+                                                         q, ldq, wkv, bkv, kv, ldkv, H, W, C, kv_stride, Ho, Wo, kv_dy, kv_dx,     \
+                                                         tiles_x, tiles_y, groups, M);                                        \
+    break;
+  switch (k) { VB_DW_CASE(1) VB_DW_CASE(2) VB_DW_CASE(3) VB_DW_CASE(4) VB_DW_CASE(5) VB_DW_CASE(6) VB_DW_CASE(7) }
+#undef VB_DW_CASE
+  VB_LAUNCHED();
+}
+
 // ------------------------------------------------------------------------------------------ instantiations
 #define VB_INST_T(T)                                                                                                         \
   template void im2col<T>(const float*, T*, int, int, int, int, int, int, int, int, cudaStream_t);                          \
   template void build_embed_residual<T>(T*, const float*, const float*, const float*, int, int, int, int, cudaStream_t);    \
-  template void layernorm<T>(const T*, int, const float*, const float*, T*, int, int, int, cudaStream_t, int);                   \
+  template void layernorm<T>(const T*, int, const float*, const float*, T*, int, int, int, cudaStream_t, int, float);            \
   template void attn_scores<T>(const T*, int, const T*, int, float*, int, int, int, int, int, float, cudaStream_t);         \
   template void attn_pv<T>(const float*, const T*, int, T*, int, int, int, int, int, int, cudaStream_t, int);               \
   template void gather_grid<T>(const T*, int, T*, int, int, int, int, int, int, cudaStream_t);                              \
@@ -1105,7 +1249,9 @@ void row_stats_bf16(const __nv_bfloat16* X, int ldx, float* stats, int M, int D,
   template void unfold_same<float, T>(const float*, T*, int, int, int, int, int, int, int, int, cudaStream_t, int);         \
   template void convert_rows<float, T>(const float*, int, T*, int, long long, int, cudaStream_t);                           \
   template void maxpool_relu_same<T>(const T*, T*, int, int, int, int, int, int, const float*, int, cudaStream_t);         \
-  template void seq_pool<T>(const T*, int, int, const float*, const float*, const float*, const float*, float*, int, cudaStream_t);
+  template void seq_pool<T>(const T*, int, int, const float*, const float*, const float*, const float*, float*, int, cudaStream_t); \
+  template void dwconv_qkv<T>(const T*, int, const float*, const float*, const float*, int, float, const float*, const float*, T*, int, \
+                              const float*, const float*, T*, int, int, int, int, int, int, int, cudaStream_t);
 VB_INST_T(float)
 VB_INST_T(__nv_bfloat16)
 

@@ -17,10 +17,12 @@ template <typename T>
 void build_embed_residual(T* R, const float* pos, const float* cls, const float* bias, int B, int rows, int dim,
                           int has_cls, cudaStream_t s);
 
-// LayerNorm over the last axis (Keras: eps 1e-3, biased variance; vit.py:18).  x [M, ldx] -> out [M, ldo].
-// pad_to > D: columns [D, pad_to) of every output row are zeroed (pitch-padded token rows feeding a K-padded GEMM).
+// LayerNorm over the last axis (biased variance; Keras eps 1e-3, vit.py:18; CvT's own LayerNorm eps 1e-5, cvt.py:30-43).
+// x [M, ldx] -> out [M, ldo].  pad_to > D: columns [D, pad_to) of every output row are zeroed (pitch-padded token rows feeding a
+// K-padded GEMM).
 template <typename T>
-void layernorm(const T* x, int ldx, const float* gamma, const float* beta, T* out, int ldo, int M, int D, cudaStream_t s, int pad_to = 0);
+void layernorm(const T* x, int ldx, const float* gamma, const float* beta, T* out, int ldo, int M, int D, cudaStream_t s, int pad_to = 0,
+               float eps = 1e-3f);
 
 // Row softmax of materialised fp32 scores -> bf16 probabilities: P[r, j] = softmax_j(S[r, j] * scale), j < n; P[r, n..npad) = 0.
 // scale_log2 = scale * log2(e).  Rows of up to 4096 keys stay in registers; longer rows take a three-pass kernel.
@@ -55,6 +57,18 @@ void attn_pos_bias(float* S, const PosBias& pb, int B, int heads, int nq, int nk
 // out [B, ceil(H/step) * ceil(W/step), C] rows of pitch ldo, out pixel (r, c) = in pixel (step*r, step*c).
 template <typename T>
 void gather_grid(const T* in, int ldi, T* out, int ldo, int B, int H, int W, int C, int step, cudaStream_t s);
+
+// CvT's attention projections up to the pointwise convolutions (cvt.py:79-92,103-104), both depthwise convolutions of a block
+// from one read of the input: q = dw_q(y) (stride 1) and kv = dw_kv(y) (stride kv_stride: 1 or 2), k x k (k <= 7), TF SAME
+// padding (total max((out - 1) * stride + k - in, 0), the smaller half first), then + a per-channel shift.
+//   x [B*H*W, ldx] NHWC rows; y = LN(x) when stats != null: the rows' (sum, sumsq) partials [C/64][B*H*W] (the GEMM epilogue's
+//   stats_out format) over D true columns with eps, times gamma plus beta ([C], zero on pad channels); y = x when stats == null.
+//   The padding is zeros of y.  wq / wkv: taps [k*k][C] (row-major window, BatchNorm scale folded in), bq / bkv: shifts [C].
+//   q [B*H*W, ldq], kv [B*ceil(H/s)*ceil(W/s), ldkv]: columns [0, C) written.
+template <typename T>
+void dwconv_qkv(const T* x, int ldx, const float* stats, const float* gamma, const float* beta, int D, float eps, const float* wq,
+                const float* bq, T* q, int ldq, const float* wkv, const float* bkv, T* kv, int ldkv, int B, int H, int W, int C, int k,
+                int kv_stride, cudaStream_t s);
 
 // z[b,:] = LN(pool(X[b]))  with pool = row 0 (cls) or mean over the n rows; fp32 out [B, D].  gamma == null: no LayerNorm.
 template <typename T>

@@ -5,6 +5,7 @@
     parallel_vit.ViT  parallel_vit.py:120-185        DistillableViT  distill.py:47-58 (forward)
     T2TViT    vit_tensorflow/t2t.py:50-116           vit_with_patch_merger.ViT / PatchMerger  vit_with_patch_merger.py:42-55,134-185
     efficient.ViT  vit_tensorflow/efficient.py:12-55 (injected transformer between the engine's embed and head stages)
+    CvT       vit_tensorflow/cvt.py:149-202
 
 Same constructor kwargs, defaults and assertion messages; `model(img, training=True, **kwargs) -> logits`
 with `img` NHWC float32 `[b, H, W, 3]` and logits float32 `[b, num_classes]`.  Everything below the call is
@@ -860,8 +861,127 @@ LEVIT_CTOR_KEYS = ("image_size", "num_classes", "dim", "depth", "heads", "mlp_mu
                    "num_distill_classes")
 
 
+CVT_STAGE_KEYS = ("emb_dim", "emb_kernel", "emb_stride", "proj_kernel", "kv_proj_stride", "heads", "depth", "mlp_mult")
+
+
+class CvT(_EngineModel):
+    """cvt.py:149-202: three stages of Conv2D (SAME) + channel LayerNorm + Transformer, whose attention projects q and k|v with
+    depthwise convolutions, BatchNormalization and 1x1 convolutions (heads of 64), then GlobalAvgPool2D and Dense.
+
+    Inference only: the reference's call defaults to training=True, which makes every BatchNormalization use the batch's statistics
+    and the dropout layers draw masks; a call without training=False raises NotImplementedError here.  There are no position
+    embeddings and no image_size: any h x w image runs.  proj_kernel must be in [1, 7] and kv_proj_stride 1 or 2.
+    Weights (SURVEY.md App. B) keep the reference's attribute paths: cvt_layers.{s}.0 (stem Conv2D), cvt_layers.{s}.1.g / .b
+    (LayerNorm), cvt_layers.{s}.2.layers.{l}.0.norm / .0.fn.to_q.net.{0,1,2} / .0.fn.to_kv.net.{0,1,2} / .0.fn.to_out.0,
+    cvt_layers.{s}.2.layers.{l}.1.norm / .1.fn.net.{0,3}, cvt_layers.3.1 (the Dense head)."""
+    _kind = "cvt"
+
+    def __init__(self,
+                 num_classes,
+                 s1_emb_dim=64,
+                 s1_emb_kernel=7,
+                 s1_emb_stride=4,
+                 s1_proj_kernel=3,
+                 s1_kv_proj_stride=2,
+                 s1_heads=1,
+                 s1_depth=1,
+                 s1_mlp_mult=4,
+                 s2_emb_dim=192,
+                 s2_emb_kernel=3,
+                 s2_emb_stride=2,
+                 s2_proj_kernel=3,
+                 s2_kv_proj_stride=2,
+                 s2_heads=3,
+                 s2_depth=2,
+                 s2_mlp_mult=4,
+                 s3_emb_dim=384,
+                 s3_emb_kernel=3,
+                 s3_emb_stride=2,
+                 s3_proj_kernel=3,
+                 s3_kv_proj_stride=2,
+                 s3_heads=6,
+                 s3_depth=10,
+                 s3_mlp_mult=4,
+                 dropout=0.,
+                 *, precision="bf16", device=0, seed=None):
+        kw = dict(locals())
+        self.num_classes = num_classes
+        self.stages = tuple({k: kw[f"s{i}_{k}"] for k in CVT_STAGE_KEYS} for i in (1, 2, 3))
+        self._dropout_rates = (dropout,)
+        for st in self.stages:
+            if not 1 <= st["proj_kernel"] <= 7:
+                raise ValueError(f"CvT: proj_kernel {st['proj_kernel']} is not supported (1 to 7)")
+            if st["kv_proj_stride"] not in (1, 2):
+                raise ValueError(f"CvT: kv_proj_stride {st['kv_proj_stride']} is not supported (1 or 2)")
+        self.precision = precision
+        self.device = int(device)
+        cfg = _lib.VbConfig()
+        cfg.struct_size = C.sizeof(_lib.VbConfig)
+        cfg.kind = _lib.KIND["cvt"]
+        if precision not in _lib.PRECISION:
+            raise ValueError(f"precision must be one of {sorted(_lib.PRECISION)}")
+        cfg.precision = _lib.PRECISION[precision]
+        cfg.channels, cfg.num_classes = 3, num_classes
+        cfg.dim = self.stages[-1]["emb_dim"]
+        cv = _lib.VbCvtConfig()
+        cv.struct_size = C.sizeof(_lib.VbCvtConfig)
+        for i, st in enumerate(self.stages):
+            for k in CVT_STAGE_KEYS:
+                getattr(cv, k)[i] = int(st[k])
+        self._cfg, self._cv = cfg, cv
+        self._lib = _lib.load()
+        h = C.c_void_p()
+        _lib.check(self._lib.vb_create_cvt(C.byref(cfg), C.byref(cv), self.device, C.byref(h)))
+        self._h = h
+        self._finalized = False
+        self._specs = collections.OrderedDict()
+        name, shape, ndim = C.c_char_p(), (C.c_int64 * 4)(), C.c_int32()
+        for i in range(self._lib.vb_num_weights(h)):
+            _lib.check(self._lib.vb_weight_info(h, i, C.byref(name), shape, C.byref(ndim)), h)
+            self._specs[name.value.decode()] = tuple(int(shape[j]) for j in range(ndim.value))
+        self._weights = collections.OrderedDict()
+        self.init_weights(seed)
+
+    def init_weights(self, seed=None):
+        """The reference's initialisers: glorot-uniform over the receptive field (a depthwise kernel [k, k, 1, dim] has fan_in k^2 and
+        fan_out k^2 * dim) and zero biases, BatchNormalization gamma 1 / beta 0 / moving statistics 0 and 1, LayerNorm g 1 / b 0."""
+        rng = np.random.default_rng(seed)
+        w = collections.OrderedDict()
+        for name, shape in self._specs.items():
+            leaf = name.rsplit(".", 1)[-1]
+            if leaf == "kernel":
+                receptive = int(np.prod(shape[:-2]))
+                lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
+                a = rng.uniform(-lim, lim, size=shape)
+            elif leaf in ("bias", "beta", "moving_mean", "b"):
+                a = np.zeros(shape)
+            elif leaf in ("gamma", "moving_variance", "g"):
+                a = np.ones(shape)
+            else:
+                raise AssertionError(name)
+            w[name] = a.astype(np.float32)
+        self.set_weights_dict(w)
+
+    def _check_training(self, training):
+        if training is None or training:
+            raise NotImplementedError(
+                "CvT runs inference only: with training=True (the reference's default, cvt.py:200) every BatchNormalization "
+                "normalises with the batch's own statistics and dropout draws masks; pass training=False")
+
+    def __call__(self, img, training=True, **kwargs):
+        """cvt.py:200: NHWC float images of any size -> logits [b, num_classes].  training must be False."""
+        return super().__call__(img, training=training)
+
+    call = __call__
+
+
+CVT_CTOR_KEYS = ("num_classes",) + tuple(f"s{i}_{k}" for i in (1, 2, 3) for k in CVT_STAGE_KEYS) + ("dropout",)
+
+
 def from_config(cfg: dict, precision="bf16", device=0, seed=None):
     """Build a model from an oracle-style config dict (kind + reference kwargs)."""
+    if cfg["kind"] == "cvt":
+        return CvT(**{k: v for k, v in cfg.items() if k in CVT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "levit":
         return LeViT(**{k: v for k, v in cfg.items() if k in LEVIT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "cct":
