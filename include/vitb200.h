@@ -12,6 +12,7 @@
  *     efficient.ViT(...)(img)        vit_tensorflow/efficient.py:13-14,39-55 = vb_forward_embed -> caller's transformer -> vb_forward_head
  *     LeViT(...)(img)                vit_tensorflow/levit.py:164-226 (vb_create_levit; distillation head: vb_forward_distill)
  *     CvT(...)(img)                  vit_tensorflow/cvt.py:149-202 (vb_create_cvt)
+ *     TwinsSVT(...)(img)             vit_tensorflow/twins_svt.py:215-268 (vb_create_twins_svt)
  * and this header is what the Python host classes (vit_tensorflow_b200/models.py, _lib.py) bind with ctypes.
  * Plain pointers and sizes only; no torch / C++ types cross the boundary.
  *
@@ -42,7 +43,7 @@ typedef struct vb_handle vb_handle;
 
 enum { VB_KIND_VIT = 0, VB_KIND_DEEPVIT = 1, VB_KIND_CAIT = 2, VB_KIND_CROSSVIT = 3, VB_KIND_PARALLEL_VIT = 4,
        VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6, VB_KIND_CCT = 7, VB_KIND_LEVIT = 8,
-       VB_KIND_CVT = 9 };
+       VB_KIND_CVT = 9, VB_KIND_TWINS_SVT = 10 };
 enum { VB_CCT_POS_SINE = 0, VB_CCT_POS_LEARNABLE = 1, VB_CCT_POS_NONE = 2 };   /* cct.py:233-234,250-256 */
 enum { VB_PRECISION_FP32 = 0, VB_PRECISION_BF16 = 1 };
 enum { VB_POOL_CLS = 0, VB_POOL_MEAN = 1 };
@@ -86,8 +87,8 @@ typedef struct vb_config {
 
 VB_API int vb_abi_version(void);
 
-/* Replaces <Model>.__init__ (vit.py:107-157 etc.): validates the config and allocates device state.  VB_KIND_LEVIT and
- * VB_KIND_CVT are refused here: their handles come from vb_create_levit and vb_create_cvt. */
+/* Replaces <Model>.__init__ (vit.py:107-157 etc.): validates the config and allocates device state.  VB_KIND_LEVIT, VB_KIND_CVT
+ * and VB_KIND_TWINS_SVT are refused here: their handles come from vb_create_levit, vb_create_cvt and vb_create_twins_svt. */
 VB_API int vb_create(const vb_config* cfg, int device, vb_handle** out);
 
 /* LeViT (levit.py:164-212), appended within ABI 7.  `dims`, `depths` and `heads` hold `stages` entries each (cast_tuple already
@@ -139,6 +140,32 @@ typedef struct vb_cvt_config {
  * per-channel shift. */
 VB_API int vb_create_cvt(const vb_config* base, const vb_cvt_config* cvt, int device, vb_handle** out);
 
+/* Twins-SVT (twins_svt.py:215-268), appended within ABI 7: the reference's four stages s1 .. s4 (index 0 .. 3).  Stage s is
+ * PatchEmbedding ('b (h p1) (w p2) c -> b h w (c p1 p2)', then a 1x1 Conv2D with bias), Transformer(depth 1), PEG (x + a
+ * depthwise peg_kernel_size SAME Conv2D with bias), Transformer(depth[s]).  A Transformer layer is x = x + f(LN(x)) for f = local
+ * attention within local_patch_size windows, MLP, global attention against the keys of a Conv2D(global_k, stride global_k, VALID),
+ * MLP; stage 4 has no local attention and no first MLP (has_local=False, :255).  Every stage has 8 heads of 64 and an MLP
+ * multiplier of 4 (Transformer is never passed them, :254-258); the LayerNorm is the module's own (eps 1e-5, :45-58).  Head:
+ * GlobalAvgPool2D -> Dense(num_classes).  No position embeddings: any image whose maps are divisible by each patch_size and, in
+ * stages 1-3, local_patch_size, and are at least global_k on each side. */
+#define VB_TWINS_STAGES 4
+typedef struct vb_twins_svt_config {
+  int32_t struct_size;            /* sizeof(vb_twins_svt_config) */
+  int32_t emb_dim[VB_TWINS_STAGES], patch_size[VB_TWINS_STAGES], local_patch_size[VB_TWINS_STAGES], global_k[VB_TWINS_STAGES];
+  int32_t depth[VB_TWINS_STAGES];
+  int32_t peg_kernel_size;        /* 1 .. 7 */
+} vb_twins_svt_config;
+
+/* TwinsSVT.__init__: `base` supplies precision, channels, num_classes and max_batch; its kind must be VB_KIND_TWINS_SVT and its
+ * other fields are ignored.  Weights (SURVEY.md App. B) are named by the reference's attribute paths, for stage s and layer l:
+ * svt_layers.{s}.0.proj.kernel [1, 1, cin * p^2, emb_dim] / .bias (the c-slowest patch vector), svt_layers.{s}.{1|3}.layers.{l}.{0|1|2|3}
+ * .fn.norm.g / .b [1, 1, 1, emb_dim] (0 local attention, 1 and 3 MLPs, 2 global attention), ....0.fn.fn.to_q.kernel [1, 1, emb_dim,
+ * 512], ....0.fn.fn.to_kv.kernel [1, 1, emb_dim, 1024], ....{0|2}.fn.fn.to_out.0.kernel [1, 1, 512, emb_dim] / .bias,
+ * ....{1|3}.fn.fn.net.0.kernel [1, 1, emb_dim, 4 emb_dim] / .bias, ....net.3.kernel / .bias, ....2.fn.fn.to_q.kernel,
+ * ....2.fn.fn.to_kv.kernel [global_k, global_k, emb_dim, 1024], svt_layers.{s}.2.proj.fn.kernel [k, k, 1, emb_dim] / .bias (PEG),
+ * svt_layers.4.1.kernel / .bias (the Dense head).  Stage 4 has no .0 / .1 sub-blocks. */
+VB_API int vb_create_twins_svt(const vb_config* base, const vb_twins_svt_config* tw, int device, vb_handle** out);
+
 /* Replaces Keras variable assignment: one call per weight, names/shapes/layouts per SURVEY.md App. B
  * (Dense kernel [in,out], float32).  shape/ndim are checked against the config. */
 VB_API int vb_set_weight(vb_handle* h, const char* name, const float* host_data, const int64_t* shape, int32_t ndim);
@@ -180,8 +207,8 @@ VB_API int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, i
                        const float* distill_token, float* logits, float* distill_out, int32_t out_mem, void* stream);
 
 /* ---- the stages of <Model>.call on their own (SURVEY.md 8f f1/f4): the attribute surface the reference's wrappers and the
- * injected-transformer shell use.  ViT / DeepViT / parallel ViT / CaiT / patch-merger ViT / T2TViT; not CrossViT, CCT, LeViT or
- * CvT. */
+ * injected-transformer shell use.  ViT / DeepViT / parallel ViT / CaiT / patch-merger ViT / T2TViT; not CrossViT, CCT, LeViT,
+ * CvT or Twins-SVT. */
 
 /* Number of token rows vb_forward_embed produces for an img_h x img_w image (patches + cls where the model has one);
  * negative on error. */
@@ -257,6 +284,10 @@ VB_API int32_t vb_last_attention_path(void);
  * CvT: the stems' unfold is 3 and their convolutions 0, the stem LayerNorm (and its row statistics) and the average pool 2; the
  * depthwise q / k|v convolutions (one launch per block) are 4, the pointwise projections 0, attention 1, the LayerNorm-folded GELU
  * fc1 5, the residual to_out / fc2 6 (the fp32 engine adds its separate PreNorm LayerNorms to 2).
+ * Twins-SVT: the patch embeddings' unfold and the global to_kv's patch rows are 3; the patch-embedding convolutions, the fused
+ * local q|k|v, the global to_q and to_kv are 0; local and global attention 1 (a windowed attention off the flash kernel adds its
+ * row permutations to 4); the PEG depthwise convolution (one per stage) 4; the LayerNorm-folded GELU fc1 5; the residual to_out /
+ * fc2 6; row statistics and the average pool 2 (the fp32 engine adds its separate LayerNorms to 2).
  * vb_profile_read synchronises the device and returns accumulated milliseconds, algorithmic FLOPs, algorithmic
  * bytes and launch counts per class (arrays of VB_PROF_NUM); reset != 0 clears the accumulators. */
 #define VB_PROF_NUM 7
@@ -351,6 +382,15 @@ VB_API int vb_op_attention_bias(int32_t precision, const float* q, int32_t ldq, 
 VB_API int vb_op_dwconv(int32_t precision, const float* x, int32_t B, int32_t H, int32_t W, int32_t C, const float* ln_gamma,
                         const float* ln_beta, int32_t k, int32_t kv_stride, const float* wq, const float* bn_q, const float* wkv,
                         const float* bn_kv, float* q, float* kv, int32_t iters, float* elapsed_ms);
+
+/* Twins-SVT's local attention (twins_svt.py:135-156) as the engine runs it: the map's p x p windows each attend within themselves.
+ * qkv: the fused q|k|v rows of a pixel-major [B, H, W] map, [B*H*W, ld] with q, k and v at columns [0, heads*dh), [heads*dh,
+ * 2*heads*dh) and [2*heads*dh, 3*heads*dh), head h at [h*dh, (h+1)*dh) of each; H and W multiples of p; out [B*H*W, ldo]
+ * pixel-major, uploaded and downloaded whole.  Scale dh^-0.5.  bf16 with dh == 64 runs the windowed flash kernel on the rows in
+ * place; every fp32 call and any shape it refuses permute the rows to window-major order, run the materialised-scores path and
+ * permute back (vb_last_attention_path tells which). */
+VB_API int vb_op_window_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t H, int32_t W, int32_t p,
+                                  int32_t heads, int32_t dh, float* out, int32_t ldo, int32_t iters, float* elapsed_ms);
 
 /* Row softmax of fp32 scores into bf16 probabilities (the T2T attention): p[r, j] = softmax_j(s[r, j] * scale) for j < n,
  * p[r, n..npad) = 0.  s [rows, lds], p [rows, ldp] (uploaded and downloaded whole); n <= npad <= ldp. */

@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "libvitb200.so")   # VB_LIB_PATH: developer A/B builds
 
 KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6, "cct": 7, "levit": 8,
-        "cvt": 9}
+        "cvt": 9, "twins_svt": 10}
 PRECISION = {"fp32": 0, "float32": 0, "bf16": 1, "bfloat16": 1}
 MEM_HOST, MEM_DEVICE = 0, 1
 ABI_VERSION = 7                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
@@ -50,6 +50,14 @@ class VbCvtConfig(C.Structure):
         "emb_dim", "emb_kernel", "emb_stride", "proj_kernel", "kv_proj_stride", "heads", "depth", "mlp_mult")]
 
 
+TWINS_STAGES = 4                                    # VB_TWINS_STAGES
+
+
+class VbTwinsSvtConfig(C.Structure):
+    _fields_ = [("struct_size", C.c_int32)] + [(n, C.c_int32 * TWINS_STAGES) for n in (
+        "emb_dim", "patch_size", "local_patch_size", "global_k", "depth")] + [("peg_kernel_size", C.c_int32)]
+
+
 class VbError(RuntimeError):
     pass
 
@@ -63,6 +71,7 @@ SIGNATURES = {
     "vb_create": (C.c_int, [C.POINTER(VbConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_levit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbLevitConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_cvt": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbCvtConfig), C.c_int, C.POINTER(C.c_void_p)]),
+    "vb_create_twins_svt": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbTwinsSvtConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, _i64p, C.c_int32]),
     "vb_num_weights": (C.c_int, [C.c_void_p]),
     "vb_weight_info": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), _i64p, C.POINTER(C.c_int32)]),
@@ -99,6 +108,7 @@ SIGNATURES = {
                                        C.c_void_p] + [C.c_int32] * 6 + [C.c_float, C.c_int32, C.c_int32, _f32p]),
     "vb_op_dwconv": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 2 + [C.c_int32] * 2 + [C.c_void_p] * 6 +
                      [C.c_int32, _f32p]),
+    "vb_op_window_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 7 + [C.c_void_p, C.c_int32, C.c_int32, _f32p]),
     "vb_op_softmax_rows": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 4 + [C.c_float, C.c_int32, _f32p]),
 }
 
@@ -258,6 +268,19 @@ def op_dwconv(x, ln_gamma, ln_beta, wq, bn_q, wkv, bn_kv, kv_stride, precision="
     check(load().vb_op_dwconv(PRECISION[precision], _ptr(x), B, H, W, Cc, _ptr(ln_gamma), _ptr(ln_beta), k, kv_stride, _ptr(wq),
                               _ptr(bn_q), _ptr(wkv), _ptr(bn_kv), _ptr(q), _ptr(kv), iters, C.byref(ms)))
     return q, kv, (ms.value if iters > 0 else None)
+
+
+def op_window_attention(qkv, H, W, p, heads, dh, precision="bf16", iters=0):
+    """Twins-SVT's local attention (vb_op_window_attention): qkv [B*H*W, ld] fused q|k|v rows of a pixel-major map.  Returns
+    (out [B*H*W, heads*dh] pixel-major, ms or None)."""
+    qkv = _f32(qkv)
+    rows, ld = qkv.shape
+    B = rows // (H * W)
+    out = np.zeros((rows, heads * dh), np.float32)
+    ms = C.c_float(0)
+    check(load().vb_op_window_attention(PRECISION[precision], _ptr(qkv), ld, B, H, W, p, heads, dh, _ptr(out), heads * dh, iters,
+                                        C.byref(ms)))
+    return out, (ms.value if iters > 0 else None)
 
 
 def op_softmax_rows(s, n, npad, scale, p, iters=0):

@@ -59,7 +59,8 @@ template void attention_generic<float>(const float*, int, const float*, int, con
 
 template <>
 bool attention_fast<float>(const float*, int, const float*, int, const float*, int, float*, int, int, int, int, int, int, int,
-                           const float*, const float*, const float*, const float*, cudaStream_t, float, const PosBias*) {
+                           const float*, const float*, const float*, const float*, cudaStream_t, float, const PosBias*,
+                           const Window*) {
   return false;  // the fp32 gate path always takes the exact SIMT kernels
 }
 

@@ -19,7 +19,8 @@ int take_last_attention_path();                  // and reset it to ATTN_PATH_NO
 // variant 2: CaiT talking heads: mix_a before softmax, mix_b after (cait.py:121-127)
 // scale: softmax scale; <= 0 means dh^-0.5 (vit.py:57).  A layer whose heads were zero-padded to the kernels' head width
 // (engine.cu: dh 48 -> 64) passes its true dim_head^-0.5 here.  pb (variant 0 only, may be null): LeViT's relative-position
-// bias and output GELU (common.h).
+// bias and output GELU (common.h).  win (attention_fast only, may be null): Twins-SVT's windowed attention, B = the number of
+// windows and nq == nk == p^2 (common.h).
 template <typename T>
 void attention_generic(const T* q, int ldq, const T* k, int ldk, const T* v, int ldv, T* out, int ldo, float* S, int B, int nq,
                        int nk, int heads, int dh, int variant, const float* mix_a, const float* mix_b, const float* ln_gamma,
@@ -28,7 +29,8 @@ void attention_generic(const T* q, int ldq, const T* k, int ldk, const T* v, int
 template <typename T>
 bool attention_fast(const T* q, int ldq, const T* k, int ldk, const T* v, int ldv, T* out, int ldo, int B, int nq, int nk,
                     int heads, int dh, int variant, const float* mix_a, const float* mix_b, const float* ln_gamma,
-                    const float* ln_beta, cudaStream_t s, float scale = 0.f, const PosBias* pb = nullptr);
+                    const float* ln_beta, cudaStream_t s, float scale = 0.f, const PosBias* pb = nullptr,
+                    const Window* win = nullptr);
 
 // The talking-heads / re-attention path keeps host copies of the head-mix weights keyed by their device pointers (one process-
 // wide cache for all handles); whoever frees or rewrites such weights (vb_finalize, vb_destroy, the op-level test entries) must

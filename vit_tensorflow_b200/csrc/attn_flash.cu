@@ -15,6 +15,10 @@
 // BIAS (LeViT, levit.py:114-117,94): the head's [fmap^2] relative-position table sits in shared memory (in log2 units); every
 // score gets table[pos_bias_index(i, j)] added before the online softmax, and the stored rows optionally go through GELU.
 // With BIAS the scores are moved to log2 units as soon as they are computed, so the softmax below runs with a unit scale.
+//
+// WIN (Twins-SVT local attention, twins_svt.py:135-156): the flat batch index is a p x p window of a pixel-major map (Window,
+// common.h), nq == nk == p^2.  Q, K and V rows are loaded from, and the output rows stored to, the map's own pixel rows, so the
+// window split and merge rearranges (:141,153) cost no copies.  p^2 > 64 takes several query tiles and key blocks as any n does.
 #include "attention.cuh"
 #include "kernels.cuh"
 #include "ptx.cuh"
@@ -40,11 +44,11 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
 
 constexpr int FLASH_BIAS_MAX = 4096;   // fmap^2 of the largest relative-position table (16 KB of shared memory)
 
-template <bool BIAS>
+template <bool BIAS, bool WIN>
 __global__ void __launch_bounds__(128)
 attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloat16* __restrict__ k, int ldk,
                   const __nv_bfloat16* __restrict__ v, int ldv, __nv_bfloat16* __restrict__ out, int ldo, int heads, int nq, int nk,
-                  float scale_log2, const float* __restrict__ pos_tab, int fmap, int step, int gelu_out) {
+                  float scale_log2, const float* __restrict__ pos_tab, int fmap, int step, int gelu_out, Window win) {
   extern __shared__ float tab[];                                     // BIAS: [fmap^2] of this head, times log2(e)
   __shared__ __align__(16) __nv_bfloat16 Qs[FQ][FP];
   __shared__ __align__(16) __nv_bfloat16 Ks[2][FK][FP];
@@ -54,6 +58,9 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
   const int i0 = (blockIdx.x % qtiles) * FQ;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nblk = (nk + FK - 1) / FK;
+  // row of token i of this CTA's batch entry in the q / k / v / out matrices
+  auto qrow_of = [&](int i) -> size_t { return WIN ? static_cast<size_t>(win.row(b, i)) : static_cast<size_t>(b) * nq + i; };
+  auto krow_of = [&](int i) -> size_t { return WIN ? static_cast<size_t>(win.row(b, i)) : static_cast<size_t>(b) * nk + i; };
 
   pdl_wait();                 // Q/K/V come from the previous kernel of the stream
   pdl_launch_dependents();
@@ -61,7 +68,7 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
   // rows past n are zero-filled (never read from the next image); 8 16-byte vectors per 64-column row
   for (int e = threadIdx.x; e < FQ * 8; e += 128) {
     const int r = e >> 3, c = (e & 7) * 8;
-    if (i0 + r < nq) cp_async16(smem_u32(&Qs[r][c]), q + (static_cast<size_t>(b) * nq + i0 + r) * ldq + h * DH + c);
+    if (i0 + r < nq) cp_async16(smem_u32(&Qs[r][c]), q + qrow_of(i0 + r) * ldq + h * DH + c);
     else *reinterpret_cast<uint4*>(&Qs[r][c]) = make_uint4(0, 0, 0, 0);
   }
   auto stage = [&](int j) {
@@ -70,7 +77,7 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
       for (int e = threadIdx.x; e < FK * 8; e += 128) {
         const int r = e >> 3, c = (e & 7) * 8;
         if (j0 + r < nk) {
-          const size_t row = static_cast<size_t>(b) * nk + j0 + r;
+          const size_t row = krow_of(j0 + r);
           cp_async16(smem_u32(&Ks[s][r][c]), k + row * ldk + h * DH + c);
           cp_async16(smem_u32(&Vs[s][r][c]), v + row * ldv + h * DH + c);
         } else {                                                     // zero V rows: 0 * garbage could be NaN
@@ -187,7 +194,7 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
   for (int r = 0; r < 2; ++r) {
     const int row = i0 + warp * 16 + qr + 8 * r;
     if (row >= nq) continue;
-    __nv_bfloat16* orow = out + (static_cast<size_t>(b) * nq + row) * ldo + h * DH + qc;
+    __nv_bfloat16* orow = out + qrow_of(row) * ldo + h * DH + qc;
 #pragma unroll
     for (int n = 0; n < DH / 8; ++n) {
       float a0 = o[n][2 * r] * l_run[r], a1 = o[n][2 * r + 1] * l_run[r];
@@ -203,8 +210,9 @@ template <>
 bool attention_fast<__nv_bfloat16>(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, int ldk, const __nv_bfloat16* v, int ldv,
                                    __nv_bfloat16* out, int ldo, int B, int nq, int nk, int heads, int dh, int variant,
                                    const float* mix_a, const float* mix_b, const float* ln_g, const float* ln_b, cudaStream_t s,
-                                   float scale, const PosBias* pb) {
-  if (nq == 1 && pb == nullptr && attention_cls(q, ldq, k, ldk, v, ldv, out, ldo, B, nk, heads, dh, variant, mix_a, mix_b, ln_g, ln_b, s, scale)) return true;
+                                   float scale, const PosBias* pb, const Window* win) {
+  if (win != nullptr && (pb != nullptr || nq != win->p * win->p || nk != nq)) return false;
+  if (nq == 1 && pb == nullptr && win == nullptr && attention_cls(q, ldq, k, ldk, v, ldv, out, ldo, B, nk, heads, dh, variant, mix_a, mix_b, ln_g, ln_b, s, scale)) return true;
   // DeepViT re-attention / CaiT talking heads: the materialised-scores path (attn_generic_mma.cu) -- a fused form with all heads'
   // scores of a 16-row tile in shared memory measured 9-11 % slower on the H100 (one CTA per SM at 16 heads)
   if (variant != 0 || dh != DH || (nq < 2 && pb == nullptr)) return false;
@@ -222,7 +230,7 @@ bool attention_fast<__nv_bfloat16>(const __nv_bfloat16* q, int ldq, const __nv_b
   if (pb != nullptr) {
     static unsigned long long seen[4] = {0, 0, 0, 0};
     if (first_use_on_this_device(seen))
-      VB_CUDA(cudaFuncSetAttribute(attn_flash_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FLASH_BIAS_MAX * 4));
+      VB_CUDA(cudaFuncSetAttribute(attn_flash_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FLASH_BIAS_MAX * 4));
     cfg.dynamicSmemBytes = static_cast<size_t>(pb->fmap) * pb->fmap * sizeof(float);
   }
   cudaLaunchAttribute attr[1];
@@ -231,11 +239,14 @@ bool attention_fast<__nv_bfloat16>(const __nv_bfloat16* q, int ldq, const __nv_b
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   if (pb != nullptr)
-    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<true>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2, pb->table,
-                               pb->fmap, pb->step, static_cast<int>(pb->gelu_out)));
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<true, false>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
+                               pb->table, pb->fmap, pb->step, static_cast<int>(pb->gelu_out), Window()));
+  else if (win != nullptr)
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<false, true>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
+                               static_cast<const float*>(nullptr), 0, 1, 0, *win));
   else
-    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<false>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
-                               static_cast<const float*>(nullptr), 0, 1, 0));
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<false, false>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
+                               static_cast<const float*>(nullptr), 0, 1, 0, Window()));
   count_launch();
   note_attention_path(ATTN_PATH_FLASH);
   return true;

@@ -75,6 +75,18 @@ __device__ __forceinline__ int pos_bias_index(int i, int j, int fmap, int step, 
 }
 __device__ __forceinline__ float gelu_exact(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
+// Twins-SVT's local attention (twins_svt.py:135-156): each p x p window of a pixel-major [B, H, W] map attends within itself.  The
+// flat batch index of the attention is (image, window row, window column) over nx x ny windows (W = nx * p, H = ny * p), and token
+// i < p^2 of window bw is the map's row row(bw, i) = (b * H + wy * p + i / p) * W + wx * p + i % p.  nq == nk == p^2.
+struct Window {
+  int p = 0, nx = 0, ny = 0;
+  __host__ __device__ long long row(long long bw, int i) const {
+    const long long per = static_cast<long long>(nx) * ny, b = bw / per;
+    const int w = static_cast<int>(bw - b * per), wy = w / nx, wx = w - wy * nx, r = i / p;
+    return ((b * ny + wy) * p + r) * (static_cast<long long>(nx) * p) + wx * p + (i - r * p);
+  }
+};
+
 // 2-D bf16 (or fp32) tensor map (innermost dimension first), 128-byte swizzle unless swizzle128 == false.
 CUtensorMap make_tmap_2d(const void* base, uint64_t inner, uint64_t outer, uint64_t outer_stride_bytes,
                          uint32_t box_inner, uint32_t box_outer, bool swizzle128 = true, bool f32 = false);

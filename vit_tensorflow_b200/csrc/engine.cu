@@ -174,6 +174,24 @@ inline void cvt_fold_dw(const std::vector<double>& taps, const std::vector<doubl
   }
 }
 
+// One Twins-SVT Transformer layer (twins_svt.py:192-213) on channel rows zero-padded to dp (bf16) / dim (fp32): x = x + f(LN(x))
+// for local attention, MLP, global attention, MLP; stage 4 has no local attention and no first MLP (has_local=False, :255).  The
+// bf16 engine folds the PreNorm LayerNorms of the fused local q|k|v, the global to_q and the fc1s into those GEMMs.
+struct TwinsMlpW { Norm norm; Linear fc1, fc2; };
+struct TwinsLayerW {
+  bool local = false;
+  Norm local_norm, global_norm;      // gamma / beta [dp], zero on pad channels
+  Linear qkv, local_out;             // local: to_q | to_kv as one [dp, 1536] GEMM, to_out
+  Linear to_q, to_kv, global_out;    // global: to_q [dp, 512], to_kv [k * k * dim, 1024] over the VALID k x k patch rows
+  TwinsMlpW ff1, ff2;
+};
+struct TwinsStageW {                 // twins_svt.py:252-259: PatchEmbedding, Transformer(depth 1), PEG, Transformer(depth)
+  int dim = 0, dp = 0, patch = 1, local = 0, global_k = 1, peg_k = 3;
+  Linear proj;                       // rows in unfold_same's (p1, p2, c) order
+  const float *peg_w = nullptr, *peg_b = nullptr;   // PEG taps [k*k][dp] with the residual on the centre tap, bias [dp]
+  std::vector<TwinsLayerW> pre, post;
+};
+
 struct EmbedW { Linear patch; const float* pos = nullptr; const float* cls = nullptr; int dim = 0, n_pos = 0; };
 struct CrossW { bool proj = false; Linear project_in, project_out, to_q, to_kv, to_out; Norm norm; };
 
@@ -371,6 +389,12 @@ struct vb_handle {
   std::vector<CvtStageW> cvt_stages;
   static std::string cvt_pre(int st) { return "cvt_layers." + std::to_string(st) + "."; }
   int cvt_cin(int st) const { return st == 0 ? cfg.channels : cv.emb_dim[st - 1]; }
+  // Twins-SVT (twins_svt.py:215-268): the four stages, then the average pool and the Dense head (`head`)
+  vb_twins_svt_config tw{};
+  std::vector<TwinsStageW> twins_stages;
+  static std::string twins_pre(int st) { return "svt_layers." + std::to_string(st) + "."; }
+  int twins_cin(int st) const { return st == 0 ? cfg.channels : tw.emb_dim[st - 1]; }
+  static constexpr int kTwinsInner = 512;        // 8 heads of 64: Transformer is never passed heads / dim_head (twins_svt.py:254-258)
   struct XBlock { std::vector<LayerW> sm_layers, lg_layers; Norm sm_final, lg_final; std::vector<CrossW> sm_attend_lg, lg_attend_sm; };
   std::vector<XBlock> xblocks;
   Norm head_norm, sm_head_norm, lg_head_norm;
@@ -552,6 +576,46 @@ struct vb_handle {
         }
       }
       expect_dense("cvt_layers.3.1", cv.emb_dim[VB_CVT_STAGES - 1], c.num_classes);   // cvt.py:195-198
+    } else if (c.kind == VB_KIND_TWINS_SVT) {
+      auto expect_ln4 = [&](const std::string& n, int d) { expect(n + ".g", {1, 1, 1, d}); expect(n + ".b", {1, 1, 1, d}); };   // :50-51
+      const int I = kTwinsInner;
+      for (int st = 0; st < VB_TWINS_STAGES; ++st) {
+        const std::string p = twins_pre(st);
+        const int d = tw.emb_dim[st], ps = tw.patch_size[st], kg = tw.global_k[st], k = tw.peg_kernel_size;
+        auto expect_mlp = [&](const std::string& m) {                      // Residual(PreNorm(MLP)) :78-92,201,203
+          expect_ln4(m + ".fn.norm", d);
+          expect(m + ".fn.fn.net.0.kernel", {1, 1, d, 4 * d});
+          expect(m + ".fn.fn.net.0.bias", {4 * d});
+          expect(m + ".fn.fn.net.3.kernel", {1, 1, 4 * d, d});
+          expect(m + ".fn.fn.net.3.bias", {d});
+        };
+        expect(p + "0.proj.kernel", {1, 1, twins_cin(st) * ps * ps, d});   // PatchEmbedding :99
+        expect(p + "0.proj.bias", {d});
+        for (int t : {1, 3}) {
+          for (int L = 0; L < (t == 1 ? 1 : tw.depth[st]); ++L) {
+            const std::string b = p + std::to_string(t) + ".layers." + std::to_string(L) + ".";
+            if (st < VB_TWINS_STAGES - 1) {                                  // LocalAttention :127-133
+              expect_ln4(b + "0.fn.norm", d);
+              expect(b + "0.fn.fn.to_q.kernel", {1, 1, d, I});
+              expect(b + "0.fn.fn.to_kv.kernel", {1, 1, d, 2 * I});
+              expect(b + "0.fn.fn.to_out.0.kernel", {1, 1, I, d});
+              expect(b + "0.fn.fn.to_out.0.bias", {d});
+              expect_mlp(b + "1");
+            }
+            expect_ln4(b + "2.fn.norm", d);                                  // GlobalAttention :167-173
+            expect(b + "2.fn.fn.to_q.kernel", {1, 1, d, I});
+            expect(b + "2.fn.fn.to_kv.kernel", {kg, kg, d, 2 * I});
+            expect(b + "2.fn.fn.to_out.0.kernel", {1, 1, I, d});
+            expect(b + "2.fn.fn.to_out.0.bias", {d});
+            expect_mlp(b + "3");
+          }
+          if (t == 1) {
+            expect(p + "2.proj.fn.kernel", {k, k, 1, d});                    // PEG :111
+            expect(p + "2.proj.fn.bias", {d});
+          }
+        }
+      }
+      expect_dense("svt_layers.4.1", tw.emb_dim[VB_TWINS_STAGES - 1], c.num_classes);   // :261-264
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       expect("pos_embedding", {1, np, c.dim});
@@ -776,7 +840,7 @@ struct vb_handle {
     for (auto& w : weights) VB_CHECK(w.set, "vb_finalize: weight '" + w.name + "' was never set");
     VB_CUDA(cudaSetDevice(device));
     owned.clear(); layers.clear(); cls_layers.clear(); t2t_layers.clear(); xblocks.clear(); plans.clear(); embed_res.clear(); cct_convs.clear();
-    lv_stem.clear(); lv_blocks.clear(); cvt_stages.clear();
+    lv_stem.clear(); lv_blocks.clear(); cvt_stages.clear(); twins_stages.clear();
     woverride.clear();
     drop_graphs();
     const vb_config& c = cfg;
@@ -829,6 +893,8 @@ struct vb_handle {
       finalize_levit();
     } else if (c.kind == VB_KIND_CVT) {
       finalize_cvt();
+    } else if (c.kind == VB_KIND_TWINS_SVT) {
+      finalize_twins();
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       embed = make_embed("", c.patch_h, c.patch_w, c.dim, np, false);
@@ -958,6 +1024,80 @@ struct vb_handle {
     }
     head = make_linear_f32("cvt_layers.3.1", cv.emb_dim[VB_CVT_STAGES - 1], cfg.num_classes);
   }
+  // ---- Twins-SVT weight packing: channel widths zero-padded (bf16), the patch kernel's rows permuted, the PEG residual folded
+  TwinsMlpW twins_mlp(const std::string& m, int d, int dp) {
+    TwinsMlpW w;
+    const int hidden = 4 * d, hp = channel_width(hidden);
+    const std::string n0 = m + ".fn.fn.net.0", n3 = m + ".fn.fn.net.3";
+    w.norm = padded_norm(m + ".fn.norm", d, dp);
+    w.fc1 = linear_from_host("twins." + n0, pad_kn(host_weight(n0 + ".kernel"), d, hidden, dp, hp), pad_n(host_weight(n0 + ".bias"), hp), dp,
+                             hp, bf16() ? &w.norm : nullptr);
+    w.fc1.ln_d = d;
+    w.fc1.ln_eps = 1e-5f;
+    w.fc2 = linear_from_host("twins." + n3, pad_kn(host_weight(n3 + ".kernel"), hidden, d, hp, dp), pad_n(host_weight(n3 + ".bias"), dp), hp, dp);
+    return w;
+  }
+  TwinsLayerW twins_layer_weights(const std::string& b, int st, int d, int dp) {
+    TwinsLayerW w;
+    const int I = kTwinsInner, kg = tw.global_k[st];
+    auto folded = [&](Linear L) { L.ln_d = d; L.ln_eps = 1e-5f; return L; };   // twins_svt.py:46: eps 1e-5
+    auto to_out = [&](const std::string& n) {
+      return linear_from_host("twins." + n, pad_kn(host_weight(n + ".kernel"), I, d, I, dp), pad_n(host_weight(n + ".bias"), dp), I, dp);
+    };
+    w.local = st < VB_TWINS_STAGES - 1;
+    if (w.local) {
+      w.local_norm = padded_norm(b + "0.fn.norm", d, dp);
+      const auto q = host_weight(b + "0.fn.fn.to_q.kernel"), kv = host_weight(b + "0.fn.fn.to_kv.kernel");
+      std::vector<double> qkv(static_cast<size_t>(d) * 3 * I);           // [d, q | k | v]
+      for (int r = 0; r < d; ++r) {
+        std::copy(q.begin() + static_cast<size_t>(r) * I, q.begin() + static_cast<size_t>(r + 1) * I, qkv.begin() + static_cast<size_t>(r) * 3 * I);
+        std::copy(kv.begin() + static_cast<size_t>(r) * 2 * I, kv.begin() + static_cast<size_t>(r + 1) * 2 * I,
+                  qkv.begin() + static_cast<size_t>(r) * 3 * I + I);
+      }
+      w.qkv = folded(linear_from_host("twins." + b + "0.qkv", pad_kn(qkv, d, 3 * I, dp, 3 * I), {}, dp, 3 * I, bf16() ? &w.local_norm : nullptr));
+      w.local_out = to_out(b + "0.fn.fn.to_out.0");
+      w.ff1 = twins_mlp(b + "1", d, dp);
+    }
+    w.global_norm = padded_norm(b + "2.fn.norm", d, dp);
+    w.to_q = folded(linear_from_host("twins." + b + "2.to_q", pad_kn(host_weight(b + "2.fn.fn.to_q.kernel"), d, I, dp, I), {}, dp, I,
+                                     bf16() ? &w.global_norm : nullptr));
+    // [kg, kg, d, 2I] is the Dense [kg*kg*d, 2I] over unfold_same's (row, column, channel) vectors of the true d channels
+    w.to_kv = linear_from_host("twins." + b + "2.to_kv", host_weight(b + "2.fn.fn.to_kv.kernel"), {}, kg * kg * d, 2 * I);
+    w.global_out = to_out(b + "2.fn.fn.to_out.0");
+    w.ff2 = twins_mlp(b + "3", d, dp);
+    return w;
+  }
+  void finalize_twins() {
+    for (int st = 0; st < VB_TWINS_STAGES; ++st) {
+      TwinsStageW S;
+      const std::string p = twins_pre(st);
+      const int d = tw.emb_dim[st], dp = channel_width(d), ps = tw.patch_size[st], cin = twins_cin(st), K = ps * ps * cin, k = tw.peg_kernel_size;
+      S.dim = d; S.dp = dp; S.patch = ps; S.local = tw.local_patch_size[st]; S.global_k = tw.global_k[st]; S.peg_k = k;
+      // 'b (h p1) (w p2) c -> b h w (c p1 p2)' (twins_svt.py:103): the reference's row c * p^2 + p1 * p + p2 is unfold_same's
+      // row (p1 * p + p2) * cin + c
+      const auto wr = host_weight(p + "0.proj.kernel");
+      std::vector<double> wp(static_cast<size_t>(K) * d);
+      for (int c = 0; c < cin; ++c)
+        for (int t = 0; t < ps * ps; ++t)
+          std::copy(wr.begin() + static_cast<size_t>(c * ps * ps + t) * d, wr.begin() + static_cast<size_t>(c * ps * ps + t + 1) * d,
+                    wp.begin() + static_cast<size_t>(t * cin + c) * d);
+      S.proj = linear_from_host("twins." + p + "0.proj", pad_kn(wp, K, d, K, dp), pad_n(host_weight(p + "0.proj.bias"), dp), K, dp);
+      // PEG (:108-115): x + dw(x) + b is one depthwise convolution whose centre tap ((k-1)/2, (k-1)/2) has 1 added (TF SAME at
+      // stride 1 pads (k-1)/2 on the top / left, so that tap reads the pixel itself)
+      const auto taps = host_weight(p + "2.proj.fn.kernel");
+      std::vector<double> pw(static_cast<size_t>(k) * k * dp, 0.0);
+      const int centre = ((k - 1) / 2) * k + (k - 1) / 2;
+      for (int t = 0; t < k * k; ++t)
+        for (int c = 0; c < d; ++c) pw[static_cast<size_t>(t) * dp + c] = taps[static_cast<size_t>(t) * d + c] + (t == centre ? 1.0 : 0.0);
+      S.peg_w = upload_owned(pw);
+      S.peg_b = upload_owned(pad_n(host_weight(p + "2.proj.fn.bias"), dp));
+      for (int t : {1, 3})
+        for (int L = 0; L < (t == 1 ? 1 : tw.depth[st]); ++L)
+          (t == 1 ? S.pre : S.post).push_back(twins_layer_weights(p + std::to_string(t) + ".layers." + std::to_string(L) + ".", st, d, dp));
+      twins_stages.push_back(std::move(S));
+    }
+    head = make_linear_f32("svt_layers.4.1", tw.emb_dim[VB_TWINS_STAGES - 1], cfg.num_classes);
+  }
   void finalize_levit() {
     const int dh = levit_dh();
     int cin = cfg.channels;
@@ -1051,7 +1191,7 @@ struct vb_handle {
   template <typename T>
   void attention_dispatch(const T* q, int ldq, const T* k, int ldk, const T* v, int ldv, T* out, int ldo, int B, int nq, int nk,
                           int heads, int dh, int variant, const float* mix_a, const float* mix_b, const float* g, const float* b,
-                          cudaStream_t s, float scale = 0.f);
+                          cudaStream_t s, float scale = 0.f, const Window* win = nullptr);
 
   template <typename T>
   const T* embed_residual(const EmbedW& e, int B, int rows, cudaStream_t s) {
@@ -1510,6 +1650,8 @@ struct vb_handle {
       levit_forward<T>(img, B, H, Wd, logits, nullptr, s);
     } else if (c.kind == VB_KIND_CVT) {
       cvt_forward<T>(img, B, H, Wd, logits, s);
+    } else if (c.kind == VB_KIND_TWINS_SVT) {
+      twins_forward<T>(img, B, H, Wd, logits, s);
     } else if (c.kind == VB_KIND_CCT) {                   // CCT.call cct.py:342-345, TransformerClassifier.call :277-305
       int rows = 0;
       T* X = tokenize_cct<T>(img, B, H, Wd, &rows, s);
@@ -1744,6 +1886,134 @@ struct vb_handle {
     linear<T>(Hb, b.fc1.N, M, b.fc2, X, dp, e2, s);
   }
 
+  // TwinsSVT.call (twins_svt.py:266-268): per stage, PatchEmbedding -> Transformer(1) -> PEG -> Transformer(depth); then
+  // GlobalAvgPool2D -> Dense.  Token rows are the NHWC map, pixel-major, channel widths zero-padded to channel_width; no stage
+  // permutes its map.  bf16: `stats` holds the (sum, sumsq) partials of X's rows between sub-blocks (emitted by the patch
+  // embedding's and the residual GEMMs' epilogues, and after the PEG by a row-statistics pass).
+  static constexpr const char* kTwinsNoStages =
+      "Twins-SVT runs as a whole forward only: its patch-embedding / stage / head steps have no entry of their own";
+  // The reference's shape rules (twins_svt.py:103,141,168 through einops and Keras), checked before anything runs.
+  void twins_check_size(int H, int Wd) const {
+    int h = H, w = Wd;
+    for (int st = 0; st < VB_TWINS_STAGES; ++st) {
+      const std::string where = "Twins-SVT stage " + std::to_string(st + 1) + ": the " + std::to_string(h) + " x " + std::to_string(w) + " map ";
+      const int ps = tw.patch_size[st], pl = tw.local_patch_size[st], kg = tw.global_k[st];
+      VB_CHECK(h % ps == 0 && w % ps == 0, where + "is not divisible by patch_size " + std::to_string(ps));
+      h /= ps; w /= ps;
+      const std::string after = "Twins-SVT stage " + std::to_string(st + 1) + ": the " + std::to_string(h) + " x " + std::to_string(w) + " map ";
+      VB_CHECK(st == VB_TWINS_STAGES - 1 || (h % pl == 0 && w % pl == 0),
+               after + "is not divisible by local_patch_size " + std::to_string(pl));
+      VB_CHECK(h >= kg && w >= kg, after + "is smaller than global_k " + std::to_string(kg) + " (a VALID convolution)");
+    }
+  }
+  template <typename T>
+  void twins_forward(const float* img, int B, int H, int Wd, float* logits, cudaStream_t s) {
+    twins_check_size(H, Wd);
+    int mh = H, mw = Wd, mc = cfg.channels, ld_in = 0;
+    const T* map = nullptr;
+    T* X = nullptr;
+    for (const TwinsStageW& S : twins_stages) {
+      const int oh = mh / S.patch, ow = mw / S.patch, M = B * oh * ow;
+      const int Kp = bf16() ? S.proj.ldw : S.proj.K;
+      T* col = arena.get<T>(static_cast<size_t>(M) * Kp);
+      {
+        ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(map == nullptr ? 4 : sizeof(T)) * B * mh * mw * mc +
+                                                 static_cast<double>(sizeof(T)) * M * Kp, s);
+        if (map == nullptr) unfold_same<float, T>(img, col, B, mh, mw, mc, S.patch, S.patch, 0, Kp, s);
+        else unfold_same<T, T>(map, col, B, mh, mw, mc, S.patch, S.patch, 0, Kp, s, ld_in);
+      }
+      X = arena.get<T>(static_cast<size_t>(M) * S.dp);
+      float* stats = bf16() ? arena.get<float>(static_cast<size_t>(M) * (S.dp / 64) * 2) : nullptr;
+      Linear L = S.proj;
+      L.K = Kp;
+      Epi e; e.bias = S.proj.bias; e.stats_out = stats;
+      linear<T>(col, Kp, M, L, X, S.dp, e, s);
+      for (const TwinsLayerW& l : S.pre) twins_layer<T>(X, B, oh, ow, S, l, stats, s);
+      T* Y = arena.get<T>(static_cast<size_t>(M) * S.dp);             // the PEG's halo reads the unmodified map
+      {
+        ProfScope ps(this, PROF_OTHER, 2.0 * S.peg_k * S.peg_k * M * S.dim, 2.0 * sizeof(T) * M * S.dp, s);
+        dwconv_qkv<T>(X, S.dp, nullptr, nullptr, nullptr, S.dim, 1e-5f, S.peg_w, S.peg_b, Y, S.dp, nullptr, nullptr, nullptr, S.dp, B, oh, ow,
+                      S.dp, S.peg_k, 1, s);
+      }
+      X = Y;
+      if (bf16()) ensure_stats<T>(X, S.dp, stats, M, s);
+      for (const TwinsLayerW& l : S.post) twins_layer<T>(X, B, oh, ow, S, l, stats, s);
+      map = X; mh = oh; mw = ow; mc = S.dim; ld_in = S.dp;
+    }
+    const int dl = tw.emb_dim[VB_TWINS_STAGES - 1];
+    float* z = arena.get<float>(static_cast<size_t>(B) * dl);
+    {
+      ProfScope ps(this, PROF_LN, 1.0 * B * mh * mw * dl, static_cast<double>(sizeof(T)) * B * mh * mw * dl, s);
+      pool_layernorm<T>(X, mh * mw, ld_in, nullptr, nullptr, z, B, dl, 1, s);   // GlobalAvgPool2D twins_svt.py:262
+    }
+    gemm_simt<float, float, float>(z, dl, head.W, head.N, 1, logits, head.N, B, head.N, dl, head.bias, nullptr, nullptr, head.N, 0, s);
+  }
+  // One Transformer layer (twins_svt.py:206-211) in place on X [B*H*W, dp].  bf16: the PreNorm LayerNorms are folded into the
+  // fused local q|k|v, the global to_q and the fc1s (from `stats`), and applied on load by the global to_kv's patch gather; fp32:
+  // separate LayerNorms.
+  template <typename T>
+  void twins_layer(T* X, int B, int H, int Wd, const TwinsStageW& S, const TwinsLayerW& l, float* stats, cudaStream_t s) {
+    const int dp = S.dp, d = S.dim, M = B * H * Wd, I = kTwinsInner;
+    T* Y = bf16() ? nullptr : arena.get<T>(static_cast<size_t>(M) * dp);
+    auto prenorm = [&](const Norm& n) -> const T* {
+      if (Y == nullptr) return X;
+      ProfScope ps(this, PROF_LN, 8.0 * M * d, 2.0 * sizeof(T) * M * dp, s);
+      layernorm<T>(X, dp, n.gamma, n.beta, Y, dp, M, d, s, dp, 1e-5f);
+      return Y;
+    };
+    auto folded = [&](const Linear& L) {
+      Epi e;
+      if (Y == nullptr) { e.bias = L.ln_c2; e.ln_stats = stats; } else { e.bias = L.bias; }
+      return e;
+    };
+    auto residual = [&](const T* A, int lda, const Linear& L) {     // X = A W + b + X, and X's new row statistics
+      Epi e; e.bias = L.bias; e.res = X; e.ldr = dp; e.stats_out = stats;
+      linear<T>(A, lda, M, L, X, dp, e, s);
+    };
+    auto mlp = [&](const TwinsMlpW& m) {                              // twins_svt.py:78-92
+      const T* a = prenorm(m.norm);
+      T* Hb = arena.get<T>(static_cast<size_t>(M) * m.fc1.N);
+      Epi e1 = folded(m.fc1);
+      e1.gelu = true;
+      linear<T>(a, dp, M, m.fc1, Hb, m.fc1.N, e1, s);
+      residual(Hb, m.fc1.N, m.fc2);
+    };
+    T* O = arena.get<T>(static_cast<size_t>(M) * I);
+    if (l.local) {                                                    // LocalAttention twins_svt.py:135-156
+      const T* a = prenorm(l.local_norm);
+      T* QKV = arena.get<T>(static_cast<size_t>(M) * 3 * I);
+      linear<T>(a, dp, M, l.qkv, QKV, 3 * I, folded(l.qkv), s);
+      Window win;
+      win.p = S.local; win.nx = Wd / S.local; win.ny = H / S.local;
+      const int n = S.local * S.local;
+      attention_dispatch<T>(QKV, 3 * I, QKV + I, 3 * I, QKV + 2 * I, 3 * I, O, I, B * win.nx * win.ny, n, n, I / 64, 64, 0, nullptr, nullptr,
+                            nullptr, nullptr, s, 0.f, &win);
+      residual(O, I, l.local_out);
+      mlp(l.ff1);
+    }
+    // GlobalAttention twins_svt.py:175-190: q from every pixel, k|v from the VALID k x k stride-k convolution of LN(x)
+    const T* a = prenorm(l.global_norm);
+    T* Q = arena.get<T>(static_cast<size_t>(M) * I);
+    linear<T>(a, dp, M, l.to_q, Q, I, folded(l.to_q), s);
+    const int k = S.global_k, kh = (H - k) / k + 1, kw = (Wd - k) / k + 1, Mk = B * kh * kw;
+    const int Kp = bf16() ? l.to_kv.ldw : l.to_kv.K;
+    T* col = arena.get<T>(static_cast<size_t>(Mk) * Kp);
+    {
+      ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(sizeof(T)) * Mk * Kp * 2.0, s);
+      UnfoldMode um;
+      um.valid = true;
+      if (Y == nullptr) { um.stats = stats; um.parts = dp / 64; um.d = d; um.eps = 1e-5f; um.gamma = l.global_norm.gamma; um.beta = l.global_norm.beta; }
+      unfold_same<T, T>(a, col, B, H, Wd, d, k, k, 0, Kp, s, dp, &um);
+    }
+    T* KV = arena.get<T>(static_cast<size_t>(Mk) * 2 * I);
+    Linear Lk = l.to_kv;
+    Lk.K = Kp;
+    linear<T>(col, Kp, Mk, Lk, KV, 2 * I, Epi(), s);
+    attention_dispatch<T>(Q, I, KV, 2 * I, KV + I, 2 * I, O, I, B, H * Wd, kh * kw, I / 64, 64, 0, nullptr, nullptr, nullptr, nullptr, s);
+    residual(O, I, l.global_out);
+    mlp(l.ff2);
+  }
+
   // DistillMixin.call (distill.py:16-45) on top of a ViT: embed -> append the distillation token as the LAST row ->
   // transformer over n + 2 rows -> head on the first n + 1 rows, and the last row returned as is.
   template <typename T>
@@ -1799,6 +2069,7 @@ struct vb_handle {
     VB_CHECK(cfg.kind != VB_KIND_CCT, kCctNoStages);
     VB_CHECK(cfg.kind != VB_KIND_LEVIT, kLevitNoStages);
     VB_CHECK(cfg.kind != VB_KIND_CVT, kCvtNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_TWINS_SVT, kTwinsNoStages);
     if (cfg.kind == VB_KIND_T2T_VIT) {
       int h = H, w = Wd;
       for (const auto& st : t2t_stages()) { h = (h + st.stride - 1) / st.stride; w = (w + st.stride - 1) / st.stride; }
@@ -1826,6 +2097,7 @@ struct vb_handle {
     VB_CHECK(cfg.kind != VB_KIND_CCT, kCctNoStages);
     VB_CHECK(cfg.kind != VB_KIND_LEVIT, kLevitNoStages);
     VB_CHECK(cfg.kind != VB_KIND_CVT, kCvtNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_TWINS_SVT, kTwinsNoStages);
     arena.reset();
     const long long count = static_cast<long long>(B) * n * cfg.dim;
     T* X = arena.get<T>(count);
@@ -1839,6 +2111,7 @@ struct vb_handle {
     VB_CHECK(cfg.kind != VB_KIND_CCT, kCctNoStages);
     VB_CHECK(cfg.kind != VB_KIND_LEVIT, kLevitNoStages);
     VB_CHECK(cfg.kind != VB_KIND_CVT, kCvtNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_TWINS_SVT, kTwinsNoStages);
     arena.reset();
     const int K = embed.patch.K, Kp = bf16() ? embed.patch.ldw : K;
     T* col = arena.get<T>(static_cast<size_t>(rows) * Kp);
@@ -1964,7 +2237,30 @@ void vb_handle::layer_t2t<__nv_bfloat16>(__nv_bfloat16* X, int B, int n, const L
 template <typename T>
 void vb_handle::attention_dispatch(const T* q, int ldq, const T* k, int ldk, const T* v, int ldv, T* out, int ldo, int B, int nq,
                                    int nk, int heads, int dh, int variant, const float* mix_a, const float* mix_b, const float* g,
-                                   const float* b, cudaStream_t s, float scale) {
+                                   const float* b, cudaStream_t s, float scale, const Window* win) {
+  if (win != nullptr) {                       // Twins-SVT's local attention: B windows of nq = nk = p^2 tokens in the map's own rows
+    const int HD = heads * dh;
+    VB_CHECK(k == q + HD && v == q + 2 * HD && ldk == ldq && ldv == ldq && variant == 0, "internal: windowed attention reads fused q|k|v rows");
+    const double fl = 4.0 * B * heads * nq * nk * dh, by = static_cast<double>(sizeof(T)) * B * heads * dh * (2.0 * nq + 2.0 * nk);
+    {
+      ProfScope ps(this, PROF_ATTN, fl, by, s);
+      if (attention_fast<T>(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, heads, dh, 0, nullptr, nullptr, nullptr, nullptr, s, 0.f, nullptr, win))
+        return;
+    }
+    // off the flash kernel: the rows permuted to window-major order, the materialised-scores path, the output rows permuted back
+    const long long rows = static_cast<long long>(B) * nq;
+    T* qkvw = arena.get<T>(static_cast<size_t>(rows) * 3 * HD);
+    T* ow = arena.get<T>(static_cast<size_t>(rows) * HD);
+    { ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * rows * 3 * HD, s); window_rows<T>(q, ldq, qkvw, 3 * HD, 3 * HD, *win, rows, true, s); }
+    {
+      ProfScope ps(this, PROF_ATTN, fl, by, s);
+      float* S = arena.get<float>(static_cast<size_t>(B) * heads * nq * ((nk + 15) & ~15));
+      attention_generic<T>(qkvw, 3 * HD, qkvw + HD, 3 * HD, qkvw + 2 * HD, 3 * HD, ow, HD, S, B, nq, nk, heads, dh, 0, nullptr, nullptr, nullptr,
+                           nullptr, s);
+    }
+    { ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * rows * HD, s); window_rows<T>(ow, HD, out, ldo, HD, *win, rows, false, s); }
+    return;
+  }
   ProfScope ps(this, PROF_ATTN, 4.0 * B * heads * nq * nk * dh + (variant == 1 ? 2.0 : variant == 2 ? 4.0 : 0.0) * B * nq * nk * heads * heads,
                static_cast<double>(sizeof(T)) * B * heads * dh * (2.0 * nq + 2.0 * nk), s);
   if (attention_fast<T>(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, heads, dh, variant, mix_a, mix_b, g, b, s, scale)) return;
@@ -2011,6 +2307,7 @@ void validate(const vb_config& c) {
            "vb_config.struct_size mismatch (ABI)");
   VB_CHECK(c.kind != VB_KIND_LEVIT, "LeViT: create the handle with vb_create_levit (its stages are a vb_levit_config)");
   VB_CHECK(c.kind != VB_KIND_CVT, "CvT: create the handle with vb_create_cvt (its stages are a vb_cvt_config)");
+  VB_CHECK(c.kind != VB_KIND_TWINS_SVT, "Twins-SVT: create the handle with vb_create_twins_svt (its stages are a vb_twins_svt_config)");
   VB_CHECK(c.kind >= VB_KIND_VIT && c.kind <= VB_KIND_CCT, "unknown model kind");
   if (c.kind == VB_KIND_CCT) {
     VB_CHECK(c.channels == 3 && c.num_classes > 0 && c.image_h > 0 && c.image_w > 0, "bad image / class configuration");
@@ -2078,6 +2375,15 @@ void validate_cvt(const vb_config& c, const vb_cvt_config& cv) {
     VB_CHECK(cv.proj_kernel[st] >= 1 && cv.proj_kernel[st] <= 7, "CvT: proj_kernel must be in [1, 7] (the depthwise kernel's halo tile)");
     VB_CHECK(cv.kv_proj_stride[st] == 1 || cv.kv_proj_stride[st] == 2, "CvT: kv_proj_stride must be 1 or 2");
   }
+}
+
+void validate_twins(const vb_config& c, const vb_twins_svt_config& tw) {
+  VB_CHECK(c.precision == VB_PRECISION_FP32 || c.precision == VB_PRECISION_BF16, "unknown precision");
+  VB_CHECK(c.channels > 0 && c.num_classes > 0, "Twins-SVT: bad channel / class configuration");
+  for (int st = 0; st < VB_TWINS_STAGES; ++st)
+    VB_CHECK(tw.emb_dim[st] > 0 && tw.patch_size[st] > 0 && tw.local_patch_size[st] > 0 && tw.global_k[st] > 0 && tw.depth[st] >= 0,
+             "Twins-SVT: bad stage configuration");
+  VB_CHECK(tw.peg_kernel_size >= 1 && tw.peg_kernel_size <= 7, "Twins-SVT: peg_kernel_size must be in [1, 7] (the depthwise kernel's halo tile)");
 }
 
 }  // namespace
@@ -2258,6 +2564,35 @@ int vb_create_cvt(const vb_config* base, const vb_cvt_config* cvt, int device, v
   });
 }
 
+int vb_create_twins_svt(const vb_config* base, const vb_twins_svt_config* tw, int device, vb_handle** out) {
+  return guarded(nullptr, [&] {
+    VB_CHECK(base != nullptr && tw != nullptr && out != nullptr, "vb_create_twins_svt: null argument");
+    VB_CHECK(base->struct_size == static_cast<int32_t>(sizeof(vb_config)) || base->struct_size == VB_CONFIG_SIZE_ABI7,
+             "vb_config.struct_size mismatch (ABI)");
+    VB_CHECK(tw->struct_size == static_cast<int32_t>(sizeof(vb_twins_svt_config)), "vb_twins_svt_config.struct_size mismatch (ABI)");
+    vb_config c;
+    memset(&c, 0, sizeof c);
+    memcpy(&c, base, static_cast<size_t>(base->struct_size));
+    VB_CHECK(c.kind == VB_KIND_TWINS_SVT, "vb_create_twins_svt: base.kind must be VB_KIND_TWINS_SVT");
+    validate_twins(c, *tw);
+    int ndev = 0;
+    cudaError_t e = cudaGetDeviceCount(&ndev);
+    VB_CHECK(e == cudaSuccess && ndev > 0, "vb_create_twins_svt: no CUDA device available -- libvitb200 has no CPU fallback");
+    VB_CHECK(device >= 0 && device < ndev, "vb_create_twins_svt: bad device index");
+    VB_CUDA(cudaSetDevice(device));
+    cudaDeviceProp prop;
+    VB_CUDA(cudaGetDeviceProperties(&prop, device));
+    VB_CHECK(prop.major == 9 && prop.minor == 0, "vb_create_twins_svt: libvitb200 is built for sm_90a (Hopper H100) only");
+    std::unique_ptr<vb_handle> h(new vb_handle());
+    h->cfg = c;
+    h->cfg.dim = tw->emb_dim[VB_TWINS_STAGES - 1];
+    h->tw = *tw;
+    h->device = device;
+    h->build_expected();
+    *out = h.release();
+  });
+}
+
 int vb_num_weights(vb_handle* h) { return h ? static_cast<int>(h->weights.size()) : -1; }
 
 int vb_weight_info(vb_handle* h, int32_t index, const char** name, int64_t* shape4, int32_t* ndim) {
@@ -2382,6 +2717,7 @@ int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, int32_t 
     VB_CHECK(h->finalized, "vb_forward_distill: call vb_finalize after setting the weights");
     VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_forward_distill: bad batch / image size");
     VB_CHECK(h->cfg.kind != VB_KIND_CVT, "vb_forward_distill: CvT has no distillation head");
+    VB_CHECK(h->cfg.kind != VB_KIND_TWINS_SVT, "vb_forward_distill: Twins-SVT has no distillation head");
     const bool levit = h->cfg.kind == VB_KIND_LEVIT;
     VB_CHECK(levit || distill_token != nullptr, "vb_forward_distill: null argument");
     VB_CHECK(!levit || (distill_token == nullptr && h->lv.num_distill_classes > 0),
@@ -2438,6 +2774,7 @@ int vb_forward_tokens(vb_handle* h, const float* tokens, int32_t tokens_mem, int
     VB_CHECK(h->finalized, "vb_forward_tokens: call vb_finalize after setting the weights");
     VB_CHECK(batch > 0 && n > 0, "vb_forward_tokens: bad shape");
     VB_CHECK(h->cfg.kind != VB_KIND_CVT, vb_handle::kCvtNoStages);
+    VB_CHECK(h->cfg.kind != VB_KIND_TWINS_SVT, vb_handle::kTwinsNoStages);
     VB_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const long long before = launch_counter();
@@ -2507,7 +2844,8 @@ int vb_to_patch(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, 
   return guarded(h, [&] {
     VB_CHECK(h != nullptr && img != nullptr && patches != nullptr, "vb_to_patch: null argument");
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT && h->cfg.kind != VB_KIND_T2T_VIT && h->cfg.kind != VB_KIND_CCT &&
-             h->cfg.kind != VB_KIND_LEVIT && h->cfg.kind != VB_KIND_CVT, "vb_to_patch: the model has no single Rearrange patch layer");
+             h->cfg.kind != VB_KIND_LEVIT && h->cfg.kind != VB_KIND_CVT && h->cfg.kind != VB_KIND_TWINS_SVT,
+             "vb_to_patch: the model has no single Rearrange patch layer");
     VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_to_patch: bad batch / image size");
     const vb_config& c = h->cfg;
     VB_CHECK(img_h % c.patch_h == 0 && img_w % c.patch_w == 0, "Image dimensions must be divisible by the patch size.");
@@ -2529,6 +2867,7 @@ int vb_patch_to_emb(vb_handle* h, const float* patches, int32_t patches_mem, int
     VB_CHECK(h->cfg.kind != VB_KIND_CCT, vb_handle::kCctNoStages);
     VB_CHECK(h->cfg.kind != VB_KIND_LEVIT, vb_handle::kLevitNoStages);
     VB_CHECK(h->cfg.kind != VB_KIND_CVT, vb_handle::kCvtNoStages);
+    VB_CHECK(h->cfg.kind != VB_KIND_TWINS_SVT, vb_handle::kTwinsNoStages);
     VB_CHECK(rows > 0, "vb_patch_to_emb: bad shape");
     const size_t in_bytes = static_cast<size_t>(rows) * h->embed.patch.K * sizeof(float);
     const size_t out_bytes = static_cast<size_t>(rows) * h->cfg.dim * sizeof(float);
@@ -2965,6 +3304,44 @@ int vb_op_dwconv(int32_t precision, const float* x, int32_t B, int32_t H, int32_
     else run(float());
     for (size_t r = 0; r < M; ++r) std::copy(qh.begin() + r * Cp, qh.begin() + r * Cp + C, q + r * C);
     for (size_t r = 0; r < Mk; ++r) std::copy(kvh.begin() + r * Cp, kvh.begin() + r * Cp + C, kv + r * C);
+  });
+}
+
+int vb_op_window_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t H, int32_t W, int32_t p, int32_t heads,
+                           int32_t dh, float* out, int32_t ldo, int32_t iters, float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    const int HD = heads * dh;
+    VB_CHECK(qkv && out && B > 0 && p > 0 && H > 0 && W > 0 && H % p == 0 && W % p == 0 && heads > 0 && dh > 0 && ld >= 3 * HD && ldo >= HD,
+             "vb_op_window_attention: bad arguments");
+    Window win;
+    win.p = p; win.nx = W / p; win.ny = H / p;
+    const int n = p * p, Bw = B * win.nx * win.ny;
+    const long long rows = static_cast<long long>(B) * H * W;
+    DevMem dX, dO, dW, dOw, dS;
+    auto run = [&](auto tag) {
+      using T = decltype(tag);
+      const T* x_d = upload<T>(dX, qkv, static_cast<size_t>(rows) * ld);
+      T* o_d = upload<T>(dO, out, static_cast<size_t>(rows) * ldo);
+      // vb_handle::attention_dispatch's windowed branch without the handle's arena and profiler
+      timed(iters, elapsed_ms, [&] {
+        if (attention_fast<T>(x_d, ld, x_d + HD, ld, x_d + 2 * HD, ld, o_d, ldo, Bw, n, n, heads, dh, 0, nullptr, nullptr, nullptr, nullptr, 0, 0.f,
+                              nullptr, &win))
+          return;
+        dW.ensure(static_cast<size_t>(rows) * 3 * HD * sizeof(T));
+        dOw.ensure(static_cast<size_t>(rows) * HD * sizeof(T));
+        dS.ensure(static_cast<size_t>(Bw) * heads * n * ((n + 15) & ~15) * sizeof(float));
+        T* w_d = static_cast<T*>(dW.p);
+        T* ow_d = static_cast<T*>(dOw.p);
+        window_rows<T>(x_d, ld, w_d, 3 * HD, 3 * HD, win, rows, true, 0);
+        attention_generic<T>(w_d, 3 * HD, w_d + HD, 3 * HD, w_d + 2 * HD, 3 * HD, ow_d, HD, static_cast<float*>(dS.p), Bw, n, n, heads, dh, 0,
+                             nullptr, nullptr, nullptr, nullptr, 0);
+        window_rows<T>(ow_d, HD, o_d, ldo, HD, win, rows, false, 0);
+      });
+      download<T>(o_d, out, static_cast<size_t>(rows) * ldo);
+    };
+    if (precision == VB_PRECISION_FP32) run(float());
+    else run(__nv_bfloat16());
   });
 }
 

@@ -604,9 +604,21 @@ __global__ void broadcast_rows_kernel(const float* __restrict__ vec, T* __restri
 // element would cost six divisions each, two of them 64-bit).
 // C >= 32 (the 147-channel layers): the threads walk the k*k taps and copy each tap's C contiguous channels;
 // small C (the image, C = 3): one thread per column with 32-bit divisions.
+// stats (UnfoldMode, may be null): the pixel's LayerNorm from its (sum, sumsq) partials, applied on load.
+__device__ __forceinline__ float2 unfold_ln(const float2* __restrict__ stats, int parts, long long M, long long pix, float inv_d, float eps) {
+  float s1 = 0.f, s2 = 0.f;
+  for (int j = 0; j < parts; ++j) {
+    const float2 v = __ldg(stats + j * M + pix);
+    s1 += v.x;
+    s2 += v.y;
+  }
+  const float m = s1 * inv_d;
+  return make_float2(m, rsqrtf(fmaxf(s2 * inv_d - m * m, 0.f) + eps));
+}
 template <typename TI, typename TO>
 __global__ void unfold_same_kernel(const TI* __restrict__ in, int ldi, TO* __restrict__ out, int B, int H, int W, int C, int k, int stride,
-                                   int oh, int ow, int pad_top, int pad_left, int cls_row, int ldo) {
+                                   int oh, int ow, int pad_top, int pad_left, int cls_row, int ldo, const float2* __restrict__ stats,
+                                   int parts, float inv_d, float eps, const float* __restrict__ gamma, const float* __restrict__ beta) {
   const int rows = cls_row + oh * ow;
   const int K = k * k * C;
   const int r = blockIdx.x;                                    // (b, t): B * rows CTAs
@@ -627,7 +639,12 @@ __global__ void unfold_same_kernel(const TI* __restrict__ in, int ldi, TO* __res
       const bool inside = y >= 0 && y < H && x >= 0 && x < W;
       const TI* __restrict__ src = img + (static_cast<size_t>(inside ? y : 0) * W + (inside ? x : 0)) * ldi;
       TO* __restrict__ dst = orow + tap * C;
-      for (int c = threadIdx.x; c < C; c += blockDim.x) dst[c] = from_f<TO>(inside ? to_f(src[c]) : 0.f);
+      if (stats != nullptr && inside) {
+        const float2 mr = unfold_ln(stats, parts, static_cast<long long>(B) * H * W, (static_cast<long long>(b) * H + y) * W + x, inv_d, eps);
+        for (int c = threadIdx.x; c < C; c += blockDim.x) dst[c] = from_f<TO>((to_f(src[c]) - mr.x) * mr.y * gamma[c] + beta[c]);
+      } else {
+        for (int c = threadIdx.x; c < C; c += blockDim.x) dst[c] = from_f<TO>(inside ? to_f(src[c]) : 0.f);
+      }
     }
   } else {
     const int kC = k * C;
@@ -636,11 +653,27 @@ __global__ void unfold_same_kernel(const TI* __restrict__ in, int ldi, TO* __res
       const int kx = rem / C, c = rem - kx * C;
       const int y = y0 + ky, x = x0 + kx;
       float v = 0.f;
-      if (y >= 0 && y < H && x >= 0 && x < W) v = to_f(img[(static_cast<size_t>(y) * W + x) * ldi + c]);
+      if (y >= 0 && y < H && x >= 0 && x < W) {
+        v = to_f(img[(static_cast<size_t>(y) * W + x) * ldi + c]);
+        if (stats != nullptr) {
+          const float2 mr = unfold_ln(stats, parts, static_cast<long long>(B) * H * W, (static_cast<long long>(b) * H + y) * W + x, inv_d, eps);
+          v = (v - mr.x) * mr.y * gamma[c] + beta[c];
+        }
+      }
       orow[col] = from_f<TO>(v);
     }
   }
   for (int col = K + threadIdx.x; col < ldo; col += blockDim.x) orow[col] = from_f<TO>(0.f);   // pitch padding
+}
+
+// One CTA per window-major row.
+template <typename T>
+__global__ void window_rows_kernel(const T* __restrict__ in, int ldi, T* __restrict__ out, int ldo, int cols, Window win, int n,
+                                   bool to_window) {
+  const long long t = blockIdx.x, px = win.row(t / n, static_cast<int>(t % n));
+  const T* __restrict__ src = in + (to_window ? px : t) * ldi;
+  T* __restrict__ dst = out + (to_window ? t : px) * ldo;
+  for (int c = threadIdx.x; c < cols; c += blockDim.x) dst[c] = src[c];
 }
 
 // One thread per output element (b, t, c), c fastest: the k*k taps of a thread are C apart, so a warp reads whole channel runs.
@@ -909,7 +942,7 @@ dwconv_qkv_kernel(const T* __restrict__ x, int ldx, const float2* __restrict__ s
   for (int i = threadIdx.x; i < K * K * DW_CG; i += DW_THREADS) {
     const int t = i / DW_CG, cc = c0 + i % DW_CG;
     tq[t][i % DW_CG] = cc < C ? __ldg(wq + static_cast<size_t>(t) * C + cc) : 0.f;
-    tkv[t][i % DW_CG] = cc < C ? __ldg(wkv + static_cast<size_t>(t) * C + cc) : 0.f;
+    tkv[t][i % DW_CG] = (wkv != nullptr && cc < C) ? __ldg(wkv + static_cast<size_t>(t) * C + cc) : 0.f;
   }
   if (stats != nullptr) {
     for (int p = threadIdx.x; p < P; p += DW_THREADS) {
@@ -944,7 +977,8 @@ dwconv_qkv_kernel(const T* __restrict__ x, int ldx, const float2* __restrict__ s
   __syncthreads();
   const int oy = y0 + row;
   if (oy < H && cok) dw_conv_row<T, K>(tile, tq, bq[c], q + ((b * H + oy) * W + x0) * ldq + c, ldq, row, lane, W - x0);
-  if (kv_stride == 1) {
+  if (kv == nullptr) {
+  } else if (kv_stride == 1) {
     if (oy < H && cok) dw_conv_row<T, K>(tile, tkv, bkv[c], kv + ((b * H + oy) * W + x0) * ldkv + c, ldkv, row, lane, W - x0);
   } else if (row < DW_T / 2 && cok) {                            // stride 2: outputs (y0/2 + row, x0/2 + xx), xx < DW_T/2
     const int r = y0 / 2 + row;
@@ -1136,14 +1170,32 @@ void broadcast_rows(const float* vec, T* dst, int B, int nt, int D, cudaStream_t
 }
 
 template <typename TI, typename TO>
-void unfold_same(const TI* in, TO* out, int B, int H, int W, int C, int k, int stride, int cls_row, int ldo, cudaStream_t s, int ldi) {
+void unfold_same(const TI* in, TO* out, int B, int H, int W, int C, int k, int stride, int cls_row, int ldo, cudaStream_t s, int ldi,
+                 const UnfoldMode* mode) {
   if (ldi <= 0) ldi = C;
-  const int oh = (H + stride - 1) / stride, ow = (W + stride - 1) / stride;
-  const int ph = (oh - 1) * stride + k > H ? (oh - 1) * stride + k - H : 0, pw = (ow - 1) * stride + k > W ? (ow - 1) * stride + k - W : 0;
+  const bool valid = mode != nullptr && mode->valid;
+  const int oh = valid ? (H - k) / stride + 1 : (H + stride - 1) / stride, ow = valid ? (W - k) / stride + 1 : (W + stride - 1) / stride;
+  VB_CHECK(!valid || (H >= k && W >= k), "unfold_same: a VALID window larger than the map");
+  const int ph = !valid && (oh - 1) * stride + k > H ? (oh - 1) * stride + k - H : 0;
+  const int pw = !valid && (ow - 1) * stride + k > W ? (ow - 1) * stride + k - W : 0;
   const long long rows_total = static_cast<long long>(B) * (cls_row + oh * ow);
   VB_CHECK(rows_total > 0 && rows_total < (1ll << 31), "unfold_same: B * rows out of range");
+  const float2* stats = mode != nullptr ? reinterpret_cast<const float2*>(mode->stats) : nullptr;
+  VB_CHECK(stats == nullptr || (mode->parts > 0 && mode->d > 0 && mode->gamma != nullptr && mode->beta != nullptr),
+           "unfold_same: LayerNorm statistics without their width / gamma / beta");
   const int threads = C >= 128 ? 160 : (C >= 32 ? 64 : (k * k * C >= 128 ? 160 : 64));
-  unfold_same_kernel<TI, TO><<<static_cast<unsigned>(rows_total), threads, 0, s>>>(in, ldi, out, B, H, W, C, k, stride, oh, ow, ph / 2, pw / 2, cls_row, ldo);
+  unfold_same_kernel<TI, TO><<<static_cast<unsigned>(rows_total), threads, 0, s>>>(
+      in, ldi, out, B, H, W, C, k, stride, oh, ow, ph / 2, pw / 2, cls_row, ldo, stats, stats ? mode->parts : 0,
+      stats ? 1.0f / static_cast<float>(mode->d) : 0.f, stats ? mode->eps : 0.f, stats ? mode->gamma : nullptr, stats ? mode->beta : nullptr);
+  VB_LAUNCHED();
+}
+
+template <typename T>
+void window_rows(const T* in, int ldi, T* out, int ldo, int cols, const Window& win, long long rows, bool to_window, cudaStream_t s) {
+  const int n = win.p * win.p;
+  VB_CHECK(n > 0 && rows % n == 0 && rows < (1ll << 31), "window_rows: rows must be whole windows, fewer than 2^31");
+  if (rows == 0) return;
+  window_rows_kernel<T><<<static_cast<unsigned>(rows), cols >= 256 ? 256 : 128, 0, s>>>(in, ldi, out, ldo, cols, win, n, to_window);
   VB_LAUNCHED();
 }
 
@@ -1246,7 +1298,8 @@ void dwconv_qkv(const T* x, int ldx, const float* stats, const float* gamma, con
   template void copy_tokens<T>(const T*, int, int, T*, int, int, int, int, int, cudaStream_t);                              \
   template void broadcast_row<T>(const float*, T*, int, int, int, cudaStream_t);                                            \
   template void broadcast_rows<T>(const float*, T*, int, int, int, cudaStream_t);                                           \
-  template void unfold_same<float, T>(const float*, T*, int, int, int, int, int, int, int, int, cudaStream_t, int);         \
+  template void unfold_same<float, T>(const float*, T*, int, int, int, int, int, int, int, int, cudaStream_t, int, const UnfoldMode*); \
+  template void window_rows<T>(const T*, int, T*, int, int, const Window&, long long, bool, cudaStream_t);                   \
   template void convert_rows<float, T>(const float*, int, T*, int, long long, int, cudaStream_t);                           \
   template void maxpool_relu_same<T>(const T*, T*, int, int, int, int, int, int, const float*, int, cudaStream_t);         \
   template void seq_pool<T>(const T*, int, int, const float*, const float*, const float*, const float*, float*, int, cudaStream_t); \
@@ -1261,7 +1314,7 @@ template void gemm_simt<__nv_bfloat16, __nv_bfloat16, __nv_bfloat16>(const __nv_
                                                                      __nv_bfloat16*, int, int, int, int, const float*,
                                                                      const float*, const __nv_bfloat16*, int, int, cudaStream_t);
 template void unfold_same<__nv_bfloat16, __nv_bfloat16>(const __nv_bfloat16*, __nv_bfloat16*, int, int, int, int, int, int, int, int,
-                                                        cudaStream_t, int);
+                                                        cudaStream_t, int, const UnfoldMode*);
 template void convert_rows<__nv_bfloat16, float>(const __nv_bfloat16*, int, float*, int, long long, int, cudaStream_t);
 template void convert<float, __nv_bfloat16>(const float*, __nv_bfloat16*, long long, cudaStream_t);
 template void convert<__nv_bfloat16, float>(const __nv_bfloat16*, float*, long long, cudaStream_t);

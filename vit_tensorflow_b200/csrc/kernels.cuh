@@ -59,7 +59,7 @@ template <typename T>
 void gather_grid(const T* in, int ldi, T* out, int ldo, int B, int H, int W, int C, int step, cudaStream_t s);
 
 // CvT's attention projections up to the pointwise convolutions (cvt.py:79-92,103-104), both depthwise convolutions of a block
-// from one read of the input: q = dw_q(y) (stride 1) and kv = dw_kv(y) (stride kv_stride: 1 or 2), k x k (k <= 7), TF SAME
+// from one read of the input (kv == null: the q map only, Twins-SVT's PEG with its residual folded into the centre tap): q = dw_q(y) (stride 1) and kv = dw_kv(y) (stride kv_stride: 1 or 2), k x k (k <= 7), TF SAME
 // padding (total max((out - 1) * stride + k - in, 0), the smaller half first), then + a per-channel shift.
 //   x [B*H*W, ldx] NHWC rows; y = LN(x) when stats != null: the rows' (sum, sumsq) partials [C/64][B*H*W] (the GEMM epilogue's
 //   stats_out format) over D true columns with eps, times gamma plus beta ([C], zero on pad channels); y = x when stats == null.
@@ -89,9 +89,27 @@ void broadcast_rows(const float* vec, T* dst, int B, int nt, int D, cudaStream_t
 // T2T soft split (t2t.py:43-44): tf.image.extract_patches(sizes k, strides `stride`, rates 1, padding SAME) +
 // 'b h w c -> b (h w) c'.  in [B,H,W,C] (image or token map) -> out [B*(cls_row + oh*ow), ldo], oh = ceil(H/stride);
 // columns [0, k*k*C) hold the patch vector ((k_row, k_col, c), c fastest), [.., ldo) and the optional cls row are zero.
-// ldi: pitch of one input pixel's channel vector (0 = C).
+// ldi: pitch of one input pixel's channel vector (0 = C).  mode (may be null): see UnfoldMode.
+// Twins-SVT's global to_kv (twins_svt.py:168,180), Conv2D(k, stride k, VALID) of the PreNorm LayerNorm of the map: `valid` takes
+// floor((H - k) / stride) + 1 windows per side with no padding, and `stats` applies the LayerNorm on load from the pixels' (sum,
+// sumsq) partials [C_pitch/64][B*H*W] (the GEMM epilogue's stats_out format) over d true channels with eps, times gamma plus beta.
+// A folded LayerNorm cannot serve this GEMM: one patch row spans k^2 pixels with different statistics.
+struct UnfoldMode {
+  bool valid = false;
+  const float* stats = nullptr;
+  int parts = 0, d = 0;
+  float eps = 1e-5f;
+  const float *gamma = nullptr, *beta = nullptr;
+};
 template <typename TI, typename TO>
-void unfold_same(const TI* in, TO* out, int B, int H, int W, int C, int k, int stride, int cls_row, int ldo, cudaStream_t s, int ldi = 0);
+void unfold_same(const TI* in, TO* out, int B, int H, int W, int C, int k, int stride, int cls_row, int ldo, cudaStream_t s, int ldi = 0,
+                 const UnfoldMode* mode = nullptr);
+
+// Rows of a pixel-major map <-> window-major order (the fallback of the windowed attention, common.h Window): window-major row
+// t = bw * p^2 + i is the map's row win.row(bw, i).  to_window: out[t] = in[win.row(t)]; else out[win.row(t)] = in[t].  `cols`
+// columns of `rows` = (number of windows) * p^2 rows.
+template <typename T>
+void window_rows(const T* in, int ldi, T* out, int ldo, int cols, const Window& win, long long rows, bool to_window, cudaStream_t s);
 
 // CCT tokenizer tail (cct.py:196-200,213): ReLU -> MaxPool2D(k, stride, padding 'SAME') -> 'b h w c -> b (h w) c', NHWC.
 // in [B, H, W, C] -> out [B, rows, C], oh = ceil(H / stride), rows >= oh * ow; total padding max((oh-1)*stride + k - H, 0) with

@@ -6,6 +6,7 @@
     T2TViT    vit_tensorflow/t2t.py:50-116           vit_with_patch_merger.ViT / PatchMerger  vit_with_patch_merger.py:42-55,134-185
     efficient.ViT  vit_tensorflow/efficient.py:12-55 (injected transformer between the engine's embed and head stages)
     CvT       vit_tensorflow/cvt.py:149-202
+    TwinsSVT  vit_tensorflow/twins_svt.py:215-268
 
 Same constructor kwargs, defaults and assertion messages; `model(img, training=True, **kwargs) -> logits`
 with `img` NHWC float32 `[b, H, W, 3]` and logits float32 `[b, num_classes]`.  Everything below the call is
@@ -978,8 +979,139 @@ class CvT(_EngineModel):
 CVT_CTOR_KEYS = ("num_classes",) + tuple(f"s{i}_{k}" for i in (1, 2, 3) for k in CVT_STAGE_KEYS) + ("dropout",)
 
 
+TWINS_STAGE_KEYS = ("emb_dim", "patch_size", "local_patch_size", "global_k", "depth")
+
+
+def twins_size_error(stages, h, w):
+    """The reference's shape rules (twins_svt.py:103,141,168, enforced there by einops and Keras) for an h x w image: None, or
+    what the first stage that breaks one says."""
+    for i, st in enumerate(stages, 1):
+        ps = st["patch_size"]
+        if h % ps or w % ps:
+            return f"Twins-SVT stage {i}: the {h} x {w} map is not divisible by patch_size {ps}"
+        h, w = h // ps, w // ps
+        if i < len(stages) and (h % st["local_patch_size"] or w % st["local_patch_size"]):
+            return f"Twins-SVT stage {i}: the {h} x {w} map is not divisible by local_patch_size {st['local_patch_size']}"
+        if h < st["global_k"] or w < st["global_k"]:
+            return f"Twins-SVT stage {i}: the {h} x {w} map is smaller than global_k {st['global_k']} (a VALID convolution)"
+    return None
+
+
+class TwinsSVT(_EngineModel):
+    """twins_svt.py:215-268: four stages of PatchEmbedding (c-slowest patch vectors, 1x1 Conv2D), a Transformer of depth 1, the PEG
+    (x + a depthwise SAME convolution) and a Transformer of depth s{i}_depth, then GlobalAvgPool2D and Dense.  A Transformer layer
+    is local attention within local_patch_size windows, an MLP, global attention against the keys of a global_k x global_k stride
+    global_k VALID convolution, and an MLP, each PreNorm and residual; stage 4 has no local attention and no first MLP.  Every stage
+    has 8 heads of 64 and an MLP multiplier of 4, whatever emb_dim is: the reference never passes them to Transformer.
+
+    There are no position embeddings and no image_size: any image whose maps are divisible by every patch_size and, in stages 1-3,
+    local_patch_size, and are at least global_k on each side runs; other sizes raise ValueError naming the stage.  There is no
+    BatchNormalization, so with dropout = 0 training=True computes what training=False does.  peg_kernel_size must be in [1, 7].
+    Weights (SURVEY.md App. B) keep the reference's attribute paths: svt_layers.{s}.0.proj, svt_layers.{s}.{1|3}.layers.{l}.{0..3}
+    .fn.norm / .fn.fn.{to_q, to_kv, to_out.0, net.0, net.3}, svt_layers.{s}.2.proj.fn (PEG), svt_layers.4.1 (the Dense head)."""
+    _kind = "twins_svt"
+
+    def __init__(self,
+                 num_classes,
+                 s1_emb_dim=64,
+                 s1_patch_size=4,
+                 s1_local_patch_size=7,
+                 s1_global_k=7,
+                 s1_depth=1,
+                 s2_emb_dim=128,
+                 s2_patch_size=2,
+                 s2_local_patch_size=7,
+                 s2_global_k=7,
+                 s2_depth=1,
+                 s3_emb_dim=256,
+                 s3_patch_size=2,
+                 s3_local_patch_size=7,
+                 s3_global_k=7,
+                 s3_depth=5,
+                 s4_emb_dim=512,
+                 s4_patch_size=2,
+                 s4_local_patch_size=7,
+                 s4_global_k=7,
+                 s4_depth=4,
+                 peg_kernel_size=3,
+                 dropout=0.0,
+                 *, precision="bf16", device=0, seed=None):
+        kw = dict(locals())
+        self.num_classes = num_classes
+        self.stages = tuple({k: kw[f"s{i}_{k}"] for k in TWINS_STAGE_KEYS} for i in (1, 2, 3, 4))
+        self.peg_kernel_size = peg_kernel_size
+        self._dropout_rates = (dropout,)
+        if not 1 <= peg_kernel_size <= 7:
+            raise ValueError(f"Twins-SVT: peg_kernel_size {peg_kernel_size} is not supported (1 to 7)")
+        self.precision = precision
+        self.device = int(device)
+        cfg = _lib.VbConfig()
+        cfg.struct_size = C.sizeof(_lib.VbConfig)
+        cfg.kind = _lib.KIND["twins_svt"]
+        if precision not in _lib.PRECISION:
+            raise ValueError(f"precision must be one of {sorted(_lib.PRECISION)}")
+        cfg.precision = _lib.PRECISION[precision]
+        cfg.channels, cfg.num_classes = 3, num_classes
+        cfg.dim = self.stages[-1]["emb_dim"]
+        tw = _lib.VbTwinsSvtConfig()
+        tw.struct_size = C.sizeof(_lib.VbTwinsSvtConfig)
+        for i, st in enumerate(self.stages):
+            for k in TWINS_STAGE_KEYS:
+                getattr(tw, k)[i] = int(st[k])
+        tw.peg_kernel_size = int(peg_kernel_size)
+        self._cfg, self._tw = cfg, tw
+        self._lib = _lib.load()
+        h = C.c_void_p()
+        _lib.check(self._lib.vb_create_twins_svt(C.byref(cfg), C.byref(tw), self.device, C.byref(h)))
+        self._h = h
+        self._finalized = False
+        self._specs = collections.OrderedDict()
+        name, shape, ndim = C.c_char_p(), (C.c_int64 * 4)(), C.c_int32()
+        for i in range(self._lib.vb_num_weights(h)):
+            _lib.check(self._lib.vb_weight_info(h, i, C.byref(name), shape, C.byref(ndim)), h)
+            self._specs[name.value.decode()] = tuple(int(shape[j]) for j in range(ndim.value))
+        self._weights = collections.OrderedDict()
+        self.init_weights(seed)
+
+    def init_weights(self, seed=None):
+        """The reference's initialisers: glorot-uniform over the receptive field (the PEG's depthwise kernel [k, k, 1, dim] has fan_in
+        k^2 and fan_out k^2 * dim), zero biases, LayerNorm g 1 / b 0."""
+        rng = np.random.default_rng(seed)
+        w = collections.OrderedDict()
+        for name, shape in self._specs.items():
+            leaf = name.rsplit(".", 1)[-1]
+            if leaf == "kernel":
+                receptive = int(np.prod(shape[:-2]))
+                lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
+                a = rng.uniform(-lim, lim, size=shape)
+            elif leaf in ("bias", "b"):
+                a = np.zeros(shape)
+            elif leaf == "g":
+                a = np.ones(shape)
+            else:
+                raise AssertionError(name)
+            w[name] = a.astype(np.float32)
+        self.set_weights_dict(w)
+
+    def __call__(self, img, training=True, **kwargs):
+        """twins_svt.py:266-268: NHWC float images -> logits [b, num_classes]; extra kwargs are accepted and ignored, as there."""
+        x = np.asarray(img)
+        if x.ndim == 4:
+            err = twins_size_error(self.stages, x.shape[1], x.shape[2])
+            if err is not None:
+                raise ValueError(err)
+        return super().__call__(img, training=training)
+
+    call = __call__
+
+
+TWINS_CTOR_KEYS = ("num_classes",) + tuple(f"s{i}_{k}" for i in (1, 2, 3, 4) for k in TWINS_STAGE_KEYS) + ("peg_kernel_size", "dropout")
+
+
 def from_config(cfg: dict, precision="bf16", device=0, seed=None):
     """Build a model from an oracle-style config dict (kind + reference kwargs)."""
+    if cfg["kind"] == "twins_svt":
+        return TwinsSVT(**{k: v for k, v in cfg.items() if k in TWINS_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "cvt":
         return CvT(**{k: v for k, v in cfg.items() if k in CVT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "levit":
