@@ -13,6 +13,7 @@
  *     LeViT(...)(img)                vit_tensorflow/levit.py:164-226 (vb_create_levit; distillation head: vb_forward_distill)
  *     CvT(...)(img)                  vit_tensorflow/cvt.py:149-202 (vb_create_cvt)
  *     TwinsSVT(...)(img)             vit_tensorflow/twins_svt.py:215-268 (vb_create_twins_svt)
+ *     CrossFormer(...)(img)          vit_tensorflow/crossformer.py:205-269 (vb_create_crossformer)
  * and this header is what the Python host classes (vit_tensorflow_b200/models.py, _lib.py) bind with ctypes.
  * Plain pointers and sizes only; no torch / C++ types cross the boundary.
  *
@@ -43,7 +44,7 @@ typedef struct vb_handle vb_handle;
 
 enum { VB_KIND_VIT = 0, VB_KIND_DEEPVIT = 1, VB_KIND_CAIT = 2, VB_KIND_CROSSVIT = 3, VB_KIND_PARALLEL_VIT = 4,
        VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6, VB_KIND_CCT = 7, VB_KIND_LEVIT = 8,
-       VB_KIND_CVT = 9, VB_KIND_TWINS_SVT = 10 };
+       VB_KIND_CVT = 9, VB_KIND_TWINS_SVT = 10, VB_KIND_CROSSFORMER = 11 };
 enum { VB_CCT_POS_SINE = 0, VB_CCT_POS_LEARNABLE = 1, VB_CCT_POS_NONE = 2 };   /* cct.py:233-234,250-256 */
 enum { VB_PRECISION_FP32 = 0, VB_PRECISION_BF16 = 1 };
 enum { VB_POOL_CLS = 0, VB_POOL_MEAN = 1 };
@@ -87,8 +88,9 @@ typedef struct vb_config {
 
 VB_API int vb_abi_version(void);
 
-/* Replaces <Model>.__init__ (vit.py:107-157 etc.): validates the config and allocates device state.  VB_KIND_LEVIT, VB_KIND_CVT
- * and VB_KIND_TWINS_SVT are refused here: their handles come from vb_create_levit, vb_create_cvt and vb_create_twins_svt. */
+/* Replaces <Model>.__init__ (vit.py:107-157 etc.): validates the config and allocates device state.  VB_KIND_LEVIT, VB_KIND_CVT,
+ * VB_KIND_TWINS_SVT and VB_KIND_CROSSFORMER are refused here: their handles come from vb_create_levit, vb_create_cvt,
+ * vb_create_twins_svt and vb_create_crossformer. */
 VB_API int vb_create(const vb_config* cfg, int device, vb_handle** out);
 
 /* LeViT (levit.py:164-212), appended within ABI 7.  `dims`, `depths` and `heads` hold `stages` entries each (cast_tuple already
@@ -166,6 +168,40 @@ typedef struct vb_twins_svt_config {
  * svt_layers.4.1.kernel / .bias (the Dense head).  Stage 4 has no .0 / .1 sub-blocks. */
 VB_API int vb_create_twins_svt(const vb_config* base, const vb_twins_svt_config* tw, int device, vb_handle** out);
 
+/* CrossFormer (crossformer.py:205-269), appended within ABI 7: four stages, each a CrossEmbedLayer (:30-48: one SAME Conv2D with
+ * bias per kernel size, strides `stride`, the kernel sizes sorted, dim / 2, dim / 4, ... channels and the rest for the largest,
+ * concatenated in sorted order) and a Transformer of `depth` layers x = short(x) + x, x = mlp(x) + x, x = long(x) + x,
+ * x = mlp(x) + x (:196-203).  Attention (:104-180): the module's LayerNorm (eps 1e-5), heads = dim / 32 of width 32, a bias-free
+ * 1x1 q|k|v, scores q k^T * 32^-0.5 plus a DynamicPositionBias scalar per in-window offset shared by the heads, softmax, a 1x1
+ * to_out with bias; short attention within the local_wsz x local_wsz blocks of the map, long attention within the global_wsz x
+ * global_wsz dilated windows (pixels (l1 H / wsz + y, l2 W / wsz + x)).  MLP (:89-102): LayerNorm, 1x1 to 4 dim, exact GELU, 1x1
+ * back.  Head: the mean over the map, Dense(num_classes).  Any image whose every stage map (ceil(prev / stride)) is divisible by
+ * that stage's local_wsz and global_wsz runs.  The engine runs the cross-scale embedding as one convolution of the largest kernel
+ * with the smaller ones nested at its centre, exact for every image size when the stage's kernels share one parity and are all
+ * at least its stride; other stages are refused. */
+#define VB_CROSSFORMER_STAGES 4
+#define VB_CROSSFORMER_MAX_KERNELS 4
+typedef struct vb_crossformer_config {
+  int32_t struct_size;            /* sizeof(vb_crossformer_config) */
+  int32_t dim[VB_CROSSFORMER_STAGES], depth[VB_CROSSFORMER_STAGES], global_wsz[VB_CROSSFORMER_STAGES];
+  int32_t local_wsz[VB_CROSSFORMER_STAGES], stride[VB_CROSSFORMER_STAGES];
+  int32_t n_kernels[VB_CROSSFORMER_STAGES];                               /* 1 .. VB_CROSSFORMER_MAX_KERNELS */
+  int32_t kernels[VB_CROSSFORMER_STAGES][VB_CROSSFORMER_MAX_KERNELS];     /* the first n_kernels[s] entries, any order */
+} vb_crossformer_config;
+
+/* CrossFormer.__init__: `base` supplies precision, channels, num_classes and max_batch; its kind must be VB_KIND_CROSSFORMER and
+ * its other fields are ignored.  Weights (SURVEY.md App. B) are named by the reference's attribute paths, for stage s, layer l,
+ * attention sub-block a in {0 (short), 2 (long)} and MLP sub-block m in {1, 3}:
+ *   crossformer_layers.{s}.0.convs.{i}.kernel [k_i, k_i, cin, dim_i] / .bias [dim_i]      (i-th kernel size in sorted order)
+ *   crossformer_layers.{s}.1.layers.{l}.{a}.norm.g / .b [1, 1, 1, dim]
+ *   ....{a}.to_qkv.kernel [1, 1, dim, 3 * 32 * heads], ....{a}.to_out.kernel [1, 1, 32 * heads, dim] / .bias [dim]
+ *   ....{a}.dpb.dpb_layers.{0,3,6}.kernel [2 | dim/4, dim/4] / .bias [dim/4], ....{a}.dpb.dpb_layers.9.kernel [dim/4, 1] / .bias [1],
+ *   ....{a}.dpb.dpb_layers.{1,4,7}.gamma / .beta [dim/4]                                  (Keras LayerNormalization, eps 1e-3)
+ *   ....{m}.net.0.g / .b [1, 1, 1, dim], ....{m}.net.1.kernel [1, 1, dim, 4 dim] / .bias, ....{m}.net.4.kernel [1, 1, 4 dim, dim] / .bias
+ *   to_logits.1.kernel [dim, num_classes] / .bias
+ * vb_finalize evaluates every DynamicPositionBias on the host: it depends on the weights alone. */
+VB_API int vb_create_crossformer(const vb_config* base, const vb_crossformer_config* cf, int device, vb_handle** out);
+
 /* Replaces Keras variable assignment: one call per weight, names/shapes/layouts per SURVEY.md App. B
  * (Dense kernel [in,out], float32).  shape/ndim are checked against the config. */
 VB_API int vb_set_weight(vb_handle* h, const char* name, const float* host_data, const int64_t* shape, int32_t ndim);
@@ -208,7 +244,7 @@ VB_API int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, i
 
 /* ---- the stages of <Model>.call on their own (SURVEY.md 8f f1/f4): the attribute surface the reference's wrappers and the
  * injected-transformer shell use.  ViT / DeepViT / parallel ViT / CaiT / patch-merger ViT / T2TViT; not CrossViT, CCT, LeViT,
- * CvT or Twins-SVT. */
+ * CvT, Twins-SVT or CrossFormer. */
 
 /* Number of token rows vb_forward_embed produces for an img_h x img_w image (patches + cls where the model has one);
  * negative on error. */
@@ -288,6 +324,9 @@ VB_API int32_t vb_last_attention_path(void);
  * local q|k|v, the global to_q and to_kv are 0; local and global attention 1 (a windowed attention off the flash kernel adds its
  * row permutations to 4); the PEG depthwise convolution (one per stage) 4; the LayerNorm-folded GELU fc1 5; the residual to_out /
  * fc2 6; row statistics and the average pool 2 (the fp32 engine adds its separate LayerNorms to 2).
+ * CrossFormer: the cross-scale embeddings' unfold is 3 and their convolution 0; the LayerNorm-folded q|k|v (or v alone for
+ * one-token windows) 0; short and long attention 1 (off the flash kernel the row permutations are 4); the LayerNorm-folded GELU
+ * fc1 5; the residual to_out / fc2 6; the average pool 2 (the fp32 engine adds its separate LayerNorms to 2).
  * vb_profile_read synchronises the device and returns accumulated milliseconds, algorithmic FLOPs, algorithmic
  * bytes and launch counts per class (arrays of VB_PROF_NUM); reset != 0 clears the accumulators. */
 #define VB_PROF_NUM 7
@@ -391,6 +430,16 @@ VB_API int vb_op_dwconv(int32_t precision, const float* x, int32_t B, int32_t H,
  * permute back (vb_last_attention_path tells which). */
 VB_API int vb_op_window_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t H, int32_t W, int32_t p,
                                   int32_t heads, int32_t dh, float* out, int32_t ldo, int32_t iters, float* elapsed_ms);
+
+/* CrossFormer's attention (crossformer.py:141-172) as the engine runs it: vb_op_window_attention's layout with windows of
+ * wsz x wsz tokens, contiguous blocks (is_long == 0) or the dilated windows of the long attention (is_long != 0: token (l1, l2) of
+ * window (y, x) is the pixel (l1 H / wsz + y, l2 W / wsz + x)), and every score plus table[(dr + wsz - 1) * (2 wsz - 1) + dc + wsz
+ * - 1] for the in-window offset (dr, dc) of query and key; table: (2 wsz - 1)^2 floats, shared by the heads.  Scale dh^-0.5.  bf16
+ * with dh 32 or 64 and wsz <= 32 runs the windowed-bias flash kernel in place; every fp32 call and any shape it refuses permute
+ * the rows, run the materialised-scores path with the table added and permute back (vb_last_attention_path tells which). */
+VB_API int vb_op_window_bias_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t H, int32_t W, int32_t wsz,
+                                       int32_t is_long, int32_t heads, int32_t dh, const float* table, float* out, int32_t ldo,
+                                       int32_t iters, float* elapsed_ms);
 
 /* Row softmax of fp32 scores into bf16 probabilities (the T2T attention): p[r, j] = softmax_j(s[r, j] * scale) for j < n,
  * p[r, n..npad) = 0.  s [rows, lds], p [rows, ldp] (uploaded and downloaded whole); n <= npad <= ldp. */

@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "libvitb200.so")   # VB_LIB_PATH: developer A/B builds
 
 KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6, "cct": 7, "levit": 8,
-        "cvt": 9, "twins_svt": 10}
+        "cvt": 9, "twins_svt": 10, "crossformer": 11}
 PRECISION = {"fp32": 0, "float32": 0, "bf16": 1, "bfloat16": 1}
 MEM_HOST, MEM_DEVICE = 0, 1
 ABI_VERSION = 7                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
@@ -58,6 +58,15 @@ class VbTwinsSvtConfig(C.Structure):
         "emb_dim", "patch_size", "local_patch_size", "global_k", "depth")] + [("peg_kernel_size", C.c_int32)]
 
 
+CROSSFORMER_STAGES, CROSSFORMER_MAX_KERNELS = 4, 4  # VB_CROSSFORMER_STAGES, VB_CROSSFORMER_MAX_KERNELS
+
+
+class VbCrossformerConfig(C.Structure):
+    _fields_ = [("struct_size", C.c_int32)] + [(n, C.c_int32 * CROSSFORMER_STAGES) for n in (
+        "dim", "depth", "global_wsz", "local_wsz", "stride", "n_kernels")] + [
+        ("kernels", (C.c_int32 * CROSSFORMER_MAX_KERNELS) * CROSSFORMER_STAGES)]
+
+
 class VbError(RuntimeError):
     pass
 
@@ -72,6 +81,7 @@ SIGNATURES = {
     "vb_create_levit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbLevitConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_cvt": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbCvtConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_twins_svt": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbTwinsSvtConfig), C.c_int, C.POINTER(C.c_void_p)]),
+    "vb_create_crossformer": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbCrossformerConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, _i64p, C.c_int32]),
     "vb_num_weights": (C.c_int, [C.c_void_p]),
     "vb_weight_info": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), _i64p, C.POINTER(C.c_int32)]),
@@ -109,6 +119,8 @@ SIGNATURES = {
     "vb_op_dwconv": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 2 + [C.c_int32] * 2 + [C.c_void_p] * 6 +
                      [C.c_int32, _f32p]),
     "vb_op_window_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 7 + [C.c_void_p, C.c_int32, C.c_int32, _f32p]),
+    "vb_op_window_bias_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 8 + [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                                                                           _f32p]),
     "vb_op_softmax_rows": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 4 + [C.c_float, C.c_int32, _f32p]),
 }
 
@@ -280,6 +292,19 @@ def op_window_attention(qkv, H, W, p, heads, dh, precision="bf16", iters=0):
     ms = C.c_float(0)
     check(load().vb_op_window_attention(PRECISION[precision], _ptr(qkv), ld, B, H, W, p, heads, dh, _ptr(out), heads * dh, iters,
                                         C.byref(ms)))
+    return out, (ms.value if iters > 0 else None)
+
+
+def op_window_bias_attention(qkv, H, W, wsz, is_long, heads, dh, table, precision="bf16", iters=0):
+    """CrossFormer's attention (vb_op_window_bias_attention): qkv [B*H*W, ld] fused q|k|v rows of a pixel-major map, table the
+    (2 wsz - 1)^2 window table.  Returns (out [B*H*W, heads*dh] pixel-major, ms or None)."""
+    qkv, table = _f32(qkv), _f32(table)
+    rows, ld = qkv.shape
+    B = rows // (H * W)
+    out = np.zeros((rows, heads * dh), np.float32)
+    ms = C.c_float(0)
+    check(load().vb_op_window_bias_attention(PRECISION[precision], _ptr(qkv), ld, B, H, W, wsz, int(bool(is_long)), heads, dh, _ptr(table),
+                                             _ptr(out), heads * dh, iters, C.byref(ms)))
     return out, (ms.value if iters > 0 else None)
 
 

@@ -19,8 +19,9 @@ int take_last_attention_path();                  // and reset it to ATTN_PATH_NO
 // variant 2: CaiT talking heads: mix_a before softmax, mix_b after (cait.py:121-127)
 // scale: softmax scale; <= 0 means dh^-0.5 (vit.py:57).  A layer whose heads were zero-padded to the kernels' head width
 // (engine.cu: dh 48 -> 64) passes its true dim_head^-0.5 here.  pb (variant 0 only, may be null): LeViT's relative-position
-// bias and output GELU (common.h).  win (attention_fast only, may be null): Twins-SVT's windowed attention, B = the number of
-// windows and nq == nk == p^2 (common.h).
+// bias and output GELU (common.h), or CrossFormer's window table (PosBias::wsz > 0, B windows of nq == nk == wsz^2 window-major
+// rows).  win (attention_fast only, may be null): windowed attention in the map's own rows, B = the number of windows and
+// nq == nk == p^2 (common.h); with pb (the window-table form, dh 32 or 64) CrossFormer's windowed-bias flash kernel.
 template <typename T>
 void attention_generic(const T* q, int ldq, const T* k, int ldk, const T* v, int ldv, T* out, int ldo, float* S, int B, int nq,
                        int nk, int heads, int dh, int variant, const float* mix_a, const float* mix_b, const float* ln_gamma,

@@ -1,4 +1,4 @@
-// Tensor-core multi-head attention for the bf16 engine (bf16 operands, fp32 accumulation, dim_head = 64).
+// Tensor-core multi-head attention for the bf16 engine (bf16 operands, fp32 accumulation, dim_head = 64; 32 in the windowed-bias form).
 //
 //   out[b, i, h, :] = softmax_j( scale * q[b,i,h,:] . k[b,j,h,:] ) @ v[b,j,h,:]        (vit.py:77-82)
 //
@@ -19,6 +19,11 @@
 // WIN (Twins-SVT local attention, twins_svt.py:135-156): the flat batch index is a p x p window of a pixel-major map (Window,
 // common.h), nq == nk == p^2.  Q, K and V rows are loaded from, and the output rows stored to, the map's own pixel rows, so the
 // window split and merge rearranges (:141,153) cost no copies.  p^2 > 64 takes several query tiles and key blocks as any n does.
+//
+// BIAS and WIN (CrossFormer, crossformer.py:104-180; head width 32 or 64): windows as WIN, contiguous or dilated (Window), every
+// score plus the window table of PosBias::wsz (one (2p-1)^2 table for all heads, in log2 units in shared memory).  Windows of up
+// to 32 tokens share a 64-row query tile floor(64 / p^2) at a time, a block-diagonal mask keeping each to its own keys: the
+// 4-token windows of CrossFormer's stage-3 long attention then fill 16 times fewer CTAs.
 #include "attention.cuh"
 #include "kernels.cuh"
 #include "ptx.cuh"
@@ -28,10 +33,9 @@
 namespace vb {
 namespace {
 
-constexpr int DH = 64;
+constexpr int DH = 64;             // head width of every path but the windowed-bias one (which also runs 32)
 constexpr int FQ = 64;             // query rows per CTA
 constexpr int FK = 64;             // keys per block
-constexpr int FP = DH + 8;         // smem row pitch (bf16): +16 bytes keeps the fragment loads bank-conflict free
 
 __device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
@@ -44,12 +48,14 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
 
 constexpr int FLASH_BIAS_MAX = 4096;   // fmap^2 of the largest relative-position table (16 KB of shared memory)
 
-template <bool BIAS, bool WIN>
+template <int D, bool BIAS, bool WIN>
 __global__ void __launch_bounds__(128)
 attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloat16* __restrict__ k, int ldk,
                   const __nv_bfloat16* __restrict__ v, int ldv, __nv_bfloat16* __restrict__ out, int ldo, int heads, int nq, int nk,
                   float scale_log2, const float* __restrict__ pos_tab, int fmap, int step, int gelu_out, Window win) {
-  extern __shared__ float tab[];                                     // BIAS: [fmap^2] of this head, times log2(e)
+  constexpr int FP = D + 8;          // smem row pitch (bf16): +16 bytes keeps the fragment loads bank-conflict free
+  constexpr bool WB = BIAS && WIN;   // the windowed-bias form (below)
+  extern __shared__ float tab[];     // BIAS: [fmap^2] of this head / WB: the (2p-1)^2 window table; times log2(e)
   __shared__ __align__(16) __nv_bfloat16 Qs[FQ][FP];
   __shared__ __align__(16) __nv_bfloat16 Ks[2][FK][FP];
   __shared__ __align__(16) __nv_bfloat16 Vs[2][FK][FP];
@@ -58,28 +64,40 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
   const int i0 = (blockIdx.x % qtiles) * FQ;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nblk = (nk + FK - 1) / FK;
+  // WB: batch entry b is windows [b * G, b * G + G) of the win.count windows, G = floor(64 / p^2) for p^2 <= 32 and 1 above, so
+  // nq == nk == G * p^2; token t of the entry is token t % p^2 of window b * G + t / p^2.  The last entry may hold fewer windows:
+  // nqv / nkv are the entry's live tokens.
+  const int wn = WB ? win.p * win.p : 1, G = WB ? (wn <= 32 ? FQ / wn : 1) : 1;
+  const int nqv = WB ? min(nq, (win.count - b * G) * wn) : nq, nkv = WB ? nqv : nk;
   // row of token i of this CTA's batch entry in the q / k / v / out matrices
-  auto qrow_of = [&](int i) -> size_t { return WIN ? static_cast<size_t>(win.row(b, i)) : static_cast<size_t>(b) * nq + i; };
-  auto krow_of = [&](int i) -> size_t { return WIN ? static_cast<size_t>(win.row(b, i)) : static_cast<size_t>(b) * nk + i; };
+  auto qrow_of = [&](int i) -> size_t {
+    if (WB) return static_cast<size_t>(win.row(static_cast<long long>(b) * G + i / wn, i % wn));
+    return WIN ? static_cast<size_t>(win.row(b, i)) : static_cast<size_t>(b) * nq + i;
+  };
+  auto krow_of = [&](int i) -> size_t {
+    if (WB) return static_cast<size_t>(win.row(static_cast<long long>(b) * G + i / wn, i % wn));
+    return WIN ? static_cast<size_t>(win.row(b, i)) : static_cast<size_t>(b) * nk + i;
+  };
 
   pdl_wait();                 // Q/K/V come from the previous kernel of the stream
   pdl_launch_dependents();
 
-  // rows past n are zero-filled (never read from the next image); 8 16-byte vectors per 64-column row
-  for (int e = threadIdx.x; e < FQ * 8; e += 128) {
-    const int r = e >> 3, c = (e & 7) * 8;
-    if (i0 + r < nq) cp_async16(smem_u32(&Qs[r][c]), q + qrow_of(i0 + r) * ldq + h * DH + c);
+  // rows past n are zero-filled (never read from the next image); D / 8 16-byte vectors per row
+  constexpr int VR = D / 8, VS = D == 64 ? 3 : 2;                  // VR = 2^VS
+  for (int e = threadIdx.x; e < FQ * VR; e += 128) {
+    const int r = e >> VS, c = (e & (VR - 1)) * 8;
+    if (i0 + r < nqv) cp_async16(smem_u32(&Qs[r][c]), q + qrow_of(i0 + r) * ldq + h * D + c);
     else *reinterpret_cast<uint4*>(&Qs[r][c]) = make_uint4(0, 0, 0, 0);
   }
   auto stage = [&](int j) {
     if (j < nblk) {
       const int s = j & 1, j0 = j * FK;
-      for (int e = threadIdx.x; e < FK * 8; e += 128) {
-        const int r = e >> 3, c = (e & 7) * 8;
-        if (j0 + r < nk) {
+      for (int e = threadIdx.x; e < FK * VR; e += 128) {
+        const int r = e >> VS, c = (e & (VR - 1)) * 8;
+        if (j0 + r < nkv) {
           const size_t row = krow_of(j0 + r);
-          cp_async16(smem_u32(&Ks[s][r][c]), k + row * ldk + h * DH + c);
-          cp_async16(smem_u32(&Vs[s][r][c]), v + row * ldv + h * DH + c);
+          cp_async16(smem_u32(&Ks[s][r][c]), k + row * ldk + h * D + c);
+          cp_async16(smem_u32(&Vs[s][r][c]), v + row * ldv + h * D + c);
         } else {                                                     // zero V rows: 0 * garbage could be NaN
           *reinterpret_cast<uint4*>(&Ks[s][r][c]) = make_uint4(0, 0, 0, 0);
           *reinterpret_cast<uint4*>(&Vs[s][r][c]) = make_uint4(0, 0, 0, 0);
@@ -90,7 +108,17 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
   };
   stage(0);
   int nqs = 1, qrow[2] = {0, 0};
-  if (BIAS) {
+  int qwin[2] = {0, 0}, qy[2] = {0, 0}, qx[2] = {0, 0};             // WB: window and in-window position of the two rows
+  if (WB) {
+    const int p = win.p, t2 = (2 * p - 1) * (2 * p - 1);
+    for (int e = threadIdx.x; e < t2; e += 128) tab[e] = pos_tab[e] * 1.4426950408889634f;
+    for (int r = 0; r < 2; ++r) {
+      const int t = min(i0 + warp * 16 + (lane >> 2) + 8 * r, nqv - 1);   // rows past nqv: any live row
+      qwin[r] = t / wn;
+      qy[r] = (t - qwin[r] * wn) / p;
+      qx[r] = t - qwin[r] * wn - qy[r] * p;
+    }
+  } else if (BIAS) {
     const int f2 = fmap * fmap;
     for (int e = threadIdx.x; e < f2; e += 128) tab[e] = pos_tab[static_cast<size_t>(h) * f2 + e] * 1.4426950408889634f;
     nqs = (fmap + step - 1) / step;
@@ -98,10 +126,10 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
   }
 
   const int qr = lane >> 2, qc = 2 * (lane & 3);                     // fragment row (and row + 8) / column pair of this lane
-  uint32_t qf[DH / 16][4];
-  float o[DH / 8][4];
+  uint32_t qf[D / 16][4];
+  float o[D / 8][4];
 #pragma unroll
-  for (int n = 0; n < DH / 8; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
+  for (int n = 0; n < D / 8; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};    // running max (log2 units) / partial row sums
 
   for (int j = 0; j < nblk; ++j) {
@@ -111,7 +139,7 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
     if (j == 0) {
       const uint32_t qa = smem_u32(&Qs[warp * 16 + (lane & 15)][8 * (lane >> 4)]);
 #pragma unroll
-      for (int kk = 0; kk < DH / 16; ++kk)
+      for (int kk = 0; kk < D / 16; ++kk)
         asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
                      : "=r"(qf[kk][0]), "=r"(qf[kk][1]), "=r"(qf[kk][2]), "=r"(qf[kk][3]) : "r"(qa + kk * 32));
     }
@@ -122,20 +150,34 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
     for (int n = 0; n < FK / 8; ++n) {
       sc[n][0] = sc[n][1] = sc[n][2] = sc[n][3] = 0.f;
 #pragma unroll
-      for (int kk = 0; kk < DH / 16; ++kk) {
+      for (int kk = 0; kk < D / 16; ++kk) {
         const uint32_t b0 = *reinterpret_cast<const uint32_t*>(&Ks[s][n * 8 + qr][kk * 16 + qc]);
         const uint32_t b1 = *reinterpret_cast<const uint32_t*>(&Ks[s][n * 8 + qr][kk * 16 + qc + 8]);
         mma_bf16_16816(sc[n], qf[kk], b0, b1);
       }
     }
     // ---- online softmax (rows qr and qr + 8 of the warp's tile)
-    const int valid = nk - j * FK;
+    const int valid = nkv - j * FK;
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int n = 0; n < FK / 8; ++n) {
+      int kwin[2] = {0, 0}, ky[2] = {0, 0}, kx[2] = {0, 0};          // WB: window and in-window position of the two key columns
+      if (WB) {
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int u = j * FK + n * 8 + qc + c;
+          kwin[c] = u / wn;
+          ky[c] = (u - kwin[c] * wn) / win.p;
+          kx[c] = u - kwin[c] * wn - ky[c] * win.p;
+        }
+      }
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        if (BIAS && n * 8 + qc + (e & 1) < valid)
+        if (WB) {                                                    // the block-diagonal mask, then the window table
+          const int c = e & 1, r = e >> 1;
+          if (kwin[c] != qwin[r]) sc[n][e] = -INFINITY;
+          else sc[n][e] = fmaf(sc[n][e], scale_log2, tab[(qy[r] - ky[c] + win.p - 1) * (2 * win.p - 1) + qx[r] - kx[c] + win.p - 1]);
+        } else if (BIAS && n * 8 + qc + (e & 1) < valid)
           sc[n][e] = fmaf(sc[n][e], scale_log2, tab[pos_bias_index(qrow[e >> 1], j * FK + n * 8 + qc + (e & 1), fmap, step, nqs)]);
         if (n * 8 + qc + (e & 1) >= valid) sc[n][e] = -INFINITY;
         mx[e >> 1] = fmaxf(mx[e >> 1], sc[n][e]);
@@ -153,7 +195,7 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
       l_run[r] *= alpha[r];
     }
 #pragma unroll
-    for (int n = 0; n < DH / 8; ++n) {
+    for (int n = 0; n < D / 8; ++n) {
       o[n][0] *= alpha[0]; o[n][1] *= alpha[0];
       o[n][2] *= alpha[1]; o[n][3] *= alpha[1];
     }
@@ -174,7 +216,7 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
 #pragma unroll
     for (int kk = 0; kk < FK / 16; ++kk) {
 #pragma unroll
-      for (int n = 0; n < DH / 8; ++n) {
+      for (int n = 0; n < D / 8; ++n) {
         uint32_t b0, b1;
         asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0, %1}, [%2];"
                      : "=r"(b0), "=r"(b1) : "r"(va + (kk * 16 * FP + n * 8) * 2));
@@ -193,15 +235,61 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int row = i0 + warp * 16 + qr + 8 * r;
-    if (row >= nq) continue;
-    __nv_bfloat16* orow = out + qrow_of(row) * ldo + h * DH + qc;
+    if (row >= nqv) continue;
+    __nv_bfloat16* orow = out + qrow_of(row) * ldo + h * D + qc;
 #pragma unroll
-    for (int n = 0; n < DH / 8; ++n) {
+    for (int n = 0; n < D / 8; ++n) {
       float a0 = o[n][2 * r] * l_run[r], a1 = o[n][2 * r + 1] * l_run[r];
       if (BIAS && gelu_out) { a0 = gelu_exact(a0); a1 = gelu_exact(a1); }
       *reinterpret_cast<uint32_t*>(orow + n * 8) = pack_bf16x2(a0, a1);
     }
   }
+}
+
+template <int D>
+void launch_window_bias(cudaLaunchConfig_t& cfg, const __nv_bfloat16* q, int ldq, __nv_bfloat16* out, int ldo, int heads, int n,
+                        float scale_log2, const PosBias& pb, const Window& win) {
+  static unsigned long long seen[4] = {0, 0, 0, 0};
+  if (first_use_on_this_device(seen))
+    VB_CUDA(cudaFuncSetAttribute(attn_flash_kernel<D, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FLASH_BIAS_MAX * 4));
+  const int HD = heads * D;
+  VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<D, true, true>, q, ldq, q + HD, ldq, q + 2 * HD, ldq, out, ldo, heads, n, n,
+                             scale_log2, pb.table, 0, 1, 0, win));
+}
+
+// CrossFormer's attention: windows of B = win.count images' maps, q | k | v at columns [0, HD), [HD, 2 HD), [2 HD, 3 HD) of the
+// fused rows (HD = heads * dh), the window table of pb added to every score.  p^2 <= 32 packs floor(64 / p^2) windows into a
+// tile; 32 < p^2 <= 64 is one window per tile; larger windows take several query tiles and key blocks.
+bool attention_window_bias(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, int ldk, const __nv_bfloat16* v, int ldv,
+                           __nv_bfloat16* out, int ldo, int B, int nq, int nk, int heads, int dh, cudaStream_t s, float scale,
+                           const PosBias& pb, const Window& win) {
+  const int n = win.p * win.p, HD = heads * dh;
+  if (pb.wsz != win.p || nq != n || nk != n || (dh != 32 && dh != 64)) return false;
+  if ((2 * win.p - 1) * (2 * win.p - 1) > FLASH_BIAS_MAX) return false;
+  if (k != q + HD || v != q + 2 * HD || ldk != ldq || ldv != ldq || (ldq % 8) || (ldo % 2)) return false;
+  if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(out)) % 16) return false;
+  const int G = n <= 32 ? FQ / n : 1, tile = G * n;
+  const long long entries = (static_cast<long long>(B) + G - 1) / G;
+  const long long blocks = entries * heads * ((tile + FQ - 1) / FQ);
+  if (blocks > 0x7fffffffLL || B <= 0) return false;
+  Window w = win;
+  w.count = B;
+  const float scale_log2 = (scale > 0.f ? scale : 1.0f / sqrtf(static_cast<float>(dh))) * 1.4426950408889634f;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(static_cast<unsigned>(blocks));
+  cfg.blockDim = dim3(128);
+  cfg.stream = s;
+  cfg.dynamicSmemBytes = static_cast<size_t>(2 * win.p - 1) * (2 * win.p - 1) * sizeof(float);
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  if (dh == 32) launch_window_bias<32>(cfg, q, ldq, out, ldo, heads, tile, scale_log2, pb, w);
+  else launch_window_bias<64>(cfg, q, ldq, out, ldo, heads, tile, scale_log2, pb, w);
+  count_launch();
+  note_attention_path(ATTN_PATH_FLASH);
+  return true;
 }
 
 }  // namespace
@@ -211,7 +299,9 @@ bool attention_fast<__nv_bfloat16>(const __nv_bfloat16* q, int ldq, const __nv_b
                                    __nv_bfloat16* out, int ldo, int B, int nq, int nk, int heads, int dh, int variant,
                                    const float* mix_a, const float* mix_b, const float* ln_g, const float* ln_b, cudaStream_t s,
                                    float scale, const PosBias* pb, const Window* win) {
-  if (win != nullptr && (pb != nullptr || nq != win->p * win->p || nk != nq)) return false;
+  if (win != nullptr && pb != nullptr) return attention_window_bias(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, heads, dh, s, scale, *pb, *win);
+  if (pb != nullptr && pb->wsz > 0) return false;
+  if (win != nullptr && (nq != win->p * win->p || nk != nq)) return false;
   if (nq == 1 && pb == nullptr && win == nullptr && attention_cls(q, ldq, k, ldk, v, ldv, out, ldo, B, nk, heads, dh, variant, mix_a, mix_b, ln_g, ln_b, s, scale)) return true;
   // DeepViT re-attention / CaiT talking heads: the materialised-scores path (attn_generic_mma.cu) -- a fused form with all heads'
   // scores of a 16-row tile in shared memory measured 9-11 % slower on the H100 (one CTA per SM at 16 heads)
@@ -230,7 +320,7 @@ bool attention_fast<__nv_bfloat16>(const __nv_bfloat16* q, int ldq, const __nv_b
   if (pb != nullptr) {
     static unsigned long long seen[4] = {0, 0, 0, 0};
     if (first_use_on_this_device(seen))
-      VB_CUDA(cudaFuncSetAttribute(attn_flash_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FLASH_BIAS_MAX * 4));
+      VB_CUDA(cudaFuncSetAttribute(attn_flash_kernel<DH, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FLASH_BIAS_MAX * 4));
     cfg.dynamicSmemBytes = static_cast<size_t>(pb->fmap) * pb->fmap * sizeof(float);
   }
   cudaLaunchAttribute attr[1];
@@ -239,13 +329,13 @@ bool attention_fast<__nv_bfloat16>(const __nv_bfloat16* q, int ldq, const __nv_b
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   if (pb != nullptr)
-    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<true, false>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<DH, true, false>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
                                pb->table, pb->fmap, pb->step, static_cast<int>(pb->gelu_out), Window()));
   else if (win != nullptr)
-    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<false, true>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<DH, false, true>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
                                static_cast<const float*>(nullptr), 0, 1, 0, *win));
   else
-    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<false, false>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<DH, false, false>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
                                static_cast<const float*>(nullptr), 0, 1, 0, Window()));
   count_launch();
   note_attention_path(ATTN_PATH_FLASH);

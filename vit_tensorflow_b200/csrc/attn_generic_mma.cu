@@ -657,7 +657,7 @@ bool attention_generic_mma(const __nv_bfloat16* q, int ldq, const __nv_bfloat16*
   if (dh % 16 != 0 || dh > MAXDH || heads > MIX_MAX_HEADS) return false;
   if ((ldq % 8) || (ldk % 8) || (ldv % 8) || (ldo % 2)) return false;
   if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k)) % 16) return false;
-  if (pb != nullptr && variant != 0) return false;
+  if (pb != nullptr && (variant != 0 || pb->wsz > 0)) return false;   // the window table: the SIMT kernels (attn_pos_bias)
   if (pb == nullptr && attention_rows_path(q, ldq, k, ldk, v, ldv, out, ldo, S, B, nq, nk, heads, dh, variant, mix_a, mix_b, ln_gamma, ln_beta, s)) return true;
   const size_t smem = (static_cast<size_t>(heads) * nk + 2 * heads * heads) * sizeof(float);
   if (smem > 200 * 1024) return false;

@@ -63,27 +63,46 @@ inline unsigned flat_blocks(long long tiles, long long items, const char* what =
 // with key j at grid position (kr, kc) = (j / fmap, j % fmap) and query i at (qr, qc) = step * (i / nqs, i % nqs), nqs =
 // ceil(fmap / step): the queries of a stride-2 "shrink" attention sit on the even pixels of the key grid.  `table` is fp32
 // [heads][fmap^2] in the units of the scaled scores (the reference adds pos_bias / scale, levit.py:117).  nk == fmap^2, nq == nqs^2.
+//
+// wsz > 0 (CrossFormer, crossformer.py:126-131,158-165) replaces that form: within a wsz x wsz window, token i at (i / wsz, i % wsz)
+// and key j at (j / wsz, j % wsz) give the signed offsets (dr, dc), and every head adds
+//   table[(dr + wsz - 1) * (2 wsz - 1) + (dc + wsz - 1)]
+// from one shared fp32 table of (2 wsz - 1)^2 entries, in the units of the scaled scores.  nq == nk == wsz^2; fmap / step unused.
 struct PosBias {
   const float* table = nullptr;
   int fmap = 0, step = 1;
   bool gelu_out = false;                  // levit.py:94: to_out starts with an exact-erf GELU of the attention output
+  int wsz = 0;
   __host__ __device__ int q_side() const { return (fmap + step - 1) / step; }
 };
+__host__ __device__ __forceinline__ int window_bias_index(int i, int j, int wsz) {
+  const int ri = i / wsz, rj = j / wsz;
+  return (ri - rj + wsz - 1) * (2 * wsz - 1) + (i - ri * wsz) - (j - rj * wsz) + wsz - 1;
+}
 __device__ __forceinline__ int pos_bias_index(int i, int j, int fmap, int step, int nqs) {
   const int qr = (i / nqs) * step, qc = (i % nqs) * step, kr = j / fmap, kc = j - kr * fmap;
   return abs(qr - kr) * fmap + abs(qc - kc);
 }
 __device__ __forceinline__ float gelu_exact(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
-// Twins-SVT's local attention (twins_svt.py:135-156): each p x p window of a pixel-major [B, H, W] map attends within itself.  The
-// flat batch index of the attention is (image, window row, window column) over nx x ny windows (W = nx * p, H = ny * p), and token
-// i < p^2 of window bw is the map's row row(bw, i) = (b * H + wy * p + i / p) * W + wx * p + i % p.  nq == nk == p^2.
+// Windowed attention on a pixel-major [B, H, W] map: each window of p x p tokens attends within itself.  The flat batch index of
+// the attention is (image, window row, window column) over nx x ny windows (W = nx * p, H = ny * p), and token i < p^2 of window
+// bw = (b, wy, wx), at (r, c) = (i / p, i % p) in the window, is the map's row (b * H + y) * W + x with
+//   y = wy * oy + r * sy,  x = wx * ox + c * sx,
+//   contiguous blocks (dilated == 0; Twins-SVT twins_svt.py:141, CrossFormer's short attention crossformer.py:144):
+//     oy = ox = p, sy = sx = 1;
+//   dilated windows (dilated != 0; CrossFormer's long attention, crossformer.py:146 'b (l1 h) (l2 w) d -> (b h w) l1 l2 d'):
+//     oy = ox = 1, sy = ny, sx = nx.
+// nq == nk == p^2.
 struct Window {
   int p = 0, nx = 0, ny = 0;
+  int dilated = 0;
+  int count = 0;                          // windows in the batch: the windowed-bias flash kernel packs several into one query tile
   __host__ __device__ long long row(long long bw, int i) const {
     const long long per = static_cast<long long>(nx) * ny, b = bw / per;
-    const int w = static_cast<int>(bw - b * per), wy = w / nx, wx = w - wy * nx, r = i / p;
-    return ((b * ny + wy) * p + r) * (static_cast<long long>(nx) * p) + wx * p + (i - r * p);
+    const int w = static_cast<int>(bw - b * per), wy = w / nx, wx = w - wy * nx, r = i / p, c = i - r * p;
+    const int oy = dilated ? 1 : p, sy = dilated ? ny : 1, ox = dilated ? 1 : p, sx = dilated ? nx : 1;
+    return (b * ny * p + wy * oy + r * sy) * (static_cast<long long>(nx) * p) + wx * ox + c * sx;
   }
 };
 

@@ -177,19 +177,37 @@ inline void cvt_fold_dw(const std::vector<double>& taps, const std::vector<doubl
 // One Twins-SVT Transformer layer (twins_svt.py:192-213) on channel rows zero-padded to dp (bf16) / dim (fp32): x = x + f(LN(x))
 // for local attention, MLP, global attention, MLP; stage 4 has no local attention and no first MLP (has_local=False, :255).  The
 // bf16 engine folds the PreNorm LayerNorms of the fused local q|k|v, the global to_q and the fc1s into those GEMMs.
-struct TwinsMlpW { Norm norm; Linear fc1, fc2; };
+struct MlpW { Norm norm; Linear fc1, fc2; };   // PreNorm MLP (Twins-SVT, CrossFormer): LayerNorm eps 1e-5, fc1, GELU, fc2
 struct TwinsLayerW {
   bool local = false;
   Norm local_norm, global_norm;      // gamma / beta [dp], zero on pad channels
   Linear qkv, local_out;             // local: to_q | to_kv as one [dp, 1536] GEMM, to_out
   Linear to_q, to_kv, global_out;    // global: to_q [dp, 512], to_kv [k * k * dim, 1024] over the VALID k x k patch rows
-  TwinsMlpW ff1, ff2;
+  MlpW ff1, ff2;
 };
 struct TwinsStageW {                 // twins_svt.py:252-259: PatchEmbedding, Transformer(depth 1), PEG, Transformer(depth)
   int dim = 0, dp = 0, patch = 1, local = 0, global_k = 1, peg_k = 3;
   Linear proj;                       // rows in unfold_same's (p1, p2, c) order
   const float *peg_w = nullptr, *peg_b = nullptr;   // PEG taps [k*k][dp] with the residual on the centre tap, bias [dp]
   std::vector<TwinsLayerW> pre, post;
+};
+
+// One CrossFormer Transformer layer (crossformer.py:196-203) on channel rows zero-padded to dp (bf16) / dim (fp32): short attention,
+// MLP, long attention, MLP, each x = f(x) + x with f's own LayerNorm first (eps 1e-5); the bf16 engine folds those LayerNorms into
+// the q|k|v and fc1 GEMMs.  Attention has heads = dim / 32 of width 32, inner width I = 32 * heads.
+struct CrossformerAttnW {
+  int wsz = 1;
+  bool dilated = false;              // the long attention's windows (crossformer.py:146)
+  Norm norm;
+  Linear qkv;                        // [q | k | v], 3 I columns (bf16: padded to a multiple of 64); wsz == 1: v alone, I columns
+  Linear to_out;                     // [I, dp]
+  const float* table = nullptr;      // the DynamicPositionBias window table, (2 wsz - 1)^2 (wsz > 1)
+};
+struct CrossformerLayerW { CrossformerAttnW short_attn, long_attn; MlpW ff1, ff2; };
+struct CrossformerStageW {           // crossformer.py:248-255: CrossEmbedLayer, Transformer
+  int dim = 0, dp = 0, heads = 0, kmax = 1, stride = 1;
+  Linear embed;                      // every kernel nested in the kmax x kmax one, rows in unfold_same's (row, column, channel) order
+  std::vector<CrossformerLayerW> layers;
 };
 
 struct EmbedW { Linear patch; const float* pos = nullptr; const float* cls = nullptr; int dim = 0, n_pos = 0; };
@@ -395,6 +413,24 @@ struct vb_handle {
   static std::string twins_pre(int st) { return "svt_layers." + std::to_string(st) + "."; }
   int twins_cin(int st) const { return st == 0 ? cfg.channels : tw.emb_dim[st - 1]; }
   static constexpr int kTwinsInner = 512;        // 8 heads of 64: Transformer is never passed heads / dim_head (twins_svt.py:254-258)
+  // CrossFormer (crossformer.py:205-269): the four stages, then the average pool and the Dense head (`head`)
+  vb_crossformer_config cf{};
+  std::vector<CrossformerStageW> cf_stages;
+  static std::string cf_pre(int st) { return "crossformer_layers." + std::to_string(st) + "."; }
+  int cf_cin(int st) const { return st == 0 ? cfg.channels : cf.dim[st - 1]; }
+  std::vector<int> cf_kernels(int st) const {                // CrossEmbedLayer sorts them (crossformer.py:34)
+    std::vector<int> k(cf.kernels[st], cf.kernels[st] + cf.n_kernels[st]);
+    std::sort(k.begin(), k.end());
+    return k;
+  }
+  std::vector<int> cf_dim_scales(int st) const {             // crossformer.py:38-39
+    const int d = cf.dim[st], n = cf.n_kernels[st];
+    std::vector<int> v;
+    int sum = 0;
+    for (int i = 1; i < n; ++i) { v.push_back(d >> i); sum += d >> i; }
+    v.push_back(d - sum);
+    return v;
+  }
   struct XBlock { std::vector<LayerW> sm_layers, lg_layers; Norm sm_final, lg_final; std::vector<CrossW> sm_attend_lg, lg_attend_sm; };
   std::vector<XBlock> xblocks;
   Norm head_norm, sm_head_norm, lg_head_norm;
@@ -616,6 +652,40 @@ struct vb_handle {
         }
       }
       expect_dense("svt_layers.4.1", tw.emb_dim[VB_TWINS_STAGES - 1], c.num_classes);   // :261-264
+    } else if (c.kind == VB_KIND_CROSSFORMER) {
+      auto expect_ln4 = [&](const std::string& n, int d) { expect(n + ".g", {1, 1, 1, d}); expect(n + ".b", {1, 1, 1, d}); };   // :77-78
+      for (int st = 0; st < VB_CROSSFORMER_STAGES; ++st) {
+        const std::string p = cf_pre(st);
+        const int d = cf.dim[st], I = 32 * (d / 32), d4 = d / 4;
+        const auto ks = cf_kernels(st), ds = cf_dim_scales(st);
+        for (size_t i = 0; i < ks.size(); ++i) {                          // CrossEmbedLayer :41-43
+          expect(p + "0.convs." + std::to_string(i) + ".kernel", {ks[i], ks[i], cf_cin(st), ds[i]});
+          expect(p + "0.convs." + std::to_string(i) + ".bias", {ds[i]});
+        }
+        for (int L = 0; L < cf.depth[st]; ++L) {
+          const std::string b = p + "1.layers." + std::to_string(L) + ".";
+          for (const char* a : {"0.", "2."}) {                            // Attention :104-131
+            expect_ln4(b + a + "norm", d);
+            expect(b + a + "to_qkv.kernel", {1, 1, d, 3 * I});
+            expect(b + a + "to_out.kernel", {1, 1, I, d});
+            expect(b + a + "to_out.bias", {d});
+            const std::string dpb = b + a + "dpb.dpb_layers.";             // DynamicPositionBias :51-71
+            for (int li : {0, 3, 6, 9}) {
+              expect(dpb + std::to_string(li) + ".kernel", {li == 0 ? 2 : d4, li == 9 ? 1 : d4});
+              expect(dpb + std::to_string(li) + ".bias", {li == 9 ? 1 : d4});
+            }
+            for (int li : {1, 4, 7}) expect_ln(dpb + std::to_string(li), d4);
+          }
+          for (const char* m : {"1.", "3."}) {                            // MLP :89-102
+            expect_ln4(b + m + "net.0", d);
+            expect(b + m + "net.1.kernel", {1, 1, d, 4 * d});
+            expect(b + m + "net.1.bias", {4 * d});
+            expect(b + m + "net.4.kernel", {1, 1, 4 * d, d});
+            expect(b + m + "net.4.bias", {d});
+          }
+        }
+      }
+      expect_dense("to_logits.1", cf.dim[VB_CROSSFORMER_STAGES - 1], c.num_classes);   // :258-261
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       expect("pos_embedding", {1, np, c.dim});
@@ -840,7 +910,7 @@ struct vb_handle {
     for (auto& w : weights) VB_CHECK(w.set, "vb_finalize: weight '" + w.name + "' was never set");
     VB_CUDA(cudaSetDevice(device));
     owned.clear(); layers.clear(); cls_layers.clear(); t2t_layers.clear(); xblocks.clear(); plans.clear(); embed_res.clear(); cct_convs.clear();
-    lv_stem.clear(); lv_blocks.clear(); cvt_stages.clear(); twins_stages.clear();
+    lv_stem.clear(); lv_blocks.clear(); cvt_stages.clear(); twins_stages.clear(); cf_stages.clear();
     woverride.clear();
     drop_graphs();
     const vb_config& c = cfg;
@@ -895,6 +965,8 @@ struct vb_handle {
       finalize_cvt();
     } else if (c.kind == VB_KIND_TWINS_SVT) {
       finalize_twins();
+    } else if (c.kind == VB_KIND_CROSSFORMER) {
+      finalize_crossformer();
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       embed = make_embed("", c.patch_h, c.patch_w, c.dim, np, false);
@@ -1025,17 +1097,21 @@ struct vb_handle {
     head = make_linear_f32("cvt_layers.3.1", cv.emb_dim[VB_CVT_STAGES - 1], cfg.num_classes);
   }
   // ---- Twins-SVT weight packing: channel widths zero-padded (bf16), the patch kernel's rows permuted, the PEG residual folded
-  TwinsMlpW twins_mlp(const std::string& m, int d, int dp) {
-    TwinsMlpW w;
+  // A PreNorm MLP of width 4 d: the LayerNorm `norm` (g / b), the Dense layers n0 (d -> 4 d) and n3 (4 d -> d) as 1x1 Conv2D
+  // kernels, widths padded, the LayerNorm folded into fc1 in the bf16 engine.  key: the packed copies' own names.
+  MlpW prenorm_mlp(const std::string& key, const std::string& norm, const std::string& n0, const std::string& n3, int d, int dp) {
+    MlpW w;
     const int hidden = 4 * d, hp = channel_width(hidden);
-    const std::string n0 = m + ".fn.fn.net.0", n3 = m + ".fn.fn.net.3";
-    w.norm = padded_norm(m + ".fn.norm", d, dp);
-    w.fc1 = linear_from_host("twins." + n0, pad_kn(host_weight(n0 + ".kernel"), d, hidden, dp, hp), pad_n(host_weight(n0 + ".bias"), hp), dp,
+    w.norm = padded_norm(norm, d, dp);
+    w.fc1 = linear_from_host(key + n0, pad_kn(host_weight(n0 + ".kernel"), d, hidden, dp, hp), pad_n(host_weight(n0 + ".bias"), hp), dp,
                              hp, bf16() ? &w.norm : nullptr);
     w.fc1.ln_d = d;
     w.fc1.ln_eps = 1e-5f;
-    w.fc2 = linear_from_host("twins." + n3, pad_kn(host_weight(n3 + ".kernel"), hidden, d, hp, dp), pad_n(host_weight(n3 + ".bias"), dp), hp, dp);
+    w.fc2 = linear_from_host(key + n3, pad_kn(host_weight(n3 + ".kernel"), hidden, d, hp, dp), pad_n(host_weight(n3 + ".bias"), dp), hp, dp);
     return w;
+  }
+  MlpW twins_mlp(const std::string& m, int d, int dp) {
+    return prenorm_mlp("twins.", m + ".fn.norm", m + ".fn.fn.net.0", m + ".fn.fn.net.3", d, dp);
   }
   TwinsLayerW twins_layer_weights(const std::string& b, int st, int d, int dp) {
     TwinsLayerW w;
@@ -1097,6 +1173,98 @@ struct vb_handle {
       twins_stages.push_back(std::move(S));
     }
     head = make_linear_f32("svt_layers.4.1", tw.emb_dim[VB_TWINS_STAGES - 1], cfg.num_classes);
+  }
+  // ---- CrossFormer weight packing: the nested cross-scale kernel, the DynamicPositionBias tables, channel widths zero-padded (bf16)
+  // DynamicPositionBias (crossformer.py:51-71,158-165) on the offsets range(-w, w + 1)^2 in (row, column) order: 3 x [Dense ->
+  // LayerNormalization (eps 1e-3) -> ReLU], Dense(1).  The reference indexes the result with rel_pos_indices (:126-131), whose
+  // offset w - 1 and row pitch 2 w - 1 read only its first (2 w - 1)^2 entries: those are the table (PosBias::wsz).
+  std::vector<double> cf_window_table(const std::string& n, int w, int d4) const {
+    const int side = 2 * w + 1, t = (2 * w - 1) * (2 * w - 1);
+    std::vector<double> Wl[4], bl[4], g[3], be[3];
+    for (int i = 0; i < 4; ++i) { Wl[i] = host_weight(n + std::to_string(3 * i) + ".kernel"); bl[i] = host_weight(n + std::to_string(3 * i) + ".bias"); }
+    for (int i = 0; i < 3; ++i) { g[i] = host_weight(n + std::to_string(3 * i + 1) + ".gamma"); be[i] = host_weight(n + std::to_string(3 * i + 1) + ".beta"); }
+    std::vector<double> table(t);
+    for (int e = 0; e < t; ++e) {
+      std::vector<double> x = {static_cast<double>(e / side - w), static_cast<double>(e % side - w)};
+      for (int i = 0; i < 4; ++i) {
+        const int din = static_cast<int>(x.size()), dout = i == 3 ? 1 : d4;
+        std::vector<double> y(bl[i].begin(), bl[i].end());
+        for (int k = 0; k < din; ++k)
+          for (int o = 0; o < dout; ++o) y[o] += x[k] * Wl[i][static_cast<size_t>(k) * dout + o];
+        if (i < 3) {
+          double mean = 0.0, var = 0.0;
+          for (double v : y) mean += v;
+          mean /= dout;
+          for (double v : y) var += (v - mean) * (v - mean);
+          const double rstd = 1.0 / std::sqrt(var / dout + 1e-3);
+          for (int o = 0; o < dout; ++o) y[o] = std::max(0.0, (y[o] - mean) * rstd * g[i][o] + be[i][o]);
+        }
+        x.swap(y);
+      }
+      table[e] = x[0];
+    }
+    return table;
+  }
+  CrossformerAttnW cf_attention(const std::string& a, int d, int dp, int wsz, bool dilated) {
+    CrossformerAttnW w;
+    const int I = 32 * (d / 32), key_n = wsz == 1 ? I : 3 * I, N = bf16() ? round_up(key_n, 64) : key_n;
+    w.wsz = wsz;
+    w.dilated = dilated;
+    w.norm = padded_norm(a + "norm", d, dp);
+    auto qkv = host_weight(a + "to_qkv.kernel");                   // [d, q | k | v]
+    if (wsz == 1) {                                                // softmax over one score is 1: only v is needed (its third)
+      std::vector<double> v(static_cast<size_t>(d) * I);
+      for (int r = 0; r < d; ++r)
+        std::copy(qkv.begin() + static_cast<size_t>(r) * 3 * I + 2 * I, qkv.begin() + static_cast<size_t>(r + 1) * 3 * I, v.begin() + static_cast<size_t>(r) * I);
+      qkv.swap(v);
+    } else {
+      w.table = upload_owned(cf_window_table(a + "dpb.dpb_layers.", wsz, d / 4));
+    }
+    w.qkv = linear_from_host("cf." + a + "qkv", pad_kn(qkv, d, key_n, dp, N), {}, dp, N, bf16() ? &w.norm : nullptr);
+    w.qkv.ln_d = d;
+    w.qkv.ln_eps = 1e-5f;                                          // crossformer.py:74
+    w.to_out = linear_from_host("cf." + a + "to_out", pad_kn(host_weight(a + "to_out.kernel"), I, d, I, dp), pad_n(host_weight(a + "to_out.bias"), dp),
+                                I, dp);
+    return w;
+  }
+  void finalize_crossformer() {
+    for (int st = 0; st < VB_CROSSFORMER_STAGES; ++st) {
+      CrossformerStageW S;
+      const std::string p = cf_pre(st);
+      const int d = cf.dim[st], dp = channel_width(d), cin = cf_cin(st);
+      const auto ks = cf_kernels(st), ds = cf_dim_scales(st);
+      const int K = ks.back();
+      S.dim = d; S.dp = dp; S.heads = d / 32; S.kmax = K; S.stride = cf.stride[st];
+      // CrossEmbedLayer (:45-48) as one K x K convolution: kernel i sits at offset (K - k_i) / 2 of the K x K grid (TF SAME pads the
+      // smaller half first; with equal parities and every k_i >= stride the offset is exact for any map), its outputs at columns
+      // [sum of the earlier dim_scales, + ds[i]) -- the concat order
+      std::vector<double> Wn(static_cast<size_t>(K) * K * cin * dp, 0.0), bn(dp, 0.0);
+      int col0 = 0;
+      for (size_t i = 0; i < ks.size(); ++i) {
+        const std::string n = p + "0.convs." + std::to_string(i);
+        const int k = ks[i], o = (K - k) / 2, dsi = ds[i];
+        const auto wk = host_weight(n + ".kernel"), bk = host_weight(n + ".bias");
+        for (int ky = 0; ky < k; ++ky)
+          for (int kx = 0; kx < k; ++kx)
+            for (int c = 0; c < cin; ++c)
+              for (int oc = 0; oc < dsi; ++oc)
+                Wn[((static_cast<size_t>(ky + o) * K + kx + o) * cin + c) * dp + col0 + oc] = wk[((static_cast<size_t>(ky) * k + kx) * cin + c) * dsi + oc];
+        for (int oc = 0; oc < dsi; ++oc) bn[col0 + oc] = bk[oc];
+        col0 += dsi;
+      }
+      S.embed = linear_from_host("cf." + p + "0", Wn, bn, K * K * cin, dp);
+      for (int L = 0; L < cf.depth[st]; ++L) {
+        const std::string b = p + "1.layers." + std::to_string(L) + ".";
+        CrossformerLayerW l;
+        l.short_attn = cf_attention(b + "0.", d, dp, cf.local_wsz[st], false);
+        l.ff1 = prenorm_mlp("cf.", b + "1.net.0", b + "1.net.1", b + "1.net.4", d, dp);
+        l.long_attn = cf_attention(b + "2.", d, dp, cf.global_wsz[st], true);
+        l.ff2 = prenorm_mlp("cf.", b + "3.net.0", b + "3.net.1", b + "3.net.4", d, dp);
+        S.layers.push_back(std::move(l));
+      }
+      cf_stages.push_back(std::move(S));
+    }
+    head = make_linear_f32("to_logits.1", cf.dim[VB_CROSSFORMER_STAGES - 1], cfg.num_classes);
   }
   void finalize_levit() {
     const int dh = levit_dh();
@@ -1191,7 +1359,7 @@ struct vb_handle {
   template <typename T>
   void attention_dispatch(const T* q, int ldq, const T* k, int ldk, const T* v, int ldv, T* out, int ldo, int B, int nq, int nk,
                           int heads, int dh, int variant, const float* mix_a, const float* mix_b, const float* g, const float* b,
-                          cudaStream_t s, float scale = 0.f, const Window* win = nullptr);
+                          cudaStream_t s, float scale = 0.f, const Window* win = nullptr, const PosBias* pb = nullptr);
 
   template <typename T>
   const T* embed_residual(const EmbedW& e, int B, int rows, cudaStream_t s) {
@@ -1652,6 +1820,8 @@ struct vb_handle {
       cvt_forward<T>(img, B, H, Wd, logits, s);
     } else if (c.kind == VB_KIND_TWINS_SVT) {
       twins_forward<T>(img, B, H, Wd, logits, s);
+    } else if (c.kind == VB_KIND_CROSSFORMER) {
+      crossformer_forward<T>(img, B, H, Wd, logits, s);
     } else if (c.kind == VB_KIND_CCT) {                   // CCT.call cct.py:342-345, TransformerClassifier.call :277-305
       int rows = 0;
       T* X = tokenize_cct<T>(img, B, H, Wd, &rows, s);
@@ -1970,7 +2140,7 @@ struct vb_handle {
       Epi e; e.bias = L.bias; e.res = X; e.ldr = dp; e.stats_out = stats;
       linear<T>(A, lda, M, L, X, dp, e, s);
     };
-    auto mlp = [&](const TwinsMlpW& m) {                              // twins_svt.py:78-92
+    auto mlp = [&](const MlpW& m) {                              // twins_svt.py:78-92
       const T* a = prenorm(m.norm);
       T* Hb = arena.get<T>(static_cast<size_t>(M) * m.fc1.N);
       Epi e1 = folded(m.fc1);
@@ -2011,6 +2181,107 @@ struct vb_handle {
     linear<T>(col, Kp, Mk, Lk, KV, 2 * I, Epi(), s);
     attention_dispatch<T>(Q, I, KV, 2 * I, KV + I, 2 * I, O, I, B, H * Wd, kh * kw, I / 64, 64, 0, nullptr, nullptr, nullptr, nullptr, s);
     residual(O, I, l.global_out);
+    mlp(l.ff2);
+  }
+
+  // CrossFormer.call (crossformer.py:263-269): per stage, CrossEmbedLayer -> Transformer; then the mean over the map -> Dense.
+  // Token rows are the NHWC map, pixel-major, channel widths zero-padded to channel_width; no stage permutes its map (the windowed
+  // attention reads and writes the map's own rows).  bf16: `stats` holds the (sum, sumsq) partials of X's rows between sub-blocks
+  // (emitted by the embedding's and the residual GEMMs' epilogues).
+  static constexpr const char* kCrossformerNoStages =
+      "CrossFormer runs as a whole forward only: its embedding / stage / head steps have no entry of their own";
+  // The reference's shape rule (crossformer.py:144,146 through einops), checked before anything runs.
+  void cf_check_size(int H, int Wd) const {
+    int h = H, w = Wd;
+    for (int st = 0; st < VB_CROSSFORMER_STAGES; ++st) {
+      h = (h + cf.stride[st] - 1) / cf.stride[st];
+      w = (w + cf.stride[st] - 1) / cf.stride[st];
+      const std::string where = "CrossFormer stage " + std::to_string(st + 1) + ": the " + std::to_string(h) + " x " + std::to_string(w) + " map ";
+      VB_CHECK(h % cf.local_wsz[st] == 0 && w % cf.local_wsz[st] == 0, where + "is not divisible by local_window_size " + std::to_string(cf.local_wsz[st]));
+      VB_CHECK(h % cf.global_wsz[st] == 0 && w % cf.global_wsz[st] == 0, where + "is not divisible by global_window_size " + std::to_string(cf.global_wsz[st]));
+    }
+  }
+  template <typename T>
+  void crossformer_forward(const float* img, int B, int H, int Wd, float* logits, cudaStream_t s) {
+    cf_check_size(H, Wd);
+    int mh = H, mw = Wd, mc = cfg.channels, ld_in = 0;
+    const T* map = nullptr;
+    T* X = nullptr;
+    for (const CrossformerStageW& S : cf_stages) {
+      const int oh = (mh + S.stride - 1) / S.stride, ow = (mw + S.stride - 1) / S.stride, M = B * oh * ow;
+      const int Kp = bf16() ? S.embed.ldw : S.embed.K;
+      T* col = arena.get<T>(static_cast<size_t>(M) * Kp);
+      {
+        ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(map == nullptr ? 4 : sizeof(T)) * B * mh * mw * mc +
+                                                 static_cast<double>(sizeof(T)) * M * Kp, s);
+        if (map == nullptr) unfold_same<float, T>(img, col, B, mh, mw, mc, S.kmax, S.stride, 0, Kp, s);
+        else unfold_same<T, T>(map, col, B, mh, mw, mc, S.kmax, S.stride, 0, Kp, s, ld_in);
+      }
+      X = arena.get<T>(static_cast<size_t>(M) * S.dp);
+      float* stats = bf16() ? arena.get<float>(static_cast<size_t>(M) * (S.dp / 64) * 2) : nullptr;
+      Linear L = S.embed;
+      L.K = Kp;
+      Epi e; e.bias = S.embed.bias; e.stats_out = stats;
+      linear<T>(col, Kp, M, L, X, S.dp, e, s);
+      for (const CrossformerLayerW& l : S.layers) crossformer_layer<T>(X, B, oh, ow, S, l, stats, s);
+      map = X; mh = oh; mw = ow; mc = S.dim; ld_in = S.dp;
+    }
+    const int dl = cf.dim[VB_CROSSFORMER_STAGES - 1];
+    float* z = arena.get<float>(static_cast<size_t>(B) * dl);
+    {
+      ProfScope ps(this, PROF_LN, 1.0 * B * mh * mw * dl, static_cast<double>(sizeof(T)) * B * mh * mw * dl, s);
+      pool_layernorm<T>(X, mh * mw, ld_in, nullptr, nullptr, z, B, dl, 1, s);   // Reduce('b h w c -> b c', 'mean') crossformer.py:259
+    }
+    gemm_simt<float, float, float>(z, dl, head.W, head.N, 1, logits, head.N, B, head.N, dl, head.bias, nullptr, nullptr, head.N, 0, s);
+  }
+  // One Transformer layer (crossformer.py:198-202) in place on X [B*H*W, dp].  bf16: the LayerNorms folded into q|k|v and fc1 (from
+  // `stats`); fp32: separate LayerNorms.
+  template <typename T>
+  void crossformer_layer(T* X, int B, int H, int Wd, const CrossformerStageW& S, const CrossformerLayerW& l, float* stats, cudaStream_t s) {
+    const int dp = S.dp, d = S.dim, M = B * H * Wd, I = 32 * S.heads;
+    T* Y = bf16() ? nullptr : arena.get<T>(static_cast<size_t>(M) * dp);
+    auto prenorm = [&](const Norm& n) -> const T* {
+      if (Y == nullptr) return X;
+      ProfScope ps(this, PROF_LN, 8.0 * M * d, 2.0 * sizeof(T) * M * dp, s);
+      layernorm<T>(X, dp, n.gamma, n.beta, Y, dp, M, d, s, dp, 1e-5f);
+      return Y;
+    };
+    auto folded = [&](const Linear& L) {
+      Epi e;
+      if (Y == nullptr) { e.bias = L.ln_c2; e.ln_stats = stats; } else { e.bias = L.bias; }
+      return e;
+    };
+    auto residual = [&](const T* A, int lda, const Linear& L) {     // X = A W + b + X, and X's new row statistics
+      Epi e; e.bias = L.bias; e.res = X; e.ldr = dp; e.stats_out = stats;
+      linear<T>(A, lda, M, L, X, dp, e, s);
+    };
+    auto mlp = [&](const MlpW& m) {                                   // crossformer.py:89-102
+      const T* a = prenorm(m.norm);
+      T* Hb = arena.get<T>(static_cast<size_t>(M) * m.fc1.N);
+      Epi e1 = folded(m.fc1);
+      e1.gelu = true;
+      linear<T>(a, dp, M, m.fc1, Hb, m.fc1.N, e1, s);
+      residual(Hb, m.fc1.N, m.fc2);
+    };
+    auto attend = [&](const CrossformerAttnW& at) {                   // crossformer.py:133-180
+      const T* a = prenorm(at.norm);
+      const int ld = at.qkv.N;
+      T* QKV = arena.get<T>(static_cast<size_t>(M) * ld);
+      linear<T>(a, dp, M, at.qkv, QKV, ld, folded(at.qkv), s);
+      if (at.wsz > 1) {                                               // wsz == 1: the output is v itself, which QKV holds
+        Window win;
+        win.p = at.wsz; win.nx = Wd / at.wsz; win.ny = H / at.wsz; win.dilated = at.dilated;
+        PosBias pb;
+        pb.table = at.table; pb.wsz = at.wsz;
+        const int n = at.wsz * at.wsz;
+        attention_dispatch<T>(QKV, ld, QKV + I, ld, QKV + 2 * I, ld, QKV, ld, B * win.nx * win.ny, n, n, S.heads, 32, 0, nullptr, nullptr,
+                              nullptr, nullptr, s, 0.f, &win, &pb);
+      }
+      residual(QKV, ld, at.to_out);                                   // to_out reads the I output (or v) columns
+    };
+    attend(l.short_attn);
+    mlp(l.ff1);
+    attend(l.long_attn);
     mlp(l.ff2);
   }
 
@@ -2070,6 +2341,7 @@ struct vb_handle {
     VB_CHECK(cfg.kind != VB_KIND_LEVIT, kLevitNoStages);
     VB_CHECK(cfg.kind != VB_KIND_CVT, kCvtNoStages);
     VB_CHECK(cfg.kind != VB_KIND_TWINS_SVT, kTwinsNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_CROSSFORMER, kCrossformerNoStages);
     if (cfg.kind == VB_KIND_T2T_VIT) {
       int h = H, w = Wd;
       for (const auto& st : t2t_stages()) { h = (h + st.stride - 1) / st.stride; w = (w + st.stride - 1) / st.stride; }
@@ -2098,6 +2370,7 @@ struct vb_handle {
     VB_CHECK(cfg.kind != VB_KIND_LEVIT, kLevitNoStages);
     VB_CHECK(cfg.kind != VB_KIND_CVT, kCvtNoStages);
     VB_CHECK(cfg.kind != VB_KIND_TWINS_SVT, kTwinsNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_CROSSFORMER, kCrossformerNoStages);
     arena.reset();
     const long long count = static_cast<long long>(B) * n * cfg.dim;
     T* X = arena.get<T>(count);
@@ -2112,6 +2385,7 @@ struct vb_handle {
     VB_CHECK(cfg.kind != VB_KIND_LEVIT, kLevitNoStages);
     VB_CHECK(cfg.kind != VB_KIND_CVT, kCvtNoStages);
     VB_CHECK(cfg.kind != VB_KIND_TWINS_SVT, kTwinsNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_CROSSFORMER, kCrossformerNoStages);
     arena.reset();
     const int K = embed.patch.K, Kp = bf16() ? embed.patch.ldw : K;
     T* col = arena.get<T>(static_cast<size_t>(rows) * Kp);
@@ -2237,14 +2511,16 @@ void vb_handle::layer_t2t<__nv_bfloat16>(__nv_bfloat16* X, int B, int n, const L
 template <typename T>
 void vb_handle::attention_dispatch(const T* q, int ldq, const T* k, int ldk, const T* v, int ldv, T* out, int ldo, int B, int nq,
                                    int nk, int heads, int dh, int variant, const float* mix_a, const float* mix_b, const float* g,
-                                   const float* b, cudaStream_t s, float scale, const Window* win) {
-  if (win != nullptr) {                       // Twins-SVT's local attention: B windows of nq = nk = p^2 tokens in the map's own rows
+                                   const float* b, cudaStream_t s, float scale, const Window* win, const PosBias* pb) {
+  // windowed attention (Twins-SVT's local, CrossFormer's short / long with pb, its window table): B windows of nq = nk = p^2
+  // tokens in the map's own rows
+  if (win != nullptr) {
     const int HD = heads * dh;
     VB_CHECK(k == q + HD && v == q + 2 * HD && ldk == ldq && ldv == ldq && variant == 0, "internal: windowed attention reads fused q|k|v rows");
     const double fl = 4.0 * B * heads * nq * nk * dh, by = static_cast<double>(sizeof(T)) * B * heads * dh * (2.0 * nq + 2.0 * nk);
     {
       ProfScope ps(this, PROF_ATTN, fl, by, s);
-      if (attention_fast<T>(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, heads, dh, 0, nullptr, nullptr, nullptr, nullptr, s, 0.f, nullptr, win))
+      if (attention_fast<T>(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, heads, dh, 0, nullptr, nullptr, nullptr, nullptr, s, 0.f, pb, win))
         return;
     }
     // off the flash kernel: the rows permuted to window-major order, the materialised-scores path, the output rows permuted back
@@ -2256,7 +2532,7 @@ void vb_handle::attention_dispatch(const T* q, int ldq, const T* k, int ldk, con
       ProfScope ps(this, PROF_ATTN, fl, by, s);
       float* S = arena.get<float>(static_cast<size_t>(B) * heads * nq * ((nk + 15) & ~15));
       attention_generic<T>(qkvw, 3 * HD, qkvw + HD, 3 * HD, qkvw + 2 * HD, 3 * HD, ow, HD, S, B, nq, nk, heads, dh, 0, nullptr, nullptr, nullptr,
-                           nullptr, s);
+                           nullptr, s, 0.f, pb);
     }
     { ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * rows * HD, s); window_rows<T>(ow, HD, out, ldo, HD, *win, rows, false, s); }
     return;
@@ -2308,6 +2584,7 @@ void validate(const vb_config& c) {
   VB_CHECK(c.kind != VB_KIND_LEVIT, "LeViT: create the handle with vb_create_levit (its stages are a vb_levit_config)");
   VB_CHECK(c.kind != VB_KIND_CVT, "CvT: create the handle with vb_create_cvt (its stages are a vb_cvt_config)");
   VB_CHECK(c.kind != VB_KIND_TWINS_SVT, "Twins-SVT: create the handle with vb_create_twins_svt (its stages are a vb_twins_svt_config)");
+  VB_CHECK(c.kind != VB_KIND_CROSSFORMER, "CrossFormer: create the handle with vb_create_crossformer (its stages are a vb_crossformer_config)");
   VB_CHECK(c.kind >= VB_KIND_VIT && c.kind <= VB_KIND_CCT, "unknown model kind");
   if (c.kind == VB_KIND_CCT) {
     VB_CHECK(c.channels == 3 && c.num_classes > 0 && c.image_h > 0 && c.image_w > 0, "bad image / class configuration");
@@ -2384,6 +2661,30 @@ void validate_twins(const vb_config& c, const vb_twins_svt_config& tw) {
     VB_CHECK(tw.emb_dim[st] > 0 && tw.patch_size[st] > 0 && tw.local_patch_size[st] > 0 && tw.global_k[st] > 0 && tw.depth[st] >= 0,
              "Twins-SVT: bad stage configuration");
   VB_CHECK(tw.peg_kernel_size >= 1 && tw.peg_kernel_size <= 7, "Twins-SVT: peg_kernel_size must be in [1, 7] (the depthwise kernel's halo tile)");
+}
+
+void validate_crossformer(const vb_config& c, const vb_crossformer_config& cf) {
+  VB_CHECK(c.precision == VB_PRECISION_FP32 || c.precision == VB_PRECISION_BF16, "unknown precision");
+  VB_CHECK(c.channels > 0 && c.num_classes > 0, "CrossFormer: bad channel / class configuration");
+  for (int st = 0; st < VB_CROSSFORMER_STAGES; ++st) {
+    const std::string stage = "CrossFormer stage " + std::to_string(st + 1) + ": ";
+    VB_CHECK(cf.dim[st] >= 32, stage + "dim must be at least 32 (heads = dim // 32 of width 32)");
+    VB_CHECK(cf.depth[st] >= 0 && cf.global_wsz[st] > 0 && cf.local_wsz[st] > 0 && cf.stride[st] > 0, stage + "bad depth / window / stride");
+    VB_CHECK(cf.n_kernels[st] >= 1 && cf.n_kernels[st] <= VB_CROSSFORMER_MAX_KERNELS,
+             stage + "between 1 and " + std::to_string(VB_CROSSFORMER_MAX_KERNELS) + " cross-embedding kernel sizes are supported");
+    std::string ks;
+    bool pos = true, parity = true, above = true;
+    for (int i = 0; i < cf.n_kernels[st]; ++i) {
+      const int k = cf.kernels[st][i];
+      ks += (i ? ", " : "") + std::to_string(k);
+      pos = pos && k > 0;
+      parity = parity && (k - cf.kernels[st][0]) % 2 == 0;
+      above = above && k >= cf.stride[st];
+    }
+    VB_CHECK(pos, stage + "kernel sizes must be positive");
+    VB_CHECK(parity && above, stage + "kernel sizes (" + ks + ") at stride " + std::to_string(cf.stride[st]) +
+                                  ": the nested cross-scale embedding needs kernels of one parity, each at least the stride");
+  }
 }
 
 }  // namespace
@@ -2593,6 +2894,35 @@ int vb_create_twins_svt(const vb_config* base, const vb_twins_svt_config* tw, in
   });
 }
 
+int vb_create_crossformer(const vb_config* base, const vb_crossformer_config* cfc, int device, vb_handle** out) {
+  return guarded(nullptr, [&] {
+    VB_CHECK(base != nullptr && cfc != nullptr && out != nullptr, "vb_create_crossformer: null argument");
+    VB_CHECK(base->struct_size == static_cast<int32_t>(sizeof(vb_config)) || base->struct_size == VB_CONFIG_SIZE_ABI7,
+             "vb_config.struct_size mismatch (ABI)");
+    VB_CHECK(cfc->struct_size == static_cast<int32_t>(sizeof(vb_crossformer_config)), "vb_crossformer_config.struct_size mismatch (ABI)");
+    vb_config c;
+    memset(&c, 0, sizeof c);
+    memcpy(&c, base, static_cast<size_t>(base->struct_size));
+    VB_CHECK(c.kind == VB_KIND_CROSSFORMER, "vb_create_crossformer: base.kind must be VB_KIND_CROSSFORMER");
+    validate_crossformer(c, *cfc);
+    int ndev = 0;
+    cudaError_t e = cudaGetDeviceCount(&ndev);
+    VB_CHECK(e == cudaSuccess && ndev > 0, "vb_create_crossformer: no CUDA device available -- libvitb200 has no CPU fallback");
+    VB_CHECK(device >= 0 && device < ndev, "vb_create_crossformer: bad device index");
+    VB_CUDA(cudaSetDevice(device));
+    cudaDeviceProp prop;
+    VB_CUDA(cudaGetDeviceProperties(&prop, device));
+    VB_CHECK(prop.major == 9 && prop.minor == 0, "vb_create_crossformer: libvitb200 is built for sm_90a (Hopper H100) only");
+    std::unique_ptr<vb_handle> h(new vb_handle());
+    h->cfg = c;
+    h->cfg.dim = cfc->dim[VB_CROSSFORMER_STAGES - 1];
+    h->cf = *cfc;
+    h->device = device;
+    h->build_expected();
+    *out = h.release();
+  });
+}
+
 int vb_num_weights(vb_handle* h) { return h ? static_cast<int>(h->weights.size()) : -1; }
 
 int vb_weight_info(vb_handle* h, int32_t index, const char** name, int64_t* shape4, int32_t* ndim) {
@@ -2718,6 +3048,7 @@ int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, int32_t 
     VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_forward_distill: bad batch / image size");
     VB_CHECK(h->cfg.kind != VB_KIND_CVT, "vb_forward_distill: CvT has no distillation head");
     VB_CHECK(h->cfg.kind != VB_KIND_TWINS_SVT, "vb_forward_distill: Twins-SVT has no distillation head");
+    VB_CHECK(h->cfg.kind != VB_KIND_CROSSFORMER, "vb_forward_distill: CrossFormer has no distillation head");
     const bool levit = h->cfg.kind == VB_KIND_LEVIT;
     VB_CHECK(levit || distill_token != nullptr, "vb_forward_distill: null argument");
     VB_CHECK(!levit || (distill_token == nullptr && h->lv.num_distill_classes > 0),
@@ -2775,6 +3106,7 @@ int vb_forward_tokens(vb_handle* h, const float* tokens, int32_t tokens_mem, int
     VB_CHECK(batch > 0 && n > 0, "vb_forward_tokens: bad shape");
     VB_CHECK(h->cfg.kind != VB_KIND_CVT, vb_handle::kCvtNoStages);
     VB_CHECK(h->cfg.kind != VB_KIND_TWINS_SVT, vb_handle::kTwinsNoStages);
+    VB_CHECK(h->cfg.kind != VB_KIND_CROSSFORMER, vb_handle::kCrossformerNoStages);
     VB_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const long long before = launch_counter();
@@ -2844,7 +3176,8 @@ int vb_to_patch(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, 
   return guarded(h, [&] {
     VB_CHECK(h != nullptr && img != nullptr && patches != nullptr, "vb_to_patch: null argument");
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT && h->cfg.kind != VB_KIND_T2T_VIT && h->cfg.kind != VB_KIND_CCT &&
-             h->cfg.kind != VB_KIND_LEVIT && h->cfg.kind != VB_KIND_CVT && h->cfg.kind != VB_KIND_TWINS_SVT,
+             h->cfg.kind != VB_KIND_LEVIT && h->cfg.kind != VB_KIND_CVT && h->cfg.kind != VB_KIND_TWINS_SVT &&
+             h->cfg.kind != VB_KIND_CROSSFORMER,
              "vb_to_patch: the model has no single Rearrange patch layer");
     VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_to_patch: bad batch / image size");
     const vb_config& c = h->cfg;
@@ -2868,6 +3201,7 @@ int vb_patch_to_emb(vb_handle* h, const float* patches, int32_t patches_mem, int
     VB_CHECK(h->cfg.kind != VB_KIND_LEVIT, vb_handle::kLevitNoStages);
     VB_CHECK(h->cfg.kind != VB_KIND_CVT, vb_handle::kCvtNoStages);
     VB_CHECK(h->cfg.kind != VB_KIND_TWINS_SVT, vb_handle::kTwinsNoStages);
+    VB_CHECK(h->cfg.kind != VB_KIND_CROSSFORMER, vb_handle::kCrossformerNoStages);
     VB_CHECK(rows > 0, "vb_patch_to_emb: bad shape");
     const size_t in_bytes = static_cast<size_t>(rows) * h->embed.patch.K * sizeof(float);
     const size_t out_bytes = static_cast<size_t>(rows) * h->cfg.dim * sizeof(float);
@@ -3336,6 +3670,47 @@ int vb_op_window_attention(int32_t precision, const float* qkv, int32_t ld, int3
         window_rows<T>(x_d, ld, w_d, 3 * HD, 3 * HD, win, rows, true, 0);
         attention_generic<T>(w_d, 3 * HD, w_d + HD, 3 * HD, w_d + 2 * HD, 3 * HD, ow_d, HD, static_cast<float*>(dS.p), Bw, n, n, heads, dh, 0,
                              nullptr, nullptr, nullptr, nullptr, 0);
+        window_rows<T>(ow_d, HD, o_d, ldo, HD, win, rows, false, 0);
+      });
+      download<T>(o_d, out, static_cast<size_t>(rows) * ldo);
+    };
+    if (precision == VB_PRECISION_FP32) run(float());
+    else run(__nv_bfloat16());
+  });
+}
+
+int vb_op_window_bias_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t H, int32_t W, int32_t wsz,
+                                int32_t is_long, int32_t heads, int32_t dh, const float* table, float* out, int32_t ldo, int32_t iters,
+                                float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    const int HD = heads * dh;
+    VB_CHECK(qkv && table && out && B > 0 && wsz > 0 && H > 0 && W > 0 && H % wsz == 0 && W % wsz == 0 && heads > 0 && dh > 0 &&
+             ld >= 3 * HD && ldo >= HD, "vb_op_window_bias_attention: bad arguments");
+    Window win;
+    win.p = wsz; win.nx = W / wsz; win.ny = H / wsz; win.dilated = is_long != 0;
+    const int n = wsz * wsz, Bw = B * win.nx * win.ny, t = (2 * wsz - 1) * (2 * wsz - 1);
+    const long long rows = static_cast<long long>(B) * H * W;
+    DevMem dX, dO, dW, dOw, dS, dT;
+    PosBias pb;
+    pb.table = upload<float>(dT, table, t); pb.wsz = wsz;
+    auto run = [&](auto tag) {
+      using T = decltype(tag);
+      const T* x_d = upload<T>(dX, qkv, static_cast<size_t>(rows) * ld);
+      T* o_d = upload<T>(dO, out, static_cast<size_t>(rows) * ldo);
+      // vb_handle::attention_dispatch's windowed branch without the handle's arena and profiler
+      timed(iters, elapsed_ms, [&] {
+        if (attention_fast<T>(x_d, ld, x_d + HD, ld, x_d + 2 * HD, ld, o_d, ldo, Bw, n, n, heads, dh, 0, nullptr, nullptr, nullptr, nullptr, 0, 0.f,
+                              &pb, &win))
+          return;
+        dW.ensure(static_cast<size_t>(rows) * 3 * HD * sizeof(T));
+        dOw.ensure(static_cast<size_t>(rows) * HD * sizeof(T));
+        dS.ensure(static_cast<size_t>(Bw) * heads * n * ((n + 15) & ~15) * sizeof(float));
+        T* w_d = static_cast<T*>(dW.p);
+        T* ow_d = static_cast<T*>(dOw.p);
+        window_rows<T>(x_d, ld, w_d, 3 * HD, 3 * HD, win, rows, true, 0);
+        attention_generic<T>(w_d, 3 * HD, w_d + HD, 3 * HD, w_d + 2 * HD, 3 * HD, ow_d, HD, static_cast<float*>(dS.p), Bw, n, n, heads, dh, 0,
+                             nullptr, nullptr, nullptr, nullptr, 0, 0.f, &pb);
         window_rows<T>(ow_d, HD, o_d, ldo, HD, win, rows, false, 0);
       });
       download<T>(o_d, out, static_cast<size_t>(rows) * ldo);

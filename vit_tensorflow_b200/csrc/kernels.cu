@@ -499,6 +499,15 @@ __global__ void attn_pos_bias_kernel(float* __restrict__ S, const float* __restr
   }
 }
 
+// S[w,h,i,j] += table[window_bias_index(i, j, wsz)]  (CrossFormer's window table, shared by the heads; row pitch nk = wsz^2)
+__global__ void attn_window_bias_kernel(float* __restrict__ S, const float* __restrict__ table, int nk, int wsz, long long total) {
+  for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
+       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int j = static_cast<int>(idx % nk), i = static_cast<int>((idx / nk) % nk);
+    S[idx] += table[window_bias_index(i, j, wsz)];
+  }
+}
+
 // out[b, r*ow + c, :] = in[b, (step*r)*W + step*c, :]  (16-byte vectors when C, ld are multiples of the vector width)
 template <typename T>
 __global__ void gather_grid_kernel(const T* __restrict__ in, int ldi, T* __restrict__ out, int ldo, int H, int W, int C, int step,
@@ -1128,6 +1137,12 @@ void attn_pv(const float* S, const T* v, int ldv, T* out, int ldo, int B, int he
 
 void attn_pos_bias(float* S, const PosBias& pb, int B, int heads, int nq, int nk, cudaStream_t s) {
   const long long total = static_cast<long long>(B) * heads * nq * nk;
+  if (pb.wsz > 0) {
+    VB_CHECK(nq == pb.wsz * pb.wsz && nk == nq, "attention: the window table needs nq == nk == wsz^2");
+    attn_window_bias_kernel<<<grid_1d(total, 256), 256, 0, s>>>(S, pb.table, nk, pb.wsz, total);
+    VB_LAUNCHED();
+    return;
+  }
   attn_pos_bias_kernel<<<grid_1d(total, 256), 256, 0, s>>>(S, pb.table, heads, nq, nk, pb.fmap, pb.step, total);
   VB_LAUNCHED();
 }

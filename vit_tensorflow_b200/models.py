@@ -7,6 +7,7 @@
     efficient.ViT  vit_tensorflow/efficient.py:12-55 (injected transformer between the engine's embed and head stages)
     CvT       vit_tensorflow/cvt.py:149-202
     TwinsSVT  vit_tensorflow/twins_svt.py:215-268
+    CrossFormer  vit_tensorflow/crossformer.py:205-269
 
 Same constructor kwargs, defaults and assertion messages; `model(img, training=True, **kwargs) -> logits`
 with `img` NHWC float32 `[b, H, W, 3]` and logits float32 `[b, num_classes]`.  Everything below the call is
@@ -1108,8 +1109,148 @@ class TwinsSVT(_EngineModel):
 TWINS_CTOR_KEYS = ("num_classes",) + tuple(f"s{i}_{k}" for i in (1, 2, 3, 4) for k in TWINS_STAGE_KEYS) + ("peg_kernel_size", "dropout")
 
 
+def _cast_tuple(val, length=1):                     # crossformer.py:11-12
+    return val if isinstance(val, tuple) else ((val,) * length)
+
+
+def crossformer_size_error(stages, h, w):
+    """The reference's shape rule (crossformer.py:144,146, enforced there by einops) for an h x w image: None, or what the first
+    stage that breaks it says.  Each stage map is ceil(previous / stride) (the SAME convolutions)."""
+    for i, st in enumerate(stages, 1):
+        h, w = -(-h // st["stride"]), -(-w // st["stride"])
+        for key, name in (("local_wsz", "local_window_size"), ("global_wsz", "global_window_size")):
+            if h % st[key] or w % st[key]:
+                return f"CrossFormer stage {i}: the {h} x {w} map is not divisible by {name} {st[key]}"
+    return None
+
+
+class CrossFormer(_EngineModel):
+    """crossformer.py:205-269: four stages of a CrossEmbedLayer (one SAME Conv2D per kernel size at the stage's stride, the kernel
+    sizes sorted, dim / 2, dim / 4, ... channels and the rest for the largest, concatenated) and a Transformer whose layers are
+    short attention within local_window_size blocks, an MLP, long attention within global_window_size dilated windows and an MLP,
+    each with its own LayerNorm and a residual; then the mean over the map and Dense(num_classes).  Attention has dim // 32 heads
+    of 32 and a DynamicPositionBias scalar per in-window offset, shared by the heads.
+
+    There are no position embeddings and no image_size: any image whose every stage map is divisible by that stage's local and
+    global window sizes runs; other sizes raise ValueError naming the stage.  The engine runs a stage's cross-scale embedding as
+    one convolution with the smaller kernels nested at the centre of the largest, which is exact for every image when the
+    stage's kernel sizes share one parity and are all at least its stride (the reference's defaults are); other kernel sets,
+    more than 4 kernel sizes and dims below 32 raise ValueError.  attn_dropout is accepted and unused, as in the reference; with
+    ff_dropout > 0 only training=False runs.  Weights (SURVEY.md App. B) keep the reference's attribute paths:
+    crossformer_layers.{s}.0.convs.{i}, crossformer_layers.{s}.1.layers.{l}.{0|2}.{norm, to_qkv, to_out, dpb.dpb_layers.{0..9}},
+    crossformer_layers.{s}.1.layers.{l}.{1|3}.net.{0, 1, 4}, to_logits.1 (the Dense head)."""
+    _kind = "crossformer"
+
+    def __init__(self,
+                 dim=(64, 128, 256, 512),
+                 depth=(2, 2, 8, 2),
+                 global_window_size=(8, 4, 2, 1),
+                 local_window_size=7,
+                 cross_embed_kernel_sizes=((4, 8, 16, 32), (2, 4), (2, 4), (2, 4)),
+                 cross_embed_strides=(4, 2, 2, 2),
+                 num_classes=1000,
+                 attn_dropout=0.0,
+                 ff_dropout=0.0,
+                 *, precision="bf16", device=0, seed=None):
+        dim = _cast_tuple(dim, 4)
+        depth = _cast_tuple(depth, 4)
+        global_window_size = _cast_tuple(global_window_size, 4)
+        local_window_size = _cast_tuple(local_window_size, 4)
+        cross_embed_kernel_sizes = _cast_tuple(cross_embed_kernel_sizes, 4)
+        cross_embed_strides = _cast_tuple(cross_embed_strides, 4)
+        assert len(dim) == 4
+        assert len(depth) == 4
+        assert len(global_window_size) == 4
+        assert len(local_window_size) == 4
+        assert len(cross_embed_kernel_sizes) == 4
+        assert len(cross_embed_strides) == 4
+        self.num_classes = num_classes
+        self.stages = tuple(dict(dim=int(d), depth=int(n), global_wsz=int(g), local_wsz=int(lw), kernels=tuple(sorted(k)), stride=int(st))
+                            for d, n, g, lw, k, st in zip(dim, depth, global_window_size, local_window_size, cross_embed_kernel_sizes,
+                                                          cross_embed_strides))
+        self._dropout_rates = (ff_dropout,)
+        for i, st in enumerate(self.stages, 1):
+            ks = st["kernels"]
+            if st["dim"] < 32:
+                raise ValueError(f"CrossFormer stage {i}: dim {st['dim']} is not supported (at least 32: dim // 32 heads of 32)")
+            if not 1 <= len(ks) <= _lib.CROSSFORMER_MAX_KERNELS:
+                raise ValueError(f"CrossFormer stage {i}: {len(ks)} cross-embedding kernel sizes {ks}; at most "
+                                 f"{_lib.CROSSFORMER_MAX_KERNELS} are supported")
+            if len({k % 2 for k in ks}) != 1 or min(ks) < st["stride"]:
+                raise ValueError(f"CrossFormer stage {i}: kernel sizes {ks} at stride {st['stride']} are not supported: the nested "
+                                 "cross-scale embedding needs kernel sizes of one parity, each at least the stride")
+        self.precision = precision
+        self.device = int(device)
+        cfg = _lib.VbConfig()
+        cfg.struct_size = C.sizeof(_lib.VbConfig)
+        cfg.kind = _lib.KIND["crossformer"]
+        if precision not in _lib.PRECISION:
+            raise ValueError(f"precision must be one of {sorted(_lib.PRECISION)}")
+        cfg.precision = _lib.PRECISION[precision]
+        cfg.channels, cfg.num_classes = 3, num_classes
+        cfg.dim = self.stages[-1]["dim"]
+        cf = _lib.VbCrossformerConfig()
+        cf.struct_size = C.sizeof(_lib.VbCrossformerConfig)
+        for i, st in enumerate(self.stages):
+            for k in ("dim", "depth", "global_wsz", "local_wsz", "stride"):
+                getattr(cf, k)[i] = st[k]
+            cf.n_kernels[i] = len(st["kernels"])
+            for j, k in enumerate(st["kernels"]):
+                cf.kernels[i][j] = int(k)
+        self._cfg, self._cf = cfg, cf
+        self._lib = _lib.load()
+        h = C.c_void_p()
+        _lib.check(self._lib.vb_create_crossformer(C.byref(cfg), C.byref(cf), self.device, C.byref(h)))
+        self._h = h
+        self._finalized = False
+        self._specs = collections.OrderedDict()
+        name, shape, ndim = C.c_char_p(), (C.c_int64 * 4)(), C.c_int32()
+        for i in range(self._lib.vb_num_weights(h)):
+            _lib.check(self._lib.vb_weight_info(h, i, C.byref(name), shape, C.byref(ndim)), h)
+            self._specs[name.value.decode()] = tuple(int(shape[j]) for j in range(ndim.value))
+        self._weights = collections.OrderedDict()
+        self.init_weights(seed)
+
+    def init_weights(self, seed=None):
+        """The reference's initialisers: glorot-uniform over the receptive field for every Conv2D and Dense kernel, zero biases,
+        LayerNorm g 1 / b 0 and LayerNormalization gamma 1 / beta 0."""
+        rng = np.random.default_rng(seed)
+        w = collections.OrderedDict()
+        for name, shape in self._specs.items():
+            leaf = name.rsplit(".", 1)[-1]
+            if leaf == "kernel":
+                receptive = int(np.prod(shape[:-2]))
+                lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
+                a = rng.uniform(-lim, lim, size=shape)
+            elif leaf in ("bias", "b", "beta"):
+                a = np.zeros(shape)
+            elif leaf in ("g", "gamma"):
+                a = np.ones(shape)
+            else:
+                raise AssertionError(name)
+            w[name] = a.astype(np.float32)
+        self.set_weights_dict(w)
+
+    def __call__(self, img, training=True, **kwargs):
+        """crossformer.py:263-269: NHWC float images -> logits [b, num_classes]; extra kwargs are accepted and ignored, as there."""
+        x = np.asarray(img)
+        if x.ndim == 4:
+            err = crossformer_size_error(self.stages, x.shape[1], x.shape[2])
+            if err is not None:
+                raise ValueError(err)
+        return super().__call__(img, training=training)
+
+    call = __call__
+
+
+CROSSFORMER_CTOR_KEYS = ("dim", "depth", "global_window_size", "local_window_size", "cross_embed_kernel_sizes", "cross_embed_strides",
+                         "num_classes", "attn_dropout", "ff_dropout")
+
+
 def from_config(cfg: dict, precision="bf16", device=0, seed=None):
     """Build a model from an oracle-style config dict (kind + reference kwargs)."""
+    if cfg["kind"] == "crossformer":
+        return CrossFormer(**{k: v for k, v in cfg.items() if k in CROSSFORMER_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "twins_svt":
         return TwinsSVT(**{k: v for k, v in cfg.items() if k in TWINS_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "cvt":
