@@ -109,6 +109,10 @@ struct Window {
 // 2-D bf16 (or fp32) tensor map (innermost dimension first), 128-byte swizzle unless swizzle128 == false.
 CUtensorMap make_tmap_2d(const void* base, uint64_t inner, uint64_t outer, uint64_t outer_stride_bytes,
                          uint32_t box_inner, uint32_t box_outer, bool swizzle128 = true, bool f32 = false);
+// 3-D bf16 tensor map {d0, d1, d2} (innermost first; strides of d1 and d2 in bytes), box {box0, box1, 1}, 128-byte swizzle.
+// Coordinates past d1 read as zero.
+CUtensorMap make_tmap_3d(const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1_bytes, uint64_t stride2_bytes,
+                         uint32_t box0, uint32_t box1);
 
 // Activation of a GEMM epilogue: exact-erf GELU (vit.py:34) or hard-swish x * relu6(x + 3) / 6 (levit.py:36-38).  ACT_GELU is 1,
 // so the `gelu` flags (bool / int 0-1) of the older entry points convert to it unchanged.

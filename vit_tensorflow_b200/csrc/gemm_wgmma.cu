@@ -355,6 +355,20 @@ CUtensorMap make_tmap_2d(const void* base, uint64_t inner, uint64_t outer, uint6
   return m;
 }
 
+CUtensorMap make_tmap_3d(const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1_bytes, uint64_t stride2_bytes,
+                         uint32_t box0, uint32_t box1) {
+  CUtensorMap m;
+  cuuint64_t dims[3] = {d0, d1, d2};
+  cuuint64_t strides[2] = {stride1_bytes, stride2_bytes};
+  cuuint32_t box[3] = {box0, box1, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = get_encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
+                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  VB_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(3d) failed with CUresult " + std::to_string(static_cast<int>(r)));
+  return m;
+}
+
 bool gemm_bf16_supported(int M, int N, int K, int lda, int ldw, int ldc) {
   return M > 0 && N > 0 && K > 0 && (N % 64 == 0) && (K % 8 == 0) && (lda % 8 == 0) && (ldw % 8 == 0) && (ldc % 8 == 0);
 }
