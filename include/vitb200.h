@@ -14,6 +14,7 @@
  *     CvT(...)(img)                  vit_tensorflow/cvt.py:149-202 (vb_create_cvt)
  *     TwinsSVT(...)(img)             vit_tensorflow/twins_svt.py:215-268 (vb_create_twins_svt)
  *     CrossFormer(...)(img)          vit_tensorflow/crossformer.py:205-269 (vb_create_crossformer)
+ *     NesT(...)(img)                 vit_tensorflow/nest.py:150-216 (vb_create_nest)
  * and this header is what the Python host classes (vit_tensorflow_b200/models.py, _lib.py) bind with ctypes.
  * Plain pointers and sizes only; no torch / C++ types cross the boundary.
  *
@@ -44,7 +45,7 @@ typedef struct vb_handle vb_handle;
 
 enum { VB_KIND_VIT = 0, VB_KIND_DEEPVIT = 1, VB_KIND_CAIT = 2, VB_KIND_CROSSVIT = 3, VB_KIND_PARALLEL_VIT = 4,
        VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6, VB_KIND_CCT = 7, VB_KIND_LEVIT = 8,
-       VB_KIND_CVT = 9, VB_KIND_TWINS_SVT = 10, VB_KIND_CROSSFORMER = 11 };
+       VB_KIND_CVT = 9, VB_KIND_TWINS_SVT = 10, VB_KIND_CROSSFORMER = 11, VB_KIND_NEST = 12 };
 enum { VB_CCT_POS_SINE = 0, VB_CCT_POS_LEARNABLE = 1, VB_CCT_POS_NONE = 2 };   /* cct.py:233-234,250-256 */
 enum { VB_PRECISION_FP32 = 0, VB_PRECISION_BF16 = 1 };
 enum { VB_POOL_CLS = 0, VB_POOL_MEAN = 1 };
@@ -89,8 +90,8 @@ typedef struct vb_config {
 VB_API int vb_abi_version(void);
 
 /* Replaces <Model>.__init__ (vit.py:107-157 etc.): validates the config and allocates device state.  VB_KIND_LEVIT, VB_KIND_CVT,
- * VB_KIND_TWINS_SVT and VB_KIND_CROSSFORMER are refused here: their handles come from vb_create_levit, vb_create_cvt,
- * vb_create_twins_svt and vb_create_crossformer. */
+ * VB_KIND_TWINS_SVT, VB_KIND_CROSSFORMER and VB_KIND_NEST are refused here: their handles come from vb_create_levit,
+ * vb_create_cvt, vb_create_twins_svt, vb_create_crossformer and vb_create_nest. */
 VB_API int vb_create(const vb_config* cfg, int device, vb_handle** out);
 
 /* LeViT (levit.py:164-212), appended within ABI 7.  `dims`, `depths` and `heads` hold `stages` entries each (cast_tuple already
@@ -202,6 +203,46 @@ typedef struct vb_crossformer_config {
  * vb_finalize evaluates every DynamicPositionBias on the host: it depends on the weights alone. */
 VB_API int vb_create_crossformer(const vb_config* base, const vb_crossformer_config* cf, int device, vb_handle** out);
 
+/* NesT (nest.py:150-216), appended within ABI 7.  Patch embedding 'b (h p1) (w p2) c -> b h w (p1 p2 c)' and a 1x1 Conv2D(dim)
+ * with bias.  `levels` = len(zip(hierarchies, ..., block_repeats)) (nest.py:187): the cast_tuple'd block_repeats truncated to
+ * num_hierarchies, or fewer levels when the tuple is shorter; block_repeats[i] is level i's depth.  Level i (bottom first) has
+ * width dim * 2^i, heads * 2^i heads of dim_head = dim / heads (inner = dim_head * heads * 2^i may be below the width), and
+ * runs on blocks of 2^(levels - 1 - i) x 2^(levels - 1 - i) per map (:208-209): x += pos_emb[:h w] (one scalar per in-block
+ * position r * w + c of an h x w block, added to every channel), then block_repeats[i] x [x = Attention(LN(x)) + x,
+ * x = MLP(LN(x)) + x] within each block, then Aggregate (Conv2D(3, SAME) with bias to width dim * 2^(i+1), LayerNorm,
+ * MaxPool2D(3, 2, SAME)) unless i == num_hierarchies - 1.  Attention (:77-109): a bias-free 1x1 to_qkv, softmax(q k^T *
+ * dim_head^-0.5) v per head, a 1x1 to_out with bias.  MLP (:61-75): 1x1 to width * mlp_mult, exact GELU, 1x1 back.  Every
+ * LayerNorm is the module's own (eps 1e-5, biased variance, :28-41).  Head: LayerNorm(dim * 2^(num_hierarchies - 1)) per pixel,
+ * the mean over the map, Dense(num_classes).  Any image runs whose sides are multiples of patch_size and whose maps are whole
+ * blocks of at most seq_len tokens at every level. */
+#define VB_NEST_MAX_LEVELS 8
+typedef struct vb_nest_config {
+  int32_t struct_size;            /* sizeof(vb_nest_config) */
+  int32_t patch_size, dim, heads;
+  int32_t num_hierarchies;        /* 1 .. VB_NEST_MAX_LEVELS */
+  int32_t levels;                 /* 0 .. num_hierarchies: the levels the zip leaves */
+  int32_t block_repeats[VB_NEST_MAX_LEVELS];   /* the first `levels` entries */
+  int32_t mlp_mult;
+  int32_t seq_len;                /* (image_size / patch_size / 2^(num_hierarchies - 1))^2: the length of every pos_emb */
+} vb_nest_config;
+
+/* NesT.__init__: `base` supplies precision, channels, num_classes and max_batch; its kind must be VB_KIND_NEST and its other
+ * fields are ignored.  Weights (SURVEY.md App. B) are named by the reference's attribute paths, for level i, layer l, width d
+ * (d_next the next level's), inner = (dim / heads) * heads * 2^i:
+ *   patch_embedding.1.kernel [1, 1, p^2 * channels, dim] / .bias [dim]            (rows in (p1, p2, c) order, c fastest)
+ *   nest_layers.{i}.0.pos_emb [seq_len]
+ *   nest_layers.{i}.0.layers.{l}.0.norm.g / .b [1, 1, 1, d]
+ *   nest_layers.{i}.0.layers.{l}.0.fn.to_qkv.kernel [1, 1, d, 3 * inner]
+ *   nest_layers.{i}.0.layers.{l}.0.fn.to_out.0.kernel [1, 1, inner, d] / .bias [d]
+ *   nest_layers.{i}.0.layers.{l}.1.norm.g / .b [1, 1, 1, d]
+ *   nest_layers.{i}.0.layers.{l}.1.fn.net.0.kernel [1, 1, d, d * mlp_mult] / .bias, ....1.fn.net.3.kernel [1, 1, d * mlp_mult, d] / .bias
+ *   nest_layers.{i}.1.ag_layers.0.kernel [3, 3, d, d_next] / .bias [d_next]     (levels with an Aggregate only)
+ *   nest_layers.{i}.1.ag_layers.1.g / .b [1, 1, 1, d_next]                      (levels with an Aggregate only)
+ *   mlp_head.0.g / .b [1, 1, 1, last_dim], mlp_head.2.kernel [last_dim, num_classes] / .bias
+ * A configuration whose last map does not have last_dim = dim * 2^(num_hierarchies - 1) channels (a block_repeats tuple more than
+ * one level short) is accepted, as the reference accepts it, and vb_forward refuses it. */
+VB_API int vb_create_nest(const vb_config* base, const vb_nest_config* nest, int device, vb_handle** out);
+
 /* Replaces Keras variable assignment: one call per weight, names/shapes/layouts per SURVEY.md App. B
  * (Dense kernel [in,out], float32).  shape/ndim are checked against the config. */
 VB_API int vb_set_weight(vb_handle* h, const char* name, const float* host_data, const int64_t* shape, int32_t ndim);
@@ -244,7 +285,7 @@ VB_API int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, i
 
 /* ---- the stages of <Model>.call on their own (SURVEY.md 8f f1/f4): the attribute surface the reference's wrappers and the
  * injected-transformer shell use.  ViT / DeepViT / parallel ViT / CaiT / patch-merger ViT / T2TViT; not CrossViT, CCT, LeViT,
- * CvT, Twins-SVT or CrossFormer. */
+ * CvT, Twins-SVT, CrossFormer or NesT. */
 
 /* Number of token rows vb_forward_embed produces for an img_h x img_w image (patches + cls where the model has one);
  * negative on error. */
@@ -327,6 +368,10 @@ VB_API int32_t vb_last_attention_path(void);
  * CrossFormer: the cross-scale embeddings' unfold is 3 and their convolution 0; the LayerNorm-folded q|k|v (or v alone for
  * one-token windows) 0; short and long attention 1 (off the flash kernel the row permutations are 4); the LayerNorm-folded GELU
  * fc1 5; the residual to_out / fc2 6; the average pool 2 (the fp32 engine adds its separate LayerNorms to 2).
+ * NesT: the patch embedding's and the aggregations' unfold is 3 and their convolutions 0; the LayerNorm-folded q|k|v 0; block
+ * attention 1 (off the flash kernel the row permutations are 4); the LayerNorm-folded GELU fc1 5; the residual to_out / fc2 6;
+ * the level-0 position add and the aggregation tails (LayerNorm, max-pool, position add) 4; the head's LayerNorm and mean 2 (the
+ * fp32 engine adds its separate LayerNorms to 2).
  * vb_profile_read synchronises the device and returns accumulated milliseconds, algorithmic FLOPs, algorithmic
  * bytes and launch counts per class (arrays of VB_PROF_NUM); reset != 0 clears the accumulators. */
 #define VB_PROF_NUM 7
@@ -440,6 +485,23 @@ VB_API int vb_op_window_attention(int32_t precision, const float* qkv, int32_t l
 VB_API int vb_op_window_bias_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t H, int32_t W, int32_t wsz,
                                        int32_t is_long, int32_t heads, int32_t dh, const float* table, float* out, int32_t ldo,
                                        int32_t iters, float* elapsed_ms);
+
+/* NesT's block attention (nest.py:93-109) as the engine runs it: vb_op_window_attention's layout with contiguous bh x bw blocks
+ * (H a multiple of bh, W of bw; token r * bw + c of a block), each attending within itself.  Scale dh^-0.5.  bf16 with dh 32 or
+ * 64 runs the windowed flash kernel in place; every fp32 call and any other dh permute the rows to block-major order, run the
+ * materialised-scores path and permute back (vb_last_attention_path tells which). */
+VB_API int vb_op_block_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t H, int32_t W, int32_t bh,
+                                 int32_t bw, int32_t heads, int32_t dh, float* out, int32_t ldo, int32_t iters, float* elapsed_ms);
+
+/* NesT's aggregation tail (nest.py:111-123 after the convolution, then :140-142 of the next level) as the engine runs it:
+ * x [B, H, W, C] NHWC -> y = LayerNorm(x) over C (eps 1e-5, gamma / beta [C]) -> MaxPool2D(3, 2, 'SAME') -> + pos[(r % bh) * bw
+ * + c % bw] on every channel of output pixel (r, c) (pos may be NULL: no add) -> out [B, ceil(H/2), ceil(W/2), C].  bf16
+ * (precision 1): x in bf16 with C zero-padded to a multiple of 64, the LayerNorm applied on load from the rows' (sum, sumsq)
+ * statistics, and stats_out (may be NULL) receives the output rows' [Cp/64][rows] (sum, sumsq) float pairs; fp32: a separate
+ * LayerNorm, then the pool (stats_out unused).  All buffers are host memory. */
+VB_API int vb_op_nest_aggregate(int32_t precision, const float* x, int32_t B, int32_t H, int32_t W, int32_t C, const float* gamma,
+                                const float* beta, const float* pos, int32_t bh, int32_t bw, float* out, float* stats_out,
+                                int32_t iters, float* elapsed_ms);
 
 /* Row softmax of fp32 scores into bf16 probabilities (the T2T attention): p[r, j] = softmax_j(s[r, j] * scale) for j < n,
  * p[r, n..npad) = 0.  s [rows, lds], p [rows, ldp] (uploaded and downloaded whole); n <= npad <= ldp. */

@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "libvitb200.so")   # VB_LIB_PATH: developer A/B builds
 
 KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6, "cct": 7, "levit": 8,
-        "cvt": 9, "twins_svt": 10, "crossformer": 11}
+        "cvt": 9, "twins_svt": 10, "crossformer": 11, "nest": 12}
 PRECISION = {"fp32": 0, "float32": 0, "bf16": 1, "bfloat16": 1}
 MEM_HOST, MEM_DEVICE = 0, 1
 ABI_VERSION = 7                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
@@ -67,6 +67,14 @@ class VbCrossformerConfig(C.Structure):
         ("kernels", (C.c_int32 * CROSSFORMER_MAX_KERNELS) * CROSSFORMER_STAGES)]
 
 
+NEST_MAX_LEVELS = 8                                  # VB_NEST_MAX_LEVELS
+
+
+class VbNestConfig(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("struct_size", "patch_size", "dim", "heads", "num_hierarchies", "levels")] + [
+        ("block_repeats", C.c_int32 * NEST_MAX_LEVELS), ("mlp_mult", C.c_int32), ("seq_len", C.c_int32)]
+
+
 class VbError(RuntimeError):
     pass
 
@@ -82,6 +90,7 @@ SIGNATURES = {
     "vb_create_cvt": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbCvtConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_twins_svt": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbTwinsSvtConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_crossformer": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbCrossformerConfig), C.c_int, C.POINTER(C.c_void_p)]),
+    "vb_create_nest": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbNestConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, _i64p, C.c_int32]),
     "vb_num_weights": (C.c_int, [C.c_void_p]),
     "vb_weight_info": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), _i64p, C.POINTER(C.c_int32)]),
@@ -121,6 +130,9 @@ SIGNATURES = {
     "vb_op_window_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 7 + [C.c_void_p, C.c_int32, C.c_int32, _f32p]),
     "vb_op_window_bias_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 8 + [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                                                                            _f32p]),
+    "vb_op_block_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 8 + [C.c_void_p, C.c_int32, C.c_int32, _f32p]),
+    "vb_op_nest_aggregate": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 3 + [C.c_int32] * 2 +
+                             [C.c_void_p, C.c_void_p, C.c_int32, _f32p]),
     "vb_op_softmax_rows": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 4 + [C.c_float, C.c_int32, _f32p]),
 }
 
@@ -306,6 +318,36 @@ def op_window_bias_attention(qkv, H, W, wsz, is_long, heads, dh, table, precisio
     check(load().vb_op_window_bias_attention(PRECISION[precision], _ptr(qkv), ld, B, H, W, wsz, int(bool(is_long)), heads, dh, _ptr(table),
                                              _ptr(out), heads * dh, iters, C.byref(ms)))
     return out, (ms.value if iters > 0 else None)
+
+
+def op_block_attention(qkv, H, W, bh, bw, heads, dh, precision="bf16", iters=0):
+    """NesT's block attention (vb_op_block_attention): qkv [B*H*W, ld] fused q|k|v rows of a pixel-major map, attention within
+    each bh x bw block.  Returns (out [B*H*W, heads*dh] pixel-major, ms or None)."""
+    qkv = _f32(qkv)
+    rows, ld = qkv.shape
+    B = rows // (H * W)
+    out = np.zeros((rows, heads * dh), np.float32)
+    ms = C.c_float(0)
+    check(load().vb_op_block_attention(PRECISION[precision], _ptr(qkv), ld, B, H, W, bh, bw, heads, dh, _ptr(out), heads * dh, iters,
+                                       C.byref(ms)))
+    return out, (ms.value if iters > 0 else None)
+
+
+def op_nest_aggregate(x, gamma, beta, pos=None, bh=1, bw=1, precision="bf16", iters=0):
+    """NesT's aggregation tail (vb_op_nest_aggregate): x [B, H, W, C] -> LayerNorm (eps 1e-5) -> MaxPool2D(3, 2, SAME) -> + pos
+    [bh * bw] per in-block position.  Returns (out [B, ceil(H/2), ceil(W/2), C], stats [ceil(C/64), rows, 2] of the bf16 rows
+    (None in fp32), ms or None)."""
+    x, gamma, beta = map(_f32, (x, gamma, beta))
+    B, H, W, Cc = x.shape
+    Ho, Wo = -(-H // 2), -(-W // 2)
+    out = np.empty((B, Ho, Wo, Cc), np.float32)
+    bf = PRECISION[precision] == PRECISION["bf16"]
+    stats = np.zeros((-(-Cc // 64), B * Ho * Wo, 2), np.float32) if bf else None
+    pos = _f32(pos)
+    ms = C.c_float(0)
+    check(load().vb_op_nest_aggregate(PRECISION[precision], _ptr(x), B, H, W, Cc, _ptr(gamma), _ptr(beta), _ptr(pos), bh, bw, _ptr(out),
+                                      _ptr(stats) if stats is not None else None, iters, C.byref(ms)))
+    return out, stats, (ms.value if iters > 0 else None)
 
 
 def op_softmax_rows(s, n, npad, scale, p, iters=0):

@@ -1,4 +1,4 @@
-// Tensor-core multi-head attention for the bf16 engine (bf16 operands, fp32 accumulation, dim_head = 64; 32 in the windowed-bias form).
+// Tensor-core multi-head attention for the bf16 engine (bf16 operands, fp32 accumulation, dim_head = 64; 32 in the windowed-bias and block forms).
 //
 //   out[b, i, h, :] = softmax_j( scale * q[b,i,h,:] . k[b,j,h,:] ) @ v[b,j,h,:]        (vit.py:77-82)
 //
@@ -24,6 +24,10 @@
 // score plus the window table of PosBias::wsz (one (2p-1)^2 table for all heads, in log2 units in shared memory).  Windows of up
 // to 32 tokens share a 64-row query tile floor(64 / p^2) at a time, a block-diagonal mask keeping each to its own keys: the
 // 4-token windows of CrossFormer's stage-3 long attention then fill 16 times fewer CTAs.
+//
+// WIN alone at head width 32 (NesT's block attention, nest.py:93-109; attention_block below): the same windowed form over
+// rectangular bh x bw blocks (Window::pw), reached only through attention_block.  NesT's 14 x 14 blocks of 196 tokens take four
+// query tiles and four key blocks each.
 #include "attention.cuh"
 #include "kernels.cuh"
 #include "ptx.cuh"
@@ -531,6 +535,36 @@ bool attention_window_bias(const __nv_bfloat16* q, int ldq, const __nv_bfloat16*
 }
 
 }  // namespace
+
+bool attention_block(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* out, int ldo, int heads, int dh, cudaStream_t s, float scale,
+                     const Window& win) {
+  const int n = win.p * win.width();
+  const long long B = static_cast<long long>(win.count);
+  if ((dh != 32 && dh != 64) || win.dilated || n <= 0 || B <= 0) return false;
+  if ((ld % 8) || (ldo % 2) || ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(out)) % 16)) return false;
+  const long long blocks = B * heads * ((n + FQ - 1) / FQ);
+  if (blocks > 0x7fffffffLL) return false;
+  const int HD = heads * dh;
+  const float scale_log2 = (scale > 0.f ? scale : 1.0f / sqrtf(static_cast<float>(dh))) * 1.4426950408889634f;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(static_cast<unsigned>(blocks));
+  cfg.blockDim = dim3(128);
+  cfg.stream = s;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  if (dh == 32)
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<32, false, true>, qkv, ld, qkv + HD, ld, qkv + 2 * HD, ld, out, ldo, heads, n, n,
+                               scale_log2, static_cast<const float*>(nullptr), 0, 1, 0, win));
+  else
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<64, false, true>, qkv, ld, qkv + HD, ld, qkv + 2 * HD, ld, out, ldo, heads, n, n,
+                               scale_log2, static_cast<const float*>(nullptr), 0, 1, 0, win));
+  count_launch();
+  note_attention_path(ATTN_PATH_FLASH);
+  return true;
+}
 
 template <>
 bool attention_fast<__nv_bfloat16>(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, int ldk, const __nv_bfloat16* v, int ldv,

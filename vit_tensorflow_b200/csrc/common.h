@@ -85,24 +85,30 @@ __device__ __forceinline__ int pos_bias_index(int i, int j, int fmap, int step, 
 }
 __device__ __forceinline__ float gelu_exact(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
-// Windowed attention on a pixel-major [B, H, W] map: each window of p x p tokens attends within itself.  The flat batch index of
-// the attention is (image, window row, window column) over nx x ny windows (W = nx * p, H = ny * p), and token i < p^2 of window
-// bw = (b, wy, wx), at (r, c) = (i / p, i % p) in the window, is the map's row (b * H + y) * W + x with
+// Windowed attention on a pixel-major [B, H, W] map: each window of p x q tokens (p rows, q = width() columns) attends within
+// itself.  The flat batch index of the attention is (image, window row, window column) over nx x ny windows (W = nx * q,
+// H = ny * p), and token i < p q of window bw = (b, wy, wx), at (r, c) = (i / q, i % q) in the window, is the map's row
+// (b * H + y) * W + x with
 //   y = wy * oy + r * sy,  x = wx * ox + c * sx,
-//   contiguous blocks (dilated == 0; Twins-SVT twins_svt.py:141, CrossFormer's short attention crossformer.py:144):
-//     oy = ox = p, sy = sx = 1;
-//   dilated windows (dilated != 0; CrossFormer's long attention, crossformer.py:146 'b (l1 h) (l2 w) d -> (b h w) l1 l2 d'):
+//   contiguous blocks (dilated == 0; Twins-SVT twins_svt.py:141, CrossFormer's short attention crossformer.py:144, NesT's
+//   rectangular blocks nest.py:209):
+//     oy = p, ox = q, sy = sx = 1;
+//   dilated windows (dilated != 0, square only; CrossFormer's long attention, crossformer.py:146 'b (l1 h) (l2 w) d -> (b h w) l1
+//   l2 d'):
 //     oy = ox = 1, sy = ny, sx = nx.
-// nq == nk == p^2.
+// nq == nk == p q.  pw == 0 means a square window (q = p): every caller but NesT's block attention.
 struct Window {
   int p = 0, nx = 0, ny = 0;
   int dilated = 0;
   int count = 0;                          // windows in the batch: the windowed-bias flash kernel packs several into one query tile
+  int pw = 0;                             // the window's width q when it differs from p (NesT's rectangular blocks)
+  __host__ __device__ int width() const { return pw > 0 ? pw : p; }
   __host__ __device__ long long row(long long bw, int i) const {
+    const int q = width();
     const long long per = static_cast<long long>(nx) * ny, b = bw / per;
-    const int w = static_cast<int>(bw - b * per), wy = w / nx, wx = w - wy * nx, r = i / p, c = i - r * p;
-    const int oy = dilated ? 1 : p, sy = dilated ? ny : 1, ox = dilated ? 1 : p, sx = dilated ? nx : 1;
-    return (b * ny * p + wy * oy + r * sy) * (static_cast<long long>(nx) * p) + wx * ox + c * sx;
+    const int w = static_cast<int>(bw - b * per), wy = w / nx, wx = w - wy * nx, r = i / q, c = i - r * q;
+    const int oy = dilated ? 1 : p, sy = dilated ? ny : 1, ox = dilated ? 1 : q, sx = dilated ? nx : 1;
+    return (b * ny * p + wy * oy + r * sy) * (static_cast<long long>(nx) * q) + wx * ox + c * sx;
   }
 };
 

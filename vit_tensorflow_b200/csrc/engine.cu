@@ -210,6 +210,28 @@ struct CrossformerStageW {           // crossformer.py:248-255: CrossEmbedLayer,
   std::vector<CrossformerLayerW> layers;
 };
 
+// One NesT level (nest.py:125-148 and its Aggregate :111-123) on channel rows zero-padded to dp (bf16) / dim (fp32): x +=
+// pos_emb[:h w], then `depth` blocks of x = to_out(attention(LN(x))) + x and x = MLP(LN(x)) + x within bs x bs blocks per map,
+// then (aggregate) Conv2D(3, SAME) to dim_out, LayerNorm, MaxPool2D(3, 2, SAME).  The bf16 engine folds the PreNorm LayerNorms
+// into q|k|v and fc1.  Heads of width dh = dim / heads of the model; inner = heads * dh may be below dim.
+struct NestBlockW { Norm attn_norm; Linear qkv, to_out; MlpW ff; };
+struct NestLevelW {
+  int dim = 0, dp = 0, heads = 0, dh = 0, inner = 0, bs = 1;   // bs: blocks per map side (nest.py:208)
+  const float* pos = nullptr;        // pos_emb [seq_len]
+  std::vector<NestBlockW> blocks;
+  bool aggregate = false;
+  int dim_out = 0, dp_out = 0;
+  Linear agg;                        // the 3 x 3 convolution as a Dense over unfold_same's (row, column, channel) vectors
+  Norm agg_norm;                     // ag_layers.1, [dp_out]
+};
+
+// NesT's block attention on the windowed flash kernel (attn_flash.cu): bf16 only, false for a shape it does not take.
+inline bool block_attention_fast(const float*, int, float*, int, int, int, cudaStream_t, const Window&) { return false; }
+inline bool block_attention_fast(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* out, int ldo, int heads, int dh, cudaStream_t s,
+                                 const Window& win) {
+  return attention_block(qkv, ld, out, ldo, heads, dh, s, 0.f, win);
+}
+
 struct EmbedW { Linear patch; const float* pos = nullptr; const float* cls = nullptr; int dim = 0, n_pos = 0; };
 struct CrossW { bool proj = false; Linear project_in, project_out, to_q, to_kv, to_out; Norm norm; };
 
@@ -430,6 +452,19 @@ struct vb_handle {
     for (int i = 1; i < n; ++i) { v.push_back(d >> i); sum += d >> i; }
     v.push_back(d - sum);
     return v;
+  }
+  // NesT (nest.py:150-216): the patch embedding (`nest_patch`), the levels, the head LayerNorm (`head_norm`) and Dense (`head`)
+  vb_nest_config ns{};
+  Linear nest_patch;
+  std::vector<NestLevelW> nest_levels;
+  static std::string nest_pre(int i) { return "nest_layers." + std::to_string(i) + "."; }
+  int nest_dim(int i) const { return ns.dim << i; }                  // nest.py:169-172: level i has dim * 2^i channels, heads * 2^i heads
+  int nest_last_dim() const { return nest_dim(ns.num_hierarchies - 1); }
+  bool nest_aggregates(int i) const { return i != ns.num_hierarchies - 1; }   // is_last (nest.py:188): hierarchies[i] == 0
+  // channels of the map the head sees: the last level's output (its Aggregate's when it has one), or the patch embedding's
+  int nest_final_dim() const {
+    if (ns.levels == 0) return ns.dim;
+    return nest_aggregates(ns.levels - 1) ? nest_dim(ns.levels) : nest_dim(ns.levels - 1);
   }
   struct XBlock { std::vector<LayerW> sm_layers, lg_layers; Norm sm_final, lg_final; std::vector<CrossW> sm_attend_lg, lg_attend_sm; };
   std::vector<XBlock> xblocks;
@@ -686,6 +721,36 @@ struct vb_handle {
         }
       }
       expect_dense("to_logits.1", cf.dim[VB_CROSSFORMER_STAGES - 1], c.num_classes);   // :258-261
+    } else if (c.kind == VB_KIND_NEST) {
+      auto expect_ln4 = [&](const std::string& n, int d) { expect(n + ".g", {1, 1, 1, d}); expect(n + ".b", {1, 1, 1, d}); };   // :33-34
+      const int dh = ns.dim / ns.heads;
+      expect("patch_embedding.1.kernel", {1, 1, ns.patch_size * ns.patch_size * c.channels, ns.dim});   // :178-181
+      expect("patch_embedding.1.bias", {ns.dim});
+      for (int i = 0; i < ns.levels; ++i) {
+        const std::string p = nest_pre(i);
+        const int d = nest_dim(i), inner = dh * (ns.heads << i), hidden = d * ns.mlp_mult;
+        expect(p + "0.pos_emb", {ns.seq_len});                           // Transformer :129
+        for (int L = 0; L < ns.block_repeats[i]; ++L) {
+          const std::string b = p + "0.layers." + std::to_string(L) + ".";
+          expect_ln4(b + "0.norm", d);                                   // PreNorm(Attention) :133, :77-91
+          expect(b + "0.fn.to_qkv.kernel", {1, 1, d, 3 * inner});
+          expect(b + "0.fn.to_out.0.kernel", {1, 1, inner, d});
+          expect(b + "0.fn.to_out.0.bias", {d});
+          expect_ln4(b + "1.norm", d);                                   // PreNorm(MLP) :134, :61-72
+          expect(b + "1.fn.net.0.kernel", {1, 1, d, hidden});
+          expect(b + "1.fn.net.0.bias", {hidden});
+          expect(b + "1.fn.net.3.kernel", {1, 1, hidden, d});
+          expect(b + "1.fn.net.3.bias", {d});
+        }
+        if (nest_aggregates(i)) {                                        // Aggregate :111-119
+          const int dn = nest_dim(i + 1);
+          expect(p + "1.ag_layers.0.kernel", {3, 3, d, dn});
+          expect(p + "1.ag_layers.0.bias", {dn});
+          expect_ln4(p + "1.ag_layers.1", dn);
+        }
+      }
+      expect_ln4("mlp_head.0", nest_last_dim());                        // :196-200
+      expect_dense("mlp_head.2", nest_last_dim(), c.num_classes);
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       expect("pos_embedding", {1, np, c.dim});
@@ -910,7 +975,7 @@ struct vb_handle {
     for (auto& w : weights) VB_CHECK(w.set, "vb_finalize: weight '" + w.name + "' was never set");
     VB_CUDA(cudaSetDevice(device));
     owned.clear(); layers.clear(); cls_layers.clear(); t2t_layers.clear(); xblocks.clear(); plans.clear(); embed_res.clear(); cct_convs.clear();
-    lv_stem.clear(); lv_blocks.clear(); cvt_stages.clear(); twins_stages.clear(); cf_stages.clear();
+    lv_stem.clear(); lv_blocks.clear(); cvt_stages.clear(); twins_stages.clear(); cf_stages.clear(); nest_levels.clear();
     woverride.clear();
     drop_graphs();
     const vb_config& c = cfg;
@@ -967,6 +1032,8 @@ struct vb_handle {
       finalize_twins();
     } else if (c.kind == VB_KIND_CROSSFORMER) {
       finalize_crossformer();
+    } else if (c.kind == VB_KIND_NEST) {
+      finalize_nest();
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       embed = make_embed("", c.patch_h, c.patch_w, c.dim, np, false);
@@ -1097,11 +1164,12 @@ struct vb_handle {
     head = make_linear_f32("cvt_layers.3.1", cv.emb_dim[VB_CVT_STAGES - 1], cfg.num_classes);
   }
   // ---- Twins-SVT weight packing: channel widths zero-padded (bf16), the patch kernel's rows permuted, the PEG residual folded
-  // A PreNorm MLP of width 4 d: the LayerNorm `norm` (g / b), the Dense layers n0 (d -> 4 d) and n3 (4 d -> d) as 1x1 Conv2D
-  // kernels, widths padded, the LayerNorm folded into fc1 in the bf16 engine.  key: the packed copies' own names.
-  MlpW prenorm_mlp(const std::string& key, const std::string& norm, const std::string& n0, const std::string& n3, int d, int dp) {
+  // A PreNorm MLP of width mult * d: the LayerNorm `norm` (g / b), the Dense layers n0 (d -> mult d) and n3 (mult d -> d) as 1x1
+  // Conv2D kernels, widths padded, the LayerNorm folded into fc1 in the bf16 engine.  key: the packed copies' own names.
+  MlpW prenorm_mlp(const std::string& key, const std::string& norm, const std::string& n0, const std::string& n3, int d, int dp,
+                   int mult = 4) {
     MlpW w;
-    const int hidden = 4 * d, hp = channel_width(hidden);
+    const int hidden = mult * d, hp = channel_width(hidden);
     w.norm = padded_norm(norm, d, dp);
     w.fc1 = linear_from_host(key + n0, pad_kn(host_weight(n0 + ".kernel"), d, hidden, dp, hp), pad_n(host_weight(n0 + ".bias"), hp), dp,
                              hp, bf16() ? &w.norm : nullptr);
@@ -1265,6 +1333,47 @@ struct vb_handle {
       cf_stages.push_back(std::move(S));
     }
     head = make_linear_f32("to_logits.1", cf.dim[VB_CROSSFORMER_STAGES - 1], cfg.num_classes);
+  }
+  // ---- NesT weight packing: channel widths zero-padded (bf16), the to_out rows padded to the q|k|v pitch the attention leaves
+  void finalize_nest() {
+    const int K0 = ns.patch_size * ns.patch_size * cfg.channels, dp0 = channel_width(ns.dim), dh = ns.dim / ns.heads;
+    // 'b (h p1) (w p2) c -> b h w (p1 p2 c)' (nest.py:179) is unfold_same's (p1, p2, c) order: the kernel's rows as they are
+    nest_patch = linear_from_host("nest.patch", pad_kn(host_weight("patch_embedding.1.kernel"), K0, ns.dim, K0, dp0),
+                                  pad_n(host_weight("patch_embedding.1.bias"), dp0), K0, dp0);
+    for (int i = 0; i < ns.levels; ++i) {
+      NestLevelW V;
+      const std::string p = nest_pre(i);
+      const int d = nest_dim(i), dp = channel_width(d);
+      V.dim = d; V.dp = dp; V.heads = ns.heads << i; V.dh = dh; V.inner = dh * V.heads; V.bs = 1 << (ns.levels - 1 - i);
+      V.pos = W(p + "0.pos_emb");
+      const int I = V.inner, N = bf16() ? round_up(3 * I, 64) : 3 * I, Ko = bf16() ? round_up(I, 64) : I;
+      for (int L = 0; L < ns.block_repeats[i]; ++L) {
+        const std::string b = p + "0.layers." + std::to_string(L) + ".", key = "nest." + b;
+        NestBlockW w;
+        w.attn_norm = padded_norm(b + "0.norm", d, dp);
+        w.qkv = linear_from_host(key + "qkv", pad_kn(host_weight(b + "0.fn.to_qkv.kernel"), d, 3 * I, dp, N), {}, dp, N,
+                                 bf16() ? &w.attn_norm : nullptr);
+        w.qkv.ln_d = d;
+        w.qkv.ln_eps = 1e-5f;                                        // nest.py:29
+        // to_out reads the attention output in place of q: K rows [I, Ko) meet k / v columns and are zero
+        w.to_out = linear_from_host(key + "to_out", pad_kn(host_weight(b + "0.fn.to_out.0.kernel"), I, d, Ko, dp),
+                                    pad_n(host_weight(b + "0.fn.to_out.0.bias"), dp), Ko, dp);
+        w.ff = prenorm_mlp("nest.", b + "1.norm", b + "1.fn.net.0", b + "1.fn.net.3", d, dp, ns.mlp_mult);
+        V.blocks.push_back(std::move(w));
+      }
+      V.aggregate = nest_aggregates(i);
+      if (V.aggregate) {
+        const int dn = nest_dim(i + 1), dpn = channel_width(dn);
+        V.dim_out = dn; V.dp_out = dpn;
+        // [3, 3, d, dn] is the Dense [9 d, dn] over unfold_same's (row, column, channel) vectors of the true d channels
+        V.agg = linear_from_host("nest." + p + "1.conv", pad_kn(host_weight(p + "1.ag_layers.0.kernel"), 9 * d, dn, 9 * d, dpn),
+                                 pad_n(host_weight(p + "1.ag_layers.0.bias"), dpn), 9 * d, dpn);
+        V.agg_norm = padded_norm(p + "1.ag_layers.1", dn, dpn);
+      }
+      nest_levels.push_back(std::move(V));
+    }
+    head_norm = padded_norm("mlp_head.0", nest_last_dim(), channel_width(nest_last_dim()));
+    head = make_linear_f32("mlp_head.2", nest_last_dim(), cfg.num_classes);
   }
   void finalize_levit() {
     const int dh = levit_dh();
@@ -1822,6 +1931,8 @@ struct vb_handle {
       twins_forward<T>(img, B, H, Wd, logits, s);
     } else if (c.kind == VB_KIND_CROSSFORMER) {
       crossformer_forward<T>(img, B, H, Wd, logits, s);
+    } else if (c.kind == VB_KIND_NEST) {
+      nest_forward<T>(img, B, H, Wd, logits, s);
     } else if (c.kind == VB_KIND_CCT) {                   // CCT.call cct.py:342-345, TransformerClassifier.call :277-305
       int rows = 0;
       T* X = tokenize_cct<T>(img, B, H, Wd, &rows, s);
@@ -2285,6 +2396,170 @@ struct vb_handle {
     mlp(l.ff2);
   }
 
+  // NesT.call (nest.py:202-216): the patch embedding, then per level the position add, the Transformer within blocks and the
+  // Aggregate; then the head's LayerNorm per pixel, the mean over the map and the Dense.  Token rows are the NHWC map, pixel-major,
+  // channel widths zero-padded to channel_width; no level permutes its map (the block attention reads and writes the map's own
+  // rows).  The position scalar is added by the kernel that last wrote the rows: a small pass after the patch embedding at level
+  // 0, the aggregation tail of the level below otherwise.  bf16: `stats` holds the (sum, sumsq) partials of X's rows between
+  // sub-blocks (emitted by those kernels and the residual GEMMs' epilogues).
+  static constexpr const char* kNestNoStages =
+      "NesT runs as a whole forward only: its patch-embedding / level / head steps have no entry of their own";
+  // The reference's shape rules (nest.py:179,140-142,209 through einops, and the head LayerNorm's broadcast), checked before
+  // anything runs.
+  void nest_check_size(int H, int Wd) const {
+    const int p = ns.patch_size;
+    VB_CHECK(H % p == 0 && Wd % p == 0, "NesT: the " + std::to_string(H) + " x " + std::to_string(Wd) +
+                                          " image is not divisible by patch_size " + std::to_string(p));
+    int h = H / p, w = Wd / p;
+    for (int i = 0; i < ns.levels; ++i) {
+      const int bs = 1 << (ns.levels - 1 - i);
+      const std::string where = "NesT level " + std::to_string(i) + ": the " + std::to_string(h) + " x " + std::to_string(w) + " map ";
+      VB_CHECK(h % bs == 0 && w % bs == 0, where + "is not divisible into " + std::to_string(bs) + " x " + std::to_string(bs) + " blocks");
+      VB_CHECK(static_cast<long long>(h / bs) * (w / bs) <= ns.seq_len,
+               where + "has blocks of " + std::to_string(h / bs) + " x " + std::to_string(w / bs) + " tokens, more than seq_len " +
+                   std::to_string(ns.seq_len) + " positions");
+      if (nest_aggregates(i)) { h = (h + 1) / 2; w = (w + 1) / 2; }
+    }
+    VB_CHECK(nest_final_dim() == nest_last_dim(),
+             "NesT: the last map has " + std::to_string(nest_final_dim()) + " channels but the head's LayerNorm has " +
+                 std::to_string(nest_last_dim()) + " (block_repeats has fewer than num_hierarchies - 1 entries)");
+  }
+  template <typename T>
+  void nest_forward(const float* img, int B, int H, int Wd, float* logits, cudaStream_t s) {
+    nest_check_size(H, Wd);
+    int mh = H / ns.patch_size, mw = Wd / ns.patch_size, d = ns.dim, dp = channel_width(ns.dim);
+    const int M0 = B * mh * mw, Kp = bf16() ? nest_patch.ldw : nest_patch.K;
+    T* col = arena.get<T>(static_cast<size_t>(M0) * Kp);
+    {
+      ProfScope ps(this, PROF_EMBED, 0.0, 4.0 * B * H * Wd * cfg.channels + static_cast<double>(sizeof(T)) * M0 * Kp, s);
+      unfold_same<float, T>(img, col, B, H, Wd, cfg.channels, ns.patch_size, ns.patch_size, 0, Kp, s);
+    }
+    T* X = arena.get<T>(static_cast<size_t>(M0) * dp);
+    float* stats = bf16() ? arena.get<float>(static_cast<size_t>(M0) * (dp / 64) * 2) : nullptr;
+    {
+      Linear L = nest_patch;
+      L.K = Kp;
+      Epi e; e.bias = nest_patch.bias;
+      linear<T>(col, Kp, M0, L, X, dp, e, s);
+    }
+    for (size_t i = 0; i < nest_levels.size(); ++i) {
+      const NestLevelW& V = nest_levels[i];
+      const int M = B * mh * mw;
+      if (i == 0) {                                                   // x + pos_emb (nest.py:140-142), in place, and the row statistics
+        ProfScope ps(this, PROF_OTHER, 1.0 * M * V.dim, 2.0 * sizeof(T) * M * dp, s);
+        nest_pool<T>(X, dp, nullptr, B, mh, mw, V.dim, false, V.pos, mh / V.bs, mw / V.bs, X, dp, stats, s);
+      }
+      for (const NestBlockW& b : V.blocks) nest_block<T>(X, B, mh, mw, V, b, stats, s);
+      if (!V.aggregate) continue;
+      // Aggregate (nest.py:111-123): the 3 x 3 SAME convolution as unfold_same + GEMM with the conv rows' statistics, then one pass
+      // for the LayerNorm, the max-pool and the next level's position add
+      const int Kc = bf16() ? V.agg.ldw : V.agg.K;
+      T* ccol = arena.get<T>(static_cast<size_t>(M) * Kc);
+      {
+        ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(sizeof(T)) * M * (dp + Kc), s);
+        unfold_same<T, T>(X, ccol, B, mh, mw, V.dim, 3, 1, 0, Kc, s, dp);
+      }
+      T* Y = arena.get<T>(static_cast<size_t>(M) * V.dp_out);
+      float* ystats = bf16() ? arena.get<float>(static_cast<size_t>(M) * (V.dp_out / 64) * 2) : nullptr;
+      {
+        Linear L = V.agg;
+        L.K = Kc;
+        Epi e; e.bias = V.agg.bias; e.stats_out = ystats;
+        linear<T>(ccol, Kc, M, L, Y, V.dp_out, e, s);
+      }
+      const NestLevelW* next = i + 1 < nest_levels.size() ? &nest_levels[i + 1] : nullptr;
+      const int oh = (mh + 1) / 2, ow = (mw + 1) / 2, Mo = B * oh * ow;
+      T* Xn = arena.get<T>(static_cast<size_t>(Mo) * V.dp_out);
+      float* nstats = bf16() ? arena.get<float>(static_cast<size_t>(Mo) * (V.dp_out / 64) * 2) : nullptr;
+      const T* src = Y;
+      NestPoolLn ln;
+      if (bf16()) {
+        ln.stats = ystats; ln.parts = V.dp_out / 64; ln.d = V.dim_out; ln.eps = 1e-5f; ln.gamma = V.agg_norm.gamma; ln.beta = V.agg_norm.beta;
+      } else {
+        T* Z = arena.get<T>(static_cast<size_t>(M) * V.dp_out);
+        ProfScope ps(this, PROF_LN, 8.0 * M * V.dim_out, 2.0 * sizeof(T) * M * V.dp_out, s);
+        layernorm<T>(Y, V.dp_out, V.agg_norm.gamma, V.agg_norm.beta, Z, V.dp_out, M, V.dim_out, s, V.dp_out, 1e-5f);
+        src = Z;
+      }
+      {
+        ProfScope ps(this, PROF_OTHER, 9.0 * Mo * V.dim_out, static_cast<double>(sizeof(T)) * (static_cast<double>(M) + Mo) * V.dp_out, s);
+        nest_pool<T>(src, V.dp_out, bf16() ? &ln : nullptr, B, mh, mw, V.dim_out, true, next ? next->pos : nullptr, next ? oh / next->bs : 1,
+                     next ? ow / next->bs : 1, Xn, V.dp_out, nstats, s);
+      }
+      X = Xn; stats = nstats; mh = oh; mw = ow; d = V.dim_out; dp = V.dp_out;
+    }
+    if (!nest_levels.empty() && !nest_levels.back().aggregate) { d = nest_levels.back().dim; dp = nest_levels.back().dp; }
+    // mlp_head (nest.py:196-200): LayerNorm(last_dim) per pixel, the mean over the map, Dense
+    const int M = B * mh * mw;
+    T* Y = arena.get<T>(static_cast<size_t>(M) * dp);
+    float* z = arena.get<float>(static_cast<size_t>(B) * d);
+    {
+      ProfScope ps(this, PROF_LN, 9.0 * M * d, static_cast<double>(sizeof(T)) * 3.0 * M * dp, s);
+      layernorm<T>(X, dp, head_norm.gamma, head_norm.beta, Y, dp, M, d, s, dp, 1e-5f);
+      pool_layernorm<T>(Y, mh * mw, dp, nullptr, nullptr, z, B, d, 1, s);
+    }
+    gemm_simt<float, float, float>(z, d, head.W, head.N, 1, logits, head.N, B, head.N, d, head.bias, nullptr, nullptr, head.N, 0, s);
+  }
+  // One Transformer block (nest.py:144-146) in place on X [B*H*W, dp]: attention within the level's bs x bs blocks per map, then
+  // the MLP.  bf16: the LayerNorms folded into q|k|v and fc1 (from `stats`); fp32: separate LayerNorms.
+  template <typename T>
+  void nest_block(T* X, int B, int H, int Wd, const NestLevelW& V, const NestBlockW& l, float* stats, cudaStream_t s) {
+    const int dp = V.dp, d = V.dim, M = B * H * Wd;
+    T* Y = bf16() ? nullptr : arena.get<T>(static_cast<size_t>(M) * dp);
+    auto prenorm = [&](const Norm& n) -> const T* {
+      if (Y == nullptr) return X;
+      ProfScope ps(this, PROF_LN, 8.0 * M * d, 2.0 * sizeof(T) * M * dp, s);
+      layernorm<T>(X, dp, n.gamma, n.beta, Y, dp, M, d, s, dp, 1e-5f);
+      return Y;
+    };
+    auto folded = [&](const Linear& L) {
+      Epi e;
+      if (Y == nullptr) { e.bias = L.ln_c2; e.ln_stats = stats; } else { e.bias = L.bias; }
+      return e;
+    };
+    auto residual = [&](const T* A, int lda, const Linear& L) {     // X = A W + b + X, and X's new row statistics
+      Epi e; e.bias = L.bias; e.res = X; e.ldr = dp; e.stats_out = stats;
+      linear<T>(A, lda, M, L, X, dp, e, s);
+    };
+    const T* a = prenorm(l.attn_norm);                                // Attention nest.py:93-109
+    const int ld = l.qkv.N;
+    T* QKV = arena.get<T>(static_cast<size_t>(M) * ld);
+    linear<T>(a, dp, M, l.qkv, QKV, ld, folded(l.qkv), s);
+    Window win;
+    win.p = H / V.bs; win.pw = Wd / V.bs; win.nx = V.bs; win.ny = V.bs; win.count = B * V.bs * V.bs;
+    block_attention<T>(QKV, ld, QKV, ld, V.heads, V.dh, win, s);      // the output overwrites q
+    residual(QKV, ld, l.to_out);
+    const T* f = prenorm(l.ff.norm);                                  // MLP nest.py:61-75
+    T* Hb = arena.get<T>(static_cast<size_t>(M) * l.ff.fc1.N);
+    Epi e1 = folded(l.ff.fc1);
+    e1.gelu = true;
+    linear<T>(f, dp, M, l.ff.fc1, Hb, l.ff.fc1.N, e1, s);
+    residual(Hb, l.ff.fc1.N, l.ff.fc2);
+  }
+  // NesT's block attention: win.count blocks of p x width() tokens of fused q|k|v rows [.., ld], the output rows written to out
+  // [.., ldo] pixel-major.  The windowed flash kernel where it serves (bf16, dh 32 or 64); otherwise the rows permuted to
+  // block-major order, the materialised-scores path, and the output rows permuted back.
+  template <typename T>
+  void block_attention(const T* qkv, int ld, T* out, int ldo, int heads, int dh, const Window& win, cudaStream_t s) {
+    const int n = win.p * win.width(), HD = heads * dh;
+    const long long B = win.count, rows = B * n;
+    const double fl = 4.0 * B * heads * n * n * dh, by = static_cast<double>(sizeof(T)) * B * heads * dh * 4.0 * n;
+    {
+      ProfScope ps(this, PROF_ATTN, fl, by, s);
+      if (block_attention_fast(qkv, ld, out, ldo, heads, dh, s, win)) return;
+    }
+    T* qkvw = arena.get<T>(static_cast<size_t>(rows) * 3 * HD);
+    T* ow = arena.get<T>(static_cast<size_t>(rows) * HD);
+    { ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * rows * 3 * HD, s); window_rows<T>(qkv, ld, qkvw, 3 * HD, 3 * HD, win, rows, true, s); }
+    {
+      ProfScope ps(this, PROF_ATTN, fl, by, s);
+      float* S = arena.get<float>(static_cast<size_t>(B) * heads * n * ((n + 15) & ~15));
+      attention_generic<T>(qkvw, 3 * HD, qkvw + HD, 3 * HD, qkvw + 2 * HD, 3 * HD, ow, HD, S, static_cast<int>(B), n, n, heads, dh, 0, nullptr,
+                           nullptr, nullptr, nullptr, s);
+    }
+    { ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * rows * HD, s); window_rows<T>(ow, HD, out, ldo, HD, win, rows, false, s); }
+  }
+
   // DistillMixin.call (distill.py:16-45) on top of a ViT: embed -> append the distillation token as the LAST row ->
   // transformer over n + 2 rows -> head on the first n + 1 rows, and the last row returned as is.
   template <typename T>
@@ -2342,6 +2617,7 @@ struct vb_handle {
     VB_CHECK(cfg.kind != VB_KIND_CVT, kCvtNoStages);
     VB_CHECK(cfg.kind != VB_KIND_TWINS_SVT, kTwinsNoStages);
     VB_CHECK(cfg.kind != VB_KIND_CROSSFORMER, kCrossformerNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_NEST, kNestNoStages);
     if (cfg.kind == VB_KIND_T2T_VIT) {
       int h = H, w = Wd;
       for (const auto& st : t2t_stages()) { h = (h + st.stride - 1) / st.stride; w = (w + st.stride - 1) / st.stride; }
@@ -2371,6 +2647,7 @@ struct vb_handle {
     VB_CHECK(cfg.kind != VB_KIND_CVT, kCvtNoStages);
     VB_CHECK(cfg.kind != VB_KIND_TWINS_SVT, kTwinsNoStages);
     VB_CHECK(cfg.kind != VB_KIND_CROSSFORMER, kCrossformerNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_NEST, kNestNoStages);
     arena.reset();
     const long long count = static_cast<long long>(B) * n * cfg.dim;
     T* X = arena.get<T>(count);
@@ -2386,6 +2663,7 @@ struct vb_handle {
     VB_CHECK(cfg.kind != VB_KIND_CVT, kCvtNoStages);
     VB_CHECK(cfg.kind != VB_KIND_TWINS_SVT, kTwinsNoStages);
     VB_CHECK(cfg.kind != VB_KIND_CROSSFORMER, kCrossformerNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_NEST, kNestNoStages);
     arena.reset();
     const int K = embed.patch.K, Kp = bf16() ? embed.patch.ldw : K;
     T* col = arena.get<T>(static_cast<size_t>(rows) * Kp);
@@ -2585,6 +2863,7 @@ void validate(const vb_config& c) {
   VB_CHECK(c.kind != VB_KIND_CVT, "CvT: create the handle with vb_create_cvt (its stages are a vb_cvt_config)");
   VB_CHECK(c.kind != VB_KIND_TWINS_SVT, "Twins-SVT: create the handle with vb_create_twins_svt (its stages are a vb_twins_svt_config)");
   VB_CHECK(c.kind != VB_KIND_CROSSFORMER, "CrossFormer: create the handle with vb_create_crossformer (its stages are a vb_crossformer_config)");
+  VB_CHECK(c.kind != VB_KIND_NEST, "NesT: create the handle with vb_create_nest (its levels are a vb_nest_config)");
   VB_CHECK(c.kind >= VB_KIND_VIT && c.kind <= VB_KIND_CCT, "unknown model kind");
   if (c.kind == VB_KIND_CCT) {
     VB_CHECK(c.channels == 3 && c.num_classes > 0 && c.image_h > 0 && c.image_w > 0, "bad image / class configuration");
@@ -2661,6 +2940,19 @@ void validate_twins(const vb_config& c, const vb_twins_svt_config& tw) {
     VB_CHECK(tw.emb_dim[st] > 0 && tw.patch_size[st] > 0 && tw.local_patch_size[st] > 0 && tw.global_k[st] > 0 && tw.depth[st] >= 0,
              "Twins-SVT: bad stage configuration");
   VB_CHECK(tw.peg_kernel_size >= 1 && tw.peg_kernel_size <= 7, "Twins-SVT: peg_kernel_size must be in [1, 7] (the depthwise kernel's halo tile)");
+}
+
+void validate_nest(const vb_config& c, const vb_nest_config& n) {
+  VB_CHECK(c.precision == VB_PRECISION_FP32 || c.precision == VB_PRECISION_BF16, "unknown precision");
+  VB_CHECK(c.channels > 0 && c.num_classes > 0, "NesT: bad channel / class configuration");
+  VB_CHECK(n.num_hierarchies >= 1 && n.num_hierarchies <= VB_NEST_MAX_LEVELS,
+           "NesT: num_hierarchies " + std::to_string(n.num_hierarchies) + " is not supported (1 to VB_NEST_MAX_LEVELS = " +
+               std::to_string(VB_NEST_MAX_LEVELS) + ")");
+  VB_CHECK(n.levels >= 0 && n.levels <= n.num_hierarchies, "NesT: levels must be in [0, num_hierarchies] (the zip with block_repeats)");
+  VB_CHECK(n.patch_size > 0 && n.heads > 0 && n.dim >= n.heads && n.mlp_mult > 0 && n.seq_len > 0,
+           "NesT: bad patch_size / dim / heads / mlp_mult / seq_len");
+  VB_CHECK((static_cast<long long>(n.dim) << (n.num_hierarchies - 1)) <= 65536, "NesT: dim * 2^(num_hierarchies - 1) is too large");
+  for (int i = 0; i < n.levels; ++i) VB_CHECK(n.block_repeats[i] >= 0, "NesT: block_repeats must not be negative");
 }
 
 void validate_crossformer(const vb_config& c, const vb_crossformer_config& cf) {
@@ -2923,6 +3215,35 @@ int vb_create_crossformer(const vb_config* base, const vb_crossformer_config* cf
   });
 }
 
+int vb_create_nest(const vb_config* base, const vb_nest_config* nc, int device, vb_handle** out) {
+  return guarded(nullptr, [&] {
+    VB_CHECK(base != nullptr && nc != nullptr && out != nullptr, "vb_create_nest: null argument");
+    VB_CHECK(base->struct_size == static_cast<int32_t>(sizeof(vb_config)) || base->struct_size == VB_CONFIG_SIZE_ABI7,
+             "vb_config.struct_size mismatch (ABI)");
+    VB_CHECK(nc->struct_size == static_cast<int32_t>(sizeof(vb_nest_config)), "vb_nest_config.struct_size mismatch (ABI)");
+    vb_config c;
+    memset(&c, 0, sizeof c);
+    memcpy(&c, base, static_cast<size_t>(base->struct_size));
+    VB_CHECK(c.kind == VB_KIND_NEST, "vb_create_nest: base.kind must be VB_KIND_NEST");
+    validate_nest(c, *nc);
+    int ndev = 0;
+    cudaError_t e = cudaGetDeviceCount(&ndev);
+    VB_CHECK(e == cudaSuccess && ndev > 0, "vb_create_nest: no CUDA device available -- libvitb200 has no CPU fallback");
+    VB_CHECK(device >= 0 && device < ndev, "vb_create_nest: bad device index");
+    VB_CUDA(cudaSetDevice(device));
+    cudaDeviceProp prop;
+    VB_CUDA(cudaGetDeviceProperties(&prop, device));
+    VB_CHECK(prop.major == 9 && prop.minor == 0, "vb_create_nest: libvitb200 is built for sm_90a (Hopper H100) only");
+    std::unique_ptr<vb_handle> h(new vb_handle());
+    h->cfg = c;
+    h->ns = *nc;
+    h->cfg.dim = h->nest_last_dim();
+    h->device = device;
+    h->build_expected();
+    *out = h.release();
+  });
+}
+
 int vb_num_weights(vb_handle* h) { return h ? static_cast<int>(h->weights.size()) : -1; }
 
 int vb_weight_info(vb_handle* h, int32_t index, const char** name, int64_t* shape4, int32_t* ndim) {
@@ -3049,6 +3370,7 @@ int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, int32_t 
     VB_CHECK(h->cfg.kind != VB_KIND_CVT, "vb_forward_distill: CvT has no distillation head");
     VB_CHECK(h->cfg.kind != VB_KIND_TWINS_SVT, "vb_forward_distill: Twins-SVT has no distillation head");
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSFORMER, "vb_forward_distill: CrossFormer has no distillation head");
+    VB_CHECK(h->cfg.kind != VB_KIND_NEST, "vb_forward_distill: NesT has no distillation head");
     const bool levit = h->cfg.kind == VB_KIND_LEVIT;
     VB_CHECK(levit || distill_token != nullptr, "vb_forward_distill: null argument");
     VB_CHECK(!levit || (distill_token == nullptr && h->lv.num_distill_classes > 0),
@@ -3107,6 +3429,7 @@ int vb_forward_tokens(vb_handle* h, const float* tokens, int32_t tokens_mem, int
     VB_CHECK(h->cfg.kind != VB_KIND_CVT, vb_handle::kCvtNoStages);
     VB_CHECK(h->cfg.kind != VB_KIND_TWINS_SVT, vb_handle::kTwinsNoStages);
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSFORMER, vb_handle::kCrossformerNoStages);
+    VB_CHECK(h->cfg.kind != VB_KIND_NEST, vb_handle::kNestNoStages);
     VB_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const long long before = launch_counter();
@@ -3177,7 +3500,7 @@ int vb_to_patch(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, 
     VB_CHECK(h != nullptr && img != nullptr && patches != nullptr, "vb_to_patch: null argument");
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT && h->cfg.kind != VB_KIND_T2T_VIT && h->cfg.kind != VB_KIND_CCT &&
              h->cfg.kind != VB_KIND_LEVIT && h->cfg.kind != VB_KIND_CVT && h->cfg.kind != VB_KIND_TWINS_SVT &&
-             h->cfg.kind != VB_KIND_CROSSFORMER,
+             h->cfg.kind != VB_KIND_CROSSFORMER && h->cfg.kind != VB_KIND_NEST,
              "vb_to_patch: the model has no single Rearrange patch layer");
     VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_to_patch: bad batch / image size");
     const vb_config& c = h->cfg;
@@ -3202,6 +3525,7 @@ int vb_patch_to_emb(vb_handle* h, const float* patches, int32_t patches_mem, int
     VB_CHECK(h->cfg.kind != VB_KIND_CVT, vb_handle::kCvtNoStages);
     VB_CHECK(h->cfg.kind != VB_KIND_TWINS_SVT, vb_handle::kTwinsNoStages);
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSFORMER, vb_handle::kCrossformerNoStages);
+    VB_CHECK(h->cfg.kind != VB_KIND_NEST, vb_handle::kNestNoStages);
     VB_CHECK(rows > 0, "vb_patch_to_emb: bad shape");
     const size_t in_bytes = static_cast<size_t>(rows) * h->embed.patch.K * sizeof(float);
     const size_t out_bytes = static_cast<size_t>(rows) * h->cfg.dim * sizeof(float);
@@ -3717,6 +4041,95 @@ int vb_op_window_bias_attention(int32_t precision, const float* qkv, int32_t ld,
     };
     if (precision == VB_PRECISION_FP32) run(float());
     else run(__nv_bfloat16());
+  });
+}
+
+int vb_op_block_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t H, int32_t W, int32_t bh, int32_t bw,
+                          int32_t heads, int32_t dh, float* out, int32_t ldo, int32_t iters, float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    const int HD = heads * dh;
+    VB_CHECK(qkv && out && B > 0 && bh > 0 && bw > 0 && H > 0 && W > 0 && H % bh == 0 && W % bw == 0 && heads > 0 && dh > 0 && ld >= 3 * HD &&
+             ldo >= HD, "vb_op_block_attention: bad arguments");
+    Window win;
+    win.p = bh; win.pw = bw; win.nx = W / bw; win.ny = H / bh; win.count = B * win.nx * win.ny;
+    const int n = bh * bw, Bw = win.count;
+    const long long rows = static_cast<long long>(B) * H * W;
+    DevMem dX, dO, dW, dOw, dS;
+    auto run = [&](auto tag) {
+      using T = decltype(tag);
+      const T* x_d = upload<T>(dX, qkv, static_cast<size_t>(rows) * ld);
+      T* o_d = upload<T>(dO, out, static_cast<size_t>(rows) * ldo);
+      // vb_handle::block_attention without the handle's arena and profiler
+      timed(iters, elapsed_ms, [&] {
+        if (block_attention_fast(x_d, ld, o_d, ldo, heads, dh, 0, win)) return;
+        dW.ensure(static_cast<size_t>(rows) * 3 * HD * sizeof(T));
+        dOw.ensure(static_cast<size_t>(rows) * HD * sizeof(T));
+        dS.ensure(static_cast<size_t>(Bw) * heads * n * ((n + 15) & ~15) * sizeof(float));
+        T* w_d = static_cast<T*>(dW.p);
+        T* ow_d = static_cast<T*>(dOw.p);
+        window_rows<T>(x_d, ld, w_d, 3 * HD, 3 * HD, win, rows, true, 0);
+        attention_generic<T>(w_d, 3 * HD, w_d + HD, 3 * HD, w_d + 2 * HD, 3 * HD, ow_d, HD, static_cast<float*>(dS.p), Bw, n, n, heads, dh, 0,
+                             nullptr, nullptr, nullptr, nullptr, 0);
+        window_rows<T>(ow_d, HD, o_d, ldo, HD, win, rows, false, 0);
+      });
+      download<T>(o_d, out, static_cast<size_t>(rows) * ldo);
+    };
+    if (precision == VB_PRECISION_FP32) run(float());
+    else run(__nv_bfloat16());
+  });
+}
+
+int vb_op_nest_aggregate(int32_t precision, const float* x, int32_t B, int32_t H, int32_t W, int32_t C, const float* gamma, const float* beta,
+                         const float* pos, int32_t bh, int32_t bw, float* out, float* stats_out, int32_t iters, float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    VB_CHECK(x && gamma && beta && out && B > 0 && H > 0 && W > 0 && C > 0, "vb_op_nest_aggregate: bad arguments");
+    const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;
+    VB_CHECK(pos == nullptr || (bh > 0 && bw > 0 && Ho % bh == 0 && Wo % bw == 0), "vb_op_nest_aggregate: the pooled map is not whole blocks");
+    const bool bf = precision == VB_PRECISION_BF16;
+    const int Cp = bf ? round_up(C, 64) : C;
+    const size_t M = static_cast<size_t>(B) * H * W, Mo = static_cast<size_t>(B) * Ho * Wo;
+    std::vector<float> xp(M * Cp, 0.f), gp(Cp, 0.f), bp(Cp, 0.f), oh(Mo * Cp), sh(Mo * (Cp / 64 + 1) * 2, 0.f);
+    for (size_t r = 0; r < M; ++r) std::copy(x + r * C, x + (r + 1) * C, xp.begin() + r * Cp);
+    std::copy(gamma, gamma + C, gp.begin());
+    std::copy(beta, beta + C, bp.begin());
+    DevMem dX, dG, dB, dP, dO, dS, dSo, dY;
+    const float* g_d = upload<float>(dG, gp.data(), Cp);
+    const float* b_d = upload<float>(dB, bp.data(), Cp);
+    const float* p_d = pos ? upload<float>(dP, pos, static_cast<size_t>(bh) * bw) : nullptr;
+    auto run = [&](auto tag) {
+      using T = decltype(tag);
+      const T* x_d = upload<T>(dX, xp.data(), M * Cp);
+      dO.ensure(Mo * Cp * sizeof(T));
+      T* o_d = static_cast<T*>(dO.p);
+      // vb_handle::nest_forward's aggregation tail, without the handle's arena and profiler
+      if constexpr (std::is_same<T, __nv_bfloat16>::value) {
+        dS.ensure(M * (Cp / 64) * 2 * sizeof(float));
+        dSo.ensure(Mo * (Cp / 64) * 2 * sizeof(float));
+        float* st = static_cast<float*>(dS.p);
+        float* so = static_cast<float*>(dSo.p);
+        NestPoolLn ln;
+        ln.stats = st; ln.parts = Cp / 64; ln.d = C; ln.eps = 1e-5f; ln.gamma = g_d; ln.beta = b_d;
+        timed(iters, elapsed_ms, [&] {
+          row_stats_bf16(x_d, Cp, st, static_cast<int>(M), Cp, 0);
+          nest_pool<T>(x_d, Cp, &ln, B, H, W, C, true, p_d, bh, bw, o_d, Cp, so, 0);
+        });
+        VB_CUDA(cudaMemcpy(sh.data(), so, Mo * (Cp / 64) * 2 * sizeof(float), cudaMemcpyDeviceToHost));
+      } else {
+        dY.ensure(M * Cp * sizeof(T));
+        T* y = static_cast<T*>(dY.p);
+        timed(iters, elapsed_ms, [&] {
+          layernorm<T>(x_d, Cp, g_d, b_d, y, Cp, static_cast<int>(M), C, 0, Cp, 1e-5f);
+          nest_pool<T>(y, Cp, nullptr, B, H, W, C, true, p_d, bh, bw, o_d, Cp, nullptr, 0);
+        });
+      }
+      download<T>(o_d, oh.data(), Mo * Cp);
+    };
+    if (bf) run(__nv_bfloat16());
+    else run(float());
+    for (size_t r = 0; r < Mo; ++r) std::copy(oh.begin() + r * Cp, oh.begin() + r * Cp + C, out + r * C);
+    if (bf && stats_out != nullptr) std::copy(sh.begin(), sh.begin() + Mo * (Cp / 64) * 2, stats_out);
   });
 }
 

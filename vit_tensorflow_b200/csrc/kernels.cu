@@ -685,6 +685,70 @@ __global__ void window_rows_kernel(const T* __restrict__ in, int ldi, T* __restr
   for (int c = threadIdx.x; c < cols; c += blockDim.x) dst[c] = src[c];
 }
 
+// One warp per output pixel, lane l holding columns 64 j + 2 l and 64 j + 2 l + 1 of chunk j: each tap's LayerNorm (mean, rstd)
+// comes from that input pixel's statistics once per tap, and the chunk's (sum, sumsq) by a warp reduction of the stored values.
+// `in` may alias `out` when pool == 0 (every element is read and written by the same lane).
+constexpr int NEST_POOL_WARPS = 8;
+template <typename T>
+__global__ void __launch_bounds__(NEST_POOL_WARPS * 32, 4)
+nest_pool_kernel(const T* in, int ldi, const float2* __restrict__ stats, int parts, float inv_d, float eps,
+                 const float* __restrict__ gamma, const float* __restrict__ beta, int C, int H, int W, int pool, int oh, int ow,
+                 int pad_top, int pad_left, const float* __restrict__ pos, int bh, int bw, T* out, int ldo,
+                 float2* __restrict__ stats_out, long long pixels) {
+  const long long px = static_cast<long long>(blockIdx.x) * NEST_POOL_WARPS + (threadIdx.x >> 5);
+  if (px >= pixels) return;
+  const int lane = threadIdx.x & 31;
+  const long long b = px / (static_cast<long long>(oh) * ow);
+  const int t = static_cast<int>(px - b * oh * ow), oy = t / ow, ox = t - oy * ow;
+  const long long in_pixels = static_cast<long long>(pixels / (static_cast<long long>(oh) * ow)) * H * W;
+  const int k = pool ? 3 : 1, st = pool ? 2 : 1;
+  const int y0 = oy * st - pad_top, x0 = ox * st - pad_left;
+  const float p = pos != nullptr ? __ldg(pos + (oy % bh) * bw + (ox % bw)) : 0.f;
+  for (int c0 = 0; c0 < ldo; c0 += 64) {
+    const int c = c0 + 2 * lane;
+    float m0 = -INFINITY, m1 = -INFINITY;
+    for (int ky = 0; ky < k; ++ky) {
+      const int y = y0 + ky;
+      if (y < 0 || y >= H) continue;                               // TF SAME: padded taps never win
+      for (int kx = 0; kx < k; ++kx) {
+        const int x = x0 + kx;
+        if (x < 0 || x >= W) continue;
+        const long long ip = (b * H + y) * W + x;
+        const T* src = in + ip * ldi;
+        float v0 = c < C ? to_f(src[c]) : 0.f, v1 = c + 1 < C ? to_f(src[c + 1]) : 0.f;
+        if (stats != nullptr) {
+          float s1 = 0.f, s2 = 0.f;
+          for (int j = 0; j < parts; ++j) {
+            const float2 sv = __ldg(stats + j * in_pixels + ip);
+            s1 += sv.x;
+            s2 += sv.y;
+          }
+          const float mean = s1 * inv_d, rstd = rsqrtf(fmaxf(s2 * inv_d - mean * mean, 0.f) + eps);
+          if (c < C) v0 = (v0 - mean) * rstd * gamma[c] + beta[c];
+          if (c + 1 < C) v1 = (v1 - mean) * rstd * gamma[c + 1] + beta[c + 1];
+        }
+        m0 = fmaxf(m0, v0);
+        m1 = fmaxf(m1, v1);
+      }
+    }
+    // the position scalar goes to the true channels only; pad channels stay zero
+    const T o0 = from_f<T>(c < C ? m0 + p : 0.f), o1 = from_f<T>(c + 1 < C ? m1 + p : 0.f);
+    T* dst = out + px * ldo;
+    if (c < ldo) dst[c] = o0;
+    if (c + 1 < ldo) dst[c + 1] = o1;
+    if (stats_out != nullptr) {
+      const float f0 = to_f(o0), f1 = to_f(o1);
+      float s1 = f0 + f1, s2 = f0 * f0 + f1 * f1;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+        s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+      }
+      if (lane == 0) stats_out[(c0 / 64) * pixels + px] = make_float2(s1, s2);
+    }
+  }
+}
+
 // One thread per output element (b, t, c), c fastest: the k*k taps of a thread are C apart, so a warp reads whole channel runs.
 template <typename T>
 __global__ void maxpool_relu_same_kernel(const T* __restrict__ in, T* __restrict__ out, int H, int W, int C, int k, int stride, int oh,
@@ -1207,7 +1271,7 @@ void unfold_same(const TI* in, TO* out, int B, int H, int W, int C, int k, int s
 
 template <typename T>
 void window_rows(const T* in, int ldi, T* out, int ldo, int cols, const Window& win, long long rows, bool to_window, cudaStream_t s) {
-  const int n = win.p * win.p;
+  const int n = win.p * win.width();
   VB_CHECK(n > 0 && rows % n == 0 && rows < (1ll << 31), "window_rows: rows must be whole windows, fewer than 2^31");
   if (rows == 0) return;
   window_rows_kernel<T><<<static_cast<unsigned>(rows), cols >= 256 ? 256 : 128, 0, s>>>(in, ldi, out, ldo, cols, win, n, to_window);
@@ -1221,6 +1285,27 @@ void maxpool_relu_same(const T* in, T* out, int B, int H, int W, int C, int k, i
   const int ph = std::max((oh - 1) * stride + k - H, 0), pw = std::max((ow - 1) * stride + k - W, 0);
   const long long total = static_cast<long long>(B) * rows * C;
   maxpool_relu_same_kernel<T><<<grid_1d(total), 256, 0, s>>>(in, out, H, W, C, k, stride, oh, ow, ph / 2, pw / 2, pos, rows, total);
+  VB_LAUNCHED();
+}
+
+template <typename T>
+void nest_pool(const T* in, int ldi, const NestPoolLn* ln, int B, int H, int W, int C, bool pool, const float* pos, int bh, int bw,
+               T* out, int ldo, float* stats_out, cudaStream_t s) {
+  const int oh = pool ? (H + 1) / 2 : H, ow = pool ? (W + 1) / 2 : W;
+  const int ph = pool ? std::max((oh - 1) * 2 + 3 - H, 0) : 0, pw = pool ? std::max((ow - 1) * 2 + 3 - W, 0) : 0;
+  const long long pixels = static_cast<long long>(B) * oh * ow;
+  VB_CHECK(pixels > 0 && (pixels + NEST_POOL_WARPS - 1) / NEST_POOL_WARPS < (1ll << 31) && C <= ldo && C <= ldi,
+           "nest_pool: bad shape");
+  VB_CHECK(stats_out == nullptr || ldo % 64 == 0, "nest_pool: row statistics need a multiple of 64 columns");
+  VB_CHECK(pos == nullptr || (bh > 0 && bw > 0 && oh % bh == 0 && ow % bw == 0), "nest_pool: the map is not whole blocks");
+  VB_CHECK(ln == nullptr || (ln->stats != nullptr && ln->parts > 0 && ln->d > 0 && ln->gamma != nullptr && ln->beta != nullptr),
+           "nest_pool: LayerNorm statistics without their width / gamma / beta");
+  VB_CHECK(pool || ln == nullptr, "nest_pool: the LayerNorm on load is for the pooling form");
+  const unsigned grid = static_cast<unsigned>((pixels + NEST_POOL_WARPS - 1) / NEST_POOL_WARPS);
+  nest_pool_kernel<T><<<grid, NEST_POOL_WARPS * 32, 0, s>>>(
+      in, ldi, ln ? reinterpret_cast<const float2*>(ln->stats) : nullptr, ln ? ln->parts : 0, ln ? 1.0f / static_cast<float>(ln->d) : 0.f,
+      ln ? ln->eps : 0.f, ln ? ln->gamma : nullptr, ln ? ln->beta : nullptr, C, H, W, pool ? 1 : 0, oh, ow, ph / 2, pw / 2, pos, bh, bw,
+      out, ldo, reinterpret_cast<float2*>(stats_out), pixels);
   VB_LAUNCHED();
 }
 
@@ -1317,6 +1402,8 @@ void dwconv_qkv(const T* x, int ldx, const float* stats, const float* gamma, con
   template void window_rows<T>(const T*, int, T*, int, int, const Window&, long long, bool, cudaStream_t);                   \
   template void convert_rows<float, T>(const float*, int, T*, int, long long, int, cudaStream_t);                           \
   template void maxpool_relu_same<T>(const T*, T*, int, int, int, int, int, int, const float*, int, cudaStream_t);         \
+  template void nest_pool<T>(const T*, int, const NestPoolLn*, int, int, int, int, bool, const float*, int, int, T*, int, float*,   \
+                             cudaStream_t);                                                                                  \
   template void seq_pool<T>(const T*, int, int, const float*, const float*, const float*, const float*, float*, int, cudaStream_t); \
   template void dwconv_qkv<T>(const T*, int, const float*, const float*, const float*, int, float, const float*, const float*, T*, int, \
                               const float*, const float*, T*, int, int, int, int, int, int, int, cudaStream_t);

@@ -118,6 +118,24 @@ void window_rows(const T* in, int ldi, T* out, int ldo, int cols, const Window& 
 template <typename T>
 void maxpool_relu_same(const T* in, T* out, int B, int H, int W, int C, int k, int stride, const float* pos, int rows, cudaStream_t s);
 
+// NesT's aggregation tail and position add (nest.py:111-123,140-142), NHWC rows: in [B*H*W, ldi] -> out [B*oh*ow, ldo].
+//   ln (may be null): LayerNorm each input pixel on load from its (sum, sumsq) partials [parts][B*H*W] (the GEMM epilogue's
+//     stats_out format) over d true channels with eps, times gamma plus beta; the fp32 engine passes null after its own LayerNorm.
+//   pool: MaxPool2D(3, 2, 'SAME'), oh = ceil(H / 2), total padding max((oh - 1) * 2 + 3 - H, 0) with the smaller half first, and
+//     padded taps never win; !pool: oh = H, each pixel as it is (in may equal out).
+//   pos (may be null): the next Transformer's scalar pos[(y % bh) * bw + x % bw] added to the C true channels of output pixel
+//     (y, x) of bh x bw blocks; columns [C, ldo) are written as zero.
+//   stats_out (may be null; ldo % 64 == 0): the stored rows' (sum, sumsq) partials [ldo/64][B*oh*ow].
+struct NestPoolLn {
+  const float* stats = nullptr;
+  int parts = 0, d = 0;
+  float eps = 1e-5f;
+  const float *gamma = nullptr, *beta = nullptr;
+};
+template <typename T>
+void nest_pool(const T* in, int ldi, const NestPoolLn* ln, int B, int H, int W, int C, bool pool, const float* pos, int bh, int bw,
+               T* out, int ldo, float* stats_out, cudaStream_t s);
+
 // CCT sequence pooling (cct.py:291-299): per image b, y_t = LayerNorm(X[b, t]) (eps 1e-3), w_t = softmax_t(y_t . pw + pb),
 // z[b] = sum_t w_t y_t.  X [B, n, D] -> z fp32 [B, D]; D <= 1024.  One CTA per image, fp32 statistics, online softmax.
 template <typename T>

@@ -8,6 +8,7 @@
     CvT       vit_tensorflow/cvt.py:149-202
     TwinsSVT  vit_tensorflow/twins_svt.py:215-268
     CrossFormer  vit_tensorflow/crossformer.py:205-269
+    NesT      vit_tensorflow/nest.py:150-216
 
 Same constructor kwargs, defaults and assertion messages; `model(img, training=True, **kwargs) -> logits`
 with `img` NHWC float32 `[b, H, W, 3]` and logits float32 `[b, num_classes]`.  Everything below the call is
@@ -1247,8 +1248,149 @@ CROSSFORMER_CTOR_KEYS = ("dim", "depth", "global_window_size", "local_window_siz
                          "num_classes", "attn_dropout", "ff_dropout")
 
 
+def nest_plan(image_size, patch_size, dim, heads, num_hierarchies, block_repeats):
+    """NesT.__init__'s construction (nest.py:163-194) as data: seq_len and the levels the zip of hierarchies, heads, dim pairs and
+    the cast_tuple'd block_repeats leaves (a longer tuple is truncated, a shorter one gives fewer levels, each keeping its
+    is_last / width / heads).  Raises what the reference raises for a bad block_repeats entry (range(depth), :131)."""
+    assert (image_size % patch_size) == 0, 'Image dimensions must be divisible by the patch size.'
+    if not 1 <= num_hierarchies <= _lib.NEST_MAX_LEVELS:
+        raise ValueError(f"NesT: num_hierarchies {num_hierarchies} is not supported (1 to {_lib.NEST_MAX_LEVELS})")
+    fmap_size = image_size // patch_size
+    seq_len = (fmap_size // 2 ** (num_hierarchies - 1)) ** 2
+    block_repeats = _cast_tuple(block_repeats, num_hierarchies)
+    levels = []
+    for i, depth in zip(range(num_hierarchies), block_repeats):
+        len(range(depth))                               # the reference's `for _ in range(depth)`: TypeError for a non-int
+        levels.append(dict(dim=dim * 2 ** i, heads=heads * 2 ** i, depth=int(depth), aggregate=i != num_hierarchies - 1))
+    return dict(patch_size=patch_size, dim=dim, heads=heads, num_hierarchies=num_hierarchies, seq_len=seq_len, levels=levels,
+                last_dim=dim * 2 ** (num_hierarchies - 1))
+
+
+def nest_size_error(plan, h, w):
+    """The reference's shape rules (nest.py:179,209,140-142 through einops, and the head LayerNorm's broadcast) for an h x w image:
+    None, or what the first level that breaks one says."""
+    p = plan["patch_size"]
+    if h % p or w % p:
+        return f"NesT: the {h} x {w} image is not divisible by patch_size {p}"
+    h, w = h // p, w // p
+    n = len(plan["levels"])
+    for i, lv in enumerate(plan["levels"]):
+        bs = 2 ** (n - 1 - i)
+        if h % bs or w % bs:
+            return f"NesT level {i}: the {h} x {w} map is not divisible into {bs} x {bs} blocks"
+        if (h // bs) * (w // bs) > plan["seq_len"]:
+            return (f"NesT level {i}: the {h} x {w} map has blocks of {h // bs} x {w // bs} tokens, more than seq_len "
+                    f"{plan['seq_len']} positions")
+        if lv["aggregate"]:
+            h, w = -(-h // 2), -(-w // 2)
+    final = plan["dim"] if n == 0 else plan["levels"][-1]["dim"] * (2 if plan["levels"][-1]["aggregate"] else 1)
+    if final != plan["last_dim"]:
+        return (f"NesT: the last map has {final} channels but the head's LayerNorm has {plan['last_dim']} (block_repeats has fewer "
+                "than num_hierarchies - 1 entries)")
+    return None
+
+
+class NesT(_EngineModel):
+    """nest.py:150-216: a patch embedding (patches with c fastest, 1x1 Conv2D), then per level i (bottom first, width dim * 2^i,
+    heads * 2^i heads of dim // heads) the map split into 2^level x 2^level contiguous blocks, a Transformer (+ pos_emb[:h w], one
+    scalar per in-block position on every channel; block_repeats[i] x [PreNorm attention within the block, PreNorm MLP], each
+    residual) and, below the top, an Aggregate (Conv2D(3, SAME), LayerNorm, MaxPool2D(3, 2, SAME)); then LayerNorm per pixel, the
+    mean over the map and Dense(num_classes).  Every LayerNorm is the module's own (eps 1e-5).
+
+    block_repeats is zipped with the hierarchies as in the reference: a longer tuple is truncated and a shorter one builds fewer
+    levels.  One handle runs any image whose sides are multiples of patch_size and whose maps are whole blocks of at most seq_len
+    tokens at every level; other sizes raise ValueError naming the level.  There is no BatchNormalization, so with dropout = 0
+    training=True computes what training=False does; with dropout > 0 only training=False runs.  Weights (SURVEY.md App. B) keep
+    the reference's attribute paths: patch_embedding.1, nest_layers.{i}.0.pos_emb, nest_layers.{i}.0.layers.{l}.{0|1}.norm,
+    ....0.fn.to_qkv / to_out.0, ....1.fn.net.{0|3}, nest_layers.{i}.1.ag_layers.{0|1}, mlp_head.0 (LayerNorm), mlp_head.2."""
+    _kind = "nest"
+
+    def __init__(self,
+                 image_size,
+                 patch_size,
+                 num_classes,
+                 dim,
+                 heads,
+                 num_hierarchies,
+                 block_repeats,
+                 mlp_mult=4,
+                 dropout=0.0,
+                 *, precision="bf16", device=0, seed=None):
+        self.plan = nest_plan(image_size, patch_size, dim, heads, num_hierarchies, block_repeats)
+        self.num_classes = num_classes
+        self._dropout_rates = (dropout,)
+        self.precision = precision
+        self.device = int(device)
+        cfg = _lib.VbConfig()
+        cfg.struct_size = C.sizeof(_lib.VbConfig)
+        cfg.kind = _lib.KIND["nest"]
+        if precision not in _lib.PRECISION:
+            raise ValueError(f"precision must be one of {sorted(_lib.PRECISION)}")
+        cfg.precision = _lib.PRECISION[precision]
+        cfg.channels, cfg.num_classes = 3, num_classes
+        cfg.dim = self.plan["last_dim"]
+        nc = _lib.VbNestConfig()
+        nc.struct_size = C.sizeof(_lib.VbNestConfig)
+        nc.patch_size, nc.dim, nc.heads, nc.num_hierarchies = patch_size, dim, heads, num_hierarchies
+        nc.levels = len(self.plan["levels"])
+        for i, lv in enumerate(self.plan["levels"]):
+            nc.block_repeats[i] = lv["depth"]
+        nc.mlp_mult, nc.seq_len = mlp_mult, self.plan["seq_len"]
+        self._cfg, self._nc = cfg, nc
+        self._lib = _lib.load()
+        h = C.c_void_p()
+        _lib.check(self._lib.vb_create_nest(C.byref(cfg), C.byref(nc), self.device, C.byref(h)))
+        self._h = h
+        self._finalized = False
+        self._specs = collections.OrderedDict()
+        name, shape, ndim = C.c_char_p(), (C.c_int64 * 4)(), C.c_int32()
+        for i in range(self._lib.vb_num_weights(h)):
+            _lib.check(self._lib.vb_weight_info(h, i, C.byref(name), shape, C.byref(ndim)), h)
+            self._specs[name.value.decode()] = tuple(int(shape[j]) for j in range(ndim.value))
+        self._weights = collections.OrderedDict()
+        self.init_weights(seed)
+
+    def init_weights(self, seed=None):
+        """The reference's initialisers: glorot-uniform over the receptive field for every Conv2D and Dense kernel, zero biases,
+        LayerNorm g 1 / b 0, pos_emb N(0, 1) (nest.py:129)."""
+        rng = np.random.default_rng(seed)
+        w = collections.OrderedDict()
+        for name, shape in self._specs.items():
+            leaf = name.rsplit(".", 1)[-1]
+            if leaf == "kernel":
+                receptive = int(np.prod(shape[:-2]))
+                lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
+                a = rng.uniform(-lim, lim, size=shape)
+            elif leaf in ("bias", "b"):
+                a = np.zeros(shape)
+            elif leaf == "g":
+                a = np.ones(shape)
+            elif leaf == "pos_emb":
+                a = rng.standard_normal(shape)
+            else:
+                raise AssertionError(name)
+            w[name] = a.astype(np.float32)
+        self.set_weights_dict(w)
+
+    def __call__(self, img, training=True, **kwargs):
+        """nest.py:202-216: NHWC float images -> logits [b, num_classes]; extra kwargs are accepted and ignored, as there."""
+        x = np.asarray(img)
+        if x.ndim == 4:
+            err = nest_size_error(self.plan, x.shape[1], x.shape[2])
+            if err is not None:
+                raise ValueError(err)
+        return super().__call__(img, training=training)
+
+    call = __call__
+
+
+NEST_CTOR_KEYS = ("image_size", "patch_size", "num_classes", "dim", "heads", "num_hierarchies", "block_repeats", "mlp_mult", "dropout")
+
+
 def from_config(cfg: dict, precision="bf16", device=0, seed=None):
     """Build a model from an oracle-style config dict (kind + reference kwargs)."""
+    if cfg["kind"] == "nest":
+        return NesT(**{k: v for k, v in cfg.items() if k in NEST_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "crossformer":
         return CrossFormer(**{k: v for k, v in cfg.items() if k in CROSSFORMER_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "twins_svt":
