@@ -15,6 +15,7 @@
  *     TwinsSVT(...)(img)             vit_tensorflow/twins_svt.py:215-268 (vb_create_twins_svt)
  *     CrossFormer(...)(img)          vit_tensorflow/crossformer.py:205-269 (vb_create_crossformer)
  *     NesT(...)(img)                 vit_tensorflow/nest.py:150-216 (vb_create_nest)
+ *     RegionViT(...)(img)            vit_tensorflow/regionvit.py:184-263 (vb_create_regionvit)
  * and this header is what the Python host classes (vit_tensorflow_b200/models.py, _lib.py) bind with ctypes.
  * Plain pointers and sizes only; no torch / C++ types cross the boundary.
  *
@@ -45,7 +46,7 @@ typedef struct vb_handle vb_handle;
 
 enum { VB_KIND_VIT = 0, VB_KIND_DEEPVIT = 1, VB_KIND_CAIT = 2, VB_KIND_CROSSVIT = 3, VB_KIND_PARALLEL_VIT = 4,
        VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6, VB_KIND_CCT = 7, VB_KIND_LEVIT = 8,
-       VB_KIND_CVT = 9, VB_KIND_TWINS_SVT = 10, VB_KIND_CROSSFORMER = 11, VB_KIND_NEST = 12 };
+       VB_KIND_CVT = 9, VB_KIND_TWINS_SVT = 10, VB_KIND_CROSSFORMER = 11, VB_KIND_NEST = 12, VB_KIND_REGIONVIT = 13 };
 enum { VB_CCT_POS_SINE = 0, VB_CCT_POS_LEARNABLE = 1, VB_CCT_POS_NONE = 2 };   /* cct.py:233-234,250-256 */
 enum { VB_PRECISION_FP32 = 0, VB_PRECISION_BF16 = 1 };
 enum { VB_POOL_CLS = 0, VB_POOL_MEAN = 1 };
@@ -90,8 +91,8 @@ typedef struct vb_config {
 VB_API int vb_abi_version(void);
 
 /* Replaces <Model>.__init__ (vit.py:107-157 etc.): validates the config and allocates device state.  VB_KIND_LEVIT, VB_KIND_CVT,
- * VB_KIND_TWINS_SVT, VB_KIND_CROSSFORMER and VB_KIND_NEST are refused here: their handles come from vb_create_levit,
- * vb_create_cvt, vb_create_twins_svt, vb_create_crossformer and vb_create_nest. */
+ * VB_KIND_TWINS_SVT, VB_KIND_CROSSFORMER, VB_KIND_NEST and VB_KIND_REGIONVIT are refused here: their handles come from
+ * vb_create_levit, vb_create_cvt, vb_create_twins_svt, vb_create_crossformer, vb_create_nest and vb_create_regionvit. */
 VB_API int vb_create(const vb_config* cfg, int device, vb_handle** out);
 
 /* LeViT (levit.py:164-212), appended within ABI 7.  `dims`, `depths` and `heads` hold `stages` entries each (cast_tuple already
@@ -243,6 +244,45 @@ typedef struct vb_nest_config {
  * one level short) is accepted, as the reference accepts it, and vb_forward refuses it. */
 VB_API int vb_create_nest(const vb_config* base, const vb_nest_config* nest, int device, vb_handle** out);
 
+/* RegionViT (regionvit.py:184-263), appended within ABI 7.  dims / depth are the cast_tuple'd 4-tuples (:197-200).  Local tokens:
+ * Conv2D(dims[0], 8, stride 4, SAME) of the image, or with tokenize_local_3_conv Conv3x3 s2 -> LayerNormalization -> GELU ->
+ * Conv3x3 s2 -> LayerNormalization -> GELU -> Conv3x3 s1 (:210-221).  Regional tokens: 'b (h p1) (w p2) c -> b h w (c p1 p2)',
+ * p = local_patch_size * window_size, then a 1x1 Conv2D (:223-226).  Stage s >= 1 applies ONE Downsample Conv2D(dims[s], 3,
+ * stride 2, SAME) to both maps (shared weights) and, with use_peg, a depthwise 3x3 PEG plus residual to the local map (:231-240,
+ * :257-260).  Then depth[s] R2L layers (:135-182; 4 heads of 32): r = Attention(r) + r over the image's regional tokens; then per
+ * lh/rh x lw/rw window [r; window] = Attention([r; window], bias) + [r; window], then MLP + residual, one Attention module used
+ * for both.  Attention (:79-116): LayerNormalization, bias-free to_qkv, softmax(q k^T / sqrt(32) + bias) v, to_out with bias;
+ * the bias is the window's relative-position Embedding((2 window_size - 1)^2, 4) row (dr + ws - 1) + (dc + ws - 1) (2 ws - 1),
+ * zero on the regional token's row and column.  MLP (:64-77): LayerNormalization, Dense(mlp_mult d), exact GELU, Dense(d).  Head
+ * (:243-247): the mean over the regional tokens, LayerNormalization, Dense(num_classes).  Every LayerNormalization is Keras's
+ * (eps 1e-3).  Any image runs whose sides are multiples of p and whose local map at every stage is a whole number of windows of
+ * at most window_size x window_size tokens per regional token. */
+#define VB_REGIONVIT_STAGES 4
+typedef struct vb_regionvit_config {
+  int32_t struct_size;            /* sizeof(vb_regionvit_config) */
+  int32_t dims[VB_REGIONVIT_STAGES], depth[VB_REGIONVIT_STAGES];
+  int32_t window_size, local_patch_size;
+  int32_t tokenize_local_3_conv, use_peg;   /* 0 / 1 */
+  int32_t mlp_mult;               /* 4 (regionvit.py:65) */
+} vb_regionvit_config;
+
+/* RegionViT.__init__: `base` supplies precision, channels, num_classes and max_batch; its kind must be VB_KIND_REGIONVIT and its
+ * other fields are ignored.  Weights (SURVEY.md App. B), for stage s, layer l, width d = dims[s], p = local_patch_size *
+ * window_size, t = (2 window_size - 1)^2:
+ *   local_encoder.kernel [8, 8, channels, dims[0]] / .bias, or with tokenize_local_3_conv local_encoder.{0,3,6}.kernel [3, 3,
+ *     channels | dims[0], dims[0]] / .bias and local_encoder.{1,4}.gamma / .beta [dims[0]]
+ *   region_encoder.1.kernel [1, 1, channels * p^2, dims[0]] / .bias   (rows in (c, p1, p2) order, c slowest)
+ *   region_layers.{s}.0.conv.kernel [3, 3, dims[s - 1], d] / .bias [d]               (s >= 1)
+ *   region_layers.{s}.1.proj.kernel [3, 3, 1, d] / .bias [d]                         (s >= 1 with use_peg)
+ *   region_layers.{s}.2.local_rel_pos_bias.embeddings [t, 4]
+ *   region_layers.{s}.2.layers.{l}.0.norm.gamma / .beta [d], ....0.to_qkv.kernel [d, 384], ....0.to_out.kernel [128, d] / .bias
+ *   region_layers.{s}.2.layers.{l}.1.net.0.gamma / .beta [d], ....1.net.1.kernel [d, mlp_mult d] / .bias, ....1.net.4.kernel
+ *     [mlp_mult d, d] / .bias
+ *   to_logits.1.gamma / .beta [dims[3]], to_logits.2.kernel [dims[3], num_classes] / .bias
+ * vb_finalize stores each stage's Embedding transposed to [4][(2 ws - 1)^2] with the row offset slowest, the index convention of
+ * the windowed attention kernels. */
+VB_API int vb_create_regionvit(const vb_config* base, const vb_regionvit_config* rv, int device, vb_handle** out);
+
 /* Replaces Keras variable assignment: one call per weight, names/shapes/layouts per SURVEY.md App. B
  * (Dense kernel [in,out], float32).  shape/ndim are checked against the config. */
 VB_API int vb_set_weight(vb_handle* h, const char* name, const float* host_data, const int64_t* shape, int32_t ndim);
@@ -285,7 +325,7 @@ VB_API int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, i
 
 /* ---- the stages of <Model>.call on their own (SURVEY.md 8f f1/f4): the attribute surface the reference's wrappers and the
  * injected-transformer shell use.  ViT / DeepViT / parallel ViT / CaiT / patch-merger ViT / T2TViT; not CrossViT, CCT, LeViT,
- * CvT, Twins-SVT, CrossFormer or NesT. */
+ * CvT, Twins-SVT, CrossFormer, NesT or RegionViT. */
 
 /* Number of token rows vb_forward_embed produces for an img_h x img_w image (patches + cls where the model has one);
  * negative on error. */
@@ -372,6 +412,9 @@ VB_API int32_t vb_last_attention_path(void);
  * attention 1 (off the flash kernel the row permutations are 4); the LayerNorm-folded GELU fc1 5; the residual to_out / fc2 6;
  * the level-0 position add and the aggregation tails (LayerNorm, max-pool, position add) 4; the head's LayerNorm and mean 2 (the
  * fp32 engine adds its separate LayerNorms to 2).
+ * RegionViT: the encoders' and the Downsample's unfold is 3 and their convolutions 0; the LayerNorm-folded q|k|v 0; the regional attention and the R2L attention 1 (off the flash kernel
+ * the row gathers are 4); the LayerNorm-folded GELU fc1 5; the residual to_out / fc2 6; row statistics, the head's LayerNorm
+ * and mean 2; the PEG 4 (the fp32 engine adds its separate LayerNorms to 2).
  * vb_profile_read synchronises the device and returns accumulated milliseconds, algorithmic FLOPs, algorithmic
  * bytes and launch counts per class (arrays of VB_PROF_NUM); reset != 0 clears the accumulators. */
 #define VB_PROF_NUM 7
@@ -492,6 +535,17 @@ VB_API int vb_op_window_bias_attention(int32_t precision, const float* qkv, int3
  * materialised-scores path and permute back (vb_last_attention_path tells which). */
 VB_API int vb_op_block_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t H, int32_t W, int32_t bh,
                                  int32_t bw, int32_t heads, int32_t dh, float* out, int32_t ldo, int32_t iters, float* elapsed_ms);
+
+/* RegionViT's regional-to-local attention (regionvit.py:143-177) as the engine runs it: qkv [B*lh*lw + B*rh*rw, ld] holds the
+ * fused q|k|v rows of the pixel-major local map followed by those of the pixel-major region map (lh = rh * wh, lw = rw * ww,
+ * wh and ww <= window_size).  Window (b, wy, wx) attends over its regional row (b * rh + wy) * rw + wx and its wh x ww local
+ * rows, scale dh^-0.5, with table[(dr + ws - 1) + (dc + ws - 1) (2 ws - 1), h] (the reference's Embedding layout [(2 ws - 1)^2,
+ * heads]) added to the local-local scores.  out [rows, ldo] receives every row's output in place.  bf16 with dh 32 runs the
+ * R2L flash kernel; fp32, any other dh and tables past the kernel's shared-memory table gather the windows, run the
+ * materialised-scores path and scatter back (vb_last_attention_path tells which). */
+VB_API int vb_op_r2l_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t lh, int32_t lw, int32_t rh,
+                               int32_t rw, int32_t heads, int32_t dh, const float* table, int32_t window_size, float* out,
+                               int32_t ldo, int32_t iters, float* elapsed_ms);
 
 /* NesT's aggregation tail (nest.py:111-123 after the convolution, then :140-142 of the next level) as the engine runs it:
  * x [B, H, W, C] NHWC -> y = LayerNorm(x) over C (eps 1e-5, gamma / beta [C]) -> MaxPool2D(3, 2, 'SAME') -> + pos[(r % bh) * bw

@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "libvitb200.so")   # VB_LIB_PATH: developer A/B builds
 
 KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6, "cct": 7, "levit": 8,
-        "cvt": 9, "twins_svt": 10, "crossformer": 11, "nest": 12}
+        "cvt": 9, "twins_svt": 10, "crossformer": 11, "nest": 12, "regionvit": 13}
 PRECISION = {"fp32": 0, "float32": 0, "bf16": 1, "bfloat16": 1}
 MEM_HOST, MEM_DEVICE = 0, 1
 ABI_VERSION = 7                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
@@ -75,6 +75,14 @@ class VbNestConfig(C.Structure):
         ("block_repeats", C.c_int32 * NEST_MAX_LEVELS), ("mlp_mult", C.c_int32), ("seq_len", C.c_int32)]
 
 
+REGIONVIT_STAGES = 4                                 # VB_REGIONVIT_STAGES
+
+
+class VbRegionvitConfig(C.Structure):
+    _fields_ = [("struct_size", C.c_int32), ("dims", C.c_int32 * REGIONVIT_STAGES), ("depth", C.c_int32 * REGIONVIT_STAGES)] + [
+        (n, C.c_int32) for n in ("window_size", "local_patch_size", "tokenize_local_3_conv", "use_peg", "mlp_mult")]
+
+
 class VbError(RuntimeError):
     pass
 
@@ -91,6 +99,7 @@ SIGNATURES = {
     "vb_create_twins_svt": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbTwinsSvtConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_crossformer": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbCrossformerConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_nest": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbNestConfig), C.c_int, C.POINTER(C.c_void_p)]),
+    "vb_create_regionvit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbRegionvitConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, _i64p, C.c_int32]),
     "vb_num_weights": (C.c_int, [C.c_void_p]),
     "vb_weight_info": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), _i64p, C.POINTER(C.c_int32)]),
@@ -133,6 +142,8 @@ SIGNATURES = {
     "vb_op_block_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 8 + [C.c_void_p, C.c_int32, C.c_int32, _f32p]),
     "vb_op_nest_aggregate": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 3 + [C.c_int32] * 2 +
                              [C.c_void_p, C.c_void_p, C.c_int32, _f32p]),
+    "vb_op_r2l_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 8 + [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32,
+                                                                                   _f32p]),
     "vb_op_softmax_rows": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 4 + [C.c_float, C.c_int32, _f32p]),
 }
 
@@ -348,6 +359,19 @@ def op_nest_aggregate(x, gamma, beta, pos=None, bh=1, bw=1, precision="bf16", it
     check(load().vb_op_nest_aggregate(PRECISION[precision], _ptr(x), B, H, W, Cc, _ptr(gamma), _ptr(beta), _ptr(pos), bh, bw, _ptr(out),
                                       _ptr(stats) if stats is not None else None, iters, C.byref(ms)))
     return out, stats, (ms.value if iters > 0 else None)
+
+
+def op_r2l_attention(qkv, B, lh, lw, rh, rw, heads, dh, table, window_size, precision="bf16", ldo=None, iters=0):
+    """RegionViT's regional-to-local attention (vb_op_r2l_attention): qkv [B*lh*lw + B*rh*rw, ld] fused q|k|v rows, the local map's
+    then the region map's, table [(2 ws - 1)^2, heads] (the reference's Embedding).  Returns (out [rows, ldo], ms or None)."""
+    qkv, table = _f32(qkv), _f32(table)
+    rows, ld = qkv.shape
+    ldo = heads * dh if ldo is None else ldo
+    out = np.zeros((rows, ldo), np.float32)
+    ms = C.c_float(0)
+    check(load().vb_op_r2l_attention(PRECISION[precision], _ptr(qkv), ld, B, lh, lw, rh, rw, heads, dh, _ptr(table), window_size, _ptr(out),
+                                     ldo, iters, C.byref(ms)))
+    return out, (ms.value if iters > 0 else None)
 
 
 def op_softmax_rows(s, n, npad, scale, p, iters=0):

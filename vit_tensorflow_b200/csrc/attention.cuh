@@ -41,6 +41,15 @@ bool attention_fast(const T* q, int ldq, const T* k, int ldk, const T* v, int ld
 bool attention_block(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* out, int ldo, int heads, int dh, cudaStream_t s, float scale,
                      const Window& win);
 
+// RegionViT's regional-to-local attention (regionvit.py:163-177) on its flash kernel: each of the win.count windows (contiguous
+// p x width() blocks of the local map, Window in common.h) attends together with its regional token, row reg_row0 + (window
+// index) of the same fused rows qkv [.., ld] (q, k, v at columns [0, HD), [HD, 2 HD), [2 HD, 3 HD), HD = heads * dh), with pb's
+// R2L window table (PosBias::r2l_ws) on the local-local scores.  Output rows (the regional one and the window's) go to the same
+// rows of out [.., ldo] (may be qkv itself).  dh 32, tables of up to FLASH_BIAS_MAX entries; false for any other shape, which the
+// caller then runs on the materialised-scores path over gathered windows.  bf16 only.
+bool attention_r2l(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* out, int ldo, int heads, int dh, long long reg_row0,
+                   const PosBias& pb, const Window& win, cudaStream_t s, float scale = 0.f);
+
 // The talking-heads / re-attention path keeps host copies of the head-mix weights keyed by their device pointers (one process-
 // wide cache for all handles); whoever frees or rewrites such weights (vb_finalize, vb_destroy, the op-level test entries) must
 // erase the entries that name any of those pointers -- and only those: another handle's entries must survive, because a miss

@@ -28,6 +28,9 @@
 // WIN alone at head width 32 (NesT's block attention, nest.py:93-109; attention_block below): the same windowed form over
 // rectangular bh x bw blocks (Window::pw), reached only through attention_block.  NesT's 14 x 14 blocks of 196 tokens take four
 // query tiles and four key blocks each.
+//
+// RegionViT's regional-to-local attention (attn_r2l_kernel, attention_r2l below) is a kernel of its own with the same tiles and
+// online softmax: each window attends together with one regional row from elsewhere in the rows, under a per-head window table.
 #include "attention.cuh"
 #include "kernels.cuh"
 #include "ptx.cuh"
@@ -534,7 +537,192 @@ bool attention_window_bias(const __nv_bfloat16* q, int ldq, const __nv_bfloat16*
   return true;
 }
 
+// ---- RegionViT's regional-to-local attention (regionvit.py:163-177; attention_r2l below), head width 32.  One CTA per (64 query
+// rows, window, head) as attn_flash_kernel, over the n = 1 + p q tokens of window bw = (b, wy, wx): token 0 is the regional row
+// reg_row0 + bw of the fused q|k|v rows ((b * rh + wy) * rw + wx: the region map's own pixel order), token t > 0 the window's
+// local row win.row(bw, t - 1).  Scores are moved to log2 units as computed, plus (i, j > 0) the head's table entry of the
+// window offset (PosBias::r2l_ws, common.h); row 0 and column 0 take no bias.  Output row 0 goes to the regional row, the others
+// to the local rows, so nothing is gathered, scattered or materialised.  n > 64 (14 x 14 windows: 197 tokens) takes several
+// query tiles and key blocks.
+__global__ void __launch_bounds__(128)
+attn_r2l_kernel(const __nv_bfloat16* __restrict__ qkv, int ld, __nv_bfloat16* __restrict__ out, int ldo, int heads, long long reg_row0,
+                float scale_log2, const float* __restrict__ table, int ws, Window win) {
+  constexpr int D = 32, FP = D + 8, VR = D / 8;
+  extern __shared__ float tab[];     // this head's (2 ws - 1)^2 table, times log2(e)
+  __shared__ __align__(16) __nv_bfloat16 Qs[FQ][FP];
+  __shared__ __align__(16) __nv_bfloat16 Ks[2][FK][FP];
+  __shared__ __align__(16) __nv_bfloat16 Vs[2][FK][FP];
+  const int ww = win.width(), n = 1 + win.p * ww, HD = heads * D, side = 2 * ws - 1;
+  const int qtiles = (n + FQ - 1) / FQ;
+  const long long wh = blockIdx.x / qtiles, bw = wh / heads;
+  const int h = static_cast<int>(wh - bw * heads);
+  const int i0 = (blockIdx.x % qtiles) * FQ;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nblk = (n + FK - 1) / FK;
+  auto row_of = [&](int t) -> size_t { return static_cast<size_t>(t == 0 ? reg_row0 + bw : win.row(bw, t - 1)); };
+
+  pdl_wait();                 // q|k|v come from the previous kernel of the stream
+  pdl_launch_dependents();
+
+  for (int e = threadIdx.x; e < FQ * VR; e += 128) {
+    const int r = e >> 2, c = (e & (VR - 1)) * 8;
+    if (i0 + r < n) cp_async16(smem_u32(&Qs[r][c]), qkv + row_of(i0 + r) * ld + h * D + c);
+    else *reinterpret_cast<uint4*>(&Qs[r][c]) = make_uint4(0, 0, 0, 0);
+  }
+  auto stage = [&](int j) {
+    if (j < nblk) {
+      const int s = j & 1, j0 = j * FK;
+      for (int e = threadIdx.x; e < FK * VR; e += 128) {
+        const int r = e >> 2, c = (e & (VR - 1)) * 8;
+        if (j0 + r < n) {
+          const __nv_bfloat16* src = qkv + row_of(j0 + r) * ld + h * D + c;
+          cp_async16(smem_u32(&Ks[s][r][c]), src + HD);
+          cp_async16(smem_u32(&Vs[s][r][c]), src + 2 * HD);
+        } else {                                                     // zero V rows: 0 * garbage could be NaN
+          *reinterpret_cast<uint4*>(&Ks[s][r][c]) = make_uint4(0, 0, 0, 0);
+          *reinterpret_cast<uint4*>(&Vs[s][r][c]) = make_uint4(0, 0, 0, 0);
+        }
+      }
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+  stage(0);
+  for (int e = threadIdx.x; e < side * side; e += 128) tab[e] = table[static_cast<size_t>(h) * side * side + e] * 1.4426950408889634f;
+  int qy[2], qx[2];                                                  // window position of the lane's two rows; qy = -1: the regional row
+  for (int r = 0; r < 2; ++r) {
+    const int t = min(i0 + warp * 16 + (lane >> 2) + 8 * r, n - 1);  // rows past n: any live row
+    qy[r] = t == 0 ? -1 : (t - 1) / ww;
+    qx[r] = t == 0 ? 0 : t - 1 - qy[r] * ww;
+  }
+
+  const int qr = lane >> 2, qc = 2 * (lane & 3);
+  uint32_t qf[D / 16][4];
+  float o[D / 8][4];
+#pragma unroll
+  for (int k = 0; k < D / 8; ++k) o[k][0] = o[k][1] = o[k][2] = o[k][3] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+
+  for (int j = 0; j < nblk; ++j) {
+    stage(j + 1);
+    asm volatile("cp.async.wait_group 1;" ::: "memory");
+    __syncthreads();
+    if (j == 0) {
+      const uint32_t qa = smem_u32(&Qs[warp * 16 + (lane & 15)][8 * (lane >> 4)]);
+#pragma unroll
+      for (int kk = 0; kk < D / 16; ++kk)
+        asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                     : "=r"(qf[kk][0]), "=r"(qf[kk][1]), "=r"(qf[kk][2]), "=r"(qf[kk][3]) : "r"(qa + kk * 32));
+    }
+    const int s = j & 1;
+    float sc[FK / 8][4];
+#pragma unroll
+    for (int g = 0; g < FK / 8; ++g) {
+      sc[g][0] = sc[g][1] = sc[g][2] = sc[g][3] = 0.f;
+#pragma unroll
+      for (int kk = 0; kk < D / 16; ++kk) {
+        const uint32_t b0 = *reinterpret_cast<const uint32_t*>(&Ks[s][g * 8 + qr][kk * 16 + qc]);
+        const uint32_t b1 = *reinterpret_cast<const uint32_t*>(&Ks[s][g * 8 + qr][kk * 16 + qc + 8]);
+        mma_bf16_16816(sc[g], qf[kk], b0, b1);
+      }
+    }
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int g = 0; g < FK / 8; ++g) {
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const int u = j * FK + g * 8 + qc + c;
+        const int ky = u > 0 ? (u - 1) / ww : -1, kx = u > 0 ? u - 1 - ky * ww : 0;
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          float& v = sc[g][2 * r + c];
+          if (u >= n) v = -INFINITY;
+          else v = v * scale_log2 + (qy[r] >= 0 && ky >= 0 ? tab[(qy[r] - ky + ws - 1) * side + qx[r] - kx + ws - 1] : 0.f);
+          mx[r] = fmaxf(mx[r], v);
+        }
+      }
+    }
+    float alpha[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      const float m_new = fmaxf(m_run[r], mx[r]);                    // every block holds at least one valid key: finite
+      alpha[r] = ex2_approx(m_run[r] - m_new);
+      m_run[r] = m_new;
+      l_run[r] *= alpha[r];
+    }
+#pragma unroll
+    for (int k = 0; k < D / 8; ++k) {
+      o[k][0] *= alpha[0]; o[k][1] *= alpha[0];
+      o[k][2] *= alpha[1]; o[k][3] *= alpha[1];
+    }
+    uint32_t pf[FK / 16][4];
+#pragma unroll
+    for (int g = 0; g < FK / 8; ++g) {
+      const float p0 = ex2_approx(sc[g][0] - m_run[0]), p1 = ex2_approx(sc[g][1] - m_run[0]);
+      const float p2 = ex2_approx(sc[g][2] - m_run[1]), p3 = ex2_approx(sc[g][3] - m_run[1]);
+      l_run[0] += p0 + p1;
+      l_run[1] += p2 + p3;
+      pf[g >> 1][(g & 1) * 2 + 0] = pack_bf16x2(p0, p1);
+      pf[g >> 1][(g & 1) * 2 + 1] = pack_bf16x2(p2, p3);
+    }
+    const uint32_t va = smem_u32(&Vs[s][lane & 15][0]);
+#pragma unroll
+    for (int kk = 0; kk < FK / 16; ++kk) {
+#pragma unroll
+      for (int k = 0; k < D / 8; ++k) {
+        uint32_t b0, b1;
+        asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0, %1}, [%2];"
+                     : "=r"(b0), "=r"(b1) : "r"(va + (kk * 16 * FP + k * 8) * 2));
+        mma_bf16_16816(o[k], pf[kk], b0, b1);
+      }
+    }
+    __syncthreads();
+  }
+
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
+    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
+    l_run[r] = 1.0f / l_run[r];
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = i0 + warp * 16 + qr + 8 * r;
+    if (row >= n) continue;
+    __nv_bfloat16* orow = out + row_of(row) * ldo + h * D + qc;
+#pragma unroll
+    for (int k = 0; k < D / 8; ++k)
+      *reinterpret_cast<uint32_t*>(orow + k * 8) = pack_bf16x2(o[k][2 * r] * l_run[r], o[k][2 * r + 1] * l_run[r]);
+  }
+}
+
 }  // namespace
+
+bool attention_r2l(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* out, int ldo, int heads, int dh, long long reg_row0,
+                   const PosBias& pb, const Window& win, cudaStream_t s, float scale) {
+  const int ws = pb.r2l_ws, side = 2 * ws - 1, n = 1 + win.p * win.width();
+  if (dh != 32 || ws <= 0 || side * side > FLASH_BIAS_MAX || win.dilated || win.count <= 0 || n <= 1) return false;
+  if (pb.r2l_h != win.p || pb.r2l_w != win.width() || win.p > ws || win.width() > ws) return false;
+  if ((ld % 8) || (ldo % 2) || ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(out)) % 16)) return false;
+  const long long blocks = static_cast<long long>(win.count) * heads * ((n + FQ - 1) / FQ);
+  if (blocks > 0x7fffffffLL) return false;
+  const float scale_log2 = (scale > 0.f ? scale : 1.0f / sqrtf(static_cast<float>(dh))) * 1.4426950408889634f;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(static_cast<unsigned>(blocks));
+  cfg.blockDim = dim3(128);
+  cfg.dynamicSmemBytes = static_cast<size_t>(side) * side * sizeof(float);   // with the 25.6 KB static tiles: under 48 KB
+  cfg.stream = s;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  VB_CUDA(cudaLaunchKernelEx(&cfg, attn_r2l_kernel, qkv, ld, out, ldo, heads, reg_row0, scale_log2, pb.table, ws, win));
+  count_launch();
+  note_attention_path(ATTN_PATH_FLASH);
+  return true;
+}
 
 bool attention_block(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* out, int ldo, int heads, int dh, cudaStream_t s, float scale,
                      const Window& win) {

@@ -68,13 +68,24 @@ inline unsigned flat_blocks(long long tiles, long long items, const char* what =
 // and key j at (j / wsz, j % wsz) give the signed offsets (dr, dc), and every head adds
 //   table[(dr + wsz - 1) * (2 wsz - 1) + (dc + wsz - 1)]
 // from one shared fp32 table of (2 wsz - 1)^2 entries, in the units of the scaled scores.  nq == nk == wsz^2; fmap / step unused.
+//
+// r2l_ws > 0 (RegionViT's regional-to-local attention, regionvit.py:143-155,168-169) replaces both: token 0 is the regional token
+// and tokens 1 .. r2l_h * r2l_w the r2l_h x r2l_w local window, token t > 0 at (r, c) = ((t - 1) / r2l_w, (t - 1) % r2l_w).  For
+// i, j > 0 head h adds
+//   table[h * (2 ws - 1)^2 + (dr + ws - 1) * (2 ws - 1) + (dc + ws - 1)]     (ws = r2l_ws; r2l_h, r2l_w <= ws)
+// and row 0 / column 0 get nothing.  The table is [heads][(2 ws - 1)^2], in the units of the scaled scores.  nq == nk == 1 + r2l_h r2l_w.
 struct PosBias {
   const float* table = nullptr;
   int fmap = 0, step = 1;
   bool gelu_out = false;                  // levit.py:94: to_out starts with an exact-erf GELU of the attention output
   int wsz = 0;
+  int r2l_ws = 0, r2l_h = 0, r2l_w = 0;
   __host__ __device__ int q_side() const { return (fmap + step - 1) / step; }
 };
+__host__ __device__ __forceinline__ int r2l_bias_index(int i, int j, int ww, int ws) {   // i, j > 0
+  const int ri = (i - 1) / ww, ci = i - 1 - ri * ww, rj = (j - 1) / ww, cj = j - 1 - rj * ww;
+  return (ri - rj + ws - 1) * (2 * ws - 1) + ci - cj + ws - 1;
+}
 __host__ __device__ __forceinline__ int window_bias_index(int i, int j, int wsz) {
   const int ri = i / wsz, rj = j / wsz;
   return (ri - rj + wsz - 1) * (2 * wsz - 1) + (i - ri * wsz) - (j - rj * wsz) + wsz - 1;

@@ -232,6 +232,42 @@ inline bool block_attention_fast(const __nv_bfloat16* qkv, int ld, __nv_bfloat16
   return attention_block(qkv, ld, out, ldo, heads, dh, s, 0.f, win);
 }
 
+// One RegionViT stage (regionvit.py:231-240) on channel rows zero-padded to dp (bf16) / dim (fp32): the shared Downsample (s >= 1),
+// the PEG (s >= 1 with use_peg), then the R2L layers.  Each layer's one Attention module (4 heads of 32, inner 128) serves the
+// regional self-attention and the regional-to-local attention; the bf16 engine folds its LayerNorm (and the MLP's) into q|k|v
+// (fc1).
+struct RegionLayerW { Norm attn_norm; Linear qkv, to_out; MlpW ff; };
+struct RegionStageW {
+  int dim = 0, dp = 0;
+  bool down = false, peg = false;
+  Linear down_conv;                  // Conv2D(3, 2, SAME) as a Dense over unfold_same's (row, column, channel) vectors
+  const float* peg_w = nullptr;      // PEG taps [9][dp] with the residual folded into the centre tap, and its bias [dp]
+  const float* peg_b = nullptr;
+  const float* table = nullptr;      // local_rel_pos_bias as [4][(2 ws - 1)^2], row offset slowest (PosBias::r2l_ws)
+  std::vector<RegionLayerW> layers;
+};
+
+// RegionViT's Embedding((2 ws - 1)^2, heads) (regionvit.py:126), looked up at row (dr + ws - 1) + (dc + ws - 1) (2 ws - 1) (:152),
+// as [heads][(dr + ws - 1) (2 ws - 1) + dc + ws - 1]: the row-offset-slowest convention of the windowed attention kernels
+template <typename F>
+std::vector<double> r2l_table_from_embedding(const F* emb, int ws, int heads) {
+  const int side = 2 * ws - 1;
+  std::vector<double> t(static_cast<size_t>(heads) * side * side);
+  for (int h = 0; h < heads; ++h)
+    for (int a = 0; a < side; ++a)
+      for (int c = 0; c < side; ++c) t[(static_cast<size_t>(h) * side + a) * side + c] = emb[(static_cast<size_t>(a) + c * side) * heads + h];
+  return t;
+}
+
+// RegionViT's regional-to-local attention on its flash kernel (attn_flash.cu): bf16 only, false for a shape it does not take.
+inline bool r2l_attention_fast(const float*, int, float*, int, int, int, long long, const PosBias&, const Window&, cudaStream_t) {
+  return false;
+}
+inline bool r2l_attention_fast(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* out, int ldo, int heads, int dh, long long reg_row0,
+                               const PosBias& pb, const Window& win, cudaStream_t s) {
+  return attention_r2l(qkv, ld, out, ldo, heads, dh, reg_row0, pb, win, s);
+}
+
 struct EmbedW { Linear patch; const float* pos = nullptr; const float* cls = nullptr; int dim = 0, n_pos = 0; };
 struct CrossW { bool proj = false; Linear project_in, project_out, to_q, to_kv, to_out; Norm norm; };
 
@@ -466,6 +502,15 @@ struct vb_handle {
     if (ns.levels == 0) return ns.dim;
     return nest_aggregates(ns.levels - 1) ? nest_dim(ns.levels) : nest_dim(ns.levels - 1);
   }
+  // RegionViT (regionvit.py:184-263): the local encoder (one 8x8 stride-4 convolution, or three 3x3 with two LayerNorms), the
+  // region encoder, the stages, the head LayerNorm (`head_norm`) and Dense (`head`)
+  vb_regionvit_config rv{};
+  Linear rv_local[3], rv_region;
+  Norm rv_local_norm[2];
+  std::vector<RegionStageW> rv_stages;
+  static std::string rv_pre(int s) { return "region_layers." + std::to_string(s) + "."; }
+  int rv_region_patch() const { return rv.local_patch_size * rv.window_size; }   // regionvit.py:204
+  static constexpr int kRvHeads = 4, kRvDh = 32, kRvInner = kRvHeads * kRvDh;   // R2LTransformer's defaults (:119, :239)
   struct XBlock { std::vector<LayerW> sm_layers, lg_layers; Norm sm_final, lg_final; std::vector<CrossW> sm_attend_lg, lg_attend_sm; };
   std::vector<XBlock> xblocks;
   Norm head_norm, sm_head_norm, lg_head_norm;
@@ -751,6 +796,38 @@ struct vb_handle {
       }
       expect_ln4("mlp_head.0", nest_last_dim());                        // :196-200
       expect_dense("mlp_head.2", nest_last_dim(), c.num_classes);
+    } else if (c.kind == VB_KIND_REGIONVIT) {
+      auto expect_ln = [&](const std::string& n, int d) { expect(n + ".gamma", {d}); expect(n + ".beta", {d}); };
+      auto expect_conv = [&](const std::string& n, int k, int cin, int cout) { expect(n + ".kernel", {k, k, cin, cout}); expect(n + ".bias", {cout}); };
+      const int d0 = rv.dims[0], p = rv_region_patch(), t = (2 * rv.window_size - 1) * (2 * rv.window_size - 1);
+      if (rv.tokenize_local_3_conv) {                                  // regionvit.py:210-219
+        expect_conv("local_encoder.0", 3, c.channels, d0);
+        expect_ln("local_encoder.1", d0);
+        expect_conv("local_encoder.3", 3, d0, d0);
+        expect_ln("local_encoder.4", d0);
+        expect_conv("local_encoder.6", 3, d0, d0);
+      } else {
+        expect_conv("local_encoder", 8, c.channels, d0);                // :221
+      }
+      expect_conv("region_encoder.1", 1, c.channels * p * p, d0);       // :223-226
+      for (int s = 0; s < VB_REGIONVIT_STAGES; ++s) {
+        const std::string pre = rv_pre(s);
+        const int d = rv.dims[s], hidden = d * rv.mlp_mult;
+        if (s > 0) expect_conv(pre + "0.conv", 3, rv.dims[s - 1], d);   // Downsample :45-52
+        if (s > 0 && rv.use_peg) expect_conv(pre + "1.proj", 3, 1, d);   // PEG :54-61 (groups = dim)
+        expect(pre + "2.local_rel_pos_bias.embeddings", {t, kRvHeads});  // :126
+        for (int L = 0; L < rv.depth[s]; ++L) {
+          const std::string b = pre + "2.layers." + std::to_string(L) + ".";
+          expect_ln(b + "0.norm", d);                                    // Attention :79-91
+          expect_dense(b + "0.to_qkv", d, 3 * kRvInner, false);
+          expect_dense(b + "0.to_out", kRvInner, d);
+          expect_ln(b + "1.net.0", d);                                   // MLP :64-74
+          expect_dense(b + "1.net.1", d, hidden);
+          expect_dense(b + "1.net.4", hidden, d);
+        }
+      }
+      expect_ln("to_logits.1", rv.dims[VB_REGIONVIT_STAGES - 1]);       // :243-247
+      expect_dense("to_logits.2", rv.dims[VB_REGIONVIT_STAGES - 1], c.num_classes);
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       expect("pos_embedding", {1, np, c.dim});
@@ -975,7 +1052,7 @@ struct vb_handle {
     for (auto& w : weights) VB_CHECK(w.set, "vb_finalize: weight '" + w.name + "' was never set");
     VB_CUDA(cudaSetDevice(device));
     owned.clear(); layers.clear(); cls_layers.clear(); t2t_layers.clear(); xblocks.clear(); plans.clear(); embed_res.clear(); cct_convs.clear();
-    lv_stem.clear(); lv_blocks.clear(); cvt_stages.clear(); twins_stages.clear(); cf_stages.clear(); nest_levels.clear();
+    lv_stem.clear(); lv_blocks.clear(); cvt_stages.clear(); twins_stages.clear(); cf_stages.clear(); nest_levels.clear(); rv_stages.clear();
     woverride.clear();
     drop_graphs();
     const vb_config& c = cfg;
@@ -1034,6 +1111,8 @@ struct vb_handle {
       finalize_crossformer();
     } else if (c.kind == VB_KIND_NEST) {
       finalize_nest();
+    } else if (c.kind == VB_KIND_REGIONVIT) {
+      finalize_regionvit();
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       embed = make_embed("", c.patch_h, c.patch_w, c.dim, np, false);
@@ -1374,6 +1453,73 @@ struct vb_handle {
     }
     head_norm = padded_norm("mlp_head.0", nest_last_dim(), channel_width(nest_last_dim()));
     head = make_linear_f32("mlp_head.2", nest_last_dim(), cfg.num_classes);
+  }
+  // ---- RegionViT weight packing: channel widths zero-padded (bf16), the region kernel's rows permuted, the PEG residual folded,
+  // every Attention / MLP LayerNorm (Keras, eps 1e-3) folded into q|k|v / fc1 in the bf16 engine, the window tables transposed
+  Norm rv_norm(const std::string& n, int d, int dp) {
+    return Norm{upload_owned(pad_n(host_weight(n + ".gamma"), dp)), upload_owned(pad_n(host_weight(n + ".beta"), dp)), d};
+  }
+  Linear rv_conv(const std::string& n, int K, int d, int dp) {     // a Conv2D kernel [kh, kw, cin, d] is the Dense [kh kw cin, d]
+    return linear_from_host("rv." + n, pad_kn(host_weight(n + ".kernel"), K, d, K, dp), pad_n(host_weight(n + ".bias"), dp), K, dp);
+  }
+  void finalize_regionvit() {
+    const int C = cfg.channels, d0 = rv.dims[0], dp0 = channel_width(d0), p = rv_region_patch(), ws = rv.window_size;
+    if (rv.tokenize_local_3_conv) {
+      for (int i = 0; i < 3; ++i) rv_local[i] = rv_conv("local_encoder." + std::to_string(3 * i), 9 * (i == 0 ? C : d0), d0, dp0);
+      for (int i = 0; i < 2; ++i) rv_local_norm[i] = rv_norm("local_encoder." + std::to_string(3 * i + 1), d0, dp0);
+    } else {
+      rv_local[0] = rv_conv("local_encoder", 64 * C, d0, dp0);
+    }
+    // 'b (h p1) (w p2) c -> b h w (c p1 p2)' (regionvit.py:224): the reference's row c p^2 + p1 p + p2 is unfold_same's row
+    // (p1 p + p2) C + c
+    {
+      const auto wr = host_weight("region_encoder.1.kernel");
+      const int K = C * p * p;
+      std::vector<double> wp(static_cast<size_t>(K) * d0);
+      for (int c = 0; c < C; ++c)
+        for (int t = 0; t < p * p; ++t)
+          std::copy(wr.begin() + static_cast<size_t>(c * p * p + t) * d0, wr.begin() + static_cast<size_t>(c * p * p + t + 1) * d0,
+                    wp.begin() + static_cast<size_t>(t * C + c) * d0);
+      rv_region = linear_from_host("rv.region_encoder", pad_kn(wp, K, d0, K, dp0), pad_n(host_weight("region_encoder.1.bias"), dp0), K, dp0);
+    }
+    for (int s = 0; s < VB_REGIONVIT_STAGES; ++s) {
+      RegionStageW S;
+      const std::string pre = rv_pre(s);
+      const int d = rv.dims[s], dp = channel_width(d), hidden = d * rv.mlp_mult, hp = channel_width(hidden);
+      S.dim = d; S.dp = dp; S.down = s > 0; S.peg = s > 0 && rv.use_peg;
+      if (S.down) S.down_conv = rv_conv(pre + "0.conv", 9 * rv.dims[s - 1], d, dp);
+      if (S.peg) {       // x + dw(x) + b: the depthwise 3x3 with 1 added to its centre tap (TF SAME pads 1 at stride 1)
+        const auto taps = host_weight(pre + "1.proj.kernel");
+        std::vector<double> pw(static_cast<size_t>(9) * dp, 0.0);
+        for (int t = 0; t < 9; ++t)
+          for (int c = 0; c < d; ++c) pw[static_cast<size_t>(t) * dp + c] = taps[static_cast<size_t>(t) * d + c] + (t == 4 ? 1.0 : 0.0);
+        S.peg_w = upload_owned(pw);
+        S.peg_b = upload_owned(pad_n(host_weight(pre + "1.proj.bias"), dp));
+      }
+      S.table = upload_owned(r2l_table_from_embedding(host_weight(pre + "2.local_rel_pos_bias.embeddings").data(), ws, kRvHeads));
+      for (int L = 0; L < rv.depth[s]; ++L) {
+        const std::string b = pre + "2.layers." + std::to_string(L) + ".", key = "rv." + b;
+        RegionLayerW w;
+        w.attn_norm = rv_norm(b + "0.norm", d, dp);
+        w.qkv = linear_from_host(key + "qkv", pad_kn(host_weight(b + "0.to_qkv.kernel"), d, 3 * kRvInner, dp, 3 * kRvInner), {}, dp,
+                                 3 * kRvInner, bf16() ? &w.attn_norm : nullptr);
+        w.qkv.ln_d = d;
+        // to_out reads the attention output in place of q: its K is the inner width, the rows' pitch is that of q|k|v
+        w.to_out = linear_from_host(key + "to_out", pad_kn(host_weight(b + "0.to_out.kernel"), kRvInner, d, kRvInner, dp),
+                                    pad_n(host_weight(b + "0.to_out.bias"), dp), kRvInner, dp);
+        w.ff.norm = rv_norm(b + "1.net.0", d, dp);
+        w.ff.fc1 = linear_from_host(key + "fc1", pad_kn(host_weight(b + "1.net.1.kernel"), d, hidden, dp, hp),
+                                    pad_n(host_weight(b + "1.net.1.bias"), hp), dp, hp, bf16() ? &w.ff.norm : nullptr);
+        w.ff.fc1.ln_d = d;
+        w.ff.fc2 = linear_from_host(key + "fc2", pad_kn(host_weight(b + "1.net.4.kernel"), hidden, d, hp, dp),
+                                    pad_n(host_weight(b + "1.net.4.bias"), dp), hp, dp);
+        S.layers.push_back(std::move(w));
+      }
+      rv_stages.push_back(std::move(S));
+    }
+    const int dl = rv.dims[VB_REGIONVIT_STAGES - 1];
+    head_norm = make_norm("to_logits.1", dl);
+    head = make_linear_f32("to_logits.2", dl, cfg.num_classes);
   }
   void finalize_levit() {
     const int dh = levit_dh();
@@ -1933,6 +2079,8 @@ struct vb_handle {
       crossformer_forward<T>(img, B, H, Wd, logits, s);
     } else if (c.kind == VB_KIND_NEST) {
       nest_forward<T>(img, B, H, Wd, logits, s);
+    } else if (c.kind == VB_KIND_REGIONVIT) {
+      regionvit_forward<T>(img, B, H, Wd, logits, s);
     } else if (c.kind == VB_KIND_CCT) {                   // CCT.call cct.py:342-345, TransformerClassifier.call :277-305
       int rows = 0;
       T* X = tokenize_cct<T>(img, B, H, Wd, &rows, s);
@@ -2560,6 +2708,205 @@ struct vb_handle {
     { ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * rows * HD, s); window_rows<T>(ow, HD, out, ldo, HD, win, rows, false, s); }
   }
 
+  // RegionViT.call (regionvit.py:249-263): the local and region encoders, then per stage the shared Downsample of both maps, the
+  // PEG of the local map and the R2L layers; then the mean over the regional tokens, LayerNorm and Dense.  Each stage keeps its
+  // local rows (the pixel-major B x lh x lw map) followed by its regional rows (the B x rh x rw map) in one arena, so every
+  // token-wise step is one launch over both; the R2L attention reads and writes both in place.  Channel widths are zero-padded to
+  // channel_width.  bf16: `stats` holds the (sum, sumsq) partials of all rows between sub-blocks, pitch M.
+  static constexpr const char* kRegionNoStages =
+      "RegionViT runs as a whole forward only: its encoder / stage / head steps have no entry of their own";
+  // The reference's shape rules (the call-time asserts :251-252, the window rearranges and concat :163-168, the bias Embedding
+  // :153), checked before anything runs.  The local encoder's SAME stride 4 (or two SAME stride 2) gives ceil(H / 4).
+  void rv_check_size(int H, int Wd) const {
+    const int p = rv_region_patch(), lp = rv.local_patch_size, ws = rv.window_size;
+    VB_CHECK(H % p == 0 && Wd % p == 0, "height and width must be divisible by region patch size");
+    VB_CHECK(H % lp == 0 && Wd % lp == 0, "height and width must be divisible by local patch size");
+    int lh = (H + 3) / 4, lw = (Wd + 3) / 4, rh = H / p, rw = Wd / p;
+    for (int s = 0; s < VB_REGIONVIT_STAGES; ++s) {
+      if (s > 0) { lh = (lh + 1) / 2; lw = (lw + 1) / 2; rh = (rh + 1) / 2; rw = (rw + 1) / 2; }
+      const std::string where = "RegionViT stage " + std::to_string(s + 1) + ": the " + std::to_string(lh) + " x " + std::to_string(lw) +
+                                " local map and the " + std::to_string(rh) + " x " + std::to_string(rw) + " region map ";
+      VB_CHECK(lh >= rh && lw >= rw && lh % rh == 0 && lw % rw == 0,
+               where + "do not make whole windows (the local map must be the region map times the window)");
+      VB_CHECK(lh / rh <= ws && lw / rw <= ws, where + "make " + std::to_string(lh / rh) + " x " + std::to_string(lw / rw) +
+                                                   " windows, larger than window_size " + std::to_string(ws) +
+                                                   " (the relative-position table's reach)");
+    }
+  }
+  // The row statistics of the regional rows at pitch M, after their own residual update (bf16; the fp32 engine keeps none).
+  template <typename T>
+  void rv_region_stats(const T* Xr, int dp, float* stats, int Mr, long long pitch, cudaStream_t s) {
+    if constexpr (std::is_same<T, __nv_bfloat16>::value) {
+      ProfScope ps(this, PROF_LN, 0.0, 2.0 * Mr * dp, s);
+      row_stats_bf16(Xr, dp, stats, Mr, dp, s, pitch);
+    }
+  }
+  template <typename T>
+  void regionvit_forward(const float* img, int B, int H, int Wd, float* logits, cudaStream_t s) {
+    rv_check_size(H, Wd);
+    const int C = cfg.channels, p = rv_region_patch();
+    int lh = (H + 3) / 4, lw = (Wd + 3) / 4, rh = H / p, rw = Wd / p;
+    int Ml = B * lh * lw, Mr = B * rh * rw, M = Ml + Mr, d = rv.dims[0], dp = rv_stages[0].dp;
+    T* X = arena.get<T>(static_cast<size_t>(M) * dp);
+    float* stats = bf16() ? arena.get<float>(static_cast<size_t>(M) * (dp / 64) * 2) : nullptr;
+    // a SAME convolution as unfold_same + GEMM into out [rows, dp]; src == null reads the image
+    auto conv = [&](const T* src, int h, int w, int cin, int k, int stride, const UnfoldMode* um, const Linear& Lw, T* out, float* st) {
+      const int oh = (h + stride - 1) / stride, ow = (w + stride - 1) / stride, rows = B * oh * ow, Kp = bf16() ? Lw.ldw : Lw.K;
+      T* col = arena.get<T>(static_cast<size_t>(rows) * Kp);
+      {
+        ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(src ? sizeof(T) : 4) * B * h * w * cin + static_cast<double>(sizeof(T)) * rows * Kp, s);
+        if (src == nullptr) unfold_same<float, T>(img, col, B, h, w, cin, k, stride, 0, Kp, s);
+        else unfold_same<T, T>(src, col, B, h, w, cin, k, stride, 0, Kp, s, dp, um);
+      }
+      Linear L = Lw;
+      L.K = Kp;
+      Epi e; e.bias = Lw.bias; e.stats_out = st;
+      linear<T>(col, Kp, rows, L, out, dp, e, s);
+    };
+    if (rv.tokenize_local_3_conv) {                                  // regionvit.py:211-218: the LayerNorm + GELU applied on load
+      int h = H, w = Wd;
+      const T* src = nullptr;
+      for (int i = 0; i < 3; ++i) {
+        const int stride = i < 2 ? 2 : 1, oh = (h + stride - 1) / stride, ow = (w + stride - 1) / stride, rows = B * oh * ow;
+        UnfoldMode um;
+        um.gelu = true;
+        if (i > 0 && bf16()) {
+          um.stats = stats; um.parts = dp / 64; um.d = d; um.eps = 1e-3f; um.gamma = rv_local_norm[i - 1].gamma; um.beta = rv_local_norm[i - 1].beta;
+        } else if (i > 0) {
+          T* Z = arena.get<T>(static_cast<size_t>(B) * h * w * dp);
+          ProfScope ps(this, PROF_LN, 8.0 * B * h * w * d, 2.0 * sizeof(T) * B * h * w * dp, s);
+          layernorm<T>(src, dp, rv_local_norm[i - 1].gamma, rv_local_norm[i - 1].beta, Z, dp, B * h * w, d, s, dp, 1e-3f);
+          src = Z;
+        }
+        T* out = i == 2 ? X : arena.get<T>(static_cast<size_t>(rows) * dp);
+        float* st = bf16() && i < 2 ? arena.get<float>(static_cast<size_t>(rows) * (dp / 64) * 2) : nullptr;
+        conv(src, h, w, i == 0 ? C : d, 3, stride, i > 0 ? &um : nullptr, rv_local[i], out, st);
+        src = out; h = oh; w = ow;
+        if (st != nullptr) stats = st;                               // the next unfold's LayerNorm statistics
+      }
+      stats = bf16() ? arena.get<float>(static_cast<size_t>(M) * (dp / 64) * 2) : nullptr;
+    } else {
+      conv(nullptr, H, Wd, C, 8, 4, nullptr, rv_local[0], X, nullptr);   // :221
+    }
+    conv(nullptr, H, Wd, C, p, p, nullptr, rv_region, X + static_cast<size_t>(Ml) * dp, nullptr);   // :223-226
+    if (bf16()) ensure_stats<T>(X, dp, stats, M, s);
+    for (const RegionStageW& S : rv_stages) {
+      if (S.down) {          // :258: one Conv2D(3, 2, SAME) for both maps, both unfolded into one column buffer, one GEMM
+        const int olh = (lh + 1) / 2, olw = (lw + 1) / 2, orh = (rh + 1) / 2, orw = (rw + 1) / 2;
+        const int nMl = B * olh * olw, nMr = B * orh * orw, nM = nMl + nMr, Kp = bf16() ? S.down_conv.ldw : S.down_conv.K;
+        T* col = arena.get<T>(static_cast<size_t>(nM) * Kp);
+        {
+          ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(sizeof(T)) * (static_cast<double>(M) * dp + static_cast<double>(nM) * Kp), s);
+          unfold_same<T, T>(X, col, B, lh, lw, d, 3, 2, 0, Kp, s, dp);
+          unfold_same<T, T>(X + static_cast<size_t>(Ml) * dp, col + static_cast<size_t>(nMl) * Kp, B, rh, rw, d, 3, 2, 0, Kp, s, dp);
+        }
+        T* Xn = arena.get<T>(static_cast<size_t>(nM) * S.dp);
+        stats = bf16() ? arena.get<float>(static_cast<size_t>(nM) * (S.dp / 64) * 2) : nullptr;
+        Linear L = S.down_conv;
+        L.K = Kp;
+        Epi e; e.bias = S.down_conv.bias; e.stats_out = S.peg ? nullptr : stats;
+        linear<T>(col, Kp, nM, L, Xn, S.dp, e, s);
+        X = Xn; lh = olh; lw = olw; rh = orh; rw = orw; Ml = nMl; Mr = nMr; M = nM; d = S.dim; dp = S.dp;
+      }
+      if (S.peg) {           // :259: the local map only; the halo reads the unmodified map, so the result goes to a new arena
+        T* Y = arena.get<T>(static_cast<size_t>(M) * dp);
+        {
+          ProfScope ps(this, PROF_OTHER, 18.0 * Ml * d, 2.0 * sizeof(T) * Ml * dp, s);
+          dwconv_qkv<T>(X, dp, nullptr, nullptr, nullptr, d, 1e-5f, S.peg_w, S.peg_b, Y, dp, nullptr, nullptr, nullptr, dp, B, lh, lw, dp, 3, 1, s);
+        }
+        VB_CUDA(cudaMemcpyAsync(Y + static_cast<size_t>(Ml) * dp, X + static_cast<size_t>(Ml) * dp, static_cast<size_t>(Mr) * dp * sizeof(T),
+                                cudaMemcpyDeviceToDevice, s));
+        X = Y;
+        if (bf16()) ensure_stats<T>(X, dp, stats, M, s);
+      }
+      for (const RegionLayerW& l : S.layers) regionvit_layer<T>(X, B, lh, lw, rh, rw, S, l, stats, s);
+    }
+    // to_logits (:243-247): the mean over the regional tokens, then LayerNorm, then Dense
+    float* z = arena.get<float>(static_cast<size_t>(B) * d);
+    {
+      ProfScope ps(this, PROF_LN, 1.0 * Mr * d + 8.0 * B * d, static_cast<double>(sizeof(T)) * Mr * dp, s);
+      pool_layernorm<T>(X + static_cast<size_t>(Ml) * dp, rh * rw, dp, head_norm.gamma, head_norm.beta, z, B, d, 1, s);
+    }
+    gemm_simt<float, float, float>(z, d, head.W, head.N, 1, logits, head.N, B, head.N, d, head.bias, nullptr, nullptr, head.N, 0, s);
+  }
+  // One R2L layer (regionvit.py:158-172) in place on X [M, dp], M = B lh lw local rows + B rh rw regional rows: the regional
+  // self-attention on the regional rows, then the R2L attention and the MLP over all rows.  bf16: the LayerNorms folded into q|k|v
+  // and fc1 (from `stats`, and for the regional q|k|v from the regional rows' own statistics at pitch Mr); fp32: separate
+  // LayerNorms.
+  template <typename T>
+  void regionvit_layer(T* X, int B, int lh, int lw, int rh, int rw, const RegionStageW& S, const RegionLayerW& l, float* stats, cudaStream_t s) {
+    const int dp = S.dp, d = S.dim, Ml = B * lh * lw, Mr = B * rh * rw, M = Ml + Mr, ld = l.qkv.N;
+    T* Xr = X + static_cast<size_t>(Ml) * dp;
+    T* Y = bf16() ? nullptr : arena.get<T>(static_cast<size_t>(M) * dp);
+    T* QKV = arena.get<T>(static_cast<size_t>(M) * ld);
+    auto prenorm = [&](const T* A, int rows, const Norm& n) -> const T* {
+      if (Y == nullptr) return A;
+      ProfScope ps(this, PROF_LN, 8.0 * rows * d, 2.0 * sizeof(T) * rows * dp, s);
+      layernorm<T>(A, dp, n.gamma, n.beta, Y, dp, rows, d, s, dp, 1e-3f);
+      return Y;
+    };
+    auto folded = [&](const Linear& L, const float* st) {
+      Epi e;
+      if (Y == nullptr) { e.bias = L.ln_c2; e.ln_stats = st; } else { e.bias = L.bias; }
+      return e;
+    };
+    // region_tokens = attn(region_tokens) + region_tokens (:159): all rh x rw regional tokens of an image attend together
+    float* rstats = bf16() ? arena.get<float>(static_cast<size_t>(Mr) * (dp / 64) * 2) : nullptr;
+    if (bf16()) rv_region_stats<T>(Xr, dp, rstats, Mr, Mr, s);
+    linear<T>(prenorm(Xr, Mr, l.attn_norm), dp, Mr, l.qkv, QKV, ld, folded(l.qkv, rstats), s);
+    Window rwin;
+    rwin.p = rh; rwin.pw = rw; rwin.nx = 1; rwin.ny = 1; rwin.count = B;
+    block_attention<T>(QKV, ld, QKV, ld, kRvHeads, kRvDh, rwin, s);     // the output overwrites q
+    {
+      Epi e; e.bias = l.to_out.bias; e.res = Xr; e.ldr = dp;
+      linear<T>(QKV, ld, Mr, l.to_out, Xr, dp, e, s);
+    }
+    if (bf16()) rv_region_stats<T>(Xr, dp, stats + static_cast<size_t>(Ml) * 2, Mr, M, s);
+    // [r; window] = attn([r; window], rel_pos_bias) + [r; window] (:168-169), each window with its regional token
+    linear<T>(prenorm(X, M, l.attn_norm), dp, M, l.qkv, QKV, ld, folded(l.qkv, stats), s);
+    Window win;
+    win.p = lh / rh; win.pw = lw / rw; win.nx = rw; win.ny = rh; win.count = Mr;
+    PosBias pb;
+    pb.table = S.table; pb.r2l_ws = rv.window_size; pb.r2l_h = win.p; pb.r2l_w = win.pw;
+    r2l_attention<T>(QKV, ld, QKV, ld, Ml, pb, win, s);
+    auto residual = [&](const T* A, int lda, const Linear& L) {     // X = A W + b + X over all rows, and X's new row statistics
+      Epi e; e.bias = L.bias; e.res = X; e.ldr = dp; e.stats_out = stats;
+      linear<T>(A, lda, M, L, X, dp, e, s);
+    };
+    residual(QKV, ld, l.to_out);
+    // ff(.) + . (:172)
+    T* Hb = arena.get<T>(static_cast<size_t>(M) * l.ff.fc1.N);
+    Epi e1 = folded(l.ff.fc1, stats);
+    e1.gelu = true;
+    linear<T>(prenorm(X, M, l.ff.norm), dp, M, l.ff.fc1, Hb, l.ff.fc1.N, e1, s);
+    residual(Hb, l.ff.fc1.N, l.ff.fc2);
+  }
+  // RegionViT's R2L attention: win.count windows of p x width() local rows, each with its regional row reg_row0 + (window index),
+  // fused q|k|v rows [.., ld], the output rows written in place to out [.., ldo].  The R2L flash kernel where it serves (bf16, dh
+  // 32, tables up to its shared-memory size); otherwise the windows gathered window-major with the regional row first, the
+  // materialised-scores path with the R2L bias, and the output rows scattered back.
+  template <typename T>
+  void r2l_attention(const T* qkv, int ld, T* out, int ldo, long long reg_row0, const PosBias& pb, const Window& win, cudaStream_t s,
+                     int heads = kRvHeads, int dh = kRvDh) {
+    const int n = 1 + win.p * win.width(), HD = heads * dh;
+    const long long Bw = win.count, rows = Bw * n;
+    const double fl = 4.0 * Bw * heads * n * n * dh, by = static_cast<double>(sizeof(T)) * Bw * heads * dh * 4.0 * n;
+    {
+      ProfScope ps(this, PROF_ATTN, fl, by, s);
+      if (r2l_attention_fast(qkv, ld, out, ldo, heads, dh, reg_row0, pb, win, s)) return;
+    }
+    T* qkvw = arena.get<T>(static_cast<size_t>(rows) * 3 * HD);
+    T* ow = arena.get<T>(static_cast<size_t>(rows) * HD);
+    { ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * rows * 3 * HD, s); r2l_rows<T>(qkv, ld, qkvw, 3 * HD, 3 * HD, win, reg_row0, true, s); }
+    {
+      ProfScope ps(this, PROF_ATTN, fl, by, s);
+      float* Sc = arena.get<float>(static_cast<size_t>(Bw) * heads * n * ((n + 15) & ~15));
+      attention_generic<T>(qkvw, 3 * HD, qkvw + HD, 3 * HD, qkvw + 2 * HD, 3 * HD, ow, HD, Sc, static_cast<int>(Bw), n, n, heads, dh, 0, nullptr,
+                           nullptr, nullptr, nullptr, s, 0.f, &pb);
+    }
+    { ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * rows * HD, s); r2l_rows<T>(ow, HD, out, ldo, HD, win, reg_row0, false, s); }
+  }
+
   // DistillMixin.call (distill.py:16-45) on top of a ViT: embed -> append the distillation token as the LAST row ->
   // transformer over n + 2 rows -> head on the first n + 1 rows, and the last row returned as is.
   template <typename T>
@@ -2618,6 +2965,7 @@ struct vb_handle {
     VB_CHECK(cfg.kind != VB_KIND_TWINS_SVT, kTwinsNoStages);
     VB_CHECK(cfg.kind != VB_KIND_CROSSFORMER, kCrossformerNoStages);
     VB_CHECK(cfg.kind != VB_KIND_NEST, kNestNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_REGIONVIT, kRegionNoStages);
     if (cfg.kind == VB_KIND_T2T_VIT) {
       int h = H, w = Wd;
       for (const auto& st : t2t_stages()) { h = (h + st.stride - 1) / st.stride; w = (w + st.stride - 1) / st.stride; }
@@ -2648,6 +2996,7 @@ struct vb_handle {
     VB_CHECK(cfg.kind != VB_KIND_TWINS_SVT, kTwinsNoStages);
     VB_CHECK(cfg.kind != VB_KIND_CROSSFORMER, kCrossformerNoStages);
     VB_CHECK(cfg.kind != VB_KIND_NEST, kNestNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_REGIONVIT, kRegionNoStages);
     arena.reset();
     const long long count = static_cast<long long>(B) * n * cfg.dim;
     T* X = arena.get<T>(count);
@@ -2664,6 +3013,7 @@ struct vb_handle {
     VB_CHECK(cfg.kind != VB_KIND_TWINS_SVT, kTwinsNoStages);
     VB_CHECK(cfg.kind != VB_KIND_CROSSFORMER, kCrossformerNoStages);
     VB_CHECK(cfg.kind != VB_KIND_NEST, kNestNoStages);
+    VB_CHECK(cfg.kind != VB_KIND_REGIONVIT, kRegionNoStages);
     arena.reset();
     const int K = embed.patch.K, Kp = bf16() ? embed.patch.ldw : K;
     T* col = arena.get<T>(static_cast<size_t>(rows) * Kp);
@@ -2864,6 +3214,7 @@ void validate(const vb_config& c) {
   VB_CHECK(c.kind != VB_KIND_TWINS_SVT, "Twins-SVT: create the handle with vb_create_twins_svt (its stages are a vb_twins_svt_config)");
   VB_CHECK(c.kind != VB_KIND_CROSSFORMER, "CrossFormer: create the handle with vb_create_crossformer (its stages are a vb_crossformer_config)");
   VB_CHECK(c.kind != VB_KIND_NEST, "NesT: create the handle with vb_create_nest (its levels are a vb_nest_config)");
+  VB_CHECK(c.kind != VB_KIND_REGIONVIT, "RegionViT: create the handle with vb_create_regionvit (its stages are a vb_regionvit_config)");
   VB_CHECK(c.kind >= VB_KIND_VIT && c.kind <= VB_KIND_CCT, "unknown model kind");
   if (c.kind == VB_KIND_CCT) {
     VB_CHECK(c.channels == 3 && c.num_classes > 0 && c.image_h > 0 && c.image_w > 0, "bad image / class configuration");
@@ -2953,6 +3304,16 @@ void validate_nest(const vb_config& c, const vb_nest_config& n) {
            "NesT: bad patch_size / dim / heads / mlp_mult / seq_len");
   VB_CHECK((static_cast<long long>(n.dim) << (n.num_hierarchies - 1)) <= 65536, "NesT: dim * 2^(num_hierarchies - 1) is too large");
   for (int i = 0; i < n.levels; ++i) VB_CHECK(n.block_repeats[i] >= 0, "NesT: block_repeats must not be negative");
+}
+
+void validate_regionvit(const vb_config& c, const vb_regionvit_config& r) {
+  VB_CHECK(c.precision == VB_PRECISION_FP32 || c.precision == VB_PRECISION_BF16, "unknown precision");
+  VB_CHECK(c.channels > 0 && c.num_classes > 0, "RegionViT: bad channel / class configuration");
+  for (int s = 0; s < VB_REGIONVIT_STAGES; ++s)
+    VB_CHECK(r.dims[s] > 0 && r.dims[s] <= 65536 && r.depth[s] >= 0, "RegionViT: dims must be positive and depth not negative");
+  VB_CHECK(r.window_size > 0 && r.local_patch_size > 0 && r.mlp_mult > 0, "RegionViT: bad window_size / local_patch_size / mlp_mult");
+  VB_CHECK(static_cast<long long>(r.local_patch_size) * r.window_size <= 4096, "RegionViT: the region patch size is too large");
+  VB_CHECK(r.window_size <= 1024, "RegionViT: window_size is too large");
 }
 
 void validate_crossformer(const vb_config& c, const vb_crossformer_config& cf) {
@@ -3244,6 +3605,35 @@ int vb_create_nest(const vb_config* base, const vb_nest_config* nc, int device, 
   });
 }
 
+int vb_create_regionvit(const vb_config* base, const vb_regionvit_config* rc, int device, vb_handle** out) {
+  return guarded(nullptr, [&] {
+    VB_CHECK(base != nullptr && rc != nullptr && out != nullptr, "vb_create_regionvit: null argument");
+    VB_CHECK(base->struct_size == static_cast<int32_t>(sizeof(vb_config)) || base->struct_size == VB_CONFIG_SIZE_ABI7,
+             "vb_config.struct_size mismatch (ABI)");
+    VB_CHECK(rc->struct_size == static_cast<int32_t>(sizeof(vb_regionvit_config)), "vb_regionvit_config.struct_size mismatch (ABI)");
+    vb_config c;
+    memset(&c, 0, sizeof c);
+    memcpy(&c, base, static_cast<size_t>(base->struct_size));
+    VB_CHECK(c.kind == VB_KIND_REGIONVIT, "vb_create_regionvit: base.kind must be VB_KIND_REGIONVIT");
+    validate_regionvit(c, *rc);
+    int ndev = 0;
+    cudaError_t e = cudaGetDeviceCount(&ndev);
+    VB_CHECK(e == cudaSuccess && ndev > 0, "vb_create_regionvit: no CUDA device available -- libvitb200 has no CPU fallback");
+    VB_CHECK(device >= 0 && device < ndev, "vb_create_regionvit: bad device index");
+    VB_CUDA(cudaSetDevice(device));
+    cudaDeviceProp prop;
+    VB_CUDA(cudaGetDeviceProperties(&prop, device));
+    VB_CHECK(prop.major == 9 && prop.minor == 0, "vb_create_regionvit: libvitb200 is built for sm_90a (Hopper H100) only");
+    std::unique_ptr<vb_handle> h(new vb_handle());
+    h->cfg = c;
+    h->rv = *rc;
+    h->cfg.dim = rc->dims[VB_REGIONVIT_STAGES - 1];
+    h->device = device;
+    h->build_expected();
+    *out = h.release();
+  });
+}
+
 int vb_num_weights(vb_handle* h) { return h ? static_cast<int>(h->weights.size()) : -1; }
 
 int vb_weight_info(vb_handle* h, int32_t index, const char** name, int64_t* shape4, int32_t* ndim) {
@@ -3371,6 +3761,7 @@ int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, int32_t 
     VB_CHECK(h->cfg.kind != VB_KIND_TWINS_SVT, "vb_forward_distill: Twins-SVT has no distillation head");
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSFORMER, "vb_forward_distill: CrossFormer has no distillation head");
     VB_CHECK(h->cfg.kind != VB_KIND_NEST, "vb_forward_distill: NesT has no distillation head");
+    VB_CHECK(h->cfg.kind != VB_KIND_REGIONVIT, "vb_forward_distill: RegionViT has no distillation head");
     const bool levit = h->cfg.kind == VB_KIND_LEVIT;
     VB_CHECK(levit || distill_token != nullptr, "vb_forward_distill: null argument");
     VB_CHECK(!levit || (distill_token == nullptr && h->lv.num_distill_classes > 0),
@@ -3430,6 +3821,7 @@ int vb_forward_tokens(vb_handle* h, const float* tokens, int32_t tokens_mem, int
     VB_CHECK(h->cfg.kind != VB_KIND_TWINS_SVT, vb_handle::kTwinsNoStages);
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSFORMER, vb_handle::kCrossformerNoStages);
     VB_CHECK(h->cfg.kind != VB_KIND_NEST, vb_handle::kNestNoStages);
+    VB_CHECK(h->cfg.kind != VB_KIND_REGIONVIT, vb_handle::kRegionNoStages);
     VB_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const long long before = launch_counter();
@@ -3500,7 +3892,7 @@ int vb_to_patch(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, 
     VB_CHECK(h != nullptr && img != nullptr && patches != nullptr, "vb_to_patch: null argument");
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT && h->cfg.kind != VB_KIND_T2T_VIT && h->cfg.kind != VB_KIND_CCT &&
              h->cfg.kind != VB_KIND_LEVIT && h->cfg.kind != VB_KIND_CVT && h->cfg.kind != VB_KIND_TWINS_SVT &&
-             h->cfg.kind != VB_KIND_CROSSFORMER && h->cfg.kind != VB_KIND_NEST,
+             h->cfg.kind != VB_KIND_CROSSFORMER && h->cfg.kind != VB_KIND_NEST && h->cfg.kind != VB_KIND_REGIONVIT,
              "vb_to_patch: the model has no single Rearrange patch layer");
     VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_to_patch: bad batch / image size");
     const vb_config& c = h->cfg;
@@ -3526,6 +3918,7 @@ int vb_patch_to_emb(vb_handle* h, const float* patches, int32_t patches_mem, int
     VB_CHECK(h->cfg.kind != VB_KIND_TWINS_SVT, vb_handle::kTwinsNoStages);
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSFORMER, vb_handle::kCrossformerNoStages);
     VB_CHECK(h->cfg.kind != VB_KIND_NEST, vb_handle::kNestNoStages);
+    VB_CHECK(h->cfg.kind != VB_KIND_REGIONVIT, vb_handle::kRegionNoStages);
     VB_CHECK(rows > 0, "vb_patch_to_emb: bad shape");
     const size_t in_bytes = static_cast<size_t>(rows) * h->embed.patch.K * sizeof(float);
     const size_t out_bytes = static_cast<size_t>(rows) * h->cfg.dim * sizeof(float);
@@ -4072,6 +4465,49 @@ int vb_op_block_attention(int32_t precision, const float* qkv, int32_t ld, int32
         attention_generic<T>(w_d, 3 * HD, w_d + HD, 3 * HD, w_d + 2 * HD, 3 * HD, ow_d, HD, static_cast<float*>(dS.p), Bw, n, n, heads, dh, 0,
                              nullptr, nullptr, nullptr, nullptr, 0);
         window_rows<T>(ow_d, HD, o_d, ldo, HD, win, rows, false, 0);
+      });
+      download<T>(o_d, out, static_cast<size_t>(rows) * ldo);
+    };
+    if (precision == VB_PRECISION_FP32) run(float());
+    else run(__nv_bfloat16());
+  });
+}
+
+int vb_op_r2l_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t lh, int32_t lw, int32_t rh, int32_t rw,
+                        int32_t heads, int32_t dh, const float* table, int32_t window_size, float* out, int32_t ldo, int32_t iters,
+                        float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    const int HD = heads * dh, ws = window_size;
+    VB_CHECK(qkv && table && out && B > 0 && lh > 0 && lw > 0 && rh > 0 && rw > 0 && lh % rh == 0 && lw % rw == 0 && heads > 0 && dh > 0 &&
+             ws > 0 && ws <= 1024 && lh / rh <= ws && lw / rw <= ws && ld >= 3 * HD && ldo >= HD, "vb_op_r2l_attention: bad arguments");
+    Window win;
+    win.p = lh / rh; win.pw = lw / rw; win.nx = rw; win.ny = rh; win.count = B * rh * rw;
+    const long long Ml = static_cast<long long>(B) * lh * lw, rows = Ml + static_cast<long long>(B) * rh * rw;
+    const int n = 1 + win.p * win.pw;
+    DevMem dX, dO, dT, dW, dOw, dS;
+    const auto tab = r2l_table_from_embedding(table, ws, heads);   // transposed as vb_finalize does
+    const std::vector<float> tab_f(tab.begin(), tab.end());
+    PosBias pb;
+    pb.table = upload<float>(dT, tab_f.data(), tab_f.size());
+    pb.r2l_ws = ws; pb.r2l_h = win.p; pb.r2l_w = win.pw;
+    auto run = [&](auto tag) {
+      using T = decltype(tag);
+      const T* x_d = upload<T>(dX, qkv, static_cast<size_t>(rows) * ld);
+      T* o_d = upload<T>(dO, out, static_cast<size_t>(rows) * ldo);
+      // vb_handle::r2l_attention without the handle's arena and profiler
+      timed(iters, elapsed_ms, [&] {
+        if (r2l_attention_fast(x_d, ld, o_d, ldo, heads, dh, Ml, pb, win, 0)) return;
+        const size_t wrows = static_cast<size_t>(win.count) * n;
+        dW.ensure(wrows * 3 * HD * sizeof(T));
+        dOw.ensure(wrows * HD * sizeof(T));
+        dS.ensure(static_cast<size_t>(win.count) * heads * n * ((n + 15) & ~15) * sizeof(float));
+        T* w_d = static_cast<T*>(dW.p);
+        T* ow_d = static_cast<T*>(dOw.p);
+        r2l_rows<T>(x_d, ld, w_d, 3 * HD, 3 * HD, win, Ml, true, 0);
+        attention_generic<T>(w_d, 3 * HD, w_d + HD, 3 * HD, w_d + 2 * HD, 3 * HD, ow_d, HD, static_cast<float*>(dS.p), win.count, n, n, heads,
+                             dh, 0, nullptr, nullptr, nullptr, nullptr, 0, 0.f, &pb);
+        r2l_rows<T>(ow_d, HD, o_d, ldo, HD, win, Ml, false, 0);
       });
       download<T>(o_d, out, static_cast<size_t>(rows) * ldo);
     };

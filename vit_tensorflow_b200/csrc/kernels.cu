@@ -508,6 +508,31 @@ __global__ void attn_window_bias_kernel(float* __restrict__ S, const float* __re
   }
 }
 
+// S[w,h,i,j] += table[h, r2l_bias_index(i, j)] for i, j > 0  (RegionViT's window table; row pitch nk = 1 + wh * ww)
+__global__ void attn_r2l_bias_kernel(float* __restrict__ S, const float* __restrict__ table, int heads, int nk, int ww, int ws,
+                                     long long total) {
+  const int t2 = (2 * ws - 1) * (2 * ws - 1);
+  for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
+       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int j = static_cast<int>(idx % nk);
+    const long long r = idx / nk;
+    const int i = static_cast<int>(r % nk), h = static_cast<int>((r / nk) % heads);
+    if (i > 0 && j > 0) S[idx] += table[static_cast<long long>(h) * t2 + r2l_bias_index(i, j, ww, ws)];
+  }
+}
+
+// One CTA per window-major row t = bw * n + i: i == 0 is the regional row reg_row0 + bw, i > 0 the local row win.row(bw, i - 1).
+template <typename T>
+__global__ void r2l_rows_kernel(const T* __restrict__ in, int ldi, T* __restrict__ out, int ldo, int cols, Window win, int n,
+                                long long reg_row0, bool to_window) {
+  const long long t = blockIdx.x, bw = t / n;
+  const int i = static_cast<int>(t - bw * n);
+  const long long px = i == 0 ? reg_row0 + bw : win.row(bw, i - 1);
+  const T* __restrict__ src = in + (to_window ? px : t) * ldi;
+  T* __restrict__ dst = out + (to_window ? t : px) * ldo;
+  for (int c = threadIdx.x; c < cols; c += blockDim.x) dst[c] = src[c];
+}
+
 // out[b, r*ow + c, :] = in[b, (step*r)*W + step*c, :]  (16-byte vectors when C, ld are multiples of the vector width)
 template <typename T>
 __global__ void gather_grid_kernel(const T* __restrict__ in, int ldi, T* __restrict__ out, int ldo, int H, int W, int C, int step,
@@ -627,7 +652,8 @@ __device__ __forceinline__ float2 unfold_ln(const float2* __restrict__ stats, in
 template <typename TI, typename TO>
 __global__ void unfold_same_kernel(const TI* __restrict__ in, int ldi, TO* __restrict__ out, int B, int H, int W, int C, int k, int stride,
                                    int oh, int ow, int pad_top, int pad_left, int cls_row, int ldo, const float2* __restrict__ stats,
-                                   int parts, float inv_d, float eps, const float* __restrict__ gamma, const float* __restrict__ beta) {
+                                   int parts, float inv_d, float eps, const float* __restrict__ gamma, const float* __restrict__ beta,
+                                   int gelu) {
   const int rows = cls_row + oh * ow;
   const int K = k * k * C;
   const int r = blockIdx.x;                                    // (b, t): B * rows CTAs
@@ -650,9 +676,15 @@ __global__ void unfold_same_kernel(const TI* __restrict__ in, int ldi, TO* __res
       TO* __restrict__ dst = orow + tap * C;
       if (stats != nullptr && inside) {
         const float2 mr = unfold_ln(stats, parts, static_cast<long long>(B) * H * W, (static_cast<long long>(b) * H + y) * W + x, inv_d, eps);
-        for (int c = threadIdx.x; c < C; c += blockDim.x) dst[c] = from_f<TO>((to_f(src[c]) - mr.x) * mr.y * gamma[c] + beta[c]);
+        for (int c = threadIdx.x; c < C; c += blockDim.x) {
+          const float v = (to_f(src[c]) - mr.x) * mr.y * gamma[c] + beta[c];
+          dst[c] = from_f<TO>(gelu ? gelu_exact(v) : v);
+        }
       } else {
-        for (int c = threadIdx.x; c < C; c += blockDim.x) dst[c] = from_f<TO>(inside ? to_f(src[c]) : 0.f);
+        for (int c = threadIdx.x; c < C; c += blockDim.x) {
+          const float v = inside ? to_f(src[c]) : 0.f;
+          dst[c] = from_f<TO>(gelu && inside ? gelu_exact(v) : v);
+        }
       }
     }
   } else {
@@ -668,6 +700,7 @@ __global__ void unfold_same_kernel(const TI* __restrict__ in, int ldi, TO* __res
           const float2 mr = unfold_ln(stats, parts, static_cast<long long>(B) * H * W, (static_cast<long long>(b) * H + y) * W + x, inv_d, eps);
           v = (v - mr.x) * mr.y * gamma[c] + beta[c];
         }
+        if (gelu) v = gelu_exact(v);
       }
       orow[col] = from_f<TO>(v);
     }
@@ -923,7 +956,8 @@ __global__ void ln_fold_consts_kernel(const float* __restrict__ W, const __nv_bf
 }
 
 // one thread per (row, 64-column chunk)
-__global__ void row_stats_kernel(const __nv_bfloat16* __restrict__ X, int ldx, float2* __restrict__ stats, int M, int parts) {
+__global__ void row_stats_kernel(const __nv_bfloat16* __restrict__ X, int ldx, float2* __restrict__ stats, int M, int parts,
+                                 long long pitch) {
   const long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
   if (idx >= static_cast<long long>(M) * parts) return;
   const int c = static_cast<int>(idx % parts);
@@ -941,7 +975,7 @@ __global__ void row_stats_kernel(const __nv_bfloat16* __restrict__ X, int ldx, f
       s2 = fmaf(a, a, fmaf(b, b, s2));
     }
   }
-  stats[static_cast<long long>(c) * M + m] = make_float2(s1, s2);      // [part][M], the layout the GEMM epilogue emits
+  stats[c * pitch + m] = make_float2(s1, s2);      // [part][pitch], the layout the GEMM epilogue emits (pitch M)
 }
 
 __global__ void pad_heads_kernel(const float* __restrict__ W, float* __restrict__ Wp, int other, int groups, int heads, int dh, int dhp,
@@ -1201,6 +1235,13 @@ void attn_pv(const float* S, const T* v, int ldv, T* out, int ldo, int B, int he
 
 void attn_pos_bias(float* S, const PosBias& pb, int B, int heads, int nq, int nk, cudaStream_t s) {
   const long long total = static_cast<long long>(B) * heads * nq * nk;
+  if (pb.r2l_ws > 0) {
+    VB_CHECK(nq == 1 + pb.r2l_h * pb.r2l_w && nk == nq && pb.r2l_h <= pb.r2l_ws && pb.r2l_w <= pb.r2l_ws,
+             "attention: the R2L window table needs nq == nk == 1 + wh * ww with wh, ww <= window_size");
+    attn_r2l_bias_kernel<<<grid_1d(total, 256), 256, 0, s>>>(S, pb.table, heads, nk, pb.r2l_w, pb.r2l_ws, total);
+    VB_LAUNCHED();
+    return;
+  }
   if (pb.wsz > 0) {
     VB_CHECK(nq == pb.wsz * pb.wsz && nk == nq, "attention: the window table needs nq == nk == wsz^2");
     attn_window_bias_kernel<<<grid_1d(total, 256), 256, 0, s>>>(S, pb.table, nk, pb.wsz, total);
@@ -1265,7 +1306,8 @@ void unfold_same(const TI* in, TO* out, int B, int H, int W, int C, int k, int s
   const int threads = C >= 128 ? 160 : (C >= 32 ? 64 : (k * k * C >= 128 ? 160 : 64));
   unfold_same_kernel<TI, TO><<<static_cast<unsigned>(rows_total), threads, 0, s>>>(
       in, ldi, out, B, H, W, C, k, stride, oh, ow, ph / 2, pw / 2, cls_row, ldo, stats, stats ? mode->parts : 0,
-      stats ? 1.0f / static_cast<float>(mode->d) : 0.f, stats ? mode->eps : 0.f, stats ? mode->gamma : nullptr, stats ? mode->beta : nullptr);
+      stats ? 1.0f / static_cast<float>(mode->d) : 0.f, stats ? mode->eps : 0.f, stats ? mode->gamma : nullptr, stats ? mode->beta : nullptr,
+      mode != nullptr && mode->gelu ? 1 : 0);
   VB_LAUNCHED();
 }
 
@@ -1275,6 +1317,16 @@ void window_rows(const T* in, int ldi, T* out, int ldo, int cols, const Window& 
   VB_CHECK(n > 0 && rows % n == 0 && rows < (1ll << 31), "window_rows: rows must be whole windows, fewer than 2^31");
   if (rows == 0) return;
   window_rows_kernel<T><<<static_cast<unsigned>(rows), cols >= 256 ? 256 : 128, 0, s>>>(in, ldi, out, ldo, cols, win, n, to_window);
+  VB_LAUNCHED();
+}
+
+template <typename T>
+void r2l_rows(const T* in, int ldi, T* out, int ldo, int cols, const Window& win, long long reg_row0, bool to_window, cudaStream_t s) {
+  const int n = 1 + win.p * win.width();
+  const long long rows = static_cast<long long>(win.count) * n;
+  VB_CHECK(win.count >= 0 && rows < (1ll << 31), "r2l_rows: fewer than 2^31 window-major rows");
+  if (rows == 0) return;
+  r2l_rows_kernel<T><<<static_cast<unsigned>(rows), cols >= 256 ? 256 : 128, 0, s>>>(in, ldi, out, ldo, cols, win, n, reg_row0, to_window);
   VB_LAUNCHED();
 }
 
@@ -1353,11 +1405,13 @@ void ln_fold_consts(const float* W, const __nv_bfloat16* Wt, int ldw, const floa
   VB_LAUNCHED();
 }
 
-void row_stats_bf16(const __nv_bfloat16* X, int ldx, float* stats, int M, int D, cudaStream_t s) {
+void row_stats_bf16(const __nv_bfloat16* X, int ldx, float* stats, int M, int D, cudaStream_t s, long long pitch) {
   VB_CHECK(D % 64 == 0 && ldx % 8 == 0, "row_stats_bf16: D must be a multiple of 64");
+  VB_CHECK(pitch == 0 || pitch >= M, "row_stats_bf16: the statistics pitch is below M");
   const int parts = D / 64;
   const long long total = static_cast<long long>(M) * parts;
-  row_stats_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(X, ldx, reinterpret_cast<float2*>(stats), M, parts);
+  row_stats_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(X, ldx, reinterpret_cast<float2*>(stats), M, parts,
+                                                                             pitch > 0 ? pitch : M);
   VB_LAUNCHED();
 }
 
@@ -1400,6 +1454,7 @@ void dwconv_qkv(const T* x, int ldx, const float* stats, const float* gamma, con
   template void broadcast_rows<T>(const float*, T*, int, int, int, cudaStream_t);                                           \
   template void unfold_same<float, T>(const float*, T*, int, int, int, int, int, int, int, int, cudaStream_t, int, const UnfoldMode*); \
   template void window_rows<T>(const T*, int, T*, int, int, const Window&, long long, bool, cudaStream_t);                   \
+  template void r2l_rows<T>(const T*, int, T*, int, int, const Window&, long long, bool, cudaStream_t);                      \
   template void convert_rows<float, T>(const float*, int, T*, int, long long, int, cudaStream_t);                           \
   template void maxpool_relu_same<T>(const T*, T*, int, int, int, int, int, int, const float*, int, cudaStream_t);         \
   template void nest_pool<T>(const T*, int, const NestPoolLn*, int, int, int, int, bool, const float*, int, int, T*, int, float*,   \

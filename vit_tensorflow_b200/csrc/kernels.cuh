@@ -93,13 +93,16 @@ void broadcast_rows(const float* vec, T* dst, int B, int nt, int D, cudaStream_t
 // Twins-SVT's global to_kv (twins_svt.py:168,180), Conv2D(k, stride k, VALID) of the PreNorm LayerNorm of the map: `valid` takes
 // floor((H - k) / stride) + 1 windows per side with no padding, and `stats` applies the LayerNorm on load from the pixels' (sum,
 // sumsq) partials [C_pitch/64][B*H*W] (the GEMM epilogue's stats_out format) over d true channels with eps, times gamma plus beta.
-// A folded LayerNorm cannot serve this GEMM: one patch row spans k^2 pixels with different statistics.
+// A folded LayerNorm cannot serve this GEMM: one patch row spans k^2 pixels with different statistics.  `gelu`: the exact-erf
+// GELU of every loaded value, after the LayerNorm when there is one (RegionViT's 3-conv local tokenizer, regionvit.py:211-218);
+// padded taps stay zero.
 struct UnfoldMode {
   bool valid = false;
   const float* stats = nullptr;
   int parts = 0, d = 0;
   float eps = 1e-5f;
   const float *gamma = nullptr, *beta = nullptr;
+  bool gelu = false;
 };
 template <typename TI, typename TO>
 void unfold_same(const TI* in, TO* out, int B, int H, int W, int C, int k, int stride, int cls_row, int ldo, cudaStream_t s, int ldi = 0,
@@ -110,6 +113,10 @@ void unfold_same(const TI* in, TO* out, int B, int H, int W, int C, int k, int s
 // columns of `rows` = (number of windows) * p^2 rows.
 template <typename T>
 void window_rows(const T* in, int ldi, T* out, int ldo, int cols, const Window& win, long long rows, bool to_window, cudaStream_t s);
+// The same for RegionViT's regional-to-local windows (the fallback of attention_r2l): window-major row t = bw * n + i, n = 1 +
+// p * width(), is the regional row reg_row0 + bw for i == 0 and the map's row win.row(bw, i - 1) otherwise; win.count windows.
+template <typename T>
+void r2l_rows(const T* in, int ldi, T* out, int ldo, int cols, const Window& win, long long reg_row0, bool to_window, cudaStream_t s);
 
 // CCT tokenizer tail (cct.py:196-200,213): ReLU -> MaxPool2D(k, stride, padding 'SAME') -> 'b h w c -> b (h w) c', NHWC.
 // in [B, H, W, C] -> out [B, rows, C], oh = ceil(H / stride), rows >= oh * ow; total padding max((oh-1)*stride + k - H, 0) with
@@ -163,8 +170,9 @@ void pad_heads_f32(const float* W, float* Wp, int other, int groups, int heads, 
 void ln_fold_consts(const float* W, const __nv_bfloat16* Wt, int ldw, const float* beta, const float* bias, float* c1, float* c2,
                     int K, int N, cudaStream_t s);
 // stats[c, m] = (sum, sum of squares) of X[m, 64c .. 64c+63]  ([D/64][M] float2: the format the GEMM epilogue emits and the
-// LayerNorm-folded GEMM's statistics warp reduces); D % 64 == 0
-void row_stats_bf16(const __nv_bfloat16* X, int ldx, float* stats, int M, int D, cudaStream_t s);
+// LayerNorm-folded GEMM's statistics warp reduces); D % 64 == 0.  pitch > 0: stats[c * pitch + m] instead, for rows that are
+// the tail of a longer statistics buffer (RegionViT's regional rows after the local ones).
+void row_stats_bf16(const __nv_bfloat16* X, int ldx, float* stats, int M, int D, cudaStream_t s, long long pitch = 0);
 
 long long launch_counter();      // number of kernel launches issued through these wrappers (process-wide)
 void count_launch(int n = 1);

@@ -9,6 +9,7 @@
     TwinsSVT  vit_tensorflow/twins_svt.py:215-268
     CrossFormer  vit_tensorflow/crossformer.py:205-269
     NesT      vit_tensorflow/nest.py:150-216
+    RegionViT vit_tensorflow/regionvit.py:184-263
 
 Same constructor kwargs, defaults and assertion messages; `model(img, training=True, **kwargs) -> logits`
 with `img` NHWC float32 `[b, H, W, 3]` and logits float32 `[b, num_classes]`.  Everything below the call is
@@ -1387,8 +1388,147 @@ class NesT(_EngineModel):
 NEST_CTOR_KEYS = ("image_size", "patch_size", "num_classes", "dim", "heads", "num_hierarchies", "block_repeats", "mlp_mult", "dropout")
 
 
+def regionvit_maps(h, w, local_patch_size, window_size):
+    """The (local, region) map sides of every RegionViT stage for an h x w image: the local encoder's SAME stride 4 (or two SAME
+    stride 2) gives ceil(h / 4), the region encoder h // (local_patch_size * window_size), each Downsample ceil(. / 2)."""
+    p = local_patch_size * window_size
+    lh, lw, rh, rw = -(-h // 4), -(-w // 4), h // p, w // p
+    maps = []
+    for s in range(4):
+        if s:
+            lh, lw, rh, rw = -(-lh // 2), -(-lw // 2), -(-rh // 2), -(-rw // 2)
+        maps.append(((lh, lw), (rh, rw)))
+    return maps
+
+
+def regionvit_size_error(h, w, local_patch_size, window_size):
+    """The shape rules the reference enforces after its call-time asserts (regionvit.py:163-168 through einops and the concat,
+    :153 through the Embedding lookup) for an h x w image: None, or what the first stage that breaks one says."""
+    for s, ((lh, lw), (rh, rw)) in enumerate(regionvit_maps(h, w, local_patch_size, window_size), 1):
+        where = f"RegionViT stage {s}: the {lh} x {lw} local map and the {rh} x {rw} region map "
+        if lh < rh or lw < rw or lh % rh or lw % rw:
+            return where + "do not make whole windows (the local map must be the region map times the window)"
+        if lh // rh > window_size or lw // rw > window_size:
+            return (where + f"make {lh // rh} x {lw // rw} windows, larger than window_size {window_size} (the relative-position "
+                    "table's reach)")
+    return None
+
+
+class RegionViT(_EngineModel):
+    """regionvit.py:184-263: local tokens from Conv2D(dim[0], 8, 4, SAME) (or the 3-conv tokenizer: Conv3x3 s2, LayerNorm, GELU,
+    Conv3x3 s2, LayerNorm, GELU, Conv3x3), regional tokens from 'b (h p1) (w p2) c -> b h w (c p1 p2)' (p = local_patch_size *
+    window_size) and a 1x1 Conv2D; per stage s the shared Downsample Conv2D(dim[s], 3, 2, SAME) of both maps (s >= 1), the PEG
+    of the local map (s >= 1 with use_peg), then depth[s] R2L layers: the regional tokens attend among themselves, then every
+    lh/rh x lw/rw window of local tokens attends together with its regional token under the window's relative-position bias,
+    then the MLP; one Attention module (4 heads of 32) serves both attentions.  Head: the mean over the regional tokens,
+    LayerNorm, Dense.  Every LayerNorm is Keras's (eps 1e-3).
+
+    One handle runs any image the reference runs: sides divisible by the region patch size (the reference's assert messages) and,
+    at every stage, a local map that is a whole number of windows of at most window_size x window_size tokens per regional
+    token; other sizes raise ValueError naming the stage.  attn_dropout builds no layer in the reference and changes nothing;
+    with ff_dropout > 0 only training=False runs.  Weights (SURVEY.md App. B) keep the reference's attribute paths:
+    local_encoder[.{0,1,3,4,6}], region_encoder.1, region_layers.{s}.{0.conv|1.proj|2.local_rel_pos_bias},
+    region_layers.{s}.2.layers.{l}.0.{norm, to_qkv, to_out}, ....1.net.{0,1,4}, to_logits.{1,2}."""
+    _kind = "regionvit"
+
+    def __init__(self,
+                 dim=(64, 128, 256, 512),
+                 depth=(2, 2, 8, 2),
+                 window_size=7,
+                 num_classes=1000,
+                 tokenize_local_3_conv=False,
+                 local_patch_size=4,
+                 use_peg=False,
+                 attn_dropout=0.0,
+                 ff_dropout=0.0,
+                 *, precision="bf16", device=0, seed=None):
+        dim = _cast_tuple(dim, 4)                         # regionvit.py:197-200
+        depth = _cast_tuple(depth, 4)
+        assert len(dim) == 4, 'dim needs to be a single value or a tuple of length 4'
+        assert len(depth) == 4, 'depth needs to be a single value or a tuple of length 4'
+        self.dims, self.depths = tuple(int(d) for d in dim), tuple(int(d) for d in depth)
+        self.window_size, self.local_patch_size = window_size, local_patch_size
+        self.region_patch_size = local_patch_size * window_size
+        self.tokenize_local_3_conv, self.use_peg = bool(tokenize_local_3_conv), bool(use_peg)
+        self.num_classes = num_classes
+        self._dropout_rates = (ff_dropout,)               # Attention never builds its Dropout (:80-91)
+        self.precision = precision
+        self.device = int(device)
+        cfg = _lib.VbConfig()
+        cfg.struct_size = C.sizeof(_lib.VbConfig)
+        cfg.kind = _lib.KIND["regionvit"]
+        if precision not in _lib.PRECISION:
+            raise ValueError(f"precision must be one of {sorted(_lib.PRECISION)}")
+        cfg.precision = _lib.PRECISION[precision]
+        cfg.channels, cfg.num_classes = 3, num_classes
+        cfg.dim = self.dims[-1]
+        rc = _lib.VbRegionvitConfig()
+        rc.struct_size = C.sizeof(_lib.VbRegionvitConfig)
+        for i in range(4):
+            rc.dims[i], rc.depth[i] = self.dims[i], self.depths[i]
+        rc.window_size, rc.local_patch_size = window_size, local_patch_size
+        rc.tokenize_local_3_conv, rc.use_peg, rc.mlp_mult = int(self.tokenize_local_3_conv), int(self.use_peg), 4
+        self._cfg, self._rc = cfg, rc
+        self._lib = _lib.load()
+        h = C.c_void_p()
+        _lib.check(self._lib.vb_create_regionvit(C.byref(cfg), C.byref(rc), self.device, C.byref(h)))
+        self._h = h
+        self._finalized = False
+        self._specs = collections.OrderedDict()
+        name, shape, ndim = C.c_char_p(), (C.c_int64 * 4)(), C.c_int32()
+        for i in range(self._lib.vb_num_weights(h)):
+            _lib.check(self._lib.vb_weight_info(h, i, C.byref(name), shape, C.byref(ndim)), h)
+            self._specs[name.value.decode()] = tuple(int(shape[j]) for j in range(ndim.value))
+        self._weights = collections.OrderedDict()
+        self.init_weights(seed)
+
+    def init_weights(self, seed=None):
+        """Keras's initialisers: glorot-uniform over the receptive field for every Conv2D and Dense kernel (the depthwise PEG's
+        fan-in is its 9 taps), zero biases, LayerNorm gamma 1 / beta 0, the Embedding U(-0.05, 0.05)."""
+        rng = np.random.default_rng(seed)
+        w = collections.OrderedDict()
+        for name, shape in self._specs.items():
+            leaf = name.rsplit(".", 1)[-1]
+            if leaf == "kernel":
+                receptive = int(np.prod(shape[:-2]))
+                lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
+                a = rng.uniform(-lim, lim, size=shape)
+            elif leaf in ("bias", "beta"):
+                a = np.zeros(shape)
+            elif leaf == "gamma":
+                a = np.ones(shape)
+            elif leaf == "embeddings":
+                a = rng.uniform(-0.05, 0.05, size=shape)
+            else:
+                raise AssertionError(name)
+            w[name] = a.astype(np.float32)
+        self.set_weights_dict(w)
+
+    def __call__(self, x, training=True, **kwargs):
+        """regionvit.py:249-263: NHWC float images -> logits [b, num_classes]; extra kwargs are accepted and ignored, as there."""
+        a = np.asarray(x)
+        if a.ndim == 4:
+            h, w = a.shape[1], a.shape[2]
+            assert h % self.region_patch_size == 0 and w % self.region_patch_size == 0, \
+                'height and width must be divisible by region patch size'
+            assert h % self.local_patch_size == 0 and w % self.local_patch_size == 0, \
+                'height and width must be divisible by local patch size'
+            err = regionvit_size_error(h, w, self.local_patch_size, self.window_size)
+            if err is not None:
+                raise ValueError(err)
+        return super().__call__(x, training=training)
+
+    call = __call__
+
+
+REGIONVIT_CTOR_KEYS = ("dim", "depth", "window_size", "num_classes", "tokenize_local_3_conv", "local_patch_size", "use_peg",
+                       "attn_dropout", "ff_dropout")
+
+
 def from_config(cfg: dict, precision="bf16", device=0, seed=None):
     """Build a model from an oracle-style config dict (kind + reference kwargs)."""
+    if cfg["kind"] == "regionvit":
+        return RegionViT(**{k: v for k, v in cfg.items() if k in REGIONVIT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "nest":
         return NesT(**{k: v for k, v in cfg.items() if k in NEST_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "crossformer":
