@@ -140,8 +140,9 @@ enum Act { ACT_NONE = 0, ACT_GELU = 1, ACT_HSWISH = 2 };
 // epilogue: (+bias[n]) -> (activation) -> (*scale[n]) -> (+res[m,n]); out bf16.
 struct GemmBf16 {
   CUtensorMap tmap_a, tmap_b;           // A, B (weights)
+  CUtensorMap tmap_out = {}, tmap_res = {};   // bf16 out and res, which the epilogue stores and loads by TMA
   int M = 0, N = 0, K = 0;
-  __nv_bfloat16* out = nullptr;         // [M, ldc] (the epilogue stores rows straight from registers)
+  __nv_bfloat16* out = nullptr;         // [M, ldc] (fp32: stored straight from the accumulator registers)
   int ldc = 0;
   bool out_f32 = false;                 // `out` is float* (ldc in floats): plain / bias epilogue only
   const float* bias = nullptr;          // [N] or null

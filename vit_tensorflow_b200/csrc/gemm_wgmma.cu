@@ -9,16 +9,21 @@
 //
 // Structure: persistent, one CTA of 384 threads per SM; CTA b computes the 128 x 128 output tiles b, b + gridDim.x, ...
 // of the flat tile order (n fastest).
-//   producer        warpgroup 0 (its registers handed to the consumers by setmaxnreg); one thread streams the A (128 x 64)
+//   producer        warpgroup 0 (its registers handed to the consumers by setmaxnreg).  Thread 0 streams the A (128 x 64)
 //                   and B (128 x 64) k-blocks of the CTA's tiles, one tile after the other, into a STAGES-deep ring of
-//                   128B-swizzled tiles (mbarrier full / empty pairs).
+//                   128B-swizzled tiles (mbarrier full / empty pairs).  Warps 1-3 prepare each tile's epilogue operands
+//                   ahead of it, in the buffers of the consumer warpgroup that will run it: the residual tile (TMA load into
+//                   the warpgroup's output staging tile), the bias / ln_c1 / scale of its columns and the folded
+//                   LayerNorm's (rstd, -mu rstd) of its rows (mbarrier epi_full / epi_empty pair per warpgroup).
 //   2 consumer warpgroups, ping-pong: warpgroup w computes the CTA's tiles i = w (mod 2), each whole: two wgmma
 //                   m64 x 128 x 16 per k16 step (rows 0-63 and 64-127 of the tile) into register accumulators, one k-block
-//                   in flight while the previous one's stage is released; then the epilogue straight from the accumulator
-//                   registers (bias / folded LayerNorm / GELU / LayerScale / residual, bf16 or fp32 stores, optional
-//                   per-64-column row statistics of the stored values).  Two named barriers pass the main loop from one
-//                   warpgroup to the other, so the main loops take turns on the tensor cores and one tile's epilogue
-//                   runs under the next tile's main loop.
+//                   in flight while the previous one's stage is released; then the epilogue from the accumulator
+//                   registers (bias / folded LayerNorm / GELU / LayerScale / residual, optional per-64-column row
+//                   statistics of the stored values), reading its operands from shared memory only.  A bf16 tile is
+//                   written into the staging tile (over its residual) and leaves by two TMA stores of 64 x 128; an fp32
+//                   tile is stored straight from registers.  Two named barriers pass the main loop from one warpgroup to
+//                   the other, so the main loops take turns on the tensor cores and one tile's epilogue runs under the
+//                   next tile's main loop.
 #include "common.h"
 #include "kernels.cuh"
 #include "ptx.cuh"
@@ -34,9 +39,13 @@ constexpr int THREADS = 384;
 constexpr int A_BYTES = BM * BK * 2;
 constexpr int B_BYTES = BN * BK * 2;
 constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr int STAGES = 6;          // 6 x 32 KB of the 227 KB a CTA may use
-constexpr int COLS_BYTES = 2 * 3 * BN * 4;   // per consumer warpgroup: bias, ln_c1 and scale of its tile's columns
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 /*barriers*/ + COLS_BYTES + 1024 /*align*/;
+constexpr int STAGES = 4;          // 4 x 32 KB ring + 2 x 32 KB output staging of the 227 KB a CTA may use
+constexpr int HALF_BYTES = BM * 64 * 2;      // 64 columns of an output tile: 128 rows of 128 bytes, 128B-swizzled
+constexpr int STG_BYTES = 2 * HALF_BYTES;    // per consumer warpgroup: its bf16 output tile (and residual tile before it)
+constexpr int PARAM_FLOATS = 3 * BN + 2 * BM;   // per consumer warpgroup: bias, ln_c1, scale of its tile's columns; the
+                                                // folded LayerNorm's rstd and -mu rstd of its rows
+constexpr int EPI_THREADS = 96;    // producer warps 1-3
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * STG_BYTES + 256 /*barriers*/ + 2 * PARAM_FLOATS * 4 + 1024 /*align*/;
 static_assert(SMEM_BYTES <= 227 * 1024, "ring does not fit in shared memory");
 
 // Exact-erf GELU (vit.py:34), written as  gelu(x) = x/2 - |x| * (E(|x|) - 1/2),  E(a) = erfc(a/sqrt2) / 2  (for x > 0
@@ -69,16 +78,22 @@ __device__ __forceinline__ void ring_advance(int& stage, uint32_t& phase, int n)
 // EPI: 0 = no per-column addend, 1 = + bias[n], 2 = folded LayerNorm (c1 = ln_c1, c2 = bias)
 template <int ACT, bool RES, int EPI, bool OF32>
 __global__ void __launch_bounds__(THREADS, 1)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, int M, int N, int K,
-                 void* __restrict__ out, int ldc, const float* __restrict__ bias, const float* __restrict__ scale,
-                 const __nv_bfloat16* res, int ldr, const float* __restrict__ ln_c1, const float2* ln_stats, int ln_parts,
-                 float ln_inv_d, float ln_eps, float2* __restrict__ stats_out) {
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                 const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_res, int M, int N, int K,
+                 float* __restrict__ out_f32, int ldc, const float* __restrict__ bias, const float* __restrict__ scale,
+                 const float* __restrict__ ln_c1, const float2* ln_stats, int ln_parts, float ln_inv_d, float ln_eps,
+                 float2* __restrict__ stats_out) {
   static_assert(!OF32 || (ACT == ACT_NONE && !RES && EPI != 2), "fp32 output: plain / bias epilogue only");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + STAGES * STAGE_BYTES;
+  const uint32_t stg_base = smem_base + STAGES * STAGE_BYTES;     // consumer warpgroup w's staging tile at + w STG_BYTES
+  const uint32_t bar_base = stg_base + 2 * STG_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  auto epi_full = [&](int w) { return bar_base + 8u * (2 * STAGES + w); };        // warpgroup w's epilogue operands staged
+  auto epi_empty = [&](int w) { return bar_base + 8u * (2 * STAGES + 2 + w); };   // ... and consumed (staging tile stored)
+  uint8_t* const smem = smem_raw + (smem_base - smem_u32(smem_raw));
+  float* const params = reinterpret_cast<float*>(smem + (bar_base + 256 - smem_base));   // [2][PARAM_FLOATS]
 
   const int wg = threadIdx.x >> 7;
   const int tid = threadIdx.x & 127;
@@ -91,9 +106,15 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
+    if (!OF32) tma_prefetch_desc(&tmap_out);
+    if (RES) tma_prefetch_desc(&tmap_res);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), 1);                                  // released by the warpgroup that consumed the stage
+    }
+    for (int w = 0; w < 2; ++w) {
+      mbar_init(epi_full(w), EPI_THREADS);
+      mbar_init(epi_empty(w), 1);                                  // thread 0 of the consumer warpgroup
     }
     fence_mbar_init();
   }
@@ -120,6 +141,61 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
+    } else if (tid >= 32) {
+      // ------------------------------------------------------------------- epilogue operands of the CTA's tiles, in order:
+      // tile i goes to consumer warpgroup w = i % 2 as soon as that warpgroup's tile i - 2 has left its buffers, i.e.
+      // while the other warpgroup runs tile i - 1's main loop, well before tile i's epilogue needs them
+      const int pt = tid - 32;
+      int i = 0;
+      for (long long t = blockIdx.x; t < tiles; t += gridDim.x, ++i) {
+        const int w = i & 1;
+        const int n0 = static_cast<int>(t % n_tiles) * BN;
+        const int m0 = static_cast<int>(t / n_tiles) * BM;
+        mbar_wait(epi_empty(w), ((i >> 1) & 1) ^ 1);
+        if (RES && pt == 0) {
+          // rows >= M are zero-filled; N % 64 == 0, so a 64-column half is entirely in or out
+          const int halves = N - n0 >= BN ? 2 : 1;
+          const uint32_t stg = stg_base + w * STG_BYTES;
+          fence_proxy_async_smem();
+          mbar_expect_tx(epi_full(w), halves * HALF_BYTES);
+          for (int c = 0; c < halves; ++c) tma_load_2d(stg + c * HALF_BYTES, &tmap_res, epi_full(w), n0 + 64 * c, m0);
+        }
+        float* const par = params + w * PARAM_FLOATS;
+        for (int c = pt; c < BN; c += EPI_THREADS) {
+          float b = 0.f, c1 = 0.f, s = 1.f;
+          if (n0 + c < N) {
+            if (EPI >= 1) b = __ldg(bias + n0 + c);
+            if (EPI == 2) c1 = __ldg(ln_c1 + n0 + c);
+            if (scale != nullptr) s = __ldg(scale + n0 + c);
+          }
+          par[c] = b;
+          par[BN + c] = c1;
+          par[2 * BN + c] = s;
+        }
+        // folded LayerNorm of the A operand: y = rstd * acc + (-rstd * mu) * c1[n] + c2[n]   (c2 arrives through `bias`); the
+        // rows' statistics arrive as `ln_parts` (sum, sumsq) partials [part][M], reduced in a fixed order
+        if (EPI == 2) {
+          for (int r = pt; r < BM; r += EPI_THREADS) {
+            const int m = m0 + r;
+            float rstd = 0.f, nmr = 0.f;
+            if (m < M) {
+              float s1 = 0.f, s2 = 0.f;
+#pragma unroll 4
+              for (int p = 0; p < ln_parts; ++p) {
+                const float2 v = __ldg(ln_stats + static_cast<size_t>(p) * M + m);
+                s1 += v.x;
+                s2 += v.y;
+              }
+              const float mu = s1 * ln_inv_d;
+              rstd = rsqrtf(fmaxf(fmaf(s2, ln_inv_d, -__fmul_rn(mu, mu)), 0.f) + ln_eps);
+              nmr = -mu * rstd;
+            }
+            par[3 * BN + r] = rstd;
+            par[3 * BN + BM + r] = nmr;
+          }
+        }
+        mbar_arrive(epi_full(w));
+      }
     }
     return;
   }
@@ -132,55 +208,20 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   // Named barrier 1 + w: warpgroup w waits there for its turn at the main loop, which the other warpgroup hands over
   // (bar.arrive) when it has issued its own.  The turns alternate, so the ring's k-blocks are consumed in the order the
   // producer fills them and a warpgroup never waits on a stage more than one ring lap ahead of the producer.
-  const uint32_t my_turn = 1 + cw, other_turn = 2 - cw, cols_ready = 3 + cw;
-  // The tile's per-column epilogue parameters, staged in shared memory: loaded before the main loop, so the epilogue
-  // does not wait on a global load for every 8 columns.
-  float* cols = reinterpret_cast<float*>(smem_raw + (bar_base + 256 - smem_u32(smem_raw))) + cw * 3 * BN;
+  const uint32_t my_turn = 1 + cw, other_turn = 2 - cw, epi_done = 3 + cw;
+  const float* const par = params + cw * PARAM_FLOATS;
+  uint8_t* const stg = smem + STAGES * STAGE_BYTES + cw * STG_BYTES;
+  const int row_l = warp * 16 + (lane >> 2);                       // this thread's accumulator rows in the tile: row_l +
+                                                                   // 64 hm + 8 h, q = 2 hm + h below; all = lane / 4 (mod 8)
   int stage = 0;
-  uint32_t phase = 0;
+  uint32_t phase = 0, epi_phase = 0;
   ring_advance(stage, phase, cw * num_kb);                         // warpgroup 1 starts after tile 0's k-blocks
 
   for (long long t = blockIdx.x + static_cast<long long>(cw) * gridDim.x; t < tiles; t += 2LL * gridDim.x) {
     const int n0 = static_cast<int>(t % n_tiles) * BN;
     const int m0 = static_cast<int>(t / n_tiles) * BM;
-    const int row_a = m0 + warp * 16 + (lane >> 2);                // this thread's accumulator rows: row_a + 64 hm + 8 h,
-                                                                   // q = 2 hm + h below
 
-    // folded LayerNorm of the A operand: y = rstd * acc + (-rstd * mu) * c1[n] + c2[n]   (c2 arrives through `bias`); the
-    // rows' statistics arrive as `ln_parts` (sum, sumsq) partials [part][M], reduced here in a fixed order while the other
-    // warpgroup runs its main loop
-    float ln_rstd[4] = {0.f, 0.f, 0.f, 0.f}, ln_nmr[4] = {0.f, 0.f, 0.f, 0.f};   // rows row_a + 64 (q / 2) + 8 (q % 2)
-    if (EPI == 2) {
-      float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll 4
-      for (int i = 0; i < ln_parts; ++i)                           // the four rows' loads in flight together
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int r = row_a + 64 * (q >> 1) + 8 * (q & 1);
-          if (r < M) {
-            const float2 v = __ldg(ln_stats + static_cast<size_t>(i) * M + r);
-            s1[q] += v.x;
-            s2[q] += v.y;
-          }
-        }
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float mu = s1[q] * ln_inv_d;
-        const float rstd = rsqrtf(fmaxf(s2[q] * ln_inv_d - mu * mu, 0.f) + ln_eps);
-        ln_rstd[q] = rstd;
-        ln_nmr[q] = -mu * rstd;
-      }
-    }
-
-    float col_b = 0.f, col_c1 = 0.f, col_s = 1.f;
-    if (n0 + tid < N) {
-      if (EPI >= 1) col_b = __ldg(bias + n0 + tid);
-      if (EPI == 2) col_c1 = __ldg(ln_c1 + n0 + tid);
-      if (scale != nullptr) col_s = __ldg(scale + n0 + tid);
-    }
-
-    // the CTA's first tile starts at once; for the others, this also means the warpgroup's previous epilogue is done
-    // with `cols`
+    // the CTA's first tile starts at once
     if (cw == 1 || t != blockIdx.x) named_bar_sync(my_turn, 256);
     float acc[2][64];                                              // [64-row half of the tile][wgmma fragment]
 #pragma unroll
@@ -212,40 +253,35 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     wgmma_fence_operand(acc[1]);
     if (tid == 0) mbar_arrive(empty_bar(stage == 0 ? STAGES - 1 : stage - 1));
     ring_advance(stage, phase, num_kb);                            // skip the other warpgroup's tile
-    cols[tid] = col_b;
-    cols[BN + tid] = col_c1;
-    cols[2 * BN + tid] = col_s;
-    named_bar_sync(cols_ready, 128);
 
     // =================================================================== epilogue, 64-column chunks
+    mbar_wait(epi_full(cw), epi_phase);                            // operands (and residual tile) staged by warps 1-3
+    epi_phase ^= 1;
+    float ln_rstd[4] = {0.f, 0.f, 0.f, 0.f}, ln_nmr[4] = {0.f, 0.f, 0.f, 0.f};   // rows row_l + 64 (q / 2) + 8 (q % 2)
+    if (EPI == 2) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        ln_rstd[q] = par[3 * BN + row_l + 64 * (q >> 1) + 8 * (q & 1)];
+        ln_nmr[q] = par[3 * BN + BM + row_l + 64 * (q >> 1) + 8 * (q & 1)];
+      }
+    }
 #pragma unroll
     for (int c = 0; c < BN / 64; ++c) {
       const int nc = n0 + c * 64;
       if (nc >= N) break;                                          // N % 64 == 0: a chunk is entirely in or out
       float st1[4] = {0.f, 0.f, 0.f, 0.f}, st2[4] = {0.f, 0.f, 0.f, 0.f};   // (sum, sumsq) of the stored bf16 outputs, per row
-      // The chunk's residuals, all loaded before its first store: one memory round trip instead of one per store.  `res`
-      // may alias `out`; each element is still read before it is written, by the thread that writes it.
-      uint32_t rw[8][4];
-      if (RES) {
-#pragma unroll
-        for (int jj = 0; jj < 8; ++jj)
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int r = row_a + 64 * (q >> 1) + 8 * (q & 1);
-            rw[jj][q] = r < M ? *reinterpret_cast<const uint32_t*>(res + static_cast<size_t>(r) * ldr + nc + jj * 8 + col_t) : 0u;
-          }
-      }
+      uint8_t* const half = stg + c * HALF_BYTES;
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj) {
         const int j = c * 8 + jj;
         const int n = nc + jj * 8 + col_t;
         float cb0 = 0.f, cb1 = 0.f, c10 = 0.f, c11 = 0.f, sc0 = 1.f, sc1 = 1.f;
-        if (EPI >= 1) { const float2 b2 = *reinterpret_cast<const float2*>(cols + (n - n0)); cb0 = b2.x; cb1 = b2.y; }
-        if (EPI == 2) { const float2 c2 = *reinterpret_cast<const float2*>(cols + BN + (n - n0)); c10 = c2.x; c11 = c2.y; }
-        if (scale != nullptr) { const float2 s2 = *reinterpret_cast<const float2*>(cols + 2 * BN + (n - n0)); sc0 = s2.x; sc1 = s2.y; }
+        if (EPI >= 1) { const float2 b2 = *reinterpret_cast<const float2*>(par + (n - n0)); cb0 = b2.x; cb1 = b2.y; }
+        if (EPI == 2) { const float2 c2 = *reinterpret_cast<const float2*>(par + BN + (n - n0)); c10 = c2.x; c11 = c2.y; }
+        if (scale != nullptr) { const float2 s2 = *reinterpret_cast<const float2*>(par + 2 * BN + (n - n0)); sc0 = s2.x; sc1 = s2.y; }
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
-          const int r = row_a + 64 * (q >> 1) + 8 * (q & 1);
+          const int rl = row_l + 64 * (q >> 1) + 8 * (q & 1);
           float v0 = acc[q >> 1][4 * j + 2 * (q & 1)], v1 = acc[q >> 1][4 * j + 2 * (q & 1) + 1];
           if (EPI == 2) {
             v0 = fmaf(v0, ln_rstd[q], fmaf(c10, ln_nmr[q], cb0));
@@ -258,16 +294,21 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           if (ACT == ACT_HSWISH) { v0 = hard_swish(v0); v1 = hard_swish(v1); }
           // rounded on its own, as the reference's LayerScale is, never fused with the residual add into one FMA
           if (scale != nullptr) { v0 = __fmul_rn(v0, sc0); v1 = __fmul_rn(v1, sc1); }
-          if (r >= M) continue;
-          if (RES) {
-            v0 += bf16_lo(rw[jj][q]);
-            v1 += bf16_hi(rw[jj][q]);
-          }
           if (OF32) {
-            *reinterpret_cast<float2*>(static_cast<float*>(out) + static_cast<size_t>(r) * ldc + n) = make_float2(v0, v1);
+            if (m0 + rl < M)
+              *reinterpret_cast<float2*>(out_f32 + static_cast<size_t>(m0 + rl) * ldc + n) = make_float2(v0, v1);
           } else {
+            // the staging tile in TMA's 128B-swizzled layout: 16-byte chunk jj of row rl at chunk jj ^ (rl % 8), so the
+            // 8 rows x 4 lanes of a warp's access hit 32 distinct banks.  The residual (zero in rows >= M, which the store
+            // clips) is read here and overwritten by the output, by the same thread.
+            uint32_t* const p = reinterpret_cast<uint32_t*>(half + rl * 128 + ((jj ^ (lane >> 2)) << 4) + 4 * (lane & 3));
+            if (RES) {
+              const uint32_t rw = *p;
+              v0 += bf16_lo(rw);
+              v1 += bf16_hi(rw);
+            }
             const uint32_t pk = pack_bf16x2(v0, v1);
-            *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(out) + static_cast<size_t>(r) * ldc + n) = pk;
+            *p = pk;
             if (stats_out != nullptr) {
               const float a0 = bf16_lo(pk), a1 = bf16_hi(pk);
               st1[q] += a0 + a1;
@@ -283,12 +324,28 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           st2[q] += __shfl_xor_sync(0xffffffffu, st2[q], 1);
           st1[q] += __shfl_xor_sync(0xffffffffu, st1[q], 2);
           st2[q] += __shfl_xor_sync(0xffffffffu, st2[q], 2);
-          const int r = row_a + 64 * (q >> 1) + 8 * (q & 1);
+          const int r = m0 + row_l + 64 * (q >> 1) + 8 * (q & 1);
           if ((lane & 3) == 0 && r < M) stats_out[static_cast<size_t>(nc >> 6) * M + r] = make_float2(st1[q], st2[q]);   // [part][M]
         }
       }
     }
+    // The staged bf16 tile leaves by TMA (rows >= M clipped); once it has been read out, the buffers go back to warps 1-3.
+    // `res` may alias `out`: the tile's residual was loaded before this store, and no other tile touches these elements.
+    if (!OF32) fence_proxy_async_smem();
+    named_bar_sync(epi_done, 128);
+    if (tid == 0) {
+      if (!OF32) {
+        const uint32_t s = stg_base + cw * STG_BYTES;
+        tma_store_2d(&tmap_out, s, n0, m0);
+        if (n0 + 64 < N) tma_store_2d(&tmap_out, s + HALF_BYTES, n0 + 64, m0);
+        bulk_commit_group();
+        bulk_wait_group_read<0>();
+      }
+      mbar_arrive(epi_empty(cw));
+    }
   }
+  // the CTA's stores are complete before it exits: a dependent kernel's griddepcontrol.wait waits for the grid's exit only
+  if (!OF32 && tid == 0) bulk_wait_group<0>();
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -322,9 +379,10 @@ void launch(const GemmBf16& g, cudaStream_t stream) {
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  VB_CUDA(cudaLaunchKernelEx(&cfg, kern, g.tmap_a, g.tmap_b, g.M, g.N, g.K, static_cast<void*>(g.out), g.ldc, g.bias, g.scale, g.res,
-                             g.ldr, g.ln_c1, reinterpret_cast<const float2*>(g.ln_stats), g.ln_parts, g.ln_inv_d,
-                             g.ln_eps, reinterpret_cast<float2*>(g.stats_out)));
+  VB_CUDA(cudaLaunchKernelEx(&cfg, kern, g.tmap_a, g.tmap_b, g.tmap_out, g.tmap_res, g.M, g.N, g.K,
+                             OF32 ? reinterpret_cast<float*>(g.out) : nullptr, g.ldc, g.bias, g.scale, g.ln_c1,
+                             reinterpret_cast<const float2*>(g.ln_stats), g.ln_parts, g.ln_inv_d, g.ln_eps,
+                             reinterpret_cast<float2*>(g.stats_out)));
   count_launch();
 }
 
@@ -387,6 +445,9 @@ GemmBf16 gemm_bf16_plan(const __nv_bfloat16* A, int lda, const __nv_bfloat16* Wt
   g.tmap_a = make_tmap_2d(A, K, M, static_cast<uint64_t>(lda) * 2, BK, BM);
   // b_rows: rows of Wt that exist (< N when the output is column-padded: TMA zero-fills the rest instead of reading on)
   g.tmap_b = make_tmap_2d(Wt, K, b_rows > 0 ? b_rows : N, static_cast<uint64_t>(ldw) * 2, BK, BN);
+  // bf16 output and residual tiles move as 64-column halves; TMA clips the store and zero-fills the load past row M
+  if (!out_f32) g.tmap_out = make_tmap_2d(out, N, M, static_cast<uint64_t>(ldc) * 2, 64, BM);
+  if (res != nullptr) g.tmap_res = make_tmap_2d(res, N, M, static_cast<uint64_t>(ldr) * 2, 64, BM);
   return g;
 }
 
