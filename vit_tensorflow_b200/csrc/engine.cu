@@ -146,11 +146,13 @@ struct LevitBlockW {
 // One CvT Transformer layer (cvt.py:142-147) on channel rows zero-padded to dp (bf16) / dim (fp32).  The depthwise convolutions
 // carry their BatchNormalization folded (taps [k*k][dp] scaled, plus a per-channel shift); the MLP's PreNorm is folded into fc1
 // in the bf16 engine.
+struct MlpW { Norm norm; Linear fc1, fc2; };   // PreNorm MLP: LayerNorm, fc1, GELU, fc2
 struct CvtBlockW {
   int dim = 0, dp = 0, heads = 0, k = 0, kv_stride = 1;
-  Norm attn_norm, ff_norm;           // gamma / beta [dp], zero on pad channels
+  Norm attn_norm;                    // gamma / beta [dp], zero on pad channels
   const float *wq = nullptr, *bq = nullptr, *wkv = nullptr, *bkv = nullptr;
-  Linear pw_q, pw_kv, to_out, fc1, fc2;
+  Linear pw_q, pw_kv, to_out;
+  MlpW ff;
 };
 struct CvtStageW {                   // cvt.py:186-192: Conv2D (SAME, bias) + LayerNorm + Transformer
   int dim = 0, dp = 0, k = 0, stride = 1;
@@ -177,7 +179,6 @@ inline void cvt_fold_dw(const std::vector<double>& taps, const std::vector<doubl
 // One Twins-SVT Transformer layer (twins_svt.py:192-213) on channel rows zero-padded to dp (bf16) / dim (fp32): x = x + f(LN(x))
 // for local attention, MLP, global attention, MLP; stage 4 has no local attention and no first MLP (has_local=False, :255).  The
 // bf16 engine folds the PreNorm LayerNorms of the fused local q|k|v, the global to_q and the fc1s into those GEMMs.
-struct MlpW { Norm norm; Linear fc1, fc2; };   // PreNorm MLP (Twins-SVT, CrossFormer): LayerNorm eps 1e-5, fc1, GELU, fc2
 struct TwinsLayerW {
   bool local = false;
   Norm local_norm, global_norm;      // gamma / beta [dp], zero on pad channels
@@ -1199,74 +1200,89 @@ struct vb_handle {
     if (!bias.empty()) woverride[key + ".bias"] = upload_owned(bias);
     return make_linear(key, K, N, !bias.empty(), fold);
   }
-  // ---- CvT weight packing: channel widths zero-padded (bf16), BatchNormalizations folded into the depthwise taps and a shift
-  Norm padded_norm(const std::string& n, int d, int dp) {        // CvT's LayerNorm g / b [1, 1, 1, d] -> [dp]
-    return Norm{upload_owned(pad_n(host_weight(n + ".g"), dp)), upload_owned(pad_n(host_weight(n + ".b"), dp)), d};
+  // The Dense (or Conv2D as a Dense) `name`: its kernel [K, N] as the top-left block of a zero [Kp, Np], its bias (when it has one)
+  // padded to Np, packed under `key`.  With `fold`: that LayerNorm (true width K, epsilon eps) folded in by the bf16 engine.
+  Linear padded_dense(const std::string& key, const std::string& name, int K, int N, int Kp, int Np, const Norm* fold = nullptr,
+                      float eps = 1e-5f) {
+    const std::vector<double> bias = has(name + ".bias") ? pad_n(host_weight(name + ".bias"), Np) : std::vector<double>();
+    Linear L = linear_from_host(key, pad_kn(host_weight(name + ".kernel"), K, N, Kp, Np), bias, Kp, Np, bf16() ? fold : nullptr);
+    if (fold != nullptr) { L.ln_d = K; L.ln_eps = eps; }
+    return L;
   }
+  // A LayerNorm's gamma / beta [d] (leaves `g` / `b`: the models' own LayerNorm, or Keras' gamma / beta) zero-padded to [dp]
+  Norm padded_norm(const std::string& n, int d, int dp, const char* g = ".g", const char* b = ".b") {
+    return Norm{upload_owned(pad_n(host_weight(n + g), dp)), upload_owned(pad_n(host_weight(n + b), dp)), d};
+  }
+  // 'b (h p1) (w p2) c -> b h w (c p1 p2)': the reference's kernel row c p^2 + p1 p + p2 [.., d] is unfold_same's row (p1 p + p2) cin + c
+  static std::vector<double> patch_rows_channel_last(const std::vector<double>& wr, int cin, int p, int d) {
+    std::vector<double> wp(wr.size());
+    for (int c = 0; c < cin; ++c)
+      for (int t = 0; t < p * p; ++t)
+        std::copy(wr.begin() + static_cast<size_t>(c * p * p + t) * d, wr.begin() + static_cast<size_t>(c * p * p + t + 1) * d,
+                  wp.begin() + static_cast<size_t>(t * cin + c) * d);
+    return wp;
+  }
+  // PEG: x + dw(x) + b is one depthwise k x k convolution whose centre tap ((k-1)/2, (k-1)/2) has 1 added (TF SAME at stride 1 pads
+  // (k-1)/2 on the top / left, so that tap reads the pixel itself).  taps [k*k][d] -> [k*k][dp]
+  const float* peg_taps(const std::vector<double>& taps, int k, int d, int dp) {
+    std::vector<double> pw(static_cast<size_t>(k) * k * dp, 0.0);
+    const int centre = ((k - 1) / 2) * k + (k - 1) / 2;
+    for (int t = 0; t < k * k; ++t)
+      for (int c = 0; c < d; ++c) pw[static_cast<size_t>(t) * dp + c] = taps[static_cast<size_t>(t) * d + c] + (t == centre ? 1.0 : 0.0);
+    return upload_owned(pw);
+  }
+  // ---- CvT weight packing: channel widths zero-padded (bf16), BatchNormalizations folded into the depthwise taps and a shift
   void finalize_cvt() {
     for (int st = 0; st < VB_CVT_STAGES; ++st) {
       CvtStageW S;
       const std::string p = cvt_pre(st);
       const int d = cv.emb_dim[st], dp = channel_width(d), ke = cv.emb_kernel[st], K = ke * ke * cvt_cin(st);
       S.dim = d; S.dp = dp; S.k = ke; S.stride = cv.emb_stride[st];
-      S.conv = linear_from_host("cvt." + p + "0", pad_kn(host_weight(p + "0.kernel"), K, d, K, dp), pad_n(host_weight(p + "0.bias"), dp), K, dp);
+      S.conv = padded_dense("cvt." + p + "0", p + "0", K, d, K, dp);
       S.norm = padded_norm(p + "1", d, dp);
-      const int inner = 64 * cv.heads[st], hidden = d * cv.mlp_mult[st], hp = channel_width(hidden), k = cv.proj_kernel[st];
+      const int inner = 64 * cv.heads[st], k = cv.proj_kernel[st];
       for (int L = 0; L < cv.depth[st]; ++L) {
         const std::string b = p + "2.layers." + std::to_string(L) + ".", key = "cvt." + b;
         CvtBlockW w;
         w.dim = d; w.dp = dp; w.heads = cv.heads[st]; w.k = k; w.kv_stride = cv.kv_proj_stride[st];
         w.attn_norm = padded_norm(b + "0.norm", d, dp);
-        w.ff_norm = padded_norm(b + "1.norm", d, dp);
         for (int kv = 0; kv < 2; ++kv) {
           const std::string n = b + (kv ? "0.fn.to_kv.net." : "0.fn.to_q.net.");
           std::vector<double> taps, shift;
           cvt_fold_dw(host_weight(n + "0.kernel"), host_weight(n + "1.gamma"), host_weight(n + "1.beta"), host_weight(n + "1.moving_mean"),
                       host_weight(n + "1.moving_variance"), k, d, dp, taps, shift);
           const int N = (kv ? 2 : 1) * inner;
-          Linear pw = linear_from_host(key + (kv ? "pw_kv" : "pw_q"), pad_kn(host_weight(n + "2.kernel"), d, N, dp, N), {}, dp, N);
+          Linear pw = padded_dense(key + (kv ? "pw_kv" : "pw_q"), n + "2", d, N, dp, N);
           if (kv) { w.wkv = upload_owned(taps); w.bkv = upload_owned(shift); w.pw_kv = pw; }
           else { w.wq = upload_owned(taps); w.bq = upload_owned(shift); w.pw_q = pw; }
         }
-        const std::string o = b + "0.fn.to_out.0", m0 = b + "1.fn.net.0", m3 = b + "1.fn.net.3";
-        w.to_out = linear_from_host(key + "to_out", pad_kn(host_weight(o + ".kernel"), inner, d, inner, dp), pad_n(host_weight(o + ".bias"), dp),
-                                    inner, dp);
-        w.fc1 = linear_from_host(key + "fc1", pad_kn(host_weight(m0 + ".kernel"), d, hidden, dp, hp), pad_n(host_weight(m0 + ".bias"), hp), dp, hp,
-                                 bf16() ? &w.ff_norm : nullptr);
-        w.fc1.ln_d = d;
-        w.fc1.ln_eps = 1e-5f;
-        w.fc2 = linear_from_host(key + "fc2", pad_kn(host_weight(m3 + ".kernel"), hidden, d, hp, dp), pad_n(host_weight(m3 + ".bias"), dp), hp, dp);
+        w.to_out = padded_dense(key + "to_out", b + "0.fn.to_out.0", inner, d, inner, dp);
+        w.ff = prenorm_mlp("cvt.", b + "1.norm", b + "1.fn.net.0", b + "1.fn.net.3", d, dp, cv.mlp_mult[st]);
         S.blocks.push_back(std::move(w));
       }
       cvt_stages.push_back(std::move(S));
     }
     head = make_linear_f32("cvt_layers.3.1", cv.emb_dim[VB_CVT_STAGES - 1], cfg.num_classes);
   }
-  // ---- Twins-SVT weight packing: channel widths zero-padded (bf16), the patch kernel's rows permuted, the PEG residual folded
-  // A PreNorm MLP of width mult * d: the LayerNorm `norm` (g / b), the Dense layers n0 (d -> mult d) and n3 (mult d -> d) as 1x1
-  // Conv2D kernels, widths padded, the LayerNorm folded into fc1 in the bf16 engine.  key: the packed copies' own names.
+  // A PreNorm MLP of width mult * d: the LayerNorm `norm` (leaves g / b, epsilon eps), the Dense layers n0 (d -> mult d) and n3
+  // (mult d -> d), widths padded, the LayerNorm folded into fc1 in the bf16 engine.  key: the packed copies' own names.
   MlpW prenorm_mlp(const std::string& key, const std::string& norm, const std::string& n0, const std::string& n3, int d, int dp,
-                   int mult = 4) {
+                   int mult = 4, float eps = 1e-5f, const char* g = ".g", const char* b = ".b") {
     MlpW w;
     const int hidden = mult * d, hp = channel_width(hidden);
-    w.norm = padded_norm(norm, d, dp);
-    w.fc1 = linear_from_host(key + n0, pad_kn(host_weight(n0 + ".kernel"), d, hidden, dp, hp), pad_n(host_weight(n0 + ".bias"), hp), dp,
-                             hp, bf16() ? &w.norm : nullptr);
-    w.fc1.ln_d = d;
-    w.fc1.ln_eps = 1e-5f;
-    w.fc2 = linear_from_host(key + n3, pad_kn(host_weight(n3 + ".kernel"), hidden, d, hp, dp), pad_n(host_weight(n3 + ".bias"), dp), hp, dp);
+    w.norm = padded_norm(norm, d, dp, g, b);
+    w.fc1 = padded_dense(key + n0, n0, d, hidden, dp, hp, &w.norm, eps);
+    w.fc2 = padded_dense(key + n3, n3, hidden, d, hp, dp);
     return w;
   }
+  // ---- Twins-SVT weight packing: channel widths zero-padded (bf16), the patch kernel's rows permuted, the PEG residual folded
   MlpW twins_mlp(const std::string& m, int d, int dp) {
     return prenorm_mlp("twins.", m + ".fn.norm", m + ".fn.fn.net.0", m + ".fn.fn.net.3", d, dp);
   }
   TwinsLayerW twins_layer_weights(const std::string& b, int st, int d, int dp) {
     TwinsLayerW w;
     const int I = kTwinsInner, kg = tw.global_k[st];
-    auto folded = [&](Linear L) { L.ln_d = d; L.ln_eps = 1e-5f; return L; };   // twins_svt.py:46: eps 1e-5
-    auto to_out = [&](const std::string& n) {
-      return linear_from_host("twins." + n, pad_kn(host_weight(n + ".kernel"), I, d, I, dp), pad_n(host_weight(n + ".bias"), dp), I, dp);
-    };
+    auto to_out = [&](const std::string& n) { return padded_dense("twins." + n, n, I, d, I, dp); };
     w.local = st < VB_TWINS_STAGES - 1;
     if (w.local) {
       w.local_norm = padded_norm(b + "0.fn.norm", d, dp);
@@ -1277,13 +1293,14 @@ struct vb_handle {
         std::copy(kv.begin() + static_cast<size_t>(r) * 2 * I, kv.begin() + static_cast<size_t>(r + 1) * 2 * I,
                   qkv.begin() + static_cast<size_t>(r) * 3 * I + I);
       }
-      w.qkv = folded(linear_from_host("twins." + b + "0.qkv", pad_kn(qkv, d, 3 * I, dp, 3 * I), {}, dp, 3 * I, bf16() ? &w.local_norm : nullptr));
+      w.qkv = linear_from_host("twins." + b + "0.qkv", pad_kn(qkv, d, 3 * I, dp, 3 * I), {}, dp, 3 * I, bf16() ? &w.local_norm : nullptr);
+      w.qkv.ln_d = d;
+      w.qkv.ln_eps = 1e-5f;                                          // twins_svt.py:46
       w.local_out = to_out(b + "0.fn.fn.to_out.0");
       w.ff1 = twins_mlp(b + "1", d, dp);
     }
     w.global_norm = padded_norm(b + "2.fn.norm", d, dp);
-    w.to_q = folded(linear_from_host("twins." + b + "2.to_q", pad_kn(host_weight(b + "2.fn.fn.to_q.kernel"), d, I, dp, I), {}, dp, I,
-                                     bf16() ? &w.global_norm : nullptr));
+    w.to_q = padded_dense("twins." + b + "2.to_q", b + "2.fn.fn.to_q", d, I, dp, I, &w.global_norm);
     // [kg, kg, d, 2I] is the Dense [kg*kg*d, 2I] over unfold_same's (row, column, channel) vectors of the true d channels
     w.to_kv = linear_from_host("twins." + b + "2.to_kv", host_weight(b + "2.fn.fn.to_kv.kernel"), {}, kg * kg * d, 2 * I);
     w.global_out = to_out(b + "2.fn.fn.to_out.0");
@@ -1296,23 +1313,9 @@ struct vb_handle {
       const std::string p = twins_pre(st);
       const int d = tw.emb_dim[st], dp = channel_width(d), ps = tw.patch_size[st], cin = twins_cin(st), K = ps * ps * cin, k = tw.peg_kernel_size;
       S.dim = d; S.dp = dp; S.patch = ps; S.local = tw.local_patch_size[st]; S.global_k = tw.global_k[st]; S.peg_k = k;
-      // 'b (h p1) (w p2) c -> b h w (c p1 p2)' (twins_svt.py:103): the reference's row c * p^2 + p1 * p + p2 is unfold_same's
-      // row (p1 * p + p2) * cin + c
-      const auto wr = host_weight(p + "0.proj.kernel");
-      std::vector<double> wp(static_cast<size_t>(K) * d);
-      for (int c = 0; c < cin; ++c)
-        for (int t = 0; t < ps * ps; ++t)
-          std::copy(wr.begin() + static_cast<size_t>(c * ps * ps + t) * d, wr.begin() + static_cast<size_t>(c * ps * ps + t + 1) * d,
-                    wp.begin() + static_cast<size_t>(t * cin + c) * d);
+      const auto wp = patch_rows_channel_last(host_weight(p + "0.proj.kernel"), cin, ps, d);   // twins_svt.py:103
       S.proj = linear_from_host("twins." + p + "0.proj", pad_kn(wp, K, d, K, dp), pad_n(host_weight(p + "0.proj.bias"), dp), K, dp);
-      // PEG (:108-115): x + dw(x) + b is one depthwise convolution whose centre tap ((k-1)/2, (k-1)/2) has 1 added (TF SAME at
-      // stride 1 pads (k-1)/2 on the top / left, so that tap reads the pixel itself)
-      const auto taps = host_weight(p + "2.proj.fn.kernel");
-      std::vector<double> pw(static_cast<size_t>(k) * k * dp, 0.0);
-      const int centre = ((k - 1) / 2) * k + (k - 1) / 2;
-      for (int t = 0; t < k * k; ++t)
-        for (int c = 0; c < d; ++c) pw[static_cast<size_t>(t) * dp + c] = taps[static_cast<size_t>(t) * d + c] + (t == centre ? 1.0 : 0.0);
-      S.peg_w = upload_owned(pw);
+      S.peg_w = peg_taps(host_weight(p + "2.proj.fn.kernel"), k, d, dp);                      // PEG (:108-115)
       S.peg_b = upload_owned(pad_n(host_weight(p + "2.proj.fn.bias"), dp));
       for (int t : {1, 3})
         for (int L = 0; L < (t == 1 ? 1 : tw.depth[st]); ++L)
@@ -1370,8 +1373,7 @@ struct vb_handle {
     w.qkv = linear_from_host("cf." + a + "qkv", pad_kn(qkv, d, key_n, dp, N), {}, dp, N, bf16() ? &w.norm : nullptr);
     w.qkv.ln_d = d;
     w.qkv.ln_eps = 1e-5f;                                          // crossformer.py:74
-    w.to_out = linear_from_host("cf." + a + "to_out", pad_kn(host_weight(a + "to_out.kernel"), I, d, I, dp), pad_n(host_weight(a + "to_out.bias"), dp),
-                                I, dp);
+    w.to_out = padded_dense("cf." + a + "to_out", a + "to_out", I, d, I, dp);
     return w;
   }
   void finalize_crossformer() {
@@ -1417,8 +1419,7 @@ struct vb_handle {
   void finalize_nest() {
     const int K0 = ns.patch_size * ns.patch_size * cfg.channels, dp0 = channel_width(ns.dim), dh = ns.dim / ns.heads;
     // 'b (h p1) (w p2) c -> b h w (p1 p2 c)' (nest.py:179) is unfold_same's (p1, p2, c) order: the kernel's rows as they are
-    nest_patch = linear_from_host("nest.patch", pad_kn(host_weight("patch_embedding.1.kernel"), K0, ns.dim, K0, dp0),
-                                  pad_n(host_weight("patch_embedding.1.bias"), dp0), K0, dp0);
+    nest_patch = padded_dense("nest.patch", "patch_embedding.1", K0, ns.dim, K0, dp0);
     for (int i = 0; i < ns.levels; ++i) {
       NestLevelW V;
       const std::string p = nest_pre(i);
@@ -1430,13 +1431,9 @@ struct vb_handle {
         const std::string b = p + "0.layers." + std::to_string(L) + ".", key = "nest." + b;
         NestBlockW w;
         w.attn_norm = padded_norm(b + "0.norm", d, dp);
-        w.qkv = linear_from_host(key + "qkv", pad_kn(host_weight(b + "0.fn.to_qkv.kernel"), d, 3 * I, dp, N), {}, dp, N,
-                                 bf16() ? &w.attn_norm : nullptr);
-        w.qkv.ln_d = d;
-        w.qkv.ln_eps = 1e-5f;                                        // nest.py:29
+        w.qkv = padded_dense(key + "qkv", b + "0.fn.to_qkv", d, 3 * I, dp, N, &w.attn_norm);   // nest.py:29: eps 1e-5
         // to_out reads the attention output in place of q: K rows [I, Ko) meet k / v columns and are zero
-        w.to_out = linear_from_host(key + "to_out", pad_kn(host_weight(b + "0.fn.to_out.0.kernel"), I, d, Ko, dp),
-                                    pad_n(host_weight(b + "0.fn.to_out.0.bias"), dp), Ko, dp);
+        w.to_out = padded_dense(key + "to_out", b + "0.fn.to_out.0", I, d, Ko, dp);
         w.ff = prenorm_mlp("nest.", b + "1.norm", b + "1.fn.net.0", b + "1.fn.net.3", d, dp, ns.mlp_mult);
         V.blocks.push_back(std::move(w));
       }
@@ -1445,8 +1442,7 @@ struct vb_handle {
         const int dn = nest_dim(i + 1), dpn = channel_width(dn);
         V.dim_out = dn; V.dp_out = dpn;
         // [3, 3, d, dn] is the Dense [9 d, dn] over unfold_same's (row, column, channel) vectors of the true d channels
-        V.agg = linear_from_host("nest." + p + "1.conv", pad_kn(host_weight(p + "1.ag_layers.0.kernel"), 9 * d, dn, 9 * d, dpn),
-                                 pad_n(host_weight(p + "1.ag_layers.0.bias"), dpn), 9 * d, dpn);
+        V.agg = padded_dense("nest." + p + "1.conv", p + "1.ag_layers.0", 9 * d, dn, 9 * d, dpn);
         V.agg_norm = padded_norm(p + "1.ag_layers.1", dn, dpn);
       }
       nest_levels.push_back(std::move(V));
@@ -1456,63 +1452,40 @@ struct vb_handle {
   }
   // ---- RegionViT weight packing: channel widths zero-padded (bf16), the region kernel's rows permuted, the PEG residual folded,
   // every Attention / MLP LayerNorm (Keras, eps 1e-3) folded into q|k|v / fc1 in the bf16 engine, the window tables transposed
-  Norm rv_norm(const std::string& n, int d, int dp) {
-    return Norm{upload_owned(pad_n(host_weight(n + ".gamma"), dp)), upload_owned(pad_n(host_weight(n + ".beta"), dp)), d};
-  }
-  Linear rv_conv(const std::string& n, int K, int d, int dp) {     // a Conv2D kernel [kh, kw, cin, d] is the Dense [kh kw cin, d]
-    return linear_from_host("rv." + n, pad_kn(host_weight(n + ".kernel"), K, d, K, dp), pad_n(host_weight(n + ".bias"), dp), K, dp);
-  }
   void finalize_regionvit() {
     const int C = cfg.channels, d0 = rv.dims[0], dp0 = channel_width(d0), p = rv_region_patch(), ws = rv.window_size;
     if (rv.tokenize_local_3_conv) {
-      for (int i = 0; i < 3; ++i) rv_local[i] = rv_conv("local_encoder." + std::to_string(3 * i), 9 * (i == 0 ? C : d0), d0, dp0);
-      for (int i = 0; i < 2; ++i) rv_local_norm[i] = rv_norm("local_encoder." + std::to_string(3 * i + 1), d0, dp0);
+      for (int i = 0; i < 3; ++i) {
+        const std::string n = "local_encoder." + std::to_string(3 * i);
+        const int K = 9 * (i == 0 ? C : d0);
+        rv_local[i] = padded_dense("rv." + n, n, K, d0, K, dp0);
+      }
+      for (int i = 0; i < 2; ++i) rv_local_norm[i] = padded_norm("local_encoder." + std::to_string(3 * i + 1), d0, dp0, ".gamma", ".beta");
     } else {
-      rv_local[0] = rv_conv("local_encoder", 64 * C, d0, dp0);
+      rv_local[0] = padded_dense("rv.local_encoder", "local_encoder", 64 * C, d0, 64 * C, dp0);
     }
-    // 'b (h p1) (w p2) c -> b h w (c p1 p2)' (regionvit.py:224): the reference's row c p^2 + p1 p + p2 is unfold_same's row
-    // (p1 p + p2) C + c
-    {
-      const auto wr = host_weight("region_encoder.1.kernel");
-      const int K = C * p * p;
-      std::vector<double> wp(static_cast<size_t>(K) * d0);
-      for (int c = 0; c < C; ++c)
-        for (int t = 0; t < p * p; ++t)
-          std::copy(wr.begin() + static_cast<size_t>(c * p * p + t) * d0, wr.begin() + static_cast<size_t>(c * p * p + t + 1) * d0,
-                    wp.begin() + static_cast<size_t>(t * C + c) * d0);
-      rv_region = linear_from_host("rv.region_encoder", pad_kn(wp, K, d0, K, dp0), pad_n(host_weight("region_encoder.1.bias"), dp0), K, dp0);
-    }
+    const int K = C * p * p;                                             // regionvit.py:224
+    rv_region = linear_from_host("rv.region_encoder", pad_kn(patch_rows_channel_last(host_weight("region_encoder.1.kernel"), C, p, d0), K, d0, K, dp0),
+                                 pad_n(host_weight("region_encoder.1.bias"), dp0), K, dp0);
     for (int s = 0; s < VB_REGIONVIT_STAGES; ++s) {
       RegionStageW S;
       const std::string pre = rv_pre(s);
-      const int d = rv.dims[s], dp = channel_width(d), hidden = d * rv.mlp_mult, hp = channel_width(hidden);
+      const int d = rv.dims[s], dp = channel_width(d);
       S.dim = d; S.dp = dp; S.down = s > 0; S.peg = s > 0 && rv.use_peg;
-      if (S.down) S.down_conv = rv_conv(pre + "0.conv", 9 * rv.dims[s - 1], d, dp);
-      if (S.peg) {       // x + dw(x) + b: the depthwise 3x3 with 1 added to its centre tap (TF SAME pads 1 at stride 1)
-        const auto taps = host_weight(pre + "1.proj.kernel");
-        std::vector<double> pw(static_cast<size_t>(9) * dp, 0.0);
-        for (int t = 0; t < 9; ++t)
-          for (int c = 0; c < d; ++c) pw[static_cast<size_t>(t) * dp + c] = taps[static_cast<size_t>(t) * d + c] + (t == 4 ? 1.0 : 0.0);
-        S.peg_w = upload_owned(pw);
+      if (S.down) S.down_conv = padded_dense("rv." + pre + "0.conv", pre + "0.conv", 9 * rv.dims[s - 1], d, 9 * rv.dims[s - 1], dp);
+      if (S.peg) {                                                      // :54-61, the residual folded
+        S.peg_w = peg_taps(host_weight(pre + "1.proj.kernel"), 3, d, dp);
         S.peg_b = upload_owned(pad_n(host_weight(pre + "1.proj.bias"), dp));
       }
       S.table = upload_owned(r2l_table_from_embedding(host_weight(pre + "2.local_rel_pos_bias.embeddings").data(), ws, kRvHeads));
       for (int L = 0; L < rv.depth[s]; ++L) {
         const std::string b = pre + "2.layers." + std::to_string(L) + ".", key = "rv." + b;
         RegionLayerW w;
-        w.attn_norm = rv_norm(b + "0.norm", d, dp);
-        w.qkv = linear_from_host(key + "qkv", pad_kn(host_weight(b + "0.to_qkv.kernel"), d, 3 * kRvInner, dp, 3 * kRvInner), {}, dp,
-                                 3 * kRvInner, bf16() ? &w.attn_norm : nullptr);
-        w.qkv.ln_d = d;
+        w.attn_norm = padded_norm(b + "0.norm", d, dp, ".gamma", ".beta");
+        w.qkv = padded_dense(key + "qkv", b + "0.to_qkv", d, 3 * kRvInner, dp, 3 * kRvInner, &w.attn_norm, 1e-3f);
         // to_out reads the attention output in place of q: its K is the inner width, the rows' pitch is that of q|k|v
-        w.to_out = linear_from_host(key + "to_out", pad_kn(host_weight(b + "0.to_out.kernel"), kRvInner, d, kRvInner, dp),
-                                    pad_n(host_weight(b + "0.to_out.bias"), dp), kRvInner, dp);
-        w.ff.norm = rv_norm(b + "1.net.0", d, dp);
-        w.ff.fc1 = linear_from_host(key + "fc1", pad_kn(host_weight(b + "1.net.1.kernel"), d, hidden, dp, hp),
-                                    pad_n(host_weight(b + "1.net.1.bias"), hp), dp, hp, bf16() ? &w.ff.norm : nullptr);
-        w.ff.fc1.ln_d = d;
-        w.ff.fc2 = linear_from_host(key + "fc2", pad_kn(host_weight(b + "1.net.4.kernel"), hidden, d, hp, dp),
-                                    pad_n(host_weight(b + "1.net.4.bias"), dp), hp, dp);
+        w.to_out = padded_dense(key + "to_out", b + "0.to_out", kRvInner, d, kRvInner, dp);
+        w.ff = prenorm_mlp("rv.", b + "1.net.0", b + "1.net.1", b + "1.net.4", d, dp, rv.mlp_mult, 1e-3f, ".gamma", ".beta");
         S.layers.push_back(std::move(w));
       }
       rv_stages.push_back(std::move(S));
@@ -1527,8 +1500,7 @@ struct vb_handle {
     for (int i = 0; i < 4; ++i) {                                       // stem; the 32-channel map is written 64 wide (zero columns)
       const std::string n = "conv_embedding." + std::to_string(i);
       const int cout = levit_stem_cout(i), np = i == 0 ? 64 : channel_width(cout), K = 9 * cin;
-      lv_stem.push_back(linear_from_host("levit." + n, pad_kn(host_weight(n + ".kernel"), K, cout, K, np),
-                                         pad_n(host_weight(n + ".bias"), np), K, np));
+      lv_stem.push_back(padded_dense("levit." + n, n, K, cout, K, np));
       cin = cout;
     }
     for (const auto& p : levit_plan()) {
@@ -1574,11 +1546,8 @@ struct vb_handle {
       b.scale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(dk)));
       b.pos = upload_owned(levit_pos_table(host_weight(a + "pos_bias.embeddings"), p.fmap * p.fmap, H, dk));
       const int hidden = p.dim_out * p.mult, hp = channel_width(hidden);
-      const std::string m0 = p.pre + "1.net.0", m3 = p.pre + "1.net.3";
-      b.fc1 = linear_from_host(key + "fc1", pad_kn(host_weight(m0 + ".kernel"), p.dim_out, hidden, dpo, hp), pad_n(host_weight(m0 + ".bias"), hp),
-                               dpo, hp);
-      b.fc2 = linear_from_host(key + "fc2", pad_kn(host_weight(m3 + ".kernel"), hidden, p.dim_out, hp, dpo), pad_n(host_weight(m3 + ".bias"), dpo),
-                               hp, dpo);
+      b.fc1 = padded_dense(key + "fc1", p.pre + "1.net.0", p.dim_out, hidden, dpo, hp);
+      b.fc2 = padded_dense(key + "fc2", p.pre + "1.net.3", hidden, p.dim_out, hp, dpo);
       lv_blocks.push_back(std::move(b));
     }
     const int dl = lv.dims[lv.stages - 1];
@@ -1660,7 +1629,7 @@ struct vb_handle {
     T* X = arena.get<T>(static_cast<size_t>(M) * e.dim);
     Epi ep; ep.bias = e.patch.bias; ep.res = R; ep.ldr = e.dim;
     if (stats_out != nullptr && bf16() && e.dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr) {
-      *stats_out = arena.get<float>(static_cast<size_t>(M) * (e.dim / 64) * 2);
+      *stats_out = row_stats(M, e.dim);
       ep.stats_out = *stats_out;
     }
     Linear L = e.patch;
@@ -1714,19 +1683,10 @@ struct vb_handle {
     T* out = nullptr;
     int mh = H, mw = Wd, mc = c.channels;
     for (int i = 0; i < c.cct_conv_layers; ++i) {
-      const Linear& conv = cct_convs[i];
-      const int oh = (mh + c.cct_stride - 1) / c.cct_stride, ow = (mw + c.cct_stride - 1) / c.cct_stride;
-      const int M = B * oh * ow, Kp = bf16() ? conv.ldw : conv.K;
-      T* col = arena.get<T>(static_cast<size_t>(M) * Kp);
-      {
-        ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(i == 0 ? 4 : sizeof(T)) * B * mh * mw * mc + static_cast<double>(sizeof(T)) * M * Kp, s);
-        if (i == 0) unfold_same<float, T>(img, col, B, mh, mw, mc, c.cct_kernel, c.cct_stride, 0, Kp, s);
-        else unfold_same<T, T>(map, col, B, mh, mw, mc, c.cct_kernel, c.cct_stride, 0, Kp, s);
-      }
-      T* conv_out = arena.get<T>(static_cast<size_t>(M) * conv.N);
-      Linear L = conv;
-      L.K = Kp;
-      linear<T>(col, Kp, M, L, conv_out, conv.N, Epi(), s);
+      const Linear& cw = cct_convs[i];
+      const int oh = (mh + c.cct_stride - 1) / c.cct_stride, ow = (mw + c.cct_stride - 1) / c.cct_stride, M = B * oh * ow;
+      T* conv_out = arena.get<T>(static_cast<size_t>(M) * cw.N);
+      conv<T>(img, map, mc, B, mh, mw, mc, c.cct_kernel, c.cct_stride, cw, conv_out, nullptr, s);   // bias-free
       const int ph = (oh + c.cct_pool_stride - 1) / c.cct_pool_stride, pw = (ow + c.cct_pool_stride - 1) / c.cct_pool_stride;
       int rows = ph * pw;
       const float* pos = nullptr;
@@ -1740,12 +1700,12 @@ struct vb_handle {
           rows = n_seq;                                                  // cct.py:278-280: zero rows up to sequence_length
         }
       }
-      out = arena.get<T>(static_cast<size_t>(B) * rows * conv.N);
+      out = arena.get<T>(static_cast<size_t>(B) * rows * cw.N);
       {
-        ProfScope ps(this, PROF_OTHER, 0.0, static_cast<double>(sizeof(T)) * (static_cast<double>(M) + static_cast<double>(B) * rows) * conv.N, s);
-        maxpool_relu_same<T>(conv_out, out, B, oh, ow, conv.N, c.cct_pool_kernel, c.cct_pool_stride, pos, rows, s);
+        ProfScope ps(this, PROF_OTHER, 0.0, static_cast<double>(sizeof(T)) * (static_cast<double>(M) + static_cast<double>(B) * rows) * cw.N, s);
+        maxpool_relu_same<T>(conv_out, out, B, oh, ow, cw.N, c.cct_pool_kernel, c.cct_pool_stride, pos, rows, s);
       }
-      map = out; mh = ph; mw = pw; mc = conv.N;
+      map = out; mh = ph; mw = pw; mc = cw.N;
       *rows_out = rows;
     }
     return out;
@@ -2084,8 +2044,7 @@ struct vb_handle {
     } else if (c.kind == VB_KIND_CCT) {                   // CCT.call cct.py:342-345, TransformerClassifier.call :277-305
       int rows = 0;
       T* X = tokenize_cct<T>(img, B, H, Wd, &rows, s);
-      float* stats = (bf16() && c.dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr)
-                         ? arena.get<float>(static_cast<size_t>(B) * rows * (c.dim / 64) * 2) : nullptr;
+      float* stats = c.dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr ? row_stats(static_cast<long long>(B) * rows, c.dim) : nullptr;
       bool sv = false;
       for (const auto& l : layers) layer_cct<T>(X, B, rows, c.dim, l, s, stats, &sv);
       float* z = arena.get<float>(static_cast<size_t>(B) * c.dim);
@@ -2093,8 +2052,7 @@ struct vb_handle {
         ProfScope ps(this, PROF_LN, 4.0 * B * rows * c.dim, static_cast<double>(sizeof(T)) * B * rows * c.dim, s);
         seq_pool<T>(X, rows, c.dim, cct_norm.gamma, cct_norm.beta, cct_pool_w, cct_pool_b, z, B, s);   // :291-299
       }
-      gemm_simt<float, float, float>(z, c.dim, head.W, head.N, 1, logits, head.N, B, head.N, c.dim, head.bias, nullptr, nullptr,
-                                     head.N, 0, s);                                                   // fc :303
+      dense_head(z, c.dim, head, B, logits, s);                                                         // fc :303
     } else {
       int ns = 0, nl = 0;
       float *st_s = nullptr, *st_g = nullptr;
@@ -2136,9 +2094,83 @@ struct vb_handle {
     }
   }
 
+  float* row_stats(long long M, int dp) {       // (sum, sumsq) partials per 64-column chunk of M rows: bf16 only
+    return bf16() ? arena.get<float>(static_cast<size_t>(M) * (dp / 64) * 2) : nullptr;
+  }
+  // A convolution as unfold_same + GEMM: the fp32 image (map == null, cin channels) or the first cin channels of the token map
+  // [B h w, ld], unfolded at the packed weight pitch (`um`: VALID, or the LayerNorm / GELU applied on load), then out [rows, L.N] =
+  // col W + b, with the output rows' statistics when stats_out is given
+  template <typename T>
+  void conv(const float* img, const T* map, int ld, int B, int h, int w, int cin, int k, int stride, const Linear& L, T* out,
+            float* stats_out, cudaStream_t s, const UnfoldMode* um = nullptr) {
+    const bool valid = um != nullptr && um->valid;
+    const int oh = valid ? (h - k) / stride + 1 : (h + stride - 1) / stride, ow = valid ? (w - k) / stride + 1 : (w + stride - 1) / stride;
+    const int rows = B * oh * ow, Kp = bf16() ? L.ldw : L.K;
+    T* col = arena.get<T>(static_cast<size_t>(rows) * Kp);
+    {
+      ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(map ? sizeof(T) : 4) * B * h * w * cin + static_cast<double>(sizeof(T)) * rows * Kp, s);
+      if (map == nullptr) unfold_same<float, T>(img, col, B, h, w, cin, k, stride, 0, Kp, s);
+      else unfold_same<T, T>(map, col, B, h, w, cin, k, stride, 0, Kp, s, ld, um);
+    }
+    Linear Lk = L;
+    Lk.K = Kp;                      // unfold_same zero-pads the patch vectors to the packed weight pitch
+    Epi e; e.bias = L.bias; e.stats_out = stats_out;
+    linear<T>(col, Kp, rows, Lk, out, L.N, e, s);
+  }
+  // The pre-norm sub-blocks x = f(LN(x)) + x over X [M, dp] (true width d).  bf16 folds the LayerNorm into f's first GEMM from
+  // the row statistics `stats`, which the residual epilogues keep current; fp32 runs it into the scratch Y first.
+  template <typename T>
+  struct PreNorm {
+    vb_handle& h;
+    T* X;
+    int M, d, dp;
+    float* stats;
+    float eps;
+    T* Y;                           // fp32 only
+    cudaStream_t s;
+    PreNorm rows(T* X0, int M0, float* st) const { PreNorm r = *this; r.X = X0; r.M = M0; r.stats = st; return r; }
+    const T* norm(const Norm& n) const {          // the A operand of the GEMM that folded_epi's Epi goes with
+      if (Y == nullptr) return X;
+      ProfScope ps(&h, PROF_LN, 8.0 * M * d, 2.0 * sizeof(T) * M * dp, s);
+      layernorm<T>(X, dp, n.gamma, n.beta, Y, dp, M, d, s, dp, eps);
+      return Y;
+    }
+    Epi folded_epi(const Linear& L) const {
+      Epi e;
+      if (Y == nullptr) { e.bias = L.ln_c2; e.ln_stats = stats; } else { e.bias = L.bias; }
+      return e;
+    }
+    void residual(const T* A, int lda, const Linear& L) const {   // X = A W + b + X, and X's new row statistics
+      Epi e; e.bias = L.bias; e.res = X; e.ldr = dp; e.stats_out = stats;
+      h.linear<T>(A, lda, M, L, X, dp, e, s);
+    }
+    void mlp(const MlpW& m) const {                               // X = fc2(GELU(fc1(LN(X)))) + X
+      const T* a = norm(m.norm);
+      T* Hb = h.arena.get<T>(static_cast<size_t>(M) * m.fc1.N);
+      Epi e1 = folded_epi(m.fc1);
+      e1.gelu = true;
+      h.linear<T>(a, dp, M, m.fc1, Hb, m.fc1.N, e1, s);
+      residual(Hb, m.fc1.N, m.fc2);
+    }
+  };
+  template <typename T>
+  PreNorm<T> prenorm(T* X, int M, int d, int dp, float* stats, float eps, cudaStream_t s) {
+    return PreNorm<T>{*this, X, M, d, dp, stats, eps, bf16() ? nullptr : arena.get<T>(static_cast<size_t>(M) * dp), s};
+  }
+  // The mean over each image's `rows` token rows [.., ld] of their first d columns -> z [B, d]
+  template <typename T>
+  float* mean_pool(const T* X, int rows, int ld, int d, int B, cudaStream_t s) {
+    float* z = arena.get<float>(static_cast<size_t>(B) * d);
+    ProfScope ps(this, PROF_LN, 1.0 * B * rows * d, static_cast<double>(sizeof(T)) * B * rows * d, s);
+    pool_layernorm<T>(X, rows, ld, nullptr, nullptr, z, B, d, 1, s);
+    return z;
+  }
+  void dense_head(const float* z, int d, const Linear& L, int B, float* out, cudaStream_t s) {   // fp32 Dense on pooled rows
+    gemm_simt<float, float, float>(z, d, L.W, L.N, 1, out, L.N, B, L.N, d, L.bias, nullptr, nullptr, L.N, 0, s);
+  }
+
   // LeViT.call (levit.py:214-226): stem -> backbone -> GlobalAvgPool2D -> mlp_head (and distill_head when distill != null).
   // The token rows of every block are the NHWC map, pixel-major: row b * fmap^2 + r * fmap + c.
-  static constexpr const char* kLevitNoStages = "LeViT runs as a whole forward only: its stem / backbone / head stages have no entry of their own";
   template <typename T>
   void levit_forward(const float* img, int B, int H, int Wd, float* logits, float* distill, cudaStream_t s) {
     const int fmap = cfg.image_h / 16;
@@ -2152,36 +2184,21 @@ struct vb_handle {
     const T* map = nullptr;
     T* X = nullptr;
     for (int i = 0; i < 4; ++i) {                                       // conv_embedding levit.py:187-192
-      const Linear& conv = lv_stem[i];
-      const int oh = (mh + 1) / 2, ow = (mw + 1) / 2, M = B * oh * ow, Kp = bf16() ? conv.ldw : conv.K;
-      T* col = arena.get<T>(static_cast<size_t>(M) * Kp);
-      {
-        ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(i == 0 ? 4 : sizeof(T)) * B * mh * mw * mc + static_cast<double>(sizeof(T)) * M * Kp, s);
-        if (i == 0) unfold_same<float, T>(img, col, B, mh, mw, mc, 3, 2, 0, Kp, s);
-        else unfold_same<T, T>(map, col, B, mh, mw, mc, 3, 2, 0, Kp, s, ld_in);
-      }
-      X = arena.get<T>(static_cast<size_t>(M) * conv.N);
-      Linear L = conv;
-      L.K = Kp;
-      Epi e; e.bias = conv.bias;
-      linear<T>(col, Kp, M, L, X, conv.N, e, s);
-      map = X; mh = oh; mw = ow; mc = levit_stem_cout(i); ld_in = conv.N;
+      const Linear& L = lv_stem[i];
+      const int oh = (mh + 1) / 2, ow = (mw + 1) / 2;
+      X = arena.get<T>(static_cast<size_t>(B) * oh * ow * L.N);
+      conv<T>(img, map, ld_in, B, mh, mw, mc, 3, 2, L, X, nullptr, s);
+      map = X; mh = oh; mw = ow; mc = levit_stem_cout(i); ld_in = L.N;
     }
     int f = fmap;
     for (const auto& b : lv_blocks) {
       X = levit_block<T>(X, B, b, s);
       f = (b.fmap + b.step - 1) / b.step;
     }
-    const int dl = lv.dims[lv.stages - 1], ldl = channel_width(dl);
-    float* z = arena.get<float>(static_cast<size_t>(B) * dl);
-    {
-      ProfScope ps(this, PROF_LN, 1.0 * B * f * f * dl, static_cast<double>(sizeof(T)) * B * f * f * dl, s);
-      pool_layernorm<T>(X, f * f, ldl, nullptr, nullptr, z, B, dl, 1, s);  // GlobalAvgPool2D (levit.py:206-208)
-    }
-    gemm_simt<float, float, float>(z, dl, head.W, head.N, 1, logits, head.N, B, head.N, dl, head.bias, nullptr, nullptr, head.N, 0, s);
-    if (distill != nullptr)
-      gemm_simt<float, float, float>(z, dl, lv_distill.W, lv_distill.N, 1, distill, lv_distill.N, B, lv_distill.N, dl, lv_distill.bias,
-                                     nullptr, nullptr, lv_distill.N, 0, s);
+    const int dl = lv.dims[lv.stages - 1];
+    const float* z = mean_pool<T>(X, f * f, channel_width(dl), dl, B, s);   // GlobalAvgPool2D (levit.py:206-208)
+    dense_head(z, dl, head, B, logits, s);
+    if (distill != nullptr) dense_head(z, dl, lv_distill, B, distill, s);
   }
   // One LeViT block (levit.py:156-162): x = attn(x) + (x if attn_residual else 0); x = mlp(x) + x.  X [B * fmap^2, dp] ->
   // [B * nq, dp_out] (a new buffer when the block shrinks the map, X updated in place otherwise); pad columns stay zero.
@@ -2234,7 +2251,6 @@ struct vb_handle {
 
   // CvT.call (cvt.py:182-202): per stage, Conv2D (SAME, bias) -> LayerNorm -> blocks; then GlobalAvgPool2D -> Dense.  Token rows
   // are the NHWC map, pixel-major, channel widths zero-padded to channel_width.  Any h x w: each SAME stride gives ceil.
-  static constexpr const char* kCvtNoStages = "CvT runs as a whole forward only: its stem / stage / head steps have no entry of their own";
   template <typename T>
   void cvt_forward(const float* img, int B, int H, int Wd, float* logits, cudaStream_t s) {
     int mh = H, mw = Wd, mc = cfg.channels, ld_in = 0;
@@ -2242,21 +2258,10 @@ struct vb_handle {
     T* X = nullptr;
     for (const CvtStageW& S : cvt_stages) {
       const int oh = (mh + S.stride - 1) / S.stride, ow = (mw + S.stride - 1) / S.stride, M = B * oh * ow;
-      const int Kp = bf16() ? S.conv.ldw : S.conv.K;
-      T* col = arena.get<T>(static_cast<size_t>(M) * Kp);
-      {
-        ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(map == nullptr ? 4 : sizeof(T)) * B * mh * mw * mc +
-                                                 static_cast<double>(sizeof(T)) * M * Kp, s);
-        if (map == nullptr) unfold_same<float, T>(img, col, B, mh, mw, mc, S.k, S.stride, 0, Kp, s);
-        else unfold_same<T, T>(map, col, B, mh, mw, mc, S.k, S.stride, 0, Kp, s, ld_in);
-      }
       T* Y = arena.get<T>(static_cast<size_t>(M) * S.dp);
-      Linear L = S.conv;
-      L.K = Kp;
-      Epi e; e.bias = S.conv.bias;
-      linear<T>(col, Kp, M, L, Y, S.dp, e, s);
+      conv<T>(img, map, ld_in, B, mh, mw, mc, S.k, S.stride, S.conv, Y, nullptr, s);
       X = arena.get<T>(static_cast<size_t>(M) * S.dp);
-      float* stats = bf16() ? arena.get<float>(static_cast<size_t>(M) * (S.dp / 64) * 2) : nullptr;
+      float* stats = row_stats(M, S.dp);
       {
         ProfScope ps(this, PROF_LN, 8.0 * M * S.dim, 2.0 * sizeof(T) * M * S.dp, s);
         layernorm<T>(Y, S.dp, S.norm.gamma, S.norm.beta, X, S.dp, M, S.dim, s, S.dp, 1e-5f);   // cvt.py:188
@@ -2266,12 +2271,7 @@ struct vb_handle {
       map = X; mh = oh; mw = ow; mc = S.dim; ld_in = S.dp;
     }
     const int dl = cv.emb_dim[VB_CVT_STAGES - 1];
-    float* z = arena.get<float>(static_cast<size_t>(B) * dl);
-    {
-      ProfScope ps(this, PROF_LN, 1.0 * B * mh * mw * dl, static_cast<double>(sizeof(T)) * B * mh * mw * dl, s);
-      pool_layernorm<T>(X, mh * mw, ld_in, nullptr, nullptr, z, B, dl, 1, s);   // GlobalAvgPool2D cvt.py:196
-    }
-    gemm_simt<float, float, float>(z, dl, head.W, head.N, 1, logits, head.N, B, head.N, dl, head.bias, nullptr, nullptr, head.N, 0, s);
+    dense_head(mean_pool<T>(X, mh * mw, ld_in, dl, B, s), dl, head, B, logits, s);   // GlobalAvgPool2D cvt.py:196
   }
   // One CvT layer (cvt.py:144-145): x = attn(LN(x)) + x; x = mlp(LN(x)) + x, in place on X [B*H*W, dp].  bf16: `stats` holds the
   // (sum, sumsq) partials of X's rows on entry and on exit (emitted by the residual epilogues), and the depthwise kernel and fc1
@@ -2282,15 +2282,12 @@ struct vb_handle {
     const int Ho = (H + st - 1) / st, Wo = (Wd + st - 1) / st, M = B * H * Wd, Mk = B * Ho * Wo;
     T* Qd = arena.get<T>(static_cast<size_t>(M) * dp);
     T* KVd = arena.get<T>(static_cast<size_t>(Mk) * dp);
-    T* Y = bf16() ? nullptr : arena.get<T>(static_cast<size_t>(M) * dp);
-    if (Y != nullptr) {                                                 // fp32: PreNorm LayerNorm of the attention (cvt.py:53)
-      ProfScope ps(this, PROF_LN, 8.0 * M * b.dim, 2.0 * sizeof(T) * M * dp, s);
-      layernorm<T>(X, dp, b.attn_norm.gamma, b.attn_norm.beta, Y, dp, M, b.dim, s, dp, 1e-5f);
-    }
+    const PreNorm<T> p = prenorm<T>(X, M, b.dim, dp, stats, 1e-5f, s);
+    const T* a = p.norm(b.attn_norm);                                   // PreNorm of the attention (cvt.py:53)
     {
       ProfScope ps(this, PROF_OTHER, 2.0 * b.k * b.k * b.dim * (static_cast<double>(M) + Mk),
                    static_cast<double>(sizeof(T)) * dp * (2.0 * M + Mk) + (stats ? 8.0 * M * (dp / 64) : 0.0), s);
-      dwconv_qkv<T>(Y ? Y : X, dp, Y ? nullptr : stats, b.attn_norm.gamma, b.attn_norm.beta, b.dim, 1e-5f, b.wq, b.bq, Qd, dp, b.wkv, b.bkv,
+      dwconv_qkv<T>(a, dp, p.Y ? nullptr : stats, b.attn_norm.gamma, b.attn_norm.beta, b.dim, 1e-5f, b.wq, b.bq, Qd, dp, b.wkv, b.bkv,
                     KVd, dp, B, H, Wd, dp, b.k, st, s);
     }
     T* Q = arena.get<T>(static_cast<size_t>(M) * HD);
@@ -2299,28 +2296,14 @@ struct vb_handle {
     linear<T>(KVd, dp, Mk, b.pw_kv, KV, 2 * HD, Epi(), s);
     T* O = arena.get<T>(static_cast<size_t>(M) * HD);
     attention_dispatch<T>(Q, HD, KV, 2 * HD, KV + HD, 2 * HD, O, HD, B, H * Wd, Ho * Wo, b.heads, 64, 0, nullptr, nullptr, nullptr, nullptr, s);
-    Epi eo; eo.bias = b.to_out.bias; eo.res = X; eo.ldr = dp; eo.stats_out = stats;
-    linear<T>(O, HD, M, b.to_out, X, dp, eo, s);
-    const T* fin = X;
-    if (Y != nullptr) {
-      ProfScope ps(this, PROF_LN, 8.0 * M * b.dim, 2.0 * sizeof(T) * M * dp, s);
-      layernorm<T>(X, dp, b.ff_norm.gamma, b.ff_norm.beta, Y, dp, M, b.dim, s, dp, 1e-5f);
-      fin = Y;
-    }
-    T* Hb = arena.get<T>(static_cast<size_t>(M) * b.fc1.N);
-    Epi e1; e1.gelu = true;
-    if (Y == nullptr) { e1.bias = b.fc1.ln_c2; e1.ln_stats = stats; } else { e1.bias = b.fc1.bias; }
-    linear<T>(fin, dp, M, b.fc1, Hb, b.fc1.N, e1, s);
-    Epi e2; e2.bias = b.fc2.bias; e2.res = X; e2.ldr = dp; e2.stats_out = stats;
-    linear<T>(Hb, b.fc1.N, M, b.fc2, X, dp, e2, s);
+    p.residual(O, HD, b.to_out);
+    p.mlp(b.ff);
   }
 
   // TwinsSVT.call (twins_svt.py:266-268): per stage, PatchEmbedding -> Transformer(1) -> PEG -> Transformer(depth); then
   // GlobalAvgPool2D -> Dense.  Token rows are the NHWC map, pixel-major, channel widths zero-padded to channel_width; no stage
   // permutes its map.  bf16: `stats` holds the (sum, sumsq) partials of X's rows between sub-blocks (emitted by the patch
   // embedding's and the residual GEMMs' epilogues, and after the PEG by a row-statistics pass).
-  static constexpr const char* kTwinsNoStages =
-      "Twins-SVT runs as a whole forward only: its patch-embedding / stage / head steps have no entry of their own";
   // The reference's shape rules (twins_svt.py:103,141,168 through einops and Keras), checked before anything runs.
   void twins_check_size(int H, int Wd) const {
     int h = H, w = Wd;
@@ -2343,20 +2326,9 @@ struct vb_handle {
     T* X = nullptr;
     for (const TwinsStageW& S : twins_stages) {
       const int oh = mh / S.patch, ow = mw / S.patch, M = B * oh * ow;
-      const int Kp = bf16() ? S.proj.ldw : S.proj.K;
-      T* col = arena.get<T>(static_cast<size_t>(M) * Kp);
-      {
-        ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(map == nullptr ? 4 : sizeof(T)) * B * mh * mw * mc +
-                                                 static_cast<double>(sizeof(T)) * M * Kp, s);
-        if (map == nullptr) unfold_same<float, T>(img, col, B, mh, mw, mc, S.patch, S.patch, 0, Kp, s);
-        else unfold_same<T, T>(map, col, B, mh, mw, mc, S.patch, S.patch, 0, Kp, s, ld_in);
-      }
       X = arena.get<T>(static_cast<size_t>(M) * S.dp);
-      float* stats = bf16() ? arena.get<float>(static_cast<size_t>(M) * (S.dp / 64) * 2) : nullptr;
-      Linear L = S.proj;
-      L.K = Kp;
-      Epi e; e.bias = S.proj.bias; e.stats_out = stats;
-      linear<T>(col, Kp, M, L, X, S.dp, e, s);
+      float* stats = row_stats(M, S.dp);
+      conv<T>(img, map, ld_in, B, mh, mw, mc, S.patch, S.patch, S.proj, X, stats, s);
       for (const TwinsLayerW& l : S.pre) twins_layer<T>(X, B, oh, ow, S, l, stats, s);
       T* Y = arena.get<T>(static_cast<size_t>(M) * S.dp);             // the PEG's halo reads the unmodified map
       {
@@ -2370,12 +2342,7 @@ struct vb_handle {
       map = X; mh = oh; mw = ow; mc = S.dim; ld_in = S.dp;
     }
     const int dl = tw.emb_dim[VB_TWINS_STAGES - 1];
-    float* z = arena.get<float>(static_cast<size_t>(B) * dl);
-    {
-      ProfScope ps(this, PROF_LN, 1.0 * B * mh * mw * dl, static_cast<double>(sizeof(T)) * B * mh * mw * dl, s);
-      pool_layernorm<T>(X, mh * mw, ld_in, nullptr, nullptr, z, B, dl, 1, s);   // GlobalAvgPool2D twins_svt.py:262
-    }
-    gemm_simt<float, float, float>(z, dl, head.W, head.N, 1, logits, head.N, B, head.N, dl, head.bias, nullptr, nullptr, head.N, 0, s);
+    dense_head(mean_pool<T>(X, mh * mw, ld_in, dl, B, s), dl, head, B, logits, s);   // GlobalAvgPool2D twins_svt.py:262
   }
   // One Transformer layer (twins_svt.py:206-211) in place on X [B*H*W, dp].  bf16: the PreNorm LayerNorms are folded into the
   // fused local q|k|v, the global to_q and the fc1s (from `stats`), and applied on load by the global to_kv's patch gather; fp32:
@@ -2383,72 +2350,39 @@ struct vb_handle {
   template <typename T>
   void twins_layer(T* X, int B, int H, int Wd, const TwinsStageW& S, const TwinsLayerW& l, float* stats, cudaStream_t s) {
     const int dp = S.dp, d = S.dim, M = B * H * Wd, I = kTwinsInner;
-    T* Y = bf16() ? nullptr : arena.get<T>(static_cast<size_t>(M) * dp);
-    auto prenorm = [&](const Norm& n) -> const T* {
-      if (Y == nullptr) return X;
-      ProfScope ps(this, PROF_LN, 8.0 * M * d, 2.0 * sizeof(T) * M * dp, s);
-      layernorm<T>(X, dp, n.gamma, n.beta, Y, dp, M, d, s, dp, 1e-5f);
-      return Y;
-    };
-    auto folded = [&](const Linear& L) {
-      Epi e;
-      if (Y == nullptr) { e.bias = L.ln_c2; e.ln_stats = stats; } else { e.bias = L.bias; }
-      return e;
-    };
-    auto residual = [&](const T* A, int lda, const Linear& L) {     // X = A W + b + X, and X's new row statistics
-      Epi e; e.bias = L.bias; e.res = X; e.ldr = dp; e.stats_out = stats;
-      linear<T>(A, lda, M, L, X, dp, e, s);
-    };
-    auto mlp = [&](const MlpW& m) {                              // twins_svt.py:78-92
-      const T* a = prenorm(m.norm);
-      T* Hb = arena.get<T>(static_cast<size_t>(M) * m.fc1.N);
-      Epi e1 = folded(m.fc1);
-      e1.gelu = true;
-      linear<T>(a, dp, M, m.fc1, Hb, m.fc1.N, e1, s);
-      residual(Hb, m.fc1.N, m.fc2);
-    };
+    const PreNorm<T> p = prenorm<T>(X, M, d, dp, stats, 1e-5f, s);   // the MLPs: twins_svt.py:78-92
     T* O = arena.get<T>(static_cast<size_t>(M) * I);
     if (l.local) {                                                    // LocalAttention twins_svt.py:135-156
-      const T* a = prenorm(l.local_norm);
+      const T* a = p.norm(l.local_norm);
       T* QKV = arena.get<T>(static_cast<size_t>(M) * 3 * I);
-      linear<T>(a, dp, M, l.qkv, QKV, 3 * I, folded(l.qkv), s);
+      linear<T>(a, dp, M, l.qkv, QKV, 3 * I, p.folded_epi(l.qkv), s);
       Window win;
       win.p = S.local; win.nx = Wd / S.local; win.ny = H / S.local;
       const int n = S.local * S.local;
       attention_dispatch<T>(QKV, 3 * I, QKV + I, 3 * I, QKV + 2 * I, 3 * I, O, I, B * win.nx * win.ny, n, n, I / 64, 64, 0, nullptr, nullptr,
                             nullptr, nullptr, s, 0.f, &win);
-      residual(O, I, l.local_out);
-      mlp(l.ff1);
+      p.residual(O, I, l.local_out);
+      p.mlp(l.ff1);
     }
     // GlobalAttention twins_svt.py:175-190: q from every pixel, k|v from the VALID k x k stride-k convolution of LN(x)
-    const T* a = prenorm(l.global_norm);
+    const T* a = p.norm(l.global_norm);
     T* Q = arena.get<T>(static_cast<size_t>(M) * I);
-    linear<T>(a, dp, M, l.to_q, Q, I, folded(l.to_q), s);
+    linear<T>(a, dp, M, l.to_q, Q, I, p.folded_epi(l.to_q), s);
     const int k = S.global_k, kh = (H - k) / k + 1, kw = (Wd - k) / k + 1, Mk = B * kh * kw;
-    const int Kp = bf16() ? l.to_kv.ldw : l.to_kv.K;
-    T* col = arena.get<T>(static_cast<size_t>(Mk) * Kp);
-    {
-      ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(sizeof(T)) * Mk * Kp * 2.0, s);
-      UnfoldMode um;
-      um.valid = true;
-      if (Y == nullptr) { um.stats = stats; um.parts = dp / 64; um.d = d; um.eps = 1e-5f; um.gamma = l.global_norm.gamma; um.beta = l.global_norm.beta; }
-      unfold_same<T, T>(a, col, B, H, Wd, d, k, k, 0, Kp, s, dp, &um);
-    }
+    UnfoldMode um;                                                    // bf16: the LayerNorm applied on load
+    um.valid = true;
+    if (p.Y == nullptr) { um.stats = stats; um.parts = dp / 64; um.d = d; um.eps = 1e-5f; um.gamma = l.global_norm.gamma; um.beta = l.global_norm.beta; }
     T* KV = arena.get<T>(static_cast<size_t>(Mk) * 2 * I);
-    Linear Lk = l.to_kv;
-    Lk.K = Kp;
-    linear<T>(col, Kp, Mk, Lk, KV, 2 * I, Epi(), s);
+    conv<T>(nullptr, a, dp, B, H, Wd, d, k, k, l.to_kv, KV, nullptr, s, &um);
     attention_dispatch<T>(Q, I, KV, 2 * I, KV + I, 2 * I, O, I, B, H * Wd, kh * kw, I / 64, 64, 0, nullptr, nullptr, nullptr, nullptr, s);
-    residual(O, I, l.global_out);
-    mlp(l.ff2);
+    p.residual(O, I, l.global_out);
+    p.mlp(l.ff2);
   }
 
   // CrossFormer.call (crossformer.py:263-269): per stage, CrossEmbedLayer -> Transformer; then the mean over the map -> Dense.
   // Token rows are the NHWC map, pixel-major, channel widths zero-padded to channel_width; no stage permutes its map (the windowed
   // attention reads and writes the map's own rows).  bf16: `stats` holds the (sum, sumsq) partials of X's rows between sub-blocks
   // (emitted by the embedding's and the residual GEMMs' epilogues).
-  static constexpr const char* kCrossformerNoStages =
-      "CrossFormer runs as a whole forward only: its embedding / stage / head steps have no entry of their own";
   // The reference's shape rule (crossformer.py:144,146 through einops), checked before anything runs.
   void cf_check_size(int H, int Wd) const {
     int h = H, w = Wd;
@@ -2468,65 +2402,26 @@ struct vb_handle {
     T* X = nullptr;
     for (const CrossformerStageW& S : cf_stages) {
       const int oh = (mh + S.stride - 1) / S.stride, ow = (mw + S.stride - 1) / S.stride, M = B * oh * ow;
-      const int Kp = bf16() ? S.embed.ldw : S.embed.K;
-      T* col = arena.get<T>(static_cast<size_t>(M) * Kp);
-      {
-        ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(map == nullptr ? 4 : sizeof(T)) * B * mh * mw * mc +
-                                                 static_cast<double>(sizeof(T)) * M * Kp, s);
-        if (map == nullptr) unfold_same<float, T>(img, col, B, mh, mw, mc, S.kmax, S.stride, 0, Kp, s);
-        else unfold_same<T, T>(map, col, B, mh, mw, mc, S.kmax, S.stride, 0, Kp, s, ld_in);
-      }
       X = arena.get<T>(static_cast<size_t>(M) * S.dp);
-      float* stats = bf16() ? arena.get<float>(static_cast<size_t>(M) * (S.dp / 64) * 2) : nullptr;
-      Linear L = S.embed;
-      L.K = Kp;
-      Epi e; e.bias = S.embed.bias; e.stats_out = stats;
-      linear<T>(col, Kp, M, L, X, S.dp, e, s);
+      float* stats = row_stats(M, S.dp);
+      conv<T>(img, map, ld_in, B, mh, mw, mc, S.kmax, S.stride, S.embed, X, stats, s);
       for (const CrossformerLayerW& l : S.layers) crossformer_layer<T>(X, B, oh, ow, S, l, stats, s);
       map = X; mh = oh; mw = ow; mc = S.dim; ld_in = S.dp;
     }
     const int dl = cf.dim[VB_CROSSFORMER_STAGES - 1];
-    float* z = arena.get<float>(static_cast<size_t>(B) * dl);
-    {
-      ProfScope ps(this, PROF_LN, 1.0 * B * mh * mw * dl, static_cast<double>(sizeof(T)) * B * mh * mw * dl, s);
-      pool_layernorm<T>(X, mh * mw, ld_in, nullptr, nullptr, z, B, dl, 1, s);   // Reduce('b h w c -> b c', 'mean') crossformer.py:259
-    }
-    gemm_simt<float, float, float>(z, dl, head.W, head.N, 1, logits, head.N, B, head.N, dl, head.bias, nullptr, nullptr, head.N, 0, s);
+    dense_head(mean_pool<T>(X, mh * mw, ld_in, dl, B, s), dl, head, B, logits, s);   // Reduce('b h w c -> b c', 'mean') crossformer.py:259
   }
   // One Transformer layer (crossformer.py:198-202) in place on X [B*H*W, dp].  bf16: the LayerNorms folded into q|k|v and fc1 (from
   // `stats`); fp32: separate LayerNorms.
   template <typename T>
   void crossformer_layer(T* X, int B, int H, int Wd, const CrossformerStageW& S, const CrossformerLayerW& l, float* stats, cudaStream_t s) {
     const int dp = S.dp, d = S.dim, M = B * H * Wd, I = 32 * S.heads;
-    T* Y = bf16() ? nullptr : arena.get<T>(static_cast<size_t>(M) * dp);
-    auto prenorm = [&](const Norm& n) -> const T* {
-      if (Y == nullptr) return X;
-      ProfScope ps(this, PROF_LN, 8.0 * M * d, 2.0 * sizeof(T) * M * dp, s);
-      layernorm<T>(X, dp, n.gamma, n.beta, Y, dp, M, d, s, dp, 1e-5f);
-      return Y;
-    };
-    auto folded = [&](const Linear& L) {
-      Epi e;
-      if (Y == nullptr) { e.bias = L.ln_c2; e.ln_stats = stats; } else { e.bias = L.bias; }
-      return e;
-    };
-    auto residual = [&](const T* A, int lda, const Linear& L) {     // X = A W + b + X, and X's new row statistics
-      Epi e; e.bias = L.bias; e.res = X; e.ldr = dp; e.stats_out = stats;
-      linear<T>(A, lda, M, L, X, dp, e, s);
-    };
-    auto mlp = [&](const MlpW& m) {                                   // crossformer.py:89-102
-      const T* a = prenorm(m.norm);
-      T* Hb = arena.get<T>(static_cast<size_t>(M) * m.fc1.N);
-      Epi e1 = folded(m.fc1);
-      e1.gelu = true;
-      linear<T>(a, dp, M, m.fc1, Hb, m.fc1.N, e1, s);
-      residual(Hb, m.fc1.N, m.fc2);
-    };
+    const PreNorm<T> p = prenorm<T>(X, M, d, dp, stats, 1e-5f, s);   // the MLPs: crossformer.py:89-102
     auto attend = [&](const CrossformerAttnW& at) {                   // crossformer.py:133-180
-      const T* a = prenorm(at.norm);
+      const T* a = p.norm(at.norm);
       const int ld = at.qkv.N;
       T* QKV = arena.get<T>(static_cast<size_t>(M) * ld);
-      linear<T>(a, dp, M, at.qkv, QKV, ld, folded(at.qkv), s);
+      linear<T>(a, dp, M, at.qkv, QKV, ld, p.folded_epi(at.qkv), s);
       if (at.wsz > 1) {                                               // wsz == 1: the output is v itself, which QKV holds
         Window win;
         win.p = at.wsz; win.nx = Wd / at.wsz; win.ny = H / at.wsz; win.dilated = at.dilated;
@@ -2536,12 +2431,12 @@ struct vb_handle {
         attention_dispatch<T>(QKV, ld, QKV + I, ld, QKV + 2 * I, ld, QKV, ld, B * win.nx * win.ny, n, n, S.heads, 32, 0, nullptr, nullptr,
                               nullptr, nullptr, s, 0.f, &win, &pb);
       }
-      residual(QKV, ld, at.to_out);                                   // to_out reads the I output (or v) columns
+      p.residual(QKV, ld, at.to_out);                                 // to_out reads the I output (or v) columns
     };
     attend(l.short_attn);
-    mlp(l.ff1);
+    p.mlp(l.ff1);
     attend(l.long_attn);
-    mlp(l.ff2);
+    p.mlp(l.ff2);
   }
 
   // NesT.call (nest.py:202-216): the patch embedding, then per level the position add, the Transformer within blocks and the
@@ -2550,8 +2445,6 @@ struct vb_handle {
   // rows).  The position scalar is added by the kernel that last wrote the rows: a small pass after the patch embedding at level
   // 0, the aggregation tail of the level below otherwise.  bf16: `stats` holds the (sum, sumsq) partials of X's rows between
   // sub-blocks (emitted by those kernels and the residual GEMMs' epilogues).
-  static constexpr const char* kNestNoStages =
-      "NesT runs as a whole forward only: its patch-embedding / level / head steps have no entry of their own";
   // The reference's shape rules (nest.py:179,140-142,209 through einops, and the head LayerNorm's broadcast), checked before
   // anything runs.
   void nest_check_size(int H, int Wd) const {
@@ -2576,20 +2469,10 @@ struct vb_handle {
   void nest_forward(const float* img, int B, int H, int Wd, float* logits, cudaStream_t s) {
     nest_check_size(H, Wd);
     int mh = H / ns.patch_size, mw = Wd / ns.patch_size, d = ns.dim, dp = channel_width(ns.dim);
-    const int M0 = B * mh * mw, Kp = bf16() ? nest_patch.ldw : nest_patch.K;
-    T* col = arena.get<T>(static_cast<size_t>(M0) * Kp);
-    {
-      ProfScope ps(this, PROF_EMBED, 0.0, 4.0 * B * H * Wd * cfg.channels + static_cast<double>(sizeof(T)) * M0 * Kp, s);
-      unfold_same<float, T>(img, col, B, H, Wd, cfg.channels, ns.patch_size, ns.patch_size, 0, Kp, s);
-    }
+    const int M0 = B * mh * mw;
     T* X = arena.get<T>(static_cast<size_t>(M0) * dp);
-    float* stats = bf16() ? arena.get<float>(static_cast<size_t>(M0) * (dp / 64) * 2) : nullptr;
-    {
-      Linear L = nest_patch;
-      L.K = Kp;
-      Epi e; e.bias = nest_patch.bias;
-      linear<T>(col, Kp, M0, L, X, dp, e, s);
-    }
+    float* stats = row_stats(M0, dp);
+    conv<T>(img, nullptr, 0, B, H, Wd, cfg.channels, ns.patch_size, ns.patch_size, nest_patch, X, nullptr, s);
     for (size_t i = 0; i < nest_levels.size(); ++i) {
       const NestLevelW& V = nest_levels[i];
       const int M = B * mh * mw;
@@ -2601,24 +2484,13 @@ struct vb_handle {
       if (!V.aggregate) continue;
       // Aggregate (nest.py:111-123): the 3 x 3 SAME convolution as unfold_same + GEMM with the conv rows' statistics, then one pass
       // for the LayerNorm, the max-pool and the next level's position add
-      const int Kc = bf16() ? V.agg.ldw : V.agg.K;
-      T* ccol = arena.get<T>(static_cast<size_t>(M) * Kc);
-      {
-        ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(sizeof(T)) * M * (dp + Kc), s);
-        unfold_same<T, T>(X, ccol, B, mh, mw, V.dim, 3, 1, 0, Kc, s, dp);
-      }
       T* Y = arena.get<T>(static_cast<size_t>(M) * V.dp_out);
-      float* ystats = bf16() ? arena.get<float>(static_cast<size_t>(M) * (V.dp_out / 64) * 2) : nullptr;
-      {
-        Linear L = V.agg;
-        L.K = Kc;
-        Epi e; e.bias = V.agg.bias; e.stats_out = ystats;
-        linear<T>(ccol, Kc, M, L, Y, V.dp_out, e, s);
-      }
+      float* ystats = row_stats(M, V.dp_out);
+      conv<T>(nullptr, X, dp, B, mh, mw, V.dim, 3, 1, V.agg, Y, ystats, s);
       const NestLevelW* next = i + 1 < nest_levels.size() ? &nest_levels[i + 1] : nullptr;
       const int oh = (mh + 1) / 2, ow = (mw + 1) / 2, Mo = B * oh * ow;
       T* Xn = arena.get<T>(static_cast<size_t>(Mo) * V.dp_out);
-      float* nstats = bf16() ? arena.get<float>(static_cast<size_t>(Mo) * (V.dp_out / 64) * 2) : nullptr;
+      float* nstats = row_stats(Mo, V.dp_out);
       const T* src = Y;
       NestPoolLn ln;
       if (bf16()) {
@@ -2646,43 +2518,23 @@ struct vb_handle {
       layernorm<T>(X, dp, head_norm.gamma, head_norm.beta, Y, dp, M, d, s, dp, 1e-5f);
       pool_layernorm<T>(Y, mh * mw, dp, nullptr, nullptr, z, B, d, 1, s);
     }
-    gemm_simt<float, float, float>(z, d, head.W, head.N, 1, logits, head.N, B, head.N, d, head.bias, nullptr, nullptr, head.N, 0, s);
+    dense_head(z, d, head, B, logits, s);
   }
   // One Transformer block (nest.py:144-146) in place on X [B*H*W, dp]: attention within the level's bs x bs blocks per map, then
   // the MLP.  bf16: the LayerNorms folded into q|k|v and fc1 (from `stats`); fp32: separate LayerNorms.
   template <typename T>
   void nest_block(T* X, int B, int H, int Wd, const NestLevelW& V, const NestBlockW& l, float* stats, cudaStream_t s) {
     const int dp = V.dp, d = V.dim, M = B * H * Wd;
-    T* Y = bf16() ? nullptr : arena.get<T>(static_cast<size_t>(M) * dp);
-    auto prenorm = [&](const Norm& n) -> const T* {
-      if (Y == nullptr) return X;
-      ProfScope ps(this, PROF_LN, 8.0 * M * d, 2.0 * sizeof(T) * M * dp, s);
-      layernorm<T>(X, dp, n.gamma, n.beta, Y, dp, M, d, s, dp, 1e-5f);
-      return Y;
-    };
-    auto folded = [&](const Linear& L) {
-      Epi e;
-      if (Y == nullptr) { e.bias = L.ln_c2; e.ln_stats = stats; } else { e.bias = L.bias; }
-      return e;
-    };
-    auto residual = [&](const T* A, int lda, const Linear& L) {     // X = A W + b + X, and X's new row statistics
-      Epi e; e.bias = L.bias; e.res = X; e.ldr = dp; e.stats_out = stats;
-      linear<T>(A, lda, M, L, X, dp, e, s);
-    };
-    const T* a = prenorm(l.attn_norm);                                // Attention nest.py:93-109
+    const PreNorm<T> p = prenorm<T>(X, M, d, dp, stats, 1e-5f, s);
+    const T* a = p.norm(l.attn_norm);                                 // Attention nest.py:93-109
     const int ld = l.qkv.N;
     T* QKV = arena.get<T>(static_cast<size_t>(M) * ld);
-    linear<T>(a, dp, M, l.qkv, QKV, ld, folded(l.qkv), s);
+    linear<T>(a, dp, M, l.qkv, QKV, ld, p.folded_epi(l.qkv), s);
     Window win;
     win.p = H / V.bs; win.pw = Wd / V.bs; win.nx = V.bs; win.ny = V.bs; win.count = B * V.bs * V.bs;
     block_attention<T>(QKV, ld, QKV, ld, V.heads, V.dh, win, s);      // the output overwrites q
-    residual(QKV, ld, l.to_out);
-    const T* f = prenorm(l.ff.norm);                                  // MLP nest.py:61-75
-    T* Hb = arena.get<T>(static_cast<size_t>(M) * l.ff.fc1.N);
-    Epi e1 = folded(l.ff.fc1);
-    e1.gelu = true;
-    linear<T>(f, dp, M, l.ff.fc1, Hb, l.ff.fc1.N, e1, s);
-    residual(Hb, l.ff.fc1.N, l.ff.fc2);
+    p.residual(QKV, ld, l.to_out);
+    p.mlp(l.ff);                                                      // MLP nest.py:61-75
   }
   // NesT's block attention: win.count blocks of p x width() tokens of fused q|k|v rows [.., ld], the output rows written to out
   // [.., ldo] pixel-major.  The windowed flash kernel where it serves (bf16, dh 32 or 64); otherwise the rows permuted to
@@ -2713,8 +2565,6 @@ struct vb_handle {
   // local rows (the pixel-major B x lh x lw map) followed by its regional rows (the B x rh x rw map) in one arena, so every
   // token-wise step is one launch over both; the R2L attention reads and writes both in place.  Channel widths are zero-padded to
   // channel_width.  bf16: `stats` holds the (sum, sumsq) partials of all rows between sub-blocks, pitch M.
-  static constexpr const char* kRegionNoStages =
-      "RegionViT runs as a whole forward only: its encoder / stage / head steps have no entry of their own";
   // The reference's shape rules (the call-time asserts :251-252, the window rearranges and concat :163-168, the bias Embedding
   // :153), checked before anything runs.  The local encoder's SAME stride 4 (or two SAME stride 2) gives ceil(H / 4).
   void rv_check_size(int H, int Wd) const {
@@ -2748,21 +2598,7 @@ struct vb_handle {
     int lh = (H + 3) / 4, lw = (Wd + 3) / 4, rh = H / p, rw = Wd / p;
     int Ml = B * lh * lw, Mr = B * rh * rw, M = Ml + Mr, d = rv.dims[0], dp = rv_stages[0].dp;
     T* X = arena.get<T>(static_cast<size_t>(M) * dp);
-    float* stats = bf16() ? arena.get<float>(static_cast<size_t>(M) * (dp / 64) * 2) : nullptr;
-    // a SAME convolution as unfold_same + GEMM into out [rows, dp]; src == null reads the image
-    auto conv = [&](const T* src, int h, int w, int cin, int k, int stride, const UnfoldMode* um, const Linear& Lw, T* out, float* st) {
-      const int oh = (h + stride - 1) / stride, ow = (w + stride - 1) / stride, rows = B * oh * ow, Kp = bf16() ? Lw.ldw : Lw.K;
-      T* col = arena.get<T>(static_cast<size_t>(rows) * Kp);
-      {
-        ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(src ? sizeof(T) : 4) * B * h * w * cin + static_cast<double>(sizeof(T)) * rows * Kp, s);
-        if (src == nullptr) unfold_same<float, T>(img, col, B, h, w, cin, k, stride, 0, Kp, s);
-        else unfold_same<T, T>(src, col, B, h, w, cin, k, stride, 0, Kp, s, dp, um);
-      }
-      Linear L = Lw;
-      L.K = Kp;
-      Epi e; e.bias = Lw.bias; e.stats_out = st;
-      linear<T>(col, Kp, rows, L, out, dp, e, s);
-    };
+    float* stats = row_stats(M, dp);
     if (rv.tokenize_local_3_conv) {                                  // regionvit.py:211-218: the LayerNorm + GELU applied on load
       int h = H, w = Wd;
       const T* src = nullptr;
@@ -2779,16 +2615,16 @@ struct vb_handle {
           src = Z;
         }
         T* out = i == 2 ? X : arena.get<T>(static_cast<size_t>(rows) * dp);
-        float* st = bf16() && i < 2 ? arena.get<float>(static_cast<size_t>(rows) * (dp / 64) * 2) : nullptr;
-        conv(src, h, w, i == 0 ? C : d, 3, stride, i > 0 ? &um : nullptr, rv_local[i], out, st);
+        float* st = i < 2 ? row_stats(rows, dp) : nullptr;
+        conv<T>(img, src, dp, B, h, w, i == 0 ? C : d, 3, stride, rv_local[i], out, st, s, i > 0 ? &um : nullptr);
         src = out; h = oh; w = ow;
         if (st != nullptr) stats = st;                               // the next unfold's LayerNorm statistics
       }
-      stats = bf16() ? arena.get<float>(static_cast<size_t>(M) * (dp / 64) * 2) : nullptr;
+      stats = row_stats(M, dp);
     } else {
-      conv(nullptr, H, Wd, C, 8, 4, nullptr, rv_local[0], X, nullptr);   // :221
+      conv<T>(img, nullptr, 0, B, H, Wd, C, 8, 4, rv_local[0], X, nullptr, s);   // :221
     }
-    conv(nullptr, H, Wd, C, p, p, nullptr, rv_region, X + static_cast<size_t>(Ml) * dp, nullptr);   // :223-226
+    conv<T>(img, nullptr, 0, B, H, Wd, C, p, p, rv_region, X + static_cast<size_t>(Ml) * dp, nullptr, s);   // :223-226
     if (bf16()) ensure_stats<T>(X, dp, stats, M, s);
     for (const RegionStageW& S : rv_stages) {
       if (S.down) {          // :258: one Conv2D(3, 2, SAME) for both maps, both unfolded into one column buffer, one GEMM
@@ -2801,7 +2637,7 @@ struct vb_handle {
           unfold_same<T, T>(X + static_cast<size_t>(Ml) * dp, col + static_cast<size_t>(nMl) * Kp, B, rh, rw, d, 3, 2, 0, Kp, s, dp);
         }
         T* Xn = arena.get<T>(static_cast<size_t>(nM) * S.dp);
-        stats = bf16() ? arena.get<float>(static_cast<size_t>(nM) * (S.dp / 64) * 2) : nullptr;
+        stats = row_stats(nM, S.dp);
         Linear L = S.down_conv;
         L.K = Kp;
         Epi e; e.bias = S.down_conv.bias; e.stats_out = S.peg ? nullptr : stats;
@@ -2827,7 +2663,7 @@ struct vb_handle {
       ProfScope ps(this, PROF_LN, 1.0 * Mr * d + 8.0 * B * d, static_cast<double>(sizeof(T)) * Mr * dp, s);
       pool_layernorm<T>(X + static_cast<size_t>(Ml) * dp, rh * rw, dp, head_norm.gamma, head_norm.beta, z, B, d, 1, s);
     }
-    gemm_simt<float, float, float>(z, d, head.W, head.N, 1, logits, head.N, B, head.N, d, head.bias, nullptr, nullptr, head.N, 0, s);
+    dense_head(z, d, head, B, logits, s);
   }
   // One R2L layer (regionvit.py:158-172) in place on X [M, dp], M = B lh lw local rows + B rh rw regional rows: the regional
   // self-attention on the regional rows, then the R2L attention and the MLP over all rows.  bf16: the LayerNorms folded into q|k|v
@@ -2837,49 +2673,28 @@ struct vb_handle {
   void regionvit_layer(T* X, int B, int lh, int lw, int rh, int rw, const RegionStageW& S, const RegionLayerW& l, float* stats, cudaStream_t s) {
     const int dp = S.dp, d = S.dim, Ml = B * lh * lw, Mr = B * rh * rw, M = Ml + Mr, ld = l.qkv.N;
     T* Xr = X + static_cast<size_t>(Ml) * dp;
-    T* Y = bf16() ? nullptr : arena.get<T>(static_cast<size_t>(M) * dp);
+    const PreNorm<T> p = prenorm<T>(X, M, d, dp, stats, 1e-3f, s);
     T* QKV = arena.get<T>(static_cast<size_t>(M) * ld);
-    auto prenorm = [&](const T* A, int rows, const Norm& n) -> const T* {
-      if (Y == nullptr) return A;
-      ProfScope ps(this, PROF_LN, 8.0 * rows * d, 2.0 * sizeof(T) * rows * dp, s);
-      layernorm<T>(A, dp, n.gamma, n.beta, Y, dp, rows, d, s, dp, 1e-3f);
-      return Y;
-    };
-    auto folded = [&](const Linear& L, const float* st) {
-      Epi e;
-      if (Y == nullptr) { e.bias = L.ln_c2; e.ln_stats = st; } else { e.bias = L.bias; }
-      return e;
-    };
-    // region_tokens = attn(region_tokens) + region_tokens (:159): all rh x rw regional tokens of an image attend together
-    float* rstats = bf16() ? arena.get<float>(static_cast<size_t>(Mr) * (dp / 64) * 2) : nullptr;
+    // region_tokens = attn(region_tokens) + region_tokens (:159): all rh x rw regional tokens of an image attend together, their
+    // LayerNorm folded from the regional rows' own statistics
+    float* rstats = row_stats(Mr, dp);
     if (bf16()) rv_region_stats<T>(Xr, dp, rstats, Mr, Mr, s);
-    linear<T>(prenorm(Xr, Mr, l.attn_norm), dp, Mr, l.qkv, QKV, ld, folded(l.qkv, rstats), s);
+    const PreNorm<T> pr = p.rows(Xr, Mr, rstats);
+    linear<T>(pr.norm(l.attn_norm), dp, Mr, l.qkv, QKV, ld, pr.folded_epi(l.qkv), s);
     Window rwin;
     rwin.p = rh; rwin.pw = rw; rwin.nx = 1; rwin.ny = 1; rwin.count = B;
     block_attention<T>(QKV, ld, QKV, ld, kRvHeads, kRvDh, rwin, s);     // the output overwrites q
-    {
-      Epi e; e.bias = l.to_out.bias; e.res = Xr; e.ldr = dp;
-      linear<T>(QKV, ld, Mr, l.to_out, Xr, dp, e, s);
-    }
+    p.rows(Xr, Mr, nullptr).residual(QKV, ld, l.to_out);               // its statistics: the next pass, at pitch M
     if (bf16()) rv_region_stats<T>(Xr, dp, stats + static_cast<size_t>(Ml) * 2, Mr, M, s);
     // [r; window] = attn([r; window], rel_pos_bias) + [r; window] (:168-169), each window with its regional token
-    linear<T>(prenorm(X, M, l.attn_norm), dp, M, l.qkv, QKV, ld, folded(l.qkv, stats), s);
+    linear<T>(p.norm(l.attn_norm), dp, M, l.qkv, QKV, ld, p.folded_epi(l.qkv), s);
     Window win;
     win.p = lh / rh; win.pw = lw / rw; win.nx = rw; win.ny = rh; win.count = Mr;
     PosBias pb;
     pb.table = S.table; pb.r2l_ws = rv.window_size; pb.r2l_h = win.p; pb.r2l_w = win.pw;
     r2l_attention<T>(QKV, ld, QKV, ld, Ml, pb, win, s);
-    auto residual = [&](const T* A, int lda, const Linear& L) {     // X = A W + b + X over all rows, and X's new row statistics
-      Epi e; e.bias = L.bias; e.res = X; e.ldr = dp; e.stats_out = stats;
-      linear<T>(A, lda, M, L, X, dp, e, s);
-    };
-    residual(QKV, ld, l.to_out);
-    // ff(.) + . (:172)
-    T* Hb = arena.get<T>(static_cast<size_t>(M) * l.ff.fc1.N);
-    Epi e1 = folded(l.ff.fc1, stats);
-    e1.gelu = true;
-    linear<T>(prenorm(X, M, l.ff.norm), dp, M, l.ff.fc1, Hb, l.ff.fc1.N, e1, s);
-    residual(Hb, l.ff.fc1.N, l.ff.fc2);
+    p.residual(QKV, ld, l.to_out);
+    p.mlp(l.ff);                                                        // ff(.) + . (:172)
   }
   // RegionViT's R2L attention: win.count windows of p x width() local rows, each with its regional row reg_row0 + (window index),
   // fused q|k|v rows [.., ld], the output rows written in place to out [.., ldo].  The R2L flash kernel where it serves (bf16, dh
@@ -2921,7 +2736,7 @@ struct vb_handle {
     copy_tokens<T>(E, rows, 0, X, rd, 0, rows, B, c.dim, s);
     T* last = X + static_cast<size_t>(rows) * c.dim;                 // row `rows` of image 0; image pitch rd rows
     broadcast_row<T>(distill_token, last, rd, B, c.dim, s);
-    float* stats = (bf16() && c.dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr) ? arena.get<float>(static_cast<size_t>(B) * rd * (c.dim / 64) * 2) : nullptr;
+    float* stats = c.dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr ? row_stats(static_cast<long long>(B) * rd, c.dim) : nullptr;
     bool sv = false;
     for (const auto& l : layers) layer_self<T>(X, B, rd, c.dim, l, s, stats, &sv);
     T* Xh = arena.get<T>(static_cast<size_t>(B) * rows * c.dim);     // x[:, :-1]
@@ -2948,7 +2763,7 @@ struct vb_handle {
       X = arena.get<T>(count);
       convert<float, __nv_bfloat16>(tok, reinterpret_cast<__nv_bfloat16*>(X), count, s);
     }
-    float* stats = (bf16() && cfg.dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr) ? arena.get<float>(static_cast<size_t>(B) * n * (cfg.dim / 64) * 2) : nullptr;
+    float* stats = cfg.dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr ? row_stats(static_cast<long long>(B) * n, cfg.dim) : nullptr;
     bool sv = false;
     for (const auto& l : layers) layer_self<T>(X, B, n, cfg.dim, l, s, stats, &sv);
     if (sizeof(T) == 4) VB_CUDA(cudaMemcpyAsync(out, X, count * 4, cudaMemcpyDeviceToDevice, s));
@@ -2956,16 +2771,26 @@ struct vb_handle {
   }
 
   // ---------------------------------------------------------------- stage entries (vb_forward_embed / _head / vb_patch_to_emb)
-  static constexpr const char* kCctNoStages = "CCT runs as a whole forward only: its tokenizer / classifier stages have no entry of their own";
+  // The kinds that run as a whole forward only refuse the stage entries (and vb_forward_tokens) with a message of their own
+  static const char* whole_forward_only(int kind) {
+    switch (kind) {
+      case VB_KIND_CCT: return "CCT runs as a whole forward only: its tokenizer / classifier stages have no entry of their own";
+      case VB_KIND_LEVIT: return "LeViT runs as a whole forward only: its stem / backbone / head stages have no entry of their own";
+      case VB_KIND_CVT: return "CvT runs as a whole forward only: its stem / stage / head steps have no entry of their own";
+      case VB_KIND_TWINS_SVT: return "Twins-SVT runs as a whole forward only: its patch-embedding / stage / head steps have no entry of their own";
+      case VB_KIND_CROSSFORMER: return "CrossFormer runs as a whole forward only: its embedding / stage / head steps have no entry of their own";
+      case VB_KIND_NEST: return "NesT runs as a whole forward only: its patch-embedding / level / head steps have no entry of their own";
+      case VB_KIND_REGIONVIT: return "RegionViT runs as a whole forward only: its encoder / stage / head steps have no entry of their own";
+      default: return nullptr;
+    }
+  }
+  void check_stage_entries() const {
+    const char* msg = whole_forward_only(cfg.kind);
+    VB_CHECK(msg == nullptr, msg);
+  }
   int embed_rows(int H, int Wd) const {
     VB_CHECK(cfg.kind != VB_KIND_CROSSVIT, "CrossViT has two token streams: no single embedding stage");
-    VB_CHECK(cfg.kind != VB_KIND_CCT, kCctNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_LEVIT, kLevitNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_CVT, kCvtNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_TWINS_SVT, kTwinsNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_CROSSFORMER, kCrossformerNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_NEST, kNestNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_REGIONVIT, kRegionNoStages);
+    check_stage_entries();
     if (cfg.kind == VB_KIND_T2T_VIT) {
       int h = H, w = Wd;
       for (const auto& st : t2t_stages()) { h = (h + st.stride - 1) / st.stride; w = (w + st.stride - 1) / st.stride; }
@@ -2990,13 +2815,7 @@ struct vb_handle {
   template <typename T>
   void head_impl(const float* tok, int B, int n, float* logits, cudaStream_t s) {
     VB_CHECK(cfg.kind != VB_KIND_CROSSVIT, "CrossViT sums two heads: no single mlp_head stage");
-    VB_CHECK(cfg.kind != VB_KIND_CCT, kCctNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_LEVIT, kLevitNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_CVT, kCvtNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_TWINS_SVT, kTwinsNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_CROSSFORMER, kCrossformerNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_NEST, kNestNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_REGIONVIT, kRegionNoStages);
+    check_stage_entries();
     arena.reset();
     const long long count = static_cast<long long>(B) * n * cfg.dim;
     T* X = arena.get<T>(count);
@@ -3007,13 +2826,7 @@ struct vb_handle {
   template <typename T>
   void patch_to_emb_impl(const float* patches, int rows, float* out, cudaStream_t s) {
     VB_CHECK(cfg.kind != VB_KIND_CROSSVIT, "CrossViT has two patch embeddings");
-    VB_CHECK(cfg.kind != VB_KIND_CCT, kCctNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_LEVIT, kLevitNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_CVT, kCvtNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_TWINS_SVT, kTwinsNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_CROSSFORMER, kCrossformerNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_NEST, kNestNoStages);
-    VB_CHECK(cfg.kind != VB_KIND_REGIONVIT, kRegionNoStages);
+    check_stage_entries();
     arena.reset();
     const int K = embed.patch.K, Kp = bf16() ? embed.patch.ldw : K;
     T* col = arena.get<T>(static_cast<size_t>(rows) * Kp);
@@ -3428,6 +3241,38 @@ void staged_call(vb_handle* h, const float* in, int32_t in_mem, size_t in_bytes,
     VB_CUDA(cudaStreamSynchronize(s));
   }
 }
+// vb_create_<kind> for the kinds whose stages come in an extension config: `fn` and `ext_name` name the entry point and the
+// config struct in the messages; `validate` checks the config against the base, `adopt` stores it in the handle and sets cfg.dim.
+template <typename Ext, typename Validate, typename Adopt>
+int create_with(const char* fn, const char* ext_name, int kind, const char* kind_name, const vb_config* base, const Ext* ext, int device,
+                vb_handle** out, Validate validate, Adopt adopt) {
+  const std::string f(fn);
+  return guarded(nullptr, [&] {
+    VB_CHECK(base != nullptr && ext != nullptr && out != nullptr, f + ": null argument");
+    VB_CHECK(base->struct_size == static_cast<int32_t>(sizeof(vb_config)) || base->struct_size == VB_CONFIG_SIZE_ABI7,
+             "vb_config.struct_size mismatch (ABI)");
+    VB_CHECK(ext->struct_size == static_cast<int32_t>(sizeof(Ext)), std::string(ext_name) + ".struct_size mismatch (ABI)");
+    vb_config c;
+    memset(&c, 0, sizeof c);
+    memcpy(&c, base, static_cast<size_t>(base->struct_size));
+    VB_CHECK(c.kind == kind, f + ": base.kind must be " + kind_name);
+    validate(c, *ext);
+    int ndev = 0;
+    cudaError_t e = cudaGetDeviceCount(&ndev);
+    VB_CHECK(e == cudaSuccess && ndev > 0, f + ": no CUDA device available -- libvitb200 has no CPU fallback");
+    VB_CHECK(device >= 0 && device < ndev, f + ": bad device index");
+    VB_CUDA(cudaSetDevice(device));
+    cudaDeviceProp prop;
+    VB_CUDA(cudaGetDeviceProperties(&prop, device));
+    VB_CHECK(prop.major == 9 && prop.minor == 0, f + ": libvitb200 is built for sm_90a (Hopper H100) only");
+    std::unique_ptr<vb_handle> h(new vb_handle());
+    h->cfg = c;
+    adopt(*h);
+    h->device = device;
+    h->build_expected();
+    *out = h.release();
+  });
+}
 }  // namespace
 
 extern "C" {
@@ -3461,177 +3306,31 @@ int vb_create(const vb_config* cfg, int device, vb_handle** out) {
 }
 
 int vb_create_levit(const vb_config* base, const vb_levit_config* lv, int device, vb_handle** out) {
-  return guarded(nullptr, [&] {
-    VB_CHECK(base != nullptr && lv != nullptr && out != nullptr, "vb_create_levit: null argument");
-    VB_CHECK(base->struct_size == static_cast<int32_t>(sizeof(vb_config)) || base->struct_size == VB_CONFIG_SIZE_ABI7,
-             "vb_config.struct_size mismatch (ABI)");
-    VB_CHECK(lv->struct_size == static_cast<int32_t>(sizeof(vb_levit_config)), "vb_levit_config.struct_size mismatch (ABI)");
-    vb_config c;
-    memset(&c, 0, sizeof c);
-    memcpy(&c, base, static_cast<size_t>(base->struct_size));
-    VB_CHECK(c.kind == VB_KIND_LEVIT, "vb_create_levit: base.kind must be VB_KIND_LEVIT");
-    validate_levit(c, *lv);
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    VB_CHECK(e == cudaSuccess && ndev > 0, "vb_create_levit: no CUDA device available -- libvitb200 has no CPU fallback");
-    VB_CHECK(device >= 0 && device < ndev, "vb_create_levit: bad device index");
-    VB_CUDA(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    VB_CUDA(cudaGetDeviceProperties(&prop, device));
-    VB_CHECK(prop.major == 9 && prop.minor == 0, "vb_create_levit: libvitb200 is built for sm_90a (Hopper H100) only");
-    std::unique_ptr<vb_handle> h(new vb_handle());
-    h->cfg = c;
-    h->cfg.dim = lv->dims[lv->stages - 1];
-    h->lv = *lv;
-    h->device = device;
-    h->build_expected();
-    *out = h.release();
-  });
+  return create_with("vb_create_levit", "vb_levit_config", VB_KIND_LEVIT, "VB_KIND_LEVIT", base, lv, device, out,
+                                      validate_levit, [&](vb_handle& h) { h.lv = *lv; h.cfg.dim = lv->dims[lv->stages - 1]; });
 }
-
 int vb_create_cvt(const vb_config* base, const vb_cvt_config* cvt, int device, vb_handle** out) {
-  return guarded(nullptr, [&] {
-    VB_CHECK(base != nullptr && cvt != nullptr && out != nullptr, "vb_create_cvt: null argument");
-    VB_CHECK(base->struct_size == static_cast<int32_t>(sizeof(vb_config)) || base->struct_size == VB_CONFIG_SIZE_ABI7,
-             "vb_config.struct_size mismatch (ABI)");
-    VB_CHECK(cvt->struct_size == static_cast<int32_t>(sizeof(vb_cvt_config)), "vb_cvt_config.struct_size mismatch (ABI)");
-    vb_config c;
-    memset(&c, 0, sizeof c);
-    memcpy(&c, base, static_cast<size_t>(base->struct_size));
-    VB_CHECK(c.kind == VB_KIND_CVT, "vb_create_cvt: base.kind must be VB_KIND_CVT");
-    validate_cvt(c, *cvt);
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    VB_CHECK(e == cudaSuccess && ndev > 0, "vb_create_cvt: no CUDA device available -- libvitb200 has no CPU fallback");
-    VB_CHECK(device >= 0 && device < ndev, "vb_create_cvt: bad device index");
-    VB_CUDA(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    VB_CUDA(cudaGetDeviceProperties(&prop, device));
-    VB_CHECK(prop.major == 9 && prop.minor == 0, "vb_create_cvt: libvitb200 is built for sm_90a (Hopper H100) only");
-    std::unique_ptr<vb_handle> h(new vb_handle());
-    h->cfg = c;
-    h->cfg.dim = cvt->emb_dim[VB_CVT_STAGES - 1];
-    h->cv = *cvt;
-    h->device = device;
-    h->build_expected();
-    *out = h.release();
-  });
+  return create_with("vb_create_cvt", "vb_cvt_config", VB_KIND_CVT, "VB_KIND_CVT", base, cvt, device, out, validate_cvt,
+                                    [&](vb_handle& h) { h.cv = *cvt; h.cfg.dim = cvt->emb_dim[VB_CVT_STAGES - 1]; });
 }
-
 int vb_create_twins_svt(const vb_config* base, const vb_twins_svt_config* tw, int device, vb_handle** out) {
-  return guarded(nullptr, [&] {
-    VB_CHECK(base != nullptr && tw != nullptr && out != nullptr, "vb_create_twins_svt: null argument");
-    VB_CHECK(base->struct_size == static_cast<int32_t>(sizeof(vb_config)) || base->struct_size == VB_CONFIG_SIZE_ABI7,
-             "vb_config.struct_size mismatch (ABI)");
-    VB_CHECK(tw->struct_size == static_cast<int32_t>(sizeof(vb_twins_svt_config)), "vb_twins_svt_config.struct_size mismatch (ABI)");
-    vb_config c;
-    memset(&c, 0, sizeof c);
-    memcpy(&c, base, static_cast<size_t>(base->struct_size));
-    VB_CHECK(c.kind == VB_KIND_TWINS_SVT, "vb_create_twins_svt: base.kind must be VB_KIND_TWINS_SVT");
-    validate_twins(c, *tw);
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    VB_CHECK(e == cudaSuccess && ndev > 0, "vb_create_twins_svt: no CUDA device available -- libvitb200 has no CPU fallback");
-    VB_CHECK(device >= 0 && device < ndev, "vb_create_twins_svt: bad device index");
-    VB_CUDA(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    VB_CUDA(cudaGetDeviceProperties(&prop, device));
-    VB_CHECK(prop.major == 9 && prop.minor == 0, "vb_create_twins_svt: libvitb200 is built for sm_90a (Hopper H100) only");
-    std::unique_ptr<vb_handle> h(new vb_handle());
-    h->cfg = c;
-    h->cfg.dim = tw->emb_dim[VB_TWINS_STAGES - 1];
-    h->tw = *tw;
-    h->device = device;
-    h->build_expected();
-    *out = h.release();
-  });
+  return create_with("vb_create_twins_svt", "vb_twins_svt_config", VB_KIND_TWINS_SVT, "VB_KIND_TWINS_SVT", base, tw,
+                                          device, out, validate_twins,
+                                          [&](vb_handle& h) { h.tw = *tw; h.cfg.dim = tw->emb_dim[VB_TWINS_STAGES - 1]; });
 }
-
 int vb_create_crossformer(const vb_config* base, const vb_crossformer_config* cfc, int device, vb_handle** out) {
-  return guarded(nullptr, [&] {
-    VB_CHECK(base != nullptr && cfc != nullptr && out != nullptr, "vb_create_crossformer: null argument");
-    VB_CHECK(base->struct_size == static_cast<int32_t>(sizeof(vb_config)) || base->struct_size == VB_CONFIG_SIZE_ABI7,
-             "vb_config.struct_size mismatch (ABI)");
-    VB_CHECK(cfc->struct_size == static_cast<int32_t>(sizeof(vb_crossformer_config)), "vb_crossformer_config.struct_size mismatch (ABI)");
-    vb_config c;
-    memset(&c, 0, sizeof c);
-    memcpy(&c, base, static_cast<size_t>(base->struct_size));
-    VB_CHECK(c.kind == VB_KIND_CROSSFORMER, "vb_create_crossformer: base.kind must be VB_KIND_CROSSFORMER");
-    validate_crossformer(c, *cfc);
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    VB_CHECK(e == cudaSuccess && ndev > 0, "vb_create_crossformer: no CUDA device available -- libvitb200 has no CPU fallback");
-    VB_CHECK(device >= 0 && device < ndev, "vb_create_crossformer: bad device index");
-    VB_CUDA(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    VB_CUDA(cudaGetDeviceProperties(&prop, device));
-    VB_CHECK(prop.major == 9 && prop.minor == 0, "vb_create_crossformer: libvitb200 is built for sm_90a (Hopper H100) only");
-    std::unique_ptr<vb_handle> h(new vb_handle());
-    h->cfg = c;
-    h->cfg.dim = cfc->dim[VB_CROSSFORMER_STAGES - 1];
-    h->cf = *cfc;
-    h->device = device;
-    h->build_expected();
-    *out = h.release();
-  });
+  return create_with("vb_create_crossformer", "vb_crossformer_config", VB_KIND_CROSSFORMER, "VB_KIND_CROSSFORMER",
+                                            base, cfc, device, out, validate_crossformer,
+                                            [&](vb_handle& h) { h.cf = *cfc; h.cfg.dim = cfc->dim[VB_CROSSFORMER_STAGES - 1]; });
 }
-
 int vb_create_nest(const vb_config* base, const vb_nest_config* nc, int device, vb_handle** out) {
-  return guarded(nullptr, [&] {
-    VB_CHECK(base != nullptr && nc != nullptr && out != nullptr, "vb_create_nest: null argument");
-    VB_CHECK(base->struct_size == static_cast<int32_t>(sizeof(vb_config)) || base->struct_size == VB_CONFIG_SIZE_ABI7,
-             "vb_config.struct_size mismatch (ABI)");
-    VB_CHECK(nc->struct_size == static_cast<int32_t>(sizeof(vb_nest_config)), "vb_nest_config.struct_size mismatch (ABI)");
-    vb_config c;
-    memset(&c, 0, sizeof c);
-    memcpy(&c, base, static_cast<size_t>(base->struct_size));
-    VB_CHECK(c.kind == VB_KIND_NEST, "vb_create_nest: base.kind must be VB_KIND_NEST");
-    validate_nest(c, *nc);
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    VB_CHECK(e == cudaSuccess && ndev > 0, "vb_create_nest: no CUDA device available -- libvitb200 has no CPU fallback");
-    VB_CHECK(device >= 0 && device < ndev, "vb_create_nest: bad device index");
-    VB_CUDA(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    VB_CUDA(cudaGetDeviceProperties(&prop, device));
-    VB_CHECK(prop.major == 9 && prop.minor == 0, "vb_create_nest: libvitb200 is built for sm_90a (Hopper H100) only");
-    std::unique_ptr<vb_handle> h(new vb_handle());
-    h->cfg = c;
-    h->ns = *nc;
-    h->cfg.dim = h->nest_last_dim();
-    h->device = device;
-    h->build_expected();
-    *out = h.release();
-  });
+  return create_with("vb_create_nest", "vb_nest_config", VB_KIND_NEST, "VB_KIND_NEST", base, nc, device, out, validate_nest,
+                                     [&](vb_handle& h) { h.ns = *nc; h.cfg.dim = h.nest_last_dim(); });
 }
-
 int vb_create_regionvit(const vb_config* base, const vb_regionvit_config* rc, int device, vb_handle** out) {
-  return guarded(nullptr, [&] {
-    VB_CHECK(base != nullptr && rc != nullptr && out != nullptr, "vb_create_regionvit: null argument");
-    VB_CHECK(base->struct_size == static_cast<int32_t>(sizeof(vb_config)) || base->struct_size == VB_CONFIG_SIZE_ABI7,
-             "vb_config.struct_size mismatch (ABI)");
-    VB_CHECK(rc->struct_size == static_cast<int32_t>(sizeof(vb_regionvit_config)), "vb_regionvit_config.struct_size mismatch (ABI)");
-    vb_config c;
-    memset(&c, 0, sizeof c);
-    memcpy(&c, base, static_cast<size_t>(base->struct_size));
-    VB_CHECK(c.kind == VB_KIND_REGIONVIT, "vb_create_regionvit: base.kind must be VB_KIND_REGIONVIT");
-    validate_regionvit(c, *rc);
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    VB_CHECK(e == cudaSuccess && ndev > 0, "vb_create_regionvit: no CUDA device available -- libvitb200 has no CPU fallback");
-    VB_CHECK(device >= 0 && device < ndev, "vb_create_regionvit: bad device index");
-    VB_CUDA(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    VB_CUDA(cudaGetDeviceProperties(&prop, device));
-    VB_CHECK(prop.major == 9 && prop.minor == 0, "vb_create_regionvit: libvitb200 is built for sm_90a (Hopper H100) only");
-    std::unique_ptr<vb_handle> h(new vb_handle());
-    h->cfg = c;
-    h->rv = *rc;
-    h->cfg.dim = rc->dims[VB_REGIONVIT_STAGES - 1];
-    h->device = device;
-    h->build_expected();
-    *out = h.release();
-  });
+  return create_with("vb_create_regionvit", "vb_regionvit_config", VB_KIND_REGIONVIT, "VB_KIND_REGIONVIT", base, rc,
+                                          device, out, validate_regionvit,
+                                          [&](vb_handle& h) { h.rv = *rc; h.cfg.dim = rc->dims[VB_REGIONVIT_STAGES - 1]; });
 }
 
 int vb_num_weights(vb_handle* h) { return h ? static_cast<int>(h->weights.size()) : -1; }
@@ -3817,11 +3516,7 @@ int vb_forward_tokens(vb_handle* h, const float* tokens, int32_t tokens_mem, int
     VB_CHECK(h != nullptr && tokens != nullptr && out != nullptr, "vb_forward_tokens: null argument");
     VB_CHECK(h->finalized, "vb_forward_tokens: call vb_finalize after setting the weights");
     VB_CHECK(batch > 0 && n > 0, "vb_forward_tokens: bad shape");
-    VB_CHECK(h->cfg.kind != VB_KIND_CVT, vb_handle::kCvtNoStages);
-    VB_CHECK(h->cfg.kind != VB_KIND_TWINS_SVT, vb_handle::kTwinsNoStages);
-    VB_CHECK(h->cfg.kind != VB_KIND_CROSSFORMER, vb_handle::kCrossformerNoStages);
-    VB_CHECK(h->cfg.kind != VB_KIND_NEST, vb_handle::kNestNoStages);
-    VB_CHECK(h->cfg.kind != VB_KIND_REGIONVIT, vb_handle::kRegionNoStages);
+    h->check_stage_entries();
     VB_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const long long before = launch_counter();
@@ -3912,13 +3607,7 @@ int vb_patch_to_emb(vb_handle* h, const float* patches, int32_t patches_mem, int
     VB_CHECK(h != nullptr && patches != nullptr && out != nullptr, "vb_patch_to_emb: null argument");
     VB_CHECK(h->finalized, "vb_patch_to_emb: call vb_finalize after setting the weights");
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT, "vb_patch_to_emb: CrossViT has two patch embeddings");
-    VB_CHECK(h->cfg.kind != VB_KIND_CCT, vb_handle::kCctNoStages);
-    VB_CHECK(h->cfg.kind != VB_KIND_LEVIT, vb_handle::kLevitNoStages);
-    VB_CHECK(h->cfg.kind != VB_KIND_CVT, vb_handle::kCvtNoStages);
-    VB_CHECK(h->cfg.kind != VB_KIND_TWINS_SVT, vb_handle::kTwinsNoStages);
-    VB_CHECK(h->cfg.kind != VB_KIND_CROSSFORMER, vb_handle::kCrossformerNoStages);
-    VB_CHECK(h->cfg.kind != VB_KIND_NEST, vb_handle::kNestNoStages);
-    VB_CHECK(h->cfg.kind != VB_KIND_REGIONVIT, vb_handle::kRegionNoStages);
+    h->check_stage_entries();
     VB_CHECK(rows > 0, "vb_patch_to_emb: bad shape");
     const size_t in_bytes = static_cast<size_t>(rows) * h->embed.patch.K * sizeof(float);
     const size_t out_bytes = static_cast<size_t>(rows) * h->cfg.dim * sizeof(float);
