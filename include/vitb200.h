@@ -46,7 +46,8 @@ typedef struct vb_handle vb_handle;
 
 enum { VB_KIND_VIT = 0, VB_KIND_DEEPVIT = 1, VB_KIND_CAIT = 2, VB_KIND_CROSSVIT = 3, VB_KIND_PARALLEL_VIT = 4,
        VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6, VB_KIND_CCT = 7, VB_KIND_LEVIT = 8,
-       VB_KIND_CVT = 9, VB_KIND_TWINS_SVT = 10, VB_KIND_CROSSFORMER = 11, VB_KIND_NEST = 12, VB_KIND_REGIONVIT = 13 };
+       VB_KIND_CVT = 9, VB_KIND_TWINS_SVT = 10, VB_KIND_CROSSFORMER = 11, VB_KIND_NEST = 12, VB_KIND_REGIONVIT = 13,
+       VB_KIND_ATS_VIT = 14 };
 enum { VB_CCT_POS_SINE = 0, VB_CCT_POS_LEARNABLE = 1, VB_CCT_POS_NONE = 2 };   /* cct.py:233-234,250-256 */
 enum { VB_PRECISION_FP32 = 0, VB_PRECISION_BF16 = 1 };
 enum { VB_POOL_CLS = 0, VB_POOL_MEAN = 1 };
@@ -282,6 +283,48 @@ typedef struct vb_regionvit_config {
  * vb_finalize stores each stage's Embedding transposed to [4][(2 ws - 1)^2] with the row offset slowest, the index convention of
  * the windowed attention kernels. */
 VB_API int vb_create_regionvit(const vb_config* base, const vb_regionvit_config* rv, int device, vb_handle** out);
+
+/* ATS-ViT (ats_vit.py:260-318, adaptive token sampling), appended within ABI 7.  Layer L samples at most
+ * max_tokens_per_depth[L] tokens when the batch's padded token count exceeds it (ats_vit.py:213); the first `depth` entries are
+ * used, non-increasing and positive (the reference's assert messages). */
+#define VB_ATS_MAX_DEPTH 64
+typedef struct vb_ats_vit_config {
+  int32_t struct_size;            /* sizeof(vb_ats_vit_config) */
+  int32_t max_tokens_per_depth[VB_ATS_MAX_DEPTH];
+} vb_ats_vit_config;
+
+/* ats_vit.ViT.__init__: `base` supplies the ViT fields (precision, image / patch sizes, channels, num_classes, dim, depth, heads,
+ * dim_head, mlp_dim, max_batch); its kind must be VB_KIND_ATS_VIT, the pool is always the cls row.  Weights are ViT's names and
+ * shapes (SURVEY.md App. B), to_out always present.  Images may have at most 65,535 patches.  The sampling noise is
+ * u = (word 0 of Philox4x32-10 >> 8) * 2^-24 with the 64-bit seed as key and the counter (j | k << 16, b, d_lo, d_hi): j the
+ * column of the reference's left-padded [b, K, n - 1] noise tensor, k the draw, b the image, d a 64-bit counter on the device
+ * that advances once per layer that samples.  The seed is 0 at creation. */
+VB_API int vb_create_ats_vit(const vb_config* base, const vb_ats_vit_config* ats, int device, vb_handle** out);
+/* Sets the Philox key and resets the draw counter d to 0 (waits for the device first). */
+VB_API int vb_ats_set_seed(vb_handle* h, uint64_t seed);
+/* vb_forward (same graph capture and replay) plus the returned token ids: logits [batch, num_classes], token_ids
+ * int32 [batch, P - 1] and count (one int32) in host memory, P - 1 the most tokens the last layer can keep.  Columns [0, count) are
+ * the reference's `token_ids[:, 1:] - 1` (ats_vit.py:315): each image's kept patch ids in ascending order, left-padded with -1;
+ * the columns from count on are -1.  Results depend on the whole batch (through the padded length), as in the reference. */
+VB_API int vb_forward_ats(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, int32_t img_h, int32_t img_w, float* logits,
+                          int32_t* token_ids, int32_t* count, void* stream);
+/* After a forward: whether layer `layer` sampled (*sampled = 1 when the batch's token count exceeded K there), the positions its K
+ * draws chose, draws int32 [batch, K] (argmax + 1 in the reference's left-padded layout; all -1 when it did not sample), and the
+ * tokens each image kept after it, counts int32 [batch].  A layer whose input can never exceed K is refused. */
+VB_API int vb_ats_last_draws(vb_handle* h, int32_t layer, int32_t* draws, int32_t* counts, int32_t* sampled);
+/* One ATS sampling step on its own (the engine's ats_sample): qkv float32 [B * P, ld] fused q|k|v rows of B images at pitch P
+ * (head h at columns h*dh, HD + h*dh, 2 HD + h*dh), rows int32 [B] the live rows of each image (cls + its c_b tokens; C = the
+ * maximum c_b), K draws per image with the Philox key `seed` and draw counter `counter`, scale the softmax scale.  Outputs:
+ * sel int32 [B, 1 + min(P - 1, K)] (0, then the kept compact indices in ascending order), rows_new int32 [B] and draws int32
+ * [B, K] (argmax + 1 in the left-padded layout; -1 when C <= K and nothing was drawn).  bf16 rounds qkv to bfloat16 first. */
+VB_API int vb_op_ats_sample(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t P, int32_t heads, int32_t dh, float scale,
+                            const int32_t* rows, int32_t K, uint64_t seed, uint64_t counter, int32_t* sel, int32_t* rows_new,
+                            int32_t* draws);
+/* Plain attention over fused q|k|v rows (qkv float32 [B * n, ld]) with image b's keys j >= nk_img[b] masked (weight 0), scale
+ * dh^-0.5: the dim_head-64 flash kernels in bf16 (resident for n <= 256, streaming above), else the materialised-scores path.
+ * out float32 [B * n, ldo]; every row is written, the rows of masked queries too (finite). */
+VB_API int vb_op_masked_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t n, int32_t heads, int32_t dh,
+                                  const int32_t* nk_img, float* out, int32_t ldo, int32_t iters, float* elapsed_ms);
 
 /* Replaces Keras variable assignment: one call per weight, names/shapes/layouts per SURVEY.md App. B
  * (Dense kernel [in,out], float32).  shape/ndim are checked against the config. */

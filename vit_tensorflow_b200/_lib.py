@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "libvitb200.so")   # VB_LIB_PATH: developer A/B builds
 
 KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6, "cct": 7, "levit": 8,
-        "cvt": 9, "twins_svt": 10, "crossformer": 11, "nest": 12, "regionvit": 13}
+        "cvt": 9, "twins_svt": 10, "crossformer": 11, "nest": 12, "regionvit": 13, "ats_vit": 14}
 PRECISION = {"fp32": 0, "float32": 0, "bf16": 1, "bfloat16": 1}
 MEM_HOST, MEM_DEVICE = 0, 1
 ABI_VERSION = 7                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
@@ -83,6 +83,13 @@ class VbRegionvitConfig(C.Structure):
         (n, C.c_int32) for n in ("window_size", "local_patch_size", "tokenize_local_3_conv", "use_peg", "mlp_mult")]
 
 
+ATS_MAX_DEPTH = 64                                   # VB_ATS_MAX_DEPTH
+
+
+class VbAtsVitConfig(C.Structure):
+    _fields_ = [("struct_size", C.c_int32), ("max_tokens_per_depth", C.c_int32 * ATS_MAX_DEPTH)]
+
+
 class VbError(RuntimeError):
     pass
 
@@ -100,6 +107,14 @@ SIGNATURES = {
     "vb_create_crossformer": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbCrossformerConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_nest": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbNestConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_regionvit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbRegionvitConfig), C.c_int, C.POINTER(C.c_void_p)]),
+    "vb_create_ats_vit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbAtsVitConfig), C.c_int, C.POINTER(C.c_void_p)]),
+    "vb_ats_set_seed": (C.c_int, [C.c_void_p, C.c_uint64]),
+    "vb_forward_ats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                 C.c_void_p]),
+    "vb_ats_last_draws": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vb_op_ats_sample": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 5 + [C.c_float, C.c_void_p, C.c_int32, C.c_uint64, C.c_uint64] +
+                         [C.c_void_p] * 3),
+    "vb_op_masked_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, _f32p]),
     "vb_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, _i64p, C.c_int32]),
     "vb_num_weights": (C.c_int, [C.c_void_p]),
     "vb_weight_info": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), _i64p, C.POINTER(C.c_int32)]),
@@ -371,6 +386,30 @@ def op_r2l_attention(qkv, B, lh, lw, rh, rw, heads, dh, table, window_size, prec
     ms = C.c_float(0)
     check(load().vb_op_r2l_attention(PRECISION[precision], _ptr(qkv), ld, B, lh, lw, rh, rw, heads, dh, _ptr(table), window_size, _ptr(out),
                                      ldo, iters, C.byref(ms)))
+    return out, (ms.value if iters > 0 else None)
+
+
+def op_ats_sample(qkv, B, P, heads, dh, scale, rows, K, seed=0, counter=0, precision="bf16"):
+    """ATS-ViT's sampling step (vb_op_ats_sample) on fused q|k|v rows [B*P, ld] of images with rows[b] live rows.  Returns
+    (sel [B, 1 + min(P - 1, K)], rows_new [B], draws [B, K])."""
+    qkv = _f32(qkv)
+    rows = np.ascontiguousarray(rows, np.int32)
+    Pn = 1 + min(P - 1, K)
+    sel, rows_new, draws = np.zeros((B, Pn), np.int32), np.zeros(B, np.int32), np.zeros((B, K), np.int32)
+    check(load().vb_op_ats_sample(PRECISION[precision], _ptr(qkv), qkv.shape[1], B, P, heads, dh, scale, _ptr(rows), K, seed, counter,
+                                  _ptr(sel), _ptr(rows_new), _ptr(draws)))
+    return sel, rows_new, draws
+
+
+def op_masked_attention(qkv, B, n, heads, dh, nk_img, precision="bf16", iters=0):
+    """Attention with a key count per image (vb_op_masked_attention): qkv [B*n, ld] fused q|k|v rows.  Returns (out [B*n, heads*dh],
+    ms or None)."""
+    qkv = _f32(qkv)
+    nk = np.ascontiguousarray(nk_img, np.int32)
+    out = np.zeros((B * n, heads * dh), np.float32)
+    ms = C.c_float(0)
+    check(load().vb_op_masked_attention(PRECISION[precision], _ptr(qkv), qkv.shape[1], B, n, heads, dh, _ptr(nk), _ptr(out), heads * dh,
+                                        iters, C.byref(ms)))
     return out, (ms.value if iters > 0 else None)
 
 

@@ -56,11 +56,12 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
 
 constexpr int FLASH_BIAS_MAX = 4096;   // fmap^2 of the largest relative-position table (16 KB of shared memory)
 
-template <int D, bool BIAS, bool WIN>
+template <int D, bool BIAS, bool WIN, bool MASK = false>
 __global__ void __launch_bounds__(128)
 attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloat16* __restrict__ k, int ldk,
                   const __nv_bfloat16* __restrict__ v, int ldv, __nv_bfloat16* __restrict__ out, int ldo, int heads, int nq, int nk,
-                  float scale_log2, const float* __restrict__ pos_tab, int fmap, int step, int gelu_out, Window win) {
+                  float scale_log2, const float* __restrict__ pos_tab, int fmap, int step, int gelu_out, Window win,
+                  const int* __restrict__ nk_img) {
   constexpr int FP = D + 8;          // smem row pitch (bf16): +16 bytes keeps the fragment loads bank-conflict free
   constexpr bool WB = BIAS && WIN;   // the windowed-bias form (below)
   extern __shared__ float tab[];     // BIAS: [fmap^2] of this head / WB: the (2p-1)^2 window table; times log2(e)
@@ -71,12 +72,13 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
   const int bh = blockIdx.x / qtiles, b = bh / heads, h = bh % heads;
   const int i0 = (blockIdx.x % qtiles) * FQ;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nblk = (nk + FK - 1) / FK;
+  int nblk = (nk + FK - 1) / FK;
   // WB: batch entry b is windows [b * G, b * G + G) of the win.count windows, G = floor(64 / p^2) for p^2 <= 32 and 1 above, so
   // nq == nk == G * p^2; token t of the entry is token t % p^2 of window b * G + t / p^2.  The last entry may hold fewer windows:
   // nqv / nkv are the entry's live tokens.
   const int wn = WB ? win.p * win.p : 1, G = WB ? (wn <= 32 ? FQ / wn : 1) : 1;
-  const int nqv = WB ? min(nq, (win.count - b * G) * wn) : nq, nkv = WB ? nqv : nk;
+  const int nqv = WB ? min(nq, (win.count - b * G) * wn) : nq;
+  int nkv = WB ? nqv : nk;
   // row of token i of this CTA's batch entry in the q / k / v / out matrices
   auto qrow_of = [&](int i) -> size_t {
     if (WB) return static_cast<size_t>(win.row(static_cast<long long>(b) * G + i / wn, i % wn));
@@ -89,6 +91,10 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
 
   pdl_wait();                 // Q/K/V come from the previous kernel of the stream
   pdl_launch_dependents();
+  if (MASK) {                 // keys >= nk_img[b] masked: only the blocks that hold a valid key (at least one: the cls row)
+    nkv = min(nk, nk_img[b]);
+    nblk = (nkv + FK - 1) / FK;
+  }
 
   // rows past n are zero-filled (never read from the next image); D / 8 16-byte vectors per row
   constexpr int VR = D / 8, VS = D == 64 ? 3 : 2;                  // VR = 2^VS
@@ -365,10 +371,12 @@ __device__ __forceinline__ void resident_block(const uint32_t (&qf)[DH / 16][4],
   }
 }
 
+// MASK: image b's keys >= nk_img[b] are masked; only the key blocks that hold a valid key run.
+template <bool MASK>
 __global__ void __launch_bounds__((RW + 1) * 32, 1)
 attn_resident_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
                      const __grid_constant__ CUtensorMap tv, __nv_bfloat16* __restrict__ out, int ldo, int heads, int nq, int nk,
-                     int qbox, int kbox, long long units, float scale_log2) {
+                     int qbox, int kbox, long long units, float scale_log2, const int* __restrict__ nk_img) {
   extern __shared__ __align__(16) uint8_t rsmem[];
   const uint32_t base = (smem_u32(rsmem) + 1023) & ~1023u;
   const uint32_t bars = base + 2 * RBUF;   // full[0], full[1], empty[0], empty[1]
@@ -419,6 +427,7 @@ attn_resident_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
     const int c = static_cast<int>(bc % chunks), b = static_cast<int>(bc / chunks);
     const int i0 = c * RQ, slices = (min(RQ, nq - i0) + 15) / 16;
     const uint32_t tQ = base + s * RBUF, tK = tQ + RTILE, tV = tQ + 2 * RTILE;
+    const int nkb = MASK ? min(nk, nk_img[b]) : nk;
     mbar_wait(full_bar(s), (it >> 1) & 1);
     for (int sl = (warp - rot + RW) % RW; sl < slices; sl += RW) {
       const int r16 = sl * 16;
@@ -430,8 +439,8 @@ attn_resident_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
       for (int n = 0; n < DH / 8; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
       float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
 
-      for (int j0 = 0; j0 + 64 <= nk; j0 += 64) resident_block<false>(qf, o, m_run, l_run, tK, tV, j0, nk, scale_log2, lane);
-      if (nk % 64) resident_block<true>(qf, o, m_run, l_run, tK, tV, nk & ~63, nk, scale_log2, lane);
+      for (int j0 = 0; j0 + 64 <= nkb; j0 += 64) resident_block<false>(qf, o, m_run, l_run, tK, tV, j0, nkb, scale_log2, lane);
+      if (nkb % 64) resident_block<true>(qf, o, m_run, l_run, tK, tV, nkb & ~63, nkb, scale_log2, lane);
 
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
@@ -465,8 +474,10 @@ attn_resident_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
 }
 
 // The resident-head form of attention_fast's plain case; false (nothing launched) when the shape is not one it covers.
+// nk_img (may be null): per-image key counts (attention_masked).
 bool attention_resident(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, int ldk, const __nv_bfloat16* v, int ldv,
-                        __nv_bfloat16* out, int ldo, int B, int nq, int nk, int heads, float scale_log2, cudaStream_t s) {
+                        __nv_bfloat16* out, int ldo, int B, int nq, int nk, int heads, float scale_log2, cudaStream_t s,
+                        const int* nk_img = nullptr) {
   if (nk > RQ || (ldo % 8)) return false;
   const int qbox = std::min(RQ, (nq + 15) & ~15), kbox = (nk + 15) & ~15;
   const uint64_t inner = static_cast<uint64_t>(heads) * DH;
@@ -475,8 +486,10 @@ bool attention_resident(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k,
   const CUtensorMap tv = make_tmap_3d(v, inner, nk, B, static_cast<uint64_t>(ldv) * 2, static_cast<uint64_t>(nk) * ldv * 2, DH, kbox);
   const long long units = static_cast<long long>(B) * heads * ((nq + RQ - 1) / RQ);
   static unsigned long long seen[4] = {0, 0, 0, 0};
-  if (first_use_on_this_device(seen))
-    VB_CUDA(cudaFuncSetAttribute(attn_resident_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RSMEM));
+  if (first_use_on_this_device(seen)) {
+    VB_CUDA(cudaFuncSetAttribute(attn_resident_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, RSMEM));
+    VB_CUDA(cudaFuncSetAttribute(attn_resident_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, RSMEM));
+  }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(static_cast<unsigned>(units < sm_count() ? units : sm_count()));
   cfg.blockDim = dim3((RW + 1) * 32);
@@ -487,7 +500,11 @@ bool attention_resident(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k,
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  VB_CUDA(cudaLaunchKernelEx(&cfg, attn_resident_kernel, tq, tk, tv, out, ldo, heads, nq, nk, qbox, kbox, units, scale_log2));
+  if (nk_img != nullptr)
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_resident_kernel<true>, tq, tk, tv, out, ldo, heads, nq, nk, qbox, kbox, units, scale_log2, nk_img));
+  else
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_resident_kernel<false>, tq, tk, tv, out, ldo, heads, nq, nk, qbox, kbox, units, scale_log2,
+                               static_cast<const int*>(nullptr)));
   return true;
 }
 
@@ -499,7 +516,7 @@ void launch_window_bias(cudaLaunchConfig_t& cfg, const __nv_bfloat16* q, int ldq
     VB_CUDA(cudaFuncSetAttribute(attn_flash_kernel<D, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FLASH_BIAS_MAX * 4));
   const int HD = heads * D;
   VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<D, true, true>, q, ldq, q + HD, ldq, q + 2 * HD, ldq, out, ldo, heads, n, n,
-                             scale_log2, pb.table, 0, 1, 0, win));
+                             scale_log2, pb.table, 0, 1, 0, win, static_cast<const int*>(nullptr)));
 }
 
 // CrossFormer's attention: windows of B = win.count images' maps, q | k | v at columns [0, HD), [HD, 2 HD), [2 HD, 3 HD) of the
@@ -745,10 +762,10 @@ bool attention_block(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* out, int l
   cfg.numAttrs = 1;
   if (dh == 32)
     VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<32, false, true>, qkv, ld, qkv + HD, ld, qkv + 2 * HD, ld, out, ldo, heads, n, n,
-                               scale_log2, static_cast<const float*>(nullptr), 0, 1, 0, win));
+                               scale_log2, static_cast<const float*>(nullptr), 0, 1, 0, win, static_cast<const int*>(nullptr)));
   else
     VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<64, false, true>, qkv, ld, qkv + HD, ld, qkv + 2 * HD, ld, out, ldo, heads, n, n,
-                               scale_log2, static_cast<const float*>(nullptr), 0, 1, 0, win));
+                               scale_log2, static_cast<const float*>(nullptr), 0, 1, 0, win, static_cast<const int*>(nullptr)));
   count_launch();
   note_attention_path(ATTN_PATH_FLASH);
   return true;
@@ -795,13 +812,41 @@ bool attention_fast<__nv_bfloat16>(const __nv_bfloat16* q, int ldq, const __nv_b
   cfg.numAttrs = 1;
   if (pb != nullptr)
     VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<DH, true, false>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
-                               pb->table, pb->fmap, pb->step, static_cast<int>(pb->gelu_out), Window()));
+                               pb->table, pb->fmap, pb->step, static_cast<int>(pb->gelu_out), Window(),
+                               static_cast<const int*>(nullptr)));
   else if (win != nullptr)
     VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<DH, false, true>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
-                               static_cast<const float*>(nullptr), 0, 1, 0, *win));
+                               static_cast<const float*>(nullptr), 0, 1, 0, *win, static_cast<const int*>(nullptr)));
   else
     VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<DH, false, false>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
-                               static_cast<const float*>(nullptr), 0, 1, 0, Window()));
+                               static_cast<const float*>(nullptr), 0, 1, 0, Window(), static_cast<const int*>(nullptr)));
+  count_launch();
+  note_attention_path(ATTN_PATH_FLASH);
+  return true;
+}
+
+bool attention_masked(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, int ldk, const __nv_bfloat16* v, int ldv,
+                      __nv_bfloat16* out, int ldo, int B, int nq, int nk, int heads, int dh, cudaStream_t s, float scale,
+                      const int* nk_img) {
+  if (dh != DH || nq < 1 || nk < 1 || B < 1 || (ldq % 8) || (ldk % 8) || (ldv % 8) || (ldo % 2)) return false;
+  if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
+       reinterpret_cast<uintptr_t>(out)) % 16) return false;
+  const float scale_log2 = (scale > 0.f ? scale : 1.0f / sqrtf(static_cast<float>(dh))) * 1.4426950408889634f;
+  if (!attention_resident(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, heads, scale_log2, s, nk_img)) {
+    const long long blocks = static_cast<long long>(B) * heads * ((nq + FQ - 1) / FQ);
+    if (blocks > 0x7fffffffLL) return false;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(static_cast<unsigned>(blocks));
+    cfg.blockDim = dim3(128);
+    cfg.stream = s;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<DH, false, false, true>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
+                               static_cast<const float*>(nullptr), 0, 1, 0, Window(), nk_img));
+  }
   count_launch();
   note_attention_path(ATTN_PATH_FLASH);
   return true;

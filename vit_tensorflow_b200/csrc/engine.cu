@@ -514,6 +514,65 @@ struct vb_handle {
   static constexpr int kRvHeads = 4, kRvDh = 32, kRvInner = kRvHeads * kRvDh;   // R2LTransformer's defaults (:119, :239)
   struct XBlock { std::vector<LayerW> sm_layers, lg_layers; Norm sm_final, lg_final; std::vector<CrossW> sm_attend_lg, lg_attend_sm; };
   std::vector<XBlock> xblocks;
+  // ATS-ViT (ats_vit.py:222-318): ViT's weights and layers; the sampling state of a forward lives in ats_dev (AtsPlan), the
+  // Philox key and the 64-bit draw counter in ats_rng
+  vb_ats_vit_config ats{};
+  DevMem ats_dev, ats_rng;
+  // Layer L runs at row pitch P[L]; P[L + 1] = 1 + min(P[L] - 1, K_L).  A layer with P[L] - 1 <= K_L can never sample and launches
+  // nothing beyond a ViT layer.  The int state: per slot (one for the embedding, one more per layer that can sample) the live
+  // rows of every image (rows, slot-major), C, and the token ids at the slot's pitch; the draws of every layer that can sample;
+  // the returned ids [B, P[depth] - 1].
+  struct AtsPlan {
+    int B = 0;
+    std::vector<int> P, slot, slot_P;
+    std::vector<bool> can;
+    std::vector<size_t> ids, draws;
+    size_t rows = 0, C = 0, out = 0, total = 0;
+  };
+  AtsPlan ats_last;
+  AtsPlan ats_plan(int B, int n0) const {
+    AtsPlan p;
+    p.B = B;
+    p.P.push_back(n0); p.slot.push_back(0); p.slot_P.push_back(n0);
+    for (int L = 0; L < cfg.depth; ++L) {
+      const int P = p.P.back(), K = ats.max_tokens_per_depth[L];
+      const bool can = P - 1 > K;
+      p.can.push_back(can);
+      if (can) p.slot_P.push_back(1 + K);
+      p.P.push_back(can ? 1 + K : P);
+      p.slot.push_back(static_cast<int>(p.slot_P.size()) - 1);
+    }
+    const size_t slots = p.slot_P.size();
+    size_t off = 0;
+    p.rows = off; off += slots * B;
+    p.C = off; off += slots;
+    for (size_t i = 0; i < slots; ++i) { p.ids.push_back(off); off += static_cast<size_t>(B) * p.slot_P[i]; }
+    for (int L = 0; L < cfg.depth; ++L) { p.draws.push_back(off); if (p.can[L]) off += static_cast<size_t>(B) * ats.max_tokens_per_depth[L]; }
+    p.out = off; off += static_cast<size_t>(B) * (p.P.back() - 1);
+    p.total = off;
+    return p;
+  }
+  unsigned long long* ats_rng_ptr() {
+    if (ats_rng.p == nullptr) {
+      ats_rng.ensure(2 * sizeof(unsigned long long));
+      VB_CUDA(cudaMemset(ats_rng.p, 0, 2 * sizeof(unsigned long long)));
+      VB_CUDA(cudaDeviceSynchronize());                // before any forward reads it, on whatever stream that runs
+    }
+    return static_cast<unsigned long long*>(ats_rng.p);
+  }
+  // the host side of an ATS forward of a batch of h x w images, before the launches or graph lookup: the state buffer (a new
+  // allocation invalidates the captured graphs that point into the old one)
+  void ats_prepare(int B, int H, int Wd) {
+    VB_CHECK(H % cfg.patch_h == 0 && Wd % cfg.patch_w == 0, "Image dimensions must be divisible by the patch size.");
+    const long long np = static_cast<long long>(H / cfg.patch_h) * (Wd / cfg.patch_w);
+    VB_CHECK(np + 1 <= ATS_MAX_TOKENS, "ATS-ViT: at most 65,535 patches per image (the sampling noise keys a token by 16 bits)");
+    VB_CHECK(np + 1 <= embed.n_pos, "image has more patches than pos_embedding rows");
+    ats_last = ats_plan(B, static_cast<int>(np) + 1);
+    const void* before = ats_dev.p;
+    ats_dev.ensure(ats_last.total * sizeof(int));
+    if (before != nullptr && ats_dev.p != before) drop_graphs();
+    ats_rng_ptr();
+  }
   Norm head_norm, sm_head_norm, lg_head_norm;
   Linear head, sm_head, lg_head;
 
@@ -571,7 +630,7 @@ struct vb_handle {
   void expect_layer(const std::string& pre, int dim, int heads, int dh, int mlp, int kind) {
     const int inner = heads * dh;
     expect_ln(pre + "attn_norm", dim);
-    if (kind == VB_KIND_VIT || kind == VB_KIND_DEEPVIT) expect_dense(pre + "to_qkv", dim, 3 * inner, false);
+    if (kind == VB_KIND_VIT || kind == VB_KIND_DEEPVIT || kind == VB_KIND_ATS_VIT) expect_dense(pre + "to_qkv", dim, 3 * inner, false);
     else { expect_dense(pre + "to_q", dim, inner, false); expect_dense(pre + "to_kv", dim, 2 * inner, false); }
     if (kind == VB_KIND_DEEPVIT) { expect(pre + "reattn_weights", {heads, heads}); expect_ln(pre + "reattn_norm", heads); }
     if (kind == VB_KIND_CAIT) { expect(pre + "mix_pre", {heads, heads}); expect(pre + "mix_post", {heads, heads}); }
@@ -584,7 +643,7 @@ struct vb_handle {
   void build_expected() {
     const vb_config& c = cfg;
     const int C = c.channels;
-    if (c.kind == VB_KIND_VIT || c.kind == VB_KIND_DEEPVIT || c.kind == VB_KIND_PARALLEL_VIT) {
+    if (c.kind == VB_KIND_VIT || c.kind == VB_KIND_DEEPVIT || c.kind == VB_KIND_PARALLEL_VIT || c.kind == VB_KIND_ATS_VIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       expect("pos_embedding", {1, np + 1, c.dim});
       expect("cls_token", {1, 1, c.dim});
@@ -954,7 +1013,7 @@ struct vb_handle {
     // the tensor-core attention path for e.g. dim_head 48 / 32 (the head-mixing variants have their own kernel, attn_mix).
     const bool to_out_present = has(pre + "to_out.kernel");
     if (bf16() && dh < 64 && dh % 8 == 0 && to_out_present && dim % 8 == 0 && getenv("VB_NO_HEAD_PAD") == nullptr &&
-        (kind == VB_KIND_VIT || kind == VB_KIND_CROSSVIT)) {
+        (kind == VB_KIND_VIT || kind == VB_KIND_CROSSVIT || kind == VB_KIND_ATS_VIT)) {
       const int dhp = 64;
       auto padded = [&](const std::string& n, int other, int groups, int pad_rows) {
         owned.emplace_back(new DevMem());
@@ -963,7 +1022,7 @@ struct vb_handle {
         pad_heads_f32(W(n), wp, other, groups, heads, dh, dhp, pad_rows, 0);
         woverride[n] = wp;
       };
-      if (kind == VB_KIND_VIT) padded(pre + "to_qkv.kernel", dim, 3, 0);
+      if (kind == VB_KIND_VIT || kind == VB_KIND_ATS_VIT) padded(pre + "to_qkv.kernel", dim, 3, 0);
       else { padded(pre + "to_q.kernel", dim, 1, 0); padded(pre + "to_kv.kernel", dim, 2, 0); }
       padded(pre + "to_out.kernel", dim, 1, 1);
       dh = dhp;
@@ -976,7 +1035,7 @@ struct vb_handle {
     l.folded = bf16() && fold_ok && dim % 64 == 0 && inner % 64 == 0 && mlp % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr;
     const Norm* fa = l.folded ? &l.attn_norm : nullptr;
     const Norm* ff = l.folded ? &l.ff_norm : nullptr;
-    if (kind == VB_KIND_VIT || kind == VB_KIND_DEEPVIT) { l.fused_qkv = true; l.to_qkv = make_linear(pre + "to_qkv", dim, 3 * inner, false, fa); }
+    if (kind == VB_KIND_VIT || kind == VB_KIND_DEEPVIT || kind == VB_KIND_ATS_VIT) { l.fused_qkv = true; l.to_qkv = make_linear(pre + "to_qkv", dim, 3 * inner, false, fa); }
     else if (bf16() && fold_ok && dim % 8 == 0) {   // self-attention only: q and kv read the same rows -> one GEMM
       l.fused_qkv = true;
       l.to_qkv = make_linear_pair(pre + "to_q", inner, pre + "to_kv", 2 * inner, dim, fa);
@@ -1057,7 +1116,7 @@ struct vb_handle {
     woverride.clear();
     drop_graphs();
     const vb_config& c = cfg;
-    if (c.kind == VB_KIND_VIT || c.kind == VB_KIND_DEEPVIT || c.kind == VB_KIND_PARALLEL_VIT) {
+    if (c.kind == VB_KIND_VIT || c.kind == VB_KIND_DEEPVIT || c.kind == VB_KIND_PARALLEL_VIT || c.kind == VB_KIND_ATS_VIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       embed = make_embed("", c.patch_h, c.patch_w, c.dim, np + 1);
       for (int L = 0; L < c.depth; ++L) {
@@ -1766,10 +1825,22 @@ struct vb_handle {
   template <typename T>
   void layer_self(T* X, int B, int rows, int dim, const LayerW& l, cudaStream_t s, float* stats = nullptr,
                   bool* stats_valid = nullptr) {
-    const int M = B * rows, inner = l.heads * l.dim_head;
+    const int M = B * rows;
     const bool fold = l.folded && stats != nullptr;
     if (fold && !*stats_valid) { ensure_stats(X, dim, stats, M, s); *stats_valid = true; }
     T* Y = arena.get<T>(static_cast<size_t>(M) * dim);
+    attend_self<T>(X, B, rows, dim, l, s, fold ? stats : nullptr, Y);
+    feed_forward<T>(X, M, dim, l, Y, s, fold ? stats : nullptr);
+  }
+  // The attention half of layer_self: X += to_out(attention(LN(X))) (the residual carried by to_out's epilogue), with the row
+  // statistics `stats` (non-null iff the layer is folded; valid on entry) kept up to date.  Y [M, dim]: LayerNorm scratch of the
+  // unfolded layer.  nk_img (may be null): image b's keys >= nk_img[b] masked (ATS-ViT's dead rows).  Returns the fused q|k|v rows
+  // (null for separate to_q / to_kv).
+  template <typename T>
+  const T* attend_self(T* X, int B, int rows, int dim, const LayerW& l, cudaStream_t s, float* stats, T* Y, const int* nk_img = nullptr) {
+    const int M = B * rows, inner = l.heads * l.dim_head;
+    const bool fold = stats != nullptr;
+    const T* qkv = nullptr;
     T* O = arena.get<T>(static_cast<size_t>(M) * inner);
     const T* A = X;
     Epi eq;
@@ -1779,8 +1850,11 @@ struct vb_handle {
       T* QKV = arena.get<T>(static_cast<size_t>(M) * 3 * inner);
       Epi e = eq; e.bias = l.to_qkv.ln_c2;
       linear<T>(A, dim, M, l.to_qkv, QKV, 3 * inner, e, s);
-      attention<T>(QKV, 3 * inner, QKV + inner, 3 * inner, QKV + 2 * inner, 3 * inner, O, inner, B, rows, rows, l, s);
+      if (nk_img != nullptr) attention_masked_dispatch<T>(QKV, 3 * inner, O, inner, B, rows, l, s, nk_img);
+      else attention<T>(QKV, 3 * inner, QKV + inner, 3 * inner, QKV + 2 * inner, 3 * inner, O, inner, B, rows, rows, l, s);
+      qkv = QKV;
     } else {
+      VB_CHECK(nk_img == nullptr, "internal: masked attention reads fused q|k|v rows");
       T* Q = arena.get<T>(static_cast<size_t>(M) * inner);
       T* KV = arena.get<T>(static_cast<size_t>(M) * 2 * inner);
       Epi e1 = eq; e1.bias = l.to_q.ln_c2;
@@ -1797,7 +1871,82 @@ struct vb_handle {
       add_tokens<T>(X, O, static_cast<long long>(M) * dim, s);   // vit.py:53: identity out-projection
       if (fold) ensure_stats(X, dim, stats, M, s);
     }
-    feed_forward<T>(X, M, dim, l, Y, s, fold ? stats : nullptr);
+    return qkv;
+  }
+  // Plain attention over the fused q|k|v rows with image b's keys >= nk_img[b] masked: the flash kernels at dh 64 (bf16), else the
+  // materialised-scores path with the mask in its softmax
+  template <typename T>
+  void attention_masked_dispatch(const T* qkv, int ld, T* out, int ldo, int B, int n, const LayerW& l, cudaStream_t s, const int* nk_img) {
+    const int heads = l.heads, dh = l.dim_head, HD = heads * dh;
+    const float scale = 1.0f / sqrtf(static_cast<float>(l.dh_model));
+    ProfScope ps(this, PROF_ATTN, 4.0 * B * heads * n * n * dh, static_cast<double>(sizeof(T)) * B * heads * dh * 4.0 * n, s);
+    if (masked_flash(qkv, ld, out, ldo, B, n, heads, dh, s, scale, nk_img)) return;
+    VB_CHECK(dh == l.dh_model, "internal: a head-padded layer must run on the fused attention kernel");
+    float* S = arena.get<float>(static_cast<size_t>(B) * heads * n * n);
+    attention_generic_masked<T>(qkv, ld, qkv + HD, ld, qkv + 2 * HD, ld, out, ldo, S, B, n, n, heads, dh, s, scale, nk_img);
+  }
+  static bool masked_flash(const float*, int, float*, int, int, int, int, int, cudaStream_t, float, const int*) { return false; }
+  static bool masked_flash(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* out, int ldo, int B, int n, int heads, int dh, cudaStream_t s,
+                           float scale, const int* nk_img) {
+    const int HD = heads * dh;
+    return attention_masked(qkv, ld, qkv + HD, ld, qkv + 2 * HD, ld, out, ldo, B, n, n, heads, dh, s, scale, nk_img);
+  }
+
+  // ATS-ViT's forward (ats_vit.py:300-318, Transformer.call :236-258) in the compact row layout of ats.cu: image b's rows at the
+  // layer's pitch P[L] are [cls, its kept tokens in ascending id order, dead rows].  Masked keys get weight exactly 0 in the
+  // reference (exp(-FLT_MAX - max) underflows), and its pad rows never reach the cls row or a kept row, so the logits depend on
+  // the kept rows alone.  Every decision that depends on the data (whether a layer samples, C > K) is taken on the device.
+  template <typename T>
+  void ats_forward(const float* img, int B, int H, int Wd, float* logits, cudaStream_t s) {
+    const vb_config& c = cfg;
+    int rows = 0;
+    float* stats = nullptr;
+    T* X = embed_tokens<T>(embed, img, B, H, Wd, c.patch_h, c.patch_w, &rows, s, &stats);
+    const AtsPlan& p = ats_last;
+    VB_CHECK(p.B == B && p.P[0] == rows && ats_dev.bytes >= p.total * sizeof(int), "internal: ATS state not prepared for this batch");
+    int* st = static_cast<int*>(ats_dev.p);
+    unsigned long long* rng = ats_rng_ptr();
+    { ProfScope ps(this, PROF_OTHER, 0.0, 4.0 * B * rows, s); ats_init(st + p.rows, st + p.C, st + p.ids[0], B, rows, s); }
+    bool sv = stats != nullptr;
+    for (int L = 0; L < c.depth; ++L) X = ats_layer<T>(X, B, L, p, st, rng, s, stats, &sv);
+    classify<T>(X, p.P[c.depth], c.dim, head_norm, head, B, 0, logits, false, s);
+    const int f = p.slot[c.depth];
+    ProfScope ps(this, PROF_OTHER, 0.0, 8.0 * B * p.P[c.depth], s);
+    ats_ids_out(st + p.ids[f], p.P[c.depth], st + p.rows + static_cast<size_t>(f) * B, st + p.C + f, st + p.out, B, s);
+  }
+  // One ATS layer (ats_vit.py:246-256): the LayerNorm-folded to_qkv, the masked attention and the residual to_out over all P[L]
+  // rows; on a layer that can sample, ats_sample and ats_gather into the next pitch; the MLP over P[L + 1] rows.
+  template <typename T>
+  T* ats_layer(T* X, int B, int L, const AtsPlan& p, int* st, unsigned long long* rng, cudaStream_t s, float* stats, bool* sv) {
+    const LayerW& l = layers[L];
+    const int dim = cfg.dim, P = p.P[L], Pn = p.P[L + 1], M = B * P, K = ats.max_tokens_per_depth[L];
+    const int si = p.slot[L];
+    const int* nk = st + p.rows + static_cast<size_t>(si) * B;
+    const bool fold = l.folded && stats != nullptr;
+    if (fold && !*sv) { ensure_stats(X, dim, stats, M, s); *sv = true; }
+    T* Y = arena.get<T>(static_cast<size_t>(M) * dim);
+    const T* qkv = attend_self<T>(X, B, P, dim, l, s, fold ? stats : nullptr, Y, nk);
+    if (p.can[L]) {
+      const int so = p.slot[L + 1], ld = 3 * l.heads * l.dim_head;
+      int* rows_new = st + p.rows + static_cast<size_t>(so) * B;
+      int* sel = arena.get<int>(static_cast<size_t>(B) * Pn);
+      float* scratch = arena.get<float>(static_cast<size_t>(3) * B * P);
+      T* Xn = arena.get<T>(static_cast<size_t>(B) * Pn * dim);
+      {
+        ProfScope ps(this, PROF_OTHER, 4.0 * B * P * l.heads * l.dim_head + 60.0 * B * K * P,
+                     static_cast<double>(sizeof(T)) * B * P * 3 * l.heads * l.dim_head, s);
+        ats_sample<T>(qkv, ld, B, P, l.heads, l.dim_head, 1.0f / sqrtf(static_cast<float>(l.dh_model)), nk, st + p.C + si, K, rng,
+                      scratch, sel, Pn, rows_new, st + p.draws[L], s);
+      }
+      {
+        ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * B * Pn * dim, s);
+        ats_gather<T>(X, P, Xn, Pn, dim, sel, rows_new, st + p.ids[si], st + p.ids[so], B, st + p.C + si, K, st + p.C + so, rng, s);
+      }
+      X = Xn;
+      if (fold) ensure_stats(X, dim, stats, B * Pn, s);
+    }
+    feed_forward<T>(X, B * Pn, dim, l, Y, s, fold ? stats : nullptr);
+    return X;
   }
   // One CCT TransformerEncoderLayer (cct.py:159-174, dropout / drop-path the identity):
   //   x = x + proj(MHA(pre_norm(x)));  x = norm1(x);  x = x + linear2(GELU(linear1(x)))
@@ -2041,6 +2190,8 @@ struct vb_handle {
       nest_forward<T>(img, B, H, Wd, logits, s);
     } else if (c.kind == VB_KIND_REGIONVIT) {
       regionvit_forward<T>(img, B, H, Wd, logits, s);
+    } else if (c.kind == VB_KIND_ATS_VIT) {
+      ats_forward<T>(img, B, H, Wd, logits, s);
     } else if (c.kind == VB_KIND_CCT) {                   // CCT.call cct.py:342-345, TransformerClassifier.call :277-305
       int rows = 0;
       T* X = tokenize_cct<T>(img, B, H, Wd, &rows, s);
@@ -2781,6 +2932,7 @@ struct vb_handle {
       case VB_KIND_CROSSFORMER: return "CrossFormer runs as a whole forward only: its embedding / stage / head steps have no entry of their own";
       case VB_KIND_NEST: return "NesT runs as a whole forward only: its patch-embedding / level / head steps have no entry of their own";
       case VB_KIND_REGIONVIT: return "RegionViT runs as a whole forward only: its encoder / stage / head steps have no entry of their own";
+      case VB_KIND_ATS_VIT: return "ATS-ViT runs as a whole forward only: its token count changes inside the transformer, so its stages have no entry of their own";
       default: return nullptr;
     }
   }
@@ -3028,6 +3180,7 @@ void validate(const vb_config& c) {
   VB_CHECK(c.kind != VB_KIND_CROSSFORMER, "CrossFormer: create the handle with vb_create_crossformer (its stages are a vb_crossformer_config)");
   VB_CHECK(c.kind != VB_KIND_NEST, "NesT: create the handle with vb_create_nest (its levels are a vb_nest_config)");
   VB_CHECK(c.kind != VB_KIND_REGIONVIT, "RegionViT: create the handle with vb_create_regionvit (its stages are a vb_regionvit_config)");
+  VB_CHECK(c.kind != VB_KIND_ATS_VIT, "ATS-ViT: create the handle with vb_create_ats_vit (its token counts are a vb_ats_vit_config)");
   VB_CHECK(c.kind >= VB_KIND_VIT && c.kind <= VB_KIND_CCT, "unknown model kind");
   if (c.kind == VB_KIND_CCT) {
     VB_CHECK(c.channels == 3 && c.num_classes > 0 && c.image_h > 0 && c.image_w > 0, "bad image / class configuration");
@@ -3117,6 +3270,20 @@ void validate_nest(const vb_config& c, const vb_nest_config& n) {
            "NesT: bad patch_size / dim / heads / mlp_mult / seq_len");
   VB_CHECK((static_cast<long long>(n.dim) << (n.num_hierarchies - 1)) <= 65536, "NesT: dim * 2^(num_hierarchies - 1) is too large");
   for (int i = 0; i < n.levels; ++i) VB_CHECK(n.block_repeats[i] >= 0, "NesT: block_repeats must not be negative");
+}
+
+// ats_vit.py:225-227 (the reference's assert messages) on top of ViT's checks
+void validate_ats(const vb_config& c, const vb_ats_vit_config& a) {
+  vb_config v = c;
+  v.kind = VB_KIND_VIT;
+  v.pool = VB_POOL_CLS;
+  validate(v);
+  VB_CHECK(c.depth >= 1 && c.depth <= VB_ATS_MAX_DEPTH, "ATS-ViT: depth must be in [1, 64]");
+  for (int L = 1; L < c.depth; ++L)
+    VB_CHECK(a.max_tokens_per_depth[L] <= a.max_tokens_per_depth[L - 1], "max_tokens_per_depth must be in decreasing order");
+  for (int L = 0; L < c.depth; ++L)
+    VB_CHECK(a.max_tokens_per_depth[L] > 0, "max_tokens_per_depth must have at least 1 token at any layer");
+  VB_CHECK(c.dim_head <= ATS_MAX_DH, "ATS-ViT: dim_head must be at most 256");
 }
 
 void validate_regionvit(const vb_config& c, const vb_regionvit_config& r) {
@@ -3327,6 +3494,134 @@ int vb_create_nest(const vb_config* base, const vb_nest_config* nc, int device, 
   return create_with("vb_create_nest", "vb_nest_config", VB_KIND_NEST, "VB_KIND_NEST", base, nc, device, out, validate_nest,
                                      [&](vb_handle& h) { h.ns = *nc; h.cfg.dim = h.nest_last_dim(); });
 }
+int vb_create_ats_vit(const vb_config* base, const vb_ats_vit_config* ac, int device, vb_handle** out) {
+  return create_with("vb_create_ats_vit", "vb_ats_vit_config", VB_KIND_ATS_VIT, "VB_KIND_ATS_VIT", base, ac, device, out, validate_ats,
+                     [&](vb_handle& h) { h.ats = *ac; h.cfg.pool = VB_POOL_CLS; });
+}
+
+int vb_ats_set_seed(vb_handle* h, uint64_t seed) {
+  return guarded(h, [&] {
+    VB_CHECK(h != nullptr, "null handle");
+    VB_CHECK(h->cfg.kind == VB_KIND_ATS_VIT, "vb_ats_set_seed: not an ATS-ViT handle");
+    VB_CUDA(cudaSetDevice(h->device));
+    VB_CUDA(cudaDeviceSynchronize());                  // no forward in flight reads the old key and counter
+    const unsigned long long v[2] = {static_cast<unsigned long long>(seed), 0ull};
+    VB_CUDA(cudaMemcpy(h->ats_rng_ptr(), v, sizeof v, cudaMemcpyHostToDevice));
+    VB_CUDA(cudaDeviceSynchronize());                  // a pageable copy may return before it lands
+  });
+}
+
+int vb_forward_ats(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, int32_t img_h, int32_t img_w, float* logits,
+                   int32_t* token_ids, int32_t* count, void* stream) {
+  const int rc = guarded(h, [&] {
+    VB_CHECK(h != nullptr && token_ids != nullptr && count != nullptr, "vb_forward_ats: null argument");
+    VB_CHECK(h->cfg.kind == VB_KIND_ATS_VIT, "vb_forward_ats: not an ATS-ViT handle");
+  });
+  if (rc != 0) return rc;
+  const int fr = vb_forward(h, img, img_mem, batch, img_h, img_w, logits, VB_MEM_HOST, stream);
+  if (fr != 0) return fr;
+  return guarded(h, [&] {
+    const vb_handle::AtsPlan& p = h->ats_last;
+    const int* st = static_cast<const int*>(h->ats_dev.p);
+    const int depth = h->cfg.depth, f = p.slot[depth];
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    VB_CUDA(cudaMemcpyAsync(token_ids, st + p.out, static_cast<size_t>(batch) * (p.P[depth] - 1) * sizeof(int), cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaMemcpyAsync(count, st + p.C + f, sizeof(int), cudaMemcpyDeviceToHost, s));
+    VB_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
+int vb_ats_last_draws(vb_handle* h, int32_t layer, int32_t* draws, int32_t* counts, int32_t* sampled) {
+  return guarded(h, [&] {
+    VB_CHECK(h != nullptr && draws != nullptr && counts != nullptr && sampled != nullptr, "vb_ats_last_draws: null argument");
+    VB_CHECK(h->cfg.kind == VB_KIND_ATS_VIT, "vb_ats_last_draws: not an ATS-ViT handle");
+    const vb_handle::AtsPlan& p = h->ats_last;
+    VB_CHECK(p.B > 0, "vb_ats_last_draws: no forward has run");
+    VB_CHECK(layer >= 0 && layer < h->cfg.depth && p.can[layer], "vb_ats_last_draws: layer " + std::to_string(layer) + " never samples");
+    VB_CUDA(cudaSetDevice(h->device));
+    VB_CUDA(cudaDeviceSynchronize());
+    const int* st = static_cast<const int*>(h->ats_dev.p);
+    const int K = h->ats.max_tokens_per_depth[layer];
+    VB_CUDA(cudaMemcpy(draws, st + p.draws[layer], static_cast<size_t>(p.B) * K * sizeof(int), cudaMemcpyDeviceToHost));
+    VB_CUDA(cudaMemcpy(counts, st + p.rows + static_cast<size_t>(p.slot[layer + 1]) * p.B, static_cast<size_t>(p.B) * sizeof(int),
+                       cudaMemcpyDeviceToHost));
+    for (int b = 0; b < p.B; ++b) counts[b] -= 1;      // live rows -> kept tokens
+    int C_in = 0;
+    VB_CUDA(cudaMemcpy(&C_in, st + p.C + p.slot[layer], sizeof(int), cudaMemcpyDeviceToHost));
+    *sampled = C_in > K ? 1 : 0;                       // ats_vit.py:213 on the batch's padded length
+    if (!*sampled) std::fill(draws, draws + static_cast<size_t>(p.B) * K, -1);
+  });
+}
+
+int vb_op_ats_sample(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t P, int32_t heads, int32_t dh, float scale,
+                     const int32_t* rows, int32_t K, uint64_t seed, uint64_t counter, int32_t* sel, int32_t* rows_new, int32_t* draws) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    VB_CHECK(qkv && rows && sel && rows_new && draws && B > 0 && P > 1 && heads > 0 && dh > 0 && ld >= 3 * heads * dh && K > 0,
+             "vb_op_ats_sample: bad arguments");
+    int C = 0;
+    for (int b = 0; b < B; ++b) {
+      VB_CHECK(rows[b] >= 2 && rows[b] <= P, "vb_op_ats_sample: rows[b] must be in [2, P]");
+      C = std::max(C, rows[b] - 1);
+    }
+    const int Pn = 1 + std::min(P - 1, K);
+    DevMem dX, dI, dR, dS, dF;
+    const size_t nint = static_cast<size_t>(B) + 1 + static_cast<size_t>(B) * Pn + B + static_cast<size_t>(B) * K;
+    dI.ensure(nint * sizeof(int));
+    int* i_d = static_cast<int*>(dI.p);
+    int *rows_d = i_d, *C_d = i_d + B, *sel_d = C_d + 1, *rn_d = sel_d + static_cast<size_t>(B) * Pn, *dr_d = rn_d + B;
+    VB_CUDA(cudaMemcpy(rows_d, rows, static_cast<size_t>(B) * sizeof(int), cudaMemcpyHostToDevice));
+    VB_CUDA(cudaMemcpy(C_d, &C, sizeof(int), cudaMemcpyHostToDevice));
+    VB_CUDA(cudaMemset(dr_d, 0xff, static_cast<size_t>(B) * K * sizeof(int)));
+    const unsigned long long rng[2] = {static_cast<unsigned long long>(seed), static_cast<unsigned long long>(counter)};
+    dR.ensure(sizeof rng);
+    VB_CUDA(cudaMemcpy(dR.p, rng, sizeof rng, cudaMemcpyHostToDevice));
+    dF.ensure(static_cast<size_t>(3) * B * P * sizeof(float));
+    auto run = [&](auto tag) {
+      using T = decltype(tag);
+      const T* x_d = upload<T>(dX, qkv, static_cast<size_t>(B) * P * ld);
+      ats_sample<T>(x_d, ld, B, P, heads, dh, scale, rows_d, C_d, K, static_cast<const unsigned long long*>(dR.p), static_cast<float*>(dF.p),
+                    sel_d, Pn, rn_d, dr_d, 0);
+    };
+    if (precision == VB_PRECISION_FP32) run(float());
+    else run(__nv_bfloat16());
+    VB_CUDA(cudaDeviceSynchronize());
+    VB_CUDA(cudaMemcpy(sel, sel_d, static_cast<size_t>(B) * Pn * sizeof(int), cudaMemcpyDeviceToHost));
+    VB_CUDA(cudaMemcpy(rows_new, rn_d, static_cast<size_t>(B) * sizeof(int), cudaMemcpyDeviceToHost));
+    VB_CUDA(cudaMemcpy(draws, dr_d, static_cast<size_t>(B) * K * sizeof(int), cudaMemcpyDeviceToHost));
+  });
+}
+
+int vb_op_masked_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t n, int32_t heads, int32_t dh,
+                           const int32_t* nk_img, float* out, int32_t ldo, int32_t iters, float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    const int HD = heads * dh;
+    VB_CHECK(qkv && nk_img && out && B > 0 && n > 0 && heads > 0 && dh > 0 && ld >= 3 * HD && ldo >= HD, "vb_op_masked_attention: bad arguments");
+    for (int b = 0; b < B; ++b) VB_CHECK(nk_img[b] >= 1 && nk_img[b] <= n, "vb_op_masked_attention: nk_img[b] must be in [1, n]");
+    DevMem dX, dO, dN, dS;
+    dN.ensure(static_cast<size_t>(B) * sizeof(int));
+    VB_CUDA(cudaMemcpy(dN.p, nk_img, static_cast<size_t>(B) * sizeof(int), cudaMemcpyHostToDevice));
+    const int* nk_d = static_cast<const int*>(dN.p);
+    const float scale = 1.0f / sqrtf(static_cast<float>(dh));
+    auto run = [&](auto tag) {
+      using T = decltype(tag);
+      const T* x_d = upload<T>(dX, qkv, static_cast<size_t>(B) * n * ld);
+      T* o_d = upload<T>(dO, out, static_cast<size_t>(B) * n * ldo);
+      // vb_handle::attention_masked_dispatch without the handle's arena and profiler
+      timed(iters, elapsed_ms, [&] {
+        if (vb_handle::masked_flash(x_d, ld, o_d, ldo, B, n, heads, dh, 0, scale, nk_d)) return;
+        dS.ensure(static_cast<size_t>(B) * heads * n * n * sizeof(float));
+        attention_generic_masked<T>(x_d, ld, x_d + HD, ld, x_d + 2 * HD, ld, o_d, ldo, static_cast<float*>(dS.p), B, n, n, heads, dh, 0, scale,
+                                    nk_d);
+      });
+      download<T>(o_d, out, static_cast<size_t>(B) * n * ldo);
+    };
+    if (precision == VB_PRECISION_FP32) run(float());
+    else run(__nv_bfloat16());
+  });
+}
+
 int vb_create_regionvit(const vb_config* base, const vb_regionvit_config* rc, int device, vb_handle** out) {
   return create_with("vb_create_regionvit", "vb_regionvit_config", VB_KIND_REGIONVIT, "VB_KIND_REGIONVIT", base, rc,
                                           device, out, validate_regionvit,
@@ -3393,6 +3688,7 @@ int vb_forward(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, i
       h->logits_dev.ensure(out_bytes);
       out_d = static_cast<float*>(h->logits_dev.p);
     }
+    if (h->cfg.kind == VB_KIND_ATS_VIT) h->ats_prepare(batch, img_h, img_w);
     auto run_eager = [&] {
       if (h->bf16()) h->forward_impl<__nv_bfloat16>(img_d, batch, img_h, img_w, out_d, s);
       else h->forward_impl<float>(img_d, batch, img_h, img_w, out_d, s);
@@ -3461,6 +3757,7 @@ int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, int32_t 
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSFORMER, "vb_forward_distill: CrossFormer has no distillation head");
     VB_CHECK(h->cfg.kind != VB_KIND_NEST, "vb_forward_distill: NesT has no distillation head");
     VB_CHECK(h->cfg.kind != VB_KIND_REGIONVIT, "vb_forward_distill: RegionViT has no distillation head");
+    VB_CHECK(h->cfg.kind != VB_KIND_ATS_VIT, h->whole_forward_only(VB_KIND_ATS_VIT));
     const bool levit = h->cfg.kind == VB_KIND_LEVIT;
     VB_CHECK(levit || distill_token != nullptr, "vb_forward_distill: null argument");
     VB_CHECK(!levit || (distill_token == nullptr && h->lv.num_distill_classes > 0),

@@ -174,6 +174,32 @@ void ln_fold_consts(const float* W, const __nv_bfloat16* Wt, int ldw, const floa
 // the tail of a longer statistics buffer (RegionViT's regional rows after the local ones).
 void row_stats_bf16(const __nv_bfloat16* X, int ldx, float* stats, int M, int D, cudaStream_t s, long long pitch = 0);
 
+// ---- adaptive token sampling (ATS-ViT, ats_vit.py:77-132, 191-258; ats.cu).  Image b's rows sit at pitch P as [cls, its
+// c_b kept tokens in ascending id order, dead rows]; rows[b] = c_b + 1 (the live rows: the key count of its masked attention),
+// and C (one int on the device) is the batch maximum of the c_b.
+constexpr int ATS_MAX_DH = 256;          // widest head ats_sample reads
+constexpr int ATS_MAX_TOKENS = 65536;    // the noise counter holds the column in 16 bits: patches + 1 <= 65,536
+// rows[b] = P, *C = P - 1, ids[b, t] = t
+void ats_init(int* rows, int* C, int* ids, int B, int P, cudaStream_t s);
+// One CTA per image.  When *C <= K the layer keeps every row: sel[b, t] = t for t < rows[b], rows_new = rows.  Otherwise,
+// from the fused q | k | v rows (head h at columns h*dh, HD + h*dh, 2 HD + h*dh; dh the stored width, pad columns zero): the cls
+// query's softmax over its valid keys 0..c (fp32, `scale`), weighted by the value norms and summed over heads, normalised and
+// logged; then K Gumbel-max draws with u = (Philox4x32-10 word 0 >> 8) * 2^-24, key rng[0], counter (j | k << 16, b, rng[1]),
+// j = C - c + i - 1 for compact token i.  draws[b, k] = the winner's position in the reference's left-padded layout (argmax + 1);
+// sel[b, 0 .. rows_new[b]) = 0 then the distinct winners in ascending order.  scratch: 3 * B * P floats.
+template <typename T>
+void ats_sample(const T* qkv, int ld, int B, int P, int heads, int dh, float scale, const int* rows, const int* C, int K,
+                const unsigned long long* rng, float* scratch, int* sel, int Pn, int* rows_new, int* draws, cudaStream_t s);
+// Xn [B * Pn, dim] = the rows sel picks from X [B * P, dim] (zero rows from rows_new[b] on), ids_n likewise from ids (0 on dead
+// rows); *C_new = max(rows_new) - 1; rng[1] += 1 when *C_old > K (the layer sampled).
+template <typename T>
+void ats_gather(const T* X, int P, T* Xn, int Pn, int dim, const int* sel, const int* rows_new, const int* ids, int* ids_n, int B,
+                const int* C_old, int K, int* C_new, unsigned long long* rng, cudaStream_t s);
+// out [B, P - 1] = the reference's returned token ids (ats_vit.py:315): image b's kept patch ids in columns [C - c_b, C), -1 elsewhere
+void ats_ids_out(const int* ids, int P, const int* rows, const int* C, int* out, int B, cudaStream_t s);
+// attn_softmax with the keys j >= nk_img[row / rows_per_img] of every row masked: their weight is exactly 0
+void attn_softmax_masked(float* S, long long rows, int nk, long long rows_per_img, const int* nk_img, cudaStream_t s);
+
 long long launch_counter();      // number of kernel launches issued through these wrappers (process-wide)
 void count_launch(int n = 1);
 

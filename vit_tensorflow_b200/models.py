@@ -121,7 +121,7 @@ class _EngineModel:
 
     _kind = None
 
-    def _create(self, precision, device, **cfgkw):
+    def _create(self, precision, device, create=None, **cfgkw):
         self.precision = precision
         self.device = int(device)
         cfg = _lib.VbConfig()
@@ -136,7 +136,10 @@ class _EngineModel:
         self._cfg = cfg
         self._lib = _lib.load()
         h = C.c_void_p()
-        _lib.check(self._lib.vb_create(C.byref(cfg), self.device, C.byref(h)))
+        if create is None:
+            _lib.check(self._lib.vb_create(C.byref(cfg), self.device, C.byref(h)))
+        else:                                             # a kind with an extension config: create(cfg, device, &h) -> rc
+            _lib.check(create(C.byref(cfg), self.device, C.byref(h)))
         self._h = h
         self._finalized = False
         self._specs = collections.OrderedDict()
@@ -1521,12 +1524,104 @@ class RegionViT(_EngineModel):
     call = __call__
 
 
+class ATSViT(_EngineModel):
+    """ats_vit.py:260-318 (`ats_vit.ViT`, adaptive token sampling): a ViT whose layer L keeps at most max_tokens_per_depth[L]
+    tokens, drawn by Gumbel-max from the cls token's attention weighted by the value norms, whenever the batch's padded token
+    count exceeds that number.  The pool is always the cls token and to_out is always present.  The draws are random whatever
+    `training` is; the noise is the engine's Philox stream (include/vitb200.h), keyed by set_sampling_seed (0 at construction)
+    and advancing with every layer that samples, so repeated calls draw fresh tokens.  An image's result depends on the rest of
+    its batch, as in the reference.  With dropout > 0 only training=False runs.  Weights keep ViT's names (SURVEY.md App. B)."""
+    _kind = "ats_vit"
+
+    def __init__(self, image_size, patch_size, num_classes, dim, depth, max_tokens_per_depth, heads, mlp_dim, dim_head=64,
+                 dropout=0.0, emb_dropout=0.0, *, precision="bf16", device=0, seed=None):
+        image_height, image_width = pair(image_size)
+        patch_height, patch_width = pair(patch_size)
+        assert image_height % patch_height == 0 and image_width % patch_width == 0, 'Image dimensions must be divisible by the patch size.'
+        assert len(max_tokens_per_depth) == depth, 'max_tokens_per_depth must be a tuple of length that is equal to the depth of the transformer'
+        assert sorted(max_tokens_per_depth, reverse=True) == list(max_tokens_per_depth), 'max_tokens_per_depth must be in decreasing order'
+        assert min(max_tokens_per_depth) > 0, 'max_tokens_per_depth must have at least 1 token at any layer'
+        if depth > _lib.ATS_MAX_DEPTH:
+            raise ValueError(f"ATS-ViT: depth must be at most {_lib.ATS_MAX_DEPTH}")
+        self.num_classes, self.dim = num_classes, dim
+        self.max_tokens_per_depth = tuple(int(k) for k in max_tokens_per_depth)
+        self._dropout_rates = (dropout, emb_dropout)
+        ac = _lib.VbAtsVitConfig()
+        ac.struct_size = C.sizeof(_lib.VbAtsVitConfig)
+        for i, k in enumerate(self.max_tokens_per_depth):
+            ac.max_tokens_per_depth[i] = k
+        self._ac = ac
+        lib = _lib.load()
+        self._create(precision, device, create=lambda cfg, dev, h: lib.vb_create_ats_vit(cfg, C.byref(ac), dev, h),
+                     image_h=image_height, image_w=image_width, patch_h=patch_height, patch_w=patch_width, num_classes=num_classes,
+                     dim=dim, depth=depth, heads=heads, dim_head=dim_head, mlp_dim=mlp_dim)
+        self.init_weights(seed)
+
+    def set_sampling_seed(self, seed):
+        """The Philox key of the sampling noise; also restarts its draw counter, so the next calls repeat the draws made after
+        the previous set_sampling_seed(seed) (on the same images and batch)."""
+        _lib.check(self._lib.vb_ats_set_seed(self._h, int(seed) & 0xFFFFFFFFFFFFFFFF), self._h)
+
+    def forward_ats(self, img, stream=None):
+        """One forward: (logits [b, num_classes], token_ids [b, count]) with the reference's id layout (ats_vit.py:313-316).
+        stream: a cudaStream_t, as in forward_raw (the forward is captured into a CUDA graph on its second call there)."""
+        self._finalize()
+        x = self._img(img)
+        b, h, w, _ = x.shape
+        logits = np.empty((b, self.num_classes), np.float32)
+        self._last_batch = b
+        ids = np.empty((b, self._last_pitch(h, w) - 1), np.int32)
+        count = C.c_int32()
+        _lib.check(self._lib.vb_forward_ats(self._h, x.ctypes.data_as(C.c_void_p), _lib.MEM_HOST, b, h, w, logits.ctypes.data_as(C.c_void_p),
+                                            ids.ctypes.data_as(C.c_void_p), C.byref(count), C.c_void_p(stream) if stream else None),
+                   self._h)
+        return logits, ids[:, :count.value].copy()
+
+    def _last_pitch(self, h, w):
+        """Rows of the last layer: P_0 = patches + 1, P_{L+1} = 1 + min(P_L - 1, K_L)."""
+        p = (h // self._cfg.patch_h) * (w // self._cfg.patch_w) + 1
+        for k in self.max_tokens_per_depth:
+            p = 1 + min(p - 1, k)
+        return p
+
+    def last_draws(self, layer):
+        """After a forward: (draws [b, K] as argmax + 1 in the reference's left-padded layout, counts [b] of tokens kept, sampled)
+        of a layer that can sample; when it did not sample (the batch already had at most K tokens) sampled is False and the
+        draws are -1."""
+        k = self.max_tokens_per_depth[layer]
+        b = self._last_batch
+        draws, counts, sampled = np.empty((b, k), np.int32), np.empty((b,), np.int32), C.c_int32()
+        _lib.check(self._lib.vb_ats_last_draws(self._h, layer, draws.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.c_void_p),
+                                               C.byref(sampled)), self._h)
+        return draws, counts, bool(sampled.value)
+
+    def forward_raw(self, img_ptr, img_mem, batch, h, w, logits_ptr, logits_mem, stream=None):
+        self._last_batch = batch
+        super().forward_raw(img_ptr, img_mem, batch, h, w, logits_ptr, logits_mem, stream)
+
+    def __call__(self, img, return_sampled_token_ids=False, training=True, **kwargs):
+        """ats_vit.py:300-318: NHWC images -> logits, or (logits, token_ids) with return_sampled_token_ids."""
+        self._check_training(training)
+        logits, ids = self.forward_ats(img)
+        if return_sampled_token_ids:
+            return _as_tensor(logits), _as_tensor(ids)
+        return _as_tensor(logits)
+
+    call = __call__
+
+
+ATS_CTOR_KEYS = ("image_size", "patch_size", "num_classes", "dim", "depth", "max_tokens_per_depth", "heads", "mlp_dim", "dim_head",
+                 "dropout", "emb_dropout")
+
+
 REGIONVIT_CTOR_KEYS = ("dim", "depth", "window_size", "num_classes", "tokenize_local_3_conv", "local_patch_size", "use_peg",
                        "attn_dropout", "ff_dropout")
 
 
 def from_config(cfg: dict, precision="bf16", device=0, seed=None):
     """Build a model from an oracle-style config dict (kind + reference kwargs)."""
+    if cfg["kind"] == "ats_vit":
+        return ATSViT(**{k: v for k, v in cfg.items() if k in ATS_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "regionvit":
         return RegionViT(**{k: v for k, v in cfg.items() if k in REGIONVIT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "nest":
