@@ -47,7 +47,7 @@ typedef struct vb_handle vb_handle;
 enum { VB_KIND_VIT = 0, VB_KIND_DEEPVIT = 1, VB_KIND_CAIT = 2, VB_KIND_CROSSVIT = 3, VB_KIND_PARALLEL_VIT = 4,
        VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6, VB_KIND_CCT = 7, VB_KIND_LEVIT = 8,
        VB_KIND_CVT = 9, VB_KIND_TWINS_SVT = 10, VB_KIND_CROSSFORMER = 11, VB_KIND_NEST = 12, VB_KIND_REGIONVIT = 13,
-       VB_KIND_ATS_VIT = 14 };
+       VB_KIND_ATS_VIT = 14, VB_KIND_SMALL_DATASET_VIT = 15 };
 enum { VB_CCT_POS_SINE = 0, VB_CCT_POS_LEARNABLE = 1, VB_CCT_POS_NONE = 2 };   /* cct.py:233-234,250-256 */
 enum { VB_PRECISION_FP32 = 0, VB_PRECISION_BF16 = 1 };
 enum { VB_POOL_CLS = 0, VB_POOL_MEAN = 1 };
@@ -325,6 +325,26 @@ VB_API int vb_op_ats_sample(int32_t precision, const float* qkv, int32_t ld, int
  * out float32 [B * n, ldo]; every row is written, the rows of masked queries too (finite). */
 VB_API int vb_op_masked_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t n, int32_t heads, int32_t dh,
                                   const int32_t* nk_img, float* out, int32_t ldo, int32_t iters, float* elapsed_ms);
+
+/* The small-dataset ViT (vit_for_small_dataset.py:159-215: shifted patch tokens and locality self-attention), appended within
+ * ABI 7.  vb_create with kind VB_KIND_SMALL_DATASET_VIT: the ViT fields of vb_config are the whole configuration (patch_h ==
+ * patch_w, channels 3, pool cls or mean).  Weights are ViT's names and shapes (SURVEY.md App. B), to_out always present, plus
+ * patch_norm.gamma / .beta [p^2 * 15] and patch.kernel [p^2 * 15, dim] / .bias (SPT's LayerNormalization and Dense over the
+ * (p1, p2, view, c) vector of the image and its four one-pixel shifts) and layers.L.temperature, a scalar (shape (), ndim 0):
+ * layer L's softmax scale is exp(temperature) and each token's own key is masked.  vb_forward only: the stage entries and
+ * vb_forward_distill refuse the handle. */
+/* SPT on its own, plus the cls row and positions (the engine's embedding): img float32 NHWC [B, H, W, 3], patch size p; gamma /
+ * beta [p^2 * 15], kernel [p^2 * 15, dim], bias [dim]; cls [dim] and pos [(1 + np) * dim] (either may be NULL: zero).  out float32
+ * [B, 1 + np, dim]: row 0 = cls + pos[0], row 1 + t = Dense(LayerNorm(patch t)) + pos[1 + t].  bf16 runs the LayerNorm folded
+ * into the wgmma GEMM over rows zero-padded to a multiple of 64 columns, fp32 the LayerNorm kernel and the fp32 GEMM. */
+VB_API int vb_op_spt(int32_t precision, const float* img, int32_t B, int32_t H, int32_t W, int32_t p, int32_t dim, const float* gamma,
+                     const float* beta, const float* kernel, const float* bias, const float* cls, const float* pos, float* out);
+/* Locality self-attention over fused q|k|v rows (qkv float32 [B * n, ld], head h at columns h*dh, HD + h*dh, 2 HD + h*dh): scores
+ * q.k * scale with each query's own key masked (weight 0), softmax, times v.  n >= 2.  bf16: the dim_head-64 flash kernels
+ * (resident for n <= 256, streaming above), heads narrower than 64 (dh % 8 == 0) zero-padded to 64 as the engine's layers are;
+ * other widths and fp32: the materialised-scores path.  out float32 [B * n, ldo]. */
+VB_API int vb_op_lsa_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t n, int32_t heads, int32_t dh,
+                               float scale, float* out, int32_t ldo, int32_t iters, float* elapsed_ms);
 
 /* Replaces Keras variable assignment: one call per weight, names/shapes/layouts per SURVEY.md App. B
  * (Dense kernel [in,out], float32).  shape/ndim are checked against the config. */

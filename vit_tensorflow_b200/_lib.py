@@ -12,7 +12,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "libvitb200.so")   # VB_LIB_PATH: developer A/B builds
 
 KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6, "cct": 7, "levit": 8,
-        "cvt": 9, "twins_svt": 10, "crossformer": 11, "nest": 12, "regionvit": 13, "ats_vit": 14}
+        "cvt": 9, "twins_svt": 10, "crossformer": 11, "nest": 12, "regionvit": 13, "ats_vit": 14,
+        "small_dataset_vit": 15}
 PRECISION = {"fp32": 0, "float32": 0, "bf16": 1, "bfloat16": 1}
 MEM_HOST, MEM_DEVICE = 0, 1
 ABI_VERSION = 7                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
@@ -115,6 +116,8 @@ SIGNATURES = {
     "vb_op_ats_sample": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 5 + [C.c_float, C.c_void_p, C.c_int32, C.c_uint64, C.c_uint64] +
                          [C.c_void_p] * 3),
     "vb_op_masked_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, _f32p]),
+    "vb_op_spt": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p] * 7),
+    "vb_op_lsa_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 5 + [C.c_float, C.c_void_p, C.c_int32, C.c_int32, _f32p]),
     "vb_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, _i64p, C.c_int32]),
     "vb_num_weights": (C.c_int, [C.c_void_p]),
     "vb_weight_info": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), _i64p, C.POINTER(C.c_int32)]),
@@ -410,6 +413,32 @@ def op_masked_attention(qkv, B, n, heads, dh, nk_img, precision="bf16", iters=0)
     ms = C.c_float(0)
     check(load().vb_op_masked_attention(PRECISION[precision], _ptr(qkv), qkv.shape[1], B, n, heads, dh, _ptr(nk), _ptr(out), heads * dh,
                                         iters, C.byref(ms)))
+    return out, (ms.value if iters > 0 else None)
+
+
+def op_spt(img, p, gamma, beta, kernel, bias, cls=None, pos=None, precision="bf16"):
+    """The small-dataset ViT's SPT plus cls row and positions (vb_op_spt): img [B, H, W, 3] -> [B, 1 + np, dim], row 0 = cls + pos[0],
+    row 1 + t = Dense(LayerNorm(shifted patch t)) + pos[1 + t]; cls / pos None: zero."""
+    img = _f32(img)
+    B, H, W, _ = img.shape
+    kernel = _f32(kernel)
+    dim = kernel.shape[1]
+    rows = 1 + (H // p) * (W // p)
+    out = np.zeros((B, rows, dim), np.float32)
+    opt = [None if a is None else _f32(a) for a in (cls, pos)]
+    check(load().vb_op_spt(PRECISION[precision], _ptr(img), B, H, W, p, dim, _ptr(_f32(gamma)), _ptr(_f32(beta)), _ptr(kernel),
+                           _ptr(_f32(bias)), *[None if a is None else _ptr(a) for a in opt], _ptr(out)))
+    return out
+
+
+def op_lsa_attention(qkv, B, n, heads, dh, scale, precision="bf16", iters=0):
+    """Locality self-attention (vb_op_lsa_attention) on fused q|k|v rows [B*n, ld]: the diagonal masked, scores times `scale`.
+    Returns (out [B*n, heads*dh], ms or None)."""
+    qkv = _f32(qkv)
+    out = np.zeros((B * n, heads * dh), np.float32)
+    ms = C.c_float(0)
+    check(load().vb_op_lsa_attention(PRECISION[precision], _ptr(qkv), qkv.shape[1], B, n, heads, dh, scale, _ptr(out), heads * dh, iters,
+                                     C.byref(ms)))
     return out, (ms.value if iters > 0 else None)
 
 

@@ -196,19 +196,21 @@ __global__ void ats_ids_out_kernel(const int* __restrict__ ids, int P, const int
   }
 }
 
-// Row softmax of materialised scores with the keys j >= nk_img[row / rows_per_img] masked (weight exactly 0)
+// Row softmax of materialised scores with the keys j >= nk_img[row / rows_per_img] (nk_img non-null) and the key j == row % diag_nq
+// (diag_nq > 0) masked: weight exactly 0
 __global__ void attn_softmax_masked_kernel(float* __restrict__ S, long long rows, int nk, long long rows_per_img,
-                                           const int* __restrict__ nk_img) {
+                                           const int* __restrict__ nk_img, int diag_nq) {
   const long long row = blockIdx.x * static_cast<long long>(blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= rows) return;
-  const int lane = threadIdx.x & 31, valid = min(nk, nk_img[row / rows_per_img]);
+  const int lane = threadIdx.x & 31, valid = nk_img != nullptr ? min(nk, nk_img[row / rows_per_img]) : nk;
+  const int dj = diag_nq > 0 ? static_cast<int>(row % diag_nq) : -1;
   float* r = S + row * nk;
   float mx = -INFINITY;
-  for (int j = lane; j < valid; j += 32) mx = fmaxf(mx, r[j]);
+  for (int j = lane; j < valid; j += 32) if (j != dj) mx = fmaxf(mx, r[j]);
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
   float sum = 0.f;
-  for (int j = lane; j < valid; j += 32) { const float e = expf(r[j] - mx); r[j] = e; sum += e; }
+  for (int j = lane; j < valid; j += 32) { const float e = j != dj ? expf(r[j] - mx) : 0.f; r[j] = e; sum += e; }
   const float inv = 1.0f / ats_warp_sum(sum);
   for (int j = lane; j < nk; j += 32) r[j] = j < valid ? r[j] * inv : 0.f;
 }
@@ -251,9 +253,10 @@ void ats_ids_out(const int* ids, int P, const int* rows, const int* C, int* out,
   count_launch();
 }
 
-void attn_softmax_masked(float* S, long long rows, int nk, long long rows_per_img, const int* nk_img, cudaStream_t s) {
+void attn_softmax_masked(float* S, long long rows, int nk, long long rows_per_img, const int* nk_img, cudaStream_t s, int diag_nq) {
   const int warps = 8;
-  attn_softmax_masked_kernel<<<static_cast<unsigned>((rows + warps - 1) / warps), warps * 32, 0, s>>>(S, rows, nk, rows_per_img, nk_img);
+  attn_softmax_masked_kernel<<<static_cast<unsigned>((rows + warps - 1) / warps), warps * 32, 0, s>>>(S, rows, nk, rows_per_img, nk_img,
+                                                                                                       diag_nq);
   VB_CUDA(cudaGetLastError());
   count_launch();
 }

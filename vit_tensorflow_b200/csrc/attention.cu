@@ -58,16 +58,19 @@ template void attention_generic<float>(const float*, int, const float*, int, con
 
 template <typename T>
 void attention_generic_masked(const T* q, int ldq, const T* k, int ldk, const T* v, int ldv, T* out, int ldo, float* S, int B, int nq,
-                              int nk, int heads, int dh, cudaStream_t s, float scale, const int* nk_img) {
+                              int nk, int heads, int dh, cudaStream_t s, float scale, const int* nk_img, int mask) {
   note_attention_path(ATTN_PATH_SIMT);
   attn_scores<T>(q, ldq, k, ldk, S, B, heads, nq, nk, dh, scale > 0.f ? scale : 1.0f / sqrtf(static_cast<float>(dh)), s);
-  attn_softmax_masked(S, static_cast<long long>(B) * heads * nq, nk, static_cast<long long>(heads) * nq, nk_img, s);
+  const bool diag = mask == ATTN_MASK_DIAG;
+  attn_softmax_masked(S, static_cast<long long>(B) * heads * nq, nk, static_cast<long long>(heads) * nq, diag ? nullptr : nk_img, s,
+                      diag ? nq : 0);
   attn_pv<T>(S, v, ldv, out, ldo, B, heads, nq, nk, dh, s);
 }
 template void attention_generic_masked<float>(const float*, int, const float*, int, const float*, int, float*, int, float*, int, int, int,
-                                              int, int, cudaStream_t, float, const int*);
+                                              int, int, cudaStream_t, float, const int*, int);
 template void attention_generic_masked<__nv_bfloat16>(const __nv_bfloat16*, int, const __nv_bfloat16*, int, const __nv_bfloat16*, int,
-                                                      __nv_bfloat16*, int, float*, int, int, int, int, int, cudaStream_t, float, const int*);
+                                                      __nv_bfloat16*, int, float*, int, int, int, int, int, cudaStream_t, float, const int*,
+                                                      int);
 
 
 template <>

@@ -50,16 +50,22 @@ bool attention_block(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* out, int l
 bool attention_r2l(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* out, int ldo, int heads, int dh, long long reg_row0,
                    const PosBias& pb, const Window& win, cudaStream_t s, float scale = 0.f);
 
-// Plain softmax attention with a key count per image (ATS-ViT's kept tokens, ats_vit.py:200-207): keys j >= nk_img[b] of image b
-// (a device array, B entries) get weight exactly 0.  Every image needs nk_img[b] >= 1.  attention_masked: the dim_head-64 flash
-// kernels (the resident one for nk <= 256, else the streaming one), bf16; false when the shape is not covered.
-// attention_generic_masked: the materialised-scores path, any dh, both precisions; S fp32 [B, heads, nq, nk].
+// The key masks of the dim_head-64 flash kernels (their MASK template parameter) and of attention_masked:
+//   ATTN_MASK_KEYS: keys j >= nk_img[b] of image b are masked (ATS-ViT's kept tokens, ats_vit.py:200-207).
+//   ATTN_MASK_DIAG: key j == query i of the same image is masked (locality self-attention's tf.eye mask,
+//                   vit_for_small_dataset.py:111-113; needs nq == nk >= 2, so every row keeps a key).
+enum AttnMask { ATTN_MASK_NONE = 0, ATTN_MASK_KEYS = 1, ATTN_MASK_DIAG = 2 };
+
+// Plain softmax attention with masked keys, which get weight exactly 0: mask ATTN_MASK_KEYS with nk_img a device array of B
+// counts, each >= 1, or ATTN_MASK_DIAG (nk_img unused).  attention_masked: the dim_head-64 flash kernels (the resident one for
+// nk <= 256, else the streaming one), bf16; false when the shape is not covered.  attention_generic_masked: the materialised-
+// scores path, any dh, both precisions; S fp32 [B, heads, nq, nk].
 bool attention_masked(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, int ldk, const __nv_bfloat16* v, int ldv,
                       __nv_bfloat16* out, int ldo, int B, int nq, int nk, int heads, int dh, cudaStream_t s, float scale,
-                      const int* nk_img);
+                      const int* nk_img, int mask = ATTN_MASK_KEYS);
 template <typename T>
 void attention_generic_masked(const T* q, int ldq, const T* k, int ldk, const T* v, int ldv, T* out, int ldo, float* S, int B, int nq,
-                              int nk, int heads, int dh, cudaStream_t s, float scale, const int* nk_img);
+                              int nk, int heads, int dh, cudaStream_t s, float scale, const int* nk_img, int mask = ATTN_MASK_KEYS);
 
 // The talking-heads / re-attention path keeps host copies of the head-mix weights keyed by their device pointers (one process-
 // wide cache for all handles); whoever frees or rewrites such weights (vb_finalize, vb_destroy, the op-level test entries) must

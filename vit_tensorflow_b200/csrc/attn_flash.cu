@@ -56,7 +56,9 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
 
 constexpr int FLASH_BIAS_MAX = 4096;   // fmap^2 of the largest relative-position table (16 KB of shared memory)
 
-template <int D, bool BIAS, bool WIN, bool MASK = false>
+// MASK (attention.cuh's AttnMask): ATTN_MASK_KEYS masks image b's keys >= nk_img[b] and runs only the key blocks that hold a
+// valid key; ATTN_MASK_DIAG masks key j == query i (plain attention, nq == nk).
+template <int D, bool BIAS, bool WIN, int MASK = ATTN_MASK_NONE>
 __global__ void __launch_bounds__(128)
 attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloat16* __restrict__ k, int ldk,
                   const __nv_bfloat16* __restrict__ v, int ldv, __nv_bfloat16* __restrict__ out, int ldo, int heads, int nq, int nk,
@@ -91,7 +93,7 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
 
   pdl_wait();                 // Q/K/V come from the previous kernel of the stream
   pdl_launch_dependents();
-  if (MASK) {                 // keys >= nk_img[b] masked: only the blocks that hold a valid key (at least one: the cls row)
+  if (MASK == ATTN_MASK_KEYS) {   // keys >= nk_img[b] masked: only the blocks that hold a valid key (at least one: the cls row)
     nkv = min(nk, nk_img[b]);
     nblk = (nkv + FK - 1) / FK;
   }
@@ -194,6 +196,7 @@ attn_flash_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloa
         } else if (BIAS && n * 8 + qc + (e & 1) < valid)
           sc[n][e] = fmaf(sc[n][e], scale_log2, tab[pos_bias_index(qrow[e >> 1], j * FK + n * 8 + qc + (e & 1), fmap, step, nqs)]);
         if (n * 8 + qc + (e & 1) >= valid) sc[n][e] = -INFINITY;
+        if (MASK == ATTN_MASK_DIAG && j * FK + n * 8 + qc + (e & 1) == i0 + warp * 16 + qr + 8 * (e >> 1)) sc[n][e] = -INFINITY;
         mx[e >> 1] = fmaxf(mx[e >> 1], sc[n][e]);
       }
     }
@@ -299,11 +302,12 @@ __device__ __forceinline__ void mma_16816(float (&c)[4], const uint32_t (&a)[4],
 
 // One 64-key block of a 16-row query slice: S = Q K^T, the online-softmax update, O += P V.  PART (the last block, nk % 64
 // keys): only the 8-key S groups and 16-key PV steps that hold a valid key, keys >= nk masked to -inf.  Full blocks take no
-// per-group branch, so the products of all eight groups are in flight together.
-template <bool PART>
+// per-group branch, so the products of all eight groups are in flight together.  DIAG: key qrow (this lane's first row) and
+// qrow + 8 (its second) masked to -inf as well.
+template <bool PART, bool DIAG = false>
 __device__ __forceinline__ void resident_block(const uint32_t (&qf)[DH / 16][4], float (&o)[DH / 8][4], float (&m_run)[2],
                                                float (&l_run)[2], uint32_t tK, uint32_t tV, int j0, int nk, float scale_log2,
-                                               int lane) {
+                                               int lane, int qrow = 0) {
   const int qc = 2 * (lane & 3);
   float sc[8][4];
 #pragma unroll
@@ -328,6 +332,7 @@ __device__ __forceinline__ void resident_block(const uint32_t (&qf)[DH / 16][4],
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       if (PART && j0 + n * 8 + qc + (e & 1) >= nk) sc[n][e] = -INFINITY;
+      if (DIAG && j0 + n * 8 + qc + (e & 1) == qrow + 8 * (e >> 1)) sc[n][e] = -INFINITY;
       mx[e >> 1] = fmaxf(mx[e >> 1], sc[n][e]);
     }
   float alpha[2];
@@ -371,8 +376,9 @@ __device__ __forceinline__ void resident_block(const uint32_t (&qf)[DH / 16][4],
   }
 }
 
-// MASK: image b's keys >= nk_img[b] are masked; only the key blocks that hold a valid key run.
-template <bool MASK>
+// MASK (AttnMask): ATTN_MASK_KEYS masks image b's keys >= nk_img[b] and runs only the key blocks that hold a valid key;
+// ATTN_MASK_DIAG masks key j == query i.
+template <int MASK>
 __global__ void __launch_bounds__((RW + 1) * 32, 1)
 attn_resident_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
                      const __grid_constant__ CUtensorMap tv, __nv_bfloat16* __restrict__ out, int ldo, int heads, int nq, int nk,
@@ -427,7 +433,7 @@ attn_resident_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
     const int c = static_cast<int>(bc % chunks), b = static_cast<int>(bc / chunks);
     const int i0 = c * RQ, slices = (min(RQ, nq - i0) + 15) / 16;
     const uint32_t tQ = base + s * RBUF, tK = tQ + RTILE, tV = tQ + 2 * RTILE;
-    const int nkb = MASK ? min(nk, nk_img[b]) : nk;
+    const int nkb = MASK == ATTN_MASK_KEYS ? min(nk, nk_img[b]) : nk;
     mbar_wait(full_bar(s), (it >> 1) & 1);
     for (int sl = (warp - rot + RW) % RW; sl < slices; sl += RW) {
       const int r16 = sl * 16;
@@ -439,8 +445,10 @@ attn_resident_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
       for (int n = 0; n < DH / 8; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
       float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
 
-      for (int j0 = 0; j0 + 64 <= nkb; j0 += 64) resident_block<false>(qf, o, m_run, l_run, tK, tV, j0, nkb, scale_log2, lane);
-      if (nkb % 64) resident_block<true>(qf, o, m_run, l_run, tK, tV, nkb & ~63, nkb, scale_log2, lane);
+      constexpr bool DG = MASK == ATTN_MASK_DIAG;
+      const int qrow = i0 + r16 + qr;
+      for (int j0 = 0; j0 + 64 <= nkb; j0 += 64) resident_block<false, DG>(qf, o, m_run, l_run, tK, tV, j0, nkb, scale_log2, lane, qrow);
+      if (nkb % 64) resident_block<true, DG>(qf, o, m_run, l_run, tK, tV, nkb & ~63, nkb, scale_log2, lane, qrow);
 
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
@@ -474,10 +482,10 @@ attn_resident_kernel(const __grid_constant__ CUtensorMap tq, const __grid_consta
 }
 
 // The resident-head form of attention_fast's plain case; false (nothing launched) when the shape is not one it covers.
-// nk_img (may be null): per-image key counts (attention_masked).
+// mask (AttnMask) and nk_img (attention_masked): ATTN_MASK_KEYS takes the per-image key counts nk_img.
 bool attention_resident(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, int ldk, const __nv_bfloat16* v, int ldv,
                         __nv_bfloat16* out, int ldo, int B, int nq, int nk, int heads, float scale_log2, cudaStream_t s,
-                        const int* nk_img = nullptr) {
+                        const int* nk_img = nullptr, int mask = ATTN_MASK_NONE) {
   if (nk > RQ || (ldo % 8)) return false;
   const int qbox = std::min(RQ, (nq + 15) & ~15), kbox = (nk + 15) & ~15;
   const uint64_t inner = static_cast<uint64_t>(heads) * DH;
@@ -487,8 +495,9 @@ bool attention_resident(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k,
   const long long units = static_cast<long long>(B) * heads * ((nq + RQ - 1) / RQ);
   static unsigned long long seen[4] = {0, 0, 0, 0};
   if (first_use_on_this_device(seen)) {
-    VB_CUDA(cudaFuncSetAttribute(attn_resident_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, RSMEM));
-    VB_CUDA(cudaFuncSetAttribute(attn_resident_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, RSMEM));
+    VB_CUDA(cudaFuncSetAttribute(attn_resident_kernel<ATTN_MASK_NONE>, cudaFuncAttributeMaxDynamicSharedMemorySize, RSMEM));
+    VB_CUDA(cudaFuncSetAttribute(attn_resident_kernel<ATTN_MASK_KEYS>, cudaFuncAttributeMaxDynamicSharedMemorySize, RSMEM));
+    VB_CUDA(cudaFuncSetAttribute(attn_resident_kernel<ATTN_MASK_DIAG>, cudaFuncAttributeMaxDynamicSharedMemorySize, RSMEM));
   }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(static_cast<unsigned>(units < sm_count() ? units : sm_count()));
@@ -500,10 +509,14 @@ bool attention_resident(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k,
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  if (nk_img != nullptr)
-    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_resident_kernel<true>, tq, tk, tv, out, ldo, heads, nq, nk, qbox, kbox, units, scale_log2, nk_img));
+  if (mask == ATTN_MASK_KEYS)
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_resident_kernel<ATTN_MASK_KEYS>, tq, tk, tv, out, ldo, heads, nq, nk, qbox, kbox, units, scale_log2,
+                               nk_img));
+  else if (mask == ATTN_MASK_DIAG)
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_resident_kernel<ATTN_MASK_DIAG>, tq, tk, tv, out, ldo, heads, nq, nk, qbox, kbox, units, scale_log2,
+                               static_cast<const int*>(nullptr)));
   else
-    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_resident_kernel<false>, tq, tk, tv, out, ldo, heads, nq, nk, qbox, kbox, units, scale_log2,
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_resident_kernel<ATTN_MASK_NONE>, tq, tk, tv, out, ldo, heads, nq, nk, qbox, kbox, units, scale_log2,
                                static_cast<const int*>(nullptr)));
   return true;
 }
@@ -827,12 +840,13 @@ bool attention_fast<__nv_bfloat16>(const __nv_bfloat16* q, int ldq, const __nv_b
 
 bool attention_masked(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, int ldk, const __nv_bfloat16* v, int ldv,
                       __nv_bfloat16* out, int ldo, int B, int nq, int nk, int heads, int dh, cudaStream_t s, float scale,
-                      const int* nk_img) {
+                      const int* nk_img, int mask) {
   if (dh != DH || nq < 1 || nk < 1 || B < 1 || (ldq % 8) || (ldk % 8) || (ldv % 8) || (ldo % 2)) return false;
+  if (mask == ATTN_MASK_DIAG && (nq != nk || nk < 2)) return false;
   if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
        reinterpret_cast<uintptr_t>(out)) % 16) return false;
   const float scale_log2 = (scale > 0.f ? scale : 1.0f / sqrtf(static_cast<float>(dh))) * 1.4426950408889634f;
-  if (!attention_resident(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, heads, scale_log2, s, nk_img)) {
+  if (!attention_resident(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, heads, scale_log2, s, nk_img, mask)) {
     const long long blocks = static_cast<long long>(B) * heads * ((nq + FQ - 1) / FQ);
     if (blocks > 0x7fffffffLL) return false;
     cudaLaunchConfig_t cfg = {};
@@ -844,8 +858,12 @@ bool attention_masked(const __nv_bfloat16* q, int ldq, const __nv_bfloat16* k, i
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<DH, false, false, true>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
-                               static_cast<const float*>(nullptr), 0, 1, 0, Window(), nk_img));
+    if (mask == ATTN_MASK_DIAG)
+      VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<DH, false, false, ATTN_MASK_DIAG>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk,
+                                 scale_log2, static_cast<const float*>(nullptr), 0, 1, 0, Window(), static_cast<const int*>(nullptr)));
+    else
+      VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<DH, false, false, ATTN_MASK_KEYS>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk,
+                                 scale_log2, static_cast<const float*>(nullptr), 0, 1, 0, Window(), nk_img));
   }
   count_launch();
   note_attention_path(ATTN_PATH_FLASH);

@@ -128,6 +128,8 @@ struct LayerW {                    // one pre-norm transformer layer in any of t
   int dh_model = 0;                  // the model's dim_head: softmax scale dh_model^-0.5 (vit.py:57)
   int t2t_D = 0, t2t_Dp = 0;         // tensor-core T2T soft-split layer: true width D (LayerNorm, softmax scale), padded width Dp
   bool folded = false;               // attn_norm / ff_norm folded into to_qkv (to_q, to_kv) / fc1
+  bool lsa = false;                  // locality self-attention (vit_for_small_dataset.py:88-121): the diagonal masked, scale lsa_scale
+  float lsa_scale = 0.f;             // exp(temperature), taken in fp32 as TensorFlow does
 };
 
 // One LeViT Transformer layer (levit.py:141-162): attention (queries on every step-th pixel of the fmap x fmap map) + MLP.
@@ -269,7 +271,9 @@ inline bool r2l_attention_fast(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* 
   return attention_r2l(qkv, ld, out, ldo, heads, dh, reg_row0, pb, win, s);
 }
 
-struct EmbedW { Linear patch; const float* pos = nullptr; const float* cls = nullptr; int dim = 0, n_pos = 0; };
+// res_bias (may be null: patch.bias): what the patch Dense yields on an all-zero (cls) row when that is not its bias -- beta . W +
+// bias when a LayerNorm runs before it (SPT, vit_for_small_dataset.py:148-149)
+struct EmbedW { Linear patch; const float* pos = nullptr; const float* cls = nullptr; int dim = 0, n_pos = 0; const float* res_bias = nullptr; };
 struct CrossW { bool proj = false; Linear project_in, project_out, to_q, to_kv, to_out; Norm norm; };
 
 inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
@@ -575,6 +579,7 @@ struct vb_handle {
   }
   Norm head_norm, sm_head_norm, lg_head_norm;
   Linear head, sm_head, lg_head;
+  Norm spt_norm;                     // SPT's LayerNorm over the p^2 * 5 C patch vector (bf16: padded to the GEMM's K, folded into it)
 
   // cached patch-embedding residual terms, keyed by (embed ptr, batch, rows)
   struct ResKey { const void* e; int B, rows; bool operator<(const ResKey& o) const { return std::tie(e, B, rows) < std::tie(o.e, o.B, o.rows); } };
@@ -630,7 +635,8 @@ struct vb_handle {
   void expect_layer(const std::string& pre, int dim, int heads, int dh, int mlp, int kind) {
     const int inner = heads * dh;
     expect_ln(pre + "attn_norm", dim);
-    if (kind == VB_KIND_VIT || kind == VB_KIND_DEEPVIT || kind == VB_KIND_ATS_VIT) expect_dense(pre + "to_qkv", dim, 3 * inner, false);
+    if (kind == VB_KIND_VIT || kind == VB_KIND_DEEPVIT || kind == VB_KIND_ATS_VIT || kind == VB_KIND_SMALL_DATASET_VIT)
+      expect_dense(pre + "to_qkv", dim, 3 * inner, false);
     else { expect_dense(pre + "to_q", dim, inner, false); expect_dense(pre + "to_kv", dim, 2 * inner, false); }
     if (kind == VB_KIND_DEEPVIT) { expect(pre + "reattn_weights", {heads, heads}); expect_ln(pre + "reattn_norm", heads); }
     if (kind == VB_KIND_CAIT) { expect(pre + "mix_pre", {heads, heads}); expect(pre + "mix_post", {heads, heads}); }
@@ -655,6 +661,19 @@ struct vb_handle {
         } else {
           expect_layer("layers." + std::to_string(L) + ".", c.dim, c.heads, c.dim_head, c.mlp_dim, c.kind);
         }
+      }
+      expect_ln("head_norm", c.dim);
+      expect_dense("head", c.dim, c.num_classes);
+    } else if (c.kind == VB_KIND_SMALL_DATASET_VIT) {                   // vit_for_small_dataset.py:142-195
+      const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w), K = c.patch_h * c.patch_w * 5 * C;
+      expect("pos_embedding", {1, np + 1, c.dim});
+      expect("cls_token", {1, 1, c.dim});
+      expect_ln("patch_norm", K);                                        // to_patch_tokens.layers[1]
+      expect_dense("patch", K, c.dim);                                   // to_patch_tokens.layers[2]
+      for (int L = 0; L < c.depth; ++L) {
+        const std::string pre = "layers." + std::to_string(L) + ".";
+        expect_layer(pre, c.dim, c.heads, c.dim_head, c.mlp_dim, c.kind);   // to_out always present (no project_out skip, :99-102)
+        expect(pre + "temperature", {});                                 // LSA's scalar tf.Variable (:94)
       }
       expect_ln("head_norm", c.dim);
       expect_dense("head", c.dim, c.num_classes);
@@ -1013,7 +1032,7 @@ struct vb_handle {
     // the tensor-core attention path for e.g. dim_head 48 / 32 (the head-mixing variants have their own kernel, attn_mix).
     const bool to_out_present = has(pre + "to_out.kernel");
     if (bf16() && dh < 64 && dh % 8 == 0 && to_out_present && dim % 8 == 0 && getenv("VB_NO_HEAD_PAD") == nullptr &&
-        (kind == VB_KIND_VIT || kind == VB_KIND_CROSSVIT || kind == VB_KIND_ATS_VIT)) {
+        (kind == VB_KIND_VIT || kind == VB_KIND_CROSSVIT || kind == VB_KIND_ATS_VIT || kind == VB_KIND_SMALL_DATASET_VIT)) {
       const int dhp = 64;
       auto padded = [&](const std::string& n, int other, int groups, int pad_rows) {
         owned.emplace_back(new DevMem());
@@ -1022,7 +1041,7 @@ struct vb_handle {
         pad_heads_f32(W(n), wp, other, groups, heads, dh, dhp, pad_rows, 0);
         woverride[n] = wp;
       };
-      if (kind == VB_KIND_VIT || kind == VB_KIND_ATS_VIT) padded(pre + "to_qkv.kernel", dim, 3, 0);
+      if (kind == VB_KIND_VIT || kind == VB_KIND_ATS_VIT || kind == VB_KIND_SMALL_DATASET_VIT) padded(pre + "to_qkv.kernel", dim, 3, 0);
       else { padded(pre + "to_q.kernel", dim, 1, 0); padded(pre + "to_kv.kernel", dim, 2, 0); }
       padded(pre + "to_out.kernel", dim, 1, 1);
       dh = dhp;
@@ -1035,7 +1054,10 @@ struct vb_handle {
     l.folded = bf16() && fold_ok && dim % 64 == 0 && inner % 64 == 0 && mlp % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr;
     const Norm* fa = l.folded ? &l.attn_norm : nullptr;
     const Norm* ff = l.folded ? &l.ff_norm : nullptr;
-    if (kind == VB_KIND_VIT || kind == VB_KIND_DEEPVIT || kind == VB_KIND_ATS_VIT) { l.fused_qkv = true; l.to_qkv = make_linear(pre + "to_qkv", dim, 3 * inner, false, fa); }
+    if (kind == VB_KIND_VIT || kind == VB_KIND_DEEPVIT || kind == VB_KIND_ATS_VIT || kind == VB_KIND_SMALL_DATASET_VIT) {
+      l.fused_qkv = true;
+      l.to_qkv = make_linear(pre + "to_qkv", dim, 3 * inner, false, fa);
+    }
     else if (bf16() && fold_ok && dim % 8 == 0) {   // self-attention only: q and kv read the same rows -> one GEMM
       l.fused_qkv = true;
       l.to_qkv = make_linear_pair(pre + "to_q", inner, pre + "to_kv", 2 * inner, dim, fa);
@@ -1129,6 +1151,8 @@ struct vb_handle {
       }
       head_norm = make_norm("head_norm", c.dim);
       head = make_linear_f32("head", c.dim, c.num_classes);
+    } else if (c.kind == VB_KIND_SMALL_DATASET_VIT) {
+      finalize_small_dataset_vit();
     } else if (c.kind == VB_KIND_PATCH_MERGER_VIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       embed = make_embed("", c.patch_h, c.patch_w, c.dim, np + 1, false);
@@ -1622,6 +1646,40 @@ struct vb_handle {
     return t;
   }
 
+  // vit_for_small_dataset.ViT (:159-195).  SPT's LayerNorm over K = p^2 * 5 C (eps 1e-3) and Dense: the bf16 engine zero-pads K
+  // to Kp = round_up(K, 64) and folds the LayerNorm into the wgmma GEMM (dim % 64 == 0); the fp32 engine keeps K and runs the
+  // LayerNorm kernel.  Either way the Dense yields beta . W + bias on the all-zero cls row, so that is the term the embedding
+  // residual takes off (res_bias).  The layers are ViT's with LSA: the diagonal mask and exp(temperature) as the softmax scale.
+  void finalize_small_dataset_vit() {
+    const vb_config& c = cfg;
+    const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w), K = c.patch_h * c.patch_w * 5 * c.channels;
+    const int Kp = bf16() ? round_up(K, 64) : K;
+    const bool fold = bf16() && c.dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr;
+    embed = EmbedW();
+    spt_norm = padded_norm("patch_norm", K, Kp, ".gamma", ".beta");
+    embed.patch = padded_dense("spt.patch", "patch", K, c.dim, Kp, c.dim, fold ? &spt_norm : nullptr, 1e-3f);
+    if (fold) {
+      embed.res_bias = embed.patch.ln_c2;
+    } else {
+      const std::vector<double> beta = host_weight("patch_norm.beta"), Wk = host_weight("patch.kernel");
+      std::vector<double> c2 = host_weight("patch.bias");
+      for (int k = 0; k < K; ++k)
+        for (int n = 0; n < c.dim; ++n) c2[n] += beta[k] * Wk[static_cast<size_t>(k) * c.dim + n];
+      embed.res_bias = upload_owned(c2);
+    }
+    embed.pos = W("pos_embedding");
+    embed.cls = W("cls_token");
+    embed.dim = c.dim; embed.n_pos = np + 1;
+    for (int L = 0; L < c.depth; ++L) {
+      const std::string pre = "layers." + std::to_string(L) + ".";
+      layers.push_back(make_layer(pre, c.dim, c.heads, c.dim_head, c.mlp_dim, c.kind));
+      layers.back().lsa = true;
+      layers.back().lsa_scale = expf(static_cast<float>(host_weight(pre + "temperature")[0]));
+    }
+    head_norm = make_norm("head_norm", c.dim);
+    head = make_linear_f32("head", c.dim, c.num_classes);
+  }
+
   Linear make_linear_f32(const std::string& n, int K, int N) {  // classifier head always runs in fp32
     Linear L;
     L.W = W(n + ".kernel"); L.bias = W(n + ".bias"); L.K = K; L.N = N; L.ldw = K;
@@ -1654,7 +1712,8 @@ struct vb_handle {
       if (embed_res.size() >= 6) { VB_CUDA(cudaStreamSynchronize(s)); embed_res.clear(); drop_graphs(); }
       std::unique_ptr<DevMem> m(new DevMem());
       m->ensure(static_cast<size_t>(B) * rows * e.dim * sizeof(T));
-      build_embed_residual<T>(static_cast<T*>(m->p), e.pos, e.cls, e.patch.bias, B, rows, e.dim, e.cls != nullptr, s);
+      build_embed_residual<T>(static_cast<T*>(m->p), e.pos, e.cls, e.res_bias != nullptr ? e.res_bias : e.patch.bias, B, rows, e.dim,
+                              e.cls != nullptr, s);
       it = embed_res.emplace(key, std::move(m)).first;
     }
     return static_cast<const T*>(it->second->p);
@@ -1680,13 +1739,16 @@ struct vb_handle {
     return embed_from_cols<T>(e, col, Kp, B, rows, s, stats_out);
   }
   // X = cols . W + bias + (pos (+ cls on row 0)): the Dense of the patch embedding with cls concat and positions folded
-  // into its residual operand.  cols [B*rows, Kp]: patch vectors, zero in the cls rows and in the pad columns.
+  // into its residual operand.  cols [B*rows, Kp]: patch vectors, zero in the cls rows and in the pad columns.  ln_stats (bf16, a
+  // patch Dense with a LayerNorm folded in): the row statistics of cols.
   template <typename T>
-  T* embed_from_cols(const EmbedW& e, const T* col, int Kp, int B, int rows, cudaStream_t s, float** stats_out) {
+  T* embed_from_cols(const EmbedW& e, const T* col, int Kp, int B, int rows, cudaStream_t s, float** stats_out,
+                     const float* ln_stats = nullptr) {
     const int M = B * rows;
     const T* R = embed_residual<T>(e, B, rows, s);
     T* X = arena.get<T>(static_cast<size_t>(M) * e.dim);
     Epi ep; ep.bias = e.patch.bias; ep.res = R; ep.ldr = e.dim;
+    if (ln_stats != nullptr) { ep.ln_stats = ln_stats; ep.bias = e.patch.ln_c2; }
     if (stats_out != nullptr && bf16() && e.dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr) {
       *stats_out = row_stats(M, e.dim);
       ep.stats_out = *stats_out;
@@ -1695,6 +1757,34 @@ struct vb_handle {
     L.K = Kp;  // im2col zero-pads the patch vector to the packed weight pitch
     linear<T>(col, Kp, M, L, X, e.dim, ep, s);
     return X;
+  }
+
+  // SPT + cls token + positions (vit_for_small_dataset.py:152-157, 198-203) -> X [B*rows, dim]: spt_rows writes the patch vectors
+  // of the image and its four shifts (zero cls rows and pad columns), then the LayerNorm (folded into the GEMM in bf16, from the
+  // rows' statistics) and the Dense with cls and positions in its residual operand.
+  template <typename T>
+  T* spt_tokens(const float* img, int B, int H, int Wd, int* rows_out, cudaStream_t s, float** stats_out) {
+    const int p = cfg.patch_h;
+    VB_CHECK(H % p == 0 && Wd % p == 0, "Image dimensions must be divisible by the patch size.");
+    const int rows = (H / p) * (Wd / p) + 1, M = B * rows, Kp = embed.patch.K;
+    VB_CHECK(rows <= embed.n_pos, "image has more patches than pos_embedding rows");
+    T* col = arena.get<T>(static_cast<size_t>(M) * Kp);
+    {
+      ProfScope ps(this, PROF_EMBED, 0.0, 4.0 * B * H * Wd * cfg.channels + static_cast<double>(sizeof(T)) * M * Kp, s);
+      spt_rows<T>(img, col, B, H, Wd, cfg.channels, p, Kp, s);
+    }
+    *rows_out = rows;
+    if (embed.patch.ln_c1 != nullptr) {
+      float* st = row_stats(M, Kp);
+      ensure_stats(col, Kp, st, M, s);
+      return embed_from_cols<T>(embed, col, Kp, B, rows, s, stats_out, st);
+    }
+    T* Y = arena.get<T>(static_cast<size_t>(M) * Kp);
+    {
+      ProfScope ps(this, PROF_LN, 0.0, 2.0 * sizeof(T) * M * Kp, s);
+      layernorm<T>(col, Kp, spt_norm.gamma, spt_norm.beta, Y, Kp, M, spt_norm.D, s, Kp);   // Keras eps 1e-3, pad columns zero
+    }
+    return embed_from_cols<T>(embed, Y, Kp, B, rows, s, stats_out);
   }
 
   // T2TViT.patch_embedding + cls + positions (t2t.py:58-74,97-103): soft split i = unfold_same over the previous token map
@@ -1850,7 +1940,7 @@ struct vb_handle {
       T* QKV = arena.get<T>(static_cast<size_t>(M) * 3 * inner);
       Epi e = eq; e.bias = l.to_qkv.ln_c2;
       linear<T>(A, dim, M, l.to_qkv, QKV, 3 * inner, e, s);
-      if (nk_img != nullptr) attention_masked_dispatch<T>(QKV, 3 * inner, O, inner, B, rows, l, s, nk_img);
+      if (nk_img != nullptr || l.lsa) attention_masked_dispatch<T>(QKV, 3 * inner, O, inner, B, rows, l, s, nk_img);
       else attention<T>(QKV, 3 * inner, QKV + inner, 3 * inner, QKV + 2 * inner, 3 * inner, O, inner, B, rows, rows, l, s);
       qkv = QKV;
     } else {
@@ -1873,23 +1963,26 @@ struct vb_handle {
     }
     return qkv;
   }
-  // Plain attention over the fused q|k|v rows with image b's keys >= nk_img[b] masked: the flash kernels at dh 64 (bf16), else the
-  // materialised-scores path with the mask in its softmax
+  // Plain attention over the fused q|k|v rows with masked keys: image b's keys >= nk_img[b] (ATS-ViT), or the diagonal with the
+  // scale exp(temperature) for an LSA layer.  The flash kernels at dh 64 (bf16), else the materialised-scores path with the mask in
+  // its softmax.
   template <typename T>
   void attention_masked_dispatch(const T* qkv, int ld, T* out, int ldo, int B, int n, const LayerW& l, cudaStream_t s, const int* nk_img) {
     const int heads = l.heads, dh = l.dim_head, HD = heads * dh;
-    const float scale = 1.0f / sqrtf(static_cast<float>(l.dh_model));
+    const float scale = l.lsa ? l.lsa_scale : 1.0f / sqrtf(static_cast<float>(l.dh_model));
+    const int mask = l.lsa ? ATTN_MASK_DIAG : ATTN_MASK_KEYS;
+    VB_CHECK(!l.lsa || n >= 2, "locality self-attention needs at least 2 tokens (every row keeps a key besides its own)");
     ProfScope ps(this, PROF_ATTN, 4.0 * B * heads * n * n * dh, static_cast<double>(sizeof(T)) * B * heads * dh * 4.0 * n, s);
-    if (masked_flash(qkv, ld, out, ldo, B, n, heads, dh, s, scale, nk_img)) return;
+    if (masked_flash(qkv, ld, out, ldo, B, n, heads, dh, s, scale, nk_img, mask)) return;
     VB_CHECK(dh == l.dh_model, "internal: a head-padded layer must run on the fused attention kernel");
     float* S = arena.get<float>(static_cast<size_t>(B) * heads * n * n);
-    attention_generic_masked<T>(qkv, ld, qkv + HD, ld, qkv + 2 * HD, ld, out, ldo, S, B, n, n, heads, dh, s, scale, nk_img);
+    attention_generic_masked<T>(qkv, ld, qkv + HD, ld, qkv + 2 * HD, ld, out, ldo, S, B, n, n, heads, dh, s, scale, nk_img, mask);
   }
-  static bool masked_flash(const float*, int, float*, int, int, int, int, int, cudaStream_t, float, const int*) { return false; }
+  static bool masked_flash(const float*, int, float*, int, int, int, int, int, cudaStream_t, float, const int*, int) { return false; }
   static bool masked_flash(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* out, int ldo, int B, int n, int heads, int dh, cudaStream_t s,
-                           float scale, const int* nk_img) {
+                           float scale, const int* nk_img, int mask) {
     const int HD = heads * dh;
-    return attention_masked(qkv, ld, qkv + HD, ld, qkv + 2 * HD, ld, out, ldo, B, n, n, heads, dh, s, scale, nk_img);
+    return attention_masked(qkv, ld, qkv + HD, ld, qkv + 2 * HD, ld, out, ldo, B, n, n, heads, dh, s, scale, nk_img, mask);
   }
 
   // ATS-ViT's forward (ats_vit.py:300-318, Transformer.call :236-258) in the compact row layout of ats.cu: image b's rows at the
@@ -2192,6 +2285,13 @@ struct vb_handle {
       regionvit_forward<T>(img, B, H, Wd, logits, s);
     } else if (c.kind == VB_KIND_ATS_VIT) {
       ats_forward<T>(img, B, H, Wd, logits, s);
+    } else if (c.kind == VB_KIND_SMALL_DATASET_VIT) {     // vit_for_small_dataset.py:197-215, Transformer.call :135-140
+      int rows = 0;
+      float* stats = nullptr;
+      T* X = spt_tokens<T>(img, B, H, Wd, &rows, s, &stats);
+      bool sv = stats != nullptr;
+      for (const auto& l : layers) layer_self<T>(X, B, rows, c.dim, l, s, stats, &sv);
+      classify<T>(X, rows, c.dim, head_norm, head, B, c.pool == VB_POOL_MEAN, logits, false, s);
     } else if (c.kind == VB_KIND_CCT) {                   // CCT.call cct.py:342-345, TransformerClassifier.call :277-305
       int rows = 0;
       T* X = tokenize_cct<T>(img, B, H, Wd, &rows, s);
@@ -2933,6 +3033,7 @@ struct vb_handle {
       case VB_KIND_NEST: return "NesT runs as a whole forward only: its patch-embedding / level / head steps have no entry of their own";
       case VB_KIND_REGIONVIT: return "RegionViT runs as a whole forward only: its encoder / stage / head steps have no entry of their own";
       case VB_KIND_ATS_VIT: return "ATS-ViT runs as a whole forward only: its token count changes inside the transformer, so its stages have no entry of their own";
+      case VB_KIND_SMALL_DATASET_VIT: return "the small-dataset ViT runs as a whole forward only: its SPT embedding / transformer / head steps have no entry of their own";
       default: return nullptr;
     }
   }
@@ -3181,7 +3282,12 @@ void validate(const vb_config& c) {
   VB_CHECK(c.kind != VB_KIND_NEST, "NesT: create the handle with vb_create_nest (its levels are a vb_nest_config)");
   VB_CHECK(c.kind != VB_KIND_REGIONVIT, "RegionViT: create the handle with vb_create_regionvit (its stages are a vb_regionvit_config)");
   VB_CHECK(c.kind != VB_KIND_ATS_VIT, "ATS-ViT: create the handle with vb_create_ats_vit (its token counts are a vb_ats_vit_config)");
-  VB_CHECK(c.kind >= VB_KIND_VIT && c.kind <= VB_KIND_CCT, "unknown model kind");
+  VB_CHECK((c.kind >= VB_KIND_VIT && c.kind <= VB_KIND_CCT) || c.kind == VB_KIND_SMALL_DATASET_VIT, "unknown model kind");
+  if (c.kind == VB_KIND_SMALL_DATASET_VIT) {
+    // SPT's Rearrange takes one patch size for both sides (vit_for_small_dataset.py:147) and shift() one image of 3 channels
+    VB_CHECK(c.patch_h == c.patch_w, "the small-dataset ViT takes one integer patch_size (SPT's Rearrange uses it for both sides)");
+    VB_CHECK(c.channels == 3, "the small-dataset ViT takes images of 3 channels");
+  }
   if (c.kind == VB_KIND_CCT) {
     VB_CHECK(c.channels == 3 && c.num_classes > 0 && c.image_h > 0 && c.image_w > 0, "bad image / class configuration");
     VB_CHECK(c.cct_conv_layers >= 1 && c.cct_conv_layers <= 8, "CCT: n_conv_layers must be in [1, 8]");
@@ -3610,7 +3716,7 @@ int vb_op_masked_attention(int32_t precision, const float* qkv, int32_t ld, int3
       T* o_d = upload<T>(dO, out, static_cast<size_t>(B) * n * ldo);
       // vb_handle::attention_masked_dispatch without the handle's arena and profiler
       timed(iters, elapsed_ms, [&] {
-        if (vb_handle::masked_flash(x_d, ld, o_d, ldo, B, n, heads, dh, 0, scale, nk_d)) return;
+        if (vb_handle::masked_flash(x_d, ld, o_d, ldo, B, n, heads, dh, 0, scale, nk_d, ATTN_MASK_KEYS)) return;
         dS.ensure(static_cast<size_t>(B) * heads * n * n * sizeof(float));
         attention_generic_masked<T>(x_d, ld, x_d + HD, ld, x_d + 2 * HD, ld, o_d, ldo, static_cast<float*>(dS.p), B, n, n, heads, dh, 0, scale,
                                     nk_d);
@@ -3619,6 +3725,123 @@ int vb_op_masked_attention(int32_t precision, const float* qkv, int32_t ld, int3
     };
     if (precision == VB_PRECISION_FP32) run(float());
     else run(__nv_bfloat16());
+  });
+}
+
+int vb_op_spt(int32_t precision, const float* img, int32_t B, int32_t H, int32_t W, int32_t p, int32_t dim, const float* gamma,
+              const float* beta, const float* kernel, const float* bias, const float* cls, const float* pos, float* out) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    VB_CHECK(img && gamma && beta && kernel && bias && out && B > 0 && H > 0 && W > 0 && p > 0 && dim > 0, "vb_op_spt: bad arguments");
+    VB_CHECK(H % p == 0 && W % p == 0, "Image dimensions must be divisible by the patch size.");
+    // vb_handle::spt_tokens with the weights of finalize_small_dataset_vit, outside a handle
+    const bool bf = precision == VB_PRECISION_BF16, fold = bf && dim % 64 == 0;
+    const int C = 3, K = p * p * 5 * C, Kp = bf ? round_up(K, 64) : K, rows = 1 + (H / p) * (W / p), M = B * rows;
+    std::vector<float> g(Kp, 0.f), bt(Kp, 0.f), w(static_cast<size_t>(Kp) * dim, 0.f), c2(bias, bias + dim), cl(dim, 0.f),
+        ps(static_cast<size_t>(rows) * dim, 0.f);
+    std::copy(gamma, gamma + K, g.begin());
+    std::copy(beta, beta + K, bt.begin());
+    std::copy(kernel, kernel + static_cast<size_t>(K) * dim, w.begin());
+    if (cls) std::copy(cls, cls + dim, cl.begin());
+    if (pos) std::copy(pos, pos + static_cast<size_t>(rows) * dim, ps.begin());
+    for (int k = 0; k < K; ++k)                                    // beta . W + bias: the Dense on the LayerNorm of a zero row
+      for (int n = 0; n < dim; ++n) c2[n] += beta[k] * kernel[static_cast<size_t>(k) * dim + n];
+    DevMem dI, dG, dBt, dW, dB, dC2, dCl, dP, dCol, dY, dR, dO, dWt, dF, dSt;
+    const float* img_d = upload<float>(dI, img, static_cast<size_t>(B) * H * W * C);
+    const float* g_d = upload<float>(dG, g.data(), Kp);
+    const float* bt_d = upload<float>(dBt, bt.data(), Kp);
+    const float* w_d = upload<float>(dW, w.data(), w.size());
+    const float* b_d = upload<float>(dB, bias, dim);
+    const float* cl_d = upload<float>(dCl, cl.data(), dim);
+    const float* p_d = upload<float>(dP, ps.data(), ps.size());
+    auto run = [&](auto tag) {
+      using T = decltype(tag);
+      dCol.ensure(static_cast<size_t>(M) * Kp * sizeof(T));
+      T* col = static_cast<T*>(dCol.p);
+      spt_rows<T>(img_d, col, B, H, W, C, p, Kp, 0);
+      dR.ensure(static_cast<size_t>(M) * dim * sizeof(T));
+      dO.ensure(static_cast<size_t>(M) * dim * sizeof(T));
+      T* R = static_cast<T*>(dR.p);
+      T* o_d = static_cast<T*>(dO.p);
+      if constexpr (sizeof(T) == 2) {
+        dWt.ensure(static_cast<size_t>(dim) * Kp * sizeof(T));
+        T* wt = static_cast<T*>(dWt.p);
+        if (fold) {
+          pack_weight_bf16(w_d, wt, Kp, dim, Kp, 0, g_d);
+          dF.ensure(static_cast<size_t>(dim) * 2 * sizeof(float));
+          float* c = static_cast<float*>(dF.p);
+          ln_fold_consts(w_d, wt, Kp, bt_d, b_d, c, c + dim, Kp, dim, 0);
+          dSt.ensure(static_cast<size_t>(M) * (Kp / 64) * 2 * sizeof(float));
+          float* st = static_cast<float*>(dSt.p);
+          row_stats_bf16(col, Kp, st, M, Kp, 0);
+          build_embed_residual<T>(R, p_d, cl_d, c + dim, B, rows, dim, 1, 0);
+          GemmBf16 gm = gemm_bf16_plan(col, Kp, wt, Kp, o_d, dim, M, dim, Kp, c + dim, nullptr, R, dim, ACT_NONE);
+          gm.ln_c1 = c; gm.ln_stats = st; gm.ln_parts = Kp / 64; gm.ln_inv_d = 1.0f / static_cast<float>(K); gm.ln_eps = 1e-3f;
+          gemm_bf16_run(gm, 0);
+          download<T>(o_d, out, static_cast<size_t>(M) * dim);
+          return;
+        }
+        pack_weight_bf16(w_d, wt, Kp, dim, Kp, 0);
+      }
+      dY.ensure(static_cast<size_t>(M) * Kp * sizeof(T));
+      T* Y = static_cast<T*>(dY.p);
+      layernorm<T>(col, Kp, g_d, bt_d, Y, Kp, M, K, 0, Kp);
+      const float* c2_d = upload<float>(dC2, c2.data(), dim);
+      build_embed_residual<T>(R, p_d, cl_d, c2_d, B, rows, dim, 1, 0);
+      if constexpr (sizeof(T) == 2)
+        gemm_simt<T, T, T>(Y, Kp, static_cast<const T*>(dWt.p), 1, Kp, o_d, dim, M, dim, Kp, b_d, nullptr, R, dim, ACT_NONE, 0);
+      else
+        gemm_simt<float, float, float>(Y, Kp, w_d, dim, 1, o_d, dim, M, dim, Kp, b_d, nullptr, R, dim, ACT_NONE, 0);
+      download<T>(o_d, out, static_cast<size_t>(M) * dim);
+    };
+    if (bf) run(__nv_bfloat16());
+    else run(float());
+    VB_CUDA(cudaDeviceSynchronize());
+  });
+}
+
+int vb_op_lsa_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t n, int32_t heads, int32_t dh, float scale,
+                        float* out, int32_t ldo, int32_t iters, float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    const int HD = heads * dh;
+    VB_CHECK(qkv && out && B > 0 && n > 0 && heads > 0 && dh > 0 && ld >= 3 * HD && ldo >= HD && scale > 0.f,
+             "vb_op_lsa_attention: bad arguments");
+    VB_CHECK(n >= 2, "vb_op_lsa_attention: locality self-attention needs n >= 2 (every row keeps a key besides its own)");
+    // bf16 heads narrower than 64 run widened with zero columns, as make_layer widens an LSA layer's to_qkv / to_out
+    const bool widen = precision == VB_PRECISION_BF16 && dh < 64 && dh % 8 == 0;
+    const int dw = widen ? 64 : dh, HW = heads * dw, ldw = widen ? 3 * HW : ld, ldow = widen ? HW : ldo;
+    std::vector<float> wide, wout;
+    const float* src = qkv;
+    if (widen) {
+      wide.assign(static_cast<size_t>(B) * n * ldw, 0.f);
+      for (size_t r = 0; r < static_cast<size_t>(B) * n; ++r)
+        for (int g = 0; g < 3; ++g)
+          for (int h = 0; h < heads; ++h)
+            std::copy(qkv + r * ld + g * HD + h * dh, qkv + r * ld + g * HD + h * dh + dh, wide.begin() + r * ldw + g * HW + h * dw);
+      wout.assign(static_cast<size_t>(B) * n * ldow, 0.f);
+      src = wide.data();
+    }
+    DevMem dX, dO, dS;
+    auto run = [&](auto tag) {
+      using T = decltype(tag);
+      const T* x_d = upload<T>(dX, src, static_cast<size_t>(B) * n * ldw);
+      T* o_d = upload<T>(dO, widen ? wout.data() : out, static_cast<size_t>(B) * n * ldow);
+      // vb_handle::attention_masked_dispatch of an LSA layer without the handle's arena and profiler
+      timed(iters, elapsed_ms, [&] {
+        if (vb_handle::masked_flash(x_d, ldw, o_d, ldow, B, n, heads, dw, 0, scale, nullptr, ATTN_MASK_DIAG)) return;
+        dS.ensure(static_cast<size_t>(B) * heads * n * n * sizeof(float));
+        attention_generic_masked<T>(x_d, ldw, x_d + HW, ldw, x_d + 2 * HW, ldw, o_d, ldow, static_cast<float*>(dS.p), B, n, n, heads, dw, 0,
+                                    scale, nullptr, ATTN_MASK_DIAG);
+      });
+      download<T>(o_d, widen ? wout.data() : out, static_cast<size_t>(B) * n * ldow);
+    };
+    if (precision == VB_PRECISION_FP32) run(float());
+    else run(__nv_bfloat16());
+    if (widen)
+      for (size_t r = 0; r < static_cast<size_t>(B) * n; ++r)
+        for (int h = 0; h < heads; ++h)
+          std::copy(wout.begin() + r * ldow + h * dw, wout.begin() + r * ldow + h * dw + dh, out + r * ldo + h * dh);
   });
 }
 
@@ -3758,6 +3981,7 @@ int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, int32_t 
     VB_CHECK(h->cfg.kind != VB_KIND_NEST, "vb_forward_distill: NesT has no distillation head");
     VB_CHECK(h->cfg.kind != VB_KIND_REGIONVIT, "vb_forward_distill: RegionViT has no distillation head");
     VB_CHECK(h->cfg.kind != VB_KIND_ATS_VIT, h->whole_forward_only(VB_KIND_ATS_VIT));
+    VB_CHECK(h->cfg.kind != VB_KIND_SMALL_DATASET_VIT, h->whole_forward_only(VB_KIND_SMALL_DATASET_VIT));
     const bool levit = h->cfg.kind == VB_KIND_LEVIT;
     VB_CHECK(levit || distill_token != nullptr, "vb_forward_distill: null argument");
     VB_CHECK(!levit || (distill_token == nullptr && h->lv.num_distill_classes > 0),
@@ -3882,6 +4106,7 @@ int vb_to_patch(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, 
                 int32_t patches_mem, void* stream) {
   return guarded(h, [&] {
     VB_CHECK(h != nullptr && img != nullptr && patches != nullptr, "vb_to_patch: null argument");
+    VB_CHECK(h->cfg.kind != VB_KIND_SMALL_DATASET_VIT, h->whole_forward_only(VB_KIND_SMALL_DATASET_VIT));
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT && h->cfg.kind != VB_KIND_T2T_VIT && h->cfg.kind != VB_KIND_CCT &&
              h->cfg.kind != VB_KIND_LEVIT && h->cfg.kind != VB_KIND_CVT && h->cfg.kind != VB_KIND_TWINS_SVT &&
              h->cfg.kind != VB_KIND_CROSSFORMER && h->cfg.kind != VB_KIND_NEST && h->cfg.kind != VB_KIND_REGIONVIT,

@@ -197,8 +197,17 @@ void ats_gather(const T* X, int P, T* Xn, int Pn, int dim, const int* sel, const
                 const int* C_old, int K, int* C_new, unsigned long long* rng, cudaStream_t s);
 // out [B, P - 1] = the reference's returned token ids (ats_vit.py:315): image b's kept patch ids in columns [C - c_b, C), -1 elsewhere
 void ats_ids_out(const int* ids, int P, const int* rows, const int* C, int* out, int B, cudaStream_t s);
-// attn_softmax with the keys j >= nk_img[row / rows_per_img] of every row masked: their weight is exactly 0
-void attn_softmax_masked(float* S, long long rows, int nk, long long rows_per_img, const int* nk_img, cudaStream_t s);
+// attn_softmax with the keys j >= nk_img[row / rows_per_img] of every row masked (nk_img may be null: none), and with
+// diag_nq > 0 also the key j == row % diag_nq (locality self-attention's diagonal, rows [.., nq] with nq == diag_nq == nk): their
+// weight is exactly 0
+void attn_softmax_masked(float* S, long long rows, int nk, long long rows_per_img, const int* nk_img, cudaStream_t s, int diag_nq = 0);
+
+// ---- shifted patch tokens (vit_for_small_dataset.py:15-47, 142-157; small_vit.cu).  out [B * (1 + np), ldo]: per image a zero
+// cls row, then patch t = (gy, gx) of the (H / p) x (W / p) grid as the vector [p1][p2][view][c] of the image concatenated with
+// its four one-pixel shifts (view 1: x[:, w - 1], 2: x[:, w + 1], 3: x[h - 1], 4: x[h + 1], zero past the edge), so element
+// ((p1 p + p2) 5 + view) C + c; columns from 5 C p^2 to ldo are zero.  img fp32 NHWC [B, H, W, C].
+template <typename T>
+void spt_rows(const float* img, T* out, int B, int H, int W, int C, int p, int ldo, cudaStream_t s);
 
 long long launch_counter();      // number of kernel launches issued through these wrappers (process-wide)
 void count_launch(int n = 1);

@@ -185,7 +185,7 @@ class _EngineModel:
         for name, arr in weights.items():
             if name not in self._specs:
                 raise KeyError(f"{type(self).__name__} has no weight named {name!r}")
-            a = np.ascontiguousarray(arr, dtype=np.float32)
+            a = np.asarray(arr, dtype=np.float32, order="C")   # (not ascontiguousarray: a scalar weight keeps shape ())
             if tuple(a.shape) != self._specs[name]:
                 raise ValueError(f"weight {name!r}: expected shape {self._specs[name]}, got {tuple(a.shape)}")
             shape = (C.c_int64 * a.ndim)(*a.shape)
@@ -1610,6 +1610,92 @@ class ATSViT(_EngineModel):
     call = __call__
 
 
+def _spt_patch_size(patch_size):
+    """SPT's Rearrange gets p1 = p2 = patch_size as given (vit_for_small_dataset.py:147): a tuple passes pair() and then fails
+    inside einops in the reference, so it is refused here when the model is built."""
+    if isinstance(patch_size, tuple):
+        raise ValueError("the small-dataset ViT's SPT takes one integer patch_size (its Rearrange uses it for both sides); "
+                         f"got {patch_size!r}")
+    return int(patch_size)
+
+
+class SmallDatasetViT(_EngineModel):
+    """vit_for_small_dataset.py:159-215 (`vit_for_small_dataset.ViT`, "Vision Transformer for Small Datasets"): ViT with shifted
+    patch tokens (SPT: the image and its four one-pixel shifts, LayerNorm, Dense) and locality self-attention (LSA: each token's
+    own key masked, the scale exp(temperature) a learned scalar per layer).  to_out is always present.  Weights are ViT's names
+    (SURVEY.md App. B) plus patch_norm.gamma / .beta, patch.kernel / .bias over p^2 * 15 inputs and layers.L.temperature, a
+    scalar.  Runs as a whole forward only.  Images must have 3 channels."""
+    _kind = "small_dataset_vit"
+
+    def __init__(self, image_size, patch_size, num_classes, dim, depth, heads, mlp_dim, pool='cls', dim_head=64, dropout=0.0,
+                 emb_dropout=0.0, *, precision="bf16", device=0, seed=None):
+        image_height, image_width = pair(image_size)
+        patch_height, patch_width = pair(patch_size)
+        assert image_height % patch_height == 0 and image_width % patch_width == 0, 'Image dimensions must be divisible by the patch size.'
+        assert pool in {'cls', 'mean'}, 'pool type must be either cls (cls token) or mean (mean pooling)'
+        p = _spt_patch_size(patch_size)
+        self.num_classes, self.pool, self.dim, self.dim_head = num_classes, pool, dim, dim_head
+        self._dropout_rates = (dropout, emb_dropout)
+        self._create(precision, device, image_h=image_height, image_w=image_width, patch_h=p, patch_w=p, num_classes=num_classes,
+                     dim=dim, depth=depth, heads=heads, dim_head=dim_head, mlp_dim=mlp_dim, pool=0 if pool == 'cls' else 1)
+        self.init_weights(seed)
+
+    def init_weights(self, seed=None):
+        """As the base class, with every layer's temperature at its initial value log(dim_head^-0.5) in float32 (:94)."""
+        super().init_weights(seed)
+        t = np.float32(np.log(np.float32(self.dim_head ** -0.5)))
+        self.set_weights_dict({n: np.array(t, np.float32) for n in self._specs if n.endswith(".temperature")})
+
+
+class SPT:
+    """vit_for_small_dataset.py:142-157 on its own: `SPT(dim, patch_size)(img)` -> tokens [b, (H / p) (W / p), dim] of NHWC images
+    with 3 channels.  Weights: patch_norm.gamma / .beta [p^2 * 15] and patch.kernel [p^2 * 15, dim] / .bias (Keras' initial values
+    at construction; set_weights_dict replaces them).  Runs the engine's SPT kernel and the LayerNorm-folded GEMM (vb_op_spt)."""
+
+    def __init__(self, dim, patch_size, *, precision="bf16", seed=None):
+        self.dim, self.patch_size, self.precision = int(dim), _spt_patch_size(patch_size), precision
+        k = self.patch_size ** 2 * 15
+        lim = np.sqrt(6.0 / (k + self.dim))
+        rng = np.random.default_rng(seed)
+        self._specs = collections.OrderedDict([("patch_norm.gamma", (k,)), ("patch_norm.beta", (k,)), ("patch.kernel", (k, self.dim)),
+                                               ("patch.bias", (self.dim,))])
+        self._weights = collections.OrderedDict([
+            ("patch_norm.gamma", np.ones(k, np.float32)), ("patch_norm.beta", np.zeros(k, np.float32)),
+            ("patch.kernel", rng.uniform(-lim, lim, size=(k, self.dim)).astype(np.float32)), ("patch.bias", np.zeros(self.dim, np.float32))])
+
+    def weight_specs(self):
+        return collections.OrderedDict(self._specs)
+
+    def set_weights_dict(self, weights):
+        for name, arr in weights.items():
+            if name not in self._specs:
+                raise KeyError(f"SPT has no weight named {name!r}")
+            a = np.ascontiguousarray(arr, dtype=np.float32)
+            if tuple(a.shape) != self._specs[name]:
+                raise ValueError(f"weight {name!r}: expected shape {self._specs[name]}, got {tuple(a.shape)}")
+            self._weights[name] = a
+
+    def get_weights_dict(self):
+        return collections.OrderedDict((k, v.copy()) for k, v in self._weights.items())
+
+    def __call__(self, x, training=True):
+        img = np.ascontiguousarray(x, dtype=np.float32)
+        if img.ndim != 4 or img.shape[3] != 3:
+            raise ValueError("img must be NHWC float [b, H, W, 3]")
+        if img.shape[1] % self.patch_size or img.shape[2] % self.patch_size:
+            raise ValueError("Image dimensions must be divisible by the patch size.")
+        w = self._weights
+        out = _lib.op_spt(img, self.patch_size, w["patch_norm.gamma"], w["patch_norm.beta"], w["patch.kernel"], w["patch.bias"],
+                          precision=self.precision)
+        return _as_tensor(out[:, 1:])
+
+    call = __call__
+
+
+SMALL_DATASET_VIT_CTOR_KEYS = ("image_size", "patch_size", "num_classes", "dim", "depth", "heads", "mlp_dim", "pool", "dim_head",
+                               "dropout", "emb_dropout")
+
+
 ATS_CTOR_KEYS = ("image_size", "patch_size", "num_classes", "dim", "depth", "max_tokens_per_depth", "heads", "mlp_dim", "dim_head",
                  "dropout", "emb_dropout")
 
@@ -1620,6 +1706,9 @@ REGIONVIT_CTOR_KEYS = ("dim", "depth", "window_size", "num_classes", "tokenize_l
 
 def from_config(cfg: dict, precision="bf16", device=0, seed=None):
     """Build a model from an oracle-style config dict (kind + reference kwargs)."""
+    if cfg["kind"] == "small_dataset_vit":
+        return SmallDatasetViT(**{k: v for k, v in cfg.items() if k in SMALL_DATASET_VIT_CTOR_KEYS}, precision=precision, device=device,
+                               seed=seed)
     if cfg["kind"] == "ats_vit":
         return ATSViT(**{k: v for k, v in cfg.items() if k in ATS_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "regionvit":
