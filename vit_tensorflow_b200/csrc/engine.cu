@@ -973,10 +973,15 @@ struct vb_handle {
   bool has(const std::string& name) const { return windex.count(name) != 0; }
 
   Linear make_linear(const std::string& n, int K, int N, bool bias = true, const Norm* fold = nullptr, int ldw_min = 0) {
+    return pack_linear(W(n + ".kernel"), bias ? W(n + ".bias") : nullptr, K, N, std::max(round_up(K, 8), ldw_min), fold);
+  }
+  // The Dense W [K, N] (device, Keras layout) + bias (may be null); the bf16 engine packs W K-major at pitch ldw and folds the
+  // LayerNorm `fold` into it when given
+  Linear pack_linear(const float* Wk, const float* bias, int K, int N, int ldw, const Norm* fold) {
     Linear L;
-    L.W = W(n + ".kernel");
-    L.bias = bias ? W(n + ".bias") : nullptr;
-    L.K = K; L.N = N; L.ldw = round_up(K, 8) > ldw_min ? round_up(K, 8) : ldw_min;
+    L.W = Wk;
+    L.bias = bias;
+    L.K = K; L.N = N; L.ldw = ldw;
     if (bf16()) {
       owned.emplace_back(new DevMem());
       owned.back()->ensure(static_cast<size_t>(N) * L.ldw * sizeof(__nv_bfloat16));
@@ -1627,7 +1632,8 @@ struct vb_handle {
         b.to_out = linear_from_host(key + "to_out", Wp, pad_n(bo, dpo), HD, dpo);
       }
       b.scale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(dk)));
-      b.pos = upload_owned(levit_pos_table(host_weight(a + "pos_bias.embeddings"), p.fmap * p.fmap, H, dk));
+      b.pos = upload_owned(levit_pos_table(host_weight(a + "pos_bias.embeddings"), p.fmap * p.fmap, H,
+                                             std::sqrt(static_cast<double>(dk))));
       const int hidden = p.dim_out * p.mult, hp = channel_width(hidden);
       b.fc1 = padded_dense(key + "fc1", p.pre + "1.net.0", p.dim_out, hidden, dpo, hp);
       b.fc2 = padded_dense(key + "fc2", p.pre + "1.net.3", hidden, p.dim_out, hp, dpo);
@@ -1637,36 +1643,23 @@ struct vb_handle {
     head = make_linear_f32("mlp_head", dl, cfg.num_classes);
     if (lv.num_distill_classes > 0) lv_distill = make_linear_f32("distill_head", dl, lv.num_distill_classes);
   }
-  // [heads][fmap^2] = embeddings[e, h] / scale with scale = dim_key^-0.5 (levit.py:117): the table the attention kernels add
-  static std::vector<double> levit_pos_table(const std::vector<double>& emb, int f2, int heads, int dim_key) {
+  // [heads][fmap^2] = embeddings[e, h] * inv_scale, the inverse of the softmax scale dim_key^-0.5 (levit.py:117): the table the
+  // attention kernels add
+  static std::vector<double> levit_pos_table(const std::vector<double>& emb, int f2, int heads, double inv_scale) {
     std::vector<double> t(static_cast<size_t>(heads) * f2);
-    const double inv_scale = std::sqrt(static_cast<double>(dim_key));
     for (int h = 0; h < heads; ++h)
       for (int e = 0; e < f2; ++e) t[static_cast<size_t>(h) * f2 + e] = emb[static_cast<size_t>(e) * heads + h] * inv_scale;
     return t;
   }
 
-  // vit_for_small_dataset.ViT (:159-195).  SPT's LayerNorm over K = p^2 * 5 C (eps 1e-3) and Dense: the bf16 engine zero-pads K
-  // to Kp = round_up(K, 64) and folds the LayerNorm into the wgmma GEMM (dim % 64 == 0); the fp32 engine keeps K and runs the
-  // LayerNorm kernel.  Either way the Dense yields beta . W + bias on the all-zero cls row, so that is the term the embedding
-  // residual takes off (res_bias).  The layers are ViT's with LSA: the diagonal mask and exp(temperature) as the softmax scale.
+  // vit_for_small_dataset.ViT (:159-195): SPT (set_spt_patch), then ViT's layers with LSA: the diagonal mask and exp(temperature)
+  // as the softmax scale.
   void finalize_small_dataset_vit() {
     const vb_config& c = cfg;
     const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w), K = c.patch_h * c.patch_w * 5 * c.channels;
-    const int Kp = bf16() ? round_up(K, 64) : K;
-    const bool fold = bf16() && c.dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr;
     embed = EmbedW();
-    spt_norm = padded_norm("patch_norm", K, Kp, ".gamma", ".beta");
-    embed.patch = padded_dense("spt.patch", "patch", K, c.dim, Kp, c.dim, fold ? &spt_norm : nullptr, 1e-3f);
-    if (fold) {
-      embed.res_bias = embed.patch.ln_c2;
-    } else {
-      const std::vector<double> beta = host_weight("patch_norm.beta"), Wk = host_weight("patch.kernel");
-      std::vector<double> c2 = host_weight("patch.bias");
-      for (int k = 0; k < K; ++k)
-        for (int n = 0; n < c.dim; ++n) c2[n] += beta[k] * Wk[static_cast<size_t>(k) * c.dim + n];
-      embed.res_bias = upload_owned(c2);
-    }
+    set_spt_patch(host_weight("patch_norm.gamma"), host_weight("patch_norm.beta"), host_weight("patch.kernel"), host_weight("patch.bias"), K,
+                  c.dim);
     embed.pos = W("pos_embedding");
     embed.cls = W("cls_token");
     embed.dim = c.dim; embed.n_pos = np + 1;
@@ -1678,6 +1671,25 @@ struct vb_handle {
     }
     head_norm = make_norm("head_norm", c.dim);
     head = make_linear_f32("head", c.dim, c.num_classes);
+  }
+  // SPT's LayerNorm gamma / beta [K] (eps 1e-3) and patch Dense W [K, dim] + bias as spt_tokens runs them: the bf16 engine zero-pads
+  // K to Kp = round_up(K, 64) and folds the LayerNorm into the wgmma GEMM (dim % 64 == 0, unless VB_NO_LN_FOLD is set); otherwise
+  // the LayerNorm kernel runs first.  Either way the Dense yields beta . W + bias on the all-zero cls row, so that is the term the
+  // embedding residual takes off (res_bias).
+  void set_spt_patch(const std::vector<double>& gamma, const std::vector<double>& beta, const std::vector<double>& Wk,
+                     std::vector<double> bias, int K, int dim) {
+    const int Kp = bf16() ? round_up(K, 64) : K;
+    const bool fold = bf16() && dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr;
+    spt_norm = Norm{upload_owned(pad_n(gamma, Kp)), upload_owned(pad_n(beta, Kp)), K};
+    embed.patch = linear_from_host("spt.patch", pad_kn(Wk, K, dim, Kp, dim), bias, Kp, dim, fold ? &spt_norm : nullptr);
+    if (fold) {
+      embed.patch.ln_d = K; embed.patch.ln_eps = 1e-3f;
+      embed.res_bias = embed.patch.ln_c2;
+    } else {
+      for (int k = 0; k < K; ++k)
+        for (int n = 0; n < dim; ++n) bias[n] += beta[k] * Wk[static_cast<size_t>(k) * dim + n];
+      embed.res_bias = upload_owned(bias);
+    }
   }
 
   Linear make_linear_f32(const std::string& n, int K, int N) {  // classifier head always runs in fp32
@@ -1940,7 +1952,10 @@ struct vb_handle {
       T* QKV = arena.get<T>(static_cast<size_t>(M) * 3 * inner);
       Epi e = eq; e.bias = l.to_qkv.ln_c2;
       linear<T>(A, dim, M, l.to_qkv, QKV, 3 * inner, e, s);
-      if (nk_img != nullptr || l.lsa) attention_masked_dispatch<T>(QKV, 3 * inner, O, inner, B, rows, l, s, nk_img);
+      if (nk_img != nullptr || l.lsa)
+        attention_masked_dispatch<T>(QKV, 3 * inner, O, inner, B, rows, l.heads, l.dim_head, l.dh_model,
+                                     l.lsa ? l.lsa_scale : 1.0f / sqrtf(static_cast<float>(l.dh_model)),
+                                     l.lsa ? ATTN_MASK_DIAG : ATTN_MASK_KEYS, s, nk_img);
       else attention<T>(QKV, 3 * inner, QKV + inner, 3 * inner, QKV + 2 * inner, 3 * inner, O, inner, B, rows, rows, l, s);
       qkv = QKV;
     } else {
@@ -1963,26 +1978,21 @@ struct vb_handle {
     }
     return qkv;
   }
-  // Plain attention over the fused q|k|v rows with masked keys: image b's keys >= nk_img[b] (ATS-ViT), or the diagonal with the
-  // scale exp(temperature) for an LSA layer.  The flash kernels at dh 64 (bf16), else the materialised-scores path with the mask in
-  // its softmax.
+  // Plain attention over the fused q|k|v rows of `heads` heads of width dh with masked keys: image b's keys >= nk_img[b]
+  // (ATTN_MASK_KEYS, ATS-ViT), or the diagonal (ATTN_MASK_DIAG, an LSA layer, with the scale exp(temperature)).  The flash kernels
+  // at dh 64 (bf16), else the materialised-scores path with the mask in its softmax, which needs the model's own head width dh_model.
   template <typename T>
-  void attention_masked_dispatch(const T* qkv, int ld, T* out, int ldo, int B, int n, const LayerW& l, cudaStream_t s, const int* nk_img) {
-    const int heads = l.heads, dh = l.dim_head, HD = heads * dh;
-    const float scale = l.lsa ? l.lsa_scale : 1.0f / sqrtf(static_cast<float>(l.dh_model));
-    const int mask = l.lsa ? ATTN_MASK_DIAG : ATTN_MASK_KEYS;
-    VB_CHECK(!l.lsa || n >= 2, "locality self-attention needs at least 2 tokens (every row keeps a key besides its own)");
+  void attention_masked_dispatch(const T* qkv, int ld, T* out, int ldo, int B, int n, int heads, int dh, int dh_model, float scale, int mask,
+                                 cudaStream_t s, const int* nk_img) {
+    const int HD = heads * dh;
+    VB_CHECK(mask != ATTN_MASK_DIAG || n >= 2, "locality self-attention needs at least 2 tokens (every row keeps a key besides its own)");
     ProfScope ps(this, PROF_ATTN, 4.0 * B * heads * n * n * dh, static_cast<double>(sizeof(T)) * B * heads * dh * 4.0 * n, s);
-    if (masked_flash(qkv, ld, out, ldo, B, n, heads, dh, s, scale, nk_img, mask)) return;
-    VB_CHECK(dh == l.dh_model, "internal: a head-padded layer must run on the fused attention kernel");
+    if constexpr (std::is_same<T, __nv_bfloat16>::value) {
+      if (attention_masked(qkv, ld, qkv + HD, ld, qkv + 2 * HD, ld, out, ldo, B, n, n, heads, dh, s, scale, nk_img, mask)) return;
+    }
+    VB_CHECK(dh == dh_model, "internal: a head-padded layer must run on the fused attention kernel");
     float* S = arena.get<float>(static_cast<size_t>(B) * heads * n * n);
     attention_generic_masked<T>(qkv, ld, qkv + HD, ld, qkv + 2 * HD, ld, out, ldo, S, B, n, n, heads, dh, s, scale, nk_img, mask);
-  }
-  static bool masked_flash(const float*, int, float*, int, int, int, int, int, cudaStream_t, float, const int*, int) { return false; }
-  static bool masked_flash(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* out, int ldo, int B, int n, int heads, int dh, cudaStream_t s,
-                           float scale, const int* nk_img, int mask) {
-    const int HD = heads * dh;
-    return attention_masked(qkv, ld, qkv + HD, ld, qkv + 2 * HD, ld, out, ldo, B, n, n, heads, dh, s, scale, nk_img, mask);
   }
 
   // ATS-ViT's forward (ats_vit.py:300-318, Transformer.call :236-258) in the compact row layout of ats.cu: image b's rows at the
@@ -2464,7 +2474,7 @@ struct vb_handle {
       T* QKV = arena.get<T>(static_cast<size_t>(Mk) * 3 * HD);
       Epi e; e.bias = b.qkv.bias;
       linear<T>(X, b.dp, Mk, b.qkv, QKV, 3 * HD, e, s);
-      attention_bias<T>(QKV, 3 * HD, QKV + HD, 3 * HD, QKV + 2 * HD, 3 * HD, O, HD, B, nq, f2, b, pb, s);
+      attention_bias<T>(QKV, 3 * HD, QKV + HD, 3 * HD, QKV + 2 * HD, 3 * HD, O, HD, B, nq, f2, b.heads, b.dh, b.scale, pb, s);
     } else {                                                            // queries of the even pixels (1x1 conv, stride 2, VALID)
       T* Xq = arena.get<T>(static_cast<size_t>(Mq) * b.dp);
       {
@@ -2477,7 +2487,7 @@ struct vb_handle {
       linear<T>(Xq, b.dp, Mq, b.q, Q, HD, eq, s);
       Epi ek; ek.bias = b.qkv.bias;
       linear<T>(X, b.dp, Mk, b.qkv, KV, 2 * HD, ek, s);
-      attention_bias<T>(Q, HD, KV, 2 * HD, KV + HD, 2 * HD, O, HD, B, nq, f2, b, pb, s);
+      attention_bias<T>(Q, HD, KV, 2 * HD, KV + HD, 2 * HD, O, HD, B, nq, f2, b.heads, b.dh, b.scale, pb, s);
     }
     T* Y = b.residual ? X : arena.get<T>(static_cast<size_t>(Mq) * b.dp_out);
     Epi eo; eo.bias = b.to_out.bias;
@@ -2491,13 +2501,13 @@ struct vb_handle {
     return Y;
   }
   template <typename T>
-  void attention_bias(const T* q, int ldq, const T* k, int ldk, const T* v, int ldv, T* out, int ldo, int B, int nq, int nk,
-                      const LevitBlockW& b, const PosBias& pb, cudaStream_t s) {
-    ProfScope ps(this, PROF_ATTN, 4.0 * B * b.heads * nq * nk * b.dh, static_cast<double>(sizeof(T)) * B * b.heads * b.dh * (2.0 * nq + 2.0 * nk), s);
-    if (attention_fast<T>(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, b.heads, b.dh, 0, nullptr, nullptr, nullptr, nullptr, s, b.scale, &pb))
+  void attention_bias(const T* q, int ldq, const T* k, int ldk, const T* v, int ldv, T* out, int ldo, int B, int nq, int nk, int heads,
+                      int dh, float scale, const PosBias& pb, cudaStream_t s) {
+    ProfScope ps(this, PROF_ATTN, 4.0 * B * heads * nq * nk * dh, static_cast<double>(sizeof(T)) * B * heads * dh * (2.0 * nq + 2.0 * nk), s);
+    if (attention_fast<T>(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, heads, dh, 0, nullptr, nullptr, nullptr, nullptr, s, scale, &pb))
       return;
-    float* S = arena.get<float>(static_cast<size_t>(B) * b.heads * nq * ((nk + 15) & ~15));
-    attention_generic<T>(q, ldq, k, ldk, v, ldv, out, ldo, S, B, nq, nk, b.heads, b.dh, 0, nullptr, nullptr, nullptr, nullptr, s, b.scale, &pb);
+    float* S = arena.get<float>(static_cast<size_t>(B) * heads * nq * ((nk + 15) & ~15));
+    attention_generic<T>(q, ldq, k, ldk, v, ldv, out, ldo, S, B, nq, nk, heads, dh, 0, nullptr, nullptr, nullptr, nullptr, s, scale, &pb);
   }
 
   // CvT.call (cvt.py:182-202): per stage, Conv2D (SAME, bias) -> LayerNorm -> blocks; then GlobalAvgPool2D -> Dense.  Token rows
@@ -2534,13 +2544,7 @@ struct vb_handle {
     T* Qd = arena.get<T>(static_cast<size_t>(M) * dp);
     T* KVd = arena.get<T>(static_cast<size_t>(Mk) * dp);
     const PreNorm<T> p = prenorm<T>(X, M, b.dim, dp, stats, 1e-5f, s);
-    const T* a = p.norm(b.attn_norm);                                   // PreNorm of the attention (cvt.py:53)
-    {
-      ProfScope ps(this, PROF_OTHER, 2.0 * b.k * b.k * b.dim * (static_cast<double>(M) + Mk),
-                   static_cast<double>(sizeof(T)) * dp * (2.0 * M + Mk) + (stats ? 8.0 * M * (dp / 64) : 0.0), s);
-      dwconv_qkv<T>(a, dp, p.Y ? nullptr : stats, b.attn_norm.gamma, b.attn_norm.beta, b.dim, 1e-5f, b.wq, b.bq, Qd, dp, b.wkv, b.bkv,
-                    KVd, dp, B, H, Wd, dp, b.k, st, s);
-    }
+    cvt_dwconv<T>(p, B, H, Wd, b, Qd, KVd, s);
     T* Q = arena.get<T>(static_cast<size_t>(M) * HD);
     T* KV = arena.get<T>(static_cast<size_t>(Mk) * 2 * HD);
     linear<T>(Qd, dp, M, b.pw_q, Q, HD, Epi(), s);                      // cvt.py:86 (no bias)
@@ -2549,6 +2553,17 @@ struct vb_handle {
     attention_dispatch<T>(Q, HD, KV, 2 * HD, KV + HD, 2 * HD, O, HD, B, H * Wd, Ho * Wo, b.heads, 64, 0, nullptr, nullptr, nullptr, nullptr, s);
     p.residual(O, HD, b.to_out);
     p.mlp(b.ff);
+  }
+  // The attention's PreNorm (cvt.py:53) and the depthwise convolutions with their BatchNormalizations (cvt.py:80-85) of a CvT
+  // layer over p's rows, the B x H x Wd map: Qd [B H Wd, dp] at stride 1, KVd [B ceil(H / s) ceil(Wd / s), dp] at kv_stride
+  template <typename T>
+  void cvt_dwconv(const PreNorm<T>& p, int B, int H, int Wd, const CvtBlockW& b, T* Qd, T* KVd, cudaStream_t s) {
+    const int dp = b.dp, st = b.kv_stride, M = B * H * Wd, Mk = B * ((H + st - 1) / st) * ((Wd + st - 1) / st);
+    const T* a = p.norm(b.attn_norm);
+    ProfScope ps(this, PROF_OTHER, 2.0 * b.k * b.k * b.dim * (static_cast<double>(M) + Mk),
+                 static_cast<double>(sizeof(T)) * dp * (2.0 * M + Mk) + (p.stats ? 8.0 * M * (dp / 64) : 0.0), s);
+    dwconv_qkv<T>(a, dp, p.Y ? nullptr : p.stats, b.attn_norm.gamma, b.attn_norm.beta, b.dim, 1e-5f, b.wq, b.bq, Qd, dp, b.wkv, b.bkv, KVd, dp,
+                  B, H, Wd, dp, b.k, st, s);
   }
 
   // TwinsSVT.call (twins_svt.py:266-268): per stage, PatchEmbedding -> Transformer(1) -> PEG -> Transformer(depth); then
@@ -2742,21 +2757,8 @@ struct vb_handle {
       const int oh = (mh + 1) / 2, ow = (mw + 1) / 2, Mo = B * oh * ow;
       T* Xn = arena.get<T>(static_cast<size_t>(Mo) * V.dp_out);
       float* nstats = row_stats(Mo, V.dp_out);
-      const T* src = Y;
-      NestPoolLn ln;
-      if (bf16()) {
-        ln.stats = ystats; ln.parts = V.dp_out / 64; ln.d = V.dim_out; ln.eps = 1e-5f; ln.gamma = V.agg_norm.gamma; ln.beta = V.agg_norm.beta;
-      } else {
-        T* Z = arena.get<T>(static_cast<size_t>(M) * V.dp_out);
-        ProfScope ps(this, PROF_LN, 8.0 * M * V.dim_out, 2.0 * sizeof(T) * M * V.dp_out, s);
-        layernorm<T>(Y, V.dp_out, V.agg_norm.gamma, V.agg_norm.beta, Z, V.dp_out, M, V.dim_out, s, V.dp_out, 1e-5f);
-        src = Z;
-      }
-      {
-        ProfScope ps(this, PROF_OTHER, 9.0 * Mo * V.dim_out, static_cast<double>(sizeof(T)) * (static_cast<double>(M) + Mo) * V.dp_out, s);
-        nest_pool<T>(src, V.dp_out, bf16() ? &ln : nullptr, B, mh, mw, V.dim_out, true, next ? next->pos : nullptr, next ? oh / next->bs : 1,
-                     next ? ow / next->bs : 1, Xn, V.dp_out, nstats, s);
-      }
+      nest_aggregate_tail<T>(Y, ystats, B, mh, mw, V.dim_out, V.dp_out, V.agg_norm, next ? next->pos : nullptr, next ? oh / next->bs : 1,
+                             next ? ow / next->bs : 1, Xn, nstats, s);
       X = Xn; stats = nstats; mh = oh; mw = ow; d = V.dim_out; dp = V.dp_out;
     }
     if (!nest_levels.empty() && !nest_levels.back().aggregate) { d = nest_levels.back().dim; dp = nest_levels.back().dp; }
@@ -2770,6 +2772,26 @@ struct vb_handle {
       pool_layernorm<T>(Y, mh * mw, dp, nullptr, nullptr, z, B, d, 1, s);
     }
     dense_head(z, d, head, B, logits, s);
+  }
+  // Aggregate's tail (nest.py:117-123) on Y [B h w, dp], the convolution's output of true width d: the LayerNorm `norm` (bf16: applied
+  // on load from Y's row statistics ystats), then MaxPool2D(3, 2, SAME) with the next level's position add (pos, may be null, over
+  // pbh x pbw blocks) -> Xn [B ceil(h / 2) ceil(w / 2), dp] and, bf16, its row statistics nstats
+  template <typename T>
+  void nest_aggregate_tail(const T* Y, const float* ystats, int B, int h, int w, int d, int dp, const Norm& norm, const float* pos, int pbh,
+                           int pbw, T* Xn, float* nstats, cudaStream_t s) {
+    const int M = B * h * w, Mo = B * ((h + 1) / 2) * ((w + 1) / 2);
+    const T* src = Y;
+    NestPoolLn ln;
+    if (bf16()) {
+      ln.stats = ystats; ln.parts = dp / 64; ln.d = d; ln.eps = 1e-5f; ln.gamma = norm.gamma; ln.beta = norm.beta;
+    } else {
+      T* Z = arena.get<T>(static_cast<size_t>(M) * dp);
+      ProfScope ps(this, PROF_LN, 8.0 * M * d, 2.0 * sizeof(T) * M * dp, s);
+      layernorm<T>(Y, dp, norm.gamma, norm.beta, Z, dp, M, d, s, dp, 1e-5f);
+      src = Z;
+    }
+    ProfScope ps(this, PROF_OTHER, 9.0 * Mo * d, static_cast<double>(sizeof(T)) * (static_cast<double>(M) + Mo) * dp, s);
+    nest_pool<T>(src, dp, bf16() ? &ln : nullptr, B, h, w, d, true, pos, pbh, pbw, Xn, dp, nstats, s);
   }
   // One Transformer block (nest.py:144-146) in place on X [B*H*W, dp]: attention within the level's bs x bs blocks per map, then
   // the MLP.  bf16: the LayerNorms folded into q|k|v and fc1 (from `stats`); fp32: separate LayerNorms.
@@ -2788,25 +2810,31 @@ struct vb_handle {
     p.mlp(l.ff);                                                      // MLP nest.py:61-75
   }
   // NesT's block attention: win.count blocks of p x width() tokens of fused q|k|v rows [.., ld], the output rows written to out
-  // [.., ldo] pixel-major.  The windowed flash kernel where it serves (bf16, dh 32 or 64); otherwise the rows permuted to
-  // block-major order, the materialised-scores path, and the output rows permuted back.
+  // [.., ldo] pixel-major.  The windowed flash kernel where it serves (bf16, dh 32 or 64), else window_attention_generic.
   template <typename T>
   void block_attention(const T* qkv, int ld, T* out, int ldo, int heads, int dh, const Window& win, cudaStream_t s) {
-    const int n = win.p * win.width(), HD = heads * dh;
-    const long long B = win.count, rows = B * n;
-    const double fl = 4.0 * B * heads * n * n * dh, by = static_cast<double>(sizeof(T)) * B * heads * dh * 4.0 * n;
+    const int n = win.p * win.width();
     {
-      ProfScope ps(this, PROF_ATTN, fl, by, s);
+      ProfScope ps(this, PROF_ATTN, 4.0 * win.count * heads * n * n * dh, static_cast<double>(sizeof(T)) * win.count * heads * dh * 4.0 * n, s);
       if (block_attention_fast(qkv, ld, out, ldo, heads, dh, s, win)) return;
     }
+    window_attention_generic<T>(qkv, ld, out, ldo, win.count, n, heads, dh, win, nullptr, s);
+  }
+  // Windowed attention off the flash kernel: B windows of n tokens of fused q|k|v rows [.., ld] (win's layout, with the window
+  // bias pb when given) permuted to window-major order, the materialised-scores path, the output rows permuted back to out [.., ldo]
+  template <typename T>
+  void window_attention_generic(const T* qkv, int ld, T* out, int ldo, int B, int n, int heads, int dh, const Window& win, const PosBias* pb,
+                                cudaStream_t s) {
+    const int HD = heads * dh;
+    const long long rows = static_cast<long long>(B) * n;
     T* qkvw = arena.get<T>(static_cast<size_t>(rows) * 3 * HD);
     T* ow = arena.get<T>(static_cast<size_t>(rows) * HD);
     { ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * rows * 3 * HD, s); window_rows<T>(qkv, ld, qkvw, 3 * HD, 3 * HD, win, rows, true, s); }
     {
-      ProfScope ps(this, PROF_ATTN, fl, by, s);
+      ProfScope ps(this, PROF_ATTN, 4.0 * B * heads * n * n * dh, static_cast<double>(sizeof(T)) * B * heads * dh * 4.0 * n, s);
       float* S = arena.get<float>(static_cast<size_t>(B) * heads * n * ((n + 15) & ~15));
-      attention_generic<T>(qkvw, 3 * HD, qkvw + HD, 3 * HD, qkvw + 2 * HD, 3 * HD, ow, HD, S, static_cast<int>(B), n, n, heads, dh, 0, nullptr,
-                           nullptr, nullptr, nullptr, s);
+      attention_generic<T>(qkvw, 3 * HD, qkvw + HD, 3 * HD, qkvw + 2 * HD, 3 * HD, ow, HD, S, B, n, n, heads, dh, 0, nullptr, nullptr, nullptr,
+                           nullptr, s, 0.f, pb);
     }
     { ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * rows * HD, s); window_rows<T>(ow, HD, out, ldo, HD, win, rows, false, s); }
   }
@@ -3210,31 +3238,21 @@ void vb_handle::attention_dispatch(const T* q, int ldq, const T* k, int ldk, con
   // tokens in the map's own rows
   if (win != nullptr) {
     const int HD = heads * dh;
-    VB_CHECK(k == q + HD && v == q + 2 * HD && ldk == ldq && ldv == ldq && variant == 0, "internal: windowed attention reads fused q|k|v rows");
-    const double fl = 4.0 * B * heads * nq * nk * dh, by = static_cast<double>(sizeof(T)) * B * heads * dh * (2.0 * nq + 2.0 * nk);
+    VB_CHECK(k == q + HD && v == q + 2 * HD && ldk == ldq && ldv == ldq && nq == nk && variant == 0,
+             "internal: windowed attention reads fused q|k|v rows");
     {
-      ProfScope ps(this, PROF_ATTN, fl, by, s);
+      ProfScope ps(this, PROF_ATTN, 4.0 * B * heads * nq * nk * dh, static_cast<double>(sizeof(T)) * B * heads * dh * (2.0 * nq + 2.0 * nk), s);
       if (attention_fast<T>(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, heads, dh, 0, nullptr, nullptr, nullptr, nullptr, s, 0.f, pb, win))
         return;
     }
-    // off the flash kernel: the rows permuted to window-major order, the materialised-scores path, the output rows permuted back
-    const long long rows = static_cast<long long>(B) * nq;
-    T* qkvw = arena.get<T>(static_cast<size_t>(rows) * 3 * HD);
-    T* ow = arena.get<T>(static_cast<size_t>(rows) * HD);
-    { ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * rows * 3 * HD, s); window_rows<T>(q, ldq, qkvw, 3 * HD, 3 * HD, *win, rows, true, s); }
-    {
-      ProfScope ps(this, PROF_ATTN, fl, by, s);
-      float* S = arena.get<float>(static_cast<size_t>(B) * heads * nq * ((nk + 15) & ~15));
-      attention_generic<T>(qkvw, 3 * HD, qkvw + HD, 3 * HD, qkvw + 2 * HD, 3 * HD, ow, HD, S, B, nq, nk, heads, dh, 0, nullptr, nullptr, nullptr,
-                           nullptr, s, 0.f, pb);
-    }
-    { ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * rows * HD, s); window_rows<T>(ow, HD, out, ldo, HD, *win, rows, false, s); }
+    window_attention_generic<T>(q, ldq, out, ldo, B, nq, heads, dh, *win, pb, s);
     return;
   }
   ProfScope ps(this, PROF_ATTN, 4.0 * B * heads * nq * nk * dh + (variant == 1 ? 2.0 : variant == 2 ? 4.0 : 0.0) * B * nq * nk * heads * heads,
                static_cast<double>(sizeof(T)) * B * heads * dh * (2.0 * nq + 2.0 * nk), s);
   if (attention_fast<T>(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, heads, dh, variant, mix_a, mix_b, g, b, s, scale)) return;
-  VB_CHECK(scale <= 0.f, "internal: a head-padded layer must run on the fused attention kernel");
+  // a head-padded layer passes its model's scale, which only the fused kernels take
+  VB_CHECK(scale <= 0.f, "an explicit softmax scale needs the fused attention kernels (bf16 at a head width they take)");
   float* S = arena.get<float>(static_cast<size_t>(B) * heads * nq * ((nk + 15) & ~15));   // row pitch padded for the bf16-P path
   attention_generic<T>(q, ldq, k, ldk, v, ldv, out, ldo, S, B, nq, nk, heads, dh, variant, mix_a, mix_b, g, b, s);
 }
@@ -3454,6 +3472,20 @@ void require_gpu() {
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
   VB_CHECK(e == cudaSuccess && ndev > 0, "no CUDA device available -- libvitb200 has no CPU fallback");
+}
+// f(h, T()) with T the element type of `precision` (float for fp32, __nv_bfloat16 otherwise) and h a scratch handle of that
+// precision, on which an op entry runs the forward's own members: no weights, profiling off, its arena the entry's scratch.  A
+// timed iteration resets the arena first, so the scratch pointers, and the GEMM plans cached on them, stay the same.
+template <typename F>
+void with_precision(int32_t precision, F&& f) {
+  vb_handle h{};
+  if (precision == VB_PRECISION_FP32) {
+    h.cfg.precision = VB_PRECISION_FP32;
+    f(h, float());
+  } else {
+    h.cfg.precision = VB_PRECISION_BF16;
+    f(h, __nv_bfloat16());
+  }
 }
 template <typename T>
 T* upload(DevMem& m, const float* host, size_t count) {
@@ -3705,26 +3737,20 @@ int vb_op_masked_attention(int32_t precision, const float* qkv, int32_t ld, int3
     const int HD = heads * dh;
     VB_CHECK(qkv && nk_img && out && B > 0 && n > 0 && heads > 0 && dh > 0 && ld >= 3 * HD && ldo >= HD, "vb_op_masked_attention: bad arguments");
     for (int b = 0; b < B; ++b) VB_CHECK(nk_img[b] >= 1 && nk_img[b] <= n, "vb_op_masked_attention: nk_img[b] must be in [1, n]");
-    DevMem dX, dO, dN, dS;
+    DevMem dX, dO, dN;
     dN.ensure(static_cast<size_t>(B) * sizeof(int));
     VB_CUDA(cudaMemcpy(dN.p, nk_img, static_cast<size_t>(B) * sizeof(int), cudaMemcpyHostToDevice));
     const int* nk_d = static_cast<const int*>(dN.p);
-    const float scale = 1.0f / sqrtf(static_cast<float>(dh));
-    auto run = [&](auto tag) {
+    with_precision(precision, [&](vb_handle& h, auto tag) {
       using T = decltype(tag);
       const T* x_d = upload<T>(dX, qkv, static_cast<size_t>(B) * n * ld);
       T* o_d = upload<T>(dO, out, static_cast<size_t>(B) * n * ldo);
-      // vb_handle::attention_masked_dispatch without the handle's arena and profiler
       timed(iters, elapsed_ms, [&] {
-        if (vb_handle::masked_flash(x_d, ld, o_d, ldo, B, n, heads, dh, 0, scale, nk_d, ATTN_MASK_KEYS)) return;
-        dS.ensure(static_cast<size_t>(B) * heads * n * n * sizeof(float));
-        attention_generic_masked<T>(x_d, ld, x_d + HD, ld, x_d + 2 * HD, ld, o_d, ldo, static_cast<float*>(dS.p), B, n, n, heads, dh, 0, scale,
-                                    nk_d);
+        h.arena.reset();
+        h.attention_masked_dispatch<T>(x_d, ld, o_d, ldo, B, n, heads, dh, dh, 1.0f / sqrtf(static_cast<float>(dh)), ATTN_MASK_KEYS, 0, nk_d);
       });
       download<T>(o_d, out, static_cast<size_t>(B) * n * ldo);
-    };
-    if (precision == VB_PRECISION_FP32) run(float());
-    else run(__nv_bfloat16());
+    });
   });
 }
 
@@ -3734,68 +3760,23 @@ int vb_op_spt(int32_t precision, const float* img, int32_t B, int32_t H, int32_t
     require_gpu();
     VB_CHECK(img && gamma && beta && kernel && bias && out && B > 0 && H > 0 && W > 0 && p > 0 && dim > 0, "vb_op_spt: bad arguments");
     VB_CHECK(H % p == 0 && W % p == 0, "Image dimensions must be divisible by the patch size.");
-    // vb_handle::spt_tokens with the weights of finalize_small_dataset_vit, outside a handle
-    const bool bf = precision == VB_PRECISION_BF16, fold = bf && dim % 64 == 0;
-    const int C = 3, K = p * p * 5 * C, Kp = bf ? round_up(K, 64) : K, rows = 1 + (H / p) * (W / p), M = B * rows;
-    std::vector<float> g(Kp, 0.f), bt(Kp, 0.f), w(static_cast<size_t>(Kp) * dim, 0.f), c2(bias, bias + dim), cl(dim, 0.f),
-        ps(static_cast<size_t>(rows) * dim, 0.f);
-    std::copy(gamma, gamma + K, g.begin());
-    std::copy(beta, beta + K, bt.begin());
-    std::copy(kernel, kernel + static_cast<size_t>(K) * dim, w.begin());
-    if (cls) std::copy(cls, cls + dim, cl.begin());
-    if (pos) std::copy(pos, pos + static_cast<size_t>(rows) * dim, ps.begin());
-    for (int k = 0; k < K; ++k)                                    // beta . W + bias: the Dense on the LayerNorm of a zero row
-      for (int n = 0; n < dim; ++n) c2[n] += beta[k] * kernel[static_cast<size_t>(k) * dim + n];
-    DevMem dI, dG, dBt, dW, dB, dC2, dCl, dP, dCol, dY, dR, dO, dWt, dF, dSt;
+    const int C = 3, K = p * p * 5 * C, rows = 1 + (H / p) * (W / p);
+    auto host = [](const float* a, size_t n) { return a ? std::vector<double>(a, a + n) : std::vector<double>(n, 0.0); };
+    DevMem dI;
     const float* img_d = upload<float>(dI, img, static_cast<size_t>(B) * H * W * C);
-    const float* g_d = upload<float>(dG, g.data(), Kp);
-    const float* bt_d = upload<float>(dBt, bt.data(), Kp);
-    const float* w_d = upload<float>(dW, w.data(), w.size());
-    const float* b_d = upload<float>(dB, bias, dim);
-    const float* cl_d = upload<float>(dCl, cl.data(), dim);
-    const float* p_d = upload<float>(dP, ps.data(), ps.size());
-    auto run = [&](auto tag) {
+    with_precision(precision, [&](vb_handle& h, auto tag) {
       using T = decltype(tag);
-      dCol.ensure(static_cast<size_t>(M) * Kp * sizeof(T));
-      T* col = static_cast<T*>(dCol.p);
-      spt_rows<T>(img_d, col, B, H, W, C, p, Kp, 0);
-      dR.ensure(static_cast<size_t>(M) * dim * sizeof(T));
-      dO.ensure(static_cast<size_t>(M) * dim * sizeof(T));
-      T* R = static_cast<T*>(dR.p);
-      T* o_d = static_cast<T*>(dO.p);
-      if constexpr (sizeof(T) == 2) {
-        dWt.ensure(static_cast<size_t>(dim) * Kp * sizeof(T));
-        T* wt = static_cast<T*>(dWt.p);
-        if (fold) {
-          pack_weight_bf16(w_d, wt, Kp, dim, Kp, 0, g_d);
-          dF.ensure(static_cast<size_t>(dim) * 2 * sizeof(float));
-          float* c = static_cast<float*>(dF.p);
-          ln_fold_consts(w_d, wt, Kp, bt_d, b_d, c, c + dim, Kp, dim, 0);
-          dSt.ensure(static_cast<size_t>(M) * (Kp / 64) * 2 * sizeof(float));
-          float* st = static_cast<float*>(dSt.p);
-          row_stats_bf16(col, Kp, st, M, Kp, 0);
-          build_embed_residual<T>(R, p_d, cl_d, c + dim, B, rows, dim, 1, 0);
-          GemmBf16 gm = gemm_bf16_plan(col, Kp, wt, Kp, o_d, dim, M, dim, Kp, c + dim, nullptr, R, dim, ACT_NONE);
-          gm.ln_c1 = c; gm.ln_stats = st; gm.ln_parts = Kp / 64; gm.ln_inv_d = 1.0f / static_cast<float>(K); gm.ln_eps = 1e-3f;
-          gemm_bf16_run(gm, 0);
-          download<T>(o_d, out, static_cast<size_t>(M) * dim);
-          return;
-        }
-        pack_weight_bf16(w_d, wt, Kp, dim, Kp, 0);
-      }
-      dY.ensure(static_cast<size_t>(M) * Kp * sizeof(T));
-      T* Y = static_cast<T*>(dY.p);
-      layernorm<T>(col, Kp, g_d, bt_d, Y, Kp, M, K, 0, Kp);
-      const float* c2_d = upload<float>(dC2, c2.data(), dim);
-      build_embed_residual<T>(R, p_d, cl_d, c2_d, B, rows, dim, 1, 0);
-      if constexpr (sizeof(T) == 2)
-        gemm_simt<T, T, T>(Y, Kp, static_cast<const T*>(dWt.p), 1, Kp, o_d, dim, M, dim, Kp, b_d, nullptr, R, dim, ACT_NONE, 0);
-      else
-        gemm_simt<float, float, float>(Y, Kp, w_d, dim, 1, o_d, dim, M, dim, Kp, b_d, nullptr, R, dim, ACT_NONE, 0);
-      download<T>(o_d, out, static_cast<size_t>(M) * dim);
-    };
-    if (bf) run(__nv_bfloat16());
-    else run(float());
+      h.cfg.patch_h = p;
+      h.cfg.channels = C;
+      h.set_spt_patch(host(gamma, K), host(beta, K), host(kernel, static_cast<size_t>(K) * dim), host(bias, dim), K, dim);
+      h.embed.cls = h.upload_owned(host(cls, dim));                // zero cls and positions when not given
+      h.embed.pos = h.upload_owned(host(pos, static_cast<size_t>(rows) * dim));
+      h.embed.dim = dim;
+      h.embed.n_pos = rows;
+      int r = 0;
+      const T* o_d = h.spt_tokens<T>(img_d, B, H, W, &r, 0, nullptr);
+      download<T>(o_d, out, static_cast<size_t>(B) * rows * dim);
+    });
     VB_CUDA(cudaDeviceSynchronize());
   });
 }
@@ -3822,22 +3803,17 @@ int vb_op_lsa_attention(int32_t precision, const float* qkv, int32_t ld, int32_t
       wout.assign(static_cast<size_t>(B) * n * ldow, 0.f);
       src = wide.data();
     }
-    DevMem dX, dO, dS;
-    auto run = [&](auto tag) {
+    DevMem dX, dO;
+    with_precision(precision, [&](vb_handle& h, auto tag) {
       using T = decltype(tag);
       const T* x_d = upload<T>(dX, src, static_cast<size_t>(B) * n * ldw);
       T* o_d = upload<T>(dO, widen ? wout.data() : out, static_cast<size_t>(B) * n * ldow);
-      // vb_handle::attention_masked_dispatch of an LSA layer without the handle's arena and profiler
-      timed(iters, elapsed_ms, [&] {
-        if (vb_handle::masked_flash(x_d, ldw, o_d, ldow, B, n, heads, dw, 0, scale, nullptr, ATTN_MASK_DIAG)) return;
-        dS.ensure(static_cast<size_t>(B) * heads * n * n * sizeof(float));
-        attention_generic_masked<T>(x_d, ldw, x_d + HW, ldw, x_d + 2 * HW, ldw, o_d, ldow, static_cast<float*>(dS.p), B, n, n, heads, dw, 0,
-                                    scale, nullptr, ATTN_MASK_DIAG);
+      timed(iters, elapsed_ms, [&] {                  // the scale is explicit, so the widened heads run as the model's own
+        h.arena.reset();
+        h.attention_masked_dispatch<T>(x_d, ldw, o_d, ldow, B, n, heads, dw, dw, scale, ATTN_MASK_DIAG, 0, nullptr);
       });
       download<T>(o_d, widen ? wout.data() : out, static_cast<size_t>(B) * n * ldow);
-    };
-    if (precision == VB_PRECISION_FP32) run(float());
-    else run(__nv_bfloat16());
+    });
     if (widen)
       for (size_t r = 0; r < static_cast<size_t>(B) * n; ++r)
         for (int h = 0; h < heads; ++h)
@@ -4238,29 +4214,23 @@ int vb_op_linear(int32_t precision, const float* a, const float* w, const float*
   return guarded(nullptr, [&] {
     require_gpu();
     VB_CHECK(a && w && out && M > 0 && N > 0 && K > 0, "vb_op_linear: bad arguments");
-    DevMem dA, dW, dWt, dB, dS, dR, dO;
+    DevMem dA, dW, dB, dS, dR, dO;
     const float* db = bias ? upload<float>(dB, bias, N) : nullptr;
     const float* ds = scale ? upload<float>(dS, scale, N) : nullptr;
     const float* dw = upload<float>(dW, w, static_cast<size_t>(K) * N);
-    if (precision == VB_PRECISION_FP32) {
-      const float* da = upload<float>(dA, a, static_cast<size_t>(M) * K);
-      const float* dr = res ? upload<float>(dR, res, static_cast<size_t>(M) * N) : nullptr;
-      dO.ensure(static_cast<size_t>(M) * N * 4);
-      float* dout = static_cast<float*>(dO.p);
-      timed(iters, elapsed_ms, [&] { gemm_simt<float, float, float>(da, K, dw, N, 1, dout, N, M, N, K, db, ds, dr, N, gelu, 0); });
-      download<float>(dout, out, static_cast<size_t>(M) * N);
-    } else {
-      VB_CHECK(gemm_bf16_supported(M, N, K, K, K, N), "vb_op_linear(bf16): need N % 64 == 0 and K % 8 == 0");
-      const __nv_bfloat16* da = upload<__nv_bfloat16>(dA, a, static_cast<size_t>(M) * K);
-      const __nv_bfloat16* dr = res ? upload<__nv_bfloat16>(dR, res, static_cast<size_t>(M) * N) : nullptr;
-      dWt.ensure(static_cast<size_t>(N) * K * 2);
-      pack_weight_bf16(dw, static_cast<__nv_bfloat16*>(dWt.p), K, N, K, 0);
-      dO.ensure(static_cast<size_t>(M) * N * 2);
-      __nv_bfloat16* dout = static_cast<__nv_bfloat16*>(dO.p);
-      GemmBf16 g = gemm_bf16_plan(da, K, static_cast<const __nv_bfloat16*>(dWt.p), K, dout, N, M, N, K, db, ds, dr, N, gelu != 0);
-      timed(iters, elapsed_ms, [&] { gemm_bf16_run(g, 0); });
-      download<__nv_bfloat16>(dout, out, static_cast<size_t>(M) * N);
-    }
+    with_precision(precision, [&](vb_handle& h, auto tag) {
+      using T = decltype(tag);
+      if (h.bf16()) VB_CHECK(gemm_bf16_supported(M, N, K, K, K, N), "vb_op_linear(bf16): need N % 64 == 0 and K % 8 == 0");
+      const T* da = upload<T>(dA, a, static_cast<size_t>(M) * K);
+      Epi e;
+      e.bias = db; e.scale = ds; e.gelu = gelu != 0; e.ldr = N;
+      e.res = res ? upload<T>(dR, res, static_cast<size_t>(M) * N) : nullptr;
+      const Linear L = h.pack_linear(dw, db, K, N, K, nullptr);
+      dO.ensure(static_cast<size_t>(M) * N * sizeof(T));
+      T* dout = static_cast<T*>(dO.p);
+      timed(iters, elapsed_ms, [&] { h.linear<T>(da, K, M, L, dout, N, e, 0); });
+      download<T>(dout, out, static_cast<size_t>(M) * N);
+    });
   });
 }
 
@@ -4272,30 +4242,26 @@ int vb_op_attention(int32_t precision, int32_t variant, const float* q, const fl
     VB_CHECK(q && k && v && out && B > 0 && nq > 0 && nk > 0 && heads > 0 && dim_head > 0, "vb_op_attention: bad arguments");
     VB_CHECK(variant >= 0 && variant <= 2, "vb_op_attention: variant must be 0, 1 or 2");
     const int inner = heads * dim_head;
-    DevMem dQ, dK, dV, dO, dS, dMa, dMb, dG, dBt;
+    DevMem dQ, dK, dV, dO, dMa, dMb, dG, dBt;
     const float* ma = mix_a ? upload<float>(dMa, mix_a, heads * heads) : nullptr;
     const float* mb = mix_b ? upload<float>(dMb, mix_b, heads * heads) : nullptr;
     const float* g = ln_gamma ? upload<float>(dG, ln_gamma, heads) : nullptr;
     const float* bt = ln_beta ? upload<float>(dBt, ln_beta, heads) : nullptr;
     const MixCacheScope mix_scope{{ma, mb, g, bt}};
     const size_t cq = static_cast<size_t>(B) * nq * inner, ck = static_cast<size_t>(B) * nk * inner;
-    auto run = [&](auto tag) {
+    with_precision(precision, [&](vb_handle& h, auto tag) {
       using T = decltype(tag);
       const T* q_d = upload<T>(dQ, q, cq);
       const T* k_d = upload<T>(dK, k, ck);
       const T* v_d = upload<T>(dV, v, ck);
       dO.ensure(cq * sizeof(T));
       T* o_d = static_cast<T*>(dO.p);
-      dS.ensure(static_cast<size_t>(B) * heads * nq * ((nk + 15) & ~15) * 4);
       timed(iters, elapsed_ms, [&] {
-        if (!attention_fast<T>(q_d, inner, k_d, inner, v_d, inner, o_d, inner, B, nq, nk, heads, dim_head, variant, ma, mb, g, bt, 0))
-          attention_generic<T>(q_d, inner, k_d, inner, v_d, inner, o_d, inner, static_cast<float*>(dS.p), B, nq, nk, heads,
-                               dim_head, variant, ma, mb, g, bt, 0);
+        h.arena.reset();
+        h.attention_dispatch<T>(q_d, inner, k_d, inner, v_d, inner, o_d, inner, B, nq, nk, heads, dim_head, variant, ma, mb, g, bt, 0);
       });
       download<T>(o_d, out, cq);
-    };
-    if (precision == VB_PRECISION_FP32) run(float());
-    else run(__nv_bfloat16());
+    });
   });
 }
 
@@ -4304,30 +4270,19 @@ int vb_op_patch_merger(int32_t precision, const float* x, const float* gamma, co
   return guarded(nullptr, [&] {
     require_gpu();
     VB_CHECK(x && gamma && beta && queries && out && B > 0 && n > 0 && D > 0 && nt > 0, "vb_op_patch_merger: bad arguments");
-    DevMem dX, dG, dB, dQf, dY, dQ, dO, dS;
-    const float* g = upload<float>(dG, gamma, D);
-    const float* b = upload<float>(dB, beta, D);
+    DevMem dX, dG, dB, dQf;
+    const Norm norm{upload<float>(dG, gamma, D), upload<float>(dB, beta, D), D};
     const float* qf = upload<float>(dQf, queries, static_cast<size_t>(nt) * D);
-    const size_t cx = static_cast<size_t>(B) * n * D, co = static_cast<size_t>(B) * nt * D;
-    auto run = [&](auto tag) {
+    with_precision(precision, [&](vb_handle& h, auto tag) {
       using T = decltype(tag);
-      const T* x_d = upload<T>(dX, x, cx);
-      dY.ensure(cx * sizeof(T) + 16); dQ.ensure(co * sizeof(T) + 16); dO.ensure(co * sizeof(T) + 16);
-      dS.ensure(static_cast<size_t>(B) * nt * ((n + 15) & ~15) * 4);
-      T* y_d = static_cast<T*>(dY.p);
-      T* q_d = static_cast<T*>(dQ.p);
-      T* o_d = static_cast<T*>(dO.p);
+      const T* x_d = upload<T>(dX, x, static_cast<size_t>(B) * n * D);
+      const T* o_d = nullptr;
       timed(iters, elapsed_ms, [&] {
-        layernorm<T>(x_d, D, g, b, y_d, D, B * n, D, 0);
-        broadcast_rows<T>(qf, q_d, B, nt, D, 0);
-        if (!attention_fast<T>(q_d, D, y_d, D, y_d, D, o_d, D, B, nt, n, 1, D, 0, nullptr, nullptr, nullptr, nullptr, 0))
-          attention_generic<T>(q_d, D, y_d, D, y_d, D, o_d, D, static_cast<float*>(dS.p), B, nt, n, 1, D, 0, nullptr, nullptr, nullptr,
-                               nullptr, 0);
+        h.arena.reset();
+        o_d = h.patch_merge<T>(x_d, B, n, D, norm, qf, nt, 0);
       });
-      download<T>(o_d, out, co);
-    };
-    if (precision == VB_PRECISION_FP32) run(float());
-    else run(__nv_bfloat16());
+      download<T>(o_d, out, static_cast<size_t>(B) * nt * D);
+    });
   });
 }
 
@@ -4337,19 +4292,16 @@ int vb_op_layernorm(int32_t precision, const float* x, const float* gamma, const
     require_gpu();
     VB_CHECK(x && gamma && beta && out && M > 0 && D > 0, "vb_op_layernorm: bad arguments");
     DevMem dX, dG, dB, dO;
-    const float* g = upload<float>(dG, gamma, D);
-    const float* b = upload<float>(dB, beta, D);
+    const Norm norm{upload<float>(dG, gamma, D), upload<float>(dB, beta, D), D};
     const size_t cnt = static_cast<size_t>(M) * D;
-    auto run = [&](auto tag) {
+    with_precision(precision, [&](vb_handle& h, auto tag) {
       using T = decltype(tag);
       const T* x_d = upload<T>(dX, x, cnt);
       dO.ensure(cnt * sizeof(T));
       T* o_d = static_cast<T*>(dO.p);
-      timed(iters, elapsed_ms, [&] { layernorm<T>(x_d, D, g, b, o_d, D, M, D, 0); });
+      timed(iters, elapsed_ms, [&] { h.ln<T>(x_d, norm, o_d, M, D, 0); });
       download<T>(o_d, out, cnt);
-    };
-    if (precision == VB_PRECISION_FP32) run(float());
-    else run(__nv_bfloat16());
+    });
   });
 }
 
@@ -4359,26 +4311,21 @@ int vb_op_ln_linear(const float* x, const float* gamma, const float* beta, const
     require_gpu();
     VB_CHECK(x && gamma && beta && w && out && M > 0 && N > 0 && K > 0, "vb_op_ln_linear: bad arguments");
     VB_CHECK(N % 64 == 0 && K % 64 == 0, "vb_op_ln_linear: the folded form needs N % 64 == 0 and K % 64 == 0");
-    DevMem dX, dG, dBt, dW, dWt, dB, dC, dSt, dO;
-    const __nv_bfloat16* dx = upload<__nv_bfloat16>(dX, x, static_cast<size_t>(M) * K);
-    const float* g = upload<float>(dG, gamma, K);
-    const float* bt = upload<float>(dBt, beta, K);
-    const float* dw = upload<float>(dW, w, static_cast<size_t>(K) * N);
+    using bf = __nv_bfloat16;
+    vb_handle h{};
+    h.cfg.precision = VB_PRECISION_BF16;
+    DevMem dX, dG, dBt, dW, dB, dO;
+    const bf* dx = upload<bf>(dX, x, static_cast<size_t>(M) * K);
+    const Norm norm{upload<float>(dG, gamma, K), upload<float>(dBt, beta, K), K};
     const float* db = bias ? upload<float>(dB, bias, N) : nullptr;
-    dWt.ensure(static_cast<size_t>(N) * K * 2);
-    __nv_bfloat16* wt = static_cast<__nv_bfloat16*>(dWt.p);
-    pack_weight_bf16(dw, wt, K, N, K, 0, g);                       // gamma folded into the packed weight rows
-    dC.ensure(static_cast<size_t>(N) * 2 * sizeof(float));
-    float* c = static_cast<float*>(dC.p);
-    ln_fold_consts(dw, wt, K, bt, db, c, c + N, K, N, 0);
-    dSt.ensure(static_cast<size_t>(M) * (K / 64) * 2 * sizeof(float));
-    float* st = static_cast<float*>(dSt.p);
+    const Linear L = h.pack_linear(upload<float>(dW, w, static_cast<size_t>(K) * N), db, K, N, K, &norm);
+    float* st = h.row_stats(M, K);
     dO.ensure(static_cast<size_t>(M) * N * 2);
-    __nv_bfloat16* dout = static_cast<__nv_bfloat16*>(dO.p);
-    GemmBf16 gm = gemm_bf16_plan(dx, K, wt, K, dout, N, M, N, K, c + N, nullptr, nullptr, 0, gelu != 0);
-    gm.ln_c1 = c; gm.ln_stats = st; gm.ln_parts = K / 64; gm.ln_inv_d = 1.0f / static_cast<float>(K);
-    timed(iters, elapsed_ms, [&] { row_stats_bf16(dx, K, st, M, K, 0); gemm_bf16_run(gm, 0); });
-    download<__nv_bfloat16>(dout, out, static_cast<size_t>(M) * N);
+    bf* dout = static_cast<bf*>(dO.p);
+    Epi e;
+    e.bias = L.ln_c2; e.ln_stats = st; e.gelu = gelu != 0;
+    timed(iters, elapsed_ms, [&] { h.ensure_stats<bf>(dx, K, st, M, 0); h.linear<bf>(dx, K, M, L, dout, N, e, 0); });
+    download<bf>(dout, out, static_cast<size_t>(M) * N);
   });
 }
 
@@ -4436,32 +4383,25 @@ int vb_op_attention_ex(int32_t precision, int32_t variant, const float* q, int32
     VB_CHECK(q && out && B > 0 && nq > 0 && nk > 0 && heads > 0 && dh > 0 && ldq >= inner && ldo >= inner && k_off >= 0 &&
              v_off >= 0 && k_off + inner <= ldk && v_off + inner <= ldk && (!fused || nk == nq), "vb_op_attention_ex: bad arguments");
     VB_CHECK(variant >= 0 && variant <= 2, "vb_op_attention_ex: variant must be 0, 1 or 2");
-    DevMem dQ, dKV, dO, dS, dMa, dMb, dG, dBt;
+    DevMem dQ, dKV, dO, dMa, dMb, dG, dBt;
     const float* ma = mix_a ? upload<float>(dMa, mix_a, heads * heads) : nullptr;
     const float* mb = mix_b ? upload<float>(dMb, mix_b, heads * heads) : nullptr;
     const float* g = ln_gamma ? upload<float>(dG, ln_gamma, heads) : nullptr;
     const float* bt = ln_beta ? upload<float>(dBt, ln_beta, heads) : nullptr;
     const MixCacheScope mix_scope{{ma, mb, g, bt}};
     const size_t cq = static_cast<size_t>(B) * nq * ldq, ckv = static_cast<size_t>(B) * nk * ldk, co = static_cast<size_t>(B) * nq * ldo;
-    auto run = [&](auto tag) {
+    with_precision(precision, [&](vb_handle& h, auto tag) {
       using T = decltype(tag);
       const T* q_d = upload<T>(dQ, q, cq);
       const T* kv_d = fused ? q_d : upload<T>(dKV, kv, ckv);
       T* o_d = upload<T>(dO, out, co);
-      dS.ensure(static_cast<size_t>(B) * heads * nq * ((nk + 15) & ~15) * 4);
-      // vb_handle::attention_dispatch without the handle's arena and profiler
       timed(iters, elapsed_ms, [&] {
-        if (attention_fast<T>(q_d, ldq, kv_d + k_off, ldk, kv_d + v_off, ldk, o_d, ldo, B, nq, nk, heads, dh, variant, ma, mb, g, bt, 0,
-                              scale))
-          return;
-        VB_CHECK(scale <= 0.f, "vb_op_attention_ex: an explicit softmax scale needs the fused attention kernels");
-        attention_generic<T>(q_d, ldq, kv_d + k_off, ldk, kv_d + v_off, ldk, o_d, ldo, static_cast<float*>(dS.p), B, nq, nk, heads, dh,
-                             variant, ma, mb, g, bt, 0);
+        h.arena.reset();
+        h.attention_dispatch<T>(q_d, ldq, kv_d + k_off, ldk, kv_d + v_off, ldk, o_d, ldo, B, nq, nk, heads, dh, variant, ma, mb, g, bt, 0,
+                                scale);
       });
       download<T>(o_d, out, co);
-    };
-    if (precision == VB_PRECISION_FP32) run(float());
-    else run(__nv_bfloat16());
+    });
   });
 }
 
@@ -4474,34 +4414,24 @@ int vb_op_attention_bias(int32_t precision, const float* q, int32_t ldq, const f
     VB_CHECK(q && k && v && pos_bias && out && B > 0 && heads > 0 && dh > 0 && fmap > 0 && (q_step == 1 || q_step == 2) && scale > 0.f &&
              ldq >= inner && ldk >= inner && ldv >= inner && ldo >= inner, "vb_op_attention_bias: bad arguments");
     const int f2 = fmap * fmap, nqs = (fmap + q_step - 1) / q_step, nq = nqs * nqs, nk = f2;
-    std::vector<float> tab(static_cast<size_t>(heads) * f2);        // [heads][fmap^2] / scale, as vb_finalize packs it
-    for (int h = 0; h < heads; ++h)
-      for (int e = 0; e < f2; ++e)
-        tab[static_cast<size_t>(h) * f2 + e] = static_cast<float>(static_cast<double>(pos_bias[static_cast<size_t>(e) * heads + h]) / scale);
-    DevMem dQ, dK, dV, dO, dS, dT;
-    dT.ensure(tab.size() * sizeof(float));
-    VB_CUDA(cudaMemcpy(dT.p, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice));
-    PosBias pb;
-    pb.table = static_cast<const float*>(dT.p); pb.fmap = fmap; pb.step = q_step; pb.gelu_out = gelu_out != 0;
+    DevMem dQ, dK, dV, dO;
     const size_t cq = static_cast<size_t>(B) * nq * ldq, co = static_cast<size_t>(B) * nq * ldo;
-    auto run = [&](auto tag) {
+    with_precision(precision, [&](vb_handle& h, auto tag) {
       using T = decltype(tag);
+      PosBias pb;
+      pb.table = h.upload_owned(vb_handle::levit_pos_table(std::vector<double>(pos_bias, pos_bias + static_cast<size_t>(f2) * heads), f2, heads,
+                                                           1.0 / scale));
+      pb.fmap = fmap; pb.step = q_step; pb.gelu_out = gelu_out != 0;
       const T* q_d = upload<T>(dQ, q, cq);
       const T* k_d = upload<T>(dK, k, static_cast<size_t>(B) * nk * ldk);
       const T* v_d = upload<T>(dV, v, static_cast<size_t>(B) * nk * ldv);
       T* o_d = upload<T>(dO, out, co);
-      dS.ensure(static_cast<size_t>(B) * heads * nq * ((nk + 15) & ~15) * 4);
-      // vb_handle::attention_bias without the handle's arena and profiler
       timed(iters, elapsed_ms, [&] {
-        if (attention_fast<T>(q_d, ldq, k_d, ldk, v_d, ldv, o_d, ldo, B, nq, nk, heads, dh, 0, nullptr, nullptr, nullptr, nullptr, 0, scale, &pb))
-          return;
-        attention_generic<T>(q_d, ldq, k_d, ldk, v_d, ldv, o_d, ldo, static_cast<float*>(dS.p), B, nq, nk, heads, dh, 0, nullptr, nullptr,
-                             nullptr, nullptr, 0, scale, &pb);
+        h.arena.reset();
+        h.attention_bias<T>(q_d, ldq, k_d, ldk, v_d, ldv, o_d, ldo, B, nq, nk, heads, dh, scale, pb, 0);
       });
       download<T>(o_d, out, co);
-    };
-    if (precision == VB_PRECISION_FP32) run(float());
-    else run(__nv_bfloat16());
+    });
   });
 }
 
@@ -4512,7 +4442,7 @@ int vb_op_dwconv(int32_t precision, const float* x, int32_t B, int32_t H, int32_
     require_gpu();
     VB_CHECK(x && ln_gamma && ln_beta && wq && bn_q && wkv && bn_kv && q && kv && B > 0 && H > 0 && W > 0 && C > 0 && k >= 1 && k <= 7 &&
              (kv_stride == 1 || kv_stride == 2), "vb_op_dwconv: bad arguments");
-    const bool bf = precision == VB_PRECISION_BF16;
+    const bool bf = precision != VB_PRECISION_FP32;               // as with_precision picks the element type
     const int Cp = bf ? round_up(C, 64) : C, Ho = (H + kv_stride - 1) / kv_stride, Wo = (W + kv_stride - 1) / kv_stride;
     const size_t M = static_cast<size_t>(B) * H * W, Mk = static_cast<size_t>(B) * Ho * Wo;
     auto vec = [](const float* p, size_t n) { return std::vector<double>(p, p + n); };
@@ -4528,42 +4458,31 @@ int vb_op_dwconv(int32_t precision, const float* x, int32_t B, int32_t H, int32_
     for (size_t r = 0; r < M; ++r) std::copy(x + r * C, x + (r + 1) * C, xp.begin() + r * Cp);
     std::copy(ln_gamma, ln_gamma + C, gp.begin());
     std::copy(ln_beta, ln_beta + C, bp.begin());
-    DevMem dX, dG, dB, dTq, dSq, dTkv, dSkv, dQ, dKV, dS, dY;
-    const float* g_d = upload<float>(dG, gp.data(), Cp);
-    const float* b_d = upload<float>(dB, bp.data(), Cp);
-    const float* tq_d = upload<float>(dTq, tq.data(), tq.size());
-    const float* sq_d = upload<float>(dSq, sq.data(), sq.size());
-    const float* tkv_d = upload<float>(dTkv, tkv.data(), tkv.size());
-    const float* skv_d = upload<float>(dSkv, skv.data(), skv.size());
+    DevMem dX, dG, dB, dTq, dSq, dTkv, dSkv, dQ, dKV;
+    CvtBlockW b;
+    b.dim = C; b.dp = Cp; b.k = k; b.kv_stride = kv_stride;
+    b.attn_norm = Norm{upload<float>(dG, gp.data(), Cp), upload<float>(dB, bp.data(), Cp), C};
+    b.wq = upload<float>(dTq, tq.data(), tq.size());
+    b.bq = upload<float>(dSq, sq.data(), sq.size());
+    b.wkv = upload<float>(dTkv, tkv.data(), tkv.size());
+    b.bkv = upload<float>(dSkv, skv.data(), skv.size());
     std::vector<float> qh(M * Cp), kvh(Mk * Cp);
-    auto run = [&](auto tag) {
+    with_precision(precision, [&](vb_handle& h, auto tag) {
       using T = decltype(tag);
-      const T* x_d = upload<T>(dX, xp.data(), M * Cp);
+      T* x_d = upload<T>(dX, xp.data(), M * Cp);
       dQ.ensure(M * Cp * sizeof(T));
       dKV.ensure(Mk * Cp * sizeof(T));
       T* q_d = static_cast<T*>(dQ.p);
       T* kv_d = static_cast<T*>(dKV.p);
-      // vb_handle::cvt_block's depthwise step, without the handle's arena and profiler
-      if constexpr (std::is_same<T, __nv_bfloat16>::value) {
-        dS.ensure(M * (Cp / 64) * 2 * sizeof(float));
-        float* st = static_cast<float*>(dS.p);
-        timed(iters, elapsed_ms, [&] {
-          row_stats_bf16(x_d, Cp, st, static_cast<int>(M), Cp, 0);
-          dwconv_qkv<T>(x_d, Cp, st, g_d, b_d, C, 1e-5f, tq_d, sq_d, q_d, Cp, tkv_d, skv_d, kv_d, Cp, B, H, W, Cp, k, kv_stride, 0);
-        });
-      } else {
-        dY.ensure(M * Cp * sizeof(T));
-        T* y = static_cast<T*>(dY.p);
-        timed(iters, elapsed_ms, [&] {
-          layernorm<T>(x_d, Cp, g_d, b_d, y, Cp, static_cast<int>(M), C, 0, Cp, 1e-5f);
-          dwconv_qkv<T>(y, Cp, nullptr, nullptr, nullptr, C, 1e-5f, tq_d, sq_d, q_d, Cp, tkv_d, skv_d, kv_d, Cp, B, H, W, Cp, k, kv_stride, 0);
-        });
-      }
+      timed(iters, elapsed_ms, [&] {
+        h.arena.reset();
+        float* st = h.row_stats(static_cast<long long>(M), Cp);
+        h.ensure_stats<T>(x_d, Cp, st, static_cast<int>(M), 0);
+        h.cvt_dwconv<T>(h.prenorm<T>(x_d, static_cast<int>(M), C, Cp, st, 1e-5f, 0), B, H, W, b, q_d, kv_d, 0);
+      });
       download<T>(q_d, qh.data(), M * Cp);
       download<T>(kv_d, kvh.data(), Mk * Cp);
-    };
-    if (bf) run(__nv_bfloat16());
-    else run(float());
+    });
     for (size_t r = 0; r < M; ++r) std::copy(qh.begin() + r * Cp, qh.begin() + r * Cp + C, q + r * C);
     for (size_t r = 0; r < Mk; ++r) std::copy(kvh.begin() + r * Cp, kvh.begin() + r * Cp + C, kv + r * C);
   });
@@ -4580,30 +4499,18 @@ int vb_op_window_attention(int32_t precision, const float* qkv, int32_t ld, int3
     win.p = p; win.nx = W / p; win.ny = H / p;
     const int n = p * p, Bw = B * win.nx * win.ny;
     const long long rows = static_cast<long long>(B) * H * W;
-    DevMem dX, dO, dW, dOw, dS;
-    auto run = [&](auto tag) {
+    DevMem dX, dO;
+    with_precision(precision, [&](vb_handle& h, auto tag) {
       using T = decltype(tag);
       const T* x_d = upload<T>(dX, qkv, static_cast<size_t>(rows) * ld);
       T* o_d = upload<T>(dO, out, static_cast<size_t>(rows) * ldo);
-      // vb_handle::attention_dispatch's windowed branch without the handle's arena and profiler
       timed(iters, elapsed_ms, [&] {
-        if (attention_fast<T>(x_d, ld, x_d + HD, ld, x_d + 2 * HD, ld, o_d, ldo, Bw, n, n, heads, dh, 0, nullptr, nullptr, nullptr, nullptr, 0, 0.f,
-                              nullptr, &win))
-          return;
-        dW.ensure(static_cast<size_t>(rows) * 3 * HD * sizeof(T));
-        dOw.ensure(static_cast<size_t>(rows) * HD * sizeof(T));
-        dS.ensure(static_cast<size_t>(Bw) * heads * n * ((n + 15) & ~15) * sizeof(float));
-        T* w_d = static_cast<T*>(dW.p);
-        T* ow_d = static_cast<T*>(dOw.p);
-        window_rows<T>(x_d, ld, w_d, 3 * HD, 3 * HD, win, rows, true, 0);
-        attention_generic<T>(w_d, 3 * HD, w_d + HD, 3 * HD, w_d + 2 * HD, 3 * HD, ow_d, HD, static_cast<float*>(dS.p), Bw, n, n, heads, dh, 0,
-                             nullptr, nullptr, nullptr, nullptr, 0);
-        window_rows<T>(ow_d, HD, o_d, ldo, HD, win, rows, false, 0);
+        h.arena.reset();
+        h.attention_dispatch<T>(x_d, ld, x_d + HD, ld, x_d + 2 * HD, ld, o_d, ldo, Bw, n, n, heads, dh, 0, nullptr, nullptr, nullptr, nullptr, 0,
+                                0.f, &win);
       });
       download<T>(o_d, out, static_cast<size_t>(rows) * ldo);
-    };
-    if (precision == VB_PRECISION_FP32) run(float());
-    else run(__nv_bfloat16());
+    });
   });
 }
 
@@ -4619,32 +4526,20 @@ int vb_op_window_bias_attention(int32_t precision, const float* qkv, int32_t ld,
     win.p = wsz; win.nx = W / wsz; win.ny = H / wsz; win.dilated = is_long != 0;
     const int n = wsz * wsz, Bw = B * win.nx * win.ny, t = (2 * wsz - 1) * (2 * wsz - 1);
     const long long rows = static_cast<long long>(B) * H * W;
-    DevMem dX, dO, dW, dOw, dS, dT;
+    DevMem dX, dO, dT;
     PosBias pb;
     pb.table = upload<float>(dT, table, t); pb.wsz = wsz;
-    auto run = [&](auto tag) {
+    with_precision(precision, [&](vb_handle& h, auto tag) {
       using T = decltype(tag);
       const T* x_d = upload<T>(dX, qkv, static_cast<size_t>(rows) * ld);
       T* o_d = upload<T>(dO, out, static_cast<size_t>(rows) * ldo);
-      // vb_handle::attention_dispatch's windowed branch without the handle's arena and profiler
       timed(iters, elapsed_ms, [&] {
-        if (attention_fast<T>(x_d, ld, x_d + HD, ld, x_d + 2 * HD, ld, o_d, ldo, Bw, n, n, heads, dh, 0, nullptr, nullptr, nullptr, nullptr, 0, 0.f,
-                              &pb, &win))
-          return;
-        dW.ensure(static_cast<size_t>(rows) * 3 * HD * sizeof(T));
-        dOw.ensure(static_cast<size_t>(rows) * HD * sizeof(T));
-        dS.ensure(static_cast<size_t>(Bw) * heads * n * ((n + 15) & ~15) * sizeof(float));
-        T* w_d = static_cast<T*>(dW.p);
-        T* ow_d = static_cast<T*>(dOw.p);
-        window_rows<T>(x_d, ld, w_d, 3 * HD, 3 * HD, win, rows, true, 0);
-        attention_generic<T>(w_d, 3 * HD, w_d + HD, 3 * HD, w_d + 2 * HD, 3 * HD, ow_d, HD, static_cast<float*>(dS.p), Bw, n, n, heads, dh, 0,
-                             nullptr, nullptr, nullptr, nullptr, 0, 0.f, &pb);
-        window_rows<T>(ow_d, HD, o_d, ldo, HD, win, rows, false, 0);
+        h.arena.reset();
+        h.attention_dispatch<T>(x_d, ld, x_d + HD, ld, x_d + 2 * HD, ld, o_d, ldo, Bw, n, n, heads, dh, 0, nullptr, nullptr, nullptr, nullptr, 0,
+                                0.f, &win, &pb);
       });
       download<T>(o_d, out, static_cast<size_t>(rows) * ldo);
-    };
-    if (precision == VB_PRECISION_FP32) run(float());
-    else run(__nv_bfloat16());
+    });
   });
 }
 
@@ -4657,30 +4552,18 @@ int vb_op_block_attention(int32_t precision, const float* qkv, int32_t ld, int32
              ldo >= HD, "vb_op_block_attention: bad arguments");
     Window win;
     win.p = bh; win.pw = bw; win.nx = W / bw; win.ny = H / bh; win.count = B * win.nx * win.ny;
-    const int n = bh * bw, Bw = win.count;
     const long long rows = static_cast<long long>(B) * H * W;
-    DevMem dX, dO, dW, dOw, dS;
-    auto run = [&](auto tag) {
+    DevMem dX, dO;
+    with_precision(precision, [&](vb_handle& h, auto tag) {
       using T = decltype(tag);
       const T* x_d = upload<T>(dX, qkv, static_cast<size_t>(rows) * ld);
       T* o_d = upload<T>(dO, out, static_cast<size_t>(rows) * ldo);
-      // vb_handle::block_attention without the handle's arena and profiler
       timed(iters, elapsed_ms, [&] {
-        if (block_attention_fast(x_d, ld, o_d, ldo, heads, dh, 0, win)) return;
-        dW.ensure(static_cast<size_t>(rows) * 3 * HD * sizeof(T));
-        dOw.ensure(static_cast<size_t>(rows) * HD * sizeof(T));
-        dS.ensure(static_cast<size_t>(Bw) * heads * n * ((n + 15) & ~15) * sizeof(float));
-        T* w_d = static_cast<T*>(dW.p);
-        T* ow_d = static_cast<T*>(dOw.p);
-        window_rows<T>(x_d, ld, w_d, 3 * HD, 3 * HD, win, rows, true, 0);
-        attention_generic<T>(w_d, 3 * HD, w_d + HD, 3 * HD, w_d + 2 * HD, 3 * HD, ow_d, HD, static_cast<float*>(dS.p), Bw, n, n, heads, dh, 0,
-                             nullptr, nullptr, nullptr, nullptr, 0);
-        window_rows<T>(ow_d, HD, o_d, ldo, HD, win, rows, false, 0);
+        h.arena.reset();
+        h.block_attention<T>(x_d, ld, o_d, ldo, heads, dh, win, 0);
       });
       download<T>(o_d, out, static_cast<size_t>(rows) * ldo);
-    };
-    if (precision == VB_PRECISION_FP32) run(float());
-    else run(__nv_bfloat16());
+    });
   });
 }
 
@@ -4695,35 +4578,20 @@ int vb_op_r2l_attention(int32_t precision, const float* qkv, int32_t ld, int32_t
     Window win;
     win.p = lh / rh; win.pw = lw / rw; win.nx = rw; win.ny = rh; win.count = B * rh * rw;
     const long long Ml = static_cast<long long>(B) * lh * lw, rows = Ml + static_cast<long long>(B) * rh * rw;
-    const int n = 1 + win.p * win.pw;
-    DevMem dX, dO, dT, dW, dOw, dS;
-    const auto tab = r2l_table_from_embedding(table, ws, heads);   // transposed as vb_finalize does
-    const std::vector<float> tab_f(tab.begin(), tab.end());
-    PosBias pb;
-    pb.table = upload<float>(dT, tab_f.data(), tab_f.size());
-    pb.r2l_ws = ws; pb.r2l_h = win.p; pb.r2l_w = win.pw;
-    auto run = [&](auto tag) {
+    DevMem dX, dO;
+    with_precision(precision, [&](vb_handle& h, auto tag) {
       using T = decltype(tag);
+      PosBias pb;
+      pb.table = h.upload_owned(r2l_table_from_embedding(table, ws, heads));   // transposed as vb_finalize does
+      pb.r2l_ws = ws; pb.r2l_h = win.p; pb.r2l_w = win.pw;
       const T* x_d = upload<T>(dX, qkv, static_cast<size_t>(rows) * ld);
       T* o_d = upload<T>(dO, out, static_cast<size_t>(rows) * ldo);
-      // vb_handle::r2l_attention without the handle's arena and profiler
       timed(iters, elapsed_ms, [&] {
-        if (r2l_attention_fast(x_d, ld, o_d, ldo, heads, dh, Ml, pb, win, 0)) return;
-        const size_t wrows = static_cast<size_t>(win.count) * n;
-        dW.ensure(wrows * 3 * HD * sizeof(T));
-        dOw.ensure(wrows * HD * sizeof(T));
-        dS.ensure(static_cast<size_t>(win.count) * heads * n * ((n + 15) & ~15) * sizeof(float));
-        T* w_d = static_cast<T*>(dW.p);
-        T* ow_d = static_cast<T*>(dOw.p);
-        r2l_rows<T>(x_d, ld, w_d, 3 * HD, 3 * HD, win, Ml, true, 0);
-        attention_generic<T>(w_d, 3 * HD, w_d + HD, 3 * HD, w_d + 2 * HD, 3 * HD, ow_d, HD, static_cast<float*>(dS.p), win.count, n, n, heads,
-                             dh, 0, nullptr, nullptr, nullptr, nullptr, 0, 0.f, &pb);
-        r2l_rows<T>(ow_d, HD, o_d, ldo, HD, win, Ml, false, 0);
+        h.arena.reset();
+        h.r2l_attention<T>(x_d, ld, o_d, ldo, Ml, pb, win, 0, heads, dh);
       });
       download<T>(o_d, out, static_cast<size_t>(rows) * ldo);
-    };
-    if (precision == VB_PRECISION_FP32) run(float());
-    else run(__nv_bfloat16());
+    });
   });
 }
 
@@ -4734,47 +4602,32 @@ int vb_op_nest_aggregate(int32_t precision, const float* x, int32_t B, int32_t H
     VB_CHECK(x && gamma && beta && out && B > 0 && H > 0 && W > 0 && C > 0, "vb_op_nest_aggregate: bad arguments");
     const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;
     VB_CHECK(pos == nullptr || (bh > 0 && bw > 0 && Ho % bh == 0 && Wo % bw == 0), "vb_op_nest_aggregate: the pooled map is not whole blocks");
-    const bool bf = precision == VB_PRECISION_BF16;
+    const bool bf = precision != VB_PRECISION_FP32;               // as with_precision picks the element type
     const int Cp = bf ? round_up(C, 64) : C;
     const size_t M = static_cast<size_t>(B) * H * W, Mo = static_cast<size_t>(B) * Ho * Wo;
     std::vector<float> xp(M * Cp, 0.f), gp(Cp, 0.f), bp(Cp, 0.f), oh(Mo * Cp), sh(Mo * (Cp / 64 + 1) * 2, 0.f);
     for (size_t r = 0; r < M; ++r) std::copy(x + r * C, x + (r + 1) * C, xp.begin() + r * Cp);
     std::copy(gamma, gamma + C, gp.begin());
     std::copy(beta, beta + C, bp.begin());
-    DevMem dX, dG, dB, dP, dO, dS, dSo, dY;
-    const float* g_d = upload<float>(dG, gp.data(), Cp);
-    const float* b_d = upload<float>(dB, bp.data(), Cp);
+    DevMem dX, dG, dB, dP, dO;
+    const Norm norm{upload<float>(dG, gp.data(), Cp), upload<float>(dB, bp.data(), Cp), C};
     const float* p_d = pos ? upload<float>(dP, pos, static_cast<size_t>(bh) * bw) : nullptr;
-    auto run = [&](auto tag) {
+    with_precision(precision, [&](vb_handle& h, auto tag) {
       using T = decltype(tag);
       const T* x_d = upload<T>(dX, xp.data(), M * Cp);
       dO.ensure(Mo * Cp * sizeof(T));
       T* o_d = static_cast<T*>(dO.p);
-      // vb_handle::nest_forward's aggregation tail, without the handle's arena and profiler
-      if constexpr (std::is_same<T, __nv_bfloat16>::value) {
-        dS.ensure(M * (Cp / 64) * 2 * sizeof(float));
-        dSo.ensure(Mo * (Cp / 64) * 2 * sizeof(float));
-        float* st = static_cast<float*>(dS.p);
-        float* so = static_cast<float*>(dSo.p);
-        NestPoolLn ln;
-        ln.stats = st; ln.parts = Cp / 64; ln.d = C; ln.eps = 1e-5f; ln.gamma = g_d; ln.beta = b_d;
-        timed(iters, elapsed_ms, [&] {
-          row_stats_bf16(x_d, Cp, st, static_cast<int>(M), Cp, 0);
-          nest_pool<T>(x_d, Cp, &ln, B, H, W, C, true, p_d, bh, bw, o_d, Cp, so, 0);
-        });
-        VB_CUDA(cudaMemcpy(sh.data(), so, Mo * (Cp / 64) * 2 * sizeof(float), cudaMemcpyDeviceToHost));
-      } else {
-        dY.ensure(M * Cp * sizeof(T));
-        T* y = static_cast<T*>(dY.p);
-        timed(iters, elapsed_ms, [&] {
-          layernorm<T>(x_d, Cp, g_d, b_d, y, Cp, static_cast<int>(M), C, 0, Cp, 1e-5f);
-          nest_pool<T>(y, Cp, nullptr, B, H, W, C, true, p_d, bh, bw, o_d, Cp, nullptr, 0);
-        });
-      }
+      float* so = nullptr;
+      timed(iters, elapsed_ms, [&] {
+        h.arena.reset();
+        float* st = h.row_stats(static_cast<long long>(M), Cp);
+        so = h.row_stats(static_cast<long long>(Mo), Cp);
+        h.ensure_stats<T>(x_d, Cp, st, static_cast<int>(M), 0);
+        h.nest_aggregate_tail<T>(x_d, st, B, H, W, C, Cp, norm, p_d, bh, bw, o_d, so, 0);
+      });
+      if (so) VB_CUDA(cudaMemcpy(sh.data(), so, Mo * (Cp / 64) * 2 * sizeof(float), cudaMemcpyDeviceToHost));
       download<T>(o_d, oh.data(), Mo * Cp);
-    };
-    if (bf) run(__nv_bfloat16());
-    else run(float());
+    });
     for (size_t r = 0; r < Mo; ++r) std::copy(oh.begin() + r * Cp, oh.begin() + r * Cp + C, out + r * C);
     if (bf && stats_out != nullptr) std::copy(sh.begin(), sh.begin() + Mo * (Cp / 64) * 2, stats_out);
   });
