@@ -142,6 +142,7 @@ struct GemmBf16 {
   CUtensorMap tmap_a, tmap_b;           // A, B (weights)
   CUtensorMap tmap_out = {}, tmap_res = {};   // bf16 out and res, which the epilogue stores and loads by TMA
   int M = 0, N = 0, K = 0;
+  int bn = 128;                         // tile width, 128 or 192 (gemm_bf16_plan's rule); the B tensor map's box follows it
   __nv_bfloat16* out = nullptr;         // [M, ldc] (fp32: stored straight from the accumulator registers)
   int ldc = 0;
   bool out_f32 = false;                 // `out` is float* (ldc in floats): plain / bias epilogue only

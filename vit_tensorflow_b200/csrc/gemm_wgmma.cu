@@ -7,23 +7,27 @@
 // to_out + residual (vit.py:62-69,101), MLP fc1+GELU / fc2 + residual (vit.py:38-44,102), CaiT to_q/to_kv
 // (cait.py:94-95) with LayerScale folded in (cait.py:48).
 //
-// Structure: persistent, one CTA of 384 threads per SM; CTA b computes the 128 x 128 output tiles b, b + gridDim.x, ...
-// of the flat tile order (n fastest).
+// Structure: persistent, one CTA of 384 threads per SM; CTA b computes the 128 x BN output tiles b, b + gridDim.x, ...
+// of the flat tile order (n fastest).  BN = 192 where it divides N and N >= 1536 (ViT-B/16's to_qkv and fc1), else 128
+// (gemm_bf16_plan states the rule): a 128 x 192 k-block brings 40 KB from L2 for 3.1 MFLOP against 32 KB for 2.1, and
+// each tile's fixed cost (epilogue, handover) is spread over 1.5x the work.  192 is the widest N at which one consumer
+// warpgroup still holds a whole tile's accumulators (2 x 96 fp32 registers per thread).
 //   producer        warpgroup 0 (its registers handed to the consumers by setmaxnreg).  Thread 0 streams the A (128 x 64)
-//                   and B (128 x 64) k-blocks of the CTA's tiles, one tile after the other, into a STAGES-deep ring of
-//                   128B-swizzled tiles (mbarrier full / empty pairs).  Warps 1-3 prepare each tile's epilogue operands
-//                   ahead of it, in the buffers of the consumer warpgroup that will run it: the residual tile (TMA load into
-//                   the warpgroup's output staging tile), the bias / ln_c1 / scale of its columns and the folded
-//                   LayerNorm's (rstd, -mu rstd) of its rows (mbarrier epi_full / epi_empty pair per warpgroup).
+//                   and B (BN x 64) k-blocks of the CTA's tiles, one tile after the other, into a STAGES-deep ring of
+//                   128B-swizzled tiles (mbarrier full / empty pairs; 4 x 32 KB at BN = 128, 3 x 40 KB at 192).  Warps 1-3
+//                   prepare each tile's epilogue operands ahead of it, in the buffers of the consumer warpgroup that will
+//                   run it: the residual tile (TMA loads into the warpgroup's output staging tile), the bias / ln_c1 /
+//                   scale of its columns and the folded LayerNorm's (rstd, -mu rstd) of its rows (mbarrier epi_full /
+//                   epi_empty pair per warpgroup).
 //   2 consumer warpgroups, ping-pong: warpgroup w computes the CTA's tiles i = w (mod 2), each whole: two wgmma
-//                   m64 x 128 x 16 per k16 step (rows 0-63 and 64-127 of the tile) into register accumulators, one k-block
+//                   m64 x BN x 16 per k16 step (rows 0-63 and 64-127 of the tile) into register accumulators, one k-block
 //                   in flight while the previous one's stage is released; then the epilogue from the accumulator
 //                   registers (bias / folded LayerNorm / GELU / LayerScale / residual, optional per-64-column row
 //                   statistics of the stored values), reading its operands from shared memory only.  A bf16 tile is
-//                   written into the staging tile (over its residual) and leaves by two TMA stores of 64 x 128; an fp32
-//                   tile is stored straight from registers.  Two named barriers pass the main loop from one warpgroup to
-//                   the other, so the main loops take turns on the tensor cores and one tile's epilogue runs under the
-//                   next tile's main loop.
+//                   written into the staging tile (over its residual) and leaves by one TMA store per 64 x 128 half; an
+//                   fp32 tile is stored straight from registers.  Two named barriers pass the main loop from one
+//                   warpgroup to the other, so the main loops take turns on the tensor cores and one tile's epilogue runs
+//                   under the next tile's main loop.
 #include "common.h"
 #include "kernels.cuh"
 #include "ptx.cuh"
@@ -33,20 +37,33 @@ namespace vb {
 namespace {
 
 constexpr int BM = 128;
-constexpr int BN = 128;
 constexpr int BK = 64;             // 64 bf16 = 128 bytes = one swizzle row
 constexpr int THREADS = 384;
 constexpr int A_BYTES = BM * BK * 2;
-constexpr int B_BYTES = BN * BK * 2;
-constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr int STAGES = 4;          // 4 x 32 KB ring + 2 x 32 KB output staging of the 227 KB a CTA may use
 constexpr int HALF_BYTES = BM * 64 * 2;      // 64 columns of an output tile: 128 rows of 128 bytes, 128B-swizzled
-constexpr int STG_BYTES = 2 * HALF_BYTES;    // per consumer warpgroup: its bf16 output tile (and residual tile before it)
-constexpr int PARAM_FLOATS = 3 * BN + 2 * BM;   // per consumer warpgroup: bias, ln_c1, scale of its tile's columns; the
-                                                // folded LayerNorm's rstd and -mu rstd of its rows
 constexpr int EPI_THREADS = 96;    // producer warps 1-3
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * STG_BYTES + 256 /*barriers*/ + 2 * PARAM_FLOATS * 4 + 1024 /*align*/;
-static_assert(SMEM_BYTES <= 227 * 1024, "ring does not fit in shared memory");
+
+// Everything that follows the tile width BN (128 or 192).
+template <int BN>
+struct Tile {
+  static constexpr int B_BYTES = BN * BK * 2;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  // of the 227 KB a CTA may use: 4 x 32 KB ring + 2 x 32 KB output staging, or 3 x 40 KB + 2 x 48 KB.  Both rings hold
+  // about the same tensor-core time (8.4 and 9.4 MFLOP), and a stage is refilled while the two after it are computed.
+  static constexpr int STAGES = BN == 128 ? 4 : 3;
+  static constexpr int STG_BYTES = BN / 64 * HALF_BYTES;   // per consumer warpgroup: its bf16 output tile (and residual
+                                                          // tile before it), one 128B-swizzled box per 64-column half
+  static constexpr int PARAM_FLOATS = 3 * BN + 2 * BM;    // per consumer warpgroup: bias, ln_c1, scale of its tile's
+                                                          // columns; the folded LayerNorm's rstd and -mu rstd of its rows
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * STG_BYTES + 256 /*barriers*/ + 2 * PARAM_FLOATS * 4 + 1024 /*align*/;
+  static_assert(SMEM_BYTES <= 227 * 1024, "ring does not fit in shared memory");
+};
+// setmaxnreg: the launch gives every thread 168 registers (65,536 / 384, rounded down to a multiple of 8); the producer
+// warpgroup hands what it does not need to the consumers, whose accumulators take BN fp32 registers per thread.  At BN = 192
+// the 192 accumulators and the epilogue's state fit in 232 without spilling; the producer's warps need 40.
+constexpr int PRODUCER_REGS = 40;
+constexpr int CONSUMER_REGS = 232;
+static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= 168 * THREADS, "setmaxnreg exceeds the CTA's registers");
 
 // Exact-erf GELU (vit.py:34), written as  gelu(x) = x/2 - |x| * (E(|x|) - 1/2),  E(a) = erfc(a/sqrt2) / 2  (for x > 0
 // this is x - x E, for x < 0 it is x E), with E evaluated as 2^q(a): q is a degree-5 polynomial (weighted minimax fit
@@ -69,6 +86,7 @@ __device__ __forceinline__ float gelu_erf(float x) {
 __device__ __forceinline__ float hard_swish(float x) { return __fdiv_rn(x * fminf(fmaxf(x + 3.0f, 0.0f), 6.0f), 6.0f); }
 
 // Advance a ring position (stage, phase) by n k-blocks.
+template <int STAGES>
 __device__ __forceinline__ void ring_advance(int& stage, uint32_t& phase, int n) {
   stage += n % STAGES;
   phase ^= static_cast<uint32_t>(n / STAGES) & 1u;
@@ -76,7 +94,7 @@ __device__ __forceinline__ void ring_advance(int& stage, uint32_t& phase, int n)
 }
 
 // EPI: 0 = no per-column addend, 1 = + bias[n], 2 = folded LayerNorm (c1 = ln_c1, c2 = bias)
-template <int ACT, bool RES, int EPI, bool OF32>
+template <int BN, int ACT, bool RES, int EPI, bool OF32>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                  const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_res, int M, int N, int K,
@@ -84,6 +102,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
                  const float* __restrict__ ln_c1, const float2* ln_stats, int ln_parts, float ln_inv_d, float ln_eps,
                  float2* __restrict__ stats_out) {
   static_assert(!OF32 || (ACT == ACT_NONE && !RES && EPI != 2), "fp32 output: plain / bias epilogue only");
+  static_assert(BN == 128 || BN == 192, "tile width");
+  using T = Tile<BN>;
+  constexpr int STAGES = T::STAGES, STAGE_BYTES = T::STAGE_BYTES, STG_BYTES = T::STG_BYTES, PARAM_FLOATS = T::PARAM_FLOATS;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t stg_base = smem_base + STAGES * STAGE_BYTES;     // consumer warpgroup w's staging tile at + w STG_BYTES
@@ -125,7 +146,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 
   if (wg == 0) {
     // ===================================================================== TMA producer
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<PRODUCER_REGS>();
     if (tid == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -154,7 +175,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         mbar_wait(epi_empty(w), ((i >> 1) & 1) ^ 1);
         if (RES && pt == 0) {
           // rows >= M are zero-filled; N % 64 == 0, so a 64-column half is entirely in or out
-          const int halves = N - n0 >= BN ? 2 : 1;
+          const int halves = (N - n0 >= BN ? BN : N - n0) / 64;
           const uint32_t stg = stg_base + w * STG_BYTES;
           fence_proxy_async_smem();
           mbar_expect_tx(epi_full(w), halves * HALF_BYTES);
@@ -201,7 +222,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   }
 
   // ===================================================================== consumers
-  setmaxnreg_inc<232>();
+  setmaxnreg_inc<CONSUMER_REGS>();
   const int cw = wg - 1;                                           // takes the CTA's tiles i = cw (mod 2)
   const int warp = tid >> 5, lane = tid & 31;
   const int col_t = 2 * (lane & 3);
@@ -215,7 +236,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
                                                                    // 64 hm + 8 h, q = 2 hm + h below; all = lane / 4 (mod 8)
   int stage = 0;
   uint32_t phase = 0, epi_phase = 0;
-  ring_advance(stage, phase, cw * num_kb);                         // warpgroup 1 starts after tile 0's k-blocks
+  ring_advance<STAGES>(stage, phase, cw * num_kb);                 // warpgroup 1 starts after tile 0's k-blocks
 
   for (long long t = blockIdx.x + static_cast<long long>(cw) * gridDim.x; t < tiles; t += 2LL * gridDim.x) {
     const int n0 = static_cast<int>(t % n_tiles) * BN;
@@ -223,9 +244,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 
     // the CTA's first tile starts at once
     if (cw == 1 || t != blockIdx.x) named_bar_sync(my_turn, 256);
-    float acc[2][64];                                              // [64-row half of the tile][wgmma fragment]
+    float acc[2][BN / 2];                                          // [64-row half of the tile][wgmma fragment]
 #pragma unroll
-    for (int i = 0; i < 64; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+    for (int i = 0; i < BN / 2; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
     wgmma_fence_operand(acc[0]);
     wgmma_fence_operand(acc[1]);
     for (int kb = 0; kb < num_kb; ++kb) {
@@ -239,8 +260,13 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         // advance 16 bf16 = 32 bytes along K inside the 128-byte swizzle row: +2 in the 16-byte address field; rows 64-127
         // start 64 x 128 bytes = +512 further
         const uint32_t acc_on = (kb | k) != 0 ? 1u : 0u;
-        wgmma_m64n128k16_bf16(acc[0], da + 2u * k, db + 2u * k, acc_on);
-        wgmma_m64n128k16_bf16(acc[1], da + 512u + 2u * k, db + 2u * k, acc_on);
+        if constexpr (BN == 128) {
+          wgmma_m64n128k16_bf16(acc[0], da + 2u * k, db + 2u * k, acc_on);
+          wgmma_m64n128k16_bf16(acc[1], da + 512u + 2u * k, db + 2u * k, acc_on);
+        } else {
+          wgmma_m64n192k16_bf16(acc[0], da + 2u * k, db + 2u * k, acc_on);
+          wgmma_m64n192k16_bf16(acc[1], da + 512u + 2u * k, db + 2u * k, acc_on);
+        }
       }
       wgmma_commit();
       wgmma_wait<1>();                                             // the previous k-block's products have retired
@@ -252,7 +278,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     wgmma_fence_operand(acc[0]);
     wgmma_fence_operand(acc[1]);
     if (tid == 0) mbar_arrive(empty_bar(stage == 0 ? STAGES - 1 : stage - 1));
-    ring_advance(stage, phase, num_kb);                            // skip the other warpgroup's tile
+    ring_advance<STAGES>(stage, phase, num_kb);                    // skip the other warpgroup's tile
 
     // =================================================================== epilogue, 64-column chunks
     mbar_wait(epi_full(cw), epi_phase);                            // operands (and residual tile) staged by warps 1-3
@@ -336,16 +362,19 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     if (tid == 0) {
       if (!OF32) {
         const uint32_t s = stg_base + cw * STG_BYTES;
-        tma_store_2d(&tmap_out, s, n0, m0);
-        if (n0 + 64 < N) tma_store_2d(&tmap_out, s + HALF_BYTES, n0 + 64, m0);
+#pragma unroll
+        for (int c = 0; c < BN / 64; ++c)
+          if (n0 + 64 * c < N) tma_store_2d(&tmap_out, s + c * HALF_BYTES, n0 + 64 * c, m0);
         bulk_commit_group();
-        bulk_wait_group_read<0>();
+        // the CTA's stores are complete before it exits (a dependent kernel's griddepcontrol.wait waits for the grid's
+        // exit only): after its last tile the warpgroup waits for the store's writes, not just its reads.  (Waiting after
+        // the loop instead costs the 192-wide instances their registers: ptxas then spills the accumulators.)
+        if (t + 2LL * gridDim.x < tiles) bulk_wait_group_read<0>();
+        else bulk_wait_group<0>();
       }
       mbar_arrive(epi_empty(cw));
     }
   }
-  // the CTA's stores are complete before it exits: a dependent kernel's griddepcontrol.wait waits for the grid's exit only
-  if (!OF32 && tid == 0) bulk_wait_group<0>();
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -363,16 +392,17 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-template <int ACT, bool RES, int EPI, bool OF32 = false>
+template <int BN, int ACT, bool RES, int EPI, bool OF32 = false>
 void launch(const GemmBf16& g, cudaStream_t stream) {
-  auto kern = gemm_bf16_kernel<ACT, RES, EPI, OF32>;
+  auto kern = gemm_bf16_kernel<BN, ACT, RES, EPI, OF32>;
+  constexpr int smem = Tile<BN>::SMEM_BYTES;
   static unsigned long long seen[4] = {0, 0, 0, 0};
-  if (first_use_on_this_device(seen)) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+  if (first_use_on_this_device(seen)) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   const long long tiles = static_cast<long long>((g.N + BN - 1) / BN) * ((g.M + BM - 1) / BM);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(static_cast<unsigned>(tiles < sm_count() ? tiles : sm_count()));
   cfg.blockDim = dim3(THREADS);
-  cfg.dynamicSmemBytes = SMEM_BYTES;
+  cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
@@ -384,6 +414,25 @@ void launch(const GemmBf16& g, cudaStream_t stream) {
                              reinterpret_cast<const float2*>(g.ln_stats), g.ln_parts, g.ln_inv_d, g.ln_eps,
                              reinterpret_cast<float2*>(g.stats_out)));
   count_launch();
+}
+
+template <int BN>
+void dispatch(const GemmBf16& g, bool res, int epi, cudaStream_t stream) {
+  if constexpr (BN == 128) {                                          // fp32 output: 128-wide only (gemm_bf16_plan)
+    if (g.out_f32) {
+      if (epi == 0) return launch<BN, ACT_NONE, false, 0, true>(g, stream);
+      return launch<BN, ACT_NONE, false, 1, true>(g, stream);
+    }
+  }
+  VB_CHECK(!g.out_f32, "gemm_bf16: fp32 output runs the 128-wide tile only");
+#define VB_GEMM_CASE(A, R, E) if (g.act == A && res == R && epi == E) return launch<BN, A, R, E>(g, stream)
+  VB_GEMM_CASE(ACT_NONE, false, 0); VB_GEMM_CASE(ACT_NONE, false, 1); VB_GEMM_CASE(ACT_NONE, false, 2);
+  VB_GEMM_CASE(ACT_GELU, false, 0); VB_GEMM_CASE(ACT_GELU, false, 1); VB_GEMM_CASE(ACT_GELU, false, 2);
+  VB_GEMM_CASE(ACT_NONE, true, 0);  VB_GEMM_CASE(ACT_NONE, true, 1);  VB_GEMM_CASE(ACT_NONE, true, 2);
+  VB_GEMM_CASE(ACT_GELU, true, 0);  VB_GEMM_CASE(ACT_GELU, true, 1);  VB_GEMM_CASE(ACT_GELU, true, 2);
+  VB_GEMM_CASE(ACT_HSWISH, false, 1);                                  // LeViT MLP fc1 (levit.py:53-54)
+#undef VB_GEMM_CASE
+  VB_CHECK(false, "gemm_bf16: no kernel instance for this epilogue (activation " + std::to_string(g.act) + ")");
 }
 
 }  // namespace
@@ -442,9 +491,14 @@ GemmBf16 gemm_bf16_plan(const __nv_bfloat16* A, int lda, const __nv_bfloat16* Wt
   g.M = M; g.N = N; g.K = K;
   g.bias = bias; g.scale = scale; g.res = res; g.ldr = ldr; g.act = act;
   g.out = out; g.ldc = ldc; g.out_f32 = out_f32;
+  // The wider tile where it covers N exactly (no half-empty last column of tiles) in at least 8 column tiles.  Measured on
+  // an H100 at ViT-B/16's shapes, it takes N = 2304 / 3072 at K = 768 from 0.320 / 0.448 ms to 0.281 / 0.423-0.433, but
+  // N = 768 (4 column tiles) runs no faster at K = 768 and 3 % slower at K = 3072, so those keep the 128-wide tile.
+  // An fp32 output (the classifier heads) keeps it too: its 64-bit row addresses next to 192 accumulators make ptxas spill.
+  g.bn = N % 192 == 0 && N >= 8 * 192 && !out_f32 ? 192 : 128;
   g.tmap_a = make_tmap_2d(A, K, M, static_cast<uint64_t>(lda) * 2, BK, BM);
   // b_rows: rows of Wt that exist (< N when the output is column-padded: TMA zero-fills the rest instead of reading on)
-  g.tmap_b = make_tmap_2d(Wt, K, b_rows > 0 ? b_rows : N, static_cast<uint64_t>(ldw) * 2, BK, BN);
+  g.tmap_b = make_tmap_2d(Wt, K, b_rows > 0 ? b_rows : N, static_cast<uint64_t>(ldw) * 2, BK, g.bn);
   // bf16 output and residual tiles move as 64-column halves; TMA clips the store and zero-fills the load past row M
   if (!out_f32) g.tmap_out = make_tmap_2d(out, N, M, static_cast<uint64_t>(ldc) * 2, 64, BM);
   if (res != nullptr) g.tmap_res = make_tmap_2d(res, N, M, static_cast<uint64_t>(ldr) * 2, 64, BM);
@@ -455,19 +509,11 @@ void gemm_bf16_run(const GemmBf16& g, cudaStream_t stream) {
   const bool res = g.res != nullptr;
   const int epi = g.ln_c1 != nullptr ? 2 : g.bias != nullptr ? 1 : 0;
   VB_CHECK(epi != 2 || (g.bias != nullptr && g.ln_stats != nullptr && g.ln_parts > 0), "folded LayerNorm needs c1, c2 and the row statistics");
-  if (g.out_f32) {
+  if (g.out_f32)
     VB_CHECK(g.act == ACT_NONE && !res && epi != 2 && g.scale == nullptr && g.stats_out == nullptr, "fp32-output GEMM: plain or bias epilogue only");
-    if (epi == 0) return launch<ACT_NONE, false, 0, true>(g, stream);
-    return launch<ACT_NONE, false, 1, true>(g, stream);
-  }
-#define VB_GEMM_CASE(A, R, E) if (g.act == A && res == R && epi == E) return launch<A, R, E>(g, stream)
-  VB_GEMM_CASE(ACT_NONE, false, 0); VB_GEMM_CASE(ACT_NONE, false, 1); VB_GEMM_CASE(ACT_NONE, false, 2);
-  VB_GEMM_CASE(ACT_GELU, false, 0); VB_GEMM_CASE(ACT_GELU, false, 1); VB_GEMM_CASE(ACT_GELU, false, 2);
-  VB_GEMM_CASE(ACT_NONE, true, 0);  VB_GEMM_CASE(ACT_NONE, true, 1);  VB_GEMM_CASE(ACT_NONE, true, 2);
-  VB_GEMM_CASE(ACT_GELU, true, 0);  VB_GEMM_CASE(ACT_GELU, true, 1);  VB_GEMM_CASE(ACT_GELU, true, 2);
-  VB_GEMM_CASE(ACT_HSWISH, false, 1);                                  // LeViT MLP fc1 (levit.py:53-54)
-#undef VB_GEMM_CASE
-  VB_CHECK(false, "gemm_bf16: no kernel instance for this epilogue (activation " + std::to_string(g.act) + ")");
+  if (g.bn == 192) return dispatch<192>(g, res, epi, stream);
+  VB_CHECK(g.bn == 128, "gemm_bf16: tile width " + std::to_string(g.bn) + " has no kernel");
+  dispatch<128>(g, res, epi, stream);
 }
 
 }  // namespace vb
