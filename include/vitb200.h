@@ -47,7 +47,7 @@ typedef struct vb_handle vb_handle;
 enum { VB_KIND_VIT = 0, VB_KIND_DEEPVIT = 1, VB_KIND_CAIT = 2, VB_KIND_CROSSVIT = 3, VB_KIND_PARALLEL_VIT = 4,
        VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6, VB_KIND_CCT = 7, VB_KIND_LEVIT = 8,
        VB_KIND_CVT = 9, VB_KIND_TWINS_SVT = 10, VB_KIND_CROSSFORMER = 11, VB_KIND_NEST = 12, VB_KIND_REGIONVIT = 13,
-       VB_KIND_ATS_VIT = 14, VB_KIND_SMALL_DATASET_VIT = 15 };
+       VB_KIND_ATS_VIT = 14, VB_KIND_SMALL_DATASET_VIT = 15, VB_KIND_MOBILEVIT = 16 };
 enum { VB_CCT_POS_SINE = 0, VB_CCT_POS_LEARNABLE = 1, VB_CCT_POS_NONE = 2 };   /* cct.py:233-234,250-256 */
 enum { VB_PRECISION_FP32 = 0, VB_PRECISION_BF16 = 1 };
 enum { VB_POOL_CLS = 0, VB_POOL_MEAN = 1 };
@@ -530,7 +530,8 @@ VB_API int vb_op_ln_linear(const float* x, const float* gamma, const float* beta
  *   wt      the weight in its K-major packed form [b_rows, ldw] (b_rows = 0: N); rows [b_rows, N) read as zero.
  *   out     [M, ldc]: the whole buffer is uploaded (rounded to bf16 unless out_f32) and downloaded again, so columns the
  *           GEMM does not write come back unchanged.  out_f32 != 0: fp32 output, plain or bias epilogue only.
- *   epi     (+bias[N]) -> exact-erf GELU (gelu != 0) -> (*scale[N]) -> (+res[m, n]).  res == out: the residual is the
+ *   epi     (+bias[N]) -> activation -> (*scale[N]) -> (+res[m, n]); gelu: 0 none, 3 SiLU (with a bias or the folded
+ *           LayerNorm), any other value exact-erf GELU (as every nonzero value meant before SiLU).  res == out: the residual is the
  *           output region itself (in place, ldr must equal ldc); otherwise res is a separate [M, ldr] buffer at column 0.
  *   ln_stats, ln_c1: folded LayerNorm of the A rows (as vb_op_ln_linear runs it): wt must hold gamma-scaled weights, bias the
  *           c2 = beta.W + bias term, ln_c1[N] the row sums of wt, ln_stats [K/64][M] (sum, sumsq) float pairs of the rows.
@@ -619,6 +620,56 @@ VB_API int vb_op_r2l_attention(int32_t precision, const float* qkv, int32_t ld, 
 VB_API int vb_op_nest_aggregate(int32_t precision, const float* x, int32_t B, int32_t H, int32_t W, int32_t C, const float* gamma,
                                 const float* beta, const float* pos, int32_t bh, int32_t bw, float* out, float* stats_out,
                                 int32_t iters, float* elapsed_ms);
+
+/* MobileViT (mobile_vit.py:209-271), appended within ABI 7.  conv1: Conv_NxN_BN(channels[0], 3, stride 2); stem: MV2 blocks 0-3;
+ * trunk: per stage s an MV2 block (4 + s, stride 2) and a MobileViTBlock(dims[s], depths[s], channels[5 + 2 s], kernel_size,
+ * (ph, pw), mlp dims[s] * (2, 4, 4)[s]); to_logits: Conv_NxN_BN(last_dim, 1), the mean over pixels, a bias-free Dense.  Conv_NxN_BN
+ * is a bias-free SAME Conv2D, BatchNormalization (eps 1e-5, moving statistics) and SiLU.  An MV2 block (:130-170) is [1x1 conv + BN
+ * + SiLU when mv2_expand], 3x3 depthwise conv (stride mv2_stride, SAME) + BN + SiLU, 1x1 conv + BN, plus its input when
+ * mv2_residual; mv2_in / mv2_hidden / mv2_out are its widths as the host computed them (hidden = int(dim_in * expansion) of the
+ * reference's dim_in; mv2_hidden == mv2_in without the expand conv).  A MobileViTBlock (:173-206) runs k x k and 1x1 Conv_NxN_BN to
+ * dims[s], then depths[s] pre-norm layers (LayerNormalization eps 1e-3; attention of 4 heads of 8 within each of the ph * pw
+ * patch positions, 'b (h ph) (w pw) d -> b (ph pw) (h w) d', scale 8^-0.5, bias-free to_qkv, to_out with bias; MLP Dense, SiLU,
+ * Dense), a 1x1 Conv_NxN_BN back to channels[5 + 2 s], the concat with the block's input and a k x k Conv_NxN_BN.  Every trunk map
+ * (1/8, 1/16 and 1/32 of the image under SAME's ceil) must be divisible by (ph, pw). */
+#define VB_MOBILEVIT_MV2 7
+typedef struct vb_mobilevit_config {
+  int32_t struct_size;            /* sizeof(vb_mobilevit_config) */
+  int32_t channels[10];           /* the reference's channels[0..9] */
+  int32_t last_dim;               /* channels[-1] */
+  int32_t dims[3], depths[3];
+  int32_t kernel_size, ph, pw;
+  int32_t mv2_in[VB_MOBILEVIT_MV2], mv2_hidden[VB_MOBILEVIT_MV2], mv2_out[VB_MOBILEVIT_MV2], mv2_stride[VB_MOBILEVIT_MV2];
+  int32_t mv2_expand[VB_MOBILEVIT_MV2], mv2_residual[VB_MOBILEVIT_MV2];   /* 0 / 1 */
+} vb_mobilevit_config;
+
+/* MobileViT.__init__: `base` supplies precision, channels (3), num_classes and max_batch; its kind must be VB_KIND_MOBILEVIT and
+ * its other fields are ignored.  Weights (SURVEY.md App. B) are named by the reference's attribute paths; BN stands for the
+ * BatchNormalization leaves .gamma / .beta / .moving_mean / .moving_variance [width]:
+ *   conv1.layers.0.kernel [3, 3, 3, channels[0]], conv1.layers.1 BN
+ *   MV2 block i (stem.{i}.conv for i < 4, trunk.{i - 4}.0.conv after), with expand: .0.kernel [1, 1, in, hidden], .1 BN,
+ *     .3.kernel [3, 3, 1, hidden], .4 BN, .6.kernel [1, 1, hidden, out], .7 BN; without: .0.kernel [3, 3, 1, hidden], .1 BN,
+ *     .3.kernel [1, 1, hidden, out], .4 BN
+ *   trunk.{s}.1.conv1.layers.0.kernel [k, k, channels[4 + 2 s], c], .1 BN (c = channels[5 + 2 s]); conv2 [1, 1, c, dims[s]];
+ *     conv3 [1, 1, dims[s], c]; conv4 [k, k, c + channels[4 + 2 s], c]; each with its .layers.1 BN
+ *   trunk.{s}.1.transformer.layers.{l}.0.norm.gamma / .beta, .0.fn.to_qkv.kernel [dims[s], 96], .0.fn.to_out.0.kernel [32,
+ *     dims[s]] / .bias, .1.norm.gamma / .beta, .1.fn.net.0.kernel [dims[s], mlp] / .bias, .1.fn.net.3.kernel [mlp, dims[s]] / .bias
+ *   to_logits.0.layers.0.kernel [1, 1, channels[9], last_dim], to_logits.0.layers.1 BN, to_logits.2.kernel [last_dim, num_classes]
+ * vb_forward only: the stage entries and vb_forward_distill refuse the handle. */
+VB_API int vb_create_mobilevit(const vb_config* base, const vb_mobilevit_config* mv, int device, vb_handle** out);
+/* MobileViT's MV2 depthwise step as the engine runs it: x [B, H, W, C] NHWC; w the depthwise kernel [3, 3, 1, C]; bn [4, C] =
+ * gamma, beta, moving_mean, moving_variance (folded on the host as vb_finalize folds it); out [B, ceil(H/s), ceil(W/s), Cp] =
+ * SiLU(BN(dw(x))) with TF SAME padding at stride 1 or 2, Cp = C in fp32 and C rounded up to a multiple of 64 in bf16 (x in bf16
+ * at that pitch), columns [C, Cp) as the kernel wrote them.  All buffers are host memory. */
+VB_API int vb_op_mv2_dwconv(int32_t precision, const float* x, int32_t B, int32_t H, int32_t W, int32_t C, int32_t stride, const float* w,
+                            const float* bn, float* out, int32_t iters, float* elapsed_ms);
+/* MobileViT's attention (mobile_vit.py:95-107,196-199) as the engine runs it: qkv [B*H*W, ld] the fused q|k|v rows of a
+ * pixel-major [B, H, W] map (head h at columns h*dh, HD + h*dh, 2 HD + h*dh, HD = heads * dh); the pixels (y, x) with the same
+ * (y % ph, x % pw) attend together, softmax(q k^T * scale) v; out [B*H*W, ldo] pixel-major, uploaded and downloaded whole.  bf16
+ * with dh 32 or 64 runs the windowed flash kernel on the rows in place; fp32 and any other shape permute the rows, run the
+ * materialised-scores path and permute back (vb_last_attention_path tells which). */
+VB_API int vb_op_patch_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t H, int32_t W, int32_t ph, int32_t pw,
+                                 int32_t heads, int32_t dh, float scale, float* out, int32_t ldo, int32_t iters, float* elapsed_ms);
 
 /* Row softmax of fp32 scores into bf16 probabilities (the T2T attention): p[r, j] = softmax_j(s[r, j] * scale) for j < n,
  * p[r, n..npad) = 0.  s [rows, lds], p [rows, ldp] (uploaded and downloaded whole); n <= npad <= ldp. */

@@ -13,7 +13,7 @@ LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "libvitb200.so")
 
 KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6, "cct": 7, "levit": 8,
         "cvt": 9, "twins_svt": 10, "crossformer": 11, "nest": 12, "regionvit": 13, "ats_vit": 14,
-        "small_dataset_vit": 15}
+        "small_dataset_vit": 15, "mobilevit": 16}
 PRECISION = {"fp32": 0, "float32": 0, "bf16": 1, "bfloat16": 1}
 MEM_HOST, MEM_DEVICE = 0, 1
 ABI_VERSION = 7                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
@@ -91,6 +91,15 @@ class VbAtsVitConfig(C.Structure):
     _fields_ = [("struct_size", C.c_int32), ("max_tokens_per_depth", C.c_int32 * ATS_MAX_DEPTH)]
 
 
+MOBILEVIT_MV2 = 7                                    # VB_MOBILEVIT_MV2
+
+
+class VbMobilevitConfig(C.Structure):
+    _fields_ = [("struct_size", C.c_int32), ("channels", C.c_int32 * 10), ("last_dim", C.c_int32), ("dims", C.c_int32 * 3),
+                ("depths", C.c_int32 * 3), ("kernel_size", C.c_int32), ("ph", C.c_int32), ("pw", C.c_int32)] + \
+               [(f, C.c_int32 * MOBILEVIT_MV2) for f in ("mv2_in", "mv2_hidden", "mv2_out", "mv2_stride", "mv2_expand", "mv2_residual")]
+
+
 class VbError(RuntimeError):
     pass
 
@@ -109,6 +118,9 @@ SIGNATURES = {
     "vb_create_nest": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbNestConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_regionvit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbRegionvitConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_ats_vit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbAtsVitConfig), C.c_int, C.POINTER(C.c_void_p)]),
+    "vb_create_mobilevit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbMobilevitConfig), C.c_int, C.POINTER(C.c_void_p)]),
+    "vb_op_mv2_dwconv": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p] * 3 + [C.c_int32, _f32p]),
+    "vb_op_patch_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 8 + [C.c_float, C.c_void_p, C.c_int32, C.c_int32, _f32p]),
     "vb_ats_set_seed": (C.c_int, [C.c_void_p, C.c_uint64]),
     "vb_forward_ats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p]),
@@ -256,11 +268,11 @@ def op_ln_linear(x, gamma, beta, w, bias=None, gelu=False, iters=0):
 
 
 def op_gemm(a, wt, N, K, out, bias=None, scale=None, gelu=False, res=None, out_off=0, out_f32=False, ln_stats=None, ln_c1=None,
-            want_stats=False, iters=0):
+            want_stats=False, iters=0, silu=False):
     """The bf16 wgmma GEMM in the engine's operand layouts (vb_op_gemm): a [M, lda], wt K-major [b_rows, ldw] (b_rows < N: the
     missing rows read as zero), out [M, ldc] initial contents (columns [out_off, out_off + N) are written); res: None, a
-    separate [M, ldr] array, or the string "out" for the in-place residual.  Returns (out [M, ldc], stats [N/64, M, 2] or None,
-    ms per launch or None)."""
+    separate [M, ldr] array, or the string "out" for the in-place residual; silu: the SiLU epilogue instead of GELU.  Returns (out
+    [M, ldc], stats [N/64, M, 2] or None, ms per launch or None)."""
     a, wt, bias, scale, ln_stats, ln_c1 = map(_f32, (a, wt, bias, scale, ln_stats, ln_c1))
     out = np.array(out, dtype=np.float32, order="C", copy=True)
     M, lda = a.shape
@@ -274,7 +286,8 @@ def op_gemm(a, wt, N, K, out, bias=None, scale=None, gelu=False, res=None, out_o
         res_p, ldr = _ptr(res), (0 if res is None else res.shape[1])
     stats = np.empty((N // 64, M, 2), np.float32) if want_stats else None
     ms = C.c_float(0)
-    check(load().vb_op_gemm(_ptr(a), lda, _ptr(wt), ldw, b_rows, _ptr(bias), _ptr(scale), int(bool(gelu)), res_p, ldr, _ptr(ln_stats),
+    act = 3 if silu else int(bool(gelu))                 # Act: ACT_SILU = 3, ACT_GELU = 1
+    check(load().vb_op_gemm(_ptr(a), lda, _ptr(wt), ldw, b_rows, _ptr(bias), _ptr(scale), act, res_p, ldr, _ptr(ln_stats),
                             _ptr(ln_c1), _ptr(out), ldc, out_off, int(bool(out_f32)), _ptr(stats), M, N, K, iters, C.byref(ms)))
     return out, stats, (ms.value if iters > 0 else None)
 
@@ -359,6 +372,32 @@ def op_block_attention(qkv, H, W, bh, bw, heads, dh, precision="bf16", iters=0):
     ms = C.c_float(0)
     check(load().vb_op_block_attention(PRECISION[precision], _ptr(qkv), ld, B, H, W, bh, bw, heads, dh, _ptr(out), heads * dh, iters,
                                        C.byref(ms)))
+    return out, (ms.value if iters > 0 else None)
+
+
+def op_mv2_dwconv(x, w, bn, stride, precision="bf16", iters=0):
+    """MobileViT's MV2 depthwise step (vb_op_mv2_dwconv): x [B, H, W, C], the depthwise kernel [3, 3, 1, C], the BatchNormalization
+    [4, C] (gamma, beta, moving_mean, moving_variance).  Returns (out [B, ceil(H/s), ceil(W/s), Cp] with Cp = C (fp32) or C rounded
+    up to a multiple of 64 (bf16), ms or None)."""
+    x, w, bn = map(_f32, (x, w, bn))
+    B, H, W, Cc = x.shape
+    cp = Cc if PRECISION[precision] == 0 else -(-Cc // 64) * 64
+    out = np.empty((B, -(-H // stride), -(-W // stride), cp), np.float32)
+    ms = C.c_float(0)
+    check(load().vb_op_mv2_dwconv(PRECISION[precision], _ptr(x), B, H, W, Cc, stride, _ptr(w), _ptr(bn), _ptr(out), iters, C.byref(ms)))
+    return out, (ms.value if iters > 0 else None)
+
+
+def op_patch_attention(qkv, H, W, ph, pw, heads, dh, scale=0.0, precision="bf16", iters=0):
+    """MobileViT's attention (vb_op_patch_attention): qkv [B*H*W, ld] fused q|k|v rows of a pixel-major map; the pixels of one
+    patch position (y % ph, x % pw) attend together.  Returns (out [B*H*W, heads*dh] pixel-major, ms or None)."""
+    qkv = _f32(qkv)
+    rows, ld = qkv.shape
+    B = rows // (H * W)
+    out = np.zeros((rows, heads * dh), np.float32)
+    ms = C.c_float(0)
+    check(load().vb_op_patch_attention(PRECISION[precision], _ptr(qkv), ld, B, H, W, ph, pw, heads, dh, float(scale), _ptr(out), heads * dh,
+                                       iters, C.byref(ms)))
     return out, (ms.value if iters > 0 else None)
 
 

@@ -33,8 +33,9 @@ bool attention_fast(const T* q, int ldq, const T* k, int ldk, const T* v, int ld
                     const float* ln_beta, cudaStream_t s, float scale = 0.f, const PosBias* pb = nullptr,
                     const Window* win = nullptr);
 
-// NesT's block attention (nest.py:93-109) on the windowed flash kernel: the win.count windows (contiguous p x width() blocks of
-// a pixel-major map, Window in common.h) each attend within themselves; q, k and v at columns [0, HD), [HD, 2 HD), [2 HD, 3 HD)
+// NesT's block attention (nest.py:93-109) and MobileViT's patch-position attention (mobile_vit.py:196-199) on the windowed flash
+// kernel: the win.count windows (p x width() blocks of a pixel-major map, contiguous or dilated, Window in common.h) each attend
+// within themselves; q, k and v at columns [0, HD), [HD, 2 HD), [2 HD, 3 HD)
 // of the fused rows qkv [.., ld] (HD = heads * dh), the output rows written pixel-major to out [.., ldo] (may be qkv itself: each
 // CTA overwrites only its own query rows' q columns).  dh 32 or 64; false for any other shape, which the caller then runs on
 // the materialised-scores path.  bf16 only.

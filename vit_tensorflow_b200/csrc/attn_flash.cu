@@ -27,7 +27,8 @@
 //
 // WIN alone at head width 32 (NesT's block attention, nest.py:93-109; attention_block below): the same windowed form over
 // rectangular bh x bw blocks (Window::pw), reached only through attention_block.  NesT's 14 x 14 blocks of 196 tokens take four
-// query tiles and four key blocks each.
+// query tiles and four key blocks each.  MobileViT's patch-position groups (mobile_vit.py:196-199) are dilated rectangular windows
+// of the same form: the kernel reads every row through Window::row.
 //
 // RegionViT's regional-to-local attention (attn_r2l_kernel, attention_r2l below) is a kernel of its own with the same tiles and
 // online softmax: each window attends together with one regional row from elsewhere in the rows, under a per-head window table.
@@ -758,7 +759,7 @@ bool attention_block(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* out, int l
                      const Window& win) {
   const int n = win.p * win.width();
   const long long B = static_cast<long long>(win.count);
-  if ((dh != 32 && dh != 64) || win.dilated || n <= 0 || B <= 0) return false;
+  if ((dh != 32 && dh != 64) || n <= 0 || B <= 0) return false;
   if ((ld % 8) || (ldo % 2) || ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(out)) % 16)) return false;
   const long long blocks = B * heads * ((n + FQ - 1) / FQ);
   if (blocks > 0x7fffffffLL) return false;

@@ -104,10 +104,10 @@ __device__ __forceinline__ float gelu_exact(float x) { return 0.5f * x * (1.0f +
 //   contiguous blocks (dilated == 0; Twins-SVT twins_svt.py:141, CrossFormer's short attention crossformer.py:144, NesT's
 //   rectangular blocks nest.py:209):
 //     oy = p, ox = q, sy = sx = 1;
-//   dilated windows (dilated != 0, square only; CrossFormer's long attention, crossformer.py:146 'b (l1 h) (l2 w) d -> (b h w) l1
-//   l2 d'):
+//   dilated windows (dilated != 0; CrossFormer's long attention, crossformer.py:146 'b (l1 h) (l2 w) d -> (b h w) l1 l2 d', and
+//   MobileViT's patch positions, mobile_vit.py:196 'b (h ph) (w pw) d -> b (ph pw) (h w) d' with p = h, q = w, ny = ph, nx = pw):
 //     oy = ox = 1, sy = ny, sx = nx.
-// nq == nk == p q.  pw == 0 means a square window (q = p): every caller but NesT's block attention.
+// nq == nk == p q.  pw == 0 means a square window (q = p): every caller but NesT's block attention and MobileViT's.
 struct Window {
   int p = 0, nx = 0, ny = 0;
   int dilated = 0;
@@ -131,9 +131,18 @@ CUtensorMap make_tmap_2d(const void* base, uint64_t inner, uint64_t outer, uint6
 CUtensorMap make_tmap_3d(const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1_bytes, uint64_t stride2_bytes,
                          uint32_t box0, uint32_t box1);
 
-// Activation of a GEMM epilogue: exact-erf GELU (vit.py:34) or hard-swish x * relu6(x + 3) / 6 (levit.py:36-38).  ACT_GELU is 1,
-// so the `gelu` flags (bool / int 0-1) of the older entry points convert to it unchanged.
-enum Act { ACT_NONE = 0, ACT_GELU = 1, ACT_HSWISH = 2 };
+// Activation of a GEMM epilogue: exact-erf GELU (vit.py:34), hard-swish x * relu6(x + 3) / 6 (levit.py:36-38) or SiLU / Keras
+// swish x * sigmoid(x) (mobile_vit.py:33).  ACT_GELU is 1, so the `gelu` flags (bool / int 0-1) of the older entry points convert
+// to it unchanged.
+enum Act { ACT_NONE = 0, ACT_GELU = 1, ACT_HSWISH = 2, ACT_SILU = 3 };
+
+#ifdef __CUDACC__
+// SiLU, x * sigmoid(x) = x / (1 + e^-x), the one definition every kernel applying it uses (the GEMM epilogues, dwconv_bn_act).  The
+// fast intrinsics: __expf is within 2 + 1.17 |x| ulp, __fdividef within 2 ulp while 1 + e^-x < 2^126 and 0 beyond (x < -87, where
+// SiLU is below 1e-36); a few ulp of fp32 against bf16 storage or the fp32 engine's 1e-5 relative bound.  The IEEE expf and division
+// add a slow path whose registers make the 192-wide LayerNorm-folded wgmma instance spill.
+__device__ __forceinline__ float silu(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
+#endif
 
 // ------------------------------------------------------------------------------------------ wgmma GEMM
 // out[M,N] = epilogue(A[M,K] * Wt[N,K]^T): bf16 operands (K-major), fp32 accumulation in registers.

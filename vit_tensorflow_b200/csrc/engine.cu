@@ -110,7 +110,9 @@ struct Epi {
   int ldr = 0;
   bool gelu = false;
   bool hswish = false;               // hard-swish instead (LeViT MLP, levit.py:37)
-  int act() const { return gelu ? ACT_GELU : hswish ? ACT_HSWISH : ACT_NONE; }
+  bool silu = false;                 // SiLU instead (MobileViT, mobile_vit.py:33)
+  int act() const { return gelu ? ACT_GELU : hswish ? ACT_HSWISH : silu ? ACT_SILU : ACT_NONE; }
+  void set_act(int a) { gelu = a == ACT_GELU; hswish = a == ACT_HSWISH; silu = a == ACT_SILU; }
   const float* ln_stats = nullptr;   // (sum, sumsq) partials per 64-column chunk of the A operand's rows for a LayerNorm-folded Dense, [M, K/64, 2]
   float* stats_out = nullptr;        // emit (sum, sumsq) partials of every 64-column chunk of the output rows, [M, N/64, 2]
 };
@@ -148,7 +150,7 @@ struct LevitBlockW {
 // One CvT Transformer layer (cvt.py:142-147) on channel rows zero-padded to dp (bf16) / dim (fp32).  The depthwise convolutions
 // carry their BatchNormalization folded (taps [k*k][dp] scaled, plus a per-channel shift); the MLP's PreNorm is folded into fc1
 // in the bf16 engine.
-struct MlpW { Norm norm; Linear fc1, fc2; };   // PreNorm MLP: LayerNorm, fc1, GELU, fc2
+struct MlpW { Norm norm; Linear fc1, fc2; int act = ACT_GELU; };   // PreNorm MLP: LayerNorm, fc1, activation (Act), fc2
 struct CvtBlockW {
   int dim = 0, dp = 0, heads = 0, k = 0, kv_stride = 1;
   Norm attn_norm;                    // gamma / beta [dp], zero on pad channels
@@ -228,11 +230,29 @@ struct NestLevelW {
   Norm agg_norm;                     // ag_layers.1, [dp_out]
 };
 
-// NesT's block attention on the windowed flash kernel (attn_flash.cu): bf16 only, false for a shape it does not take.
-inline bool block_attention_fast(const float*, int, float*, int, int, int, cudaStream_t, const Window&) { return false; }
+// MobileViT (mobile_vit.py:130-206) on channel rows zero-padded to channel_width (bf16) / unpadded (fp32).  Every Conv_NxN_BN and
+// MV2 convolution carries its BatchNormalization folded (a Dense with bias, or depthwise taps and a shift).
+struct Mv2W {                        // one MV2Block (:130-170)
+  int cin = 0, hidden = 0, cout = 0, stride = 1, cp_in = 0, hp = 0, cp_out = 0;
+  bool expand = false, residual = false;
+  Linear pw1;                        // 1x1 expand + BN, SiLU: [cp_in, hp]
+  const float* dw_w = nullptr;       // 3x3 depthwise + BN: taps [9][hp] and shift [hp], zero on pad channels; SiLU
+  const float* dw_b = nullptr;
+  Linear pw2;                        // 1x1 project + BN: [hp, cp_out]
+};
+struct MvitLayerW { Norm attn_norm; Linear qkv, to_out; MlpW ff; };
+struct MvitBlockW {                  // one MobileViTBlock (:173-206): the concat [conv3 out | block input] lives in one [rows, chp + cp_in] buffer
+  int cin = 0, ch = 0, dim = 0, cp_in = 0, chp = 0, dp = 0, k = 3;
+  Linear conv1, conv2, conv3, conv4;   // conv1 over unfold_same of the input's cin channels, conv4 over all chp + cp_in columns
+  std::vector<MvitLayerW> layers;
+};
+
+// NesT's block attention and MobileViT's patch-position attention on the windowed flash kernel (attn_flash.cu): bf16 only, false
+// for a shape it does not take.
+inline bool block_attention_fast(const float*, int, float*, int, int, int, cudaStream_t, const Window&, float) { return false; }
 inline bool block_attention_fast(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* out, int ldo, int heads, int dh, cudaStream_t s,
-                                 const Window& win) {
-  return attention_block(qkv, ld, out, ldo, heads, dh, s, 0.f, win);
+                                 const Window& win, float scale) {
+  return attention_block(qkv, ld, out, ldo, heads, dh, s, scale, win);
 }
 
 // One RegionViT stage (regionvit.py:231-240) on channel rows zero-padded to dp (bf16) / dim (fp32): the shared Downsample (s >= 1),
@@ -577,6 +597,18 @@ struct vb_handle {
     if (before != nullptr && ats_dev.p != before) drop_graphs();
     ats_rng_ptr();
   }
+  // MobileViT (mobile_vit.py:209-271): conv1, the seven MV2 blocks (stem 0-3, trunk 4-6), the three MobileViTBlocks, to_logits
+  vb_mobilevit_config mv{};
+  Linear mv_conv1, mv_logits;
+  std::vector<Mv2W> mv_mv2;
+  std::vector<MvitBlockW> mv_vit;
+  static std::string mv2_pre(int i) { return i < 4 ? "stem." + std::to_string(i) + ".conv." : "trunk." + std::to_string(i - 4) + ".0.conv."; }
+  static std::string mvit_pre(int s) { return "trunk." + std::to_string(s) + ".1."; }
+  int mvit_cin(int s) const { return mv.channels[4 + 2 * s]; }
+  int mvit_ch(int s) const { return mv.channels[5 + 2 * s]; }
+  int mvit_mlp(int s) const { return mv.dims[s] * (s == 0 ? 2 : 4); }            // mobile_vit.py:241,246,251
+  static constexpr int kMvHeads = 4, kMvDh = 8;                                    // MobileViTBlock's Transformer (:182)
+  int mvit_dh() const { return bf16() ? 32 : kMvDh; }                             // bf16: heads widened to the flash kernel's 32
   Norm head_norm, sm_head_norm, lg_head_norm;
   Linear head, sm_head, lg_head;
   Norm spt_norm;                     // SPT's LayerNorm over the p^2 * 5 C patch vector (bf16: padded to the GEMM's K, folded into it)
@@ -907,6 +939,46 @@ struct vb_handle {
       }
       expect_ln("to_logits.1", rv.dims[VB_REGIONVIT_STAGES - 1]);       // :243-247
       expect_dense("to_logits.2", rv.dims[VB_REGIONVIT_STAGES - 1], c.num_classes);
+    } else if (c.kind == VB_KIND_MOBILEVIT) {
+      auto expect_bn = [&](const std::string& n, int d) {
+        for (const char* leaf : {"gamma", "beta", "moving_mean", "moving_variance"}) expect(n + "." + leaf, {d});
+      };
+      auto expect_cbn = [&](const std::string& n, int k, int cin, int cout) {   // Conv_NxN_BN (:37-49)
+        expect(n + ".layers.0.kernel", {k, k, cin, cout});
+        expect_bn(n + ".layers.1", cout);
+      };
+      expect_cbn("conv1", 3, c.channels, mv.channels[0]);
+      for (int i = 0; i < VB_MOBILEVIT_MV2; ++i) {                       // MV2Block (:139-164)
+        const std::string p = mv2_pre(i);
+        const int hid = mv.mv2_hidden[i];
+        if (mv.mv2_expand[i]) {
+          expect(p + "0.kernel", {1, 1, mv.mv2_in[i], hid}); expect_bn(p + "1", hid);
+          expect(p + "3.kernel", {3, 3, 1, hid}); expect_bn(p + "4", hid);
+          expect(p + "6.kernel", {1, 1, hid, mv.mv2_out[i]}); expect_bn(p + "7", mv.mv2_out[i]);
+        } else {
+          expect(p + "0.kernel", {3, 3, 1, hid}); expect_bn(p + "1", hid);
+          expect(p + "3.kernel", {1, 1, hid, mv.mv2_out[i]}); expect_bn(p + "4", mv.mv2_out[i]);
+        }
+      }
+      for (int s = 0; s < 3; ++s) {                                      // MobileViTBlock (:173-185)
+        const std::string p = mvit_pre(s);
+        const int d = mv.dims[s], ch = mvit_ch(s), cin = mvit_cin(s), k = mv.kernel_size, I = kMvHeads * kMvDh;
+        expect_cbn(p + "conv1", k, cin, ch);
+        expect_cbn(p + "conv2", 1, ch, d);
+        for (int L = 0; L < mv.depths[s]; ++L) {                         // Transformer (:110-127)
+          const std::string b = p + "transformer.layers." + std::to_string(L) + ".";
+          expect_ln(b + "0.norm", d);
+          expect_dense(b + "0.fn.to_qkv", d, 3 * I, false);
+          expect_dense(b + "0.fn.to_out.0", I, d);
+          expect_ln(b + "1.norm", d);
+          expect_dense(b + "1.fn.net.0", d, mvit_mlp(s));
+          expect_dense(b + "1.fn.net.3", mvit_mlp(s), d);
+        }
+        expect_cbn(p + "conv3", 1, d, ch);
+        expect_cbn(p + "conv4", k, ch + cin, ch);
+      }
+      expect_cbn("to_logits.0", 1, mv.channels[9], mv.last_dim);         // :254-258
+      expect("to_logits.2.kernel", {mv.last_dim, c.num_classes});
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       expect("pos_embedding", {1, np, c.dim});
@@ -1140,6 +1212,7 @@ struct vb_handle {
     VB_CUDA(cudaSetDevice(device));
     owned.clear(); layers.clear(); cls_layers.clear(); t2t_layers.clear(); xblocks.clear(); plans.clear(); embed_res.clear(); cct_convs.clear();
     lv_stem.clear(); lv_blocks.clear(); cvt_stages.clear(); twins_stages.clear(); cf_stages.clear(); nest_levels.clear(); rv_stages.clear();
+    mv_mv2.clear(); mv_vit.clear();
     woverride.clear();
     drop_graphs();
     const vb_config& c = cfg;
@@ -1202,6 +1275,8 @@ struct vb_handle {
       finalize_nest();
     } else if (c.kind == VB_KIND_REGIONVIT) {
       finalize_regionvit();
+    } else if (c.kind == VB_KIND_MOBILEVIT) {
+      finalize_mobilevit();
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       embed = make_embed("", c.patch_h, c.patch_w, c.dim, np, false);
@@ -1650,6 +1725,82 @@ struct vb_handle {
     for (int h = 0; h < heads; ++h)
       for (int e = 0; e < f2; ++e) t[static_cast<size_t>(h) * f2 + e] = emb[static_cast<size_t>(e) * heads + h] * inv_scale;
     return t;
+  }
+
+  // ---- MobileViT weight packing: every BatchNorm folded on the host, channel widths zero-padded (bf16), heads widened to 32 (bf16)
+  // A bias-free Conv2D `conv` [k, k, cin, N] and the BatchNormalization `bn` after it as one Dense: input channel c of tap t at row
+  // t * pitch + (c < split ? c : split_at + c - split) (split 0: row t * pitch + c) of a zero [k * k * pitch, Np]
+  Linear mv_conv_bn(const std::string& conv, const std::string& bn, int k, int cin, int N, int pitch, int Np, int split = 0, int split_at = 0) {
+    auto Wk = host_weight(conv + ".kernel");
+    std::vector<double> bias(N, 0.0);
+    fold_bn(Wk, bias, k * k * cin, N, bn);
+    std::vector<double> Wp(static_cast<size_t>(k) * k * pitch * Np, 0.0);
+    for (int t = 0; t < k * k; ++t)
+      for (int c = 0; c < cin; ++c) {
+        const int row = t * pitch + (split > 0 && c >= split ? split_at + c - split : c);
+        for (int n = 0; n < N; ++n) Wp[static_cast<size_t>(row) * Np + n] = Wk[(static_cast<size_t>(t) * cin + c) * N + n];
+      }
+    return linear_from_host("mv." + conv, Wp, pad_n(bias, Np), k * k * pitch, Np);
+  }
+  Linear mv_cbn(const std::string& n, int k, int cin, int N, int pitch, int split = 0, int split_at = 0) {   // Conv_NxN_BN `n`
+    return mv_conv_bn(n + ".layers.0", n + ".layers.1", k, cin, N, pitch, channel_width(N), split, split_at);
+  }
+  void finalize_mobilevit() {
+    mv_conv1 = mv_cbn("conv1", 3, cfg.channels, mv.channels[0], cfg.channels);
+    for (int i = 0; i < VB_MOBILEVIT_MV2; ++i) {
+      Mv2W m;
+      const std::string p = mv2_pre(i);
+      m.cin = mv.mv2_in[i]; m.hidden = mv.mv2_hidden[i]; m.cout = mv.mv2_out[i]; m.stride = mv.mv2_stride[i];
+      m.cp_in = channel_width(m.cin); m.hp = channel_width(m.hidden); m.cp_out = channel_width(m.cout);
+      m.expand = mv.mv2_expand[i] != 0; m.residual = mv.mv2_residual[i] != 0;
+      const std::string dw = m.expand ? "3" : "0", dwbn = m.expand ? "4" : "1", pw = m.expand ? "6" : "3", pwbn = m.expand ? "7" : "4";
+      if (m.expand) m.pw1 = mv_conv_bn(p + "0", p + "1", 1, m.cin, m.hidden, m.cp_in, m.hp);
+      std::vector<double> taps, shift;
+      cvt_fold_dw(host_weight(p + dw + ".kernel"), host_weight(p + dwbn + ".gamma"), host_weight(p + dwbn + ".beta"),
+                  host_weight(p + dwbn + ".moving_mean"), host_weight(p + dwbn + ".moving_variance"), 3, m.hidden, m.hp, taps, shift);
+      m.dw_w = upload_owned(taps);
+      m.dw_b = upload_owned(shift);
+      m.pw2 = mv_conv_bn(p + pw, p + pwbn, 1, m.hidden, m.cout, m.hp, m.cp_out);
+      mv_mv2.push_back(std::move(m));
+    }
+    const int dh = mvit_dh(), I = kMvHeads * kMvDh, Ip = kMvHeads * dh;
+    for (int s = 0; s < 3; ++s) {
+      MvitBlockW v;
+      const std::string p = mvit_pre(s);
+      v.cin = mvit_cin(s); v.ch = mvit_ch(s); v.dim = mv.dims[s]; v.k = mv.kernel_size;
+      v.cp_in = channel_width(v.cin); v.chp = channel_width(v.ch); v.dp = channel_width(v.dim);
+      v.conv1 = mv_cbn(p + "conv1", v.k, v.cin, v.ch, v.cin);
+      v.conv2 = mv_cbn(p + "conv2", 1, v.ch, v.dim, v.chp);
+      for (int L = 0; L < mv.depths[s]; ++L) {
+        const std::string b = p + "transformer.layers." + std::to_string(L) + ".", key = "mv." + b;
+        MvitLayerW l;
+        l.attn_norm = padded_norm(b + "0.norm", v.dim, v.dp, ".gamma", ".beta");
+        // head h's 8 columns of q, k and v at g * Ip + h * dh; to_out's rows likewise (zero rows meet the pad columns)
+        const auto wq = host_weight(b + "0.fn.to_qkv.kernel"), wo = host_weight(b + "0.fn.to_out.0.kernel");
+        std::vector<double> Wqkv(static_cast<size_t>(v.dp) * 3 * Ip, 0.0), Wout(static_cast<size_t>(Ip) * v.dp, 0.0);
+        for (int g = 0; g < 3; ++g)
+          for (int h = 0; h < kMvHeads; ++h)
+            for (int d = 0; d < kMvDh; ++d) {
+              for (int r = 0; r < v.dim; ++r)
+                Wqkv[static_cast<size_t>(r) * 3 * Ip + g * Ip + h * dh + d] = wq[static_cast<size_t>(r) * 3 * I + g * I + h * kMvDh + d];
+              if (g == 0)
+                for (int o = 0; o < v.dim; ++o) Wout[static_cast<size_t>(h * dh + d) * v.dp + o] = wo[static_cast<size_t>(h * kMvDh + d) * v.dim + o];
+            }
+        l.qkv = linear_from_host(key + "qkv", Wqkv, {}, v.dp, 3 * Ip, bf16() ? &l.attn_norm : nullptr);
+        l.qkv.ln_d = v.dim;
+        l.qkv.ln_eps = 1e-3f;                                          // Keras LayerNormalization (:56)
+        l.to_out = linear_from_host(key + "to_out", Wout, pad_n(host_weight(b + "0.fn.to_out.0.bias"), v.dp), Ip, v.dp);
+        l.ff = prenorm_mlp("mv.", b + "1.norm", b + "1.fn.net.0", b + "1.fn.net.3", v.dim, v.dp, mvit_mlp(s) / v.dim, 1e-3f, ".gamma", ".beta");
+        l.ff.act = ACT_SILU;                                           // MLP (:67-73)
+        v.layers.push_back(std::move(l));
+      }
+      v.conv3 = mv_cbn(p + "conv3", 1, v.dim, v.ch, v.dp);
+      v.conv4 = mv_cbn(p + "conv4", v.k, v.ch + v.cin, v.ch, v.chp + v.cp_in, v.ch, v.chp);   // concat([x, y]) (:203)
+      mv_vit.push_back(std::move(v));
+    }
+    mv_logits = mv_cbn("to_logits.0", 1, mv.channels[9], mv.last_dim, channel_width(mv.channels[9]));
+    head = Linear();
+    head.W = W("to_logits.2.kernel"); head.K = mv.last_dim; head.N = cfg.num_classes; head.ldw = mv.last_dim;   // Dense without bias
   }
 
   // vit_for_small_dataset.ViT (:159-195): SPT (set_spt_patch), then ViT's layers with LSA: the diagonal mask and exp(temperature)
@@ -2295,6 +2446,8 @@ struct vb_handle {
       regionvit_forward<T>(img, B, H, Wd, logits, s);
     } else if (c.kind == VB_KIND_ATS_VIT) {
       ats_forward<T>(img, B, H, Wd, logits, s);
+    } else if (c.kind == VB_KIND_MOBILEVIT) {
+      mobilevit_forward<T>(img, B, H, Wd, logits, s);
     } else if (c.kind == VB_KIND_SMALL_DATASET_VIT) {     // vit_for_small_dataset.py:197-215, Transformer.call :135-140
       int rows = 0;
       float* stats = nullptr;
@@ -2360,10 +2513,10 @@ struct vb_handle {
   }
   // A convolution as unfold_same + GEMM: the fp32 image (map == null, cin channels) or the first cin channels of the token map
   // [B h w, ld], unfolded at the packed weight pitch (`um`: VALID, or the LayerNorm / GELU applied on load), then out [rows, L.N] =
-  // col W + b, with the output rows' statistics when stats_out is given
+  // act(col W + b) (Act), with the output rows' statistics when stats_out is given
   template <typename T>
   void conv(const float* img, const T* map, int ld, int B, int h, int w, int cin, int k, int stride, const Linear& L, T* out,
-            float* stats_out, cudaStream_t s, const UnfoldMode* um = nullptr) {
+            float* stats_out, cudaStream_t s, const UnfoldMode* um = nullptr, int act = ACT_NONE) {
     const bool valid = um != nullptr && um->valid;
     const int oh = valid ? (h - k) / stride + 1 : (h + stride - 1) / stride, ow = valid ? (w - k) / stride + 1 : (w + stride - 1) / stride;
     const int rows = B * oh * ow, Kp = bf16() ? L.ldw : L.K;
@@ -2375,7 +2528,7 @@ struct vb_handle {
     }
     Linear Lk = L;
     Lk.K = Kp;                      // unfold_same zero-pads the patch vectors to the packed weight pitch
-    Epi e; e.bias = L.bias; e.stats_out = stats_out;
+    Epi e; e.bias = L.bias; e.stats_out = stats_out; e.set_act(act);
     linear<T>(col, Kp, rows, Lk, out, L.N, e, s);
   }
   // The pre-norm sub-blocks x = f(LN(x)) + x over X [M, dp] (true width d).  bf16 folds the LayerNorm into f's first GEMM from
@@ -2405,11 +2558,11 @@ struct vb_handle {
       Epi e; e.bias = L.bias; e.res = X; e.ldr = dp; e.stats_out = stats;
       h.linear<T>(A, lda, M, L, X, dp, e, s);
     }
-    void mlp(const MlpW& m) const {                               // X = fc2(GELU(fc1(LN(X)))) + X
+    void mlp(const MlpW& m) const {                               // X = fc2(act(fc1(LN(X)))) + X
       const T* a = norm(m.norm);
       T* Hb = h.arena.get<T>(static_cast<size_t>(M) * m.fc1.N);
       Epi e1 = folded_epi(m.fc1);
-      e1.gelu = true;
+      e1.set_act(m.act);
       h.linear<T>(a, dp, M, m.fc1, Hb, m.fc1.N, e1, s);
       residual(Hb, m.fc1.N, m.fc2);
     }
@@ -2809,22 +2962,23 @@ struct vb_handle {
     p.residual(QKV, ld, l.to_out);
     p.mlp(l.ff);                                                      // MLP nest.py:61-75
   }
-  // NesT's block attention: win.count blocks of p x width() tokens of fused q|k|v rows [.., ld], the output rows written to out
-  // [.., ldo] pixel-major.  The windowed flash kernel where it serves (bf16, dh 32 or 64), else window_attention_generic.
+  // NesT's block attention and MobileViT's patch-position attention: win.count blocks of p x width() tokens of fused q|k|v rows
+  // [.., ld], the output rows written to out [.., ldo] pixel-major; scale <= 0: dh^-0.5.  The windowed flash kernel where it serves
+  // (bf16, dh 32 or 64), else window_attention_generic.
   template <typename T>
-  void block_attention(const T* qkv, int ld, T* out, int ldo, int heads, int dh, const Window& win, cudaStream_t s) {
+  void block_attention(const T* qkv, int ld, T* out, int ldo, int heads, int dh, const Window& win, cudaStream_t s, float scale = 0.f) {
     const int n = win.p * win.width();
     {
       ProfScope ps(this, PROF_ATTN, 4.0 * win.count * heads * n * n * dh, static_cast<double>(sizeof(T)) * win.count * heads * dh * 4.0 * n, s);
-      if (block_attention_fast(qkv, ld, out, ldo, heads, dh, s, win)) return;
+      if (block_attention_fast(qkv, ld, out, ldo, heads, dh, s, win, scale)) return;
     }
-    window_attention_generic<T>(qkv, ld, out, ldo, win.count, n, heads, dh, win, nullptr, s);
+    window_attention_generic<T>(qkv, ld, out, ldo, win.count, n, heads, dh, win, nullptr, s, scale);
   }
   // Windowed attention off the flash kernel: B windows of n tokens of fused q|k|v rows [.., ld] (win's layout, with the window
   // bias pb when given) permuted to window-major order, the materialised-scores path, the output rows permuted back to out [.., ldo]
   template <typename T>
   void window_attention_generic(const T* qkv, int ld, T* out, int ldo, int B, int n, int heads, int dh, const Window& win, const PosBias* pb,
-                                cudaStream_t s) {
+                                cudaStream_t s, float scale = 0.f) {
     const int HD = heads * dh;
     const long long rows = static_cast<long long>(B) * n;
     T* qkvw = arena.get<T>(static_cast<size_t>(rows) * 3 * HD);
@@ -2834,9 +2988,101 @@ struct vb_handle {
       ProfScope ps(this, PROF_ATTN, 4.0 * B * heads * n * n * dh, static_cast<double>(sizeof(T)) * B * heads * dh * 4.0 * n, s);
       float* S = arena.get<float>(static_cast<size_t>(B) * heads * n * ((n + 15) & ~15));
       attention_generic<T>(qkvw, 3 * HD, qkvw + HD, 3 * HD, qkvw + 2 * HD, 3 * HD, ow, HD, S, B, n, n, heads, dh, 0, nullptr, nullptr, nullptr,
-                           nullptr, s, 0.f, pb);
+                           nullptr, s, scale, pb);
     }
     { ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * rows * HD, s); window_rows<T>(ow, HD, out, ldo, HD, win, rows, false, s); }
+  }
+
+  // MobileViT.call (mobile_vit.py:260-271): conv1, the stem, per trunk stage an MV2 block and a MobileViTBlock, then to_logits.
+  // Token rows are the NHWC map, pixel-major, channel widths zero-padded to channel_width.  Every SAME stride gives ceil; the
+  // reference's regrouping (:196) needs every trunk map divisible by (ph, pw), checked before anything runs.
+  void mvit_check_size(int H, int Wd) const {
+    int h = (H + 3) / 4, w = (Wd + 3) / 4;                              // conv1 and stem block 1: stride 2 each
+    for (int s = 0; s < 3; ++s) {
+      h = (h + 1) / 2; w = (w + 1) / 2;
+      VB_CHECK(h % mv.ph == 0 && w % mv.pw == 0,
+               "MobileViT stage " + std::to_string(s + 1) + ": the " + std::to_string(h) + " x " + std::to_string(w) + " map is not divisible by "
+               "patch_size (" + std::to_string(mv.ph) + ", " + std::to_string(mv.pw) + "); every trunk map (1/8, 1/16 and 1/32 of the "
+               "image, rounded up) must be");
+    }
+  }
+  template <typename T>
+  void mobilevit_forward(const float* img, int B, int H, int Wd, float* logits, cudaStream_t s) {
+    mvit_check_size(H, Wd);
+    int h = (H + 1) / 2, w = (Wd + 1) / 2, ld = mv_conv1.N;
+    T* X = arena.get<T>(static_cast<size_t>(B) * h * w * ld);
+    conv<T>(img, nullptr, 0, B, H, Wd, cfg.channels, 3, 2, mv_conv1, X, nullptr, s, nullptr, ACT_SILU);   // conv1 (:230)
+    for (int i = 0; i < 4; ++i) {                                         // stem (:232-236)
+      const Mv2W& m = mv_mv2[i];
+      X = mv2_block<T>(X, ld, B, h, w, m, nullptr, 0, s);
+      h = (h + m.stride - 1) / m.stride; w = (w + m.stride - 1) / m.stride; ld = m.cp_out;
+    }
+    for (int st = 0; st < 3; ++st) {
+      const Mv2W& m = mv_mv2[4 + st];
+      const MvitBlockW& v = mv_vit[st];
+      const int oh = (h + 1) / 2, ow = (w + 1) / 2, ldc = v.chp + v.cp_in;
+      T* Cat = arena.get<T>(static_cast<size_t>(B) * oh * ow * ldc);      // [conv3 out | y]: the MV2 block writes y, the block's input
+      mv2_block<T>(X, ld, B, h, w, m, Cat + v.chp, ldc, s);
+      X = mobilevit_block<T>(Cat, B, oh, ow, v, s);
+      h = oh; w = ow; ld = v.chp;
+    }
+    const int M = B * h * w;
+    T* Y = arena.get<T>(static_cast<size_t>(M) * mv_logits.N);
+    Epi e; e.bias = mv_logits.bias; e.silu = true;
+    linear<T>(X, ld, M, mv_logits, Y, mv_logits.N, e, s);               // to_logits.0 (:255)
+    dense_head(mean_pool<T>(Y, h * w, mv_logits.N, mv.last_dim, B, s), mv.last_dim, head, B, logits, s);   // Reduce, Dense (:256-257)
+  }
+  // One MV2Block (mobile_vit.py:166-170) on X [B*h*w, ldx] -> out [B*oh*ow, ldo] (a new buffer when out is null)
+  template <typename T>
+  T* mv2_block(const T* X, int ldx, int B, int h, int w, const Mv2W& m, T* out, int ldo, cudaStream_t s) {
+    const int oh = (h + m.stride - 1) / m.stride, ow = (w + m.stride - 1) / m.stride, M = B * h * w, Mo = B * oh * ow;
+    const T* a = X;
+    int lda = ldx;
+    if (m.expand) {
+      T* E = arena.get<T>(static_cast<size_t>(M) * m.hp);
+      Epi e; e.bias = m.pw1.bias; e.silu = true;
+      linear<T>(X, ldx, M, m.pw1, E, m.hp, e, s);
+      a = E; lda = m.hp;
+    }
+    T* D = arena.get<T>(static_cast<size_t>(Mo) * m.hp);
+    {
+      ProfScope ps(this, PROF_OTHER, 20.0 * Mo * m.hidden, static_cast<double>(sizeof(T)) * (static_cast<double>(M) * m.hidden + static_cast<double>(Mo) * m.hp), s);
+      dwconv_bn_act<T>(a, lda, m.dw_w, m.dw_b, D, m.hp, B, h, w, m.hidden, m.hp, m.stride, s);
+    }
+    if (out == nullptr) { out = arena.get<T>(static_cast<size_t>(Mo) * m.cp_out); ldo = m.cp_out; }
+    Epi e2; e2.bias = m.pw2.bias;
+    if (m.residual) { e2.res = X; e2.ldr = ldx; }
+    linear<T>(D, m.hp, Mo, m.pw2, out, ldo, e2, s);
+    return out;
+  }
+  // One MobileViTBlock (mobile_vit.py:187-206) on Cat [B*h*w, chp + cp_in] whose right half holds its input y -> a new [B*h*w, chp]
+  template <typename T>
+  T* mobilevit_block(T* Cat, int B, int h, int w, const MvitBlockW& v, cudaStream_t s) {
+    const int ldc = v.chp + v.cp_in, M = B * h * w, dh = mvit_dh(), ld = 3 * kMvHeads * dh;
+    T* Y1 = arena.get<T>(static_cast<size_t>(M) * v.chp);
+    conv<T>(nullptr, Cat + v.chp, ldc, B, h, w, v.cin, v.k, 1, v.conv1, Y1, nullptr, s, nullptr, ACT_SILU);
+    T* X = arena.get<T>(static_cast<size_t>(M) * v.dp);
+    float* stats = row_stats(M, v.dp);
+    Epi e2; e2.bias = v.conv2.bias; e2.silu = true; e2.stats_out = stats;
+    linear<T>(Y1, v.chp, M, v.conv2, X, v.dp, e2, s);
+    // 'b (h ph) (w pw) d -> b (ph pw) (h w) d': the pixels of one patch position are a dilated h/ph x w/pw window of the map
+    Window win;
+    win.p = h / mv.ph; win.pw = w / mv.pw; win.ny = mv.ph; win.nx = mv.pw; win.dilated = 1; win.count = B * mv.ph * mv.pw;
+    const float scale = 1.0f / sqrtf(static_cast<float>(kMvDh));
+    for (const MvitLayerW& l : v.layers) {
+      const PreNorm<T> p = prenorm<T>(X, M, v.dim, v.dp, stats, 1e-3f, s);
+      const T* a = p.norm(l.attn_norm);
+      T* QKV = arena.get<T>(static_cast<size_t>(M) * ld);
+      linear<T>(a, v.dp, M, l.qkv, QKV, ld, p.folded_epi(l.qkv), s);
+      block_attention<T>(QKV, ld, QKV, ld, kMvHeads, dh, win, s, scale);   // the output overwrites q
+      p.residual(QKV, ld, l.to_out);
+      p.mlp(l.ff);
+    }
+    Epi e3; e3.bias = v.conv3.bias; e3.silu = true;
+    linear<T>(X, v.dp, M, v.conv3, Cat, ldc, e3, s);                     // the concat's left half
+    T* out = arena.get<T>(static_cast<size_t>(M) * v.chp);
+    conv<T>(nullptr, Cat, ldc, B, h, w, ldc, v.k, 1, v.conv4, out, nullptr, s, nullptr, ACT_SILU);
+    return out;
   }
 
   // RegionViT.call (regionvit.py:249-263): the local and region encoders, then per stage the shared Downsample of both maps, the
@@ -3062,6 +3308,7 @@ struct vb_handle {
       case VB_KIND_REGIONVIT: return "RegionViT runs as a whole forward only: its encoder / stage / head steps have no entry of their own";
       case VB_KIND_ATS_VIT: return "ATS-ViT runs as a whole forward only: its token count changes inside the transformer, so its stages have no entry of their own";
       case VB_KIND_SMALL_DATASET_VIT: return "the small-dataset ViT runs as a whole forward only: its SPT embedding / transformer / head steps have no entry of their own";
+      case VB_KIND_MOBILEVIT: return "MobileViT runs as a whole forward only: its stem / trunk / head steps have no entry of their own";
       default: return nullptr;
     }
   }
@@ -3300,6 +3547,7 @@ void validate(const vb_config& c) {
   VB_CHECK(c.kind != VB_KIND_NEST, "NesT: create the handle with vb_create_nest (its levels are a vb_nest_config)");
   VB_CHECK(c.kind != VB_KIND_REGIONVIT, "RegionViT: create the handle with vb_create_regionvit (its stages are a vb_regionvit_config)");
   VB_CHECK(c.kind != VB_KIND_ATS_VIT, "ATS-ViT: create the handle with vb_create_ats_vit (its token counts are a vb_ats_vit_config)");
+  VB_CHECK(c.kind != VB_KIND_MOBILEVIT, "MobileViT: create the handle with vb_create_mobilevit (its blocks are a vb_mobilevit_config)");
   VB_CHECK((c.kind >= VB_KIND_VIT && c.kind <= VB_KIND_CCT) || c.kind == VB_KIND_SMALL_DATASET_VIT, "unknown model kind");
   if (c.kind == VB_KIND_SMALL_DATASET_VIT) {
     // SPT's Rearrange takes one patch size for both sides (vit_for_small_dataset.py:147) and shift() one image of 3 channels
@@ -3418,6 +3666,26 @@ void validate_regionvit(const vb_config& c, const vb_regionvit_config& r) {
   VB_CHECK(r.window_size > 0 && r.local_patch_size > 0 && r.mlp_mult > 0, "RegionViT: bad window_size / local_patch_size / mlp_mult");
   VB_CHECK(static_cast<long long>(r.local_patch_size) * r.window_size <= 4096, "RegionViT: the region patch size is too large");
   VB_CHECK(r.window_size <= 1024, "RegionViT: window_size is too large");
+}
+
+// The widths the host computed must chain as mobile_vit.py:230-252 wires the blocks
+void validate_mobilevit(const vb_config& c, const vb_mobilevit_config& m) {
+  VB_CHECK(c.precision == VB_PRECISION_FP32 || c.precision == VB_PRECISION_BF16, "unknown precision");
+  VB_CHECK(c.channels == 3 && c.num_classes > 0, "MobileViT: images of 3 channels and a positive num_classes");
+  for (int i = 0; i < 10; ++i) VB_CHECK(m.channels[i] > 0 && m.channels[i] <= 65536, "MobileViT: channels must be positive");
+  VB_CHECK(m.last_dim > 0 && m.last_dim <= 65536, "MobileViT: channels[-1] must be positive");
+  for (int s = 0; s < 3; ++s) VB_CHECK(m.dims[s] > 0 && m.dims[s] <= 65536 && m.depths[s] >= 0, "MobileViT: dims must be positive and depths not negative");
+  VB_CHECK(m.kernel_size >= 1 && m.kernel_size <= 15 && m.ph > 0 && m.pw > 0, "MobileViT: bad kernel_size / patch_size");
+  const int in[VB_MOBILEVIT_MV2] = {m.channels[0], m.channels[1], m.channels[2], m.channels[3], m.channels[3], m.channels[5], m.channels[7]};
+  const int out[VB_MOBILEVIT_MV2] = {m.channels[1], m.channels[2], m.channels[3], m.channels[3], m.channels[4], m.channels[6], m.channels[8]};
+  const int stride[VB_MOBILEVIT_MV2] = {1, 2, 1, 1, 2, 2, 2};
+  for (int i = 0; i < VB_MOBILEVIT_MV2; ++i) {
+    const std::string b = "MobileViT MV2 block " + std::to_string(i) + ": ";
+    VB_CHECK(m.mv2_in[i] == in[i] && m.mv2_out[i] == out[i] && m.mv2_stride[i] == stride[i], b + "widths or stride do not chain");
+    VB_CHECK(m.mv2_hidden[i] > 0 && m.mv2_hidden[i] <= 262144, b + "bad hidden width");
+    VB_CHECK(m.mv2_expand[i] || m.mv2_hidden[i] == m.mv2_in[i], b + "without the expand convolution the depthwise step needs hidden == input width");
+    VB_CHECK(!m.mv2_residual[i] || (stride[i] == 1 && in[i] == out[i]), b + "a residual needs stride 1 and equal widths");
+  }
 }
 
 void validate_crossformer(const vb_config& c, const vb_crossformer_config& cf) {
@@ -3821,6 +4089,11 @@ int vb_op_lsa_attention(int32_t precision, const float* qkv, int32_t ld, int32_t
   });
 }
 
+int vb_create_mobilevit(const vb_config* base, const vb_mobilevit_config* mc, int device, vb_handle** out) {
+  return create_with("vb_create_mobilevit", "vb_mobilevit_config", VB_KIND_MOBILEVIT, "VB_KIND_MOBILEVIT", base, mc, device, out,
+                     validate_mobilevit, [&](vb_handle& h) { h.mv = *mc; h.cfg.dim = mc->last_dim; });
+}
+
 int vb_create_regionvit(const vb_config* base, const vb_regionvit_config* rc, int device, vb_handle** out) {
   return create_with("vb_create_regionvit", "vb_regionvit_config", VB_KIND_REGIONVIT, "VB_KIND_REGIONVIT", base, rc,
                                           device, out, validate_regionvit,
@@ -3958,6 +4231,7 @@ int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, int32_t 
     VB_CHECK(h->cfg.kind != VB_KIND_REGIONVIT, "vb_forward_distill: RegionViT has no distillation head");
     VB_CHECK(h->cfg.kind != VB_KIND_ATS_VIT, h->whole_forward_only(VB_KIND_ATS_VIT));
     VB_CHECK(h->cfg.kind != VB_KIND_SMALL_DATASET_VIT, h->whole_forward_only(VB_KIND_SMALL_DATASET_VIT));
+    VB_CHECK(h->cfg.kind != VB_KIND_MOBILEVIT, h->whole_forward_only(VB_KIND_MOBILEVIT));
     const bool levit = h->cfg.kind == VB_KIND_LEVIT;
     VB_CHECK(levit || distill_token != nullptr, "vb_forward_distill: null argument");
     VB_CHECK(!levit || (distill_token == nullptr && h->lv.num_distill_classes > 0),
@@ -4083,6 +4357,7 @@ int vb_to_patch(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, 
   return guarded(h, [&] {
     VB_CHECK(h != nullptr && img != nullptr && patches != nullptr, "vb_to_patch: null argument");
     VB_CHECK(h->cfg.kind != VB_KIND_SMALL_DATASET_VIT, h->whole_forward_only(VB_KIND_SMALL_DATASET_VIT));
+    VB_CHECK(h->cfg.kind != VB_KIND_MOBILEVIT, h->whole_forward_only(VB_KIND_MOBILEVIT));
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT && h->cfg.kind != VB_KIND_T2T_VIT && h->cfg.kind != VB_KIND_CCT &&
              h->cfg.kind != VB_KIND_LEVIT && h->cfg.kind != VB_KIND_CVT && h->cfg.kind != VB_KIND_TWINS_SVT &&
              h->cfg.kind != VB_KIND_CROSSFORMER && h->cfg.kind != VB_KIND_NEST && h->cfg.kind != VB_KIND_REGIONVIT,
@@ -4352,7 +4627,8 @@ int vb_op_gemm(const float* a, int32_t lda, const float* wt, int32_t ldw, int32_
     const __nv_bfloat16* dr = in_place ? static_cast<const __nv_bfloat16*>(dout)
                               : res ? upload<__nv_bfloat16>(dR, res, static_cast<size_t>(M) * ldr) : nullptr;
     // the plan exactly as vb_handle::linear / gemm_cached build it
-    GemmBf16 g = gemm_bf16_plan(da, lda, dw, ldw, static_cast<__nv_bfloat16*>(dout), ldc, M, N, K, db, ds, dr, ldr, gelu != 0,
+    const int act = gelu == 0 ? ACT_NONE : gelu == ACT_SILU ? ACT_SILU : ACT_GELU;   // any other nonzero value: GELU, as it always was
+    GemmBf16 g = gemm_bf16_plan(da, lda, dw, ldw, static_cast<__nv_bfloat16*>(dout), ldc, M, N, K, db, ds, dr, ldr, act,
                                 out_f32 != 0, b_rows);
     if (ln_c1) {
       g.ln_c1 = upload<float>(dC1, ln_c1, N);
@@ -4561,6 +4837,59 @@ int vb_op_block_attention(int32_t precision, const float* qkv, int32_t ld, int32
       timed(iters, elapsed_ms, [&] {
         h.arena.reset();
         h.block_attention<T>(x_d, ld, o_d, ldo, heads, dh, win, 0);
+      });
+      download<T>(o_d, out, static_cast<size_t>(rows) * ldo);
+    });
+  });
+}
+
+int vb_op_mv2_dwconv(int32_t precision, const float* x, int32_t B, int32_t H, int32_t W, int32_t C, int32_t stride, const float* w,
+                     const float* bn, float* out, int32_t iters, float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    VB_CHECK(x && w && bn && out && B > 0 && H > 0 && W > 0 && C > 0 && (stride == 1 || stride == 2), "vb_op_mv2_dwconv: bad arguments");
+    const bool bf = precision != VB_PRECISION_FP32;               // as with_precision picks the element type
+    const int Cp = bf ? round_up(C, 64) : C, Ho = (H + stride - 1) / stride, Wo = (W + stride - 1) / stride;
+    const size_t M = static_cast<size_t>(B) * H * W, Mo = static_cast<size_t>(B) * Ho * Wo;
+    auto vec = [](const float* p, size_t n) { return std::vector<double>(p, p + n); };
+    std::vector<double> wd, sd;                                   // as vb_finalize folds it
+    cvt_fold_dw(vec(w, static_cast<size_t>(9) * C), vec(bn, C), vec(bn + C, C), vec(bn + 2 * C, C), vec(bn + 3 * C, C), 3, C, Cp, wd, sd);
+    const std::vector<float> taps(wd.begin(), wd.end()), shift(sd.begin(), sd.end());
+    std::vector<float> xp(M * Cp, 0.f);
+    for (size_t r = 0; r < M; ++r) std::copy(x + r * C, x + (r + 1) * C, xp.begin() + r * Cp);
+    DevMem dX, dT, dS, dO;
+    const float* t_d = upload<float>(dT, taps.data(), taps.size());
+    const float* s_d = upload<float>(dS, shift.data(), shift.size());
+    with_precision(precision, [&](vb_handle& h, auto tag) {
+      using T = decltype(tag);
+      const T* x_d = upload<T>(dX, xp.data(), M * Cp);
+      dO.ensure(Mo * Cp * sizeof(T));
+      T* o_d = static_cast<T*>(dO.p);
+      timed(iters, elapsed_ms, [&] { dwconv_bn_act<T>(x_d, Cp, t_d, s_d, o_d, Cp, B, H, W, C, Cp, stride, 0); });
+      (void)h;
+      download<T>(o_d, out, Mo * Cp);
+    });
+  });
+}
+
+int vb_op_patch_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t H, int32_t W, int32_t ph, int32_t pw,
+                          int32_t heads, int32_t dh, float scale, float* out, int32_t ldo, int32_t iters, float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    const int HD = heads * dh;
+    VB_CHECK(qkv && out && B > 0 && ph > 0 && pw > 0 && H > 0 && W > 0 && H % ph == 0 && W % pw == 0 && heads > 0 && dh > 0 && ld >= 3 * HD &&
+             ldo >= HD, "vb_op_patch_attention: bad arguments");
+    Window win;                                                   // as mobilevit_block builds it
+    win.p = H / ph; win.pw = W / pw; win.ny = ph; win.nx = pw; win.dilated = 1; win.count = B * ph * pw;
+    const long long rows = static_cast<long long>(B) * H * W;
+    DevMem dX, dO;
+    with_precision(precision, [&](vb_handle& h, auto tag) {
+      using T = decltype(tag);
+      const T* x_d = upload<T>(dX, qkv, static_cast<size_t>(rows) * ld);
+      T* o_d = upload<T>(dO, out, static_cast<size_t>(rows) * ldo);
+      timed(iters, elapsed_ms, [&] {
+        h.arena.reset();
+        h.block_attention<T>(x_d, ld, o_d, ldo, heads, dh, win, 0, scale);
       });
       download<T>(o_d, out, static_cast<size_t>(rows) * ldo);
     });

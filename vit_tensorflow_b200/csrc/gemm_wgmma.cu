@@ -1,7 +1,7 @@
 // Warp-specialised wgmma GEMM for sm_90a with fused epilogues.
 //
 //   out[M,N] (bf16) = epi( A[M,K] (bf16, K-major) x Wt[N,K]^T (bf16, K-major) ),  fp32 accumulation in registers
-//   epi(v) = (+bias[n]) -> exact-erf GELU or hard-swish -> (*scale[n]) -> (+res[m,n])
+//   epi(v) = (+bias[n]) -> exact-erf GELU, hard-swish or SiLU -> (*scale[n]) -> (+res[m,n])
 //
 // Replaces, on the reference's hot path, every nn.Dense: patch embedding (vit.py:143), to_qkv (vit.py:59,72),
 // to_out + residual (vit.py:62-69,101), MLP fc1+GELU / fc2 + residual (vit.py:38-44,102), CaiT to_q/to_kv
@@ -318,6 +318,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           }
           if (ACT == ACT_GELU) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
           if (ACT == ACT_HSWISH) { v0 = hard_swish(v0); v1 = hard_swish(v1); }
+          if (ACT == ACT_SILU) { v0 = silu(v0); v1 = silu(v1); }
           // rounded on its own, as the reference's LayerScale is, never fused with the residual add into one FMA
           if (scale != nullptr) { v0 = __fmul_rn(v0, sc0); v1 = __fmul_rn(v1, sc1); }
           if (OF32) {
@@ -431,6 +432,8 @@ void dispatch(const GemmBf16& g, bool res, int epi, cudaStream_t stream) {
   VB_GEMM_CASE(ACT_NONE, true, 0);  VB_GEMM_CASE(ACT_NONE, true, 1);  VB_GEMM_CASE(ACT_NONE, true, 2);
   VB_GEMM_CASE(ACT_GELU, true, 0);  VB_GEMM_CASE(ACT_GELU, true, 1);  VB_GEMM_CASE(ACT_GELU, true, 2);
   VB_GEMM_CASE(ACT_HSWISH, false, 1);                                  // LeViT MLP fc1 (levit.py:53-54)
+  VB_GEMM_CASE(ACT_SILU, false, 1);                                    // MobileViT Conv_NxN_BN, MV2 expand (mobile_vit.py:41-45,152-155)
+  VB_GEMM_CASE(ACT_SILU, false, 2);                                    // MobileViT MLP fc1, LayerNorm folded (mobile_vit.py:67-70)
 #undef VB_GEMM_CASE
   VB_CHECK(false, "gemm_bf16: no kernel instance for this epilogue (activation " + std::to_string(g.act) + ")");
 }

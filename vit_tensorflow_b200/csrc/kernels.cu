@@ -296,7 +296,8 @@ __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.0f +
 
 // (16*TM)x64 output tile, 16x16 threads x (TM x 4) micro-tile, BK = 16; exact fp32 FMA accumulation in k order.
 // TM = 4: 64-row tiles; TM = 1: 16-row tiles for small-M problems (the classifier head) so the grid still fills the GPU.
-template <typename TA, typename TW, typename TO, int TM>
+// SILU: the SiLU epilogue (act is then ignored), an instance of its own so that the others keep their registers.
+template <typename TA, typename TW, typename TO, int TM, bool SILU = false>
 __global__ void __launch_bounds__(256)
 gemm_simt_kernel(const TA* __restrict__ A, int lda, const TW* __restrict__ W, int wsk, int wsn, TO* out, int ldc, int M, int N,
                  int K, const float* __restrict__ bias, const float* __restrict__ scale, const TO* res, int ldr, int act) {
@@ -352,7 +353,8 @@ gemm_simt_kernel(const TA* __restrict__ A, int lda, const TW* __restrict__ W, in
       if (n >= N) continue;
       float v = acc[i][j];
       if (bias) v += bias[n];
-      if (act == ACT_GELU) v = gelu_erf_f(v);
+      if (SILU) v = silu(v);                                                      // mobile_vit.py:33
+      else if (act == ACT_GELU) v = gelu_erf_f(v);
       else if (act == ACT_HSWISH) v = v * fminf(fmaxf(v + 3.0f, 0.0f), 6.0f) / 6.0f;   // levit.py:37
       if (scale) v *= scale[n];
       if (res) v += to_f(res[static_cast<long long>(m) * ldr + n]);
@@ -1194,10 +1196,12 @@ void gemm_simt(const TA* A, int lda, const TW* W, int wsk, int wsn, TO* out, int
                const float* scale, const TO* res, int ldr, int act, cudaStream_t s) {
   if (static_cast<long long>((N + 63) / 64) * ((M + 63) / 64) >= 2 * sm_count()) {
     const unsigned grid = flat_blocks((N + 63) / 64, (M + 63) / 64, "gemm_simt");
-    gemm_simt_kernel<TA, TW, TO, 4><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act);
+    if (act == ACT_SILU) gemm_simt_kernel<TA, TW, TO, 4, true><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act);
+    else gemm_simt_kernel<TA, TW, TO, 4><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act);
   } else {
     const unsigned grid = flat_blocks((N + 63) / 64, (M + 15) / 16, "gemm_simt");
-    gemm_simt_kernel<TA, TW, TO, 1><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act);
+    if (act == ACT_SILU) gemm_simt_kernel<TA, TW, TO, 1, true><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act);
+    else gemm_simt_kernel<TA, TW, TO, 1><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act);
   }
   VB_LAUNCHED();
 }
@@ -1440,6 +1444,94 @@ void dwconv_qkv(const T* x, int ldx, const float* stats, const float* gamma, con
   VB_LAUNCHED();
 }
 
+// ------------------------------------------------------------------------------------------ MV2 depthwise convolution
+namespace {
+// V channels of one pixel: 8 bf16 in one 16-byte access, or one float (the fp32 engine's unpadded widths); load(const float*)
+// reads V fp32 taps or shifts (two 16-byte accesses for V = 8: Cp and c0 are multiples of 8, w and shift 16-byte aligned)
+template <typename T, int V> struct DwVec;
+template <> struct DwVec<__nv_bfloat16, 8> {
+  static __device__ __forceinline__ void load(const float* p, float (&v)[8]) {   // 8 fp32 taps / shifts, 32-byte aligned
+    const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 1);
+    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+  }
+  static __device__ __forceinline__ void load(const __nv_bfloat16* p, float (&v)[8]) {
+    const uint4 u = __ldg(reinterpret_cast<const uint4*>(p));
+    const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) { const float2 f = __bfloat1622float2(h[i]); v[2 * i] = f.x; v[2 * i + 1] = f.y; }
+  }
+  static __device__ __forceinline__ void store(__nv_bfloat16* p, const float (&v)[8]) {
+    uint4 u;
+    __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&u);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) h[i] = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
+    *reinterpret_cast<uint4*>(p) = u;
+  }
+};
+template <> struct DwVec<float, 1> {
+  static __device__ __forceinline__ void load(const float* p, float (&v)[1]) { v[0] = __ldg(p); }
+  static __device__ __forceinline__ void store(float* p, const float (&v)[1]) { *p = v[0]; }
+};
+
+// One thread per (output pixel, V channels), channel groups fastest so that a warp reads whole pixel rows.  Taps [9][Cp] and the
+// shift [Cp] carry the folded BatchNorm and are zero on the pad channels; groups wholly past C store zeros without reading.
+template <typename T, int V>
+__global__ void __launch_bounds__(256)
+dwconv_bn_act_kernel(const T* __restrict__ x, int ldx, const float* __restrict__ w, const float* __restrict__ shift, T* __restrict__ out,
+                     int ldo, int H, int W, int C, int Cp, int stride, int Ho, int Wo, int pt, int pl, long long total) {
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int G = Cp / V, g = static_cast<int>(idx % G), c0 = g * V;
+  const long long pix = idx / G;
+  const int ox = static_cast<int>(pix % Wo), oy = static_cast<int>(pix / Wo % Ho);
+  const long long b = pix / (static_cast<long long>(Wo) * Ho);
+  float acc[V];
+  if (c0 >= C) {
+#pragma unroll
+    for (int v = 0; v < V; ++v) acc[v] = 0.f;
+    DwVec<T, V>::store(out + pix * ldo + c0, acc);
+    return;
+  }
+  DwVec<T, V>::load(shift + c0, acc);
+#pragma unroll
+  for (int ky = 0; ky < 3; ++ky) {
+    const int iy = oy * stride - pt + ky;
+    if (iy < 0 || iy >= H) continue;
+#pragma unroll
+    for (int kx = 0; kx < 3; ++kx) {
+      const int ix = ox * stride - pl + kx;
+      if (ix < 0 || ix >= W) continue;
+      float xv[V];
+      DwVec<T, V>::load(x + ((b * H + iy) * W + ix) * ldx + c0, xv);
+      float tap[V];
+      DwVec<T, V>::load(w + (ky * 3 + kx) * Cp + c0, tap);
+#pragma unroll
+      for (int v = 0; v < V; ++v) acc[v] = fmaf(xv[v], tap[v], acc[v]);
+    }
+  }
+#pragma unroll
+  for (int v = 0; v < V; ++v) acc[v] = silu(acc[v]);
+  DwVec<T, V>::store(out + pix * ldo + c0, acc);
+}
+}  // namespace
+
+template <typename T>
+void dwconv_bn_act(const T* x, int ldx, const float* w, const float* shift, T* out, int ldo, int B, int H, int W, int C, int Cp, int stride,
+                   cudaStream_t s) {
+  constexpr int V = sizeof(T) == 2 ? 8 : 1;
+  VB_CHECK(stride == 1 || stride == 2, "dwconv_bn_act: stride 1 or 2 only");
+  VB_CHECK(C > 0 && Cp >= C && Cp % V == 0 && ldx >= Cp && ldo >= Cp, "dwconv_bn_act: bad channel widths");
+  VB_CHECK(V == 1 || (ldx % 8 == 0 && ldo % 8 == 0 && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out) |
+                                                       reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(shift)) % 16) == 0),
+           "dwconv_bn_act: bf16 rows need 16-byte aligned pitches and pointers");
+  const int Ho = (H + stride - 1) / stride, Wo = (W + stride - 1) / stride;
+  const int pt = std::max((Ho - 1) * stride + 3 - H, 0) / 2, pl = std::max((Wo - 1) * stride + 3 - W, 0) / 2;   // TF SAME, smaller half first
+  const long long total = static_cast<long long>(B) * Ho * Wo * (Cp / V);
+  dwconv_bn_act_kernel<T, V><<<flat_blocks((total + 255) / 256, 1, "dwconv_bn_act"), 256, 0, s>>>(x, ldx, w, shift, out, ldo, H, W, C, Cp, stride,
+                                                                                               Ho, Wo, pt, pl, total);
+  VB_LAUNCHED();
+}
+
 // ------------------------------------------------------------------------------------------ instantiations
 #define VB_INST_T(T)                                                                                                         \
   template void im2col<T>(const float*, T*, int, int, int, int, int, int, int, int, cudaStream_t);                          \
@@ -1461,7 +1553,8 @@ void dwconv_qkv(const T* x, int ldx, const float* stats, const float* gamma, con
                              cudaStream_t);                                                                                  \
   template void seq_pool<T>(const T*, int, int, const float*, const float*, const float*, const float*, float*, int, cudaStream_t); \
   template void dwconv_qkv<T>(const T*, int, const float*, const float*, const float*, int, float, const float*, const float*, T*, int, \
-                              const float*, const float*, T*, int, int, int, int, int, int, int, cudaStream_t);
+                              const float*, const float*, T*, int, int, int, int, int, int, int, cudaStream_t);            \
+  template void dwconv_bn_act<T>(const T*, int, const float*, const float*, T*, int, int, int, int, int, int, int, cudaStream_t);
 VB_INST_T(float)
 VB_INST_T(__nv_bfloat16)
 

@@ -32,7 +32,7 @@ void transpose_rows_bf16(const __nv_bfloat16* in, int ldi, long long in_batch, _
                          int n, int npad, int cols, cudaStream_t s);
 
 // out[M,N] (TO) = epi(A[M,K] (TA, lda) x W), W element (k,n) at W[k*wsk + n*wsn]; fp32 FMA accumulation.
-// epi = (+bias) -> act (Act: GELU(erf) / hard-swish) -> (*scale) -> (+res[m*ldr + n]).
+// epi = (+bias) -> act (Act: GELU(erf) / hard-swish / SiLU) -> (*scale) -> (+res[m*ldr + n]).
 template <typename TA, typename TW, typename TO>
 void gemm_simt(const TA* A, int lda, const TW* W, int wsk, int wsn, TO* out, int ldc, int M, int N, int K,
                const float* bias, const float* scale, const TO* res, int ldr, int act, cudaStream_t s);
@@ -69,6 +69,15 @@ template <typename T>
 void dwconv_qkv(const T* x, int ldx, const float* stats, const float* gamma, const float* beta, int D, float eps, const float* wq,
                 const float* bq, T* q, int ldq, const float* wkv, const float* bkv, T* kv, int ldkv, int B, int H, int W, int C, int k,
                 int kv_stride, cudaStream_t s);
+
+// MobileViT's MV2 depthwise step (mobile_vit.py:142-145,157-160): a 3 x 3 depthwise convolution with stride 1 or 2 and TF SAME
+// padding (total max((out - 1) * stride + 3 - in, 0), the smaller half first), its BatchNorm folded into the taps and a shift,
+// then SiLU on store.  x [B*H*W, ldx] NHWC rows -> out [B*ceil(H/s)*ceil(W/s), ldo]; w: taps [9][Cp] (row-major window), shift
+// [Cp], both zero on channels >= C; columns [C, Cp) of out are written as zero.  bf16: 8 channels per thread in 16-byte
+// accesses (Cp, ldx, ldo multiples of 8); fp32: one channel per thread.
+template <typename T>
+void dwconv_bn_act(const T* x, int ldx, const float* w, const float* shift, T* out, int ldo, int B, int H, int W, int C, int Cp, int stride,
+                   cudaStream_t s);
 
 // z[b,:] = LN(pool(X[b]))  with pool = row 0 (cls) or mean over the n rows; fp32 out [B, D].  gamma == null: no LayerNorm.
 template <typename T>

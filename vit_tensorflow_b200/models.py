@@ -1704,8 +1704,110 @@ REGIONVIT_CTOR_KEYS = ("dim", "depth", "window_size", "num_classes", "tokenize_l
                        "attn_dropout", "ff_dropout")
 
 
+def mobilevit_size_error(h, w, ph, pw):
+    """The reference's regrouping rule (mobile_vit.py:196, enforced there by einops) for an h x w image: None, or what the first
+    trunk stage that breaks it says.  conv1 and the second stem block halve the map (SAME: ceil), each trunk stage halves it again."""
+    h, w = -(-h // 4), -(-w // 4)
+    for s in range(3):
+        h, w = -(-h // 2), -(-w // 2)
+        if h % ph or w % pw:
+            return (f"MobileViT stage {s + 1}: the {h} x {w} map is not divisible by patch_size ({ph}, {pw}); every trunk map (1/8, 1/16 "
+                    "and 1/32 of the image, rounded up) must be")
+    return None
+
+
+def mobilevit_blocks(channels, expansion):
+    """The seven MV2 blocks as mobile_vit.py:233-252 builds them: (attribute path, actual input width, hidden, output width, stride,
+    expand, residual).  Keras infers input widths, so the reference's dim_in sets only hidden = int(dim_in * expansion) and the
+    residual test; the fourth stem block is built as MV2Block(channels[2], channels[3]) but reads channels[3] channels."""
+    c = channels
+    spec = [("stem.0", c[0], c[0], c[1], 1), ("stem.1", c[1], c[1], c[2], 2), ("stem.2", c[2], c[2], c[3], 1), ("stem.3", c[2], c[3], c[3], 1),
+            ("trunk.0.0", c[3], c[3], c[4], 2), ("trunk.1.0", c[5], c[5], c[6], 2), ("trunk.2.0", c[7], c[7], c[8], 2)]
+    out = []
+    for path, dim_in, cin, cout, stride in spec:
+        hidden = int(dim_in * expansion)
+        if expansion == 1 and hidden != cin:
+            raise ValueError(f"MobileViT {path}: with expansion 1 the block is MV2Block({dim_in}, {cout}) whose depthwise convolution has "
+                             f"{hidden} filters with groups={hidden}, but its input has {cin} channels (channels[2] != channels[3]); "
+                             "the reference builds a grouped convolution or fails there")
+        out.append((path, cin, hidden, cout, stride, expansion != 1, stride == 1 and dim_in == cout))
+    return out
+
+
+class MobileViT(_EngineModel):
+    """mobile_vit.py:209-271: a stride-2 Conv_NxN_BN, four MobileNetV2 blocks (1x1 expand, 3x3 depthwise, 1x1 project, BatchNorm and
+    SiLU), three trunk stages of a stride-2 MV2 block and a MobileViTBlock (k x k and 1x1 convolutions, a Transformer of 4 heads of 8
+    within each of the ph * pw patch positions, a 1x1 convolution back, the concat with the block's input and a k x k convolution),
+    then a 1x1 Conv_NxN_BN, the mean over pixels and a bias-free Dense.
+
+    Inference only: the reference's call defaults to training=True, which makes every BatchNormalization use the batch's statistics;
+    a call without training=False raises NotImplementedError here.  Every trunk map (1/8, 1/16 and 1/32 of the image, rounded up)
+    must be divisible by patch_size: other image sizes raise ValueError naming the stage, at construction and at call time.  With
+    expansion 1 and channels[2] != channels[3] the fourth stem block is refused (ValueError).
+    Weights (SURVEY.md App. B) keep the reference's attribute paths: conv1.layers.{0,1} (Conv2D, BatchNormalization),
+    stem.{i}.conv.{j} and trunk.{s}.0.conv.{j} (MV2 blocks: j = 0, 1, 3, 4, 6, 7 with the expand convolution, 0, 1, 3, 4 without),
+    trunk.{s}.1.conv{1,2,3,4}.layers.{0,1}, trunk.{s}.1.transformer.layers.{l}.0.{norm, fn.to_qkv, fn.to_out.0},
+    trunk.{s}.1.transformer.layers.{l}.1.{norm, fn.net.0, fn.net.3}, to_logits.0.layers.{0,1}, to_logits.2 (the Dense head)."""
+    _kind = "mobilevit"
+
+    def __init__(self, image_size, dims, channels, num_classes, expansion=4, kernel_size=3, patch_size=(2, 2), depths=(2, 4, 3),
+                 *, precision="bf16", device=0, seed=None):
+        assert len(dims) == 3, 'dims must be a tuple of 3'
+        assert len(depths) == 3, 'depths must be a tuple of 3'
+        ih, iw = image_size
+        ph, pw = patch_size
+        assert ih % ph == 0 and iw % pw == 0
+        init_dim, *_, last_dim = channels
+        err = mobilevit_size_error(ih, iw, ph, pw)
+        if err is not None:
+            raise ValueError(err + " (the reference fails at its first call)")
+        self.num_classes, self.image_size, self.patch_size = num_classes, (ih, iw), (ph, pw)
+        self.blocks = mobilevit_blocks(channels, expansion)
+        mc = _lib.VbMobilevitConfig()
+        mc.struct_size = C.sizeof(_lib.VbMobilevitConfig)
+        for i in range(10):
+            mc.channels[i] = int(channels[i])
+        mc.last_dim = int(last_dim)
+        for i in range(3):
+            mc.dims[i], mc.depths[i] = int(dims[i]), int(depths[i])
+        mc.kernel_size, mc.ph, mc.pw = int(kernel_size), int(ph), int(pw)
+        for i, (_, cin, hidden, cout, stride, expand, residual) in enumerate(self.blocks):
+            mc.mv2_in[i], mc.mv2_hidden[i], mc.mv2_out[i], mc.mv2_stride[i] = cin, hidden, cout, stride
+            mc.mv2_expand[i], mc.mv2_residual[i] = int(expand), int(residual)
+        self._mc = mc
+        lib = _lib.load()
+        self._create(precision, device, create=lambda cfg, dev, h: lib.vb_create_mobilevit(cfg, C.byref(mc), dev, h),
+                     image_h=ih, image_w=iw, num_classes=num_classes, dim=last_dim)
+        self.init_weights(seed)
+
+    init_weights = CvT.init_weights      # the same initialisers: glorot over the receptive field, zero biases, BatchNorm 1 / 0 / 0 / 1
+
+    def _check_training(self, training):
+        if training is None or training:
+            raise NotImplementedError(
+                "MobileViT runs inference only: with training=True (the reference's default, mobile_vit.py:260) every BatchNormalization "
+                "normalises with the batch's own statistics; pass training=False")
+
+    def __call__(self, img, training=True, **kwargs):
+        """mobile_vit.py:260-271: NHWC float images -> logits [b, num_classes].  training must be False."""
+        self._check_training(training)
+        x = np.asarray(img)
+        if x.ndim == 4:
+            err = mobilevit_size_error(x.shape[1], x.shape[2], *self.patch_size)
+            if err is not None:
+                raise ValueError(err)
+        return super().__call__(img, training=False)
+
+    call = __call__
+
+
+MOBILEVIT_CTOR_KEYS = ("image_size", "dims", "channels", "num_classes", "expansion", "kernel_size", "patch_size", "depths")
+
+
 def from_config(cfg: dict, precision="bf16", device=0, seed=None):
     """Build a model from an oracle-style config dict (kind + reference kwargs)."""
+    if cfg["kind"] == "mobilevit":
+        return MobileViT(**{k: v for k, v in cfg.items() if k in MOBILEVIT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "small_dataset_vit":
         return SmallDatasetViT(**{k: v for k, v in cfg.items() if k in SMALL_DATASET_VIT_CTOR_KEYS}, precision=precision, device=device,
                                seed=seed)
