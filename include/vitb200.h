@@ -16,6 +16,7 @@
  *     CrossFormer(...)(img)          vit_tensorflow/crossformer.py:205-269 (vb_create_crossformer)
  *     NesT(...)(img)                 vit_tensorflow/nest.py:150-216 (vb_create_nest)
  *     RegionViT(...)(img)            vit_tensorflow/regionvit.py:184-263 (vb_create_regionvit)
+ *     ScalableViT(...)(img)          vit_tensorflow/scalable_vit.py:250-319 (vb_create_scalable_vit)
  * and this header is what the Python host classes (vit_tensorflow_b200/models.py, _lib.py) bind with ctypes.
  * Plain pointers and sizes only; no torch / C++ types cross the boundary.
  *
@@ -47,7 +48,8 @@ typedef struct vb_handle vb_handle;
 enum { VB_KIND_VIT = 0, VB_KIND_DEEPVIT = 1, VB_KIND_CAIT = 2, VB_KIND_CROSSVIT = 3, VB_KIND_PARALLEL_VIT = 4,
        VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6, VB_KIND_CCT = 7, VB_KIND_LEVIT = 8,
        VB_KIND_CVT = 9, VB_KIND_TWINS_SVT = 10, VB_KIND_CROSSFORMER = 11, VB_KIND_NEST = 12, VB_KIND_REGIONVIT = 13,
-       VB_KIND_ATS_VIT = 14, VB_KIND_SMALL_DATASET_VIT = 15, VB_KIND_MOBILEVIT = 16 };
+       VB_KIND_ATS_VIT = 14, VB_KIND_SMALL_DATASET_VIT = 15, VB_KIND_MOBILEVIT = 16,
+       VB_KIND_SCALABLE_VIT = 17 };
 enum { VB_CCT_POS_SINE = 0, VB_CCT_POS_LEARNABLE = 1, VB_CCT_POS_NONE = 2 };   /* cct.py:233-234,250-256 */
 enum { VB_PRECISION_FP32 = 0, VB_PRECISION_BF16 = 1 };
 enum { VB_POOL_CLS = 0, VB_POOL_MEAN = 1 };
@@ -670,6 +672,45 @@ VB_API int vb_op_mv2_dwconv(int32_t precision, const float* x, int32_t B, int32_
  * materialised-scores path and permute back (vb_last_attention_path tells which). */
 VB_API int vb_op_patch_attention(int32_t precision, const float* qkv, int32_t ld, int32_t B, int32_t H, int32_t W, int32_t ph, int32_t pw,
                                  int32_t heads, int32_t dh, float scale, float* out, int32_t ldo, int32_t iters, float* elapsed_ms);
+
+/* ScalableViT (scalable_vit.py:250-319), appended within ABI 7.  to_patches: Conv2D(dim[0], 7, stride 4, SAME, bias); stage s <
+ * num_stages: a Transformer of depth[s] blocks on the dim[s] = dim * 2^s map, its own LayerNorm (eps 1e-5), then (s < num_stages - 1)
+ * Downsample: Conv2D(dim[s + 1], 3, stride 2, SAME, bias); the head: the mean over pixels, LayerNormalization (eps 1e-3), Dense.
+ * Each block is built [SSA, MLP, PEG (first block only), MLP, IWSA] (:222-231) but unpacked as ssa, ff1, peg, iwsa, ff2 (:236), so
+ * it runs x = SSA(LN x) + x, x = MLP(LN x) + x, x = PEG(x), x = MLP(LN x) + x, x = IWSA(LN x) + x, every LN the model's own
+ * (biased variance, eps 1e-5).  SSA (:104-143): q a bias-free 1x1 convolution to heads * ssa_dim_key, k and v bias-free r x r
+ * stride-r VALID convolutions to heads * ssa_dim_key / ssa_dim_value (r = reduction_factor), softmax(q k^T * ssa_dim_key^-0.5) v,
+ * to_out a 1x1 convolution with bias.  IWSA (:145-198): bias-free 1x1 q / k / v, attention within window x window windows (0:
+ * the whole map), plus LIM(v), a full 3x3 SAME convolution with bias over v's heads * iwsa_dim_value channels, then to_out.  MLP:
+ * 1x1 convolution to ff_expansion_factor * dim[s], exact-erf GELU, 1x1 convolution back, both with bias.  PEG: x + a depthwise 3x3
+ * SAME convolution with bias.  Any image size runs whose stage maps (ceil(H / 4), then ceil(/ 2) per stage) are at least
+ * reduction_factor on each side and divisible by their window. */
+#define VB_SCALABLE_VIT_STAGES 4
+typedef struct vb_scalable_vit_config {
+  int32_t struct_size;            /* sizeof(vb_scalable_vit_config) */
+  int32_t num_stages;             /* 1 to VB_SCALABLE_VIT_STAGES */
+  int32_t dim[VB_SCALABLE_VIT_STAGES], depth[VB_SCALABLE_VIT_STAGES], heads[VB_SCALABLE_VIT_STAGES];
+  int32_t ssa_dim_key[VB_SCALABLE_VIT_STAGES], ssa_dim_value[VB_SCALABLE_VIT_STAGES], reduction_factor[VB_SCALABLE_VIT_STAGES];
+  int32_t iwsa_dim_key[VB_SCALABLE_VIT_STAGES], iwsa_dim_value[VB_SCALABLE_VIT_STAGES];
+  int32_t window[VB_SCALABLE_VIT_STAGES];   /* 0: the whole map is one window (window_size None) */
+  int32_t ff_expansion_factor;
+} vb_scalable_vit_config;
+
+/* ScalableViT.__init__: `base` supplies precision, channels, num_classes and max_batch; its kind must be VB_KIND_SCALABLE_VIT and
+ * its other fields are ignored.  Weights (SURVEY.md App. B) are named by the reference's attribute paths (d = dim[s], h = heads[s],
+ * the reference's LayerNorm leaves .g / .b of shape [1, 1, 1, d]); block l of stage s is scalable_layers.{s}.0.layers.{l}.{j} with
+ * j the construction index:
+ *   to_patches.kernel [7, 7, channels, dim[0]] / .bias
+ *   j = 0 (SSA): .0.norm.g / .b, .0.fn.to_q.kernel [1, 1, d, h dk], .0.fn.to_k.kernel [r, r, d, h dk], .0.fn.to_v.kernel [r, r, d,
+ *     h dv], .0.fn.to_out.0.kernel [1, 1, h dv, d] / .bias
+ *   j = 1, 3 (MLP): .norm.g / .b, .fn.net.0.kernel [1, 1, d, f d] / .bias, .fn.net.3.kernel [1, 1, f d, d] / .bias
+ *   j = 2 (PEG, l = 0 only): .proj.kernel [3, 3, 1, d] / .bias
+ *   j = 4 (IWSA): .4.norm.g / .b, .4.fn.local_interactive_module.kernel [3, 3, h dv, h dv] / .bias, .4.fn.to_q.kernel / .to_k.kernel
+ *     [1, 1, d, h dk], .4.fn.to_v.kernel [1, 1, d, h dv], .4.fn.to_out.0.kernel [1, 1, h dv, d] / .bias
+ *   scalable_layers.{s}.0.norm.g / .b; scalable_layers.{s}.1.conv.kernel [3, 3, d, 2 d] / .bias (s < num_stages - 1)
+ *   mlp_head.1.gamma / .beta [dim[-1]], mlp_head.2.kernel [dim[-1], num_classes] / .bias
+ * vb_forward only: the stage entries and vb_forward_distill refuse the handle. */
+VB_API int vb_create_scalable_vit(const vb_config* base, const vb_scalable_vit_config* sv, int device, vb_handle** out);
 
 /* Row softmax of fp32 scores into bf16 probabilities (the T2T attention): p[r, j] = softmax_j(s[r, j] * scale) for j < n,
  * p[r, n..npad) = 0.  s [rows, lds], p [rows, ldp] (uploaded and downloaded whole); n <= npad <= ldp. */

@@ -13,7 +13,7 @@ LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "libvitb200.so")
 
 KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6, "cct": 7, "levit": 8,
         "cvt": 9, "twins_svt": 10, "crossformer": 11, "nest": 12, "regionvit": 13, "ats_vit": 14,
-        "small_dataset_vit": 15, "mobilevit": 16}
+        "small_dataset_vit": 15, "mobilevit": 16, "scalable_vit": 17}
 PRECISION = {"fp32": 0, "float32": 0, "bf16": 1, "bfloat16": 1}
 MEM_HOST, MEM_DEVICE = 0, 1
 ABI_VERSION = 7                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
@@ -100,6 +100,16 @@ class VbMobilevitConfig(C.Structure):
                [(f, C.c_int32 * MOBILEVIT_MV2) for f in ("mv2_in", "mv2_hidden", "mv2_out", "mv2_stride", "mv2_expand", "mv2_residual")]
 
 
+SCALABLE_VIT_STAGES = 4                              # VB_SCALABLE_VIT_STAGES
+
+
+class VbScalableVitConfig(C.Structure):
+    _fields_ = ([("struct_size", C.c_int32), ("num_stages", C.c_int32)] +
+                [(f, C.c_int32 * SCALABLE_VIT_STAGES) for f in ("dim", "depth", "heads", "ssa_dim_key", "ssa_dim_value", "reduction_factor",
+                                                                "iwsa_dim_key", "iwsa_dim_value", "window")] +
+                [("ff_expansion_factor", C.c_int32)])
+
+
 class VbError(RuntimeError):
     pass
 
@@ -119,6 +129,7 @@ SIGNATURES = {
     "vb_create_regionvit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbRegionvitConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_ats_vit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbAtsVitConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_mobilevit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbMobilevitConfig), C.c_int, C.POINTER(C.c_void_p)]),
+    "vb_create_scalable_vit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbScalableVitConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_op_mv2_dwconv": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p] * 3 + [C.c_int32, _f32p]),
     "vb_op_patch_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 8 + [C.c_float, C.c_void_p, C.c_int32, C.c_int32, _f32p]),
     "vb_ats_set_seed": (C.c_int, [C.c_void_p, C.c_uint64]),

@@ -1,4 +1,5 @@
-// Tensor-core multi-head attention for the bf16 engine (bf16 operands, fp32 accumulation, dim_head = 64; 32 in the windowed-bias and block forms).
+// Tensor-core multi-head attention for the bf16 engine (bf16 operands, fp32 accumulation, dim_head = 64; 32 in the windowed-bias and
+// block forms and in the plain streaming form).
 //
 //   out[b, i, h, :] = softmax_j( scale * q[b,i,h,:] . k[b,j,h,:] ) @ v[b,j,h,:]        (vit.py:77-82)
 //
@@ -29,6 +30,10 @@
 // rectangular bh x bw blocks (Window::pw), reached only through attention_block.  NesT's 14 x 14 blocks of 196 tokens take four
 // query tiles and four key blocks each.  MobileViT's patch-position groups (mobile_vit.py:196-199) are dilated rectangular windows
 // of the same form: the kernel reads every row through Window::row.
+//
+// Plain attention at head width 32 (ScalableViT's scalable self-attention, scalable_vit.py:123-143: h x w queries against the keys of
+// an r x r stride-r convolution, nq != nk) runs the streaming form above, attn_flash_kernel<32, false, false>; the resident form
+// below stays at 64.
 //
 // RegionViT's regional-to-local attention (attn_r2l_kernel, attention_r2l below) is a kernel of its own with the same tiles and
 // online softmax: each window attends together with one regional row from elsewhere in the rows, under a per-head window table.
@@ -796,13 +801,14 @@ bool attention_fast<__nv_bfloat16>(const __nv_bfloat16* q, int ldq, const __nv_b
   if (nq == 1 && pb == nullptr && win == nullptr && attention_cls(q, ldq, k, ldk, v, ldv, out, ldo, B, nk, heads, dh, variant, mix_a, mix_b, ln_g, ln_b, s, scale)) return true;
   // DeepViT re-attention / CaiT talking heads: the materialised-scores path (attn_generic_mma.cu) -- a fused form with all heads'
   // scores of a 16-row tile in shared memory measured 9-11 % slower on the H100 (one CTA per SM at 16 heads)
-  if (variant != 0 || dh != DH || (nq < 2 && pb == nullptr)) return false;
+  const bool narrow = dh == 32 && pb == nullptr && win == nullptr;   // plain attention at head width 32: the streaming kernel
+  if (variant != 0 || (dh != DH && !narrow) || (nq < 2 && pb == nullptr)) return false;
   if (pb != nullptr && (pb->fmap * pb->fmap > FLASH_BIAS_MAX || nk != pb->fmap * pb->fmap || nq != pb->q_side() * pb->q_side())) return false;
   if ((ldq % 8) || (ldk % 8) || (ldv % 8) || (ldo % 2)) return false;
   if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
        reinterpret_cast<uintptr_t>(out)) % 16) return false;
   const float scale_log2 = (scale > 0.f ? scale : 1.0f / sqrtf(static_cast<float>(dh))) * 1.4426950408889634f;
-  if (pb == nullptr && win == nullptr && attention_resident(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, heads, scale_log2, s)) {
+  if (pb == nullptr && win == nullptr && !narrow && attention_resident(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, heads, scale_log2, s)) {
     count_launch();
     note_attention_path(ATTN_PATH_FLASH);
     return true;
@@ -831,6 +837,9 @@ bool attention_fast<__nv_bfloat16>(const __nv_bfloat16* q, int ldq, const __nv_b
   else if (win != nullptr)
     VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<DH, false, true>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
                                static_cast<const float*>(nullptr), 0, 1, 0, *win, static_cast<const int*>(nullptr)));
+  else if (narrow)
+    VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<32, false, false>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
+                               static_cast<const float*>(nullptr), 0, 1, 0, Window(), static_cast<const int*>(nullptr)));
   else
     VB_CUDA(cudaLaunchKernelEx(&cfg, attn_flash_kernel<DH, false, false>, q, ldq, k, ldk, v, ldv, out, ldo, heads, nq, nk, scale_log2,
                                static_cast<const float*>(nullptr), 0, 1, 0, Window(), static_cast<const int*>(nullptr)));

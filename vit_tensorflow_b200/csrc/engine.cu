@@ -247,6 +247,31 @@ struct MvitBlockW {                  // one MobileViTBlock (:173-206): the conca
   std::vector<MvitLayerW> layers;
 };
 
+// ScalableViT (scalable_vit.py:145-304) on channel rows zero-padded to channel_width (bf16) / unpadded (fp32).  q, k and v of each
+// attention share one activation head width (SvitStageW::dhs / dhi): the largest of dim_key and dim_value, widened in bf16 to the
+// flash kernels' 32 or 64 (or a multiple of 8 above 64) with zero weight columns; the to_out rows and the LIM's input rows and
+// output columns follow the same head layout, with zero rows and columns at the pad positions.
+struct SvitBlockW {                  // one block, in the order it runs (:236-245)
+  Norm ssa_norm, iwsa_norm;          // g / b [dp], zero on pad channels
+  Linear ssa_q;                      // [dp, ldq]: q at h * dhs
+  Linear ssa_kv;                     // [r * r * dim, ldkv] over unfold's (row, column, channel) vectors: k at h * dhs, v at HS + h * dhs
+  Linear ssa_out;                    // [ldq, dp]
+  MlpW mlp1, mlp3;                   // construction elements 1 and 3
+  const float *peg_w = nullptr, *peg_b = nullptr;   // element 2 (first block only): taps [9][dp] with the residual on the centre tap
+  Linear iwsa_qkv;                   // [dp, ldqkv]: q | k | v, each HI = heads * dhi wide
+  Linear lim;                        // [9 HI, ldlim] over unfold's vectors of v's HI channels
+  Linear iwsa_out;                   // [ldlim, dp]
+};
+struct SvitStageW {
+  int dim = 0, dp = 0, heads = 0, r = 1, window = 0, dhs = 0, dhi = 0;
+  int ldq = 0, ldkv = 0, ldqkv = 0, ldlim = 0;   // row pitches of the SSA q (and its output), k|v, IWSA q|k|v and LIM output
+  float ssa_scale = 0.f, iwsa_scale = 0.f;       // dim_key^-0.5 of the model
+  std::vector<SvitBlockW> blocks;
+  Norm norm;                         // the Transformer's LayerNorm (norm_output, :233)
+  bool down = false;
+  Linear down_conv;                  // Downsample (:71-78): [9 dim, channel_width(2 dim)] over unfold's vectors
+};
+
 // NesT's block attention and MobileViT's patch-position attention on the windowed flash kernel (attn_flash.cu): bf16 only, false
 // for a shape it does not take.
 inline bool block_attention_fast(const float*, int, float*, int, int, int, cudaStream_t, const Window&, float) { return false; }
@@ -609,6 +634,17 @@ struct vb_handle {
   int mvit_mlp(int s) const { return mv.dims[s] * (s == 0 ? 2 : 4); }            // mobile_vit.py:241,246,251
   static constexpr int kMvHeads = 4, kMvDh = 8;                                    // MobileViTBlock's Transformer (:182)
   int mvit_dh() const { return bf16() ? 32 : kMvDh; }                             // bf16: heads widened to the flash kernel's 32
+  // ScalableViT (scalable_vit.py:250-319): to_patches (`sv_stem`), the stages, the head LayerNormalization (`head_norm`) and Dense
+  vb_scalable_vit_config sv{};
+  Linear sv_stem;
+  std::vector<SvitStageW> sv_stages;
+  static std::string sv_pre(int s) { return "scalable_layers." + std::to_string(s) + "."; }
+  int sv_dim(int s) const { return sv.dim[0] << s; }
+  // activation head width of an attention whose keys are dk and values dv wide (SvitStageW)
+  int sv_head_width(int dk, int dv) const {
+    const int m = std::max(dk, dv);
+    return !bf16() ? m : m <= 32 ? 32 : m <= 64 ? 64 : round_up(m, 8);
+  }
   Norm head_norm, sm_head_norm, lg_head_norm;
   Linear head, sm_head, lg_head;
   Norm spt_norm;                     // SPT's LayerNorm over the p^2 * 5 C patch vector (bf16: padded to the GEMM's K, folded into it)
@@ -979,6 +1015,44 @@ struct vb_handle {
       }
       expect_cbn("to_logits.0", 1, mv.channels[9], mv.last_dim);         // :254-258
       expect("to_logits.2.kernel", {mv.last_dim, c.num_classes});
+    } else if (c.kind == VB_KIND_SCALABLE_VIT) {
+      auto expect_ln4 = [&](const std::string& n, int d) { expect(n + ".g", {1, 1, 1, d}); expect(n + ".b", {1, 1, 1, d}); };   // :46-52
+      auto expect_conv = [&](const std::string& n, int k, int cin, int cout, bool bias) {
+        expect(n + ".kernel", {k, k, cin, cout});
+        if (bias) expect(n + ".bias", {cout});
+      };
+      expect_conv("to_patches", 7, c.channels, sv.dim[0], true);        // :261
+      for (int st = 0; st < sv.num_stages; ++st) {
+        const int d = sv_dim(st), h = sv.heads[st], r = sv.reduction_factor[st], f = sv.ff_expansion_factor;
+        const int sk = sv.ssa_dim_key[st], svv = sv.ssa_dim_value[st], ik = sv.iwsa_dim_key[st], iv = sv.iwsa_dim_value[st];
+        for (int L = 0; L < sv.depth[st]; ++L) {
+          const std::string b = sv_pre(st) + "0.layers." + std::to_string(L) + ".";
+          auto expect_mlp = [&](const std::string& m) {                  // PreNorm(MLP) :61-69, :89-102
+            expect_ln4(m + "norm", d);
+            expect_conv(m + "fn.net.0", 1, d, f * d, true);
+            expect_conv(m + "fn.net.3", 1, f * d, d, true);
+          };
+          expect_ln4(b + "0.norm", d);                                   // ScalableSelfAttention :104-121
+          expect_conv(b + "0.fn.to_q", 1, d, h * sk, false);
+          expect_conv(b + "0.fn.to_k", r, d, h * sk, false);
+          expect_conv(b + "0.fn.to_v", r, d, h * svv, false);
+          expect_conv(b + "0.fn.to_out.0", 1, h * svv, d, true);
+          expect_mlp(b + "1.");
+          if (L == 0) expect_conv(b + "2.proj", 3, 1, d, true);          // PEG :80-87 (groups = dim)
+          expect_mlp(b + "3.");
+          expect_ln4(b + "4.norm", d);                                   // InteractiveWindowedSelfAttention :145-163
+          expect_conv(b + "4.fn.local_interactive_module", 3, h * iv, h * iv, true);
+          expect_conv(b + "4.fn.to_q", 1, d, h * ik, false);
+          expect_conv(b + "4.fn.to_k", 1, d, h * ik, false);
+          expect_conv(b + "4.fn.to_v", 1, d, h * iv, false);
+          expect_conv(b + "4.fn.to_out.0", 1, h * iv, d, true);
+        }
+        expect_ln4(sv_pre(st) + "0.norm", d);                            // :233
+        if (st < sv.num_stages - 1) expect_conv(sv_pre(st) + "1.conv", 3, d, 2 * d, true);   // Downsample :71-78
+      }
+      const int dl = sv_dim(sv.num_stages - 1);
+      expect_ln("mlp_head.1", dl);                                       // :302-306
+      expect_dense("mlp_head.2", dl, c.num_classes);
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       expect("pos_embedding", {1, np, c.dim});
@@ -1212,7 +1286,7 @@ struct vb_handle {
     VB_CUDA(cudaSetDevice(device));
     owned.clear(); layers.clear(); cls_layers.clear(); t2t_layers.clear(); xblocks.clear(); plans.clear(); embed_res.clear(); cct_convs.clear();
     lv_stem.clear(); lv_blocks.clear(); cvt_stages.clear(); twins_stages.clear(); cf_stages.clear(); nest_levels.clear(); rv_stages.clear();
-    mv_mv2.clear(); mv_vit.clear();
+    mv_mv2.clear(); mv_vit.clear(); sv_stages.clear();
     woverride.clear();
     drop_graphs();
     const vb_config& c = cfg;
@@ -1277,6 +1351,8 @@ struct vb_handle {
       finalize_regionvit();
     } else if (c.kind == VB_KIND_MOBILEVIT) {
       finalize_mobilevit();
+    } else if (c.kind == VB_KIND_SCALABLE_VIT) {
+      finalize_scalable_vit();
     } else if (c.kind == VB_KIND_CAIT) {
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       embed = make_embed("", c.patch_h, c.patch_w, c.dim, np, false);
@@ -1801,6 +1877,90 @@ struct vb_handle {
     mv_logits = mv_cbn("to_logits.0", 1, mv.channels[9], mv.last_dim, channel_width(mv.channels[9]));
     head = Linear();
     head.W = W("to_logits.2.kernel"); head.K = mv.last_dim; head.N = cfg.num_classes; head.ldw = mv.last_dim;   // Dense without bias
+  }
+
+  // ---- ScalableViT weight packing: q, k and v in the stage's head layout (SvitStageW), channel widths zero-padded (bf16), the PEG
+  // residual folded, the pre-norm LayerNorms (eps 1e-5) folded into the SSA q and IWSA q|k|v GEMMs in the bf16 engine
+  // The [K, heads * w] kernel `src` into dst [.., N]: its row k at row rowmap(k), head h's column j at column off + h * dh + j
+  template <typename RowMap>
+  static void sv_place(const std::vector<double>& src, int K, int heads, int w, std::vector<double>& dst, int N, int off, int dh,
+                       RowMap rowmap) {
+    for (int k = 0; k < K; ++k)
+      for (int h = 0; h < heads; ++h)
+        for (int j = 0; j < w; ++j) dst[static_cast<size_t>(rowmap(k)) * N + off + h * dh + j] = src[(static_cast<size_t>(k) * heads + h) * w + j];
+  }
+  Linear sv_folded(const std::string& key, const std::vector<double>& Wkn, int K, int N, const Norm& norm, int d) {
+    Linear L = linear_from_host(key, Wkn, {}, K, N, bf16() ? &norm : nullptr);
+    L.ln_d = d;
+    L.ln_eps = 1e-5f;                                                // scalable_vit.py:47
+    return L;
+  }
+  // to_out `n` [heads * w, d] + bias as [K, dp]: head h's row j at row h * dh + j, the other rows zero
+  Linear sv_head_rows(const std::string& key, const std::string& n, int heads, int w, int dh, int K, int d, int dp) {
+    const auto src = host_weight(n + ".kernel");
+    std::vector<double> Wo(static_cast<size_t>(K) * dp, 0.0);
+    for (int h = 0; h < heads; ++h)
+      for (int j = 0; j < w; ++j)
+        for (int o = 0; o < d; ++o) Wo[(static_cast<size_t>(h) * dh + j) * dp + o] = src[(static_cast<size_t>(h) * w + j) * d + o];
+    return linear_from_host(key, Wo, pad_n(host_weight(n + ".bias"), dp), K, dp);
+  }
+  void finalize_scalable_vit() {
+    const int C = cfg.channels, d0 = sv.dim[0];
+    sv_stem = padded_dense("sv.to_patches", "to_patches", 49 * C, d0, 49 * C, channel_width(d0));   // :261
+    const auto same = [](int k) { return k; };
+    for (int st = 0; st < sv.num_stages; ++st) {
+      SvitStageW S;
+      const std::string p = sv_pre(st);
+      const int d = sv_dim(st), dp = channel_width(d), H = sv.heads[st], r = sv.reduction_factor[st], f = sv.ff_expansion_factor;
+      const int sk = sv.ssa_dim_key[st], svv = sv.ssa_dim_value[st], ik = sv.iwsa_dim_key[st], iv = sv.iwsa_dim_value[st];
+      S.dim = d; S.dp = dp; S.heads = H; S.r = r; S.window = sv.window[st];
+      S.dhs = sv_head_width(sk, svv); S.dhi = sv_head_width(ik, iv);
+      const int HS = H * S.dhs, HI = H * S.dhi;
+      S.ldq = channel_width(HS); S.ldkv = channel_width(2 * HS); S.ldqkv = channel_width(3 * HI); S.ldlim = channel_width(HI);
+      S.ssa_scale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(sk)));    // :109, :151
+      S.iwsa_scale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(ik)));
+      for (int L = 0; L < sv.depth[st]; ++L) {
+        const std::string b = p + "0.layers." + std::to_string(L) + ".", key = "sv." + b;
+        SvitBlockW w;
+        w.ssa_norm = padded_norm(b + "0.norm", d, dp);
+        std::vector<double> Wq(static_cast<size_t>(dp) * S.ldq, 0.0);
+        sv_place(host_weight(b + "0.fn.to_q.kernel"), d, H, sk, Wq, S.ldq, 0, S.dhs, same);
+        w.ssa_q = sv_folded(key + "ssa_q", Wq, dp, S.ldq, w.ssa_norm, d);
+        std::vector<double> Wkv(static_cast<size_t>(r) * r * d * S.ldkv, 0.0);
+        sv_place(host_weight(b + "0.fn.to_k.kernel"), r * r * d, H, sk, Wkv, S.ldkv, 0, S.dhs, same);
+        sv_place(host_weight(b + "0.fn.to_v.kernel"), r * r * d, H, svv, Wkv, S.ldkv, HS, S.dhs, same);
+        w.ssa_kv = linear_from_host(key + "ssa_kv", Wkv, {}, r * r * d, S.ldkv);
+        w.ssa_out = sv_head_rows(key + "ssa_out", b + "0.fn.to_out.0", H, svv, S.dhs, S.ldq, d, dp);
+        w.mlp1 = prenorm_mlp("sv.", b + "1.norm", b + "1.fn.net.0", b + "1.fn.net.3", d, dp, f);
+        if (L == 0) {
+          w.peg_w = peg_taps(host_weight(b + "2.proj.kernel"), 3, d, dp);
+          w.peg_b = upload_owned(pad_n(host_weight(b + "2.proj.bias"), dp));
+        }
+        w.mlp3 = prenorm_mlp("sv.", b + "3.norm", b + "3.fn.net.0", b + "3.fn.net.3", d, dp, f);
+        w.iwsa_norm = padded_norm(b + "4.norm", d, dp);
+        std::vector<double> Wqkv(static_cast<size_t>(dp) * S.ldqkv, 0.0);
+        sv_place(host_weight(b + "4.fn.to_q.kernel"), d, H, ik, Wqkv, S.ldqkv, 0, S.dhi, same);
+        sv_place(host_weight(b + "4.fn.to_k.kernel"), d, H, ik, Wqkv, S.ldqkv, HI, S.dhi, same);
+        sv_place(host_weight(b + "4.fn.to_v.kernel"), d, H, iv, Wqkv, S.ldqkv, 2 * HI, S.dhi, same);
+        w.iwsa_qkv = sv_folded(key + "iwsa_qkv", Wqkv, dp, S.ldqkv, w.iwsa_norm, d);
+        // the LIM's input channel c = h iv + j of tap t is row t HI + h dhi + j; its output channels take the same head layout
+        std::vector<double> Wl(static_cast<size_t>(9) * HI * S.ldlim, 0.0), bl(S.ldlim, 0.0);
+        const int ci = H * iv;
+        sv_place(host_weight(b + "4.fn.local_interactive_module.kernel"), 9 * ci, H, iv, Wl, S.ldlim, 0, S.dhi,
+                 [&](int k) { return (k / ci) * HI + (k % ci) / iv * S.dhi + k % iv; });
+        sv_place(host_weight(b + "4.fn.local_interactive_module.bias"), 1, H, iv, bl, S.ldlim, 0, S.dhi, same);
+        w.lim = linear_from_host(key + "lim", Wl, bl, 9 * HI, S.ldlim);
+        w.iwsa_out = sv_head_rows(key + "iwsa_out", b + "4.fn.to_out.0", H, iv, S.dhi, S.ldlim, d, dp);
+        S.blocks.push_back(std::move(w));
+      }
+      S.norm = padded_norm(p + "0.norm", d, dp);
+      S.down = st < sv.num_stages - 1;
+      if (S.down) S.down_conv = padded_dense("sv." + p + "1.conv", p + "1.conv", 9 * d, 2 * d, 9 * d, channel_width(2 * d));
+      sv_stages.push_back(std::move(S));
+    }
+    const int dl = sv_dim(sv.num_stages - 1);
+    head_norm = make_norm("mlp_head.1", dl);
+    head = make_linear_f32("mlp_head.2", dl, cfg.num_classes);
   }
 
   // vit_for_small_dataset.ViT (:159-195): SPT (set_spt_patch), then ViT's layers with LSA: the diagonal mask and exp(temperature)
@@ -2448,6 +2608,8 @@ struct vb_handle {
       ats_forward<T>(img, B, H, Wd, logits, s);
     } else if (c.kind == VB_KIND_MOBILEVIT) {
       mobilevit_forward<T>(img, B, H, Wd, logits, s);
+    } else if (c.kind == VB_KIND_SCALABLE_VIT) {
+      svit_forward<T>(img, B, H, Wd, logits, s);
     } else if (c.kind == VB_KIND_SMALL_DATASET_VIT) {     // vit_for_small_dataset.py:197-215, Transformer.call :135-140
       int rows = 0;
       float* stats = nullptr;
@@ -2513,10 +2675,10 @@ struct vb_handle {
   }
   // A convolution as unfold_same + GEMM: the fp32 image (map == null, cin channels) or the first cin channels of the token map
   // [B h w, ld], unfolded at the packed weight pitch (`um`: VALID, or the LayerNorm / GELU applied on load), then out [rows, L.N] =
-  // act(col W + b) (Act), with the output rows' statistics when stats_out is given
+  // act(col W + b) (Act) (+ res [rows, ldr] when given), with the output rows' statistics when stats_out is given
   template <typename T>
   void conv(const float* img, const T* map, int ld, int B, int h, int w, int cin, int k, int stride, const Linear& L, T* out,
-            float* stats_out, cudaStream_t s, const UnfoldMode* um = nullptr, int act = ACT_NONE) {
+            float* stats_out, cudaStream_t s, const UnfoldMode* um = nullptr, int act = ACT_NONE, const T* res = nullptr, int ldr = 0) {
     const bool valid = um != nullptr && um->valid;
     const int oh = valid ? (h - k) / stride + 1 : (h + stride - 1) / stride, ow = valid ? (w - k) / stride + 1 : (w + stride - 1) / stride;
     const int rows = B * oh * ow, Kp = bf16() ? L.ldw : L.K;
@@ -2528,7 +2690,7 @@ struct vb_handle {
     }
     Linear Lk = L;
     Lk.K = Kp;                      // unfold_same zero-pads the patch vectors to the packed weight pitch
-    Epi e; e.bias = L.bias; e.stats_out = stats_out; e.set_act(act);
+    Epi e; e.bias = L.bias; e.stats_out = stats_out; e.set_act(act); e.res = res; e.ldr = ldr;
     linear<T>(col, Kp, rows, Lk, out, L.N, e, s);
   }
   // The pre-norm sub-blocks x = f(LN(x)) + x over X [M, dp] (true width d).  bf16 folds the LayerNorm into f's first GEMM from
@@ -3085,6 +3247,114 @@ struct vb_handle {
     return out;
   }
 
+  // ScalableViT.call (scalable_vit.py:308-319): to_patches, per stage the Transformer (its blocks, then its LayerNorm) and the
+  // Downsample, then the mean over the map, LayerNormalization and Dense.  Token rows are the NHWC map, pixel-major, channel widths
+  // zero-padded to channel_width; no step permutes the map (the windowed attention reads and writes the map's own rows).  bf16:
+  // `stats` holds the (sum, sumsq) partials of X's rows between sub-blocks (emitted by to_patches', the Downsample's and the
+  // residual GEMMs' epilogues, and after the PEG by a row-statistics pass).
+  // The reference's shape rules, checked before anything runs: the SSA's VALID r x r convolution needs a map of at least r on each
+  // side, and IWSA asserts that its window divides the map (:171).  The SAME stride-4 stem and stride-2 Downsamples give ceil.
+  void svit_check_size(int H, int Wd) const {
+    int h = (H + 3) / 4, w = (Wd + 3) / 4;
+    for (int st = 0; st < sv.num_stages; ++st) {
+      if (st > 0) { h = (h + 1) / 2; w = (w + 1) / 2; }
+      if (sv.depth[st] == 0) continue;
+      const int r = sv.reduction_factor[st], wh = sv.window[st] > 0 ? sv.window[st] : h, ww = sv.window[st] > 0 ? sv.window[st] : w;
+      const std::string where = "ScalableViT stage " + std::to_string(st + 1) + ": ";
+      VB_CHECK(h >= r && w >= r, where + "the " + std::to_string(h) + " x " + std::to_string(w) + " map is smaller than reduction_factor " +
+                                     std::to_string(r) + " (a VALID convolution)");
+      VB_CHECK(h % wh == 0 && w % ww == 0, where + "height (" + std::to_string(h) + ") or width (" + std::to_string(w) +
+                                               ") of feature map is not divisible by the window size (" + std::to_string(wh) + ", " +
+                                               std::to_string(ww) + ")");
+    }
+  }
+  template <typename T>
+  void svit_forward(const float* img, int B, int H, int Wd, float* logits, cudaStream_t s) {
+    svit_check_size(H, Wd);
+    int h = (H + 3) / 4, w = (Wd + 3) / 4;
+    T* X = arena.get<T>(static_cast<size_t>(B) * h * w * sv_stages[0].dp);
+    float* stats = row_stats(static_cast<long long>(B) * h * w, sv_stages[0].dp);
+    conv<T>(img, nullptr, 0, B, H, Wd, cfg.channels, 7, 4, sv_stem, X, stats, s);       // to_patches (:310)
+    for (const SvitStageW& S : sv_stages) {
+      const int M = B * h * w;
+      for (const SvitBlockW& l : S.blocks) X = svit_block<T>(X, B, h, w, S, l, stats, s);
+      const PreNorm<T> p = prenorm<T>(X, M, S.dim, S.dp, stats, 1e-5f, s);
+      if (!S.down) {                                                   // the last stage's LayerNorm, the mean, mlp_head (:302-306)
+        const T* a = p.norm(S.norm);
+        if (p.Y == nullptr) {
+          T* Y = arena.get<T>(static_cast<size_t>(M) * S.dp);
+          ProfScope ps(this, PROF_LN, 8.0 * M * S.dim, 2.0 * sizeof(T) * M * S.dp, s);
+          layernorm<T>(X, S.dp, S.norm.gamma, S.norm.beta, Y, S.dp, M, S.dim, s, S.dp, 1e-5f);
+          a = Y;
+        }
+        float* z = arena.get<float>(static_cast<size_t>(B) * S.dim);
+        {
+          ProfScope ps(this, PROF_LN, 2.0 * M * S.dim, static_cast<double>(sizeof(T)) * M * S.dp, s);
+          pool_layernorm<T>(a, h * w, S.dp, head_norm.gamma, head_norm.beta, z, B, S.dim, 1, s);
+        }
+        dense_head(z, S.dim, head, B, logits, s);
+        return;
+      }
+      // Downsample (:71-78) of the Transformer's LayerNorm output: bf16 applies that LayerNorm on load from the row statistics
+      UnfoldMode um;
+      um.stats = stats; um.parts = S.dp / 64; um.d = S.dim; um.eps = 1e-5f; um.gamma = S.norm.gamma; um.beta = S.norm.beta;
+      const T* a = p.norm(S.norm);
+      const int oh = (h + 1) / 2, ow = (w + 1) / 2, dpn = S.down_conv.N;
+      T* Xn = arena.get<T>(static_cast<size_t>(B) * oh * ow * dpn);
+      stats = row_stats(static_cast<long long>(B) * oh * ow, dpn);
+      conv<T>(nullptr, a, S.dp, B, h, w, S.dim, 3, 2, S.down_conv, Xn, stats, s, p.Y == nullptr ? &um : nullptr);
+      X = Xn; h = oh; w = ow;
+    }
+  }
+  // One block (scalable_vit.py:237-245) on X [B*h*w, dp]; returns the block's output rows (a new buffer after the PEG).  bf16: the
+  // LayerNorms folded into the SSA q, the MLPs' fc1 and the IWSA q|k|v (from `stats`), and applied on load by the SSA's k|v unfold;
+  // fp32: separate LayerNorms.
+  template <typename T>
+  T* svit_block(T* X, int B, int h, int w, const SvitStageW& S, const SvitBlockW& l, float* stats, cudaStream_t s) {
+    const int dp = S.dp, d = S.dim, M = B * h * w, HS = S.heads * S.dhs, HI = S.heads * S.dhi;
+    const PreNorm<T> p0 = prenorm<T>(X, M, d, dp, stats, 1e-5f, s);
+    {                                                                 // ScalableSelfAttention (:121-143)
+      const T* a = p0.norm(l.ssa_norm);
+      T* Q = arena.get<T>(static_cast<size_t>(M) * S.ldq);
+      linear<T>(a, dp, M, l.ssa_q, Q, S.ldq, p0.folded_epi(l.ssa_q), s);
+      const int kh = h / S.r, kw = w / S.r;
+      UnfoldMode um;                                                  // to_k | to_v: the VALID r x r stride-r convolution
+      um.valid = true;
+      if (p0.Y == nullptr) { um.stats = stats; um.parts = dp / 64; um.d = d; um.eps = 1e-5f; um.gamma = l.ssa_norm.gamma; um.beta = l.ssa_norm.beta; }
+      T* KV = arena.get<T>(static_cast<size_t>(B) * kh * kw * S.ldkv);
+      conv<T>(nullptr, a, dp, B, h, w, d, S.r, S.r, l.ssa_kv, KV, nullptr, s, &um);
+      attention_dispatch<T>(Q, S.ldq, KV, S.ldkv, KV + HS, S.ldkv, Q, S.ldq, B, h * w, kh * kw, S.heads, S.dhs, 0, nullptr, nullptr, nullptr,
+                            nullptr, s, S.ssa_scale);               // the output overwrites q
+      p0.residual(Q, S.ldq, l.ssa_out);
+    }
+    p0.mlp(l.mlp1);
+    if (l.peg_w != nullptr) {                                         // PEG (:85-87), the residual folded into the centre tap
+      T* Y = arena.get<T>(static_cast<size_t>(M) * dp);               // the halo reads the unmodified map
+      {
+        ProfScope ps(this, PROF_OTHER, 18.0 * M * d, 2.0 * sizeof(T) * M * dp, s);
+        dwconv_qkv<T>(X, dp, nullptr, nullptr, nullptr, d, 1e-5f, l.peg_w, l.peg_b, Y, dp, nullptr, nullptr, nullptr, dp, B, h, w, dp, 3, 1, s);
+      }
+      X = Y;
+      if (bf16()) ensure_stats<T>(X, dp, stats, M, s);
+    }
+    const PreNorm<T> p = p0.rows(X, M, stats);
+    p.mlp(l.mlp3);
+    {                                                                 // InteractiveWindowedSelfAttention (:165-198)
+      const T* a = p.norm(l.iwsa_norm);
+      T* QKV = arena.get<T>(static_cast<size_t>(M) * S.ldqkv);
+      linear<T>(a, dp, M, l.iwsa_qkv, QKV, S.ldqkv, p.folded_epi(l.iwsa_qkv), s);
+      Window win;                                                     // window 0 (None): one window per image
+      win.p = S.window > 0 ? S.window : h; win.pw = S.window > 0 ? S.window : w;
+      win.ny = h / win.p; win.nx = w / win.pw; win.count = B * win.nx * win.ny;
+      block_attention<T>(QKV, S.ldqkv, QKV, S.ldqkv, S.heads, S.dhi, win, s, S.iwsa_scale);   // the output overwrites q
+      // LIM(v) + the attention output: the 3x3 convolution over v's columns of the same rows, the output as its residual
+      T* LO = arena.get<T>(static_cast<size_t>(M) * S.ldlim);
+      conv<T>(nullptr, QKV + 2 * HI, S.ldqkv, B, h, w, HI, 3, 1, l.lim, LO, nullptr, s, nullptr, ACT_NONE, QKV, S.ldqkv);
+      p.residual(LO, S.ldlim, l.iwsa_out);
+    }
+    return X;
+  }
+
   // RegionViT.call (regionvit.py:249-263): the local and region encoders, then per stage the shared Downsample of both maps, the
   // PEG of the local map and the R2L layers; then the mean over the regional tokens, LayerNorm and Dense.  Each stage keeps its
   // local rows (the pixel-major B x lh x lw map) followed by its regional rows (the B x rh x rw map) in one arena, so every
@@ -3309,6 +3579,7 @@ struct vb_handle {
       case VB_KIND_ATS_VIT: return "ATS-ViT runs as a whole forward only: its token count changes inside the transformer, so its stages have no entry of their own";
       case VB_KIND_SMALL_DATASET_VIT: return "the small-dataset ViT runs as a whole forward only: its SPT embedding / transformer / head steps have no entry of their own";
       case VB_KIND_MOBILEVIT: return "MobileViT runs as a whole forward only: its stem / trunk / head steps have no entry of their own";
+      case VB_KIND_SCALABLE_VIT: return "ScalableViT runs as a whole forward only: its patch-embedding / stage / head steps have no entry of their own";
       default: return nullptr;
     }
   }
@@ -3498,10 +3769,8 @@ void vb_handle::attention_dispatch(const T* q, int ldq, const T* k, int ldk, con
   ProfScope ps(this, PROF_ATTN, 4.0 * B * heads * nq * nk * dh + (variant == 1 ? 2.0 : variant == 2 ? 4.0 : 0.0) * B * nq * nk * heads * heads,
                static_cast<double>(sizeof(T)) * B * heads * dh * (2.0 * nq + 2.0 * nk), s);
   if (attention_fast<T>(q, ldq, k, ldk, v, ldv, out, ldo, B, nq, nk, heads, dh, variant, mix_a, mix_b, g, b, s, scale)) return;
-  // a head-padded layer passes its model's scale, which only the fused kernels take
-  VB_CHECK(scale <= 0.f, "an explicit softmax scale needs the fused attention kernels (bf16 at a head width they take)");
   float* S = arena.get<float>(static_cast<size_t>(B) * heads * nq * ((nk + 15) & ~15));   // row pitch padded for the bf16-P path
-  attention_generic<T>(q, ldq, k, ldk, v, ldv, out, ldo, S, B, nq, nk, heads, dh, variant, mix_a, mix_b, g, b, s);
+  attention_generic<T>(q, ldq, k, ldk, v, ldv, out, ldo, S, B, nq, nk, heads, dh, variant, mix_a, mix_b, g, b, s, scale);
 }
 
 template <>
@@ -3548,6 +3817,7 @@ void validate(const vb_config& c) {
   VB_CHECK(c.kind != VB_KIND_REGIONVIT, "RegionViT: create the handle with vb_create_regionvit (its stages are a vb_regionvit_config)");
   VB_CHECK(c.kind != VB_KIND_ATS_VIT, "ATS-ViT: create the handle with vb_create_ats_vit (its token counts are a vb_ats_vit_config)");
   VB_CHECK(c.kind != VB_KIND_MOBILEVIT, "MobileViT: create the handle with vb_create_mobilevit (its blocks are a vb_mobilevit_config)");
+  VB_CHECK(c.kind != VB_KIND_SCALABLE_VIT, "ScalableViT: create the handle with vb_create_scalable_vit (its stages are a vb_scalable_vit_config)");
   VB_CHECK((c.kind >= VB_KIND_VIT && c.kind <= VB_KIND_CCT) || c.kind == VB_KIND_SMALL_DATASET_VIT, "unknown model kind");
   if (c.kind == VB_KIND_SMALL_DATASET_VIT) {
     // SPT's Rearrange takes one patch size for both sides (vit_for_small_dataset.py:147) and shift() one image of 3 channels
@@ -3685,6 +3955,25 @@ void validate_mobilevit(const vb_config& c, const vb_mobilevit_config& m) {
     VB_CHECK(m.mv2_hidden[i] > 0 && m.mv2_hidden[i] <= 262144, b + "bad hidden width");
     VB_CHECK(m.mv2_expand[i] || m.mv2_hidden[i] == m.mv2_in[i], b + "without the expand convolution the depthwise step needs hidden == input width");
     VB_CHECK(!m.mv2_residual[i] || (stride[i] == 1 && in[i] == out[i]), b + "a residual needs stride 1 and equal widths");
+  }
+}
+
+void validate_scalable_vit(const vb_config& c, const vb_scalable_vit_config& v) {
+  VB_CHECK(c.precision == VB_PRECISION_FP32 || c.precision == VB_PRECISION_BF16, "unknown precision");
+  VB_CHECK(c.channels > 0 && c.channels <= 64 && c.num_classes > 0, "ScalableViT: bad channel / class configuration");
+  VB_CHECK(v.num_stages >= 1 && v.num_stages <= VB_SCALABLE_VIT_STAGES, "ScalableViT: num_stages must be in [1, 4]");
+  VB_CHECK(v.ff_expansion_factor >= 1 && v.ff_expansion_factor <= 64, "ScalableViT: bad ff_expansion_factor");
+  VB_CHECK(v.dim[0] > 0 && (static_cast<long long>(v.dim[0]) << (v.num_stages - 1)) <= 8192, "ScalableViT: bad dim");
+  for (int st = 0; st < v.num_stages; ++st) {
+    const std::string stage = "ScalableViT stage " + std::to_string(st + 1) + ": ";
+    VB_CHECK(v.dim[st] == v.dim[0] << st, stage + "dim must be dim[0] * 2^s");
+    VB_CHECK(v.depth[st] >= 0 && v.depth[st] <= 256, stage + "bad depth");
+    VB_CHECK(v.heads[st] >= 1 && v.heads[st] <= 64, stage + "bad heads");
+    VB_CHECK(v.ssa_dim_key[st] >= 1 && v.ssa_dim_value[st] >= 1 && v.iwsa_dim_key[st] >= 1 && v.iwsa_dim_value[st] >= 1 &&
+             v.ssa_dim_key[st] <= 512 && v.ssa_dim_value[st] <= 512 && v.iwsa_dim_key[st] <= 512 && v.iwsa_dim_value[st] <= 512,
+             stage + "bad key / value widths");
+    VB_CHECK(v.reduction_factor[st] >= 1 && v.reduction_factor[st] <= 64, stage + "bad reduction_factor");
+    VB_CHECK(v.window[st] >= 0, stage + "bad window");
   }
 }
 
@@ -4094,6 +4383,11 @@ int vb_create_mobilevit(const vb_config* base, const vb_mobilevit_config* mc, in
                      validate_mobilevit, [&](vb_handle& h) { h.mv = *mc; h.cfg.dim = mc->last_dim; });
 }
 
+int vb_create_scalable_vit(const vb_config* base, const vb_scalable_vit_config* sc, int device, vb_handle** out) {
+  return create_with("vb_create_scalable_vit", "vb_scalable_vit_config", VB_KIND_SCALABLE_VIT, "VB_KIND_SCALABLE_VIT", base, sc, device,
+                     out, validate_scalable_vit, [&](vb_handle& h) { h.sv = *sc; h.cfg.dim = sc->dim[sc->num_stages - 1]; });
+}
+
 int vb_create_regionvit(const vb_config* base, const vb_regionvit_config* rc, int device, vb_handle** out) {
   return create_with("vb_create_regionvit", "vb_regionvit_config", VB_KIND_REGIONVIT, "VB_KIND_REGIONVIT", base, rc,
                                           device, out, validate_regionvit,
@@ -4232,6 +4526,7 @@ int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, int32_t 
     VB_CHECK(h->cfg.kind != VB_KIND_ATS_VIT, h->whole_forward_only(VB_KIND_ATS_VIT));
     VB_CHECK(h->cfg.kind != VB_KIND_SMALL_DATASET_VIT, h->whole_forward_only(VB_KIND_SMALL_DATASET_VIT));
     VB_CHECK(h->cfg.kind != VB_KIND_MOBILEVIT, h->whole_forward_only(VB_KIND_MOBILEVIT));
+    VB_CHECK(h->cfg.kind != VB_KIND_SCALABLE_VIT, h->whole_forward_only(VB_KIND_SCALABLE_VIT));
     const bool levit = h->cfg.kind == VB_KIND_LEVIT;
     VB_CHECK(levit || distill_token != nullptr, "vb_forward_distill: null argument");
     VB_CHECK(!levit || (distill_token == nullptr && h->lv.num_distill_classes > 0),
@@ -4358,6 +4653,7 @@ int vb_to_patch(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, 
     VB_CHECK(h != nullptr && img != nullptr && patches != nullptr, "vb_to_patch: null argument");
     VB_CHECK(h->cfg.kind != VB_KIND_SMALL_DATASET_VIT, h->whole_forward_only(VB_KIND_SMALL_DATASET_VIT));
     VB_CHECK(h->cfg.kind != VB_KIND_MOBILEVIT, h->whole_forward_only(VB_KIND_MOBILEVIT));
+    VB_CHECK(h->cfg.kind != VB_KIND_SCALABLE_VIT, h->whole_forward_only(VB_KIND_SCALABLE_VIT));
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT && h->cfg.kind != VB_KIND_T2T_VIT && h->cfg.kind != VB_KIND_CCT &&
              h->cfg.kind != VB_KIND_LEVIT && h->cfg.kind != VB_KIND_CVT && h->cfg.kind != VB_KIND_TWINS_SVT &&
              h->cfg.kind != VB_KIND_CROSSFORMER && h->cfg.kind != VB_KIND_NEST && h->cfg.kind != VB_KIND_REGIONVIT,

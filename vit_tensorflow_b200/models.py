@@ -10,6 +10,7 @@
     CrossFormer  vit_tensorflow/crossformer.py:205-269
     NesT      vit_tensorflow/nest.py:150-216
     RegionViT vit_tensorflow/regionvit.py:184-263
+    ScalableViT  vit_tensorflow/scalable_vit.py:250-319
 
 Same constructor kwargs, defaults and assertion messages; `model(img, training=True, **kwargs) -> logits`
 with `img` NHWC float32 `[b, H, W, 3]` and logits float32 `[b, num_classes]`.  Everything below the call is
@@ -1804,8 +1805,126 @@ class MobileViT(_EngineModel):
 MOBILEVIT_CTOR_KEYS = ("image_size", "dims", "channels", "num_classes", "expansion", "kernel_size", "patch_size", "depths")
 
 
+SCALABLE_VIT_STAGE_KEYS = ("heads", "ssa_dim_key", "ssa_dim_value", "reduction_factor", "iwsa_dim_key", "iwsa_dim_value", "window_size")
+
+
+def scalable_vit_size_error(stages, h, w):
+    """The reference's shape rules for an h x w image: None, or (exception type, message) of the first stage that breaks one, in the
+    order the reference meets them.  to_patches (SAME, stride 4) and each Downsample (SAME, stride 2) round up; in every stage with
+    blocks the SSA's r x r stride-r VALID convolution needs a map of at least r on each side (TensorFlow refuses a negative output
+    size), and IWSA asserts that its window divides the map (scalable_vit.py:171; None is the whole map)."""
+    h, w = -(-h // 4), -(-w // 4)
+    for i, st in enumerate(stages, 1):
+        if i > 1:
+            h, w = -(-h // 2), -(-w // 2)
+        if st["depth"] == 0:
+            continue
+        r = st["reduction_factor"]
+        if h < r or w < r:
+            return ValueError, f"ScalableViT stage {i}: the {h} x {w} map is smaller than reduction_factor {r} (a VALID convolution)"
+        wh, ww = st["window_size"] or h, st["window_size"] or w
+        if h % wh or w % ww:
+            return AssertionError, (f"ScalableViT stage {i}: height ({h}) or width ({w}) of feature map is not divisible by the window size "
+                                    f"({wh}, {ww})")
+    return None
+
+
+class ScalableViT(_EngineModel):
+    """scalable_vit.py:250-319: to_patches (Conv2D(dim, 7, stride 4, SAME)), then per stage s a Transformer on dim * 2^s channels and,
+    between stages, Downsample (Conv2D(2 dim_s, 3, stride 2, SAME)); then the mean over the map, LayerNormalization and Dense.  Each
+    block is built [SSA, MLP, PEG (first block only), MLP, IWSA] but unpacked as ssa, ff1, peg, iwsa, ff2 (:236), so it runs SSA,
+    MLP, PEG, MLP, IWSA, each but the PEG pre-norm and residual; every Transformer ends with its own LayerNorm.  SSA: q from every
+    pixel against keys and values of an r x r stride-r VALID convolution, scale ssa_dim_key^-0.5.  IWSA: attention within
+    window_size windows (None: the whole map), plus a full 3x3 convolution (the LIM) of v, then to_out.
+
+    There is no image_size: any image whose stage maps (ceil(H / 4), halved and rounded up per stage) are at least reduction_factor
+    on each side and divisible by their window_size runs; a map smaller than reduction_factor raises ValueError naming the stage,
+    a window that does not divide its map the reference's AssertionError.  There is no BatchNormalization: with dropout = 0
+    training=True computes what training=False does.  At most 4 stages.
+    Weights (SURVEY.md App. B) keep the reference's attribute paths: to_patches, scalable_layers.{s}.0.layers.{l}.{j} with j the
+    construction index (0 SSA: .norm, .fn.to_q / to_k / to_v / to_out.0; 1 and 3 MLP: .norm, .fn.net.0 / net.3; 2 PEG: .proj;
+    4 IWSA: .norm, .fn.local_interactive_module / to_q / to_k / to_v / to_out.0), scalable_layers.{s}.0.norm,
+    scalable_layers.{s}.1.conv (Downsample), mlp_head.1 (LayerNormalization), mlp_head.2 (Dense)."""
+    _kind = "scalable_vit"
+
+    def __init__(self, num_classes, dim, depth, heads, reduction_factor, window_size=None, iwsa_dim_key=32, iwsa_dim_value=32,
+                 ssa_dim_key=32, ssa_dim_value=32, ff_expansion_factor=4, channels=3, dropout=0.0, *, precision="bf16", device=0,
+                 seed=None):
+        assert isinstance(depth, tuple), 'depth needs to be tuple if integers indicating number of transformer blocks at that stage'
+        num_stages = len(depth)
+        per_stage = [_cast_tuple(v, num_stages) for v in (heads, ssa_dim_key, ssa_dim_value, reduction_factor, iwsa_dim_key,
+                                                          iwsa_dim_value, window_size)]
+        assert all(len(a) == num_stages for a in per_stage)
+        if not 1 <= num_stages <= _lib.SCALABLE_VIT_STAGES:
+            raise NotImplementedError(f"ScalableViT: the engine runs 1 to {_lib.SCALABLE_VIT_STAGES} stages; depth has {num_stages} entries")
+        self.num_classes, self.channels = num_classes, channels
+        self.stages = tuple(dict(depth=depth[i], **{k: per_stage[j][i] for j, k in enumerate(SCALABLE_VIT_STAGE_KEYS)})
+                            for i in range(num_stages))
+        self._dropout_rates = (dropout,)
+        sc = _lib.VbScalableVitConfig()
+        sc.struct_size = C.sizeof(_lib.VbScalableVitConfig)
+        sc.num_stages = num_stages
+        sc.ff_expansion_factor = int(ff_expansion_factor)
+        for i, st in enumerate(self.stages):
+            sc.dim[i], sc.depth[i] = int(dim) << i, int(st["depth"])
+            for k in SCALABLE_VIT_STAGE_KEYS[:-1]:
+                getattr(sc, k)[i] = int(st[k])
+            sc.window[i] = 0 if st["window_size"] is None else int(st["window_size"])
+            if st["window_size"] is not None and sc.window[i] <= 0:
+                raise ValueError(f"ScalableViT stage {i + 1}: window_size must be positive or None")
+        self._sc = sc
+        lib = _lib.load()
+        self._create(precision, device, create=lambda cfg, dev, h: lib.vb_create_scalable_vit(cfg, C.byref(sc), dev, h),
+                     channels=channels, num_classes=num_classes, dim=int(dim) << (num_stages - 1))
+        self.init_weights(seed)
+
+    def init_weights(self, seed=None):
+        """The reference's initialisers: glorot-uniform over the receptive field (the PEG's depthwise kernel [3, 3, 1, dim] has fan_in
+        9 and fan_out 9 * dim), zero biases, LayerNorm g / LayerNormalization gamma 1, b / beta 0."""
+        rng = np.random.default_rng(seed)
+        w = collections.OrderedDict()
+        for name, shape in self._specs.items():
+            leaf = name.rsplit(".", 1)[-1]
+            if leaf == "kernel":
+                receptive = int(np.prod(shape[:-2]))
+                lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
+                a = rng.uniform(-lim, lim, size=shape)
+            elif leaf in ("bias", "b", "beta"):
+                a = np.zeros(shape)
+            elif leaf in ("g", "gamma"):
+                a = np.ones(shape)
+            else:
+                raise AssertionError(name)
+            w[name] = a.astype(np.float32)
+        self.set_weights_dict(w)
+
+    def __call__(self, img, training=True, **kwargs):
+        """scalable_vit.py:308-319: NHWC float images [b, H, W, channels] -> logits [b, num_classes]; extra kwargs are accepted and
+        ignored, as there."""
+        self._check_training(training)
+        x = np.ascontiguousarray(img, dtype=np.float32)
+        if x.ndim != 4 or x.shape[3] != self.channels:
+            raise ValueError(f"ScalableViT: img must be NHWC float [b, H, W, {self.channels}] (channels={self.channels}), got shape "
+                             f"{tuple(x.shape)}")
+        err = scalable_vit_size_error(self.stages, x.shape[1], x.shape[2])
+        if err is not None:
+            raise err[0](err[1])
+        b, h, w, _ = x.shape
+        out = np.empty((b, self.num_classes), np.float32)
+        self.forward_raw(x.ctypes.data, _lib.MEM_HOST, b, h, w, out.ctypes.data, _lib.MEM_HOST, None)
+        return _as_tensor(out)
+
+    call = __call__
+
+
+SCALABLE_VIT_CTOR_KEYS = ("num_classes", "dim", "depth", "heads", "reduction_factor", "window_size", "iwsa_dim_key", "iwsa_dim_value",
+                          "ssa_dim_key", "ssa_dim_value", "ff_expansion_factor", "channels", "dropout")
+
+
 def from_config(cfg: dict, precision="bf16", device=0, seed=None):
     """Build a model from an oracle-style config dict (kind + reference kwargs)."""
+    if cfg["kind"] == "scalable_vit":
+        return ScalableViT(**{k: v for k, v in cfg.items() if k in SCALABLE_VIT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "mobilevit":
         return MobileViT(**{k: v for k, v in cfg.items() if k in MOBILEVIT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "small_dataset_vit":
