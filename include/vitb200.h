@@ -17,6 +17,7 @@
  *     NesT(...)(img)                 vit_tensorflow/nest.py:150-216 (vb_create_nest)
  *     RegionViT(...)(img)            vit_tensorflow/regionvit.py:184-263 (vb_create_regionvit)
  *     ScalableViT(...)(img)          vit_tensorflow/scalable_vit.py:250-319 (vb_create_scalable_vit)
+ *     PiT(...)(img)                  vit_tensorflow/pit.py:158-219 (vb_create_pit)
  * and this header is what the Python host classes (vit_tensorflow_b200/models.py, _lib.py) bind with ctypes.
  * Plain pointers and sizes only; no torch / C++ types cross the boundary.
  *
@@ -49,7 +50,7 @@ enum { VB_KIND_VIT = 0, VB_KIND_DEEPVIT = 1, VB_KIND_CAIT = 2, VB_KIND_CROSSVIT 
        VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6, VB_KIND_CCT = 7, VB_KIND_LEVIT = 8,
        VB_KIND_CVT = 9, VB_KIND_TWINS_SVT = 10, VB_KIND_CROSSFORMER = 11, VB_KIND_NEST = 12, VB_KIND_REGIONVIT = 13,
        VB_KIND_ATS_VIT = 14, VB_KIND_SMALL_DATASET_VIT = 15, VB_KIND_MOBILEVIT = 16,
-       VB_KIND_SCALABLE_VIT = 17 };
+       VB_KIND_SCALABLE_VIT = 17, VB_KIND_PIT = 18 };
 enum { VB_CCT_POS_SINE = 0, VB_CCT_POS_LEARNABLE = 1, VB_CCT_POS_NONE = 2 };   /* cct.py:233-234,250-256 */
 enum { VB_PRECISION_FP32 = 0, VB_PRECISION_BF16 = 1 };
 enum { VB_POOL_CLS = 0, VB_POOL_MEAN = 1 };
@@ -711,6 +712,36 @@ typedef struct vb_scalable_vit_config {
  *   mlp_head.1.gamma / .beta [dim[-1]], mlp_head.2.kernel [dim[-1], num_classes] / .bias
  * vb_forward only: the stage entries and vb_forward_distill refuse the handle. */
 VB_API int vb_create_scalable_vit(const vb_config* base, const vb_scalable_vit_config* sv, int device, vb_handle** out);
+
+/* PiT (pit.py:158-219) as the reference runs it, appended within ABI 7.  No pooling stage is ever built (`ind < (len(depth) < 1)`
+ * is `ind < 0`, pit.py:194), so the model is one token stream of width dim: patch embedding = tf.image.extract_patches(p, stride
+ * p / 2, VALID) ((k_row, k_col, c) vectors, c fastest) then Dense(dim); cls row and pos_embedding[:, :n + 1]; the stages in order,
+ * stage s a ViT Transformer of depth[s] layers with heads[s] heads of dim_head (pre-norm attention with a bias-free to_qkv, to_out
+ * unless heads[s] == 1 and dim_head == dim; pre-norm MLP with exact-erf GELU; Keras LayerNormalization, eps 1e-3); head: the cls
+ * row, LayerNormalization, Dense(num_classes).  `stages` counts what the reference's zip(depth, cast_tuple(heads)) leaves. */
+#define VB_PIT_MAX_STAGES 8
+typedef struct vb_pit_config {
+  int32_t struct_size;            /* sizeof(vb_pit_config) */
+  int32_t stages;                 /* 0 .. VB_PIT_MAX_STAGES (0: embedding and head only) */
+  int32_t depth[VB_PIT_MAX_STAGES], heads[VB_PIT_MAX_STAGES];   /* the first `stages` entries */
+} vb_pit_config;
+
+/* PiT.__init__: `base` supplies precision, image_h == image_w (image_size), patch_h == patch_w (patch_size, at least 2: the
+ * stride is patch_size / 2), channels, num_classes, dim, dim_head, mlp_dim and max_batch; its kind must be VB_KIND_PIT and its
+ * other fields are ignored.  The table has num_patches + 1 rows, num_patches = ((image_size - p) / (p / 2) + 1)^2.  Weights are
+ * ViT's names and shapes (SURVEY.md App. B), with layer L counted across the stages in order:
+ *   patch.kernel [p^2 * channels, dim] / .bias          patch_embedding.layers[1]
+ *   pos_embedding [1, num_patches + 1, dim], cls_token [1, 1, dim]
+ *   layers.L.attn_norm.gamma / .beta, layers.L.to_qkv.kernel [dim, 3 heads[s] dim_head]     transformer_layers.{s}.layers.{l}.0
+ *     (.norm, .fn.to_qkv)
+ *   layers.L.to_out.kernel [heads[s] dim_head, dim] / .bias   ....{l}.0.fn.to_out.layers[0]; absent where heads[s] == 1 and
+ *     dim_head == dim
+ *   layers.L.ff_norm.gamma / .beta, layers.L.fc1 / .fc2 .kernel / .bias   ....{l}.1 (.norm, .fn.net.layers[0], .fn.net.layers[3])
+ *   head_norm.gamma / .beta, head.kernel / .bias        mlp_head.layers[0], mlp_head.layers[1]
+ * for stage s and its layer l (L = depth[0] + ... + depth[s - 1] + l).  vb_forward takes any image of at least p x p whose
+ * (floor((h - p) / (p / 2)) + 1) (floor((w - p) / (p / 2)) + 1) patches fit the table (the reference reads its first n + 1
+ * rows); the stage entries and vb_forward_distill refuse the handle. */
+VB_API int vb_create_pit(const vb_config* base, const vb_pit_config* pit, int device, vb_handle** out);
 
 /* Row softmax of fp32 scores into bf16 probabilities (the T2T attention): p[r, j] = softmax_j(s[r, j] * scale) for j < n,
  * p[r, n..npad) = 0.  s [rows, lds], p [rows, ldp] (uploaded and downloaded whole); n <= npad <= ldp. */

@@ -13,7 +13,7 @@ LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "libvitb200.so")
 
 KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6, "cct": 7, "levit": 8,
         "cvt": 9, "twins_svt": 10, "crossformer": 11, "nest": 12, "regionvit": 13, "ats_vit": 14,
-        "small_dataset_vit": 15, "mobilevit": 16, "scalable_vit": 17}
+        "small_dataset_vit": 15, "mobilevit": 16, "scalable_vit": 17, "pit": 18}
 PRECISION = {"fp32": 0, "float32": 0, "bf16": 1, "bfloat16": 1}
 MEM_HOST, MEM_DEVICE = 0, 1
 ABI_VERSION = 7                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
@@ -110,6 +110,14 @@ class VbScalableVitConfig(C.Structure):
                 [("ff_expansion_factor", C.c_int32)])
 
 
+PIT_MAX_STAGES = 8                                   # VB_PIT_MAX_STAGES
+
+
+class VbPitConfig(C.Structure):
+    _fields_ = [("struct_size", C.c_int32), ("stages", C.c_int32), ("depth", C.c_int32 * PIT_MAX_STAGES),
+                ("heads", C.c_int32 * PIT_MAX_STAGES)]
+
+
 class VbError(RuntimeError):
     pass
 
@@ -130,6 +138,7 @@ SIGNATURES = {
     "vb_create_ats_vit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbAtsVitConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_mobilevit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbMobilevitConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_create_scalable_vit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbScalableVitConfig), C.c_int, C.POINTER(C.c_void_p)]),
+    "vb_create_pit": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbPitConfig), C.c_int, C.POINTER(C.c_void_p)]),
     "vb_op_mv2_dwconv": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p] * 3 + [C.c_int32, _f32p]),
     "vb_op_patch_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 8 + [C.c_float, C.c_void_p, C.c_int32, C.c_int32, _f32p]),
     "vb_ats_set_seed": (C.c_int, [C.c_void_p, C.c_uint64]),

@@ -645,6 +645,16 @@ struct vb_handle {
     const int m = std::max(dk, dv);
     return !bf16() ? m : m <= 32 ? 32 : m <= 64 ? 64 : round_up(m, 8);
   }
+  // PiT (pit.py:158-219): ViT's weights and layers; layer L belongs to stage pit_stage(L) and has that stage's heads
+  vb_pit_config pit{};
+  int pit_stage(int L) const {
+    int s = 0;
+    for (int end = pit.depth[0]; L >= end && s + 1 < pit.stages; end += pit.depth[++s]) {}
+    return s;
+  }
+  int layer_heads(int L) const { return cfg.kind == VB_KIND_PIT ? pit.heads[pit_stage(L)] : cfg.heads; }
+  // extract_patches(p, stride p / 2, VALID) positions along a side of n pixels (pit.py:16-17,184 for n >= p)
+  int pit_side(int n) const { return (n - cfg.patch_h) / (cfg.patch_h / 2) + 1; }
   Norm head_norm, sm_head_norm, lg_head_norm;
   Linear head, sm_head, lg_head;
   Norm spt_norm;                     // SPT's LayerNorm over the p^2 * 5 C patch vector (bf16: padded to the GEMM's K, folded into it)
@@ -717,8 +727,9 @@ struct vb_handle {
   void build_expected() {
     const vb_config& c = cfg;
     const int C = c.channels;
-    if (c.kind == VB_KIND_VIT || c.kind == VB_KIND_DEEPVIT || c.kind == VB_KIND_PARALLEL_VIT || c.kind == VB_KIND_ATS_VIT) {
-      const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
+    if (c.kind == VB_KIND_VIT || c.kind == VB_KIND_DEEPVIT || c.kind == VB_KIND_PARALLEL_VIT || c.kind == VB_KIND_ATS_VIT ||
+        c.kind == VB_KIND_PIT) {
+      const int np = c.kind == VB_KIND_PIT ? pit_side(c.image_h) * pit_side(c.image_w) : (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       expect("pos_embedding", {1, np + 1, c.dim});
       expect("cls_token", {1, 1, c.dim});
       expect_dense("patch", c.patch_h * c.patch_w * C, c.dim);
@@ -726,8 +737,9 @@ struct vb_handle {
         if (c.kind == VB_KIND_PARALLEL_VIT) {   // branch i = (attention fn i, feed-forward fn i) of layer L (parallel_vit.py:109-112)
           for (int i = 0; i < c.parallel_branches; ++i)
             expect_layer("layers." + std::to_string(L) + ".branch" + std::to_string(i) + ".", c.dim, c.heads, c.dim_head, c.mlp_dim, VB_KIND_VIT);
-        } else {
-          expect_layer("layers." + std::to_string(L) + ".", c.dim, c.heads, c.dim_head, c.mlp_dim, c.kind);
+        } else {                                // PiT: ViT's layer with its stage's heads, the to_out rule per stage (pit.py:59)
+          expect_layer("layers." + std::to_string(L) + ".", c.dim, layer_heads(L), c.dim_head, c.mlp_dim,
+                       c.kind == VB_KIND_PIT ? VB_KIND_VIT : c.kind);
         }
       }
       expect_ln("head_norm", c.dim);
@@ -1290,15 +1302,17 @@ struct vb_handle {
     woverride.clear();
     drop_graphs();
     const vb_config& c = cfg;
-    if (c.kind == VB_KIND_VIT || c.kind == VB_KIND_DEEPVIT || c.kind == VB_KIND_PARALLEL_VIT || c.kind == VB_KIND_ATS_VIT) {
-      const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
+    if (c.kind == VB_KIND_VIT || c.kind == VB_KIND_DEEPVIT || c.kind == VB_KIND_PARALLEL_VIT || c.kind == VB_KIND_ATS_VIT ||
+        c.kind == VB_KIND_PIT) {
+      const int np = c.kind == VB_KIND_PIT ? pit_side(c.image_h) * pit_side(c.image_w) : (c.image_h / c.patch_h) * (c.image_w / c.patch_w);
       embed = make_embed("", c.patch_h, c.patch_w, c.dim, np + 1);
       for (int L = 0; L < c.depth; ++L) {
         if (c.kind == VB_KIND_PARALLEL_VIT) {   // `layers` holds depth x parallel_branches entries, branches of a layer adjacent
           for (int i = 0; i < c.parallel_branches; ++i)
             layers.push_back(make_layer("layers." + std::to_string(L) + ".branch" + std::to_string(i) + ".", c.dim, c.heads, c.dim_head, c.mlp_dim, VB_KIND_VIT));
         } else {
-          layers.push_back(make_layer("layers." + std::to_string(L) + ".", c.dim, c.heads, c.dim_head, c.mlp_dim, c.kind));
+          layers.push_back(make_layer("layers." + std::to_string(L) + ".", c.dim, layer_heads(L), c.dim_head, c.mlp_dim,
+                                      c.kind == VB_KIND_PIT ? VB_KIND_VIT : c.kind));
         }
       }
       head_norm = make_norm("head_norm", c.dim);
@@ -2145,6 +2159,28 @@ struct vb_handle {
     return nullptr;
   }
 
+  // PiT.patch_embedding + cls + positions (pit.py:179-182,208-213): extract_patches(p, stride p / 2, VALID) is unfold_same's VALID
+  // mode with its (k_row, k_col, c) vectors, written with the zero cls row at the packed weight pitch; the Dense folds cls and
+  // positions into its residual operand.
+  template <typename T>
+  T* embed_pit(const float* img, int B, int H, int Wd, int* rows_out, cudaStream_t s, float** stats_out) {
+    const int p = cfg.patch_h, stride = p / 2;
+    VB_CHECK(H >= p && Wd >= p, "PiT: a " + std::to_string(H) + " x " + std::to_string(Wd) + " image is smaller than one " +
+                                    std::to_string(p) + " x " + std::to_string(p) + " patch");
+    const int rows = pit_side(H) * pit_side(Wd) + 1, Kp = bf16() ? embed.patch.ldw : embed.patch.K;
+    VB_CHECK(rows <= embed.n_pos, "PiT: the image gives " + std::to_string(rows - 1) + " patches but pos_embedding has rows for " +
+                                      std::to_string(embed.n_pos - 1));
+    T* col = arena.get<T>(static_cast<size_t>(B) * rows * Kp);
+    UnfoldMode um;
+    um.valid = true;
+    {
+      ProfScope ps(this, PROF_EMBED, 0.0, 4.0 * B * H * Wd * cfg.channels + static_cast<double>(sizeof(T)) * B * rows * Kp, s);
+      unfold_same<float, T>(img, col, B, H, Wd, cfg.channels, p, stride, 1, Kp, s, 0, &um);
+    }
+    *rows_out = rows;
+    return embed_from_cols<T>(embed, col, Kp, B, rows, s, stats_out);
+  }
+
   // CCT Tokenizer + positional embedding (cct.py:211-215,278-286): per conv layer, unfold_same of the previous map (the fp32
   // image first) into the Dense operand (zero-padded to the packed weight pitch), the GEMM, then ReLU + SAME max-pool.  The last
   // pool adds the positions ('sine' / 'learnable') or writes zero rows up to sequence_length ('none').  -> X [B*rows, dim]
@@ -2188,6 +2224,7 @@ struct vb_handle {
   T* embed_any(const float* img, int B, int H, int Wd, int* rows_out, cudaStream_t s, float** stats_out) {
     VB_CHECK(cfg.kind != VB_KIND_CROSSVIT, "CrossViT has two token streams: no single embedding stage");
     if (cfg.kind == VB_KIND_T2T_VIT) return embed_t2t<T>(img, B, H, Wd, rows_out, s, stats_out);
+    if (cfg.kind == VB_KIND_PIT) return embed_pit<T>(img, B, H, Wd, rows_out, s, stats_out);
     return embed_tokens<T>(embed, img, B, H, Wd, cfg.patch_h, cfg.patch_w, rows_out, s, stats_out);
   }
 
@@ -2244,6 +2281,9 @@ struct vb_handle {
     T* Y = arena.get<T>(static_cast<size_t>(M) * dim);
     attend_self<T>(X, B, rows, dim, l, s, fold ? stats : nullptr, Y);
     feed_forward<T>(X, M, dim, l, Y, s, fold ? stats : nullptr);
+    // an unfolded layer rewrote X without updating the statistics: a folded layer after it (PiT, whose stages' head counts can
+    // fold one stage and not the next) recomputes them
+    if (!fold && stats_valid != nullptr) *stats_valid = false;
   }
   // The attention half of layer_self: X += to_out(attention(LN(X))) (the residual carried by to_out's epilogue), with the row
   // statistics `stats` (non-null iff the layer is folded; valid on entry) kept up to date.  Y [M, dim]: LayerNorm scratch of the
@@ -2550,7 +2590,7 @@ struct vb_handle {
   template <typename T>
   void forward_body(const float* img, int B, int H, int Wd, float* logits, cudaStream_t s) {
     const vb_config& c = cfg;
-    if (c.kind == VB_KIND_VIT || c.kind == VB_KIND_DEEPVIT || c.kind == VB_KIND_T2T_VIT) {
+    if (c.kind == VB_KIND_VIT || c.kind == VB_KIND_DEEPVIT || c.kind == VB_KIND_T2T_VIT || c.kind == VB_KIND_PIT) {
       int rows = 0;
       float* stats = nullptr;
       T* X = embed_any<T>(img, B, H, Wd, &rows, s, &stats);
@@ -3580,6 +3620,7 @@ struct vb_handle {
       case VB_KIND_SMALL_DATASET_VIT: return "the small-dataset ViT runs as a whole forward only: its SPT embedding / transformer / head steps have no entry of their own";
       case VB_KIND_MOBILEVIT: return "MobileViT runs as a whole forward only: its stem / trunk / head steps have no entry of their own";
       case VB_KIND_SCALABLE_VIT: return "ScalableViT runs as a whole forward only: its patch-embedding / stage / head steps have no entry of their own";
+      case VB_KIND_PIT: return "PiT runs as a whole forward only: it has no `transformer` attribute, so its patch-embedding / stage / head steps have no entry of their own";
       default: return nullptr;
     }
   }
@@ -3818,6 +3859,7 @@ void validate(const vb_config& c) {
   VB_CHECK(c.kind != VB_KIND_ATS_VIT, "ATS-ViT: create the handle with vb_create_ats_vit (its token counts are a vb_ats_vit_config)");
   VB_CHECK(c.kind != VB_KIND_MOBILEVIT, "MobileViT: create the handle with vb_create_mobilevit (its blocks are a vb_mobilevit_config)");
   VB_CHECK(c.kind != VB_KIND_SCALABLE_VIT, "ScalableViT: create the handle with vb_create_scalable_vit (its stages are a vb_scalable_vit_config)");
+  VB_CHECK(c.kind != VB_KIND_PIT, "PiT: create the handle with vb_create_pit (its stages' depths and heads are a vb_pit_config)");
   VB_CHECK((c.kind >= VB_KIND_VIT && c.kind <= VB_KIND_CCT) || c.kind == VB_KIND_SMALL_DATASET_VIT, "unknown model kind");
   if (c.kind == VB_KIND_SMALL_DATASET_VIT) {
     // SPT's Rearrange takes one patch size for both sides (vit_for_small_dataset.py:147) and shift() one image of 3 channels
@@ -3926,6 +3968,23 @@ void validate_ats(const vb_config& c, const vb_ats_vit_config& a) {
   for (int L = 0; L < c.depth; ++L)
     VB_CHECK(a.max_tokens_per_depth[L] > 0, "max_tokens_per_depth must have at least 1 token at any layer");
   VB_CHECK(c.dim_head <= ATS_MAX_DH, "ATS-ViT: dim_head must be at most 256");
+}
+
+// pit.py:173 and ViT's checks on the model the stages make: one stream of width dim, the depths summed, every stage's heads in [1, 32]
+void validate_pit(const vb_config& c, const vb_pit_config& p) {
+  VB_CHECK(p.stages >= 0 && p.stages <= VB_PIT_MAX_STAGES, "PiT: stages must be in [0, " + std::to_string(VB_PIT_MAX_STAGES) + "]");
+  VB_CHECK(c.image_h == c.image_w && c.patch_h == c.patch_w, "PiT takes one integer image_size and one integer patch_size");
+  VB_CHECK(c.patch_h >= 2, "PiT: patch_size must be at least 2 (the patch stride is patch_size // 2)");
+  vb_config v = c;
+  v.kind = VB_KIND_VIT;
+  v.pool = VB_POOL_CLS;
+  v.heads = 1;
+  v.depth = 0;
+  for (int s = 0; s < p.stages; ++s) {
+    VB_CHECK(p.depth[s] >= 0 && p.heads[s] >= 1 && p.heads[s] <= 32, "PiT: every stage needs depth >= 0 and 1 to 32 heads");
+    v.depth += p.depth[s];
+  }
+  validate(v);
 }
 
 void validate_regionvit(const vb_config& c, const vb_regionvit_config& r) {
@@ -4388,6 +4447,16 @@ int vb_create_scalable_vit(const vb_config* base, const vb_scalable_vit_config* 
                      out, validate_scalable_vit, [&](vb_handle& h) { h.sv = *sc; h.cfg.dim = sc->dim[sc->num_stages - 1]; });
 }
 
+int vb_create_pit(const vb_config* base, const vb_pit_config* pc, int device, vb_handle** out) {
+  return create_with("vb_create_pit", "vb_pit_config", VB_KIND_PIT, "VB_KIND_PIT", base, pc, device, out, validate_pit, [&](vb_handle& h) {
+    h.pit = *pc;
+    h.cfg.depth = 0;
+    for (int s = 0; s < pc->stages; ++s) h.cfg.depth += pc->depth[s];
+    h.cfg.heads = pc->stages > 0 ? pc->heads[0] : 1;
+    h.cfg.pool = VB_POOL_CLS;
+  });
+}
+
 int vb_create_regionvit(const vb_config* base, const vb_regionvit_config* rc, int device, vb_handle** out) {
   return create_with("vb_create_regionvit", "vb_regionvit_config", VB_KIND_REGIONVIT, "VB_KIND_REGIONVIT", base, rc,
                                           device, out, validate_regionvit,
@@ -4527,6 +4596,7 @@ int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, int32_t 
     VB_CHECK(h->cfg.kind != VB_KIND_SMALL_DATASET_VIT, h->whole_forward_only(VB_KIND_SMALL_DATASET_VIT));
     VB_CHECK(h->cfg.kind != VB_KIND_MOBILEVIT, h->whole_forward_only(VB_KIND_MOBILEVIT));
     VB_CHECK(h->cfg.kind != VB_KIND_SCALABLE_VIT, h->whole_forward_only(VB_KIND_SCALABLE_VIT));
+    VB_CHECK(h->cfg.kind != VB_KIND_PIT, h->whole_forward_only(VB_KIND_PIT));
     const bool levit = h->cfg.kind == VB_KIND_LEVIT;
     VB_CHECK(levit || distill_token != nullptr, "vb_forward_distill: null argument");
     VB_CHECK(!levit || (distill_token == nullptr && h->lv.num_distill_classes > 0),
@@ -4654,6 +4724,7 @@ int vb_to_patch(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, 
     VB_CHECK(h->cfg.kind != VB_KIND_SMALL_DATASET_VIT, h->whole_forward_only(VB_KIND_SMALL_DATASET_VIT));
     VB_CHECK(h->cfg.kind != VB_KIND_MOBILEVIT, h->whole_forward_only(VB_KIND_MOBILEVIT));
     VB_CHECK(h->cfg.kind != VB_KIND_SCALABLE_VIT, h->whole_forward_only(VB_KIND_SCALABLE_VIT));
+    VB_CHECK(h->cfg.kind != VB_KIND_PIT, h->whole_forward_only(VB_KIND_PIT));
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT && h->cfg.kind != VB_KIND_T2T_VIT && h->cfg.kind != VB_KIND_CCT &&
              h->cfg.kind != VB_KIND_LEVIT && h->cfg.kind != VB_KIND_CVT && h->cfg.kind != VB_KIND_TWINS_SVT &&
              h->cfg.kind != VB_KIND_CROSSFORMER && h->cfg.kind != VB_KIND_NEST && h->cfg.kind != VB_KIND_REGIONVIT,

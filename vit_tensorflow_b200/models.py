@@ -11,6 +11,7 @@
     NesT      vit_tensorflow/nest.py:150-216
     RegionViT vit_tensorflow/regionvit.py:184-263
     ScalableViT  vit_tensorflow/scalable_vit.py:250-319
+    PiT       vit_tensorflow/pit.py:158-219
 
 Same constructor kwargs, defaults and assertion messages; `model(img, training=True, **kwargs) -> logits`
 with `img` NHWC float32 `[b, H, W, 3]` and logits float32 `[b, num_classes]`.  Everything below the call is
@@ -1921,8 +1922,92 @@ SCALABLE_VIT_CTOR_KEYS = ("num_classes", "dim", "depth", "heads", "reduction_fac
                           "ssa_dim_key", "ssa_dim_value", "ff_expansion_factor", "channels", "dropout")
 
 
+def pit_stages(depth, heads):
+    """pit.py:177,193: heads = cast_tuple(heads, len(depth)), then zip(depth, heads) -- a heads tuple shorter than depth drops the
+    trailing stages, a longer one is cut.  The (depth, heads) pairs that run."""
+    if isinstance(heads, tuple):
+        if not all(isinstance(h, (int, np.integer)) and not isinstance(h, bool) for h in heads):
+            raise TypeError(f"PiT: heads must be an int or a tuple of ints, got {heads!r}")
+    elif isinstance(heads, (int, np.integer)) and not isinstance(heads, bool):
+        heads = (heads,) * len(depth)
+    else:
+        raise TypeError(f"PiT: heads must be an int or a tuple of ints, got {heads!r}")
+    return tuple((int(d), int(h)) for d, h in zip(depth, heads))
+
+
+def pit_num_patches(side, patch_size):
+    """Patches along one side: conv_output_size(side, p, p // 2) (pit.py:16-17), which for side >= p is extract_patches' VALID
+    count floor((side - p) / (p // 2)) + 1."""
+    return int(((side - patch_size) / (patch_size // 2)) + 1)
+
+
+class PiT(_EngineModel):
+    """pit.py:158-219 as the reference runs it.  `not_last = ind < (len(depth) < 1)` (:194) is `ind < 0`, never true, so no Pool is
+    ever built and dim never doubles: the model is tf.image.extract_patches(patch_size, stride patch_size // 2, VALID) + Dense(dim),
+    the cls row and positions, then one ViT Transformer(dim, depth[s], heads[s], dim_head, mlp_dim) per (depth, heads) pair of
+    zip(depth, cast_tuple(heads)), then LayerNormalization + Dense on the cls row.  to_out is absent in a stage whose heads == 1
+    and dim_head == dim (:59).
+    Weights are ViT's names (SURVEY.md App. B) with layers.L counted across the stages in order.  There is no `transformer`
+    attribute (the reference has none), so this runs as a whole forward only.
+    A call-time image may be rectangular and give fewer patches than image_size (the first n + 1 rows of pos_embedding are used,
+    :213); more patches than that raise ValueError (the reference fails to broadcast there), and so does an image smaller than one
+    patch, where the reference's behaviour (extract_patches with no window) is not verifiable without TensorFlow.
+    Limits the reference does not have: at most 8 stages after the zip and 1 to 32 heads per stage (NotImplementedError), and heads
+    must be an int or a tuple of ints (TypeError; a bool, which cast_tuple would repeat as one head, is refused too)."""
+    _kind = "pit"
+
+    def __init__(self, image_size, patch_size, num_classes, dim, depth, heads, mlp_dim, dim_head=64, dropout=0.0, emb_dropout=0.0,
+                 *, precision="bf16", device=0, seed=None):
+        assert image_size % patch_size == 0, 'Image dimensions must be divisible by the patch size.'
+        assert isinstance(depth, tuple), 'depth must be a tuple of integers, specifying the number of blocks before each downsizing'
+        stages = pit_stages(depth, heads)
+        side = pit_num_patches(image_size, patch_size)            # ZeroDivisionError for patch_size 1, as conv_output_size raises
+        if len(stages) > _lib.PIT_MAX_STAGES:
+            raise NotImplementedError(f"PiT: the engine runs at most {_lib.PIT_MAX_STAGES} stages; zip(depth, heads) gives {len(stages)}")
+        if any(not 1 <= h <= 32 for _, h in stages):
+            raise NotImplementedError(f"PiT: the engine runs 1 to 32 heads per stage; got {tuple(h for _, h in stages)}")
+        self.num_classes, self.dim, self.dim_head, self.patch_size = num_classes, dim, dim_head, int(patch_size)
+        self.stages, self.num_patches = stages, side * side
+        self._dropout_rates = (dropout, emb_dropout)
+        pc = _lib.VbPitConfig()
+        pc.struct_size = C.sizeof(_lib.VbPitConfig)
+        pc.stages = len(stages)
+        for s, (d, h) in enumerate(stages):
+            pc.depth[s], pc.heads[s] = d, h
+        self._pc = pc
+        lib = _lib.load()
+        self._create(precision, device, create=lambda cfg, dev, h: lib.vb_create_pit(cfg, C.byref(pc), dev, h), image_h=image_size,
+                     image_w=image_size, patch_h=patch_size, patch_w=patch_size, num_classes=num_classes, dim=dim, dim_head=dim_head,
+                     mlp_dim=mlp_dim)
+        self.init_weights(seed)
+
+    def __call__(self, img, training=True, **kwargs):
+        """pit.py:207-219: NHWC float images [b, H, W, 3] -> logits [b, num_classes]; extra kwargs are accepted and ignored, as there."""
+        self._check_training(training)
+        x = np.ascontiguousarray(img, dtype=np.float32)
+        if x.ndim != 4 or x.shape[3] != 3:
+            raise ValueError(f"PiT: img must be NHWC float [b, H, W, 3], got shape {tuple(x.shape)}")
+        b, h, w, _ = x.shape
+        p = self.patch_size
+        if h < p or w < p:
+            raise ValueError(f"PiT: a {h} x {w} image is smaller than one {p} x {p} patch")
+        n = pit_num_patches(h, p) * pit_num_patches(w, p)
+        if n > self.num_patches:
+            raise ValueError(f"PiT: the {h} x {w} image gives {n} patches but pos_embedding has rows for {self.num_patches}")
+        out = np.empty((b, self.num_classes), np.float32)
+        self.forward_raw(x.ctypes.data, _lib.MEM_HOST, b, h, w, out.ctypes.data, _lib.MEM_HOST, None)
+        return _as_tensor(out)
+
+    call = __call__
+
+
+PIT_CTOR_KEYS = ("image_size", "patch_size", "num_classes", "dim", "depth", "heads", "mlp_dim", "dim_head", "dropout", "emb_dropout")
+
+
 def from_config(cfg: dict, precision="bf16", device=0, seed=None):
     """Build a model from an oracle-style config dict (kind + reference kwargs)."""
+    if cfg["kind"] == "pit":
+        return PiT(**{k: v for k, v in cfg.items() if k in PIT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "scalable_vit":
         return ScalableViT(**{k: v for k, v in cfg.items() if k in SCALABLE_VIT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
     if cfg["kind"] == "mobilevit":
