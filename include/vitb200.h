@@ -379,9 +379,11 @@ VB_API int vb_forward(vb_handle* h, const float* img, int32_t img_mem, int32_t b
 VB_API int vb_forward_tokens(vb_handle* h, const float* tokens, int32_t tokens_mem, int32_t batch, int32_t n,
                       float* out, int32_t out_mem, void* stream);
 
-/* DistillMixin.call with a distillation token (reference: distill.py:16-45, DistillableViT distill.py:47-58; ViT only):
- * patch embedding + cls + positions, the token appended as the LAST row, the transformer over n + 2 rows, then
- * logits = mlp_head(pool(x[:, :-1])) and distill_out = x[:, -1].
+/* DistillMixin.call with a distillation token (reference: distill.py:16-45; DistillableViT distill.py:47-58 on a ViT handle,
+ * DistillableT2TViT distill.py:61-72 on a T2TViT handle): patch embedding (T2T: the soft splits and the Dense) + cls +
+ * positions, the token appended as the LAST row, the transformer over n + 2 rows, then
+ * logits = mlp_head(pool(x[:, :-1])) and distill_out = x[:, -1].  A T2TViT handle created with depth 0 (for an injected
+ * transformer) holds no transformer and is refused.
  * distill_token: HOST float32 [dim] (the caller's trainable variable, distill.py:133).  logits [batch, num_classes] and
  * distill_out [batch, dim] live in `out_mem` memory.  img as in vb_forward.
  * LeViT with a distillation head (levit.py:210,220-224): distill_token must be NULL; logits [batch, num_classes] =

@@ -1,2 +1,3 @@
-"""`from vit_tensorflow.distill import DistillableViT` (reference distill.py:47) -- forward path only, on the H100 engine."""
-from vit_tensorflow_b200 import DistillableViT  # noqa: F401
+"""`from vit_tensorflow.distill import DistillableViT, DistillableT2TViT, DistillableEfficientViT` (reference distill.py:47, :61,
+:74) -- forward path only, on the H100 engine."""
+from vit_tensorflow_b200 import DistillableEfficientViT, DistillableT2TViT, DistillableViT  # noqa: F401

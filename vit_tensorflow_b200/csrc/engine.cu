@@ -3557,15 +3557,19 @@ struct vb_handle {
     { ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * rows * HD, s); r2l_rows<T>(ow, HD, out, ldo, HD, win, reg_row0, false, s); }
   }
 
-  // DistillMixin.call (distill.py:16-45) on top of a ViT: embed -> append the distillation token as the LAST row ->
-  // transformer over n + 2 rows -> head on the first n + 1 rows, and the last row returned as is.
+  // DistillMixin.call (distill.py:16-45) on top of a ViT or a T2TViT: embed (the patch Dense, or T2T's soft splits and their
+  // one-layer transformers, as vb_forward runs them) -> append the distillation token as the LAST row -> transformer over
+  // n + 2 rows -> head on the first n + 1 rows, and the last row returned as is.
   template <typename T>
   void distill_impl(const float* img, int B, int H, int Wd, const float* distill_token, float* logits, float* distill_out, cudaStream_t s) {
     const vb_config& c = cfg;
-    VB_CHECK(c.kind == VB_KIND_VIT, "vb_forward_distill supports ViT (distill.py:47 DistillableViT)");
+    VB_CHECK(c.kind == VB_KIND_VIT || c.kind == VB_KIND_T2T_VIT, "vb_forward_distill supports ViT and T2TViT (distill.py:47, :61)");
+    VB_CHECK(c.kind != VB_KIND_T2T_VIT || c.depth > 0,
+             "vb_forward_distill: this T2TViT was built for an injected transformer (depth 0) and holds no main transformer; "
+             "run vb_forward_embed, the injected transformer over the rows with the token appended, and vb_forward_head");
     arena.reset();
     int rows = 0;
-    T* E = embed_tokens<T>(embed, img, B, H, Wd, c.patch_h, c.patch_w, &rows, s, nullptr);
+    T* E = embed_any<T>(img, B, H, Wd, &rows, s, nullptr);
     const int rd = rows + 1;
     T* X = arena.get<T>(static_cast<size_t>(B) * rd * c.dim);
     copy_tokens<T>(E, rows, 0, X, rd, 0, rows, B, c.dim, s);

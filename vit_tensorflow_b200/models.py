@@ -3,6 +3,7 @@
     ViT       vit_tensorflow/vit.py:106-177          DeepViT   vit_tensorflow/deepvit.py:112-157
     CaiT      vit_tensorflow/cait.py:155-194         CrossViT  vit_tensorflow/cross_vit.py:232-303
     parallel_vit.ViT  parallel_vit.py:120-185        DistillableViT  distill.py:47-58 (forward)
+    DistillableT2TViT  distill.py:61-72 (forward)    DistillableEfficientViT  distill.py:74-85 (raises as the reference does)
     T2TViT    vit_tensorflow/t2t.py:50-116           vit_with_patch_merger.ViT / PatchMerger  vit_with_patch_merger.py:42-55,134-185
     efficient.ViT  vit_tensorflow/efficient.py:12-55 (injected transformer between the engine's embed and head stages)
     CvT       vit_tensorflow/cvt.py:149-202
@@ -435,22 +436,31 @@ class DistillableViT(ViT):
         if distill_token is None:
             return super().__call__(img, training=training)
         self._check_training(training)
-        self._finalize()
-        x = np.ascontiguousarray(img, dtype=np.float32)
-        if x.ndim != 4 or x.shape[3] != 3:
-            raise ValueError("img must be NHWC float [b, H, W, 3]")
-        tok = np.ascontiguousarray(distill_token, dtype=np.float32).reshape(-1)
-        if tok.size != self.dim:
-            raise ValueError(f"distill_token must hold dim = {self.dim} values, got shape {np.shape(distill_token)}")
-        b, h, w, _ = x.shape
-        logits = np.empty((b, self.num_classes), np.float32)
-        dist = np.empty((b, self.dim), np.float32)
-        _lib.check(self._lib.vb_forward_distill(self._h, x.ctypes.data_as(C.c_void_p), _lib.MEM_HOST, b, h, w,
-                                                tok.ctypes.data_as(C.c_void_p), logits.ctypes.data_as(C.c_void_p),
-                                                dist.ctypes.data_as(C.c_void_p), _lib.MEM_HOST, None), self._h)
-        return _as_tensor(logits), _as_tensor(dist)
+        return _forward_distill(self, img, distill_token)
 
     call = __call__
+
+
+def _distill_token(model, distill_token):
+    """The caller's distillation token `[1, 1, dim]` (distill.py:101) as a flat float32 vector of `dim` values."""
+    tok = np.ascontiguousarray(distill_token, dtype=np.float32).reshape(-1)
+    if tok.size != model.dim:
+        raise ValueError(f"distill_token must hold dim = {model.dim} values, got shape {np.shape(distill_token)}")
+    return tok
+
+
+def _forward_distill(model, img, distill_token):
+    """DistillMixin.call with a token (distill.py:17-45) on the engine: vb_forward_distill -> (logits, distill_tokens [b, dim])."""
+    model._finalize()
+    x = model._img(img)
+    tok = _distill_token(model, distill_token)
+    b, h, w, _ = x.shape
+    logits = np.empty((b, model.num_classes), np.float32)
+    dist = np.empty((b, model.dim), np.float32)
+    _lib.check(model._lib.vb_forward_distill(model._h, x.ctypes.data_as(C.c_void_p), _lib.MEM_HOST, b, h, w,
+                                             tok.ctypes.data_as(C.c_void_p), logits.ctypes.data_as(C.c_void_p),
+                                             dist.ctypes.data_as(C.c_void_p), _lib.MEM_HOST, None), model._h)
+    return _as_tensor(logits), _as_tensor(dist)
 
 
 class DeepViT(ViT):
@@ -552,6 +562,31 @@ class T2TViT(_EngineModel):
     call = __call__
 
 
+class DistillableT2TViT(T2TViT):
+    """distill.py:61-72 (DistillMixin.call distill.py:16-45): a T2TViT whose call takes an optional distillation token
+    `[1, 1, dim]`; with it the call returns `(logits, distill_tokens [b, dim])`, without it plain T2TViT logits.  With an
+    injected `transformer=` the call is composed on the host around it.  Forward only, as DistillableViT."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.args, self.kwargs = args, kwargs
+        self.dim, self.num_classes = kwargs["dim"], kwargs["num_classes"]
+
+    def __call__(self, img, distill_token=None, training=True):
+        if distill_token is None:
+            return super().__call__(img, training=training)
+        self._check_training(training)
+        if self._injected is None:
+            return _forward_distill(self, img, distill_token)
+        tok = _distill_token(self, distill_token)
+        x = self.forward_embed(img)                                   # distill.py:19-24: n + 1 rows
+        x = np.concatenate([x, np.broadcast_to(tok, (x.shape[0], 1, self.dim))], axis=1)   # :26-28: the token as the last row
+        x = np.asarray(self._injected(x, training=training), dtype=np.float32)             # :30, _attend :69-72
+        return self.forward_head(x[:, :-1]), _as_tensor(np.ascontiguousarray(x[:, -1]))    # :32-43
+
+    call = __call__
+
+
 class PatchMergerViT(_EngineModel):
     """vit_with_patch_merger.py:134-185 (`vit_with_patch_merger.ViT`): no cls token, a PatchMerger after layer
     `patch_merge_layer` (default depth // 2) shrinking the stream to `patch_merge_num_tokens` rows, mean pooling."""
@@ -614,6 +649,23 @@ class EfficientViT(_EngineModel):
         x = self.forward_embed(img)                                              # efficient.py:40-45
         x = np.asarray(self.transformer(x, training=training), dtype=np.float32)  # :46
         return self.forward_head(x)                                              # :48-55
+
+    call = __call__
+
+
+class DistillableEfficientViT(EfficientViT):
+    """distill.py:74-85 as the reference runs it: its `_attend` reads `self.dropout` (:83), which efficient.ViT never defines
+    (efficient.py:13-55), so every call, with or without a token, raises AttributeError (SURVEY.md App. D).  It constructs and
+    carries `dim`, `num_classes`, `args` and `kwargs`, which DistillWrapper's constructor reads (distill.py:91-97)."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        del self.dropout                                  # the shell's identity stand-in; efficient.ViT has no `dropout`
+        self.args, self.kwargs = args, kwargs
+        self.dim, self.num_classes = kwargs["dim"], kwargs["num_classes"]
+
+    def __call__(self, img, distill_token=None, training=True):
+        raise AttributeError(f"'{type(self).__name__}' object has no attribute 'dropout'")
 
     call = __call__
 
