@@ -26,12 +26,6 @@
 #include <type_traits>
 #include <vector>
 
-#ifndef VB_FWD_STREAMS
-#define VB_FWD_STREAMS 1                 // 2 = split a large ViT batch into two half-batches on two streams (forward_impl); measured no gain
-#endif
-#ifndef VB_FWD_SPLIT_MIN_HALF
-#define VB_FWD_SPLIT_MIN_HALF 64         // smallest half-batch worth a stream of its own
-#endif
 namespace vb {
 namespace {
 
@@ -396,13 +390,8 @@ struct vb_handle {
   static constexpr int T2T_MAX_STREAMS = 4;
   cudaStream_t side_streams[T2T_MAX_STREAMS - 1] = {nullptr, nullptr, nullptr};
   cudaEvent_t fork_event = nullptr, join_events[T2T_MAX_STREAMS - 1] = {nullptr, nullptr, nullptr};
-  cudaStream_t half_stream = nullptr;                    // second half-batch of a split forward (forward_impl)
-  cudaEvent_t fwd_fork_event = nullptr, fwd_join_event = nullptr;
   void ensure_side_streams() {
     if (fork_event != nullptr) return;
-    VB_CUDA(cudaStreamCreateWithFlags(&half_stream, cudaStreamNonBlocking));
-    VB_CUDA(cudaEventCreateWithFlags(&fwd_fork_event, cudaEventDisableTiming));
-    VB_CUDA(cudaEventCreateWithFlags(&fwd_join_event, cudaEventDisableTiming));
     VB_CUDA(cudaEventCreateWithFlags(&fork_event, cudaEventDisableTiming));
     for (int i = 0; i < T2T_MAX_STREAMS - 1; ++i) {
       VB_CUDA(cudaStreamCreateWithFlags(&side_streams[i], cudaStreamNonBlocking));
@@ -412,7 +401,6 @@ struct vb_handle {
   void destroy_side_streams() {
     if (fork_event == nullptr) return;
     cudaEventDestroy(fork_event);
-    cudaEventDestroy(fwd_fork_event); cudaEventDestroy(fwd_join_event); cudaStreamDestroy(half_stream);
     for (int i = 0; i < T2T_MAX_STREAMS - 1; ++i) { cudaEventDestroy(join_events[i]); cudaStreamDestroy(side_streams[i]); }
     fork_event = nullptr;
   }
@@ -1194,7 +1182,7 @@ struct vb_handle {
     // real PV columns are unchanged) and zero to_out input rows.  Costs (64 / dh - 1) more flops in those two GEMMs and buys
     // the tensor-core attention path for e.g. dim_head 48 / 32 (the head-mixing variants have their own kernel, attn_mix).
     const bool to_out_present = has(pre + "to_out.kernel");
-    if (bf16() && dh < 64 && dh % 8 == 0 && to_out_present && dim % 8 == 0 && getenv("VB_NO_HEAD_PAD") == nullptr &&
+    if (bf16() && dh < 64 && dh % 8 == 0 && to_out_present && dim % 8 == 0 &&
         (kind == VB_KIND_VIT || kind == VB_KIND_CROSSVIT || kind == VB_KIND_ATS_VIT || kind == VB_KIND_SMALL_DATASET_VIT)) {
       const int dhp = 64;
       auto padded = [&](const std::string& n, int other, int groups, int pad_rows) {
@@ -1214,7 +1202,7 @@ struct vb_handle {
     l.attn_norm = make_norm(pre + "attn_norm", dim);
     l.ff_norm = make_norm(pre + "ff_norm", dim);
     // LayerNorm folding needs every GEMM of the layer on the wgmma path (all widths multiples of 64)
-    l.folded = bf16() && fold_ok && dim % 64 == 0 && inner % 64 == 0 && mlp % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr;
+    l.folded = bf16() && fold_ok && dim % 64 == 0 && inner % 64 == 0 && mlp % 64 == 0;
     const Norm* fa = l.folded ? &l.attn_norm : nullptr;
     const Norm* ff = l.folded ? &l.ff_norm : nullptr;
     if (kind == VB_KIND_VIT || kind == VB_KIND_DEEPVIT || kind == VB_KIND_ATS_VIT || kind == VB_KIND_SMALL_DATASET_VIT) {
@@ -1241,7 +1229,6 @@ struct vb_handle {
   // Dp = round_up(D, 64) -- token rows [n, Dp] with zero pad columns, to_qkv columns [q | k | v] each Dp wide, fc1 / fc2 Dp x Dp --
   // so that all four GEMMs and the per-image QK^T / PV products run on the wgmma GEMM kernel; LayerNorm and the softmax scale keep
   // the true D.  Zero weights and biases keep the pad columns exactly zero through the layer (GELU(0) = 0).
-  static bool t2t_tensor_path_enabled() { static const bool off = getenv("VB_NO_T2T_TC") != nullptr; return !off; }
   LayerW make_t2t_layer(const std::string& pre, int D) {
     const int Dp = round_up(D, 64);
     auto padded = [&](const std::string& n, int other, int groups, int pad_rows, const float* src, int dh_src) {
@@ -1276,7 +1263,7 @@ struct vb_handle {
     l.heads = heads; l.dim_head = dim / heads; l.dh_model = l.dim_head;
     l.attn_norm = make_norm(pre + "attn_norm", dim);
     l.ff_norm = make_norm(pre + "norm1", dim);
-    l.folded = bf16() && dim % 64 == 0 && mlp % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr;   // every GEMM on the wgmma path
+    l.folded = bf16() && dim % 64 == 0 && mlp % 64 == 0;   // every GEMM on the wgmma path
     l.fused_qkv = true;
     l.to_qkv = make_linear(pre + "to_qkv", dim, 3 * dim, false, l.folded ? &l.attn_norm : nullptr);
     l.to_out = make_linear(pre + "to_out", dim, dim);
@@ -1334,7 +1321,7 @@ struct vb_handle {
         out = conv_output_size(out, st[i].k, st[i].stride);
         if (i + 1 < st.size()) {
           const std::string pre = "t2t." + std::to_string(i) + ".layers.0.";
-          if (bf16() && t2t_tensor_path_enabled()) t2t_layers.push_back(make_t2t_layer(pre, st[i].dim));
+          if (bf16()) t2t_layers.push_back(make_t2t_layer(pre, st[i].dim));
           else t2t_layers.push_back(make_layer(pre, st[i].dim, 1, st[i].dim, st[i].dim, VB_KIND_VIT, false));
         }
       }
@@ -1998,13 +1985,13 @@ struct vb_handle {
     head = make_linear_f32("head", c.dim, c.num_classes);
   }
   // SPT's LayerNorm gamma / beta [K] (eps 1e-3) and patch Dense W [K, dim] + bias as spt_tokens runs them: the bf16 engine zero-pads
-  // K to Kp = round_up(K, 64) and folds the LayerNorm into the wgmma GEMM (dim % 64 == 0, unless VB_NO_LN_FOLD is set); otherwise
+  // K to Kp = round_up(K, 64) and folds the LayerNorm into the wgmma GEMM (dim % 64 == 0); otherwise
   // the LayerNorm kernel runs first.  Either way the Dense yields beta . W + bias on the all-zero cls row, so that is the term the
   // embedding residual takes off (res_bias).
   void set_spt_patch(const std::vector<double>& gamma, const std::vector<double>& beta, const std::vector<double>& Wk,
                      std::vector<double> bias, int K, int dim) {
     const int Kp = bf16() ? round_up(K, 64) : K;
-    const bool fold = bf16() && dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr;
+    const bool fold = bf16() && dim % 64 == 0;
     spt_norm = Norm{upload_owned(pad_n(gamma, Kp)), upload_owned(pad_n(beta, Kp)), K};
     embed.patch = linear_from_host("spt.patch", pad_kn(Wk, K, dim, Kp, dim), bias, Kp, dim, fold ? &spt_norm : nullptr);
     if (fold) {
@@ -2086,7 +2073,7 @@ struct vb_handle {
     T* X = arena.get<T>(static_cast<size_t>(M) * e.dim);
     Epi ep; ep.bias = e.patch.bias; ep.res = R; ep.ldr = e.dim;
     if (ln_stats != nullptr) { ep.ln_stats = ln_stats; ep.bias = e.patch.ln_c2; }
-    if (stats_out != nullptr && bf16() && e.dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr) {
+    if (stats_out != nullptr && bf16() && e.dim % 64 == 0) {
       *stats_out = row_stats(M, e.dim);
       ep.stats_out = *stats_out;
     }
@@ -2137,7 +2124,7 @@ struct vb_handle {
       const int D = st[i].dim, n = oh * ow;
       VB_CHECK(i == 0 || mh == mw, "T2TViT: token maps after the first soft split must be square (t2t.py:41)");
       const bool last = i + 1 == st.size();
-      const bool tc = !last && t2t_layers[i].t2t_Dp > 0;               // tensor-core layer: token rows padded to Dp columns
+      const bool tc = !last && bf16();                                 // tensor-core layer: token rows padded to Dp columns
       const int ld = last ? (bf16() ? embed.patch.ldw : embed.patch.K) : (tc ? t2t_layers[i].t2t_Dp : D);
       const int cls_row = last ? 1 : 0;
       T* out = arena.get<T>(static_cast<size_t>(B) * (n + cls_row) * ld);
@@ -2561,34 +2548,9 @@ struct vb_handle {
                                    accumulate ? logits : nullptr, hd.N, 0, s);
   }
 
-  // Images are independent, so a large batch can run as two half-batches on two streams (the forward's own and `half_stream`,
-  // forked / joined with timing-less events and therefore part of a captured graph): while one half's kernel drains -- last
-  // epilogues, CTAs finishing at different times, the dependent launch waiting for the whole grid -- the other half's next
-  // kernel already has CTAs on the freed SMs.  Results are bit-identical to the unsplit forward (every kernel's tile
-  // arithmetic is independent of the batch, tests: test_batch_independence_and_determinism).  ViT, DeepViT and CaiT only (T2T
-  // and CrossViT fork streams of their own).
-  // The split doubles the number of launches (half the tiles per kernel); its speed on the H100 is not measured.  Off by
-  // default (VB_FWD_STREAMS=2 enables it).
   template <typename T>
   void forward_impl(const float* img, int B, int H, int Wd, float* logits, cudaStream_t s) {
     arena.reset();
-    static const char* fs_env = getenv("VB_FWD_STREAMS");
-    const int want = fs_env != nullptr ? atoi(fs_env) : VB_FWD_STREAMS;
-    const bool split = want >= 2 && !profiling && bf16() && B >= 2 * VB_FWD_SPLIT_MIN_HALF &&
-                       (cfg.kind == VB_KIND_VIT || cfg.kind == VB_KIND_DEEPVIT || cfg.kind == VB_KIND_CAIT);
-    if (!split) { forward_body<T>(img, B, H, Wd, logits, s); return; }
-    ensure_side_streams();
-    const int B0 = (B + 1) / 2;
-    VB_CUDA(cudaEventRecord(fwd_fork_event, s));
-    VB_CUDA(cudaStreamWaitEvent(half_stream, fwd_fork_event, 0));
-    forward_body<T>(img, B0, H, Wd, logits, s);
-    forward_body<T>(img + static_cast<size_t>(B0) * H * Wd * cfg.channels, B - B0, H, Wd, logits + static_cast<size_t>(B0) * cfg.num_classes, half_stream);
-    VB_CUDA(cudaEventRecord(fwd_join_event, half_stream));
-    VB_CUDA(cudaStreamWaitEvent(s, fwd_join_event, 0));
-  }
-
-  template <typename T>
-  void forward_body(const float* img, int B, int H, int Wd, float* logits, cudaStream_t s) {
     const vb_config& c = cfg;
     if (c.kind == VB_KIND_VIT || c.kind == VB_KIND_DEEPVIT || c.kind == VB_KIND_T2T_VIT || c.kind == VB_KIND_PIT) {
       int rows = 0;
@@ -2660,7 +2622,7 @@ struct vb_handle {
     } else if (c.kind == VB_KIND_CCT) {                   // CCT.call cct.py:342-345, TransformerClassifier.call :277-305
       int rows = 0;
       T* X = tokenize_cct<T>(img, B, H, Wd, &rows, s);
-      float* stats = c.dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr ? row_stats(static_cast<long long>(B) * rows, c.dim) : nullptr;
+      float* stats = c.dim % 64 == 0 ? row_stats(static_cast<long long>(B) * rows, c.dim) : nullptr;
       bool sv = false;
       for (const auto& l : layers) layer_cct<T>(X, B, rows, c.dim, l, s, stats, &sv);
       float* z = arena.get<float>(static_cast<size_t>(B) * c.dim);
@@ -2681,9 +2643,8 @@ struct vb_handle {
       T* ctx_sm = arena.get<T>(static_cast<size_t>(B) * ns * c.sm_dim);   // [LN(Pin(lg_cls)) ; sm patches]
       // The two towers of a multi-scale block are independent until the cross-attention (cross_vit.py:185-190): the large-patch
       // tower (n = 17 at the README configuration: GEMMs of a few tiles) runs on a side stream beside the small-patch one, forked
-      // and joined with timing-less events (part of the captured graph).  VB_CROSSVIT_STREAMS=1 keeps one stream.
-      static const char* xs_env = getenv("VB_CROSSVIT_STREAMS");
-      const bool two = (xs_env != nullptr ? atoi(xs_env) : 2) >= 2 && !profiling && bf16();
+      // and joined with timing-less events (part of the captured graph).  Profiling keeps one stream: per-class event timing wants it.
+      const bool two = !profiling && bf16();
       cudaStream_t sg = s;
       if (two) { ensure_side_streams(); sg = side_streams[0]; }
       for (const auto& xb : xblocks) {
@@ -3575,7 +3536,7 @@ struct vb_handle {
     copy_tokens<T>(E, rows, 0, X, rd, 0, rows, B, c.dim, s);
     T* last = X + static_cast<size_t>(rows) * c.dim;                 // row `rows` of image 0; image pitch rd rows
     broadcast_row<T>(distill_token, last, rd, B, c.dim, s);
-    float* stats = c.dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr ? row_stats(static_cast<long long>(B) * rd, c.dim) : nullptr;
+    float* stats = c.dim % 64 == 0 ? row_stats(static_cast<long long>(B) * rd, c.dim) : nullptr;
     bool sv = false;
     for (const auto& l : layers) layer_self<T>(X, B, rd, c.dim, l, s, stats, &sv);
     T* Xh = arena.get<T>(static_cast<size_t>(B) * rows * c.dim);     // x[:, :-1]
@@ -3602,7 +3563,7 @@ struct vb_handle {
       X = arena.get<T>(count);
       convert<float, __nv_bfloat16>(tok, reinterpret_cast<__nv_bfloat16*>(X), count, s);
     }
-    float* stats = cfg.dim % 64 == 0 && getenv("VB_NO_LN_FOLD") == nullptr ? row_stats(static_cast<long long>(B) * n, cfg.dim) : nullptr;
+    float* stats = cfg.dim % 64 == 0 ? row_stats(static_cast<long long>(B) * n, cfg.dim) : nullptr;
     bool sv = false;
     for (const auto& l : layers) layer_self<T>(X, B, n, cfg.dim, l, s, stats, &sv);
     if (sizeof(T) == 4) VB_CUDA(cudaMemcpyAsync(out, X, count * 4, cudaMemcpyDeviceToDevice, s));
@@ -3749,9 +3710,7 @@ void vb_handle::layer_t2t<__nv_bfloat16>(__nv_bfloat16* X, int B, int n, const L
   // stream leaves most SMs idle and pays every launch gap (389 launches per T2T step at batch 64).  Two streams
   // when one image's buffers are large (n = 3136: 59 MB each, more than the 50 MB L2 already), four otherwise.
   const size_t s_elems = static_cast<size_t>(n) * npad;
-  static const char* ns_env = getenv("VB_T2T_STREAMS");
-  int ns = ns_env != nullptr ? atoi(ns_env) : (s_elems * 6 > (48u << 20) ? 2 : 4);
-  ns = std::max(1, std::min(ns, std::min(B, static_cast<int>(T2T_MAX_STREAMS))));
+  int ns = std::min(s_elems * 6 > (48u << 20) ? 2 : T2T_MAX_STREAMS, B);
   if (profiling) ns = 1;                                         // per-class event timing wants one stream
   float* S[T2T_MAX_STREAMS];
   bf* P[T2T_MAX_STREAMS];
