@@ -24,10 +24,12 @@
 //                   in flight while the previous one's stage is released; then the epilogue from the accumulator
 //                   registers (bias / folded LayerNorm / GELU / LayerScale / residual, optional per-64-column row
 //                   statistics of the stored values), reading its operands from shared memory only.  A bf16 tile is
-//                   written into the staging tile (over its residual) and leaves by one TMA store per 64 x 128 half; an
+//                   written into the staging tile (over its residual) by stmatrix and leaves by one TMA store per 64 x 128 half; an
 //                   fp32 tile is stored straight from registers.  Two named barriers pass the main loop from one
 //                   warpgroup to the other, so the main loops take turns on the tensor cores and one tile's epilogue runs
 //                   under the next tile's main loop.
+#include <type_traits>
+
 #include "common.h"
 #include "kernels.cuh"
 #include "ptx.cuh"
@@ -71,15 +73,19 @@ static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= 168 * THREADS, "setma
 // leading coefficient is negative and q is monotone beyond the fit range, so no clamp is needed: for |x| > 6 the tail
 // term |x| 2^q is below 6 * 2^-29 and shrinks.  Max abs error of the GELU 5.7e-7 = 0.003 bf16 ulp of the result for
 // every finite x; gelu(+inf) = +inf and gelu(-inf) = NaN as in the reference's x * Phi(x).
-__device__ __forceinline__ float gelu_erf(float x) {
-  const float na = -fabsf(x);
-  float q = fmaf(4.881368368e-04f, na, 7.198925130e-03f);          // odd coefficients negated: q(-na)
-  q = fmaf(q, na, 5.214704946e-02f);
-  q = fmaf(q, na, -4.595955014e-01f);
-  q = fmaf(q, na, 1.151000619e+00f);
+// It takes h = x / 2, which the epilogue's bias / folded-LayerNorm FMAs produce at no cost (their operands are staged
+// halved), and returns  h - |h| (2 E - 1)  with q's k-th coefficient scaled by 2^k for the argument -|h|.  Every scaling
+// is by a power of two, so each rounding is the one  x/2 - |x| (E - 1/2)  makes from x (outside the subnormal range),
+// without its multiply by 1/2.
+__device__ __forceinline__ float gelu_erf_half(float h) {
+  const float na = -fabsf(h);                                        // -|x| / 2
+  float q = fmaf(4.881368368e-04f * 32.f, na, 7.198925130e-03f * 16.f);   // odd coefficients negated: q(-2 na)
+  q = fmaf(q, na, 5.214704946e-02f * 8.f);
+  q = fmaf(q, na, -4.595955014e-01f * 4.f);
+  q = fmaf(q, na, 1.151000619e+00f * 2.f);
   q = fmaf(q, na, -1.0f);
   const float e = ex2_approx(q);                                     // erfc(|x|/sqrt2) / 2
-  return fmaf(na, e + -0.5f, x * 0.5f);
+  return fmaf(na, fmaf(2.f, e, -1.f), h);
 }
 
 // levit.py:37: x * relu6(x + 3) / 6, rounded in the reference's order
@@ -167,6 +173,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       // tile i goes to consumer warpgroup w = i % 2 as soon as that warpgroup's tile i - 2 has left its buffers, i.e.
       // while the other warpgroup runs tile i - 1's main loop, well before tile i's epilogue needs them
       const int pt = tid - 32;
+      // the GELU epilogue computes x / 2 (gelu_erf_half's argument): the bias (c2) and the rows' rstd, -mu rstd are staged
+      // halved, which leaves every rounding of the bias / folded-LayerNorm FMAs as it is, halved
+      constexpr float HALF = ACT == ACT_GELU ? 0.5f : 1.f;
       int i = 0;
       for (long long t = blockIdx.x; t < tiles; t += gridDim.x, ++i) {
         const int w = i & 1;
@@ -189,7 +198,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
             if (EPI == 2) c1 = __ldg(ln_c1 + n0 + c);
             if (scale != nullptr) s = __ldg(scale + n0 + c);
           }
-          par[c] = b;
+          par[c] = b * HALF;
           par[BN + c] = c1;
           par[2 * BN + c] = s;
         }
@@ -211,8 +220,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
               rstd = rsqrtf(fmaxf(fmaf(s2, ln_inv_d, -__fmul_rn(mu, mu)), 0.f) + ln_eps);
               nmr = -mu * rstd;
             }
-            par[3 * BN + r] = rstd;
-            par[3 * BN + BM + r] = nmr;
+            par[3 * BN + r] = rstd * HALF;
+            par[3 * BN + BM + r] = nmr * HALF;
           }
         }
         mbar_arrive(epi_full(w));
@@ -233,7 +242,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const float* const par = params + cw * PARAM_FLOATS;
   uint8_t* const stg = smem + STAGES * STAGE_BYTES + cw * STG_BYTES;
   const int row_l = warp * 16 + (lane >> 2);                       // this thread's accumulator rows in the tile: row_l +
-                                                                   // 64 hm + 8 h, q = 2 hm + h below; all = lane / 4 (mod 8)
+                                                                   // 64 hm + 8 h; all = lane / 4 (mod 8)
   int stage = 0;
   uint32_t phase = 0, epi_phase = 0;
   ring_advance<STAGES>(stage, phase, cw * num_kb);                 // warpgroup 1 starts after tile 0's k-blocks
@@ -283,79 +292,128 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     // =================================================================== epilogue, 64-column chunks
     mbar_wait(epi_full(cw), epi_phase);                            // operands (and residual tile) staged by warps 1-3
     epi_phase ^= 1;
-    float ln_rstd[4] = {0.f, 0.f, 0.f, 0.f}, ln_nmr[4] = {0.f, 0.f, 0.f, 0.f};   // rows row_l + 64 (q / 2) + 8 (q % 2)
-    if (EPI == 2) {
+    // The tile in groups of 8 accumulators per thread: two 8-column blocks jj = 2 jp, 2 jp + 1 of one 64-column chunk c, in
+    // the rows row_l + 64 hm + 8 h (h = 0, 1) of one 64-row half hm.  A group's 8 elements are independent from the
+    // accumulator to the store, so the activation's dependent chains (about eight FP32 operations and one MUFU each) overlap
+    // each other, and the group leaves as the four 8 x 8 matrices of one stmatrix.x4 (its residual arrives by the matching
+    // ldmatrix.x4).  The halves go one after the other, so only their two rows' LayerNorm terms are held in registers.
+    // LEAN: neither LayerScale nor row statistics, decided once per tile instead of paying a multiply by 1 and the
+    // predicated statistics on every element (fc1 and to_qkv run LEAN).
+    auto epilogue = [&](auto lean) {
+      constexpr bool LEAN = decltype(lean)::value;
+      const bool has_scale = !LEAN && scale != nullptr, has_stats = !LEAN && stats_out != nullptr;
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        ln_rstd[q] = par[3 * BN + row_l + 64 * (q >> 1) + 8 * (q & 1)];
-        ln_nmr[q] = par[3 * BN + BM + row_l + 64 * (q >> 1) + 8 * (q & 1)];
-      }
-    }
+      for (int hm = 0; hm < 2; ++hm) {
+        float ln_rstd[2] = {0.f, 0.f}, ln_nmr[2] = {0.f, 0.f};   // rows row_l + 64 hm + 8 h
+        if (EPI == 2) {
 #pragma unroll
-    for (int c = 0; c < BN / 64; ++c) {
-      const int nc = n0 + c * 64;
-      if (nc >= N) break;                                          // N % 64 == 0: a chunk is entirely in or out
-      float st1[4] = {0.f, 0.f, 0.f, 0.f}, st2[4] = {0.f, 0.f, 0.f, 0.f};   // (sum, sumsq) of the stored bf16 outputs, per row
-      uint8_t* const half = stg + c * HALF_BYTES;
-#pragma unroll
-      for (int jj = 0; jj < 8; ++jj) {
-        const int j = c * 8 + jj;
-        const int n = nc + jj * 8 + col_t;
-        float cb0 = 0.f, cb1 = 0.f, c10 = 0.f, c11 = 0.f, sc0 = 1.f, sc1 = 1.f;
-        if (EPI >= 1) { const float2 b2 = *reinterpret_cast<const float2*>(par + (n - n0)); cb0 = b2.x; cb1 = b2.y; }
-        if (EPI == 2) { const float2 c2 = *reinterpret_cast<const float2*>(par + BN + (n - n0)); c10 = c2.x; c11 = c2.y; }
-        if (scale != nullptr) { const float2 s2 = *reinterpret_cast<const float2*>(par + 2 * BN + (n - n0)); sc0 = s2.x; sc1 = s2.y; }
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int rl = row_l + 64 * (q >> 1) + 8 * (q & 1);
-          float v0 = acc[q >> 1][4 * j + 2 * (q & 1)], v1 = acc[q >> 1][4 * j + 2 * (q & 1) + 1];
-          if (EPI == 2) {
-            v0 = fmaf(v0, ln_rstd[q], fmaf(c10, ln_nmr[q], cb0));
-            v1 = fmaf(v1, ln_rstd[q], fmaf(c11, ln_nmr[q], cb1));
-          } else if (EPI == 1) {
-            v0 += cb0;
-            v1 += cb1;
+          for (int h = 0; h < 2; ++h) {
+            ln_rstd[h] = par[3 * BN + row_l + 64 * hm + 8 * h];
+            ln_nmr[h] = par[3 * BN + BM + row_l + 64 * hm + 8 * h];
           }
-          if (ACT == ACT_GELU) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
-          if (ACT == ACT_HSWISH) { v0 = hard_swish(v0); v1 = hard_swish(v1); }
-          if (ACT == ACT_SILU) { v0 = silu(v0); v1 = silu(v1); }
-          // rounded on its own, as the reference's LayerScale is, never fused with the residual add into one FMA
-          if (scale != nullptr) { v0 = __fmul_rn(v0, sc0); v1 = __fmul_rn(v1, sc1); }
-          if (OF32) {
-            if (m0 + rl < M)
-              *reinterpret_cast<float2*>(out_f32 + static_cast<size_t>(m0 + rl) * ldc + n) = make_float2(v0, v1);
-          } else {
-            // the staging tile in TMA's 128B-swizzled layout: 16-byte chunk jj of row rl at chunk jj ^ (rl % 8), so the
-            // 8 rows x 4 lanes of a warp's access hit 32 distinct banks.  The residual (zero in rows >= M, which the store
-            // clips) is read here and overwritten by the output, by the same thread.
-            uint32_t* const p = reinterpret_cast<uint32_t*>(half + rl * 128 + ((jj ^ (lane >> 2)) << 4) + 4 * (lane & 3));
-            if (RES) {
-              const uint32_t rw = *p;
-              v0 += bf16_lo(rw);
-              v1 += bf16_hi(rw);
+        }
+#pragma unroll
+        for (int c = 0; c < BN / 64; ++c) {
+          const int nc = n0 + c * 64;
+          if (nc >= N) break;                                      // N % 64 == 0: a chunk is entirely in or out
+          float st1[2] = {0.f, 0.f}, st2[2] = {0.f, 0.f};          // (sum, sumsq) of the stored bf16 outputs, per row
+          // the staging tile in TMA's 128B-swizzled layout: 16-byte chunk k of row r at chunk k ^ (r % 8), so the 8 rows a
+          // matrix's lanes address hit 8 distinct 16-byte bank groups.  Lane t addresses row t % 8 of matrix i = t / 8 of a
+          // group: row warp 16 + 64 hm + 8 (i % 2) + t % 8, 16-byte chunk 2 jp + i / 2, so r[i] holds (h, jj) = (i % 2, 2 jp + i / 2)
+          const uint32_t rows = smem_u32(stg) + c * HALF_BYTES + (warp * 16 + 64 * hm + 8 * ((lane >> 3) & 1) + (lane & 7)) * 128;
+          const uint32_t swz = (lane >> 4) ^ (lane & 7);
+#pragma unroll
+          for (int jp = 0; jp < 4; ++jp) {
+            float v[4][2];                                         // [i = 2 u + h][column 0 / 1]
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {                          // columns (2 jp + u) 8 + col_t, + 1 of the chunk
+              const int cn = c * 64 + (2 * jp + u) * 8 + col_t;
+              float cb[2] = {0.f, 0.f}, c1[2] = {0.f, 0.f};
+              if (EPI >= 1) { const float2 b2 = *reinterpret_cast<const float2*>(par + cn); cb[0] = b2.x; cb[1] = b2.y; }
+              if (EPI == 2) { const float2 c2 = *reinterpret_cast<const float2*>(par + BN + cn); c1[0] = c2.x; c1[1] = c2.y; }
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  float x = acc[hm][4 * (c * 8 + 2 * jp + u) + 2 * h + e];
+                  if (EPI == 2) x = fmaf(x, ln_rstd[h], fmaf(c1[e], ln_nmr[h], cb[e]));
+                  else if (EPI == 1) x = ACT == ACT_GELU ? fmaf(x, 0.5f, cb[e]) : x + cb[e];
+                  else if (ACT == ACT_GELU) x *= 0.5f;
+                  v[2 * u + h][e] = x;
+                }
+              }
             }
-            const uint32_t pk = pack_bf16x2(v0, v1);
-            *p = pk;
-            if (stats_out != nullptr) {
-              const float a0 = bf16_lo(pk), a1 = bf16_hi(pk);
-              st1[q] += a0 + a1;
-              st2[q] = fmaf(a0, a0, fmaf(a1, a1, st2[q]));
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                if (ACT == ACT_GELU) v[i][e] = gelu_erf_half(v[i][e]);   // of 2 v: see the staging of par
+                if (ACT == ACT_HSWISH) v[i][e] = hard_swish(v[i][e]);
+                if (ACT == ACT_SILU) v[i][e] = silu(v[i][e]);
+              }
+            }
+            if (has_scale) {
+#pragma unroll
+              for (int u = 0; u < 2; ++u) {
+                const float2 s2 = *reinterpret_cast<const float2*>(par + 2 * BN + c * 64 + (2 * jp + u) * 8 + col_t);
+                // rounded on its own, as the reference's LayerScale is, never fused with the residual add into one FMA
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  v[2 * u + h][0] = __fmul_rn(v[2 * u + h][0], s2.x);
+                  v[2 * u + h][1] = __fmul_rn(v[2 * u + h][1], s2.y);
+                }
+              }
+            }
+            if (OF32) {
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                const int rl = row_l + 64 * hm + 8 * (i & 1);
+                if (m0 + rl < M)
+                  *reinterpret_cast<float2*>(out_f32 + static_cast<size_t>(m0 + rl) * ldc + nc + (2 * jp + (i >> 1)) * 8 + col_t) =
+                      make_float2(v[i][0], v[i][1]);
+              }
+            } else {
+              const uint32_t addr = rows + (((2u * jp) ^ swz) << 4);
+              uint32_t r[4];
+              // the residual (zero in rows >= M, which the store clips) is read here and overwritten by the output, by the
+              // same warp
+              if (RES) ldmatrix_x4(addr, r);
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                if (RES) {
+                  v[i][0] += bf16_lo(r[i]);
+                  v[i][1] += bf16_hi(r[i]);
+                }
+                r[i] = pack_bf16x2(v[i][0], v[i][1]);
+              }
+              stmatrix_x4(addr, r);
+              if (has_stats) {
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                  const float a0 = bf16_lo(r[i]), a1 = bf16_hi(r[i]);
+                  st1[i & 1] += a0 + a1;
+                  st2[i & 1] = fmaf(a0, a0, fmaf(a1, a1, st2[i & 1]));
+                }
+              }
+            }
+          }
+          if (has_stats) {                                         // the row's 64 columns are spread over the 4 lanes of a quad
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              st1[h] += __shfl_xor_sync(0xffffffffu, st1[h], 1);
+              st2[h] += __shfl_xor_sync(0xffffffffu, st2[h], 1);
+              st1[h] += __shfl_xor_sync(0xffffffffu, st1[h], 2);
+              st2[h] += __shfl_xor_sync(0xffffffffu, st2[h], 2);
+              const int r = m0 + row_l + 64 * hm + 8 * h;
+              if ((lane & 3) == 0 && r < M) stats_out[static_cast<size_t>(nc >> 6) * M + r] = make_float2(st1[h], st2[h]);   // [part][M]
             }
           }
         }
       }
-      if (stats_out != nullptr) {                                  // the row's 64 columns are spread over the 4 lanes of a quad
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          st1[q] += __shfl_xor_sync(0xffffffffu, st1[q], 1);
-          st2[q] += __shfl_xor_sync(0xffffffffu, st2[q], 1);
-          st1[q] += __shfl_xor_sync(0xffffffffu, st1[q], 2);
-          st2[q] += __shfl_xor_sync(0xffffffffu, st2[q], 2);
-          const int r = m0 + row_l + 64 * (q >> 1) + 8 * (q & 1);
-          if ((lane & 3) == 0 && r < M) stats_out[static_cast<size_t>(nc >> 6) * M + r] = make_float2(st1[q], st2[q]);   // [part][M]
-        }
-      }
-    }
+    };
+    if constexpr (OF32) epilogue(std::true_type{});
+    else if (scale == nullptr && stats_out == nullptr) epilogue(std::true_type{});
+    else epilogue(std::false_type{});
     // The staged bf16 tile leaves by TMA (rows >= M clipped); once it has been read out, the buffers go back to warps 1-3.
     // `res` may alias `out`: the tile's residual was loaded before this store, and no other tile touches these elements.
     if (!OF32) fence_proxy_async_smem();

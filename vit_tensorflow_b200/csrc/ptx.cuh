@@ -153,6 +153,18 @@ __device__ __forceinline__ void wgmma_m64n192k16_bf16(float (&d)[96], uint64_t d
       : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
 
+// Four 8 x 8 b16 matrices between shared memory and registers, one instruction per warp: lanes 8 i .. 8 i + 7 give the
+// addresses of matrix i's rows (16 contiguous bytes each), and lane t holds row t / 4, columns 2 (t % 4) and + 1 of
+// matrix i in r[i] -- the layout of an mma / wgmma accumulator fragment.
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};"
+               ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]) : "memory");
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
+}
+
 // ------------------------------------------------------------------------------------------ misc
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
