@@ -18,6 +18,7 @@
  *     RegionViT(...)(img)            vit_tensorflow/regionvit.py:184-263 (vb_create_regionvit)
  *     ScalableViT(...)(img)          vit_tensorflow/scalable_vit.py:250-319 (vb_create_scalable_vit)
  *     PiT(...)(img)                  vit_tensorflow/pit.py:158-219 (vb_create_pit)
+ *     MAE(...)(img) / SimMIM(...)(img)   vit_tensorflow/mae.py:49-92, simmim.py:82-129 (vb_create_mim, vb_forward_mim)
  * and this header is what the Python host classes (vit_tensorflow_b200/models.py, _lib.py) bind with ctypes.
  * Plain pointers and sizes only; no torch / C++ types cross the boundary.
  *
@@ -50,7 +51,7 @@ enum { VB_KIND_VIT = 0, VB_KIND_DEEPVIT = 1, VB_KIND_CAIT = 2, VB_KIND_CROSSVIT 
        VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6, VB_KIND_CCT = 7, VB_KIND_LEVIT = 8,
        VB_KIND_CVT = 9, VB_KIND_TWINS_SVT = 10, VB_KIND_CROSSFORMER = 11, VB_KIND_NEST = 12, VB_KIND_REGIONVIT = 13,
        VB_KIND_ATS_VIT = 14, VB_KIND_SMALL_DATASET_VIT = 15, VB_KIND_MOBILEVIT = 16,
-       VB_KIND_SCALABLE_VIT = 17, VB_KIND_PIT = 18 };
+       VB_KIND_SCALABLE_VIT = 17, VB_KIND_PIT = 18, VB_KIND_MAE = 19, VB_KIND_SIMMIM = 20 };
 enum { VB_CCT_POS_SINE = 0, VB_CCT_POS_LEARNABLE = 1, VB_CCT_POS_NONE = 2 };   /* cct.py:233-234,250-256 */
 enum { VB_PRECISION_FP32 = 0, VB_PRECISION_BF16 = 1 };
 enum { VB_POOL_CLS = 0, VB_POOL_MEAN = 1 };
@@ -96,7 +97,8 @@ VB_API int vb_abi_version(void);
 
 /* Replaces <Model>.__init__ (vit.py:107-157 etc.): validates the config and allocates device state.  VB_KIND_LEVIT, VB_KIND_CVT,
  * VB_KIND_TWINS_SVT, VB_KIND_CROSSFORMER, VB_KIND_NEST and VB_KIND_REGIONVIT are refused here: their handles come from
- * vb_create_levit, vb_create_cvt, vb_create_twins_svt, vb_create_crossformer, vb_create_nest and vb_create_regionvit. */
+ * vb_create_levit, vb_create_cvt, vb_create_twins_svt, vb_create_crossformer, vb_create_nest and vb_create_regionvit (and the
+ * other extension kinds from their own vb_create_*; VB_KIND_MAE and VB_KIND_SIMMIM from vb_create_mim). */
 VB_API int vb_create(const vb_config* cfg, int device, vb_handle** out);
 
 /* LeViT (levit.py:164-212), appended within ABI 7.  `dims`, `depths` and `heads` hold `stages` entries each (cast_tuple already
@@ -483,6 +485,9 @@ VB_API int32_t vb_last_attention_path(void);
  * RegionViT: the encoders' and the Downsample's unfold is 3 and their convolutions 0; the LayerNorm-folded q|k|v 0; the regional attention and the R2L attention 1 (off the flash kernel
  * the row gathers are 4); the LayerNorm-folded GELU fc1 5; the residual to_out / fc2 6; row statistics, the head's LayerNorm
  * and mean 2; the PEG 4 (the fp32 engine adds its separate LayerNorms to 2).
+ * MAE / SimMIM: the kept-patch gather (patch vectors and position rows) is 3; the patch GEMM 6; the encoder's and decoder's layers
+ * as ViT's (0, 1, 5, 6, 2); enc_to_dec and to_pixels 0 (off the wgmma path 4); the mask kernel, the decoder-input assembly, SimMIM's
+ * mask-token rows, the row gathers, the pred / masked_patches outputs and the loss reductions 4.
  * vb_profile_read synchronises the device and returns accumulated milliseconds, algorithmic FLOPs, algorithmic
  * bytes and launch counts per class (arrays of VB_PROF_NUM); reset != 0 clears the accumulators. */
 #define VB_PROF_NUM 7
@@ -744,6 +749,56 @@ typedef struct vb_pit_config {
  * (floor((h - p) / (p / 2)) + 1) (floor((w - p) / (p / 2)) + 1) patches fit the table (the reference reads its first n + 1
  * rows); the stage entries and vb_forward_distill refuse the handle. */
 VB_API int vb_create_pit(const vb_config* base, const vb_pit_config* pit, int device, vb_handle** out);
+
+/* Masked image modelling (MAE, mae.py:49-92; SimMIM, simmim.py:82-129), appended within ABI 7: inference semantics, the loss value
+ * and what it is computed from.  For an image of n = (h / patch_h) (w / patch_w) patches, num_masked = (int)(masking_ratio * n) in
+ * IEEE double (0.29 * 100 gives 28).
+ *   Noise: u[b, j] = (word 0 of Philox4x32-10 >> 8) * 2^-24, j < n, with the 64-bit seed as key and the counter (j, b, d_lo, d_hi),
+ *   d a 64-bit counter on the device that advances once per forward (graph replays draw fresh masks).  The seed is 0 at creation.
+ *   Order: MAE sorts the ids ascending by (u, j) (the reference's argsort); SimMIM descending by u with ties to the smaller j (its
+ *   top_k).  The first num_masked ids of that permutation are masked.  With 24-bit noise ties occur (about a quarter of the
+ *   calls at n = 196 and batch 256 hold one), so the order is defined exactly.
+ *   MAE: tokens = patch_to_emb(kept patches) + pos_embedding[1 + id] (no cls row); the encoder's transformer over the n -
+ *   num_masked kept rows; enc_to_dec (a Dense, or the identity when dim == decoder_dim) + decoder_pos_emb[id]; the decoder input is
+ *   the num_masked rows mask_token + decoder_pos_emb[masked id] and the kept rows; the decoder (a ViT Transformer of decoder_depth
+ *   layers, decoder_heads heads of decoder_dim_head, mlp 4 decoder_dim, no final norm, to_out dropped when decoder_heads == 1 and
+ *   decoder_dim_head == decoder_dim); pred = to_pixels(the mask rows).  loss = mean(pred^2): the reference's
+ *   tf.reduce_mean(tf.square(pred, masked_patches)) passes masked_patches as tf.square's `name` (mae.py:90).
+ *   SimMIM: tokens = patch_to_emb(patches) + pos_embedding[1 + j], the masked rows replaced by mask_token + pos_embedding[1 + j];
+ *   the encoder's transformer over all n rows; pred = to_pixels(the encoded rows at the masked ids, in top_k order);
+ *   loss = mean(|pred - masked_patches|) / num_masked (simmim.py:128, the extra division is the reference's).
+ * VB_MIM_MAX_PATCHES: the most patches per image the mask kernel sorts (in shared memory). */
+#define VB_MIM_MAX_PATCHES 4096
+typedef struct vb_mim_config {
+  int32_t struct_size;            /* sizeof(vb_mim_config) */
+  double masking_ratio;           /* in (0, 1) */
+  int32_t decoder_dim, decoder_depth, decoder_heads, decoder_dim_head;   /* MAE only */
+} vb_mim_config;
+
+/* MAE.__init__ / SimMIM.__init__: `encoder` supplies the encoder ViT's fields (precision, image / patch sizes, channels, dim, depth,
+ * heads, dim_head, mlp_dim, max_batch); its kind must be VB_KIND_MAE or VB_KIND_SIMMIM, num_classes and pool are ignored.
+ * Weights (SURVEY.md App. B): the encoder's ViT names without cls_token, head_norm.* and head.* -- pos_embedding [1, n_p + 1, dim],
+ * patch.kernel [patch_h patch_w channels, dim] / .bias, layers.L.* -- plus
+ *   MAE:    mask_token [decoder_dim]; enc_to_dec.kernel [dim, decoder_dim] / .bias (only when dim != decoder_dim);
+ *           decoder.layers.L.* (ViT's layer names and shapes at width decoder_dim); decoder_pos_emb.embeddings [n_p + 1, decoder_dim]
+ *           (Embedding(num_patches, decoder_dim) with num_patches = pos_embedding.shape[-2]); to_pixels.kernel [decoder_dim,
+ *           patch_dim] / .bias
+ *   SimMIM: mask_token [dim]; to_pixels.kernel [dim, patch_dim] / .bias
+ * with patch_dim = patch_h patch_w channels and n_p the configured patch count. */
+VB_API int vb_create_mim(const vb_config* encoder, const vb_mim_config* mim, int device, vb_handle** out);
+/* Sets the Philox key of the mask noise and resets the draw counter d to 0 (waits for the device first). */
+VB_API int vb_mim_set_seed(vb_handle* h, uint64_t seed);
+/* One MAE / SimMIM call: img NHWC float32 [batch, img_h, img_w, channels] in img_mem memory; loss: one float; pred and
+ * masked_patches [batch, num_masked, patch_dim] (may be NULL); indices int32 [batch, n], each image's noise permutation with the
+ * masked ids first (may be NULL); all outputs in out_mem memory.  Graph capture and replay follow vb_forward's rules, keyed also by
+ * which of pred / masked_patches are requested.  Refused: sides not divisible by the patch, more than n_p patches or more than
+ * VB_MIM_MAX_PATCHES, and num_masked == 0 (the reference's mean over no rows would be NaN).  An image's masks and pred do not
+ * depend on the rest of the batch; the loss is a fixed-order reduction, so eager, captured and replayed calls give the same bits. */
+VB_API int vb_forward_mim(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, int32_t img_h, int32_t img_w, float* loss,
+                          float* pred, float* masked_patches, int32_t* indices, int32_t out_mem, void* stream);
+/* The mask kernel on its own: indices int32 [B, n] (host) for the Philox key `seed` and draw counter `counter`; descending = 0
+ * MAE's order, 1 SimMIM's.  1 <= n <= VB_MIM_MAX_PATCHES. */
+VB_API int vb_op_mim_mask(int32_t descending, int32_t B, int32_t n, uint64_t seed, uint64_t counter, int32_t* indices);
 
 /* Row softmax of fp32 scores into bf16 probabilities (the T2T attention): p[r, j] = softmax_j(s[r, j] * scale) for j < n,
  * p[r, n..npad) = 0.  s [rows, lds], p [rows, ldp] (uploaded and downloaded whole); n <= npad <= ldp. */

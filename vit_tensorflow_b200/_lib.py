@@ -13,7 +13,7 @@ LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "libvitb200.so")
 
 KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6, "cct": 7, "levit": 8,
         "cvt": 9, "twins_svt": 10, "crossformer": 11, "nest": 12, "regionvit": 13, "ats_vit": 14,
-        "small_dataset_vit": 15, "mobilevit": 16, "scalable_vit": 17, "pit": 18}
+        "small_dataset_vit": 15, "mobilevit": 16, "scalable_vit": 17, "pit": 18, "mae": 19, "simmim": 20}
 PRECISION = {"fp32": 0, "float32": 0, "bf16": 1, "bfloat16": 1}
 MEM_HOST, MEM_DEVICE = 0, 1
 ABI_VERSION = 7                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
@@ -118,6 +118,14 @@ class VbPitConfig(C.Structure):
                 ("heads", C.c_int32 * PIT_MAX_STAGES)]
 
 
+MIM_MAX_PATCHES = 4096                               # VB_MIM_MAX_PATCHES
+
+
+class VbMimConfig(C.Structure):
+    _fields_ = [("struct_size", C.c_int32), ("masking_ratio", C.c_double), ("decoder_dim", C.c_int32), ("decoder_depth", C.c_int32),
+                ("decoder_heads", C.c_int32), ("decoder_dim_head", C.c_int32)]
+
+
 class VbError(RuntimeError):
     pass
 
@@ -150,6 +158,10 @@ SIGNATURES = {
     "vb_op_masked_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, _f32p]),
     "vb_op_spt": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 5 + [C.c_void_p] * 7),
     "vb_op_lsa_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 5 + [C.c_float, C.c_void_p, C.c_int32, C.c_int32, _f32p]),
+    "vb_create_mim": (C.c_int, [C.POINTER(VbConfig), C.POINTER(VbMimConfig), C.c_int, C.POINTER(C.c_void_p)]),
+    "vb_mim_set_seed": (C.c_int, [C.c_void_p, C.c_uint64]),
+    "vb_forward_mim": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 4 + [C.c_int32, C.c_void_p]),
+    "vb_op_mim_mask": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, C.c_void_p]),
     "vb_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, _i64p, C.c_int32]),
     "vb_num_weights": (C.c_int, [C.c_void_p]),
     "vb_weight_info": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), _i64p, C.POINTER(C.c_int32)]),
@@ -520,3 +532,11 @@ def op_patch_merger(x, gamma, beta, queries, precision="bf16", iters=0):
     check(load().vb_op_patch_merger(PRECISION[precision], _ptr(x), _ptr(gamma), _ptr(beta), _ptr(queries), _ptr(out), B, n, D, nt,
                                     iters, C.byref(ms)))
     return out, (ms.value if iters > 0 else None)
+
+
+def op_mim_mask(B, n, seed=0, counter=0, descending=False):
+    """The MAE / SimMIM mask kernel on its own (vb_op_mim_mask): indices int32 [B, n], each image's noise permutation with the
+    masked ids first (descending: SimMIM's top_k order, else MAE's argsort order)."""
+    out = np.zeros((B, n), np.int32)
+    check(load().vb_op_mim_mask(int(bool(descending)), B, n, int(seed) & 0xFFFFFFFFFFFFFFFF, int(counter) & 0xFFFFFFFFFFFFFFFF, _ptr(out)))
+    return out

@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libvitb200.so")
 SOURCES = ["engine.cu", "kernels.cu", "attention.cu", "attn_generic_mma.cu", "attn_flash.cu", "attn_cls.cu", "gemm_wgmma.cu", "ats.cu",
-           "small_vit.cu"]
+           "small_vit.cu", "mim.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr",

@@ -3,6 +3,7 @@
 // counts decides on the device whether a layer samples (C > K, ats_vit.py:213), so the whole forward is one fixed launch
 // sequence that a CUDA graph can replay.  See kernels.cuh for the contracts.
 #include "kernels.cuh"
+#include "philox.cuh"
 
 #include <cmath>
 
@@ -37,19 +38,6 @@ __device__ float ats_block_reduce(float v, float* red) {
   float r = red[0];
   for (int w = 1; w < ATS_WARPS; ++w) r = MAX ? fmaxf(r, red[w]) : r + red[w];
   return r;
-}
-
-// Philox4x32-10 (Salmon et al., SC'11; the Random123 constants)
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
-    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
-    k0 += 0x9E3779B9u;
-    k1 += 0xBB67AE85u;
-  }
-  return c;
 }
 
 __global__ void ats_init_kernel(int* rows, int* C, int* ids, int B, int P) {

@@ -643,6 +643,56 @@ struct vb_handle {
   int layer_heads(int L) const { return cfg.kind == VB_KIND_PIT ? pit.heads[pit_stage(L)] : cfg.heads; }
   // extract_patches(p, stride p / 2, VALID) positions along a side of n pixels (pit.py:16-17,184 for n >= p)
   int pit_side(int n) const { return (n - cfg.patch_h) / (cfg.patch_h / 2) + 1; }
+  // MAE / SimMIM (mae.py:49-92, simmim.py:82-129): the encoder ViT's embedding and `layers`; MAE's enc_to_dec (a Dense when
+  // dim != decoder_dim), decoder layers and decoder_pos_emb table; both kinds' mask_token and to_pixels.  The mask noise's Philox
+  // key, draw counter and the mask kernel's completion counter live in mim_rng; mim_dev holds the permutation [B, n] and the
+  // pred / masked_patches outputs [B, num_masked, patch_dim] at stable addresses (a new allocation drops the captured graphs).
+  vb_mim_config mim{};
+  std::vector<LayerW> dec_layers;
+  Linear enc_to_dec, to_pixels;
+  bool enc_to_dec_dense = false;
+  const float* mask_token = nullptr;
+  const float* dec_pos = nullptr;
+  DevMem mim_dev, mim_rng;
+  struct MimPlan { int B = 0, n = 0, nm = 0; size_t pred = 0, patches = 0; };
+  MimPlan mim_last;
+  bool is_mim() const { return cfg.kind == VB_KIND_MAE || cfg.kind == VB_KIND_SIMMIM; }
+  int mim_dim() const { return cfg.kind == VB_KIND_MAE ? mim.decoder_dim : cfg.dim; }    // width of the rows to_pixels reads
+  int patch_dim() const { return cfg.patch_h * cfg.patch_w * cfg.channels; }
+  unsigned long long* mim_rng_ptr() {
+    if (mim_rng.p == nullptr) {
+      mim_rng.ensure(3 * sizeof(unsigned long long));
+      VB_CUDA(cudaMemset(mim_rng.p, 0, 3 * sizeof(unsigned long long)));
+      VB_CUDA(cudaDeviceSynchronize());                // before any forward reads it, on whatever stream that runs
+    }
+    return static_cast<unsigned long long*>(mim_rng.p);
+  }
+  // the host side of a MAE / SimMIM call of a batch of h x w images, before the launches or graph lookup: the shape checks,
+  // num_masked = int(masking_ratio * n) in double (mae.py:57, simmim.py:106) and the output buffers
+  void mim_prepare(int B, int H, int Wd) {
+    VB_CHECK(H % cfg.patch_h == 0 && Wd % cfg.patch_w == 0, "Image dimensions must be divisible by the patch size.");
+    const long long n = static_cast<long long>(H / cfg.patch_h) * (Wd / cfg.patch_w);
+    VB_CHECK(n + 1 <= embed.n_pos, "MAE / SimMIM: the image has " + std::to_string(n) + " patches but pos_embedding has rows for " +
+                                       std::to_string(embed.n_pos - 1));
+    VB_CHECK(n <= MIM_MAX_PATCHES, "MAE / SimMIM: the image has " + std::to_string(n) + " patches; the mask kernel takes at most " +
+                                       std::to_string(MIM_MAX_PATCHES) + " per image");
+    const int nm = static_cast<int>(mim.masking_ratio * static_cast<double>(n));
+    VB_CHECK(nm >= 1, "MAE / SimMIM: num_masked = int(masking_ratio * " + std::to_string(n) + ") is 0: the loss would be a mean over no "
+                      "patches (NaN in the reference)");
+    MimPlan p;
+    p.B = B; p.n = static_cast<int>(n); p.nm = nm;
+    const size_t out = static_cast<size_t>(B) * nm * patch_dim();
+    p.pred = round_up(B * p.n, 64);
+    p.patches = p.pred + out;
+    mim_last = p;
+    const void* before = mim_dev.p;
+    mim_dev.ensure((p.patches + out) * sizeof(float));
+    if (before != nullptr && mim_dev.p != before) drop_graphs();
+    mim_rng_ptr();
+  }
+  int* mim_idx() const { return static_cast<int*>(mim_dev.p); }
+  float* mim_pred() const { return static_cast<float*>(mim_dev.p) + mim_last.pred; }
+  float* mim_patches() const { return static_cast<float*>(mim_dev.p) + mim_last.patches; }
   Norm head_norm, sm_head_norm, lg_head_norm;
   Linear head, sm_head, lg_head;
   Norm spt_norm;                     // SPT's LayerNorm over the p^2 * 5 C patch vector (bf16: padded to the GEMM's K, folded into it)
@@ -663,7 +713,10 @@ struct vb_handle {
   // stream (which cannot be captured) always run eagerly.
   struct GraphKey {
     const void* img; void* out; int B, H, W; cudaStream_t s;
-    bool operator<(const GraphKey& o) const { return std::tie(img, out, B, H, W, s) < std::tie(o.img, o.out, o.B, o.H, o.W, o.s); }
+    int flags = 0;                                       // vb_forward_mim: which optional outputs the launches write
+    bool operator<(const GraphKey& o) const {
+      return std::tie(img, out, B, H, W, s, flags) < std::tie(o.img, o.out, o.B, o.H, o.W, o.s, o.flags);
+    }
   };
   struct GraphEntry { cudaGraphExec_t exec = nullptr; int calls = 0; long long launches = 0; bool failed = false; };
   std::map<GraphKey, GraphEntry> graphs;
@@ -732,6 +785,20 @@ struct vb_handle {
       }
       expect_ln("head_norm", c.dim);
       expect_dense("head", c.dim, c.num_classes);
+    } else if (c.kind == VB_KIND_MAE || c.kind == VB_KIND_SIMMIM) {   // the encoder ViT without cls_token / mlp_head (mae.py:33-47)
+      const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w), pd = patch_dim();
+      expect("pos_embedding", {1, np + 1, c.dim});
+      expect_dense("patch", pd, c.dim);
+      for (int L = 0; L < c.depth; ++L) expect_layer("layers." + std::to_string(L) + ".", c.dim, c.heads, c.dim_head, c.mlp_dim, VB_KIND_VIT);
+      const int Dd = mim_dim();
+      expect("mask_token", {Dd});
+      if (c.kind == VB_KIND_MAE) {
+        if (c.dim != Dd) expect_dense("enc_to_dec", c.dim, Dd);                        // mae.py:42
+        for (int L = 0; L < mim.decoder_depth; ++L)                                    // vit.Transformer (mae.py:44)
+          expect_layer("decoder.layers." + std::to_string(L) + ".", Dd, mim.decoder_heads, mim.decoder_dim_head, 4 * Dd, VB_KIND_VIT);
+        expect("decoder_pos_emb.embeddings", {np + 1, Dd});                            // Embedding(num_patches, decoder_dim) :45
+      }
+      expect_dense("to_pixels", Dd, pd);                                               // mae.py:46, simmim.py:86
     } else if (c.kind == VB_KIND_SMALL_DATASET_VIT) {                   // vit_for_small_dataset.py:142-195
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w), K = c.patch_h * c.patch_w * 5 * C;
       expect("pos_embedding", {1, np + 1, c.dim});
@@ -1285,7 +1352,7 @@ struct vb_handle {
     VB_CUDA(cudaSetDevice(device));
     owned.clear(); layers.clear(); cls_layers.clear(); t2t_layers.clear(); xblocks.clear(); plans.clear(); embed_res.clear(); cct_convs.clear();
     lv_stem.clear(); lv_blocks.clear(); cvt_stages.clear(); twins_stages.clear(); cf_stages.clear(); nest_levels.clear(); rv_stages.clear();
-    mv_mv2.clear(); mv_vit.clear(); sv_stages.clear();
+    mv_mv2.clear(); mv_vit.clear(); sv_stages.clear(); dec_layers.clear();
     woverride.clear();
     drop_graphs();
     const vb_config& c = cfg;
@@ -1304,6 +1371,19 @@ struct vb_handle {
       }
       head_norm = make_norm("head_norm", c.dim);
       head = make_linear_f32("head", c.dim, c.num_classes);
+    } else if (c.kind == VB_KIND_MAE || c.kind == VB_KIND_SIMMIM) {
+      const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w), Dd = mim_dim();
+      embed = make_embed("", c.patch_h, c.patch_w, c.dim, np + 1, false);
+      for (int L = 0; L < c.depth; ++L) layers.push_back(make_layer("layers." + std::to_string(L) + ".", c.dim, c.heads, c.dim_head, c.mlp_dim, VB_KIND_VIT));
+      mask_token = W("mask_token");
+      if (c.kind == VB_KIND_MAE) {
+        enc_to_dec_dense = has("enc_to_dec.kernel");
+        if (enc_to_dec_dense) enc_to_dec = make_linear("enc_to_dec", c.dim, Dd);
+        for (int L = 0; L < mim.decoder_depth; ++L)
+          dec_layers.push_back(make_layer("decoder.layers." + std::to_string(L) + ".", Dd, mim.decoder_heads, mim.decoder_dim_head, 4 * Dd, VB_KIND_VIT));
+        dec_pos = W("decoder_pos_emb.embeddings");
+      }
+      to_pixels = make_linear("to_pixels", Dd, patch_dim());
     } else if (c.kind == VB_KIND_SMALL_DATASET_VIT) {
       finalize_small_dataset_vit();
     } else if (c.kind == VB_KIND_PATCH_MERGER_VIT) {
@@ -3518,6 +3598,98 @@ struct vb_handle {
     { ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * rows * HD, s); r2l_rows<T>(ow, HD, out, ldo, HD, win, reg_row0, false, s); }
   }
 
+  // MAE.call (mae.py:49-92) and SimMIM.call (simmim.py:82-129) as mim_prepare planned them, writing the loss to `loss` (device)
+  // and, per `flags` (1: pred, 2: masked_patches), the outputs to mim_pred() / mim_patches().  The masks come from the device's
+  // own noise counter; every step after them is a fixed launch sequence.
+  template <typename T>
+  void mim_forward(const float* img, int B, int H, int Wd, float* loss, int flags, cudaStream_t s) {
+    const vb_config& c = cfg;
+    const MimPlan& p = mim_last;
+    VB_CHECK(p.B == B && p.n == (H / c.patch_h) * (Wd / c.patch_w) && mim_dev.p != nullptr, "internal: MIM state not prepared for this batch");
+    arena.reset();
+    const bool mae = c.kind == VB_KIND_MAE;
+    const int n = p.n, nm = p.nm, nk = n - nm, dim = c.dim, pd = patch_dim(), Dd = mim_dim();
+    int* idx = mim_idx();
+    {
+      ProfScope ps(this, PROF_OTHER, 0.0, 4.0 * B * n, s);
+      mim_mask(B, n, mae ? 0 : 1, mim_rng_ptr(), idx, s);
+    }
+    // the patch embedding of the kept rows (MAE: per row the reference's embed-then-gather) or of all rows (SimMIM)
+    const int rows = mae ? nk : n, M = B * rows, Kp = bf16() ? embed.patch.ldw : embed.patch.K;
+    T* col = arena.get<T>(static_cast<size_t>(M) * Kp);
+    T* R = arena.get<T>(static_cast<size_t>(M) * dim);
+    {
+      ProfScope ps(this, PROF_EMBED, 0.0, 4.0 * M * pd + static_cast<double>(sizeof(T)) * M * (Kp + dim), s);
+      mim_patch_rows<T>(img, B, H, Wd, c.channels, c.patch_h, c.patch_w, mae ? idx : nullptr, n, nm, rows, col, Kp, embed.pos, R, dim, s);
+    }
+    T* X = arena.get<T>(static_cast<size_t>(M) * dim);
+    float* stats = nullptr;
+    {
+      Epi ep; ep.bias = embed.patch.bias; ep.res = R; ep.ldr = dim;
+      if (mae && bf16() && dim % 64 == 0) { stats = row_stats(M, dim); ep.stats_out = stats; }
+      Linear L = embed.patch;
+      L.K = Kp;
+      linear<T>(col, Kp, M, L, X, dim, ep, s);
+    }
+    if (!mae) {
+      ProfScope ps(this, PROF_OTHER, 0.0, static_cast<double>(sizeof(T)) * B * nm * dim, s);
+      mim_mask_tokens<T>(X, idx, B, n, nm, mask_token, embed.pos, dim, s);
+      stats = dim % 64 == 0 ? row_stats(M, dim) : nullptr;   // recomputed by the first layer: the mask rows replaced the GEMM's
+    }
+    bool sv = mae && stats != nullptr;
+    for (const auto& l : layers) layer_self<T>(X, B, rows, dim, l, s, stats, &sv);
+    const T* Xp = X;                                            // the rows to_pixels reads, nm per image
+    if (mae) {
+      const T* E = X;
+      if (enc_to_dec_dense) {
+        T* Ed = arena.get<T>(static_cast<size_t>(M) * Dd);
+        Epi e; e.bias = enc_to_dec.bias;
+        linear<T>(X, dim, M, enc_to_dec, Ed, Dd, e, s);
+        E = Ed;
+      }
+      T* Z = arena.get<T>(static_cast<size_t>(B) * n * Dd);
+      {
+        ProfScope ps(this, PROF_OTHER, 0.0, static_cast<double>(sizeof(T)) * B * (nk + n) * Dd + 4.0 * B * n * Dd, s);
+        mim_decoder_rows<T>(E, idx, B, n, nm, mask_token, dec_pos, Z, Dd, s);
+      }
+      float* dstats = Dd % 64 == 0 ? row_stats(static_cast<long long>(B) * n, Dd) : nullptr;
+      bool dsv = false;
+      for (const auto& l : dec_layers) layer_self<T>(Z, B, n, Dd, l, s, dstats, &dsv);
+      T* Zm = arena.get<T>(static_cast<size_t>(B) * nm * Dd);
+      {
+        ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * B * nm * Dd, s);
+        mim_take_rows<T>(Z, n, nullptr, Zm, B, nm, Dd, s);   // the mask rows: first in every image (mae.py:84)
+      }
+      Xp = Zm;
+    } else {
+      T* Xm = arena.get<T>(static_cast<size_t>(B) * nm * dim);
+      {
+        ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * B * nm * dim, s);
+        mim_take_rows<T>(X, n, idx, Xm, B, nm, dim, s);      // simmim.py:119: the encoded rows at the masked ids, top_k order
+      }
+      Xp = Xm;
+    }
+    const long long Mp = static_cast<long long>(B) * nm;
+    T* P = arena.get<T>(static_cast<size_t>(Mp) * pd);
+    {
+      Epi e; e.bias = to_pixels.bias;
+      linear<T>(Xp, Dd, static_cast<int>(Mp), to_pixels, P, pd, e, s);
+    }
+    double* partial = arena.get<double>(static_cast<size_t>(mim_loss_blocks(Mp)));
+    {
+      ProfScope ps(this, PROF_OTHER, 3.0 * Mp * pd, static_cast<double>(sizeof(T)) * Mp * pd + (mae ? 0.0 : 4.0 * Mp * pd), s);
+      mim_loss<T>(P, pd, B, nm, mae ? nullptr : img, H, Wd, c.channels, c.patch_h, c.patch_w, idx, n, partial, loss, s);
+    }
+    if (flags & 1) {
+      ProfScope ps(this, PROF_OTHER, 0.0, (static_cast<double>(sizeof(T)) + 4.0) * Mp * pd, s);
+      to_f32<T>(P, mim_pred(), Mp * pd, s);
+    }
+    if (flags & 2) {
+      ProfScope ps(this, PROF_OTHER, 0.0, 8.0 * Mp * pd, s);
+      mim_patch_rows<float>(img, B, H, Wd, c.channels, c.patch_h, c.patch_w, idx, n, 0, nm, mim_patches(), pd, nullptr, nullptr, 0, s);
+    }
+  }
+
   // DistillMixin.call (distill.py:16-45) on top of a ViT or a T2TViT: embed (the patch Dense, or T2T's soft splits and their
   // one-layer transformers, as vb_forward runs them) -> append the distillation token as the LAST row -> transformer over
   // n + 2 rows -> head on the first n + 1 rows, and the last row returned as is.
@@ -3586,6 +3758,8 @@ struct vb_handle {
       case VB_KIND_MOBILEVIT: return "MobileViT runs as a whole forward only: its stem / trunk / head steps have no entry of their own";
       case VB_KIND_SCALABLE_VIT: return "ScalableViT runs as a whole forward only: its patch-embedding / stage / head steps have no entry of their own";
       case VB_KIND_PIT: return "PiT runs as a whole forward only: it has no `transformer` attribute, so its patch-embedding / stage / head steps have no entry of their own";
+      case VB_KIND_MAE: return "MAE runs through vb_forward_mim only: its encoder and decoder steps have no entry of their own";
+      case VB_KIND_SIMMIM: return "SimMIM runs through vb_forward_mim only: its encoder steps have no entry of their own";
       default: return nullptr;
     }
   }
@@ -3823,6 +3997,8 @@ void validate(const vb_config& c) {
   VB_CHECK(c.kind != VB_KIND_MOBILEVIT, "MobileViT: create the handle with vb_create_mobilevit (its blocks are a vb_mobilevit_config)");
   VB_CHECK(c.kind != VB_KIND_SCALABLE_VIT, "ScalableViT: create the handle with vb_create_scalable_vit (its stages are a vb_scalable_vit_config)");
   VB_CHECK(c.kind != VB_KIND_PIT, "PiT: create the handle with vb_create_pit (its stages' depths and heads are a vb_pit_config)");
+  VB_CHECK(c.kind != VB_KIND_MAE, "MAE: create the handle with vb_create_mim (its masking ratio and decoder are a vb_mim_config)");
+  VB_CHECK(c.kind != VB_KIND_SIMMIM, "SimMIM: create the handle with vb_create_mim (its masking ratio is a vb_mim_config)");
   VB_CHECK((c.kind >= VB_KIND_VIT && c.kind <= VB_KIND_CCT) || c.kind == VB_KIND_SMALL_DATASET_VIT, "unknown model kind");
   if (c.kind == VB_KIND_SMALL_DATASET_VIT) {
     // SPT's Rearrange takes one patch size for both sides (vit_for_small_dataset.py:147) and shift() one image of 3 channels
@@ -3948,6 +4124,20 @@ void validate_pit(const vb_config& c, const vb_pit_config& p) {
     v.depth += p.depth[s];
   }
   validate(v);
+}
+
+// mae.py:28 / simmim.py:74 (the reference's assert message) and the decoder's Transformer on top of ViT's checks of the encoder
+void validate_mim(const vb_config& c, const vb_mim_config& m) {
+  vb_config v = c;
+  v.kind = VB_KIND_VIT;
+  v.pool = VB_POOL_CLS;
+  v.num_classes = 1;                                     // the encoder's mlp_head is not part of the model
+  validate(v);
+  VB_CHECK(m.masking_ratio > 0.0 && m.masking_ratio < 1.0, "masking ratio must be kept between 0 and 1");
+  if (c.kind == VB_KIND_MAE) {
+    VB_CHECK(m.decoder_dim > 0 && m.decoder_depth >= 0 && m.decoder_heads > 0 && m.decoder_dim_head > 0, "MAE: bad decoder dimensions");
+    VB_CHECK(m.decoder_heads <= 32, "MAE: at most 32 decoder heads");
+  }
 }
 
 void validate_regionvit(const vb_config& c, const vb_regionvit_config& r) {
@@ -4157,6 +4347,58 @@ int create_with(const char* fn, const char* ext_name, int kind, const char* kind
     *out = h.release();
   });
 }
+// The whole-forward CUDA graph of vb_forward / vb_forward_mim (see vb_handle::graphs): the key's second call on a capturable stream
+// is captured and launched, later calls replay it; otherwise, and when the capture fails, run_eager runs the launches directly.
+template <typename F>
+void run_graphed(vb_handle* h, const vb_handle::GraphKey& key, F&& run_eager) {
+  cudaStream_t s = key.s;
+  static const bool graphs_off = getenv("VB_NO_GRAPH") != nullptr;
+  const bool graphable = !graphs_off && !h->profiling && s != nullptr && s != cudaStreamLegacy;
+  bool done = false;
+  if (graphable) {
+    if (h->graphs.size() > 64) h->drop_graphs();                         // shape / pointer sweeps: bounded
+    vb_handle::GraphEntry& ge = h->graphs[key];
+    ++ge.calls;
+    if (ge.exec != nullptr) {
+      VB_CUDA(cudaGraphLaunch(ge.exec, s));
+      count_launch(static_cast<int>(ge.launches));
+      ++h->graph_replays;
+      done = true;
+    } else if (ge.calls == 2 && !ge.failed) {
+      cudaGraph_t graph = nullptr;
+      const long long l0 = launch_counter();
+      std::string why;
+      const cudaError_t eb = cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal);
+      if (eb == cudaSuccess) {
+        bool ok = true;
+        try { run_eager(); } catch (const std::exception& e) { ok = false; why = e.what(); }
+        const cudaError_t ec = cudaStreamEndCapture(s, &graph);
+        cudaError_t ei = cudaSuccess;
+        if (ok && ec == cudaSuccess && graph != nullptr && (ei = cudaGraphInstantiate(&ge.exec, graph, 0)) == cudaSuccess) {
+          ge.launches = launch_counter() - l0;
+          VB_CUDA(cudaGraphLaunch(ge.exec, s));
+          ++h->graph_captures;
+          done = true;
+        } else {
+          if (ok) why = std::string(ec != cudaSuccess ? "cudaStreamEndCapture: " : "cudaGraphInstantiate: ") +
+                        cudaGetErrorString(ec != cudaSuccess ? ec : ei);
+          ge.exec = nullptr;
+        }
+        if (graph != nullptr) cudaGraphDestroy(graph);
+      } else {
+        why = std::string("cudaStreamBeginCapture: ") + cudaGetErrorString(eb);
+      }
+      if (!done) {                                                        // stay eager for this key
+        ge.failed = true;
+        ++h->graph_failures;
+        h->graph_last_failure = why;
+        cudaGetLastError();
+      }
+    }
+  }
+  if (!done) run_eager();
+}
+
 }  // namespace
 
 extern "C" {
@@ -4420,6 +4662,91 @@ int vb_create_pit(const vb_config* base, const vb_pit_config* pc, int device, vb
   });
 }
 
+int vb_create_mim(const vb_config* encoder, const vb_mim_config* mc, int device, vb_handle** out) {
+  const int rc = guarded(nullptr, [&] {
+    VB_CHECK(encoder != nullptr && mc != nullptr && out != nullptr, "vb_create_mim: null argument");
+    VB_CHECK(encoder->kind == VB_KIND_MAE || encoder->kind == VB_KIND_SIMMIM, "vb_create_mim: encoder.kind must be VB_KIND_MAE or VB_KIND_SIMMIM");
+  });
+  if (rc != 0) return rc;
+  return create_with("vb_create_mim", "vb_mim_config", encoder->kind, encoder->kind == VB_KIND_MAE ? "VB_KIND_MAE" : "VB_KIND_SIMMIM", encoder,
+                     mc, device, out, validate_mim, [&](vb_handle& h) { h.mim = *mc; h.cfg.pool = VB_POOL_CLS; });
+}
+
+int vb_mim_set_seed(vb_handle* h, uint64_t seed) {
+  return guarded(h, [&] {
+    VB_CHECK(h != nullptr, "null handle");
+    VB_CHECK(h->is_mim(), "vb_mim_set_seed: not a MAE / SimMIM handle");
+    VB_CUDA(cudaSetDevice(h->device));
+    VB_CUDA(cudaDeviceSynchronize());                  // no forward in flight reads the old key and counter
+    const unsigned long long v[3] = {static_cast<unsigned long long>(seed), 0ull, 0ull};
+    VB_CUDA(cudaMemcpy(h->mim_rng_ptr(), v, sizeof v, cudaMemcpyHostToDevice));
+    VB_CUDA(cudaDeviceSynchronize());                  // a pageable copy may return before it lands
+  });
+}
+
+int vb_forward_mim(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, int32_t img_h, int32_t img_w, float* loss, float* pred,
+                   float* masked_patches, int32_t* indices, int32_t out_mem, void* stream) {
+  return guarded(h, [&] {
+    VB_CHECK(h != nullptr && img != nullptr && loss != nullptr, "vb_forward_mim: null argument");
+    VB_CHECK(h->is_mim(), "vb_forward_mim: not a MAE / SimMIM handle");
+    VB_CHECK(h->finalized, "vb_forward_mim: call vb_finalize after setting the weights");
+    VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_forward_mim: bad batch / image size");
+    VB_CUDA(cudaSetDevice(h->device));
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const long long before = launch_counter();
+    const size_t img_bytes = static_cast<size_t>(batch) * img_h * img_w * h->cfg.channels * sizeof(float);
+    const float* img_d = img;
+    if (img_mem == VB_MEM_HOST) {
+      h->img_dev.ensure(img_bytes);
+      VB_CUDA(cudaMemcpyAsync(h->img_dev.p, img, img_bytes, cudaMemcpyHostToDevice, s));
+      img_d = static_cast<const float*>(h->img_dev.p);
+    }
+    float* loss_d = loss;
+    if (out_mem == VB_MEM_HOST) {
+      h->logits_dev.ensure(sizeof(float));
+      loss_d = static_cast<float*>(h->logits_dev.p);
+    }
+    h->mim_prepare(batch, img_h, img_w);
+    const int flags = (pred != nullptr ? 1 : 0) | (masked_patches != nullptr ? 2 : 0);
+    vb_handle::GraphKey key{img_d, loss_d, batch, img_h, img_w, s};
+    key.flags = flags;
+    run_graphed(h, key, [&] {
+      if (h->bf16()) h->mim_forward<__nv_bfloat16>(img_d, batch, img_h, img_w, loss_d, flags, s);
+      else h->mim_forward<float>(img_d, batch, img_h, img_w, loss_d, flags, s);
+    });
+    h->last_launches = launch_counter() - before;
+    const vb_handle::MimPlan& p = h->mim_last;
+    const size_t out_bytes = static_cast<size_t>(batch) * p.nm * h->patch_dim() * sizeof(float);
+    const cudaMemcpyKind kind = out_mem == VB_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+    if (pred != nullptr) VB_CUDA(cudaMemcpyAsync(pred, h->mim_pred(), out_bytes, kind, s));
+    if (masked_patches != nullptr) VB_CUDA(cudaMemcpyAsync(masked_patches, h->mim_patches(), out_bytes, kind, s));
+    if (indices != nullptr) VB_CUDA(cudaMemcpyAsync(indices, h->mim_idx(), static_cast<size_t>(batch) * p.n * sizeof(int), kind, s));
+    if (out_mem == VB_MEM_HOST) {
+      VB_CUDA(cudaMemcpyAsync(loss, loss_d, sizeof(float), cudaMemcpyDeviceToHost, s));
+      VB_CUDA(cudaStreamSynchronize(s));
+    }
+  });
+}
+
+int vb_op_mim_mask(int32_t descending, int32_t B, int32_t n, uint64_t seed, uint64_t counter, int32_t* indices) {
+  return guarded(nullptr, [&] {
+    VB_CHECK(indices != nullptr && B > 0 && (descending == 0 || descending == 1), "vb_op_mim_mask: bad arguments");
+    VB_CHECK(n >= 1 && n <= MIM_MAX_PATCHES, "vb_op_mim_mask: n = " + std::to_string(n) + " is outside 1 .. " + std::to_string(MIM_MAX_PATCHES) +
+                                                 " (the patches per image the mask kernel sorts)");
+    require_gpu();
+    DevMem rng, idx;
+    rng.ensure(3 * sizeof(unsigned long long));
+    const unsigned long long v[3] = {static_cast<unsigned long long>(seed), static_cast<unsigned long long>(counter), 0ull};
+    VB_CUDA(cudaMemcpy(rng.p, v, sizeof v, cudaMemcpyHostToDevice));
+    idx.ensure(static_cast<size_t>(B) * n * sizeof(int));
+    mim_mask(B, n, descending, static_cast<unsigned long long*>(rng.p), static_cast<int*>(idx.p), 0);
+    VB_CUDA(cudaMemcpy(indices, idx.p, static_cast<size_t>(B) * n * sizeof(int), cudaMemcpyDeviceToHost));
+    unsigned long long after[3];
+    VB_CUDA(cudaMemcpy(after, rng.p, sizeof after, cudaMemcpyDeviceToHost));
+    VB_CHECK(after[1] == counter + 1 && after[2] == 0, "vb_op_mim_mask: the mask kernel did not advance its counter once");
+  });
+}
+
 int vb_create_regionvit(const vb_config* base, const vb_regionvit_config* rc, int device, vb_handle** out) {
   return create_with("vb_create_regionvit", "vb_regionvit_config", VB_KIND_REGIONVIT, "VB_KIND_REGIONVIT", base, rc,
                                           device, out, validate_regionvit,
@@ -4469,6 +4796,7 @@ int vb_forward(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, i
   return guarded(h, [&] {
     VB_CHECK(h != nullptr && img != nullptr && logits != nullptr, "vb_forward: null argument");
     VB_CHECK(h->finalized, "vb_forward: call vb_finalize after setting the weights");
+    VB_CHECK(!h->is_mim(), h->whole_forward_only(h->cfg.kind));
     VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_forward: bad batch / image size");
     VB_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -4487,55 +4815,10 @@ int vb_forward(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, i
       out_d = static_cast<float*>(h->logits_dev.p);
     }
     if (h->cfg.kind == VB_KIND_ATS_VIT) h->ats_prepare(batch, img_h, img_w);
-    auto run_eager = [&] {
+    run_graphed(h, vb_handle::GraphKey{img_d, out_d, batch, img_h, img_w, s}, [&] {
       if (h->bf16()) h->forward_impl<__nv_bfloat16>(img_d, batch, img_h, img_w, out_d, s);
       else h->forward_impl<float>(img_d, batch, img_h, img_w, out_d, s);
-    };
-    static const bool graphs_off = getenv("VB_NO_GRAPH") != nullptr;
-    const bool graphable = !graphs_off && !h->profiling && s != nullptr && s != cudaStreamLegacy;
-    bool done = false;
-    if (graphable) {
-      if (h->graphs.size() > 64) h->drop_graphs();                         // shape / pointer sweeps: bounded
-      vb_handle::GraphEntry& ge = h->graphs[vb_handle::GraphKey{img_d, out_d, batch, img_h, img_w, s}];
-      ++ge.calls;
-      if (ge.exec != nullptr) {
-        VB_CUDA(cudaGraphLaunch(ge.exec, s));
-        count_launch(static_cast<int>(ge.launches));
-        ++h->graph_replays;
-        done = true;
-      } else if (ge.calls == 2 && !ge.failed) {
-        cudaGraph_t graph = nullptr;
-        const long long l0 = launch_counter();
-        std::string why;
-        const cudaError_t eb = cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal);
-        if (eb == cudaSuccess) {
-          bool ok = true;
-          try { run_eager(); } catch (const std::exception& e) { ok = false; why = e.what(); }
-          const cudaError_t ec = cudaStreamEndCapture(s, &graph);
-          cudaError_t ei = cudaSuccess;
-          if (ok && ec == cudaSuccess && graph != nullptr && (ei = cudaGraphInstantiate(&ge.exec, graph, 0)) == cudaSuccess) {
-            ge.launches = launch_counter() - l0;
-            VB_CUDA(cudaGraphLaunch(ge.exec, s));
-            ++h->graph_captures;
-            done = true;
-          } else {
-            if (ok) why = std::string(ec != cudaSuccess ? "cudaStreamEndCapture: " : "cudaGraphInstantiate: ") +
-                          cudaGetErrorString(ec != cudaSuccess ? ec : ei);
-            ge.exec = nullptr;
-          }
-          if (graph != nullptr) cudaGraphDestroy(graph);
-        } else {
-          why = std::string("cudaStreamBeginCapture: ") + cudaGetErrorString(eb);
-        }
-        if (!done) {                                                        // stay eager for this key
-          ge.failed = true;
-          ++h->graph_failures;
-          h->graph_last_failure = why;
-          cudaGetLastError();
-        }
-      }
-    }
-    if (!done) run_eager();
+    });
     h->last_launches = launch_counter() - before;
     if (logits_mem == VB_MEM_HOST) {
       VB_CUDA(cudaMemcpyAsync(logits, out_d, out_bytes, cudaMemcpyDeviceToHost, s));
@@ -4560,6 +4843,7 @@ int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, int32_t 
     VB_CHECK(h->cfg.kind != VB_KIND_MOBILEVIT, h->whole_forward_only(VB_KIND_MOBILEVIT));
     VB_CHECK(h->cfg.kind != VB_KIND_SCALABLE_VIT, h->whole_forward_only(VB_KIND_SCALABLE_VIT));
     VB_CHECK(h->cfg.kind != VB_KIND_PIT, h->whole_forward_only(VB_KIND_PIT));
+    VB_CHECK(!h->is_mim(), h->whole_forward_only(h->cfg.kind));
     const bool levit = h->cfg.kind == VB_KIND_LEVIT;
     VB_CHECK(levit || distill_token != nullptr, "vb_forward_distill: null argument");
     VB_CHECK(!levit || (distill_token == nullptr && h->lv.num_distill_classes > 0),
@@ -4688,6 +4972,7 @@ int vb_to_patch(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, 
     VB_CHECK(h->cfg.kind != VB_KIND_MOBILEVIT, h->whole_forward_only(VB_KIND_MOBILEVIT));
     VB_CHECK(h->cfg.kind != VB_KIND_SCALABLE_VIT, h->whole_forward_only(VB_KIND_SCALABLE_VIT));
     VB_CHECK(h->cfg.kind != VB_KIND_PIT, h->whole_forward_only(VB_KIND_PIT));
+    VB_CHECK(!h->is_mim(), h->whole_forward_only(h->cfg.kind));
     VB_CHECK(h->cfg.kind != VB_KIND_CROSSVIT && h->cfg.kind != VB_KIND_T2T_VIT && h->cfg.kind != VB_KIND_CCT &&
              h->cfg.kind != VB_KIND_LEVIT && h->cfg.kind != VB_KIND_CVT && h->cfg.kind != VB_KIND_TWINS_SVT &&
              h->cfg.kind != VB_KIND_CROSSFORMER && h->cfg.kind != VB_KIND_NEST && h->cfg.kind != VB_KIND_REGIONVIT,

@@ -218,6 +218,36 @@ void attn_softmax_masked(float* S, long long rows, int nk, long long rows_per_im
 template <typename T>
 void spt_rows(const float* img, T* out, int B, int H, int W, int C, int p, int ldo, cudaStream_t s);
 
+// ---- masked image modelling (MAE, mae.py:49-92; SimMIM, simmim.py:82-129; mim.cu).  idx [B, n] holds each image's noise
+// permutation, the masked patch ids first: MAE's argsort of u ascending (ties to the smaller id), SimMIM's top_k order (u
+// descending, ties to the smaller id).
+constexpr int MIM_MAX_PATCHES = 4096;    // patches per image the mask kernel sorts in shared memory
+// One CTA per image: u[b, j] = (Philox4x32-10 word 0 >> 8) * 2^-24, key rng[0], counter (j, b, rng[1] low, rng[1] high), sorted
+// into idx (descending != 0: SimMIM's order).  rng[1] advances by one per launch; rng[2] is the kernel's CTA-completion counter (0
+// between launches).
+void mim_mask(int B, int n, int descending, unsigned long long* rng, int* idx, cudaStream_t s);
+// out [B * count, ldo]: row b * count + i = the (p1, p2, c) patch vector of id j = idx[b * n + off + i] (idx null: j = i) read from
+// the NHWC image, columns [ph pw C, ldo) zero; R (may be null) [B * count, dim]: pos[1 + j] (pos_embedding [np + 1, dim]).
+template <typename T>
+void mim_patch_rows(const float* img, int B, int H, int W, int C, int ph, int pw, const int* idx, int n, int off, int count, T* out, int ldo,
+                    const float* pos, T* R, int dim, cudaStream_t s);
+// Z [B * n, D]: image b's row t < nm = mask_token + dpe[idx[b, t]], row t >= nm = E[b (n - nm) + t - nm] + dpe[idx[b, t]]
+template <typename T>
+void mim_decoder_rows(const T* E, const int* idx, int B, int n, int nm, const float* mask_token, const float* dpe, T* Z, int D, cudaStream_t s);
+// X [B * n, D]: image b's rows idx[b, i], i < nm, replaced by mask_token + pos[1 + idx[b, i]]
+template <typename T>
+void mim_mask_tokens(T* X, const int* idx, int B, int n, int nm, const float* mask_token, const float* pos, int D, cudaStream_t s);
+// out [B * count, D]: row b * count + i = X row b * n + (idx ? idx[b * n + i] : i)
+template <typename T>
+void mim_take_rows(const T* X, int n, const int* idx, T* out, int B, int count, int D, cudaStream_t s);
+// *loss = mean(pred^2) over pred [B * nm, pd] (img null: MAE), or mean(|pred - masked patch|) / nm with the patch of row b nm + i
+// read from the image at id idx[b * n + i] (SimMIM).  Two fixed-order passes in double, no atomics: partial holds
+// mim_loss_blocks(B * nm) doubles.
+int mim_loss_blocks(long long rows);
+template <typename T>
+void mim_loss(const T* pred, int pd, int B, int nm, const float* img, int H, int W, int C, int ph, int pw, const int* idx, int n,
+              double* partial, float* loss, cudaStream_t s);
+
 long long launch_counter();      // number of kernel launches issued through these wrappers (process-wide)
 void count_launch(int n = 1);
 

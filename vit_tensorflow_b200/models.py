@@ -13,6 +13,7 @@
     RegionViT vit_tensorflow/regionvit.py:184-263
     ScalableViT  vit_tensorflow/scalable_vit.py:250-319
     PiT       vit_tensorflow/pit.py:158-219
+    MAE / SimMIM  vit_tensorflow/mae.py:17-92, simmim.py:72-129 (around a ViT encoder)
 
 Same constructor kwargs, defaults and assertion messages; `model(img, training=True, **kwargs) -> logits`
 with `img` NHWC float32 `[b, H, W, 3]` and logits float32 `[b, num_classes]`.  Everything below the call is
@@ -1662,6 +1663,148 @@ class ATSViT(_EngineModel):
         return _as_tensor(logits)
 
     call = __call__
+
+
+class _MaskedImageModel(_EngineModel):
+    """What MAE and SimMIM share: a handle of their own built from the encoder ViT's configuration, the encoder's current weights
+    pushed into it before every call that follows a change, the engine's mask noise (set_seed) and the call itself."""
+
+    def _build(self, image_size, encoder, masking_ratio, seed, decoder=(0, 0, 0, 0)):
+        if not (isinstance(encoder, ViT) and encoder._kind == "vit"):
+            raise TypeError(f"{type(self).__name__}: the encoder must be a vit_tensorflow_b200.ViT (or DistillableViT), got "
+                            f"{type(encoder).__name__}")
+        encoder.build(input_shape=(1, image_size, image_size, 3))      # mae.py:32, simmim.py:77
+        self.encoder = encoder
+        self.masking_ratio = masking_ratio
+        self._dropout_rates = encoder._dropout_rates
+        ec = encoder._cfg
+        mc = _lib.VbMimConfig()
+        mc.struct_size = C.sizeof(_lib.VbMimConfig)
+        mc.masking_ratio = float(masking_ratio)
+        mc.decoder_dim, mc.decoder_depth, mc.decoder_heads, mc.decoder_dim_head = (int(v) for v in decoder)
+        self._mc = mc
+        lib = _lib.load()
+        self._create(encoder.precision, encoder.device, create=lambda cfg, dev, h: lib.vb_create_mim(cfg, C.byref(mc), dev, h),
+                     image_h=ec.image_h, image_w=ec.image_w, patch_h=ec.patch_h, patch_w=ec.patch_w, num_classes=ec.num_classes,
+                     dim=ec.dim, depth=ec.depth, heads=ec.heads, dim_head=ec.dim_head, mlp_dim=ec.mlp_dim)
+        self._encoder_names = tuple(n for n in self._specs if n in encoder._specs)
+        self._pushed = {}
+        self.init_weights(seed)
+
+    def init_weights(self, seed=None):
+        """The reference's initial distributions for the model's own weights (the encoder keeps its own): Dense glorot-uniform /
+        zero bias, LayerNormalization ones / zeros, mask_token tf.random.normal N(0, 1) (mae.py:43, simmim.py:85) and the Embedding
+        uniform(-0.05, 0.05) (Keras' default, mae.py:45)."""
+        rng = np.random.default_rng(seed)
+        w = collections.OrderedDict()
+        for name, shape in self._specs.items():
+            if name in self._encoder_names:
+                continue
+            leaf = name.rsplit(".", 1)[-1]
+            if leaf == "kernel":
+                lim = np.sqrt(6.0 / (shape[0] + shape[1]))
+                a = rng.uniform(-lim, lim, size=shape)
+            elif leaf in ("bias", "beta"):
+                a = np.zeros(shape)
+            elif leaf == "gamma":
+                a = np.ones(shape)
+            elif leaf == "embeddings":
+                a = rng.uniform(-0.05, 0.05, size=shape)
+            else:                                          # mask_token
+                a = rng.standard_normal(shape)
+            w[name] = a.astype(np.float32)
+        self.set_weights_dict(w)
+
+    def set_weights_dict(self, weights):
+        """The model's own weights (SURVEY.md App. B); the encoder's are set on the encoder and picked up by the next call."""
+        shared = [n for n in weights if n in self._encoder_names]
+        if shared:
+            raise KeyError(f"{type(self).__name__}: {shared[0]!r} belongs to the encoder: set it with encoder.set_weights_dict")
+        super().set_weights_dict(weights)
+
+    def _push_encoder(self):
+        changed = collections.OrderedDict((n, self.encoder.get_weight(n)) for n in self._encoder_names
+                                          if self._pushed.get(n) is not self.encoder.get_weight(n))
+        if changed:
+            _EngineModel.set_weights_dict(self, changed)
+            self._pushed.update(changed)
+
+    def _finalize(self):
+        self._push_encoder()
+        super()._finalize()
+
+    def set_seed(self, seed):
+        """The Philox key of the mask noise (include/vitb200.h); also restarts its draw counter, so the next calls repeat the masks
+        drawn after the previous set_seed(seed).  The seed is 0 at construction."""
+        _lib.check(self._lib.vb_mim_set_seed(self._h, int(seed) & 0xFFFFFFFFFFFFFFFF), self._h)
+
+    def _shapes(self, h, w):
+        ph, pw = self._cfg.patch_h, self._cfg.patch_w
+        if h % ph or w % pw:
+            raise ValueError("Image dimensions must be divisible by the patch size.")
+        n = (h // ph) * (w // pw)
+        return n, int(self.masking_ratio * n), ph * pw * 3
+
+    def forward_raw(self, img_ptr, img_mem, batch, h, w, loss_ptr, out_mem, stream=None, pred_ptr=None, patches_ptr=None,
+                    indices_ptr=None):
+        """Pointer-level call (vb_forward_mim): host or device buffers, optional cudaStream_t; pred / masked_patches [batch,
+        num_masked, patch_dim] and indices [batch, n] are written when their pointers are given."""
+        self._finalize()
+        p = [C.c_void_p(v) if v else None for v in (pred_ptr, patches_ptr, indices_ptr)]
+        _lib.check(self._lib.vb_forward_mim(self._h, C.c_void_p(img_ptr), img_mem, batch, h, w, C.c_void_p(loss_ptr), *p, out_mem,
+                                            C.c_void_p(stream) if stream else None), self._h)
+
+    def forward_mim(self, img, stream=None):
+        """One call: (loss, pred [b, num_masked, patch_dim], masked_patches [b, num_masked, patch_dim], indices [b, n]).  indices
+        is each image's noise permutation with the masked patch ids first; masked_patches are the image's patches at those ids, so
+        mean((pred - masked_patches) ** 2) is the MSE the MAE paper trains with."""
+        x = self._img(img)
+        b, h, w, _ = x.shape
+        n, nm, pd = self._shapes(h, w)
+        loss = np.zeros(1, np.float32)
+        pred, patches = np.empty((b, nm, pd), np.float32), np.empty((b, nm, pd), np.float32)
+        idx = np.empty((b, n), np.int32)
+        self.forward_raw(x.ctypes.data, _lib.MEM_HOST, b, h, w, loss.ctypes.data, _lib.MEM_HOST, stream, pred.ctypes.data,
+                         patches.ctypes.data, idx.ctypes.data)
+        return _as_tensor(loss.reshape(())), _as_tensor(pred), _as_tensor(patches), idx
+
+    def __call__(self, img, training=True, **kwargs):
+        """The reference's call: the reconstruction loss as a float32 0-d array (answers `.numpy()`)."""
+        self._check_training(training)
+        x = self._img(img)
+        b, h, w, _ = x.shape
+        self._shapes(h, w)
+        loss = np.zeros(1, np.float32)
+        self.forward_raw(x.ctypes.data, _lib.MEM_HOST, b, h, w, loss.ctypes.data, _lib.MEM_HOST)
+        return _as_tensor(loss.reshape(()))
+
+    call = __call__
+
+
+class MAE(_MaskedImageModel):
+    """mae.py:17-92 (masked autoencoder): the encoder ViT over a random quarter (1 - masking_ratio) of the patches, the decoder
+    over those and mask tokens, pixels predicted for the masked patches.  The call returns what the reference returns,
+    mean(pred^2): its tf.square(pred, masked_patches) passes the patches as tf.square's `name` (SURVEY.md App. D); forward_mim
+    also returns the masked patches.  The masks come from the engine's Philox noise (set_seed); precision and device are the
+    encoder's, and the encoder's weights are read at every call that follows a change."""
+    _kind = "mae"
+
+    def __init__(self, image_size, encoder, decoder_dim, masking_ratio=0.75, decoder_depth=1, decoder_heads=8, decoder_dim_head=64, *,
+                 seed=None):
+        assert masking_ratio > 0 and masking_ratio < 1, 'masking ratio must be kept between 0 and 1'
+        self.decoder_dim = decoder_dim
+        self._build(image_size, encoder, masking_ratio, seed, (decoder_dim, decoder_depth, decoder_heads, decoder_dim_head))
+
+
+class SimMIM(_MaskedImageModel):
+    """simmim.py:72-129: the encoder ViT over all patches with the masked ones replaced by the mask token, a linear head on the
+    masked rows, loss mean(|pred - masked_patches|) / num_masked (the reference's extra division kept).  Masks, precision, device
+    and encoder weights as for MAE."""
+    _kind = "simmim"
+
+    def __init__(self, image_size, encoder, masking_ratio=0.5, *, seed=None):
+        assert masking_ratio > 0 and masking_ratio < 1, 'masking ratio must be kept between 0 and 1'
+        self._build(image_size, encoder, masking_ratio, seed)
 
 
 def _spt_patch_size(patch_size):
