@@ -124,8 +124,23 @@ class _EngineModel:
     """Common machinery: engine handle, weight dict, forward call."""
 
     _kind = None
+    _encoder_names = ()         # weights another model owns and initialises (MAE / SimMIM: the encoder's)
+    _inference_only = None      # the message of a family whose every call without training=False raises NotImplementedError
+    # tf.random.normal Variables, N(0, 1): vit.py:146-147, deepvit.py:57, cait.py:97-98, vit_with_patch_merger.py:47,
+    # nest.py:129, mae.py:43, simmim.py:85; vit_for_small_dataset.py:94's temperature is drawn too, then set (SmallDatasetViT)
+    _NORMAL_LEAVES = ("pos_embedding", "cls_token", "reattn_weights", "mix_pre", "mix_post", "queries", "pos_emb", "mask_token",
+                      "temperature")
 
-    def _create(self, precision, device, create=None, **cfgkw):
+    def _create(self, precision, device, ext=None, create="vb_create", **cfgkw):
+        """`_config`, then every VbConfig field of `cfgkw` as int(value), then `_open`."""
+        cfg = self._config(precision, device)
+        for k, v in cfgkw.items():
+            setattr(cfg, k, int(v))
+        self._open(cfg, create, ext)
+
+    def _config(self, precision, device):
+        """The family's VbConfig at `precision` with 3 channels, for the caller to fill and hand to `_open`.  A field assigned
+        directly refuses a non-integer with ctypes' TypeError; `_create` converts with int() instead."""
         self.precision = precision
         self.device = int(device)
         cfg = _lib.VbConfig()
@@ -135,15 +150,19 @@ class _EngineModel:
             raise ValueError(f"precision must be one of {sorted(_lib.PRECISION)}")
         cfg.precision = _lib.PRECISION[precision]
         cfg.channels = 3
-        for k, v in cfgkw.items():
-            setattr(cfg, k, int(v))
         self._cfg = cfg
+        return cfg
+
+    def _open(self, cfg, create="vb_create", ext=None):
+        """Create the engine handle and read its weight list.  A family with an extension config passes the filled struct as
+        `ext` and its entry point as `create` (e.g. "vb_create_levit")."""
         self._lib = _lib.load()
         h = C.c_void_p()
-        if create is None:
-            _lib.check(self._lib.vb_create(C.byref(cfg), self.device, C.byref(h)))
-        else:                                             # a kind with an extension config: create(cfg, device, &h) -> rc
-            _lib.check(create(C.byref(cfg), self.device, C.byref(h)))
+        if ext is None:
+            _lib.check(getattr(self._lib, create)(C.byref(cfg), self.device, C.byref(h)))
+        else:
+            ext.struct_size = C.sizeof(ext)
+            _lib.check(getattr(self._lib, create)(C.byref(cfg), C.byref(ext), self.device, C.byref(h)))
         self._h = h
         self._finalized = False
         self._specs = collections.OrderedDict()
@@ -158,31 +177,36 @@ class _EngineModel:
         return collections.OrderedDict(self._specs)
 
     def init_weights(self, seed=None):
-        """The reference's initial distributions: Dense glorot-uniform / zero bias (Keras defaults),
-        LayerNormalization ones/zeros, tf.random.normal Variables N(0,1) (vit.py:146-147, deepvit.py:57,
-        cait.py:97-98), LayerScale fill (cait.py:36-44)."""
+        """The reference's initial distributions, drawn from one generator in weight-list order (see `_initial_value`)."""
         rng = np.random.default_rng(seed)
-        w = collections.OrderedDict()
-        for name, shape in self._specs.items():
-            leaf = name.rsplit(".", 1)[-1]
-            if leaf == "kernel":
-                receptive = int(np.prod(shape[:-2]))          # Conv2D kernel [k, k, cin, cout]: fans count the window (1 for Dense)
-                lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
-                a = rng.uniform(-lim, lim, size=shape)
-            elif leaf in ("bias", "beta"):
-                a = np.zeros(shape)
-            elif leaf == "gamma":
-                a = np.ones(shape)
-            elif leaf in ("attn_scale", "ff_scale"):
-                layer = int(name.split(".layers.")[1].split(".")[0])
-                a = np.full(shape, _layerscale_eps(layer + 1))
-            elif leaf == "positional_emb":                   # CCT cct.py:251-254
-                a = (sinusoidal_embedding(shape[1], shape[2]) if self._positional_embedding == "sine"
-                     else _truncated_normal(rng, shape, 0.2))
-            else:  # pos_embedding, cls_token, reattn_weights, mix_pre, mix_post
-                a = rng.standard_normal(shape)
-            w[name] = a.astype(np.float32)
-        self.set_weights_dict(w)
+        self.set_weights_dict(collections.OrderedDict((name, self._initial_value(name, shape, rng).astype(np.float32))
+                                                      for name, shape in self._specs.items() if name not in self._encoder_names))
+
+    def _initial_value(self, name, shape, rng):
+        """Keras' defaults by leaf name: Conv2D / Dense kernels glorot-uniform over the receptive field (a depthwise kernel
+        [k, k, 1, dim] has fan_in k^2 and fan_out k^2 * dim), zero biases, LayerNorm / LayerNormalization / BatchNormalization
+        gamma 1 and beta 0 with moving statistics 0 and 1, Embedding U(-0.05, 0.05); LayerScale fill (cait.py:36-44), CCT's
+        positional embedding (cct.py:251-254) and the tf.random.normal Variables of _NORMAL_LEAVES."""
+        leaf = name.rsplit(".", 1)[-1]
+        if leaf == "kernel":
+            receptive = int(np.prod(shape[:-2]))              # Conv2D kernel [k, k, cin, cout]: fans count the window (1 for Dense)
+            lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
+            return rng.uniform(-lim, lim, size=shape)
+        if leaf in ("bias", "beta", "b", "moving_mean"):
+            return np.zeros(shape)
+        if leaf in ("gamma", "g", "moving_variance"):
+            return np.ones(shape)
+        if leaf == "embeddings":
+            return rng.uniform(-0.05, 0.05, size=shape)
+        if leaf in ("attn_scale", "ff_scale"):
+            layer = int(name.split(".layers.")[1].split(".")[0])
+            return np.full(shape, _layerscale_eps(layer + 1))
+        if leaf == "positional_emb":
+            return (sinusoidal_embedding(shape[1], shape[2]) if self._positional_embedding == "sine"
+                    else _truncated_normal(rng, shape, 0.2))
+        if leaf in self._NORMAL_LEAVES:
+            return rng.standard_normal(shape)
+        raise AssertionError(f"{type(self).__name__}: no initial distribution for weight {name!r}")
 
     def set_weights_dict(self, weights):
         """weights: mapping name -> array in the Keras layout (SURVEY.md App. B).  Missing names keep their value."""
@@ -239,7 +263,10 @@ class _EngineModel:
 
     # ---- forward ------------------------------------------------------------------------------------
     def _check_training(self, training):
-        if training and any(r != 0 for r in self._dropout_rates):
+        if self._inference_only is not None:
+            if training is None or training:
+                raise NotImplementedError(self._inference_only)
+        elif training and any(r != 0 for r in self._dropout_rates):
             raise NotImplementedError(
                 "libvitb200 implements inference semantics: stochastic dropout (rate > 0 with training=True, the "
                 "reference's default) is not reproducible; pass training=False or construct with dropout = 0")
@@ -256,6 +283,12 @@ class _EngineModel:
         return _as_tensor(out)
 
     call = __call__
+
+    def __init_subclass__(cls, **kwargs):
+        """Keras' name of the forward: every class's `call` is its own `__call__`, so it keeps that call's signature.  This
+        replaces any `call` a subclass defines: a family changes its forward through `__call__`."""
+        super().__init_subclass__(**kwargs)
+        cls.call = cls.__call__
 
     def forward_raw(self, img_ptr, img_mem, batch, h, w, logits_ptr, logits_mem, stream=None):
         """Pointer-level forward: host or device (e.g. torch tensor .data_ptr()) buffers, optional cudaStream_t."""
@@ -439,8 +472,6 @@ class DistillableViT(ViT):
         self._check_training(training)
         return _forward_distill(self, img, distill_token)
 
-    call = __call__
-
 
 def _distill_token(model, distill_token):
     """The caller's distillation token `[1, 1, dim]` (distill.py:101) as a flat float32 vector of `dim` values."""
@@ -560,8 +591,6 @@ class T2TViT(_EngineModel):
         x = np.asarray(self._injected(x, training=training), dtype=np.float32)   # :105
         return self.forward_head(x)                                   # :107-112
 
-    call = __call__
-
 
 class DistillableT2TViT(T2TViT):
     """distill.py:61-72 (DistillMixin.call distill.py:16-45): a T2TViT whose call takes an optional distillation token
@@ -584,8 +613,6 @@ class DistillableT2TViT(T2TViT):
         x = np.concatenate([x, np.broadcast_to(tok, (x.shape[0], 1, self.dim))], axis=1)   # :26-28: the token as the last row
         x = np.asarray(self._injected(x, training=training), dtype=np.float32)             # :30, _attend :69-72
         return self.forward_head(x[:, :-1]), _as_tensor(np.ascontiguousarray(x[:, -1]))    # :32-43
-
-    call = __call__
 
 
 class PatchMergerViT(_EngineModel):
@@ -651,8 +678,6 @@ class EfficientViT(_EngineModel):
         x = np.asarray(self.transformer(x, training=training), dtype=np.float32)  # :46
         return self.forward_head(x)                                              # :48-55
 
-    call = __call__
-
 
 class DistillableEfficientViT(EfficientViT):
     """distill.py:74-85 as the reference runs it: its `_attend` reads `self.dropout` (:83), which efficient.ViT never defines
@@ -667,8 +692,6 @@ class DistillableEfficientViT(EfficientViT):
 
     def __call__(self, img, distill_token=None, training=True):
         raise AttributeError(f"'{type(self).__name__}' object has no attribute 'dropout'")
-
-    call = __call__
 
 
 def sinusoidal_embedding(n_channels, dim):
@@ -728,6 +751,8 @@ class CCT(_EngineModel):
     Weights (SURVEY.md App. B): tokenizer.conv.{i}.kernel [k, k, cin, cout], positional_emb [1, n, dim],
     layers.L.{attn_norm, to_qkv, to_out, norm1, fc1, fc2}, norm, attention_pool [dim, 1] + [1], head."""
     _kind = "cct"
+    _inference_only = ("CCT runs inference only: the reference's call resolves training=None to True and then applies its "
+                       "hard-coded attention dropout and stochastic depth of 0.1 (cct.py:336-338); pass training=False")
 
     def __init__(self, img_size=224, embedding_dim=768, n_input_channels=3, n_conv_layers=1, kernel_size=7, stride=2,
                  pooling_kernel_size=3, pooling_stride=2, *args, precision="bf16", device=0, seed=None, **kwargs):
@@ -749,17 +774,9 @@ class CCT(_EngineModel):
                      cct_pool_stride=pooling_stride, cct_pos_emb=_lib.CCT_POS[tc.positional_embedding])
         self.init_weights(seed)
 
-    def _check_training(self, training):
-        if training is None or training:
-            raise NotImplementedError(
-                "CCT runs inference only: the reference's call resolves training=None to True and then applies its "
-                "hard-coded attention dropout and stochastic depth of 0.1 (cct.py:336-338); pass training=False")
-
     def __call__(self, img, training=None, **kwargs):
         """cct.py:342: NHWC float image batch -> float32 logits [b, num_classes]; training must be False."""
         return super().__call__(img, training=training)
-
-    call = __call__
 
 
 def _cct(num_layers, num_heads, mlp_ratio, embedding_dim, kernel_size=3, stride=None, *args, **kwargs):   # cct.py:51-61
@@ -818,6 +835,8 @@ class LeViT(_EngineModel):
     to_q / to_k / to_v .0 conv + .1 BatchNormalization, pos_bias.embeddings, to_out.1 conv + .2 BatchNormalization),
     backbone.{t}.layers.{l}.1.net.{0,3} (MLP), mlp_head, distill_head."""
     _kind = "levit"
+    _inference_only = ("LeViT runs inference only: with training=True (the reference's default, levit.py:214) every BatchNormalization "
+                       "normalises with the batch's own statistics and dropout draws masks; pass training=False")
 
     def __init__(self, image_size, num_classes, dim, depth, heads, mlp_mult, stages=3, dim_key=32, dim_value=64, dropout=0.0,
                  num_distill_classes=None, *, precision="bf16", device=0, seed=None):
@@ -839,66 +858,23 @@ class LeViT(_EngineModel):
         self.dims, self.depths, self.layer_heads = dims, depths, layer_heads
         self.image_size, self.dim_key, self.dim_value, self.mlp_mult, self.stages = image_size, dim_key, dim_value, mlp_mult, stages
         self._dropout_rates = (dropout,)
-        self.precision = precision
-        self.device = int(device)
-        cfg = _lib.VbConfig()
-        cfg.struct_size = C.sizeof(_lib.VbConfig)
-        cfg.kind = _lib.KIND["levit"]
-        if precision not in _lib.PRECISION:
-            raise ValueError(f"precision must be one of {sorted(_lib.PRECISION)}")
-        cfg.precision = _lib.PRECISION[precision]
-        cfg.channels, cfg.image_h, cfg.image_w, cfg.num_classes = 3, image_size, image_size, num_classes
+        cfg = self._config(precision, device)
+        cfg.image_h, cfg.image_w, cfg.num_classes = image_size, image_size, num_classes
         cfg.dim = dims[-1]                               # the pooled width (what the engine's handle records as dim)
         lv = _lib.VbLevitConfig()
-        lv.struct_size = C.sizeof(_lib.VbLevitConfig)
         lv.stages = stages
         for i in range(stages):
             lv.dims[i], lv.depths[i], lv.heads[i] = dims[i], depths[i], layer_heads[i]
         lv.dim_key, lv.dim_value, lv.mlp_mult = dim_key, dim_value, mlp_mult
         lv.num_distill_classes = num_distill_classes or 0
-        self._cfg, self._lv = cfg, lv
-        self._lib = _lib.load()
-        h = C.c_void_p()
-        _lib.check(self._lib.vb_create_levit(C.byref(cfg), C.byref(lv), self.device, C.byref(h)))
-        self._h = h
-        self._finalized = False
-        self._specs = collections.OrderedDict()
-        name, shape, ndim = C.c_char_p(), (C.c_int64 * 4)(), C.c_int32()
-        for i in range(self._lib.vb_num_weights(h)):
-            _lib.check(self._lib.vb_weight_info(h, i, C.byref(name), shape, C.byref(ndim)), h)
-            self._specs[name.value.decode()] = tuple(int(shape[j]) for j in range(ndim.value))
-        self._weights = collections.OrderedDict()
+        self._lv = lv
+        self._open(cfg, "vb_create_levit", lv)
         self.init_weights(seed)
 
-    def init_weights(self, seed=None):
-        """The reference's initialisers: glorot-uniform over the receptive field and zero biases (Conv2D / Dense), BatchNormalization
-        gamma 1 / beta 0 / moving statistics 0 and 1 with the to_out gamma at 0 (levit.py:91), Embedding U(-0.05, 0.05)."""
-        rng = np.random.default_rng(seed)
-        w = collections.OrderedDict()
-        for name, shape in self._specs.items():
-            leaf = name.rsplit(".", 1)[-1]
-            if leaf == "kernel":
-                receptive = int(np.prod(shape[:-2]))
-                lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
-                a = rng.uniform(-lim, lim, size=shape)
-            elif leaf in ("bias", "beta", "moving_mean"):
-                a = np.zeros(shape)
-            elif leaf == "moving_variance":
-                a = np.ones(shape)
-            elif leaf == "gamma":
-                a = np.zeros(shape) if ".to_out." in name else np.ones(shape)
-            elif leaf == "embeddings":
-                a = rng.uniform(-0.05, 0.05, size=shape)
-            else:
-                raise AssertionError(name)
-            w[name] = a.astype(np.float32)
-        self.set_weights_dict(w)
-
-    def _check_training(self, training):
-        if training is None or training:
-            raise NotImplementedError(
-                "LeViT runs inference only: with training=True (the reference's default, levit.py:214) every BatchNormalization "
-                "normalises with the batch's own statistics and dropout draws masks; pass training=False")
+    def _initial_value(self, name, shape, rng):
+        if ".to_out." in name and name.endswith(".gamma"):    # the to_out BatchNormalization starts at 0 (levit.py:91)
+            return np.zeros(shape)
+        return super()._initial_value(name, shape, rng)
 
     def __call__(self, img, training=True, **kwargs):
         """levit.py:214: NHWC float images -> logits [b, num_classes], or (logits, distill [b, num_distill_classes]) with a
@@ -915,8 +891,6 @@ class LeViT(_EngineModel):
                                                 logits.ctypes.data_as(C.c_void_p), dist.ctypes.data_as(C.c_void_p), _lib.MEM_HOST,
                                                 None), self._h)
         return _as_tensor(logits), _as_tensor(dist)
-
-    call = __call__
 
 
 LEVIT_CTOR_KEYS = ("image_size", "num_classes", "dim", "depth", "heads", "mlp_mult", "stages", "dim_key", "dim_value", "dropout",
@@ -937,6 +911,8 @@ class CvT(_EngineModel):
     (LayerNorm), cvt_layers.{s}.2.layers.{l}.0.norm / .0.fn.to_q.net.{0,1,2} / .0.fn.to_kv.net.{0,1,2} / .0.fn.to_out.0,
     cvt_layers.{s}.2.layers.{l}.1.norm / .1.fn.net.{0,3}, cvt_layers.3.1 (the Dense head)."""
     _kind = "cvt"
+    _inference_only = ("CvT runs inference only: with training=True (the reference's default, cvt.py:200) every BatchNormalization "
+                       "normalises with the batch's own statistics and dropout draws masks; pass training=False")
 
     def __init__(self,
                  num_classes,
@@ -975,66 +951,19 @@ class CvT(_EngineModel):
                 raise ValueError(f"CvT: proj_kernel {st['proj_kernel']} is not supported (1 to 7)")
             if st["kv_proj_stride"] not in (1, 2):
                 raise ValueError(f"CvT: kv_proj_stride {st['kv_proj_stride']} is not supported (1 or 2)")
-        self.precision = precision
-        self.device = int(device)
-        cfg = _lib.VbConfig()
-        cfg.struct_size = C.sizeof(_lib.VbConfig)
-        cfg.kind = _lib.KIND["cvt"]
-        if precision not in _lib.PRECISION:
-            raise ValueError(f"precision must be one of {sorted(_lib.PRECISION)}")
-        cfg.precision = _lib.PRECISION[precision]
-        cfg.channels, cfg.num_classes = 3, num_classes
-        cfg.dim = self.stages[-1]["emb_dim"]
+        cfg = self._config(precision, device)
+        cfg.num_classes, cfg.dim = num_classes, self.stages[-1]["emb_dim"]
         cv = _lib.VbCvtConfig()
-        cv.struct_size = C.sizeof(_lib.VbCvtConfig)
         for i, st in enumerate(self.stages):
             for k in CVT_STAGE_KEYS:
                 getattr(cv, k)[i] = int(st[k])
-        self._cfg, self._cv = cfg, cv
-        self._lib = _lib.load()
-        h = C.c_void_p()
-        _lib.check(self._lib.vb_create_cvt(C.byref(cfg), C.byref(cv), self.device, C.byref(h)))
-        self._h = h
-        self._finalized = False
-        self._specs = collections.OrderedDict()
-        name, shape, ndim = C.c_char_p(), (C.c_int64 * 4)(), C.c_int32()
-        for i in range(self._lib.vb_num_weights(h)):
-            _lib.check(self._lib.vb_weight_info(h, i, C.byref(name), shape, C.byref(ndim)), h)
-            self._specs[name.value.decode()] = tuple(int(shape[j]) for j in range(ndim.value))
-        self._weights = collections.OrderedDict()
+        self._cv = cv
+        self._open(cfg, "vb_create_cvt", cv)
         self.init_weights(seed)
-
-    def init_weights(self, seed=None):
-        """The reference's initialisers: glorot-uniform over the receptive field (a depthwise kernel [k, k, 1, dim] has fan_in k^2 and
-        fan_out k^2 * dim) and zero biases, BatchNormalization gamma 1 / beta 0 / moving statistics 0 and 1, LayerNorm g 1 / b 0."""
-        rng = np.random.default_rng(seed)
-        w = collections.OrderedDict()
-        for name, shape in self._specs.items():
-            leaf = name.rsplit(".", 1)[-1]
-            if leaf == "kernel":
-                receptive = int(np.prod(shape[:-2]))
-                lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
-                a = rng.uniform(-lim, lim, size=shape)
-            elif leaf in ("bias", "beta", "moving_mean", "b"):
-                a = np.zeros(shape)
-            elif leaf in ("gamma", "moving_variance", "g"):
-                a = np.ones(shape)
-            else:
-                raise AssertionError(name)
-            w[name] = a.astype(np.float32)
-        self.set_weights_dict(w)
-
-    def _check_training(self, training):
-        if training is None or training:
-            raise NotImplementedError(
-                "CvT runs inference only: with training=True (the reference's default, cvt.py:200) every BatchNormalization "
-                "normalises with the batch's own statistics and dropout draws masks; pass training=False")
 
     def __call__(self, img, training=True, **kwargs):
         """cvt.py:200: NHWC float images of any size -> logits [b, num_classes].  training must be False."""
         return super().__call__(img, training=training)
-
-    call = __call__
 
 
 CVT_CTOR_KEYS = ("num_classes",) + tuple(f"s{i}_{k}" for i in (1, 2, 3) for k in CVT_STAGE_KEYS) + ("dropout",)
@@ -1104,55 +1033,16 @@ class TwinsSVT(_EngineModel):
         self._dropout_rates = (dropout,)
         if not 1 <= peg_kernel_size <= 7:
             raise ValueError(f"Twins-SVT: peg_kernel_size {peg_kernel_size} is not supported (1 to 7)")
-        self.precision = precision
-        self.device = int(device)
-        cfg = _lib.VbConfig()
-        cfg.struct_size = C.sizeof(_lib.VbConfig)
-        cfg.kind = _lib.KIND["twins_svt"]
-        if precision not in _lib.PRECISION:
-            raise ValueError(f"precision must be one of {sorted(_lib.PRECISION)}")
-        cfg.precision = _lib.PRECISION[precision]
-        cfg.channels, cfg.num_classes = 3, num_classes
-        cfg.dim = self.stages[-1]["emb_dim"]
+        cfg = self._config(precision, device)
+        cfg.num_classes, cfg.dim = num_classes, self.stages[-1]["emb_dim"]
         tw = _lib.VbTwinsSvtConfig()
-        tw.struct_size = C.sizeof(_lib.VbTwinsSvtConfig)
         for i, st in enumerate(self.stages):
             for k in TWINS_STAGE_KEYS:
                 getattr(tw, k)[i] = int(st[k])
         tw.peg_kernel_size = int(peg_kernel_size)
-        self._cfg, self._tw = cfg, tw
-        self._lib = _lib.load()
-        h = C.c_void_p()
-        _lib.check(self._lib.vb_create_twins_svt(C.byref(cfg), C.byref(tw), self.device, C.byref(h)))
-        self._h = h
-        self._finalized = False
-        self._specs = collections.OrderedDict()
-        name, shape, ndim = C.c_char_p(), (C.c_int64 * 4)(), C.c_int32()
-        for i in range(self._lib.vb_num_weights(h)):
-            _lib.check(self._lib.vb_weight_info(h, i, C.byref(name), shape, C.byref(ndim)), h)
-            self._specs[name.value.decode()] = tuple(int(shape[j]) for j in range(ndim.value))
-        self._weights = collections.OrderedDict()
+        self._tw = tw
+        self._open(cfg, "vb_create_twins_svt", tw)
         self.init_weights(seed)
-
-    def init_weights(self, seed=None):
-        """The reference's initialisers: glorot-uniform over the receptive field (the PEG's depthwise kernel [k, k, 1, dim] has fan_in
-        k^2 and fan_out k^2 * dim), zero biases, LayerNorm g 1 / b 0."""
-        rng = np.random.default_rng(seed)
-        w = collections.OrderedDict()
-        for name, shape in self._specs.items():
-            leaf = name.rsplit(".", 1)[-1]
-            if leaf == "kernel":
-                receptive = int(np.prod(shape[:-2]))
-                lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
-                a = rng.uniform(-lim, lim, size=shape)
-            elif leaf in ("bias", "b"):
-                a = np.zeros(shape)
-            elif leaf == "g":
-                a = np.ones(shape)
-            else:
-                raise AssertionError(name)
-            w[name] = a.astype(np.float32)
-        self.set_weights_dict(w)
 
     def __call__(self, img, training=True, **kwargs):
         """twins_svt.py:266-268: NHWC float images -> logits [b, num_classes]; extra kwargs are accepted and ignored, as there."""
@@ -1162,8 +1052,6 @@ class TwinsSVT(_EngineModel):
             if err is not None:
                 raise ValueError(err)
         return super().__call__(img, training=training)
-
-    call = __call__
 
 
 TWINS_CTOR_KEYS = ("num_classes",) + tuple(f"s{i}_{k}" for i in (1, 2, 3, 4) for k in TWINS_STAGE_KEYS) + ("peg_kernel_size", "dropout")
@@ -1239,57 +1127,18 @@ class CrossFormer(_EngineModel):
             if len({k % 2 for k in ks}) != 1 or min(ks) < st["stride"]:
                 raise ValueError(f"CrossFormer stage {i}: kernel sizes {ks} at stride {st['stride']} are not supported: the nested "
                                  "cross-scale embedding needs kernel sizes of one parity, each at least the stride")
-        self.precision = precision
-        self.device = int(device)
-        cfg = _lib.VbConfig()
-        cfg.struct_size = C.sizeof(_lib.VbConfig)
-        cfg.kind = _lib.KIND["crossformer"]
-        if precision not in _lib.PRECISION:
-            raise ValueError(f"precision must be one of {sorted(_lib.PRECISION)}")
-        cfg.precision = _lib.PRECISION[precision]
-        cfg.channels, cfg.num_classes = 3, num_classes
-        cfg.dim = self.stages[-1]["dim"]
+        cfg = self._config(precision, device)
+        cfg.num_classes, cfg.dim = num_classes, self.stages[-1]["dim"]
         cf = _lib.VbCrossformerConfig()
-        cf.struct_size = C.sizeof(_lib.VbCrossformerConfig)
         for i, st in enumerate(self.stages):
             for k in ("dim", "depth", "global_wsz", "local_wsz", "stride"):
                 getattr(cf, k)[i] = st[k]
             cf.n_kernels[i] = len(st["kernels"])
             for j, k in enumerate(st["kernels"]):
                 cf.kernels[i][j] = int(k)
-        self._cfg, self._cf = cfg, cf
-        self._lib = _lib.load()
-        h = C.c_void_p()
-        _lib.check(self._lib.vb_create_crossformer(C.byref(cfg), C.byref(cf), self.device, C.byref(h)))
-        self._h = h
-        self._finalized = False
-        self._specs = collections.OrderedDict()
-        name, shape, ndim = C.c_char_p(), (C.c_int64 * 4)(), C.c_int32()
-        for i in range(self._lib.vb_num_weights(h)):
-            _lib.check(self._lib.vb_weight_info(h, i, C.byref(name), shape, C.byref(ndim)), h)
-            self._specs[name.value.decode()] = tuple(int(shape[j]) for j in range(ndim.value))
-        self._weights = collections.OrderedDict()
+        self._cf = cf
+        self._open(cfg, "vb_create_crossformer", cf)
         self.init_weights(seed)
-
-    def init_weights(self, seed=None):
-        """The reference's initialisers: glorot-uniform over the receptive field for every Conv2D and Dense kernel, zero biases,
-        LayerNorm g 1 / b 0 and LayerNormalization gamma 1 / beta 0."""
-        rng = np.random.default_rng(seed)
-        w = collections.OrderedDict()
-        for name, shape in self._specs.items():
-            leaf = name.rsplit(".", 1)[-1]
-            if leaf == "kernel":
-                receptive = int(np.prod(shape[:-2]))
-                lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
-                a = rng.uniform(-lim, lim, size=shape)
-            elif leaf in ("bias", "b", "beta"):
-                a = np.zeros(shape)
-            elif leaf in ("g", "gamma"):
-                a = np.ones(shape)
-            else:
-                raise AssertionError(name)
-            w[name] = a.astype(np.float32)
-        self.set_weights_dict(w)
 
     def __call__(self, img, training=True, **kwargs):
         """crossformer.py:263-269: NHWC float images -> logits [b, num_classes]; extra kwargs are accepted and ignored, as there."""
@@ -1299,8 +1148,6 @@ class CrossFormer(_EngineModel):
             if err is not None:
                 raise ValueError(err)
         return super().__call__(img, training=training)
-
-    call = __call__
 
 
 CROSSFORMER_CTOR_KEYS = ("dim", "depth", "global_window_size", "local_window_size", "cross_embed_kernel_sizes", "cross_embed_strides",
@@ -1378,58 +1225,17 @@ class NesT(_EngineModel):
         self.plan = nest_plan(image_size, patch_size, dim, heads, num_hierarchies, block_repeats)
         self.num_classes = num_classes
         self._dropout_rates = (dropout,)
-        self.precision = precision
-        self.device = int(device)
-        cfg = _lib.VbConfig()
-        cfg.struct_size = C.sizeof(_lib.VbConfig)
-        cfg.kind = _lib.KIND["nest"]
-        if precision not in _lib.PRECISION:
-            raise ValueError(f"precision must be one of {sorted(_lib.PRECISION)}")
-        cfg.precision = _lib.PRECISION[precision]
-        cfg.channels, cfg.num_classes = 3, num_classes
-        cfg.dim = self.plan["last_dim"]
+        cfg = self._config(precision, device)
+        cfg.num_classes, cfg.dim = num_classes, self.plan["last_dim"]
         nc = _lib.VbNestConfig()
-        nc.struct_size = C.sizeof(_lib.VbNestConfig)
         nc.patch_size, nc.dim, nc.heads, nc.num_hierarchies = patch_size, dim, heads, num_hierarchies
         nc.levels = len(self.plan["levels"])
         for i, lv in enumerate(self.plan["levels"]):
             nc.block_repeats[i] = lv["depth"]
         nc.mlp_mult, nc.seq_len = mlp_mult, self.plan["seq_len"]
-        self._cfg, self._nc = cfg, nc
-        self._lib = _lib.load()
-        h = C.c_void_p()
-        _lib.check(self._lib.vb_create_nest(C.byref(cfg), C.byref(nc), self.device, C.byref(h)))
-        self._h = h
-        self._finalized = False
-        self._specs = collections.OrderedDict()
-        name, shape, ndim = C.c_char_p(), (C.c_int64 * 4)(), C.c_int32()
-        for i in range(self._lib.vb_num_weights(h)):
-            _lib.check(self._lib.vb_weight_info(h, i, C.byref(name), shape, C.byref(ndim)), h)
-            self._specs[name.value.decode()] = tuple(int(shape[j]) for j in range(ndim.value))
-        self._weights = collections.OrderedDict()
+        self._nc = nc
+        self._open(cfg, "vb_create_nest", nc)
         self.init_weights(seed)
-
-    def init_weights(self, seed=None):
-        """The reference's initialisers: glorot-uniform over the receptive field for every Conv2D and Dense kernel, zero biases,
-        LayerNorm g 1 / b 0, pos_emb N(0, 1) (nest.py:129)."""
-        rng = np.random.default_rng(seed)
-        w = collections.OrderedDict()
-        for name, shape in self._specs.items():
-            leaf = name.rsplit(".", 1)[-1]
-            if leaf == "kernel":
-                receptive = int(np.prod(shape[:-2]))
-                lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
-                a = rng.uniform(-lim, lim, size=shape)
-            elif leaf in ("bias", "b"):
-                a = np.zeros(shape)
-            elif leaf == "g":
-                a = np.ones(shape)
-            elif leaf == "pos_emb":
-                a = rng.standard_normal(shape)
-            else:
-                raise AssertionError(name)
-            w[name] = a.astype(np.float32)
-        self.set_weights_dict(w)
 
     def __call__(self, img, training=True, **kwargs):
         """nest.py:202-216: NHWC float images -> logits [b, num_classes]; extra kwargs are accepted and ignored, as there."""
@@ -1439,8 +1245,6 @@ class NesT(_EngineModel):
             if err is not None:
                 raise ValueError(err)
         return super().__call__(img, training=training)
-
-    call = __call__
 
 
 NEST_CTOR_KEYS = ("image_size", "patch_size", "num_classes", "dim", "heads", "num_hierarchies", "block_repeats", "mlp_mult", "dropout")
@@ -1510,57 +1314,16 @@ class RegionViT(_EngineModel):
         self.tokenize_local_3_conv, self.use_peg = bool(tokenize_local_3_conv), bool(use_peg)
         self.num_classes = num_classes
         self._dropout_rates = (ff_dropout,)               # Attention never builds its Dropout (:80-91)
-        self.precision = precision
-        self.device = int(device)
-        cfg = _lib.VbConfig()
-        cfg.struct_size = C.sizeof(_lib.VbConfig)
-        cfg.kind = _lib.KIND["regionvit"]
-        if precision not in _lib.PRECISION:
-            raise ValueError(f"precision must be one of {sorted(_lib.PRECISION)}")
-        cfg.precision = _lib.PRECISION[precision]
-        cfg.channels, cfg.num_classes = 3, num_classes
-        cfg.dim = self.dims[-1]
+        cfg = self._config(precision, device)
+        cfg.num_classes, cfg.dim = num_classes, self.dims[-1]
         rc = _lib.VbRegionvitConfig()
-        rc.struct_size = C.sizeof(_lib.VbRegionvitConfig)
         for i in range(4):
             rc.dims[i], rc.depth[i] = self.dims[i], self.depths[i]
         rc.window_size, rc.local_patch_size = window_size, local_patch_size
         rc.tokenize_local_3_conv, rc.use_peg, rc.mlp_mult = int(self.tokenize_local_3_conv), int(self.use_peg), 4
-        self._cfg, self._rc = cfg, rc
-        self._lib = _lib.load()
-        h = C.c_void_p()
-        _lib.check(self._lib.vb_create_regionvit(C.byref(cfg), C.byref(rc), self.device, C.byref(h)))
-        self._h = h
-        self._finalized = False
-        self._specs = collections.OrderedDict()
-        name, shape, ndim = C.c_char_p(), (C.c_int64 * 4)(), C.c_int32()
-        for i in range(self._lib.vb_num_weights(h)):
-            _lib.check(self._lib.vb_weight_info(h, i, C.byref(name), shape, C.byref(ndim)), h)
-            self._specs[name.value.decode()] = tuple(int(shape[j]) for j in range(ndim.value))
-        self._weights = collections.OrderedDict()
+        self._rc = rc
+        self._open(cfg, "vb_create_regionvit", rc)
         self.init_weights(seed)
-
-    def init_weights(self, seed=None):
-        """Keras's initialisers: glorot-uniform over the receptive field for every Conv2D and Dense kernel (the depthwise PEG's
-        fan-in is its 9 taps), zero biases, LayerNorm gamma 1 / beta 0, the Embedding U(-0.05, 0.05)."""
-        rng = np.random.default_rng(seed)
-        w = collections.OrderedDict()
-        for name, shape in self._specs.items():
-            leaf = name.rsplit(".", 1)[-1]
-            if leaf == "kernel":
-                receptive = int(np.prod(shape[:-2]))
-                lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
-                a = rng.uniform(-lim, lim, size=shape)
-            elif leaf in ("bias", "beta"):
-                a = np.zeros(shape)
-            elif leaf == "gamma":
-                a = np.ones(shape)
-            elif leaf == "embeddings":
-                a = rng.uniform(-0.05, 0.05, size=shape)
-            else:
-                raise AssertionError(name)
-            w[name] = a.astype(np.float32)
-        self.set_weights_dict(w)
 
     def __call__(self, x, training=True, **kwargs):
         """regionvit.py:249-263: NHWC float images -> logits [b, num_classes]; extra kwargs are accepted and ignored, as there."""
@@ -1575,8 +1338,6 @@ class RegionViT(_EngineModel):
             if err is not None:
                 raise ValueError(err)
         return super().__call__(x, training=training)
-
-    call = __call__
 
 
 class ATSViT(_EngineModel):
@@ -1602,14 +1363,12 @@ class ATSViT(_EngineModel):
         self.max_tokens_per_depth = tuple(int(k) for k in max_tokens_per_depth)
         self._dropout_rates = (dropout, emb_dropout)
         ac = _lib.VbAtsVitConfig()
-        ac.struct_size = C.sizeof(_lib.VbAtsVitConfig)
         for i, k in enumerate(self.max_tokens_per_depth):
             ac.max_tokens_per_depth[i] = k
         self._ac = ac
-        lib = _lib.load()
-        self._create(precision, device, create=lambda cfg, dev, h: lib.vb_create_ats_vit(cfg, C.byref(ac), dev, h),
-                     image_h=image_height, image_w=image_width, patch_h=patch_height, patch_w=patch_width, num_classes=num_classes,
-                     dim=dim, depth=depth, heads=heads, dim_head=dim_head, mlp_dim=mlp_dim)
+        self._create(precision, device, ext=ac, create="vb_create_ats_vit", image_h=image_height, image_w=image_width,
+                     patch_h=patch_height, patch_w=patch_width, num_classes=num_classes, dim=dim, depth=depth, heads=heads,
+                     dim_head=dim_head, mlp_dim=mlp_dim)
         self.init_weights(seed)
 
     def set_sampling_seed(self, seed):
@@ -1662,8 +1421,6 @@ class ATSViT(_EngineModel):
             return _as_tensor(logits), _as_tensor(ids)
         return _as_tensor(logits)
 
-    call = __call__
-
 
 class _MaskedImageModel(_EngineModel):
     """What MAE and SimMIM share: a handle of their own built from the encoder ViT's configuration, the encoder's current weights
@@ -1679,41 +1436,15 @@ class _MaskedImageModel(_EngineModel):
         self._dropout_rates = encoder._dropout_rates
         ec = encoder._cfg
         mc = _lib.VbMimConfig()
-        mc.struct_size = C.sizeof(_lib.VbMimConfig)
         mc.masking_ratio = float(masking_ratio)
         mc.decoder_dim, mc.decoder_depth, mc.decoder_heads, mc.decoder_dim_head = (int(v) for v in decoder)
         self._mc = mc
-        lib = _lib.load()
-        self._create(encoder.precision, encoder.device, create=lambda cfg, dev, h: lib.vb_create_mim(cfg, C.byref(mc), dev, h),
-                     image_h=ec.image_h, image_w=ec.image_w, patch_h=ec.patch_h, patch_w=ec.patch_w, num_classes=ec.num_classes,
-                     dim=ec.dim, depth=ec.depth, heads=ec.heads, dim_head=ec.dim_head, mlp_dim=ec.mlp_dim)
+        self._create(encoder.precision, encoder.device, ext=mc, create="vb_create_mim", image_h=ec.image_h, image_w=ec.image_w,
+                     patch_h=ec.patch_h, patch_w=ec.patch_w, num_classes=ec.num_classes, dim=ec.dim, depth=ec.depth, heads=ec.heads,
+                     dim_head=ec.dim_head, mlp_dim=ec.mlp_dim)
         self._encoder_names = tuple(n for n in self._specs if n in encoder._specs)
         self._pushed = {}
-        self.init_weights(seed)
-
-    def init_weights(self, seed=None):
-        """The reference's initial distributions for the model's own weights (the encoder keeps its own): Dense glorot-uniform /
-        zero bias, LayerNormalization ones / zeros, mask_token tf.random.normal N(0, 1) (mae.py:43, simmim.py:85) and the Embedding
-        uniform(-0.05, 0.05) (Keras' default, mae.py:45)."""
-        rng = np.random.default_rng(seed)
-        w = collections.OrderedDict()
-        for name, shape in self._specs.items():
-            if name in self._encoder_names:
-                continue
-            leaf = name.rsplit(".", 1)[-1]
-            if leaf == "kernel":
-                lim = np.sqrt(6.0 / (shape[0] + shape[1]))
-                a = rng.uniform(-lim, lim, size=shape)
-            elif leaf in ("bias", "beta"):
-                a = np.zeros(shape)
-            elif leaf == "gamma":
-                a = np.ones(shape)
-            elif leaf == "embeddings":
-                a = rng.uniform(-0.05, 0.05, size=shape)
-            else:                                          # mask_token
-                a = rng.standard_normal(shape)
-            w[name] = a.astype(np.float32)
-        self.set_weights_dict(w)
+        self.init_weights(seed)                                         # the model's own weights: the encoder keeps its own
 
     def set_weights_dict(self, weights):
         """The model's own weights (SURVEY.md App. B); the encoder's are set on the encoder and picked up by the next call."""
@@ -1778,8 +1509,6 @@ class _MaskedImageModel(_EngineModel):
         self.forward_raw(x.ctypes.data, _lib.MEM_HOST, b, h, w, loss.ctypes.data, _lib.MEM_HOST)
         return _as_tensor(loss.reshape(()))
 
-    call = __call__
-
 
 class MAE(_MaskedImageModel):
     """mae.py:17-92 (masked autoencoder): the encoder ViT over a random quarter (1 - masking_ratio) of the patches, the decoder
@@ -1837,11 +1566,11 @@ class SmallDatasetViT(_EngineModel):
                      dim=dim, depth=depth, heads=heads, dim_head=dim_head, mlp_dim=mlp_dim, pool=0 if pool == 'cls' else 1)
         self.init_weights(seed)
 
-    def init_weights(self, seed=None):
-        """As the base class, with every layer's temperature at its initial value log(dim_head^-0.5) in float32 (:94)."""
-        super().init_weights(seed)
-        t = np.float32(np.log(np.float32(self.dim_head ** -0.5)))
-        self.set_weights_dict({n: np.array(t, np.float32) for n in self._specs if n.endswith(".temperature")})
+    def _initial_value(self, name, shape, rng):
+        a = super()._initial_value(name, shape, rng)          # a temperature's N(0, 1) draw is made, so later weights keep theirs
+        if name.endswith(".temperature"):                     # log(dim_head^-0.5) in float32 (:94)
+            a = np.full(shape, np.log(np.float32(self.dim_head ** -0.5)))
+        return a
 
 
 class SPT:
@@ -1946,6 +1675,8 @@ class MobileViT(_EngineModel):
     trunk.{s}.1.conv{1,2,3,4}.layers.{0,1}, trunk.{s}.1.transformer.layers.{l}.0.{norm, fn.to_qkv, fn.to_out.0},
     trunk.{s}.1.transformer.layers.{l}.1.{norm, fn.net.0, fn.net.3}, to_logits.0.layers.{0,1}, to_logits.2 (the Dense head)."""
     _kind = "mobilevit"
+    _inference_only = ("MobileViT runs inference only: with training=True (the reference's default, mobile_vit.py:260) every "
+                       "BatchNormalization normalises with the batch's own statistics; pass training=False")
 
     def __init__(self, image_size, dims, channels, num_classes, expansion=4, kernel_size=3, patch_size=(2, 2), depths=(2, 4, 3),
                  *, precision="bf16", device=0, seed=None):
@@ -1961,7 +1692,6 @@ class MobileViT(_EngineModel):
         self.num_classes, self.image_size, self.patch_size = num_classes, (ih, iw), (ph, pw)
         self.blocks = mobilevit_blocks(channels, expansion)
         mc = _lib.VbMobilevitConfig()
-        mc.struct_size = C.sizeof(_lib.VbMobilevitConfig)
         for i in range(10):
             mc.channels[i] = int(channels[i])
         mc.last_dim = int(last_dim)
@@ -1972,18 +1702,9 @@ class MobileViT(_EngineModel):
             mc.mv2_in[i], mc.mv2_hidden[i], mc.mv2_out[i], mc.mv2_stride[i] = cin, hidden, cout, stride
             mc.mv2_expand[i], mc.mv2_residual[i] = int(expand), int(residual)
         self._mc = mc
-        lib = _lib.load()
-        self._create(precision, device, create=lambda cfg, dev, h: lib.vb_create_mobilevit(cfg, C.byref(mc), dev, h),
-                     image_h=ih, image_w=iw, num_classes=num_classes, dim=last_dim)
+        self._create(precision, device, ext=mc, create="vb_create_mobilevit", image_h=ih, image_w=iw, num_classes=num_classes,
+                     dim=last_dim)
         self.init_weights(seed)
-
-    init_weights = CvT.init_weights      # the same initialisers: glorot over the receptive field, zero biases, BatchNorm 1 / 0 / 0 / 1
-
-    def _check_training(self, training):
-        if training is None or training:
-            raise NotImplementedError(
-                "MobileViT runs inference only: with training=True (the reference's default, mobile_vit.py:260) every BatchNormalization "
-                "normalises with the batch's own statistics; pass training=False")
 
     def __call__(self, img, training=True, **kwargs):
         """mobile_vit.py:260-271: NHWC float images -> logits [b, num_classes].  training must be False."""
@@ -1994,8 +1715,6 @@ class MobileViT(_EngineModel):
             if err is not None:
                 raise ValueError(err)
         return super().__call__(img, training=False)
-
-    call = __call__
 
 
 MOBILEVIT_CTOR_KEYS = ("image_size", "dims", "channels", "num_classes", "expansion", "kernel_size", "patch_size", "depths")
@@ -2058,7 +1777,6 @@ class ScalableViT(_EngineModel):
                             for i in range(num_stages))
         self._dropout_rates = (dropout,)
         sc = _lib.VbScalableVitConfig()
-        sc.struct_size = C.sizeof(_lib.VbScalableVitConfig)
         sc.num_stages = num_stages
         sc.ff_expansion_factor = int(ff_expansion_factor)
         for i, st in enumerate(self.stages):
@@ -2069,30 +1787,9 @@ class ScalableViT(_EngineModel):
             if st["window_size"] is not None and sc.window[i] <= 0:
                 raise ValueError(f"ScalableViT stage {i + 1}: window_size must be positive or None")
         self._sc = sc
-        lib = _lib.load()
-        self._create(precision, device, create=lambda cfg, dev, h: lib.vb_create_scalable_vit(cfg, C.byref(sc), dev, h),
-                     channels=channels, num_classes=num_classes, dim=int(dim) << (num_stages - 1))
+        self._create(precision, device, ext=sc, create="vb_create_scalable_vit", channels=channels, num_classes=num_classes,
+                     dim=int(dim) << (num_stages - 1))
         self.init_weights(seed)
-
-    def init_weights(self, seed=None):
-        """The reference's initialisers: glorot-uniform over the receptive field (the PEG's depthwise kernel [3, 3, 1, dim] has fan_in
-        9 and fan_out 9 * dim), zero biases, LayerNorm g / LayerNormalization gamma 1, b / beta 0."""
-        rng = np.random.default_rng(seed)
-        w = collections.OrderedDict()
-        for name, shape in self._specs.items():
-            leaf = name.rsplit(".", 1)[-1]
-            if leaf == "kernel":
-                receptive = int(np.prod(shape[:-2]))
-                lim = np.sqrt(6.0 / (receptive * (shape[-2] + shape[-1])))
-                a = rng.uniform(-lim, lim, size=shape)
-            elif leaf in ("bias", "b", "beta"):
-                a = np.zeros(shape)
-            elif leaf in ("g", "gamma"):
-                a = np.ones(shape)
-            else:
-                raise AssertionError(name)
-            w[name] = a.astype(np.float32)
-        self.set_weights_dict(w)
 
     def __call__(self, img, training=True, **kwargs):
         """scalable_vit.py:308-319: NHWC float images [b, H, W, channels] -> logits [b, num_classes]; extra kwargs are accepted and
@@ -2109,8 +1806,6 @@ class ScalableViT(_EngineModel):
         out = np.empty((b, self.num_classes), np.float32)
         self.forward_raw(x.ctypes.data, _lib.MEM_HOST, b, h, w, out.ctypes.data, _lib.MEM_HOST, None)
         return _as_tensor(out)
-
-    call = __call__
 
 
 SCALABLE_VIT_CTOR_KEYS = ("num_classes", "dim", "depth", "heads", "reduction_factor", "window_size", "iwsa_dim_key", "iwsa_dim_value",
@@ -2165,15 +1860,12 @@ class PiT(_EngineModel):
         self.stages, self.num_patches = stages, side * side
         self._dropout_rates = (dropout, emb_dropout)
         pc = _lib.VbPitConfig()
-        pc.struct_size = C.sizeof(_lib.VbPitConfig)
         pc.stages = len(stages)
         for s, (d, h) in enumerate(stages):
             pc.depth[s], pc.heads[s] = d, h
         self._pc = pc
-        lib = _lib.load()
-        self._create(precision, device, create=lambda cfg, dev, h: lib.vb_create_pit(cfg, C.byref(pc), dev, h), image_h=image_size,
-                     image_w=image_size, patch_h=patch_size, patch_w=patch_size, num_classes=num_classes, dim=dim, dim_head=dim_head,
-                     mlp_dim=mlp_dim)
+        self._create(precision, device, ext=pc, create="vb_create_pit", image_h=image_size, image_w=image_size, patch_h=patch_size,
+                     patch_w=patch_size, num_classes=num_classes, dim=dim, dim_head=dim_head, mlp_dim=mlp_dim)
         self.init_weights(seed)
 
     def __call__(self, img, training=True, **kwargs):
@@ -2193,39 +1885,22 @@ class PiT(_EngineModel):
         self.forward_raw(x.ctypes.data, _lib.MEM_HOST, b, h, w, out.ctypes.data, _lib.MEM_HOST, None)
         return _as_tensor(out)
 
-    call = __call__
-
 
 PIT_CTOR_KEYS = ("image_size", "patch_size", "num_classes", "dim", "depth", "heads", "mlp_dim", "dim_head", "dropout", "emb_dropout")
 
 
+_FAMILY_CTORS = {"pit": (PiT, PIT_CTOR_KEYS), "scalable_vit": (ScalableViT, SCALABLE_VIT_CTOR_KEYS),
+                 "mobilevit": (MobileViT, MOBILEVIT_CTOR_KEYS), "small_dataset_vit": (SmallDatasetViT, SMALL_DATASET_VIT_CTOR_KEYS),
+                 "ats_vit": (ATSViT, ATS_CTOR_KEYS), "regionvit": (RegionViT, REGIONVIT_CTOR_KEYS), "nest": (NesT, NEST_CTOR_KEYS),
+                 "crossformer": (CrossFormer, CROSSFORMER_CTOR_KEYS), "twins_svt": (TwinsSVT, TWINS_CTOR_KEYS),
+                 "cvt": (CvT, CVT_CTOR_KEYS), "levit": (LeViT, LEVIT_CTOR_KEYS), "cct": (CCT, CCT_CTOR_KEYS)}
+
+
 def from_config(cfg: dict, precision="bf16", device=0, seed=None):
     """Build a model from an oracle-style config dict (kind + reference kwargs)."""
-    if cfg["kind"] == "pit":
-        return PiT(**{k: v for k, v in cfg.items() if k in PIT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
-    if cfg["kind"] == "scalable_vit":
-        return ScalableViT(**{k: v for k, v in cfg.items() if k in SCALABLE_VIT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
-    if cfg["kind"] == "mobilevit":
-        return MobileViT(**{k: v for k, v in cfg.items() if k in MOBILEVIT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
-    if cfg["kind"] == "small_dataset_vit":
-        return SmallDatasetViT(**{k: v for k, v in cfg.items() if k in SMALL_DATASET_VIT_CTOR_KEYS}, precision=precision, device=device,
-                               seed=seed)
-    if cfg["kind"] == "ats_vit":
-        return ATSViT(**{k: v for k, v in cfg.items() if k in ATS_CTOR_KEYS}, precision=precision, device=device, seed=seed)
-    if cfg["kind"] == "regionvit":
-        return RegionViT(**{k: v for k, v in cfg.items() if k in REGIONVIT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
-    if cfg["kind"] == "nest":
-        return NesT(**{k: v for k, v in cfg.items() if k in NEST_CTOR_KEYS}, precision=precision, device=device, seed=seed)
-    if cfg["kind"] == "crossformer":
-        return CrossFormer(**{k: v for k, v in cfg.items() if k in CROSSFORMER_CTOR_KEYS}, precision=precision, device=device, seed=seed)
-    if cfg["kind"] == "twins_svt":
-        return TwinsSVT(**{k: v for k, v in cfg.items() if k in TWINS_CTOR_KEYS}, precision=precision, device=device, seed=seed)
-    if cfg["kind"] == "cvt":
-        return CvT(**{k: v for k, v in cfg.items() if k in CVT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
-    if cfg["kind"] == "levit":
-        return LeViT(**{k: v for k, v in cfg.items() if k in LEVIT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
-    if cfg["kind"] == "cct":
-        return CCT(**{k: v for k, v in cfg.items() if k in CCT_CTOR_KEYS}, precision=precision, device=device, seed=seed)
+    if cfg["kind"] in _FAMILY_CTORS:
+        cls, keys = _FAMILY_CTORS[cfg["kind"]]
+        return cls(**{k: v for k, v in cfg.items() if k in keys}, precision=precision, device=device, seed=seed)
     kw = {k: v for k, v in cfg.items() if k not in ("kind", "channels", "image_h", "image_w", "patch_h", "patch_w", "num_patches",
                                                     "patch_merge_layer_index", "t2t_dims")}
     if cfg["kind"] == "patch_merger_vit":
