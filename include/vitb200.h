@@ -19,6 +19,7 @@
  *     ScalableViT(...)(img)          vit_tensorflow/scalable_vit.py:250-319 (vb_create_scalable_vit)
  *     PiT(...)(img)                  vit_tensorflow/pit.py:158-219 (vb_create_pit)
  *     MAE(...)(img) / SimMIM(...)(img)   vit_tensorflow/mae.py:49-92, simmim.py:82-129 (vb_create_mim, vb_forward_mim)
+ *     MPP(...)(img)                      vit_tensorflow/mpp.py:168-218 (vb_create_mim, vb_forward_mpp)
  * and this header is what the Python host classes (vit_tensorflow_b200/models.py, _lib.py) bind with ctypes.
  * Plain pointers and sizes only; no torch / C++ types cross the boundary.
  *
@@ -51,7 +52,7 @@ enum { VB_KIND_VIT = 0, VB_KIND_DEEPVIT = 1, VB_KIND_CAIT = 2, VB_KIND_CROSSVIT 
        VB_KIND_PATCH_MERGER_VIT = 5, VB_KIND_T2T_VIT = 6, VB_KIND_CCT = 7, VB_KIND_LEVIT = 8,
        VB_KIND_CVT = 9, VB_KIND_TWINS_SVT = 10, VB_KIND_CROSSFORMER = 11, VB_KIND_NEST = 12, VB_KIND_REGIONVIT = 13,
        VB_KIND_ATS_VIT = 14, VB_KIND_SMALL_DATASET_VIT = 15, VB_KIND_MOBILEVIT = 16,
-       VB_KIND_SCALABLE_VIT = 17, VB_KIND_PIT = 18, VB_KIND_MAE = 19, VB_KIND_SIMMIM = 20 };
+       VB_KIND_SCALABLE_VIT = 17, VB_KIND_PIT = 18, VB_KIND_MAE = 19, VB_KIND_SIMMIM = 20, VB_KIND_MPP = 21 };
 enum { VB_CCT_POS_SINE = 0, VB_CCT_POS_LEARNABLE = 1, VB_CCT_POS_NONE = 2 };   /* cct.py:233-234,250-256 */
 enum { VB_PRECISION_FP32 = 0, VB_PRECISION_BF16 = 1 };
 enum { VB_POOL_CLS = 0, VB_POOL_MEAN = 1 };
@@ -98,7 +99,7 @@ VB_API int vb_abi_version(void);
 /* Replaces <Model>.__init__ (vit.py:107-157 etc.): validates the config and allocates device state.  VB_KIND_LEVIT, VB_KIND_CVT,
  * VB_KIND_TWINS_SVT, VB_KIND_CROSSFORMER, VB_KIND_NEST and VB_KIND_REGIONVIT are refused here: their handles come from
  * vb_create_levit, vb_create_cvt, vb_create_twins_svt, vb_create_crossformer, vb_create_nest and vb_create_regionvit (and the
- * other extension kinds from their own vb_create_*; VB_KIND_MAE and VB_KIND_SIMMIM from vb_create_mim). */
+ * other extension kinds from their own vb_create_*; VB_KIND_MAE, VB_KIND_SIMMIM and VB_KIND_MPP from vb_create_mim). */
 VB_API int vb_create(const vb_config* cfg, int device, vb_handle** out);
 
 /* LeViT (levit.py:164-212), appended within ABI 7.  `dims`, `depths` and `heads` hold `stages` entries each (cast_tuple already
@@ -488,6 +489,8 @@ VB_API int32_t vb_last_attention_path(void);
  * MAE / SimMIM: the kept-patch gather (patch vectors and position rows) is 3; the patch GEMM 6; the encoder's and decoder's layers
  * as ViT's (0, 1, 5, 6, 2); enc_to_dec and to_pixels 0 (off the wgmma path 4); the mask kernel, the decoder-input assembly, SimMIM's
  * mask-token rows, the row gathers, the pred / masked_patches outputs and the loss reductions 4.
+ * MPP: the corrupted-patch gather is 3; the patch GEMM 6; the encoder's layers as ViT's; to_bits 0 (off the wgmma path 4); the mask
+ * kernel, the corruption draws, the masked-row gather, the outputs and the loss reduction 4.
  * vb_profile_read synchronises the device and returns accumulated milliseconds, algorithmic FLOPs, algorithmic
  * bytes and launch counts per class (arrays of VB_PROF_NUM); reset != 0 clears the accumulators. */
 #define VB_PROF_NUM 7
@@ -799,6 +802,53 @@ VB_API int vb_forward_mim(vb_handle* h, const float* img, int32_t img_mem, int32
 /* The mask kernel on its own: indices int32 [B, n] (host) for the Philox key `seed` and draw counter `counter`; descending = 0
  * MAE's order, 1 SimMIM's.  1 <= n <= VB_MIM_MAX_PATCHES. */
 VB_API int vb_op_mim_mask(int32_t descending, int32_t B, int32_t n, uint64_t seed, uint64_t counter, int32_t* indices);
+
+/* Masked patch prediction (MPP, mpp.py:133-218), appended within ABI 7 on the masked-image-modelling handle: inference semantics
+ * and the loss value.  For an image of n = (h / patch) (w / patch) patches:
+ *   Mask: k = ceil(mask_prob * n) in IEEE double (0.07 * 100 = 7.000000000000001 gives 8); the masked ids are the top_k of the mask
+ *   noise u0 (descending, ties to the smaller id: SimMIM's order and mim_mask's kernel).  k == 0 (the reference's mean over no rows
+ *   is NaN) and k > n are refused.
+ *   Draws: one Philox4x32-10 block per (image, position) with vb_forward_mim's key, counter (j, b, d_lo, d_hi) and per-call d;
+ *   words 0-3 are the mask noise, the random-patch coin, the random patch id and the replace coin (mpp.py:178-196), in that order,
+ *   also when random_patch_prob == 0 (the reference then draws only the mask and the replace coin).  u = (word >> 8) 2^-24; the
+ *   random id is (uint64(word 2) n) >> 32; a coin is u < p in float32, p the double rounded to float32.  The random-patch coin's
+ *   p is random_patch_prob / (1 - replace_prob), drawn only when random_patch_prob > 0 (replace_prob == 1 is then refused, the
+ *   reference's ZeroDivisionError).
+ *   Corruption, per masked position j (the reading of mpp.py:188-197 this engine takes): where the random-patch coin is true the
+ *   pixels of the ORIGINAL patch at the random id (line 191 reads randomized_input before any write); then, where the replace coin
+ *   is true, mask_token (the mask token wins).  Read literally the reference does neither: under TF 2 `.numpy()` returns a copy, so
+ *   the writes at 192 and 197 are lost and the encoder sees the clean image; were they views, line 196's int32 cast would index
+ *   the batch axis with the 0 / 1 mask, overwrite all of images 0 and 1 with the token, and raise IndexError at batch 1.
+ *   Encoder (mpp.py:199-212): row 1 + j = patch.kernel . (corrupted patch j) + patch.bias + pos_embedding[1 + j], row 0 = cls_token +
+ *   pos_embedding[0], the encoder's layers over the n + 1 rows.
+ *   Head and loss (mpp.py:108-131, 213-216): logits = to_bits(the encoded rows of the masked ids, ascending), K = 2^(bits channels)
+ *   classes.  softmax_cross_entropy_with_logits(labels=logits, logits=target [M, 1]) broadcasts the [M, 1] operand to [M, K]
+ *   before its softmax, which is then 1 / K everywhere, so loss = ln(K) * mean over the M = batch k masked rows of sum_c
+ *   logits[row, c]: the targets, clipping, bucketing, max_pixel_val, mean and std do not reach it.  Summed in double in a fixed
+ *   order over the logits as returned. */
+typedef struct vb_mpp_config {
+  vb_mim_config mim;              /* mim.struct_size = sizeof(vb_mpp_config); masking_ratio and the decoder fields unused */
+  double mask_prob;               /* k = ceil(mask_prob * n) */
+  double replace_prob;            /* the mask-token coin's probability */
+  double random_patch_prob;       /* the random-patch coin's probability is random_patch_prob / (1 - replace_prob) */
+  int32_t output_channel_bits;    /* K = 2^(output_channel_bits * channels) <= 2^16; channels must be 3 */
+} vb_mpp_config;
+
+/* MPP.__init__: vb_create_mim with encoder->kind VB_KIND_MPP and `mim` pointing at a vb_mpp_config.  Weights: the encoder ViT's
+ * names WITH cls_token and without head_norm.* / head.* -- pos_embedding [1, n_p + 1, dim], cls_token [1, 1, dim], patch.kernel
+ * [patch_dim, dim] / .bias, layers.L.* -- plus mask_token [patch_dim] (pixel space) and to_bits.kernel [dim, K] / .bias [K]. */
+
+/* One MPP call: img as in vb_forward_mim; loss: one float; logits float32 [batch, k, K] (the masked rows, ids ascending),
+ * mask_ids int32 [batch, k] (ascending), source int32 [batch, n] (j for an unchanged position, the random patch id for a
+ * random-patch one, -1 for the mask token); the three arrays may be NULL; all outputs in out_mem memory.  Graph capture and replay,
+ * the seed (vb_mim_set_seed) and the draw counter as vb_forward_mim's.  Refused: sides not divisible by the patch, more than n_p or
+ * VB_MIM_MAX_PATCHES patches, k == 0 or k > n, replace_prob == 1 with random_patch_prob > 0. */
+VB_API int vb_forward_mpp(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, int32_t img_h, int32_t img_w, float* loss,
+                          float* logits, int32_t* mask_ids, int32_t* source, int32_t out_mem, void* stream);
+/* MPP's draws on their own (mim_mask descending, then the corruption draws) for the key `seed` and draw counter `counter`:
+ * mask_ids int32 [B, k] ascending and source int32 [B, n] (host).  1 <= k <= n <= VB_MIM_MAX_PATCHES. */
+VB_API int vb_op_mpp_draws(int32_t B, int32_t n, int32_t k, double replace_prob, double random_patch_prob, uint64_t seed, uint64_t counter,
+                           int32_t* mask_ids, int32_t* source);
 
 /* Row softmax of fp32 scores into bf16 probabilities (the T2T attention): p[r, j] = softmax_j(s[r, j] * scale) for j < n,
  * p[r, n..npad) = 0.  s [rows, lds], p [rows, ldp] (uploaded and downloaded whole); n <= npad <= ldp. */

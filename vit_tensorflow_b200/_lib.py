@@ -13,7 +13,7 @@ LIB_PATH = os.environ.get("VB_LIB_PATH") or os.path.join(_HERE, "libvitb200.so")
 
 KIND = {"vit": 0, "deepvit": 1, "cait": 2, "crossvit": 3, "parallel_vit": 4, "patch_merger_vit": 5, "t2t_vit": 6, "cct": 7, "levit": 8,
         "cvt": 9, "twins_svt": 10, "crossformer": 11, "nest": 12, "regionvit": 13, "ats_vit": 14,
-        "small_dataset_vit": 15, "mobilevit": 16, "scalable_vit": 17, "pit": 18, "mae": 19, "simmim": 20}
+        "small_dataset_vit": 15, "mobilevit": 16, "scalable_vit": 17, "pit": 18, "mae": 19, "simmim": 20, "mpp": 21}
 PRECISION = {"fp32": 0, "float32": 0, "bf16": 1, "bfloat16": 1}
 MEM_HOST, MEM_DEVICE = 0, 1
 ABI_VERSION = 7                     # VB_ABI_VERSION of include/vitb200.h this binding is written against
@@ -126,6 +126,12 @@ class VbMimConfig(C.Structure):
                 ("decoder_heads", C.c_int32), ("decoder_dim_head", C.c_int32)]
 
 
+class VbMppConfig(VbMimConfig):
+    """vb_mpp_config: a vb_mim_config (its struct_size set to this struct's size) followed by MPP's fields."""
+    _fields_ = [("mask_prob", C.c_double), ("replace_prob", C.c_double), ("random_patch_prob", C.c_double),
+                ("output_channel_bits", C.c_int32)]
+
+
 class VbError(RuntimeError):
     pass
 
@@ -162,6 +168,8 @@ SIGNATURES = {
     "vb_mim_set_seed": (C.c_int, [C.c_void_p, C.c_uint64]),
     "vb_forward_mim": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 4 + [C.c_int32, C.c_void_p]),
     "vb_op_mim_mask": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, C.c_void_p]),
+    "vb_forward_mpp": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 4 + [C.c_int32, C.c_void_p]),
+    "vb_op_mpp_draws": (C.c_int, [C.c_int32] * 3 + [C.c_double, C.c_double, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]),
     "vb_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, _i64p, C.c_int32]),
     "vb_num_weights": (C.c_int, [C.c_void_p]),
     "vb_weight_info": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), _i64p, C.POINTER(C.c_int32)]),
@@ -540,3 +548,12 @@ def op_mim_mask(B, n, seed=0, counter=0, descending=False):
     out = np.zeros((B, n), np.int32)
     check(load().vb_op_mim_mask(int(bool(descending)), B, n, int(seed) & 0xFFFFFFFFFFFFFFFF, int(counter) & 0xFFFFFFFFFFFFFFFF, _ptr(out)))
     return out
+
+
+def op_mpp_draws(B, n, k, replace_prob, random_patch_prob, seed=0, counter=0):
+    """MPP's draws on their own (vb_op_mpp_draws): (mask_ids int32 [B, k] ascending, source int32 [B, n]: j, the random patch id,
+    or -1 for the mask token)."""
+    ids, src = np.empty((B, k), np.int32), np.empty((B, n), np.int32)
+    check(load().vb_op_mpp_draws(B, n, k, float(replace_prob), float(random_patch_prob), int(seed) & 0xFFFFFFFFFFFFFFFF,
+                                 int(counter) & 0xFFFFFFFFFFFFFFFF, _ptr(ids), _ptr(src)))
+    return ids, src

@@ -648,15 +648,21 @@ struct vb_handle {
   // key, draw counter and the mask kernel's completion counter live in mim_rng; mim_dev holds the permutation [B, n] and the
   // pred / masked_patches outputs [B, num_masked, patch_dim] at stable addresses (a new allocation drops the captured graphs).
   vb_mim_config mim{};
+  // MPP (mpp.py:133-218): the encoder ViT with its cls_token, mask_token in pixel space and to_bits (bf16: zero columns up to a
+  // multiple of 64, as the wgmma GEMM takes them).  mim_dev also holds the masked ids [B, n + 1], source [B, n] and logits.
+  vb_mpp_config mpp{};
+  Linear to_bits;
+  int to_bits_ld = 0;
+  int mpp_classes() const { return 1 << (mpp.output_channel_bits * cfg.channels); }
   std::vector<LayerW> dec_layers;
   Linear enc_to_dec, to_pixels;
   bool enc_to_dec_dense = false;
   const float* mask_token = nullptr;
   const float* dec_pos = nullptr;
   DevMem mim_dev, mim_rng;
-  struct MimPlan { int B = 0, n = 0, nm = 0; size_t pred = 0, patches = 0; };
+  struct MimPlan { int B = 0, n = 0, nm = 0; size_t pred = 0, patches = 0, ids = 0, src = 0; };
   MimPlan mim_last;
-  bool is_mim() const { return cfg.kind == VB_KIND_MAE || cfg.kind == VB_KIND_SIMMIM; }
+  bool is_mim() const { return cfg.kind == VB_KIND_MAE || cfg.kind == VB_KIND_SIMMIM || cfg.kind == VB_KIND_MPP; }
   int mim_dim() const { return cfg.kind == VB_KIND_MAE ? mim.decoder_dim : cfg.dim; }    // width of the rows to_pixels reads
   int patch_dim() const { return cfg.patch_h * cfg.patch_w * cfg.channels; }
   unsigned long long* mim_rng_ptr() {
@@ -676,23 +682,43 @@ struct vb_handle {
                                        std::to_string(embed.n_pos - 1));
     VB_CHECK(n <= MIM_MAX_PATCHES, "MAE / SimMIM: the image has " + std::to_string(n) + " patches; the mask kernel takes at most " +
                                        std::to_string(MIM_MAX_PATCHES) + " per image");
-    const int nm = static_cast<int>(mim.masking_ratio * static_cast<double>(n));
-    VB_CHECK(nm >= 1, "MAE / SimMIM: num_masked = int(masking_ratio * " + std::to_string(n) + ") is 0: the loss would be a mean over no "
-                      "patches (NaN in the reference)");
     MimPlan p;
-    p.B = B; p.n = static_cast<int>(n); p.nm = nm;
-    const size_t out = static_cast<size_t>(B) * nm * patch_dim();
-    p.pred = round_up(B * p.n, 64);
-    p.patches = p.pred + out;
+    p.B = B; p.n = static_cast<int>(n);
+    size_t total = 0;
+    if (cfg.kind == VB_KIND_MPP) {
+      // mpp.py:80: math.ceil(prob * seq_len) of a double
+      const double kd = std::ceil(mpp.mask_prob * static_cast<double>(n));
+      VB_CHECK(kd >= 1.0, "MPP: ceil(mask_prob * " + std::to_string(n) + ") is 0: the loss would be a mean over no patches (NaN in the "
+                          "reference)");
+      VB_CHECK(kd <= static_cast<double>(n), "MPP: ceil(mask_prob * " + std::to_string(n) + ") masks more patches than the image has");
+      VB_CHECK(!(mpp.random_patch_prob > 0.0 && mpp.replace_prob == 1.0),
+               "MPP: random_patch_prob / (1 - replace_prob) divides by zero (ZeroDivisionError in the reference)");
+      p.nm = static_cast<int>(kd);
+      p.ids = round_up(B * p.n, 64);                                     // after the top_k permutation [B, n]
+      p.src = p.ids + round_up(static_cast<size_t>(B) * (p.n + 1), 64);  // masked ids at pitch n + 1
+      p.pred = p.src + round_up(static_cast<size_t>(B) * p.n, 64);         // logits [B, k, K]
+      total = p.pred + static_cast<size_t>(B) * p.nm * mpp_classes();
+    } else {
+      const int nm = static_cast<int>(mim.masking_ratio * static_cast<double>(n));
+      VB_CHECK(nm >= 1, "MAE / SimMIM: num_masked = int(masking_ratio * " + std::to_string(n) + ") is 0: the loss would be a mean over no "
+                        "patches (NaN in the reference)");
+      p.nm = nm;
+      const size_t out = static_cast<size_t>(B) * nm * patch_dim();
+      p.pred = round_up(B * p.n, 64);
+      p.patches = p.pred + out;
+      total = p.patches + out;
+    }
     mim_last = p;
     const void* before = mim_dev.p;
-    mim_dev.ensure((p.patches + out) * sizeof(float));
+    mim_dev.ensure(total * sizeof(float));
     if (before != nullptr && mim_dev.p != before) drop_graphs();
     mim_rng_ptr();
   }
   int* mim_idx() const { return static_cast<int*>(mim_dev.p); }
   float* mim_pred() const { return static_cast<float*>(mim_dev.p) + mim_last.pred; }
   float* mim_patches() const { return static_cast<float*>(mim_dev.p) + mim_last.patches; }
+  int* mpp_ids() const { return static_cast<int*>(mim_dev.p) + mim_last.ids; }
+  int* mpp_src() const { return static_cast<int*>(mim_dev.p) + mim_last.src; }
   Norm head_norm, sm_head_norm, lg_head_norm;
   Linear head, sm_head, lg_head;
   Norm spt_norm;                     // SPT's LayerNorm over the p^2 * 5 C patch vector (bf16: padded to the GEMM's K, folded into it)
@@ -799,6 +825,14 @@ struct vb_handle {
         expect("decoder_pos_emb.embeddings", {np + 1, Dd});                            // Embedding(num_patches, decoder_dim) :45
       }
       expect_dense("to_pixels", Dd, pd);                                               // mae.py:46, simmim.py:86
+    } else if (c.kind == VB_KIND_MPP) {                                 // the encoder ViT without mlp_head (mpp.py:149-166, 199-213)
+      const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w), pd = patch_dim();
+      expect("pos_embedding", {1, np + 1, c.dim});
+      expect("cls_token", {1, 1, c.dim});
+      expect_dense("patch", pd, c.dim);
+      for (int L = 0; L < c.depth; ++L) expect_layer("layers." + std::to_string(L) + ".", c.dim, c.heads, c.dim_head, c.mlp_dim, VB_KIND_VIT);
+      expect("mask_token", {pd});                                        // tf.random.normal([1, 1, channels * patch_size ** 2]) :166
+      expect_dense("to_bits", c.dim, mpp_classes());                     // Dense(2 ** (output_channel_bits * channels)) :155
     } else if (c.kind == VB_KIND_SMALL_DATASET_VIT) {                   // vit_for_small_dataset.py:142-195
       const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w), K = c.patch_h * c.patch_w * 5 * C;
       expect("pos_embedding", {1, np + 1, c.dim});
@@ -1384,6 +1418,13 @@ struct vb_handle {
         dec_pos = W("decoder_pos_emb.embeddings");
       }
       to_pixels = make_linear("to_pixels", Dd, patch_dim());
+    } else if (c.kind == VB_KIND_MPP) {
+      const int np = (c.image_h / c.patch_h) * (c.image_w / c.patch_w), K = mpp_classes();
+      embed = make_embed("", c.patch_h, c.patch_w, c.dim, np + 1);
+      for (int L = 0; L < c.depth; ++L) layers.push_back(make_layer("layers." + std::to_string(L) + ".", c.dim, c.heads, c.dim_head, c.mlp_dim, VB_KIND_VIT));
+      mask_token = W("mask_token");
+      to_bits_ld = bf16() ? round_up(K, 64) : K;
+      to_bits = to_bits_ld == K ? make_linear("to_bits", c.dim, K) : padded_dense("to_bits.padded", "to_bits", c.dim, K, c.dim, to_bits_ld);
     } else if (c.kind == VB_KIND_SMALL_DATASET_VIT) {
       finalize_small_dataset_vit();
     } else if (c.kind == VB_KIND_PATCH_MERGER_VIT) {
@@ -3690,6 +3731,69 @@ struct vb_handle {
     }
   }
 
+  // MPP.call (mpp.py:168-218) as mim_prepare planned it, writing the loss to `loss` (device) and, when `want_logits`, the logits of
+  // the masked rows to mim_pred().  The mask and the corruption draws come from the device's own counter; every step after them is a
+  // fixed launch sequence.
+  template <typename T>
+  void mpp_forward(const float* img, int B, int H, int Wd, float* loss, bool want_logits, cudaStream_t s) {
+    const vb_config& c = cfg;
+    const MimPlan& p = mim_last;
+    VB_CHECK(p.B == B && p.n == (H / c.patch_h) * (Wd / c.patch_w) && mim_dev.p != nullptr, "internal: MPP state not prepared for this batch");
+    arena.reset();
+    const int n = p.n, k = p.nm, rows = n + 1, dim = c.dim, pd = patch_dim(), K = mpp_classes();
+    int* idx = mim_idx();
+    {
+      ProfScope ps(this, PROF_OTHER, 0.0, 4.0 * B * n, s);
+      mim_mask(B, n, 1, mim_rng_ptr(), idx, s);                       // mpp.py:78-88: the top_k of the noise
+    }
+    {
+      ProfScope ps(this, PROF_OTHER, 0.0, 4.0 * B * (n + k + n), s);
+      const double p_rand = mpp.random_patch_prob > 0.0 ? mpp.random_patch_prob / (1.0 - mpp.replace_prob) : 0.0;   // mpp.py:185
+      mpp_draws(B, n, k, idx, mim_rng_ptr(), mpp.random_patch_prob, p_rand, mpp.replace_prob, mpp_src(), mpp_ids(), rows, s);
+    }
+    // the patch Dense of the corrupted patches with cls and positions in its residual operand (mpp.py:199-208)
+    const int M = B * rows, Kp = bf16() ? embed.patch.ldw : embed.patch.K;
+    T* col = arena.get<T>(static_cast<size_t>(M) * Kp);
+    T* R = arena.get<T>(static_cast<size_t>(M) * dim);
+    {
+      ProfScope ps(this, PROF_EMBED, 0.0, 4.0 * M * pd + static_cast<double>(sizeof(T)) * M * (Kp + dim), s);
+      mim_patch_rows<T>(img, B, H, Wd, c.channels, c.patch_h, c.patch_w, nullptr, n, 0, rows, col, Kp, embed.pos, R, dim, s, mpp_src(),
+                        mask_token, embed.cls, embed.patch.bias);
+    }
+    T* X = arena.get<T>(static_cast<size_t>(M) * dim);
+    float* stats = nullptr;
+    {
+      Epi ep; ep.bias = embed.patch.bias; ep.res = R; ep.ldr = dim;
+      if (bf16() && dim % 64 == 0) { stats = row_stats(M, dim); ep.stats_out = stats; }
+      Linear L = embed.patch;
+      L.K = Kp;
+      linear<T>(col, Kp, M, L, X, dim, ep, s);
+    }
+    bool sv = stats != nullptr;
+    for (const auto& l : layers) layer_self<T>(X, B, rows, dim, l, s, stats, &sv);
+    // to_bits on the masked rows only, ids ascending (predicted_patches[mask], mpp.py:128)
+    const long long Mk = static_cast<long long>(B) * k;
+    T* Xm = arena.get<T>(static_cast<size_t>(Mk) * dim);
+    {
+      ProfScope ps(this, PROF_OTHER, 0.0, 2.0 * sizeof(T) * Mk * dim, s);
+      mim_take_rows<T>(X + dim, rows, mpp_ids(), Xm, B, k, dim, s);   // row 1 + j of each image, the ids at pitch n + 1
+    }
+    T* Lg = arena.get<T>(static_cast<size_t>(Mk) * to_bits_ld);
+    {
+      Epi e; e.bias = to_bits.bias;
+      linear<T>(Xm, dim, static_cast<int>(Mk), to_bits, Lg, to_bits_ld, e, s);
+    }
+    double* partial = arena.get<double>(static_cast<size_t>(mim_loss_blocks(Mk)));
+    {
+      ProfScope ps(this, PROF_OTHER, static_cast<double>(Mk) * K, static_cast<double>(sizeof(T)) * Mk * K, s);
+      mpp_loss<T>(Lg, to_bits_ld, K, Mk, partial, loss, s);
+    }
+    if (want_logits) {
+      ProfScope ps(this, PROF_OTHER, 0.0, (static_cast<double>(sizeof(T)) + 4.0) * Mk * K, s);
+      convert_rows<T, float>(Lg, to_bits_ld, mim_pred(), K, Mk, K, s);
+    }
+  }
+
   // DistillMixin.call (distill.py:16-45) on top of a ViT or a T2TViT: embed (the patch Dense, or T2T's soft splits and their
   // one-layer transformers, as vb_forward runs them) -> append the distillation token as the LAST row -> transformer over
   // n + 2 rows -> head on the first n + 1 rows, and the last row returned as is.
@@ -3760,6 +3864,7 @@ struct vb_handle {
       case VB_KIND_PIT: return "PiT runs as a whole forward only: it has no `transformer` attribute, so its patch-embedding / stage / head steps have no entry of their own";
       case VB_KIND_MAE: return "MAE runs through vb_forward_mim only: its encoder and decoder steps have no entry of their own";
       case VB_KIND_SIMMIM: return "SimMIM runs through vb_forward_mim only: its encoder steps have no entry of their own";
+      case VB_KIND_MPP: return "MPP runs through vb_forward_mpp only: its encoder steps have no entry of their own";
       default: return nullptr;
     }
   }
@@ -3999,6 +4104,7 @@ void validate(const vb_config& c) {
   VB_CHECK(c.kind != VB_KIND_PIT, "PiT: create the handle with vb_create_pit (its stages' depths and heads are a vb_pit_config)");
   VB_CHECK(c.kind != VB_KIND_MAE, "MAE: create the handle with vb_create_mim (its masking ratio and decoder are a vb_mim_config)");
   VB_CHECK(c.kind != VB_KIND_SIMMIM, "SimMIM: create the handle with vb_create_mim (its masking ratio is a vb_mim_config)");
+  VB_CHECK(c.kind != VB_KIND_MPP, "MPP: create the handle with vb_create_mim (its probabilities and bits are a vb_mpp_config)");
   VB_CHECK((c.kind >= VB_KIND_VIT && c.kind <= VB_KIND_CCT) || c.kind == VB_KIND_SMALL_DATASET_VIT, "unknown model kind");
   if (c.kind == VB_KIND_SMALL_DATASET_VIT) {
     // SPT's Rearrange takes one patch size for both sides (vit_for_small_dataset.py:147) and shift() one image of 3 channels
@@ -4138,6 +4244,19 @@ void validate_mim(const vb_config& c, const vb_mim_config& m) {
     VB_CHECK(m.decoder_dim > 0 && m.decoder_depth >= 0 && m.decoder_heads > 0 && m.decoder_dim_head > 0, "MAE: bad decoder dimensions");
     VB_CHECK(m.decoder_heads <= 32, "MAE: at most 32 decoder heads");
   }
+}
+
+// mpp.py's constructor arguments the engine takes: channels 3 (its Bucketize / bin_mask read three channels), at most 2^16 classes
+void validate_mpp(const vb_config& c, const vb_mpp_config& m) {
+  vb_config v = c;
+  v.kind = VB_KIND_VIT;
+  v.pool = VB_POOL_CLS;
+  v.num_classes = 1;
+  validate(v);
+  VB_CHECK(c.channels == 3, "MPP: images of 3 channels");
+  VB_CHECK(m.output_channel_bits >= 1 && m.output_channel_bits * c.channels <= 16,
+           "MPP: output_channel_bits * channels must be 1 to 16 (to_bits has 2^(bits * channels) classes)");
+  VB_CHECK(std::isfinite(m.mask_prob) && std::isfinite(m.replace_prob) && std::isfinite(m.random_patch_prob), "MPP: probabilities must be finite");
 }
 
 void validate_regionvit(const vb_config& c, const vb_regionvit_config& r) {
@@ -4315,6 +4434,9 @@ void staged_call(vb_handle* h, const float* in, int32_t in_mem, size_t in_bytes,
     VB_CUDA(cudaStreamSynchronize(s));
   }
 }
+// an extension config's struct_size: its first field, or (vb_mpp_config) that of the vb_mim_config it begins with
+template <typename Ext> int32_t ext_struct_size(const Ext& e) { return e.struct_size; }
+int32_t ext_struct_size(const vb_mpp_config& e) { return e.mim.struct_size; }
 // vb_create_<kind> for the kinds whose stages come in an extension config: `fn` and `ext_name` name the entry point and the
 // config struct in the messages; `validate` checks the config against the base, `adopt` stores it in the handle and sets cfg.dim.
 template <typename Ext, typename Validate, typename Adopt>
@@ -4325,7 +4447,7 @@ int create_with(const char* fn, const char* ext_name, int kind, const char* kind
     VB_CHECK(base != nullptr && ext != nullptr && out != nullptr, f + ": null argument");
     VB_CHECK(base->struct_size == static_cast<int32_t>(sizeof(vb_config)) || base->struct_size == VB_CONFIG_SIZE_ABI7,
              "vb_config.struct_size mismatch (ABI)");
-    VB_CHECK(ext->struct_size == static_cast<int32_t>(sizeof(Ext)), std::string(ext_name) + ".struct_size mismatch (ABI)");
+    VB_CHECK(ext_struct_size(*ext) == static_cast<int32_t>(sizeof(Ext)), std::string(ext_name) + ".struct_size mismatch (ABI)");
     vb_config c;
     memset(&c, 0, sizeof c);
     memcpy(&c, base, static_cast<size_t>(base->struct_size));
@@ -4665,9 +4787,15 @@ int vb_create_pit(const vb_config* base, const vb_pit_config* pc, int device, vb
 int vb_create_mim(const vb_config* encoder, const vb_mim_config* mc, int device, vb_handle** out) {
   const int rc = guarded(nullptr, [&] {
     VB_CHECK(encoder != nullptr && mc != nullptr && out != nullptr, "vb_create_mim: null argument");
-    VB_CHECK(encoder->kind == VB_KIND_MAE || encoder->kind == VB_KIND_SIMMIM, "vb_create_mim: encoder.kind must be VB_KIND_MAE or VB_KIND_SIMMIM");
+    VB_CHECK(encoder->kind == VB_KIND_MAE || encoder->kind == VB_KIND_SIMMIM || encoder->kind == VB_KIND_MPP,
+             "vb_create_mim: encoder.kind must be VB_KIND_MAE or VB_KIND_SIMMIM (or VB_KIND_MPP)");
   });
   if (rc != 0) return rc;
+  if (encoder->kind == VB_KIND_MPP) {                    // the vb_mpp_config begins with the vb_mim_config whose struct_size it sets
+    const vb_mpp_config* mp = reinterpret_cast<const vb_mpp_config*>(mc);
+    return create_with("vb_create_mim", "vb_mpp_config", VB_KIND_MPP, "VB_KIND_MPP", encoder, mp, device, out, validate_mpp,
+                       [&](vb_handle& h) { h.mpp = *mp; h.mim = mp->mim; h.cfg.pool = VB_POOL_CLS; });
+  }
   return create_with("vb_create_mim", "vb_mim_config", encoder->kind, encoder->kind == VB_KIND_MAE ? "VB_KIND_MAE" : "VB_KIND_SIMMIM", encoder,
                      mc, device, out, validate_mim, [&](vb_handle& h) { h.mim = *mc; h.cfg.pool = VB_POOL_CLS; });
 }
@@ -4675,7 +4803,7 @@ int vb_create_mim(const vb_config* encoder, const vb_mim_config* mc, int device,
 int vb_mim_set_seed(vb_handle* h, uint64_t seed) {
   return guarded(h, [&] {
     VB_CHECK(h != nullptr, "null handle");
-    VB_CHECK(h->is_mim(), "vb_mim_set_seed: not a MAE / SimMIM handle");
+    VB_CHECK(h->is_mim(), "vb_mim_set_seed: not a MAE / SimMIM / MPP handle");
     VB_CUDA(cudaSetDevice(h->device));
     VB_CUDA(cudaDeviceSynchronize());                  // no forward in flight reads the old key and counter
     const unsigned long long v[3] = {static_cast<unsigned long long>(seed), 0ull, 0ull};
@@ -4688,7 +4816,7 @@ int vb_forward_mim(vb_handle* h, const float* img, int32_t img_mem, int32_t batc
                    float* masked_patches, int32_t* indices, int32_t out_mem, void* stream) {
   return guarded(h, [&] {
     VB_CHECK(h != nullptr && img != nullptr && loss != nullptr, "vb_forward_mim: null argument");
-    VB_CHECK(h->is_mim(), "vb_forward_mim: not a MAE / SimMIM handle");
+    VB_CHECK(h->is_mim() && h->cfg.kind != VB_KIND_MPP, "vb_forward_mim: not a MAE / SimMIM handle (MPP runs through vb_forward_mpp)");
     VB_CHECK(h->finalized, "vb_forward_mim: call vb_finalize after setting the weights");
     VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_forward_mim: bad batch / image size");
     VB_CUDA(cudaSetDevice(h->device));
@@ -4744,6 +4872,76 @@ int vb_op_mim_mask(int32_t descending, int32_t B, int32_t n, uint64_t seed, uint
     unsigned long long after[3];
     VB_CUDA(cudaMemcpy(after, rng.p, sizeof after, cudaMemcpyDeviceToHost));
     VB_CHECK(after[1] == counter + 1 && after[2] == 0, "vb_op_mim_mask: the mask kernel did not advance its counter once");
+  });
+}
+
+int vb_forward_mpp(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, int32_t img_h, int32_t img_w, float* loss, float* logits,
+                   int32_t* mask_ids, int32_t* source, int32_t out_mem, void* stream) {
+  return guarded(h, [&] {
+    VB_CHECK(h != nullptr && img != nullptr && loss != nullptr, "vb_forward_mpp: null argument");
+    VB_CHECK(h->cfg.kind == VB_KIND_MPP, "vb_forward_mpp: not a MPP handle");
+    VB_CHECK(h->finalized, "vb_forward_mpp: call vb_finalize after setting the weights");
+    VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_forward_mpp: bad batch / image size");
+    VB_CUDA(cudaSetDevice(h->device));
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const long long before = launch_counter();
+    const size_t img_bytes = static_cast<size_t>(batch) * img_h * img_w * h->cfg.channels * sizeof(float);
+    const float* img_d = img;
+    if (img_mem == VB_MEM_HOST) {
+      h->img_dev.ensure(img_bytes);
+      VB_CUDA(cudaMemcpyAsync(h->img_dev.p, img, img_bytes, cudaMemcpyHostToDevice, s));
+      img_d = static_cast<const float*>(h->img_dev.p);
+    }
+    float* loss_d = loss;
+    if (out_mem == VB_MEM_HOST) {
+      h->logits_dev.ensure(sizeof(float));
+      loss_d = static_cast<float*>(h->logits_dev.p);
+    }
+    h->mim_prepare(batch, img_h, img_w);
+    const bool want_logits = logits != nullptr;
+    vb_handle::GraphKey key{img_d, loss_d, batch, img_h, img_w, s};
+    key.flags = want_logits ? 1 : 0;
+    run_graphed(h, key, [&] {
+      if (h->bf16()) h->mpp_forward<__nv_bfloat16>(img_d, batch, img_h, img_w, loss_d, want_logits, s);
+      else h->mpp_forward<float>(img_d, batch, img_h, img_w, loss_d, want_logits, s);
+    });
+    h->last_launches = launch_counter() - before;
+    const vb_handle::MimPlan& p = h->mim_last;
+    const cudaMemcpyKind kind = out_mem == VB_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+    if (logits != nullptr)
+      VB_CUDA(cudaMemcpyAsync(logits, h->mim_pred(), static_cast<size_t>(batch) * p.nm * h->mpp_classes() * sizeof(float), kind, s));
+    if (mask_ids != nullptr)
+      VB_CUDA(cudaMemcpy2DAsync(mask_ids, static_cast<size_t>(p.nm) * sizeof(int), h->mpp_ids(), static_cast<size_t>(p.n + 1) * sizeof(int),
+                                static_cast<size_t>(p.nm) * sizeof(int), batch, kind, s));
+    if (source != nullptr) VB_CUDA(cudaMemcpyAsync(source, h->mpp_src(), static_cast<size_t>(batch) * p.n * sizeof(int), kind, s));
+    if (out_mem == VB_MEM_HOST) {
+      VB_CUDA(cudaMemcpyAsync(loss, loss_d, sizeof(float), cudaMemcpyDeviceToHost, s));
+      VB_CUDA(cudaStreamSynchronize(s));
+    }
+  });
+}
+
+int vb_op_mpp_draws(int32_t B, int32_t n, int32_t k, double replace_prob, double random_patch_prob, uint64_t seed, uint64_t counter,
+                    int32_t* mask_ids, int32_t* source) {
+  return guarded(nullptr, [&] {
+    VB_CHECK(mask_ids != nullptr && source != nullptr && B > 0, "vb_op_mpp_draws: bad arguments");
+    VB_CHECK(n >= 1 && n <= MIM_MAX_PATCHES && k >= 1 && k <= n, "vb_op_mpp_draws: need 1 <= k <= n <= " + std::to_string(MIM_MAX_PATCHES));
+    VB_CHECK(!(random_patch_prob > 0.0 && replace_prob == 1.0), "vb_op_mpp_draws: random_patch_prob / (1 - replace_prob) divides by zero");
+    require_gpu();
+    DevMem rng, idx, ids, src;
+    rng.ensure(3 * sizeof(unsigned long long));
+    const unsigned long long v[3] = {static_cast<unsigned long long>(seed), static_cast<unsigned long long>(counter), 0ull};
+    VB_CUDA(cudaMemcpy(rng.p, v, sizeof v, cudaMemcpyHostToDevice));
+    idx.ensure(static_cast<size_t>(B) * n * sizeof(int));
+    ids.ensure(static_cast<size_t>(B) * k * sizeof(int));
+    src.ensure(static_cast<size_t>(B) * n * sizeof(int));
+    unsigned long long* r = static_cast<unsigned long long*>(rng.p);
+    mim_mask(B, n, 1, r, static_cast<int*>(idx.p), 0);
+    const double p_rand = random_patch_prob > 0.0 ? random_patch_prob / (1.0 - replace_prob) : 0.0;
+    mpp_draws(B, n, k, static_cast<const int*>(idx.p), r, random_patch_prob, p_rand, replace_prob, static_cast<int*>(src.p),
+              static_cast<int*>(ids.p), k, 0);
+    VB_CUDA(cudaMemcpy(mask_ids, ids.p, static_cast<size_t>(B) * k * sizeof(int), cudaMemcpyDeviceToHost));
+    VB_CUDA(cudaMemcpy(source, src.p, static_cast<size_t>(B) * n * sizeof(int), cudaMemcpyDeviceToHost));
   });
 }
 

@@ -228,9 +228,22 @@ constexpr int MIM_MAX_PATCHES = 4096;    // patches per image the mask kernel so
 void mim_mask(int B, int n, int descending, unsigned long long* rng, int* idx, cudaStream_t s);
 // out [B * count, ldo]: row b * count + i = the (p1, p2, c) patch vector of id j = idx[b * n + off + i] (idx null: j = i) read from
 // the NHWC image, columns [ph pw C, ldo) zero; R (may be null) [B * count, dim]: pos[1 + j] (pos_embedding [np + 1, dim]).
+// MPP (cls non-null, idx null, count = n + 1): row 0 of each image is the cls row (zero, R = pos[0] + cls - bias) and row 1 + j
+// takes the pixels of patch src[b * n + j], or mask_row [ph pw C] where that is -1, with R = pos[1 + j].
 template <typename T>
 void mim_patch_rows(const float* img, int B, int H, int W, int C, int ph, int pw, const int* idx, int n, int off, int count, T* out, int ldo,
-                    const float* pos, T* R, int dim, cudaStream_t s);
+                    const float* pos, T* R, int dim, cudaStream_t s, const int* src = nullptr, const float* mask_row = nullptr,
+                    const float* cls = nullptr, const float* bias = nullptr);
+// MPP's corruption draws (mpp.py:181-197) after mim_mask (descending) drew the call's mask into idx: source [B, n] (j, the random
+// patch id, or -1 for the mask token) and mask_ids [B, ldm] (the first k ids of idx, ascending), from words 1-3 of the Philox
+// block mim_mask used (counter rng[1] - 1).  p_rand = random_patch_prob / (1 - replace_prob); the random-patch coin is drawn only
+// when random_patch_prob > 0.
+void mpp_draws(int B, int n, int k, const int* idx, const unsigned long long* rng, double random_patch_prob, double p_rand,
+               double replace_prob, int* source, int* mask_ids, int ldm, cudaStream_t s);
+// *loss = ln(K) * (sum of logits [rows, ldl] over the columns [0, K)) / rows, a fixed-order reduction in double as mim_loss's
+// (partial: mim_loss_blocks(rows) doubles)
+template <typename T>
+void mpp_loss(const T* logits, int ldl, int K, long long rows, double* partial, float* loss, cudaStream_t s);
 // Z [B * n, D]: image b's row t < nm = mask_token + dpe[idx[b, t]], row t >= nm = E[b (n - nm) + t - nm] + dpe[idx[b, t]]
 template <typename T>
 void mim_decoder_rows(const T* E, const int* idx, int B, int n, int nm, const float* mask_token, const float* dpe, T* Z, int D, cudaStream_t s);

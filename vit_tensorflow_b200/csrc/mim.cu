@@ -14,6 +14,7 @@ template <> __device__ __forceinline__ float mim_f<__nv_bfloat16>(__nv_bfloat16 
 constexpr int MIM_MASK_THREADS = 1024;
 constexpr int MIM_LOSS_THREADS = 256;
 constexpr int MIM_LOSS_BLOCKS = 1024;
+constexpr int MPP_DRAW_THREADS = 256;
 
 // One CTA per image: u[b, j] = (Philox4x32-10 word 0 >> 8) for j < n with counter (j, b, d_lo, d_hi), sorted as the 64-bit keys
 // (u << 32 | j) ascending (MAE's stable argsort) or ((2^24 - 1 - u) << 32 | j) ascending (SimMIM's top_k: u descending, ties to
@@ -64,23 +65,36 @@ mim_mask_kernel(int n, int descending, unsigned long long* rng, unsigned int* do
 }
 
 // Row r = b * count + i of `out` [B * count, ldo]: the (p1, p2, c) vector of patch j = idx[b * n + off + i] (j = i without idx),
-// zero in the columns [pd, ldo); with R, R row r = pos[1 + j] (the patch GEMM's residual operand).
-template <typename T>
+// zero in the columns [pd, ldo); with R, R row r = pos[1 + j] (the patch GEMM's residual operand).  MPP's corrupted rows (cls
+// non-null): each image's row 0 is the cls row (A zero, R = pos[0] + cls - bias, which the GEMM's bias completes to cls + pos[0],
+// as the ViT embedding's residual does); row 1 + j reads its pixels from patch src[b * n + j] rather than j, or mask_row where
+// that is -1, and keeps R = pos[1 + j].  MPP is a template flag, so MAE's and SimMIM's instances carry none of its branches.
+template <typename T, bool MPP>
 __global__ void __launch_bounds__(128)
 mim_patch_rows_kernel(const float* __restrict__ img, int H, int W, int C, int ph, int pw, const int* __restrict__ idx, int n, int off,
-                      int count, T* __restrict__ out, int ldo, const float* __restrict__ pos, T* __restrict__ R, int dim, long long rows) {
+                      int count, T* __restrict__ out, int ldo, const float* __restrict__ pos, T* __restrict__ R, int dim, long long rows,
+                      const int* __restrict__ src, const float* __restrict__ mask_row, const float* __restrict__ cls,
+                      const float* __restrict__ bias) {
   const int pd = ph * pw * C, gw = W / pw;
   for (long long r = blockIdx.x; r < rows; r += gridDim.x) {
     const int b = static_cast<int>(r / count), i = static_cast<int>(r % count);
-    const int j = idx != nullptr ? idx[static_cast<size_t>(b) * n + off + i] : i;
-    const int gy = j / gw, gx = j % gw;
-    const float* base = img + ((static_cast<size_t>(b) * H + static_cast<size_t>(gy) * ph) * W + static_cast<size_t>(gx) * pw) * C;
     T* o = out + r * ldo;
+    if (MPP && i == 0) {
+      for (int e = threadIdx.x; e < ldo; e += blockDim.x) o[e] = T(0.f);
+      T* rr = R + r * dim;
+      for (int e = threadIdx.x; e < dim; e += blockDim.x) rr[e] = T(pos[e] + cls[e] - bias[e]);
+      continue;
+    }
+    const int t = MPP ? i - 1 : i;
+    const int j = idx != nullptr ? idx[static_cast<size_t>(b) * n + off + t] : t;
+    const int sj = MPP ? src[static_cast<size_t>(b) * n + j] : j;
+    const int gy = sj / gw, gx = sj % gw;
+    const float* base = img + ((static_cast<size_t>(b) * H + static_cast<size_t>(gy) * ph) * W + static_cast<size_t>(gx) * pw) * C;
     for (int e = threadIdx.x; e < ldo; e += blockDim.x) {
       float v = 0.f;
       if (e < pd) {
         const int p1 = e / (pw * C), rem = e - p1 * pw * C;
-        v = base[static_cast<size_t>(p1) * W * C + rem];     // rem = p2 * C + c: contiguous along the image row
+        v = MPP && sj < 0 ? mask_row[e] : base[static_cast<size_t>(p1) * W * C + rem];   // rem = p2 * C + c: contiguous along the image row
       }
       o[e] = T(v);
     }
@@ -89,6 +103,48 @@ mim_patch_rows_kernel(const float* __restrict__ img, int H, int W, int C, int ph
       T* rr = R + r * dim;
       for (int e = threadIdx.x; e < dim; e += blockDim.x) rr[e] = T(pr[e]);
     }
+  }
+}
+
+// MPP's corruption draws (mpp.py:178-197), one CTA per image, after mim_mask_kernel drew this call's mask at counter d = rng[1] - 1
+// (it has advanced rng[1] since).  The first k ids of idx (the top_k) become a bitmap.  Per masked position j, words 1-3 of
+// Philox4x32-10 at counter (j, b, d_lo, d_hi) give the random-patch coin u1 < p_rand (when use_rand), the random id
+// (word 2 * n) >> 32 and the replace coin u3 < p_repl, with u = (word >> 8) 2^-24 compared in float32.  source[b, j] is j, the
+// random id where the random-patch coin is true, or -1 (the mask token) where the replace coin is true.  mask_ids[b * ldm + i],
+// i < k: the masked ids ascending (the order of predicted_patches[mask]).
+__global__ void __launch_bounds__(MPP_DRAW_THREADS)
+mpp_draws_kernel(int n, int k, const int* __restrict__ idx, const unsigned long long* __restrict__ rng, int use_rand, float p_rand,
+                 float p_repl, int* __restrict__ source, int* __restrict__ mask_ids, int ldm) {
+  constexpr int WORDS = MIM_MAX_PATCHES / 32;
+  __shared__ uint32_t bits[WORDS];
+  __shared__ int before[WORDS];
+  const int b = blockIdx.x, tid = threadIdx.x, nw = (n + 31) / 32;
+  for (int w = tid; w < WORDS; w += MPP_DRAW_THREADS) bits[w] = 0u;
+  __syncthreads();
+  for (int i = tid; i < k; i += MPP_DRAW_THREADS) {
+    const int j = idx[static_cast<size_t>(b) * n + i];
+    atomicOr(&bits[j >> 5], 1u << (j & 31));
+  }
+  __syncthreads();
+  if (tid == 0) {
+    int run = 0;
+    for (int w = 0; w < nw; ++w) { before[w] = run; run += __popc(bits[w]); }
+  }
+  __syncthreads();
+  const uint32_t k0 = static_cast<uint32_t>(rng[0]), k1 = static_cast<uint32_t>(rng[0] >> 32);
+  const unsigned long long d = rng[1] - 1ull;
+  for (int j = tid; j < n; j += MPP_DRAW_THREADS) {
+    const uint32_t word = bits[j >> 5], bit = 1u << (j & 31);
+    int s = j;
+    if (word & bit) {
+      const uint4 x = philox4x32_10(make_uint4(static_cast<uint32_t>(j), static_cast<uint32_t>(b), static_cast<uint32_t>(d),
+                                               static_cast<uint32_t>(d >> 32)), k0, k1);
+      const float u1 = static_cast<float>(x.y >> 8) * 0x1p-24f, u3 = static_cast<float>(x.w >> 8) * 0x1p-24f;
+      if (use_rand && u1 < p_rand) s = static_cast<int>((static_cast<unsigned long long>(x.z) * static_cast<unsigned>(n)) >> 32);
+      if (u3 < p_repl) s = -1;
+      mask_ids[static_cast<size_t>(b) * ldm + before[j >> 5] + __popc(word & (bit - 1u))] = j;
+    }
+    source[static_cast<size_t>(b) * n + j] = s;
   }
 }
 
@@ -185,6 +241,20 @@ mim_loss_final_kernel(const double* __restrict__ partial, int G, double scale, f
   if (threadIdx.x == 0) *loss = static_cast<float>(s * scale);
 }
 
+// MPP: block g's partial sum of the logits over the rows g, g + G, ... of L [rows, ldl], columns [0, K)
+template <typename T>
+__global__ void __launch_bounds__(MIM_LOSS_THREADS)
+mpp_logit_sum_kernel(const T* __restrict__ L, int ldl, int K, long long rows, double* __restrict__ partial) {
+  __shared__ double red[MIM_LOSS_THREADS];
+  double acc = 0.0;
+  for (long long r = blockIdx.x; r < rows; r += gridDim.x) {
+    const T* l = L + r * ldl;
+    for (int e = threadIdx.x; e < K; e += MIM_LOSS_THREADS) acc += static_cast<double>(mim_f(l[e]));
+  }
+  const double s = mim_block_sum(acc, red);
+  if (threadIdx.x == 0) partial[blockIdx.x] = s;
+}
+
 unsigned mim_grid(long long rows) {
   const long long cap = static_cast<long long>(sm_count()) * 16;
   return static_cast<unsigned>(rows < 1 ? 1 : (rows > cap ? cap : rows));
@@ -203,9 +273,25 @@ void mim_mask(int B, int n, int descending, unsigned long long* rng, int* idx, c
 
 template <typename T>
 void mim_patch_rows(const float* img, int B, int H, int W, int C, int ph, int pw, const int* idx, int n, int off, int count, T* out, int ldo,
-                    const float* pos, T* R, int dim, cudaStream_t s) {
+                    const float* pos, T* R, int dim, cudaStream_t s, const int* src, const float* mask_row, const float* cls,
+                    const float* bias) {
   const long long rows = static_cast<long long>(B) * count;
-  mim_patch_rows_kernel<T><<<mim_grid(rows), 128, 0, s>>>(img, H, W, C, ph, pw, idx, n, off, count, out, ldo, pos, R, dim, rows);
+  if (cls != nullptr)
+    mim_patch_rows_kernel<T, true><<<mim_grid(rows), 128, 0, s>>>(img, H, W, C, ph, pw, idx, n, off, count, out, ldo, pos, R, dim, rows,
+                                                                  src, mask_row, cls, bias);
+  else
+    mim_patch_rows_kernel<T, false><<<mim_grid(rows), 128, 0, s>>>(img, H, W, C, ph, pw, idx, n, off, count, out, ldo, pos, R, dim, rows,
+                                                                   src, mask_row, cls, bias);
+  VB_CUDA(cudaGetLastError());
+  count_launch();
+}
+
+void mpp_draws(int B, int n, int k, const int* idx, const unsigned long long* rng, double random_patch_prob, double p_rand,
+               double replace_prob, int* source, int* mask_ids, int ldm, cudaStream_t s) {
+  VB_CHECK(n >= 1 && n <= MIM_MAX_PATCHES && k >= 1 && k <= n && ldm >= k, "MPP: bad draw shape");
+  // the coins compare float32 noise with the probabilities as TF converts a Python float: rounded to float32
+  mpp_draws_kernel<<<B, MPP_DRAW_THREADS, 0, s>>>(n, k, idx, rng, random_patch_prob > 0.0 ? 1 : 0, static_cast<float>(p_rand),
+                                                  static_cast<float>(replace_prob), source, mask_ids, ldm);
   VB_CUDA(cudaGetLastError());
   count_launch();
 }
@@ -250,9 +336,21 @@ void mim_loss(const T* pred, int pd, int B, int nm, const float* img, int H, int
   count_launch(2);
 }
 
+template <typename T>
+void mpp_loss(const T* logits, int ldl, int K, long long rows, double* partial, float* loss, cudaStream_t s) {
+  const int G = mim_loss_blocks(rows);
+  mpp_logit_sum_kernel<T><<<G, MIM_LOSS_THREADS, 0, s>>>(logits, ldl, K, rows, partial);
+  VB_CUDA(cudaGetLastError());
+  // mpp.py:128-129 as TF computes it: every row's cross-entropy is ln(K) times the sum of its logits (see vitb200.h)
+  mim_loss_final_kernel<<<1, MIM_LOSS_THREADS, 0, s>>>(partial, G, std::log(static_cast<double>(K)) / static_cast<double>(rows), loss);
+  VB_CUDA(cudaGetLastError());
+  count_launch(2);
+}
+
 #define VB_MIM_INSTANTIATE(T)                                                                                                   \
   template void mim_patch_rows<T>(const float*, int, int, int, int, int, int, const int*, int, int, int, T*, int, const float*, T*, \
-                                  int, cudaStream_t);                                                                           \
+                                  int, cudaStream_t, const int*, const float*, const float*, const float*);                    \
+  template void mpp_loss<T>(const T*, int, int, long long, double*, float*, cudaStream_t);                                     \
   template void mim_decoder_rows<T>(const T*, const int*, int, int, int, const float*, const float*, T*, int, cudaStream_t);     \
   template void mim_mask_tokens<T>(T*, const int*, int, int, int, const float*, const float*, int, cudaStream_t);                \
   template void mim_take_rows<T>(const T*, int, const int*, T*, int, int, int, cudaStream_t);                                   \

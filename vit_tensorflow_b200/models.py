@@ -30,6 +30,7 @@ from __future__ import annotations
 
 import collections
 import ctypes as C
+import math
 
 import numpy as np
 
@@ -1426,7 +1427,7 @@ class _MaskedImageModel(_EngineModel):
     """What MAE and SimMIM share: a handle of their own built from the encoder ViT's configuration, the encoder's current weights
     pushed into it before every call that follows a change, the engine's mask noise (set_seed) and the call itself."""
 
-    def _build(self, image_size, encoder, masking_ratio, seed, decoder=(0, 0, 0, 0)):
+    def _build(self, image_size, encoder, masking_ratio, seed, decoder=(0, 0, 0, 0), mc=None):
         if not (isinstance(encoder, ViT) and encoder._kind == "vit"):
             raise TypeError(f"{type(self).__name__}: the encoder must be a vit_tensorflow_b200.ViT (or DistillableViT), got "
                             f"{type(encoder).__name__}")
@@ -1435,7 +1436,7 @@ class _MaskedImageModel(_EngineModel):
         self.masking_ratio = masking_ratio
         self._dropout_rates = encoder._dropout_rates
         ec = encoder._cfg
-        mc = _lib.VbMimConfig()
+        mc = _lib.VbMimConfig() if mc is None else mc                   # MPP passes its VbMppConfig
         mc.masking_ratio = float(masking_ratio)
         mc.decoder_dim, mc.decoder_depth, mc.decoder_heads, mc.decoder_dim_head = (int(v) for v in decoder)
         self._mc = mc
@@ -1534,6 +1535,81 @@ class SimMIM(_MaskedImageModel):
     def __init__(self, image_size, encoder, masking_ratio=0.5, *, seed=None):
         assert masking_ratio > 0 and masking_ratio < 1, 'masking ratio must be kept between 0 and 1'
         self._build(image_size, encoder, masking_ratio, seed)
+
+
+class MPP(_MaskedImageModel):
+    """mpp.py:133-218 (masked patch prediction): ceil(mask_prob * n) patches per image masked by the top_k of the engine's Philox
+    noise, each masked patch replaced by the original patch at a random id (random-patch coin) and then by the pixel-space
+    mask_token (replace coin), the encoder ViT (cls row included) over the corrupted image, to_bits on the masked rows.  The call
+    returns the loss TF computes from mpp.py:128 as written: ln(K) times the mean over the masked rows of the sum of their logits
+    (include/vitb200.h states every reading).  Draws, precision, device and encoder weights as for MAE."""
+    _kind = "mpp"
+
+    def __init__(self, image_size, transformer, patch_size, output_channel_bits=3, channels=3, max_pixel_val=1.0, mask_prob=0.15,
+                 replace_prob=0.5, random_patch_prob=0.5, mean=None, std=None, *, seed=None):
+        if isinstance(transformer, ViT) and not (isinstance(patch_size, int) and
+                                                 (transformer._cfg.patch_h, transformer._cfg.patch_w) == (patch_size, patch_size)):
+            raise ValueError(f"MPP: patch_size must be one int equal to both of the encoder's patch sides "
+                             f"({transformer._cfg.patch_h} x {transformer._cfg.patch_w}); got {patch_size!r}")
+        if channels != 3:
+            raise ValueError(f"MPP: images of 3 channels (the encoder's patch Dense reads 3); got channels={channels!r}")
+        if output_channel_bits * channels > 16:
+            raise ValueError(f"MPP: to_bits would have 2^{output_channel_bits * channels} classes; at most 2^16 are supported")
+        self.patch_size, self.output_channel_bits, self.channels = patch_size, output_channel_bits, channels
+        self.max_pixel_val = max_pixel_val                               # no effect on the loss (see include/vitb200.h)
+        self.mask_prob, self.replace_prob, self.random_patch_prob = mask_prob, replace_prob, random_patch_prob
+        self.mean, self.std = mean, std
+        mc = _lib.VbMppConfig()
+        mc.mask_prob, mc.replace_prob, mc.random_patch_prob = float(mask_prob), float(replace_prob), float(random_patch_prob)
+        mc.output_channel_bits = int(output_channel_bits)
+        self._build(image_size, transformer, mask_prob, seed, mc=mc)
+        self.transformer = self.encoder
+
+    def _shapes(self, h, w):
+        p = self.patch_size
+        if h % p or w % p:
+            raise ValueError("Image dimensions must be divisible by the patch size.")
+        if self.random_patch_prob > 0:
+            self.random_patch_prob / (1 - self.replace_prob)              # mpp.py:185: ZeroDivisionError when replace_prob == 1
+        if self.mean and self.std:                                       # mpp.py:105-106,113-114: [c, 1, 1] against NHWC
+            for v in (self.mean, self.std):
+                c = int(np.size(v))
+                if not (h == c or h == 1 or c == 1):
+                    raise ValueError(f"MPP: mean / std of {c} values reshaped to [{c}, 1, 1] do not broadcast against images of "
+                                     f"height {h} (mpp.py:114)")
+        n = (h // p) * (w // p)
+        return n, math.ceil(self.mask_prob * n), 2 ** (self.output_channel_bits * self.channels)
+
+    def forward_raw(self, img_ptr, img_mem, batch, h, w, loss_ptr, out_mem, stream=None, logits_ptr=None, mask_ids_ptr=None,
+                    source_ptr=None):
+        """Pointer-level call (vb_forward_mpp): host or device buffers, optional cudaStream_t; logits [batch, k, K], mask_ids
+        [batch, k] and source [batch, n] are written when their pointers are given."""
+        self._finalize()
+        p = [C.c_void_p(v) if v else None for v in (logits_ptr, mask_ids_ptr, source_ptr)]
+        _lib.check(self._lib.vb_forward_mpp(self._h, C.c_void_p(img_ptr), img_mem, batch, h, w, C.c_void_p(loss_ptr), *p, out_mem,
+                                            C.c_void_p(stream) if stream else None), self._h)
+
+    def forward_mpp(self, img, stream=None):
+        """One call: (loss, logits [b, k, K] of the masked rows, mask_ids [b, k] ascending, source [b, n]).  source[b, j] is j
+        for an unchanged position, the random patch id whose pixels it took, or -1 where it took the mask token."""
+        x = self._img(img)
+        b, h, w, _ = x.shape
+        n, k, K = self._shapes(h, w)
+        loss = np.zeros(1, np.float32)
+        logits, ids, src = np.empty((b, k, K), np.float32), np.empty((b, k), np.int32), np.empty((b, n), np.int32)
+        self.forward_raw(x.ctypes.data, _lib.MEM_HOST, b, h, w, loss.ctypes.data, _lib.MEM_HOST, stream, logits.ctypes.data,
+                         ids.ctypes.data, src.ctypes.data)
+        return _as_tensor(loss.reshape(())), _as_tensor(logits), ids, src
+
+    def __call__(self, inputs, training=True, **kwargs):
+        """The reference's call: the loss as a float32 0-d array (answers `.numpy()`)."""
+        self._check_training(training)
+        x = self._img(inputs)
+        b, h, w, _ = x.shape
+        self._shapes(h, w)
+        loss = np.zeros(1, np.float32)
+        self.forward_raw(x.ctypes.data, _lib.MEM_HOST, b, h, w, loss.ctypes.data, _lib.MEM_HOST)
+        return _as_tensor(loss.reshape(()))
 
 
 def _spt_patch_size(patch_size):
