@@ -20,6 +20,7 @@
  *     PiT(...)(img)                  vit_tensorflow/pit.py:158-219 (vb_create_pit)
  *     MAE(...)(img) / SimMIM(...)(img)   vit_tensorflow/mae.py:49-92, simmim.py:82-129 (vb_create_mim, vb_forward_mim)
  *     MPP(...)(img)                      vit_tensorflow/mpp.py:168-218 (vb_create_mim, vb_forward_mpp)
+ *     DistillWrapper(...)([img, labels])  vit_tensorflow/distill.py:87-134 (vb_create_distill, vb_forward_distill_loss)
  * and this header is what the Python host classes (vit_tensorflow_b200/models.py, _lib.py) bind with ctypes.
  * Plain pointers and sizes only; no torch / C++ types cross the boundary.
  *
@@ -849,6 +850,45 @@ VB_API int vb_forward_mpp(vb_handle* h, const float* img, int32_t img_mem, int32
  * mask_ids int32 [B, k] ascending and source int32 [B, n] (host).  1 <= k <= n <= VB_MIM_MAX_PATCHES. */
 VB_API int vb_op_mpp_draws(int32_t B, int32_t n, int32_t k, double replace_prob, double random_patch_prob, uint64_t seed, uint64_t counter,
                            int32_t* mask_ids, int32_t* source);
+
+/* DistillWrapper (distill.py:87-134), appended within ABI 7: inference semantics and the loss value of the soft branch.
+ *   call([img, labels], T, alpha) = ce * (1 - alpha) + distill_loss * alpha, a float32 vector [b], with
+ *   ce[i] = categorical_crossentropy(labels[i], student_logits[i], from_logits=True) = sum_c labels[i, c] (lse(s_i) - s_i[c]), the
+ *   labels used as given (one-hot or any soft rows, not renormalised), and the distillation term read as Keras computes it:
+ *   KLDivergence(y_true, y_pred) clips BOTH arguments to [1e-7, 1].  Here y_pred = log_softmax(distill_logits / T) is <= 0, so it
+ *   always clips to 1e-7 and the term never reads the student: per image q[j] = sum_c y'[j, c] (ln y'[j, c] - ln 1e-7) with
+ *   y' = clip(softmax(teacher_logits[j] / T), 1e-7, 1) (the clip applied to the float32 softmax, at 1e-7f), and
+ *       out[i] = (1 - alpha) ce[i] + alpha T^2 (1 / b) sum_j q[j].
+ *   The distillation token still reaches the loss through student_logits; distill_logits and distill_mlp's weights do not (for
+ *   finite logits).  This reading comes from Keras' source; the numpy stand-in of the tests clips the same way, and the unmodified
+ *   reference DistillWrapper over it returns this vector.  It has not been checked against TensorFlow itself.
+ *   hard=True cannot run in the reference: tf.argmax gives [b] integer labels, which categorical_crossentropy refuses against the
+ *   [b, K] logits (ValueError "Shapes (b,) and (b, K) are incompatible") at every batch size.  The host class raises that error;
+ *   the engine implements no hard distillation.  T == 0 (inf / NaN in the reference) is refused.
+ *   Per image, ce and q are sums in double over max-subtracted softmaxes (logits of magnitude ~100 do not overflow); the mean of q
+ *   is vb_forward_mim's fixed-order reduction, so eager, captured and replayed calls give the same bits.
+ * vb_create_distill: `student` is the student's own vb_config (kind VB_KIND_VIT or VB_KIND_T2T_VIT; a T2TViT of depth 0, built for
+ * an injected transformer, is refused: its call is composed on the host).  Weights: the student's names (SURVEY.md App. B) plus
+ *   distillation_token [1, 1, dim], distill_mlp.0.gamma / .beta [dim] (the LayerNormalization, eps 1e-3),
+ *   distill_mlp.1.kernel [dim, num_classes] / .bias [num_classes] (the Dense).
+ * The handle is a student handle: vb_forward and vb_forward_distill run on it as on the student's. */
+VB_API int vb_create_distill(const vb_config* student, int device, vb_handle** out);
+/* One DistillWrapper call.  img as in vb_forward (img_mem); labels float32 [batch, num_classes] and teacher_logits float32
+ * [batch, num_classes] in in_mem memory.  Exactly one of `teacher` (a classifier handle on the same device with num_classes
+ * classes) and `teacher_logits` is given.  With a teacher handle the image is uploaded once and the teacher runs through its
+ * own vb_forward on `stream`, under its own graph rules, into a buffer of this handle; it is not part of this handle's graph.
+ * Then the student with the handle's distillation token (vb_forward_distill's semantics), distill_mlp on the token's row and the
+ * loss are captured and replayed under vb_forward's rules, keyed also by the labels and teacher-logit pointers and the bit
+ * patterns of temperature and alpha.  Outputs in out_mem memory: loss float32 [batch]; student_logits, distill_logits and
+ * teacher_logits_out [batch, num_classes] when not NULL. */
+VB_API int vb_forward_distill_loss(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, int32_t img_h, int32_t img_w,
+                                   const float* labels, vb_handle* teacher, const float* teacher_logits, int32_t in_mem,
+                                   double temperature, double alpha, float* loss, float* student_logits, float* distill_logits,
+                                   float* teacher_logits_out, int32_t out_mem, void* stream);
+/* The loss kernels of vb_forward_distill_loss on their own, over host buffers: student_logits, labels, teacher_logits float32
+ * [B, K] -> out float32 [B].  T == 0 is refused. */
+VB_API int vb_op_distill_loss(const float* student_logits, const float* labels, const float* teacher_logits, int32_t B, int32_t K,
+                              double temperature, double alpha, float* out);
 
 /* Row softmax of fp32 scores into bf16 probabilities (the T2T attention): p[r, j] = softmax_j(s[r, j] * scale) for j < n,
  * p[r, n..npad) = 0.  s [rows, lds], p [rows, ldp] (uploaded and downloaded whole); n <= npad <= ldp. */

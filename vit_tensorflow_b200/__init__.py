@@ -10,9 +10,10 @@ or an H100 is missing -- there is no CPU / PyTorch fallback.
 from .models import (ViT, DeepViT, CaiT, CrossViT, DistillableViT, ParallelViT, T2TViT, PatchMergerViT, PatchMerger,  # noqa: F401
                      EfficientViT, DistillableT2TViT, DistillableEfficientViT, CCT, cct_2, cct_4, cct_6, cct_7, cct_8, cct_14, cct_16, LeViT, CvT, TwinsSVT,
                      CrossFormer, NesT, RegionViT, ATSViT, SmallDatasetViT, SPT, MobileViT, ScalableViT, PiT, MAE, SimMIM, MPP,
+                     DistillWrapper,
                      from_config, pair)
 
 __all__ = ["ViT", "DeepViT", "CaiT", "CrossViT", "DistillableViT", "ParallelViT", "T2TViT", "PatchMergerViT", "PatchMerger",
            "EfficientViT", "DistillableT2TViT", "DistillableEfficientViT", "CCT", "cct_2", "cct_4", "cct_6", "cct_7", "cct_8", "cct_14", "cct_16", "LeViT", "CvT", "TwinsSVT",
            "CrossFormer", "NesT", "RegionViT", "ATSViT", "SmallDatasetViT", "SPT", "MobileViT", "ScalableViT", "PiT", "MAE",
-           "SimMIM", "MPP", "from_config"]
+           "SimMIM", "MPP", "DistillWrapper", "from_config"]

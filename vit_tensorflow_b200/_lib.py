@@ -170,6 +170,10 @@ SIGNATURES = {
     "vb_op_mim_mask": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, C.c_void_p]),
     "vb_forward_mpp": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 4 + [C.c_int32, C.c_void_p]),
     "vb_op_mpp_draws": (C.c_int, [C.c_int32] * 3 + [C.c_double, C.c_double, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]),
+    "vb_create_distill": (C.c_int, [C.POINTER(VbConfig), C.c_int, C.POINTER(C.c_void_p)]),
+    "vb_forward_distill_loss": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 3 +
+                                [C.c_int32, C.c_double, C.c_double] + [C.c_void_p] * 4 + [C.c_int32, C.c_void_p]),
+    "vb_op_distill_loss": (C.c_int, [C.c_void_p] * 3 + [C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_void_p]),
     "vb_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, _i64p, C.c_int32]),
     "vb_num_weights": (C.c_int, [C.c_void_p]),
     "vb_weight_info": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), _i64p, C.POINTER(C.c_int32)]),
@@ -557,3 +561,14 @@ def op_mpp_draws(B, n, k, replace_prob, random_patch_prob, seed=0, counter=0):
     check(load().vb_op_mpp_draws(B, n, k, float(replace_prob), float(random_patch_prob), int(seed) & 0xFFFFFFFFFFFFFFFF,
                                  int(counter) & 0xFFFFFFFFFFFFFFFF, _ptr(ids), _ptr(src)))
     return ids, src
+
+
+def op_distill_loss(student_logits, labels, teacher_logits, temperature, alpha):
+    """DistillWrapper's loss kernels on their own (vb_op_distill_loss): float32 [B, K] rows -> the loss float32 [B]."""
+    s, y, t = (np.ascontiguousarray(a, dtype=np.float32) for a in (student_logits, labels, teacher_logits))
+    if s.ndim != 2 or y.shape != s.shape or t.shape != s.shape:
+        raise ValueError(f"op_distill_loss: student_logits, labels and teacher_logits must be [B, K] alike, got {s.shape}, {y.shape}, "
+                         f"{t.shape}")
+    out = np.empty(s.shape[0], np.float32)
+    check(load().vb_op_distill_loss(_ptr(s), _ptr(y), _ptr(t), s.shape[0], s.shape[1], float(temperature), float(alpha), _ptr(out)))
+    return out

@@ -719,6 +719,35 @@ struct vb_handle {
   float* mim_patches() const { return static_cast<float*>(mim_dev.p) + mim_last.patches; }
   int* mpp_ids() const { return static_cast<int*>(mim_dev.p) + mim_last.ids; }
   int* mpp_src() const { return static_cast<int*>(mim_dev.p) + mim_last.src; }
+  // DistillWrapper (distill.py:87-134, vb_create_distill): a ViT / T2TViT student handle that also holds distillation_token and
+  // distill_mlp (LayerNorm "distill_mlp.0", Dense "distill_mlp.1").  dw_dev holds one call's float rows at stable addresses:
+  // teacher logits, labels, student logits, distill logits [B, K], distill tokens [B, dim], the loss [B], then ce and q [B]
+  // (doubles) and the distillation term (a new allocation drops the captured graphs).
+  bool distill_wrapper = false;
+  Norm dmlp_norm;
+  Linear dmlp;
+  DevMem dw_dev;
+  struct DistillPlan { int B = 0; size_t teacher = 0, labels = 0, student = 0, dlogits = 0, tokens = 0, loss = 0, ce = 0, q = 0, dterm = 0; };
+  DistillPlan dw_last;
+  void distill_prepare(int B) {
+    auto up = [](size_t v) { return (v + 63) / 64 * 64; };
+    const size_t rows = up(static_cast<size_t>(B) * cfg.num_classes);
+    DistillPlan p;
+    p.B = B;
+    p.labels = rows;
+    p.student = 2 * rows;
+    p.dlogits = 3 * rows;
+    p.tokens = 4 * rows;
+    p.loss = p.tokens + up(static_cast<size_t>(B) * cfg.dim);
+    p.ce = p.loss + up(B);                                   // float offsets; ce and q are doubles, 256-byte aligned
+    p.q = p.ce + up(2 * static_cast<size_t>(B));
+    p.dterm = p.q + up(2 * static_cast<size_t>(B));
+    dw_last = p;
+    const void* before = dw_dev.p;
+    dw_dev.ensure((p.dterm + 64) * sizeof(float));
+    if (before != nullptr && dw_dev.p != before) drop_graphs();
+  }
+  float* dw(size_t off) const { return static_cast<float*>(dw_dev.p) + off; }
   Norm head_norm, sm_head_norm, lg_head_norm;
   Linear head, sm_head, lg_head;
   Norm spt_norm;                     // SPT's LayerNorm over the p^2 * 5 C patch vector (bf16: padded to the GEMM's K, folded into it)
@@ -740,8 +769,12 @@ struct vb_handle {
   struct GraphKey {
     const void* img; void* out; int B, H, W; cudaStream_t s;
     int flags = 0;                                       // vb_forward_mim: which optional outputs the launches write
+    // vb_forward_distill_loss: the labels and teacher-logit rows the loss reads, and the bit patterns of T and alpha
+    const void* labels = nullptr; const void* teacher = nullptr;
+    uint64_t t_bits = 0, alpha_bits = 0;
     bool operator<(const GraphKey& o) const {
-      return std::tie(img, out, B, H, W, s, flags) < std::tie(o.img, o.out, o.B, o.H, o.W, o.s, o.flags);
+      return std::tie(img, out, B, H, W, s, flags, labels, teacher, t_bits, alpha_bits) <
+             std::tie(o.img, o.out, o.B, o.H, o.W, o.s, o.flags, o.labels, o.teacher, o.t_bits, o.alpha_bits);
     }
   };
   struct GraphEntry { cudaGraphExec_t exec = nullptr; int calls = 0; long long launches = 0; bool failed = false; };
@@ -1206,6 +1239,11 @@ struct vb_handle {
       expect_ln("sm_head_norm", c.sm_dim); expect_dense("sm_head", c.sm_dim, c.num_classes);
       expect_ln("lg_head_norm", c.lg_dim); expect_dense("lg_head", c.lg_dim, c.num_classes);
     }
+    if (distill_wrapper) {                                    // distill.py:101-106, after the student's own weights
+      expect("distillation_token", {1, 1, c.dim});
+      expect_ln("distill_mlp.0", c.dim);
+      expect_dense("distill_mlp.1", c.dim, c.num_classes);
+    }
   }
 
   // finalize-time replacements of registered weights by derived device copies (head-padded kernels)
@@ -1513,6 +1551,10 @@ struct vb_handle {
       }
       sm_head_norm = make_norm("sm_head_norm", c.sm_dim); sm_head = make_linear_f32("sm_head", c.sm_dim, c.num_classes);
       lg_head_norm = make_norm("lg_head_norm", c.lg_dim); lg_head = make_linear_f32("lg_head", c.lg_dim, c.num_classes);
+    }
+    if (distill_wrapper) {
+      dmlp_norm = make_norm("distill_mlp.0", c.dim);
+      dmlp = make_linear_f32("distill_mlp.1", c.dim, c.num_classes);
     }
     VB_CUDA(cudaDeviceSynchronize());
     finalized = true;
@@ -3825,6 +3867,18 @@ struct vb_handle {
     else convert<__nv_bfloat16, float>(reinterpret_cast<const __nv_bfloat16*>(D), distill_out, count, s);
   }
 
+  // DistillWrapper.call after the teacher (distill.py:116-134): the student over the handle's own distillation token, distill_mlp
+  // on the token's row, and the loss from the labels and teacher logits at `labels` / `tlog` [B, num_classes] into loss [B]
+  template <typename T>
+  void distill_loss_forward(const float* img, int B, int H, int Wd, const float* labels, const float* tlog, double temperature,
+                            double alpha, float* loss, cudaStream_t s) {
+    const DistillPlan& p = dw_last;
+    distill_impl<T>(img, B, H, Wd, W("distillation_token"), dw(p.student), dw(p.tokens), s);
+    classify<float>(dw(p.tokens), 1, cfg.dim, dmlp_norm, dmlp, B, 0, dw(p.dlogits), false, s);
+    distill_loss(dw(p.student), labels, tlog, B, cfg.num_classes, temperature, alpha, reinterpret_cast<double*>(dw(p.ce)),
+                 reinterpret_cast<double*>(dw(p.q)), dw(p.dterm), loss, s);
+  }
+
   template <typename T>
   void tokens_impl(const float* tok, int B, int n, float* out, cudaStream_t s) {
     VB_CHECK(cfg.kind == VB_KIND_VIT || cfg.kind == VB_KIND_DEEPVIT || cfg.kind == VB_KIND_T2T_VIT,
@@ -4434,6 +4488,39 @@ void staged_call(vb_handle* h, const float* in, int32_t in_mem, size_t in_bytes,
     VB_CUDA(cudaStreamSynchronize(s));
   }
 }
+// vb_create, and vb_create_distill (distill_wrapper: a ViT / T2TViT student handle that also registers DistillWrapper's weights)
+int create_base(const char* fn, const vb_config* cfg, int device, vb_handle** out, bool distill_wrapper) {
+  const std::string f(fn);
+  return guarded(nullptr, [&] {
+    VB_CHECK(cfg != nullptr && out != nullptr, f + ": null argument");
+    // a client of the ABI-7 struct without the CCT fields passes the shorter size: read only its bytes, zero the rest
+    const int32_t size = cfg->struct_size;
+    VB_CHECK(size == static_cast<int32_t>(sizeof(vb_config)) || size == VB_CONFIG_SIZE_ABI7, "vb_config.struct_size mismatch (ABI)");
+    vb_config c;
+    memset(&c, 0, sizeof c);
+    memcpy(&c, cfg, static_cast<size_t>(size));
+    if (distill_wrapper) {
+      VB_CHECK(c.kind == VB_KIND_VIT || c.kind == VB_KIND_T2T_VIT, f + " supports ViT and T2TViT (distill.py:47, :61)");
+      VB_CHECK(c.kind != VB_KIND_T2T_VIT || c.depth > 0,
+               f + ": this T2TViT was built for an injected transformer (depth 0); its distillation call is composed on the host");
+    }
+    validate(c);
+    int ndev = 0;
+    cudaError_t e = cudaGetDeviceCount(&ndev);
+    VB_CHECK(e == cudaSuccess && ndev > 0, f + ": no CUDA device available -- libvitb200 has no CPU fallback");
+    VB_CHECK(device >= 0 && device < ndev, f + ": bad device index");
+    VB_CUDA(cudaSetDevice(device));
+    cudaDeviceProp prop;
+    VB_CUDA(cudaGetDeviceProperties(&prop, device));
+    VB_CHECK(prop.major == 9 && prop.minor == 0, f + ": libvitb200 is built for sm_90a (Hopper H100) only");
+    std::unique_ptr<vb_handle> h(new vb_handle());
+    h->cfg = c;
+    h->device = device;
+    h->distill_wrapper = distill_wrapper;
+    h->build_expected();
+    *out = h.release();
+  });
+}
 // an extension config's struct_size: its first field, or (vb_mpp_config) that of the vb_mim_config it begins with
 template <typename Ext> int32_t ext_struct_size(const Ext& e) { return e.struct_size; }
 int32_t ext_struct_size(const vb_mpp_config& e) { return e.mim.struct_size; }
@@ -4527,30 +4614,10 @@ extern "C" {
 
 int vb_abi_version(void) { return VB_ABI_VERSION; }
 
-int vb_create(const vb_config* cfg, int device, vb_handle** out) {
-  return guarded(nullptr, [&] {
-    VB_CHECK(cfg != nullptr && out != nullptr, "vb_create: null argument");
-    // a client of the ABI-7 struct without the CCT fields passes the shorter size: read only its bytes, zero the rest
-    const int32_t size = cfg->struct_size;
-    VB_CHECK(size == static_cast<int32_t>(sizeof(vb_config)) || size == VB_CONFIG_SIZE_ABI7, "vb_config.struct_size mismatch (ABI)");
-    vb_config c;
-    memset(&c, 0, sizeof c);
-    memcpy(&c, cfg, static_cast<size_t>(size));
-    validate(c);
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    VB_CHECK(e == cudaSuccess && ndev > 0, "vb_create: no CUDA device available -- libvitb200 has no CPU fallback");
-    VB_CHECK(device >= 0 && device < ndev, "vb_create: bad device index");
-    VB_CUDA(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    VB_CUDA(cudaGetDeviceProperties(&prop, device));
-    VB_CHECK(prop.major == 9 && prop.minor == 0, "vb_create: libvitb200 is built for sm_90a (Hopper H100) only");
-    std::unique_ptr<vb_handle> h(new vb_handle());
-    h->cfg = c;
-    h->device = device;
-    h->build_expected();
-    *out = h.release();
-  });
+int vb_create(const vb_config* cfg, int device, vb_handle** out) { return create_base("vb_create", cfg, device, out, false); }
+
+int vb_create_distill(const vb_config* student, int device, vb_handle** out) {
+  return create_base("vb_create_distill", student, device, out, true);
 }
 
 int vb_create_levit(const vb_config* base, const vb_levit_config* lv, int device, vb_handle** out) {
@@ -5088,6 +5155,97 @@ int vb_forward_distill(vb_handle* h, const float* img, int32_t img_mem, int32_t 
       VB_CUDA(cudaMemcpyAsync(distill_out, dis_d, dis_bytes, cudaMemcpyDeviceToHost, s));
       VB_CUDA(cudaStreamSynchronize(s));
     }
+  });
+}
+
+int vb_forward_distill_loss(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, int32_t img_h, int32_t img_w,
+                            const float* labels, vb_handle* teacher, const float* teacher_logits, int32_t in_mem, double temperature,
+                            double alpha, float* loss, float* student_logits, float* distill_logits, float* teacher_logits_out,
+                            int32_t out_mem, void* stream) {
+  return guarded(h, [&] {
+    VB_CHECK(h != nullptr && img != nullptr && labels != nullptr && loss != nullptr, "vb_forward_distill_loss: null argument");
+    VB_CHECK(h->distill_wrapper, "vb_forward_distill_loss: not a DistillWrapper handle (create it with vb_create_distill)");
+    VB_CHECK(h->finalized, "vb_forward_distill_loss: call vb_finalize after setting the weights");
+    VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_forward_distill_loss: bad batch / image size");
+    VB_CHECK((teacher != nullptr) != (teacher_logits != nullptr), "vb_forward_distill_loss: pass exactly one of teacher and teacher_logits");
+    VB_CHECK(temperature != 0.0, "DistillWrapper: temperature 0 divides the logits by zero (inf / NaN in the reference)");
+    if (teacher != nullptr) {
+      VB_CHECK(teacher != h, "vb_forward_distill_loss: the teacher must be another handle");
+      VB_CHECK(teacher->device == h->device, "vb_forward_distill_loss: the teacher handle is on another device");
+      VB_CHECK(!teacher->is_mim() && !teacher->distill_wrapper, "vb_forward_distill_loss: the teacher must be a classifier handle");
+      VB_CHECK(teacher->cfg.num_classes == h->cfg.num_classes,
+               "vb_forward_distill_loss: the teacher has " + std::to_string(teacher->cfg.num_classes) +
+                   " classes; the teacher logits must be [b, num_classes] with num_classes = " + std::to_string(h->cfg.num_classes));
+    }
+    VB_CUDA(cudaSetDevice(h->device));
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const long long before = launch_counter();
+    const size_t img_bytes = static_cast<size_t>(batch) * img_h * img_w * h->cfg.channels * sizeof(float);
+    const size_t row_bytes = static_cast<size_t>(batch) * h->cfg.num_classes * sizeof(float);
+    const float* img_d = img;
+    if (img_mem == VB_MEM_HOST) {                             // uploaded once: the teacher and the student read the same copy
+      h->img_dev.ensure(img_bytes);
+      VB_CUDA(cudaMemcpyAsync(h->img_dev.p, img, img_bytes, cudaMemcpyHostToDevice, s));
+      img_d = static_cast<const float*>(h->img_dev.p);
+    }
+    h->distill_prepare(batch);
+    const vb_handle::DistillPlan& p = h->dw_last;
+    const float* labels_d = labels;
+    if (in_mem == VB_MEM_HOST) {
+      VB_CUDA(cudaMemcpyAsync(h->dw(p.labels), labels, row_bytes, cudaMemcpyHostToDevice, s));
+      labels_d = h->dw(p.labels);
+    }
+    const float* tlog_d = teacher_logits;
+    if (teacher != nullptr) {
+      // the teacher's own vb_forward, under its own graph rules, outside this handle's graph: a teacher that re-finalizes or
+      // grows its arena cannot leave a stale capture here
+      const int rc = vb_forward(teacher, img_d, VB_MEM_DEVICE, batch, img_h, img_w, h->dw(p.teacher), VB_MEM_DEVICE, stream);
+      if (rc != 0) throw Error(rc, "vb_forward_distill_loss: the teacher's forward failed: " + teacher->error);
+      tlog_d = h->dw(p.teacher);
+    } else if (in_mem == VB_MEM_HOST) {
+      VB_CUDA(cudaMemcpyAsync(h->dw(p.teacher), teacher_logits, row_bytes, cudaMemcpyHostToDevice, s));
+      tlog_d = h->dw(p.teacher);
+    }
+    float* loss_d = out_mem == VB_MEM_HOST ? h->dw(p.loss) : loss;
+    // the optional outputs are copied from dw_dev after the launches, so they do not change what is captured
+    vb_handle::GraphKey key{img_d, loss_d, batch, img_h, img_w, s};
+    key.labels = labels_d;
+    key.teacher = tlog_d;
+    memcpy(&key.t_bits, &temperature, sizeof temperature);
+    memcpy(&key.alpha_bits, &alpha, sizeof alpha);
+    run_graphed(h, key, [&] {
+      if (h->bf16()) h->distill_loss_forward<__nv_bfloat16>(img_d, batch, img_h, img_w, labels_d, tlog_d, temperature, alpha, loss_d, s);
+      else h->distill_loss_forward<float>(img_d, batch, img_h, img_w, labels_d, tlog_d, temperature, alpha, loss_d, s);
+    });
+    h->last_launches = launch_counter() - before;
+    const cudaMemcpyKind kind = out_mem == VB_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+    if (student_logits != nullptr) VB_CUDA(cudaMemcpyAsync(student_logits, h->dw(p.student), row_bytes, kind, s));
+    if (distill_logits != nullptr) VB_CUDA(cudaMemcpyAsync(distill_logits, h->dw(p.dlogits), row_bytes, kind, s));
+    if (teacher_logits_out != nullptr) VB_CUDA(cudaMemcpyAsync(teacher_logits_out, tlog_d, row_bytes, kind, s));
+    if (out_mem == VB_MEM_HOST) {
+      VB_CUDA(cudaMemcpyAsync(loss, loss_d, static_cast<size_t>(batch) * sizeof(float), cudaMemcpyDeviceToHost, s));
+      VB_CUDA(cudaStreamSynchronize(s));
+    }
+  });
+}
+
+int vb_op_distill_loss(const float* student_logits, const float* labels, const float* teacher_logits, int32_t B, int32_t K,
+                       double temperature, double alpha, float* out) {
+  return guarded(nullptr, [&] {
+    VB_CHECK(student_logits && labels && teacher_logits && out && B > 0 && K > 0, "vb_op_distill_loss: bad arguments");
+    VB_CHECK(temperature != 0.0, "DistillWrapper: temperature 0 divides the logits by zero (inf / NaN in the reference)");
+    require_gpu();
+    const size_t rows = static_cast<size_t>(B) * K;
+    DevMem dS, dY, dT, dw;
+    const float* s_d = upload<float>(dS, student_logits, rows);
+    const float* y_d = upload<float>(dY, labels, rows);
+    const float* t_d = upload<float>(dT, teacher_logits, rows);
+    dw.ensure(2 * static_cast<size_t>(B) * sizeof(double) + (static_cast<size_t>(B) + 64) * sizeof(float));
+    double* ce = static_cast<double*>(dw.p);
+    float* dterm = reinterpret_cast<float*>(ce + 2 * static_cast<size_t>(B));
+    float* o_d = dterm + 64;
+    distill_loss(s_d, y_d, t_d, B, K, temperature, alpha, ce, ce + B, dterm, o_d, 0);
+    VB_CUDA(cudaMemcpy(out, o_d, static_cast<size_t>(B) * sizeof(float), cudaMemcpyDeviceToHost));
   });
 }
 

@@ -260,6 +260,13 @@ int mim_loss_blocks(long long rows);
 template <typename T>
 void mim_loss(const T* pred, int pd, int B, int nm, const float* img, int H, int W, int C, int ph, int pw, const int* idx, int n,
               double* partial, float* loss, cudaStream_t s);
+// *loss = float(scale * (the sum of partial [G])), summed in double by one CTA in a fixed order (the final step of mim_loss)
+void mim_loss_final(const double* partial, int G, double scale, float* loss, cudaStream_t s);
+// DistillWrapper's soft loss (distill.py:119-134, the reading of include/vitb200.h), B images of K classes, all [B, K] float32 rows
+// on the device: ce [B] and q [B] (doubles) get each image's cross-entropy and KL term, *dterm = alpha T^2 mean(q) through
+// mim_loss_final, and out [B] = (1 - alpha) ce + dterm.  T == 0 is refused.
+void distill_loss(const float* student_logits, const float* labels, const float* teacher_logits, int B, int K, double T, double alpha,
+                  double* ce, double* q, float* dterm, float* out, cudaStream_t s);
 
 long long launch_counter();      // number of kernel launches issued through these wrappers (process-wide)
 void count_launch(int n = 1);

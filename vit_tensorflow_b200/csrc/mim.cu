@@ -322,6 +322,12 @@ void mim_take_rows(const T* X, int n, const int* idx, T* out, int B, int count, 
 
 int mim_loss_blocks(long long rows) { return static_cast<int>(rows < MIM_LOSS_BLOCKS ? rows : MIM_LOSS_BLOCKS); }
 
+void mim_loss_final(const double* partial, int G, double scale, float* loss, cudaStream_t s) {
+  mim_loss_final_kernel<<<1, MIM_LOSS_THREADS, 0, s>>>(partial, G, scale, loss);
+  VB_CUDA(cudaGetLastError());
+  count_launch();
+}
+
 template <typename T>
 void mim_loss(const T* pred, int pd, int B, int nm, const float* img, int H, int W, int C, int ph, int pw, const int* idx, int n,
               double* partial, float* loss, cudaStream_t s) {
@@ -329,11 +335,10 @@ void mim_loss(const T* pred, int pd, int B, int nm, const float* img, int H, int
   const int G = mim_loss_blocks(rows);
   mim_loss_partial_kernel<T><<<G, MIM_LOSS_THREADS, 0, s>>>(pred, pd, rows, img, H, W, C, ph, pw, idx, n, nm, partial);
   VB_CUDA(cudaGetLastError());
+  count_launch();
   double scale = 1.0 / (static_cast<double>(rows) * pd);
   if (img != nullptr) scale /= nm;                           // simmim.py:128: the mean divided by num_masked once more
-  mim_loss_final_kernel<<<1, MIM_LOSS_THREADS, 0, s>>>(partial, G, scale, loss);
-  VB_CUDA(cudaGetLastError());
-  count_launch(2);
+  mim_loss_final(partial, G, scale, loss, s);
 }
 
 template <typename T>
@@ -341,10 +346,9 @@ void mpp_loss(const T* logits, int ldl, int K, long long rows, double* partial, 
   const int G = mim_loss_blocks(rows);
   mpp_logit_sum_kernel<T><<<G, MIM_LOSS_THREADS, 0, s>>>(logits, ldl, K, rows, partial);
   VB_CUDA(cudaGetLastError());
+  count_launch();
   // mpp.py:128-129 as TF computes it: every row's cross-entropy is ln(K) times the sum of its logits (see vitb200.h)
-  mim_loss_final_kernel<<<1, MIM_LOSS_THREADS, 0, s>>>(partial, G, std::log(static_cast<double>(K)) / static_cast<double>(rows), loss);
-  VB_CUDA(cudaGetLastError());
-  count_launch(2);
+  mim_loss_final(partial, G, std::log(static_cast<double>(K)) / static_cast<double>(rows), loss, s);
 }
 
 #define VB_MIM_INSTANTIATE(T)                                                                                                   \

@@ -14,6 +14,7 @@
     ScalableViT  vit_tensorflow/scalable_vit.py:250-319
     PiT       vit_tensorflow/pit.py:158-219
     MAE / SimMIM  vit_tensorflow/mae.py:17-92, simmim.py:72-129 (around a ViT encoder)
+    DistillWrapper  vit_tensorflow/distill.py:87-134 (around a distillable student and any teacher)
 
 Same constructor kwargs, defaults and assertion messages; `model(img, training=True, **kwargs) -> logits`
 with `img` NHWC float32 `[b, H, W, 3]` and logits float32 `[b, num_classes]`.  Everything below the call is
@@ -125,12 +126,13 @@ class _EngineModel:
     """Common machinery: engine handle, weight dict, forward call."""
 
     _kind = None
-    _encoder_names = ()         # weights another model owns and initialises (MAE / SimMIM: the encoder's)
+    _encoder_names = ()         # weights another model owns and initialises (MAE / SimMIM: the encoder's; DistillWrapper: the student's)
     _inference_only = None      # the message of a family whose every call without training=False raises NotImplementedError
     # tf.random.normal Variables, N(0, 1): vit.py:146-147, deepvit.py:57, cait.py:97-98, vit_with_patch_merger.py:47,
-    # nest.py:129, mae.py:43, simmim.py:85; vit_for_small_dataset.py:94's temperature is drawn too, then set (SmallDatasetViT)
+    # nest.py:129, mae.py:43, simmim.py:85, distill.py:101; vit_for_small_dataset.py:94's temperature is drawn too, then set
+    # (SmallDatasetViT)
     _NORMAL_LEAVES = ("pos_embedding", "cls_token", "reattn_weights", "mix_pre", "mix_post", "queries", "pos_emb", "mask_token",
-                      "temperature")
+                      "temperature", "distillation_token")
 
     def _create(self, precision, device, ext=None, create="vb_create", **cfgkw):
         """`_config`, then every VbConfig field of `cfgkw` as int(value), then `_open`."""
@@ -1423,9 +1425,40 @@ class ATSViT(_EngineModel):
         return _as_tensor(logits)
 
 
-class _MaskedImageModel(_EngineModel):
+class _WrapperModel(_EngineModel):
+    """A handle of its own that also registers the weights of the model it wraps (the attribute `_wrapped_name`): those stay
+    the wrapped model's, and their current values are pushed into this handle before every call that follows a change."""
+    _wrapped_name = None
+
+    def _share_weights(self):
+        self._encoder_names = tuple(n for n in self._specs if n in getattr(self, self._wrapped_name)._specs)
+        self._pushed = {}
+
+    def set_weights_dict(self, weights):
+        """The model's own weights (SURVEY.md App. B); the wrapped model's are set on it and picked up by the next call."""
+        shared = [n for n in weights if n in self._encoder_names]
+        if shared:
+            w = self._wrapped_name
+            raise KeyError(f"{type(self).__name__}: {shared[0]!r} belongs to the {w}: set it with {w}.set_weights_dict")
+        super().set_weights_dict(weights)
+
+    def _push_wrapped(self):
+        src = getattr(self, self._wrapped_name)
+        changed = collections.OrderedDict((n, src.get_weight(n)) for n in self._encoder_names
+                                          if self._pushed.get(n) is not src.get_weight(n))
+        if changed:
+            _EngineModel.set_weights_dict(self, changed)
+            self._pushed.update(changed)
+
+    def _finalize(self):
+        self._push_wrapped()
+        super()._finalize()
+
+
+class _MaskedImageModel(_WrapperModel):
     """What MAE and SimMIM share: a handle of their own built from the encoder ViT's configuration, the encoder's current weights
     pushed into it before every call that follows a change, the engine's mask noise (set_seed) and the call itself."""
+    _wrapped_name = "encoder"
 
     def _build(self, image_size, encoder, masking_ratio, seed, decoder=(0, 0, 0, 0), mc=None):
         if not (isinstance(encoder, ViT) and encoder._kind == "vit"):
@@ -1443,27 +1476,8 @@ class _MaskedImageModel(_EngineModel):
         self._create(encoder.precision, encoder.device, ext=mc, create="vb_create_mim", image_h=ec.image_h, image_w=ec.image_w,
                      patch_h=ec.patch_h, patch_w=ec.patch_w, num_classes=ec.num_classes, dim=ec.dim, depth=ec.depth, heads=ec.heads,
                      dim_head=ec.dim_head, mlp_dim=ec.mlp_dim)
-        self._encoder_names = tuple(n for n in self._specs if n in encoder._specs)
-        self._pushed = {}
+        self._share_weights()
         self.init_weights(seed)                                         # the model's own weights: the encoder keeps its own
-
-    def set_weights_dict(self, weights):
-        """The model's own weights (SURVEY.md App. B); the encoder's are set on the encoder and picked up by the next call."""
-        shared = [n for n in weights if n in self._encoder_names]
-        if shared:
-            raise KeyError(f"{type(self).__name__}: {shared[0]!r} belongs to the encoder: set it with encoder.set_weights_dict")
-        super().set_weights_dict(weights)
-
-    def _push_encoder(self):
-        changed = collections.OrderedDict((n, self.encoder.get_weight(n)) for n in self._encoder_names
-                                          if self._pushed.get(n) is not self.encoder.get_weight(n))
-        if changed:
-            _EngineModel.set_weights_dict(self, changed)
-            self._pushed.update(changed)
-
-    def _finalize(self):
-        self._push_encoder()
-        super()._finalize()
 
     def set_seed(self, seed):
         """The Philox key of the mask noise (include/vitb200.h); also restarts its draw counter, so the next calls repeat the masks
@@ -1963,6 +1977,109 @@ class PiT(_EngineModel):
 
 
 PIT_CTOR_KEYS = ("image_size", "patch_size", "num_classes", "dim", "depth", "heads", "mlp_dim", "dim_head", "dropout", "emb_dropout")
+
+
+class DistillWrapper(_WrapperModel):
+    """distill.py:87-134: the teacher, the student over the wrapper's distillation token, distill_mlp (LayerNormalization + Dense)
+    on the token's row and the soft-distillation loss, with the student, distill_mlp and the loss on the engine.  `wrapper([img,
+    labels])` returns what the reference returns, a float32 loss vector [b], read as include/vitb200.h states: Keras'
+    KLDivergence clips the log-probabilities to 1e-7, so the distillation term reads the teacher only.  An engine classifier on
+    the student's device (_ENGINE_TEACHERS) runs as the teacher through its own handle, with no host copy of its logits; any
+    other teacher is called on the host as `teacher(img, training=training)`.  hard=True constructs, and every call raises the
+    reference's ValueError.  Precision and device are the student's; the student's weights are read at every call that follows
+    a change."""
+    _wrapped_name = "student"
+
+    def __init__(self, teacher, student, temperature=1.0, alpha=0.5, hard=False, *, seed=None):
+        assert (isinstance(student, (DistillableViT, DistillableT2TViT, DistillableEfficientViT))), 'student must be a vision transformer'
+        if isinstance(student, DistillableT2TViT) and student._injected is not None:
+            raise NotImplementedError("DistillWrapper: a DistillableT2TViT built around an injected transformer= runs its distillation "
+                                      "call on the host around that transformer, so the wrapper has no device path for it")
+        self.teacher, self.student = teacher, student
+        self.dim, self.num_classes = student.dim, student.num_classes              # distill.py:96-97
+        self.temperature, self.alpha, self.hard = temperature, alpha, hard
+        self._dropout_rates = student._dropout_rates
+        self.precision, self.device = student.precision, student.device
+        self._cfg = _lib.VbConfig.from_buffer_copy(student._cfg)
+        self._open(self._cfg, "vb_create_distill")
+        self._share_weights()
+        self.init_weights(seed)                        # distillation_token N(0, 1) and distill_mlp's Keras defaults
+
+    @property
+    def distillation_token(self):
+        return self._weight_view("distillation_token")
+
+    def _engine_teacher(self):
+        """Whether the teacher runs through its own handle: one of _ENGINE_TEACHERS (exactly), open, on the student's device, and
+        in a configuration whose call is vb_forward's logits."""
+        t = self.teacher
+        if type(t) not in _ENGINE_TEACHERS or getattr(t, "_h", None) is None or t.device != self.device:
+            return False
+        return not (isinstance(t, T2TViT) and t._injected is not None) and not (isinstance(t, LeViT) and t.num_distill_classes is not None)
+
+    def forward_raw(self, img_ptr, img_mem, batch, h, w, labels_ptr, in_mem, temperature, alpha, loss_ptr, out_mem, stream=None,
+                    teacher=None, teacher_logits_ptr=None, student_logits_ptr=None, distill_logits_ptr=None, teacher_logits_out_ptr=None):
+        """Pointer-level call (vb_forward_distill_loss): host or device buffers, optional cudaStream_t.  Pass exactly one of
+        `teacher` (an engine model) and `teacher_logits_ptr` ([batch, num_classes] in in_mem memory, as the labels); loss [batch]
+        and the optional [batch, num_classes] outputs go to out_mem memory."""
+        self._finalize()
+        th = None
+        if teacher is not None:
+            teacher._finalize()
+            th = teacher._h
+        p = [C.c_void_p(v) if v else None for v in (teacher_logits_ptr, loss_ptr, student_logits_ptr, distill_logits_ptr,
+                                                    teacher_logits_out_ptr)]
+        _lib.check(self._lib.vb_forward_distill_loss(self._h, C.c_void_p(img_ptr), img_mem, batch, h, w, C.c_void_p(labels_ptr), th, p[0],
+                                                     in_mem, float(temperature), float(alpha), *p[1:], out_mem,
+                                                     C.c_void_p(stream) if stream else None), self._h)
+
+    def _call(self, inputs, temperature, alpha, training, outputs):
+        img, labels = inputs                                                      # distill.py:109
+        alpha = alpha if alpha is not None else self.alpha
+        T = temperature if temperature is not None else self.temperature
+        if isinstance(self.student, DistillableEfficientViT):
+            self.student(img, distill_token=self.distillation_token, training=training)   # raises, as distill.py:83 does
+        on_engine = self._engine_teacher()
+        if on_engine:
+            self.teacher._check_training(training)
+        self._check_training(training)
+        if T == 0:
+            raise ValueError("DistillWrapper: temperature 0 divides the logits by zero (inf / NaN in the reference)")
+        x = self._img(img)
+        b, h, w, _ = x.shape
+        K = self.num_classes
+        y = np.ascontiguousarray(labels, dtype=np.float32)
+        if y.shape != (b, K):                                                     # categorical_crossentropy's shape check (:119)
+            raise ValueError(f"Shapes {y.shape} and {(b, K)} are incompatible")
+        if self.hard:                                                             # :131-132: argmax labels [b] against [b, K]
+            raise ValueError(f"Shapes {(b,)} and {(b, K)} are incompatible")
+        tl = None
+        if not on_engine:
+            t = self.teacher(img, training=training)                               # :114, with the caller's img object
+            tl = np.ascontiguousarray(t.numpy() if hasattr(t, "numpy") else t, dtype=np.float32)
+            if tl.shape != (b, K):
+                raise ValueError(f"DistillWrapper: the teacher returned logits of shape {tl.shape}; expected [b, num_classes] = {(b, K)}")
+        loss = np.empty(b, np.float32)
+        rows = [np.empty((b, K), np.float32) for _ in range(3)] if outputs else [None] * 3
+        ptr = lambda a: a.ctypes.data if a is not None else None
+        self.forward_raw(x.ctypes.data, _lib.MEM_HOST, b, h, w, y.ctypes.data, _lib.MEM_HOST, T, alpha, loss.ctypes.data, _lib.MEM_HOST,
+                         teacher=self.teacher if on_engine else None, teacher_logits_ptr=ptr(tl), student_logits_ptr=ptr(rows[0]),
+                         distill_logits_ptr=ptr(rows[1]), teacher_logits_out_ptr=ptr(rows[2]))
+        return (_as_tensor(loss),) + tuple(_as_tensor(r) for r in rows if r is not None)
+
+    def __call__(self, inputs, temperature=None, alpha=None, training=True, **kwargs):
+        """distill.py:108-134: inputs = [img, labels [b, num_classes]] -> the loss, float32 [b] (answers `.numpy()`)."""
+        return self._call(inputs, temperature, alpha, training, False)[0]
+
+    def forward_distill_loss(self, inputs, temperature=None, alpha=None):
+        """One call with training=False: (loss [b], student_logits, distill_logits, teacher_logits), each [b, num_classes]."""
+        return self._call(inputs, temperature, alpha, False, True)
+
+
+# the engine classes whose `__call__(img, training=)` is exactly their vb_forward logits (T2TViT without an injected transformer,
+# LeViT without a distillation head): DistillWrapper runs such a teacher through its handle
+_ENGINE_TEACHERS = (ViT, DeepViT, CaiT, CrossViT, ParallelViT, PatchMergerViT, T2TViT, DistillableViT, DistillableT2TViT, CCT, LeViT, CvT,
+                    SmallDatasetViT)
 
 
 _FAMILY_CTORS = {"pit": (PiT, PIT_CTOR_KEYS), "scalable_vit": (ScalableViT, SCALABLE_VIT_CTOR_KEYS),
