@@ -365,7 +365,7 @@ VB_API int vb_weight_info(vb_handle* h, int32_t index, const char** name, int64_
 VB_API int vb_finalize(vb_handle* h);
 
 /* Replaces <Model>.call(img) (vit.py:159-177, deepvit.py:139-157, cait.py:180-194, cross_vit.py:290-303)
- * with inference semantics (dropout = identity).  img: NHWC float32 [batch,h,w,channels] in host or device
+ * with inference semantics (dropout = identity; vb_forward_train runs training-mode dropout).  img: NHWC float32 [batch,h,w,channels] in host or device
  * memory (img_mem); logits: float32 [batch,num_classes] written to host or device memory (logits_mem).
  * stream: a cudaStream_t (may be NULL = default stream).  With device buffers the call is asynchronous on
  * `stream`; with a host logits buffer it returns after the copy completes.
@@ -889,6 +889,34 @@ VB_API int vb_forward_distill_loss(vb_handle* h, const float* img, int32_t img_m
  * [B, K] -> out float32 [B].  T == 0 is refused. */
 VB_API int vb_op_distill_loss(const float* student_logits, const float* labels, const float* teacher_logits, int32_t B, int32_t K,
                               double temperature, double alpha, float* out);
+
+/* Training-mode dropout (appended within ABI 7): the reference's call with training=True (vit.py:159, deepvit.py:139, cait.py:180,
+ * cross_vit.py:290) and non-zero rates, on ViT, DeepViT, CaiT and CrossViT handles (not a distillation handle).
+ *   Sites.  Site s is the ordinal of a Dropout layer among all Dropout calls of the reference's forward, from 0, rate-0 layers
+ *   included: ViT / DeepViT the embedding's (0), then per layer L to_out's, the GELU's and fc2's (1 + 3 L, 2 + 3 L, 3 + 3 L; a ViT
+ *   layer without out-projection, heads == 1 and dim_head == dim, has no to_out site, so its layers have two); CaiT the embedding's,
+ *   the patch stack's layers, then the class stack's; CrossViT the small then the large embedder's, then per block the small
+ *   tower's layers, the large tower's, and per cross-attention round sm_attend_lg's to_out then lg_attend_sm's (before project_out).
+ *   The embedding site takes emb_dropout, every other site dropout.
+ *   Elements.  A site's tensor is viewed as [M, N]: m the row over all leading axes in row-major order (b * rows + t), n < N the
+ *   true width of the last axis.
+ *   Masks.  With the 64-bit seed as key (k0 = low 32 bits, k1 = high) and the handle's 32-bit draw counter d:
+ *     x = philox4x32_10(counter = (n >> 1, ((m >> 4) << 3) | (m & 7), s, d), key = (k0, k1))
+ *     word = x[2 ((m >> 3) & 1) + (n & 1)],  u = (word >> 8) 2^-24,  keep = u >= rate (float32)
+ *     out = keep ? v * float32(1 / (1 - rate)) : 0
+ *   One Philox block covers the 2 x 2 fragment (rows m, m + 8, columns n, n + 1) one thread of the wgmma epilogue holds.  Image b's
+ *   masks do not depend on the batch it sits in.
+ *   The counter.  d lives in device memory next to the key; every dropout kernel of a forward reads it, and the forward advances it
+ *   by one on the device after its last site, so graph replays draw fresh masks.
+ * vb_set_dropout: stores the rates (each in [0, 1)), sets the key and resets d to 0, after waiting for the device.  Drops the
+ * handle's captured graphs. */
+VB_API int vb_set_dropout(vb_handle* h, float dropout, float emb_dropout, uint64_t seed);
+/* vb_forward's arguments and graph rules, with every site of rate > 0 drawing its mask (the graph key carries the training flag).
+ * Fails without a prior vb_set_dropout; with all rates 0 it is vb_forward and leaves d as it is. */
+VB_API int vb_forward_train(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, int32_t img_h, int32_t img_w,
+                            float* logits, int32_t logits_mem, void* stream);
+/* The stream on its own, by the device function the epilogues use: keep uint8 [M, N] (host memory) of site `site` at draw `draw`. */
+VB_API int vb_op_dropout_mask(uint64_t seed, uint32_t draw, uint32_t site, int32_t M, int32_t N, float rate, uint8_t* keep);
 
 /* Row softmax of fp32 scores into bf16 probabilities (the T2T attention): p[r, j] = softmax_j(s[r, j] * scale) for j < n,
  * p[r, n..npad) = 0.  s [rows, lds], p [rows, ldp] (uploaded and downloaded whole); n <= npad <= ldp. */

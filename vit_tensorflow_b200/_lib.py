@@ -174,6 +174,9 @@ SIGNATURES = {
     "vb_forward_distill_loss": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 3 +
                                 [C.c_int32, C.c_double, C.c_double] + [C.c_void_p] * 4 + [C.c_int32, C.c_void_p]),
     "vb_op_distill_loss": (C.c_int, [C.c_void_p] * 3 + [C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_void_p]),
+    "vb_set_dropout": (C.c_int, [C.c_void_p, C.c_float, C.c_float, C.c_uint64]),
+    "vb_forward_train": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),
+    "vb_op_dropout_mask": (C.c_int, [C.c_uint64, C.c_uint32, C.c_uint32, C.c_int32, C.c_int32, C.c_float, C.c_void_p]),
     "vb_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, _i64p, C.c_int32]),
     "vb_num_weights": (C.c_int, [C.c_void_p]),
     "vb_weight_info": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), _i64p, C.POINTER(C.c_int32)]),
@@ -571,4 +574,12 @@ def op_distill_loss(student_logits, labels, teacher_logits, temperature, alpha):
                          f"{t.shape}")
     out = np.empty(s.shape[0], np.float32)
     check(load().vb_op_distill_loss(_ptr(s), _ptr(y), _ptr(t), s.shape[0], s.shape[1], float(temperature), float(alpha), _ptr(out)))
+    return out
+
+
+def op_dropout_mask(seed, draw, site, M, N, rate):
+    """The training-mode dropout stream on its own (vb_op_dropout_mask): keep uint8 [M, N] of site `site` at draw `draw`."""
+    out = np.zeros((M, N), np.uint8)
+    check(load().vb_op_dropout_mask(int(seed) & 0xFFFFFFFFFFFFFFFF, int(draw) & 0xFFFFFFFF, int(site) & 0xFFFFFFFF, M, N, float(rate),
+                                    _ptr(out)))
     return out

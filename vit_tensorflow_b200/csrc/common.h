@@ -144,9 +144,21 @@ enum Act { ACT_NONE = 0, ACT_GELU = 1, ACT_HSWISH = 2, ACT_SILU = 3 };
 __device__ __forceinline__ float silu(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
 #endif
 
+// Training-mode dropout in a GEMM epilogue (philox.cuh dropout_block; include/vitb200.h states the stream): site `site` masks the
+// [M, N] output at rate `rate` and scales the kept values by `scale` = fp32(1 / (1 - rate)).  DROP_BEFORE_RES masks after the
+// activation, before LayerScale and the residual; DROP_AFTER_RES masks the sum.  state: the handle's {seed, draw counter} in
+// device memory, read by the kernel.
+enum DropPos { DROP_NONE = 0, DROP_BEFORE_RES = 1, DROP_AFTER_RES = 2 };
+struct DropoutEpi {
+  int pos = DROP_NONE;
+  const unsigned long long* state = nullptr;
+  int site = 0;
+  float rate = 0.f, scale = 1.f;
+};
+
 // ------------------------------------------------------------------------------------------ wgmma GEMM
 // out[M,N] = epilogue(A[M,K] * Wt[N,K]^T): bf16 operands (K-major), fp32 accumulation in registers.
-// epilogue: (+bias[n]) -> (activation) -> (*scale[n]) -> (+res[m,n]); out bf16.
+// epilogue: (+bias[n]) -> (activation) -> (dropout) -> (*scale[n]) -> (+res[m,n]) -> (dropout); out bf16.
 struct GemmBf16 {
   CUtensorMap tmap_a, tmap_b;           // A, B (weights)
   CUtensorMap tmap_out = {}, tmap_res = {};   // bf16 out and res, which the epilogue stores and loads by TMA
@@ -171,11 +183,12 @@ struct GemmBf16 {
   float ln_eps = 1e-3f;
   // Emit (sum, sumsq) of every 64-column chunk of the stored bf16 output rows: [N/64, M, 2]
   float* stats_out = nullptr;
+  DropoutEpi drop;
 };
 // lda/ldw/ldc/ldr in elements; all must be multiples of 8 (16-byte TMA strides); N % 64 == 0.
 GemmBf16 gemm_bf16_plan(const __nv_bfloat16* A, int lda, const __nv_bfloat16* Wt, int ldw, __nv_bfloat16* out, int ldc,
                         int M, int N, int K, const float* bias, const float* scale, const __nv_bfloat16* res, int ldr,
-                        int act, bool out_f32 = false, int b_rows = 0);
+                        int act, bool out_f32 = false, int b_rows = 0, bool dropout = false);
 void gemm_bf16_run(const GemmBf16& g, cudaStream_t stream);
 bool gemm_bf16_supported(int M, int N, int K, int lda, int ldw, int ldc);
 

@@ -3,8 +3,9 @@
 //
 // The op sequences restate the reference's call graphs (SURVEY.md section 3):
 //   ViT / DeepViT  vit.py:159-177, deepvit.py:139-157      CaiT  cait.py:180-194      CrossViT  cross_vit.py:290-303
-// with inference semantics (dropout = identity).  T = float runs the exact-fp32 SIMT kernels (numerics gate),
-// T = __nv_bfloat16 runs the wgmma GEMM / tensor-core attention kernels with fp32 accumulation and statistics.
+// with inference semantics (dropout = identity; vb_forward_train masks every Dropout site instead).  T = float runs the
+// exact-fp32 SIMT kernels (numerics gate), T = __nv_bfloat16 runs the wgmma GEMM / tensor-core attention kernels with fp32
+// accumulation and statistics.
 #include "../../include/vitb200.h"
 #include "attention.cuh"
 #include "common.h"
@@ -109,6 +110,7 @@ struct Epi {
   void set_act(int a) { gelu = a == ACT_GELU; hswish = a == ACT_HSWISH; silu = a == ACT_SILU; }
   const float* ln_stats = nullptr;   // (sum, sumsq) partials per 64-column chunk of the A operand's rows for a LayerNorm-folded Dense, [M, K/64, 2]
   float* stats_out = nullptr;        // emit (sum, sumsq) partials of every 64-column chunk of the output rows, [M, N/64, 2]
+  DropoutEpi drop;                   // training-mode dropout of the output (vb_handle::dropout)
 };
 
 struct LayerW {                    // one pre-norm transformer layer in any of the four dialects
@@ -126,6 +128,7 @@ struct LayerW {                    // one pre-norm transformer layer in any of t
   bool folded = false;               // attn_norm / ff_norm folded into to_qkv (to_q, to_kv) / fc1
   bool lsa = false;                  // locality self-attention (vit_for_small_dataset.py:88-121): the diagonal masked, scale lsa_scale
   float lsa_scale = 0.f;             // exp(temperature), taken in fp32 as TensorFlow does
+  int site_out = -1, site_ff = -1;   // dropout sites (vb_handle::number_dropout_sites): to_out's; the GELU's, fc2's is site_ff + 1
 };
 
 // One LeViT Transformer layer (levit.py:141-162): attention (queries on every step-th pixel of the fmap x fmap map) + MLP.
@@ -312,8 +315,9 @@ inline bool r2l_attention_fast(const __nv_bfloat16* qkv, int ld, __nv_bfloat16* 
 
 // res_bias (may be null: patch.bias): what the patch Dense yields on an all-zero (cls) row when that is not its bias -- beta . W +
 // bias when a LayerNorm runs before it (SPT, vit_for_small_dataset.py:148-149)
-struct EmbedW { Linear patch; const float* pos = nullptr; const float* cls = nullptr; int dim = 0, n_pos = 0; const float* res_bias = nullptr; };
-struct CrossW { bool proj = false; Linear project_in, project_out, to_q, to_kv, to_out; Norm norm; };
+struct EmbedW { Linear patch; const float* pos = nullptr; const float* cls = nullptr; int dim = 0, n_pos = 0; const float* res_bias = nullptr;
+               int site = -1; };   // site: the embedding dropout's (vb_handle::number_dropout_sites)
+struct CrossW { bool proj = false; Linear project_in, project_out, to_q, to_kv, to_out; Norm norm; int site = -1; };
 
 inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
@@ -381,6 +385,24 @@ struct vb_handle {
   enum { PROF_GEMM = 0, PROF_ATTN = 1, PROF_LN = 2, PROF_EMBED = 3, PROF_OTHER = 4, PROF_GEMM_GELU = 5, PROF_GEMM_RES = 6, PROF_NUM = 7 };
   struct ProfRec { int cls; cudaEvent_t a, b; double flops; double bytes; };
   bool profiling = false;
+  // Training-mode dropout (vb_set_dropout): the rates, whether a seed is set, and the {seed, draw counter} pair in device memory
+  // that the dropout epilogues read.  `training` holds while vb_forward_train issues its launches.
+  bool drop_set = false, training = false;
+  float drop_rate = 0.f, emb_drop_rate = 0.f;
+  DevMem drop_dev;
+  static bool dropout_kind(int kind) {
+    return kind == VB_KIND_VIT || kind == VB_KIND_DEEPVIT || kind == VB_KIND_CAIT || kind == VB_KIND_CROSSVIT;
+  }
+  bool dropout_active() const { return training && (drop_rate > 0.f || emb_drop_rate > 0.f); }
+  // the epilogue of one site: off unless this is a training forward and the site's rate is > 0
+  DropoutEpi dropout(int site, bool emb, int pos) const {
+    DropoutEpi d;
+    const float rate = emb ? emb_drop_rate : drop_rate;
+    if (!training || site < 0 || rate <= 0.f) return d;
+    d.pos = pos; d.state = static_cast<const unsigned long long*>(drop_dev.p); d.site = site; d.rate = rate;
+    d.scale = static_cast<float>(1.0 / (1.0 - static_cast<double>(rate)));   // tf.nn.dropout: x * (1 / (1 - rate)) kept
+    return d;
+  }
   std::vector<ProfRec> prof_recs;
   std::vector<cudaEvent_t> event_pool;
   double prof_ms[PROF_NUM] = {0}, prof_flops[PROF_NUM] = {0}, prof_bytes[PROF_NUM] = {0};
@@ -757,7 +779,7 @@ struct vb_handle {
   std::map<ResKey, std::unique_ptr<DevMem>> embed_res;
 
   // cached wgmma GEMM plans (TMA descriptors)
-  using PlanKey = std::array<uintptr_t, 16>;
+  using PlanKey = std::array<uintptr_t, 18>;      // slots 16-17: the dropout epilogue (vb_handle::linear)
   std::map<PlanKey, GemmBf16> plans;
 
   // Whole-forward CUDA graphs (vb_forward): the launch sequence of one (image pointer, logits pointer, batch, h, w, stream)
@@ -1419,6 +1441,28 @@ struct vb_handle {
     return e;
   }
 
+  // The site of every Dropout layer the reference's call reaches, in its call order from 0 (include/vitb200.h, vb_set_dropout):
+  // the embedding's; per layer to_out's (absent without an out-projection, vit.py:53,61-67), the GELU's and fc2's (vit.py:38-44); CaiT's
+  // patch stack, then its class stack; CrossViT's small then large embedder, then per block the small tower's layers, the large tower's
+  // and the cross-attention rounds, sm_attend_lg before lg_attend_sm (cross_vit.py:187-193,147-160).
+  void number_dropout_sites() {
+    int s = 0;
+    auto layer = [&](LayerW& l) { l.site_out = l.project_out ? s++ : -1; l.site_ff = s; s += 2; };
+    if (cfg.kind == VB_KIND_CROSSVIT) {
+      sm_embed.site = s++;
+      lg_embed.site = s++;
+      for (auto& xb : xblocks) {
+        for (auto& l : xb.sm_layers) layer(l);
+        for (auto& l : xb.lg_layers) layer(l);
+        for (size_t R = 0; R < xb.sm_attend_lg.size(); ++R) { xb.sm_attend_lg[R].site = s++; xb.lg_attend_sm[R].site = s++; }
+      }
+    } else {
+      embed.site = s++;
+      for (auto& l : layers) layer(l);
+      for (auto& l : cls_layers) layer(l);
+    }
+  }
+
   void finalize() {
     for (auto& w : weights) VB_CHECK(w.set, "vb_finalize: weight '" + w.name + "' was never set");
     VB_CUDA(cudaSetDevice(device));
@@ -1552,6 +1596,7 @@ struct vb_handle {
       sm_head_norm = make_norm("sm_head_norm", c.sm_dim); sm_head = make_linear_f32("sm_head", c.sm_dim, c.num_classes);
       lg_head_norm = make_norm("lg_head_norm", c.lg_dim); lg_head = make_linear_f32("lg_head", c.lg_dim, c.num_classes);
     }
+    if (dropout_kind(c.kind)) number_dropout_sites();
     if (distill_wrapper) {
       dmlp_norm = make_norm("distill_mlp.0", c.dim);
       dmlp = make_linear_f32("distill_mlp.1", c.dim, c.num_classes);
@@ -2235,6 +2280,7 @@ struct vb_handle {
     const T* R = embed_residual<T>(e, B, rows, s);
     T* X = arena.get<T>(static_cast<size_t>(M) * e.dim);
     Epi ep; ep.bias = e.patch.bias; ep.res = R; ep.ldr = e.dim;
+    ep.drop = dropout(e.site, true, DROP_AFTER_RES);              // vit.py:166: Dropout(emb_dropout) of the sum
     if (ln_stats != nullptr) { ep.ln_stats = ln_stats; ep.bias = e.patch.ln_c2; }
     if (stats_out != nullptr && bf16() && e.dim % 64 == 0) {
       *stats_out = row_stats(M, e.dim);
@@ -2471,6 +2517,7 @@ struct vb_handle {
     }
     if (l.project_out) {
       Epi e; e.bias = l.to_out.bias; e.scale = l.attn_scale; e.res = X; e.ldr = dim;
+      e.drop = dropout(l.site_out, false, DROP_BEFORE_RES);
       if (fold) e.stats_out = stats;
       linear<T>(O, inner, M, l.to_out, X, dim, e, s);
     } else {
@@ -2644,8 +2691,10 @@ struct vb_handle {
     const T* A = X;
     if (stats != nullptr) { e1.ln_stats = stats; e1.bias = l.fc1.ln_c2; }
     else { VB_CHECK(!l.folded, "internal: folded layer without statistics"); ln<T>(X, l.ff_norm, Y, M, dim, s); A = Y; e1.bias = l.fc1.bias; }
+    e1.drop = dropout(l.site_ff, false, DROP_BEFORE_RES);
     linear<T>(A, dim, M, l.fc1, Hb, l.fc1.N, e1, s);
     Epi e2; e2.bias = l.fc2.bias; e2.scale = l.ff_scale; e2.res = X; e2.ldr = dim;
+    e2.drop = dropout(l.site_ff < 0 ? -1 : l.site_ff + 1, false, DROP_BEFORE_RES);
     e2.stats_out = stats;
     linear<T>(Hb, l.fc1.N, M, l.fc2, X, dim, e2, s);
   }
@@ -2666,6 +2715,7 @@ struct vb_handle {
     linear<T>(ctx, dim, B * nctx, l.to_kv, KV, 2 * inner, Epi(), s);
     attention<T>(Q, inner, KV, 2 * inner, KV + inner, 2 * inner, O, inner, B, 1, nctx, l, s);
     Epi e; e.bias = l.to_out.bias; e.scale = l.attn_scale; e.res = Cx; e.ldr = dim;
+    e.drop = dropout(l.site_out, false, DROP_BEFORE_RES);
     linear<T>(O, inner, B, l.to_out, Cx, dim, e, s);
     feed_forward<T>(Cx, B, dim, l, Yc, s);
   }
@@ -2693,11 +2743,13 @@ struct vb_handle {
     if (x.proj) {
       T* a = arena.get<T>(static_cast<size_t>(B) * dctx);
       Epi e1; e1.bias = x.to_out.bias;
+      e1.drop = dropout(x.site, false, DROP_BEFORE_RES);           // cross_vit.py:64-67: to_out's Dropout, before project_out
       linear<T>(O, inner, B, x.to_out, a, dctx, e1, s);
       Epi e2; e2.bias = x.project_out.bias; e2.res = cls; e2.ldr = dcls;
       linear<T>(a, dctx, B, x.project_out, cls, dcls, e2, s);
     } else {
       Epi e; e.bias = x.to_out.bias; e.res = cls; e.ldr = dcls;
+      e.drop = dropout(x.site, false, DROP_BEFORE_RES);
       linear<T>(O, inner, B, x.to_out, cls, dcls, e, s);
     }
   }
@@ -2832,6 +2884,9 @@ struct vb_handle {
       classify<T>(S, ns, c.sm_dim, sm_head_norm, sm_head, B, 0, logits, false, s);
       classify<T>(G, nl, c.lg_dim, lg_head_norm, lg_head, B, 0, logits, true, s);
     }
+    // after the last site on the forward's stream (CrossViT's side stream joined before the cross-attention), as a plain launch: it
+    // starts when every kernel before it has completed, and the next forward's dropout kernels read the counter after it
+    if (dropout_active()) { ProfScope ps(this, PROF_OTHER, 0.0, 16.0, s); dropout_advance(static_cast<unsigned long long*>(drop_dev.p), s); }
   }
 
   float* row_stats(long long M, int dp) {       // (sum, sumsq) partials per 64-column chunk of M rows: bf16 only
@@ -3982,7 +4037,7 @@ struct vb_handle {
 template <>
 void vb_handle::linear<float>(const float* A, int lda, int M, const Linear& L, float* out, int ldc, const Epi& e, cudaStream_t s) {
   gemm_simt<float, float, float>(A, lda, L.W, L.N, 1, out, ldc, M, L.N, L.K, e.bias, e.scale,
-                                 static_cast<const float*>(e.res), e.ldr, e.act(), s);
+                                 static_cast<const float*>(e.res), e.ldr, e.act(), s, e.drop);
 }
 template <>
 void vb_handle::linear<__nv_bfloat16>(const __nv_bfloat16* A, int lda, int M, const Linear& L, __nv_bfloat16* out, int ldc,
@@ -4005,19 +4060,27 @@ void vb_handle::linear<__nv_bfloat16>(const __nv_bfloat16* A, int lda, int M, co
                                  reinterpret_cast<uintptr_t>(e.ln_stats), reinterpret_cast<uintptr_t>(L.ln_c1),
                                  reinterpret_cast<uintptr_t>(e.stats_out)};
     for (int i = 0; i < 16; ++i) key[i] = parts[i];
+    if (e.drop.pos != DROP_NONE) {                  // a dropout epilogue: its position, site and rate
+      uint32_t rate_bits = 0;
+      std::memcpy(&rate_bits, &e.drop.rate, sizeof rate_bits);
+      key[16] = static_cast<uintptr_t>(e.drop.pos) | static_cast<uintptr_t>(e.drop.site) << 8;
+      key[17] = rate_bits;
+    }
     auto it = plans.find(key);
     if (it == plans.end()) {
       if (plans.size() > 8192) plans.clear();      // shape sweeps: bounded host memory (a plan is four 128-byte tensor maps)
-      GemmBf16 g = gemm_bf16_plan(A, lda, L.Wt, L.ldw, out, ldc, M, L.N, K, e.bias, e.scale, res, e.ldr, e.act());
+      GemmBf16 g = gemm_bf16_plan(A, lda, L.Wt, L.ldw, out, ldc, M, L.N, K, e.bias, e.scale, res, e.ldr, e.act(), false, 0,
+                                  e.drop.pos != DROP_NONE);
       if (folded) { g.ln_c1 = L.ln_c1; g.ln_stats = e.ln_stats; g.ln_parts = K / 64; g.ln_inv_d = 1.0f / static_cast<float>(L.ln_d > 0 ? L.ln_d : K);
                     g.ln_eps = L.ln_eps; }
       if (e.stats_out) { g.stats_out = e.stats_out; }
+      g.drop = e.drop;
       it = plans.emplace(key, g).first;
     }
     gemm_bf16_run(it->second, s);
   } else {
     gemm_simt<__nv_bfloat16, __nv_bfloat16, __nv_bfloat16>(A, lda, L.Wt, 1, L.ldw, out, ldc, M, L.N, K, e.bias, e.scale, res,
-                                                           e.ldr, e.act(), s);
+                                                           e.ldr, e.act(), s, e.drop);
   }
 }
 
@@ -5056,11 +5119,14 @@ int vb_finalize(vb_handle* h) {
   });
 }
 
-int vb_forward(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, int32_t img_h, int32_t img_w, float* logits,
-               int32_t logits_mem, void* stream) {
+namespace {
+// vb_forward and vb_forward_train: `train` runs every dropout site with a rate > 0 (vb_handle::dropout) and advances the draw counter
+int forward_entry(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, int32_t img_h, int32_t img_w, float* logits,
+                  int32_t logits_mem, void* stream, bool train) {
   return guarded(h, [&] {
     VB_CHECK(h != nullptr && img != nullptr && logits != nullptr, "vb_forward: null argument");
     VB_CHECK(h->finalized, "vb_forward: call vb_finalize after setting the weights");
+    VB_CHECK(!train || h->drop_set, "vb_forward_train: call vb_set_dropout first");
     VB_CHECK(!h->is_mim(), h->whole_forward_only(h->cfg.kind));
     VB_CHECK(batch > 0 && img_h > 0 && img_w > 0, "vb_forward: bad batch / image size");
     VB_CUDA(cudaSetDevice(h->device));
@@ -5080,7 +5146,14 @@ int vb_forward(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, i
       out_d = static_cast<float*>(h->logits_dev.p);
     }
     if (h->cfg.kind == VB_KIND_ATS_VIT) h->ats_prepare(batch, img_h, img_w);
-    run_graphed(h, vb_handle::GraphKey{img_d, out_d, batch, img_h, img_w, s}, [&] {
+    vb_handle::GraphKey key{img_d, out_d, batch, img_h, img_w, s};
+    struct Training {                                      // the flag holds while the launches are issued, exceptions included
+      vb_handle* h;
+      Training(vb_handle* hh, bool on) : h(hh) { h->training = on; }
+      ~Training() { h->training = false; }
+    } tr(h, train);
+    key.flags = h->dropout_active() ? 2 : 0;               // all rates 0: the inference forward and its graph
+    run_graphed(h, key, [&] {
       if (h->bf16()) h->forward_impl<__nv_bfloat16>(img_d, batch, img_h, img_w, out_d, s);
       else h->forward_impl<float>(img_d, batch, img_h, img_w, out_d, s);
     });
@@ -5089,6 +5162,50 @@ int vb_forward(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, i
       VB_CUDA(cudaMemcpyAsync(logits, out_d, out_bytes, cudaMemcpyDeviceToHost, s));
       VB_CUDA(cudaStreamSynchronize(s));
     }
+  });
+}
+}  // namespace
+
+int vb_forward(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, int32_t img_h, int32_t img_w, float* logits,
+               int32_t logits_mem, void* stream) {
+  return forward_entry(h, img, img_mem, batch, img_h, img_w, logits, logits_mem, stream, false);
+}
+
+int vb_forward_train(vb_handle* h, const float* img, int32_t img_mem, int32_t batch, int32_t img_h, int32_t img_w, float* logits,
+                     int32_t logits_mem, void* stream) {
+  return forward_entry(h, img, img_mem, batch, img_h, img_w, logits, logits_mem, stream, true);
+}
+
+int vb_set_dropout(vb_handle* h, float dropout, float emb_dropout, uint64_t seed) {
+  return guarded(h, [&] {
+    VB_CHECK(h != nullptr, "null handle");
+    VB_CHECK(vb_handle::dropout_kind(h->cfg.kind) && !h->distill_wrapper,
+             "vb_set_dropout: training-mode dropout runs on ViT, DeepViT, CaiT and CrossViT handles only");
+    VB_CHECK(dropout >= 0.f && dropout < 1.f, "vb_set_dropout: dropout = " + std::to_string(dropout) + " is outside [0, 1)");
+    VB_CHECK(emb_dropout >= 0.f && emb_dropout < 1.f, "vb_set_dropout: emb_dropout = " + std::to_string(emb_dropout) + " is outside [0, 1)");
+    VB_CUDA(cudaSetDevice(h->device));
+    VB_CUDA(cudaDeviceSynchronize());                    // no forward in flight reads the old key, counter or rates
+    h->drop_dev.ensure(2 * sizeof(unsigned long long));
+    const unsigned long long v[2] = {static_cast<unsigned long long>(seed), 0ull};
+    VB_CUDA(cudaMemcpy(h->drop_dev.p, v, sizeof v, cudaMemcpyHostToDevice));
+    VB_CUDA(cudaDeviceSynchronize());                    // a pageable copy may return before it lands
+    h->drop_rate = dropout;
+    h->emb_drop_rate = emb_dropout;
+    h->drop_set = true;
+    h->drop_graphs();                                    // the captured launches carry the rates
+  });
+}
+
+int vb_op_dropout_mask(uint64_t seed, uint32_t draw, uint32_t site, int32_t M, int32_t N, float rate, uint8_t* keep) {
+  return guarded(nullptr, [&] {
+    VB_CHECK(keep != nullptr && M > 0 && N > 0, "vb_op_dropout_mask: bad arguments");
+    VB_CHECK(rate >= 0.f && rate < 1.f, "vb_op_dropout_mask: rate outside [0, 1)");
+    require_gpu();
+    DevMem out;
+    const size_t n = static_cast<size_t>(M) * N;
+    out.ensure(n);
+    dropout_mask(static_cast<unsigned long long>(seed), draw, site, M, N, rate, static_cast<uint8_t*>(out.p), 0);
+    VB_CUDA(cudaMemcpy(keep, out.p, n, cudaMemcpyDeviceToHost));
   });
 }
 

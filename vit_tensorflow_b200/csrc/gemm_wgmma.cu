@@ -32,6 +32,7 @@
 
 #include "common.h"
 #include "kernels.cuh"
+#include "philox.cuh"
 #include "ptx.cuh"
 
 namespace vb {
@@ -100,14 +101,17 @@ __device__ __forceinline__ void ring_advance(int& stage, uint32_t& phase, int n)
 }
 
 // EPI: 0 = no per-column addend, 1 = + bias[n], 2 = folded LayerNorm (c1 = ln_c1, c2 = bias)
-template <int BN, int ACT, bool RES, int EPI, bool OF32>
+// DROP: training-mode dropout (DropPos), its own instances; DROP_NONE compiles the epilogue without it
+template <int BN, int ACT, bool RES, int EPI, bool OF32, int DROP = DROP_NONE>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                  const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_res, int M, int N, int K,
                  float* __restrict__ out_f32, int ldc, const float* __restrict__ bias, const float* __restrict__ scale,
                  const float* __restrict__ ln_c1, const float2* ln_stats, int ln_parts, float ln_inv_d, float ln_eps,
-                 float2* __restrict__ stats_out) {
+                 float2* __restrict__ stats_out, const unsigned long long* drop_state, uint32_t drop_site, float drop_rate,
+                 float drop_scale) {
   static_assert(!OF32 || (ACT == ACT_NONE && !RES && EPI != 2), "fp32 output: plain / bias epilogue only");
+  static_assert(DROP == DROP_NONE || (!OF32 && (DROP == DROP_BEFORE_RES || RES)), "dropout: bf16 output; after the residual needs one");
   static_assert(BN == 128 || BN == 192, "tile width");
   using T = Tile<BN>;
   constexpr int STAGES = T::STAGES, STAGE_BYTES = T::STAGE_BYTES, STG_BYTES = T::STG_BYTES, PARAM_FLOATS = T::PARAM_FLOATS;
@@ -246,6 +250,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   int stage = 0;
   uint32_t phase = 0, epi_phase = 0;
   ring_advance<STAGES>(stage, phase, cw * num_kb);                 // warpgroup 1 starts after tile 0's k-blocks
+  // the dropout key and draw counter, read after griddepcontrol.wait (the kernel that advances the counter has completed)
+  unsigned long long drop_seed = 0;
+  uint32_t drop_d = 0;
+  if constexpr (DROP != DROP_NONE) { drop_seed = drop_state[0]; drop_d = static_cast<uint32_t>(drop_state[1]); }
 
   for (long long t = blockIdx.x + static_cast<long long>(cw) * gridDim.x; t < tiles; t += 2LL * gridDim.x) {
     const int n0 = static_cast<int>(t % n_tiles) * BN;
@@ -352,6 +360,21 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
                 if (ACT == ACT_SILU) v[i][e] = silu(v[i][e]);
               }
             }
+            // the group's two 2 x 2 fragments (columns u = 0, 1) are one Philox block each: words 2 h + e
+            auto drop_mask = [&]() {
+#pragma unroll
+              for (int u = 0; u < 2; ++u) {
+                const uint4 x = dropout_block(drop_seed, drop_d, drop_site, static_cast<uint32_t>(m0 + row_l + 64 * hm),
+                                              static_cast<uint32_t>(nc + (2 * jp + u) * 8 + col_t));
+                const uint32_t wd[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                  for (int e = 0; e < 2; ++e)
+                    v[2 * u + h][e] = dropout_keep(wd[2 * h + e], drop_rate) ? v[2 * u + h][e] * drop_scale : 0.f;
+              }
+            };
+            if constexpr (DROP == DROP_BEFORE_RES) drop_mask();
             if (has_scale) {
 #pragma unroll
               for (int u = 0; u < 2; ++u) {
@@ -384,8 +407,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
                   v[i][0] += bf16_lo(r[i]);
                   v[i][1] += bf16_hi(r[i]);
                 }
-                r[i] = pack_bf16x2(v[i][0], v[i][1]);
               }
+              if constexpr (DROP == DROP_AFTER_RES) drop_mask();
+#pragma unroll
+              for (int i = 0; i < 4; ++i) r[i] = pack_bf16x2(v[i][0], v[i][1]);
               stmatrix_x4(addr, r);
               if (has_stats) {
 #pragma unroll
@@ -451,9 +476,9 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-template <int BN, int ACT, bool RES, int EPI, bool OF32 = false>
+template <int BN, int ACT, bool RES, int EPI, bool OF32 = false, int DROP = DROP_NONE>
 void launch(const GemmBf16& g, cudaStream_t stream) {
-  auto kern = gemm_bf16_kernel<BN, ACT, RES, EPI, OF32>;
+  auto kern = gemm_bf16_kernel<BN, ACT, RES, EPI, OF32, DROP>;
   constexpr int smem = Tile<BN>::SMEM_BYTES;
   static unsigned long long seen[4] = {0, 0, 0, 0};
   if (first_use_on_this_device(seen)) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -471,7 +496,8 @@ void launch(const GemmBf16& g, cudaStream_t stream) {
   VB_CUDA(cudaLaunchKernelEx(&cfg, kern, g.tmap_a, g.tmap_b, g.tmap_out, g.tmap_res, g.M, g.N, g.K,
                              OF32 ? reinterpret_cast<float*>(g.out) : nullptr, g.ldc, g.bias, g.scale, g.ln_c1,
                              reinterpret_cast<const float2*>(g.ln_stats), g.ln_parts, g.ln_inv_d, g.ln_eps,
-                             reinterpret_cast<float2*>(g.stats_out)));
+                             reinterpret_cast<float2*>(g.stats_out), g.drop.state, static_cast<uint32_t>(g.drop.site), g.drop.rate,
+                             g.drop.scale));
   count_launch();
 }
 
@@ -484,6 +510,17 @@ void dispatch(const GemmBf16& g, bool res, int epi, cudaStream_t stream) {
     }
   }
   VB_CHECK(!g.out_f32, "gemm_bf16: fp32 output runs the 128-wide tile only");
+  VB_CHECK(g.drop.pos == DROP_NONE || BN == 128, "gemm_bf16: dropout runs the 128-wide tile only");
+  if constexpr (BN == 128) if (g.drop.pos != DROP_NONE) {              // the dropout sites of ViT / DeepViT / CaiT / CrossViT
+#define VB_GEMM_DROP(A, R, E, D) if (g.act == A && res == R && epi == E && g.drop.pos == D) return launch<BN, A, R, E, false, D>(g, stream)
+    VB_GEMM_DROP(ACT_NONE, true, 1, DROP_BEFORE_RES);                   // to_out, fc2 (+ residual)
+    VB_GEMM_DROP(ACT_NONE, false, 1, DROP_BEFORE_RES);                  // CrossViT's projected to_out
+    VB_GEMM_DROP(ACT_GELU, false, 1, DROP_BEFORE_RES);                  // fc1 + GELU
+    VB_GEMM_DROP(ACT_GELU, false, 2, DROP_BEFORE_RES);                  // fc1 + GELU, LayerNorm folded
+    VB_GEMM_DROP(ACT_NONE, true, 1, DROP_AFTER_RES);                    // patch embedding + positions
+#undef VB_GEMM_DROP
+    VB_CHECK(false, "gemm_bf16: no dropout instance for this epilogue (activation " + std::to_string(g.act) + ")");
+  }
 #define VB_GEMM_CASE(A, R, E) if (g.act == A && res == R && epi == E) return launch<BN, A, R, E>(g, stream)
   VB_GEMM_CASE(ACT_NONE, false, 0); VB_GEMM_CASE(ACT_NONE, false, 1); VB_GEMM_CASE(ACT_NONE, false, 2);
   VB_GEMM_CASE(ACT_GELU, false, 0); VB_GEMM_CASE(ACT_GELU, false, 1); VB_GEMM_CASE(ACT_GELU, false, 2);
@@ -543,7 +580,7 @@ bool gemm_bf16_supported(int M, int N, int K, int lda, int ldw, int ldc) {
 
 GemmBf16 gemm_bf16_plan(const __nv_bfloat16* A, int lda, const __nv_bfloat16* Wt, int ldw, __nv_bfloat16* out, int ldc, int M,
                         int N, int K, const float* bias, const float* scale, const __nv_bfloat16* res, int ldr, int act,
-                        bool out_f32, int b_rows) {
+                        bool out_f32, int b_rows, bool dropout) {
   VB_CHECK(gemm_bf16_supported(M, N, K, lda, ldw, ldc), "gemm_bf16: unsupported shape (need N%64==0, K%8==0, ld%8==0)");
   VB_CHECK(res == nullptr || ldr % 8 == 0, "gemm_bf16: residual leading dimension must be a multiple of 8");
   VB_CHECK((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(Wt) | reinterpret_cast<uintptr_t>(out) |
@@ -555,8 +592,9 @@ GemmBf16 gemm_bf16_plan(const __nv_bfloat16* A, int lda, const __nv_bfloat16* Wt
   // The wider tile where it covers N exactly (no half-empty last column of tiles) in at least 8 column tiles.  Measured on
   // an H100 at ViT-B/16's shapes, it takes N = 2304 / 3072 at K = 768 from 0.320 / 0.448 ms to 0.281 / 0.423-0.433, but
   // N = 768 (4 column tiles) runs no faster at K = 768 and 3 % slower at K = 3072, so those keep the 128-wide tile.
-  // An fp32 output (the classifier heads) keeps it too: its 64-bit row addresses next to 192 accumulators make ptxas spill.
-  g.bn = N % 192 == 0 && N >= 8 * 192 && !out_f32 ? 192 : 128;
+  // An fp32 output (the classifier heads) keeps it too: its 64-bit row addresses next to 192 accumulators make ptxas spill; so
+  // does a dropout epilogue, whose Philox rounds need registers beyond the 232 the 192 accumulators leave.
+  g.bn = N % 192 == 0 && N >= 8 * 192 && !out_f32 && !dropout ? 192 : 128;
   g.tmap_a = make_tmap_2d(A, K, M, static_cast<uint64_t>(lda) * 2, BK, BM);
   // b_rows: rows of Wt that exist (< N when the output is column-padded: TMA zero-fills the rest instead of reading on)
   g.tmap_b = make_tmap_2d(Wt, K, b_rows > 0 ? b_rows : N, static_cast<uint64_t>(ldw) * 2, BK, g.bn);

@@ -2,6 +2,7 @@
 // and the exact-fp32 SIMT GEMM / attention used by the fp32 numerics gate (BASELINE config 1) and as the
 // general fallback of the bf16 path.  See kernels.cuh for the contracts and the reference lines replaced.
 #include "kernels.cuh"
+#include "philox.cuh"
 #include <atomic>
 
 namespace vb {
@@ -297,10 +298,12 @@ __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.0f +
 // (16*TM)x64 output tile, 16x16 threads x (TM x 4) micro-tile, BK = 16; exact fp32 FMA accumulation in k order.
 // TM = 4: 64-row tiles; TM = 1: 16-row tiles for small-M problems (the classifier head) so the grid still fills the GPU.
 // SILU: the SiLU epilogue (act is then ignored), an instance of its own so that the others keep their registers.
-template <typename TA, typename TW, typename TO, int TM, bool SILU = false>
+// DROP: training-mode dropout (DropPos), instances of their own likewise.
+template <typename TA, typename TW, typename TO, int TM, bool SILU = false, int DROP = DROP_NONE>
 __global__ void __launch_bounds__(256)
 gemm_simt_kernel(const TA* __restrict__ A, int lda, const TW* __restrict__ W, int wsk, int wsn, TO* out, int ldc, int M, int N,
-                 int K, const float* __restrict__ bias, const float* __restrict__ scale, const TO* res, int ldr, int act) {
+                 int K, const float* __restrict__ bias, const float* __restrict__ scale, const TO* res, int ldr, int act,
+                 DropoutEpi drop) {
   constexpr int BMT = 16 * TM;
   __shared__ float As[16][BMT + 1];
   __shared__ __align__(16) float Ws[16][64 + 4];   // pitch 68 floats: 16-byte aligned rows, one LDS.128 per thread and k
@@ -312,6 +315,9 @@ gemm_simt_kernel(const TA* __restrict__ A, int lda, const TW* __restrict__ W, in
   for (int i = 0; i < TM; ++i)
 #pragma unroll
     for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+  unsigned long long drop_seed = 0;
+  uint32_t drop_d = 0;
+  if constexpr (DROP != DROP_NONE) { drop_seed = drop.state[0]; drop_d = static_cast<uint32_t>(drop.state[1]); }
   for (int k0 = 0; k0 < K; k0 += 16) {
     for (int e = threadIdx.x; e < 16 * 64; e += 256) {
       if (e < 16 * BMT) {  // A tile: consecutive threads along k (contiguous in memory)
@@ -356,8 +362,11 @@ gemm_simt_kernel(const TA* __restrict__ A, int lda, const TW* __restrict__ W, in
       if (SILU) v = silu(v);                                                      // mobile_vit.py:33
       else if (act == ACT_GELU) v = gelu_erf_f(v);
       else if (act == ACT_HSWISH) v = v * fminf(fmaxf(v + 3.0f, 0.0f), 6.0f) / 6.0f;   // levit.py:37
+      const bool keep = DROP == DROP_NONE || dropout_keep_at(drop_seed, drop_d, drop.site, m, n, drop.rate);
+      if (DROP == DROP_BEFORE_RES) v = keep ? v * drop.scale : 0.f;
       if (scale) v *= scale[n];
       if (res) v += to_f(res[static_cast<long long>(m) * ldr + n]);
+      if (DROP == DROP_AFTER_RES) v = keep ? v * drop.scale : 0.f;
       out[static_cast<long long>(m) * ldc + n] = from_f<TO>(v);
     }
   }
@@ -1193,16 +1202,42 @@ void layernorm(const T* x, int ldx, const float* gamma, const float* beta, T* ou
 
 template <typename TA, typename TW, typename TO>
 void gemm_simt(const TA* A, int lda, const TW* W, int wsk, int wsn, TO* out, int ldc, int M, int N, int K, const float* bias,
-               const float* scale, const TO* res, int ldr, int act, cudaStream_t s) {
+               const float* scale, const TO* res, int ldr, int act, cudaStream_t s, const DropoutEpi& drop) {
+  VB_CHECK(drop.pos == DROP_NONE || act != ACT_SILU, "gemm_simt: no dropout instance with the SiLU epilogue");
+  VB_CHECK(drop.pos != DROP_AFTER_RES || res != nullptr, "gemm_simt: dropout after the residual needs one");
   if (static_cast<long long>((N + 63) / 64) * ((M + 63) / 64) >= 2 * sm_count()) {
     const unsigned grid = flat_blocks((N + 63) / 64, (M + 63) / 64, "gemm_simt");
-    if (act == ACT_SILU) gemm_simt_kernel<TA, TW, TO, 4, true><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act);
-    else gemm_simt_kernel<TA, TW, TO, 4><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act);
+    if (act == ACT_SILU) gemm_simt_kernel<TA, TW, TO, 4, true><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act, drop);
+    else if (drop.pos == DROP_BEFORE_RES) gemm_simt_kernel<TA, TW, TO, 4, false, DROP_BEFORE_RES><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act, drop);
+    else if (drop.pos == DROP_AFTER_RES) gemm_simt_kernel<TA, TW, TO, 4, false, DROP_AFTER_RES><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act, drop);
+    else gemm_simt_kernel<TA, TW, TO, 4><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act, drop);
   } else {
     const unsigned grid = flat_blocks((N + 63) / 64, (M + 15) / 16, "gemm_simt");
-    if (act == ACT_SILU) gemm_simt_kernel<TA, TW, TO, 1, true><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act);
-    else gemm_simt_kernel<TA, TW, TO, 1><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act);
+    if (act == ACT_SILU) gemm_simt_kernel<TA, TW, TO, 1, true><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act, drop);
+    else if (drop.pos == DROP_BEFORE_RES) gemm_simt_kernel<TA, TW, TO, 1, false, DROP_BEFORE_RES><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act, drop);
+    else if (drop.pos == DROP_AFTER_RES) gemm_simt_kernel<TA, TW, TO, 1, false, DROP_AFTER_RES><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act, drop);
+    else gemm_simt_kernel<TA, TW, TO, 1><<<grid, 256, 0, s>>>(A, lda, W, wsk, wsn, out, ldc, M, N, K, bias, scale, res, ldr, act, drop);
   }
+  VB_LAUNCHED();
+}
+
+// The draw counter's advance after a training-mode forward's last site (one thread; the launches after it wait for it)
+__global__ void dropout_advance_kernel(unsigned long long* state) { state[1] = static_cast<uint32_t>(state[1] + 1); }
+void dropout_advance(unsigned long long* state, cudaStream_t s) {
+  dropout_advance_kernel<<<1, 1, 0, s>>>(state);
+  VB_LAUNCHED();
+}
+
+// keep[m, n] of site `site` at draw d (vb_op_dropout_mask), by the function the epilogues use
+__global__ void dropout_mask_kernel(unsigned long long seed, uint32_t d, uint32_t site, int M, int N, float rate, uint8_t* __restrict__ keep) {
+  const long long total = static_cast<long long>(M) * N;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const uint32_t m = static_cast<uint32_t>(i / N), n = static_cast<uint32_t>(i % N);
+    keep[i] = dropout_keep_at(seed, d, site, m, n, rate) ? 1 : 0;
+  }
+}
+void dropout_mask(unsigned long long seed, uint32_t d, uint32_t site, int M, int N, float rate, uint8_t* keep, cudaStream_t s) {
+  dropout_mask_kernel<<<grid_1d(static_cast<long long>(M) * N), 256, 0, s>>>(seed, d, site, M, N, rate, keep);
   VB_LAUNCHED();
 }
 
@@ -1559,10 +1594,11 @@ VB_INST_T(float)
 VB_INST_T(__nv_bfloat16)
 
 template void gemm_simt<float, float, float>(const float*, int, const float*, int, int, float*, int, int, int, int, const float*,
-                                             const float*, const float*, int, int, cudaStream_t);
+                                             const float*, const float*, int, int, cudaStream_t, const DropoutEpi&);
 template void gemm_simt<__nv_bfloat16, __nv_bfloat16, __nv_bfloat16>(const __nv_bfloat16*, int, const __nv_bfloat16*, int, int,
                                                                      __nv_bfloat16*, int, int, int, int, const float*,
-                                                                     const float*, const __nv_bfloat16*, int, int, cudaStream_t);
+                                                                     const float*, const __nv_bfloat16*, int, int, cudaStream_t,
+                                                                     const DropoutEpi&);
 template void unfold_same<__nv_bfloat16, __nv_bfloat16>(const __nv_bfloat16*, __nv_bfloat16*, int, int, int, int, int, int, int, int,
                                                         cudaStream_t, int, const UnfoldMode*);
 template void convert_rows<__nv_bfloat16, float>(const __nv_bfloat16*, int, float*, int, long long, int, cudaStream_t);

@@ -32,10 +32,15 @@ void transpose_rows_bf16(const __nv_bfloat16* in, int ldi, long long in_batch, _
                          int n, int npad, int cols, cudaStream_t s);
 
 // out[M,N] (TO) = epi(A[M,K] (TA, lda) x W), W element (k,n) at W[k*wsk + n*wsn]; fp32 FMA accumulation.
-// epi = (+bias) -> act (Act: GELU(erf) / hard-swish / SiLU) -> (*scale) -> (+res[m*ldr + n]).
+// epi = (+bias) -> act (Act: GELU(erf) / hard-swish / SiLU) -> (dropout) -> (*scale) -> (+res[m*ldr + n]) -> (dropout).
 template <typename TA, typename TW, typename TO>
 void gemm_simt(const TA* A, int lda, const TW* W, int wsk, int wsn, TO* out, int ldc, int M, int N, int K,
-               const float* bias, const float* scale, const TO* res, int ldr, int act, cudaStream_t s);
+               const float* bias, const float* scale, const TO* res, int ldr, int act, cudaStream_t s,
+               const DropoutEpi& drop = DropoutEpi());
+// Training-mode dropout: advance the draw counter state[1] by one (after a forward's last site), and the keep mask [M, N] (uint8) of
+// one site on its own, by the epilogues' function (philox.cuh dropout_keep_at).
+void dropout_advance(unsigned long long* state, cudaStream_t s);
+void dropout_mask(unsigned long long seed, uint32_t d, uint32_t site, int M, int N, float rate, uint8_t* keep, cudaStream_t s);
 
 // Generic attention through materialised scores (any n, d, variant), S fp32 [B,h,nq,nk] workspace.
 // q: [B, nq, *] rows of pitch ldq with head hh at columns [hh*dh, (hh+1)*dh); k, v likewise (nk rows per batch).

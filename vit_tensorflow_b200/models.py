@@ -274,15 +274,20 @@ class _EngineModel:
                 "libvitb200 implements inference semantics: stochastic dropout (rate > 0 with training=True, the "
                 "reference's default) is not reproducible; pass training=False or construct with dropout = 0")
 
+    def _training_forward(self, training):
+        """Whether a call with `training` runs the training-mode forward (vb_forward_train); raises where the engine has none."""
+        self._check_training(training)
+        return False
+
     def __call__(self, img, training=True, **kwargs):
         """Reference call surface (vit.py:159): numpy NHWC float image batch -> numpy float32 logits."""
-        self._check_training(training)
+        train = self._training_forward(training)
         x = np.ascontiguousarray(img, dtype=np.float32)
         if x.ndim != 4 or x.shape[3] != 3:
             raise ValueError("img must be NHWC float [b, H, W, 3]")
         b, h, w, _ = x.shape
         out = np.empty((b, self.num_classes), np.float32)
-        self.forward_raw(x.ctypes.data, _lib.MEM_HOST, b, h, w, out.ctypes.data, _lib.MEM_HOST, None)
+        self.forward_raw(x.ctypes.data, _lib.MEM_HOST, b, h, w, out.ctypes.data, _lib.MEM_HOST, None, training=train)
         return _as_tensor(out)
 
     call = __call__
@@ -293,11 +298,13 @@ class _EngineModel:
         super().__init_subclass__(**kwargs)
         cls.call = cls.__call__
 
-    def forward_raw(self, img_ptr, img_mem, batch, h, w, logits_ptr, logits_mem, stream=None):
-        """Pointer-level forward: host or device (e.g. torch tensor .data_ptr()) buffers, optional cudaStream_t."""
+    def forward_raw(self, img_ptr, img_mem, batch, h, w, logits_ptr, logits_mem, stream=None, training=False):
+        """Pointer-level forward: host or device (e.g. torch tensor .data_ptr()) buffers, optional cudaStream_t.  training=True
+        runs the training-mode forward where the model has one (set_dropout_seed), and is refused as __call__ refuses it."""
         self._finalize()
-        _lib.check(self._lib.vb_forward(self._h, C.c_void_p(img_ptr), img_mem, batch, h, w, C.c_void_p(logits_ptr), logits_mem,
-                                        C.c_void_p(stream) if stream else None), self._h)
+        fn = self._lib.vb_forward_train if training and self._training_forward(True) else self._lib.vb_forward
+        _lib.check(fn(self._h, C.c_void_p(img_ptr), img_mem, batch, h, w, C.c_void_p(logits_ptr), logits_mem,
+                      C.c_void_p(stream) if stream else None), self._h)
 
     def forward_tokens(self, tokens):
         self._finalize()
@@ -418,7 +425,36 @@ class _EngineModel:
             pass
 
 
-class ViT(_EngineModel):
+class _TrainingDropout:
+    """Training-mode dropout on the device for ViT, DeepViT, CaiT and CrossViT (include/vitb200.h, vb_set_dropout): after
+    set_dropout_seed(seed), a call with training=True (the reference's default) and a rate > 0 masks every Dropout site from the
+    engine's Philox stream, keyed by the seed, with a draw counter on the device that advances once per such call."""
+
+    _dropout_seed = None
+    _dropout_pending = False
+
+    def set_dropout_seed(self, seed):
+        """Key the dropout stream by the 64-bit `seed` and reset its draw counter; from then on training-mode calls with a rate
+        > 0 run.  None restores the refusal (NotImplementedError)."""
+        self._dropout_seed = None if seed is None else int(seed) & 0xFFFFFFFFFFFFFFFF
+        self._dropout_pending = seed is not None
+
+    def _training_forward(self, training):
+        if self._dropout_seed is None or not training:
+            return super()._training_forward(training)
+        dropout, emb_dropout = self._dropout_rates
+        for r in (dropout, emb_dropout):
+            if not 0 <= r < 1:      # tf.nn.dropout (Keras Dropout's call)
+                raise ValueError(f"rate must be a scalar tensor or a float in the range [0, 1), got {r:g}")
+        if dropout == 0 and emb_dropout == 0:
+            return False
+        if self._dropout_pending:
+            _lib.check(self._lib.vb_set_dropout(self._h, float(dropout), float(emb_dropout), self._dropout_seed), self._h)
+            self._dropout_pending = False
+        return True
+
+
+class ViT(_TrainingDropout, _EngineModel):
     """vit.py:106-177."""
     _kind = "vit"
 
@@ -469,6 +505,10 @@ class DistillableViT(ViT):
         self.args, self.kwargs = args, kwargs
         self.dim, self.num_classes = kwargs["dim"], kwargs["num_classes"]
 
+    def set_dropout_seed(self, seed):
+        raise NotImplementedError("DistillableViT runs inference semantics only: training-mode dropout runs on ViT, DeepViT, CaiT "
+                                  "and CrossViT")
+
     def __call__(self, img, distill_token=None, training=True):
         if distill_token is None:
             return super().__call__(img, training=training)
@@ -509,7 +549,7 @@ class DeepViT(ViT):
                          emb_dropout, precision=precision, device=device, seed=seed)
 
 
-class CaiT(_EngineModel):
+class CaiT(_TrainingDropout, _EngineModel):
     """cait.py:155-194."""
     _kind = "cait"
 
@@ -528,7 +568,7 @@ class CaiT(_EngineModel):
         self._attach_stage_attributes()
 
 
-class CrossViT(_EngineModel):
+class CrossViT(_TrainingDropout, _EngineModel):
     """cross_vit.py:232-303."""
     _kind = "crossvit"
 
