@@ -635,6 +635,42 @@ VB_API int vb_op_nest_aggregate(int32_t precision, const float* x, int32_t B, in
                                 const float* beta, const float* pos, int32_t bh, int32_t bw, float* out, float* stats_out,
                                 int32_t iters, float* elapsed_ms);
 
+/* A Conv2D as the engine runs every convolution that is not depthwise (CCT, LeViT, CvT, Twins-SVT, CrossFormer, NesT, RegionViT,
+ * MobileViT, ScalableViT): unfold_same writes each output pixel's (k_row, k_col, channel) patch vector, the GEMM multiplies it by
+ * the kernel.  Appended within ABI 7.
+ *   x: image != 0: an NHWC image [B, H, W, cin] (read as fp32 in both precisions; ld == cin, off == 0); image == 0: a token map
+ *      [B*H*W, ld] whose channels are the columns [off, off + cin) (bf16: rounded to bf16 at a pitch of ld rounded up to 64).
+ *   kernel [k, k, cin, N] (Keras Conv2D), bias [N] or NULL, packed as vb_finalize packs a Dense (K = k*k*cin, pitch round_up(K, 8)).
+ *   valid != 0: VALID windows, floor((H - k) / stride) + 1 per side; else TF SAME, ceil(H / stride) per side with total padding
+ *      max((oh - 1) * stride + k - H, 0), the smaller half first, and the padded taps zero.
+ *   ln_gamma / ln_beta [cin] (both or neither; a map with off == 0 whose columns [cin, ld) are zero): the LayerNorm of each pixel's
+ *      cin channels (eps ln_eps) before the convolution; bf16 applies it on load from the map's row statistics, fp32 runs it first.
+ *   gelu_in != 0 (a map only): the exact-erf GELU of every loaded value, after the LayerNorm; padded taps stay zero.
+ *   act: the GEMM's activation (0 none, 1 exact-erf GELU, 2 hard-swish, 3 SiLU) after the bias; res [rows, ldr] or NULL: added last.
+ *   out [rows, N], rows = B * oh * ow pixel-major; stats_out (bf16 with N % 64 == 0, may be NULL): [N/64][rows] (sum, sumsq) float
+ *      pairs of the stored bf16 rows.  All buffers are host memory. */
+VB_API int vb_op_conv2d(int32_t precision, const float* x, int32_t image, int32_t B, int32_t H, int32_t W, int32_t cin, int32_t ld,
+                        int32_t off, const float* kernel, const float* bias, int32_t N, int32_t k, int32_t stride, int32_t valid,
+                        const float* ln_gamma, const float* ln_beta, float ln_eps, int32_t gelu_in, int32_t act, const float* res,
+                        int32_t ldr, float* out, float* stats_out, int32_t iters, float* elapsed_ms);
+/* CCT's tokenizer tail (cct.py:196-200,213,278-286) as the engine runs it: x [B, H, W, C] -> ReLU -> MaxPool2D(k, stride, 'SAME')
+ * (padded taps never win) -> + pos [oh*ow, C] (may be NULL) -> out [B, rows, C], rows >= oh * ow, rows past oh * ow zero. */
+VB_API int vb_op_cct_pool(int32_t precision, const float* x, int32_t B, int32_t H, int32_t W, int32_t C, int32_t k, int32_t stride,
+                          const float* pos, int32_t rows, float* out, int32_t iters, float* elapsed_ms);
+/* CCT's sequence pooling (cct.py:291-299) as the engine runs it: per image y_t = LayerNorm(x[b, t]) (eps 1e-3, gamma / beta [D]),
+ * w = softmax_t(y_t . pw + pb[0]), z[b] = sum_t w_t y_t.  x [B, n, D] -> z [B, D] fp32.  Refuses D > 1024 and n == 0. */
+VB_API int vb_op_seq_pool(int32_t precision, const float* x, int32_t B, int32_t n, int32_t D, const float* gamma, const float* beta,
+                          const float* pw, const float* pb, float* z, int32_t iters, float* elapsed_ms);
+/* The classifier heads' pooling as the engine runs it: x [B*n, ldx] (ldx >= D) -> z[b] = LayerNorm(pool(x[b])) over the first D
+ * columns, pool = row 0 (mean_pool == 0) or the mean over the n rows, LayerNorm eps 1e-3; gamma == beta == NULL: the pool alone.
+ * z [B, D] fp32. */
+VB_API int vb_op_pool_layernorm(int32_t precision, const float* x, int32_t B, int32_t n, int32_t ldx, int32_t D, const float* gamma,
+                                const float* beta, int32_t mean_pool, float* z, int32_t iters, float* elapsed_ms);
+/* LeViT's stride-2 query gather (levit.py:75) as the engine runs it: x [B*H*W, ldi] -> out [B*ceil(H/step)*ceil(W/step), ldo], out
+ * pixel (r, c) = the first C columns of x pixel (step*r, step*c); out is uploaded and downloaded whole. */
+VB_API int vb_op_gather_grid(int32_t precision, const float* x, int32_t ldi, int32_t B, int32_t H, int32_t W, int32_t C, int32_t step,
+                             float* out, int32_t ldo, int32_t iters, float* elapsed_ms);
+
 /* MobileViT (mobile_vit.py:209-271), appended within ABI 7.  conv1: Conv_NxN_BN(channels[0], 3, stride 2); stem: MV2 blocks 0-3;
  * trunk: per stage s an MV2 block (4 + s, stride 2) and a MobileViTBlock(dims[s], depths[s], channels[5 + 2 s], kernel_size,
  * (ph, pw), mlp dims[s] * (2, 4, 4)[s]); to_logits: Conv_NxN_BN(last_dim, 1), the mean over pixels, a bias-free Dense.  Conv_NxN_BN

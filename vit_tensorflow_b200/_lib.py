@@ -221,6 +221,13 @@ SIGNATURES = {
                              [C.c_void_p, C.c_void_p, C.c_int32, _f32p]),
     "vb_op_r2l_attention": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 8 + [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32,
                                                                                    _f32p]),
+    "vb_op_conv2d": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 7 + [C.c_void_p] * 2 + [C.c_int32] * 4 + [C.c_void_p] * 2 +
+                     [C.c_float, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, _f32p]),
+    "vb_op_cct_pool": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 6 + [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, _f32p]),
+    "vb_op_seq_pool": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p] * 5 + [C.c_int32, _f32p]),
+    "vb_op_pool_layernorm": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 2 + [C.c_int32, C.c_void_p, C.c_int32,
+                                                                                                     _f32p]),
+    "vb_op_gather_grid": (C.c_int, [C.c_int32, C.c_void_p] + [C.c_int32] * 6 + [C.c_void_p, C.c_int32, C.c_int32, _f32p]),
     "vb_op_softmax_rows": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p] + [C.c_int32] * 4 + [C.c_float, C.c_int32, _f32p]),
 }
 
@@ -463,6 +470,81 @@ def op_nest_aggregate(x, gamma, beta, pos=None, bh=1, bw=1, precision="bf16", it
     check(load().vb_op_nest_aggregate(PRECISION[precision], _ptr(x), B, H, W, Cc, _ptr(gamma), _ptr(beta), _ptr(pos), bh, bw, _ptr(out),
                                       _ptr(stats) if stats is not None else None, iters, C.byref(ms)))
     return out, stats, (ms.value if iters > 0 else None)
+
+
+ACT = {"none": 0, "gelu": 1, "hswish": 2, "silu": 3}   # Act of csrc/common.h
+
+
+def op_conv2d(x, kernel, bias=None, stride=1, valid=False, image=False, HW=None, cin=None, off=0, ln_gamma=None, ln_beta=None,
+              ln_eps=1e-5, gelu_in=False, act="none", res=None, want_stats=False, precision="bf16", iters=0):
+    """A Conv2D as the engine runs it (vb_op_conv2d): unfold_same, then the GEMM.  x: image=True, an NHWC image [B, H, W, cin];
+    else a token map [B*H*W, ld] with HW = (B, H, W) and the channels at columns [off, off + cin).  kernel [k, k, cin, N] (Keras).
+    Returns (out [B*oh*ow, N], stats [N/64, rows, 2] of the bf16 rows or None, ms or None)."""
+    x, kernel, bias, ln_gamma, ln_beta, res = map(_f32, (x, kernel, bias, ln_gamma, ln_beta, res))
+    k, _, kc, N = kernel.shape
+    if image:
+        B, H, W, ld = x.shape
+        cin = ld
+    else:
+        B, H, W = HW
+        ld = x.shape[1]
+        cin = kc if cin is None else cin
+    oh, ow = ((H - k) // stride + 1, (W - k) // stride + 1) if valid else (-(-H // stride), -(-W // stride))
+    rows = B * oh * ow
+    out = np.empty((rows, N), np.float32)
+    stats = np.zeros((N // 64, rows, 2), np.float32) if want_stats else None
+    ms = C.c_float(0)
+    check(load().vb_op_conv2d(PRECISION[precision], _ptr(x), int(bool(image)), B, H, W, cin, ld, off, _ptr(kernel), _ptr(bias), N, k,
+                              stride, int(bool(valid)), _ptr(ln_gamma), _ptr(ln_beta), float(ln_eps), int(bool(gelu_in)), ACT[act],
+                              _ptr(res), 0 if res is None else res.shape[1], _ptr(out), _ptr(stats), iters, C.byref(ms)))
+    return out, stats, (ms.value if iters > 0 else None)
+
+
+def op_cct_pool(x, k, stride, pos=None, rows=None, precision="bf16", iters=0):
+    """CCT's ReLU + MaxPool2D(k, stride, SAME) + positions (vb_op_cct_pool): x [B, H, W, C] -> (out [B, rows, C], ms or None);
+    rows None: oh * ow."""
+    x, pos = _f32(x), _f32(pos)
+    B, H, W, Cc = x.shape
+    rows = -(-H // stride) * -(-W // stride) if rows is None else rows
+    out = np.empty((B, rows, Cc), np.float32)
+    ms = C.c_float(0)
+    check(load().vb_op_cct_pool(PRECISION[precision], _ptr(x), B, H, W, Cc, k, stride, _ptr(pos), rows, _ptr(out), iters, C.byref(ms)))
+    return out, (ms.value if iters > 0 else None)
+
+
+def op_seq_pool(x, gamma, beta, pw, pb, precision="bf16", iters=0):
+    """CCT's sequence pooling (vb_op_seq_pool): x [B, n, D], pw [D], pb scalar -> (z [B, D], ms or None)."""
+    x, gamma, beta, pw = map(_f32, (x, gamma, beta, pw))
+    pb = np.asarray([pb], np.float32).reshape(1)
+    B, n, D = x.shape
+    z = np.empty((B, D), np.float32)
+    ms = C.c_float(0)
+    check(load().vb_op_seq_pool(PRECISION[precision], _ptr(x), B, n, D, _ptr(gamma), _ptr(beta), _ptr(pw), _ptr(pb), _ptr(z), iters,
+                                C.byref(ms)))
+    return z, (ms.value if iters > 0 else None)
+
+
+def op_pool_layernorm(x, D, gamma=None, beta=None, mean=False, precision="bf16", iters=0):
+    """The heads' pooling (vb_op_pool_layernorm): x [B, n, ldx] -> (z [B, D] = LayerNorm(row 0 or the mean of the rows' first D
+    columns), ms or None); gamma / beta None: the pool alone."""
+    x, gamma, beta = map(_f32, (x, gamma, beta))
+    B, n, ldx = x.shape
+    z = np.empty((B, D), np.float32)
+    ms = C.c_float(0)
+    check(load().vb_op_pool_layernorm(PRECISION[precision], _ptr(x), B, n, ldx, D, _ptr(gamma), _ptr(beta), int(bool(mean)), _ptr(z),
+                                      iters, C.byref(ms)))
+    return z, (ms.value if iters > 0 else None)
+
+
+def op_gather_grid(x, B, H, W, C_, step, out, precision="bf16", iters=0):
+    """LeViT's strided query gather (vb_op_gather_grid): x [B*H*W, ldi], out [B*ceil(H/step)*ceil(W/step), ldo] initial contents,
+    returned whole with the first C_ columns of pixel (step r, step c) in row (r, c)."""
+    x = _f32(x)
+    out = np.array(out, dtype=np.float32, order="C", copy=True)
+    ms = C.c_float(0)
+    check(load().vb_op_gather_grid(PRECISION[precision], _ptr(x), x.shape[1], B, H, W, C_, step, _ptr(out), out.shape[1], iters,
+                                   C.byref(ms)))
+    return out, (ms.value if iters > 0 else None)
 
 
 def op_r2l_attention(qkv, B, lh, lw, rh, rw, heads, dh, table, window_size, precision="bf16", ldo=None, iters=0):

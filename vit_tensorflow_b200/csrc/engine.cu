@@ -2904,7 +2904,7 @@ struct vb_handle {
     T* col = arena.get<T>(static_cast<size_t>(rows) * Kp);
     {
       ProfScope ps(this, PROF_EMBED, 0.0, static_cast<double>(map ? sizeof(T) : 4) * B * h * w * cin + static_cast<double>(sizeof(T)) * rows * Kp, s);
-      if (map == nullptr) unfold_same<float, T>(img, col, B, h, w, cin, k, stride, 0, Kp, s);
+      if (map == nullptr) unfold_same<float, T>(img, col, B, h, w, cin, k, stride, 0, Kp, s, 0, um);
       else unfold_same<T, T>(map, col, B, h, w, cin, k, stride, 0, Kp, s, ld, um);
     }
     Linear Lk = L;
@@ -6047,6 +6047,155 @@ int vb_op_nest_aggregate(int32_t precision, const float* x, int32_t B, int32_t H
     });
     for (size_t r = 0; r < Mo; ++r) std::copy(oh.begin() + r * Cp, oh.begin() + r * Cp + C, out + r * C);
     if (bf && stats_out != nullptr) std::copy(sh.begin(), sh.begin() + Mo * (Cp / 64) * 2, stats_out);
+  });
+}
+
+int vb_op_conv2d(int32_t precision, const float* x, int32_t image, int32_t B, int32_t H, int32_t W, int32_t cin, int32_t ld, int32_t off,
+                 const float* kernel, const float* bias, int32_t N, int32_t k, int32_t stride, int32_t valid, const float* ln_gamma,
+                 const float* ln_beta, float ln_eps, int32_t gelu_in, int32_t act, const float* res, int32_t ldr, float* out,
+                 float* stats_out, int32_t iters, float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    VB_CHECK(x && kernel && out && B > 0 && H > 0 && W > 0 && cin > 0 && N > 0 && k > 0 && stride > 0, "vb_op_conv2d: bad arguments");
+    VB_CHECK(image ? (ld == cin && off == 0) : (off >= 0 && ld >= off + cin), "vb_op_conv2d: the map's channels [off, off + cin) exceed ld");
+    VB_CHECK((ln_gamma == nullptr) == (ln_beta == nullptr), "vb_op_conv2d: the LayerNorm needs both gamma and beta");
+    const bool ln = ln_gamma != nullptr;
+    VB_CHECK(!image || (!ln && !gelu_in), "vb_op_conv2d: the LayerNorm and GELU on load read a token map, not the image");
+    VB_CHECK(!ln || (off == 0 && ln_eps > 0.f), "vb_op_conv2d: the LayerNorm needs off == 0 and eps > 0");
+    VB_CHECK(act >= ACT_NONE && act <= ACT_SILU, "vb_op_conv2d: act must be 0 (none), 1 (GELU), 2 (hard-swish) or 3 (SiLU)");
+    VB_CHECK(!valid || (H >= k && W >= k), "vb_op_conv2d: a VALID window larger than the map");
+    const bool bf = precision != VB_PRECISION_FP32;               // as with_precision picks the element type
+    VB_CHECK(res == nullptr || ldr >= N, "vb_op_conv2d: ldr < N");
+    VB_CHECK(stats_out == nullptr || !bf || N % 64 == 0, "vb_op_conv2d: output statistics need N % 64 == 0");
+    const long long M = static_cast<long long>(B) * H * W;
+    // the token map at the pitch the engine's zero-padded rows have: whole 64-column chunks in bf16, as row_stats reads them
+    const int P = image ? cin : bf ? round_up(ld, 64) : ld;
+    if (ln)                                                       // the row statistics sum every column: past cin, the pad's zeros
+      for (long long r = 0; r < M; ++r)
+        for (int c = cin; c < ld; ++c) VB_CHECK(x[r * ld + c] == 0.f, "vb_op_conv2d: with the LayerNorm, columns [cin, ld) must be zero");
+    const int oh = valid ? (H - k) / stride + 1 : (H + stride - 1) / stride, ow = valid ? (W - k) / stride + 1 : (W + stride - 1) / stride;
+    const long long rows = static_cast<long long>(B) * oh * ow;
+    const int K = k * k * cin;
+    std::vector<float> xp(static_cast<size_t>(M) * P, 0.f);
+    for (long long r = 0; r < M; ++r) std::copy(x + r * (image ? cin : ld), x + (r + 1) * (image ? cin : ld), xp.begin() + r * P);
+    DevMem dX, dW, dB, dG, dBt, dR, dO;
+    const float* dw = upload<float>(dW, kernel, static_cast<size_t>(K) * N);
+    const float* db = bias ? upload<float>(dB, bias, N) : nullptr;
+    const float* g_d = ln ? upload<float>(dG, ln_gamma, cin) : nullptr;
+    const float* b_d = ln ? upload<float>(dBt, ln_beta, cin) : nullptr;
+    with_precision(precision, [&](vb_handle& h, auto tag) {
+      using T = decltype(tag);
+      const Linear L = h.pack_linear(dw, db, K, N, round_up(K, 8), nullptr);   // as make_linear packs it
+      const float* img_d = image ? upload<float>(dX, xp.data(), xp.size()) : nullptr;
+      const T* map_d = image ? nullptr : upload<T>(dX, xp.data(), xp.size());
+      const T* r_d = res ? upload<T>(dR, res, static_cast<size_t>(rows) * ldr) : nullptr;
+      dO.ensure(static_cast<size_t>(rows) * N * sizeof(T));
+      T* o_d = static_cast<T*>(dO.p);
+      float* so = nullptr;
+      timed(iters, elapsed_ms, [&] {
+        h.arena.reset();
+        UnfoldMode um;
+        um.valid = valid != 0;
+        um.gelu = gelu_in != 0;
+        const T* src = map_d ? map_d + off : nullptr;
+        if (ln && h.bf16()) {                                     // the LayerNorm on load from the map's row statistics
+          float* st = h.row_stats(M, P);
+          h.ensure_stats<T>(map_d, P, st, static_cast<int>(M), 0);
+          um.stats = st; um.parts = P / 64; um.d = cin; um.eps = ln_eps; um.gamma = g_d; um.beta = b_d;
+        } else if (ln) {                                          // fp32: a separate LayerNorm into scratch first
+          T* Z = h.arena.get<T>(static_cast<size_t>(M) * P);
+          layernorm<T>(map_d, P, g_d, b_d, Z, P, static_cast<int>(M), cin, 0, P, ln_eps);
+          src = Z;
+        }
+        so = stats_out && h.bf16() ? h.row_stats(rows, N) : nullptr;
+        h.conv<T>(img_d, src, P, B, H, W, cin, k, stride, L, o_d, so, 0, &um, act, r_d, ldr);
+      });
+      download<T>(o_d, out, static_cast<size_t>(rows) * N);
+      if (so) VB_CUDA(cudaMemcpy(stats_out, so, static_cast<size_t>(N / 64) * rows * 2 * sizeof(float), cudaMemcpyDeviceToHost));
+    });
+  });
+}
+
+int vb_op_cct_pool(int32_t precision, const float* x, int32_t B, int32_t H, int32_t W, int32_t C, int32_t k, int32_t stride,
+                   const float* pos, int32_t rows, float* out, int32_t iters, float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    VB_CHECK(x && out && B > 0 && H > 0 && W > 0 && C > 0 && k > 0 && stride > 0 && rows > 0, "vb_op_cct_pool: bad arguments");
+    const int oh = (H + stride - 1) / stride, ow = (W + stride - 1) / stride;
+    VB_CHECK(rows >= oh * ow, "vb_op_cct_pool: fewer output rows than pooled positions");
+    const size_t ci = static_cast<size_t>(B) * H * W * C, co = static_cast<size_t>(B) * rows * C;
+    DevMem dX, dP, dO;
+    const float* p_d = pos ? upload<float>(dP, pos, static_cast<size_t>(oh) * ow * C) : nullptr;
+    with_precision(precision, [&](vb_handle& h, auto tag) {
+      using T = decltype(tag);
+      const T* x_d = upload<T>(dX, x, ci);
+      dO.ensure(co * sizeof(T));
+      T* o_d = static_cast<T*>(dO.p);
+      timed(iters, elapsed_ms, [&] { maxpool_relu_same<T>(x_d, o_d, B, H, W, C, k, stride, p_d, rows, 0); });
+      (void)h;
+      download<T>(o_d, out, co);
+    });
+  });
+}
+
+int vb_op_seq_pool(int32_t precision, const float* x, int32_t B, int32_t n, int32_t D, const float* gamma, const float* beta,
+                   const float* pw, const float* pb, float* z, int32_t iters, float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    VB_CHECK(x && gamma && beta && pw && pb && z && B > 0 && n >= 0 && D > 0, "vb_op_seq_pool: bad arguments");
+    DevMem dX, dG, dB, dPw, dPb, dZ;
+    const float* g_d = upload<float>(dG, gamma, D);
+    const float* b_d = upload<float>(dB, beta, D);
+    const float* pw_d = upload<float>(dPw, pw, D);
+    const float* pb_d = upload<float>(dPb, pb, 1);
+    dZ.ensure(static_cast<size_t>(B) * D * sizeof(float));
+    float* z_d = static_cast<float*>(dZ.p);
+    with_precision(precision, [&](vb_handle& h, auto tag) {
+      using T = decltype(tag);
+      const T* x_d = upload<T>(dX, x, static_cast<size_t>(B) * n * D);
+      timed(iters, elapsed_ms, [&] { seq_pool<T>(x_d, n, D, g_d, b_d, pw_d, pb_d, z_d, B, 0); });   // refuses D > 1024 and n == 0
+      (void)h;
+    });
+    download<float>(z_d, z, static_cast<size_t>(B) * D);
+  });
+}
+
+int vb_op_pool_layernorm(int32_t precision, const float* x, int32_t B, int32_t n, int32_t ldx, int32_t D, const float* gamma,
+                         const float* beta, int32_t mean_pool, float* z, int32_t iters, float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    VB_CHECK(x && z && B > 0 && n > 0 && D > 0 && ldx >= D, "vb_op_pool_layernorm: bad arguments");
+    VB_CHECK((gamma == nullptr) == (beta == nullptr), "vb_op_pool_layernorm: the LayerNorm needs both gamma and beta");
+    DevMem dX, dG, dB, dZ;
+    const float* g_d = gamma ? upload<float>(dG, gamma, D) : nullptr;
+    const float* b_d = beta ? upload<float>(dB, beta, D) : nullptr;
+    dZ.ensure(static_cast<size_t>(B) * D * sizeof(float));
+    float* z_d = static_cast<float*>(dZ.p);
+    with_precision(precision, [&](vb_handle& h, auto tag) {
+      using T = decltype(tag);
+      const T* x_d = upload<T>(dX, x, static_cast<size_t>(B) * n * ldx);
+      timed(iters, elapsed_ms, [&] { pool_layernorm<T>(x_d, n, ldx, g_d, b_d, z_d, B, D, mean_pool != 0, 0); });
+      (void)h;
+    });
+    download<float>(z_d, z, static_cast<size_t>(B) * D);
+  });
+}
+
+int vb_op_gather_grid(int32_t precision, const float* x, int32_t ldi, int32_t B, int32_t H, int32_t W, int32_t C, int32_t step, float* out,
+                      int32_t ldo, int32_t iters, float* elapsed_ms) {
+  return guarded(nullptr, [&] {
+    require_gpu();
+    VB_CHECK(x && out && B > 0 && H > 0 && W > 0 && C > 0 && step > 0 && ldi >= C && ldo >= C, "vb_op_gather_grid: bad arguments");
+    const size_t ci = static_cast<size_t>(B) * H * W * ldi, co = static_cast<size_t>(B) * ((H + step - 1) / step) * ((W + step - 1) / step) * ldo;
+    DevMem dX, dO;
+    with_precision(precision, [&](vb_handle& h, auto tag) {
+      using T = decltype(tag);
+      const T* x_d = upload<T>(dX, x, ci);
+      T* o_d = upload<T>(dO, out, co);
+      timed(iters, elapsed_ms, [&] { gather_grid<T>(x_d, ldi, o_d, ldo, B, H, W, C, step, 0); });
+      (void)h;
+      download<T>(o_d, out, co);
+    });
   });
 }
 
